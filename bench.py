@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- Llama-3-8B Q8_0 single-stream decode (tg) on B200, the BASELINE.json headline.
+"""bench.py -- Llama-3-8B Q8_0 single-stream decode (tg) on one H100, the BASELINE.json headline.
 
 A "step" is one single-token decode forward (all layers + lm_head + on-device argmax) at a
 growing KV position, on the LlamaBench synthetic token stream (`new Random(42).nextInt(vocab)`,
@@ -11,15 +11,19 @@ LlamaBench.java:188-193) over a seeded synthetic GGUF-layout model of the real L
                every step copies the token/position H2D and the argmax D2H inside the timed region
   roofline     the WHOLE decode step (default: one CUDA graph of 227 kernels per token; --decode-mode persistent: one kernel):
                achieved = algorithmic bytes per token / device time per token, peak = MEASURED_PEAKS.json
-               hbm_gbs; per launch = per token / kernels per token; the stand-alone streaming matvecs (the dominant
-               kernels by bytes and time, timed live with CUDA events on the plan's stream) are listed under
-               roofline.other_kernels; traffic = measured DRAM bytes per launch from the committed ncu capture
+               hbm_gbs if present, else the H100 SXM data-sheet 3.35 TB/s; per launch = per token / kernels per token;
+               the stand-alone streaming matvecs (the dominant kernels by bytes and time, timed live with CUDA events
+               on the plan's stream) are listed under roofline.other_kernels
   cpu_baseline the oracle (CPU restatement of the reference's onGPU=false path) on this box's
                host cores, bounded sample
   parity       in the same run: greedy ids of the first steps GPU == oracle, max|dlogit| of step 0
                (BASELINE.md section 3); a mismatch exits non-zero
 `--impl reference` times only that CPU restatement (the reference itself needs a JDK + TornadoVM,
 neither is installable here; see DESIGN.md).
+`--dump-outputs DIR` writes, after the timed steps, what the timed paths computed: the greedy ids of the timed decode
+steps, the logits of the last one, and (with the pp512 leg) the last layer's K / V cache rows the prefill chunk wrote,
+as DIR/<name>.npy (float32 / float64).  Weights and tokens are seeded, so two builds run with the same arguments can
+be compared output for output.
 """
 from __future__ import annotations
 
@@ -39,7 +43,7 @@ import __graft_entry__ as ge  # noqa: E402
 
 WORKLOAD = "llama-3-8b"
 QUANT = "q8_0"
-FALLBACK_HBM_GBS = 6650.0
+FALLBACK_HBM_GBS = 3350.0  # H100 SXM data sheet (HBM3)
 
 
 def peaks():
@@ -47,10 +51,10 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
-    return FALLBACK_HBM_GBS, "fallback"
+    return FALLBACK_HBM_GBS, "fallback (H100 SXM data sheet)"
 
 
-FALLBACK_TENSOR_TFLOPS = 2250.0  # nominal dense bf16/fp16
+FALLBACK_TENSOR_TFLOPS = 989.0  # H100 SXM data sheet, dense bf16/fp16
 
 
 def tensor_peak():
@@ -59,12 +63,13 @@ def tensor_peak():
         with open(p) as f:
             j = json.load(f)
         return float(j["bf16_tflops"]), float(j.get("bf16_tflops_sustained", j["bf16_tflops"])), "measured (cuBLAS bf16 8192^3; fp16 shares the rate)"
-    return FALLBACK_TENSOR_TFLOPS, FALLBACK_TENSOR_TFLOPS, "fallback (nominal)"
+    return FALLBACK_TENSOR_TFLOPS, FALLBACK_TENSOR_TFLOPS, "fallback (H100 SXM data sheet)"
 
 
 def prefill_leg(pkg, lb, local: int, n: int, reps: int):
     """BASELINE config 3: Llama-3-8B FP16, --batch-prefill-size 512, pp512 from depth 0 (LlamaBench `pp`
-    semantics: forward only, no logits).  Tensor-core path: TMA + tcgen05 GEMMs, csrc/prefill*.cuh."""
+    semantics: forward only, no logits).  Tensor-core path: TMA + wgmma GEMMs, csrc/prefill*.cuh.
+    Also returns the last layer's K / V cache rows of the chunk (what the prefill produces, for --dump-outputs)."""
     shape = pkg.synth.SHAPES[WORKLOAD]
     F16 = pkg.gguf.GGMLType.F16
     model = pkg.loader.model_from_tensors(shape, F16, pkg.synth.build_tensors_fast(shape, F16, seed=1234, device=f"cuda:{local}"), n + 8)
@@ -80,19 +85,21 @@ def prefill_leg(pkg, lb, local: int, n: int, reps: int):
             dev.append(plan.prefill_info()[2])
             wall.append((t1 - t0) * 1e3)
     launches = plan.prefill_info()[1]
+    nkv = n * shape.kv_dim
+    kv = {f"pp{n}_{name}_last_layer": plan.read_buffer(name, nkv, layer=shape.n_layers - 1) for name in ("key_cache", "value_cache")}
     plan.free()
     d, w = float(np.mean(dev)), float(np.mean(wall))
     gemm = 2.0 * shape.matmul_elements_no_head() * n
     att = 4.0 * shape.q_dim * shape.n_layers * (n * (n + 1) / 2.0)
     burst, sustained, src = tensor_peak()
     tf = (gemm + att) / (d * 1e-3) / 1e12
-    return {"metric": "prefill_tokens_per_s", "value": n / d * 1e3, "unit": "tok/s", "ms_per_chunk": d, "reps": reps, "dtype": "f16 operands, f32 accumulate (TMEM)",
+    return {"metric": "prefill_tokens_per_s", "value": n / d * 1e3, "unit": "tok/s", "ms_per_chunk": d, "reps": reps, "dtype": "f16 operands, f32 accumulate",
             "e2e": {"value": n / w * 1e3, "unit": "tok/s", "h2d_bytes_per_step": 4 * n, "d2h_bytes_per_step": 0},
             "gpu_launches": launches, "mode": "tensor_core" if mode == 1 else "exact",
             "config": {"workload": f"Llama-3-8B-shaped synthetic GGUF, FP16, pp{n} in one chunk (--batch-prefill-size {n}) from depth 0, KV cache only (no logits)",
                        "l2": "inputs larger than L2 (15.0 GB of FP16 weights per chunk)"},
-            "roofline": {"kernel": "whole prefill chunk (k_gemm_f16_tcgen05 = 85 % of it, profiles/)", "bound": "tensor", "achieved": tf, "peak": burst, "peak_sustained": sustained,
-                         "peak_source": src, "unit": "TFLOP/s", "frac": tf / burst, "flop_per_chunk": {"gemm": gemm, "attention": att}, "traffic": None}}
+            "roofline": {"kernel": "whole prefill chunk (GEMMs: k_gemm_f16_wgmma)", "bound": "tensor", "achieved": tf, "peak": burst, "peak_sustained": sustained,
+                         "peak_source": src, "unit": "TFLOP/s", "frac": tf / burst, "flop_per_chunk": {"gemm": gemm, "attention": att}, "traffic": None}}, kv
 
 
 class ClockSampler:
@@ -208,6 +215,7 @@ def main():
                     help="decode implementation: one persistent kernel per token, or the round-1 CUDA graph of ~7 kernels per layer")
     ap.add_argument("--quant", default="q8_0", choices=["q8_0", "f16"], help="weight type of the synthetic model (f16: the exact lane-order FP16 matvec path, graph mode)")
     ap.add_argument("--depth", type=int, default=-1, help="LlamaBench -d: KV positions filled before the timed steps (default: the warm-up steps)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the outputs of the timed paths as DIR/<name>.npy")
     ap.add_argument("--workload", default=WORKLOAD, choices=["llama-3-8b", "llama-3-70b", "llama-3.2-1b", "qwen3-4b"],
                     help="shape of the synthetic model (default: the BASELINE headline, Llama-3-8B; 70B is BASELINE config 5, meant for --gpus 2/4/8)")
     args = ap.parse_args()
@@ -228,7 +236,7 @@ def main():
     qname = "Q8_0" if QUANT == "q8_0" else "FP16"
     config = {"workload": f"{pretty}-shaped synthetic GGUF, {qname}, tg{K} single-stream decode from depth {D}",
               "weights": "seeded N(0,1/sqrt(fan_in)) quantised with the ggml Q8_0 rule; tokens java.util.Random(42)",
-              "context": ctx, "l2": f"inputs larger than L2 ({(shape.matmul_elements() // 32 * 34 if QUANT == 'q8_0' else shape.matmul_elements() * 2) / 1e9:.2f} GB of weights stream per step vs 126 MB L2)"}
+              "context": ctx, "l2": f"inputs larger than L2 ({(shape.matmul_elements() // 32 * 34 if QUANT == 'q8_0' else shape.matmul_elements() * 2) / 1e9:.2f} GB of weights stream per step vs 50 MB L2)"}
 
     if args.impl == "reference":
         if world > 1 and rank != 0:
@@ -276,6 +284,10 @@ def main():
     barrier()
     ids, ms = plan.decode_sequence(tokens[D:D + K], K, D)
     barrier()
+    dump = {}
+    if args.dump_outputs and rank == 0:  # the caller of the device loop receives the ids; the logits buffer holds the last step's
+        dump["decode_ids"] = np.asarray(ids, dtype=np.float64)
+        dump["decode_logits_last_step"] = plan.read_buffer("logits", shape.vocab)
     ms_rank = [ms]
     if world > 1:
         t = torch.tensor([ms], device=f"cuda:{local}")
@@ -330,11 +342,6 @@ def main():
             m, b = plan.time_kernel(which, reps=3 if which != 4 else 1)
             per_kernel[name] = {"ms": m, "GB/s": b / (m / 1e3) / 1e9, "bytes": b, "frac": b / (m / 1e3) / 1e9 / peak}
     persistent = dmode == 1
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r2_decode_traffic.json")  # dram bytes per launch from the committed ncu --set full capture
-    if world == 1 and WORKLOAD == "llama-3-8b" and QUANT == "q8_0" and os.path.exists(tpath):
-        with open(tpath) as f:
-            traffic = json.load(f).get("persistent" if persistent else "graph")
     line = {
         "metric": "decode_tokens_per_s", "value": value, "unit": "tok/s", "n_gpus": world, "steps": K, "warmup": W,
         "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak" if world == 1 else "strong", "vs_baseline": None,
@@ -349,7 +356,7 @@ def main():
                                + ("per GPU" if world > 1 else "single GPU"),
                      "bound": "hbm", "achieved": step_gbs, "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": step_gbs / peak,
                      "bytes_per_launch": step_bytes if persistent else step_bytes / launches_per_step, "ms_per_launch": ms / K if persistent else ms / K / launches_per_step,
-                     "algorithmic_bytes_per_token": ab, "traffic": traffic,
+                     "algorithmic_bytes_per_token": ab,
                      "persistent_kernel": {"ring_stages": ring_stages, "smem_bytes": pd_smem} if persistent else None,
                      "dominant_kernel": ({"name": ("k_stream_matvec_q8<GATEUP>" if QUANT == "q8_0" else "k_stream_matvec_f16<GATEUP>") + " (gate/up + SwiGLU: the largest share of the step's bytes and time), stand-alone, CUDA events on the plan's stream",
                                           "achieved": per_kernel["gate_up"]["GB/s"], "peak": peak, "unit": "GB/s", "frac": per_kernel["gate_up"]["frac"],
@@ -370,7 +377,12 @@ def main():
     plan.free()
     if not args.no_pp and world == 1 and WORKLOAD == "llama-3-8b" and QUANT == "q8_0":  # BASELINE config 3 is the 8B FP16 model
         del model, plan
-        line["pp512"] = prefill_leg(pkg, lb, local, 512, 5)
+        line["pp512"], kv = prefill_leg(pkg, lb, local, 512, 5)
+        dump.update(kv)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dump.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
     print(json.dumps(line))
     if world > 1:
         dist.barrier()

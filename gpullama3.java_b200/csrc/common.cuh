@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for libb200llama (sm_100a only).
+// common.cuh -- shared device helpers for libb200llama (sm_90a).
 //
 // Numerics contract: every kernel reproduces the float evaluation order of the reference's
 // CPU path (see DESIGN.md "Exactness").  The translation unit is compiled with -fmad=false
@@ -151,11 +151,13 @@ __device__ __forceinline__ int quant_block_lane(float v, float &ascale) {
     return __float2int_rz(__fadd_rn(s, copysignf(0.5f, s)));
 }
 
-// 256-bit read-only streaming load (LDG.E.256 on sm_100a): one whole Q8_0 quant block per lane.
+// One whole Q8_0 quant block (32 bytes) per lane as two 128-bit read-only streaming loads
+// (sm_90 has no 256-bit global load).
 __device__ __forceinline__ void ldg256_stream(const void *p, int (&r)[8]) {
-    asm("ld.global.nc.L1::no_allocate.v8.s32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-        : "l"(p));
+    asm("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "l"(p));
+    asm("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];"
+        : "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
+        : "l"(reinterpret_cast<const char *>(p) + 16));
 }
 
 __device__ __forceinline__ int4 ldg128_stream(const void *p) {

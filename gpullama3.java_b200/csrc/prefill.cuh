@@ -1,7 +1,7 @@
 // prefill.cuh -- batched prefill (--batch-prefill-size N) on the tensor cores.
 //
 // One chunk of n <= B prompt tokens at positions start .. start+n-1 goes through every layer as GEMMs
-// (prefill_gemm.cuh: TMA + tcgen05.mma, FP32 accumulation in TMEM) instead of n matvec passes:
+// (prefill_gemm.cuh: TMA + wgmma, FP32 accumulation in registers) instead of n matvec passes:
 //
 //   X[n][dim] <- embedding rows                                      k_pf_embed
 //   per layer:  A16 <- f16(rmsnorm(X) * w)                            k_pf_rmsnorm_f16   (batchedRmsReduce + batchedRmsApplyFP16)
@@ -25,17 +25,13 @@
 #include <vector>
 
 struct PrefillLayerMaps {
-    CUtensorMap qkv, wo, w1, w3, w2; // weight boxes of 128 rows (64 for w1 / w3: the single-CTA gate/up tile is 64 + 64)
-    CUtensorMap w1p, w3p;            // 128-row boxes for the CTA-pair gate/up tile (128 + 128)
+    CUtensorMap qkv, wo, w1, w3, w2; // weight boxes of 128 rows (64 for w1 / w3: the gate/up tile is 64 + 64)
 };
 
 struct PrefillCtx {
     int batch = 0, bpad = 0;
     bool ready = false; // tensor-core path usable for this plan
     int mode = 0;       // 0 = exact token-by-token graph, 1 = tensor-core GEMMs
-    bool pair = true;      // CTA-pair (cta_group::2) GEMMs; B200_GEMM_2CTA=0 selects the single-CTA kernels
-    bool persist = true;   // persistent CTA-pair GEMM (double-buffered TMEM accumulators) for QKV and gate/up; B200_GEMM_PERSIST=0 turns it off
-    bool persist_resid = false; // B200_GEMM_PERSIST_RESID=1: the residual GEMMs (Wo, W2) through the persistent kernel with split-K work items
     bool att_simt = false; // debug: FP32 SIMT attention instead of the mma.sync kernel (B200_PF_ATT=simt)
     float *X = nullptr, *QKV = nullptr;
     __half *A16 = nullptr, *ATT16 = nullptr, *H16 = nullptr;
@@ -295,7 +291,7 @@ __global__ void __launch_bounds__(PA_THREADS) k_pf_attention(const float *__rest
 // query rows (4 warps x 16 rows), key tiles of 64.  Q (pre-scaled), K and V are converted to f16 on their
 // way into shared memory; S = Q K^T stays in registers, its accumulator layout is re-used directly as the
 // A operand of P V, and V's B fragments come from ldmatrix.trans.  This op is 1 % of the prefill FLOPs
-// (0.07 of 7.2 TFLOP at pp512); the GEMMs that carry the rest run on tcgen05.
+// (0.07 of 7.2 TFLOP at pp512); the GEMMs that carry the rest run on wgmma.
 constexpr int PM_THREADS = 128, PM_ROWS = 64, PM_KT = 64;
 template <int HS> constexpr size_t pm_smem_bytes() { return (size_t)5 * PM_ROWS * (HS + 8) * 2; } // Q + 2 x (K, V)
 

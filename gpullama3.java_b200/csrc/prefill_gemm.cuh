@@ -1,13 +1,13 @@
 // prefill_gemm.cuh -- the batched-prefill building block: C[M,N] (fp32) = A[M,K] (fp16) * B[N,K]^T (fp16)
-// on the 5th-generation tensor cores (sm_100a): TMA (cp.async.bulk.tensor, SWIZZLE_128B) -> shared
-// memory ring -> tcgen05.mma (kind::f16, cta_group::1, 128 x BN x 16 per instruction, accumulator in
-// TMEM) -> tcgen05.ld epilogue.  Replaces the reference's mma.sync m16n8k16 GEMMs gemmMMA / gemmMMAQKV /
-// gemmMMAGateUp (TransformerBatchPrefillKernels.java:792-915, 971, 1132), which stage BK=16 through a
-// single shared-memory buffer.  A = activations rounded to FP16 (batchedRmsApplyFP16, :61), B = the FP16
-// weight matrix exactly as stored in GGUF ([N][K], K contiguous = "K-major" for both operands).
+// on the Hopper tensor cores (sm_90a): TMA (cp.async.bulk.tensor, SWIZZLE_128B) -> shared-memory ring
+// guarded by mbarriers -> wgmma.mma_async (m64n128k16, f16 x f16 -> f32, both operands read from shared
+// memory, accumulator in registers) -> epilogue.  Replaces the reference's mma.sync m16n8k16 GEMMs gemmMMA /
+// gemmMMAQKV / gemmMMAGateUp (TransformerBatchPrefillKernels.java:792-915, 971, 1132), which stage BK=16
+// through a single shared-memory buffer.  A = activations rounded to FP16 (batchedRmsApplyFP16, :61), B = the
+// FP16 weight matrix exactly as stored in GGUF ([N][K], K contiguous = "K-major" for both operands).
 //
-// Warp roles (256 threads): warp 0 lane 0 = TMA producer, warp 1 lane 0 = MMA issuer, warp 2 = TMEM
-// allocator, warps 4-7 = epilogue (warp w owns TMEM lanes 32*(w%4) .. +31, i.e. 32 rows of the tile).
+// Warp groups (384 threads): warp group 0 = TMA producer (one elected thread), warp groups 1 and 2 = consumers;
+// consumer c issues the wgmmas for rows 64*c .. 64*c+63 of the 128 x 128 tile and runs their epilogue.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -17,8 +17,9 @@
 namespace pg {
 
 constexpr int BM = 128, BK = 64, BN = 128;
-// Epilogue modes: F32 store (QKV), F32 read-add-store (x += A*W^T: Wo and W2), and the gate/up pair:
-// the B tile is 64 rows of W1 and 64 rows of W3 for the same 64 hidden units, so accumulator columns
+constexpr int GEMM_THREADS = 384;
+// Epilogue modes: F32 store (QKV), F32 reduce-add (x += A*W^T: Wo and W2, split-K partials add up), and the gate/up
+// pair: the B tile is 64 rows of W1 and 64 rows of W3 for the same 64 hidden units, so accumulator columns
 // [0,64) = gate, [64,128) = up, and the epilogue emits f16(silu(gate)*up) (InferenceCore.java:150-158).
 enum { GEMM_F32 = 0, GEMM_RESID = 1, GEMM_GATEUP = 2 };
 
@@ -27,6 +28,7 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t cnt) { asm vola
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     asm volatile(
         "{\n"
@@ -44,551 +46,161 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
                  "l"(map), "r"(c0), "r"(c1), "r"(bar)
                  : "memory");
 }
-// UMMA shared-memory matrix descriptor, K-major operand, 128-byte swizzle (cute/arch/mma_sm100_desc.hpp
-// SmemDescriptor): start address >> 4 | LBO (unused for swizzled K-major, 1) << 16 | SBO = 8 rows * 128 B >> 4
-// << 32 | version 1 << 46 | layout SWIZZLE_128B (2) << 61.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// wgmma shared-memory matrix descriptor, K-major operand, 128-byte swizzle: start address >> 4 (bits 0-13) | LBO (unused for
+// swizzled K-major, 1) << 16 | SBO = 8 rows * 128 B >> 4 << 32 | layout SWIZZLE_128B (1) << 62.  The tile base is 1024-byte aligned.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// Instruction descriptor for kind::f16: D = f32 (bit 4), A = B = f16 (0), both K-major, N >> 3 at bit 17, M >> 4 at bit 24.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n) { return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24); }
 
-__device__ __forceinline__ void umma_f16(uint32_t tmem_c, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+// d[64 rows x 128 cols] (+)= A[64 x 16] * B[128 x 16]^T.  Thread t of the warp group holds, for j = 0..15, columns
+// 8j + 2(t%4) + {0,1} of row 16(t/32) + (t%32)/4 in d[4j], d[4j+1] and of that row + 8 in d[4j+2], d[4j+3].
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db, int accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_c),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+          "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate)
         : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
-// 32 lanes x 32 consecutive fp32 accumulator columns: thread `lane` of the warp gets row (lane quarter base + lane)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
+template <int STAGES> constexpr size_t smem_bytes() { return (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + 2 * STAGES * 8 + 1024; }
 
-template <int STAGES> constexpr size_t smem_bytes() { return (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + (2 * STAGES + 1) * 8 + 16 + 1024; }
-
-// grid = (M tiles, N tiles): the CTAs that share a weight (B) tile are adjacent in launch order, so the
+// grid = (M tiles, N tiles, K splits): the CTAs that share a weight (B) tile are adjacent in launch order, so the
 // tile comes from HBM once and from L2 for the others; A (activations, a few MB) lives in L2.
-// C: row stride ldc (elements); rows >= m_valid are not stored.  GEMM_GATEUP: N tiles index 64 hidden units.
+// C: row stride ldc (elements); rows >= m_valid are not stored (GEMM_F32 / GEMM_RESID write zeros / add zeros there,
+// inside the padded buffer).  GEMM_GATEUP: N tiles index 64 hidden units.  Split z owns k-blocks [z * kb_per_split, +kb_per_split).
 template <int MODE, int STAGES>
-__global__ void __launch_bounds__(256) k_gemm_f16_tcgen05(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
-                                                         const __grid_constant__ CUtensorMap tma_b2, const __grid_constant__ CUtensorMap tma_c,
-                                                         void *__restrict__ Cv, int ldc, int m_valid, int K) {
+__global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+                                                                 const __grid_constant__ CUtensorMap tma_b2, const __grid_constant__ CUtensorMap tma_c,
+                                                                 void *__restrict__ Cv, int ldc, int m_valid, int K, int kb_per_split) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023); // SWIZZLE_128B tiles need 1024-byte alignment
     constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2;
     static_assert(STAGES * (A_BYTES + B_BYTES) >= BM * BN * 4, "the C tile is staged in the operand ring");
     uint8_t *sA = smem, *sB = smem + STAGES * A_BYTES;
     uint64_t *bars = reinterpret_cast<uint64_t *>(sB + STAGES * B_BYTES);
-    const uint32_t full0 = s32(bars), empty0 = s32(bars + STAGES), tmem_full = s32(bars + 2 * STAGES);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * STAGES + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t full0 = s32(bars), empty0 = s32(bars + STAGES);
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-        mbar_init(tmem_full, 1);
+        // empty: one arrival per consumer warp once its wgmmas have read the stage
+        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) { // TMEM: BN fp32 accumulator columns x 128 lanes
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(tmem_slot)), "r"((uint32_t)BN) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-    const int nk = (K + BK - 1) / BK, m0 = blockIdx.x * BM;
-    const int n0 = blockIdx.y * (MODE == GEMM_GATEUP ? BN / 2 : BN);
-
-    if (warp == 0 && lane == 0) {
-        // ===== TMA producer =====
-        for (int kb = 0; kb < nk; kb++) {
-            const int st = kb % STAGES;
-            mbar_wait(empty0 + 8 * st, ((kb / STAGES) & 1) ^ 1);
-            mbar_expect_tx(full0 + 8 * st, A_BYTES + B_BYTES);
-            tma_load_2d(s32(sA + st * A_BYTES), &tma_a, kb * BK, m0, full0 + 8 * st);
-            if (MODE == GEMM_GATEUP) {
-                tma_load_2d(s32(sB + st * B_BYTES), &tma_b, kb * BK, n0, full0 + 8 * st);
-                tma_load_2d(s32(sB + st * B_BYTES + B_BYTES / 2), &tma_b2, kb * BK, n0, full0 + 8 * st);
-            } else {
-                tma_load_2d(s32(sB + st * B_BYTES), &tma_b, kb * BK, n0, full0 + 8 * st);
-            }
-        }
-    } else if (warp == 1 && lane == 0) {
-        // ===== MMA issuer: one thread issues tcgen05.mma for the whole CTA =====
-        constexpr uint32_t idesc = umma_idesc_f16(BM, BN);
-        for (int kb = 0; kb < nk; kb++) {
-            const int st = kb % STAGES;
-            mbar_wait(full0 + 8 * st, (kb / STAGES) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint64_t da = umma_desc_sw128(s32(sA + st * A_BYTES)), db = umma_desc_sw128(s32(sB + st * B_BYTES));
-#pragma unroll
-            for (int k = 0; k < BK / 16; k++) // UMMA_K = 16 fp16 = 32 bytes = +2 in the (addr >> 4) field
-                umma_f16(tmem_base, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            umma_commit(empty0 + 8 * st); // smem slot free once these MMAs have read it
-        }
-        umma_commit(tmem_full); // accumulator complete
-    } else if (warp >= 4) {
-        // ===== epilogue: TMEM -> registers -> global (fp32) =====
-        mbar_wait(tmem_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int q = warp & 3; // TMEM lane quarter this warp may touch
-        const int row = m0 + q * 32 + lane;
-        const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16);
-        if (MODE == GEMM_GATEUP) {
-            __half *C = reinterpret_cast<__half *>(Cv);
-#pragma unroll 1
-            for (int c0 = 0; c0 < BN / 2; c0 += 32) {
-                uint32_t g[32], u[32];
-                tmem_ld32(tlane + (uint32_t)c0, g);
-                tmem_ld32(tlane + (uint32_t)(BN / 2 + c0), u);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (row < m_valid) {
-                    uint4 *dst = reinterpret_cast<uint4 *>(C + (size_t)row * ldc + n0 + c0);
-#pragma unroll
-                    for (int v = 0; v < 4; v++) {
-                        uint32_t w[4];
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            const float g0 = __uint_as_float(g[8 * v + 2 * e]), g1 = __uint_as_float(g[8 * v + 2 * e + 1]);
-                            const float h0 = (g0 / (1.0f + expf(-g0))) * __uint_as_float(u[8 * v + 2 * e]);
-                            const float h1 = (g1 / (1.0f + expf(-g1))) * __uint_as_float(u[8 * v + 2 * e + 1]);
-                            const __half2 hh = __floats2half2_rn(h0, h1);
-                            w[e] = *reinterpret_cast<const uint32_t *>(&hh);
-                        }
-                        dst[v] = make_uint4(w[0], w[1], w[2], w[3]);
-                    }
-                }
-            }
-        } else {
-            // FP32 tile -> shared memory (the ring is idle now: every TMA load has landed and every MMA has
-            // read it) in the SWIZZLE_128B layout of the C tensor map, then ONE thread hands the four
-            // 128 x 32 boxes to TMA: a plain tensor store (QKV) or an f32 reduce-add performed by the memory
-            // system (x += A W^T for Wo / W2 -- no read-modify-write through the SM).  Rows past m_valid add 0.
-            const int rloc = q * 32 + lane;
-#pragma unroll 1
-            for (int c = 0; c < BN / 32; c++) {
-                uint32_t r[32];
-                tmem_ld32(tlane + (uint32_t)(c * 32), r);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                uint8_t *buf = smem + c * (BM * 32 * 4) + rloc * 128;
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    uint4 o = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-                    if (row >= m_valid) o = make_uint4(0u, 0u, 0u, 0u);
-                    *reinterpret_cast<uint4 *>(buf + ((j ^ (rloc & 7)) << 4)) = o;
-                }
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("bar.sync 1, 128;" ::: "memory"); // the four epilogue warps
-            if (warp == 4 && lane == 0) {
-#pragma unroll
-                for (int c = 0; c < BN / 32; c++) {
-                    const uint32_t src = s32(smem + c * (BM * 32 * 4));
-                    if (MODE == GEMM_RESID)
-                        asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(src),
-                                     "r"(n0 + c * 32), "r"(m0)
-                                     : "memory");
-                    else
-                        asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(src), "r"(n0 + c * 32),
-                                     "r"(m0)
-                                     : "memory");
-                }
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN) : "memory");
-}
-
-// =====================================================================================================
-// CTA-pair version: two CTAs of a cluster (the two SMs of a TPC) compute one 256 x BN tile with
-// tcgen05.mma.cta_group::2.  Each CTA loads ITS 128 rows of A and ITS half of the B tile (BN/2 weight rows),
-// so an SM ingests 16 KB + BN/2 * 128 B per 128 x BN x 64 MACs -- twice the arithmetic intensity of the
-// single-CTA kernel at BN = 256 (the 128 x 128 tile is bound by the ~64 B/clk an SM can pull from L2).
-// Protocol (CUTLASS PipelineTmaUmmaAsync, cutlass/pipeline/sm100_pipeline.hpp): both producers issue
-// cta_group::2 TMA loads whose complete_tx lands on the LEADER's full barrier (peer bit cleared); only the
-// leader arms it (expect_tx for both CTAs' bytes), waits on it and issues the MMAs; tcgen05.commit with a
-// multicast mask frees the stage in both CTAs and finally publishes the accumulator (rows 0-127 in the
-// leader's TMEM, 128-255 in the peer's) to both epilogues, which are identical to the single-CTA ones.
-// GEMM_GATEUP: the leader's half of B is BN/2 rows of W1, the peer's half BN/2 rows of W3.
-// =====================================================================================================
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() { // every thread of both CTAs
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap *map, int c0, int c1, uint32_t bar) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst), "l"(map),
-                 "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-                 : "memory");
-}
-__device__ __forceinline__ void umma_f16_2cta(uint32_t tmem_c, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    const uint32_t z = 0u;
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n"
-        "}\n" ::"r"(tmem_c),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(z)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_2cta(uint32_t bar) { // arrives on the barrier at this offset in BOTH CTAs
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
-}
-
-// MT = 256-row pair tiles of M that one CTA pair computes against the SAME B tile (MT x BN TMEM columns): with MT = 2 a
-// 512-token chunk re-uses every weight tile for all its rows, so an SM ingests 32 + BN/4 KB per 2 x 128 x BN x 64 MACs
-// (170 FLOP/B at BN = 256 -- tensor-pipe bound instead of L2-ingest bound) and the fixed prologue/epilogue is paid once.
-template <int BN, int STAGES, int MT> constexpr size_t smem_bytes_2cta() {
-    return (size_t)STAGES * (MT * BM * BK * 2 + (BN / 2) * BK * 2) + (2 * STAGES + 1) * 8 + 16 + 1024;
-}
-
-template <int MODE, int BN, int STAGES, int MT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(256, 1)
-    k_gemm_f16_2cta(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const __grid_constant__ CUtensorMap tma_b2,
-                    const __grid_constant__ CUtensorMap tma_c, void *__restrict__ Cv, int ldc, int m_valid, int K, int kb_per_split) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    constexpr int A1_BYTES = BM * BK * 2, A_BYTES = MT * A1_BYTES, B_BYTES = (BN / 2) * BK * 2; // per CTA and stage
-    constexpr int TCOLS = MT * BN;
-    static_assert(TCOLS == 128 || TCOLS == 256 || TCOLS == 512, "TMEM allocations are powers of two");
-    static_assert(STAGES * (A_BYTES + B_BYTES) >= BM * BN * 4, "the C tile is staged in the operand ring");
-    uint8_t *sA = smem, *sB = smem + STAGES * A_BYTES;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + STAGES * B_BYTES);
-    const uint32_t full0 = s32(bars), empty0 = s32(bars + STAGES), tmem_full = s32(bars + 2 * STAGES);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * STAGES + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-        mbar_init(tmem_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) { // the same warp of both CTAs allocates the pair's accumulator columns
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(tmem_slot)), "r"((uint32_t)TCOLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    cluster_sync_all(); // barriers of both CTAs initialised before any remote complete_tx / commit can land
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-    // split-K (GEMM_RESID only: every split reduce-adds its partial product into x): blockIdx.z owns k-blocks [kb0, kb0 + nk)
     const int nk_all = (K + BK - 1) / BK, kb0 = blockIdx.z * kb_per_split;
     const int nk = nk_all - kb0 < kb_per_split ? nk_all - kb0 : kb_per_split;
-    // rows of this CTA in pair tile mt: m_base + mt * 256 + rank * 128 .. + 127
-    const int m_base = (int)(blockIdx.x >> 1) * (MT * 2 * BM) + (int)rank * BM;
+    const int m0 = blockIdx.x * BM;
     const int n0 = blockIdx.y * (MODE == GEMM_GATEUP ? BN / 2 : BN);
 
-    if (warp == 0 && lane == 0) {
-        // ===== TMA producer (both CTAs): own A rows of every pair tile, own half of the B tile =====
-        const CUtensorMap *bmap = (MODE == GEMM_GATEUP && rank == 1) ? &tma_b2 : &tma_b;
-        const int brow = MODE == GEMM_GATEUP ? n0 : n0 + (int)rank * (BN / 2);
-        for (int kb = 0; kb < nk; kb++) {
-            const int st = kb % STAGES;
-            mbar_wait(empty0 + 8 * st, ((kb / STAGES) & 1) ^ 1);
-            if (rank == 0) mbar_expect_tx(full0 + 8 * st, 2 * (A_BYTES + B_BYTES));
-#pragma unroll
-            for (int mt = 0; mt < MT; mt++)
-                tma_load_2d_2sm(s32(sA + st * A_BYTES + mt * A1_BYTES), &tma_a, (kb0 + kb) * BK, m_base + mt * 2 * BM, full0 + 8 * st);
-            tma_load_2d_2sm(s32(sB + st * B_BYTES), bmap, (kb0 + kb) * BK, brow, full0 + 8 * st);
-        }
-    } else if (warp == 1 && lane == 0 && rank == 0) {
-        // ===== MMA issuer: one thread of the leader CTA drives both SMs' tensor cores =====
-        constexpr uint32_t idesc = umma_idesc_f16(2 * BM, BN);
-        for (int kb = 0; kb < nk; kb++) {
-            const int st = kb % STAGES;
-            mbar_wait(full0 + 8 * st, (kb / STAGES) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint64_t db = umma_desc_sw128(s32(sB + st * B_BYTES));
-#pragma unroll
-            for (int mt = 0; mt < MT; mt++) {
-                const uint64_t da = umma_desc_sw128(s32(sA + st * A_BYTES + mt * A1_BYTES));
-#pragma unroll
-                for (int k = 0; k < BK / 16; k++) umma_f16_2cta(tmem_base + (uint32_t)(mt * BN), da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            }
-            umma_commit_2cta(empty0 + 8 * st);
-        }
-        umma_commit_2cta(tmem_full);
-    }
-    __syncwarp(); // the elected producer / MMA lanes rejoin their warps
-    {
-        // ===== epilogue (both CTAs, own 128 rows of each pair tile): all 8 warps -- warp w reads TMEM lanes 32*(w%4).., warps 0-3
-        // take the first half of the columns and warps 4-7 the second =====
-        mbar_wait(tmem_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int q = warp & 3, half = warp >> 2;
-#pragma unroll 1
-        for (int mt = 0; mt < MT; mt++) {
-            const int m0 = m_base + mt * 2 * BM;
-            const int row = m0 + q * 32 + lane;
-            const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * BN);
-            if (MODE == GEMM_GATEUP) {
-                __half *C = reinterpret_cast<__half *>(Cv);
-#pragma unroll 1
-                for (int c0 = half * (BN / 4); c0 < (half + 1) * (BN / 4); c0 += 32) {
-                    uint32_t g[32], u[32];
-                    tmem_ld32(tlane + (uint32_t)c0, g);
-                    tmem_ld32(tlane + (uint32_t)(BN / 2 + c0), u);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    if (row < m_valid) {
-                        uint4 *dst = reinterpret_cast<uint4 *>(C + (size_t)row * ldc + n0 + c0);
-#pragma unroll
-                        for (int v = 0; v < 4; v++) {
-                            uint32_t w[4];
-#pragma unroll
-                            for (int e = 0; e < 4; e++) {
-                                const float g0 = __uint_as_float(g[8 * v + 2 * e]), g1 = __uint_as_float(g[8 * v + 2 * e + 1]);
-                                const float h0 = (g0 / (1.0f + expf(-g0))) * __uint_as_float(u[8 * v + 2 * e]);
-                                const float h1 = (g1 / (1.0f + expf(-g1))) * __uint_as_float(u[8 * v + 2 * e + 1]);
-                                const __half2 hh = __floats2half2_rn(h0, h1);
-                                w[e] = *reinterpret_cast<const uint32_t *>(&hh);
-                            }
-                            dst[v] = make_uint4(w[0], w[1], w[2], w[3]);
-                        }
-                    }
-                }
-            } else {
-                if (m0 >= m_valid) break; // CTA-uniform: nothing of this (and any later) pair tile is stored
-                const int rloc = q * 32 + lane;
-#pragma unroll 1
-                for (int c = half * (BN / 64); c < (half + 1) * (BN / 64); c++) {
-                    uint32_t r[32];
-                    tmem_ld32(tlane + (uint32_t)(c * 32), r);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    uint8_t *buf = smem + c * (BM * 32 * 4) + rloc * 128;
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        uint4 o = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-                        if (row >= m_valid) o = make_uint4(0u, 0u, 0u, 0u);
-                        *reinterpret_cast<uint4 *>(buf + ((j ^ (rloc & 7)) << 4)) = o;
-                    }
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncthreads();
-                if (threadIdx.x == 0) {
-#pragma unroll
-                    for (int c = 0; c < BN / 32; c++) {
-                        const uint32_t src = s32(smem + c * (BM * 32 * 4));
-                        if (MODE == GEMM_RESID)
-                            asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(src),
-                                         "r"(n0 + c * 32), "r"(m0)
-                                         : "memory");
-                        else
-                            asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(src),
-                                         "r"(n0 + c * 32), "r"(m0)
-                                         : "memory");
-                    }
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); // also frees the staging buffer for the next pair tile
-                }
-                if (MT > 1) __syncthreads();
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    cluster_sync_all(); // neither CTA may exit (or free TMEM) while the pair can still touch its shared memory / TMEM
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TCOLS) : "memory");
-}
-
-// =====================================================================================================
-// The CTA-pair GEMM as a PERSISTENT kernel (default for the QKV and gate/up GEMMs since round 2; B200_GEMM_PERSIST=0 disables).  One cluster per TPC walks tiles t = cluster + i * clusters (M pair tiles fastest, so neighbouring
-// clusters share a weight tile in L2); the accumulator is double buffered in TMEM (2 x BN columns), so while the four
-// epilogue warps drain tile i the MMA thread already accumulates tile i+1 and the producers are loading tile i+2 --
-// prologue, pipeline fill and epilogue no longer sit on the critical path of every tile (they are ~25 % of a K = 4096 tile
-// in k_gemm_f16_2cta).  New synchronisation relative to the non-persistent kernel: tmem_full[2] (leader MMA -> both
-// epilogues, multicast commit) and tmem_empty[2] on the LEADER (count 8 = 4 epilogue warps x 2 CTAs, remote
-// mbarrier.arrive through the cluster window), plus two 16 KB C staging buffers of their own (the operand ring is busy).
-// =====================================================================================================
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar) { // arrive on the barrier at this offset in the pair's even CTA
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar & 0xFEFFFFFFu) : "memory");
-}
-
-template <int BN, int STAGES> constexpr size_t smem_bytes_2cta_persist() {
-    return (size_t)STAGES * (BM * BK * 2 + (BN / 2) * BK * 2) + 2 * (BM * 32 * 4) + (2 * STAGES + 4) * 8 + 16 + 1024;
-}
-
-template <int MODE, int BN, int STAGES>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(256, 1)
-    k_gemm_f16_2cta_persist(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const __grid_constant__ CUtensorMap tma_b2,
-                            const __grid_constant__ CUtensorMap tma_c, void *__restrict__ Cv, int ldc, int m_valid, int K, int m_pairs, int n_tiles, int splits) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    constexpr int A_BYTES = BM * BK * 2, B_BYTES = (BN / 2) * BK * 2, CST_BYTES = BM * 32 * 4;
-    static_assert(2 * BN <= 512, "two accumulators must fit the 512 TMEM columns");
-    uint8_t *sA = smem, *sB = smem + STAGES * A_BYTES, *sC = sB + STAGES * B_BYTES; // sC: two staging buffers, 1024-byte aligned
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sC + 2 * CST_BYTES);
-    const uint32_t full0 = s32(bars), empty0 = s32(bars + STAGES), tfull0 = s32(bars + 2 * STAGES), tempty0 = s32(bars + 2 * STAGES + 2);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * STAGES + 4);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-        for (int b = 0; b < 2; b++) { mbar_init(tfull0 + 8 * b, 1); mbar_init(tempty0 + 8 * b, 8); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(tmem_slot)), "r"((uint32_t)(2 * BN)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    cluster_sync_all();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-    // split-K (GEMM_RESID only: every split reduce-adds its partial product): a work item is (pair tile, k-range); items of one tile are
-    // adjacent in the walk so the B tile of neighbouring clusters differs only in k
-    const int nk_all = (K + BK - 1) / BK, nk_split = (nk_all + splits - 1) / splits;
-    const int n_clusters = (int)(gridDim.x >> 1), cid = (int)(blockIdx.x >> 1), total = m_pairs * n_tiles * splits;
-
-    if (warp == 0 && lane == 0) {
-        // ===== TMA producer (both CTAs) =====
-        const CUtensorMap *bmap = (MODE == GEMM_GATEUP && rank == 1) ? &tma_b2 : &tma_b;
-        int it = 0; // running k-block counter across tiles: the ring never drains between tiles
-        for (int t = cid; t < total; t += n_clusters) {
-            const int ks = t % splits, tt = t / splits;
-            const int mp = tt % m_pairs, nt = tt / m_pairs;
-            const int m0 = mp * 2 * BM + (int)rank * BM;
-            const int n0 = nt * (MODE == GEMM_GATEUP ? BN / 2 : BN);
-            const int brow = MODE == GEMM_GATEUP ? n0 : n0 + (int)rank * (BN / 2);
-            const int kb0 = ks * nk_split, nk = min(nk_split, nk_all - kb0);
-            for (int kb = 0; kb < nk; kb++, it++) {
-                const int st = it % STAGES;
-                mbar_wait(empty0 + 8 * st, ((it / STAGES) & 1) ^ 1);
-                if (rank == 0) mbar_expect_tx(full0 + 8 * st, 2 * (A_BYTES + B_BYTES));
-                tma_load_2d_2sm(s32(sA + st * A_BYTES), &tma_a, (kb0 + kb) * BK, m0, full0 + 8 * st);
-                tma_load_2d_2sm(s32(sB + st * B_BYTES), bmap, (kb0 + kb) * BK, brow, full0 + 8 * st);
-            }
-        }
-    } else if (warp == 1 && lane == 0 && rank == 0) {
-        // ===== MMA issuer (leader): accumulator buffer i & 1 =====
-        constexpr uint32_t idesc = umma_idesc_f16(2 * BM, BN);
-        int it = 0, i = 0;
-        for (int t = cid; t < total; t += n_clusters, i++) {
-            const int buf = i & 1;
-            const int kb0 = (t % splits) * nk_split, nk = min(nk_split, nk_all - kb0);
-            mbar_wait(tempty0 + 8 * buf, ((i >> 1) & 1) ^ 1); // both CTAs' epilogues have drained this buffer (first two uses pass at once)
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            for (int kb = 0; kb < nk; kb++, it++) {
-                const int st = it % STAGES;
-                mbar_wait(full0 + 8 * st, (it / STAGES) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint64_t da = umma_desc_sw128(s32(sA + st * A_BYTES)), db = umma_desc_sw128(s32(sB + st * B_BYTES));
-#pragma unroll
-                for (int k = 0; k < BK / 16; k++) umma_f16_2cta(tmem_base + (uint32_t)(buf * BN), da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-                umma_commit_2cta(empty0 + 8 * st);
-            }
-            umma_commit_2cta(tfull0 + 8 * buf);
-        }
-    } else if (warp >= 4) {
-        // ===== epilogue (both CTAs): four warps, warp w owns TMEM lanes 32 * (w - 4) =====
-        const int q = warp & 3, et = threadIdx.x - 128; // et: 0..127 within the epilogue group
-        int i = 0, chunk = 0;                         // chunk: running count of staged 32-column chunks (staging buffer = chunk & 1)
-        for (int t = cid; t < total; t += n_clusters, i++) {
-            const int buf = i & 1;
-            const int tt = t / splits;
-            const int mp = tt % m_pairs, nt = tt / m_pairs;
-            const int m0 = mp * 2 * BM + (int)rank * BM;
-            const int n0 = nt * (MODE == GEMM_GATEUP ? BN / 2 : BN);
-            const int row = m0 + q * 32 + lane;
-            mbar_wait(tfull0 + 8 * buf, (i >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN);
-            if (MODE == GEMM_GATEUP) {
-                __half *C = reinterpret_cast<__half *>(Cv);
-#pragma unroll 1
-                for (int c0 = 0; c0 < BN / 2; c0 += 32) {
-                    uint32_t g[32], u[32];
-                    tmem_ld32(tlane + (uint32_t)c0, g);
-                    tmem_ld32(tlane + (uint32_t)(BN / 2 + c0), u);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    if (c0 + 32 >= BN / 2) { // last TMEM read of this tile: hand the accumulator back before the (slow) stores
-                        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_leader(tempty0 + 8 * buf);
-                    }
-                    if (row < m_valid) {
-                        uint4 *dst = reinterpret_cast<uint4 *>(C + (size_t)row * ldc + n0 + c0);
-#pragma unroll
-                        for (int v = 0; v < 4; v++) {
-                            uint32_t w[4];
-#pragma unroll
-                            for (int e = 0; e < 4; e++) {
-                                const float g0 = __uint_as_float(g[8 * v + 2 * e]), g1 = __uint_as_float(g[8 * v + 2 * e + 1]);
-                                const float h0 = (g0 / (1.0f + expf(-g0))) * __uint_as_float(u[8 * v + 2 * e]);
-                                const float h1 = (g1 / (1.0f + expf(-g1))) * __uint_as_float(u[8 * v + 2 * e + 1]);
-                                const __half2 hh = __floats2half2_rn(h0, h1);
-                                w[e] = *reinterpret_cast<const uint32_t *>(&hh);
-                            }
-                            dst[v] = make_uint4(w[0], w[1], w[2], w[3]);
-                        }
-                    }
-                }
-            } else {
-                const int rloc = q * 32 + lane;
-#pragma unroll 1
-                for (int c = 0; c < BN / 32; c++, chunk++) {
-                    uint32_t r[32];
-                    tmem_ld32(tlane + (uint32_t)(c * 32), r);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                    if (c == BN / 32 - 1) {
-                        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_leader(tempty0 + 8 * buf);
-                    }
-                    uint8_t *cst = sC + (chunk & 1) * CST_BYTES;
-                    if (et == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); // the store that used this buffer two chunks ago has read it
-                    asm volatile("bar.sync 2, 128;" ::: "memory");
-                    uint8_t *dstp = cst + rloc * 128;
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        uint4 o = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-                        if (row >= m_valid) o = make_uint4(0u, 0u, 0u, 0u);
-                        *reinterpret_cast<uint4 *>(dstp + ((j ^ (rloc & 7)) << 4)) = o;
-                    }
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    asm volatile("bar.sync 2, 128;" ::: "memory");
-                    if (et == 0) {
-                        if (MODE == GEMM_RESID)
-                            asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(s32(cst)),
-                                         "r"(n0 + c * 32), "r"(m0)
-                                         : "memory");
-                        else
-                            asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(s32(cst)),
-                                         "r"(n0 + c * 32), "r"(m0)
-                                         : "memory");
-                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                    }
+    if (wg == 0) {
+        // ===== TMA producer =====
+        if (warp == 0 && lane == 0) {
+            for (int kb = 0; kb < nk; kb++) {
+                const int st = kb % STAGES;
+                mbar_wait(empty0 + 8 * st, ((kb / STAGES) & 1) ^ 1);
+                mbar_expect_tx(full0 + 8 * st, A_BYTES + B_BYTES);
+                const int kc = (kb0 + kb) * BK;
+                tma_load_2d(s32(sA + st * A_BYTES), &tma_a, kc, m0, full0 + 8 * st);
+                if (MODE == GEMM_GATEUP) {
+                    tma_load_2d(s32(sB + st * B_BYTES), &tma_b, kc, n0, full0 + 8 * st);
+                    tma_load_2d(s32(sB + st * B_BYTES + B_BYTES / 2), &tma_b2, kc, n0, full0 + 8 * st);
+                } else {
+                    tma_load_2d(s32(sB + st * B_BYTES), &tma_b, kc, n0, full0 + 8 * st);
                 }
             }
         }
-        if (et == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+        return; // the producer warp group takes no part in the epilogue (named barrier 1 counts the 256 consumer threads)
     }
-    __syncwarp(); // the elected producer / MMA / store lanes rejoin their warps before the aligned cluster barrier
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    cluster_sync_all();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN)) : "memory");
+
+    // ===== consumers: warp group c = wg - 1 owns tile rows 64c .. 64c+63 =====
+    const int c = wg - 1, t = threadIdx.x & 127;
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; i++) acc[i] = 0.0f;
+    int prev = -1;
+    for (int kb = 0; kb < nk; kb++) {
+        const int st = kb % STAGES;
+        mbar_wait(full0 + 8 * st, (kb / STAGES) & 1);
+        asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+        const uint64_t da = wgmma_desc_sw128(s32(sA + st * A_BYTES + c * (64 * 128))), db = wgmma_desc_sw128(s32(sB + st * B_BYTES));
+#pragma unroll
+        for (int k = 0; k < BK / 16; k++) // K step of 16 fp16 = 32 bytes = +2 in the (addr >> 4) field, inside the 128-byte swizzle atom
+            wgmma_m64n128k16(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
+        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+        asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); // the previous stage's wgmmas are done: hand it back
+        if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
+        prev = st;
+    }
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+
+    const int r_lo = c * 64 + (t >> 5) * 16 + ((t & 31) >> 2); // tile row of acc[4j], acc[4j+1]; acc[4j+2], acc[4j+3] are row r_lo + 8
+    const int cq = 2 * (t & 3);                                 // column offset inside each 8-column group
+    if (MODE == GEMM_GATEUP) {
+        __half *C = reinterpret_cast<__half *>(Cv);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int row = m0 + r_lo + 8 * h;
+            if (row < m_valid) {
+                __half2 *dst = reinterpret_cast<__half2 *>(C + (size_t)row * ldc + n0 + cq);
+#pragma unroll
+                for (int j = 0; j < 8; j++) { // gate column 8j + cq (+1) sits in acc[4j + 2h (+1)], its up partner 64 columns on in acc[32 + ...]
+                    const float g0 = acc[4 * j + 2 * h], g1 = acc[4 * j + 2 * h + 1];
+                    const float h0 = (g0 / (1.0f + expf(-g0))) * acc[32 + 4 * j + 2 * h];
+                    const float h1 = (g1 / (1.0f + expf(-g1))) * acc[32 + 4 * j + 2 * h + 1];
+                    dst[4 * j] = __floats2half2_rn(h0, h1);
+                }
+            }
+        }
+    } else {
+        // FP32 tile -> shared memory (the ring is idle once BOTH consumer warp groups have finished their wgmmas: every
+        // TMA load has landed and been read) in the SWIZZLE_128B layout of the C tensor map: four 128 x 32 boxes, row r of
+        // box b at b * 16 KB + 128 r, 16-byte chunk q at (q ^ (r & 7)) << 4.  Then ONE thread hands the boxes to TMA: a plain
+        // tensor store (QKV) or an f32 reduce-add performed by the memory system (x += A W^T for Wo / W2 -- no
+        // read-modify-write through the SM, and split-K partials add up).  Rows past m_valid store / add 0.
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int rloc = r_lo + 8 * h;
+            const bool live = m0 + rloc < m_valid;
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const int col = 8 * j + cq, b = col >> 5, q = (col & 31) >> 2;
+                const float2 o = live ? make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]) : make_float2(0.0f, 0.0f);
+                *reinterpret_cast<float2 *>(smem + b * (BM * 32 * 4) + rloc * 128 + ((q ^ (rloc & 7)) << 4) + (col & 3) * 4) = o;
+            }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (t == 0 && c == 0) {
+#pragma unroll
+            for (int b = 0; b < BN / 32; b++) {
+                const uint32_t src = s32(smem + b * (BM * 32 * 4));
+                if (MODE == GEMM_RESID)
+                    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(src),
+                                 "r"(n0 + b * 32), "r"(m0)
+                                 : "memory");
+                else
+                    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(src), "r"(n0 + b * 32),
+                                 "r"(m0)
+                                 : "memory");
+            }
+            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+        }
+    }
 }
 
 // ---- host side ----
@@ -632,102 +244,39 @@ inline int make_map_c(CUtensorMap *map, const void *base, uint64_t rows, uint64_
     return r == CUDA_SUCCESS ? 0 : -2;
 }
 
+// 4 stages x 32 KB of operands: the default ring (the C tile, 64 KB, is staged in it).  6 stages (192 KB) is the deep
+// variant the GEMM test also runs, so a ring that wraps at a different k-block is exercised too.
+constexpr int GEMM_STAGES = 4, GEMM_STAGES_DEEP = 6;
+
+// m_tiles x n_tiles output tiles, K split into `splits` ranges (GEMM_RESID only: every split reduce-adds its partial product).
+// B maps have box rows BN (BN / 2 for the W1 / W3 maps of GEMM_GATEUP).
 template <int MODE, int STAGES>
 inline int gemm_launch(const CUtensorMap &a, const CUtensorMap &b, const CUtensorMap &b2, const CUtensorMap &c, void *C, int ldc, int m_valid, int m_tiles,
-                       int n_tiles, int K, cudaStream_t stream) {
+                       int n_tiles, int K, cudaStream_t stream, int splits = 1) {
     static bool attr = false; // one flag per instantiation
     if (!attr) {
-        if (cudaFuncSetAttribute(k_gemm_f16_tcgen05<MODE, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<STAGES>()) != cudaSuccess) return -4;
+        if (cudaFuncSetAttribute(k_gemm_f16_wgmma<MODE, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<STAGES>()) != cudaSuccess) return -4;
         attr = true;
     }
-    k_gemm_f16_tcgen05<MODE, STAGES><<<dim3(m_tiles, n_tiles), 256, smem_bytes<STAGES>(), stream>>>(a, b, b2, c, C, ldc, m_valid, K);
-    return cudaGetLastError() == cudaSuccess ? 0 : -5;
-}
-
-// m_tiles = 128-row tiles of M, a multiple of 2 * MT (M padded to MT * 256).  B maps must have box rows = BN / 2.
-template <int MODE, int BN, int STAGES, int MT = 1>
-inline int gemm2_launch(const CUtensorMap &a, const CUtensorMap &b, const CUtensorMap &b2, const CUtensorMap &c, void *C, int ldc, int m_valid, int m_tiles,
-                        int n_tiles, int K, cudaStream_t stream, int splits = 1) {
-    static bool attr = false;
-    if (!attr) {
-        if (cudaFuncSetAttribute(k_gemm_f16_2cta<MODE, BN, STAGES, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes_2cta<BN, STAGES, MT>()) != cudaSuccess)
-            return -4;
-        attr = true;
-    }
-    if (m_tiles % (2 * MT) || splits < 1 || (splits > 1 && MODE != GEMM_RESID)) return -6;
+    if (splits < 1 || (splits > 1 && MODE != GEMM_RESID)) return -6;
     const int nk = (K + BK - 1) / BK, per = (nk + splits - 1) / splits;
-    if ((splits - 1) * per >= nk) return -6; // an empty split would publish an unwritten accumulator
-    k_gemm_f16_2cta<MODE, BN, STAGES, MT><<<dim3(m_tiles / MT, n_tiles, splits), 256, smem_bytes_2cta<BN, STAGES, MT>(), stream>>>(a, b, b2, c, C, ldc, m_valid, K, per);
+    if ((splits - 1) * per >= nk) return -6; // an empty split would store an unwritten accumulator
+    k_gemm_f16_wgmma<MODE, STAGES><<<dim3(m_tiles, n_tiles, splits), GEMM_THREADS, smem_bytes<STAGES>(), stream>>>(a, b, b2, c, C, ldc, m_valid, K, per);
     return cudaGetLastError() == cudaSuccess ? 0 : -5;
 }
-constexpr int GEMM2_STAGES_256 = 6, GEMM2_STAGES_128 = 8; // 192 KB of operand ring per CTA either way
-constexpr int GEMM2_STAGES_256_M2 = 4;                    // 4 x (32 KB of A + 16 KB of B)
-
-// Persistent variant (round-2 candidate).  n_sms: SMs of the device; the grid is the largest even number of CTAs <= n_sms.
-template <int MODE, int BN, int STAGES>
-inline int gemm2_persist_launch(const CUtensorMap &a, const CUtensorMap &b, const CUtensorMap &b2, const CUtensorMap &c, void *C, int ldc, int m_valid, int m_tiles,
-                                int n_tiles, int K, int n_sms, cudaStream_t stream, int splits = 1) {
-    static bool attr = false;
-    if (!attr) {
-        if (cudaFuncSetAttribute(k_gemm_f16_2cta_persist<MODE, BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes_2cta_persist<BN, STAGES>()) !=
-            cudaSuccess)
-            return -4;
-        attr = true;
-    }
-    if (m_tiles & 1 || splits < 1 || (splits > 1 && MODE != GEMM_RESID)) return -6;
-    {
-        const int nk = (K + BK - 1) / BK, per = (nk + splits - 1) / splits;
-        if ((splits - 1) * per >= nk) return -6; // an empty split would publish an unwritten accumulator
-    }
-    const int m_pairs = m_tiles / 2, total = m_pairs * n_tiles * splits;
-    int clusters = n_sms / 2;
-    if (clusters > total) clusters = total;
-    if (clusters < 1) return -6;
-    k_gemm_f16_2cta_persist<MODE, BN, STAGES><<<dim3(2 * clusters), 256, smem_bytes_2cta_persist<BN, STAGES>(), stream>>>(a, b, b2, c, C, ldc, m_valid, K, m_pairs, n_tiles, splits);
-    return cudaGetLastError() == cudaSuccess ? 0 : -5;
-}
-constexpr int GEMM2_PERSIST_STAGES_256 = 5; // 5 x 32 KB of operands + 2 x 16 KB of C staging
-
-// 3 stages of 32 KB: two CTAs fit one SM (2 x 99 KB shared memory, 2 x 128 TMEM columns), so one CTA's
-// epilogue overlaps the other's main loop.
-constexpr int GEMM_STAGES = 3, GEMM_STAGES_DEEP = 6;
 
 // Test/measurement entry: C[M,N] (+)= A[M,K] * B[N,K]^T ; M, N multiples of 128, K multiple of 64.  Device pointers.
-inline int gemm_f16(const __half *A, const __half *B, float *C, int M, int N, int K, int stages, int resid, int two_cta, cudaStream_t stream) {
+// resid > 0: reduce-add into C with K split resid ways.
+inline int gemm_f16(const __half *A, const __half *B, float *C, int M, int N, int K, int stages, int resid, cudaStream_t stream) {
     if (M % BM || N % BN || K % BK) return -3;
     CUtensorMap ma, mb, mc;
     int rc;
-    if (two_cta) { // two_cta = pair-tile width (256 or 128)
-        const int bn = (two_cta == 512 || two_cta == 1256) ? 256 : two_cta;
-        if (M % 256 || N % bn) return -3;
-        if ((rc = make_map(&ma, A, (uint64_t)M, (uint64_t)K, BM))) return rc;
-        if ((rc = make_map(&mb, B, (uint64_t)N, (uint64_t)K, bn / 2))) return rc;
-        if ((rc = make_map_c(&mc, C, (uint64_t)M, (uint64_t)N))) return rc;
-        if (two_cta == 1256) { // persistent CTA-pair kernel, 256-wide pair tiles (round-2 candidate)
-            int dev = 0, sms = 148;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-            return resid ? gemm2_persist_launch<GEMM_RESID, 256, GEMM2_PERSIST_STAGES_256>(ma, mb, mb, mc, C, N, M, M / BM, N / 256, K, sms, stream, resid)
-                         : gemm2_persist_launch<GEMM_F32, 256, GEMM2_PERSIST_STAGES_256>(ma, mb, mb, mc, C, N, M, M / BM, N / 256, K, sms, stream);
-        }
-        if (two_cta == 512) { // 256-wide pair tiles, two of them (512 rows) per CTA pair
-            if (M % 512) return -3;
-            return resid ? gemm2_launch<GEMM_RESID, 256, GEMM2_STAGES_256_M2, 2>(ma, mb, mb, mc, C, N, M, M / BM, N / 256, K, stream, resid)
-                         : gemm2_launch<GEMM_F32, 256, GEMM2_STAGES_256_M2, 2>(ma, mb, mb, mc, C, N, M, M / BM, N / 256, K, stream);
-        }
-        if (two_cta == 256)
-            return resid ? gemm2_launch<GEMM_RESID, 256, GEMM2_STAGES_256>(ma, mb, mb, mc, C, N, M, M / BM, N / 256, K, stream, resid)
-                         : gemm2_launch<GEMM_F32, 256, GEMM2_STAGES_256>(ma, mb, mb, mc, C, N, M, M / BM, N / 256, K, stream);
-        return resid ? gemm2_launch<GEMM_RESID, 128, GEMM2_STAGES_128>(ma, mb, mb, mc, C, N, M, M / BM, N / 128, K, stream)
-                     : gemm2_launch<GEMM_F32, 128, GEMM2_STAGES_128>(ma, mb, mb, mc, C, N, M, M / BM, N / 128, K, stream);
-    }
     if ((rc = make_map(&ma, A, (uint64_t)M, (uint64_t)K, BM))) return rc;
     if ((rc = make_map(&mb, B, (uint64_t)N, (uint64_t)K, BN))) return rc;
     if ((rc = make_map_c(&mc, C, (uint64_t)M, (uint64_t)N))) return rc;
-    if (resid && stages == 6) return gemm_launch<GEMM_RESID, 6>(ma, mb, mb, mc, C, N, M, M / BM, N / BN, K, stream);
-    if (resid) return gemm_launch<GEMM_RESID, GEMM_STAGES>(ma, mb, mb, mc, C, N, M, M / BM, N / BN, K, stream);
-    if (stages == 4) return gemm_launch<GEMM_F32, 4>(ma, mb, mb, mc, C, N, M, M / BM, N / BN, K, stream);
-    if (stages == 6) return gemm_launch<GEMM_F32, 6>(ma, mb, mb, mc, C, N, M, M / BM, N / BN, K, stream);
+    if (resid && stages == GEMM_STAGES_DEEP) return gemm_launch<GEMM_RESID, GEMM_STAGES_DEEP>(ma, mb, mb, mc, C, N, M, M / BM, N / BN, K, stream, resid);
+    if (resid) return gemm_launch<GEMM_RESID, GEMM_STAGES>(ma, mb, mb, mc, C, N, M, M / BM, N / BN, K, stream, resid);
+    if (stages == GEMM_STAGES_DEEP) return gemm_launch<GEMM_F32, GEMM_STAGES_DEEP>(ma, mb, mb, mc, C, N, M, M / BM, N / BN, K, stream);
     return gemm_launch<GEMM_F32, GEMM_STAGES>(ma, mb, mb, mc, C, N, M, M / BM, N / BN, K, stream);
 }
 

@@ -1,5 +1,5 @@
 // stream_matvec.cuh -- the decode hot kernel: Q8_0 dequant-matvec as a persistent, TMA-fed
-// weight stream (sm_100a).
+// weight stream (sm_90a).
 //
 // One CTA per SM.  A single producer thread walks this CTA's static slice of the weight matrix
 // and keeps a ring of shared-memory stages full with 1-D bulk async copies
@@ -96,7 +96,7 @@ __device__ __forceinline__ void bulk_g2s(unsigned dst, const void *src, unsigned
                  : "memory");
 }
 // The same copy with an L2 evict_first policy: single-use weight tiles must not push the KV rows, activations and norm weights out of L2
-// (measured on the persistent kernel: +6 % tokens/s, profiles/r2_run6_evict_first_qwen3.log).
+// (it made the persistent kernel faster where it was measured).
 __device__ __forceinline__ unsigned long long l2_policy_evict_first() {
     unsigned long long pol;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));

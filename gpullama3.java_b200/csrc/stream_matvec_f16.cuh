@@ -13,8 +13,8 @@
 // Lane mapping: a lane owns the chain PAIR (2u, 2u+1) of one row, so one 32-bit shared load delivers both weights as a half2 and one
 // 64-bit load both activations; L/2 lanes cover a row and a warp works on 64/L rows at once (4 for the 16-lane species).  The subnormal
 // flush is ONE packed instruction per pair: add.ftz.f16x2 w, -0 (x + -0 = x exactly for every other value; .ftz flushes subnormal
-// inputs to sign-preserving zero) -- 3.5 instructions per weight instead of the 10 of the integer-arithmetic widening (measured v1:
-// 3.0 TB/s on the 1 GB classifier, issue-bound; profiles/r2_run8_f16_stream_kquants.log).  The rows of a stage are SF_ROW_PAD bytes
+// inputs to sign-preserving zero) -- 3.5 instructions per weight instead of the 10 of the integer-arithmetic widening (v1 of the
+// kernel was issue-bound).  The rows of a stage are SF_ROW_PAD bytes
 // apart modulo 128 so the row groups of a warp hit different banks.
 //   SF_GATEUP: half of the warp's row slots are ffn_gate rows, the other half the same rows of ffn_up; SwiGLU (InferenceCore.java:150-158)
 //   is applied in the epilogue, so w1, w3 and the SwiGLU kernel of the round-1 FP16 graph collapse into one launch.

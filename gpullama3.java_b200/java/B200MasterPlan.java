@@ -113,7 +113,7 @@ public final class B200MasterPlan implements AutoCloseable {
     private static void check(int rc, String msg) {
         if (rc == 0) return;
         if (rc == -2) throw new UnsupportedOperationException(msg);            // ForwardPlanFactory.java:84-87
-        if (rc == -3) throw new OutOfMemoryError("B200 device memory: " + msg); // README.md:262-265
+        if (rc == -3) throw new OutOfMemoryError("device memory: " + msg); // README.md:262-265
         throw new IllegalStateException("b200llama error " + rc + ": " + msg);
     }
 
@@ -163,7 +163,7 @@ public final class B200MasterPlan implements AutoCloseable {
         if (rc != 0) check(rc, lastError());
     }
 
-    /** TensorCoreSupport.java's switch: 0 = exact token-by-token prefill (bit-identical KV cache), 1 = TMA + tcgen05 GEMMs. */
+    /** TensorCoreSupport.java's switch: 0 = exact token-by-token prefill (bit-identical KV cache), 1 = TMA + wgmma GEMMs. */
     public void setPrefillMode(int mode) throws Throwable {
         int rc = (int) SET_PREFILL_MODE.invokeExact(plan, mode);
         if (rc != 0) check(rc, lastError());

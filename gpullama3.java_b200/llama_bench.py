@@ -105,7 +105,7 @@ def bench_model(plan, vocab: int, tests: list[TestSpec], reps: int = 5, warmup: 
     return out
 
 
-def to_markdown(results: list[Result], model: str, quant: str, backend: str = "B200 sm_100a") -> str:
+def to_markdown(results: list[Result], model: str, quant: str, backend: str = "H100 sm_90a") -> str:
     lines = ["| model | quant | backend | test | t/s |", "| --- | --- | --- | ---: | ---: |"]
     for r in results:
         lines.append(f"| {model} | {quant} | {backend} | {r.test} | {r.avg_ts:.2f} ± {r.stddev_ts:.2f} |")

@@ -145,7 +145,7 @@ def load_model(path: str, context_length: int = -1) -> Model:
             int(md.get("phi3.attention.head_count_kv", n_heads)), dim // n_heads, int(vocab), model_ctx if context_length < 0 else context_length,
             float(md.get("phi3.attention.layer_norm_rms_epsilon", 1e-5)), float(md.get("phi3.rope.freq_base", 10000.0)))
     else:
-        raise UnsupportedModel(f"model type {typ} is outside the B200 hot-path scope (Llama / Mistral / Qwen3 / Phi-3 forward passes only)")
+        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 forward passes only)")
     return Model(g, cfg, typ)
 
 

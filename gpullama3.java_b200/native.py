@@ -122,7 +122,7 @@ def requant_kquant(ggml_type: int, raw, n_elems: int) -> np.ndarray:
 
 
 def gemm_f16(a, b, iters: int = 0):
-    """C = A @ B.T on the tcgen05 prefill GEMM (A [m,k], B [n,k] float16) -> (C float32, ms per launch or None)."""
+    """C = A @ B.T on the wgmma prefill GEMM (A [m,k], B [n,k] float16) -> (C float32, ms per launch or None)."""
     a = np.ascontiguousarray(a, dtype=np.float16)
     b = np.ascontiguousarray(b, dtype=np.float16)
     m, k = a.shape

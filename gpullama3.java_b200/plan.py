@@ -120,7 +120,7 @@ class B200MasterPlan:
     PREFILL_EXACT, PREFILL_TENSOR_CORE = 0, 1
 
     def set_prefill_mode(self, mode):
-        """"exact" (token-by-token graph, bit-identical KV cache) or "tensor_core" (tcgen05 GEMMs, FP16 tolerance)."""
+        """"exact" (token-by-token graph, bit-identical KV cache) or "tensor_core" (wgmma GEMMs, FP16 tolerance)."""
         if isinstance(mode, str):
             mode = {"exact": 0, "tensor_core": 1}[mode]
         self._native.set_prefill_mode(int(mode))

@@ -1,5 +1,5 @@
 /*
- * b200llama.h -- C ABI of libb200llama.so: the B200-native replacement for the
+ * b200llama.h -- C ABI of libb200llama.so: the H100-native replacement for the
  * TornadoVM execution-plan layer of beehive-lab/GPULlama3.java.
  *
  * One `b200_plan` plays the role of one `TornadoVMMasterPlan` instance
@@ -125,7 +125,7 @@ int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n
 /* How b200_forward_batch_prefill computes (the reference has the same two families:
  * LlamaFP16LayersBatchPrefill vs ...BatchPrefillMMA, selected by TensorCoreSupport.java):
  *   B200_PREFILL_EXACT       the single-token prefill graph per token: KV cache bit-identical to the CPU path;
- *   B200_PREFILL_TENSOR_CORE TMA + tcgen05 GEMMs over the whole chunk, FP16 operands / FP32 accumulation:
+ *   B200_PREFILL_TENSOR_CORE TMA + wgmma GEMMs over the whole chunk, FP16 operands / FP32 accumulation:
  *                            KV cache within FP16 tolerance of the CPU path.  Default for FP16 plans created
  *                            with prefill_batch_size > 1.  Opt-in for single-GPU Q8_0 plans: the first call
  *                            dequantises f16 twins of the weight matrices on the device (+2 bytes/weight);
@@ -143,7 +143,7 @@ int b200_prefill_info(b200_plan *plan, int32_t *mode, int32_t *launches, float *
  * TornadoVMMasterPlanSingleToken.tornadoVMForwardDecode's N+2 TaskGraph executions
  * (TornadoVMMasterPlanSingleToken.java:68-95) and produce bit-identical results:
  *   B200_DECODE_GRAPH       one CUDA graph of ~7 kernels per layer with programmatic-dependent-launch edges (the default:
- *                           measured 3.19 ms vs 3.51 ms per token on Llama-3-8B Q8_0, profiles/r2_final_a.log);
+ *                           every plan can run it; DESIGN.md section 6 has both measured);
  *   B200_DECODE_PERSISTENT  ONE persistent kernel per token (csrc/decode_persistent.cuh): one CTA per SM streams the
  *                           weights of every matrix through a shared-memory ring while epoch counters order the phases.
  *                           Available when the plan fits (Q8_0 streaming layout, head size 64/128); the environment
@@ -233,8 +233,8 @@ int b200_requant_kquant(int32_t ggml_type, const void *src, int64_t n_elems, voi
 
 /* Batched-prefill GEMM building block (csrc/prefill_gemm.cuh; replaces the reference's mma.sync GEMMs
  * gemmMMA / gemmMMAQKV / gemmMMAGateUp, TransformerBatchPrefillKernels.java:792-1132) exposed for
- * tests and measurement: C[m][n] (f32) = A[m][k] (f16 bits) x B[n][k]^T (f16 bits) on tcgen05 tensor
- * cores, FP32 accumulation in TMEM.  Host pointers; m % 128 == n % 128 == k % 64 == 0.
+ * tests and measurement: C[m][n] (f32) = A[m][k] (f16 bits) x B[n][k]^T (f16 bits) on the Hopper tensor
+ * cores (wgmma), FP32 accumulation.  Host pointers; m % 128 == n % 128 == k % 64 == 0.
  * iters > 0 additionally times `iters` back-to-back launches (device events) into *ms. */
 int b200_gemm_f16(const uint16_t *a, const uint16_t *b, float *c, int32_t m, int32_t n, int32_t k, int32_t iters, float *ms /* nullable */);
 
@@ -256,7 +256,7 @@ void b200_plan_free(b200_plan *plan);
 
 const char *b200_last_error(b200_plan *plan);
 
-/* Library build id, e.g. "b200llama 0.1 sm_100a". */
+/* Library build id, e.g. "b200llama 0.1 sm_90a". */
 const char *b200_version(void);
 
 #ifdef __cplusplus

@@ -11,7 +11,7 @@
  * cannot be executed here (needs JDK 21 + TornadoVM, neither present).  This
  * file is a line-by-line restatement; every function cites the reference
  * file:line it follows (paths relative to
- * /root/reference/src/main/java/org/beehive/gpullama3/).
+ * src/main/java/org/beehive/gpullama3/ of the reference).
  * What third parties pin instead (everything but the float summation order):
  * the data formats against gguf-py (tests/test_kquants.py) and the structure
  * of the forward pass against Hugging Face transformers in float64

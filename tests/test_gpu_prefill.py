@@ -81,7 +81,7 @@ def _prefill_and_compare(pkg, orc, m, n_tok, batch, tol=FP16_TOL):
                                                ("tiny-qwen3", 520, 512), ("tiny-phi3-gqa", 45, 32)])
 def test_tensor_core_prefill_within_fp16_tolerance(pkg, orc, make_model, shape, n_tok, batch):
     """Chunks that start at position > 0, a ragged last chunk, a chunk longer than one 128-row GEMM tile, chunks
-    longer than 256 rows (two CTA-pair tiles per pair, ragged and full, then an 8-token tail at position 512),
+    longer than 256 rows (ragged and full, then an 8-token tail at position 512),
     Llama (interleaved RoPE), Qwen3 (q/k norm + NeoX RoPE, q width != dim) and Phi-3 (fused qkv / gate-up source tensors, NeoX RoPE without norm)."""
     m = make_model(shape, pkg.gguf.GGMLType.F16, n_tok + 8)
     _prefill_and_compare(pkg, orc, m, n_tok, batch)

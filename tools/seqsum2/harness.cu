@@ -1,6 +1,6 @@
 // harness.cu -- runs block_seqsum_exact_v2 (csrc/seqsum2.cuh) against the literal float loop on the
 // adversarial generators of proto.c and times it next to the round-1 kernel.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -fmad=false -I gpullama3.java_b200/csrc -o /tmp/seqsum2_harness tools/seqsum2/harness.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -fmad=false -I gpullama3.java_b200/csrc -o /tmp/seqsum2_harness tools/seqsum2/harness.cu
 #include "seqsum2.cuh"
 #include <cmath>
 #include <cstdio>

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Phase timeline of the persistent decode kernel (b200_trace_persistent): where one token's time goes.
 
-    python tools/trace_persistent.py [workload] [depth] > profiles/decode_timeline_r2.txt
+    python tools/trace_persistent.py [workload] [depth] > decode_timeline.txt
 
 Every CTA stamps %globaltimer at ten points per layer (include/b200llama.h).  Reported per phase, averaged over the
 layers 1..L-1 (layer 0 starts from the embedding row): the mean and the slowest CTA's duration, and for every grid-wide

@@ -1517,6 +1517,16 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
         if (layer < 0 || layer >= c.n_layers) return fail(p, B200_ERR_BAD_ARG, "layer out of range");
         src = (s == "key_cache" ? p->key_cache : p->value_cache) + (size_t)layer * ctx_kv;
         sz = ctx_kv * 4;
+    } else if (s.rfind("pf_", 0) == 0) { // tensor-core prefill scratch: [padded rows][width], the last layer of the last chunk
+        const PrefillCtx &pc = p->prefill;
+        if (!pc.ready) return fail(p, B200_ERR_STATE, "%s: the plan has no tensor-core prefill buffers (%s)", name, pc.why);
+        const size_t rows = (size_t)pc.bpad;
+        if (s == "pf_x") { src = pc.X; sz = rows * c.dim * 4; }
+        else if (s == "pf_qkv") { src = pc.QKV; sz = rows * (p->qd + 2 * p->kvd) * 4; }
+        else if (s == "pf_a16") { src = pc.A16; sz = rows * c.dim * 2; }
+        else if (s == "pf_att16") { src = pc.ATT16; sz = rows * p->qd * 2; }
+        else if (s == "pf_h16") { src = pc.H16; sz = rows * c.hidden_dim * 2; }
+        else return fail(p, B200_ERR_BAD_ARG, "unknown buffer %s", name);
     } else return fail(p, B200_ERR_BAD_ARG, "unknown buffer %s", name);
     if (bytes < sz) sz = bytes;
     CK(cudaSetDevice(p->device));
@@ -1786,6 +1796,91 @@ int b200_gemm_f16(const uint16_t *a, const uint16_t *b, float *c, int32_t m, int
     if (e0) cudaEventDestroy(e0);
     if (e1) cudaEventDestroy(e1);
     cudaFree(da); cudaFree(db); cudaFree(dc);
+    return rc;
+}
+
+int b200_test_gemm(int32_t mode, int32_t stages, int32_t splits, int32_t m, int32_t m_valid, int32_t n, int32_t k, const uint16_t *a, const uint16_t *b,
+                   const uint16_t *b2, void *c) {
+    const bool gateup = mode == pg::GEMM_GATEUP;
+    if (mode < pg::GEMM_F32 || mode > pg::GEMM_GATEUP || (stages != pg::GEMM_STAGES && stages != pg::GEMM_STAGES_DEEP)) return B200_ERR_BAD_ARG;
+    if (!a || !b || !c || (gateup && !b2) || m <= 0 || n <= 0 || k <= 0 || m % pg::BM || k % pg::BK || n % (gateup ? pg::BN / 2 : pg::BN)) return B200_ERR_BAD_ARG;
+    if (m_valid < 1 || m_valid > m || splits < 1) return B200_ERR_BAD_ARG;
+    const size_t c_bytes = (size_t)m * n * (gateup ? 2 : 4);
+    __half *da = nullptr, *db = nullptr, *db2 = nullptr;
+    void *dc = nullptr;
+    int rc = B200_OK;
+    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
+    if (ok(cudaMalloc(&da, (size_t)m * k * 2)) && ok(cudaMalloc(&db, (size_t)n * k * 2)) && (!gateup || ok(cudaMalloc(&db2, (size_t)n * k * 2))) &&
+        ok(cudaMalloc(&dc, c_bytes)) && ok(cudaMemcpy(da, a, (size_t)m * k * 2, cudaMemcpyHostToDevice)) &&
+        ok(cudaMemcpy(db, b, (size_t)n * k * 2, cudaMemcpyHostToDevice)) && (!gateup || ok(cudaMemcpy(db2, b2, (size_t)n * k * 2, cudaMemcpyHostToDevice))) &&
+        ok(cudaMemcpy(dc, c, c_bytes, cudaMemcpyHostToDevice))) {
+        // the same maps prefill_forward builds: A boxes of 128 rows, B boxes of 128 rows (64 for each half of the gate/up tile), C boxes 128 x 32 f32
+        CUtensorMap ma, mb, mb2, mc;
+        const uint32_t b_rows = gateup ? pg::BN / 2 : pg::BN;
+        if (pg::make_map(&ma, da, (uint64_t)m, (uint64_t)k, pg::BM) || pg::make_map(&mb, db, (uint64_t)n, (uint64_t)k, b_rows) ||
+            pg::make_map(&mb2, gateup ? db2 : db, (uint64_t)n, (uint64_t)k, b_rows) || (!gateup && pg::make_map_c(&mc, dc, (uint64_t)m, (uint64_t)n)))
+            rc = B200_ERR_CUDA;
+        if (gateup) mc = mb; // unused by the gate/up epilogue, which stores f16 through plain pointers
+        int lr = 0;
+        if (rc == B200_OK) {
+            const int mt = m / pg::BM, nt = n / (gateup ? pg::BN / 2 : pg::BN);
+            const bool deep = stages == pg::GEMM_STAGES_DEEP;
+            if (mode == pg::GEMM_F32)
+                lr = deep ? pg::gemm_launch<pg::GEMM_F32, pg::GEMM_STAGES_DEEP>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits)
+                          : pg::gemm_launch<pg::GEMM_F32, pg::GEMM_STAGES>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits);
+            else if (mode == pg::GEMM_RESID)
+                lr = deep ? pg::gemm_launch<pg::GEMM_RESID, pg::GEMM_STAGES_DEEP>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits)
+                          : pg::gemm_launch<pg::GEMM_RESID, pg::GEMM_STAGES>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits);
+            else
+                lr = deep ? pg::gemm_launch<pg::GEMM_GATEUP, pg::GEMM_STAGES_DEEP>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits)
+                          : pg::gemm_launch<pg::GEMM_GATEUP, pg::GEMM_STAGES>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits);
+            if (lr == -6) rc = B200_ERR_BAD_ARG; // splits > 1 outside GEMM_RESID, or a split with no k-block
+            else if (lr) rc = B200_ERR_CUDA;
+        }
+        if (ok(cudaDeviceSynchronize()) && rc == B200_OK) ok(cudaMemcpy(c, dc, c_bytes, cudaMemcpyDeviceToHost));
+    }
+    cudaFree(da); cudaFree(db); cudaFree(db2); cudaFree(dc);
+    return rc;
+}
+
+int b200_test_pf_attention(int32_t impl, const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads, int32_t n_kv_heads,
+                           int32_t head_size, int32_t out_rows, uint16_t *out) {
+    if (!q || !k || !v || !out || (impl != 0 && impl != 1) || n < 1 || start_pos < 0 || out_rows < n || n_kv_heads < 1 || n_heads % n_kv_heads) return B200_ERR_BAD_ARG;
+    const int kv_mul = n_heads / n_kv_heads, hs = head_size;
+    if ((hs != 64 && hs != 128) || kv_mul > 64 || (kv_mul & (kv_mul - 1))) return B200_ERR_BAD_ARG; // what prefill_init accepts
+    const int qd = n_heads * hs, kvd = n_kv_heads * hs, ldq = qd + 2 * kvd, nkeys = start_pos + n;
+    const size_t kv_elems = (size_t)nkeys * kvd;
+    float *dqkv = nullptr, *dk = nullptr, *dv = nullptr;
+    __half *dkh = nullptr, *dvh = nullptr, *dout = nullptr;
+    int rc = B200_OK;
+    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
+    // q sits in the q columns of a QKV row as after k_pf_rope_kv; the k / v columns hold NaN, which the kernels must never read
+    if (ok(cudaMalloc(&dqkv, (size_t)n * ldq * 4)) && ok(cudaMalloc(&dk, kv_elems * 4)) && ok(cudaMalloc(&dv, kv_elems * 4)) &&
+        ok(cudaMalloc(&dkh, kv_elems * 2)) && ok(cudaMalloc(&dvh, kv_elems * 2)) && ok(cudaMalloc(&dout, (size_t)out_rows * qd * 2)) &&
+        ok(cudaMemset(dqkv, 0xFF, (size_t)n * ldq * 4)) && ok(cudaMemcpy2D(dqkv, (size_t)ldq * 4, q, (size_t)qd * 4, (size_t)qd * 4, n, cudaMemcpyHostToDevice)) &&
+        ok(cudaMemcpy(dk, k, kv_elems * 4, cudaMemcpyHostToDevice)) && ok(cudaMemcpy(dv, v, kv_elems * 4, cudaMemcpyHostToDevice)) &&
+        ok(cudaMemcpy(dout, out, (size_t)out_rows * qd * 2, cudaMemcpyHostToDevice))) {
+        const float inv_sqrt_hs = (float)(1.0 / sqrt((double)hs));
+        const int qt = PA_ROWS / kv_mul;
+        const dim3 ag((n + qt - 1) / qt, n_kv_heads);
+        if (impl == 0) { // f16 K / V copies as prefill_forward makes them (k_pf_kv_to_f16 and k_pf_rope_kv round the same way)
+            const size_t n4 = kv_elems / 4;
+            k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, 0>>>(dk, dv, dkh, dvh, n4);
+        }
+        if (hs == 128) {
+            if (impl == 0 && ok(cudaFuncSetAttribute(k_pf_attention_mma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>())))
+                k_pf_attention_mma<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, n, start_pos, inv_sqrt_hs, dout, qd);
+            if (impl == 1 && ok(cudaFuncSetAttribute(k_pf_attention<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pa_smem_bytes<128>())))
+                k_pf_attention<128><<<ag, PA_THREADS, pa_smem_bytes<128>(), 0>>>(dqkv, ldq, dk, dv, kvd, kv_mul, n, start_pos, inv_sqrt_hs, dout, qd);
+        } else {
+            if (impl == 0 && ok(cudaFuncSetAttribute(k_pf_attention_mma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<64>())))
+                k_pf_attention_mma<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, n, start_pos, inv_sqrt_hs, dout, qd);
+            if (impl == 1 && ok(cudaFuncSetAttribute(k_pf_attention<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pa_smem_bytes<64>())))
+                k_pf_attention<64><<<ag, PA_THREADS, pa_smem_bytes<64>(), 0>>>(dqkv, ldq, dk, dv, kvd, kv_mul, n, start_pos, inv_sqrt_hs, dout, qd);
+        }
+        if (ok(cudaGetLastError()) && ok(cudaDeviceSynchronize())) ok(cudaMemcpy(out, dout, (size_t)out_rows * qd * 2, cudaMemcpyDeviceToHost));
+    }
+    cudaFree(dqkv); cudaFree(dk); cudaFree(dv); cudaFree(dkh); cudaFree(dvh); cudaFree(dout);
     return rc;
 }
 

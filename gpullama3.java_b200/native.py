@@ -41,7 +41,7 @@ class Tensor(C.Structure):
 
 EXPORTS = ["b200_plan_create", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
-           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_test_seqsum", "b200_gemm_f16", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
+           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_test_seqsum", "b200_gemm_f16", "b200_test_gemm", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -75,6 +75,8 @@ def lib() -> C.CDLL:
     L.b200_test_seqsum2.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(i32)]
     L.b200_prefill_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
     L.b200_gemm_f16.argtypes = [vp, vp, vp, i32, i32, i32, i32, C.POINTER(C.c_float)]
+    L.b200_test_gemm.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
+    L.b200_test_pf_attention.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.b200_time_kernel.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
     L.b200_read_buffer.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
@@ -135,6 +137,53 @@ def gemm_f16(a, b, iters: int = 0):
     if rc != B200_OK:
         _raise(rc, "b200_gemm_f16 failed")
     return c, (ms.value if iters > 0 else None)
+
+
+GEMM_MODES = {"f32": 0, "resid": 1, "gateup": 2}
+
+
+def test_gemm(mode: str, a, b, c, b2=None, m_valid: int | None = None, stages: int = 4, splits: int = 1) -> np.ndarray:
+    """One launch of the prefill GEMM (csrc/prefill_gemm.cuh) as the prefill issues it.  a [M,K], b (and b2 for "gateup") [N,K]
+    float16; c is the initial output: float32 [M,N] for "f32" / "resid" (resid adds to it), float16 [M,N] for "gateup".
+    Returns the output after the launch (a new array)."""
+    a = np.ascontiguousarray(a, dtype=np.float16)
+    b = np.ascontiguousarray(b, dtype=np.float16)
+    gateup = mode == "gateup"
+    c = np.array(c, dtype=np.float16 if gateup else np.float32, order="C", copy=True)
+    m, k = a.shape
+    n = b.shape[0]
+    if b.shape != (n, k) or c.shape != (m, n):
+        raise ValueError("shapes do not match")
+    if gateup:
+        b2 = np.ascontiguousarray(b2, dtype=np.float16)
+        if b2.shape != b.shape:
+            raise ValueError("b2 must have the shape of b")
+    rc = lib().b200_test_gemm(GEMM_MODES[mode], stages, splits, m, m if m_valid is None else m_valid, n, k, a.ctypes.data, b.ctypes.data,
+                              b2.ctypes.data if gateup else None, c.ctypes.data)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_gemm failed")
+    return c
+
+
+def test_pf_attention(q, k, v, n_heads: int, n_kv_heads: int, start_pos: int, impl: str = "mma", out_rows: int | None = None,
+                      sentinel: int = 0x7E5A) -> np.ndarray:
+    """The prefill's causal attention over one chunk (csrc/prefill.cuh).  q float32 [n, n_heads*hs]; k, v float32
+    [start_pos+n, n_kv_heads*hs].  impl "mma" (k_pf_attention_mma) or "simt" (k_pf_attention).  Returns the f16 bits
+    (uint16) of [out_rows, n_heads*hs]: rows >= n keep `sentinel`."""
+    q = np.ascontiguousarray(q, dtype=np.float32)
+    k = np.ascontiguousarray(k, dtype=np.float32)
+    v = np.ascontiguousarray(v, dtype=np.float32)
+    n, qd = q.shape
+    hs = qd // n_heads
+    if k.shape != (start_pos + n, n_kv_heads * hs) or v.shape != k.shape:
+        raise ValueError("k / v must be [start_pos + n, n_kv_heads * head_size]")
+    rows = n if out_rows is None else out_rows
+    out = np.full((rows, qd), sentinel, dtype=np.uint16)
+    rc = lib().b200_test_pf_attention({"mma": 0, "simt": 1}[impl], q.ctypes.data, k.ctypes.data, v.ctypes.data, n, start_pos, n_heads, n_kv_heads, hs,
+                                      rows, out.ctypes.data)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_pf_attention failed")
+    return out
 
 
 GGML_SIZES = {0: (4, 1), 1: (2, 1), 8: (34, 32), 12: (144, 256), 13: (176, 256), 14: (210, 256)}  # (bytes, elements) per block, GGMLType.java:5-20

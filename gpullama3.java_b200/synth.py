@@ -54,6 +54,10 @@ SHAPES = {
     # Phi-3 (forwardJavaPhi3: fused attn_qkv / gate-up tensors, NeoX-pair RoPE): mini-like (multi-head, head size 96) and medium-like (GQA, 128)
     "tiny-phi3": Shape("phi3", 384, 768, 2, 4, 4, 96, 512, False, 10000.0, 1e-5, 4096),
     "tiny-phi3-gqa": Shape("phi3", 512, 1024, 2, 4, 2, 128, 512, False, 10000.0, 1e-5, 4096),
+    # GQA ratios 1, 8 (head size 64) and 4 (head size 128) for the tensor-core prefill's query-tile mapping
+    "tiny-llama-mha": Shape("llama", 256, 512, 2, 4, 4, 64, 512, False, 500000.0, 1e-5),
+    "tiny-llama-gqa8": Shape("llama", 1024, 1024, 2, 16, 2, 64, 512, False, 500000.0, 1e-5),
+    "tiny-llama-gqa4-hs128": Shape("llama", 1024, 1536, 2, 8, 2, 128, 512, False, 500000.0, 1e-5),
     "mid-phi3-mini": Shape("phi3", 3072, 8192, 2, 32, 32, 96, 8192, False, 10000.0, 1e-5, 4096),  # Phi-3-mini-4k layer geometry
     # mid shape: exercises column tails (dim not a multiple of 512) and several row tiles
     "small-llama": Shape("llama", 1536, 4096, 3, 12, 4, 128, 4096, False, 500000.0, 1e-5),

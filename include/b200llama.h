@@ -174,7 +174,10 @@ int b200_kv_reset(b200_plan *plan);
 
 /* Test/diagnostic read-back of a named device buffer into host memory.  Names:
  * "x","xb","q","k","v","hb","logits","key_cache","value_cache","xq","xs".  `layer` selects the
- * layer for the KV caches (ignored otherwise).  Copies min(bytes, buffer size). */
+ * layer for the KV caches (ignored otherwise).  The tensor-core prefill scratch, as the last layer of the last
+ * chunk left it, rows padded to a multiple of 128: "pf_x" (f32 residual, dim wide), "pf_qkv" (f32, q + k + v wide,
+ * q rotated in place, k before RoPE), "pf_a16" (f16 bits, the FFN input), "pf_att16" (f16 bits, attention output),
+ * "pf_h16" (f16 bits, SwiGLU output).  Copies min(bytes, buffer size). */
 int b200_read_buffer(b200_plan *plan, const char *name, int32_t layer, void *dst, size_t bytes);
 
 /* Measurement hook for bench.py's roofline line: launches ONE kernel family of the decode step
@@ -237,6 +240,27 @@ int b200_requant_kquant(int32_t ggml_type, const void *src, int64_t n_elems, voi
  * cores (wgmma), FP32 accumulation.  Host pointers; m % 128 == n % 128 == k % 64 == 0.
  * iters > 0 additionally times `iters` back-to-back launches (device events) into *ms. */
 int b200_gemm_f16(const uint16_t *a, const uint16_t *b, float *c, int32_t m, int32_t n, int32_t k, int32_t iters, float *ms /* nullable */);
+
+/* Test hook: ONE launch of the prefill GEMM exactly as b200_forward_batch_prefill launches it (pg::gemm_launch<mode, stages>).
+ *   mode 0 (F32):    c (f32 [m][n]) = a[m][k] x b[n][k]^T; rows >= m_valid are stored as 0.
+ *   mode 1 (RESID):  c (f32 [m][n]) += a x b^T, K split `splits` ways, every split reduce-adding its partial product;
+ *                    rows >= m_valid add 0.
+ *   mode 2 (GATEUP): c (f16 bits [m][n]) = f16(silu(a x b^T) * (a x b2^T)), b = W1, b2 = W3, N tiles of 64 columns;
+ *                    rows >= m_valid are not written.
+ * a, b, b2: f16 bits.  c is in/out: its content is uploaded first.  stages = 4 or 6 (ring depth); m % 128 == 0, k % 64 == 0,
+ * n % 128 == 0 (n % 64 == 0 for GATEUP), 1 <= m_valid <= m.  splits > 1 outside RESID, or a split left without a
+ * 64-wide k-block, is rejected with B200_ERR_BAD_ARG. */
+int b200_test_gemm(int32_t mode, int32_t stages, int32_t splits, int32_t m, int32_t m_valid, int32_t n, int32_t k, const uint16_t *a, const uint16_t *b,
+                   const uint16_t *b2 /* GATEUP only */, void *c);
+
+/* Test hook: the causal attention of the tensor-core prefill over one chunk of n query tokens at positions start_pos ..
+ * start_pos + n - 1.  q: f32 [n][n_heads * head_size] (rotated); k, v: f32 [start_pos + n][n_kv_heads * head_size] (the KV cache
+ * rows).  impl 0 = k_pf_attention_mma (f16 K / V copies built by k_pf_kv_to_f16, as in the prefill), 1 = the FP32 SIMT
+ * k_pf_attention.  q is placed in rows of stride q + 2 * kv width whose k / v columns hold NaN; grid and shared memory are the
+ * prefill's.  out: f16 bits [out_rows][n_heads * head_size], out_rows >= n, in/out: rows >= n must come back untouched.
+ * head_size 64 or 128, n_heads / n_kv_heads a power of two <= 64. */
+int b200_test_pf_attention(int32_t impl, const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads,
+                           int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out);
 
 /* Weight upload of b200_plan_create (the counterpart of the reference's load-time metrics, ModelLoader.java:102-106 and the
  * copy-in timing of TornadoVMMasterPlanSingleToken.java:51-54): wall seconds from the first tensor to the last repack kernel,

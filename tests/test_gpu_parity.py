@@ -74,6 +74,13 @@ def test_decode_f16_bit_exact(pkg, orc, make_model, shape, lanes):
     run_stream(pkg, orc, m, lanes, 12)
 
 
+@pytest.mark.parametrize("shape", ["tiny-llama-mha", "tiny-llama-gqa8", "tiny-llama-gqa4-hs128"])
+def test_decode_f16_gqa_ratios_bit_exact(pkg, orc, make_model, shape):
+    """The shapes that give the tensor-core prefill GQA ratios 1, 8 and 4 (head size 128) decode bit-exactly themselves."""
+    m = make_model(shape, pkg.gguf.GGMLType.F16, 24)
+    run_stream(pkg, orc, m, 16, 12)
+
+
 @pytest.mark.parametrize("shape,lanes", [("mid-llama-1b", 16), ("mid-llama", 16), ("mid-llama", 8), ("mid-qwen3-4b", 16)])
 def test_decode_mid_geometries_f16(pkg, orc, shape, lanes):
     """FP16 plans on the per-warp bulk-copy rings (csrc/stream_matvec_f16.cuh) at the real layer geometries, bit-exact vs the oracle:

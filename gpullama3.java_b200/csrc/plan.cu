@@ -1109,23 +1109,26 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
 }
 
 // ---- batched prefill on the tensor cores (prefill.cuh) -------------------------------------------
-int prefill_init(b200_plan *p) {
+// What both tensor-core modes need of the plan's shape; nullptr when the chunk GEMMs and the attention can run it.
+static const char *prefill_shape_why(const b200_plan *p) {
+    const b200_config &g = p->cfg;
+    const int kv_mul = g.n_heads / g.n_kv_heads, nqkv = p->qd + 2 * p->kvd;
+    if (g.tp_size > 1) return "tensor-core prefill is single-GPU";
+    if (g.head_size != 64 && g.head_size != 128) return "tensor-core prefill supports head sizes 64 and 128";
+    if (kv_mul > 64 || (kv_mul & (kv_mul - 1))) return "tensor-core prefill needs a power-of-two GQA ratio <= 64";
+    if (g.dim % 128 || p->qd % 128 || nqkv % 128 || g.hidden_dim % 64) return "tensor-core prefill needs dim, q width and q+k+v width multiples of 128, hidden a multiple of 64";
+    if (!pg::encode_fn()) return "cuTensorMapEncodeTiled not available from the driver";
+    return nullptr;
+}
+
+// The chunk's scratch buffers, their tensor maps and the attention kernels' shared-memory attributes: allocated once per
+// plan, shared by both tensor-core modes.  *ok = false if a tensor map was rejected.
+static int prefill_scratch(b200_plan *p, bool *ok) {
     PrefillCtx &c = p->prefill;
     const b200_config &g = p->cfg;
-    c.batch = p->prefill_batch;
-    c.ready = false;
-    c.mode = 0;
-    const int kv_mul = g.n_heads / g.n_kv_heads, nqkv = p->qd + 2 * p->kvd;
-    if (p->wtype != B200_GGML_F16 && !p->f16_copies) {
-        c.why = p->use_stream ? "Q8_0 plan: the tensor-core prefill is opt-in (b200_set_prefill_mode builds f16 twins of the weight matrices, +2 bytes per weight)"
-                              : "tensor-core prefill needs FP16 weight matrices or a Q8_0 plan on the streaming path";
-        return B200_OK;
-    }
-    if (g.tp_size > 1) { c.why = "tensor-core prefill is single-GPU"; return B200_OK; }
-    if (g.head_size != 64 && g.head_size != 128) { c.why = "tensor-core prefill supports head sizes 64 and 128"; return B200_OK; }
-    if (kv_mul > 64 || (kv_mul & (kv_mul - 1))) { c.why = "tensor-core prefill needs a power-of-two GQA ratio <= 64"; return B200_OK; }
-    if (g.dim % 128 || p->qd % 128 || nqkv % 128 || g.hidden_dim % 64) { c.why = "tensor-core prefill needs dim, q width and q+k+v width multiples of 128, hidden a multiple of 64"; return B200_OK; }
-    if (!pg::encode_fn()) { c.why = "cuTensorMapEncodeTiled not available from the driver"; return B200_OK; }
+    const int nqkv = p->qd + 2 * p->kvd;
+    *ok = true;
+    if (c.bpad) return B200_OK;
     c.bpad = (c.batch + pg::BM - 1) / pg::BM * pg::BM; // whole 128-row GEMM tiles
     int rc;
     if ((rc = dalloc(p, &c.X, (size_t)c.bpad * g.dim * 4))) return rc;
@@ -1142,18 +1145,9 @@ int prefill_init(b200_plan *p) {
     CK(cudaMemset(c.ATT16, 0, (size_t)c.bpad * p->qd * 2));
     CK(cudaMemset(c.H16, 0, (size_t)c.bpad * g.hidden_dim * 2));
     CK(cudaMemset(c.tok, 0, (size_t)c.bpad * 4));
-    bool ok = pg::make_map(&c.mA, c.A16, c.bpad, g.dim, pg::BM) == 0 && pg::make_map(&c.mATT, c.ATT16, c.bpad, p->qd, pg::BM) == 0 &&
-              pg::make_map(&c.mH, c.H16, c.bpad, g.hidden_dim, pg::BM) == 0 && pg::make_map_c(&c.mX, c.X, c.bpad, g.dim) == 0 &&
-              pg::make_map_c(&c.mQKV, c.QKV, c.bpad, nqkv) == 0;
-    c.maps.resize(g.n_layers);
-    for (int l = 0; ok && l < g.n_layers; l++) {
-        const LayerW &L = p->layers[l];
-        PrefillLayerMaps &m = c.maps[l];
-        ok = pg::make_map(&m.qkv, L.qkv.qs, nqkv, g.dim, pg::BN) == 0 && pg::make_map(&m.wo, L.wo.qs, g.dim, p->qd, pg::BN) == 0 &&
-             pg::make_map(&m.w1, L.w1.qs, g.hidden_dim, g.dim, pg::BN / 2) == 0 && pg::make_map(&m.w3, L.w3.qs, g.hidden_dim, g.dim, pg::BN / 2) == 0 &&
-             pg::make_map(&m.w2, L.w2.qs, g.dim, g.hidden_dim, pg::BN) == 0;
-    }
-    if (!ok) { c.why = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
+    *ok = pg::make_map(&c.mA, c.A16, c.bpad, g.dim, pg::BM) == 0 && pg::make_map(&c.mATT, c.ATT16, c.bpad, p->qd, pg::BM) == 0 &&
+          pg::make_map(&c.mH, c.H16, c.bpad, g.hidden_dim, pg::BM) == 0 && pg::make_map_c(&c.mX, c.X, c.bpad, g.dim) == 0 &&
+          pg::make_map_c(&c.mQKV, c.QKV, c.bpad, nqkv) == 0;
     if (g.head_size == 128) {
         CK(cudaFuncSetAttribute(k_pf_attention<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pa_smem_bytes<128>()));
         CK(cudaFuncSetAttribute(k_pf_attention_mma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>()));
@@ -1165,9 +1159,71 @@ int prefill_init(b200_plan *p) {
         const char *e = getenv("B200_PF_ATT");
         c.att_simt = e && !strcmp(e, "simt");
     }
+    return B200_OK;
+}
+
+int prefill_init(b200_plan *p) {
+    PrefillCtx &c = p->prefill;
+    const b200_config &g = p->cfg;
+    c.batch = p->prefill_batch;
+    c.ready = false;
+    if (c.mode == B200_PREFILL_TENSOR_CORE) c.mode = B200_PREFILL_EXACT;
+    const int nqkv = p->qd + 2 * p->kvd;
+    if (p->wtype != B200_GGML_F16 && !p->f16_copies) {
+        c.why = p->use_stream ? "Q8_0 plan: the tensor-core prefill is opt-in (b200_set_prefill_mode builds f16 twins of the weight matrices, +2 bytes per weight)"
+                              : "tensor-core prefill needs FP16 weight matrices or a Q8_0 plan on the streaming path";
+        return B200_OK;
+    }
+    if ((c.why = prefill_shape_why(p))) return B200_OK;
+    bool ok;
+    int rc;
+    if ((rc = prefill_scratch(p, &ok))) return rc;
+    c.maps.resize(g.n_layers);
+    for (int l = 0; ok && l < g.n_layers; l++) {
+        const LayerW &L = p->layers[l];
+        PrefillLayerMaps &m = c.maps[l];
+        ok = pg::make_map(&m.qkv, L.qkv.qs, nqkv, g.dim, pg::BN) == 0 && pg::make_map(&m.wo, L.wo.qs, g.dim, p->qd, pg::BN) == 0 &&
+             pg::make_map(&m.w1, L.w1.qs, g.hidden_dim, g.dim, pg::BN / 2) == 0 && pg::make_map(&m.w3, L.w3.qs, g.hidden_dim, g.dim, pg::BN / 2) == 0 &&
+             pg::make_map(&m.w2, L.w2.qs, g.dim, g.hidden_dim, pg::BN) == 0;
+    }
+    if (!ok) { c.why = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
     c.ready = true;
-    c.mode = 1;
+    c.mode = B200_PREFILL_TENSOR_CORE;
     c.why = "";
+    return B200_OK;
+}
+
+// W8A16: the GEMMs read B from the tile-major Q8_0 streams the decode kernels use (L.tqkv, L.two, L.tgu, L.tw2) -- no
+// per-weight memory.  Built on the first b200_set_prefill_mode(TENSOR_CORE_W8A16).
+int prefill_init_q8(b200_plan *p) {
+    PrefillCtx &c = p->prefill;
+    const b200_config &g = p->cfg;
+    c.batch = p->prefill_batch;
+    if (p->prefill_batch <= 1) { c.why_q8 = "the plan was created without a prefill batch size (prefill_batch_size <= 1)"; return B200_OK; }
+    if (p->wtype != B200_GGML_Q8_0) { c.why_q8 = "W8A16 prefill needs a Q8_0 plan (FP16 plans run the tensor-core prefill on their own f16 matrices)"; return B200_OK; }
+    if (g.tp_size > 1) { c.why_q8 = "tensor-core prefill is single-GPU"; return B200_OK; }
+    if (!p->use_stream) { c.why_q8 = "W8A16 prefill reads the tile-major Q8_0 streams: the plan must use the streaming layout"; return B200_OK; }
+    if ((c.why_q8 = prefill_shape_why(p))) return B200_OK;
+    for (int l = 0; l < g.n_layers; l++) {
+        const LayerW &L = p->layers[l];
+        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
+            if (t->seg % pg::BK) { c.why_q8 = "W8A16 prefill needs Q8_0 stream segments that are multiples of 64 columns"; return B200_OK; }
+    }
+    bool ok;
+    int rc;
+    if ((rc = prefill_scratch(p, &ok))) return rc;
+    c.maps_q8.resize(g.n_layers);
+    for (int l = 0; ok && l < g.n_layers; l++) {
+        const LayerW &L = p->layers[l];
+        PrefillQ8Maps &m = c.maps_q8[l];
+        auto mk = [](CUtensorMap *q, CUtensorMap *s, const TileMat &t) {
+            return pg::make_map_q8(q, t.base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 0) == 0 && pg::make_map_q8(s, t.base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 1) == 0;
+        };
+        ok = mk(&m.qkv_q, &m.qkv_s, L.tqkv) && mk(&m.wo_q, &m.wo_s, L.two) && mk(&m.gu_q, &m.gu_s, L.tgu) && mk(&m.w2_q, &m.w2_s, L.tw2);
+    }
+    if (!ok) { c.why_q8 = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
+    c.q8_ready = true;
+    c.why_q8 = "";
     return B200_OK;
 }
 
@@ -1210,6 +1266,8 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
     const float inv_sqrt_hs = (float)(1.0 / sqrt((double)g.head_size));
     int nl = 0;
     constexpr int ST = pg::GEMM_STAGES;
+    const bool q8 = c.mode == B200_PREFILL_TENSOR_CORE_W8A16; // B from the Q8_0 streams (c.maps_q8) instead of the f16 matrices (c.maps)
+    using pg::B_Q8;
     // the x += A W^T GEMMs (N = dim only) split K until the grid fills the SMs -- every split reduce-adds its partial
     // product through TMA -- keeping at least 8 k-blocks per split
     auto splits = [&](int n_tiles, int K) {
@@ -1222,10 +1280,12 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
     k_pf_embed<<<n, 256, 0, s>>>(c.tok, p->emb, c.X, g.dim); nl++;
     for (int l = 0; l < g.n_layers; l++) {
         const LayerW &L = p->layers[l];
-        const PrefillLayerMaps &m = c.maps[l];
+        const PrefillLayerMaps *m = q8 ? nullptr : &c.maps[l];
+        const PrefillQ8Maps *mq = q8 ? &c.maps_q8[l] : nullptr;
         float *kc = p->key_cache + (size_t)l * ctx_kv, *vc = p->value_cache + (size_t)l * ctx_kv;
         k_pf_rmsnorm_f16<<<n, 256, 0, s>>>(c.X, L.attn_norm, g.rms_norm_eps, g.dim, c.A16); nl++;
-        if (pg::gemm_launch<pg::GEMM_F32, ST>(c.mA, m.qkv, m.qkv, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s))
+        if (q8 ? pg::gemm_launch<pg::GEMM_F32, ST, B_Q8>(c.mA, mq->qkv_q, mq->qkv_s, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s, 1, L.tqkv.seg)
+               : pg::gemm_launch<pg::GEMM_F32, ST>(c.mA, m->qkv, m->qkv, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s))
             return fail(p, B200_ERR_CUDA, "QKV GEMM launch failed");
         nl++;
         const int qt = PA_ROWS / kv_mul;
@@ -1245,14 +1305,18 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
             else k_pf_attention_mma<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
         }
         nl += 2;
-        if (pg::gemm_launch<pg::GEMM_RESID, ST>(c.mATT, m.wo, m.wo, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, splits(g.dim / pg::BN, p->qd)))
+        const int sp_wo = splits(g.dim / pg::BN, p->qd), sp_w2 = splits(g.dim / pg::BN, g.hidden_dim);
+        if (q8 ? pg::gemm_launch<pg::GEMM_RESID, ST, B_Q8>(c.mATT, mq->wo_q, mq->wo_s, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, sp_wo, L.two.seg)
+               : pg::gemm_launch<pg::GEMM_RESID, ST>(c.mATT, m->wo, m->wo, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, sp_wo))
             return fail(p, B200_ERR_CUDA, "Wo GEMM launch failed");
         nl++;
         k_pf_rmsnorm_f16<<<n, 256, 0, s>>>(c.X, L.ffn_norm, g.rms_norm_eps, g.dim, c.A16); nl++;
-        if (pg::gemm_launch<pg::GEMM_GATEUP, ST>(c.mA, m.w1, m.w3, c.mX, c.H16, g.hidden_dim, n, mt, g.hidden_dim / (pg::BN / 2), g.dim, s))
+        if (q8 ? pg::gemm_launch<pg::GEMM_GATEUP, ST, B_Q8>(c.mA, mq->gu_q, mq->gu_s, c.mX, c.H16, g.hidden_dim, n, mt, g.hidden_dim / (pg::BN / 2), g.dim, s, 1, L.tgu.seg)
+               : pg::gemm_launch<pg::GEMM_GATEUP, ST>(c.mA, m->w1, m->w3, c.mX, c.H16, g.hidden_dim, n, mt, g.hidden_dim / (pg::BN / 2), g.dim, s))
             return fail(p, B200_ERR_CUDA, "gate/up GEMM launch failed");
         nl++;
-        if (pg::gemm_launch<pg::GEMM_RESID, ST>(c.mH, m.w2, m.w2, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, splits(g.dim / pg::BN, g.hidden_dim)))
+        if (q8 ? pg::gemm_launch<pg::GEMM_RESID, ST, B_Q8>(c.mH, mq->w2_q, mq->w2_s, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, sp_w2, L.tw2.seg)
+               : pg::gemm_launch<pg::GEMM_RESID, ST>(c.mH, m->w2, m->w2, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, sp_w2))
             return fail(p, B200_ERR_CUDA, "W2 GEMM launch failed");
         nl++;
     }
@@ -1379,7 +1443,8 @@ int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, i
     for (int i = 0; i < n; i++)
         if (tokens[i] < 0 || tokens[i] >= p->cfg.vocab_size) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
     CK(cudaSetDevice(p->device));
-    if (p->prefill.ready && p->prefill.mode == 1) { // tensor-core GEMM path (prefill.cuh)
+    if ((p->prefill.ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE) ||
+        (p->prefill.q8_ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE_W8A16)) { // tensor-core GEMM path (prefill.cuh)
         memcpy(p->h_ids, tokens, (size_t)n * 4);
         CK(cudaMemcpyAsync(p->prefill.tok, p->h_ids, (size_t)n * 4, cudaMemcpyHostToDevice, p->stream));
         CK(cudaEventRecord(p->ev0, p->stream));
@@ -1467,7 +1532,17 @@ int b200_trace_persistent(b200_plan *p, int32_t token, int32_t position, uint64_
 }
 
 int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
-    if (!p || (mode != B200_PREFILL_EXACT && mode != B200_PREFILL_TENSOR_CORE)) return B200_ERR_BAD_ARG;
+    if (!p || (mode != B200_PREFILL_EXACT && mode != B200_PREFILL_TENSOR_CORE && mode != B200_PREFILL_TENSOR_CORE_W8A16)) return B200_ERR_BAD_ARG;
+    if (mode == B200_PREFILL_TENSOR_CORE_W8A16) {
+        if (!p->prefill.q8_ready) {
+            CK(cudaSetDevice(p->device));
+            int rc = prefill_init_q8(p);
+            if (rc) return rc;
+            if (!p->prefill.q8_ready) return fail(p, B200_ERR_UNSUPPORTED, "%s", p->prefill.why_q8);
+        }
+        p->prefill.mode = mode;
+        return B200_OK;
+    }
     if (mode == B200_PREFILL_TENSOR_CORE && !p->prefill.ready && p->prefill_batch > 1 && p->wtype == B200_GGML_Q8_0 && p->use_stream && p->cfg.tp_size == 1) {
         CK(cudaSetDevice(p->device)); // opt-in on a Q8_0 plan: build the f16 twins, then the GEMM context
         int rc = build_f16_twins(p);
@@ -1481,7 +1556,7 @@ int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
 
 int b200_prefill_info(b200_plan *p, int32_t *mode, int32_t *launches, float *device_ms) {
     if (!p) return B200_ERR_BAD_ARG;
-    if (mode) *mode = p->prefill.ready ? p->prefill.mode : B200_PREFILL_EXACT;
+    if (mode) *mode = p->prefill.ready || p->prefill.q8_ready ? p->prefill.mode : B200_PREFILL_EXACT;
     if (launches) *launches = p->launches_prefill;
     if (device_ms) *device_ms = p->prefill_ms;
     return B200_OK;
@@ -1519,7 +1594,7 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
         sz = ctx_kv * 4;
     } else if (s.rfind("pf_", 0) == 0) { // tensor-core prefill scratch: [padded rows][width], the last layer of the last chunk
         const PrefillCtx &pc = p->prefill;
-        if (!pc.ready) return fail(p, B200_ERR_STATE, "%s: the plan has no tensor-core prefill buffers (%s)", name, pc.why);
+        if (!pc.ready && !pc.q8_ready) return fail(p, B200_ERR_STATE, "%s: the plan has no tensor-core prefill buffers (%s)", name, pc.why);
         const size_t rows = (size_t)pc.bpad;
         if (s == "pf_x") { src = pc.X; sz = rows * c.dim * 4; }
         else if (s == "pf_qkv") { src = pc.QKV; sz = rows * (p->qd + 2 * p->kvd) * 4; }
@@ -1840,6 +1915,62 @@ int b200_test_gemm(int32_t mode, int32_t stages, int32_t splits, int32_t m, int3
         if (ok(cudaDeviceSynchronize()) && rc == B200_OK) ok(cudaMemcpy(c, dc, c_bytes, cudaMemcpyDeviceToHost));
     }
     cudaFree(da); cudaFree(db); cudaFree(db2); cudaFree(dc);
+    return rc;
+}
+
+int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, int32_t m_valid, int32_t n, int32_t k, const uint16_t *a, const void *bq,
+                      const void *bq2, void *c) {
+    const bool gateup = mode == pg::GEMM_GATEUP;
+    if (mode < pg::GEMM_F32 || mode > pg::GEMM_GATEUP || (stages != pg::GEMM_STAGES && stages != pg::GEMM_STAGES_DEEP_Q8)) return B200_ERR_BAD_ARG;
+    if (!a || !bq || !c || (gateup && !bq2) || m <= 0 || n <= 0 || k <= 0 || m % pg::BM || k % pg::BK || n % (gateup ? pg::BN / 2 : pg::BN)) return B200_ERR_BAD_ARG;
+    if (m_valid < 1 || m_valid > m || splits < 1) return B200_ERR_BAD_ARG;
+    // the stream exactly as upload_tiles lays it out; W8A16 needs whole 64-column k-blocks inside each segment
+    const int nseg = smv_pick_nseg(k);
+    if (!nseg || (k / nseg) % pg::BK) return B200_ERR_BAD_ARG;
+    const int seg = k / nseg, unit = smv_unit_bytes(seg), rows = gateup ? 2 * n : n;
+    const size_t c_bytes = (size_t)m * n * (gateup ? 2 : 4), q8_bytes = (size_t)n * (k / 32) * 34, stream_bytes = (size_t)rows * nseg * unit;
+    __half *da = nullptr;
+    unsigned char *draw = nullptr, *dstream = nullptr;
+    void *dc = nullptr;
+    int rc = B200_OK;
+    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
+    if (ok(cudaMalloc(&da, (size_t)m * k * 2)) && ok(cudaMalloc(&draw, q8_bytes * (gateup ? 2 : 1))) && ok(cudaMalloc(&dstream, stream_bytes)) &&
+        ok(cudaMalloc(&dc, c_bytes)) && ok(cudaMemcpy(da, a, (size_t)m * k * 2, cudaMemcpyHostToDevice)) && ok(cudaMemcpy(draw, bq, q8_bytes, cudaMemcpyHostToDevice)) &&
+        (!gateup || ok(cudaMemcpy(draw + q8_bytes, bq2, q8_bytes, cudaMemcpyHostToDevice))) && ok(cudaMemcpy(dc, c, c_bytes, cudaMemcpyHostToDevice))) {
+        RepackSrc src{};
+        src.raw[0] = draw;
+        src.rows[0] = n;
+        if (gateup) { src.raw[1] = draw + q8_bytes; src.rows[1] = n; }
+        src.gateup = gateup ? 1 : 0;
+        k_repack_tiles<<<(unsigned)((size_t)rows * nseg), 128>>>(src, dstream, rows, k, seg, nseg, unit);
+        ok(cudaGetLastError());
+        // the maps prefill_init_q8 builds and the A / C maps of the prefill scratch
+        CUtensorMap ma, mq, ms, mc;
+        if (rc == B200_OK && (pg::make_map(&ma, da, (uint64_t)m, (uint64_t)k, pg::BM) || pg::make_map_q8(&mq, dstream, (uint64_t)rows, nseg, unit, 0) ||
+                              pg::make_map_q8(&ms, dstream, (uint64_t)rows, nseg, unit, 1) || (!gateup && pg::make_map_c(&mc, dc, (uint64_t)m, (uint64_t)n))))
+            rc = B200_ERR_CUDA;
+        if (gateup) mc = mq; // unused by the gate/up epilogue
+        int lr = 0;
+        if (rc == B200_OK) {
+            using pg::B_Q8;
+            constexpr int S4 = pg::GEMM_STAGES, S5 = pg::GEMM_STAGES_DEEP_Q8;
+            const int mt = m / pg::BM, nt = n / (gateup ? pg::BN / 2 : pg::BN);
+            const bool deep = stages == S5;
+            if (mode == pg::GEMM_F32)
+                lr = deep ? pg::gemm_launch<pg::GEMM_F32, S5, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg)
+                          : pg::gemm_launch<pg::GEMM_F32, S4, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg);
+            else if (mode == pg::GEMM_RESID)
+                lr = deep ? pg::gemm_launch<pg::GEMM_RESID, S5, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg)
+                          : pg::gemm_launch<pg::GEMM_RESID, S4, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg);
+            else
+                lr = deep ? pg::gemm_launch<pg::GEMM_GATEUP, S5, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg)
+                          : pg::gemm_launch<pg::GEMM_GATEUP, S4, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg);
+            if (lr == -6) rc = B200_ERR_BAD_ARG;
+            else if (lr) rc = B200_ERR_CUDA;
+        }
+        if (ok(cudaDeviceSynchronize()) && rc == B200_OK) ok(cudaMemcpy(c, dc, c_bytes, cudaMemcpyDeviceToHost));
+    }
+    cudaFree(da); cudaFree(draw); cudaFree(dstream); cudaFree(dc);
     return rc;
 }
 

@@ -28,10 +28,16 @@ struct PrefillLayerMaps {
     CUtensorMap qkv, wo, w1, w3, w2; // weight boxes of 128 rows (64 for w1 / w3: the gate/up tile is 64 + 64)
 };
 
+// W8A16: quant / scale maps (pg::make_map_q8) of the layer's tile-major Q8_0 streams; the gate/up stream is one map pair
+struct PrefillQ8Maps {
+    CUtensorMap qkv_q, qkv_s, wo_q, wo_s, gu_q, gu_s, w2_q, w2_s;
+};
+
 struct PrefillCtx {
-    int batch = 0, bpad = 0;
-    bool ready = false; // tensor-core path usable for this plan
-    int mode = 0;       // 0 = exact token-by-token graph, 1 = tensor-core GEMMs
+    int batch = 0, bpad = 0; // bpad > 0: the scratch buffers below exist
+    bool ready = false;    // tensor-core path with f16 weight matrices usable for this plan
+    bool q8_ready = false; // W8A16 tensor-core path (B from the Q8_0 streams) usable for this plan
+    int mode = 0;          // 0 = exact token-by-token graph, 1 = tensor-core GEMMs (f16 B), 2 = tensor-core GEMMs (Q8_0 B, W8A16)
     bool att_simt = false; // debug: FP32 SIMT attention instead of the mma.sync kernel (B200_PF_ATT=simt)
     float *X = nullptr, *QKV = nullptr;
     __half *A16 = nullptr, *ATT16 = nullptr, *H16 = nullptr;
@@ -40,7 +46,9 @@ struct PrefillCtx {
     CUtensorMap mA, mATT, mH; // GEMM A operands (f16 activations)
     CUtensorMap mX, mQKV;     // GEMM outputs written by TMA (f32)
     std::vector<PrefillLayerMaps> maps;
+    std::vector<PrefillQ8Maps> maps_q8;
     const char *why = "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
+    const char *why_q8 = "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
 };
 
 // ---- elementwise kernels ------------------------------------------------------------------------

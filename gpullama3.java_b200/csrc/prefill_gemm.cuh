@@ -8,6 +8,13 @@
 //
 // Warp groups (384 threads): warp group 0 = TMA producer (one elected thread), warp groups 1 and 2 = consumers;
 // consumer c issues the wgmmas for rows 64*c .. 64*c+63 of the 128 x 128 tile and runs their epilogue.
+//
+// W8A16 (BSRC = B_Q8): B comes straight from the decode kernels' tile-major Q8_0 stream (stream_matvec.cuh), as the
+// reference's gemmMMAQ8 family does with packQ8Halves (TransformerBatchPrefillKernels.java:1544-1580).  Per k-block the
+// producer thread loads 128 rows x (64 int8 quants + the 16-byte line holding their two f16 scales) into a raw ring next
+// to the operand ring; warps 1-3 of the producer warp group turn it into the f16 B tile f16(q * d) in exactly the
+// SWIZZLE_128B layout TMA gives the f16 path, then arrive on the stage's full barrier.  The wgmma loop and the
+// epilogues are the same code for both sources.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -22,6 +29,11 @@ constexpr int GEMM_THREADS = 384;
 // pair: the B tile is 64 rows of W1 and 64 rows of W3 for the same 64 hidden units, so accumulator columns
 // [0,64) = gate, [64,128) = up, and the epilogue emits f16(silu(gate)*up) (InferenceCore.java:150-158).
 enum { GEMM_F32 = 0, GEMM_RESID = 1, GEMM_GATEUP = 2 };
+// B operand sources: an f16 [N][K] matrix through TMA, or the tile-major Q8_0 stream dequantised in shared memory
+enum { B_F16 = 0, B_Q8 = 1 };
+// W8A16 raw stage: 128 rows x 64 quants, then 128 rows x the 16-byte scale line holding the k-block's two scales
+constexpr int Q8_QUANT_BYTES = BN * BK, Q8_SCALE_BYTES = BN * 16, Q8_RAW_BYTES = Q8_QUANT_BYTES + Q8_SCALE_BYTES;
+constexpr int Q8_CONVERTERS = 96; // warps 1-3 of the producer warp group
 
 __device__ __forceinline__ uint32_t s32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t cnt) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(cnt)); }
@@ -45,6 +57,30 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
                  "l"(map), "r"(c0), "r"(c1), "r"(bar)
                  : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap *map, int c0, int c1, int c2, int c3, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::"r"(dst),
+                 "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
+                 : "memory");
+}
+
+// 8 int8 quants (two words, lowest byte = lowest column) -> 8 f16 values f16(q * d), as one 16-byte chunk.  q ^ 0x80 is
+// q + 128 as an unsigned byte; under the exponent byte 0x64 it reads as the f16 1024 + (q + 128), and subtracting 1152
+// leaves q exactly.  The f16 product q * d is rounded once, so the value is __float2half_rn((float)q * (float)d): the
+// f32 product of an 8-bit and an 11-bit significand is exact.
+__device__ __forceinline__ uint4 q8_chunk_to_f16(uint2 q, __half2 d) {
+    const __half2 bias = __half2half2(__ushort_as_half((unsigned short)0x6480)); // 1152
+    const uint32_t u0 = q.x ^ 0x80808080u, u1 = q.y ^ 0x80808080u;
+    uint32_t w[4] = {__byte_perm(u0, 0x64646464u, 0x4140), __byte_perm(u0, 0x64646464u, 0x4342), __byte_perm(u1, 0x64646464u, 0x4140),
+                     __byte_perm(u1, 0x64646464u, 0x4342)};
+    uint4 o;
+    uint32_t *po = reinterpret_cast<uint32_t *>(&o);
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const __half2 v = __hmul2_rn(__hsub2(*reinterpret_cast<const __half2 *>(&w[i]), bias), d);
+        po[i] = *reinterpret_cast<const uint32_t *>(&v);
+    }
+    return o;
 }
 // wgmma shared-memory matrix descriptor, K-major operand, 128-byte swizzle: start address >> 4 (bits 0-13) | LBO (unused for
 // swizzled K-major, 1) << 16 | SBO = 8 rows * 128 B >> 4 << 32 | layout SWIZZLE_128B (1) << 62.  The tile base is 1024-byte aligned.
@@ -75,28 +111,41 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, ui
         : "memory");
 }
 
-template <int STAGES> constexpr size_t smem_bytes() { return (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + 2 * STAGES * 8 + 1024; }
+// W8A16 raw ring depth: as deep as the 227 KB budget allows next to the operand ring (at most 8), so the weight bytes are
+// requested from HBM well before the converters need them
+template <int STAGES> __host__ __device__ constexpr int q8_raw_stages() {
+    return (227 * 1024 - STAGES * (BM * BK * 2 + BN * BK * 2) - 2048) / Q8_RAW_BYTES < 8 ? (227 * 1024 - STAGES * (BM * BK * 2 + BN * BK * 2) - 2048) / Q8_RAW_BYTES : 8;
+}
+template <int STAGES, int BSRC = B_F16> constexpr size_t smem_bytes() {
+    return (size_t)STAGES * (BM * BK * 2 + BN * BK * 2) + (BSRC == B_Q8 ? (size_t)q8_raw_stages<STAGES>() * (Q8_RAW_BYTES + 8) : 0) + 2 * STAGES * 8 + 1024;
+}
 
 // grid = (M tiles, N tiles, K splits): the CTAs that share a weight (B) tile are adjacent in launch order, so the
 // tile comes from HBM once and from L2 for the others; A (activations, a few MB) lives in L2.
 // C: row stride ldc (elements); rows >= m_valid are not stored (GEMM_F32 / GEMM_RESID write zeros / add zeros there,
 // inside the padded buffer).  GEMM_GATEUP: N tiles index 64 hidden units.  Split z owns k-blocks [z * kb_per_split, +kb_per_split).
-template <int MODE, int STAGES>
+// BSRC = B_Q8: tma_b / tma_b2 are the quant / scale maps of the Q8_0 stream (make_map_q8), seg its segment width.
+template <int MODE, int STAGES, int BSRC = B_F16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                                                                  const __grid_constant__ CUtensorMap tma_b2, const __grid_constant__ CUtensorMap tma_c,
-                                                                 void *__restrict__ Cv, int ldc, int m_valid, int K, int kb_per_split) {
+                                                                 void *__restrict__ Cv, int ldc, int m_valid, int K, int kb_per_split, int seg) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023); // SWIZZLE_128B tiles need 1024-byte alignment
-    constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2;
+    constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, RAW_BYTES = BSRC == B_Q8 ? Q8_RAW_BYTES : 0;
+    constexpr int RSTAGES = BSRC == B_Q8 ? q8_raw_stages<STAGES>() : 0;
     static_assert(STAGES * (A_BYTES + B_BYTES) >= BM * BN * 4, "the C tile is staged in the operand ring");
-    uint8_t *sA = smem, *sB = smem + STAGES * A_BYTES;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + STAGES * B_BYTES);
-    const uint32_t full0 = s32(bars), empty0 = s32(bars + STAGES);
+    uint8_t *sA = smem, *sB = smem + STAGES * A_BYTES, *sR = sB + STAGES * B_BYTES;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sR + RSTAGES * RAW_BYTES);
+    // raw: a W8A16 raw stage has landed.  The converters own the raw ring: they refill a stage once all of them have
+    // converted it, so its loads run up to RSTAGES k-blocks ahead, independent of the operand ring.
+    const uint32_t full0 = s32(bars), empty0 = s32(bars + STAGES), raw0 = s32(bars + 2 * STAGES);
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        // empty: one arrival per consumer warp once its wgmmas have read the stage
-        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8); }
+        // empty: one arrival per consumer warp once its wgmmas have read the stage.  full (W8A16): the A load's expect_tx
+        // and one arrival for the converted B tile.
+        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, BSRC == B_Q8 ? 2 : 1); mbar_init(empty0 + 8 * s, 8); }
+        for (int s = 0; s < RSTAGES; s++) mbar_init(raw0 + 8 * s, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -111,14 +160,61 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid
             for (int kb = 0; kb < nk; kb++) {
                 const int st = kb % STAGES;
                 mbar_wait(empty0 + 8 * st, ((kb / STAGES) & 1) ^ 1);
-                mbar_expect_tx(full0 + 8 * st, A_BYTES + B_BYTES);
                 const int kc = (kb0 + kb) * BK;
+                if (BSRC == B_Q8) { // B arrives through the converters
+                    mbar_expect_tx(full0 + 8 * st, A_BYTES);
+                    tma_load_2d(s32(sA + st * A_BYTES), &tma_a, kc, m0, full0 + 8 * st);
+                    continue;
+                }
+                mbar_expect_tx(full0 + 8 * st, A_BYTES + B_BYTES);
                 tma_load_2d(s32(sA + st * A_BYTES), &tma_a, kc, m0, full0 + 8 * st);
                 if (MODE == GEMM_GATEUP) {
                     tma_load_2d(s32(sB + st * B_BYTES), &tma_b, kc, n0, full0 + 8 * st);
                     tma_load_2d(s32(sB + st * B_BYTES + B_BYTES / 2), &tma_b2, kc, n0, full0 + 8 * st);
                 } else {
                     tma_load_2d(s32(sB + st * B_BYTES), &tma_b, kc, n0, full0 + 8 * st);
+                }
+            }
+        } else if constexpr (BSRC == B_Q8) {
+            // ===== W8A16 converters: raw stage -> f16 B tile.  Stream row n of the tile -> B row n (gate/up: slots 0, 1 of
+            // group n / 4 are gate rows, 2, 3 up rows -> rows 2(n/4) + (n&1), +64 for up).  Work item i = (row i / 8,
+            // 8-column chunk i % 8): a warp reads 256 consecutive quant bytes and writes four whole 128-byte rows. =====
+            if (warp == 0) return;
+            const int ct = threadIdx.x - 32;
+            const int g0 = (MODE == GEMM_GATEUP ? 2 * n0 : n0) / 4; // stream rows 4 g0 .. 4 g0 + 127 (gate/up: the 64 hidden units from n0 on)
+            // k-block kb -> raw stage kb % RSTAGES: the quants of segment s, columns j .. j+63, and the 16-byte aligned line of
+            // 8 scales (256 columns) holding their two (a box starting at an unaligned byte faults; the line never passes
+            // the unit's 16-byte padded end)
+            auto load_raw = [&](int kb) {
+                const int kc = (kb0 + kb) * BK, s = kc / seg, j = kc - s * seg, rs = kb % RSTAGES;
+                mbar_expect_tx(raw0 + 8 * rs, RAW_BYTES);
+                tma_load_4d(s32(sR + rs * RAW_BYTES), &tma_b, j, 0, s, g0, raw0 + 8 * rs);
+                tma_load_4d(s32(sR + rs * RAW_BYTES + Q8_QUANT_BYTES), &tma_b2, seg + ((j >> 8) << 4), 0, s, g0, raw0 + 8 * rs);
+            };
+            if (ct == 0)
+                for (int kb = 0; kb < RSTAGES && kb < nk; kb++) load_raw(kb);
+            for (int kb = 0; kb < nk; kb++) {
+                const int st = kb % STAGES, rs = kb % RSTAGES;
+                mbar_wait(raw0 + 8 * rs, (kb / RSTAGES) & 1);
+                mbar_wait(empty0 + 8 * st, ((kb / STAGES) & 1) ^ 1); // the consumers have read the B tile this stage held
+                const int j = (kb0 + kb) * BK % seg;                 // column of the k-block in its segment
+                const uint8_t *rq = sR + rs * RAW_BYTES, *rsc = rq + Q8_QUANT_BYTES + ((j & 255) >> 4); // its first scale in the line
+                uint8_t *dst = sB + st * B_BYTES;
+#pragma unroll 4
+                for (int i = ct; i < BN * 8; i += Q8_CONVERTERS) {
+                    const int n = i >> 3, ch = i & 7;
+                    const int row = MODE == GEMM_GATEUP ? ((n & 2) << 5) + ((n >> 2) << 1) + (n & 1) : n;
+                    const uint2 q = *reinterpret_cast<const uint2 *>(rq + 64 * n + 8 * ch);
+                    const __half d = *reinterpret_cast<const __half *>(rsc + 16 * n + 2 * (ch >> 2));
+                    *reinterpret_cast<uint4 *>(dst + 128 * row + ((ch ^ (row & 7)) << 4)) = q8_chunk_to_f16(q, __half2half2(d));
+                }
+                // the generic-proxy stores (and raw reads) are ordered before wgmma's reads (and the raw stage's refill), then
+                // one thread signals the tile and refills the raw stage every converter is done with
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                asm volatile("bar.sync 2, %0;" ::"n"(Q8_CONVERTERS) : "memory");
+                if (ct == 0) {
+                    mbar_arrive(full0 + 8 * st);
+                    if (kb + RSTAGES < nk) load_raw(kb + RSTAGES);
                 }
             }
         }
@@ -244,24 +340,45 @@ inline int make_map_c(CUtensorMap *map, const void *base, uint64_t rows, uint64_
     return r == CUDA_SUCCESS ? 0 : -2;
 }
 
+// The tile-major Q8_0 stream (stream_matvec.cuh) as a 4-D byte tensor {unit byte, slot r, segment s, group G}: every
+// stride a multiple of 16.  which = 0: the quant box {64, 4, 1, 32} (128 rows x one k-block); which = 1: the scale box
+// {16, 4, 1, 32} (128 rows x the 16-byte aligned line of 8 scales that holds the k-block's two).
+inline int make_map_q8(CUtensorMap *map, const void *base, uint64_t rows, int nseg, int unit_bytes, int which) {
+    EncodeTiledFn fn = encode_fn();
+    if (!fn) return -1;
+    cuuint64_t dims[4] = {(cuuint64_t)unit_bytes, 4, (cuuint64_t)nseg, rows / 4};
+    cuuint64_t strides[3] = {(cuuint64_t)unit_bytes, 4ull * unit_bytes, 4ull * unit_bytes * nseg};
+    cuuint32_t box[4] = {which ? 16u : (cuuint32_t)BK, 4, 1, BN / 4};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                    CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS ? 0 : -2;
+}
+
 // 4 stages x 32 KB of operands: the default ring (the C tile, 64 KB, is staged in it).  6 stages (192 KB) is the deep
-// variant the GEMM test also runs, so a ring that wraps at a different k-block is exercised too.
-constexpr int GEMM_STAGES = 4, GEMM_STAGES_DEEP = 6;
+// variant the GEMM test also runs, so a ring that wraps at a different k-block is exercised too.  W8A16 adds a 10 KB
+// raw stage per stage, so its deep variant is 5 stages (211 KB).
+constexpr int GEMM_STAGES = 4, GEMM_STAGES_DEEP = 6, GEMM_STAGES_DEEP_Q8 = 5;
+static_assert(smem_bytes<GEMM_STAGES_DEEP_Q8, B_Q8>() <= 227 * 1024, "W8A16 deep ring exceeds the shared-memory budget");
 
 // m_tiles x n_tiles output tiles, K split into `splits` ranges (GEMM_RESID only: every split reduce-adds its partial product).
-// B maps have box rows BN (BN / 2 for the W1 / W3 maps of GEMM_GATEUP).
-template <int MODE, int STAGES>
+// B maps have box rows BN (BN / 2 for the W1 / W3 maps of GEMM_GATEUP).  BSRC = B_Q8: b / b2 are the make_map_q8 quant /
+// scale maps of one stream, seg its segment width (a multiple of BK, so no k-block straddles two segments).
+template <int MODE, int STAGES, int BSRC = B_F16>
 inline int gemm_launch(const CUtensorMap &a, const CUtensorMap &b, const CUtensorMap &b2, const CUtensorMap &c, void *C, int ldc, int m_valid, int m_tiles,
-                       int n_tiles, int K, cudaStream_t stream, int splits = 1) {
+                       int n_tiles, int K, cudaStream_t stream, int splits = 1, int seg = 0) {
     static bool attr = false; // one flag per instantiation
     if (!attr) {
-        if (cudaFuncSetAttribute(k_gemm_f16_wgmma<MODE, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<STAGES>()) != cudaSuccess) return -4;
+        if (cudaFuncSetAttribute(k_gemm_f16_wgmma<MODE, STAGES, BSRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<STAGES, BSRC>()) != cudaSuccess)
+            return -4;
         attr = true;
     }
     if (splits < 1 || (splits > 1 && MODE != GEMM_RESID)) return -6;
+    if (BSRC == B_Q8 && (seg <= 0 || seg % BK || K % seg)) return -6;
     const int nk = (K + BK - 1) / BK, per = (nk + splits - 1) / splits;
     if ((splits - 1) * per >= nk) return -6; // an empty split would store an unwritten accumulator
-    k_gemm_f16_wgmma<MODE, STAGES><<<dim3(m_tiles, n_tiles, splits), GEMM_THREADS, smem_bytes<STAGES>(), stream>>>(a, b, b2, c, C, ldc, m_valid, K, per);
+    k_gemm_f16_wgmma<MODE, STAGES, BSRC><<<dim3(m_tiles, n_tiles, splits), GEMM_THREADS, smem_bytes<STAGES, BSRC>(), stream>>>(a, b, b2, c, C, ldc, m_valid, K,
+                                                                                                                          per, seg);
     return cudaGetLastError() == cudaSuccess ? 0 : -5;
 }
 

@@ -163,7 +163,11 @@ public final class B200MasterPlan implements AutoCloseable {
         if (rc != 0) check(rc, lastError());
     }
 
-    /** TensorCoreSupport.java's switch: 0 = exact token-by-token prefill (bit-identical KV cache), 1 = TMA + wgmma GEMMs. */
+    public static final int PREFILL_EXACT = 0, PREFILL_TENSOR_CORE = 1, PREFILL_TENSOR_CORE_W8A16 = 2;
+
+    /** TensorCoreSupport.java's switch: 0 = exact token-by-token prefill (bit-identical KV cache), 1 = TMA + wgmma GEMMs (a Q8_0
+     *  plan first builds f16 twins of its matrices, +2 bytes per weight), 2 = the same GEMMs on a Q8_0 plan reading the Q8_0 weights
+     *  in place and dequantising them in shared memory (no twins; bit-identical to 1 where no residual GEMM splits K). */
     public void setPrefillMode(int mode) throws Throwable {
         int rc = (int) SET_PREFILL_MODE.invokeExact(plan, mode);
         if (rc != 0) check(rc, lastError());

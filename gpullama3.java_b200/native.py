@@ -41,7 +41,7 @@ class Tensor(C.Structure):
 
 EXPORTS = ["b200_plan_create", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
-           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_test_seqsum", "b200_gemm_f16", "b200_test_gemm", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
+           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_test_seqsum", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -76,6 +76,7 @@ def lib() -> C.CDLL:
     L.b200_prefill_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
     L.b200_gemm_f16.argtypes = [vp, vp, vp, i32, i32, i32, i32, C.POINTER(C.c_float)]
     L.b200_test_gemm.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
+    L.b200_test_gemm_q8.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.b200_test_pf_attention.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.b200_time_kernel.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
     L.b200_read_buffer.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
@@ -162,6 +163,29 @@ def test_gemm(mode: str, a, b, c, b2=None, m_valid: int | None = None, stages: i
                               b2.ctypes.data if gateup else None, c.ctypes.data)
     if rc != B200_OK:
         _raise(rc, "b200_test_gemm failed")
+    return c
+
+
+def test_gemm_q8(mode: str, a, bq, c, bq2=None, m_valid: int | None = None, stages: int = 4, splits: int = 1) -> np.ndarray:
+    """One launch of the W8A16 prefill GEMM (B dequantised from the tile-major Q8_0 stream in shared memory) as the
+    B200_PREFILL_TENSOR_CORE_W8A16 prefill issues it.  As test_gemm, but bq (and bq2 for "gateup") are GGUF Q8_0 blocks:
+    uint8 [N, K / 32 * 34].  stages 4 or 5."""
+    a = np.ascontiguousarray(a, dtype=np.float16)
+    bq = np.ascontiguousarray(bq, dtype=np.uint8)
+    gateup = mode == "gateup"
+    c = np.array(c, dtype=np.float16 if gateup else np.float32, order="C", copy=True)
+    m, k = a.shape
+    n = bq.shape[0]
+    if bq.shape != (n, k // 32 * 34) or k % 32 or c.shape != (m, n):
+        raise ValueError("shapes do not match")
+    if gateup:
+        bq2 = np.ascontiguousarray(bq2, dtype=np.uint8)
+        if bq2.shape != bq.shape:
+            raise ValueError("bq2 must have the shape of bq")
+    rc = lib().b200_test_gemm_q8(GEMM_MODES[mode], stages, splits, m, m if m_valid is None else m_valid, n, k, a.ctypes.data, bq.ctypes.data,
+                                 bq2.ctypes.data if gateup else None, c.ctypes.data)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_gemm_q8 failed")
     return c
 
 

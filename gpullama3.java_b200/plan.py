@@ -117,12 +117,14 @@ class B200MasterPlan:
         self._native.forward_batch_prefill(np.asarray(tokens, dtype=np.int32), start_pos)
 
     # TensorCoreSupport.java's switch between the MMA and the plain batch-prefill layer families
-    PREFILL_EXACT, PREFILL_TENSOR_CORE = 0, 1
+    PREFILL_EXACT, PREFILL_TENSOR_CORE, PREFILL_TENSOR_CORE_W8A16 = 0, 1, 2
 
     def set_prefill_mode(self, mode):
-        """"exact" (token-by-token graph, bit-identical KV cache) or "tensor_core" (wgmma GEMMs, FP16 tolerance)."""
+        """"exact" (token-by-token graph, bit-identical KV cache), "tensor_core" (wgmma GEMMs, FP16 tolerance; a Q8_0 plan
+        builds f16 twins of its matrices) or "tensor_core_w8a16" (Q8_0 plans: the same GEMMs reading the Q8_0 weights in
+        place, dequantised in shared memory; bit-identical to "tensor_core" where no residual GEMM splits K)."""
         if isinstance(mode, str):
-            mode = {"exact": 0, "tensor_core": 1}[mode]
+            mode = {"exact": 0, "tensor_core": 1, "tensor_core_w8a16": 2}[mode]
         self._native.set_prefill_mode(int(mode))
 
     def prefill_info(self):

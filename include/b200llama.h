@@ -131,9 +131,18 @@ int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n
  *                            dequantises f16 twins of the weight matrices on the device (+2 bytes/weight);
  *                            there the CPU path additionally rounds activations to int8, so agreement is
  *                            percent-level, not FP16-level -- hence not the default.  Returns
- *                            B200_ERR_UNSUPPORTED with the reason in b200_last_error when unavailable. */
+ *                            B200_ERR_UNSUPPORTED with the reason in b200_last_error when unavailable.
+ *   B200_PREFILL_TENSOR_CORE_W8A16  the same batched prefill on a single-GPU Q8_0 plan (K-quant plans included) on the
+ *                            streaming layout, with the GEMMs' B operand dequantised to f16(q * scale) in shared memory
+ *                            from the tile-major Q8_0 stream the decode kernels read: no f16 twins, 1.06 instead of
+ *                            2 bytes per weight streamed.  Bit-identical to B200_PREFILL_TENSOR_CORE except where a
+ *                            residual GEMM splits K (the order of the f32 reduce-adds is not fixed in either mode).
+ *                            The first call allocates the prefill scratch and builds tensor maps only.  Needs every
+ *                            stream segment to be a multiple of 64 columns; B200_ERR_UNSUPPORTED with the reason
+ *                            otherwise.  The two tensor-core modes can be switched in either order on one plan. */
 #define B200_PREFILL_EXACT 0
 #define B200_PREFILL_TENSOR_CORE 1
+#define B200_PREFILL_TENSOR_CORE_W8A16 2
 int b200_set_prefill_mode(b200_plan *plan, int32_t mode);
 
 /* Active mode, kernels launched and device milliseconds of the last tensor-core chunk (any pointer may be NULL). */
@@ -252,6 +261,14 @@ int b200_gemm_f16(const uint16_t *a, const uint16_t *b, float *c, int32_t m, int
  * 64-wide k-block, is rejected with B200_ERR_BAD_ARG. */
 int b200_test_gemm(int32_t mode, int32_t stages, int32_t splits, int32_t m, int32_t m_valid, int32_t n, int32_t k, const uint16_t *a, const uint16_t *b,
                    const uint16_t *b2 /* GATEUP only */, void *c);
+
+/* Test hook: ONE launch of the W8A16 prefill GEMM exactly as B200_PREFILL_TENSOR_CORE_W8A16 launches it.  As b200_test_gemm,
+ * but B (and B2 = W3 for GATEUP) are GGUF Q8_0 blocks (34 bytes per 32 weights, row-major [n][k]); they are repacked into
+ * the tile-major stream by the plan's upload kernel (gate/up interleaved as in the plan) and dequantised inside the GEMM
+ * to f16(q * scale).  stages = 4 or 5.  K whose stream segment (smv_pick_nseg) is not a multiple of 64 columns is
+ * rejected with B200_ERR_BAD_ARG, like the shapes and split counts b200_test_gemm rejects. */
+int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, int32_t m_valid, int32_t n, int32_t k, const uint16_t *a, const void *bq,
+                      const void *bq2 /* GATEUP only */, void *c);
 
 /* Test hook: the causal attention of the tensor-core prefill over one chunk of n query tokens at positions start_pos ..
  * start_pos + n - 1.  q: f32 [n][n_heads * head_size] (rotated); k, v: f32 [start_pos + n][n_kv_heads * head_size] (the KV cache

@@ -1828,6 +1828,33 @@ int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out
     return run_seqsum_hook(terms, n, threads, out, info);
 }
 
+int b200_test_sample(const float *logits, int32_t n, float temperature, float topp, float uniform01, int32_t *token_out, int32_t *info, float *probs_out) {
+    if (!logits || !token_out || n < 1) return B200_ERR_BAD_ARG;
+    if (!(temperature > 0.0f) || !(uniform01 >= 0.0f && uniform01 < 1.0f)) return B200_ERR_BAD_ARG;
+    const size_t padded = (size_t)sampler_padded(n) * 4;
+    float *dl = nullptr;
+    int *di = nullptr, *dout = nullptr;
+    int rc = B200_OK;
+    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
+    // the index scratch starts as 0xFF bytes: a slot the kernel did not write in this call reads as -1
+    if (ok(cudaMalloc(&dl, padded)) && ok(cudaMalloc(&di, (size_t)n * 4)) && ok(cudaMalloc(&dout, 8 * 4)) && ok(cudaMemset(dl, 0, padded)) &&
+        ok(cudaMemcpy(dl, logits, (size_t)n * 4, cudaMemcpyHostToDevice)) && ok(cudaMemset(di, 0xFF, (size_t)n * 4)) && ok(cudaMemset(dout, 0xFF, 8 * 4)) &&
+        ok(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()))) {
+        SamplerArgs a;
+        a.logits = dl; a.n = n; a.temperature = temperature; a.topp = topp; a.r01 = uniform01;
+        a.indices = di; a.out_id = dout; a.info = dout + 1;
+        k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(a);
+        int32_t h[5];
+        if (ok(cudaGetLastError()) && ok(cudaDeviceSynchronize()) && ok(cudaMemcpy(h, dout, 5 * 4, cudaMemcpyDeviceToHost))) {
+            *token_out = h[0];
+            if (info) for (int k = 0; k < 4; k++) info[k] = h[1 + k];
+            if (probs_out) ok(cudaMemcpy(probs_out, dl, (size_t)n * 4, cudaMemcpyDeviceToHost));
+        }
+    }
+    cudaFree(dl); cudaFree(di); cudaFree(dout);
+    return rc;
+}
+
 int b200_requant_kquant(int32_t ggml_type, const void *src, int64_t n_elems, void *dst_q8_0) {
     if (!src || !dst_q8_0 || n_elems <= 0 || n_elems % 256 || !kq_is_kquant(ggml_type)) return B200_ERR_BAD_ARG;
     const size_t raw = (size_t)(n_elems / 256) * kq_block_bytes(ggml_type), q8 = (size_t)(n_elems / 32) * 34;

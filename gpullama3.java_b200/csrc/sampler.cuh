@@ -92,7 +92,7 @@ __global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample(SamplerArgs a) {
         }
         return;
     }
-    // ---- top-p: ordered compaction of the candidates (ToppSampler.java:70-78; the rejected tail is never read again)
+    // ---- top-p: ordered compaction of the candidates (ToppSampler.java:70-78; the rejected tail is not written, see n0 == 0 below)
     const float cutoff = __fdiv_rn(__fsub_rn(1.0f, a.topp), (float)(n - 1));
     __shared__ int s_base;
     if (tid == 0) s_base = 0;
@@ -124,6 +124,14 @@ __global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample(SamplerArgs a) {
     // ---- the reference's heap, verbatim mechanics (processTopP :114-156)
     int *idx = a.indices;
     const int n0 = s_base;
+    if (n0 == 0) {
+        // No candidate (a flat row with topp < 1/n, or NaN probabilities): the reference fills rejected ids in from the tail
+        // (ToppSampler.java:71-77), so its indices[0] is n - 1, and with lastIndex = 0 it returns that slot (:155).  This kernel
+        // writes only the candidates; every other path reads idx[0, n0) alone (last <= n0 - 1, siftDown(..., i - 1) < n0).
+        *a.out_id = n - 1;
+        if (a.info) { a.info[0] = 0; a.info[1] = 0; }
+        return;
+    }
     for (int i = n0 / 2 - 1; i >= 0; --i) sampler_sift_down(idx, i, n0, p);
     float cumulative = 0.0f;
     int last = 0;

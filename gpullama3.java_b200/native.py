@@ -40,7 +40,7 @@ class Tensor(C.Structure):
 
 
 EXPORTS = ["b200_plan_create", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
-           "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
+           "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_test_seqsum", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
@@ -73,6 +73,7 @@ def lib() -> C.CDLL:
     L.b200_decode_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     L.b200_trace_persistent.argtypes = [vp, i32, i32, vp, C.c_int64, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     L.b200_test_seqsum2.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(i32)]
+    L.b200_test_sample.argtypes = [vp, i32, C.c_float, C.c_float, C.c_float, C.POINTER(i32), C.POINTER(i32), vp]
     L.b200_prefill_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
     L.b200_gemm_f16.argtypes = [vp, vp, vp, i32, i32, i32, i32, C.POINTER(C.c_float)]
     L.b200_test_gemm.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
@@ -111,6 +112,19 @@ def test_seqsum(terms, want_info: bool = False, threads: int = 0):
     if rc != B200_OK:
         _raise(rc, "b200_test_seqsum failed")
     return (out.value, info[0], info[1]) if want_info else out.value
+
+
+def test_sample(logits, temperature: float, topp: float, uniform01: float):
+    """One launch of the device sampler (csrc/sampler.cuh) as b200_forward_decode_sample issues it, on host logits.
+    Returns (token id, [top-p candidates, kept, seqsum items, seqsum fallbacks], float32 probabilities)."""
+    lg = np.ascontiguousarray(logits, dtype=np.float32)
+    probs = np.empty(len(lg), dtype=np.float32)
+    out = C.c_int32(-1)
+    info = (C.c_int32 * 4)()
+    rc = lib().b200_test_sample(lg.ctypes.data, len(lg), temperature, topp, uniform01, C.byref(out), info, probs.ctypes.data)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_sample failed")
+    return out.value, list(info), probs
 
 
 def requant_kquant(ggml_type: int, raw, n_elems: int) -> np.ndarray:

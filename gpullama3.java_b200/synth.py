@@ -58,6 +58,10 @@ SHAPES = {
     "tiny-llama-mha": Shape("llama", 256, 512, 2, 4, 4, 64, 512, False, 500000.0, 1e-5),
     "tiny-llama-gqa8": Shape("llama", 1024, 1024, 2, 16, 2, 64, 512, False, 500000.0, 1e-5),
     "tiny-llama-gqa4-hs128": Shape("llama", 1024, 1536, 2, 8, 2, 128, 512, False, 500000.0, 1e-5),
+    # the tiny geometries with the real vocabularies of Llama-3, Qwen3 and Phi-3 (the device sampler's softmax and top-p at full width)
+    "tiny-llama-vocab128k": Shape("llama", 256, 512, 2, 4, 2, 64, 128256, False, 500000.0, 1e-5),
+    "tiny-qwen3-vocab152k": Shape("qwen3", 256, 768, 2, 4, 2, 128, 151936, True, 1000000.0, 1e-6),
+    "tiny-phi3-vocab32k": Shape("phi3", 384, 768, 2, 4, 4, 96, 32064, False, 10000.0, 1e-5, 4096),
     "mid-phi3-mini": Shape("phi3", 3072, 8192, 2, 32, 32, 96, 8192, False, 10000.0, 1e-5, 4096),  # Phi-3-mini-4k layer geometry
     # mid shape: exercises column tails (dim not a multiple of 512) and several row tiles
     "small-llama": Shape("llama", 1536, 4096, 3, 12, 4, 128, 4096, False, 500000.0, 1e-5),

@@ -238,6 +238,14 @@ int b200_test_seqsum(const float *terms, int32_t n, float *out, int32_t *info /*
  * (the persistent decode kernel's form) or 256 threads; info = {items walked, fallbacks}. */
 int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out, int32_t *info /* nullable */);
 
+/* Test hook for the device-side sampler (csrc/sampler.cuh): ONE launch of k_sample as b200_forward_decode_sample issues it (same
+ * grid and shared memory, a logits buffer of whole 1024-float chunks with a zero pad) on n host logits.  Returns the sampled id, the
+ * diagnostics {top-p candidates, tokens kept, seqsum items, seqsum fallbacks} and the n probabilities the kernel leaves in place.
+ * The index scratch starts as 0xFF bytes, so a slot the kernel did not write in this call reads as -1.  temperature must be > 0
+ * (0 is the plan's argmax path, not this kernel), uniform01 in [0, 1), n >= 1; B200_ERR_BAD_ARG otherwise. */
+int b200_test_sample(const float *logits, int32_t n, float temperature, float topp, float uniform01,
+                     int32_t *token_out, int32_t *info /* nullable, 4 */, float *probs_out /* nullable, n */);
+
 /* Test hook for the device-side K-quant -> Q8_0 re-quantiser the upload pipeline applies to Q4_K / Q5_K / Q6_K tensors (csrc/kquant.cuh;
  * replaces ModelLoader.dequantizeToQ8_0TornadoTensor, model/loader/ModelLoader.java:173-224): host K-quant blocks in, host GGUF Q8_0
  * blocks (34 bytes per 32 elements) out, byte-identical to the reference's.  n_elems % 256 == 0. */

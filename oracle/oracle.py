@@ -101,35 +101,45 @@ class JavaLXM:
         return float(lib().oracle_lxm_next_float1(self._st))
 
 
-def sample(logits: np.ndarray, temperature: float, topp: float, r01: float) -> int:
-    """Sampler.selectSampler's lambda on a COPY of the logits (the reference modifies them in place)."""
+def sample(logits: np.ndarray, temperature: float, topp: float, r01: float, want_probs: bool = False):
+    """Sampler.selectSampler's lambda on a COPY of the logits (the reference modifies them in place).  want_probs: also return
+    that copy, which then holds the float32 probabilities (for temperature > 0)."""
     lg = np.ascontiguousarray(logits, dtype=np.float32).copy()
     idx = np.empty(len(lg), dtype=np.int32)
-    return int(lib().oracle_sample(lg.ctypes.data, len(lg), temperature, topp, r01, idx.ctypes.data))
+    tok = int(lib().oracle_sample(lg.ctypes.data, len(lg), temperature, topp, r01, idx.ctypes.data))
+    return (tok, lg) if want_probs else tok
 
 
-def np_sample(logits: np.ndarray, temperature: float, topp: float, r01: float) -> int:
+def np_sample(logits: np.ndarray, temperature: float, topp: float, r01: float, want_info: bool = False):
     """Second restatement of the same lines in numpy/Python (cross-check of the C code): sequential float32 sums via
-    np.add.accumulate for the categorical walk, a statement-by-statement port of the top-p heap."""
+    np.add.accumulate for the categorical walk, a statement-by-statement port of the top-p heap.  want_info: return
+    (id, candidates n0, tokens kept) -- n, n for the categorical walk, 0, 0 for greedy."""
     lg = np.asarray(logits, dtype=np.float32)
     if temperature == 0.0:
-        return int(np.argmax(lg))
-    x = (lg / np.float32(temperature)).astype(np.float32)
-    e = np.exp((x - x.max()).astype(np.float64)).astype(np.float32)
-    p = (e / np.add.accumulate(e, dtype=np.float32)[-1]).astype(np.float32)
+        tok = int(np.argmax(lg))
+        return (tok, 0, 0) if want_info else tok
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):  # x may overflow to inf (tiny T): NaN probabilities, as in Java
+        x = (lg / np.float32(temperature)).astype(np.float32)
+        e = np.exp((x - x.max()).astype(np.float64)).astype(np.float32)
+        p = (e / np.add.accumulate(e, dtype=np.float32)[-1]).astype(np.float32)
     n = len(p)
     if topp <= 0 or topp >= 1:
         cdf = np.add.accumulate(p, dtype=np.float32)
         hit = np.flatnonzero(np.float32(r01) < cdf)
-        return int(hit[0]) if len(hit) else n - 1
+        tok = int(hit[0]) if len(hit) else n - 1
+        return (tok, n, n) if want_info else tok
     # ToppSampler.sampleFromFloatTensor + processTopP, ported statement by statement (the popped order is NOT a perfect sort:
-    # the reference sifts with heap size i - 1, ToppSampler.java:131, so the heap mechanics are part of the result)
+    # the reference sifts with heap size i - 1, ToppSampler.java:131, so the heap mechanics are part of the result).
+    # indices: candidates from the head in index order, rejected ids from the tail (:71-77), so with no candidate the
+    # final `return indices[lastIndex]` (:155) gives n - 1.
     cutoff = (np.float32(1.0) - np.float32(topp)) / np.float32(n - 1)
-    idx = [i for i in range(n) if p[i] >= cutoff]
-    n0 = len(idx)
+    keep = p >= cutoff
+    idx = np.flatnonzero(keep).tolist() + np.flatnonzero(~keep)[::-1].tolist()
+    n0 = int(keep.sum())
+    pv = p.tolist()  # float32 values widened exactly: the comparisons are unchanged
 
     def less(x, y):  # comparator.compare(x, y) < 0  <=>  value(x) > value(y)
-        return p[x] > p[y]
+        return pv[x] > pv[y]
 
     def sift_down(frm, size):
         prev = frm
@@ -156,11 +166,13 @@ def np_sample(logits: np.ndarray, temperature: float, topp: float, r01: float) -
         sift_down(0, i - 1)
     r = np.float32(np.float32(r01) * cum)
     cdf = np.float32(0.0)
+    tok = int(idx[last])
     for i in range(n0 - 1, last - 1, -1):
         cdf = np.float32(cdf + p[idx[i]])
         if r < cdf:
-            return int(idx[i])
-    return int(idx[last])
+            tok = int(idx[i])
+            break
+    return (tok, n0, n0 - last) if want_info else tok
 
 
 def use_all_cores() -> int:

@@ -221,3 +221,67 @@ def test_sampler_restatements_agree(pkg, orc):
         assert orc.sample(lg, temp, topp, r) == orc.np_sample(lg, temp, topp, r), (n, temp, topp, r)
     # first strict maximum for temperature 0 (FloatTensor.argmax)
     assert orc.sample(np.array([1.0, 3.0, 3.0, 2.0], dtype=np.float32), 0.0, 0.9, 0.5) == 1
+    # real vocabulary sizes and the edges: flat rows, ties, masked (-inf) ids, overflowing logits / temperature, topp just below 1
+    for n in (2, 512, 32064, 128256):
+        flat = np.zeros(n, dtype=np.float32)
+        normal = (rng.standard_normal(n) * 3).astype(np.float32)
+        ties = (rng.integers(-12, 13, n) * 0.25).astype(np.float32)
+        masked = normal.copy()
+        masked[::7] = -np.inf
+        for r in (0.0, 0.5, TOPP_BELOW_1):
+            # no candidate passes the cutoff: the reference returns indices[0], which its tail fill set to n - 1
+            assert orc.sample(flat, 1.0, 1e-7, r) == orc.np_sample(flat, 1.0, 1e-7, r, want_info=True)[0] == n - 1, n
+            assert orc.np_sample(flat, 1.0, 1e-7, r, want_info=True)[1:] == (0, 0)
+            # NaN probabilities (logit / 1e-38 overflows to inf): no candidate either
+            if n > 2:
+                assert orc.sample(normal, 1e-38, 0.9, r) == orc.np_sample(normal, 1e-38, 0.9, r) == n - 1, n
+        for lg in (normal, ties, masked, flat):
+            for temp, topp in ((0.7, 0.9), (0.3, 0.95), (1.0, 0.0), (1.0, TOPP_BELOW_1), (2.0, 0.99)):
+                r = float(np.float32(rng.random()))
+                want, probs = orc.sample(lg, temp, topp, r, want_probs=True)
+                if 0 < topp < 1 and np.count_nonzero(probs >= np.float32(1 - np.float32(topp)) / np.float32(n - 1)) > 4000:
+                    continue  # the Python heap is too slow for ~1e5 candidates; the GPU tests cover these against the C oracle
+                assert want == orc.np_sample(lg, temp, topp, r), (n, temp, topp, r)
+
+
+TOPP_BELOW_1 = float(np.float32(1.0) - np.float32(2.0 ** -24))  # 0x1.fffffep-1, the largest float below 1
+
+
+def softmax_bound_violations(x: np.ndarray, p: np.ndarray) -> np.ndarray:
+    """Elements where the float32 probabilities p of the float32 scaled logits x = f32(l / T) leave the float64 softmax by more
+    than the error of the reference's float evaluation (max, rounded x - m, (float)Math.exp, sequential float sum, division):
+    |p_i - p64_i| <= 1.01 p64_i (d_i + max d_j + u sum_k S_k / S + 3u) + 2^-149 with u = 2^-24, d_i = u (1 + |x_i - m|) and
+    S_k the partial sums of the sequential sum."""
+    u = 2.0 ** -24
+    x64 = x.astype(np.float64)
+    m = x64.max()
+    with np.errstate(invalid="ignore"):
+        e = np.where(np.isneginf(x64), 0.0, np.exp(x64 - m))
+    S = e.sum()
+    p64 = e / S
+    d = u * (1.0 + np.where(np.isneginf(x64), 0.0, np.abs(x64 - m)))
+    bound = 1.01 * p64 * (d + d.max() + u * np.cumsum(e).sum() / S + 3 * u) + 2.0 ** -149
+    return np.flatnonzero(~(np.abs(p.astype(np.float64) - p64) <= bound))
+
+
+def test_oracle_softmax_matches_float64(orc):
+    """The oracle's probabilities (Sampler.java's divideInPlace + softmaxInPlace in float32) against the float64 softmax of the
+    same scaled logits, at real vocabulary sizes and on rows whose exponentials underflow (to zero or to subnormals)."""
+    rng = np.random.default_rng(11)
+    for n in (2, 1000, 32064, 151936):
+        normal = rng.standard_normal(n).astype(np.float32)
+        masked = (normal * 3).astype(np.float32)
+        masked[::7] = -np.inf
+        peaked = normal.copy()
+        peaked[n // 3] = normal.max() + 30
+        rows = {"normal": normal, "masked": masked, "peaked": peaked, "wide": (normal * 30).astype(np.float32),
+                "ties": (rng.integers(-12, 13, n) * 0.25).astype(np.float32), "flat": np.zeros(n, dtype=np.float32)}
+        for name, lg in rows.items():
+            for temp in (0.05, 0.3, 1.0, 2.0):
+                _, p = orc.sample(lg, temp, 0.0, 0.5, want_probs=True)
+                x = (lg / np.float32(temp)).astype(np.float32)
+                bad = softmax_bound_violations(x, p)
+                assert bad.size == 0, (n, name, temp, bad[:5], p[bad[:5]])
+                assert np.all(p[np.isneginf(lg)] == 0)
+                if name == "flat":
+                    assert np.all(p == np.float32(1) / np.float32(n))

@@ -412,7 +412,7 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ q
                                                           const StepState *__restrict__ st, const float *__restrict__ cr,
                                                           const float *__restrict__ ci, int n_heads, int n_kv_heads, int arch /* KF_* flags */,
                                                           const float *__restrict__ qnorm_w, const float *__restrict__ knorm_w,
-                                                          float eps, float sqrt_hs, int8_t *__restrict__ xq,
+                                                          const float *__restrict__ qkv_bias, float eps, float sqrt_hs, int8_t *__restrict__ xq,
                                                           float *__restrict__ xs, float *__restrict__ xb, TraceBuf tr, TpCtx tp,
                                                           unsigned tp_out_op, int head_base, float *att_scratch, int ctx) {
     extern __shared__ __align__(16) float sm[]; // q[HS] | k[HS] | out[HS] | att[ctx] (att in global scratch for long contexts)
@@ -439,7 +439,7 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ q
         }
     }
     const float *qsrc = qkv + h * HS, *ksrc = qkv + qd + kvh * HS, *vsrc = qkv + qd + kvd + kvh * HS;
-    // ---- prologue: threads [0,HALF) rotate q pairs, threads [HALF,HS) rotate k pairs
+    // ---- prologue: threads [0,HALF) rotate q pairs, threads [HALF,HS) rotate k pairs, threads [HS,2HS) take v
     if (tid < HS) {
         const bool is_q = tid < HALF;
         const int p = is_q ? tid : tid - HALF;
@@ -447,6 +447,11 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ q
         int i0, i1;
         if (arch & KF_NEOX) { i0 = p; i1 = p + HALF; } else { i0 = 2 * p; i1 = 2 * p + 1; }
         float v0 = src[i0], v1 = src[i1];
+        if (arch & KF_QKVBIAS) { // Qwen2: q / k bias (laid out like q|k|v) before the rotation
+            const float *b = qkv_bias + (is_q ? h * HS : qd + kvh * HS);
+            v0 = __fadd_rn(v0, b[i0]);
+            v1 = __fadd_rn(v1, b[i1]);
+        }
         if (arch & KF_QKNORM) { // Qwen3 per-head RMSNorm: literal sequential sum over the head
             float *sqr = is_q ? so : sk; // scratch: HS squares each
             sqr[i0] = __fmul_rn(v0, v0);
@@ -480,13 +485,19 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ q
                 const size_t o = (size_t)pos * kvd + kvh * HS;
                 kc[o + i0] = r0;
                 kc[o + i1] = r1;
-                vc[o + i0] = vsrc[i0];
-                vc[o + i1] = vsrc[i1];
                 // (the rotated k is NOT written back into qkv: the other query heads of this group read the
                 //  unrotated k from there concurrently)
             }
         }
         if (is_q) { qkv[h * HS + i0] = r0; qkv[h * HS + i1] = r1; }
+    } else if (tid < 2 * HS) { // v: the group's first head writes the cache; Qwen2 adds the bias and stages v for the weighted sum
+        const int j = tid - HS;
+        float w = vsrc[j];
+        if (arch & KF_QKVBIAS) {
+            w = __fadd_rn(w, qkv_bias[qd + kvd + kvh * HS + j]);
+            so[j] = w; // (so is scratch of the q/k norm only, which Qwen2 does not have)
+        }
+        if (h % kv_mul == 0) vc[(size_t)pos * kvd + kvh * HS + j] = w;
     }
     __syncthreads();
     // ---- scores (scalarDot, FloatTensor.java:86-92: one sequential unfused mul/add chain per key).  Four threads share a key: each loads
@@ -564,7 +575,7 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ q
         const int d = vd0 + vd;
         const bool live = d < HS;
         const float *vcol = vc + kvh * HS + d;
-        const float vcur = live ? vsrc[d] : 0.0f; // current position: straight from the packed qkv vector
+        const float vcur = live ? ((arch & KF_QKVBIAS) ? so[d] : vsrc[d]) : 0.0f; // current position: the packed qkv vector (biased: staged)
         float acc = 0.0f;
 #pragma unroll 1
         for (int r0 = 0; r0 < pos; r0 += 4 * VB) {

@@ -45,6 +45,7 @@ enum { PD_S_QKV = 0, PD_S_ATT = 1, PD_S_WO = 2, PD_S_GU = 3, PD_S_W2 = 4, PD_S_L
 struct PdLayer {
     TileMat qkv, wo, gu, w2;
     const float *attn_norm, *ffn_norm, *q_norm, *k_norm;
+    const float *qkv_bias; // Qwen2: this rank's q|k|v bias (KF_QKVBIAS), else NULL
     float *kc, *vc; // this layer's FP32 KV cache (this rank's KV heads)
 };
 
@@ -651,6 +652,7 @@ __device__ __noinline__ void pd_attention_head(const PdArgs &a, const PdLayer &L
     const int qd = a.n_heads * HS, kvd = a.n_kv_heads * HS;
     float *qkv = a.qkv, *kc = Ly.kc, *vc = Ly.vc;
     const float *qsrc = qkv + h * HS, *ksrc = qkv + qd + kvh * HS, *vsrc = qkv + qd + kvd + kvh * HS;
+    float vcur_own = 0.0f; // threads [HS,2HS): this position's v element (biased), staged in `so` once the prologue is over
     if (tid < HS) {
         const bool is_q = tid < HALF;
         const int p = is_q ? tid : tid - HALF;
@@ -658,11 +660,14 @@ __device__ __noinline__ void pd_attention_head(const PdArgs &a, const PdLayer &L
         int i0, i1;
         if (a.arch & KF_NEOX) { i0 = p; i1 = p + HALF; } else { i0 = 2 * p; i1 = 2 * p + 1; }
         float v0 = ldcg_f32c(src + i0), v1 = ldcg_f32c(src + i1); // written by other CTAs in this kernel: bypass L1
+        if (a.arch & KF_QKVBIAS) { // Qwen2: q / k bias (laid out like q|k|v) before the rotation (InferenceCore.java:456-459)
+            const float *b = Ly.qkv_bias + (is_q ? h * HS : qd + kvh * HS);
+            v0 = __fadd_rn(v0, b[i0]);
+            v1 = __fadd_rn(v1, b[i1]);
+        }
         const float *srope = reinterpret_cast<const float *>(smem + L.off_rope); // this position's rope row, staged at kernel start
         const float fcr = srope[p], fci = srope[HALF + p];
-        float cv0 = 0.f, cv1 = 0.f;
         const bool owner = (h % kv_mul == 0) && !is_q; // first query head of the KV group owns the cache write (InferenceCore.java:92-93)
-        if (owner) { cv0 = ldcg_f32c(vsrc + i0); cv1 = ldcg_f32c(vsrc + i1); }
         if (a.arch & KF_QKNORM) { // Qwen3 per-head RMSNorm: literal sequential sum over the head (InferenceCore.java:594-600)
             float *sqr = is_q ? so : sk;
             sqr[i0] = __fmul_rn(v0, v0);
@@ -691,11 +696,15 @@ __device__ __noinline__ void pd_attention_head(const PdArgs &a, const PdLayer &L
             const size_t o = (size_t)pos * kvd + kvh * HS;
             kc[o + i0] = r0;
             kc[o + i1] = r1;
-            vc[o + i0] = cv0;
-            vc[o + i1] = cv1;
         }
+    } else if (tid < 2 * HS) { // v (+ the Qwen2 bias): the group's first head writes the cache
+        const int j = tid - HS;
+        vcur_own = ldcg_f32c(vsrc + j);
+        if (a.arch & KF_QKVBIAS) vcur_own = __fadd_rn(vcur_own, Ly.qkv_bias[qd + kvd + kvh * HS + j]);
+        if (h % kv_mul == 0) vc[(size_t)pos * kvd + kvh * HS + j] = vcur_own;
     }
     pd_bar_sync();
+    if (tid >= HS && tid < 2 * HS) so[tid - HS] = vcur_own; // the q/k-norm scratch in `so` is done; read after the softmax barriers
     // ---- scores (scalarDot, FloatTensor.java:86-92: one sequential unfused mul/add chain per key).  Four threads share a key: each
     // loads ITS quarter of the K row at once (one L2 round trip per pass of PD_CT/4 keys instead of two dependent ones per key), then
     // the chain runs through the quad in element order, handed on by shuffle.  The V rows this thread will need are requested
@@ -775,7 +784,7 @@ __device__ __noinline__ void pd_attention_head(const PdArgs &a, const PdLayer &L
       // `quad` holds rows [128 r + 32 quad, +32) of round r, all requested before the chain starts; the chain itself (4 cycles per key, the
       // floor of this phase) runs through the quad in row order.
         const float *vcol = vc + kvh * HS + vd;
-        const float vcur = vlive ? ldcg_f32c(vsrc + vd) : 0.0f; // the current position's v, straight from the packed q|k|v vector
+        const float vcur = vlive ? so[vd] : 0.0f; // the current position's v, staged from the packed q|k|v vector by the prologue
         float acc = 0.0f;
 #pragma unroll 1
         for (int r0 = 0; r0 < pos; r0 += 4 * VB) {

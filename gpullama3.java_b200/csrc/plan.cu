@@ -29,6 +29,7 @@ struct LayerW {
     DevMat qkv, wo, w1, w3, w2;
     TileMat tqkv{}, two{}, tgu{}, tw2{}; // tile-major copies for the streaming kernel (Q8_0)
     float *attn_norm = nullptr, *ffn_norm = nullptr, *q_norm = nullptr, *k_norm = nullptr;
+    float *qkv_bias = nullptr; // Qwen2: this rank's q|k|v bias, laid out like the packed q|k|v vector
 };
 
 } // namespace
@@ -443,6 +444,31 @@ int upload_f32(b200_plan *p, const b200_tensor *t, int n, float **dst, const cha
     return B200_OK;
 }
 
+// Qwen2's blk.N.attn_{q,k,v}.bias (F32, one dimension of qd / kvd / kvd floats) as one packed q|k|v vector of this rank's heads:
+// q rows rank * qd_l .., k and v rows rank * kvd_l .. (the biases are row-sharded with the heads, like the matrices).
+int upload_qkv_bias(b200_plan *p, const b200_tensor *tensors, int n_tensors, int layer, float **dst) {
+    const std::string pre = "blk." + std::to_string(layer) + ".";
+    const char *names[3] = {"attn_q.bias", "attn_k.bias", "attn_v.bias"};
+    const int full[3] = {p->qd, p->kvd, p->kvd}, local[3] = {p->qd_l, p->kvd_l, p->kvd_l};
+    std::vector<float> h((size_t)p->qd_l + 2 * p->kvd_l);
+    size_t o = 0;
+    for (int i = 0; i < 3; i++) {
+        const std::string name = pre + names[i];
+        const b200_tensor *t = find(tensors, n_tensors, name);
+        if (!t) return fail(p, B200_ERR_BAD_ARG, "missing tensor %s", name.c_str());
+        if (t->ggml_type != B200_GGML_F32) return fail(p, B200_ERR_UNSUPPORTED, "tensor %s must be F32 (ggml type %d)", name.c_str(), t->ggml_type);
+        if (t->n_dims != 1 || t->dims[0] != full[i] || !t->data)
+            return fail(p, B200_ERR_BAD_ARG, "tensor %s must have one dimension of %d floats (n_dims %d, dims[0] %lld)", name.c_str(), full[i], t->n_dims,
+                        (long long)(t->n_dims > 0 ? t->dims[0] : 0));
+        memcpy(h.data() + o, (const float *)t->data + (size_t)p->tp.rank * local[i], (size_t)local[i] * 4);
+        o += local[i];
+    }
+    int rc = dalloc(p, dst, h.size() * 4);
+    if (rc) return rc;
+    CK(cudaMemcpy(*dst, h.data(), h.size() * 4, cudaMemcpyHostToDevice));
+    return B200_OK;
+}
+
 template <int MODE> int launch_matvec_q8(b200_plan *p, const DevMat &m, const int8_t *xq, const float *xs, float *out) {
     int R = (m.rows % 4 == 0 && m.rows >= 32768) ? 4 : (m.rows % 2 == 0 ? 2 : 1);
     int warps = m.rows / R;
@@ -612,7 +638,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
             auto att = [&](auto kern) {
                 return launch_k(p, pdl, kern, dim3(p->nh_l), dim3(ATT_THREADS), att_smem, p->qkv, kc, vc, (const StepState *)p->st,
                                 (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags, (const float *)L.q_norm,
-                                (const float *)L.k_norm, c.rms_norm_eps, (float)sqrt((double)c.head_size), q8 ? p->attq : nullptr, q8 ? p->atts : nullptr, xbf, TR(4),
+                                (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, (float)sqrt((double)c.head_size), q8 ? p->attq : nullptr, q8 ? p->atts : nullptr, xbf, TR(4),
                                 p->tp, (unsigned)(4 * l + 0), rank * p->nh_l, p->att_scratch, c.context_length);
             };
             if (c.head_size == 128) rc = att(k_attention<128>);
@@ -700,6 +726,7 @@ int pd_prepare(b200_plan *p) {
             const LayerW &W = p->layers[l];
             h[l].qkv = W.tqkv; h[l].wo = W.two; h[l].gu = W.tgu; h[l].w2 = W.tw2;
             h[l].attn_norm = W.attn_norm; h[l].ffn_norm = W.ffn_norm; h[l].q_norm = W.q_norm; h[l].k_norm = W.k_norm;
+            h[l].qkv_bias = W.qkv_bias;
             h[l].kc = p->key_cache + (size_t)l * ctx_kv;
             h[l].vc = p->value_cache + (size_t)l * ctx_kv;
         }
@@ -849,8 +876,9 @@ int prefill_init(b200_plan *p);
 
 int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     const b200_config &c = p->cfg;
-    if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3) return fail(p, B200_ERR_UNSUPPORTED, "unknown arch %d", c.arch);
-    p->kflags = c.arch == B200_ARCH_QWEN3 ? (KF_NEOX | KF_QKNORM) : c.arch == B200_ARCH_PHI3 ? KF_NEOX : 0;
+    if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3 && c.arch != B200_ARCH_QWEN2)
+        return fail(p, B200_ERR_UNSUPPORTED, "unknown arch %d", c.arch);
+    p->kflags = c.arch == B200_ARCH_QWEN3 ? (KF_NEOX | KF_QKNORM) : c.arch == B200_ARCH_PHI3 ? KF_NEOX : c.arch == B200_ARCH_QWEN2 ? (KF_NEOX | KF_QKVBIAS) : 0;
     if (c.dim <= 0 || c.dim % 32 || c.hidden_dim % 32 || (c.head_size != 32 && c.head_size != 64 && c.head_size != 96 && c.head_size != 128 && c.head_size != 256) || c.n_heads % c.n_kv_heads ||
         c.n_layers <= 0 || c.vocab_size <= 0 || c.context_length <= 0)
         return fail(p, B200_ERR_BAD_ARG, "unsupported shape (dim/hidden must be multiples of 32, head_size one of 32/64/96/128/256)");
@@ -858,7 +886,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         return fail(p, B200_ERR_BAD_ARG, "fp16_lanes must be 0, 4, 8, 16 or 32");
     p->qd = c.n_heads * c.head_size;
     p->kvd = c.n_kv_heads * c.head_size;
-    if (c.arch != B200_ARCH_QWEN3 && p->qd != c.dim) return fail(p, B200_ERR_BAD_ARG, "llama / phi3: n_heads*head_size must equal dim");
+    if (c.arch != B200_ARCH_QWEN3 && p->qd != c.dim) return fail(p, B200_ERR_BAD_ARG, "llama / phi3 / qwen2: n_heads*head_size must equal dim");
     {
         const int tn = c.tp_size;
         if (tn < 1 || tn > TP_MAX || c.tp_rank < 0 || c.tp_rank >= tn) return fail(p, B200_ERR_BAD_ARG, "bad tp_rank/tp_size %d/%d", c.tp_rank, tn);
@@ -964,6 +992,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
             if ((rc = upload_f32(p, T("attn_q_norm.weight"), c.head_size, &L.q_norm, "attn_q_norm.weight"))) return rc;
             if ((rc = upload_f32(p, T("attn_k_norm.weight"), c.head_size, &L.k_norm, "attn_k_norm.weight"))) return rc;
         }
+        if (c.arch == B200_ARCH_QWEN2 && (rc = upload_qkv_bias(p, tensors, n_tensors, l, &L.qkv_bias))) return rc;
         // Phi-3 stores wqkv and gate|up fused (Phi3StandardWeights: attn_qkv.weight = [q; k; v] rows, ffn_up.weight = [gate; up] rows,
         // InferenceCore.java:718-724,779-781): the row ranges below address the same source tensor; rows are independent dot products, so
         // splitting a fused matrix by rows changes nothing in the arithmetic.
@@ -1115,7 +1144,7 @@ static const char *prefill_shape_why(const b200_plan *p) {
     const int kv_mul = g.n_heads / g.n_kv_heads, nqkv = p->qd + 2 * p->kvd;
     if (g.tp_size > 1) return "tensor-core prefill is single-GPU";
     if (g.head_size != 64 && g.head_size != 128) return "tensor-core prefill supports head sizes 64 and 128";
-    if (kv_mul > 64 || (kv_mul & (kv_mul - 1))) return "tensor-core prefill needs a power-of-two GQA ratio <= 64";
+    if (g.n_heads % g.n_kv_heads || kv_mul > 64) return "tensor-core prefill needs n_heads % n_kv_heads == 0 and a GQA ratio <= 64";
     if (g.dim % 128 || p->qd % 128 || nqkv % 128 || g.hidden_dim % 64) return "tensor-core prefill needs dim, q width and q+k+v width multiples of 128, hidden a multiple of 64";
     if (!pg::encode_fn()) return "cuTensorMapEncodeTiled not available from the driver";
     return nullptr;
@@ -1296,11 +1325,11 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
             nl++;
         }
         if (g.head_size == 128) {
-            k_pf_rope_kv<128><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
+            k_pf_rope_kv<128><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
             if (c.att_simt) k_pf_attention<128><<<ag, PA_THREADS, pa_smem_bytes<128>(), s>>>(c.QKV, nqkv, kc, vc, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
             else k_pf_attention_mma<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
         } else {
-            k_pf_rope_kv<64><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
+            k_pf_rope_kv<64><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
             if (c.att_simt) k_pf_attention<64><<<ag, PA_THREADS, pa_smem_bytes<64>(), s>>>(c.QKV, nqkv, kc, vc, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
             else k_pf_attention_mma<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
         }
@@ -2005,7 +2034,7 @@ int b200_test_pf_attention(int32_t impl, const float *q, const float *k, const f
                            int32_t head_size, int32_t out_rows, uint16_t *out) {
     if (!q || !k || !v || !out || (impl != 0 && impl != 1) || n < 1 || start_pos < 0 || out_rows < n || n_kv_heads < 1 || n_heads % n_kv_heads) return B200_ERR_BAD_ARG;
     const int kv_mul = n_heads / n_kv_heads, hs = head_size;
-    if ((hs != 64 && hs != 128) || kv_mul > 64 || (kv_mul & (kv_mul - 1))) return B200_ERR_BAD_ARG; // what prefill_init accepts
+    if ((hs != 64 && hs != 128) || kv_mul > 64) return B200_ERR_BAD_ARG; // what prefill_init accepts
     const int qd = n_heads * hs, kvd = n_kv_heads * hs, ldq = qd + 2 * kvd, nkeys = start_pos + n;
     const size_t kv_elems = (size_t)nkeys * kvd;
     float *dqkv = nullptr, *dk = nullptr, *dv = nullptr;

@@ -93,13 +93,14 @@ __global__ void __launch_bounds__(256) k_pf_rmsnorm_f16(const float *__restrict_
 }
 
 // One CTA per token, one warp per head at a time.  Llama rotates interleaved pairs (InferenceCore.java:75-87);
-// Qwen3 normalises the head, then rotates NeoX pairs (:594-619).  q is rotated in place; k and v go to the
-// FP32 KV cache (what decode reads) and, as f16, to the per-layer scratch the attention kernel streams.
+// Qwen3 normalises the head, then rotates NeoX pairs (:594-619); Qwen2 adds the q / k / v biases first (:456-459),
+// exactly (one rounded add), then rotates NeoX pairs.  q is rotated in place; k and v go to the FP32 KV cache
+// (what decode reads) and, as f16, to the per-layer scratch the attention kernel streams.
 template <int HS>
 __global__ void __launch_bounds__(256) k_pf_rope_kv(float *__restrict__ qkv, int ldq, float *__restrict__ kc, float *__restrict__ vc, __half *__restrict__ kh,
                                                    __half *__restrict__ vh, int kvd, int n_heads, int n_kv_heads, int arch, const float *__restrict__ qnw,
-                                                   const float *__restrict__ knw, float eps, const float *__restrict__ cr, const float *__restrict__ ci,
-                                                   int start_pos) {
+                                                   const float *__restrict__ knw, const float *__restrict__ qkvb, float eps, const float *__restrict__ cr,
+                                                   const float *__restrict__ ci, int start_pos) {
     constexpr int HALF = HS / 2, PPL = HALF / 32; // pairs per lane
     const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, pos = start_pos + b;
     const int qd = n_heads * HS;
@@ -116,6 +117,11 @@ __global__ void __launch_bounds__(256) k_pf_rope_kv(float *__restrict__ qkv, int
             if (arch & KF_NEOX) { i0[u] = p; i1[u] = p + HALF; } else { i0[u] = 2 * p; i1[u] = 2 * p + 1; }
             v0[u] = src[i0[u]];
             v1[u] = src[i1[u]];
+            if (arch & KF_QKVBIAS) {
+                const float *bb = qkvb + (is_q ? hh * HS : qd + kvh * HS);
+                v0[u] = __fadd_rn(v0[u], bb[i0[u]]);
+                v1[u] = __fadd_rn(v1[u], bb[i1[u]]);
+            }
             ss += v0[u] * v0[u] + v1[u] * v1[u];
         }
         if (arch & KF_QKNORM) {
@@ -137,7 +143,12 @@ __global__ void __launch_bounds__(256) k_pf_rope_kv(float *__restrict__ qkv, int
             } else {
                 const size_t o = (size_t)pos * kvd + kvh * HS;
                 const float *vsrc = qkv + (size_t)b * ldq + qd + kvd + kvh * HS;
-                const float w0 = vsrc[i0[u]], w1 = vsrc[i1[u]];
+                float w0 = vsrc[i0[u]], w1 = vsrc[i1[u]];
+                if (arch & KF_QKVBIAS) {
+                    const float *bb = qkvb + qd + kvd + kvh * HS;
+                    w0 = __fadd_rn(w0, bb[i0[u]]);
+                    w1 = __fadd_rn(w1, bb[i1[u]]);
+                }
                 kc[o + i0[u]] = r0; kc[o + i1[u]] = r1;
                 vc[o + i0[u]] = w0; vc[o + i1[u]] = w1;
                 kh[o + i0[u]] = __float2half_rn(r0); kh[o + i1[u]] = __float2half_rn(r1);
@@ -162,9 +173,10 @@ __global__ void __launch_bounds__(256) k_pf_kv_to_f16(const float *__restrict__ 
 }
 
 // ---- causal attention over the chunk + everything already in the cache ---------------------------
-// CTA = one KV head x a tile of QT = 64 / kv_mul query tokens -> 64 query rows (all query heads that share
-// the KV head), so each K/V tile read from L2 serves 64 rows.  FP32 SIMT flash attention: S = Q K^T into
-// shared memory, online softmax per row, O += P V in registers.  256 threads.
+// CTA = one KV head x a tile of QT = floor(64 / kv_mul) query tokens -> QT * kv_mul query rows (all query heads that
+// share the KV head), so each K/V tile read from L2 serves up to 64 rows.  When kv_mul does not divide 64 (Qwen2's
+// ratios 5, 6, 7, ...), rows r >= QT * kv_mul are padding: no Q load, every key masked, never stored.  FP32 SIMT flash
+// attention: S = Q K^T into shared memory, online softmax per row, O += P V in registers.  256 threads.
 constexpr int PA_THREADS = 256, PA_ROWS = 64, PA_KT = 64;
 template <int HS> constexpr size_t pa_smem_bytes() { return (size_t)(2 * PA_ROWS * (HS + 4) + PA_KT * HS + PA_ROWS * (PA_KT + 1) + 3 * PA_ROWS) * 4; }
 
@@ -176,10 +188,10 @@ __global__ void __launch_bounds__(PA_THREADS) k_pf_attention(const float *__rest
     float *sQ = pa_sm, *sK = sQ + PA_ROWS * QP, *sV = sK + PA_ROWS * QP, *sS = sV + PA_KT * HS;
     float *sM = sS + PA_ROWS * SP, *sL = sM + PA_ROWS, *sA = sL + PA_ROWS;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int QT = PA_ROWS / kv_mul, q0 = blockIdx.x * QT, g = blockIdx.y;
+    const int QT = PA_ROWS / kv_mul, RV = QT * kv_mul, q0 = blockIdx.x * QT, g = blockIdx.y; // rows >= RV: padding (token n)
 
     for (int idx = tid; idx < PA_ROWS * H4; idx += PA_THREADS) {
-        const int r = idx / H4, d4 = idx % H4, b = q0 + r / kv_mul, h = g * kv_mul + r % kv_mul;
+        const int r = idx / H4, d4 = idx % H4, b = r < RV ? q0 + r / kv_mul : n, h = g * kv_mul + r % kv_mul;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (b < n) {
             v = *reinterpret_cast<const float4 *>(qkv + (size_t)b * ldq + h * HS + d4 * 4);
@@ -231,7 +243,7 @@ __global__ void __launch_bounds__(PA_THREADS) k_pf_attention(const float *__rest
         }
 #pragma unroll
         for (int i = 0; i < 4; i++) {
-            const int r = ty * 4 + i, b = q0 + r / kv_mul;
+            const int r = ty * 4 + i, b = r < RV ? q0 + r / kv_mul : n;
 #pragma unroll
             for (int j = 0; j < 4; j++) {
                 const int t = k0 + tx + 16 * j;
@@ -284,7 +296,7 @@ __global__ void __launch_bounds__(PA_THREADS) k_pf_attention(const float *__rest
     __syncthreads();
 #pragma unroll
     for (int rr = 0; rr < 8; rr++) {
-        const int r = warp * 8 + rr, b = q0 + r / kv_mul, h = g * kv_mul + r % kv_mul;
+        const int r = warp * 8 + rr, b = r < RV ? q0 + r / kv_mul : n, h = g * kv_mul + r % kv_mul;
         if (b < n) {
             const float inv = 1.0f / sL[r];
             __half *o = out + (size_t)b * ldo + h * HS + lane * CPT;
@@ -296,7 +308,7 @@ __global__ void __launch_bounds__(PA_THREADS) k_pf_attention(const float *__rest
 
 // ---- the same attention on the warp-level tensor cores ------------------------------------------
 // FlashAttention-2 layout with mma.sync.m16n8k16 (f16 operands, f32 accumulation): CTA = one KV head x 64
-// query rows (4 warps x 16 rows), key tiles of 64.  Q (pre-scaled), K and V are converted to f16 on their
+// query rows (4 warps x 16 rows; rows >= QT * kv_mul are padding, as in k_pf_attention), key tiles of 64.  Q (pre-scaled), K and V are converted to f16 on their
 // way into shared memory; S = Q K^T stays in registers, its accumulator layout is re-used directly as the
 // A operand of P V, and V's B fragments come from ldmatrix.trans.  This op is 1 % of the prefill FLOPs
 // (0.07 of 7.2 TFLOP at pp512); the GEMMs that carry the rest run on wgmma.
@@ -325,7 +337,8 @@ __global__ void __launch_bounds__(PM_THREADS) k_pf_attention_mma(const float *__
     constexpr int RP = HS + 8, H4 = HS / 4, KS = HS / 16, NB = HS / 8; // row pitch (halves): 16 B of padding keeps fragment loads conflict-free
     __half *sQ = reinterpret_cast<__half *>(pm_sm), *sKV = sQ + PM_ROWS * RP; // stage s: K at sKV + s*2*64*RP, V right after it
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
-    const int QT = PM_ROWS / kv_mul, q0 = ((int)gridDim.x - 1 - (int)blockIdx.x) * QT, grp = blockIdx.y; // longest (latest) query tiles first
+    const int QT = PM_ROWS / kv_mul, RV = QT * kv_mul; // rows >= RV: padding (token n: no Q, every key masked, not stored)
+    const int q0 = ((int)gridDim.x - 1 - (int)blockIdx.x) * QT, grp = blockIdx.y; // longest (latest) query tiles first
     const int q_end = (q0 + QT < n ? q0 + QT : n), nkeys = start_pos + q_end, ntiles = (nkeys + PM_KT - 1) / PM_KT;
     const uint32_t sKV_addr = (uint32_t)__cvta_generic_to_shared(sKV);
     // K/V tile -> shared memory with cp.async (16 bytes per request, rows past nkeys zero-filled), double buffered
@@ -349,7 +362,7 @@ __global__ void __launch_bounds__(PM_THREADS) k_pf_attention_mma(const float *__
 
     const float qscale = inv_sqrt_hs * 1.4426950408889634f;
     for (int idx = tid; idx < PM_ROWS * H4; idx += PM_THREADS) {
-        const int r = idx / H4, d4 = idx % H4, b = q0 + r / kv_mul, h = grp * kv_mul + r % kv_mul;
+        const int r = idx / H4, d4 = idx % H4, b = r < RV ? q0 + r / kv_mul : n, h = grp * kv_mul + r % kv_mul;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (b < n) v = *reinterpret_cast<const float4 *>(qkv + (size_t)b * ldq + h * HS + d4 * 4);
         uint2 pk;
@@ -374,11 +387,13 @@ __global__ void __launch_bounds__(PM_THREADS) k_pf_attention_mma(const float *__
     for (int nb = 0; nb < NB; nb++) o[nb][0] = o[nb][1] = o[nb][2] = o[nb][3] = 0.0f;
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.0f, l1 = 0.0f;
     const int row0 = warp * 16 + g, row1 = row0 + 8;
-    const int tb0 = q0 + row0 / kv_mul, tb1 = q0 + row1 / kv_mul;
+    const int tb0 = row0 < RV ? q0 + row0 / kv_mul : n, tb1 = row1 < RV ? q0 + row1 / kv_mul : n;
     const int qpos0 = tb0 < n ? start_pos + tb0 : -1, qpos1 = tb1 < n ? start_pos + tb1 : -1; // -1: every key masked
-    // smallest position among this warp's 16 rows (-1 when the warp holds padding rows): tiles entirely at or before it need no mask
-    const int wlast_tok = q0 + (warp * 16 + 15) / kv_mul;
-    const int wmin_pos = wlast_tok < n ? start_pos + q0 + (warp * 16) / kv_mul : -1;
+    // smallest position among this warp's 16 rows (-1 when the warp holds padding rows -- past n, or r >= RV): tiles entirely at or
+    // before it need no mask.  With a power-of-two kv_mul, RV = 64 and this is the plain per-warp shortcut; otherwise the one warp
+    // that holds rows >= RV masks every tile, which is what keeps its padding rows from seeing any key.
+    const int wlast_row = warp * 16 + 15;
+    const int wmin_pos = (wlast_row < RV && q0 + wlast_row / kv_mul < n) ? start_pos + q0 + (warp * 16) / kv_mul : -1;
 
 #pragma unroll 1
     for (int it = 0; it < ntiles; it++) {

@@ -67,6 +67,12 @@ def generate_tokens_qwen3(forward: Forward, latest_token: int, start_position: i
     return generated
 
 
+def loop_for(model_type: str):
+    """The generation loop the reference's model class uses: Qwen3, Qwen2 and DeepSeek-R1-Distill-Qwen run generateTokensQwen3
+    (Qwen3.java, Qwen2.java:95-115), the others generateTokensLlama."""
+    return generate_tokens_qwen3 if model_type.upper() in ("QWEN_3", "QWEN_2", "DEEPSEEK_R1_DISTILL_QWEN") else generate_tokens_llama
+
+
 def generate_tokens_llama_batch_prefill(plan, latest_token: int, start_position: int, prompt_tokens: list[int],
                                         stop_tokens: Iterable[int], max_tokens: int, context_length: int, batch_size: int) -> list[int]:
     """prefillSeq = [latestToken, prompt[0..N-2]] at positions startPosition.. in chunks of B through the batched

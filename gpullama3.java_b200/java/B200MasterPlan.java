@@ -164,6 +164,8 @@ public final class B200MasterPlan implements AutoCloseable {
     }
 
     public static final int PREFILL_EXACT = 0, PREFILL_TENSOR_CORE = 1, PREFILL_TENSOR_CORE_W8A16 = 2;
+    // b200_config.arch (include/b200llama.h): Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen pass blk.N.attn_{q,k,v}.bias (F32) with the weights
+    public static final int ARCH_LLAMA = 0, ARCH_QWEN3 = 1, ARCH_PHI3 = 2, ARCH_QWEN2 = 3;
 
     /** TensorCoreSupport.java's switch: 0 = exact token-by-token prefill (bit-identical KV cache), 1 = TMA + wgmma GEMMs (a Q8_0
      *  plan first builds f16 twins of its matrices, +2 bytes per weight), 2 = the same GEMMs on a Q8_0 plan reading the Q8_0 weights

@@ -1,6 +1,6 @@
 """Host-side mirror of the reference model loaders (metadata -> Configuration, tensor names ->
 weight slots).  Mirrors ``model/loader/ModelLoader.java:47-108`` (type detection on
-``general.name``), ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74``
+``general.name``), ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74`` / ``Qwen2ModelLoader.java:48-73``
 (configuration keys), ``AbstractModelLoader.java:40-50`` (file_type -> quantisation) and
 ``AbstractModelLoader.java:186-195`` (tied output falls back to ``token_embd.weight``).
 Weights stay in GGUF block layout; the native library repacks at upload.
@@ -16,6 +16,7 @@ from .gguf import GGMLType, GGUFFile
 ARCH_LLAMA = 0
 ARCH_QWEN3 = 1
 ARCH_PHI3 = 2
+ARCH_QWEN2 = 3  # Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen: Llama's forward + q/k/v biases, NeoX RoPE (InferenceCore.java:434-563)
 
 
 @dataclass
@@ -88,11 +89,11 @@ class Model:
 
 def model_from_tensors(shape, quant: int, tensors: dict, context_length: int) -> Model:
     """In-memory model (bench: synthetic weights never touch the disk)."""
-    arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3}[shape.arch]
+    arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3, "qwen2": ARCH_QWEN2}[shape.arch]
     cfg = Configuration(arch, "Q8_0" if quant == GGMLType.Q8_0 else "FP16",
                         shape.dim, shape.hidden, shape.n_layers, shape.n_heads, shape.n_kv_heads, shape.head_size,
                         shape.vocab, context_length, float(shape.eps), float(shape.rope_theta))
-    return Model(None, cfg, {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3"}[shape.arch], tensors)
+    return Model(None, cfg, {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3", "qwen2": "QWEN_2"}[shape.arch], tensors)
 
 
 def load_model(path: str, context_length: int = -1) -> Model:
@@ -144,8 +145,20 @@ def load_model(path: str, context_length: int = -1) -> Model:
             ARCH_PHI3, q, dim, int(md["phi3.feed_forward_length"]), int(md["phi3.block_count"]), n_heads,
             int(md.get("phi3.attention.head_count_kv", n_heads)), dim // n_heads, int(vocab), model_ctx if context_length < 0 else context_length,
             float(md.get("phi3.attention.layer_norm_rms_epsilon", 1e-5)), float(md.get("phi3.rope.freq_base", 10000.0)))
+    elif typ in ("QWEN_2", "DEEPSEEK_R1_DISTILL_QWEN"):
+        # Qwen2ModelLoader.createConfiguration (Qwen2ModelLoader.java:48-73): qwen2.* keys, head_count_kv defaults to head_count, the
+        # vocabulary size is the token list's, the context is clamped to the model's, eps and theta have no defaults;
+        # head size = dim / heads (Qwen2Configuration.java:25-32).
+        model_ctx = int(md["qwen2.context_length"])
+        ctx = model_ctx if (context_length < 0 or model_ctx < context_length) else context_length
+        n_heads = int(md["qwen2.attention.head_count"])
+        dim = int(md["qwen2.embedding_length"])
+        cfg = Configuration(
+            ARCH_QWEN2, q, dim, int(md["qwen2.feed_forward_length"]), int(md["qwen2.block_count"]), n_heads,
+            int(md.get("qwen2.attention.head_count_kv", n_heads)), dim // n_heads, len(md["tokenizer.ggml.tokens"]), ctx,
+            float(md["qwen2.attention.layer_norm_rms_epsilon"]), float(md["qwen2.rope.freq_base"]))
     else:
-        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 forward passes only)")
+        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 forward passes only)")
     return Model(g, cfg, typ)
 
 

@@ -2,7 +2,8 @@
 offline; SURVEY.md section 8d).  Tensor names/types are exactly what the reference loaders
 expect (``model/loader/LlamaModelLoader.java:78-99``, ``Qwen3ModelLoader.java:98-124``):
 norm weights F32, matrices and the embedding table in the model quantisation, metadata keys
-per ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74``.
+per ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74`` / ``Qwen2ModelLoader.java:48-73``.  Qwen2 files
+add F32 biases ``blk.N.attn_{q,k,v}.bias`` (``Qwen2ModelLoader.java:100-102``).
 """
 from __future__ import annotations
 
@@ -15,7 +16,7 @@ from .gguf import GGMLType, write_gguf
 
 @dataclass(frozen=True)
 class Shape:
-    arch: str  # "llama" | "qwen3" | "phi3"
+    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2"
     dim: int
     hidden: int
     n_layers: int
@@ -63,6 +64,15 @@ SHAPES = {
     "tiny-qwen3-vocab152k": Shape("qwen3", 256, 768, 2, 4, 2, 128, 151936, True, 1000000.0, 1e-6),
     "tiny-phi3-vocab32k": Shape("phi3", 384, 768, 2, 4, 4, 96, 32064, False, 10000.0, 1e-5, 4096),
     "mid-phi3-mini": Shape("phi3", 3072, 8192, 2, 32, 32, 96, 8192, False, 10000.0, 1e-5, 4096),  # Phi-3-mini-4k layer geometry
+    # Qwen2 (q/k/v biases, NeoX RoPE): GQA ratios that are not powers of two.  tiny-qwen2 is Qwen2.5-0.5B's head layout (14 / 2, ratio 7),
+    # tiny-qwen2-gqa6 DeepSeek-R1-Distill-Qwen-1.5B's (12 / 2, head size 128); both meet every tensor-core prefill constraint
+    "tiny-qwen2": Shape("qwen2", 896, 1024, 2, 14, 2, 64, 512, True, 1000000.0, 1e-6, 32768),
+    "tiny-qwen2-gqa6": Shape("qwen2", 1536, 1024, 2, 12, 2, 128, 640, False, 1000000.0, 1e-6, 32768),
+    "tiny-qwen2-vocab152k": Shape("qwen2", 896, 1024, 2, 14, 2, 64, 151936, True, 1000000.0, 1e-6, 32768),
+    # 2-layer cuts of the real Qwen2.5-0.5B, DeepSeek-R1-Distill-Qwen-1.5B and Qwen2.5-7B layer geometries (small vocabulary)
+    "mid-qwen2.5-0.5b": Shape("qwen2", 896, 4864, 2, 14, 2, 64, 8192, True, 1000000.0, 1e-6, 32768),
+    "mid-deepseek-r1-qwen-1.5b": Shape("qwen2", 1536, 8960, 2, 12, 2, 128, 8192, False, 10000.0, 1e-6, 131072),
+    "mid-qwen2.5-7b": Shape("qwen2", 3584, 18944, 2, 28, 4, 128, 8192, False, 1000000.0, 1e-6, 32768),
     # mid shape: exercises column tails (dim not a multiple of 512) and several row tiles
     "small-llama": Shape("llama", 1536, 4096, 3, 12, 4, 128, 4096, False, 500000.0, 1e-5),
     # the real Llama-3-8B layer geometry (7 column segments in the down projection, 4 KB rows) with 2 layers / small vocab
@@ -76,6 +86,8 @@ SHAPES = {
     "llama-3-8b": Shape("llama", 4096, 14336, 32, 32, 8, 128, 128256, False, 500000.0, 1e-5),
     "qwen3-4b": Shape("qwen3", 2560, 9728, 36, 32, 8, 128, 151936, True, 1000000.0, 1e-6, 40960),
     "llama-3-70b": Shape("llama", 8192, 28672, 80, 64, 8, 128, 128256, False, 500000.0, 1e-5),
+    # Qwen2.5-7B (tools/qwen2_bench.py)
+    "qwen2.5-7b": Shape("qwen2", 3584, 18944, 28, 28, 4, 128, 152064, False, 1000000.0, 1e-6, 32768),
 }
 
 
@@ -132,7 +144,7 @@ def gpt2_byte_symbols() -> list[str]:
 def build_vocab(vocab_size: int, arch: str = "llama", seed: int = 1234):
     """(tokens, merge_lines, token_types, base_tokens): 256 byte symbols, BPE merges trained on a small fixed corpus
     (ids in merge order, so the vocabulary is a consistent BPE vocabulary), padding tokens, then the special tokens."""
-    specials = QWEN3_SPECIALS if arch == "qwen3" else LLAMA_SPECIALS
+    specials = QWEN3_SPECIALS if arch in ("qwen3", "qwen2") else LLAMA_SPECIALS
     n_merges = vocab_size - 256 - len(specials)
     if n_merges < 0:
         raise ValueError("vocabulary too small for the byte symbols and the special tokens")
@@ -179,7 +191,7 @@ def build_vocab(vocab_size: int, arch: str = "llama", seed: int = 1234):
     types = [1] * base + [3] * len(specials)  # 1 normal, 3 control
     for i in range(base - pad, base):
         types[i] = 5
-    if arch == "qwen3":
+    if arch in ("qwen3", "qwen2"):
         for t in ("<think>", "</think>", "<tool_call>", "</tool_call>"):
             types[tokens.index(t)] = 4  # user defined: displayed (Qwen3Tokenizer.shouldDisplayToken)
     return tokens, merges, types, base
@@ -204,7 +216,7 @@ def metadata_for(shape: Shape, quant: int, name: str) -> dict:
     if a == "qwen3":
         md["qwen3.attention.key_length"] = shape.head_size
         md["qwen3.attention.value_length"] = shape.head_size
-    if shape.vocab <= 4096:  # tokenizer section (GGUF keys the loaders read: tokenizer.ggml.tokens / merges / token_type)
+    if shape.vocab <= 4096 or a == "qwen2":  # tokenizer section (Qwen2 takes its vocabulary size from the token list) (GGUF keys the loaders read: tokenizer.ggml.tokens / merges / token_type)
         tokens, merges, types, base = build_vocab(shape.vocab, a)
         md["tokenizer.ggml.model"] = "gpt2"
         md["tokenizer.ggml.tokens"] = tokens
@@ -236,6 +248,10 @@ def tensor_plan(shape: Shape, quant: int):
             (p + "attn_v.weight", quant, (shape.dim, shape.kv_dim), "w"),
             (p + "attn_output.weight", quant, (shape.q_dim, shape.dim), "w"),
         ]
+        if shape.arch == "qwen2":  # Qwen2ModelLoader.java:100-102
+            t += [(p + "attn_q.bias", GGMLType.F32, (shape.q_dim,), "b"),
+                  (p + "attn_k.bias", GGMLType.F32, (shape.kv_dim,), "b"),
+                  (p + "attn_v.bias", GGMLType.F32, (shape.kv_dim,), "b")]
         if shape.arch == "qwen3":
             t += [(p + "attn_q_norm.weight", GGMLType.F32, (shape.head_size,), "n"),
                   (p + "attn_k_norm.weight", GGMLType.F32, (shape.head_size,), "n")]
@@ -251,15 +267,26 @@ def tensor_plan(shape: Shape, quant: int):
     return t
 
 
+def qkv_bias(n: int, rng) -> np.ndarray:
+    """Synthetic Qwen2 q/k/v bias: N(0, 1) with one entry in 32 set to +-20 (real Qwen2 k biases reach tens), large enough
+    that dropping the bias changes the greedy tokens."""
+    x = rng.standard_normal(n, dtype=np.float32)
+    big = rng.choice(n, max(1, n // 32), replace=False)
+    x[big] = np.where(rng.random(len(big)) < 0.5, -20.0, 20.0).astype(np.float32)
+    return x
+
+
 def build_tensors(shape: Shape, quant: int, seed: int = 1234, w_std: float = 0.02):
     """Seeded tensors: matrices N(0, w_std) (scaled so activations stay O(1) through the
-    stack), norm weights 1 + N(0, 0.02).  Returns [(name, type, dims, raw uint8)]."""
+    stack), norm weights 1 + N(0, 0.02), Qwen2 biases as `qkv_bias`.  Returns [(name, type, dims, raw uint8)]."""
     rng = np.random.Generator(np.random.PCG64(seed))
     out = []
     for name, tt, dims, kind in tensor_plan(shape, quant):
         n = int(np.prod(dims))
         if kind == "n":
             x = (1.0 + 0.02 * rng.standard_normal(n, dtype=np.float32)).astype(np.float32)
+        elif kind == "b":
+            x = qkv_bias(n, rng)
         else:
             # fan-in scaled so that W.x of a unit-RMS vector is O(1): keeps logits in a sane range
             std = w_std if w_std > 0 else 1.0 / np.sqrt(dims[0])
@@ -309,6 +336,8 @@ def build_tensors_kquant(shape: Shape, seed: int = 1234, mix: str = "Q4_K_M") ->
         n = int(np.prod(dims))
         if kind == "n":
             out[name] = (GGMLType.F32, dims, (1.0 + 0.02 * rng.standard_normal(n, dtype=np.float32)).astype(np.float32).view(np.uint8))
+        elif kind == "b":
+            out[name] = (GGMLType.F32, dims, qkv_bias(n, rng).view(np.uint8))
         else:
             tt = pick(name)
             out[name] = (tt, dims, random_kquant(tt, n, rng, zero_blocks=1 if "attn_q" in name else 0))
@@ -318,14 +347,14 @@ def build_tensors_kquant(shape: Shape, seed: int = 1234, mix: str = "Q4_K_M") ->
 def write_model(path: str, shape_name: str, quant: int, seed: int = 1234, w_std: float = 0.0,
                 display_name: str | None = None):
     shape = SHAPES[shape_name]
-    name = display_name or {"llama": "Llama synthetic ", "qwen3": "Qwen3 synthetic ", "phi3": "Phi3 synthetic "}[shape.arch] + shape_name
+    name = display_name or {"llama": "Llama synthetic ", "qwen3": "Qwen3 synthetic ", "phi3": "Phi3 synthetic ", "qwen2": "Qwen2 synthetic "}[shape.arch] + shape_name
     write_gguf(path, metadata_for(shape, quant, name), build_tensors(shape, quant, seed, w_std))
     return shape
 
 
 def tp_row_ranges(shape: Shape, tp_rank: int, tp_size: int) -> dict:
     """Row range [r0, r1) of every sharded matrix that tensor-parallel rank `tp_rank` uploads (mirrors plan.tp_shard_plan /
-    csrc/plan.cu); tensors not listed (embedding table, norms) are needed whole."""
+    csrc/plan.cu); tensors not listed (embedding table, norms, Qwen2's q/k/v biases) are needed whole."""
     r, n = tp_rank, tp_size
     qd_l, kvd_l = shape.q_dim // n, shape.kv_dim // n
     hid_l, dim_l, voc_l = shape.hidden // n, shape.dim // n, shape.vocab // n
@@ -365,6 +394,12 @@ def build_tensors_fast(shape: Shape, quant: int, seed: int = 1234, device: str |
         n = int(np.prod(dims))
         if kind == "n":
             x = 1.0 + 0.02 * torch.randn(n, device=dev, generator=gen)
+            out[name] = (tt, dims, x.float().cpu().numpy().view(np.uint8).reshape(-1))
+            continue
+        if kind == "b":  # qkv_bias's distribution: N(0, 1), one entry in 32 at +-20
+            x = torch.randn(n, device=dev, generator=gen)
+            big = torch.randperm(n, device=dev, generator=gen)[:max(1, n // 32)]
+            x[big] = torch.where(torch.rand(len(big), device=dev, generator=gen) < 0.5, -20.0, 20.0)
             out[name] = (tt, dims, x.float().cpu().numpy().view(np.uint8).reshape(-1))
             continue
         std = 1.0 / float(np.sqrt(dims[0]))

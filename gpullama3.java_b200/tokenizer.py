@@ -189,6 +189,9 @@ def from_metadata(metadata: dict, model_type: str) -> Tokenizer:
                                    "implemented; drive the plan with token ids")
     tokens = list(metadata["tokenizer.ggml.tokens"])
     merges = list(metadata["tokenizer.ggml.merges"])
-    if model_type.upper().startswith("QWEN"):
-        return Qwen3Tokenizer(tokens, merges, list(metadata["tokenizer.ggml.token_type"]))
+    typ = model_type.upper()
+    if typ.startswith("QWEN") or typ == "DEEPSEEK_R1_DISTILL_QWEN":
+        # Qwen2ModelLoader.java:35-43: the Qwen3 vocabulary and tokenizer; DeepSeek-R1-Distill-Qwen moves the first special token
+        deepseek = typ != "QWEN_3" and metadata.get("general.basename") == "DeepSeek-R1-Distill-Qwen"
+        return Qwen3Tokenizer(tokens, merges, list(metadata["tokenizer.ggml.token_type"]), deepseek_r1_distill=deepseek)
     return LlamaTokenizer(tokens, merges, base_tokens=metadata.get("b200.synthetic.base_tokens"))

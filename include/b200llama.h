@@ -39,6 +39,10 @@ extern "C" {
 #define B200_ARCH_QWEN3 1 /* InferenceCore.forwardJavaQwen3, InferenceCore.java:565-697 */
 #define B200_ARCH_PHI3 2  /* InferenceCore.forwardJavaPhi3,  InferenceCore.java:699-800: fused blk.N.attn_qkv.weight ([q; k; v] rows) and
                            * blk.N.ffn_up.weight ([gate; up] rows), NeoX-pair RoPE without q/k norm; n_heads * head_size == dim */
+#define B200_ARCH_QWEN2 3 /* InferenceCore.forwardJavaQwen2, InferenceCore.java:434-563 (Qwen2, Qwen2.5, DeepSeek-R1-Distill-Qwen): Llama's
+                           * tensors plus F32 biases blk.N.attn_q.bias (n_heads * head_size floats), attn_k.bias and attn_v.bias
+                           * (n_kv_heads * head_size each), added to q, k and v right after their matmuls; NeoX-pair RoPE without q/k
+                           * norm; n_heads * head_size == dim.  Under tensor parallelism a rank reads the bias rows of its own heads. */
 
 /* GGML tensor type ids accepted for weights (tensor/GGMLType.java:5-20) */
 #define B200_GGML_F32 0
@@ -182,10 +186,12 @@ int b200_decode_sequence(b200_plan *plan, const int32_t *tokens, int32_t n, int3
 int b200_kv_reset(b200_plan *plan);
 
 /* Test/diagnostic read-back of a named device buffer into host memory.  Names:
- * "x","xb","q","k","v","hb","logits","key_cache","value_cache","xq","xs".  `layer` selects the
+ * "x","xb","q","k","v","hb","logits","key_cache","value_cache","xq","xs".  "q" (= "qkv") is the packed q|k|v vector of the
+ * last layer: its q part rotated (Qwen2: bias added, then rotated), its k and v parts as the matmul produced them, BEFORE any
+ * Qwen2 bias (the KV caches hold the biased k, v).  `layer` selects the
  * layer for the KV caches (ignored otherwise).  The tensor-core prefill scratch, as the last layer of the last
  * chunk left it, rows padded to a multiple of 128: "pf_x" (f32 residual, dim wide), "pf_qkv" (f32, q + k + v wide,
- * q rotated in place, k before RoPE), "pf_a16" (f16 bits, the FFN input), "pf_att16" (f16 bits, attention output),
+ * q rotated in place (after its Qwen2 bias), k before RoPE and v, both before their Qwen2 bias), "pf_a16" (f16 bits, the FFN input), "pf_att16" (f16 bits, attention output),
  * "pf_h16" (f16 bits, SwiGLU output).  Copies min(bytes, buffer size). */
 int b200_read_buffer(b200_plan *plan, const char *name, int32_t layer, void *dst, size_t bytes);
 
@@ -283,7 +289,8 @@ int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, i
  * rows).  impl 0 = k_pf_attention_mma (f16 K / V copies built by k_pf_kv_to_f16, as in the prefill), 1 = the FP32 SIMT
  * k_pf_attention.  q is placed in rows of stride q + 2 * kv width whose k / v columns hold NaN; grid and shared memory are the
  * prefill's.  out: f16 bits [out_rows][n_heads * head_size], out_rows >= n, in/out: rows >= n must come back untouched.
- * head_size 64 or 128, n_heads / n_kv_heads a power of two <= 64. */
+ * head_size 64 or 128, n_heads % n_kv_heads == 0 and n_heads / n_kv_heads <= 64 (any ratio: a CTA serves floor(64 / ratio) query
+ * tokens, the remaining rows of its 64-row tile are padding). */
 int b200_test_pf_attention(int32_t impl, const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads,
                            int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out);
 

@@ -47,13 +47,13 @@ __host__ __device__ inline size_t norm_smem_bytes(int dim, bool v2) {
     return v2 ? (size_t)norm_padded(dim) * 4 + 16 + seqsum2_scratch_bytes() : (size_t)dim * 4 + 16 + seqsum_scratch_bytes(dim);
 }
 
+// The body of k_rmsnorm_quant for one vector; `tok` is read after the dependency wait (the batched step, decode_batch.cuh,
+// runs it once per row with that row's x, token and outputs).
 template <bool EMBED, bool V2>
-__global__ void __launch_bounds__(NORM_THREADS, 1) k_rmsnorm_quant(float *__restrict__ x, const StepState *__restrict__ st,
-                                                               DevMat emb, const float *__restrict__ w, float eps, int dim,
-                                                               int8_t *__restrict__ xq, float *__restrict__ xs,
-                                                               float *__restrict__ xb, long long *__restrict__ prof, TraceBuf tr, TpCtx tp, int tp_wait_op) {
-    // One CTA of 1024 threads.  Under PDL this CTA only has to fit next to ONE streaming-matvec CTA
-    // (the following matvec's CTA for this SM simply starts a little later).
+__device__ __forceinline__ void rmsnorm_quant_row(float *__restrict__ x, const int *__restrict__ tok, const DevMat &emb,
+                                                  const float *__restrict__ w, float eps, int dim, int8_t *__restrict__ xq,
+                                                  float *__restrict__ xs, float *__restrict__ xb, long long *__restrict__ prof,
+                                                  const TraceBuf &tr, const TpCtx &tp, int tp_wait_op) {
     extern __shared__ __align__(16) float sm[];
     float *sq = sm;
     __shared__ float s_ss;
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(NORM_THREADS, 1) k_rmsnorm_quant(float *__rest
         __syncthreads();
     }
     int token = 0;
-    if (EMBED) token = st->token;
+    if (EMBED) token = *tok;
     for (int i = tid; i < dim; i += NORM_THREADS) {
         float v;
         if (EMBED) { v = emb_get(emb, token, i); x[i] = v; }
@@ -136,6 +136,16 @@ __global__ void __launch_bounds__(NORM_THREADS, 1) k_rmsnorm_quant(float *__rest
         if (tid == 0) { long long t4 = clock64(); prof[0] = t1 - t0; prof[1] = t2 - t1; prof[2] = t3 - t2; prof[3] = t4 - t3;
                         prof[4] = info0; prof[5] = info1; prof[6] = info2; }
     }
+}
+
+template <bool EMBED, bool V2>
+__global__ void __launch_bounds__(NORM_THREADS, 1) k_rmsnorm_quant(float *__restrict__ x, const StepState *__restrict__ st,
+                                                               DevMat emb, const float *__restrict__ w, float eps, int dim,
+                                                               int8_t *__restrict__ xq, float *__restrict__ xs,
+                                                               float *__restrict__ xb, long long *__restrict__ prof, TraceBuf tr, TpCtx tp, int tp_wait_op) {
+    // One CTA of 1024 threads.  Under PDL this CTA only has to fit next to ONE streaming-matvec CTA
+    // (the following matvec's CTA for this SM simply starts a little later).
+    rmsnorm_quant_row<EMBED, V2>(x, &st->token, emb, w, eps, dim, xq, xs, xb, prof, tr, tp, tp_wait_op);
 }
 
 // Test hooks: the sequential-sum emulations on arbitrary non-negative terms (padded with zeros: adding +0 never
@@ -407,14 +417,15 @@ __global__ void k_swiglu(float *__restrict__ hb, const float *__restrict__ hb2, 
 // ------------------------------------------------------------------------------------------
 #define ATT_THREADS 512 // four threads per key (scores) and per output element (weighted sum): head size <= ATT_THREADS / 4
 
+// The body of k_attention for query head blockIdx.x of one sequence; `posp` is read after the dependency wait (the batched
+// step, decode_batch.cuh, runs it per (head, row) with that row's position, cache, qkv vector, outputs and score rows).
 template <int HS>
-__global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ qkv, float *__restrict__ kc, float *__restrict__ vc,
-                                                          const StepState *__restrict__ st, const float *__restrict__ cr,
-                                                          const float *__restrict__ ci, int n_heads, int n_kv_heads, int arch /* KF_* flags */,
-                                                          const float *__restrict__ qnorm_w, const float *__restrict__ knorm_w,
-                                                          const float *__restrict__ qkv_bias, float eps, float sqrt_hs, int8_t *__restrict__ xq,
-                                                          float *__restrict__ xs, float *__restrict__ xb, TraceBuf tr, TpCtx tp,
-                                                          unsigned tp_out_op, int head_base, float *att_scratch, int ctx) {
+__device__ __forceinline__ void attention_head(float *__restrict__ qkv, float *__restrict__ kc, float *__restrict__ vc,
+                                               const int *__restrict__ posp, const float *__restrict__ cr, const float *__restrict__ ci,
+                                               int n_heads, int n_kv_heads, int arch, const float *__restrict__ qnorm_w,
+                                               const float *__restrict__ knorm_w, const float *__restrict__ qkv_bias, float eps, float sqrt_hs,
+                                               int8_t *__restrict__ xq, float *__restrict__ xs, float *__restrict__ xb, const TraceBuf &tr,
+                                               const TpCtx &tp, unsigned tp_out_op, int head_base, float *att_scratch, int ctx) {
     extern __shared__ __align__(16) float sm[]; // q[HS] | k[HS] | out[HS] | att[ctx] (att in global scratch for long contexts)
     __shared__ float red[ATT_THREADS / 32];
     __shared__ float s_val[2];
@@ -428,7 +439,7 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ q
     const int qd = n_heads * HS, kvd = n_kv_heads * HS;
     pdl_wait();
     trace_mark(tr, 2);
-    const int pos = st->pos, nt = pos + 1;
+    const int pos = *posp, nt = pos + 1;
     { // K/V rows of the earlier positions -> L2, one 128-byte line per request, so the score loads below hit L2 (the weight stream carries an
       // evict_first policy; without the prefetch these rows come from HBM every layer)
         constexpr int LINES = HS / 32;
@@ -623,6 +634,18 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ q
         if (tid == 0) tp_cta_done(tp, TP_SLOT_ATT, tp_seq(tp, tp_out_op), gridDim.x);
     }
     trace_mark(tr, 3);
+}
+
+template <int HS>
+__global__ void __launch_bounds__(ATT_THREADS) k_attention(float *__restrict__ qkv, float *__restrict__ kc, float *__restrict__ vc,
+                                                          const StepState *__restrict__ st, const float *__restrict__ cr,
+                                                          const float *__restrict__ ci, int n_heads, int n_kv_heads, int arch /* KF_* flags */,
+                                                          const float *__restrict__ qnorm_w, const float *__restrict__ knorm_w,
+                                                          const float *__restrict__ qkv_bias, float eps, float sqrt_hs, int8_t *__restrict__ xq,
+                                                          float *__restrict__ xs, float *__restrict__ xb, TraceBuf tr, TpCtx tp,
+                                                          unsigned tp_out_op, int head_base, float *att_scratch, int ctx) {
+    attention_head<HS>(qkv, kc, vc, &st->pos, cr, ci, n_heads, n_kv_heads, arch, qnorm_w, knorm_w, qkv_bias, eps, sqrt_hs, xq, xs, xb, tr, tp,
+                       tp_out_op, head_base, att_scratch, ctx);
 }
 
 // ------------------------------------------------------------------------------------------

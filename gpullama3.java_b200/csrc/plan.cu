@@ -10,6 +10,7 @@
 #include "kquant.cuh"
 #include "decode_persistent.cuh"
 #include "sampler.cuh"
+#include "decode_batch.cuh"
 
 #include <math.h>
 #include <stdarg.h>
@@ -132,6 +133,24 @@ struct b200_plan {
     unsigned long long *pd_trace = nullptr;
     unsigned pd_flags_off = 0;
     bool pd_coop = true;          // launched with the cooperative attribute (co-residency guaranteed by the driver)
+
+    // batched decode (decode_batch.cuh): n_slots KV caches [slot][layer][ctx][kvDim] and per-row activations, one graph per row count
+    struct Batch {
+        int n_slots = 0;
+        std::vector<void *> allocs;
+        float *slot_k = nullptr, *slot_v = nullptr;
+        float *x = nullptr, *qkv = nullptr, *hb = nullptr, *logits = nullptr, *xs = nullptr, *hs = nullptr, *att_scratch = nullptr;
+        int8_t *xq = nullptr, *hq = nullptr;
+        float *part_val = nullptr;
+        int *part_idx = nullptr, *ids = nullptr, *smp_out = nullptr;
+        unsigned *blk_cnt = nullptr;
+        BatchRows *rows = nullptr, *h_rows = nullptr; // device / pinned host
+        int *h_out = nullptr;                         // pinned: ids [SMB_MAX_ROWS] then sampler outputs [SMB_MAX_ROWS][8]
+        cudaGraphExec_t g[SMB_MAX_ROWS + 1] = {};
+        int launches[SMB_MAX_ROWS + 1] = {};
+        int last_n = 0;
+        float last_ms = 0.f;
+    } bt;
 };
 
 namespace {
@@ -821,6 +840,135 @@ int capture_all(b200_plan *p) {
     return B200_OK;
 }
 
+// ---- batched decode (decode_batch.cuh) -------------------------------------------------------------------------------------
+// 112 KB: two batched-stream CTAs (the gate/up and down projections, back to back under PDL) still fit on one SM together.
+const size_t SMB_SMEM_BUDGET = 112 * 1024;
+
+// Largest row count whose batched stream keeps at least 3 ring stages on every matrix of the plan.
+int batch_max_rows(const b200_plan *p) {
+    const LayerW &L0 = p->layers[0];
+    const int segs[5] = {L0.tqkv.seg, L0.two.seg, L0.tgu.seg, L0.tw2.seg, p->tout.seg};
+    for (int n = SMB_MAX_ROWS; n > 0; n--) {
+        bool ok = true;
+        for (int s : segs) ok = ok && smb_layout(s, n, SMB_SMEM_BUDGET).stages >= 3;
+        if (ok) return n;
+    }
+    return 0;
+}
+
+template <int MODE>
+int launch_stream_batch(b200_plan *p, const TileMat &W, int n, const int8_t *xq, const float *xs, float *out, int ostride, int8_t *hq = nullptr,
+                        float *hs = nullptr, bool argmax = false) {
+    const SmbSmem L = smb_layout(W.seg, n, SMB_SMEM_BUDGET);
+    SmbArgs a;
+    a.W = W; a.nrow = n; a.xq = xq; a.xs = xs; a.out = out; a.ostride = ostride; a.hq = hq; a.hs = hs; a.blk_cnt = p->bt.blk_cnt;
+    a.part_val = argmax ? p->bt.part_val : nullptr;
+    a.part_idx = argmax ? p->bt.part_idx : nullptr;
+    return launch_k(p, p->use_pdl, k_stream_matvec_q8_batch<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L);
+}
+
+// One forward step of n rows: the single-sequence graph's kernel sequence, every launch serving all n rows.
+int enqueue_batch(b200_plan *p, int n, int *launches) {
+    const b200_config &c = p->cfg;
+    auto &B = p->bt;
+    const bool pdl = p->use_pdl;
+    const int qkvd = p->qd + 2 * p->kvd;
+    const size_t ctx_kv = (size_t)c.context_length * p->kvd, slot_stride = (size_t)c.n_layers * ctx_kv;
+    const size_t norm_smem = norm_smem_bytes(c.dim, p->norm_v2);
+    TpCtx solo{};
+    solo.n = 1;
+    int k = 0, rc;
+    auto norm = [&](bool embed, const float *w) {
+        auto go = [&](auto kern) {
+            return launch_k(p, pdl, kern, dim3(n), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
+        };
+        k++;
+        if (p->norm_v2) return embed ? go(k_rmsnorm_quant_batch<true, true>) : go(k_rmsnorm_quant_batch<false, true>);
+        return embed ? go(k_rmsnorm_quant_batch<true, false>) : go(k_rmsnorm_quant_batch<false, false>);
+    };
+    for (int l = 0; l < c.n_layers; l++) {
+        const LayerW &L = p->layers[l];
+        if ((rc = norm(l == 0, L.attn_norm))) return rc;
+        if ((rc = launch_stream_batch<SMV_STORE>(p, L.tqkv, n, B.xq, B.xs, B.qkv, qkvd))) return rc;
+        float *kc = B.slot_k + (size_t)l * ctx_kv, *vc = B.slot_v + (size_t)l * ctx_kv;
+        auto att = [&](auto kern) {
+            return launch_k(p, pdl, kern, dim3(p->nh_l, n), dim3(ATT_THREADS), att_smem_bytes(c.head_size, c.context_length, B.att_scratch != nullptr), B.qkv, qkvd,
+                            kc, vc, slot_stride, (const BatchRows *)B.rows, (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags,
+                            (const float *)L.q_norm, (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, (float)sqrt((double)c.head_size), B.xq,
+                            B.xs, B.att_scratch, c.context_length, TraceBuf{nullptr, 0, 0}, solo);
+        };
+        if (c.head_size == 128) rc = att(k_attention_batch<128>);
+        else if (c.head_size == 64) rc = att(k_attention_batch<64>);
+        else if (c.head_size == 256) rc = att(k_attention_batch<256>);
+        else if (c.head_size == 96) rc = att(k_attention_batch<96>);
+        else rc = att(k_attention_batch<32>);
+        if (rc) return rc;
+        if ((rc = launch_stream_batch<SMV_RESID>(p, L.two, n, B.xq, B.xs, B.x, c.dim))) return rc;
+        if ((rc = norm(false, L.ffn_norm))) return rc;
+        if ((rc = launch_stream_batch<SMV_GATEUP>(p, L.tgu, n, B.xq, B.xs, B.hb, c.hidden_dim, B.hq, B.hs))) return rc;
+        if ((rc = launch_stream_batch<SMV_RESID>(p, L.tw2, n, B.hq, B.hs, B.x, c.dim))) return rc;
+        k += 5;
+    }
+    if ((rc = norm(false, p->out_norm))) return rc;
+    if ((rc = launch_stream_batch<SMV_STORE>(p, p->tout, n, B.xq, B.xs, B.logits, sampler_padded(c.vocab_size), nullptr, nullptr, true))) return rc;
+    if ((rc = launch_k(p, pdl, k_argmax_batch, dim3(n), dim3(32), (size_t)0, (const float *)B.part_val, (const int *)B.part_idx, p->n_sms, B.ids))) return rc;
+    if (launches) *launches = k + 2;
+    return B200_OK;
+}
+
+int capture_batch(b200_plan *p, int n) {
+    cudaGraph_t g = nullptr;
+    CK(cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal));
+    int rc = enqueue_batch(p, n, &p->bt.launches[n]);
+    cudaError_t e = cudaStreamEndCapture(p->stream, &g);
+    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+    if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(e));
+    e = cudaGraphInstantiate(&p->bt.g[n], g, 0);
+    cudaGraphDestroy(g);
+    if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e));
+    return B200_OK;
+}
+
+void batch_free(b200_plan *p) {
+    auto &B = p->bt;
+    for (cudaGraphExec_t &g : B.g)
+        if (g) { cudaGraphExecDestroy(g); g = nullptr; }
+    for (void *d : B.allocs) cudaFree(d);
+    if (B.h_rows) cudaFreeHost(B.h_rows);
+    if (B.h_out) cudaFreeHost(B.h_out);
+    B = b200_plan::Batch{};
+}
+
+template <typename T> int balloc(b200_plan *p, T **ptr, size_t n_bytes) {
+    void *d = nullptr;
+    CK(cudaMalloc(&d, n_bytes ? n_bytes : 16));
+    p->bt.allocs.push_back(d);
+    CK(cudaMemsetAsync(d, 0, n_bytes ? n_bytes : 16, p->stream));
+    *ptr = reinterpret_cast<T *>(d);
+    return B200_OK;
+}
+
+int batch_alloc(b200_plan *p, int ns) {
+    const b200_config &c = p->cfg;
+    auto &B = p->bt;
+    const int big = c.dim > p->qd ? c.dim : p->qd;
+    const size_t N = (size_t)ns, kv = (size_t)c.n_layers * c.context_length * p->kvd * 4;
+    int rc;
+    if ((rc = balloc(p, &B.slot_k, N * kv)) || (rc = balloc(p, &B.slot_v, N * kv)) || (rc = balloc(p, &B.x, N * c.dim * 4)) ||
+        (rc = balloc(p, &B.qkv, N * (p->qd + 2 * p->kvd) * 4)) || (rc = balloc(p, &B.hb, N * c.hidden_dim * 4)) ||
+        (rc = balloc(p, &B.logits, N * sampler_padded(c.vocab_size) * 4)) || (rc = balloc(p, &B.xq, N * big)) || (rc = balloc(p, &B.xs, N * (big / 32) * 4)) ||
+        (rc = balloc(p, &B.hq, N * c.hidden_dim)) || (rc = balloc(p, &B.hs, N * (c.hidden_dim / 32) * 4)) ||
+        (rc = balloc(p, &B.part_val, N * p->n_sms * 4)) || (rc = balloc(p, &B.part_idx, N * p->n_sms * 4)) || (rc = balloc(p, &B.ids, N * 4)) ||
+        (rc = balloc(p, &B.smp_out, N * 8 * 4)) || (rc = balloc(p, &B.blk_cnt, N * (c.hidden_dim / 32) * 4)) || (rc = balloc(p, &B.rows, sizeof(BatchRows))))
+        return rc;
+    if (p->att_scratch && (rc = balloc(p, &B.att_scratch, N * p->nh_l * c.context_length * 4))) return rc;
+    CK(cudaMallocHost(&B.h_rows, sizeof(BatchRows)));
+    CK(cudaMallocHost(&B.h_out, (size_t)SMB_MAX_ROWS * 9 * 4));
+    CK(cudaStreamSynchronize(p->stream));
+    B.n_slots = ns;
+    return B200_OK;
+}
+
 // cudaFuncSetAttribute is per function and process-wide: every kernel gets the device opt-in maximum ONCE, so a later plan
 // with a smaller context never lowers the limit under an earlier plan's instantiated graphs.
 const int ATT_SMEM_FLOATS_MAX = 4096; // q|k|out|scores beyond this: the score row goes to a global scratch row
@@ -868,6 +1016,18 @@ int set_smem_attrs(b200_plan *p) {
     CK(set_max_dyn(k_stream_matvec_f16<8, SF_STORE>, maxdyn));
     CK(set_max_dyn(k_stream_matvec_f16<8, SF_RESID>, maxdyn));
     CK(set_max_dyn(k_stream_matvec_f16<8, SF_GATEUP>, maxdyn));
+    CK(set_max_dyn(k_rmsnorm_quant_batch<true, false>, maxdyn));
+    CK(set_max_dyn(k_rmsnorm_quant_batch<false, false>, maxdyn));
+    CK(set_max_dyn(k_rmsnorm_quant_batch<true, true>, maxdyn));
+    CK(set_max_dyn(k_rmsnorm_quant_batch<false, true>, maxdyn));
+    CK(set_max_dyn(k_attention_batch<32>, maxdyn));
+    CK(set_max_dyn(k_attention_batch<64>, maxdyn));
+    CK(set_max_dyn(k_attention_batch<128>, maxdyn));
+    CK(set_max_dyn(k_attention_batch<96>, maxdyn));
+    CK(set_max_dyn(k_attention_batch<256>, maxdyn));
+    CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
+    CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
+    CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     done = true;
     return B200_OK;
 }
@@ -1601,6 +1761,118 @@ int b200_kv_reset(b200_plan *p) {
     return B200_OK;
 }
 
+int b200_set_decode_slots(b200_plan *p, int32_t n_slots) {
+    if (!p) return B200_ERR_BAD_ARG;
+    if (n_slots < 0) return fail(p, B200_ERR_BAD_ARG, "n_slots must be >= 0");
+    CK(cudaSetDevice(p->device));
+    CK(cudaStreamSynchronize(p->stream));
+    if (n_slots == 0) { batch_free(p); return B200_OK; }
+    if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "batched decode runs on single-GPU plans only (this plan is tensor-parallel)");
+    if (p->wtype != B200_GGML_Q8_0) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs Q8_0 weights (FP16 plans decode one sequence per step)");
+    if (!p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs the Q8_0 streaming layout (this plan uses the non-streaming matvecs)");
+    const int mx = batch_max_rows(p);
+    if (n_slots > mx) return fail(p, B200_ERR_UNSUPPORTED, "at most %d decode slots on this plan (asked for %d)", mx, n_slots);
+    batch_free(p);
+    const int rc = batch_alloc(p, n_slots);
+    if (rc) { batch_free(p); return rc; }
+    return B200_OK;
+}
+
+int b200_forward_decode_batch(b200_plan *p, int32_t n, const int32_t *slots, const int32_t *tokens, const int32_t *positions, const float *sampling,
+                              int32_t *ids_out, float *logits) {
+    if (!p) return B200_ERR_BAD_ARG;
+    auto &B = p->bt;
+    if (!B.n_slots) return fail(p, B200_ERR_STATE, "no decode slots: call b200_set_decode_slots first");
+    if (!slots || !tokens || !positions || !ids_out) return fail(p, B200_ERR_BAD_ARG, "slots, tokens, positions and ids_out must not be NULL");
+    if (n < 1 || n > B.n_slots) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (the plan's decode slots)", n, B.n_slots);
+    const b200_config &c = p->cfg;
+    for (int i = 0; i < n; i++) {
+        if (slots[i] < 0 || slots[i] >= B.n_slots) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d out of range (%d slots)", i, slots[i], B.n_slots);
+        for (int j = 0; j < i; j++)
+            if (slots[j] == slots[i]) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d repeats row %d's", i, slots[i], j);
+        if (tokens[i] < 0 || tokens[i] >= c.vocab_size) return fail(p, B200_ERR_BAD_ARG, "row %d: token %d out of range", i, tokens[i]);
+        if (positions[i] < 0 || positions[i] >= c.context_length)
+            return fail(p, B200_ERR_BAD_ARG, "row %d: position %d outside the KV cache (%d)", i, positions[i], c.context_length);
+        if (sampling) {
+            const float t = sampling[3 * i], u = sampling[3 * i + 2];
+            if (!(t >= 0.0f) || !(u >= 0.0f && u < 1.0f))
+                return fail(p, B200_ERR_BAD_ARG, "row %d: temperature must be >= 0 and the uniform number in [0, 1)", i);
+        }
+    }
+    CK(cudaSetDevice(p->device));
+    int rc;
+    if (!B.g[n] && (rc = capture_batch(p, n))) return rc;
+    for (int i = 0; i < n; i++) { B.h_rows->token[i] = tokens[i]; B.h_rows->pos[i] = positions[i]; B.h_rows->slot[i] = slots[i]; }
+    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaEventRecord(p->ev0, p->stream));
+    CK(cudaGraphLaunch(B.g[n], p->stream));
+    CK(cudaEventRecord(p->ev1, p->stream));
+    const size_t vpad = (size_t)sampler_padded(c.vocab_size);
+    if (logits) // before the sampler turns sampled rows into probabilities
+        for (int i = 0; i < n; i++) CK(cudaMemcpyAsync(logits + (size_t)i * c.vocab_size, B.logits + i * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
+    bool any_sampled = false;
+    for (int i = 0; i < n; i++) {
+        if (!sampling || sampling[3 * i] == 0.0f) continue; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed
+        static bool attr = false;
+        if (!attr) { CK(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes())); attr = true; }
+        SamplerArgs a;
+        a.logits = B.logits + i * vpad; a.n = c.vocab_size; a.temperature = sampling[3 * i]; a.topp = sampling[3 * i + 1]; a.r01 = sampling[3 * i + 2];
+        a.indices = p->smp_indices; a.out_id = B.smp_out + 8 * i; a.info = B.smp_out + 8 * i + 1;
+        k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
+        CK(cudaGetLastError());
+        any_sampled = true;
+    }
+    CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)n * 4, cudaMemcpyDeviceToHost, p->stream));
+    if (any_sampled) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)n * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
+    for (int i = 0; i < n; i++) ids_out[i] = (sampling && sampling[3 * i] != 0.0f) ? B.h_out[SMB_MAX_ROWS + 8 * i] : B.h_out[i];
+    CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
+    B.last_n = n;
+    return B200_OK;
+}
+
+int b200_slot_reset(b200_plan *p, int32_t slot) {
+    if (!p) return B200_ERR_BAD_ARG;
+    if (slot < 0 || slot >= p->bt.n_slots) return fail(p, B200_ERR_BAD_ARG, "slot %d out of range (%d slots)", slot, p->bt.n_slots);
+    CK(cudaSetDevice(p->device));
+    const size_t kv = (size_t)p->cfg.n_layers * p->cfg.context_length * p->kvd;
+    CK(cudaMemsetAsync(p->bt.slot_k + (size_t)slot * kv, 0, kv * 4, p->stream));
+    CK(cudaMemsetAsync(p->bt.slot_v + (size_t)slot * kv, 0, kv * 4, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
+    return B200_OK;
+}
+
+int b200_slot_copy_kv(b200_plan *p, int32_t slot, int32_t n_positions) {
+    if (!p) return B200_ERR_BAD_ARG;
+    const b200_config &c = p->cfg;
+    if (slot < 0 || slot >= p->bt.n_slots) return fail(p, B200_ERR_BAD_ARG, "slot %d out of range (%d slots)", slot, p->bt.n_slots);
+    if (n_positions < 0 || n_positions > c.context_length) return fail(p, B200_ERR_BAD_ARG, "n_positions %d outside [0, %d]", n_positions, c.context_length);
+    CK(cudaSetDevice(p->device));
+    const size_t ctx_kv = (size_t)c.context_length * p->kvd, head = (size_t)n_positions * p->kvd;
+    for (int l = 0; l < c.n_layers; l++) {
+        const size_t o = ((size_t)slot * c.n_layers + l) * ctx_kv;
+        float *dk = p->bt.slot_k + o, *dv = p->bt.slot_v + o;
+        if (head) {
+            CK(cudaMemcpyAsync(dk, p->key_cache + (size_t)l * ctx_kv, head * 4, cudaMemcpyDeviceToDevice, p->stream));
+            CK(cudaMemcpyAsync(dv, p->value_cache + (size_t)l * ctx_kv, head * 4, cudaMemcpyDeviceToDevice, p->stream));
+        }
+        if (head < ctx_kv) { // beyond the prefix the slot must read like a fresh State (the Qwen3 / Qwen2 loop reads a skipped, zero position)
+            CK(cudaMemsetAsync(dk + head, 0, (ctx_kv - head) * 4, p->stream));
+            CK(cudaMemsetAsync(dv + head, 0, (ctx_kv - head) * 4, p->stream));
+        }
+    }
+    CK(cudaStreamSynchronize(p->stream));
+    return B200_OK;
+}
+
+int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step) {
+    if (!p) return B200_ERR_BAD_ARG;
+    if (n_slots) *n_slots = p->bt.n_slots;
+    if (launches_per_step) *launches_per_step = p->bt.last_n ? p->bt.launches[p->bt.last_n] : 0;
+    if (device_ms_last_step) *device_ms_last_step = p->bt.last_ms;
+    return B200_OK;
+}
+
 int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, size_t bytes) {
     if (!p || !name || !dst) return B200_ERR_BAD_ARG;
     const b200_config &c = p->cfg;
@@ -1620,6 +1892,10 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
     else if (s == "key_cache" || s == "value_cache") {
         if (layer < 0 || layer >= c.n_layers) return fail(p, B200_ERR_BAD_ARG, "layer out of range");
         src = (s == "key_cache" ? p->key_cache : p->value_cache) + (size_t)layer * ctx_kv;
+        sz = ctx_kv * 4;
+    } else if (s == "slot_key_cache" || s == "slot_value_cache") {
+        if (layer < 0 || layer >= p->bt.n_slots * c.n_layers) return fail(p, B200_ERR_BAD_ARG, "slot layer %d out of range (%d slots)", layer, p->bt.n_slots);
+        src = (s == "slot_key_cache" ? p->bt.slot_k : p->bt.slot_v) + (size_t)layer * ctx_kv;
         sz = ctx_kv * 4;
     } else if (s.rfind("pf_", 0) == 0) { // tensor-core prefill scratch: [padded rows][width], the last layer of the last chunk
         const PrefillCtx &pc = p->prefill;
@@ -2090,6 +2366,7 @@ void b200_plan_free(b200_plan *p) {
     cudaSetDevice(p->device);
     if (p->stream) cudaStreamSynchronize(p->stream);
     prefill_free(p->prefill);
+    batch_free(p);
     if (p->g_decode) cudaGraphExecDestroy(p->g_decode);
     if (p->g_prefill) cudaGraphExecDestroy(p->g_prefill);
     if (p->g_trace) cudaGraphExecDestroy(p->g_trace);

@@ -7,6 +7,7 @@ Position/token conventions decide parity, so they are restated exactly:
                               including its skipped position after the last prompt token
 ``generate_tokens_llama_batch_prefill`` <- InferenceEngineWithBatchPrefillDecode.generateTokensGPULlama
                               (InferenceEngineWithBatchPrefillDecode.java:163-251)
+``generate_tokens_batch``  several requests through the first two loops in lockstep on the plan's decode slots
 The sampler is greedy (temperature 0 -> FloatTensor.argmax, Sampler.java:124-132) and runs on
 the device; ``forward`` is any callable (token, position) -> argmax so the same loops drive
 the oracle in the tests.
@@ -18,15 +19,16 @@ from typing import Callable, Iterable
 Forward = Callable[[int, int], int]
 
 
-def generate_tokens_llama(forward: Forward, latest_token: int, start_position: int, prompt_tokens: list[int],
-                          stop_tokens: Iterable[int], max_tokens: int, context_length: int) -> list[int]:
+def _llama_steps(latest_token: int, start_position: int, prompt_tokens: list[int], stop_tokens: Iterable[int], max_tokens: int,
+                 context_length: int):
+    """generate_tokens_llama as a generator: yields each forward's (token, position), receives its argmax, returns the ids."""
     if max_tokens < 0 or context_length < max_tokens:
         max_tokens = context_length
     stop = set(stop_tokens)
     generated: list[int] = []
     current, prompt_index, pos = latest_token, 0, start_position
     while pos < max_tokens:
-        am = forward(current, pos)
+        am = yield current, pos
         if prompt_index < len(prompt_tokens):
             nxt = prompt_tokens[prompt_index]
             prompt_index += 1
@@ -40,8 +42,9 @@ def generate_tokens_llama(forward: Forward, latest_token: int, start_position: i
     return generated
 
 
-def generate_tokens_qwen3(forward: Forward, latest_token: int, start_position: int, prompt_tokens: list[int],
-                          stop_tokens: Iterable[int], max_tokens: int, context_length: int) -> list[int]:
+def _qwen3_steps(latest_token: int, start_position: int, prompt_tokens: list[int], stop_tokens: Iterable[int], max_tokens: int,
+                 context_length: int):
+    """generate_tokens_qwen3 as a generator (see _llama_steps)."""
     if max_tokens < 0 or context_length < max_tokens:
         max_tokens = context_length
     stop = set(stop_tokens)
@@ -50,14 +53,14 @@ def generate_tokens_qwen3(forward: Forward, latest_token: int, start_position: i
     position = start_position
     while position < max_tokens:
         if prompt_index < len(prompt_tokens):
-            am = forward(prompt_tokens[prompt_index], position)
+            am = yield prompt_tokens[prompt_index], position
             prompt_index += 1
             if prompt_index < len(prompt_tokens):
                 position += 1
                 continue
             position += 1  # "The current logit belongs to the next position" (InferenceEngine.java:194)
         else:
-            am = forward(current, position)
+            am = yield current, position
         nxt = am
         generated.append(nxt)
         if nxt in stop:
@@ -67,10 +70,66 @@ def generate_tokens_qwen3(forward: Forward, latest_token: int, start_position: i
     return generated
 
 
+def _drive(steps, forward: Forward) -> list[int]:
+    try:
+        req = next(steps)
+        while True:
+            req = steps.send(forward(*req))
+    except StopIteration as done:
+        return done.value
+
+
+def generate_tokens_llama(forward: Forward, latest_token: int, start_position: int, prompt_tokens: list[int],
+                          stop_tokens: Iterable[int], max_tokens: int, context_length: int) -> list[int]:
+    return _drive(_llama_steps(latest_token, start_position, prompt_tokens, stop_tokens, max_tokens, context_length), forward)
+
+
+def generate_tokens_qwen3(forward: Forward, latest_token: int, start_position: int, prompt_tokens: list[int],
+                          stop_tokens: Iterable[int], max_tokens: int, context_length: int) -> list[int]:
+    return _drive(_qwen3_steps(latest_token, start_position, prompt_tokens, stop_tokens, max_tokens, context_length), forward)
+
+
 def loop_for(model_type: str):
     """The generation loop the reference's model class uses: Qwen3, Qwen2 and DeepSeek-R1-Distill-Qwen run generateTokensQwen3
     (Qwen3.java, Qwen2.java:95-115), the others generateTokensLlama."""
-    return generate_tokens_qwen3 if model_type.upper() in ("QWEN_3", "QWEN_2", "DEEPSEEK_R1_DISTILL_QWEN") else generate_tokens_llama
+    return generate_tokens_qwen3 if _is_qwen_loop(model_type) else generate_tokens_llama
+
+
+def _is_qwen_loop(model_type: str) -> bool:
+    return model_type.upper() in ("QWEN_3", "QWEN_2", "DEEPSEEK_R1_DISTILL_QWEN")
+
+
+def generate_tokens_batch(plan, model_type: str, requests: list, stop_tokens: Iterable[int], max_tokens: int,
+                          context_length: int) -> list[list[int]]:
+    """Several independent generations in lockstep on the plan's decode slots (request i on slot i, reset first): one
+    forward_decode_batch per step for every request still running.  Each request is (latest_token, start_position,
+    prompt_tokens) and follows the loop loop_for(model_type) runs, so each result equals that loop's for the request alone;
+    a request leaves the batch at its stop token or budget."""
+    n_slots = plan.batch_info()[0]
+    if len(requests) > n_slots:
+        raise ValueError(f"{len(requests)} requests but the plan has {n_slots} decode slots (set_decode_slots)")
+    make = _qwen3_steps if _is_qwen_loop(model_type) else _llama_steps
+    stop = list(stop_tokens)
+    results: list = [None] * len(requests)
+    live: dict = {}  # request index -> (generator, pending (token, position))
+    for i, (latest, start, prompt) in enumerate(requests):
+        plan.slot_reset(i)
+        g = make(latest, start, list(prompt), stop, max_tokens, context_length)
+        try:
+            live[i] = (g, next(g))
+        except StopIteration as done:
+            results[i] = done.value
+    while live:
+        rows = sorted(live)
+        ids, _ = plan.forward_decode_batch(rows, [live[i][1][0] for i in rows], [live[i][1][1] for i in rows])
+        for i, am in zip(rows, ids):
+            g = live[i][0]
+            try:
+                live[i] = (g, g.send(int(am)))
+            except StopIteration as done:
+                results[i] = done.value
+                del live[i]
+    return results
 
 
 def generate_tokens_llama_batch_prefill(plan, latest_token: int, start_position: int, prompt_tokens: list[int],

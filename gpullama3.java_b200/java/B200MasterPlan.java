@@ -61,6 +61,11 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle TP_HANDLE = fn("b200_tp_handle", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle TP_ATTACH = fn("b200_tp_attach", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, JAVA_INT));
     private static final MethodHandle KV_RESET = fn("b200_kv_reset", FunctionDescriptor.of(JAVA_INT, ADDRESS));
+    private static final MethodHandle SET_DECODE_SLOTS = fn("b200_set_decode_slots", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
+    private static final MethodHandle DECODE_BATCH = fn("b200_forward_decode_batch",
+            FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
+    private static final MethodHandle SLOT_RESET = fn("b200_slot_reset", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
+    private static final MethodHandle SLOT_COPY_KV = fn("b200_slot_copy_kv", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
     private static final MethodHandle FREE = fn("b200_plan_free", FunctionDescriptor.ofVoid(ADDRESS));
     private static final MethodHandle LAST_ERROR = fn("b200_last_error", FunctionDescriptor.of(ADDRESS, ADDRESS));
 
@@ -207,6 +212,38 @@ public final class B200MasterPlan implements AutoCloseable {
 
     public void kvReset() throws Throwable {
         int rc = (int) KV_RESET.invokeExact(plan);
+        if (rc != 0) check(rc, lastError());
+    }
+
+    /** Up to 8 KV-cache slots (one State per conversation) for forwardDecodeBatch; 0 frees them.  Q8_0 streaming plans only. */
+    public void setDecodeSlots(int nSlots) throws Throwable {
+        int rc = (int) SET_DECODE_SLOTS.invokeExact(plan, nSlots);
+        if (rc != 0) check(rc, lastError());
+    }
+
+    /** One step for tokens.length independent sequences: row i = tokens[i] at positions[i] on slot slots[i].  sampling is null
+     *  (greedy) or {temperature, topp, rng.nextFloat(1f)} per row.  Returns one token id per row; each row is bit-identical to
+     *  forwardDecode / forwardDecodeSample of its own sequence. */
+    public int[] forwardDecodeBatch(int[] slots, int[] tokens, int[] positions, float[] sampling) throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            int n = tokens.length;
+            MemorySegment ids = a.allocate(JAVA_INT, n);
+            MemorySegment smp = sampling == null ? MemorySegment.NULL : a.allocateFrom(java.lang.foreign.ValueLayout.JAVA_FLOAT, sampling);
+            int rc = (int) DECODE_BATCH.invokeExact(plan, n, a.allocateFrom(JAVA_INT, slots), a.allocateFrom(JAVA_INT, tokens),
+                    a.allocateFrom(JAVA_INT, positions), smp, ids, MemorySegment.NULL);
+            if (rc != 0) check(rc, lastError());
+            return ids.toArray(JAVA_INT);
+        }
+    }
+
+    public void slotReset(int slot) throws Throwable {
+        int rc = (int) SLOT_RESET.invokeExact(plan, slot);
+        if (rc != 0) check(rc, lastError());
+    }
+
+    /** Positions [0, nPositions) of the plan's own KV cache (a prompt after forwardBatchPrefill) into the slot; the rest of it zeroed. */
+    public void slotCopyKv(int slot, int nPositions) throws Throwable {
+        int rc = (int) SLOT_COPY_KV.invokeExact(plan, slot, nPositions);
         if (rc != 0) check(rc, lastError());
     }
 

@@ -42,6 +42,7 @@ class Tensor(C.Structure):
 EXPORTS = ["b200_plan_create", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_test_seqsum", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
+           "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_batch_info",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -81,6 +82,11 @@ def lib() -> C.CDLL:
     L.b200_test_pf_attention.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.b200_time_kernel.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
     L.b200_read_buffer.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
+    L.b200_set_decode_slots.argtypes = [vp, i32]
+    L.b200_forward_decode_batch.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]
+    L.b200_slot_reset.argtypes = [vp, i32]
+    L.b200_slot_copy_kv.argtypes = [vp, i32, i32]
+    L.b200_batch_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     L.b200_launches_per_decode.argtypes = [vp]
     L.b200_device_bytes.argtypes = [vp]
@@ -312,6 +318,41 @@ class NativePlan:
         ms = C.c_float(0)
         self._ck(lib().b200_decode_sequence(self._p, t.ctypes.data, n, start_pos, 1 if feedback else 0, out.ctypes.data, C.byref(ms)))
         return out, ms.value
+
+    def set_decode_slots(self, n_slots: int):
+        self._ck(lib().b200_set_decode_slots(self._p, n_slots))
+
+    def forward_decode_batch(self, slots, tokens, positions, sampling=None, want_logits: bool = False):
+        """One batched step (b200_forward_decode_batch): row i = tokens[i] at positions[i] on slot slots[i].  sampling: None or
+        n x (temperature, topp, uniform01).  Returns (ids int32 [n], logits float32 [n, vocab] or None)."""
+        s = np.ascontiguousarray(slots, dtype=np.int32)
+        t = np.ascontiguousarray(tokens, dtype=np.int32)
+        p = np.ascontiguousarray(positions, dtype=np.int32)
+        n = len(s)
+        if len(t) != n or len(p) != n:
+            raise ValueError("slots, tokens and positions must have the same length")
+        smp = None
+        if sampling is not None:
+            smp = np.ascontiguousarray(sampling, dtype=np.float32).reshape(-1)
+            if smp.size != 3 * n:
+                raise ValueError("sampling must hold (temperature, topp, uniform01) per row")
+        ids = np.empty(n, dtype=np.int32)
+        lg = np.empty((n, self.cfg.vocab_size), dtype=np.float32) if want_logits else None
+        self._ck(lib().b200_forward_decode_batch(self._p, n, s.ctypes.data, t.ctypes.data, p.ctypes.data, smp.ctypes.data if smp is not None else None,
+                                                 ids.ctypes.data, lg.ctypes.data if want_logits else None))
+        return ids, lg
+
+    def slot_reset(self, slot: int):
+        self._ck(lib().b200_slot_reset(self._p, slot))
+
+    def slot_copy_kv(self, slot: int, n_positions: int):
+        self._ck(lib().b200_slot_copy_kv(self._p, slot, n_positions))
+
+    def batch_info(self):
+        """(decode slots, kernels of the last batched step, its device milliseconds)."""
+        a, b, ms = C.c_int32(0), C.c_int32(0), C.c_float(0)
+        self._ck(lib().b200_batch_info(self._p, C.byref(a), C.byref(b), C.byref(ms)))
+        return a.value, b.value, ms.value
 
     def time_kernel(self, which: int, reps: int = 3):
         ms, nbytes = C.c_float(0), C.c_int64(0)

@@ -152,6 +152,28 @@ class B200MasterPlan:
     def time_kernel(self, which: int, reps: int = 3):
         return self._native.time_kernel(which, reps)
 
+    # Batched decode (csrc/decode_batch.cuh): up to 8 independent sequences per step, each on its own KV-cache slot, every weight
+    # matrix streamed once per step; each row bit-identical to forward_decode of the same token stream.  Q8_0 streaming plans only.
+    def set_decode_slots(self, n_slots: int):
+        """Allocate n_slots zeroed KV-cache slots (0 frees them); UnsupportedOperation beyond what the plan can run."""
+        self._native.set_decode_slots(n_slots)
+
+    def forward_decode_batch(self, slots, tokens, positions, sampling=None, logits: bool = False):
+        """One step for len(slots) rows -> (ids, logits [n, vocab] or None).  sampling: None (greedy) or one
+        (temperature, topp, uniform01) per row, with forward_decode_sample's contract."""
+        return self._native.forward_decode_batch(slots, tokens, positions, sampling, logits)
+
+    def slot_reset(self, slot: int):
+        self._native.slot_reset(slot)
+
+    def slot_copy_kv(self, slot: int, n_positions: int):
+        """Copy positions [0, n_positions) of the plan's own KV cache (e.g. after forward_batch_prefill) into the slot; zero the rest."""
+        self._native.slot_copy_kv(slot, n_positions)
+
+    def batch_info(self):
+        """(decode slots, kernels of the last batched step, its device milliseconds)."""
+        return self._native.batch_info()
+
     def kv_reset(self):
         self._native.kv_reset()
 

@@ -185,8 +185,42 @@ int b200_decode_sequence(b200_plan *plan, const int32_t *tokens, int32_t n, int3
  * InferenceEngine.java:175-225). */
 int b200_kv_reset(b200_plan *plan);
 
+/* ---- batched decode: up to B200_MAX_DECODE_SLOTS independent sequences per step ---------------------------------------------
+ * One step streams every weight matrix from HBM once for all its rows (csrc/decode_batch.cuh); every dot product keeps its own
+ * row, activation vector and block order, so each row is bit-identical to b200_forward_decode of the same token stream.  Single-GPU
+ * Q8_0 plans on the streaming layout only (K-quant files included; every architecture and head size); FP16 plans, the
+ * non-streaming Q8_0 layout and tensor-parallel plans get B200_ERR_UNSUPPORTED.  Batched steps always run as a multi-kernel CUDA
+ * graph with programmatic-dependent-launch edges, whatever b200_set_decode_mode selected; the plan's own KV cache, step state and
+ * graphs are not touched, so single-sequence calls can be interleaved with batched ones. */
+#define B200_MAX_DECODE_SLOTS 8
+
+/* Allocates n_slots zeroed KV caches ([layer][ctx][kvDim] f32 each, the plan's context_length), per-row activation buffers and,
+ * lazily, one graph per row count.  0 frees them.  B200_ERR_UNSUPPORTED (the message names the maximum) when the plan cannot
+ * run n_slots rows per step.  Calling it again replaces every slot with a zeroed one. */
+int b200_set_decode_slots(b200_plan *plan, int32_t n_slots);
+
+/* One forward step of n rows: row i consumes tokens[i] at positions[i] against slot slots[i]'s cache.  sampling is NULL (all rows
+ * greedy: FloatTensor.argmax, first strict maximum) or n x {temperature, topp, uniform01}: a row with temperature 0 takes the argmax,
+ * any other row runs b200_forward_decode_sample's sampler on its own logits.  ids_out receives n ids; logits (nullable) n x vocab_size
+ * floats.  B200_ERR_BAD_ARG naming the row for: n outside [1, n_slots], a repeated slot, a slot or position out of range, a bad
+ * token or sampling triple.  B200_ERR_STATE before b200_set_decode_slots. */
+int b200_forward_decode_batch(b200_plan *plan, int32_t n, const int32_t *slots, const int32_t *tokens, const int32_t *positions,
+                              const float *sampling /* nullable, 3n */, int32_t *ids_out, float *logits /* nullable, n x vocab */);
+
+/* Zero one slot's K/V cache (a fresh State). */
+int b200_slot_reset(b200_plan *plan, int32_t slot);
+
+/* Copy positions [0, n_positions) of the plan's own K/V cache into the slot and zero positions [n_positions, ctx): how a prompt
+ * prefilled with b200_forward_batch_prefill enters a slot.  The copy is exact after the exact prefill; after a tensor-core prefill it
+ * carries that mode's FP16 tolerance. */
+int b200_slot_copy_kv(b200_plan *plan, int32_t slot, int32_t n_positions);
+
+/* Decode slots, kernels of the last batched step and its device milliseconds (CUDA events around the graph); any pointer may be NULL. */
+int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step);
+
 /* Test/diagnostic read-back of a named device buffer into host memory.  Names:
- * "x","xb","q","k","v","hb","logits","key_cache","value_cache","xq","xs".  "q" (= "qkv") is the packed q|k|v vector of the
+ * "x","xb","q","k","v","hb","logits","key_cache","value_cache","xq","xs", and "slot_key_cache" / "slot_value_cache" with
+ * layer = slot * n_layers + layer.  "q" (= "qkv") is the packed q|k|v vector of the
  * last layer: its q part rotated (Qwen2: bias added, then rotated), its k and v parts as the matmul produced them, BEFORE any
  * Qwen2 bias (the KV caches hold the biased k, v).  `layer` selects the
  * layer for the KV caches (ignored otherwise).  The tensor-core prefill scratch, as the last layer of the last

@@ -24,13 +24,13 @@ struct BatchRows {
 // parameters, as the single-row kernels do: a zero-initialised local copy would be placed in local memory.
 
 // ---- RMSNorm + quantisation, one CTA per row ------------------------------------------------------------------------------
-template <bool EMBED, bool V2>
+template <bool EMBED>
 __global__ void __launch_bounds__(NORM_THREADS, 1) k_rmsnorm_quant_batch(float *__restrict__ x, const BatchRows *__restrict__ rows, DevMat emb,
                                                                      const float *__restrict__ w, float eps, int dim,
                                                                      int8_t *__restrict__ xq, float *__restrict__ xs, TraceBuf tr, TpCtx tp) {
     const int v = blockIdx.x;
-    rmsnorm_quant_row<EMBED, V2>(x + (size_t)v * dim, rows->token + v, emb, w, eps, dim, xq + (size_t)v * dim, xs + (size_t)v * (dim / 32),
-                                 nullptr, nullptr, tr, tp, -1);
+    rmsnorm_quant_row<EMBED>(x + (size_t)v * dim, rows->token + v, emb, w, eps, dim, xq + (size_t)v * dim, xs + (size_t)v * (dim / 32),
+                             nullptr, nullptr, tr, tp, -1);
 }
 
 // ---- attention, grid (heads, rows) ----------------------------------------------------------------------------------------

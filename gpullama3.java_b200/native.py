@@ -41,7 +41,7 @@ class Tensor(C.Structure):
 
 EXPORTS = ["b200_plan_create", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
-           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_test_seqsum", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
+           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_batch_info",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
@@ -68,7 +68,6 @@ def lib() -> C.CDLL:
     L.b200_trace_decode.argtypes = [vp, i32, i32, vp, i32, C.POINTER(i32)]
     L.b200_tp_handle.argtypes = [vp, vp]
     L.b200_tp_attach.argtypes = [vp, vp, i32]
-    L.b200_test_seqsum.argtypes = [vp, i32, C.POINTER(C.c_float), C.POINTER(i32)]
     L.b200_set_prefill_mode.argtypes = [vp, i32]
     L.b200_set_decode_mode.argtypes = [vp, i32]
     L.b200_decode_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
@@ -79,7 +78,7 @@ def lib() -> C.CDLL:
     L.b200_gemm_f16.argtypes = [vp, vp, vp, i32, i32, i32, i32, C.POINTER(C.c_float)]
     L.b200_test_gemm.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.b200_test_gemm_q8.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
-    L.b200_test_pf_attention.argtypes = [i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
+    L.b200_test_pf_attention.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.b200_time_kernel.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
     L.b200_read_buffer.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
     L.b200_set_decode_slots.argtypes = [vp, i32]
@@ -106,17 +105,14 @@ def _raise(code: int, msg: str):
     raise B200Error(code, msg)
 
 
-def test_seqsum(terms, want_info: bool = False, threads: int = 0):
-    """threads = 0: the round-1 accumulator (seqsum.cuh); 1024 / 256: seqsum2.cuh in the norm kernel's / persistent kernel's form."""
+def test_seqsum(terms, want_info: bool = False, threads: int = 1024):
+    """The exact sequential sum (seqsum2.cuh) with 1024 / 512 / 256 threads: the norm kernel's / persistent kernel's form."""
     t = np.ascontiguousarray(terms, dtype=np.float32)
     out = C.c_float(0)
     info = (C.c_int32 * 2)()
-    if threads:
-        rc = lib().b200_test_seqsum2(t.ctypes.data, len(t), threads, C.byref(out), info)
-    else:
-        rc = lib().b200_test_seqsum(t.ctypes.data, len(t), C.byref(out), info)
+    rc = lib().b200_test_seqsum2(t.ctypes.data, len(t), threads, C.byref(out), info)
     if rc != B200_OK:
-        _raise(rc, "b200_test_seqsum failed")
+        _raise(rc, "b200_test_seqsum2 failed")
     return (out.value, info[0], info[1]) if want_info else out.value
 
 
@@ -212,8 +208,10 @@ def test_gemm_q8(mode: str, a, bq, c, bq2=None, m_valid: int | None = None, stag
 def test_pf_attention(q, k, v, n_heads: int, n_kv_heads: int, start_pos: int, impl: str = "mma", out_rows: int | None = None,
                       sentinel: int = 0x7E5A) -> np.ndarray:
     """The prefill's causal attention over one chunk (csrc/prefill.cuh).  q float32 [n, n_heads*hs]; k, v float32
-    [start_pos+n, n_kv_heads*hs].  impl "mma" (k_pf_attention_mma) or "simt" (k_pf_attention).  Returns the f16 bits
+    [start_pos+n, n_kv_heads*hs].  impl names the kernel: "mma" (k_pf_attention_mma) is the only one.  Returns the f16 bits
     (uint16) of [out_rows, n_heads*hs]: rows >= n keep `sentinel`."""
+    if impl != "mma":
+        raise ValueError(f"no prefill attention kernel {impl!r}: the prefill runs k_pf_attention_mma (impl='mma')")
     q = np.ascontiguousarray(q, dtype=np.float32)
     k = np.ascontiguousarray(k, dtype=np.float32)
     v = np.ascontiguousarray(v, dtype=np.float32)
@@ -223,7 +221,7 @@ def test_pf_attention(q, k, v, n_heads: int, n_kv_heads: int, start_pos: int, im
         raise ValueError("k / v must be [start_pos + n, n_kv_heads * head_size]")
     rows = n if out_rows is None else out_rows
     out = np.full((rows, qd), sentinel, dtype=np.uint16)
-    rc = lib().b200_test_pf_attention({"mma": 0, "simt": 1}[impl], q.ctypes.data, k.ctypes.data, v.ctypes.data, n, start_pos, n_heads, n_kv_heads, hs,
+    rc = lib().b200_test_pf_attention(q.ctypes.data, k.ctypes.data, v.ctypes.data, n, start_pos, n_heads, n_kv_heads, hs,
                                       rows, out.ctypes.data)
     if rc != B200_OK:
         _raise(rc, "b200_test_pf_attention failed")

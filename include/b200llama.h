@@ -265,17 +265,14 @@ int b200_trace_decode(b200_plan *plan, int32_t token, int32_t position, uint64_t
 int b200_trace_persistent(b200_plan *plan, int32_t token, int32_t position, uint64_t *stamps, int64_t cap, int32_t *n_ctas, int32_t *n_rows, int32_t *n_stamps);
 
 /* Diagnostic: SM-clock cycles of the RMSNorm kernel's phases {launch->dependency wait, load+square,
- * exact sequential sum, normalise+quantise+store} followed by {entries, first fallback element or -1,
- * overflow flag} of the sequential-sum emulation, then at [8..12] the cycles of its phases
- * {group sums, head+prefix, group composition, barrier, resolve}.  cycles holds 16 int64. */
+ * exact sequential sum, normalise+quantise+store} followed by {items walked, fallbacks} of the exact
+ * sequential sum (csrc/seqsum2.cuh).  cycles holds 16 int64; [6..15] are set to 0. */
 int b200_profile_norm(b200_plan *plan, int64_t *cycles);
 
-/* Test hook for the exact parallel evaluation of the reference's sequential float sum
- * (csrc/seqsum.cuh; the RMSNorm accumulator of InferenceCore.java:39-48): sums n <= 8192
- * non-negative host floats on the device exactly as `for (i) s += t[i]` would. */
-int b200_test_seqsum(const float *terms, int32_t n, float *out, int32_t *info /* nullable: {entries, first fallback element or -1} */);
-/* Same contract for the round-2 accumulator (csrc/seqsum2.cuh) run by `threads` = 1024 (the RMSNorm kernel's form), 512
- * (the persistent decode kernel's form) or 256 threads; info = {items walked, fallbacks}. */
+/* Test hook for the exact parallel evaluation of the reference's sequential float sum (csrc/seqsum2.cuh; the RMSNorm
+ * accumulator of InferenceCore.java:39-48): sums n <= 8192 non-negative host floats on the device exactly as
+ * `for (i) s += t[i]` would, run by `threads` = 1024 (the RMSNorm kernel's form), 512 (the persistent decode kernel's form)
+ * or 256 threads; info = {items walked, fallbacks}. */
 int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out, int32_t *info /* nullable */);
 
 /* Test hook for the device-side sampler (csrc/sampler.cuh): ONE launch of k_sample as b200_forward_decode_sample issues it (same
@@ -320,19 +317,18 @@ int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, i
 
 /* Test hook: the causal attention of the tensor-core prefill over one chunk of n query tokens at positions start_pos ..
  * start_pos + n - 1.  q: f32 [n][n_heads * head_size] (rotated); k, v: f32 [start_pos + n][n_kv_heads * head_size] (the KV cache
- * rows).  impl 0 = k_pf_attention_mma (f16 K / V copies built by k_pf_kv_to_f16, as in the prefill), 1 = the FP32 SIMT
- * k_pf_attention.  q is placed in rows of stride q + 2 * kv width whose k / v columns hold NaN; grid and shared memory are the
- * prefill's.  out: f16 bits [out_rows][n_heads * head_size], out_rows >= n, in/out: rows >= n must come back untouched.
+ * rows), run by k_pf_attention_mma on f16 K / V copies built by k_pf_kv_to_f16, as in the prefill.  q is placed in rows of
+ * stride q + 2 * kv width whose k / v columns hold NaN; grid and shared memory are the prefill's.  out: f16 bits [out_rows][n_heads * head_size], out_rows >= n, in/out: rows >= n must come back untouched.
  * head_size 64 or 128, n_heads % n_kv_heads == 0 and n_heads / n_kv_heads <= 64 (any ratio: a CTA serves floor(64 / ratio) query
  * tokens, the remaining rows of its 64-row tile are padding). */
-int b200_test_pf_attention(int32_t impl, const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads,
+int b200_test_pf_attention(const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads,
                            int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out);
 
 /* Weight upload of b200_plan_create (the counterpart of the reference's load-time metrics, ModelLoader.java:102-106 and the
  * copy-in timing of TornadoVMMasterPlanSingleToken.java:51-54): wall seconds from the first tensor to the last repack kernel,
  * seconds the host spent copying mapped/pageable bytes into the pinned double buffer, and bytes sent over PCIe (a tensor-parallel
  * rank sends only its row ranges).  The pipeline: pinned double buffer filled by several host threads -> async H2D on a copy
- * stream -> double-buffered device staging -> repack kernel on the plan's stream; B200_UPLOAD_SYNC=1 selects blocking copies. */
+ * stream -> double-buffered device staging -> repack kernel on the plan's stream. */
 int b200_upload_info(b200_plan *plan, double *seconds, double *host_copy_seconds, int64_t *h2d_bytes);
 
 /* Number of kernels one decode step launches (bench.py's gpu_launches). */

@@ -22,12 +22,12 @@ def _entries(pattern):
     return out
 
 
-def test_batched_instantiations_do_not_spill():
-    """The three batched stream forms, the four batched norms, the argmax and the attention at head sizes 64 / 96 / 128 / 256 compile
+def test_batched_kernels_do_not_spill():
+    """The three batched stream forms, the two batched norms, the argmax and the attention at head sizes 64 / 96 / 128 / 256 compile
     without local-memory spills.  The head-32 attention is the exception: its single-row form (k_attention<32>) spills as well."""
     e = _entries(r"_batch")
     assert len([n for n in e if "k_stream_matvec_q8_batch" in n]) == 3
-    assert len([n for n in e if "k_rmsnorm_quant_batch" in n]) == 4
+    assert len([n for n in e if "k_rmsnorm_quant_batch" in n]) == 2
     assert len([n for n in e if "k_attention_batch" in n]) == 5
     assert len([n for n in e if "k_argmax_batch" in n]) == 1
     for name, (stack, st, ld) in e.items():

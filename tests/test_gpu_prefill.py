@@ -9,8 +9,7 @@ derived from its own arithmetic, elementwise, against a float64 evaluation of th
     bounds of g and u through silu (|silu'| <= 1.1), its own f32 arithmetic, and one f16 rounding.
   * attention (mma.sync, f16 Q / K / V / P, ex2.approx): against softmax attention on the kernel's rounded inputs, in
     log2 units; the bound sums the f16 output rounding, P rounded to f16 while l is not, the f32 score accumulation
-    (a relative error of p), ex2.approx, and the f32 sums of l and P V.  The FP32 SIMT kernel is held to the same terms
-    on unrounded inputs, without the f16 ones.
+    (a relative error of p), ex2.approx, and the f32 sums of l and P V.
   * every stage of the last layer of a real prefill chunk, against float64 evaluated from that stage's own inputs
     read back from the device, at the kernel bounds above.
 Every kernel test prints its worst error / bound ratio.  The model-level tests then bound what all of it adds up to:
@@ -190,16 +189,16 @@ def test_gemm_hook_rejections(pkg):
 
 # ---- causal attention over one chunk -------------------------------------------------------------------------------
 
-def _attention_ref(q, k, v, n_heads, n_kv, start, impl, equal_scores=False):
+def _attention_ref(q, k, v, n_heads, n_kv, start, equal_scores=False):
     """(float64 causal softmax attention, elementwise bound of the kernel's f16 output) for queries at start .. start+n-1.
 
-    impl "mma": the inputs rounded as k_pf_attention_mma rounds them -- qh = f16(f32(q) * f32(inv_sqrt_hs * log2e)),
-    kh = f16(k), vh = f16(v) -- and scores in log2 units.  "simt": the f32 inputs, q pre-scaled by inv_sqrt_hs in f32.
+    The inputs are rounded as k_pf_attention_mma rounds them -- qh = f16(f32(q) * f32(inv_sqrt_hs * log2e)),
+    kh = f16(k), vh = f16(v) -- and scores are in log2 units.
     The bound, with vmax = max |v| over the row's visible keys:
       2^-11 |ref| + 2^-25           the f16 output rounding (subnormal floor)
-      2^-10 vmax                     (mma) P rounded to f16 while l is summed unrounded
+      2^-10 vmax                     P rounded to f16 while l is summed unrounded
       2 (e^eps - 1) e^eps vmax       a relative error eps of every p: the f32 score accumulation, hs * 2^-23 * max sum|q||k|
-                                     (times ln 2 in log2 units), plus 2^-21 for ex2.approx / expf
+                                     (times ln 2 in log2 units), plus 2^-21 for ex2.approx
       (3 keys + 64) 2^-23 vmax       the f32 sums of l and of P V, the rescales, the final 1 / l, the f32 rounding of s - m.
     equal_scores: every visible score of a row is the same f32 value, so every p is 2^0 (within ex2's error) and f16(p) = 1:
     only the ex2 share of eps and the f32 sums remain."""
@@ -207,18 +206,13 @@ def _attention_ref(q, k, v, n_heads, n_kv, start, impl, equal_scores=False):
     hs = qd // n_heads
     kv_mul, nk = n_heads // n_kv, start + n
     inv = np.float32(1.0 / np.sqrt(hs))
-    if impl == "mma":
-        qh = (q * np.float32(inv * np.float32(LOG2E))).astype(np.float16).astype(np.float64)
-        kh, vh = k.astype(np.float16).astype(np.float64), v.astype(np.float16).astype(np.float64)
-        ln_base = np.log(2.0)
-    else:
-        qh = (q * inv).astype(np.float64)
-        kh, vh = k.astype(np.float64), v.astype(np.float64)
-        ln_base = 1.0
+    qh = (q * np.float32(inv * np.float32(LOG2E))).astype(np.float16).astype(np.float64)
+    kh, vh = k.astype(np.float16).astype(np.float64), v.astype(np.float16).astype(np.float64)
+    ln_base = np.log(2.0)
     pos = start + np.arange(n)
     visible = np.arange(nk)[None, :] <= pos[:, None]
     ref, bound = np.empty((n, qd)), np.empty((n, qd))
-    e_p16 = 2.0 ** -10 if impl == "mma" and not equal_scores else 0.0
+    e_p16 = 0.0 if equal_scores else 2.0 ** -10
     e_sums = (3 * (pos + 1) + 64) * 2.0 ** -23
     for g in range(n_kv):
         kg, vg = kh[:, g * hs:(g + 1) * hs], vh[:, g * hs:(g + 1) * hs]
@@ -281,15 +275,15 @@ def _check_attention(pkg, impl, q, k, v, n_heads, n_kv, start, kind, what):
     out = pkg.native.test_pf_attention(q, k, v, n_heads, n_kv, start, impl=impl, out_rows=n + 64, sentinel=ATT_SENTINEL)
     assert np.all(out[n:] == ATT_SENTINEL), f"{what}: a padding row past n was written"
     assert not np.any(out[:n] == ATT_SENTINEL), f"{what}: a (row < n, head) slot was not written"
-    ref, bound = _attention_ref(q, k, v, n_heads, n_kv, start, impl, equal_scores=kind == "equal")
+    ref, bound = _attention_ref(q, k, v, n_heads, n_kv, start, equal_scores=kind == "equal")
     return _assert_within(what, out[:n].view(np.float16), ref, bound)
 
 
-@pytest.mark.parametrize("impl", ["mma", "simt"])
+@pytest.mark.parametrize("impl", ["mma"])
 @pytest.mark.parametrize("kv_mul", [1, 2, 4, 8, 16, 64])
 def test_pf_attention_matches_float64(pkg, impl, kv_mul):
-    """k_pf_attention_mma (what the prefill runs) and the FP32 SIMT k_pf_attention, elementwise against float64 softmax
-    attention, at every GQA ratio prefill_init accepts (at 64 a query tile is one token), across key-tile boundaries."""
+    """k_pf_attention_mma (what the prefill runs), elementwise against float64 softmax attention, at every GQA ratio
+    prefill_init accepts (at 64 a query tile is one token), across key-tile boundaries."""
     n_kv = 2 if kv_mul <= 8 else 1
     n_heads = n_kv * kv_mul
     worst = 0.0
@@ -424,7 +418,7 @@ def _check_prefill_stages(pkg, m, first, second):
         kref, kbound = _k_cache_ref(m, qkv[:, qd:qd + kvd], start, L)
         r_k = _assert_within(f"{name} K cache = RoPE(k)", kc[start:], kref, kbound)
         # attention over the rotated q and the KV cache, as k_pf_attention_mma computes it
-        aref, abound = _attention_ref(qkv[:, :qd], kc, vc, c.n_heads, c.n_kv_heads, start, "mma")
+        aref, abound = _attention_ref(qkv[:, :qd], kc, vc, c.n_heads, c.n_kv_heads, start)
         r_a = _assert_within(f"{name} attention", att16, aref, abound)
         # gate/up + SwiGLU on the FFN input
         if c.arch == 2:

@@ -166,7 +166,7 @@ def test_qwen2_plan_without_a_bias_fails_and_names_it(pkg, make_model):
 ATT_STARTS = [0, 1, 63, 64, 65, 200]
 
 
-@pytest.mark.parametrize("impl", ["mma", "simt"])
+@pytest.mark.parametrize("impl", ["mma"])
 @pytest.mark.parametrize("kv_mul", [3, 5, 6, 7, 12])
 def test_pf_attention_any_gqa_ratio_matches_float64(pkg, impl, kv_mul):
     """QT = floor(64 / kv_mul) query tokens per CTA: rows QT * kv_mul .. 63 are padding.  n around QT and across tiles, several

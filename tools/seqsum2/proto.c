@@ -1,8 +1,8 @@
-/* proto.c -- CPU model of the round-2 RMSNorm accumulator ("seqsum v2"), checked against the literal loop.
+/* proto.c -- CPU model of the exact RMSNorm accumulator (csrc/seqsum2.cuh), checked against the literal loop.
  *
  * Goal: the bit-exact value of   s = 0; for (i) s = s + t[i];   (float32, round-to-nearest-even, t[i] >= 0)
  * -- InferenceCore.rmsnorm's accumulator (InferenceCore.java:39-48) -- with O(log n) parallel depth plus a
- * short serial walk, instead of the 16 us the round-1 kernel (csrc/seqsum.cuh) needs for n = 4096.
+ * short serial walk (csrc/seqsum2.cuh implements it).
  *
  * Model of the CUDA kernel (T threads, E consecutive terms per thread), every step written as the loop the
  * threads would execute in parallel:

@@ -11,6 +11,7 @@
 #include "decode_persistent.cuh"
 #include "sampler.cuh"
 #include "decode_batch.cuh"
+#include "moe.cuh"
 
 #include <math.h>
 #include <stdarg.h>
@@ -31,6 +32,10 @@ struct LayerW {
     TileMat tqkv{}, two{}, tgu{}, tw2{}; // tile-major copies for the streaming kernel (Q8_0)
     float *attn_norm = nullptr, *ffn_norm = nullptr, *q_norm = nullptr, *k_norm = nullptr;
     float *qkv_bias = nullptr; // Qwen2: this rank's q|k|v bias, laid out like the packed q|k|v vector
+    // Qwen2-MoE (moe.cuh): the shared expert's streams, the routed experts' geometry and the device tables of their stream bases
+    TileMat sgu{}, sdn{}, xgu{}, xdn{};
+    const unsigned char **gu_bases = nullptr, **dn_bases = nullptr;
+    float *router = nullptr, *shared_gate = nullptr; // F32 [n_experts][dim] and [dim]
 };
 
 } // namespace
@@ -113,6 +118,16 @@ struct b200_plan {
     int launches_decode = 0, launches_prefill = 0;
     float prefill_ms = 0.f; // device time of the last tensor-core prefill chunk
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+
+    // Qwen2-MoE: the routing buffers [layer][k] ids and [layer][k + 1] weights of the last step, the router logits scratch and
+    // arrival counters, the down projection's shared-memory layout
+    bool is_moe = false;
+    b200_moe_config moe{};
+    int moe_hv = 0; // units of the virtual hidden vector: shared_hidden_dim + n_experts_used * expert_hidden_dim
+    int *moe_ids = nullptr;
+    float *moe_w = nullptr, *moe_logits = nullptr;
+    unsigned *moe_done = nullptr;
+    MoeDownSmem moe_dl{};
 
     PrefillCtx prefill;
     // persistent decode kernel
@@ -572,6 +587,33 @@ bool gateup_fits(int hidden, int n_sms) { // epilogue buffer holds this CTA's hi
 // k_attention's dynamic shared memory: q | k | out | score row (the row lives in a global scratch buffer for long contexts).
 size_t att_smem_bytes(int head_size, int ctx, bool scratch) { return (size_t)(3 * head_size + (scratch ? 0 : ctx)) * 4; }
 
+// The FFN half of a Qwen2-MoE layer (moe.cuh): the FFN norm (float xb for the F32 router, xq/xs for the experts), the router,
+// the shared + routed gate/up stream and the down streams with the ordered combine.  Four launches, all under PDL; `tr` is the
+// norm's trace record, the three MoE kernels take the next three (trace ids 10, 11, 12).
+int enqueue_moe_ffn(b200_plan *p, int l, TraceBuf tr) {
+    const b200_config &c = p->cfg;
+    const LayerW &L = p->layers[l];
+    const int E = p->moe.n_experts, k = p->moe.n_experts_used;
+    int rc;
+    if ((rc = launch_k(p, p->use_pdl, k_rmsnorm_quant<false>, dim3(1), dim3(NORM_THREADS), norm_smem_bytes(c.dim), p->x, (const StepState *)p->st, p->emb,
+                       (const float *)L.ffn_norm, c.rms_norm_eps, c.dim, p->xq, p->xs, p->xb, (long long *)nullptr, tr, p->tp, -1)))
+        return rc;
+    int *ids = p->moe_ids + (size_t)l * k;
+    float *w = p->moe_w + (size_t)l * (k + 1);
+    MoeRouteArgs ra;
+    ra.router = L.router; ra.shared_gate = L.shared_gate; ra.xb = p->xb; ra.logits = p->moe_logits + (size_t)l * (E + 1); ra.done = p->moe_done + l;
+    ra.ids = ids; ra.weights = w; ra.dim = c.dim; ra.n_experts = E; ra.k = k; ra.tr = TraceBuf{tr.rec, tr.slot + 1, 10};
+    if ((rc = launch_k(p, p->use_pdl, k_moe_route, dim3(E + 1), dim3(MOE_ROUTE_THREADS), (size_t)c.dim * 4, ra))) return rc;
+    MoeStreamArgs a;
+    a.S = L.sgu; a.X = L.xgu; a.bases = L.gu_bases; a.ids = ids; a.weights = w; a.k = k;
+    a.xq = p->xq; a.xs = p->xs; a.out = p->hb; a.hq = p->hq; a.hs = p->hs; a.blk_cnt = p->blk_cnt; a.tr = TraceBuf{tr.rec, tr.slot + 2, 11};
+    const SmvSmem GL = smv_layout(c.dim, L.sgu.seg, SMV_SMEM_BUDGET_MAX);
+    if ((rc = launch_k(p, p->use_pdl, k_moe_gateup, dim3(p->n_sms), dim3(SMV_THREADS), GL.total, a, GL))) return rc;
+    a.S = L.sdn; a.X = L.xdn; a.bases = L.dn_bases;
+    a.xq = p->hq; a.xs = p->hs; a.out = p->x; a.hq = nullptr; a.hs = nullptr; a.blk_cnt = nullptr; a.tr = TraceBuf{tr.rec, tr.slot + 3, 12};
+    return launch_k(p, p->use_pdl, k_moe_down, dim3(p->n_sms), dim3(SMV_THREADS), p->moe_dl.total, a, p->moe_dl);
+}
+
 // Enqueue one single-token forward on p->stream (captured into a CUDA graph at creation).
 // with_logits=false is the prefill variant (InferenceCoreBatchPrefillDecode.java:166-167).
 int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = false) {
@@ -626,6 +668,11 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
         else if (sf) rc = launch_stream_f16<SF_RESID>(p, L.wo, nullptr, p->xb, p->x, TR(5));
         else rc = launch_matvec_f16<MODE_RESID>(p, L.wo, p->xb, p->x);
         if (rc) return rc; n++;
+        if (p->is_moe) {
+            if ((rc = enqueue_moe_ffn(p, l, TR(1)))) return rc;
+            n += 4;
+            continue;
+        }
         if ((rc = norm(false, L.ffn_norm, 4 * l + 1))) return rc;
         n++;
         if (st) {
@@ -676,6 +723,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
 int pd_prepare(b200_plan *p) {
     const b200_config &c = p->cfg;
     p->pd_ok = false;
+    if (p->is_moe) { p->pd_why = "the persistent decode kernel has no Qwen2-MoE layer (MoE plans decode through the CUDA graph)"; return B200_OK; }
     if (!p->use_stream) { p->pd_why = "the persistent decode kernel needs the Q8_0 streaming layout"; return B200_OK; }
     if (c.head_size != 64 && c.head_size != 128) { p->pd_why = "the persistent decode kernel supports head sizes 64 and 128"; return B200_OK; }
     if (p->nh_l > p->n_sms) { p->pd_why = "more attention heads than SMs"; return B200_OK; }
@@ -973,17 +1021,85 @@ int set_smem_attrs(b200_plan *p) {
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
+    CK(cudaFuncSetAttribute(k_moe_gateup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    CK(cudaFuncSetAttribute(k_moe_down, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     done = true;
     return B200_OK;
 }
 
 int prefill_init(b200_plan *p);
 
+// Qwen2-MoE FFN tensors of one layer (llama.cpp's names and shapes, dims[0] innermost): the F32 router and shared-expert gate, the
+// stacked routed experts [E][rows][cols] and the shared expert.  Every routed expert becomes a TileMat of its own, cut from its
+// row range of the stacked tensor (K-quant experts are re-quantised on the way like any matrix).
+int upload_moe_layer(b200_plan *p, const b200_tensor *tensors, int n_tensors, int l) {
+    const b200_config &c = p->cfg;
+    LayerW &L = p->layers[l];
+    const int E = p->moe.n_experts, He = p->moe.expert_hidden_dim, Hs = p->moe.shared_hidden_dim, D = c.dim;
+    struct Want { const char *name; int n_dims; int64_t d[3]; bool f32; };
+    const Want want[8] = {{"ffn_gate_inp.weight", 2, {D, E, 0}, true},     {"ffn_gate_inp_shexp.weight", 1, {D, 0, 0}, true},
+                          {"ffn_gate_exps.weight", 3, {D, He, E}, false},  {"ffn_up_exps.weight", 3, {D, He, E}, false},
+                          {"ffn_down_exps.weight", 3, {He, D, E}, false},  {"ffn_gate_shexp.weight", 2, {D, Hs, 0}, false},
+                          {"ffn_up_shexp.weight", 2, {D, Hs, 0}, false},   {"ffn_down_shexp.weight", 2, {Hs, D, 0}, false}};
+    const b200_tensor *t[8];
+    for (int i = 0; i < 8; i++) {
+        const std::string name = "blk." + std::to_string(l) + "." + want[i].name;
+        t[i] = find(tensors, n_tensors, name);
+        if (!t[i]) return fail(p, B200_ERR_BAD_ARG, "missing tensor %s", name.c_str());
+        if (want[i].f32 && t[i]->ggml_type != B200_GGML_F32)
+            return fail(p, B200_ERR_UNSUPPORTED, "tensor %s must be F32 (ggml type %d)", name.c_str(), t[i]->ggml_type);
+        // the shared-expert gate may also come as [dim, 1]
+        const int nd = (i == 1 && t[i]->n_dims == 2 && t[i]->dims[1] == 1) ? 1 : t[i]->n_dims;
+        bool ok = nd == want[i].n_dims && t[i]->data;
+        for (int k = 0; ok && k < nd; k++) ok = t[i]->dims[k] == want[i].d[k];
+        if (!ok)
+            return fail(p, B200_ERR_BAD_ARG, "tensor %s must have dims [%lld, %lld, %lld] (first %d used; got n_dims %d, dims [%lld, %lld, %lld])", name.c_str(),
+                        (long long)want[i].d[0], (long long)want[i].d[1], (long long)want[i].d[2], want[i].n_dims, t[i]->n_dims, (long long)t[i]->dims[0],
+                        (long long)(t[i]->n_dims > 1 ? t[i]->dims[1] : 0), (long long)(t[i]->n_dims > 2 ? t[i]->dims[2] : 0));
+    }
+    int rc;
+    if ((rc = dalloc(p, &L.router, (size_t)E * D * 4))) return rc;
+    CK(cudaMemcpy(L.router, t[0]->data, (size_t)E * D * 4, cudaMemcpyHostToDevice));
+    if ((rc = dalloc(p, &L.shared_gate, (size_t)D * 4))) return rc;
+    CK(cudaMemcpy(L.shared_gate, t[1]->data, (size_t)D * 4, cudaMemcpyHostToDevice));
+    if ((rc = upload_tiles(p, t[5], t[6], nullptr, Hs, Hs, 0, D, true, L.sgu))) return rc;
+    if ((rc = upload_tiles(p, t[7], nullptr, nullptr, D, 0, 0, Hs, false, L.sdn))) return rc;
+    std::vector<const unsigned char *> hg(E), hd(E);
+    for (int e = 0; e < E; e++) {
+        const int gr0[3] = {e * He, e * He, 0}, gfu[3] = {E * He, E * He, 0};
+        if ((rc = upload_tiles(p, t[2], t[3], nullptr, He, He, 0, D, true, L.xgu, gr0, gfu))) return rc;
+        const int dr0[3] = {e * D, 0, 0}, dfu[3] = {E * D, 0, 0};
+        if ((rc = upload_tiles(p, t[4], nullptr, nullptr, D, 0, 0, He, false, L.xdn, dr0, dfu))) return rc;
+        hg[e] = L.xgu.base;
+        hd[e] = L.xdn.base;
+    }
+    if ((rc = dalloc(p, &L.gu_bases, (size_t)E * sizeof(void *)))) return rc;
+    if ((rc = dalloc(p, &L.dn_bases, (size_t)E * sizeof(void *)))) return rc;
+    CK(cudaMemcpy(L.gu_bases, hg.data(), (size_t)E * sizeof(void *), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(L.dn_bases, hd.data(), (size_t)E * sizeof(void *), cudaMemcpyHostToDevice));
+    return B200_OK;
+}
+
 int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     const b200_config &c = p->cfg;
-    if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3 && c.arch != B200_ARCH_QWEN2)
+    if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3 && c.arch != B200_ARCH_QWEN2 && c.arch != B200_ARCH_QWEN2_MOE)
         return fail(p, B200_ERR_UNSUPPORTED, "unknown arch %d", c.arch);
-    p->kflags = c.arch == B200_ARCH_QWEN3 ? (KF_NEOX | KF_QKNORM) : c.arch == B200_ARCH_PHI3 ? KF_NEOX : c.arch == B200_ARCH_QWEN2 ? (KF_NEOX | KF_QKVBIAS) : 0;
+    p->kflags = c.arch == B200_ARCH_QWEN3 ? (KF_NEOX | KF_QKNORM) : c.arch == B200_ARCH_PHI3 ? KF_NEOX
+              : (c.arch == B200_ARCH_QWEN2 || c.arch == B200_ARCH_QWEN2_MOE) ? (KF_NEOX | KF_QKVBIAS) : 0;
+    if (p->is_moe) {
+        const b200_moe_config &m = p->moe;
+        if (c.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "Qwen2-MoE plans are single-GPU (tensor parallelism has no expert layout)");
+        if (m.n_experts < 1 || m.n_experts > MOE_MAX_EXPERTS) return fail(p, B200_ERR_BAD_ARG, "n_experts = %d: need 1..%d", m.n_experts, MOE_MAX_EXPERTS);
+        const int kmax = m.n_experts < MOE_MAX_K ? m.n_experts : MOE_MAX_K;
+        if (m.n_experts_used < 1 || m.n_experts_used > kmax)
+            return fail(p, B200_ERR_BAD_ARG, "n_experts_used = %d: need 1..%d (min(n_experts, %d))", m.n_experts_used, kmax, MOE_MAX_K);
+        if (m.expert_hidden_dim <= 0 || m.shared_hidden_dim <= 0 || m.expert_hidden_dim % 32 || m.shared_hidden_dim % 32)
+            return fail(p, B200_ERR_UNSUPPORTED, "expert hidden %d / shared hidden %d: the Q8_0 stream needs positive multiples of 32", m.expert_hidden_dim,
+                        m.shared_hidden_dim);
+        if (c.dim > 8192) // k_moe_route stages dim floats in (default-sized) dynamic shared memory, as the RMSNorm kernel caps dim
+            return fail(p, B200_ERR_UNSUPPORTED, "dim %d: the MoE router kernel supports dim <= 8192", c.dim);
+        p->moe_hv = m.shared_hidden_dim + m.n_experts_used * m.expert_hidden_dim;
+    }
     if (c.dim <= 0 || c.dim % 32 || c.hidden_dim % 32 || (c.head_size != 32 && c.head_size != 64 && c.head_size != 96 && c.head_size != 128 && c.head_size != 256) || c.n_heads % c.n_kv_heads ||
         c.n_layers <= 0 || c.vocab_size <= 0 || c.context_length <= 0)
         return fail(p, B200_ERR_BAD_ARG, "unsupported shape (dim/hidden must be multiples of 32, head_size one of 32/64/96/128/256)");
@@ -1011,6 +1127,8 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     p->wtype = eff_type(wq0->ggml_type); // K-quant matrices become Q8_0 while they are uploaded (kquant.cuh)
     if (p->wtype != B200_GGML_Q8_0 && p->wtype != B200_GGML_F16)
         return fail(p, B200_ERR_UNSUPPORTED, "Type: %d currently not supported by this engine (Q8_0, F16 and the K-quants Q4_K/Q5_K/Q6_K only)", wq0->ggml_type);
+    if (p->is_moe && p->wtype != B200_GGML_Q8_0)
+        return fail(p, B200_ERR_UNSUPPORTED, "Qwen2-MoE runs in Q8_0 only (FP16 MoE plans are not supported, as in the reference)");
     bool any_kq = false;
     for (int i = 0; i < n_tensors; i++) any_kq = any_kq || kq_is_kquant(tensors[i].ggml_type);
 
@@ -1025,12 +1143,22 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         const char *e = getenv("B200_STREAM");
         bool want = !(e && e[0] == '0');
         p->use_stream = want && p->wtype == B200_GGML_Q8_0 && stream_shape_ok(p->qd_l + 2 * p->kvd_l, c.dim) && stream_shape_ok(p->dim_l, p->qd) &&
-                        stream_shape_ok(2 * p->hid_l, c.dim) && stream_shape_ok(p->dim_l, c.hidden_dim) && stream_shape_ok(p->voc_l, c.dim) &&
+                        (p->is_moe || (stream_shape_ok(2 * p->hid_l, c.dim) && stream_shape_ok(p->dim_l, c.hidden_dim))) && stream_shape_ok(p->voc_l, c.dim) &&
                         gateup_fits(p->hid_l, p->n_sms);
         const char *e3 = getenv("B200_F16_STREAM"); // FP16 plans: 0 = the round-1 k_matvec_f16 launches
         p->use_f16_stream = !(e3 && e3[0] == '0') && p->wtype == B200_GGML_F16 && c.tp_size == 1 && sf_layout(p->qd + 2 * p->kvd, c.dim, c.fp16_lanes, false).ok &&
                             sf_layout(c.dim, p->qd, c.fp16_lanes, false).ok && sf_layout(c.hidden_dim, c.dim, c.fp16_lanes, true).ok &&
                             sf_layout(c.dim, c.hidden_dim, c.fp16_lanes, false).ok && sf_layout(c.vocab_size, c.dim, c.fp16_lanes, false).ok;
+        if (p->is_moe) { // the MoE FFN has its own streams (the dense FFN checks above are skipped)
+            const b200_moe_config &m = p->moe;
+            const int hs = m.shared_hidden_dim, he = m.expert_hidden_dim;
+            const bool cut = stream_shape_ok(2 * hs, c.dim) && stream_shape_ok(c.dim, hs) && stream_shape_ok(2 * he, c.dim) && stream_shape_ok(c.dim, he) &&
+                             gateup_fits(p->moe_hv, p->n_sms);
+            if (!cut) return fail(p, B200_ERR_UNSUPPORTED, "expert hidden %d / shared hidden %d at dim %d: the Q8_0 stream layout cannot cut these matrices", he, hs, c.dim);
+            p->moe_dl = moe_down_layout(p->moe_hv, hs / smv_pick_nseg(hs), he / smv_pick_nseg(he), SMV_SMEM_BUDGET_MAX);
+            if (p->moe_dl.stages < 3) return fail(p, B200_ERR_UNSUPPORTED, "the expert down projection leaves fewer than 3 ring stages of shared memory");
+            if (!p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "Qwen2-MoE needs the Q8_0 streaming layout (this plan would use the non-streaming matvecs)");
+        }
         p->use_pdl = p->use_stream || p->use_f16_stream;
         if (c.tp_size > 1 && !p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "tensor parallelism needs the Q8_0 streaming path");
     }
@@ -1039,6 +1167,8 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         size_t m1 = (size_t)c.vocab_size * c.dim, m2 = (size_t)2 * c.hidden_dim * c.dim, m3 = (size_t)(p->qd + 2 * p->kvd) * c.dim;
         size_t mx = m1 > m2 ? m1 : m2;
         if (m3 > mx) mx = m3;
+        const size_t m4 = (size_t)2 * p->moe.shared_hidden_dim * c.dim;
+        if (m4 > mx) mx = m4;
         size_t need = mx / 32 * 34 + 4096;
         if (need > stage_bytes) stage_bytes = need;
     }
@@ -1064,8 +1194,9 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         p->out = p->emb;
         if ((rc = dalloc(p, &p->part_val, (size_t)p->n_sms * 4))) return rc;
         if ((rc = dalloc(p, &p->part_idx, (size_t)p->n_sms * 4))) return rc;
-        if ((rc = dalloc(p, &p->blk_cnt, (size_t)(c.hidden_dim / 32) * 4))) return rc;
-        CK(cudaMemset(p->blk_cnt, 0, (size_t)(c.hidden_dim / 32) * 4));
+        const int hid = c.hidden_dim > p->moe_hv ? c.hidden_dim : p->moe_hv;
+        if ((rc = dalloc(p, &p->blk_cnt, (size_t)(hid / 32) * 4))) return rc;
+        CK(cudaMemset(p->blk_cnt, 0, (size_t)(hid / 32) * 4));
     } else if (outw) {
         if (p->use_f16_stream) { // per-CTA argmax partials of the classifier launch (at most 3 CTAs per SM)
             if ((rc = dalloc(p, &p->part_val, (size_t)p->n_sms * 4 * 4))) return rc;
@@ -1094,7 +1225,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
             if ((rc = upload_f32(p, T("attn_q_norm.weight"), c.head_size, &L.q_norm, "attn_q_norm.weight"))) return rc;
             if ((rc = upload_f32(p, T("attn_k_norm.weight"), c.head_size, &L.k_norm, "attn_k_norm.weight"))) return rc;
         }
-        if (c.arch == B200_ARCH_QWEN2 && (rc = upload_qkv_bias(p, tensors, n_tensors, l, &L.qkv_bias))) return rc;
+        if ((c.arch == B200_ARCH_QWEN2 || c.arch == B200_ARCH_QWEN2_MOE) && (rc = upload_qkv_bias(p, tensors, n_tensors, l, &L.qkv_bias))) return rc;
         // Phi-3 stores wqkv and gate|up fused (Phi3StandardWeights: attn_qkv.weight = [q; k; v] rows, ffn_up.weight = [gate; up] rows,
         // InferenceCore.java:718-724,779-781): the row ranges below address the same source tensor; rows are independent dot products, so
         // splitting a fused matrix by rows changes nothing in the arithmetic.
@@ -1109,6 +1240,10 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
             if ((rc = upload_tiles(p, tq, tk, tv, p->qd_l, p->kvd_l, p->kvd_l, c.dim, false, L.tqkv, qr0, qfu))) return rc;
             const int dr0[3] = {rk * p->dim_l, 0, 0}, dfu[3] = {c.dim, 0, 0};
             if ((rc = upload_tiles(p, T("attn_output.weight"), nullptr, nullptr, p->dim_l, 0, 0, p->qd, false, L.two, dr0, dfu))) return rc;
+            if (p->is_moe) {
+                if ((rc = upload_moe_layer(p, tensors, n_tensors, l))) return rc;
+                continue;
+            }
             const int gr0[3] = {rk * p->hid_l, u_src + rk * p->hid_l, 0}, gfu[3] = {g_full, g_full, 0};
             if ((rc = upload_tiles(p, tg, tu, nullptr, p->hid_l, p->hid_l, 0, c.dim, true, L.tgu, gr0, gfu))) return rc;
             if ((rc = upload_tiles(p, T("ffn_down.weight"), nullptr, nullptr, p->dim_l, 0, 0, c.hidden_dim, false, L.tw2, dr0, dfu))) return rc;
@@ -1183,7 +1318,8 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     } else if ((rc = dalloc(p, &p->x, (size_t)c.dim * 4))) return rc;
     if ((rc = dalloc(p, &p->xb, (size_t)big * 4))) return rc;
     if ((rc = dalloc(p, &p->qkv, (size_t)(p->qd_l + 2 * p->kvd_l) * 4))) return rc;
-    if ((rc = dalloc(p, &p->hb, (size_t)c.hidden_dim * 4))) return rc;
+    const int hid_alloc = c.hidden_dim > p->moe_hv ? c.hidden_dim : p->moe_hv; // MoE: the virtual hidden vector (moe.cuh)
+    if ((rc = dalloc(p, &p->hb, (size_t)hid_alloc * 4))) return rc;
     if ((rc = dalloc(p, &p->hb2, (size_t)c.hidden_dim * 4))) return rc;
     if ((rc = dalloc(p, &p->logits, (size_t)sampler_padded(c.vocab_size) * 4))) return rc; // zero pad: the sampler's exact sum runs over whole thread chunks
     if ((rc = dalloc(p, &p->xq, (size_t)big))) return rc;
@@ -1194,8 +1330,8 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         p->attq = reinterpret_cast<int8_t *>(p->comm + p->tp.off_attq);
         p->atts = reinterpret_cast<float *>(p->comm + p->tp.off_atts);
     } else {
-        if ((rc = dalloc(p, &p->hq, (size_t)c.hidden_dim))) return rc;
-        if ((rc = dalloc(p, &p->hs, (size_t)(c.hidden_dim / 32) * 4))) return rc;
+        if ((rc = dalloc(p, &p->hq, (size_t)hid_alloc))) return rc;
+        if ((rc = dalloc(p, &p->hs, (size_t)(hid_alloc / 32) * 4))) return rc;
         p->attq = p->xq; // the attention output is the activation of the Wo matvec
         p->atts = p->xs;
     }
@@ -1215,6 +1351,16 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     CK(cudaMemset(p->seq_tokens, 0, (size_t)p->seq_cap * 4));
     CK(cudaMallocHost(&p->h_st, sizeof(StepState)));
     CK(cudaMallocHost(&p->h_ids, (size_t)p->seq_cap * 4));
+    if (p->is_moe) {
+        const int E = p->moe.n_experts, k = p->moe.n_experts_used;
+        if ((rc = dalloc(p, &p->moe_ids, (size_t)c.n_layers * k * 4))) return rc;
+        if ((rc = dalloc(p, &p->moe_w, (size_t)c.n_layers * (k + 1) * 4))) return rc;
+        if ((rc = dalloc(p, &p->moe_logits, (size_t)c.n_layers * (E + 1) * 4))) return rc;
+        if ((rc = dalloc(p, &p->moe_done, (size_t)c.n_layers * 4))) return rc;
+        CK(cudaMemset(p->moe_ids, 0, (size_t)c.n_layers * k * 4));
+        CK(cudaMemset(p->moe_w, 0, (size_t)c.n_layers * (k + 1) * 4));
+        CK(cudaMemset(p->moe_done, 0, (size_t)c.n_layers * 4));
+    }
 
     // epoch counters of the persistent kernel + the error word every bounded device-side wait reports through
     if ((rc = dalloc(p, &p->pd_sync, PD_S_WORDS * 4))) return rc;
@@ -1237,10 +1383,12 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
 }
 
 // ---- batched prefill on the tensor cores (prefill.cuh) -------------------------------------------
+static const char *const MOE_PREFILL_WHY = "Qwen2-MoE plans have no tensor-core prefill: prompts go through the exact token-by-token prefill";
 // What both tensor-core modes need of the plan's shape; nullptr when the chunk GEMMs and the attention can run it.
 static const char *prefill_shape_why(const b200_plan *p) {
     const b200_config &g = p->cfg;
     const int kv_mul = g.n_heads / g.n_kv_heads, nqkv = p->qd + 2 * p->kvd;
+    if (p->is_moe) return MOE_PREFILL_WHY;
     if (g.tp_size > 1) return "tensor-core prefill is single-GPU";
     if (g.head_size != 64 && g.head_size != 128) return "tensor-core prefill supports head sizes 64 and 128";
     if (g.n_heads % g.n_kv_heads || kv_mul > 64) return "tensor-core prefill needs n_heads % n_kv_heads == 0 and a GQA ratio <= 64";
@@ -1473,17 +1621,23 @@ int check_pos(b200_plan *p, int token, int pos) {
 
 } // namespace
 
-extern "C" {
-
-int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
-                     int32_t device, b200_plan **out, char *err, size_t err_len) {
+// b200_plan_create and b200_plan_create_moe (moe == nullptr: a dense plan)
+static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
+                       int32_t device, b200_plan **out, char *err, size_t err_len) {
     if (out) *out = nullptr;
     if (!cfg || !tensors || !out || n_tensors <= 0) {
         if (err && err_len) snprintf(err, err_len, "null argument");
         return B200_ERR_BAD_ARG;
     }
+    if ((cfg->arch == B200_ARCH_QWEN2_MOE) != (moe != nullptr)) {
+        if (err && err_len)
+            snprintf(err, err_len, moe ? "b200_plan_create_moe needs arch B200_ARCH_QWEN2_MOE (got %d)"
+                                       : "arch %d (B200_ARCH_QWEN2_MOE) needs its expert configuration: create the plan with b200_plan_create_moe", cfg->arch);
+        return B200_ERR_BAD_ARG;
+    }
     b200_plan *p = new b200_plan();
     p->cfg = *cfg;
+    if (moe) { p->is_moe = true; p->moe = *moe; }
     if (p->cfg.tp_size <= 0) p->cfg.tp_size = 1;
     p->device = device;
     p->prefill_batch = prefill_batch_size;
@@ -1495,6 +1649,23 @@ int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t
     }
     *out = p;
     return B200_OK;
+}
+
+extern "C" {
+
+int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
+                     int32_t device, b200_plan **out, char *err, size_t err_len) {
+    return plan_create(cfg, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
+}
+
+int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
+                         int32_t device, b200_plan **out, char *err, size_t err_len) {
+    if (!moe) {
+        if (out) *out = nullptr;
+        if (err && err_len) snprintf(err, err_len, "null argument");
+        return B200_ERR_BAD_ARG;
+    }
+    return plan_create(cfg, moe, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
 }
 
 int b200_forward_decode(b200_plan *p, int32_t token, int32_t position, float *logits, int32_t *argmax) {
@@ -1653,6 +1824,7 @@ int b200_trace_persistent(b200_plan *p, int32_t token, int32_t position, uint64_
 
 int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
     if (!p || (mode != B200_PREFILL_EXACT && mode != B200_PREFILL_TENSOR_CORE && mode != B200_PREFILL_TENSOR_CORE_W8A16)) return B200_ERR_BAD_ARG;
+    if (p->is_moe && mode != B200_PREFILL_EXACT) return fail(p, B200_ERR_UNSUPPORTED, "%s", MOE_PREFILL_WHY);
     if (mode == B200_PREFILL_TENSOR_CORE_W8A16) {
         if (!p->prefill.q8_ready) {
             CK(cudaSetDevice(p->device));
@@ -1698,6 +1870,7 @@ int b200_set_decode_slots(b200_plan *p, int32_t n_slots) {
     CK(cudaSetDevice(p->device));
     CK(cudaStreamSynchronize(p->stream));
     if (n_slots == 0) { batch_free(p); return B200_OK; }
+    if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "batched decode has no Qwen2-MoE layer (MoE plans decode one sequence per step)");
     if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "batched decode runs on single-GPU plans only (this plan is tensor-parallel)");
     if (p->wtype != B200_GGML_Q8_0) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs Q8_0 weights (FP16 plans decode one sequence per step)");
     if (!p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs the Q8_0 streaming layout (this plan uses the non-streaming matvecs)");
@@ -1814,12 +1987,18 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
     if (s == "x") { src = p->x; sz = (size_t)c.dim * 4; }
     else if (s == "xb") { src = p->xb; sz = (size_t)(c.dim > p->qd ? c.dim : p->qd) * 4; }
     else if (s == "q" || s == "qkv") { src = p->qkv; sz = (size_t)(p->qd_l + 2 * p->kvd_l) * 4; }
-    else if (s == "hb") { src = p->hb; sz = (size_t)c.hidden_dim * 4; }
+    else if (s == "hb") { src = p->hb; sz = (size_t)(c.hidden_dim > p->moe_hv ? c.hidden_dim : p->moe_hv) * 4; }
     else if (s == "logits") { src = p->logits; sz = (size_t)c.vocab_size * 4; }
     else if (s == "xq") { src = p->xq; sz = (size_t)(c.dim > p->qd ? c.dim : p->qd); }
     else if (s == "xs") { src = p->xs; sz = (size_t)((c.dim > p->qd ? c.dim : p->qd) / 32) * 4; }
-    else if (s == "hq") { src = p->hq; sz = (size_t)c.hidden_dim; }
-    else if (s == "hs") { src = p->hs; sz = (size_t)(c.hidden_dim / 32) * 4; }
+    else if (s == "hq") { src = p->hq; sz = (size_t)(c.hidden_dim > p->moe_hv ? c.hidden_dim : p->moe_hv); }
+    else if (s == "hs") { src = p->hs; sz = (size_t)((c.hidden_dim > p->moe_hv ? c.hidden_dim : p->moe_hv) / 32) * 4; }
+    else if (s == "moe_ids" || s == "moe_weights") {
+        if (!p->is_moe) return fail(p, B200_ERR_BAD_ARG, "%s: not a Qwen2-MoE plan", name);
+        const size_t k = (size_t)p->moe.n_experts_used;
+        if (s == "moe_ids") { src = p->moe_ids; sz = (size_t)c.n_layers * k * 4; }
+        else { src = p->moe_w; sz = (size_t)c.n_layers * (k + 1) * 4; }
+    }
     else if (s == "key_cache" || s == "value_cache") {
         if (layer < 0 || layer >= c.n_layers) return fail(p, B200_ERR_BAD_ARG, "layer out of range");
         src = (s == "key_cache" ? p->key_cache : p->value_cache) + (size_t)layer * ctx_kv;
@@ -1849,6 +2028,7 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
 int b200_time_kernel(b200_plan *p, int32_t which, int32_t reps, float *avg_ms, int64_t *algorithmic_bytes) {
     if (!p || !avg_ms || reps <= 0) return B200_ERR_BAD_ARG;
     if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "b200_time_kernel is single-GPU only");
+    if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "b200_time_kernel times the dense FFN and attention matrices; a Qwen2-MoE plan has no dense FFN");
     const b200_config &c = p->cfg;
     const bool q8 = p->wtype == B200_GGML_Q8_0;
     CK(cudaSetDevice(p->device));

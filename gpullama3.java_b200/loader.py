@@ -17,6 +17,7 @@ ARCH_LLAMA = 0
 ARCH_QWEN3 = 1
 ARCH_PHI3 = 2
 ARCH_QWEN2 = 3  # Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen: Llama's forward + q/k/v biases, NeoX RoPE (InferenceCore.java:434-563)
+ARCH_QWEN2_MOE = 4  # Qwen1.5-MoE: Qwen2's attention + a routed mixture-of-experts FFN with a shared expert (InferenceCore.java:263-432)
 
 
 @dataclass
@@ -33,6 +34,11 @@ class Configuration:
     context_length: int
     rms_norm_eps: float
     rope_theta: float
+    # Qwen2-MoE only (Qwen2MoEConfiguration); 0 for every dense model
+    n_experts: int = 0
+    n_experts_used: int = 0
+    expert_hidden_dim: int = 0
+    shared_hidden_dim: int = 0
 
     @property
     def q_dim(self):
@@ -48,6 +54,8 @@ class UnsupportedModel(Exception):
 
 
 def detect_model_type(metadata: dict) -> str:
+    if metadata.get("general.architecture") == "qwen2moe":  # checked before the name (ModelLoader.java:50)
+        return "QWEN_2_MOE"
     name = metadata.get("general.name")
     if name is not None:
         low = name.lower()
@@ -89,11 +97,16 @@ class Model:
 
 def model_from_tensors(shape, quant: int, tensors: dict, context_length: int) -> Model:
     """In-memory model (bench: synthetic weights never touch the disk)."""
-    arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3, "qwen2": ARCH_QWEN2}[shape.arch]
+    arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3, "qwen2": ARCH_QWEN2, "qwen2moe": ARCH_QWEN2_MOE}[shape.arch]
+    moe = shape.arch == "qwen2moe"
     cfg = Configuration(arch, "Q8_0" if quant == GGMLType.Q8_0 else "FP16",
-                        shape.dim, shape.hidden, shape.n_layers, shape.n_heads, shape.n_kv_heads, shape.head_size,
+                        shape.dim, 0 if moe else shape.hidden, shape.n_layers, shape.n_heads, shape.n_kv_heads, shape.head_size,
                         shape.vocab, context_length, float(shape.eps), float(shape.rope_theta))
-    return Model(None, cfg, {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3", "qwen2": "QWEN_2"}[shape.arch], tensors)
+    if moe:
+        cfg.n_experts, cfg.n_experts_used = shape.n_experts, shape.n_experts_used
+        cfg.expert_hidden_dim, cfg.shared_hidden_dim = shape.expert_hidden, shape.hidden
+    typ = {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3", "qwen2": "QWEN_2", "qwen2moe": "QWEN_2_MOE"}[shape.arch]
+    return Model(None, cfg, typ, tensors)
 
 
 def load_model(path: str, context_length: int = -1) -> Model:
@@ -157,9 +170,35 @@ def load_model(path: str, context_length: int = -1) -> Model:
             ARCH_QWEN2, q, dim, int(md["qwen2.feed_forward_length"]), int(md["qwen2.block_count"]), n_heads,
             int(md.get("qwen2.attention.head_count_kv", n_heads)), dim // n_heads, len(md["tokenizer.ggml.tokens"]), ctx,
             float(md["qwen2.attention.layer_norm_rms_epsilon"]), float(md["qwen2.rope.freq_base"]))
+    elif typ == "QWEN_2_MOE":
+        cfg = _qwen2moe_configuration(md, g, q, context_length)
     else:
-        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 forward passes only)")
+        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 / Qwen2-MoE forward passes only)")
     return Model(g, cfg, typ)
+
+
+def _qwen2moe_configuration(md: dict, g: GGUFFile, q: str, context_length: int) -> Configuration:
+    """Qwen2MoEModelLoader.createConfiguration: qwen2moe.* keys, head_count_kv required, the vocabulary size is the token list's, the
+    context is clamped to the model's, hidden_dim is 0, the expert hidden size comes from ffn_down_exps dims[0].  The shared expert's
+    hidden size is taken from the ffn_gate_shexp tensor; where it differs from feed_forward_length (which the reference uses) the
+    reference would read the shared expert with the wrong row count, so such a file is refused.  FP16 files load (as in the reference);
+    the plan refuses them."""
+    model_ctx = int(md["qwen2moe.context_length"])
+    ctx = model_ctx if (context_length < 0 or model_ctx < context_length) else context_length
+    n_heads = int(md["qwen2moe.attention.head_count"])
+    dim = int(md["qwen2moe.embedding_length"])
+    ti = g.tensor_infos
+    expert_hidden = int(ti["blk.0.ffn_down_exps.weight"].dims[0])
+    shared_hidden = int(ti["blk.0.ffn_gate_shexp.weight"].dims[1])
+    ffl = int(md["qwen2moe.feed_forward_length"])
+    if shared_hidden != ffl:
+        raise UnsupportedModel(f"qwen2moe.feed_forward_length is {ffl} but the shared expert (blk.0.ffn_gate_shexp.weight) has {shared_hidden} rows: "
+                               "the reference sizes the shared expert by feed_forward_length and would read the wrong bytes")
+    return Configuration(
+        ARCH_QWEN2_MOE, q, dim, 0, int(md["qwen2moe.block_count"]), n_heads, int(md["qwen2moe.attention.head_count_kv"]), dim // n_heads,
+        len(md["tokenizer.ggml.tokens"]), ctx, float(md["qwen2moe.attention.layer_norm_rms_epsilon"]), float(md["qwen2moe.rope.freq_base"]),
+        n_experts=int(md["qwen2moe.expert_count"]), n_experts_used=int(md["qwen2moe.expert_used_count"]),
+        expert_hidden_dim=expert_hidden, shared_hidden_dim=shared_hidden)
 
 
 def tensor_as_f32(model: Model, name: str) -> np.ndarray:

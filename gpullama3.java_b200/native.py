@@ -34,12 +34,17 @@ class Config(C.Structure):
                 ("tp_rank", C.c_int32), ("tp_size", C.c_int32)]
 
 
+class MoeConfig(C.Structure):
+    """b200_moe_config: the expert configuration of a B200_ARCH_QWEN2_MOE plan."""
+    _fields_ = [(n, C.c_int32) for n in ("n_experts", "n_experts_used", "expert_hidden_dim", "shared_hidden_dim")]
+
+
 class Tensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("ggml_type", C.c_int32), ("n_dims", C.c_int32),
                 ("dims", C.c_int64 * 4)]
 
 
-EXPORTS = ["b200_plan_create", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
+EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_batch_info",
@@ -58,6 +63,7 @@ def lib() -> C.CDLL:
     L = C.CDLL(LIB_PATH)
     vp, i32 = C.c_void_p, C.c_int32
     L.b200_plan_create.argtypes = [C.POINTER(Config), C.POINTER(Tensor), i32, i32, i32, C.POINTER(vp), C.c_char_p, C.c_size_t]
+    L.b200_plan_create_moe.argtypes = [C.POINTER(Config), C.POINTER(MoeConfig), C.POINTER(Tensor), i32, i32, i32, C.POINTER(vp), C.c_char_p, C.c_size_t]
     L.b200_forward_decode.argtypes = [vp, i32, i32, vp, C.POINTER(i32)]
     L.b200_forward_prefill.argtypes = [vp, i32, i32]
     L.b200_forward_decode_sample.argtypes = [vp, i32, i32, C.c_float, C.c_float, C.c_float, C.POINTER(i32), C.POINTER(i32)]
@@ -234,7 +240,7 @@ GGML_SIZES = {0: (4, 1), 1: (2, 1), 8: (34, 32), 12: (144, 256), 13: (176, 256),
 class NativePlan:
     """Owns one ``b200_plan*``."""
 
-    def __init__(self, cfg: Config, tensors: dict, prefill_batch_size: int = 0, device: int = 0):
+    def __init__(self, cfg: Config, tensors: dict, prefill_batch_size: int = 0, device: int = 0, moe: MoeConfig | None = None):
         L = lib()
         arr = (Tensor * len(tensors))()
         self._keep = []
@@ -254,12 +260,16 @@ class NativePlan:
                 arr[i].dims[k] = int(d)
         out = C.c_void_p()
         err = C.create_string_buffer(512)
-        rc = L.b200_plan_create(C.byref(cfg), arr, len(tensors), prefill_batch_size, device, C.byref(out), err, 512)
+        if moe is not None:
+            rc = L.b200_plan_create_moe(C.byref(cfg), C.byref(moe), arr, len(tensors), prefill_batch_size, device, C.byref(out), err, 512)
+        else:
+            rc = L.b200_plan_create(C.byref(cfg), arr, len(tensors), prefill_batch_size, device, C.byref(out), err, 512)
         self._keep = None  # the library never touches the host pointers again
         if rc != B200_OK:
             _raise(rc, err.value.decode())
         self._p = out
         self.cfg = cfg
+        self.moe = moe
 
     def _ck(self, rc: int):
         if rc != B200_OK:
@@ -385,6 +395,14 @@ class NativePlan:
         out = np.empty(n, dtype=dtype)
         self._ck(lib().b200_read_buffer(self._p, name.encode(), layer, out.ctypes.data, out.nbytes))
         return out
+
+    def moe_routing(self):
+        """(ids int32 [layer, k], weights float32 [layer, k + 1]) of the last step: the selected experts in selection order, their
+        routing weights, then the shared-expert weight."""
+        k = self.moe.n_experts_used
+        ids = self.read_buffer("moe_ids", self.cfg.n_layers * k, np.int32).reshape(self.cfg.n_layers, k)
+        w = self.read_buffer("moe_weights", self.cfg.n_layers * (k + 1)).reshape(self.cfg.n_layers, k + 1)
+        return ids, w
 
     def upload_info(self) -> dict:
         a, b, c = C.c_double(0), C.c_double(0), C.c_int64(0)

@@ -81,7 +81,11 @@ class B200MasterPlan:
         cfg.tp_rank, cfg.tp_size = tp_rank, tp_size
         if tp_size > 1:
             tp_shard_plan(model.configuration, tp_size)  # raises early on shapes that do not split
-        self._native = native.NativePlan(cfg, model.tensors, self.prefill_batch_size, device)
+        c = model.configuration
+        moe = None
+        if c.n_experts:  # Qwen2-MoE: b200_plan_create_moe
+            moe = native.MoeConfig(c.n_experts, c.n_experts_used, c.expert_hidden_dim, c.shared_hidden_dim)
+        self._native = native.NativePlan(cfg, model.tensors, self.prefill_batch_size, device, moe=moe)
         self.tp_rank, self.tp_size = tp_rank, tp_size
         if tp_size > 1:
             # one process per GPU: swap IPC handles of the communication buffers, then wire the peers
@@ -173,6 +177,11 @@ class B200MasterPlan:
     def batch_info(self):
         """(decode slots, kernels of the last batched step, its device milliseconds)."""
         return self._native.batch_info()
+
+    def moe_routing(self):
+        """Qwen2-MoE plans: (ids [layer, k], weights [layer, k + 1]) of the last step (selected experts in selection order, their
+        routing weights, then the shared-expert weight)."""
+        return self._native.moe_routing()
 
     def kv_reset(self):
         self._native.kv_reset()

@@ -3,7 +3,9 @@ offline; SURVEY.md section 8d).  Tensor names/types are exactly what the referen
 expect (``model/loader/LlamaModelLoader.java:78-99``, ``Qwen3ModelLoader.java:98-124``):
 norm weights F32, matrices and the embedding table in the model quantisation, metadata keys
 per ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74`` / ``Qwen2ModelLoader.java:48-73``.  Qwen2 files
-add F32 biases ``blk.N.attn_{q,k,v}.bias`` (``Qwen2ModelLoader.java:100-102``).
+add F32 biases ``blk.N.attn_{q,k,v}.bias`` (``Qwen2ModelLoader.java:100-102``).  Qwen2-MoE files (``qwen2moe``) replace the dense FFN by
+an F32 router ``ffn_gate_inp``, an F32 shared-expert gate ``ffn_gate_inp_shexp``, stacked 3-D expert tensors ``ffn_{gate,up,down}_exps``
+and the shared expert ``ffn_{gate,up,down}_shexp``, as llama.cpp writes them (``Qwen2MoEModelLoader.java``).
 """
 from __future__ import annotations
 
@@ -16,9 +18,9 @@ from .gguf import GGMLType, write_gguf
 
 @dataclass(frozen=True)
 class Shape:
-    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2"
+    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2" | "qwen2moe"
     dim: int
-    hidden: int
+    hidden: int  # qwen2moe: the shared expert's hidden size
     n_layers: int
     n_heads: int
     n_kv_heads: int
@@ -28,6 +30,9 @@ class Shape:
     rope_theta: float
     eps: float
     model_ctx: int = 8192
+    n_experts: int = 0        # qwen2moe: expert_count
+    n_experts_used: int = 0   # expert_used_count
+    expert_hidden: int = 0    # the routed experts' hidden size (ffn_down_exps dims[0])
 
     @property
     def q_dim(self):
@@ -40,6 +45,7 @@ class Shape:
     def matmul_elements(self) -> int:
         """Weight elements streamed per decoded token (SURVEY.md 8d)."""
         per_layer = 2 * self.q_dim * self.dim + 2 * self.kv_dim * self.dim + 3 * self.hidden * self.dim
+        per_layer += 3 * self.n_experts_used * self.expert_hidden * self.dim  # qwen2moe: the k routed experts (active weights only)
         return self.n_layers * per_layer + self.vocab * self.dim
 
     def matmul_elements_no_head(self) -> int:
@@ -88,6 +94,12 @@ SHAPES = {
     "llama-3-70b": Shape("llama", 8192, 28672, 80, 64, 8, 128, 128256, False, 500000.0, 1e-5),
     # Qwen2.5-7B (tools/qwen2_bench.py)
     "qwen2.5-7b": Shape("qwen2", 3584, 18944, 28, 28, 4, 128, 152064, False, 1000000.0, 1e-6, 32768),
+    # Qwen2-MoE: multi-head with 8 experts, top-2; GQA with 16 experts, top-8 (the k cap); the real Qwen1.5-MoE-A2.7B layer geometry
+    # (60 experts, top-4, expert hidden 1408, shared hidden 5632) cut to 2 layers, and the whole model (tools/moe_bench.py)
+    "tiny-qwen2moe": Shape("qwen2moe", 256, 512, 2, 4, 4, 64, 512, False, 1000000.0, 1e-6, 8192, 8, 2, 256),
+    "tiny-qwen2moe-gqa": Shape("qwen2moe", 512, 512, 2, 8, 2, 64, 512, True, 1000000.0, 1e-6, 8192, 16, 8, 256),
+    "mid-qwen1.5-moe-a2.7b": Shape("qwen2moe", 2048, 5632, 2, 16, 16, 128, 8192, False, 1000000.0, 1e-6, 8192, 60, 4, 1408),
+    "qwen1.5-moe-a2.7b": Shape("qwen2moe", 2048, 5632, 24, 16, 16, 128, 151936, False, 1000000.0, 1e-6, 8192, 60, 4, 1408),
 }
 
 
@@ -144,7 +156,7 @@ def gpt2_byte_symbols() -> list[str]:
 def build_vocab(vocab_size: int, arch: str = "llama", seed: int = 1234):
     """(tokens, merge_lines, token_types, base_tokens): 256 byte symbols, BPE merges trained on a small fixed corpus
     (ids in merge order, so the vocabulary is a consistent BPE vocabulary), padding tokens, then the special tokens."""
-    specials = QWEN3_SPECIALS if arch in ("qwen3", "qwen2") else LLAMA_SPECIALS
+    specials = QWEN3_SPECIALS if arch in ("qwen3", "qwen2", "qwen2moe") else LLAMA_SPECIALS
     n_merges = vocab_size - 256 - len(specials)
     if n_merges < 0:
         raise ValueError("vocabulary too small for the byte symbols and the special tokens")
@@ -191,7 +203,7 @@ def build_vocab(vocab_size: int, arch: str = "llama", seed: int = 1234):
     types = [1] * base + [3] * len(specials)  # 1 normal, 3 control
     for i in range(base - pad, base):
         types[i] = 5
-    if arch in ("qwen3", "qwen2"):
+    if arch in ("qwen3", "qwen2", "qwen2moe"):
         for t in ("<think>", "</think>", "<tool_call>", "</tool_call>"):
             types[tokens.index(t)] = 4  # user defined: displayed (Qwen3Tokenizer.shouldDisplayToken)
     return tokens, merges, types, base
@@ -216,7 +228,13 @@ def metadata_for(shape: Shape, quant: int, name: str) -> dict:
     if a == "qwen3":
         md["qwen3.attention.key_length"] = shape.head_size
         md["qwen3.attention.value_length"] = shape.head_size
-    if shape.vocab <= 4096 or a == "qwen2":  # tokenizer section (Qwen2 takes its vocabulary size from the token list) (GGUF keys the loaders read: tokenizer.ggml.tokens / merges / token_type)
+    if a == "qwen2moe":  # Qwen2MoEModelLoader.createConfiguration
+        md["qwen2moe.expert_count"] = shape.n_experts
+        md["qwen2moe.expert_used_count"] = shape.n_experts_used
+        md["qwen2moe.expert_feed_forward_length"] = shape.expert_hidden
+        md["qwen2moe.expert_shared_feed_forward_length"] = shape.hidden
+        del md["qwen2moe.vocab_size"]  # the vocabulary size is the token list's
+    if shape.vocab <= 4096 or a in ("qwen2", "qwen2moe"):  # tokenizer section (Qwen2 takes its vocabulary size from the token list) (GGUF keys the loaders read: tokenizer.ggml.tokens / merges / token_type)
         tokens, merges, types, base = build_vocab(shape.vocab, a)
         md["tokenizer.ggml.model"] = "gpt2"
         md["tokenizer.ggml.tokens"] = tokens
@@ -248,13 +266,29 @@ def tensor_plan(shape: Shape, quant: int):
             (p + "attn_v.weight", quant, (shape.dim, shape.kv_dim), "w"),
             (p + "attn_output.weight", quant, (shape.q_dim, shape.dim), "w"),
         ]
-        if shape.arch == "qwen2":  # Qwen2ModelLoader.java:100-102
-            t += [(p + "attn_q.bias", GGMLType.F32, (shape.q_dim,), "b"),
-                  (p + "attn_k.bias", GGMLType.F32, (shape.kv_dim,), "b"),
-                  (p + "attn_v.bias", GGMLType.F32, (shape.kv_dim,), "b")]
+        if shape.arch in ("qwen2", "qwen2moe"):  # Qwen2ModelLoader.java:100-102
+            # qwen2moe: small biases ("s"), so the residual stream, and with it the routing, still varies from token to token
+            b = "b" if shape.arch == "qwen2" else "s"
+            t += [(p + "attn_q.bias", GGMLType.F32, (shape.q_dim,), b),
+                  (p + "attn_k.bias", GGMLType.F32, (shape.kv_dim,), b),
+                  (p + "attn_v.bias", GGMLType.F32, (shape.kv_dim,), b)]
         if shape.arch == "qwen3":
             t += [(p + "attn_q_norm.weight", GGMLType.F32, (shape.head_size,), "n"),
                   (p + "attn_k_norm.weight", GGMLType.F32, (shape.head_size,), "n")]
+        if shape.arch == "qwen2moe":  # llama.cpp's qwen2moe tensors; the stacked experts are [E][rows][cols] (dims innermost first)
+            E, he = shape.n_experts, shape.expert_hidden
+            t += [
+                (p + "ffn_norm.weight", GGMLType.F32, (shape.dim,), "n"),
+                (p + "ffn_gate_inp.weight", GGMLType.F32, (shape.dim, E), "r"),
+                (p + "ffn_gate_inp_shexp.weight", GGMLType.F32, (shape.dim,), "r"),
+                (p + "ffn_gate_exps.weight", quant, (shape.dim, he, E), "w"),
+                (p + "ffn_up_exps.weight", quant, (shape.dim, he, E), "w"),
+                (p + "ffn_down_exps.weight", quant, (he, shape.dim, E), "w"),
+                (p + "ffn_gate_shexp.weight", quant, (shape.dim, shape.hidden), "w"),
+                (p + "ffn_up_shexp.weight", quant, (shape.dim, shape.hidden), "w"),
+                (p + "ffn_down_shexp.weight", quant, (shape.hidden, shape.dim), "w"),
+            ]
+            continue
         t += [
             (p + "ffn_norm.weight", GGMLType.F32, (shape.dim,), "n"),
             (p + "ffn_gate.weight", quant, (shape.dim, shape.hidden), "w"),
@@ -276,9 +310,16 @@ def qkv_bias(n: int, rng) -> np.ndarray:
     return x
 
 
+# Router logits of a unit-RMS input get a standard deviation of about ROUTER_SCALE: the softmax is far from uniform, so the top-k
+# changes from token to token and every expert is picked within a short run.
+ROUTER_SCALE = 2.0
+SMALL_BIAS = 0.1
+
+
 def build_tensors(shape: Shape, quant: int, seed: int = 1234, w_std: float = 0.02):
     """Seeded tensors: matrices N(0, w_std) (scaled so activations stay O(1) through the
-    stack), norm weights 1 + N(0, 0.02), Qwen2 biases as `qkv_bias`.  Returns [(name, type, dims, raw uint8)]."""
+    stack), norm weights 1 + N(0, 0.02), Qwen2 biases as `qkv_bias`, Qwen2-MoE routers N(0, ROUTER_SCALE / sqrt(dim)).
+    Returns [(name, type, dims, raw uint8)]."""
     rng = np.random.Generator(np.random.PCG64(seed))
     out = []
     for name, tt, dims, kind in tensor_plan(shape, quant):
@@ -287,6 +328,10 @@ def build_tensors(shape: Shape, quant: int, seed: int = 1234, w_std: float = 0.0
             x = (1.0 + 0.02 * rng.standard_normal(n, dtype=np.float32)).astype(np.float32)
         elif kind == "b":
             x = qkv_bias(n, rng)
+        elif kind == "r":
+            x = rng.standard_normal(n, dtype=np.float32) * np.float32(ROUTER_SCALE / np.sqrt(dims[0]))
+        elif kind == "s":
+            x = rng.standard_normal(n, dtype=np.float32) * np.float32(SMALL_BIAS)
         else:
             # fan-in scaled so that W.x of a unit-RMS vector is O(1): keeps logits in a sane range
             std = w_std if w_std > 0 else 1.0 / np.sqrt(dims[0])
@@ -338,6 +383,10 @@ def build_tensors_kquant(shape: Shape, seed: int = 1234, mix: str = "Q4_K_M") ->
             out[name] = (GGMLType.F32, dims, (1.0 + 0.02 * rng.standard_normal(n, dtype=np.float32)).astype(np.float32).view(np.uint8))
         elif kind == "b":
             out[name] = (GGMLType.F32, dims, qkv_bias(n, rng).view(np.uint8))
+        elif kind == "r":
+            out[name] = (GGMLType.F32, dims, (rng.standard_normal(n, dtype=np.float32) * np.float32(ROUTER_SCALE / np.sqrt(dims[0]))).view(np.uint8))
+        elif kind == "s":
+            out[name] = (GGMLType.F32, dims, (rng.standard_normal(n, dtype=np.float32) * np.float32(SMALL_BIAS)).view(np.uint8))
         else:
             tt = pick(name)
             out[name] = (tt, dims, random_kquant(tt, n, rng, zero_blocks=1 if "attn_q" in name else 0))
@@ -347,7 +396,8 @@ def build_tensors_kquant(shape: Shape, seed: int = 1234, mix: str = "Q4_K_M") ->
 def write_model(path: str, shape_name: str, quant: int, seed: int = 1234, w_std: float = 0.0,
                 display_name: str | None = None):
     shape = SHAPES[shape_name]
-    name = display_name or {"llama": "Llama synthetic ", "qwen3": "Qwen3 synthetic ", "phi3": "Phi3 synthetic ", "qwen2": "Qwen2 synthetic "}[shape.arch] + shape_name
+    name = display_name or {"llama": "Llama synthetic ", "qwen3": "Qwen3 synthetic ", "phi3": "Phi3 synthetic ", "qwen2": "Qwen2 synthetic ",
+                            "qwen2moe": "Qwen1.5 MoE synthetic "}[shape.arch] + shape_name
     write_gguf(path, metadata_for(shape, quant, name), build_tensors(shape, quant, seed, w_std))
     return shape
 
@@ -396,13 +446,16 @@ def build_tensors_fast(shape: Shape, quant: int, seed: int = 1234, device: str |
             x = 1.0 + 0.02 * torch.randn(n, device=dev, generator=gen)
             out[name] = (tt, dims, x.float().cpu().numpy().view(np.uint8).reshape(-1))
             continue
+        if kind == "s":
+            out[name] = (tt, dims, (SMALL_BIAS * torch.randn(n, device=dev, generator=gen)).float().cpu().numpy().view(np.uint8).reshape(-1))
+            continue
         if kind == "b":  # qkv_bias's distribution: N(0, 1), one entry in 32 at +-20
             x = torch.randn(n, device=dev, generator=gen)
             big = torch.randperm(n, device=dev, generator=gen)[:max(1, n // 32)]
             x[big] = torch.where(torch.rand(len(big), device=dev, generator=gen) < 0.5, -20.0, 20.0)
             out[name] = (tt, dims, x.float().cpu().numpy().view(np.uint8).reshape(-1))
             continue
-        std = 1.0 / float(np.sqrt(dims[0]))
+        std = (ROUTER_SCALE if kind == "r" else 1.0) / float(np.sqrt(dims[0]))
         nbytes = GGMLType.byte_size_for(tt, n)
         host = np.empty(nbytes, dtype=np.uint8)
         cols = int(dims[0])

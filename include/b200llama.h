@@ -43,6 +43,8 @@ extern "C" {
                            * tensors plus F32 biases blk.N.attn_q.bias (n_heads * head_size floats), attn_k.bias and attn_v.bias
                            * (n_kv_heads * head_size each), added to q, k and v right after their matmuls; NeoX-pair RoPE without q/k
                            * norm; n_heads * head_size == dim.  Under tensor parallelism a rank reads the bias rows of its own heads. */
+#define B200_ARCH_QWEN2_MOE 4 /* InferenceCore.forwardJavaQwen2MoE, InferenceCore.java:263-432 (Qwen1.5-MoE-A2.7B): Qwen2's attention (q/k/v
+                               * biases, NeoX RoPE) and a mixture-of-experts FFN.  Created with b200_plan_create_moe only. */
 
 /* GGML tensor type ids accepted for weights (tensor/GGMLType.java:5-20) */
 #define B200_GGML_F32 0
@@ -86,6 +88,15 @@ typedef struct b200_tensor {
     int64_t dims[4];
 } b200_tensor;
 
+/* Expert configuration of a B200_ARCH_QWEN2_MOE plan (Qwen2MoEModelLoader.createConfiguration).  b200_config.hidden_dim is unused
+ * (0, as the reference's configuration has it). */
+typedef struct b200_moe_config {
+    int32_t n_experts;         /* expert_count (E), 1..256 */
+    int32_t n_experts_used;    /* expert_used_count (k), 1..min(E, 8) */
+    int32_t expert_hidden_dim; /* ffn_down_exps dims[0] (He) */
+    int32_t shared_hidden_dim; /* ffn_gate_shexp dims[1] (Hs) */
+} b200_moe_config;
+
 typedef struct b200_plan b200_plan;
 
 /* TornadoVMMasterPlan.initializeTornadoVMPlan(state, model) (TornadoVMMasterPlan.java:55-70)
@@ -96,6 +107,25 @@ typedef struct b200_plan b200_plan;
  * On failure *out is NULL and err (if non-NULL) receives the message. */
 int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t n_tensors,
                      int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
+
+/* b200_plan_create for cfg->arch == B200_ARCH_QWEN2_MOE (b200_plan_create refuses that arch with B200_ERR_BAD_ARG, and this call
+ * every other).  Per layer it requires, besides Qwen2's attention tensors and biases and the two norms (dims[0] innermost, as
+ * llama.cpp writes them):
+ *   blk.N.ffn_gate_inp.weight        F32 [dim, E]          the router
+ *   blk.N.ffn_gate_inp_shexp.weight  F32 [dim]             the shared-expert gate
+ *   blk.N.ffn_{gate,up}_exps.weight  [dim, He, E]          the routed experts, stacked [E][He][dim]
+ *   blk.N.ffn_down_exps.weight       [He, dim, E]          stacked [E][dim][He]
+ *   blk.N.ffn_{gate,up}_shexp.weight [dim, Hs]             the shared expert
+ *   blk.N.ffn_down_shexp.weight      [Hs, dim]
+ * Matrices are Q8_0 or K-quants (re-quantised to Q8_0 at upload).  Each layer's FFN runs the reference's order: F32 router dot
+ * products (sequential, no FMA), softmax, top-k by first strict maximum with the probabilities as weights (no renormalisation), the k
+ * routed experts' SwiGLU FFNs added to x in selection order (x[i] = w * y[i] + x[i]), then the shared expert with weight
+ * 1 / (1 + exp(-g)).  B200_ERR_BAD_ARG: a missing tensor, wrong dims, n_experts_used outside 1..min(E, 8).  B200_ERR_UNSUPPORTED
+ * (reason in the message): a router or shared gate that is not F32, FP16 weights, tp_size > 1, the non-streaming Q8_0 layout,
+ * hidden sizes the stream layout cannot cut.  The plan decodes through the CUDA graph (not the persistent kernel), prefills through
+ * the exact path only, and refuses b200_set_decode_slots (n_slots > 0) and b200_time_kernel with B200_ERR_UNSUPPORTED. */
+int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors,
+                         int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
 
 /* TornadoVMMasterPlan.tornadoVMForwardDecode(position) with the embedding gather moved
  * device-side (replaces InferenceCore.forwardTornadoVM, InferenceCore.java:956-980, which copies
@@ -226,7 +256,10 @@ int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_ste
  * layer for the KV caches (ignored otherwise).  The tensor-core prefill scratch, as the last layer of the last
  * chunk left it, rows padded to a multiple of 128: "pf_x" (f32 residual, dim wide), "pf_qkv" (f32, q + k + v wide,
  * q rotated in place (after its Qwen2 bias), k before RoPE and v, both before their Qwen2 bias), "pf_a16" (f16 bits, the FFN input), "pf_att16" (f16 bits, attention output),
- * "pf_h16" (f16 bits, SwiGLU output).  Copies min(bytes, buffer size). */
+ * "pf_h16" (f16 bits, SwiGLU output).  Qwen2-MoE plans: "hb", "hq", "hs" hold the virtual hidden vector of the last layer (the shared
+ * expert's units, then each routed slot's, shared_hidden_dim + n_experts_used * expert_hidden_dim units), "moe_ids" (int32 [layer][k], the experts the last step selected, in
+ * selection order) and "moe_weights" (f32 [layer][k + 1], their routing weights, then the shared-expert weight).
+ * Copies min(bytes, buffer size). */
 int b200_read_buffer(b200_plan *plan, const char *name, int32_t layer, void *dst, size_t bytes);
 
 /* Measurement hook for bench.py's roofline line: launches ONE kernel family of the decode step
@@ -254,7 +287,8 @@ int b200_tp_attach(b200_plan *plan, const void *handles, int32_t n);
  * programmatic-dependent-launch edges) and returns one record per kernel launch, in launch order:
  * {kernel id, earliest CTA entry, latest dependency-wait return, latest CTA exit}, the times in
  * %globaltimer nanoseconds.  ids: 1 rmsnorm, 2 qkv, 3 rope+kv, 4 attention, 5 attn-out, 6 gate/up,
- * 7 down, 8 lm_head, 9 argmax/advance.  records holds 4*cap uint64. */
+ * 7 down, 8 lm_head, 9 argmax/advance; Qwen2-MoE layers: 1 for the FFN norm, then 10 router, 11 expert gate/up, 12 expert down.
+ * records holds 4*cap uint64. */
 int b200_trace_decode(b200_plan *plan, int32_t token, int32_t position, uint64_t *records, int32_t cap, int32_t *n_out);
 
 /* Diagnostic: ONE decode step through the persistent kernel with phase stamps: stamps[cta][row][k] (uint64, %globaltimer ns),

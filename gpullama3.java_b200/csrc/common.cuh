@@ -111,9 +111,12 @@ __device__ __forceinline__ float ldcg_f32c(const float *p) {
 //   Llama / Mistral: interleaved-pair RoPE (InferenceCore.java:75-87); Qwen3: NeoX pairs + per-head q/k RMSNorm (:594-619);
 //   Phi-3: NeoX pairs, no q/k norm (forwardJavaPhi3, :726-742); Qwen2: F32 biases added to q, k and v right after their matmuls
 //   (q.addInPlace(q_bias) etc., :456-459), then NeoX pairs without q/k norm (:463-478).
+//   Granite: the attention score is multiplied by the model's attentionScale instead of divided by sqrt(head size)
+//   (forwardGranite, :868-873); the kernels' `sqrt_hs` argument then carries that multiplier.
 #define KF_NEOX 1
 #define KF_QKNORM 2
 #define KF_QKVBIAS 4
+#define KF_ATTSCALE 8
 
 // In-graph timeline tracing (diagnostic graph only; rec == nullptr in the production graphs, so the
 // branch is uniform and free).  One record per launch: {kernel id, earliest CTA entry, latest

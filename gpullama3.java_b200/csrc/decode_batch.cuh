@@ -26,10 +26,10 @@ struct BatchRows {
 // ---- RMSNorm + quantisation, one CTA per row ------------------------------------------------------------------------------
 template <bool EMBED>
 __global__ void __launch_bounds__(NORM_THREADS, 1) k_rmsnorm_quant_batch(float *__restrict__ x, const BatchRows *__restrict__ rows, DevMat emb,
-                                                                     const float *__restrict__ w, float eps, int dim,
+                                                                     float emb_scale, const float *__restrict__ w, float eps, int dim,
                                                                      int8_t *__restrict__ xq, float *__restrict__ xs, TraceBuf tr, TpCtx tp) {
     const int v = blockIdx.x;
-    rmsnorm_quant_row<EMBED>(x + (size_t)v * dim, rows->token + v, emb, w, eps, dim, xq + (size_t)v * dim, xs + (size_t)v * (dim / 32),
+    rmsnorm_quant_row<EMBED>(x + (size_t)v * dim, rows->token + v, emb, emb_scale, w, eps, dim, xq + (size_t)v * dim, xs + (size_t)v * (dim / 32),
                              nullptr, nullptr, tr, tp, -1);
 }
 
@@ -86,7 +86,8 @@ struct SmbArgs {
     int nrow;           // activation rows (sequences) of this launch
     const int8_t *xq;   // [nrow][cols] quantised activations
     const float *xs;    // [nrow][cols / 32] their block scales
-    float *out;         // STORE: out[v][row] = r; RESID: out[v][row] += r; GATEUP: hb[v][unit]
+    float *out;         // STORE: out[v][row] = r * oscale; RESID: out[v][row] += r * oscale; GATEUP: hb[v][unit]
+    float oscale;       // Granite's logitScale / residualScale (SmvArgs::oscale); 1.0f otherwise
     int ostride;        // floats between two rows' outputs
     int8_t *hq;         // GATEUP: quantised hb [nrow][ostride]
     float *hs;          // GATEUP: its block scales [nrow][ostride / 32]
@@ -102,7 +103,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8_batch(SmbAr
     const TileMat W = a.W;
     const int S = L.stages, nrow = a.nrow;
     const unsigned bar0 = smem_u32(smem + L.off_bar);
-    const int ngroups = W.rows >> 2;
+    const int ngroups = tile_groups(W);
     const int g0 = (int)(((long long)blockIdx.x * ngroups) / gridDim.x);
     const int g1 = (int)(((long long)(blockIdx.x + 1) * ngroups) / gridDim.x);
     const int nseg = W.nseg;
@@ -224,9 +225,10 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8_batch(SmbAr
             if (MODE == SMV_GATEUP) {
                 const float up = __shfl_down_sync(0xffffffffu, acc, 2); // lanes 4v, 4v+1: gate rows; 4v+2, 4v+3: up rows
                 if (lane < nchain && r < 2) a.out[(size_t)v * a.ostride + 2 * G + r] = swiglu_exact(acc, up);
-            } else if (lane < nchain) {
+            } else if (lane < nchain && 4 * G + r < W.rows) {
                 const int row = 4 * G + r;
                 float *o = a.out + (size_t)v * a.ostride + row;
+                acc = __fmul_rn(acc, a.oscale);
                 if (MODE == SMV_RESID) *o = __fadd_rn(*o, acc);
                 else {
                     *o = acc;

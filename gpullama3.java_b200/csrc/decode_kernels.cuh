@@ -20,7 +20,7 @@ enum { MODE_STORE = 0, MODE_RESID = 1 };
 // ------------------------------------------------------------------------------------------
 // Embedding row lookup: FloatTensor.copyTo -> getFloat per element (InferenceCore.java:61).
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ float emb_get(const DevMat &e, int token, int i) {
+__device__ __forceinline__ float emb_get_raw(const DevMat &e, int token, int i) {
     size_t idx = (size_t)token * e.cols + i;
     if (e.type == 8) { // Q8_0FloatTensor.getFloat: quant * scale (Q8_0FloatTensor.java:55-63)
         float q = (float)((const int8_t *)e.qs)[idx];
@@ -30,6 +30,9 @@ __device__ __forceinline__ float emb_get(const DevMat &e, int token, int i) {
     }
     return ((const float *)e.qs)[idx];
 }
+// The embedding row times the model's embedding scale: Granite's x[i] = x[i] * embeddingScale (InferenceCore.java:826-829), one
+// rounding; every other family passes 1.0f, which leaves each value bit for bit as it is.
+__device__ __forceinline__ float emb_get(const DevMat &e, int token, int i, float es) { return __fmul_rn(emb_get_raw(e, token, i), es); }
 
 // ------------------------------------------------------------------------------------------
 // RMSNorm (+ optional embedding gather, + Q8_0 activation quantisation).
@@ -45,7 +48,7 @@ __host__ __device__ inline size_t norm_smem_bytes(int dim) { return (size_t)norm
 // The body of k_rmsnorm_quant for one vector; `tok` is read after the dependency wait (the batched step, decode_batch.cuh,
 // runs it once per row with that row's x, token and outputs).
 template <bool EMBED>
-__device__ __forceinline__ void rmsnorm_quant_row(float *__restrict__ x, const int *__restrict__ tok, const DevMat &emb,
+__device__ __forceinline__ void rmsnorm_quant_row(float *__restrict__ x, const int *__restrict__ tok, const DevMat &emb, float emb_scale,
                                                   const float *__restrict__ w, float eps, int dim, int8_t *__restrict__ xq,
                                                   float *__restrict__ xs, float *__restrict__ xb, long long *__restrict__ prof,
                                                   const TraceBuf &tr, const TpCtx &tp, int tp_wait_op) {
@@ -68,7 +71,7 @@ __device__ __forceinline__ void rmsnorm_quant_row(float *__restrict__ x, const i
     if (EMBED) token = *tok;
     for (int i = tid; i < dim; i += NORM_THREADS) {
         float v;
-        if (EMBED) { v = emb_get(emb, token, i); x[i] = v; }
+        if (EMBED) { v = emb_get(emb, token, i, emb_scale); x[i] = v; }
         else v = ldcg_f32c(x + i);
         sq[i] = __fmul_rn(v, v);
     }
@@ -127,12 +130,12 @@ __device__ __forceinline__ void rmsnorm_quant_row(float *__restrict__ x, const i
 
 template <bool EMBED>
 __global__ void __launch_bounds__(NORM_THREADS, 1) k_rmsnorm_quant(float *__restrict__ x, const StepState *__restrict__ st,
-                                                               DevMat emb, const float *__restrict__ w, float eps, int dim,
+                                                               DevMat emb, float emb_scale, const float *__restrict__ w, float eps, int dim,
                                                                int8_t *__restrict__ xq, float *__restrict__ xs,
                                                                float *__restrict__ xb, long long *__restrict__ prof, TraceBuf tr, TpCtx tp, int tp_wait_op) {
     // One CTA of 1024 threads.  Under PDL this CTA only has to fit next to ONE streaming-matvec CTA
     // (the following matvec's CTA for this SM simply starts a little later).
-    rmsnorm_quant_row<EMBED>(x, &st->token, emb, w, eps, dim, xq, xs, xb, prof, tr, tp, tp_wait_op);
+    rmsnorm_quant_row<EMBED>(x, &st->token, emb, emb_scale, w, eps, dim, xq, xs, xb, prof, tr, tp, tp_wait_op);
 }
 
 // Test hook: the sequential-sum emulation on arbitrary non-negative terms (padded with zeros: adding +0 never changes a sum
@@ -219,7 +222,7 @@ __host__ __device__ inline size_t q8_smem_bytes(int cols, int rows_per_warp, int
 template <int R, int MODE>
 __global__ void __launch_bounds__(256) k_matvec_q8(const int8_t *__restrict__ qs, const __half *__restrict__ sc,
                                                    const int8_t *__restrict__ xq, const float *__restrict__ xs, int rows,
-                                                   int cols, float *__restrict__ out) {
+                                                   int cols, float *__restrict__ out, float oscale) {
     extern __shared__ __align__(16) unsigned char smraw[];
     const int nb = cols >> 5, nbp = nb | 1;
     int4 *sxq = reinterpret_cast<int4 *>(smraw);
@@ -238,6 +241,7 @@ __global__ void __launch_bounds__(256) k_matvec_q8(const int8_t *__restrict__ qs
             float acc = 0.0f;
             for (int b = 0; b < nb; b++) acc = __fadd_rn(acc, t[b]);
             size_t row = row0 + lane;
+            acc = __fmul_rn(acc, oscale); // Granite's residualScale / logitScale (1.0f: unchanged)
             if (MODE == MODE_RESID) out[row] = __fadd_rn(out[row], acc); // x[i] = x[i] + xb2[i]  (InferenceCore.java:143,164)
             else out[row] = acc;
         }
@@ -309,7 +313,7 @@ __global__ void __launch_bounds__(256) k_gateup_q8(const int8_t *__restrict__ qs
 // ------------------------------------------------------------------------------------------
 template <int MODE>
 __global__ void __launch_bounds__(256) k_matvec_f16(const __half *__restrict__ w, const float *__restrict__ x, int rows,
-                                                    int cols, int lanes, float *__restrict__ out) {
+                                                    int cols, int lanes, float *__restrict__ out, float oscale) {
     // Each warp processes RW = 32/lanes rows at once; thread t of the warp: row r = t / lanes, chain c = t % lanes.
     // Shared: activation x (cols floats) + per-warp weight tile RW x TC halves.
     extern __shared__ __align__(16) unsigned char smraw[];
@@ -366,6 +370,7 @@ __global__ void __launch_bounds__(256) k_matvec_f16(const __half *__restrict__ w
         }
         size_t row = row0 + r;
         if (c == 0 && row < (size_t)rows) {
+            result = __fmul_rn(result, oscale); // Granite's residualScale / logitScale (1.0f: unchanged)
             if (MODE == MODE_RESID) out[row] = __fadd_rn(out[row], result);
             else out[row] = result;
         }
@@ -527,7 +532,7 @@ __device__ __forceinline__ void attention_head(float *__restrict__ qkv, float *_
             acc = __shfl_sync(0xffffffffu, acc, qbase + qd4);
         }
         if (quad == 0 && t < nt) {
-            const float s = __fdiv_rn(acc, sqrt_hs);
+            const float s = (arch & KF_ATTSCALE) ? __fmul_rn(acc, sqrt_hs) : __fdiv_rn(acc, sqrt_hs); // Granite: score *= attentionScale
             att[t] = s;
             lmax = fmaxf(lmax, s);
         }

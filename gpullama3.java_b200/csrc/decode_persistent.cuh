@@ -20,7 +20,7 @@
 //   * attention heads run on the first n_heads CTAs with the consumer warps; the score row lives in shared memory, or
 //     in a global scratch row when the context is too long for it;
 //   * the embedding row is consumed in place: layer 0's norm squares the embedding row and layer 0's Wo epilogue
-//     writes x = emb + Wo*att, so there is no "x = embedding" pass and no grid sync before the first layer;
+//     writes x = emb * embeddingScale + Wo*att * residualScale (both scales 1 outside Granite), so there is no "x = embedding" pass and no grid sync before the first layer;
 //   * every spin has a deadline (%globaltimer): a lost peer or a desynchronised call sequence sets an error word the
 //     host checks after the launch instead of hanging the GPU.
 #pragma once
@@ -57,7 +57,8 @@ struct PdArgs {
     int dim, hidden, qd;     // full widths (qd = columns of Wo)
     int n_heads, n_kv_heads; // of THIS rank
     int head_size, arch /* KF_* flags */, ctx;
-    float eps, sqrt_hs;
+    float eps, sqrt_hs;      // KF_ATTSCALE: sqrt_hs holds Granite's attention multiplier
+    float emb_scale, res_scale, logit_scale; // Granite's embedding / residual / logit scales (1.0f for every other family)
     const float *rope_cr, *rope_ci;
     StepState *st;
     const int *seq_tokens;
@@ -221,7 +222,7 @@ struct PdWalk {
                 const int k = mi & 3;
                 W = k == 0 ? Ly.qkv : k == 1 ? Ly.wo : k == 2 ? Ly.gu : Ly.w2;
             } else W = a->lm_head;
-            const int ngroups = W.rows >> 2;
+            const int ngroups = tile_groups(W);
             gb = (int)(((long long)blockIdx.x * ngroups) / gridDim.x);
             g1 = (int)(((long long)(blockIdx.x + 1) * ngroups) / gridDim.x);
             if (gb < g1) {
@@ -293,7 +294,7 @@ __device__ __noinline__ int pd_quant_block(float v, float *ascale) {
     *ascale = as;
     return q;
 }
-__device__ __noinline__ float pd_emb_get(const DevMat &e, int token, int i) { return emb_get(e, token, i); }
+__device__ __noinline__ float pd_emb_get(const DevMat &e, int token, int i, float es) { return emb_get(e, token, i, es); }
 __device__ __noinline__ float pd_exp_narrow(float x) { return (float)exp((double)x); } // (float) Math.exp(double)
 
 // ---- consumers: one matrix (the loop of k_stream_matvec_q8, activation already in shared memory) --------------------------
@@ -306,7 +307,8 @@ __device__ __noinline__ void pd_consume_matrix(const TileMat &W, const PdArgs &a
     // otherwise re-read W.* (global memory) and L.* on every use inside the tile loop
     const int lane = tid & 31, warp = tid >> 5, S = L.stages, tstride = L.tstride, stage_bytes = L.stage_bytes;
     const int w_unit = W.unit_bytes, w_seg = W.seg;
-    const int ngroups = W.rows >> 2;
+    const int ngroups = tile_groups(W);
+    const float oscale = MODE == SMV_RESID ? a.res_scale : argmax ? a.logit_scale : 1.0f;
     const int g0 = (int)(((long long)blockIdx.x * ngroups) / gridDim.x), g1 = (int)(((long long)(blockIdx.x + 1) * ngroups) / gridDim.x);
     const int nseg = W.nseg, nbs = w_seg >> 5;
     const unsigned char *ring = smem + L.off_ring;
@@ -373,11 +375,12 @@ __device__ __noinline__ void pd_consume_matrix(const TileMat &W, const PdArgs &a
                     out[unit] = hval;
                     hvals[unit - 2 * g0] = hval;
                 }
-            } else if (lane < 4) {
+            } else if (lane < 4 && 4 * G + lane < W.rows) {
                 const size_t row = (size_t)4 * G + lane;
+                acc = __fmul_rn(acc, oscale);
                 if (MODE == SMV_RESID) {
                     const size_t grow = (size_t)row_base + row;
-                    const float base = l0_emb ? pd_emb_get(a.emb, token, (int)grow) : out[grow];
+                    const float base = l0_emb ? pd_emb_get(a.emb, token, (int)grow, a.emb_scale) : out[grow];
                     const float v = __fadd_rn(base, acc); // x[i] = x[i] + xb2[i]
                     if (tp_n > 1) { // all-gather of the residual stream: this rank's rows go to every rank
                         for (int k = 0; k < tp_n; k++) tp_ptr<float>(a.tp, k, a.tp.off_x)[grow] = v;
@@ -489,7 +492,8 @@ __device__ __noinline__ void pd_norm_u(const PdArgs &a, const float *wbuf, bool 
         xv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (i4 < n4) {
             if (from_emb) { // first layer: the embedding row (quantised table: element-wise, FloatTensor.copyTo)
-                xv[u] = make_float4(pd_emb_get(a.emb, token, 4 * i4), pd_emb_get(a.emb, token, 4 * i4 + 1), pd_emb_get(a.emb, token, 4 * i4 + 2), pd_emb_get(a.emb, token, 4 * i4 + 3));
+                xv[u] = make_float4(pd_emb_get(a.emb, token, 4 * i4, a.emb_scale), pd_emb_get(a.emb, token, 4 * i4 + 1, a.emb_scale),
+                                    pd_emb_get(a.emb, token, 4 * i4 + 2, a.emb_scale), pd_emb_get(a.emb, token, 4 * i4 + 3, a.emb_scale));
             } else xv[u] = pd_ldcg128(a.x + 4 * i4);
         }
     }
@@ -707,7 +711,7 @@ __device__ __noinline__ void pd_attention_head(const PdArgs &a, const PdLayer &L
             acc = __shfl_sync(0xffffffffu, acc, qbase + qd); // the chain so far, to the whole quad
         }
         if (quad == 0 && t < nt) {
-            const float sc = __fdiv_rn(acc, a.sqrt_hs);
+            const float sc = (a.arch & KF_ATTSCALE) ? __fmul_rn(acc, a.sqrt_hs) : __fdiv_rn(acc, a.sqrt_hs); // Granite: score *= attentionScale
             att[t] = sc;
             lmax = fmaxf(lmax, sc);
         }

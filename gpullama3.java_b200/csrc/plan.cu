@@ -129,6 +129,9 @@ struct b200_plan {
     unsigned *moe_done = nullptr;
     MoeDownSmem moe_dl{};
 
+    // Granite's µP scales (b200_plan_create_granite); 1.0f for every other family, where each multiply leaves its operand unchanged
+    b200_granite_config mup{1.0f, 1.0f, 1.0f, 1.0f};
+
     PrefillCtx prefill;
     // persistent decode kernel
     bool pd_ok = false;           // the plan fits the kernel's restrictions
@@ -415,12 +418,13 @@ int upload_tiles(b200_plan *p, const b200_tensor *t0, const b200_tensor *t1, con
     out.nseg = smv_pick_nseg(cols);
     out.seg = cols / out.nseg;
     out.unit_bytes = smv_unit_bytes(out.seg);
-    size_t total = (size_t)rows * out.nseg * out.unit_bytes;
+    const size_t stored_rows = (size_t)tile_groups(out) * 4; // whole 4-row groups: a ragged classifier gets zero padding rows
+    size_t total = stored_rows * out.nseg * out.unit_bytes;
     unsigned char *d;
     rc = dalloc(p, &d, total);
     if (rc) return rc;
     out.base = d;
-    k_repack_tiles<<<(unsigned)((size_t)rows * out.nseg), 128, 0, p->stream>>>(src, d, rows, cols, out.seg, out.nseg, out.unit_bytes);
+    k_repack_tiles<<<(unsigned)(stored_rows * out.nseg), 128, 0, p->stream>>>(src, d, rows, cols, out.seg, out.nseg, out.unit_bytes);
     CK(cudaGetLastError());
     return up_stage_release(p);
 }
@@ -479,15 +483,21 @@ int upload_qkv_bias(b200_plan *p, const b200_tensor *tensors, int n_tensors, int
     return B200_OK;
 }
 
+// Output scale of a STORE / RESID epilogue: Granite's residualScale on the Wo / W2 branch, its logitScale on the classifier, else 1.
+float out_scale(const b200_plan *p, bool resid, bool classifier) { return resid ? p->mup.residual_scale : classifier ? p->mup.logit_scale : 1.0f; }
+// The attention kernels' score argument: the divisor sqrt(head size), or (KF_ATTSCALE) Granite's attentionScale multiplier.
+float att_score_arg(const b200_plan *p) { return (p->kflags & KF_ATTSCALE) ? p->mup.attention_scale : (float)sqrt((double)p->cfg.head_size); }
+
 template <int MODE> int launch_matvec_q8(b200_plan *p, const DevMat &m, const int8_t *xq, const float *xs, float *out) {
     int R = (m.rows % 4 == 0 && m.rows >= 32768) ? 4 : (m.rows % 2 == 0 ? 2 : 1);
     int warps = m.rows / R;
     int ctas = (warps + 7) / 8;
     size_t smem = q8_smem_bytes(m.cols, R, 8);
     const int8_t *qs = (const int8_t *)m.qs;
-    if (R == 4) k_matvec_q8<4, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out);
-    else if (R == 2) k_matvec_q8<2, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out);
-    else k_matvec_q8<1, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out);
+    const float os = out_scale(p, MODE == MODE_RESID, &m == &p->out);
+    if (R == 4) k_matvec_q8<4, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out, os);
+    else if (R == 2) k_matvec_q8<2, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out, os);
+    else k_matvec_q8<1, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out, os);
     CK(cudaGetLastError());
     return B200_OK;
 }
@@ -503,7 +513,8 @@ template <int MODE> int launch_matvec_f16(b200_plan *p, const DevMat &m, const f
     int warps = (m.rows + rw - 1) / rw;
     int ctas = (warps + 7) / 8;
     k_matvec_f16<MODE><<<ctas, 256, f16_smem_bytes(m.cols, p->cfg.fp16_lanes), p->stream>>>((const __half *)m.qs, x, m.rows,
-                                                                                            m.cols, p->cfg.fp16_lanes, out);
+                                                                                            m.cols, p->cfg.fp16_lanes, out,
+                                                                                            out_scale(p, MODE == MODE_RESID, &m == &p->out));
     CK(cudaGetLastError());
     return B200_OK;
 }
@@ -515,7 +526,8 @@ int sf_grid(const b200_plan *p, int rows, int cols, bool gateup) { // CTAs of an
     const SfLayout L = sf_layout(rows, cols, lanes, gateup);
     const int rw = 64 / lanes, mr = gateup ? rw / 2 : rw;
     const int grid = L.ctas_per_sm * p->n_sms;
-    return grid > rows / mr ? rows / mr : grid;
+    const int groups = (rows + mr - 1) / mr; // a ragged classifier ends in a partial group
+    return grid > groups ? groups : grid;
 }
 template <int MODE> int launch_stream_f16(b200_plan *p, const DevMat &m, const DevMat *m2, const float *x, float *out, TraceBuf tr = TraceBuf{nullptr, 0, 0},
                                           bool argmax = false) {
@@ -524,6 +536,7 @@ template <int MODE> int launch_stream_f16(b200_plan *p, const DevMat &m, const D
     if (!L.ok) return fail(p, B200_ERR_STATE, "f16 streaming layout does not fit %d x %d", m.rows, m.cols);
     SfArgs a;
     a.w0 = (const __half *)m.qs; a.w1 = m2 ? (const __half *)m2->qs : nullptr; a.x = x; a.out = out; a.rows = m.rows; a.cols = m.cols;
+    a.oscale = out_scale(p, MODE == SF_RESID, &m == &p->out);
     a.seg = L.seg; a.nseg = L.nseg; a.stages = L.stages; a.tr = tr;
     a.part_val = argmax ? p->part_val : nullptr;
     a.part_idx = argmax ? p->part_idx : nullptr;
@@ -565,6 +578,7 @@ int launch_stream(b200_plan *p, const TileMat &W, const int8_t *xq, const float 
     SmvSmem L = smv_layout(W.cols, W.seg, SMV_SMEM_BUDGET_MAX);
     SmvArgs a;
     a.W = W; a.xq = xq; a.xs = xs; a.out = out; a.hq = hq; a.hs = hs; a.blk_cnt = p->blk_cnt;
+    a.oscale = out_scale(p, MODE == SMV_RESID, &W == &p->tout);
     a.part_val = argmax ? p->part_val : nullptr;
     a.part_idx = argmax ? p->part_idx : nullptr;
     a.tr = tr;
@@ -596,7 +610,7 @@ int enqueue_moe_ffn(b200_plan *p, int l, TraceBuf tr) {
     const int E = p->moe.n_experts, k = p->moe.n_experts_used;
     int rc;
     if ((rc = launch_k(p, p->use_pdl, k_rmsnorm_quant<false>, dim3(1), dim3(NORM_THREADS), norm_smem_bytes(c.dim), p->x, (const StepState *)p->st, p->emb,
-                       (const float *)L.ffn_norm, c.rms_norm_eps, c.dim, p->xq, p->xs, p->xb, (long long *)nullptr, tr, p->tp, -1)))
+                       p->mup.embedding_scale, (const float *)L.ffn_norm, c.rms_norm_eps, c.dim, p->xq, p->xs, p->xb, (long long *)nullptr, tr, p->tp, -1)))
         return rc;
     int *ids = p->moe_ids + (size_t)l * k;
     float *w = p->moe_w + (size_t)l * (k + 1);
@@ -631,7 +645,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
     const int rank = p->tp.rank;
     auto norm = [&](bool embed, const float *w, int wait_op) {
         auto go = [&](auto kern) {
-            return launch_k(p, pdl, kern, dim3(1), dim3(NORM_THREADS), norm_smem, p->x, (const StepState *)p->st, p->emb, w, c.rms_norm_eps, c.dim, xq, xs, xbf, (long long *)nullptr, TR(1), p->tp, wait_op);
+            return launch_k(p, pdl, kern, dim3(1), dim3(NORM_THREADS), norm_smem, p->x, (const StepState *)p->st, p->emb, p->mup.embedding_scale, w, c.rms_norm_eps, c.dim, xq, xs, xbf, (long long *)nullptr, TR(1), p->tp, wait_op);
         };
         return embed ? go(k_rmsnorm_quant<true>) : go(k_rmsnorm_quant<false>);
     };
@@ -652,7 +666,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
             auto att = [&](auto kern) {
                 return launch_k(p, pdl, kern, dim3(p->nh_l), dim3(ATT_THREADS), att_smem, p->qkv, kc, vc, (const StepState *)p->st,
                                 (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags, (const float *)L.q_norm,
-                                (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, (float)sqrt((double)c.head_size), q8 ? p->attq : nullptr, q8 ? p->atts : nullptr, xbf, TR(4),
+                                (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, att_score_arg(p), q8 ? p->attq : nullptr, q8 ? p->atts : nullptr, xbf, TR(4),
                                 p->tp, (unsigned)(4 * l + 0), rank * p->nh_l, p->att_scratch, c.context_length);
             };
             if (c.head_size == 128) rc = att(k_attention<128>);
@@ -770,7 +784,8 @@ int enqueue_persistent(b200_plan *p, bool with_logits, int *launches, bool trace
     a.layers = p->pd_layers; a.n_layers = c.n_layers; a.lm_head = p->tout; a.out_norm = p->out_norm; a.emb = p->emb;
     a.dim = c.dim; a.hidden = c.hidden_dim; a.qd = p->qd; a.n_heads = p->nh_l; a.n_kv_heads = p->nkv_l;
     a.head_size = c.head_size; a.arch = p->kflags; a.ctx = c.context_length;
-    a.eps = c.rms_norm_eps; a.sqrt_hs = (float)sqrt((double)c.head_size);
+    a.eps = c.rms_norm_eps; a.sqrt_hs = att_score_arg(p);
+    a.emb_scale = p->mup.embedding_scale; a.res_scale = p->mup.residual_scale; a.logit_scale = p->mup.logit_scale;
     a.rope_cr = p->rope_cr; a.rope_ci = p->rope_ci;
     a.st = p->st; a.seq_tokens = p->seq_tokens; a.out_ids = p->out_ids;
     a.x = p->x; a.qkv = p->qkv; a.hb = p->hb; a.logits = p->logits;
@@ -860,6 +875,7 @@ int launch_stream_batch(b200_plan *p, const TileMat &W, int n, const int8_t *xq,
     const SmbSmem L = smb_layout(W.seg, n, SMB_SMEM_BUDGET);
     SmbArgs a;
     a.W = W; a.nrow = n; a.xq = xq; a.xs = xs; a.out = out; a.ostride = ostride; a.hq = hq; a.hs = hs; a.blk_cnt = p->bt.blk_cnt;
+    a.oscale = out_scale(p, MODE == SMV_RESID, &W == &p->tout);
     a.part_val = argmax ? p->bt.part_val : nullptr;
     a.part_idx = argmax ? p->bt.part_idx : nullptr;
     return launch_k(p, p->use_pdl, k_stream_matvec_q8_batch<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L);
@@ -878,7 +894,7 @@ int enqueue_batch(b200_plan *p, int n, int *launches) {
     int k = 0, rc;
     auto norm = [&](bool embed, const float *w) {
         auto go = [&](auto kern) {
-            return launch_k(p, pdl, kern, dim3(n), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
+            return launch_k(p, pdl, kern, dim3(n), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, p->mup.embedding_scale, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
         };
         k++;
         return embed ? go(k_rmsnorm_quant_batch<true>) : go(k_rmsnorm_quant_batch<false>);
@@ -891,7 +907,7 @@ int enqueue_batch(b200_plan *p, int n, int *launches) {
         auto att = [&](auto kern) {
             return launch_k(p, pdl, kern, dim3(p->nh_l, n), dim3(ATT_THREADS), att_smem_bytes(c.head_size, c.context_length, B.att_scratch != nullptr), B.qkv, qkvd,
                             kc, vc, slot_stride, (const BatchRows *)B.rows, (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags,
-                            (const float *)L.q_norm, (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, (float)sqrt((double)c.head_size), B.xq,
+                            (const float *)L.q_norm, (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, att_score_arg(p), B.xq,
                             B.xs, B.att_scratch, c.context_length, TraceBuf{nullptr, 0, 0}, solo);
         };
         if (c.head_size == 128) rc = att(k_attention_batch<128>);
@@ -1082,10 +1098,11 @@ int upload_moe_layer(b200_plan *p, const b200_tensor *tensors, int n_tensors, in
 
 int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     const b200_config &c = p->cfg;
-    if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3 && c.arch != B200_ARCH_QWEN2 && c.arch != B200_ARCH_QWEN2_MOE)
+    if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3 && c.arch != B200_ARCH_QWEN2 && c.arch != B200_ARCH_QWEN2_MOE &&
+        c.arch != B200_ARCH_GRANITE)
         return fail(p, B200_ERR_UNSUPPORTED, "unknown arch %d", c.arch);
     p->kflags = c.arch == B200_ARCH_QWEN3 ? (KF_NEOX | KF_QKNORM) : c.arch == B200_ARCH_PHI3 ? KF_NEOX
-              : (c.arch == B200_ARCH_QWEN2 || c.arch == B200_ARCH_QWEN2_MOE) ? (KF_NEOX | KF_QKVBIAS) : 0;
+              : (c.arch == B200_ARCH_QWEN2 || c.arch == B200_ARCH_QWEN2_MOE) ? (KF_NEOX | KF_QKVBIAS) : c.arch == B200_ARCH_GRANITE ? KF_ATTSCALE : 0;
     if (p->is_moe) {
         const b200_moe_config &m = p->moe;
         if (c.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "Qwen2-MoE plans are single-GPU (tensor parallelism has no expert layout)");
@@ -1143,7 +1160,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         const char *e = getenv("B200_STREAM");
         bool want = !(e && e[0] == '0');
         p->use_stream = want && p->wtype == B200_GGML_Q8_0 && stream_shape_ok(p->qd_l + 2 * p->kvd_l, c.dim) && stream_shape_ok(p->dim_l, p->qd) &&
-                        (p->is_moe || (stream_shape_ok(2 * p->hid_l, c.dim) && stream_shape_ok(p->dim_l, c.hidden_dim))) && stream_shape_ok(p->voc_l, c.dim) &&
+                        (p->is_moe || (stream_shape_ok(2 * p->hid_l, c.dim) && stream_shape_ok(p->dim_l, c.hidden_dim))) && stream_shape_ok((p->voc_l + 3) & ~3, c.dim) &&
                         gateup_fits(p->hid_l, p->n_sms);
         const char *e3 = getenv("B200_F16_STREAM"); // FP16 plans: 0 = the round-1 k_matvec_f16 launches
         p->use_f16_stream = !(e3 && e3[0] == '0') && p->wtype == B200_GGML_F16 && c.tp_size == 1 && sf_layout(p->qd + 2 * p->kvd, c.dim, c.fp16_lanes, false).ok &&
@@ -1533,7 +1550,8 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
     cudaStream_t s = p->stream;
     const int nqkv = p->qd + 2 * p->kvd, mt = (n + pg::BM - 1) / pg::BM, kv_mul = g.n_heads / g.n_kv_heads;
     const size_t ctx_kv = (size_t)g.context_length * p->kvd;
-    const float inv_sqrt_hs = (float)(1.0 / sqrt((double)g.head_size));
+    // k_pf_attention_mma scales q by this times log2(e): 1/sqrt(head size), or Granite's attentionScale
+    const float inv_sqrt_hs = (p->kflags & KF_ATTSCALE) ? p->mup.attention_scale : (float)(1.0 / sqrt((double)g.head_size));
     int nl = 0;
     constexpr int ST = pg::GEMM_STAGES;
     const bool q8 = c.mode == B200_PREFILL_TENSOR_CORE_W8A16; // B from the Q8_0 streams (c.maps_q8) instead of the f16 matrices (c.maps)
@@ -1547,7 +1565,7 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
         while (sp > 1 && (nk / sp < 8 || (sp - 1) * ((nk + sp - 1) / sp) >= nk)) sp--;
         return sp < 1 ? 1 : sp;
     };
-    k_pf_embed<<<n, 256, 0, s>>>(c.tok, p->emb, c.X, g.dim); nl++;
+    k_pf_embed<<<n, 256, 0, s>>>(c.tok, p->emb, p->mup.embedding_scale, c.X, g.dim); nl++;
     for (int l = 0; l < g.n_layers; l++) {
         const LayerW &L = p->layers[l];
         const PrefillLayerMaps *m = q8 ? nullptr : &c.maps[l];
@@ -1574,8 +1592,9 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
         }
         nl += 2;
         const int sp_wo = splits(g.dim / pg::BN, p->qd), sp_w2 = splits(g.dim / pg::BN, g.hidden_dim);
-        if (q8 ? pg::gemm_launch<pg::GEMM_RESID, ST, B_Q8>(c.mATT, mq->wo_q, mq->wo_s, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, sp_wo, L.two.seg)
-               : pg::gemm_launch<pg::GEMM_RESID, ST>(c.mATT, m->wo, m->wo, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, sp_wo))
+        const float rs = p->mup.residual_scale;
+        if (q8 ? pg::gemm_launch<pg::GEMM_RESID, ST, B_Q8>(c.mATT, mq->wo_q, mq->wo_s, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, sp_wo, L.two.seg, rs)
+               : pg::gemm_launch<pg::GEMM_RESID, ST>(c.mATT, m->wo, m->wo, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, sp_wo, 0, rs))
             return fail(p, B200_ERR_CUDA, "Wo GEMM launch failed");
         nl++;
         k_pf_rmsnorm_f16<<<n, 256, 0, s>>>(c.X, L.ffn_norm, g.rms_norm_eps, g.dim, c.A16); nl++;
@@ -1583,8 +1602,8 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
                : pg::gemm_launch<pg::GEMM_GATEUP, ST>(c.mA, m->w1, m->w3, c.mX, c.H16, g.hidden_dim, n, mt, g.hidden_dim / (pg::BN / 2), g.dim, s))
             return fail(p, B200_ERR_CUDA, "gate/up GEMM launch failed");
         nl++;
-        if (q8 ? pg::gemm_launch<pg::GEMM_RESID, ST, B_Q8>(c.mH, mq->w2_q, mq->w2_s, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, sp_w2, L.tw2.seg)
-               : pg::gemm_launch<pg::GEMM_RESID, ST>(c.mH, m->w2, m->w2, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, sp_w2))
+        if (q8 ? pg::gemm_launch<pg::GEMM_RESID, ST, B_Q8>(c.mH, mq->w2_q, mq->w2_s, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, sp_w2, L.tw2.seg, rs)
+               : pg::gemm_launch<pg::GEMM_RESID, ST>(c.mH, m->w2, m->w2, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, sp_w2, 0, rs))
             return fail(p, B200_ERR_CUDA, "W2 GEMM launch failed");
         nl++;
     }
@@ -1621,9 +1640,9 @@ int check_pos(b200_plan *p, int token, int pos) {
 
 } // namespace
 
-// b200_plan_create and b200_plan_create_moe (moe == nullptr: a dense plan)
-static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
-                       int32_t device, b200_plan **out, char *err, size_t err_len) {
+// b200_plan_create, b200_plan_create_moe and b200_plan_create_granite (moe / granite == nullptr: neither)
+static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const b200_granite_config *granite, const b200_tensor *tensors, int32_t n_tensors,
+                       int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len) {
     if (out) *out = nullptr;
     if (!cfg || !tensors || !out || n_tensors <= 0) {
         if (err && err_len) snprintf(err, err_len, "null argument");
@@ -1635,9 +1654,25 @@ static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const
                                        : "arch %d (B200_ARCH_QWEN2_MOE) needs its expert configuration: create the plan with b200_plan_create_moe", cfg->arch);
         return B200_ERR_BAD_ARG;
     }
+    if ((cfg->arch == B200_ARCH_GRANITE) != (granite != nullptr)) {
+        if (err && err_len)
+            snprintf(err, err_len, granite ? "b200_plan_create_granite needs arch B200_ARCH_GRANITE (got %d)"
+                                           : "arch %d (B200_ARCH_GRANITE) needs its scales: create the plan with b200_plan_create_granite", cfg->arch);
+        return B200_ERR_BAD_ARG;
+    }
+    if (granite) {
+        const float v[4] = {granite->embedding_scale, granite->residual_scale, granite->attention_scale, granite->logit_scale};
+        const char *names[4] = {"embedding_scale", "residual_scale", "attention_scale", "logit_scale"};
+        for (int i = 0; i < 4; i++)
+            if (!isfinite(v[i])) {
+                if (err && err_len) snprintf(err, err_len, "Granite %s is not finite (%g)", names[i], (double)v[i]);
+                return B200_ERR_BAD_ARG;
+            }
+    }
     b200_plan *p = new b200_plan();
     p->cfg = *cfg;
     if (moe) { p->is_moe = true; p->moe = *moe; }
+    if (granite) p->mup = *granite;
     if (p->cfg.tp_size <= 0) p->cfg.tp_size = 1;
     p->device = device;
     p->prefill_batch = prefill_batch_size;
@@ -1655,7 +1690,7 @@ extern "C" {
 
 int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
                      int32_t device, b200_plan **out, char *err, size_t err_len) {
-    return plan_create(cfg, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
+    return plan_create(cfg, nullptr, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
 }
 
 int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
@@ -1665,7 +1700,17 @@ int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, con
         if (err && err_len) snprintf(err, err_len, "null argument");
         return B200_ERR_BAD_ARG;
     }
-    return plan_create(cfg, moe, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
+    return plan_create(cfg, moe, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
+}
+
+int b200_plan_create_granite(const b200_config *cfg, const b200_granite_config *granite, const b200_tensor *tensors, int32_t n_tensors,
+                             int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len) {
+    if (!granite) {
+        if (out) *out = nullptr;
+        if (err && err_len) snprintf(err, err_len, "null argument");
+        return B200_ERR_BAD_ARG;
+    }
+    return plan_create(cfg, nullptr, granite, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
 }
 
 int b200_forward_decode(b200_plan *p, int32_t token, int32_t position, float *logits, int32_t *argmax) {
@@ -2188,7 +2233,7 @@ int b200_profile_norm(b200_plan *p, int64_t *cycles4) {
     const size_t norm_smem = norm_smem_bytes(c.dim);
     const bool q8 = p->wtype == B200_GGML_Q8_0;
     for (int i = 0; i < 3; i++)
-        k_rmsnorm_quant<false><<<1, NORM_THREADS, norm_smem, p->stream>>>(p->x, p->st, p->emb, p->layers[0].attn_norm, c.rms_norm_eps, c.dim,
+        k_rmsnorm_quant<false><<<1, NORM_THREADS, norm_smem, p->stream>>>(p->x, p->st, p->emb, 1.0f, p->layers[0].attn_norm, c.rms_norm_eps, c.dim,
                                                                  q8 ? p->xq : nullptr, q8 ? p->xs : nullptr, q8 ? nullptr : p->xb, d, TraceBuf{nullptr, 0, 0}, p->tp, -1);
     cudaError_t e = cudaStreamSynchronize(p->stream);
     long long h[6] = {0};

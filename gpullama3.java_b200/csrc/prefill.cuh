@@ -51,9 +51,9 @@ struct PrefillCtx {
 };
 
 // ---- elementwise kernels ------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_pf_embed(const int *__restrict__ tok, DevMat emb, float *__restrict__ X, int dim) {
+__global__ void __launch_bounds__(256) k_pf_embed(const int *__restrict__ tok, DevMat emb, float emb_scale, float *__restrict__ X, int dim) {
     const int b = blockIdx.x, token = tok[b];
-    for (int i = threadIdx.x; i < dim; i += 256) X[(size_t)b * dim + i] = emb_get(emb, token, i);
+    for (int i = threadIdx.x; i < dim; i += 256) X[(size_t)b * dim + i] = emb_get(emb, token, i, emb_scale);
 }
 
 __device__ __forceinline__ float pf_block_sum(float v, float *red) { // blockDim.x multiple of 32, <= 256

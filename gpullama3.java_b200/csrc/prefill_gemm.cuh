@@ -128,7 +128,8 @@ template <int STAGES, int BSRC = B_F16> constexpr size_t smem_bytes() {
 template <int MODE, int STAGES, int BSRC = B_F16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
                                                                  const __grid_constant__ CUtensorMap tma_b2, const __grid_constant__ CUtensorMap tma_c,
-                                                                 void *__restrict__ Cv, int ldc, int m_valid, int K, int kb_per_split, int seg) {
+                                                                 void *__restrict__ Cv, int ldc, int m_valid, int K, int kb_per_split, int seg,
+                                                                 float oscale) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023); // SWIZZLE_128B tiles need 1024-byte alignment
     constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, RAW_BYTES = BSRC == B_Q8 ? Q8_RAW_BYTES : 0;
@@ -265,7 +266,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid
         // TMA load has landed and been read) in the SWIZZLE_128B layout of the C tensor map: four 128 x 32 boxes, row r of
         // box b at b * 16 KB + 128 r, 16-byte chunk q at (q ^ (r & 7)) << 4.  Then ONE thread hands the boxes to TMA: a plain
         // tensor store (QKV) or an f32 reduce-add performed by the memory system (x += A W^T for Wo / W2 -- no
-        // read-modify-write through the SM, and split-K partials add up).  Rows past m_valid store / add 0.
+        // read-modify-write through the SM, and split-K partials add up).  Rows past m_valid store / add 0.  GEMM_RESID scales
+        // the tile by oscale first (Granite's residualScale: under split-K each partial is scaled, within the FP16 tolerance).
         asm volatile("bar.sync 1, 256;" ::: "memory");
 #pragma unroll
         for (int h = 0; h < 2; h++) {
@@ -274,7 +276,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid
 #pragma unroll
             for (int j = 0; j < 16; j++) {
                 const int col = 8 * j + cq, b = col >> 5, q = (col & 31) >> 2;
-                const float2 o = live ? make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]) : make_float2(0.0f, 0.0f);
+                float2 o = live ? make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]) : make_float2(0.0f, 0.0f);
+                if (MODE == GEMM_RESID) o = make_float2(__fmul_rn(o.x, oscale), __fmul_rn(o.y, oscale));
                 *reinterpret_cast<float2 *>(smem + b * (BM * 32 * 4) + rloc * 128 + ((q ^ (rloc & 7)) << 4) + (col & 3) * 4) = o;
             }
         }
@@ -366,7 +369,7 @@ static_assert(smem_bytes<GEMM_STAGES_DEEP_Q8, B_Q8>() <= 227 * 1024, "W8A16 deep
 // scale maps of one stream, seg its segment width (a multiple of BK, so no k-block straddles two segments).
 template <int MODE, int STAGES, int BSRC = B_F16>
 inline int gemm_launch(const CUtensorMap &a, const CUtensorMap &b, const CUtensorMap &b2, const CUtensorMap &c, void *C, int ldc, int m_valid, int m_tiles,
-                       int n_tiles, int K, cudaStream_t stream, int splits = 1, int seg = 0) {
+                       int n_tiles, int K, cudaStream_t stream, int splits = 1, int seg = 0, float oscale = 1.0f) {
     static bool attr = false; // one flag per instantiation
     if (!attr) {
         if (cudaFuncSetAttribute(k_gemm_f16_wgmma<MODE, STAGES, BSRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes<STAGES, BSRC>()) != cudaSuccess)
@@ -378,7 +381,7 @@ inline int gemm_launch(const CUtensorMap &a, const CUtensorMap &b, const CUtenso
     const int nk = (K + BK - 1) / BK, per = (nk + splits - 1) / splits;
     if ((splits - 1) * per >= nk) return -6; // an empty split would store an unwritten accumulator
     k_gemm_f16_wgmma<MODE, STAGES, BSRC><<<dim3(m_tiles, n_tiles, splits), GEMM_THREADS, smem_bytes<STAGES, BSRC>(), stream>>>(a, b, b2, c, C, ldc, m_valid, K,
-                                                                                                                          per, seg);
+                                                                                                                          per, seg, oscale);
     return cudaGetLastError() == cudaSuccess ? 0 : -5;
 }
 

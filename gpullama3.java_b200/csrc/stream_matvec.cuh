@@ -16,6 +16,8 @@
 //   tile(G, s)  = units (4G..4G+3, s) back to back   -> ONE bulk copy;
 //   tiles are stored in (G, s) order, so a CTA's slice [G0, G1) is one contiguous byte range.
 //   For the fused gate/up projection group G holds rows {gate 2G, gate 2G+1, up 2G, up 2G+1}.
+//   A classifier whose vocabulary is not a multiple of 4 is padded to whole groups with zero rows at upload; STORE never writes
+//   those rows and never offers them to the argmax (a padding row's 0 would beat real logits that are all negative).
 #pragma once
 #include "common.cuh"
 
@@ -28,7 +30,7 @@ enum { SMV_STORE = 0, SMV_RESID = 1, SMV_GATEUP = 2 };
 
 struct TileMat { // device weight matrix in tile-major layout
     const unsigned char *base;
-    int rows, cols;  // rows = 4 * groups (for gate/up: 2 * hidden)
+    int rows, cols;  // rows = 4 * groups (for gate/up: 2 * hidden); a classifier may end in a partial group (tile_groups)
     int seg, nseg;   // columns per segment, segments per row
     int unit_bytes;  // seg + seg/16 rounded up to 16
 };
@@ -39,6 +41,7 @@ __host__ __device__ inline int smv_pick_nseg(int cols) {
     return 0;
 }
 __host__ __device__ inline int smv_unit_bytes(int seg) { return (seg + seg / 16 + 15) & ~15; }
+__host__ __device__ inline int tile_groups(const TileMat &W) { return (W.rows + 3) >> 2; } // 4-row groups stored, the last one zero-padded
 
 struct SmvSmem {
     size_t off_bar, off_xq, off_xs, off_terms, off_hvals, off_ring, total;
@@ -148,7 +151,8 @@ struct SmvArgs {
     TileMat W;
     const int8_t *xq;   // pre-quantised activation [cols]
     const float *xs;    // its block scales [cols/32]
-    float *out;         // STORE: out[row] = r; RESID: out[row] += r; GATEUP: hb[unit] (float, also read back)
+    float *out;         // STORE: out[row] = r * oscale; RESID: out[row] += r * oscale; GATEUP: hb[unit] (float, also read back)
+    float oscale;       // STORE / RESID: Granite's logitScale (lm_head) / residualScale (Wo, W2), one rounding; 1.0f otherwise
     int8_t *hq;         // GATEUP: quantised hb
     float *hs;          // GATEUP: hb block scales
     unsigned *blk_cnt;  // GATEUP: per-32-block arrival counters (self-resetting)
@@ -171,7 +175,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8(SmvArgs a, 
     const TileMat W = a.W;
     const int S = L.stages;
     const unsigned bar0 = smem_u32(smem + L.off_bar); // full[s] at bar0 + 8s, empty[s] at bar0 + 8(S_MAX + s)
-    const int ngroups = W.rows >> 2;
+    const int ngroups = tile_groups(W);
     const int g0 = (int)(((long long)blockIdx.x * ngroups) / gridDim.x);
     const int g1 = (int)(((long long)(blockIdx.x + 1) * ngroups) / gridDim.x);
     const int nseg = W.nseg;
@@ -297,8 +301,9 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8(SmvArgs a, 
                     a.out[unit] = hval;
                     hvals[unit - 2 * g0] = hval;
                 }
-            } else if (lane < 4) {
+            } else if (lane < 4 && 4 * G + lane < W.rows) {
                 const size_t row = (size_t)4 * G + lane;
+                acc = __fmul_rn(acc, a.oscale); // xb2 * residualScale (InferenceCore.java:889-892,907-910) / logits * logitScale (:917-918)
                 if (MODE == SMV_RESID) {
                     if (a.tp.n > 1) { // all-gather of the residual stream: this rank's rows go to every rank
                         const size_t grow = (size_t)a.row_base + row;
@@ -393,7 +398,7 @@ struct RepackSrc {
     int gateup;                  // 1: raw[0] = gate, raw[1] = up, group G = {g 2G, g 2G+1, u 2G, u 2G+1}
 };
 
-__global__ void k_repack_tiles(RepackSrc src, unsigned char *dst, int rows, int cols, int seg, int nseg, int unit_bytes) {
+__global__ void k_repack_tiles(RepackSrc src, unsigned char *dst, int rows, int cols, int seg, int nseg, int unit_bytes) { // rows: real rows (the last group may be padding)
     // grid.x over (group, segment, slot) units; threads over 16-bit words of one unit
     const long long unit_id = blockIdx.x;
     const int r = (int)(unit_id % 4);
@@ -412,12 +417,14 @@ __global__ void k_repack_tiles(RepackSrc src, unsigned char *dst, int rows, int 
         row += src.row0[k];
     }
     const int nbs = seg / 32;
-    const unsigned char *blocks = raw + ((size_t)row * (cols / 32) + (size_t)s * nbs) * 34; // first source block of this unit
+    const bool pad = !src.gateup && 4 * G + r >= rows; // zero row completing the last group of a ragged classifier
+    const unsigned char *blocks = pad ? nullptr : raw + ((size_t)row * (cols / 32) + (size_t)s * nbs) * 34; // first source block of this unit
     unsigned char *u = dst + (size_t)unit_id * unit_bytes;
     const int words = unit_bytes / 2;
     for (int w = threadIdx.x; w < words; w += blockDim.x) {
         unsigned short v = 0;
-        if (w < seg / 2) { // quant payload: word w -> block w/16, word-in-block w%16
+        if (pad) { // stays 0
+        } else if (w < seg / 2) { // quant payload: word w -> block w/16, word-in-block w%16
             int b = w >> 4, k = w & 15;
             v = *reinterpret_cast<const unsigned short *>(blocks + (size_t)b * 34 + 2 + 2 * k);
         } else if (w < seg / 2 + nbs) {

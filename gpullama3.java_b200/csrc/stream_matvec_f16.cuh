@@ -19,6 +19,9 @@
 //   SF_GATEUP: half of the warp's row slots are ffn_gate rows, the other half the same rows of ffn_up; SwiGLU (InferenceCore.java:150-158)
 //   is applied in the epilogue, so w1, w3 and the SwiGLU kernel of the round-1 FP16 graph collapse into one launch.
 // PDL: the rings are filled before griddepcontrol.wait (weights are immutable); x, and out in SF_RESID, are touched only after it.
+// Ragged rows (SF_STORE / SF_RESID; in practice a classifier whose vocabulary is not a multiple of the warp's row slots): the slots
+// of the last group past the matrix re-read its last row, so no copy leaves the matrix (a tied classifier is the embedding table
+// itself), and they are never stored nor offered to the argmax.
 #pragma once
 #include "stream_matvec.cuh"
 
@@ -32,7 +35,8 @@ enum { SF_STORE = 0, SF_RESID = 1, SF_GATEUP = 2 };
 struct SfArgs {
     const __half *w0, *w1; // [rows][cols] row-major; w1 = ffn_up (SF_GATEUP only)
     const float *x;        // activation, cols floats
-    float *out;            // rows floats
+    float *out;            // rows floats: r * oscale (SF_STORE), out + r * oscale (SF_RESID)
+    float oscale;          // Granite's logitScale (classifier) / residualScale (Wo, W2), one rounding; 1.0f otherwise
     int rows, cols;        // of ONE matrix
     int seg, nseg;         // columns per stage, stages per row
     int stages;            // ring depth per warp
@@ -54,7 +58,7 @@ static inline SfLayout sf_layout(int rows, int cols, int lanes, bool gateup) {
     if (lanes != 8 && lanes != 16) return o;
     const int rw = 64 / lanes; // a lane owns two chains: L/2 lanes per row
     if (cols % 256 || cols < 256) return o;
-    if (gateup ? rows % (rw / 2) : rows % rw) return o;
+    if (gateup && rows % (rw / 2)) return o; // other matrices may end in a partial row group
     const size_t fixed = (size_t)cols * 4 + SF_WARPS * SF_MAX_STAGES * 8 + 256;
     const size_t per_sm = 220 * 1024;
     size_t best = 0;
@@ -100,7 +104,7 @@ __global__ void __launch_bounds__(SF_THREADS) k_stream_matvec_f16(SfArgs a) {
 
     // warp-interleaved assignment: group g belongs to global warp (g mod G); consecutive groups go to different SMs
     const int G = gridDim.x * SF_WARPS, gw = warp * gridDim.x + blockIdx.x;
-    const int ngroups = a.rows / MR;
+    const int ngroups = (a.rows + MR - 1) / MR;
     const int my_groups = gw < ngroups ? (ngroups - gw + G - 1) / G : 0;
     const int n_items = my_groups * nseg;
     const size_t row_bytes = (size_t)a.cols * 2;
@@ -114,7 +118,7 @@ __global__ void __launch_bounds__(SF_THREADS) k_stream_matvec_f16(SfArgs a) {
 #pragma unroll
         for (int r = 0; r < RW; r++) {
             const __half *m = (MODE == SF_GATEUP && r >= MR) ? a.w1 : a.w0;
-            const size_t row = row0 + (MODE == SF_GATEUP ? r % MR : r);
+            const size_t rr = row0 + (MODE == SF_GATEUP ? r % MR : r), row = rr < (size_t)a.rows ? rr : (size_t)a.rows - 1;
             bulk_g2s_evict_first(ring_u + st * stage_b + r * row_b, reinterpret_cast<const unsigned char *>(m) + row * row_bytes + (size_t)s * seg * 2,
                                  (unsigned)seg * 2u, bar, pol);
         }
@@ -164,7 +168,8 @@ __global__ void __launch_bounds__(SF_THREADS) k_stream_matvec_f16(SfArgs a) {
             if (MODE == SF_GATEUP) {
                 const float up = __shfl_sync(0xffffffffu, result, ((r + MR) % RW) * LPR);
                 if (r < MR && u == 0) a.out[row] = swiglu(result, up);
-            } else if (u == 0) {
+            } else if (u == 0 && row < (size_t)a.rows) {
+                result = __fmul_rn(result, a.oscale);
                 a.out[row] = MODE == SF_RESID ? __fadd_rn(a.out[row], result) : result; // x[i] = x[i] + xb2[i] (InferenceCore.java:143,164)
                 if (MODE == SF_STORE && result > best) { best = result; best_i = (int)row; }
             }

@@ -47,6 +47,10 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final StructLayout MOE_CONFIG = MemoryLayout.structLayout(
             JAVA_INT.withName("n_experts"), JAVA_INT.withName("n_experts_used"), JAVA_INT.withName("expert_hidden_dim"), JAVA_INT.withName("shared_hidden_dim"));
 
+    // struct b200_granite_config: 4 x float (Granite plans)
+    private static final StructLayout GRANITE_CONFIG = MemoryLayout.structLayout(
+            JAVA_FLOAT.withName("embedding_scale"), JAVA_FLOAT.withName("residual_scale"), JAVA_FLOAT.withName("attention_scale"), JAVA_FLOAT.withName("logit_scale"));
+
     private static MethodHandle fn(String name, FunctionDescriptor fd) {
         return LINKER.downcallHandle(LIB.find(name).orElseThrow(), fd);
     }
@@ -54,6 +58,8 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle CREATE = fn("b200_plan_create",
             FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS, JAVA_LONG));
     private static final MethodHandle CREATE_MOE = fn("b200_plan_create_moe",
+            FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS, JAVA_LONG));
+    private static final MethodHandle CREATE_GRANITE = fn("b200_plan_create_granite",
             FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS, JAVA_LONG));
     private static final MethodHandle DECODE = fn("b200_forward_decode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle PREFILL = fn("b200_forward_prefill", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
@@ -88,16 +94,23 @@ public final class B200MasterPlan implements AutoCloseable {
 
     /** One plan per GPU for tensor-parallel decode: every rank passes the same tensors, the library uploads its row slices. */
     public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int archId, int headSize, int tpRank, int tpSize) throws Throwable {
-        this(state, model, tensors, archId, headSize, tpRank, tpSize, null);
+        this(state, model, tensors, archId, headSize, tpRank, tpSize, null, null);
     }
 
     /** Qwen2-MoE (archId = ARCH_QWEN2_MOE, single GPU): moe = {numberOfExperts, numberOfExpertsUsed, moeHiddenDim, sharedExpertHiddenDim}
      *  (Qwen2MoEConfiguration); the router, shared-expert gate, stacked experts and shared expert go in `tensors` as in the file. */
     public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int headSize, int[] moe) throws Throwable {
-        this(state, model, tensors, ARCH_QWEN2_MOE, headSize, 0, 1, moe);
+        this(state, model, tensors, ARCH_QWEN2_MOE, headSize, 0, 1, moe, null);
     }
 
-    private B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int archId, int headSize, int tpRank, int tpSize, int[] moe) throws Throwable {
+    /** Granite (archId = ARCH_GRANITE): granite = {embeddingScale, residualScale, attentionScale, logitScale} (GraniteConfiguration);
+     *  Llama's tensors, tied classifier. */
+    public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int headSize, int tpRank, int tpSize, float[] granite) throws Throwable {
+        this(state, model, tensors, ARCH_GRANITE, headSize, tpRank, tpSize, null, granite);
+    }
+
+    private B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int archId, int headSize, int tpRank, int tpSize, int[] moe,
+                           float[] granite) throws Throwable {
         Configuration c = model.configuration();
         MemorySegment cfg = arena.allocate(CONFIG);
         int[] ints = {archId, c.dim(), c.hiddenDim(), c.numberOfLayers(), c.numberOfHeads(), c.numberOfKeyValueHeads(), headSize,
@@ -129,6 +142,10 @@ public final class B200MasterPlan implements AutoCloseable {
             MemorySegment mc = arena.allocate(MOE_CONFIG);
             for (int k = 0; k < 4; k++) mc.setAtIndex(JAVA_INT, k, moe[k]);
             rc = (int) CREATE_MOE.invokeExact(cfg, mc, arr, tensors.size(), batch, Integer.getInteger("b200.device", tpRank), out, err, 512L);
+        } else if (granite != null) {
+            MemorySegment gc = arena.allocate(GRANITE_CONFIG);
+            for (int k = 0; k < 4; k++) gc.setAtIndex(JAVA_FLOAT, k, granite[k]);
+            rc = (int) CREATE_GRANITE.invokeExact(cfg, gc, arr, tensors.size(), batch, Integer.getInteger("b200.device", tpRank), out, err, 512L);
         } else {
             rc = (int) CREATE.invokeExact(cfg, arr, tensors.size(), batch, Integer.getInteger("b200.device", tpRank), out, err, 512L);
         }
@@ -193,7 +210,7 @@ public final class B200MasterPlan implements AutoCloseable {
 
     public static final int PREFILL_EXACT = 0, PREFILL_TENSOR_CORE = 1, PREFILL_TENSOR_CORE_W8A16 = 2;
     // b200_config.arch (include/b200llama.h): Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen pass blk.N.attn_{q,k,v}.bias (F32) with the weights
-    public static final int ARCH_LLAMA = 0, ARCH_QWEN3 = 1, ARCH_PHI3 = 2, ARCH_QWEN2 = 3, ARCH_QWEN2_MOE = 4;
+    public static final int ARCH_LLAMA = 0, ARCH_QWEN3 = 1, ARCH_PHI3 = 2, ARCH_QWEN2 = 3, ARCH_QWEN2_MOE = 4, ARCH_GRANITE = 5;
 
     /** TensorCoreSupport.java's switch: 0 = exact token-by-token prefill (bit-identical KV cache), 1 = TMA + wgmma GEMMs (a Q8_0
      *  plan first builds f16 twins of its matrices, +2 bytes per weight), 2 = the same GEMMs on a Q8_0 plan reading the Q8_0 weights

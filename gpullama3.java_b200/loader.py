@@ -1,6 +1,6 @@
 """Host-side mirror of the reference model loaders (metadata -> Configuration, tensor names ->
 weight slots).  Mirrors ``model/loader/ModelLoader.java:47-108`` (type detection on
-``general.name``), ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74`` / ``Qwen2ModelLoader.java:48-73``
+``general.name``), ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74`` / ``Qwen2ModelLoader.java:48-73`` / ``GraniteLoader.java:48-92``
 (configuration keys), ``AbstractModelLoader.java:40-50`` (file_type -> quantisation) and
 ``AbstractModelLoader.java:186-195`` (tied output falls back to ``token_embd.weight``).
 Weights stay in GGUF block layout; the native library repacks at upload.
@@ -18,6 +18,10 @@ ARCH_QWEN3 = 1
 ARCH_PHI3 = 2
 ARCH_QWEN2 = 3  # Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen: Llama's forward + q/k/v biases, NeoX RoPE (InferenceCore.java:434-563)
 ARCH_QWEN2_MOE = 4  # Qwen1.5-MoE: Qwen2's attention + a routed mixture-of-experts FFN with a shared expert (InferenceCore.java:263-432)
+ARCH_GRANITE = 5  # Granite 3.x: Llama's forward with four muP scales (InferenceCore.forwardGranite, InferenceCore.java:814-921)
+
+# GraniteLoader.createConfiguration's defaults for the four scales (GraniteLoader.java:55-58)
+GRANITE_DEFAULT_SCALES = {"embedding_scale": 12.0, "residual_scale": 0.22, "attention_scale": 0.0078125, "logit_scale": 16.0}
 
 
 @dataclass
@@ -39,6 +43,11 @@ class Configuration:
     n_experts_used: int = 0
     expert_hidden_dim: int = 0
     shared_hidden_dim: int = 0
+    # Granite only (GraniteConfiguration); 1.0 for every other family
+    embedding_scale: float = 1.0
+    residual_scale: float = 1.0
+    attention_scale: float = 1.0
+    logit_scale: float = 1.0
 
     @property
     def q_dim(self):
@@ -97,7 +106,7 @@ class Model:
 
 def model_from_tensors(shape, quant: int, tensors: dict, context_length: int) -> Model:
     """In-memory model (bench: synthetic weights never touch the disk)."""
-    arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3, "qwen2": ARCH_QWEN2, "qwen2moe": ARCH_QWEN2_MOE}[shape.arch]
+    arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3, "qwen2": ARCH_QWEN2, "qwen2moe": ARCH_QWEN2_MOE, "granite": ARCH_GRANITE}[shape.arch]
     moe = shape.arch == "qwen2moe"
     cfg = Configuration(arch, "Q8_0" if quant == GGMLType.Q8_0 else "FP16",
                         shape.dim, 0 if moe else shape.hidden, shape.n_layers, shape.n_heads, shape.n_kv_heads, shape.head_size,
@@ -105,7 +114,10 @@ def model_from_tensors(shape, quant: int, tensors: dict, context_length: int) ->
     if moe:
         cfg.n_experts, cfg.n_experts_used = shape.n_experts, shape.n_experts_used
         cfg.expert_hidden_dim, cfg.shared_hidden_dim = shape.expert_hidden, shape.hidden
-    typ = {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3", "qwen2": "QWEN_2", "qwen2moe": "QWEN_2_MOE"}[shape.arch]
+    if shape.arch == "granite":
+        for k, v in shape.granite_scales.items():
+            setattr(cfg, k, float(np.float32(v)))
+    typ = {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3", "qwen2": "QWEN_2", "qwen2moe": "QWEN_2_MOE", "granite": "GRANITE"}[shape.arch]
     return Model(None, cfg, typ, tensors)
 
 
@@ -172,8 +184,10 @@ def load_model(path: str, context_length: int = -1) -> Model:
             float(md["qwen2.attention.layer_norm_rms_epsilon"]), float(md["qwen2.rope.freq_base"]))
     elif typ == "QWEN_2_MOE":
         cfg = _qwen2moe_configuration(md, g, q, context_length)
+    elif typ == "GRANITE":
+        cfg = granite_configuration(md, q, context_length)
     else:
-        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 / Qwen2-MoE forward passes only)")
+        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 / Qwen2-MoE / Granite forward passes only)")
     return Model(g, cfg, typ)
 
 
@@ -199,6 +213,36 @@ def _qwen2moe_configuration(md: dict, g: GGUFFile, q: str, context_length: int) 
         len(md["tokenizer.ggml.tokens"]), ctx, float(md["qwen2moe.attention.layer_norm_rms_epsilon"]), float(md["qwen2moe.rope.freq_base"]),
         n_experts=int(md["qwen2moe.expert_count"]), n_experts_used=int(md["qwen2moe.expert_used_count"]),
         expert_hidden_dim=expert_hidden, shared_hidden_dim=shared_hidden)
+
+
+def granite_configuration(md: dict, q: str, context_length: int) -> Configuration:
+    """GraniteLoader.createConfiguration (GraniteLoader.java:48-92): granite.* keys; the vocabulary size is granite.vocab_size, else the
+    token list's length; the four scales default to 12.0 / 0.22 / 0.0078125 / 16.0 (read as Java floats); head_count_kv is a scalar or a
+    per-layer array whose first element the reference takes -- a non-uniform array is refused here, because the reference would run
+    every layer with layer 0's count; eps defaults to 1e-5 and theta to 10000; the context is the requested one when >= 0
+    (GraniteConfiguration.withContextLength), else the model's; head size = dim / heads; the classifier is tied."""
+    n_heads = int(md["granite.attention.head_count"])
+    dim = int(md["granite.embedding_length"])
+    kv = md.get("granite.attention.head_count_kv", n_heads)
+    if isinstance(kv, (list, tuple, np.ndarray)):
+        kv = [int(v) for v in kv]
+        if not kv or any(v != kv[0] for v in kv):
+            raise UnsupportedModel(f"granite.attention.head_count_kv varies across layers ({kv}): the reference runs every layer with the "
+                                   "first layer's count, which would compute the other layers wrongly")
+        kv = kv[0]
+    vocab = md.get("granite.vocab_size")
+    if vocab is None:
+        vocab = len(md["tokenizer.ggml.tokens"])
+    model_ctx = int(md["granite.context_length"])
+    f = lambda key, default: float(np.float32(md.get(key, default)))  # (float) metadata.getOrDefault(key, <float literal>)
+    return Configuration(
+        ARCH_GRANITE, q, dim, int(md["granite.feed_forward_length"]), int(md["granite.block_count"]), n_heads, int(kv), dim // n_heads,
+        int(vocab), model_ctx if context_length < 0 else context_length, f("granite.attention.layer_norm_rms_epsilon", 1e-5),
+        f("granite.rope.freq_base", 10000.0),
+        embedding_scale=f("granite.embedding_scale", GRANITE_DEFAULT_SCALES["embedding_scale"]),
+        residual_scale=f("granite.residual_scale", GRANITE_DEFAULT_SCALES["residual_scale"]),
+        attention_scale=f("granite.attention.scale", GRANITE_DEFAULT_SCALES["attention_scale"]),
+        logit_scale=f("granite.logit_scale", GRANITE_DEFAULT_SCALES["logit_scale"]))
 
 
 def tensor_as_f32(model: Model, name: str) -> np.ndarray:

@@ -13,7 +13,7 @@ import os
 import numpy as np
 
 from . import native
-from .loader import Model
+from .loader import ARCH_GRANITE, Model
 
 
 def _flag(name: str, default: str) -> str:
@@ -82,10 +82,12 @@ class B200MasterPlan:
         if tp_size > 1:
             tp_shard_plan(model.configuration, tp_size)  # raises early on shapes that do not split
         c = model.configuration
-        moe = None
+        moe = granite = None
         if c.n_experts:  # Qwen2-MoE: b200_plan_create_moe
             moe = native.MoeConfig(c.n_experts, c.n_experts_used, c.expert_hidden_dim, c.shared_hidden_dim)
-        self._native = native.NativePlan(cfg, model.tensors, self.prefill_batch_size, device, moe=moe)
+        if c.arch == ARCH_GRANITE:  # Granite: b200_plan_create_granite
+            granite = native.GraniteConfig(c.embedding_scale, c.residual_scale, c.attention_scale, c.logit_scale)
+        self._native = native.NativePlan(cfg, model.tensors, self.prefill_batch_size, device, moe=moe, granite=granite)
         self.tp_rank, self.tp_size = tp_rank, tp_size
         if tp_size > 1:
             # one process per GPU: swap IPC handles of the communication buffers, then wire the peers

@@ -18,7 +18,7 @@ from .gguf import GGMLType, write_gguf
 
 @dataclass(frozen=True)
 class Shape:
-    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2" | "qwen2moe"
+    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2" | "qwen2moe" | "granite"
     dim: int
     hidden: int  # qwen2moe: the shared expert's hidden size
     n_layers: int
@@ -42,6 +42,11 @@ class Shape:
     def kv_dim(self):
         return self.n_kv_heads * self.head_size
 
+    @property
+    def granite_scales(self) -> dict:
+        """granite: the four muP scales the synthetic file carries (GRANITE_SCALES)."""
+        return GRANITE_SCALES if self.arch == "granite" else {}
+
     def matmul_elements(self) -> int:
         """Weight elements streamed per decoded token (SURVEY.md 8d)."""
         per_layer = 2 * self.q_dim * self.dim + 2 * self.kv_dim * self.dim + 3 * self.hidden * self.dim
@@ -52,6 +57,10 @@ class Shape:
         """Weight elements a prefill token multiplies (no lm_head: prefill skips logits)."""
         return self.matmul_elements() - self.vocab * self.dim
 
+
+# Synthetic Granite scales: embedding and residual scales of Granite 3.x's order, an attention multiplier well away from 1/sqrt(head size)
+# and a logit scale that is not a power of two, so every one of the four roundings is visible in the logits.
+GRANITE_SCALES = {"embedding_scale": 12.0, "residual_scale": 0.22, "attention_scale": 0.03, "logit_scale": 0.3}
 
 SHAPES = {
     # tiny parity shapes (oracle finishes in milliseconds)
@@ -100,6 +109,15 @@ SHAPES = {
     "tiny-qwen2moe-gqa": Shape("qwen2moe", 512, 512, 2, 8, 2, 64, 512, True, 1000000.0, 1e-6, 8192, 16, 8, 256),
     "mid-qwen1.5-moe-a2.7b": Shape("qwen2moe", 2048, 5632, 2, 16, 16, 128, 8192, False, 1000000.0, 1e-6, 8192, 60, 4, 1408),
     "qwen1.5-moe-a2.7b": Shape("qwen2moe", 2048, 5632, 24, 16, 16, 128, 151936, False, 1000000.0, 1e-6, 8192, 60, 4, 1408),
+    # Granite 3.x (muP scales, tied classifier): multi-head with head size 64 and an odd vocabulary, GQA with head size 128; 2-layer cuts
+    # of the Granite-3.x-2B and -8B layer geometries with their 49155-token vocabulary, and the whole 8B model (tools/granite_bench.py)
+    "tiny-granite": Shape("granite", 256, 512, 2, 4, 4, 64, 515, True, 10000.0, 1e-5, 4096),
+    "tiny-granite-gqa": Shape("granite", 1024, 1536, 2, 8, 2, 128, 512, True, 10000.0, 1e-5, 4096),
+    "mid-granite-3-2b": Shape("granite", 2048, 8192, 2, 32, 8, 64, 49155, True, 10000.0, 1e-5, 4096),
+    "mid-granite-3-8b": Shape("granite", 4096, 12800, 2, 32, 8, 128, 49155, True, 10000.0, 1e-5, 4096),
+    "granite-3-8b": Shape("granite", 4096, 12800, 40, 32, 8, 128, 49155, True, 10000.0, 1e-5, 4096),
+    # a Llama model whose vocabulary is not a multiple of 4: the streaming classifier's padding rows
+    "tiny-llama-vocab509": Shape("llama", 256, 512, 2, 4, 2, 64, 509, False, 500000.0, 1e-5),
 }
 
 
@@ -234,6 +252,12 @@ def metadata_for(shape: Shape, quant: int, name: str) -> dict:
         md["qwen2moe.expert_feed_forward_length"] = shape.expert_hidden
         md["qwen2moe.expert_shared_feed_forward_length"] = shape.hidden
         del md["qwen2moe.vocab_size"]  # the vocabulary size is the token list's
+    if a == "granite":  # GraniteLoader.createConfiguration
+        s = shape.granite_scales
+        md["granite.embedding_scale"] = float(s["embedding_scale"])
+        md["granite.residual_scale"] = float(s["residual_scale"])
+        md["granite.attention.scale"] = float(s["attention_scale"])
+        md["granite.logit_scale"] = float(s["logit_scale"])
     if shape.vocab <= 4096 or a in ("qwen2", "qwen2moe"):  # tokenizer section (Qwen2 takes its vocabulary size from the token list) (GGUF keys the loaders read: tokenizer.ggml.tokens / merges / token_type)
         tokens, merges, types, base = build_vocab(shape.vocab, a)
         md["tokenizer.ggml.model"] = "gpt2"
@@ -397,7 +421,7 @@ def write_model(path: str, shape_name: str, quant: int, seed: int = 1234, w_std:
                 display_name: str | None = None):
     shape = SHAPES[shape_name]
     name = display_name or {"llama": "Llama synthetic ", "qwen3": "Qwen3 synthetic ", "phi3": "Phi3 synthetic ", "qwen2": "Qwen2 synthetic ",
-                            "qwen2moe": "Qwen1.5 MoE synthetic "}[shape.arch] + shape_name
+                            "qwen2moe": "Qwen1.5 MoE synthetic ", "granite": "Granite synthetic "}[shape.arch] + shape_name
     write_gguf(path, metadata_for(shape, quant, name), build_tensors(shape, quant, seed, w_std))
     return shape
 

@@ -182,9 +182,11 @@ class UnsupportedTokenizer(Exception):
 
 def from_metadata(metadata: dict, model_type: str) -> Tokenizer:
     """ModelLoader: Vocabulary.loadLlamaVocabulary / loadQwen3Vocabulary + the tokenizer constructors."""
-    if model_type.upper() in ("MISTRAL", "DEVSTRAL_2", "PHI_3") or "tokenizer.ggml.merges" not in metadata:
+    if model_type.upper() in ("MISTRAL", "DEVSTRAL_2", "PHI_3", "GRANITE") or "tokenizer.ggml.merges" not in metadata:
         # MistralTokenizer / Phi3Tokenizer (tokenizer/MistralTokenizer.java, Phi3Tokenizer.java) are SentencePiece-style scorers, not the
-        # byte-level BPE implemented here: reject up front instead of mis-tokenising (the forward pass itself is supported).
+        # byte-level BPE implemented here; GraniteTokenizer is byte-level BPE with its own pre-tokenisation patterns (REFACT / DBRX, by
+        # tokenizer.ggml.pre), which the Llama-3 tokenizer would get wrong.  Reject up front instead of mis-tokenising (the forward
+        # pass itself is supported).
         raise UnsupportedTokenizer(f"no tokenizer for model type {model_type}: only the byte-level BPE vocabularies of Llama-3 and Qwen3 are "
                                    "implemented; drive the plan with token ids")
     tokens = list(metadata["tokenizer.ggml.tokens"])

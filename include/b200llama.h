@@ -45,6 +45,8 @@ extern "C" {
                            * norm; n_heads * head_size == dim.  Under tensor parallelism a rank reads the bias rows of its own heads. */
 #define B200_ARCH_QWEN2_MOE 4 /* InferenceCore.forwardJavaQwen2MoE, InferenceCore.java:263-432 (Qwen1.5-MoE-A2.7B): Qwen2's attention (q/k/v
                                * biases, NeoX RoPE) and a mixture-of-experts FFN.  Created with b200_plan_create_moe only. */
+#define B200_ARCH_GRANITE 5 /* InferenceCore.forwardGranite, InferenceCore.java:814-921 (Granite 3.x): Llama's tensors and forward with four
+                             * muP scalars (b200_granite_config).  Created with b200_plan_create_granite only. */
 
 /* GGML tensor type ids accepted for weights (tensor/GGMLType.java:5-20) */
 #define B200_GGML_F32 0
@@ -97,6 +99,17 @@ typedef struct b200_moe_config {
     int32_t shared_hidden_dim; /* ffn_gate_shexp dims[1] (Hs) */
 } b200_moe_config;
 
+/* The four scalars of a B200_ARCH_GRANITE plan (GraniteConfiguration).  Each is ONE float multiply, rounded once, where the CPU path
+ * makes it: the embedding row (x = emb[token] * embedding_scale), every attention score (q.k * attention_scale, in place of
+ * / sqrt(head_size)), both residual branches (x += (W*v) * residual_scale: Wo and W2) and the logits (logits * logit_scale, the
+ * greedy argmax taken on the scaled values).  The reference MULTIPLIES by logit_scale; see DESIGN.md section 10. */
+typedef struct b200_granite_config {
+    float embedding_scale; /* granite.embedding_scale, default 12.0 */
+    float residual_scale;  /* granite.residual_scale, default 0.22 */
+    float attention_scale; /* granite.attention.scale, default 0.0078125 */
+    float logit_scale;     /* granite.logit_scale, default 16.0 */
+} b200_granite_config;
+
 typedef struct b200_plan b200_plan;
 
 /* TornadoVMMasterPlan.initializeTornadoVMPlan(state, model) (TornadoVMMasterPlan.java:55-70)
@@ -126,6 +139,12 @@ int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t
  * the exact path only, and refuses b200_set_decode_slots (n_slots > 0) and b200_time_kernel with B200_ERR_UNSUPPORTED. */
 int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors,
                          int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
+
+/* b200_plan_create for cfg->arch == B200_ARCH_GRANITE (b200_plan_create refuses that arch with B200_ERR_BAD_ARG, and this call every
+ * other).  The tensors are Llama's (tied classifier: output.weight may be absent).  A scale that is not finite fails with
+ * B200_ERR_BAD_ARG and names the scale.  Every decode mode, weight format and prefill mode of a Llama plan is available. */
+int b200_plan_create_granite(const b200_config *cfg, const b200_granite_config *granite, const b200_tensor *tensors, int32_t n_tensors,
+                             int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
 
 /* TornadoVMMasterPlan.tornadoVMForwardDecode(position) with the embedding gather moved
  * device-side (replaces InferenceCore.forwardTornadoVM, InferenceCore.java:956-980, which copies

@@ -25,6 +25,7 @@
 //     host checks after the launch instead of hanging the GPU.
 #pragma once
 #include "decode_kernels.cuh"
+#include "norm_slots.cuh"
 #include "seqsum2.cuh"
 #include "stream_matvec.cuh"
 
@@ -115,7 +116,7 @@ __host__ __device__ inline PdSmem pd_layout(int dim, int qd, int hidden, int hea
     o = (o + 15) & ~(size_t)15;
     L.off_terms = o; o += (size_t)PD_WARPS * 4 * L.tstride * 4;
     L.off_hvals = o; o += SMV_HVALS * 4;
-    L.off_misc = o; o += 96 * 4; // red[16], s_val[2] @16, scale @20, argmax merge scratch @32 (16 floats) / @48 (16 ints)
+    L.off_misc = o; o += 96 * 4; // red[16], s_val[2] @16, norm scale @20, argmax merge scratch @32 (16 floats) / @48 (16 ints)
     o = (o + 127) & ~(size_t)127;
     L.off_ring = o;
     long room = (long)budget - (long)o;
@@ -452,13 +453,7 @@ __device__ __noinline__ void pd_consume_matrix(const TileMat &W, const PdArgs &a
     }
 }
 
-// ---- RMSNorm of the residual stream into THIS CTA's activation buffer (arithmetic of k_rmsnorm_quant) ----------------------
-__device__ __forceinline__ float4 pd_ldcg128(const float *p) {
-    float4 v;
-    asm volatile("ld.global.cg.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
-
+// ---- RMSNorm of the residual stream into THIS CTA's activation buffer (norm_slots.cuh) --------------------------------------
 // One out-of-line copy of the exact accumulator for every caller (attn norm, ffn norm, final norm, long softmax rows): the
 // kernel's code must stay inside the instruction cache, every cold fetch queues behind the weight stream.
 __device__ __noinline__ float pd_seqsum(const float *sq, int n, int S, unsigned char *smem, const PdSmem &L, int tid) {
@@ -475,84 +470,41 @@ __device__ __forceinline__ void pd_prefetch_w(const float *w, float *sbuf, int d
     asm volatile("cp.async.commit_group;" ::: "memory");
 }
 
-// Thread t owns the 16-byte slots i4 = u * PD_CT + t (u < U) of the vector: x and the norm weights stay in REGISTERS between
-// the two passes; a 32-element quantisation block is eight consecutive slots = eight consecutive lanes, so its amax is three
-// shuffles.  Only the squares go through shared memory (the exact accumulator's chunk layout).  wbuf: this norm's weights,
-// already on their way into shared memory (pd_prefetch_w).
+// What the persistent kernel plugs into norm_quant_slots: its 512 consumer threads, its out-of-line accumulator and embedding
+// lookup, and the norm weights that pd_prefetch_w is already bringing into wbuf (slot i4 by the thread that reads slot i4, so
+// that thread's own wait_group is all it needs).
+struct PdNormOps {
+    const PdArgs &a;
+    const float *wbuf;
+    unsigned char *smem;
+    const PdSmem &L;
+    int tid, stamp_layer;
+    __device__ __forceinline__ void sync() const { pd_bar_sync(); }
+    __device__ __forceinline__ float seqsum(const float *sq, int n, int S) const { return pd_seqsum(sq, n, S, smem, L, tid); }
+    __device__ __forceinline__ float emb(int token, int i) const { return pd_emb_get(a.emb, token, i, a.emb_scale); }
+    __device__ __forceinline__ float4 x4(int i4) const { return ldcg_f32x4(a.x + 4 * i4); }
+    __device__ __forceinline__ void store_x(int, float4) const {} // layer 0's Wo epilogue adds to the embedding row itself
+    __device__ __forceinline__ float scale(float ss, int dim, float eps) const {
+        float *misc = reinterpret_cast<float *>(smem + L.off_misc);
+        if (tid == 0) {
+            ss = __fdiv_rn(ss, (float)dim);
+            ss = __fadd_rn(ss, eps);
+            misc[20] = (float)(1.0 / sqrt((double)ss));
+        }
+        asm volatile("cp.async.wait_group 0;" ::: "memory"); // this thread's slots of the norm weights have landed
+        pd_bar_sync();
+        return misc[20];
+    }
+    template <int U> __device__ __forceinline__ float4 w4(const float4 (&)[U], int, int i4) const { return *reinterpret_cast<const float4 *>(wbuf + 4 * i4); }
+    __device__ __forceinline__ void stamp(int k) const { if (stamp_layer >= 0) pd_stamp(a, stamp_layer, k, tid); }
+};
+
+// wbuf: this norm's weights, already on their way into shared memory (pd_prefetch_w).
 template <int U>
 __device__ __noinline__ void pd_norm_u(const PdArgs &a, const float *wbuf, bool from_emb, int token, unsigned char *smem, const PdSmem &L, int tid, int stamp_layer) {
-    const int dim = a.dim, n4 = dim >> 2;
-    float *sq = reinterpret_cast<float *>(smem + L.off_nbuf);
-    float *misc = reinterpret_cast<float *>(smem + L.off_misc);
-    const int E = (dim + PD_CT - 1) / PD_CT, S = seqsum2_stride(E);
-    float4 xv[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) { // every load of this thread in flight at once: one L2 round trip
-        const int i4 = u * PD_CT + tid;
-        xv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (i4 < n4) {
-            if (from_emb) { // first layer: the embedding row (quantised table: element-wise, FloatTensor.copyTo)
-                xv[u] = make_float4(pd_emb_get(a.emb, token, 4 * i4, a.emb_scale), pd_emb_get(a.emb, token, 4 * i4 + 1, a.emb_scale),
-                                    pd_emb_get(a.emb, token, 4 * i4 + 2, a.emb_scale), pd_emb_get(a.emb, token, 4 * i4 + 3, a.emb_scale));
-            } else xv[u] = pd_ldcg128(a.x + 4 * i4);
-        }
-    }
-    // squares -> chunk layout: element i belongs to accumulator thread i / E at offset i % E of its S-float chunk
-    for (int i = dim + tid; i < PD_CT * E; i += PD_CT) sq[(i / E) * S + (i % E)] = 0.0f; // zero padding of the last chunks
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-        const int i4 = u * PD_CT + tid;
-        if (i4 < n4) {
-            const int i = 4 * i4;
-            const float4 q = make_float4(__fmul_rn(xv[u].x, xv[u].x), __fmul_rn(xv[u].y, xv[u].y), __fmul_rn(xv[u].z, xv[u].z), __fmul_rn(xv[u].w, xv[u].w));
-            if ((E & 3) == 0) *reinterpret_cast<float4 *>(sq + (i / E) * S + (i % E)) = q; // the four elements share a chunk
-            else {
-                sq[(i / E) * S + (i % E)] = q.x; sq[((i + 1) / E) * S + ((i + 1) % E)] = q.y;
-                sq[((i + 2) / E) * S + ((i + 2) % E)] = q.z; sq[((i + 3) / E) * S + ((i + 3) % E)] = q.w;
-            }
-        }
-    }
-    pd_bar_sync();
-    if (stamp_layer >= 0) pd_stamp(a, stamp_layer, 10, tid);
-    float ss = pd_seqsum(sq, dim, S, smem, L, tid);
-    if (stamp_layer >= 0) pd_stamp(a, stamp_layer, 11, tid);
-    if (tid == 0) {
-        ss = __fdiv_rn(ss, (float)dim);
-        ss = __fadd_rn(ss, a.eps);
-        misc[20] = (float)(1.0 / sqrt((double)ss));
-    }
-    asm volatile("cp.async.wait_group 0;" ::: "memory"); // this thread's slots of the norm weights have landed
-    pd_bar_sync();
-    ss = misc[20];
-    unsigned *sxq = reinterpret_cast<unsigned *>(smem + L.off_xq);
-    float *sxs = reinterpret_cast<float *>(smem + L.off_xs);
-#pragma unroll
-    for (int u = 0; u < U; u++) { // out = w * (ss * x) (InferenceCore.java:45-47), then Q8_0FloatTensor.java:100-117 per 32-block
-        const int i4 = u * PD_CT + tid;
-        if (u * PD_CT < n4) { // warp-uniform (n4 is a multiple of 8 and whole 8-lane groups are in or out)
-            float v0 = 0.f, v1 = 0.f, v2 = 0.f, v3 = 0.f;
-            if (i4 < n4) {
-                const float4 wv = *reinterpret_cast<const float4 *>(wbuf + 4 * i4);
-                v0 = __fmul_rn(wv.x, __fmul_rn(ss, xv[u].x)); v1 = __fmul_rn(wv.y, __fmul_rn(ss, xv[u].y));
-                v2 = __fmul_rn(wv.z, __fmul_rn(ss, xv[u].z)); v3 = __fmul_rn(wv.w, __fmul_rn(ss, xv[u].w));
-            }
-            float amax = fmaxf(fmaxf(fabsf(v0), fabsf(v1)), fmaxf(fabsf(v2), fabsf(v3)));
-            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
-            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
-            amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
-            const float qs = __fdiv_rn(amax, 127.0f);
-            const float ascale = __half2float(__float2half_rn(qs));
-            const float ainv = qs != 0.0f ? __fdiv_rn(1.0f, qs) : 0.0f;
-            const float s0 = __fmul_rn(v0, ainv), s1 = __fmul_rn(v1, ainv), s2 = __fmul_rn(v2, ainv), s3 = __fmul_rn(v3, ainv);
-            const int q0 = __float2int_rz(__fadd_rn(s0, copysignf(0.5f, s0))), q1 = __float2int_rz(__fadd_rn(s1, copysignf(0.5f, s1)));
-            const int q2 = __float2int_rz(__fadd_rn(s2, copysignf(0.5f, s2))), q3 = __float2int_rz(__fadd_rn(s3, copysignf(0.5f, s3)));
-            if (i4 < n4) {
-                sxq[i4] = (unsigned)(q0 & 0xff) | ((unsigned)(q1 & 0xff) << 8) | ((unsigned)(q2 & 0xff) << 16) | ((unsigned)(q3 & 0xff) << 24);
-                if ((tid & 7) == 0) sxs[i4 >> 3] = ascale;
-            }
-        }
-    }
-    pd_bar_sync();
+    const float4 wv[U] = {}; // unused: the weights are read from wbuf
+    norm_quant_slots<PD_CT, U>(PdNormOps{a, wbuf, smem, L, tid, stamp_layer}, from_emb, token, a.dim, a.eps, wv, reinterpret_cast<float *>(smem + L.off_nbuf),
+                               reinterpret_cast<unsigned *>(smem + L.off_xq), reinterpret_cast<float *>(smem + L.off_xs), tid);
 }
 
 // U = 16-byte slots per consumer thread = ceil(dim / (4 * PD_CT)): only the instantiation the model needs ever executes

@@ -76,6 +76,7 @@ struct b200_plan {
     DevMat emb{}, out{};
     TileMat tout{};
     bool use_stream = false, use_pdl = false;
+    bool fuse_norm = false; // single-GPU Q8_0 streams: QKV, gate/up and lm_head compute their RMSNorm themselves (k_stream_matvec_q8_norm)
     int kflags = 0; // KF_* (common.cuh): what the attention prologues do for this architecture
     size_t kq_off = 0; // K-quant files: offset of the raw (K-quant bytes) area inside each staging buffer; 0 = no K-quant tensor in the file
     bool use_f16_stream = false; // FP16 plans: per-warp bulk-copy rings (stream_matvec_f16.cuh) instead of k_matvec_f16
@@ -567,7 +568,7 @@ const size_t SMV_SMEM_BUDGET_MAX = 96 * 1024;
 // Read ONCE per plan (b200_plan_create), never inside a launch helper.
 void read_knobs(b200_plan *p) {
     const char *d = getenv("B200_DECODE");
-    // default: the CUDA graph, which every plan can run (on one H100 the persistent kernel measured ~5 % faster, DESIGN.md section 6).  B200_DECODE=persistent or b200_set_decode_mode select the one-kernel-per-token path.
+    // default: the CUDA graph, which every plan can run (on one H100, with the fused norm, it measured ~2.5 % faster than the persistent kernel for 8B Q8_0, DESIGN.md section 6).  B200_DECODE=persistent or b200_set_decode_mode select the one-kernel-per-token path.
     p->decode_mode = (d && !strcmp(d, "persistent")) ? B200_DECODE_PERSISTENT : B200_DECODE_GRAPH;
 }
 
@@ -585,6 +586,33 @@ int launch_stream(b200_plan *p, const TileMat &W, const int8_t *xq, const float 
     a.tp = p->tp;
     a.wait_slot = wait_slot; a.wait_op = wait_op; a.out_slot = out_slot; a.out_op = out_op; a.row_base = row_base;
     return launch_k(p, p->use_pdl, k_stream_matvec_q8<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L);
+}
+
+// A stream kernel behind a fused RMSNorm of the residual stream x (weights w; from_emb: layer 0, the embedding row, which CTA 0
+// also writes to x).  MODE is SMV_STORE (QKV, lm_head) or SMV_GATEUP.
+template <int MODE>
+int launch_stream_norm(b200_plan *p, const TileMat &W, const float *w, bool from_emb, float *out, int8_t *hq, float *hs, bool argmax, TraceBuf tr, int row_base = 0) {
+    SmvNormArgs n;
+    const SmvSmem L = smv_layout_norm(W.cols, W.seg, SMV_SMEM_BUDGET_MAX, &n.off_sq, &n.off_seq);
+    n.x = p->x; n.w = w; n.st = p->st; n.emb = p->emb; n.emb_scale = p->mup.embedding_scale; n.eps = p->cfg.rms_norm_eps;
+    n.from_emb = from_emb ? 1 : 0; n.x_out = p->x;
+    SmvArgs a;
+    a.W = W; a.xq = nullptr; a.xs = nullptr; a.out = out; a.hq = hq; a.hs = hs; a.blk_cnt = p->blk_cnt;
+    a.oscale = out_scale(p, false, &W == &p->tout);
+    a.part_val = argmax ? p->part_val : nullptr;
+    a.part_idx = argmax ? p->part_idx : nullptr;
+    a.tr = tr;
+    a.tp = p->tp;
+    a.wait_slot = -1; a.wait_op = 0; a.out_slot = -1; a.out_op = 0; a.row_base = row_base;
+    return launch_k(p, p->use_pdl, k_stream_matvec_q8_norm<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L, n);
+}
+
+// The fused norm needs 256 x ceil(dim / 256) squares and the accumulator's scratch next to the ring: at least 3 stages must remain.
+bool norm_fusion_ok(int dim) {
+    const int nseg = smv_pick_nseg(dim);
+    if (!nseg || dim % 32 || dim > 5 * 4 * 256) return false; // at most 5 slots of 16 bytes per consumer thread (registers)
+    unsigned a, b;
+    return smv_layout_norm(dim, dim / nseg, SMV_SMEM_BUDGET_MAX, &a, &b).stages >= 3;
 }
 
 bool stream_shape_ok(int rows, int cols) {
@@ -635,6 +663,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
     const bool q8 = p->wtype == B200_GGML_Q8_0;
     const bool st = p->use_stream, pdl = p->use_pdl, sf = p->use_f16_stream;
     const bool tpar = p->tp.n > 1;
+    const bool fz = p->fuse_norm; // attention / FFN / final norm inside QKV / gate-up / lm_head: 5 launches per layer instead of 7
     int n = 0;
     auto TR = [&](int id) { return TraceBuf{trace ? p->trace_rec : nullptr, n, id}; };
     const size_t norm_smem = norm_smem_bytes(c.dim);
@@ -653,12 +682,15 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
         LayerW &L = p->layers[l];
         int rc;
         // TP flag epochs inside one forward: op = 4*l + {0: attention out, 1: x after Wo, 2: hb, 3: x after W2}
-        if ((rc = norm(l == 0, L.attn_norm, l == 0 ? -1 : 4 * (l - 1) + 3))) return rc;
-        n++;
-        if (st) rc = launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr, false, TR(2));
-        else if (q8) rc = launch_matvec_q8<MODE_STORE>(p, L.qkv, p->xq, p->xs, p->qkv);
-        else if (sf) rc = launch_stream_f16<SF_STORE>(p, L.qkv, nullptr, p->xb, p->qkv, TR(2));
-        else rc = launch_matvec_f16<MODE_STORE>(p, L.qkv, p->xb, p->qkv);
+        if (fz) rc = launch_stream_norm<SMV_STORE>(p, L.tqkv, L.attn_norm, l == 0, p->qkv, nullptr, nullptr, false, TR(2)); // attention norm + QKV
+        else {
+            if ((rc = norm(l == 0, L.attn_norm, l == 0 ? -1 : 4 * (l - 1) + 3))) return rc;
+            n++;
+            if (st) rc = launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr, false, TR(2));
+            else if (q8) rc = launch_matvec_q8<MODE_STORE>(p, L.qkv, p->xq, p->xs, p->qkv);
+            else if (sf) rc = launch_stream_f16<SF_STORE>(p, L.qkv, nullptr, p->xb, p->qkv, TR(2));
+            else rc = launch_matvec_f16<MODE_STORE>(p, L.qkv, p->xb, p->qkv);
+        }
         if (rc) return rc; n++;
         float *kc = p->key_cache + (size_t)l * ctx_kv, *vc = p->value_cache + (size_t)l * ctx_kv;
         {
@@ -687,10 +719,14 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
             n += 4;
             continue;
         }
-        if ((rc = norm(false, L.ffn_norm, 4 * l + 1))) return rc;
-        n++;
+        if (!fz) {
+            if ((rc = norm(false, L.ffn_norm, 4 * l + 1))) return rc;
+            n++;
+        }
         if (st) {
-            if ((rc = launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs, false, TR(6), -1, 0, tpar ? TP_SLOT_HQ : -1, 4 * l + 2, rank * p->hid_l))) return rc; n++;
+            if (fz) rc = launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, TR(6)); // FFN norm + gate/up
+            else rc = launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs, false, TR(6), -1, 0, tpar ? TP_SLOT_HQ : -1, 4 * l + 2, rank * p->hid_l);
+            if (rc) return rc; n++;
             if ((rc = launch_stream<SMV_RESID>(p, L.tw2, p->hq, p->hs, p->x, nullptr, nullptr, false, TR(7), tpar ? TP_SLOT_HQ : -1, 4 * l + 2, tpar ? TP_SLOT_X : -1, 4 * l + 3, rank * p->dim_l))) return rc; n++;
         } else if (q8) {
             k_gateup_q8<<<c.hidden_dim / 32, 256, q8_smem_bytes(c.dim, 4, 8), p->stream>>>(
@@ -712,12 +748,15 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
     if (with_logits) {
         // rmsnorm(x, x, rms_final_weight) then wcls.matmul (InferenceCore.java:167-169)
         int rc;
-        if ((rc = norm(false, p->out_norm, last_x_op))) return rc;
-        n++;
-        if (st) rc = launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr, true, TR(8), -1, 0, -1, 0, rank * p->voc_l);
-        else if (q8) rc = launch_matvec_q8<MODE_STORE>(p, p->out, p->xq, p->xs, p->logits);
-        else if (sf) rc = launch_stream_f16<SF_STORE>(p, p->out, nullptr, p->xb, p->logits, TR(8), true);
-        else rc = launch_matvec_f16<MODE_STORE>(p, p->out, p->xb, p->logits);
+        if (fz) rc = launch_stream_norm<SMV_STORE>(p, p->tout, p->out_norm, false, p->logits, nullptr, nullptr, true, TR(8)); // final norm + lm_head
+        else {
+            if ((rc = norm(false, p->out_norm, last_x_op))) return rc;
+            n++;
+            if (st) rc = launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr, true, TR(8), -1, 0, -1, 0, rank * p->voc_l);
+            else if (q8) rc = launch_matvec_q8<MODE_STORE>(p, p->out, p->xq, p->xs, p->logits);
+            else if (sf) rc = launch_stream_f16<SF_STORE>(p, p->out, nullptr, p->xb, p->logits, TR(8), true);
+            else rc = launch_matvec_f16<MODE_STORE>(p, p->out, p->xb, p->logits);
+        }
         if (rc) return rc; n++;
     }
     {
@@ -1019,6 +1058,8 @@ int set_smem_attrs(b200_plan *p) {
     CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    CK(cudaFuncSetAttribute(k_stream_matvec_q8_norm<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    CK(cudaFuncSetAttribute(k_stream_matvec_q8_norm<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(set_max_dyn(k_matvec_f16<MODE_STORE>, maxdyn));
     CK(set_max_dyn(k_matvec_f16<MODE_RESID>, maxdyn));
     CK(set_max_dyn(k_stream_matvec_f16<16, SF_STORE>, maxdyn));
@@ -1177,6 +1218,9 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
             if (!p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "Qwen2-MoE needs the Q8_0 streaming layout (this plan would use the non-streaming matvecs)");
         }
         p->use_pdl = p->use_stream || p->use_f16_stream;
+        // Tensor parallelism keeps the separate norm: its read of x waits on every rank's slice (TP_SLOT_X).  So does Qwen2-MoE,
+        // whose FFN norm must write float xb for the F32 router anyway; its plans keep 8 launches per layer.
+        p->fuse_norm = p->use_stream && c.tp_size == 1 && !p->is_moe && norm_fusion_ok(c.dim);
         if (c.tp_size > 1 && !p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "tensor parallelism needs the Q8_0 streaming path");
     }
     size_t stage_bytes = (size_t)34 * (8u << 20); // 8 Mi blocks = 272 MiB
@@ -2089,12 +2133,26 @@ int b200_time_kernel(b200_plan *p, int32_t which, int32_t reps, float *avg_ms, i
             bool keep = p->use_pdl;
             p->use_pdl = false;
             int r;
+            const bool fz = p->fuse_norm;
+            const int64_t nw = fz ? (int64_t)c.dim * 4 : 0; // a fused norm also reads its weights (x: an L2 hit)
             switch (which) {
-            case 0: bytes = tb(L.tgu); r = launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs); break;
+            case 0:
+                bytes = tb(L.tgu) + nw;
+                r = fz ? launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, TraceBuf{nullptr, 0, 0})
+                       : launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs);
+                break;
             case 1: bytes = tb(L.tw2); r = launch_stream<SMV_RESID>(p, L.tw2, p->hq, p->hs, p->x, nullptr, nullptr); break;
-            case 2: bytes = tb(L.tqkv); r = launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr); break;
+            case 2:
+                bytes = tb(L.tqkv) + nw;
+                r = fz ? launch_stream_norm<SMV_STORE>(p, L.tqkv, L.attn_norm, false, p->qkv, nullptr, nullptr, false, TraceBuf{nullptr, 0, 0})
+                       : launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr);
+                break;
             case 3: bytes = tb(L.two); r = launch_stream<SMV_RESID>(p, L.two, p->xq, p->xs, p->x, nullptr, nullptr); break;
-            default: bytes = tb(p->tout); r = launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr); break;
+            default:
+                bytes = tb(p->tout) + nw;
+                r = fz ? launch_stream_norm<SMV_STORE>(p, p->tout, p->out_norm, false, p->logits, nullptr, nullptr, false, TraceBuf{nullptr, 0, 0})
+                       : launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr);
+                break;
             }
             p->use_pdl = keep;
             return r;

@@ -20,6 +20,8 @@
 //   those rows and never offers them to the argmax (a padding row's 0 would beat real logits that are all negative).
 #pragma once
 #include "common.cuh"
+#include "decode_kernels.cuh"
+#include "norm_slots.cuh"
 
 #define SMV_CONSUMER_WARPS 8
 #define SMV_THREADS ((SMV_CONSUMER_WARPS + 1) * 32)
@@ -106,6 +108,9 @@ __device__ __forceinline__ void bulk_g2s_evict_first(unsigned dst, const void *s
                  : "memory");
 }
 __device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(SMV_CONSUMER_WARPS * 32) : "memory"); }
+struct SmvConsumerSync {
+    __device__ __forceinline__ void operator()() const { consumer_bar_sync(); }
+};
 
 __device__ __forceinline__ float ldcg_f32(const float *p) {
     float v;
@@ -168,9 +173,88 @@ struct SmvArgs {
     int row_base;       // global index of this rank's first output row (RESID/STORE) or hidden unit (GATEUP)
 };
 
-template <int MODE>
-__global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8(SmvArgs a, SmvSmem L) {
-    extern __shared__ __align__(128) unsigned char smem[];
+// The normalising form (k_stream_matvec_q8_norm): the consumer warps compute RMSNorm(x) * w themselves, redundantly in every
+// CTA, straight into the shared-memory activation buffer (norm_slots.cuh), instead of copying the xq / xs a separate
+// k_rmsnorm_quant launch wrote.  That takes one dependent launch and one global round trip of the activation off the chain.
+struct SmvNormArgs {
+    const float *x;      // residual stream (read after the dependency wait)
+    const float *w;      // norm weights [cols] (immutable: fetched before it)
+    const StepState *st; // from_emb: the step's token
+    DevMat emb;
+    float emb_scale, eps;
+    int from_emb;        // layer 0: normalise the embedding row (emb_get: Granite's embedding scale applies) ...
+    float *x_out;        // ... and CTA 0 writes it to x (the first Wo epilogue adds to it)
+    unsigned off_sq, off_seq; // shared memory: the squares and the accumulator scratch (they alias the term buffer and hvals)
+};
+
+// Layout of the normalising form: the squares and the accumulator scratch of 256 threads are dead once the activation is in
+// shared memory, so they share their bytes with the term buffer and hvals (which are live only after it); what they need
+// beyond those comes out of the ring.
+__host__ inline SmvSmem smv_layout_norm(int cols, int seg, size_t budget, unsigned *off_sq, unsigned *off_seq) {
+    SmvSmem L = smv_layout(cols, seg, budget);
+    const size_t sq = (size_t)norm_slots_sq_floats(cols, SMV_CONSUMER_WARPS * 32) * 4;
+    const size_t nb = sq + seqsum2_scratch_bytes(SMV_CONSUMER_WARPS * 32);
+    *off_sq = (unsigned)L.off_terms;
+    *off_seq = (unsigned)(L.off_terms + sq); // sq is a multiple of 16 bytes
+    const size_t dead = L.off_ring - L.off_terms;
+    size_t o = L.off_terms + (nb > dead ? nb : dead);
+    o = (o + 127) & ~(size_t)127;
+    L.off_ring = o;
+    long room = (long)budget - (long)o;
+    int s = room > 0 ? (int)(room / L.stage_bytes) : 0;
+    if (s > SMV_MAX_STAGES) s = SMV_MAX_STAGES;
+    L.stages = s;
+    L.total = o + (size_t)s * L.stage_bytes;
+    return L;
+}
+
+__device__ __noinline__ float smv_seqsum(const float *sq, int n, int S, unsigned char *scratch, int tid) {
+    return block_seqsum_exact_v2_t<SMV_CONSUMER_WARPS * 32>(sq, n, seqsum2_carve(scratch, SMV_CONSUMER_WARPS * 32), tid, SmvConsumerSync(), S);
+}
+
+// What the stream kernel plugs into norm_quant_slots: the norm weights are already in registers (loaded before the dependency
+// wait), the embedding gather is emb_get, and at layer 0 CTA 0 writes the gathered row back to x.
+struct SmvNormOps {
+    const SmvNormArgs &n;
+    unsigned char *smem;
+    int tid;
+    bool write_x;
+    __device__ __forceinline__ void sync() const { consumer_bar_sync(); }
+    __device__ __forceinline__ float seqsum(const float *sq, int cnt, int S) const { return smv_seqsum(sq, cnt, S, smem + n.off_seq, tid); }
+    __device__ __forceinline__ float emb(int token, int i) const { return emb_get(n.emb, token, i, n.emb_scale); }
+    __device__ __forceinline__ float4 x4(int i4) const { return ldcg_f32x4(n.x + 4 * i4); }
+    __device__ __forceinline__ void store_x(int i4, float4 v) const {
+        if (write_x) *reinterpret_cast<float4 *>(n.x_out + 4 * i4) = v;
+    }
+    __device__ __forceinline__ float scale(float ss, int dim, float eps) const { // every thread: no broadcast, no barrier
+        ss = __fdiv_rn(ss, (float)dim);
+        ss = __fadd_rn(ss, eps);
+        return (float)(1.0 / sqrt((double)ss));
+    }
+    template <int U> __device__ __forceinline__ float4 w4(const float4 (&wv)[U], int u, int) const { return wv[u]; }
+    __device__ __forceinline__ void stamp(int) const {}
+};
+
+// U = 16-byte slots per consumer thread; weights first (before the wait), then the norm.
+template <int U>
+__device__ __forceinline__ void smv_norm_prologue(const SmvNormArgs &n, int cols, unsigned char *smem, size_t off_xq, size_t off_xs, int tid, const TraceBuf &tr) {
+    constexpr int T = SMV_CONSUMER_WARPS * 32;
+    const int n4 = cols >> 2;
+    float4 wv[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        const int i4 = u * T + tid;
+        wv[u] = i4 < n4 ? __ldg(reinterpret_cast<const float4 *>(n.w) + i4) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    pdl_wait(); // x (and the token) come from the previous kernel
+    trace_mark(tr, 2);
+    const int token = n.from_emb ? n.st->token : 0;
+    norm_quant_slots<T, U>(SmvNormOps{n, smem, tid, n.from_emb && blockIdx.x == 0}, n.from_emb != 0, token, cols, n.eps, wv,
+                           reinterpret_cast<float *>(smem + n.off_sq), reinterpret_cast<unsigned *>(smem + off_xq), reinterpret_cast<float *>(smem + off_xs), tid);
+}
+
+template <int MODE, bool NORM>
+__device__ __forceinline__ void smv_q8_body(const SmvArgs &a, const SmvSmem &L, const SmvNormArgs &na, unsigned char *smem) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const TileMat W = a.W;
     const int S = L.stages;
@@ -221,21 +305,29 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8(SmvArgs a, 
     }
 
     // ===== consumers =====
-    pdl_wait(); // activations come from the previous kernel
-    trace_mark(a.tr, 2);
-    if (a.tp.n > 1 && a.wait_slot >= 0) { // ... and, under TP, from every rank
-        if (tid == 0) tp_wait(a.tp, a.wait_slot, tp_seq(a.tp, a.wait_op));
+    if (NORM) { // single GPU only: x needs no cross-rank wait
+        const int U = ((W.cols >> 2) + SMV_CONSUMER_WARPS * 32 - 1) / (SMV_CONSUMER_WARPS * 32); // only the instantiation the model needs executes
+        if (U <= 1) smv_norm_prologue<1>(na, W.cols, smem, L.off_xq, L.off_xs, tid, a.tr);
+        else if (U == 2) smv_norm_prologue<2>(na, W.cols, smem, L.off_xq, L.off_xs, tid, a.tr);
+        else if (U <= 4) smv_norm_prologue<4>(na, W.cols, smem, L.off_xq, L.off_xs, tid, a.tr);
+        else smv_norm_prologue<5>(na, W.cols, smem, L.off_xq, L.off_xs, tid, a.tr); // cols <= 5120 (norm_fusion_ok)
+    } else {
+        pdl_wait(); // activations come from the previous kernel
+        trace_mark(a.tr, 2);
+        if (a.tp.n > 1 && a.wait_slot >= 0) { // ... and, under TP, from every rank
+            if (tid == 0) tp_wait(a.tp, a.wait_slot, tp_seq(a.tp, a.wait_op));
+            consumer_bar_sync();
+        }
+        {
+            const int nb = W.cols >> 5;
+            int4 *sxq = reinterpret_cast<int4 *>(smem + L.off_xq);
+            float *sxs = reinterpret_cast<float *>(smem + L.off_xs);
+            const int4 *src = reinterpret_cast<const int4 *>(a.xq);
+            for (int c = tid; c < W.cols / 16; c += SMV_CONSUMER_WARPS * 32) sxq[c] = __ldcg(src + c);
+            for (int b = tid; b < nb; b += SMV_CONSUMER_WARPS * 32) sxs[b] = __ldcg(a.xs + b);
+        }
         consumer_bar_sync();
     }
-    {
-        const int nb = W.cols >> 5;
-        int4 *sxq = reinterpret_cast<int4 *>(smem + L.off_xq);
-        float *sxs = reinterpret_cast<float *>(smem + L.off_xs);
-        const int4 *src = reinterpret_cast<const int4 *>(a.xq);
-        for (int c = tid; c < W.cols / 16; c += SMV_CONSUMER_WARPS * 32) sxq[c] = __ldcg(src + c);
-        for (int b = tid; b < nb; b += SMV_CONSUMER_WARPS * 32) sxs[b] = __ldcg(a.xs + b);
-    }
-    consumer_bar_sync();
 
     const int nbs = W.seg >> 5; // blocks per segment
     float *terms = reinterpret_cast<float *>(smem + L.off_terms) + (size_t)warp * 4 * L.nbs_pad;
@@ -386,6 +478,22 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8(SmvArgs a, 
         if (tid == 0) tp_cta_done(a.tp, a.out_slot, tp_seq(a.tp, a.out_op), gridDim.x); // only the LAST CTA pays the system-scope fence
     }
     trace_mark(a.tr, 3);
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8(SmvArgs a, SmvSmem L) {
+    extern __shared__ __align__(128) unsigned char smem[]; // declared in the kernel: the alignment must not reach other kernels' dynamic smem
+    smv_q8_body<MODE, false>(a, L, SmvNormArgs{}, smem);
+}
+
+// STORE (QKV, lm_head) and GATEUP behind a fused RMSNorm; L from smv_layout_norm.  At most 96 registers, as the plain form uses:
+// with the 114 the compiler would pick, the next stream kernel's CTA no longer fits beside this one under PDL (it measured resident
+// ~5 us before its dependency instead of ~65, so its ring starts empty).
+template <int MODE>
+__global__ void __maxnreg__(96) k_stream_matvec_q8_norm(SmvArgs a, SmvSmem L, SmvNormArgs n) {
+    static_assert(MODE != SMV_RESID, "a residual matvec consumes an activation, not the residual stream");
+    extern __shared__ __align__(128) unsigned char smem[];
+    smv_q8_body<MODE, true>(a, L, n, smem);
 }
 
 // ---- upload-time repack: GGUF Q8_0 blocks (34 B: f16 scale + 32 int8) -> tile-major -----------

@@ -20,6 +20,17 @@ struct BatchRows {
     int slot[SMB_MAX_ROWS];
 };
 
+// Exact multi-slot prefill (b200_prefill_slots): the first node of each step's graph copies entry *step of the schedule uploaded
+// with the call into rows and advances *step, so the steps of one call are enqueued back to back with no host round trip.
+__global__ void __launch_bounds__(32) k_batch_rows_next(const BatchRows *__restrict__ sched, int *step, BatchRows *__restrict__ rows) {
+    const int s = *step;
+    const int *src = reinterpret_cast<const int *>(sched + s);
+    int *dst = reinterpret_cast<int *>(rows);
+    for (int i = threadIdx.x; i < (int)(sizeof(BatchRows) / 4); i += 32) dst[i] = src[i];
+    __syncwarp();
+    if (threadIdx.x == 0) *step = s + 1;
+}
+
 // The norm and attention kernels take the (unused: tr.rec == nullptr, tp.n == 1) trace and tensor-parallel contexts as kernel
 // parameters, as the single-row kernels do: a zero-initialised local copy would be placed in local memory.
 

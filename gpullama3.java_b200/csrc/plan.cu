@@ -160,6 +160,12 @@ struct b200_plan {
         int *h_out = nullptr;                         // pinned: ids [SMB_MAX_ROWS] then sampler outputs [SMB_MAX_ROWS][8]
         cudaGraphExec_t g[SMB_MAX_ROWS + 1] = {};
         int launches[SMB_MAX_ROWS + 1] = {};
+        // exact b200_prefill_slots: the per-step rows of the call [context_length], the device step index, the step graphs without the
+        // classifier (one per row count)
+        BatchRows *sched = nullptr;
+        int *step = nullptr;
+        cudaGraphExec_t gp[SMB_MAX_ROWS + 1] = {};
+        int launches_p[SMB_MAX_ROWS + 1] = {};
         int last_n = 0;
         float last_ms = 0.f;
     } bt;
@@ -920,8 +926,9 @@ int launch_stream_batch(b200_plan *p, const TileMat &W, int n, const int8_t *xq,
     return launch_k(p, p->use_pdl, k_stream_matvec_q8_batch<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L);
 }
 
-// One forward step of n rows: the single-sequence graph's kernel sequence, every launch serving all n rows.
-int enqueue_batch(b200_plan *p, int n, int *launches) {
+// One forward step of n rows: the single-sequence graph's kernel sequence, every launch serving all n rows.  prefill: a step of
+// b200_prefill_slots -- the rows come from the call's schedule (k_batch_rows_next) and there is no final norm, lm_head or argmax.
+int enqueue_batch(b200_plan *p, int n, int *launches, bool prefill = false) {
     const b200_config &c = p->cfg;
     auto &B = p->bt;
     const bool pdl = p->use_pdl;
@@ -931,9 +938,14 @@ int enqueue_batch(b200_plan *p, int n, int *launches) {
     TpCtx solo{};
     solo.n = 1;
     int k = 0, rc;
+    if (prefill) {
+        k_batch_rows_next<<<1, 32, 0, p->stream>>>(B.sched, B.step, B.rows);
+        CK(cudaGetLastError());
+        k++;
+    }
     auto norm = [&](bool embed, const float *w) {
-        auto go = [&](auto kern) {
-            return launch_k(p, pdl, kern, dim3(n), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, p->mup.embedding_scale, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
+        auto go = [&](auto kern) { // the first norm of a prefill step waits for k_batch_rows_next in full: the rows are read before any PDL wait
+            return launch_k(p, pdl && !(prefill && embed), kern, dim3(n), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, p->mup.embedding_scale, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
         };
         k++;
         return embed ? go(k_rmsnorm_quant_batch<true>) : go(k_rmsnorm_quant_batch<false>);
@@ -961,6 +973,10 @@ int enqueue_batch(b200_plan *p, int n, int *launches) {
         if ((rc = launch_stream_batch<SMV_RESID>(p, L.tw2, n, B.hq, B.hs, B.x, c.dim))) return rc;
         k += 5;
     }
+    if (prefill) {
+        if (launches) *launches = k;
+        return B200_OK;
+    }
     if ((rc = norm(false, p->out_norm))) return rc;
     if ((rc = launch_stream_batch<SMV_STORE>(p, p->tout, n, B.xq, B.xs, B.logits, sampler_padded(c.vocab_size), nullptr, nullptr, true))) return rc;
     if ((rc = launch_k(p, pdl, k_argmax_batch, dim3(n), dim3(32), (size_t)0, (const float *)B.part_val, (const int *)B.part_idx, p->n_sms, B.ids))) return rc;
@@ -968,14 +984,14 @@ int enqueue_batch(b200_plan *p, int n, int *launches) {
     return B200_OK;
 }
 
-int capture_batch(b200_plan *p, int n) {
+int capture_batch(b200_plan *p, int n, bool prefill = false) {
     cudaGraph_t g = nullptr;
     CK(cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal));
-    int rc = enqueue_batch(p, n, &p->bt.launches[n]);
+    int rc = enqueue_batch(p, n, prefill ? &p->bt.launches_p[n] : &p->bt.launches[n], prefill);
     cudaError_t e = cudaStreamEndCapture(p->stream, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
     if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(e));
-    e = cudaGraphInstantiate(&p->bt.g[n], g, 0);
+    e = cudaGraphInstantiate(prefill ? &p->bt.gp[n] : &p->bt.g[n], g, 0);
     cudaGraphDestroy(g);
     if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e));
     return B200_OK;
@@ -984,6 +1000,8 @@ int capture_batch(b200_plan *p, int n) {
 void batch_free(b200_plan *p) {
     auto &B = p->bt;
     for (cudaGraphExec_t &g : B.g)
+        if (g) { cudaGraphExecDestroy(g); g = nullptr; }
+    for (cudaGraphExec_t &g : B.gp)
         if (g) { cudaGraphExecDestroy(g); g = nullptr; }
     for (void *d : B.allocs) cudaFree(d);
     if (B.h_rows) cudaFreeHost(B.h_rows);
@@ -1011,7 +1029,8 @@ int batch_alloc(b200_plan *p, int ns) {
         (rc = balloc(p, &B.logits, N * sampler_padded(c.vocab_size) * 4)) || (rc = balloc(p, &B.xq, N * big)) || (rc = balloc(p, &B.xs, N * (big / 32) * 4)) ||
         (rc = balloc(p, &B.hq, N * c.hidden_dim)) || (rc = balloc(p, &B.hs, N * (c.hidden_dim / 32) * 4)) ||
         (rc = balloc(p, &B.part_val, N * p->n_sms * 4)) || (rc = balloc(p, &B.part_idx, N * p->n_sms * 4)) || (rc = balloc(p, &B.ids, N * 4)) ||
-        (rc = balloc(p, &B.smp_out, N * 8 * 4)) || (rc = balloc(p, &B.blk_cnt, N * (c.hidden_dim / 32) * 4)) || (rc = balloc(p, &B.rows, sizeof(BatchRows))))
+        (rc = balloc(p, &B.smp_out, N * 8 * 4)) || (rc = balloc(p, &B.blk_cnt, N * (c.hidden_dim / 32) * 4)) || (rc = balloc(p, &B.rows, sizeof(BatchRows))) ||
+        (rc = balloc(p, &B.sched, (size_t)c.context_length * sizeof(BatchRows))) || (rc = balloc(p, &B.step, 4)))
         return rc;
     if (p->att_scratch && (rc = balloc(p, &B.att_scratch, N * p->nh_l * c.context_length * 4))) return rc;
     CK(cudaMallocHost(&B.h_rows, sizeof(BatchRows)));
@@ -1487,8 +1506,10 @@ static int prefill_scratch(b200_plan *p, bool *ok) {
           pg::make_map_c(&c.mQKV, c.QKV, c.bpad, nqkv) == 0;
     if (g.head_size == 128) {
         CK(cudaFuncSetAttribute(k_pf_attention_mma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>()));
+        CK(cudaFuncSetAttribute(k_pf_attention_mma_packed<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>()));
     } else {
         CK(cudaFuncSetAttribute(k_pf_attention_mma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<64>()));
+        CK(cudaFuncSetAttribute(k_pf_attention_mma_packed<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<64>()));
     }
     return B200_OK;
 }
@@ -1587,8 +1608,19 @@ int build_f16_twins(b200_plan *p) {
     return B200_OK;
 }
 
-// n tokens already in c.tok (device), positions start_pos .. start_pos + n - 1
-int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
+// A packed chunk of b200_prefill_slots: the device tables of prefill.cuh and the f16 scratch the sequences' regions live in
+struct PfPacked {
+    const PfTok *tok;
+    const PfTile *tiles;
+    int n_tiles;
+    const PfHist *hist; // sequences with start > 0
+    int n_hist, max_start;
+    __half *KH, *VH;
+};
+
+// n tokens already in c.tok (device), positions start_pos .. start_pos + n - 1 of the plan's cache; or, with pk, the packed
+// tokens of several sequences, each written to its own decode slot (start_pos unused)
+int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfPacked *pk = nullptr) {
     PrefillCtx &c = p->prefill;
     const b200_config &g = p->cfg;
     cudaStream_t s = p->stream;
@@ -1614,25 +1646,43 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches) {
         const LayerW &L = p->layers[l];
         const PrefillLayerMaps *m = q8 ? nullptr : &c.maps[l];
         const PrefillQ8Maps *mq = q8 ? &c.maps_q8[l] : nullptr;
-        float *kc = p->key_cache + (size_t)l * ctx_kv, *vc = p->value_cache + (size_t)l * ctx_kv;
+        float *kc = (pk ? p->bt.slot_k : p->key_cache) + (size_t)l * ctx_kv, *vc = (pk ? p->bt.slot_v : p->value_cache) + (size_t)l * ctx_kv;
         k_pf_rmsnorm_f16<<<n, 256, 0, s>>>(c.X, L.attn_norm, g.rms_norm_eps, g.dim, c.A16); nl++;
         if (q8 ? pg::gemm_launch<pg::GEMM_F32, ST, B_Q8>(c.mA, mq->qkv_q, mq->qkv_s, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s, 1, L.tqkv.seg)
                : pg::gemm_launch<pg::GEMM_F32, ST>(c.mA, m->qkv, m->qkv, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s))
             return fail(p, B200_ERR_CUDA, "QKV GEMM launch failed");
         nl++;
         const int qt = PM_ROWS / kv_mul;
-        const dim3 ag((n + qt - 1) / qt, g.n_kv_heads);
-        if (start_pos > 0) { // rows written by earlier chunks / decode steps
-            const size_t n4 = (size_t)start_pos * p->kvd / 4;
-            k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, s>>>(kc, vc, c.KH, c.VH, n4);
-            nl++;
-        }
-        if (g.head_size == 128) {
-            k_pf_rope_kv<128><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
-            k_pf_attention_mma<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
+        if (pk) {
+            const size_t slot_stride = (size_t)g.n_layers * ctx_kv;
+            if (pk->n_hist) {
+                const size_t n4 = (size_t)pk->max_start * p->kvd / 4;
+                const dim3 hg((unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), pk->n_hist);
+                k_pf_kv_to_f16_packed<<<hg, 256, 0, s>>>(kc, vc, slot_stride, pk->KH, pk->VH, p->kvd, pk->hist);
+                nl++;
+            }
+            const dim3 ag(pk->n_tiles, g.n_kv_heads);
+            if (g.head_size == 128) {
+                k_pf_rope_kv_packed<128><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, slot_stride, pk->KH, pk->VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, pk->tok);
+                k_pf_attention_mma_packed<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), s>>>(c.QKV, nqkv, pk->KH, pk->VH, p->kvd, kv_mul, pk->tiles, inv_sqrt_hs, c.ATT16, p->qd);
+            } else {
+                k_pf_rope_kv_packed<64><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, slot_stride, pk->KH, pk->VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, pk->tok);
+                k_pf_attention_mma_packed<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), s>>>(c.QKV, nqkv, pk->KH, pk->VH, p->kvd, kv_mul, pk->tiles, inv_sqrt_hs, c.ATT16, p->qd);
+            }
         } else {
-            k_pf_rope_kv<64><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
-            k_pf_attention_mma<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
+            const dim3 ag((n + qt - 1) / qt, g.n_kv_heads);
+            if (start_pos > 0) { // rows written by earlier chunks / decode steps
+                const size_t n4 = (size_t)start_pos * p->kvd / 4;
+                k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, s>>>(kc, vc, c.KH, c.VH, n4);
+                nl++;
+            }
+            if (g.head_size == 128) {
+                k_pf_rope_kv<128><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
+                k_pf_attention_mma<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
+            } else {
+                k_pf_rope_kv<64><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
+                k_pf_attention_mma<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
+            }
         }
         nl += 2;
         const int sp_wo = splits(g.dim / pg::BN, p->qd), sp_w2 = splits(g.dim / pg::BN, g.hidden_dim);
@@ -2056,6 +2106,152 @@ int b200_slot_copy_kv(b200_plan *p, int32_t slot, int32_t n_positions) {
     }
     CK(cudaStreamSynchronize(p->stream));
     return B200_OK;
+}
+
+namespace {
+// Exact b200_prefill_slots: the batched step without the classifier, one step per position.  Sequences are ordered by length,
+// longest first, so the sequences that still have tokens at step s are rows 0 .. n_s - 1 of that step.  The whole schedule is
+// uploaded once; each step's graph reads its entry through the device step index.
+int prefill_slots_exact(b200_plan *p, int ns, const int *slots, const int *start, const int *len, const int *off, const int *tokens) {
+    auto &B = p->bt;
+    std::vector<int> ord(ns);
+    for (int i = 0; i < ns; i++) ord[i] = i;
+    std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return len[a] > len[b]; });
+    const int steps = len[ord[0]];
+    std::vector<BatchRows> sched(steps);
+    std::vector<int> nrows(steps);
+    for (int s = 0; s < steps; s++) {
+        int n = 0;
+        for (int i : ord) {
+            if (len[i] <= s) break;
+            sched[s].token[n] = tokens[off[i] + s];
+            sched[s].pos[n] = start[i] + s;
+            sched[s].slot[n] = slots[i];
+            n++;
+        }
+        nrows[s] = n;
+    }
+    int rc;
+    for (int s = 0; s < steps; s++)
+        if (!B.gp[nrows[s]] && (rc = capture_batch(p, nrows[s], true))) return rc;
+    CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
+    int launches = 0;
+    CK(cudaEventRecord(p->ev0, p->stream));
+    for (int s = 0; s < steps; s++) {
+        CK(cudaGraphLaunch(B.gp[nrows[s]], p->stream));
+        launches += B.launches_p[nrows[s]];
+    }
+    CK(cudaEventRecord(p->ev1, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
+    CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
+    p->launches_prefill = launches;
+    return B200_OK;
+}
+
+// Tensor-core b200_prefill_slots: one chunk of the concatenated tokens (call order, no padding).  Sequence i's f16 K / V region
+// holds its rows [0, start + len) from scratch row hrow[i]; sequences of length 0 take no part.
+int prefill_slots_tc(b200_plan *p, int ns, const int *slots, const int *start, const int *len, const int *off, const int *tokens, int total) {
+    PrefillCtx &c = p->prefill;
+    const b200_config &g = p->cfg;
+    std::vector<int> n, st, row0, hrow;
+    std::vector<PfTok> tok(total);
+    std::vector<PfHist> hist;
+    size_t rows = 0;
+    int max_start = 0;
+    for (int i = 0; i < ns; i++) {
+        if (!len[i]) continue;
+        n.push_back(len[i]); st.push_back(start[i]); row0.push_back(off[i]); hrow.push_back((int)rows);
+        for (int j = 0; j < len[i]; j++) tok[off[i] + j] = PfTok{start[i] + j, slots[i], (int)rows + start[i] + j};
+        if (start[i] > 0) {
+            hist.push_back(PfHist{slots[i], start[i], (int)rows});
+            if (start[i] > max_start) max_start = start[i];
+        }
+        rows += (size_t)start[i] + len[i];
+    }
+    const std::vector<PfTile> tiles = pf_tiles((int)n.size(), n.data(), st.data(), row0.data(), hrow.data(), g.n_heads / g.n_kv_heads);
+    CK(cudaStreamSynchronize(p->stream)); // the buffers below may be reallocated
+    PfPacked pk{};
+    pk.KH = c.KH; pk.VH = c.VH;
+    if (rows > (size_t)g.context_length) { // more than one sequence's worth: the grown regions
+        if (rows > c.pk_rows) {
+            CK(cudaFree(c.PKH)); CK(cudaFree(c.PVH));
+            c.PKH = c.PVH = nullptr; c.pk_rows = 0;
+            CK(cudaMalloc(&c.PKH, rows * p->kvd * 2));
+            CK(cudaMalloc(&c.PVH, rows * p->kvd * 2));
+            c.pk_rows = rows;
+        }
+        pk.KH = c.PKH; pk.VH = c.PVH;
+    }
+    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t o_tiles = up16(tok.size() * sizeof(PfTok)), o_hist = o_tiles + up16(tiles.size() * sizeof(PfTile));
+    const size_t bytes = o_hist + hist.size() * sizeof(PfHist) + 16;
+    if (bytes > c.ptab_bytes) {
+        CK(cudaFree(c.ptab));
+        c.ptab = nullptr; c.ptab_bytes = 0;
+        CK(cudaMalloc(&c.ptab, bytes));
+        c.ptab_bytes = bytes;
+    }
+    std::vector<unsigned char> h(bytes, 0);
+    memcpy(h.data(), tok.data(), tok.size() * sizeof(PfTok));
+    memcpy(h.data() + o_tiles, tiles.data(), tiles.size() * sizeof(PfTile));
+    if (!hist.empty()) memcpy(h.data() + o_hist, hist.data(), hist.size() * sizeof(PfHist));
+    CK(cudaMemcpyAsync(c.ptab, h.data(), bytes, cudaMemcpyHostToDevice, p->stream));
+    pk.tok = reinterpret_cast<const PfTok *>(c.ptab);
+    pk.tiles = reinterpret_cast<const PfTile *>(c.ptab + o_tiles);
+    pk.n_tiles = (int)tiles.size();
+    pk.hist = reinterpret_cast<const PfHist *>(c.ptab + o_hist);
+    pk.n_hist = (int)hist.size();
+    pk.max_start = max_start;
+    // pageable sources: both copies are staged before cudaMemcpyAsync returns (the pinned p->h_ids holds one sequence's worth)
+    CK(cudaMemcpyAsync(c.tok, tokens, (size_t)total * 4, cudaMemcpyHostToDevice, p->stream));
+    CK(cudaEventRecord(p->ev0, p->stream));
+    int rc = prefill_forward(p, total, 0, &p->launches_prefill, &pk);
+    if (rc) return rc;
+    CK(cudaEventRecord(p->ev1, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
+    CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
+    return B200_OK;
+}
+} // namespace
+
+int b200_prefill_slots(b200_plan *p, int32_t n_seqs, const int32_t *slots, const int32_t *start_positions, const int32_t *lengths, const int32_t *tokens) {
+    if (!p) return B200_ERR_BAD_ARG;
+    auto &B = p->bt;
+    const b200_config &c = p->cfg;
+    if (!B.n_slots) return fail(p, B200_ERR_STATE, "no decode slots: call b200_set_decode_slots first");
+    if (!slots || !start_positions || !lengths) return fail(p, B200_ERR_BAD_ARG, "slots, start_positions and lengths must not be NULL");
+    if (n_seqs < 1 || n_seqs > B.n_slots) return fail(p, B200_ERR_BAD_ARG, "n_seqs = %d: need 1 <= n_seqs <= %d (the plan's decode slots)", n_seqs, B.n_slots);
+    std::vector<int> off(n_seqs);
+    int64_t total = 0;
+    for (int i = 0; i < n_seqs; i++) {
+        if (slots[i] < 0 || slots[i] >= B.n_slots) return fail(p, B200_ERR_BAD_ARG, "sequence %d: slot %d out of range (%d slots)", i, slots[i], B.n_slots);
+        for (int j = 0; j < i; j++)
+            if (slots[j] == slots[i]) return fail(p, B200_ERR_BAD_ARG, "sequence %d: slot %d repeats sequence %d's", i, slots[i], j);
+        if (lengths[i] < 0) return fail(p, B200_ERR_BAD_ARG, "sequence %d: length %d is negative", i, lengths[i]);
+        if (start_positions[i] < 0 || (int64_t)start_positions[i] + lengths[i] > c.context_length)
+            return fail(p, B200_ERR_BAD_ARG, "sequence %d: positions %d..%lld outside the KV cache (%d)", i, start_positions[i],
+                        (long long)start_positions[i] + lengths[i] - 1, c.context_length);
+        off[i] = (int)total;
+        total += lengths[i];
+    }
+    if (total && !tokens) return fail(p, B200_ERR_BAD_ARG, "tokens must not be NULL");
+    for (int i = 0; i < n_seqs; i++)
+        for (int j = 0; j < lengths[i]; j++)
+            if (tokens[off[i] + j] < 0 || tokens[off[i] + j] >= c.vocab_size)
+                return fail(p, B200_ERR_BAD_ARG, "sequence %d: token %d (index %d) out of range", i, tokens[off[i] + j], j);
+    const PrefillCtx &pc = p->prefill;
+    const bool tc = (pc.ready && pc.mode == B200_PREFILL_TENSOR_CORE) || (pc.q8_ready && pc.mode == B200_PREFILL_TENSOR_CORE_W8A16);
+    if (tc && total > p->prefill_batch) {
+        int i = 0;
+        while (off[i] + lengths[i] <= p->prefill_batch) i++;
+        return fail(p, B200_ERR_BAD_ARG, "sequence %d: the call's %lld tokens exceed prefill_batch_size %d (split the prompts into chunks)", i, (long long)total,
+                    p->prefill_batch);
+    }
+    if (!total) return B200_OK;
+    CK(cudaSetDevice(p->device));
+    return tc ? prefill_slots_tc(p, n_seqs, slots, start_positions, lengths, off.data(), tokens, (int)total)
+              : prefill_slots_exact(p, n_seqs, slots, start_positions, lengths, off.data(), tokens);
 }
 
 int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step) {
@@ -2540,6 +2736,52 @@ int b200_test_pf_attention(const float *q, const float *k, const float *v, int32
         if (ok(cudaGetLastError()) && ok(cudaDeviceSynchronize())) ok(cudaMemcpy(out, dout, (size_t)out_rows * qd * 2, cudaMemcpyDeviceToHost));
     }
     cudaFree(dqkv); cudaFree(dk); cudaFree(dv); cudaFree(dkh); cudaFree(dvh); cudaFree(dout);
+    return rc;
+}
+
+int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const int32_t *start_positions, const float *q, const float *k, const float *v,
+                                  int32_t n_heads, int32_t n_kv_heads, int32_t head_size, uint16_t *out) {
+    if (!lengths || !start_positions || !q || !k || !v || !out || n_seqs < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return B200_ERR_BAD_ARG;
+    const int kv_mul = n_heads / n_kv_heads, hs = head_size;
+    if ((hs != 64 && hs != 128) || kv_mul > 64) return B200_ERR_BAD_ARG;
+    const int qd = n_heads * hs, kvd = n_kv_heads * hs, ldq = qd + 2 * kvd;
+    std::vector<int> row0(n_seqs), hrow(n_seqs);
+    int n = 0, rows = 0;
+    for (int i = 0; i < n_seqs; i++) {
+        if (lengths[i] < 1 || start_positions[i] < 0) return B200_ERR_BAD_ARG;
+        row0[i] = n; hrow[i] = rows;
+        n += lengths[i]; rows += start_positions[i] + lengths[i];
+    }
+    const std::vector<PfTile> tiles = pf_tiles(n_seqs, lengths, start_positions, row0.data(), hrow.data(), kv_mul);
+    const size_t kv_elems = (size_t)rows * kvd;
+    float *dqkv = nullptr, *dk = nullptr, *dv = nullptr;
+    __half *dkh = nullptr, *dvh = nullptr, *dout = nullptr;
+    PfTile *dt = nullptr;
+    int rc = B200_OK;
+    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
+    // q rows of every sequence back to back in the q columns of QKV rows, K / V rows [0, start + n) of each sequence back to back: the
+    // layout b200_prefill_slots gives the packed kernel
+    if (ok(cudaMalloc(&dqkv, (size_t)n * ldq * 4)) && ok(cudaMalloc(&dk, kv_elems * 4)) && ok(cudaMalloc(&dv, kv_elems * 4)) &&
+        ok(cudaMalloc(&dkh, kv_elems * 2)) && ok(cudaMalloc(&dvh, kv_elems * 2)) && ok(cudaMalloc(&dout, (size_t)n * qd * 2)) &&
+        ok(cudaMalloc(&dt, tiles.size() * sizeof(PfTile))) &&
+        ok(cudaMemset(dqkv, 0xFF, (size_t)n * ldq * 4)) && ok(cudaMemcpy2D(dqkv, (size_t)ldq * 4, q, (size_t)qd * 4, (size_t)qd * 4, n, cudaMemcpyHostToDevice)) &&
+        ok(cudaMemcpy(dk, k, kv_elems * 4, cudaMemcpyHostToDevice)) && ok(cudaMemcpy(dv, v, kv_elems * 4, cudaMemcpyHostToDevice)) &&
+        ok(cudaMemcpy(dout, out, (size_t)n * qd * 2, cudaMemcpyHostToDevice)) &&
+        ok(cudaMemcpy(dt, tiles.data(), tiles.size() * sizeof(PfTile), cudaMemcpyHostToDevice))) {
+        const float inv_sqrt_hs = (float)(1.0 / sqrt((double)hs));
+        const dim3 ag((unsigned)tiles.size(), n_kv_heads);
+        const size_t n4 = kv_elems / 4;
+        k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, 0>>>(dk, dv, dkh, dvh, n4);
+        if (hs == 128) {
+            if (ok(cudaFuncSetAttribute(k_pf_attention_mma_packed<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>())))
+                k_pf_attention_mma_packed<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, dt, inv_sqrt_hs, dout, qd);
+        } else {
+            if (ok(cudaFuncSetAttribute(k_pf_attention_mma_packed<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<64>())))
+                k_pf_attention_mma_packed<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, dt, inv_sqrt_hs, dout, qd);
+        }
+        if (ok(cudaGetLastError()) && ok(cudaDeviceSynchronize())) ok(cudaMemcpy(out, dout, (size_t)n * qd * 2, cudaMemcpyDeviceToHost));
+    }
+    cudaFree(dqkv); cudaFree(dk); cudaFree(dv); cudaFree(dkh); cudaFree(dvh); cudaFree(dout); cudaFree(dt);
     return rc;
 }
 

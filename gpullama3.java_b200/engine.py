@@ -8,6 +8,8 @@ Position/token conventions decide parity, so they are restated exactly:
 ``generate_tokens_llama_batch_prefill`` <- InferenceEngineWithBatchPrefillDecode.generateTokensGPULlama
                               (InferenceEngineWithBatchPrefillDecode.java:163-251)
 ``generate_tokens_batch``  several requests through the first two loops in lockstep on the plan's decode slots
+``generate_tokens_batch_prefill`` the third loop for several requests: prompts prefilled straight into the decode slots
+                              (prefill_slots), then lockstep decode
 The sampler is greedy (temperature 0 -> FloatTensor.argmax, Sampler.java:124-132) and runs on
 the device; ``forward`` is any callable (token, position) -> argmax so the same loops drive
 the oracle in the tests.
@@ -161,3 +163,56 @@ def generate_tokens_llama_batch_prefill(plan, latest_token: int, start_position:
         current = nxt
         pos += 1
     return generated
+
+
+def generate_tokens_batch_prefill(plan, model_type: str, requests: list, stop_tokens: Iterable[int], max_tokens: int,
+                                  context_length: int, batch_size: int) -> list[list[int]]:
+    """The batched counterpart of generate_tokens_llama_batch_prefill on the plan's decode slots (request i on slot i).  Each request
+    (latest_token, start_position, prompt_tokens) prefills [latest] + prompt[:-1] into its slot, clamped to the token budget as that
+    function clamps it; the prompts of all requests are packed into prefill_slots calls of at most batch_size tokens (a prompt may
+    span two calls).  Then every request decodes in lockstep through forward_decode_batch from prompt[-1] at start + len(prompt)
+    until its stop token or the budget, so each result equals generate_tokens_llama_batch_prefill for the request alone.  Only the
+    Llama loop has this form: a slot's rows past its prompt are never read, so the slots are not reset first."""
+    if _is_qwen_loop(model_type):
+        raise ValueError(f"{model_type} runs the Qwen3 loop, which has no batched-prefill form: use generate_tokens_batch")
+    n_slots = plan.batch_info()[0]
+    if len(requests) > n_slots:
+        raise ValueError(f"{len(requests)} requests but the plan has {n_slots} decode slots (set_decode_slots)")
+    if batch_size < 1:
+        raise ValueError("batch_size must be >= 1")
+    if max_tokens < 0 or context_length < max_tokens:
+        max_tokens = context_length
+    stop = set(stop_tokens)
+    todo = []  # per request: (slot, first position, tokens still to prefill)
+    for i, (latest, start, prompt) in enumerate(requests):
+        n = len(prompt)
+        if n == 0:
+            raise IndexError("empty prompt (the reference's promptTokens.get(N - 1) throws as well)")
+        seq = [latest] + list(prompt[: n - 1])
+        todo.append([i, start, seq[: max(0, min(n, max_tokens - start))]])
+    while any(t[2] for t in todo):
+        slots, starts, pieces, room = [], [], [], batch_size
+        for t in todo:
+            if room == 0:
+                break
+            if t[2]:
+                take = min(room, len(t[2]))
+                slots.append(t[0]); starts.append(t[1]); pieces.append(t[2][:take])
+                t[1] += take
+                t[2] = t[2][take:]
+                room -= take
+        plan.prefill_slots(slots, starts, pieces)
+    results: list = [[] for _ in requests]
+    live = {i: (int(prompt[-1]), start + len(prompt)) for i, (_, start, prompt) in enumerate(requests) if start + len(prompt) < max_tokens}
+    while live:
+        rows = sorted(live)
+        ids, _ = plan.forward_decode_batch(rows, [live[i][0] for i in rows], [live[i][1] for i in rows])
+        for i, am in zip(rows, ids):
+            nxt = int(am)
+            results[i].append(nxt)
+            pos = live[i][1] + 1
+            if nxt in stop or pos >= max_tokens:
+                del live[i]
+            else:
+                live[i] = (nxt, pos)
+    return results

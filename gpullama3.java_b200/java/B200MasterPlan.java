@@ -78,6 +78,7 @@ public final class B200MasterPlan implements AutoCloseable {
             FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
     private static final MethodHandle SLOT_RESET = fn("b200_slot_reset", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle SLOT_COPY_KV = fn("b200_slot_copy_kv", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
+    private static final MethodHandle PREFILL_SLOTS = fn("b200_prefill_slots", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
     private static final MethodHandle FREE = fn("b200_plan_free", FunctionDescriptor.ofVoid(ADDRESS));
     private static final MethodHandle LAST_ERROR = fn("b200_last_error", FunctionDescriptor.of(ADDRESS, ADDRESS));
 
@@ -285,6 +286,22 @@ public final class B200MasterPlan implements AutoCloseable {
     public void slotCopyKv(int slot, int nPositions) throws Throwable {
         int rc = (int) SLOT_COPY_KV.invokeExact(plan, slot, nPositions);
         if (rc != 0) check(rc, lastError());
+    }
+
+    /** Prefill prompts[i] straight into slot slots[i] at positions startPositions[i].. (K/V only), all in one call, in the plan's
+     *  prefill mode; a tensor-core mode takes at most prefill_batch_size tokens per call.  The plan's own cache and the other slots
+     *  are not touched. */
+    public void prefillSlots(int[] slots, int[] startPositions, int[][] prompts) throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            int n = slots.length, total = 0;
+            int[] lengths = new int[n];
+            for (int i = 0; i < n; i++) { lengths[i] = prompts[i].length; total += lengths[i]; }
+            int[] tokens = new int[total];
+            for (int i = 0, o = 0; i < n; o += lengths[i], i++) System.arraycopy(prompts[i], 0, tokens, o, lengths[i]);
+            int rc = (int) PREFILL_SLOTS.invokeExact(plan, n, a.allocateFrom(JAVA_INT, slots), a.allocateFrom(JAVA_INT, startPositions),
+                    a.allocateFrom(JAVA_INT, lengths), total == 0 ? MemorySegment.NULL : a.allocateFrom(JAVA_INT, tokens));
+            if (rc != 0) check(rc, lastError());
+        }
     }
 
     /** void freeTornadoExecutionPlan() */

@@ -52,7 +52,7 @@ class Tensor(C.Structure):
 EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
-           "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_batch_info",
+           "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -97,6 +97,8 @@ def lib() -> C.CDLL:
     L.b200_forward_decode_batch.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp]
     L.b200_slot_reset.argtypes = [vp, i32]
     L.b200_slot_copy_kv.argtypes = [vp, i32, i32]
+    L.b200_prefill_slots.argtypes = [vp, i32, vp, vp, vp, vp]
+    L.b200_test_pf_attention_packed.argtypes = [i32, vp, vp, vp, vp, vp, i32, i32, i32, vp]
     L.b200_batch_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     L.b200_launches_per_decode.argtypes = [vp]
@@ -215,6 +217,25 @@ def test_gemm_q8(mode: str, a, bq, c, bq2=None, m_valid: int | None = None, stag
     if rc != B200_OK:
         _raise(rc, "b200_test_gemm_q8 failed")
     return c
+
+
+def test_pf_attention_packed(qs, ks, vs, starts, n_heads: int, n_kv_heads: int, sentinel: int = 0x7E5A) -> list:
+    """The packed prefill attention (k_pf_attention_mma_packed) over several sequences in one launch.  qs[i] float32
+    [n_i, n_heads*hs]; ks[i], vs[i] float32 [starts[i]+n_i, n_kv_heads*hs].  Returns each sequence's f16 bits [n_i, n_heads*hs]."""
+    lens = np.array([len(q) for q in qs], dtype=np.int32)
+    st = np.ascontiguousarray(starts, dtype=np.int32)
+    hs = qs[0].shape[1] // n_heads
+    q = np.ascontiguousarray(np.concatenate(qs), dtype=np.float32)
+    k = np.ascontiguousarray(np.concatenate(ks), dtype=np.float32)
+    v = np.ascontiguousarray(np.concatenate(vs), dtype=np.float32)
+    if len(st) != len(qs) or any(len(ks[i]) != st[i] + lens[i] or len(vs[i]) != st[i] + lens[i] for i in range(len(qs))):
+        raise ValueError("ks[i] / vs[i] must be [starts[i] + n_i, n_kv_heads * head_size]")
+    out = np.full((int(lens.sum()), n_heads * hs), sentinel, dtype=np.uint16)
+    rc = lib().b200_test_pf_attention_packed(len(qs), lens.ctypes.data, st.ctypes.data, q.ctypes.data, k.ctypes.data, v.ctypes.data, n_heads,
+                                             n_kv_heads, hs, out.ctypes.data)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_pf_attention_packed failed")
+    return np.split(out, np.cumsum(lens)[:-1])
 
 
 def test_pf_attention(q, k, v, n_heads: int, n_kv_heads: int, start_pos: int, impl: str = "mma", out_rows: int | None = None,
@@ -364,6 +385,16 @@ class NativePlan:
 
     def slot_copy_kv(self, slot: int, n_positions: int):
         self._ck(lib().b200_slot_copy_kv(self._p, slot, n_positions))
+
+    def prefill_slots(self, slots, start_positions, token_lists):
+        """b200_prefill_slots: token_lists[i] into slot slots[i] at positions start_positions[i].. (K/V only)."""
+        s = np.ascontiguousarray(slots, dtype=np.int32)
+        st = np.ascontiguousarray(start_positions, dtype=np.int32)
+        if len(st) != len(s) or len(token_lists) != len(s):
+            raise ValueError("slots, start_positions and token_lists must have the same length")
+        ln = np.array([len(t) for t in token_lists], dtype=np.int32)
+        toks = np.ascontiguousarray(np.concatenate([np.asarray(t, dtype=np.int32).reshape(-1) for t in token_lists]) if len(s) else np.zeros(0), dtype=np.int32)
+        self._ck(lib().b200_prefill_slots(self._p, len(s), s.ctypes.data, st.ctypes.data, ln.ctypes.data, toks.ctypes.data))
 
     def batch_info(self):
         """(decode slots, kernels of the last batched step, its device milliseconds)."""

@@ -176,6 +176,12 @@ class B200MasterPlan:
         """Copy positions [0, n_positions) of the plan's own KV cache (e.g. after forward_batch_prefill) into the slot; zero the rest."""
         self._native.slot_copy_kv(slot, n_positions)
 
+    def prefill_slots(self, slots, start_positions, token_lists):
+        """Prefill token_lists[i] straight into decode slot slots[i] at positions start_positions[i].. in one call (K/V only, the
+        plan's prefill mode; at most prefill_batch_size tokens in all in a tensor-core mode).  The plan's own cache and the other
+        slots are left as they are."""
+        self._native.prefill_slots(slots, start_positions, token_lists)
+
     def batch_info(self):
         """(decode slots, kernels of the last batched step, its device milliseconds)."""
         return self._native.batch_info()

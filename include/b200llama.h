@@ -261,8 +261,25 @@ int b200_slot_reset(b200_plan *plan, int32_t slot);
 
 /* Copy positions [0, n_positions) of the plan's own K/V cache into the slot and zero positions [n_positions, ctx): how a prompt
  * prefilled with b200_forward_batch_prefill enters a slot.  The copy is exact after the exact prefill; after a tensor-core prefill it
- * carries that mode's FP16 tolerance. */
+ * carries that mode's FP16 tolerance.  b200_prefill_slots prefills prompts straight into their slots, several per call, without
+ * the plan's own cache or this copy. */
 int b200_slot_copy_kv(b200_plan *plan, int32_t slot, int32_t n_positions);
+
+/* Prefill n_seqs prompts, each into its own decode slot: sequence i's tokens tokens[off_i .. off_i + lengths[i]) (concatenated in
+ * call order) are processed at positions start_positions[i] .. start_positions[i] + lengths[i] - 1 of slot slots[i].  KV only, no
+ * logits.  The mode is the plan's prefill mode (b200_set_prefill_mode):
+ *   exact: the batched decode step without its final norm, lm_head and argmax, one step per position (every sequence with tokens
+ *          left advances by one); each slot's K/V is bit-identical to the CPU path;
+ *   tensor-core modes: one chunk of all the tokens through the GEMMs, at most prefill_batch_size tokens per call; each slot's K/V is
+ *          what b200_forward_batch_prefill of that prompt alone followed by b200_slot_copy_kv gives, wherever the GEMMs split K
+ *          the same way (the split depends on the chunk's total length).
+ * Only the named slots' rows at the named positions are written: the plan's own cache, the other slots and a named slot's rows
+ * outside its range keep their bytes, so a later call may continue a slot's prompt (start_positions[i] > 0).  A length of 0 takes
+ * no part.  B200_ERR_STATE without decode slots; B200_ERR_BAD_ARG (naming the sequence) for n_seqs outside 1..n_slots, a slot out
+ * of range or repeated, a negative length, positions outside the KV cache, a token out of range, or more tokens than
+ * prefill_batch_size in a tensor-core mode.  b200_prefill_info reports the call's launches and device milliseconds. */
+int b200_prefill_slots(b200_plan *plan, int32_t n_seqs, const int32_t *slots, const int32_t *start_positions, const int32_t *lengths,
+                       const int32_t *tokens);
 
 /* Decode slots, kernels of the last batched step and its device milliseconds (CUDA events around the graph); any pointer may be NULL. */
 int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step);
@@ -376,6 +393,13 @@ int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, i
  * tokens, the remaining rows of its 64-row tile are padding). */
 int b200_test_pf_attention(const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads,
                            int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out);
+
+/* Test hook: the packed form of the same attention (k_pf_attention_mma_packed, as b200_prefill_slots runs it) over n_seqs sequences
+ * at once.  Sequence i has lengths[i] >= 1 query tokens at positions start_positions[i]..; q: f32 [sum lengths][n_heads * head_size]
+ * (the sequences' rows back to back); k, v: f32 [sum (start_positions[i] + lengths[i])][n_kv_heads * head_size] (each sequence's
+ * rows 0 .. start + length - 1, back to back).  out: f16 bits [sum lengths][n_heads * head_size], in/out. */
+int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const int32_t *start_positions, const float *q, const float *k,
+                                  const float *v, int32_t n_heads, int32_t n_kv_heads, int32_t head_size, uint16_t *out);
 
 /* Weight upload of b200_plan_create (the counterpart of the reference's load-time metrics, ModelLoader.java:102-106 and the
  * copy-in timing of TornadoVMMasterPlanSingleToken.java:51-54): wall seconds from the first tensor to the last repack kernel,

@@ -5,6 +5,7 @@
 //   k_rmsnorm_quant_batch      one CTA per row: rmsnorm_quant_row (decode_kernels.cuh) on that row's x / token / outputs
 //   k_stream_matvec_q8_batch   the tile-major Q8_0 stream of stream_matvec.cuh; each tile is applied to every row's activation
 //   k_attention_batch          grid (heads, rows): attention_head (decode_kernels.cuh) on the row's slot cache and position
+//   k_rope_kv_batch + k_attention_cached_rows   the same attention split in two, for steps whose rows share a sequence
 //   k_argmax_batch             one CTA per row: merges that row's lm_head partials (first strict maximum)
 #pragma once
 #include "decode_kernels.cuh"
@@ -59,6 +60,44 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attention_batch(float *__restri
     attention_head<HS>(qkv + (size_t)v * qkv_stride, kc + base, vc + base, rows->pos + v, cr, ci, n_heads, n_kv_heads, arch, qnorm_w, knorm_w,
                        qkv_bias, eps, sqrt_hs, xq + (size_t)v * qd, xs + (size_t)v * (qd / 32), nullptr, tr, tp, 0u, 0,
                        att_scratch ? att_scratch + (size_t)v * n_heads * ctx : nullptr, ctx);
+}
+
+// ---- same-sequence steps: RoPE / KV write, then attention from the cache ----------------------------------------------------
+// Rows of one step may be consecutive positions of ONE sequence (b200_forward_decode_multi, the exact prefills): row i attends to
+// the K / V rows i' < i write.  k_attention_batch writes its row's K / V inside the attention CTA, so those rows would race;
+// here a separate grid writes every row's K / V first, and the attention reads them only after its dependency wait (the
+// previous grid complete), with no CTA ever waiting on another of its own grid.
+//   k_rope_kv_batch            grid (heads, rows), 2 x HS threads: rope_kv_prologue, rotated q back into qkv, k / v into the cache
+//   k_attention_cached_rows   grid (heads, rows): attention_head<HS, true>, every key t <= pos from the cache
+template <int HS>
+__global__ void __launch_bounds__(2 * HS) k_rope_kv_batch(float *__restrict__ qkv, int qkv_stride, float *__restrict__ kc, float *__restrict__ vc,
+                                                         size_t slot_stride, const BatchRows *__restrict__ rows, const float *__restrict__ cr,
+                                                         const float *__restrict__ ci, int n_heads, int n_kv_heads, int arch,
+                                                         const float *__restrict__ qnorm_w, const float *__restrict__ knorm_w,
+                                                         const float *__restrict__ qkv_bias, float eps) {
+    __shared__ __align__(16) float sq[HS], sk[HS], so[HS];
+    __shared__ float s_val[2];
+    const int v = blockIdx.y, h = blockIdx.x;
+    const size_t base = (size_t)rows->slot[v] * slot_stride;
+    const int kv_mul = n_heads / n_kv_heads, kvh = h / kv_mul;
+    pdl_launch_dependents();
+    pdl_wait();
+    const int qd = n_heads * HS, kvd = n_kv_heads * HS;
+    float *q = qkv + (size_t)v * qkv_stride;
+    rope_kv_prologue<HS>(q, q + h * HS, q + qd + kvh * HS, q + qd + kvd + kvh * HS, kc + base, vc + base, rows->pos[v], h, kv_mul, kvh, qd, kvd, cr,
+                         ci, arch, qnorm_w, knorm_w, qkv_bias, eps, sq, sk, so, s_val);
+}
+
+template <int HS>
+__global__ void __launch_bounds__(ATT_THREADS) k_attention_cached_rows(float *__restrict__ qkv, int qkv_stride, float *__restrict__ kc,
+                                                                       float *__restrict__ vc, size_t slot_stride, const BatchRows *__restrict__ rows,
+                                                                       int n_heads, int n_kv_heads, int arch, float sqrt_hs, int8_t *__restrict__ xq,
+                                                                       float *__restrict__ xs, float *att_scratch, int ctx, TraceBuf tr, TpCtx tp) {
+    const int v = blockIdx.y, qd = n_heads * HS;
+    const size_t base = (size_t)rows->slot[v] * slot_stride;
+    attention_head<HS, true>(qkv + (size_t)v * qkv_stride, kc + base, vc + base, rows->pos + v, nullptr, nullptr, n_heads, n_kv_heads, arch, nullptr,
+                             nullptr, nullptr, 0.0f, sqrt_hs, xq + (size_t)v * qd, xs + (size_t)v * (qd / 32), nullptr, tr, tp, 0u, 0,
+                             att_scratch ? att_scratch + (size_t)v * n_heads * ctx : nullptr, ctx);
 }
 
 // ---- the batched Q8_0 stream ----------------------------------------------------------------------------------------------

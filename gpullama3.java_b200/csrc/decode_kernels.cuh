@@ -397,40 +397,18 @@ __global__ void k_swiglu(float *__restrict__ hb, const float *__restrict__ hb2, 
 // ------------------------------------------------------------------------------------------
 #define ATT_THREADS 512 // four threads per key (scores) and per output element (weighted sum): head size <= ATT_THREADS / 4
 
-// The body of k_attention for query head blockIdx.x of one sequence; `posp` is read after the dependency wait (the batched
-// step, decode_batch.cuh, runs it per (head, row) with that row's position, cache, qkv vector, outputs and score rows).
+// The prologue of attention_head for query head h at position pos: threads [0,HALF) rotate q pairs, threads [HALF,HS) rotate
+// k pairs, threads [HS,2HS) take v.  The rotated q goes to sq and back into qkv, the rotated k to sk; the group's first head
+// writes k / v into the cache.  sk / so are the Qwen3 norm's scratch; Qwen2 stages its biased v in so.  k_rope_kv_batch
+// (decode_batch.cuh) runs it on its own, ahead of an attention that takes every key from the cache.
+// qsrc / ksrc / vsrc: this head's q, its KV head's k and v in qkv.
 template <int HS>
-__device__ __forceinline__ void attention_head(float *__restrict__ qkv, float *__restrict__ kc, float *__restrict__ vc,
-                                               const int *__restrict__ posp, const float *__restrict__ cr, const float *__restrict__ ci,
-                                               int n_heads, int n_kv_heads, int arch, const float *__restrict__ qnorm_w,
-                                               const float *__restrict__ knorm_w, const float *__restrict__ qkv_bias, float eps, float sqrt_hs,
-                                               int8_t *__restrict__ xq, float *__restrict__ xs, float *__restrict__ xb, const TraceBuf &tr,
-                                               const TpCtx &tp, unsigned tp_out_op, int head_base, float *att_scratch, int ctx) {
-    extern __shared__ __align__(16) float sm[]; // q[HS] | k[HS] | out[HS] | att[ctx] (att in global scratch for long contexts)
-    __shared__ float red[ATT_THREADS / 32];
-    __shared__ float s_val[2];
-    float *sq = sm, *sk = sm + HS, *so = sm + 2 * HS;
-    float *att = att_scratch ? att_scratch + (size_t)blockIdx.x * ctx : sm + 3 * HS;
-    const int h = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+__device__ __forceinline__ void rope_kv_prologue(float *qkv, const float *qsrc, const float *ksrc, const float *vsrc, float *kc, float *vc, int pos,
+                                                 int h, int kv_mul, int kvh, int qd, int kvd, const float *cr, const float *ci, int arch,
+                                                 const float *qnorm_w, const float *knorm_w, const float *qkv_bias, float eps, float *sq, float *sk,
+                                                 float *so, float *s_val) {
+    const int tid = threadIdx.x;
     constexpr int HALF = HS / 2;
-    trace_entry(tr);
-    pdl_launch_dependents();
-    const int kv_mul = n_heads / n_kv_heads, kvh = h / kv_mul;
-    const int qd = n_heads * HS, kvd = n_kv_heads * HS;
-    pdl_wait();
-    trace_mark(tr, 2);
-    const int pos = *posp, nt = pos + 1;
-    { // K/V rows of the earlier positions -> L2, one 128-byte line per request, so the score loads below hit L2 (the weight stream carries an
-      // evict_first policy; without the prefetch these rows come from HBM every layer)
-        constexpr int LINES = HS / 32;
-        for (int i = tid; i < pos * LINES; i += ATT_THREADS) {
-            const size_t off = (size_t)(i / LINES) * kvd + kvh * HS + (i % LINES) * 32;
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(kc + off));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(vc + off));
-        }
-    }
-    const float *qsrc = qkv + h * HS, *ksrc = qkv + qd + kvh * HS, *vsrc = qkv + qd + kvd + kvh * HS;
-    // ---- prologue: threads [0,HALF) rotate q pairs, threads [HALF,HS) rotate k pairs, threads [HS,2HS) take v
     if (tid < HS) {
         const bool is_q = tid < HALF;
         const int p = is_q ? tid : tid - HALF;
@@ -490,6 +468,55 @@ __device__ __forceinline__ void attention_head(float *__restrict__ qkv, float *_
         }
         if (h % kv_mul == 0) vc[(size_t)pos * kvd + kvh * HS + j] = w;
     }
+}
+
+// K / V cache loads of attention_head: read-only path, or L2 (ld.global.cg) for rows the previous grid wrote.
+template <bool CG, typename T> __device__ __forceinline__ T kv_ld(const T *p) {
+    if constexpr (CG) return __ldcg(p);
+    else return __ldg(p);
+}
+
+// The body of k_attention for query head blockIdx.x of one sequence; `posp` is read after the dependency wait (the batched
+// step, decode_batch.cuh, runs it per (head, row) with that row's position, cache, qkv vector, outputs and score rows).
+// CACHED: k_rope_kv_batch has run the prologue, so q is read rotated from qkv and every key t <= pos, the current one
+// included, comes from the cache -- the same floats the prologue would hold in sk / so, in the same order.  Those rows were
+// written by the previous grid, so they are read through L2 (ld.global.cg), never through the non-coherent path.
+template <int HS, bool CACHED = false>
+__device__ __forceinline__ void attention_head(float *__restrict__ qkv, float *__restrict__ kc, float *__restrict__ vc,
+                                               const int *__restrict__ posp, const float *__restrict__ cr, const float *__restrict__ ci,
+                                               int n_heads, int n_kv_heads, int arch, const float *__restrict__ qnorm_w,
+                                               const float *__restrict__ knorm_w, const float *__restrict__ qkv_bias, float eps, float sqrt_hs,
+                                               int8_t *__restrict__ xq, float *__restrict__ xs, float *__restrict__ xb, const TraceBuf &tr,
+                                               const TpCtx &tp, unsigned tp_out_op, int head_base, float *att_scratch, int ctx) {
+    extern __shared__ __align__(16) float sm[]; // q[HS] | k[HS] | out[HS] | att[ctx] (att in global scratch for long contexts)
+    __shared__ float red[ATT_THREADS / 32];
+    __shared__ float s_val[2];
+    float *sq = sm, *sk = sm + HS, *so = sm + 2 * HS;
+    float *att = att_scratch ? att_scratch + (size_t)blockIdx.x * ctx : sm + 3 * HS;
+    const int h = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    trace_entry(tr);
+    pdl_launch_dependents();
+    const int kv_mul = n_heads / n_kv_heads, kvh = h / kv_mul;
+    const int qd = n_heads * HS, kvd = n_kv_heads * HS;
+    pdl_wait();
+    trace_mark(tr, 2);
+    const int pos = *posp, nt = pos + 1;
+    { // K/V rows of the earlier positions -> L2, one 128-byte line per request, so the score loads below hit L2 (the weight stream carries an
+      // evict_first policy; without the prefetch these rows come from HBM every layer)
+        constexpr int LINES = HS / 32;
+        for (int i = tid; i < pos * LINES; i += ATT_THREADS) {
+            const size_t off = (size_t)(i / LINES) * kvd + kvh * HS + (i % LINES) * 32;
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(kc + off));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(vc + off));
+        }
+    }
+    const float *qsrc = qkv + h * HS, *ksrc = qkv + qd + kvh * HS, *vsrc = qkv + qd + kvd + kvh * HS;
+    if (CACHED) {
+        if (tid < HS) sq[tid] = qsrc[tid];
+    } else {
+        rope_kv_prologue<HS>(qkv, qsrc, ksrc, vsrc, kc, vc, pos, h, kv_mul, kvh, qd, kvd, cr, ci, arch, qnorm_w, knorm_w, qkv_bias, eps, sq, sk,
+                             so, s_val);
+    }
     __syncthreads();
     // ---- scores (scalarDot, FloatTensor.java:86-92: one sequential unfused mul/add chain per key).  Four threads share a key: each loads
     // ITS quarter of the K row at once (one round trip per pass of ATT_THREADS/4 keys), then the chain runs through the quad in element
@@ -501,17 +528,17 @@ __device__ __forceinline__ void attention_head(float *__restrict__ qkv, float *_
     {
         const float *vcol = vc + kvh * HS + vd;
 #pragma unroll
-        for (int u = 0; u < VB; u++) vv[u] = (vlive && quad * VB + u < pos) ? __ldg(vcol + (size_t)(quad * VB + u) * kvd) : 0.0f;
+        for (int u = 0; u < VB; u++) vv[u] = (vlive && quad * VB + u < pos) ? kv_ld<CACHED>(vcol + (size_t)(quad * VB + u) * kvd) : 0.0f;
     }
     float lmax = -INFINITY;
 #pragma unroll 1
     for (int t0 = 0; t0 < nt; t0 += ATT_THREADS / 4) {
         const int t = t0 + (tid >> 2);
         float4 kk[QV];
-        if (t < pos) {
+        if (t < pos || (CACHED && t == pos)) {
             const float4 *k = reinterpret_cast<const float4 *>(kc + (size_t)t * kvd + kvh * HS + quad * QE);
 #pragma unroll
-            for (int u = 0; u < QV; u++) kk[u] = __ldg(k + u);
+            for (int u = 0; u < QV; u++) kk[u] = kv_ld<CACHED>(k + u);
         } else {
 #pragma unroll
             for (int u = 0; u < QV; u++) kk[u] = t == pos ? *reinterpret_cast<const float4 *>(sk + quad * QE + 4 * u) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -566,14 +593,16 @@ __device__ __forceinline__ void attention_head(float *__restrict__ qkv, float *_
         const int d = vd0 + vd;
         const bool live = d < HS;
         const float *vcol = vc + kvh * HS + d;
-        const float vcur = live ? ((arch & KF_QKVBIAS) ? so[d] : vsrc[d]) : 0.0f; // current position: the packed qkv vector (biased: staged)
+        const float vcur = !live ? 0.0f
+                           : CACHED ? kv_ld<true>(vcol + (size_t)pos * kvd)
+                                    : ((arch & KF_QKVBIAS) ? so[d] : vsrc[d]); // current position: the packed qkv vector (biased: staged)
         float acc = 0.0f;
 #pragma unroll 1
         for (int r0 = 0; r0 < pos; r0 += 4 * VB) {
             if (r0 > 0 || vd0 > 0) { // (round 0 of the first pass was requested before the scores)
                 const int vt0 = r0 + quad * VB;
 #pragma unroll
-                for (int u = 0; u < VB; u++) vv[u] = (live && vt0 + u < pos) ? __ldg(vcol + (size_t)(vt0 + u) * kvd) : 0.0f;
+                for (int u = 0; u < VB; u++) vv[u] = (live && vt0 + u < pos) ? kv_ld<CACHED>(vcol + (size_t)(vt0 + u) * kvd) : 0.0f;
             }
 #pragma unroll 1
             for (int qd4 = 0; qd4 < 4; qd4++) {

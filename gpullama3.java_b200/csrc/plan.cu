@@ -166,6 +166,10 @@ struct b200_plan {
         int *step = nullptr;
         cudaGraphExec_t gp[SMB_MAX_ROWS + 1] = {};
         int launches_p[SMB_MAX_ROWS + 1] = {};
+        // steps whose rows may share a sequence (k_rope_kv_batch + k_attention_cached_rows), captured on first use:
+        // [target: 0 the decode slots, 1 the plan's own cache][0 schedule-driven without the classifier, 1 with it][rows]
+        cudaGraphExec_t gs[2][2][SMB_MAX_ROWS + 1] = {};
+        int launches_s[2][2][SMB_MAX_ROWS + 1] = {};
         int last_n = 0;
         float last_ms = 0.f;
     } bt;
@@ -928,7 +932,9 @@ int launch_stream_batch(b200_plan *p, const TileMat &W, int n, const int8_t *xq,
 
 // One forward step of n rows: the single-sequence graph's kernel sequence, every launch serving all n rows.  prefill: a step of
 // b200_prefill_slots -- the rows come from the call's schedule (k_batch_rows_next) and there is no final norm, lm_head or argmax.
-int enqueue_batch(b200_plan *p, int n, int *launches, bool prefill = false) {
+// split: rows may share a sequence, so the attention runs as k_rope_kv_batch + k_attention_cached_rows (one more launch per
+// layer).  own: the K / V target is the plan's cache (key_cache / value_cache, slot 0's layout) instead of the decode slots.
+int enqueue_batch(b200_plan *p, int n, int *launches, bool prefill = false, bool split = false, bool own = false) {
     const b200_config &c = p->cfg;
     auto &B = p->bt;
     const bool pdl = p->use_pdl;
@@ -954,14 +960,30 @@ int enqueue_batch(b200_plan *p, int n, int *launches, bool prefill = false) {
         const LayerW &L = p->layers[l];
         if ((rc = norm(l == 0, L.attn_norm))) return rc;
         if ((rc = launch_stream_batch<SMV_STORE>(p, L.tqkv, n, B.xq, B.xs, B.qkv, qkvd))) return rc;
-        float *kc = B.slot_k + (size_t)l * ctx_kv, *vc = B.slot_v + (size_t)l * ctx_kv;
+        float *kc = (own ? p->key_cache : B.slot_k) + (size_t)l * ctx_kv, *vc = (own ? p->value_cache : B.slot_v) + (size_t)l * ctx_kv;
+        // split: the two launches of a step whose rows may share a sequence
+        auto att2 = [&](auto rope_kern, auto att_kern, int hs) {
+            const int r = launch_k(p, pdl, rope_kern, dim3(p->nh_l, n), dim3(2 * hs), (size_t)0, B.qkv, qkvd, kc, vc, slot_stride, (const BatchRows *)B.rows,
+                                   (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags, (const float *)L.q_norm,
+                                   (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps);
+            k++;
+            return r ? r : launch_k(p, pdl, att_kern, dim3(p->nh_l, n), dim3(ATT_THREADS), att_smem_bytes(c.head_size, c.context_length, B.att_scratch != nullptr),
+                                    B.qkv, qkvd, kc, vc, slot_stride, (const BatchRows *)B.rows, p->nh_l, p->nkv_l, p->kflags, att_score_arg(p), B.xq, B.xs,
+                                    B.att_scratch, c.context_length, TraceBuf{nullptr, 0, 0}, solo);
+        };
         auto att = [&](auto kern) {
             return launch_k(p, pdl, kern, dim3(p->nh_l, n), dim3(ATT_THREADS), att_smem_bytes(c.head_size, c.context_length, B.att_scratch != nullptr), B.qkv, qkvd,
                             kc, vc, slot_stride, (const BatchRows *)B.rows, (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags,
                             (const float *)L.q_norm, (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, att_score_arg(p), B.xq,
                             B.xs, B.att_scratch, c.context_length, TraceBuf{nullptr, 0, 0}, solo);
         };
-        if (c.head_size == 128) rc = att(k_attention_batch<128>);
+        if (split) {
+            if (c.head_size == 128) rc = att2(k_rope_kv_batch<128>, k_attention_cached_rows<128>, 128);
+            else if (c.head_size == 64) rc = att2(k_rope_kv_batch<64>, k_attention_cached_rows<64>, 64);
+            else if (c.head_size == 256) rc = att2(k_rope_kv_batch<256>, k_attention_cached_rows<256>, 256);
+            else if (c.head_size == 96) rc = att2(k_rope_kv_batch<96>, k_attention_cached_rows<96>, 96);
+            else rc = att2(k_rope_kv_batch<32>, k_attention_cached_rows<32>, 32);
+        } else if (c.head_size == 128) rc = att(k_attention_batch<128>);
         else if (c.head_size == 64) rc = att(k_attention_batch<64>);
         else if (c.head_size == 256) rc = att(k_attention_batch<256>);
         else if (c.head_size == 96) rc = att(k_attention_batch<96>);
@@ -984,14 +1006,16 @@ int enqueue_batch(b200_plan *p, int n, int *launches, bool prefill = false) {
     return B200_OK;
 }
 
-int capture_batch(b200_plan *p, int n, bool prefill = false) {
+int capture_batch(b200_plan *p, int n, bool prefill = false, bool split = false, bool own = false) {
+    auto &B = p->bt;
     cudaGraph_t g = nullptr;
     CK(cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal));
-    int rc = enqueue_batch(p, n, prefill ? &p->bt.launches_p[n] : &p->bt.launches[n], prefill);
+    int *launches = split ? &B.launches_s[own][!prefill][n] : prefill ? &B.launches_p[n] : &B.launches[n];
+    int rc = enqueue_batch(p, n, launches, prefill, split, own);
     cudaError_t e = cudaStreamEndCapture(p->stream, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
     if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(e));
-    e = cudaGraphInstantiate(prefill ? &p->bt.gp[n] : &p->bt.g[n], g, 0);
+    e = cudaGraphInstantiate(split ? &B.gs[own][!prefill][n] : prefill ? &B.gp[n] : &B.g[n], g, 0);
     cudaGraphDestroy(g);
     if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e));
     return B200_OK;
@@ -1003,6 +1027,10 @@ void batch_free(b200_plan *p) {
         if (g) { cudaGraphExecDestroy(g); g = nullptr; }
     for (cudaGraphExec_t &g : B.gp)
         if (g) { cudaGraphExecDestroy(g); g = nullptr; }
+    for (auto &by_target : B.gs)
+        for (auto &by_kind : by_target)
+            for (cudaGraphExec_t &g : by_kind)
+                if (g) { cudaGraphExecDestroy(g); g = nullptr; }
     for (void *d : B.allocs) cudaFree(d);
     if (B.h_rows) cudaFreeHost(B.h_rows);
     if (B.h_out) cudaFreeHost(B.h_out);
@@ -1018,13 +1046,15 @@ template <typename T> int balloc(b200_plan *p, T **ptr, size_t n_bytes) {
     return B200_OK;
 }
 
+// ns decode slots (0: none) and the per-row scratch of batch_max_rows rows, whatever the slot count: a step of the exact prefills
+// or of b200_forward_decode_multi fills every row however many slots there are.
 int batch_alloc(b200_plan *p, int ns) {
     const b200_config &c = p->cfg;
     auto &B = p->bt;
     const int big = c.dim > p->qd ? c.dim : p->qd;
-    const size_t N = (size_t)ns, kv = (size_t)c.n_layers * c.context_length * p->kvd * 4;
+    const size_t N = (size_t)batch_max_rows(p), kv = (size_t)c.n_layers * c.context_length * p->kvd * 4;
     int rc;
-    if ((rc = balloc(p, &B.slot_k, N * kv)) || (rc = balloc(p, &B.slot_v, N * kv)) || (rc = balloc(p, &B.x, N * c.dim * 4)) ||
+    if ((rc = balloc(p, &B.slot_k, (size_t)ns * kv)) || (rc = balloc(p, &B.slot_v, (size_t)ns * kv)) || (rc = balloc(p, &B.x, N * c.dim * 4)) ||
         (rc = balloc(p, &B.qkv, N * (p->qd + 2 * p->kvd) * 4)) || (rc = balloc(p, &B.hb, N * c.hidden_dim * 4)) ||
         (rc = balloc(p, &B.logits, N * sampler_padded(c.vocab_size) * 4)) || (rc = balloc(p, &B.xq, N * big)) || (rc = balloc(p, &B.xs, N * (big / 32) * 4)) ||
         (rc = balloc(p, &B.hq, N * c.hidden_dim)) || (rc = balloc(p, &B.hs, N * (c.hidden_dim / 32) * 4)) ||
@@ -1038,6 +1068,66 @@ int batch_alloc(b200_plan *p, int ns) {
     CK(cudaStreamSynchronize(p->stream));
     B.n_slots = ns;
     return B200_OK;
+}
+
+// ---- steps whose rows may share a sequence: b200_forward_decode_multi and the exact prefills ------------------------------
+// Why a plan cannot run them (nullptr: it can): the conditions of batched decode.
+const char *multi_why(const b200_plan *p) {
+    if (p->is_moe) return "multi-position steps have no Qwen2-MoE layer (MoE plans run one position per step)";
+    if (p->cfg.tp_size > 1) return "multi-position steps run on single-GPU plans only (this plan is tensor-parallel)";
+    if (p->wtype != B200_GGML_Q8_0) return "multi-position steps need Q8_0 weights (FP16 plans run one position per step)";
+    if (!p->use_stream) return "multi-position steps need the Q8_0 streaming layout (this plan uses the non-streaming matvecs)";
+    if (!batch_max_rows(p)) return "no row count of the batched Q8_0 stream fits this plan's shapes";
+    return nullptr;
+}
+
+// The per-row scratch: a plan without decode slots allocates it on first use.
+int multi_ready(b200_plan *p) {
+    if (p->bt.x) return B200_OK;
+    const int rc = batch_alloc(p, 0);
+    if (rc) batch_free(p);
+    return rc;
+}
+
+// Enqueues the steps of one call back to back without the classifier: the schedule is uploaded once and k_batch_rows_next
+// feeds each step its entry, so the caller synchronises once.  p->ev0 / ev1 bracket the steps.  own: every row writes the plan's cache (slot 0); otherwise a
+// step whose rows name distinct slots runs the b200_prefill_slots graph, and one with a repeated slot the split form.
+int run_steps(b200_plan *p, const std::vector<BatchRows> &sched, const std::vector<int> &nrows, bool own, int *launches) {
+    auto &B = p->bt;
+    const int steps = (int)sched.size();
+    std::vector<char> split(steps, own);
+    for (int s = 0; s < steps; s++)
+        for (int i = 0; i < nrows[s] && !split[s]; i++)
+            for (int j = 0; j < i; j++)
+                if (sched[s].slot[j] == sched[s].slot[i]) { split[s] = 1; break; }
+    int rc;
+    for (int s = 0; s < steps; s++) {
+        const int n = nrows[s];
+        if (split[s] ? !B.gs[own][0][n] && (rc = capture_batch(p, n, true, true, own)) : !B.gp[n] && (rc = capture_batch(p, n, true))) return rc;
+    }
+    CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
+    CK(cudaEventRecord(p->ev0, p->stream));
+    int k = 0;
+    for (int s = 0; s < steps; s++) {
+        const int n = nrows[s];
+        CK(cudaGraphLaunch(split[s] ? B.gs[own][0][n] : B.gp[n], p->stream));
+        k += split[s] ? B.launches_s[own][0][n] : B.launches_p[n];
+    }
+    CK(cudaEventRecord(p->ev1, p->stream));
+    if (launches) *launches = k;
+    return B200_OK;
+}
+
+// Appends positions start .. start + len - 1 of one sequence to a schedule of rows-wide steps, filling the last step first.
+void pack_rows(std::vector<BatchRows> &sched, std::vector<int> &nrows, int rows, const int *tokens, int start, int len, int slot) {
+    for (int j = 0; j < len; j++) {
+        if (nrows.empty() || nrows.back() == rows) { sched.emplace_back(); nrows.push_back(0); }
+        const int v = nrows.back()++;
+        sched.back().token[v] = tokens[j];
+        sched.back().pos[v] = start + j;
+        sched.back().slot[v] = slot;
+    }
 }
 
 // cudaFuncSetAttribute is per function and process-wide: every kernel gets the device opt-in maximum ONCE, so a later plan
@@ -1094,6 +1184,11 @@ int set_smem_attrs(b200_plan *p) {
     CK(set_max_dyn(k_attention_batch<128>, maxdyn));
     CK(set_max_dyn(k_attention_batch<96>, maxdyn));
     CK(set_max_dyn(k_attention_batch<256>, maxdyn));
+    CK(set_max_dyn(k_attention_cached_rows<32>, maxdyn));
+    CK(set_max_dyn(k_attention_cached_rows<64>, maxdyn));
+    CK(set_max_dyn(k_attention_cached_rows<128>, maxdyn));
+    CK(set_max_dyn(k_attention_cached_rows<96>, maxdyn));
+    CK(set_max_dyn(k_attention_cached_rows<256>, maxdyn));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
@@ -1719,9 +1814,9 @@ int check_device_error(b200_plan *p) {
     return B200_OK;
 }
 
-int set_state(b200_plan *p, int token, int pos, int n_seq, int feedback) {
+int set_state(b200_plan *p, int token, int pos, int n_seq, int feedback, int step = 0) {
     StepState *h = p->h_st;
-    h->token = token; h->pos = pos; h->step = 0; h->n_seq = n_seq; h->feedback = feedback;
+    h->token = token; h->pos = pos; h->step = step; h->n_seq = n_seq; h->feedback = feedback;
     CK(cudaMemcpyAsync(p->st, h, sizeof(StepState), cudaMemcpyHostToDevice, p->stream));
     return B200_OK;
 }
@@ -1885,14 +1980,24 @@ int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, i
         CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
         return B200_OK;
     }
-    // Exact path: the prefill graph token by token (bit-identical KV cache to the CPU
-    // batchForwardJavaPrefill, InferenceCoreBatchPrefillDecode.java:62-168).
+    // Exact path (bit-identical KV cache to the CPU batchForwardJavaPrefill, InferenceCoreBatchPrefillDecode.java:62-168).  Plans
+    // that run multi-position steps take positions start .. start + n - 2 in steps of batch_max_rows rows into the plan's cache;
+    // the last token, and every token elsewhere, runs through the single-token prefill graph, with the step state as the
+    // token-by-token loop leaves it before its last step.
     if (n > p->seq_cap) return fail(p, B200_ERR_BAD_ARG, "chunk too long");
     memcpy(p->h_ids, tokens, (size_t)n * 4);
     CK(cudaMemcpyAsync(p->seq_tokens, p->h_ids, (size_t)n * 4, cudaMemcpyHostToDevice, p->stream));
-    int rc;
-    if ((rc = set_state(p, tokens[0], start_pos, n, 0))) return rc;
-    for (int i = 0; i < n; i++) CK(cudaGraphLaunch(prefill_graph(p), p->stream));
+    int rc, first = 0;
+    if (n > 1 && !multi_why(p)) {
+        if ((rc = multi_ready(p))) return rc;
+        std::vector<BatchRows> sched;
+        std::vector<int> nrows;
+        pack_rows(sched, nrows, batch_max_rows(p), tokens, start_pos, n - 1, 0);
+        if ((rc = run_steps(p, sched, nrows, true, nullptr))) return rc;
+        first = n - 1;
+    }
+    if ((rc = set_state(p, tokens[first], start_pos + first, n, 0, first))) return rc;
+    for (int i = first; i < n; i++) CK(cudaGraphLaunch(prefill_graph(p), p->stream));
     CK(cudaStreamSynchronize(p->stream));
     return check_device_error(p);
 }
@@ -2109,40 +2214,17 @@ int b200_slot_copy_kv(b200_plan *p, int32_t slot, int32_t n_positions) {
 }
 
 namespace {
-// Exact b200_prefill_slots: the batched step without the classifier, one step per position.  Sequences are ordered by length,
-// longest first, so the sequences that still have tokens at step s are rows 0 .. n_s - 1 of that step.  The whole schedule is
-// uploaded once; each step's graph reads its entry through the device step index.
+// Exact b200_prefill_slots: the batched step without the classifier.  The call's tokens, sequence after sequence, are cut into
+// steps of batch_max_rows rows, so a sequence contributes several consecutive positions to a step when rows are free and T tokens
+// take ceil(T / rows) steps.  Steps in which a slot repeats run the split attention form (k_rope_kv_batch, then
+// k_attention_cached_rows); the others the plain batched step.
 int prefill_slots_exact(b200_plan *p, int ns, const int *slots, const int *start, const int *len, const int *off, const int *tokens) {
-    auto &B = p->bt;
-    std::vector<int> ord(ns);
-    for (int i = 0; i < ns; i++) ord[i] = i;
-    std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return len[a] > len[b]; });
-    const int steps = len[ord[0]];
-    std::vector<BatchRows> sched(steps);
-    std::vector<int> nrows(steps);
-    for (int s = 0; s < steps; s++) {
-        int n = 0;
-        for (int i : ord) {
-            if (len[i] <= s) break;
-            sched[s].token[n] = tokens[off[i] + s];
-            sched[s].pos[n] = start[i] + s;
-            sched[s].slot[n] = slots[i];
-            n++;
-        }
-        nrows[s] = n;
-    }
-    int rc;
-    for (int s = 0; s < steps; s++)
-        if (!B.gp[nrows[s]] && (rc = capture_batch(p, nrows[s], true))) return rc;
-    CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
-    CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
-    int launches = 0;
-    CK(cudaEventRecord(p->ev0, p->stream));
-    for (int s = 0; s < steps; s++) {
-        CK(cudaGraphLaunch(B.gp[nrows[s]], p->stream));
-        launches += B.launches_p[nrows[s]];
-    }
-    CK(cudaEventRecord(p->ev1, p->stream));
+    std::vector<BatchRows> sched;
+    std::vector<int> nrows;
+    const int rows = batch_max_rows(p);
+    for (int i = 0; i < ns; i++) pack_rows(sched, nrows, rows, tokens + off[i], start[i], len[i], slots[i]);
+    int rc, launches = 0;
+    if ((rc = run_steps(p, sched, nrows, false, &launches))) return rc;
     CK(cudaStreamSynchronize(p->stream));
     CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
     p->launches_prefill = launches;
@@ -2252,6 +2334,43 @@ int b200_prefill_slots(b200_plan *p, int32_t n_seqs, const int32_t *slots, const
     CK(cudaSetDevice(p->device));
     return tc ? prefill_slots_tc(p, n_seqs, slots, start_positions, lengths, off.data(), tokens, (int)total)
               : prefill_slots_exact(p, n_seqs, slots, start_positions, lengths, off.data(), tokens);
+}
+
+int b200_decode_multi_rows(b200_plan *p, int32_t *max_rows) {
+    if (!p || !max_rows) return B200_ERR_BAD_ARG;
+    *max_rows = multi_why(p) ? 0 : batch_max_rows(p);
+    return B200_OK;
+}
+
+int b200_forward_decode_multi(b200_plan *p, int32_t slot, int32_t n, const int32_t *tokens, int32_t start_pos, int32_t *ids_out, float *logits) {
+    if (!p) return B200_ERR_BAD_ARG;
+    if (const char *why = multi_why(p)) return fail(p, B200_ERR_UNSUPPORTED, "%s", why);
+    auto &B = p->bt;
+    const b200_config &c = p->cfg;
+    const int R = batch_max_rows(p);
+    if (!tokens || !ids_out) return fail(p, B200_ERR_BAD_ARG, "tokens and ids_out must not be NULL");
+    if (n < 1 || n > R) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (b200_decode_multi_rows)", n, R);
+    if (slot < -1 || slot >= B.n_slots) return fail(p, B200_ERR_BAD_ARG, "slot %d out of range (%d slots; -1 is the plan's own cache)", slot, B.n_slots);
+    for (int i = 0; i < n; i++) {
+        if (tokens[i] < 0 || tokens[i] >= c.vocab_size) return fail(p, B200_ERR_BAD_ARG, "row %d: token %d out of range", i, tokens[i]);
+        if (start_pos < 0 || (int64_t)start_pos + i >= c.context_length)
+            return fail(p, B200_ERR_BAD_ARG, "row %d: position %lld outside the KV cache (%d)", i, (long long)start_pos + i, c.context_length);
+    }
+    CK(cudaSetDevice(p->device));
+    int rc;
+    if ((rc = multi_ready(p))) return rc;
+    const bool own = slot < 0;
+    if (!B.gs[own][1][n] && (rc = capture_batch(p, n, false, true, own))) return rc;
+    for (int i = 0; i < n; i++) { B.h_rows->token[i] = tokens[i]; B.h_rows->pos[i] = start_pos + i; B.h_rows->slot[i] = own ? 0 : slot; }
+    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaGraphLaunch(B.gs[own][1][n], p->stream));
+    const size_t vpad = (size_t)sampler_padded(c.vocab_size);
+    if (logits)
+        for (int i = 0; i < n; i++) CK(cudaMemcpyAsync(logits + (size_t)i * c.vocab_size, B.logits + i * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
+    CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)n * 4, cudaMemcpyDeviceToHost, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
+    memcpy(ids_out, B.h_out, (size_t)n * 4);
+    return B200_OK;
 }
 
 int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step) {

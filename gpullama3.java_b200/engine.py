@@ -10,6 +10,8 @@ Position/token conventions decide parity, so they are restated exactly:
 ``generate_tokens_batch``  several requests through the first two loops in lockstep on the plan's decode slots
 ``generate_tokens_batch_prefill`` the third loop for several requests: prompts prefilled straight into the decode slots
                               (prefill_slots), then lockstep decode
+``generate_tokens_lookahead`` the first loop, several positions verified per step (forward_decode_multi): the rest of the
+                              prompt, or drafted tokens, checked in one weight stream; the same ids for any draft
 The sampler is greedy (temperature 0 -> FloatTensor.argmax, Sampler.java:124-132) and runs on
 the device; ``forward`` is any callable (token, position) -> argmax so the same loops drive
 the oracle in the tests.
@@ -216,3 +218,74 @@ def generate_tokens_batch_prefill(plan, model_type: str, requests: list, stop_to
             else:
                 live[i] = (nxt, pos)
     return results
+
+
+def prompt_lookup(history: list[int], max_tokens: int = 8) -> list[int]:
+    """Draft by prompt lookup: the tokens that followed the most recent earlier occurrence of the history's last 3, 2 or 1 tokens
+    (the longest suffix that recurs wins), at most max_tokens of them; [] when none recurs."""
+    n = len(history)
+    for k in (3, 2, 1):
+        if n <= k:
+            continue
+        tail = history[n - k:]
+        for j in range(n - k - 1, -1, -1):
+            if history[j:j + k] == tail:
+                return list(history[j + k:j + k + max_tokens])
+    return []
+
+
+def generate_tokens_lookahead(plan, model_type: str, latest_token: int, start_position: int, prompt_tokens: list[int],
+                              stop_tokens: Iterable[int], max_tokens: int, context_length: int,
+                              draft: Callable[[list[int]], list[int]] = prompt_lookup, stats: dict | None = None) -> list[int]:
+    """generate_tokens_llama on the plan's own cache, verifying several positions per step with forward_decode_multi.
+
+    Each step runs [current] + drafts (up to decode_multi_rows() - 1 drafts) at consecutive positions.  While prompt tokens remain
+    the drafts are the rest of the prompt; after that draft(history) proposes them, history being [latest_token] + prompt + the
+    tokens generated so far.  The rows are then walked as generate_tokens_llama walks its steps: a prompt token is taken whatever
+    the id says, a generated token is the row's id, and the walk goes on to the next row only while that row's input equals the
+    token just taken.  A stop token or the budget ends generation at the same token as there.  Every row is bit-identical to
+    forward_decode of its token over the same cache prefix, and a rejected draft's K/V rows are rewritten before any later row
+    reads them, so the result equals generate_tokens_llama for any draft function.  stats (optional dict) receives the steps run,
+    the drafted tokens that were generated rather than forced, and how many of those were accepted.
+
+    Llama loop only: the Qwen3 loop reads a skipped position as a zero row, which a rejected draft may have written."""
+    if _is_qwen_loop(model_type):
+        raise ValueError(f"{model_type} runs the Qwen3 loop, which has no lookahead form: use generate_tokens_qwen3")
+    rows = plan.decode_multi_rows()
+    if rows < 1:
+        raise ValueError("the plan cannot run multi-position steps (decode_multi_rows() == 0)")
+    if max_tokens < 0 or context_length < max_tokens:
+        max_tokens = context_length
+    stop = set(stop_tokens)
+    prompt = list(prompt_tokens)
+    history = [latest_token] + prompt
+    generated: list[int] = []
+    current, prompt_index, pos = latest_token, 0, start_position
+    steps = drafted = accepted = 0
+    while pos < max_tokens:
+        forced = prompt_index < len(prompt)
+        guesses = prompt[prompt_index:] if forced else list(draft(list(history)))
+        guesses = [int(t) for t in guesses[:min(rows, max_tokens - pos) - 1]]
+        ids, _ = plan.forward_decode_multi(-1, [current] + guesses, pos)
+        steps += 1
+        for i, am in enumerate(ids):
+            if prompt_index < len(prompt):
+                nxt = prompt[prompt_index]
+                prompt_index += 1
+            else:
+                nxt = int(am)
+                generated.append(nxt)
+                history.append(nxt)
+                if i < len(guesses) and not forced:
+                    drafted += 1
+                    accepted += guesses[i] == nxt
+                if nxt in stop:
+                    pos = max_tokens  # ends the outer loop too
+                    break
+            current = nxt
+            pos += 1
+            if i == len(guesses) or guesses[i] != nxt:
+                break
+    if stats is not None:
+        stats.update(steps=steps, drafted=drafted, accepted=accepted)
+    return generated

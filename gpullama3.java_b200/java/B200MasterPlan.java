@@ -79,6 +79,8 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle SLOT_RESET = fn("b200_slot_reset", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle SLOT_COPY_KV = fn("b200_slot_copy_kv", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
     private static final MethodHandle PREFILL_SLOTS = fn("b200_prefill_slots", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
+    private static final MethodHandle DECODE_MULTI = fn("b200_forward_decode_multi", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS));
+    private static final MethodHandle MULTI_ROWS = fn("b200_decode_multi_rows", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle FREE = fn("b200_plan_free", FunctionDescriptor.ofVoid(ADDRESS));
     private static final MethodHandle LAST_ERROR = fn("b200_last_error", FunctionDescriptor.of(ADDRESS, ADDRESS));
 
@@ -301,6 +303,27 @@ public final class B200MasterPlan implements AutoCloseable {
             int rc = (int) PREFILL_SLOTS.invokeExact(plan, n, a.allocateFrom(JAVA_INT, slots), a.allocateFrom(JAVA_INT, startPositions),
                     a.allocateFrom(JAVA_INT, lengths), total == 0 ? MemorySegment.NULL : a.allocateFrom(JAVA_INT, tokens));
             if (rc != 0) check(rc, lastError());
+        }
+    }
+
+    /** tokens[i] at position startPos + i of ONE sequence in one step (slot -1: the plan's own cache); returns the greedy id after
+     *  each position, every row bit-identical to forwardDecode of the same token over the same cache prefix (draft verification). */
+    public int[] forwardDecodeMulti(int slot, int[] tokens, int startPos) throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            MemorySegment ids = a.allocate(JAVA_INT, Math.max(1, tokens.length));
+            int rc = (int) DECODE_MULTI.invokeExact(plan, slot, tokens.length, a.allocateFrom(JAVA_INT, tokens), startPos, ids, MemorySegment.NULL);
+            if (rc != 0) check(rc, lastError());
+            return ids.asSlice(0, 4L * tokens.length).toArray(JAVA_INT);
+        }
+    }
+
+    /** Positions per forwardDecodeMulti step; 0 where the plan cannot run it. */
+    public int decodeMultiRows() throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            MemorySegment r = a.allocate(JAVA_INT);
+            int rc = (int) MULTI_ROWS.invokeExact(plan, r);
+            if (rc != 0) check(rc, lastError());
+            return r.get(JAVA_INT, 0);
         }
     }
 

@@ -53,6 +53,7 @@ EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
+           "b200_forward_decode_multi", "b200_decode_multi_rows",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -100,6 +101,8 @@ def lib() -> C.CDLL:
     L.b200_prefill_slots.argtypes = [vp, i32, vp, vp, vp, vp]
     L.b200_test_pf_attention_packed.argtypes = [i32, vp, vp, vp, vp, vp, i32, i32, i32, vp]
     L.b200_batch_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
+    L.b200_forward_decode_multi.argtypes = [vp, i32, i32, vp, i32, vp, vp]
+    L.b200_decode_multi_rows.argtypes = [vp, C.POINTER(i32)]
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     L.b200_launches_per_decode.argtypes = [vp]
     L.b200_device_bytes.argtypes = [vp]
@@ -401,6 +404,21 @@ class NativePlan:
         a, b, ms = C.c_int32(0), C.c_int32(0), C.c_float(0)
         self._ck(lib().b200_batch_info(self._p, C.byref(a), C.byref(b), C.byref(ms)))
         return a.value, b.value, ms.value
+
+    def forward_decode_multi(self, slot: int, tokens, start_pos: int, want_logits: bool = False):
+        """b200_forward_decode_multi: tokens[i] at start_pos + i of one sequence (slot -1: the plan's own cache) in one step.
+        Returns (ids int32 [n], logits float32 [n, vocab] or None)."""
+        t = np.ascontiguousarray(tokens, dtype=np.int32).reshape(-1)
+        n = len(t)
+        ids = np.empty(max(n, 1), dtype=np.int32)
+        lg = np.empty((n, self.cfg.vocab_size), dtype=np.float32) if want_logits else None
+        self._ck(lib().b200_forward_decode_multi(self._p, slot, n, t.ctypes.data, start_pos, ids.ctypes.data, lg.ctypes.data if want_logits else None))
+        return ids[:n], lg
+
+    def decode_multi_rows(self) -> int:
+        r = C.c_int32(0)
+        self._ck(lib().b200_decode_multi_rows(self._p, C.byref(r)))
+        return r.value
 
     def time_kernel(self, which: int, reps: int = 3):
         ms, nbytes = C.c_float(0), C.c_int64(0)

@@ -186,6 +186,17 @@ class B200MasterPlan:
         """(decode slots, kernels of the last batched step, its device milliseconds)."""
         return self._native.batch_info()
 
+    def forward_decode_multi(self, slot: int, tokens, start_pos: int, logits: bool = False):
+        """Run tokens[i] at position start_pos + i of ONE sequence in one step (slot >= 0: a decode slot; -1: the plan's own cache)
+        -> (ids, logits [n, vocab] or None); ids[i] is the greedy id after position start_pos + i.  Every row is bit-identical to
+        forward_decode of the same token at the same position over the same cache prefix: the verification step of draft-and-verify
+        decoding.  1 <= len(tokens) <= decode_multi_rows(); Q8_0 streaming single-GPU plans without MoE only."""
+        return self._native.forward_decode_multi(slot, tokens, start_pos, logits)
+
+    def decode_multi_rows(self) -> int:
+        """Positions per forward_decode_multi step (8 at the 8B shapes); 0 where the plan cannot run it."""
+        return self._native.decode_multi_rows()
+
     def moe_routing(self):
         """Qwen2-MoE plans: (ids [layer, k], weights [layer, k + 1]) of the last step (selected experts in selection order, their
         routing weights, then the shared-expert weight)."""

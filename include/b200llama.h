@@ -172,12 +172,18 @@ int b200_forward_prefill(b200_plan *plan, int32_t token, int32_t position);
 /* TornadoVMMasterPlanBatchPrefillDecode.tornadoVMForwardBatchPrefill()
  * (TornadoVMMasterPlanBatchPrefillDecode.java:107-123) with explicit arguments instead of
  * state.embeddingXBatch/batchStartPosHolder: tokens[b] is processed at start_pos+b,
- * n <= prefill_batch_size.  KV cache only, no logits (InferenceCoreBatchPrefillDecode.java:166-167). */
+ * n <= prefill_batch_size.  KV cache only, no logits (InferenceCoreBatchPrefillDecode.java:166-167).
+ * In B200_PREFILL_EXACT on plans that run b200_forward_decode_multi, positions start_pos .. start_pos + n - 2 run as multi-position
+ * steps of b200_decode_multi_rows rows into the plan's cache (no classifier) and the last token runs through the single-token
+ * prefill graph, so the single-token buffers and step state are left as the token-by-token loop leaves them; other plans run
+ * every token through that graph.  Either way the KV cache is bit-identical to the CPU path. */
 int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n, int32_t start_pos);
 
 /* How b200_forward_batch_prefill computes (the reference has the same two families:
  * LlamaFP16LayersBatchPrefill vs ...BatchPrefillMMA, selected by TensorCoreSupport.java):
- *   B200_PREFILL_EXACT       the single-token prefill graph per token: KV cache bit-identical to the CPU path;
+ *   B200_PREFILL_EXACT       multi-position steps, then the single-token prefill graph for the chunk's last token (the
+ *                            graph per token on FP16, tensor-parallel, MoE and non-streaming plans): KV cache
+ *                            bit-identical to the CPU path;
  *   B200_PREFILL_TENSOR_CORE TMA + wgmma GEMMs over the whole chunk, FP16 operands / FP32 accumulation:
  *                            KV cache within FP16 tolerance of the CPU path.  Default for FP16 plans created
  *                            with prefill_batch_size > 1.  Opt-in for single-GPU Q8_0 plans: the first call
@@ -268,8 +274,9 @@ int b200_slot_copy_kv(b200_plan *plan, int32_t slot, int32_t n_positions);
 /* Prefill n_seqs prompts, each into its own decode slot: sequence i's tokens tokens[off_i .. off_i + lengths[i]) (concatenated in
  * call order) are processed at positions start_positions[i] .. start_positions[i] + lengths[i] - 1 of slot slots[i].  KV only, no
  * logits.  The mode is the plan's prefill mode (b200_set_prefill_mode):
- *   exact: the batched decode step without its final norm, lm_head and argmax, one step per position (every sequence with tokens
- *          left advances by one); each slot's K/V is bit-identical to the CPU path;
+ *   exact: the batched decode step without its final norm, lm_head and argmax.  The call's T tokens, sequence after sequence, fill
+ *          ceil(T / b200_decode_multi_rows) steps, a sequence taking several consecutive positions of a step when rows are free
+ *          (such steps write every row's K/V before any row attends); each slot's K/V is bit-identical to the CPU path;
  *   tensor-core modes: one chunk of all the tokens through the GEMMs, at most prefill_batch_size tokens per call; each slot's K/V is
  *          what b200_forward_batch_prefill of that prompt alone followed by b200_slot_copy_kv gives, wherever the GEMMs split K
  *          the same way (the split depends on the chunk's total length).
@@ -280,6 +287,20 @@ int b200_slot_copy_kv(b200_plan *plan, int32_t slot, int32_t n_positions);
  * prefill_batch_size in a tensor-core mode.  b200_prefill_info reports the call's launches and device milliseconds. */
 int b200_prefill_slots(b200_plan *plan, int32_t n_seqs, const int32_t *slots, const int32_t *start_positions, const int32_t *lengths,
                        const int32_t *tokens);
+
+/* Run tokens[i] at position start_pos + i, i < n, of ONE sequence in one step: slot >= 0 is a decode slot, slot == -1 the plan's own
+ * cache.  ids_out[i] = greedy id (FloatTensor.argmax) after position start_pos + i; logits (nullable) n x vocab_size floats.  Every
+ * row is bit-identical to b200_forward_decode of the same token at the same position over the same cache prefix; K/V is written at
+ * all n positions, each before any row attends to it, so rows written past an accepted draft are rewritten by the next call before
+ * they are read.  Greedy only: the verification step of draft-and-verify (speculative) decoding.  With slot == -1 the plan's
+ * single-token buffers and step state are not touched.  B200_ERR_BAD_ARG (naming the row) for n outside 1..b200_decode_multi_rows,
+ * a slot out of range, positions outside the KV cache or a bad token; B200_ERR_UNSUPPORTED with the reason on plans that cannot run
+ * it (FP16, tensor-parallel, Qwen2-MoE, the non-streaming Q8_0 layout).  The per-row buffers are allocated on first use. */
+int b200_forward_decode_multi(b200_plan *plan, int32_t slot, int32_t n, const int32_t *tokens, int32_t start_pos, int32_t *ids_out,
+                              float *logits /* nullable, n x vocab */);
+
+/* Rows per b200_forward_decode_multi step (and per step of the exact prefills): 8 at the 8B shapes; 0 where unsupported. */
+int b200_decode_multi_rows(b200_plan *plan, int32_t *max_rows);
 
 /* Decode slots, kernels of the last batched step and its device milliseconds (CUDA events around the graph); any pointer may be NULL. */
 int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step);

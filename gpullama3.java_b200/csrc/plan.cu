@@ -22,6 +22,7 @@
 #include <chrono>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -37,6 +38,21 @@ struct LayerW {
     const unsigned char **gu_bases = nullptr, **dn_bases = nullptr;
     float *router = nullptr, *shared_gate = nullptr; // F32 [n_experts][dim] and [dim]
 };
+
+// A captured CUDA graph and the kernel launches it holds.
+struct Graph {
+    cudaGraphExec_t exec = nullptr;
+    int launches = 0;
+};
+
+// The single-token graphs of one decode implementation: with logits, without (the prefill form), and with trace records.
+struct TokenGraphs {
+    Graph decode, prefill, trace;
+};
+
+// The forms of the batched step (enqueue_batch).  PREFILL*: a step of the exact prefills, its rows from the call's schedule and
+// without the classifier.  *_SPLIT, *_OWN and MULTI*: rows may share a sequence.  *_OWN: the K / V target is the plan's own cache.
+enum BatchKind { BK_DECODE, BK_PREFILL, BK_PREFILL_SPLIT, BK_PREFILL_OWN, BK_MULTI, BK_MULTI_OWN, BK_KINDS };
 
 } // namespace
 
@@ -100,8 +116,8 @@ struct b200_plan {
     StepState *h_st = nullptr; // pinned
     int *h_ids = nullptr;      // pinned, seq_cap
 
-    cudaGraphExec_t g_decode = nullptr, g_prefill = nullptr, g_trace = nullptr; // the multi-kernel decode graph (round 1)
-    cudaGraphExec_t g_pdecode = nullptr, g_pprefill = nullptr, g_ptrace = nullptr; // one persistent kernel per token (decode_persistent.cuh)
+    TokenGraphs graph; // the multi-kernel decode graph (round 1)
+    TokenGraphs pers;  // one persistent kernel per token (decode_persistent.cuh)
     unsigned long long *trace_rec = nullptr;
     int decode_mode = B200_DECODE_GRAPH; // which of the two the forward entry points launch
     float *att_scratch = nullptr; // [heads][ctx] score rows when the context does not fit shared memory
@@ -116,7 +132,7 @@ struct b200_plan {
     int8_t *attq = nullptr; // gathered attention output (quantised) feeding the Wo matvec
     float *atts = nullptr;
     void *peer_open[TP_MAX] = {nullptr};
-    int launches_decode = 0, launches_prefill = 0;
+    int launches_prefill = 0;
     float prefill_ms = 0.f; // device time of the last tensor-core prefill chunk
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 
@@ -146,7 +162,8 @@ struct b200_plan {
     unsigned pd_flags_off = 0;
     bool pd_coop = true;          // launched with the cooperative attribute (co-residency guaranteed by the driver)
 
-    // batched decode (decode_batch.cuh): n_slots KV caches [slot][layer][ctx][kvDim] and per-row activations, one graph per row count
+    // batched decode (decode_batch.cuh): n_slots KV caches [slot][layer][ctx][kvDim] and per-row activations, one graph per step
+    // form and row count, captured on first use
     struct Batch {
         int n_slots = 0;
         std::vector<void *> allocs;
@@ -158,18 +175,10 @@ struct b200_plan {
         unsigned *blk_cnt = nullptr;
         BatchRows *rows = nullptr, *h_rows = nullptr; // device / pinned host
         int *h_out = nullptr;                         // pinned: ids [SMB_MAX_ROWS] then sampler outputs [SMB_MAX_ROWS][8]
-        cudaGraphExec_t g[SMB_MAX_ROWS + 1] = {};
-        int launches[SMB_MAX_ROWS + 1] = {};
-        // exact b200_prefill_slots: the per-step rows of the call [context_length], the device step index, the step graphs without the
-        // classifier (one per row count)
+        // the exact prefills: the per-step rows of the call [context_length], the device step index
         BatchRows *sched = nullptr;
         int *step = nullptr;
-        cudaGraphExec_t gp[SMB_MAX_ROWS + 1] = {};
-        int launches_p[SMB_MAX_ROWS + 1] = {};
-        // steps whose rows may share a sequence (k_rope_kv_batch + k_attention_cached_rows), captured on first use:
-        // [target: 0 the decode slots, 1 the plan's own cache][0 schedule-driven without the classifier, 1 with it][rows]
-        cudaGraphExec_t gs[2][2][SMB_MAX_ROWS + 1] = {};
-        int launches_s[2][2][SMB_MAX_ROWS + 1] = {};
+        Graph g[BK_KINDS][SMB_MAX_ROWS + 1];
         int last_n = 0;
         float last_ms = 0.f;
     } bt;
@@ -201,6 +210,28 @@ template <typename K> cudaError_t set_max_dyn(K kern, int maxdyn) {
     cudaError_t e = cudaFuncGetAttributes(&fa, kern);
     if (e != cudaSuccess) return e;
     return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, maxdyn - (int)fa.sharedSizeBytes);
+}
+
+// f(std::integral_constant<int, HS>()) for a head size the decode attention kernels are compiled for (k_attention,
+// k_attention_batch, k_rope_kv_batch, k_attention_cached_rows); build() refuses every other size.
+template <typename F> int with_decode_head_size(b200_plan *p, int hs, F &&f) {
+    switch (hs) {
+    case 32: return f(std::integral_constant<int, 32>());
+    case 64: return f(std::integral_constant<int, 64>());
+    case 96: return f(std::integral_constant<int, 96>());
+    case 128: return f(std::integral_constant<int, 128>());
+    case 256: return f(std::integral_constant<int, 256>());
+    }
+    return fail(p, B200_ERR_UNSUPPORTED, "head size %d has no decode attention kernel", hs);
+}
+
+// The same for the sizes of the tensor-core prefill attention (k_pf_*) and the persistent decode kernel.
+template <typename F> int with_mma_head_size(b200_plan *p, int hs, F &&f) {
+    switch (hs) {
+    case 64: return f(std::integral_constant<int, 64>());
+    case 128: return f(std::integral_constant<int, 128>());
+    }
+    return fail(p, B200_ERR_UNSUPPORTED, "head size %d has no tensor-core prefill or persistent decode kernel", hs);
 }
 
 template <typename T> int dalloc(b200_plan *p, T **ptr, size_t n_bytes) {
@@ -703,22 +734,14 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
         }
         if (rc) return rc; n++;
         float *kc = p->key_cache + (size_t)l * ctx_kv, *vc = p->value_cache + (size_t)l * ctx_kv;
-        {
-            const size_t att_smem = att_smem_bytes(c.head_size, c.context_length, p->att_scratch != nullptr);
-            auto att = [&](auto kern) {
-                return launch_k(p, pdl, kern, dim3(p->nh_l), dim3(ATT_THREADS), att_smem, p->qkv, kc, vc, (const StepState *)p->st,
-                                (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags, (const float *)L.q_norm,
-                                (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, att_score_arg(p), q8 ? p->attq : nullptr, q8 ? p->atts : nullptr, xbf, TR(4),
-                                p->tp, (unsigned)(4 * l + 0), rank * p->nh_l, p->att_scratch, c.context_length);
-            };
-            if (c.head_size == 128) rc = att(k_attention<128>);
-            else if (c.head_size == 64) rc = att(k_attention<64>);
-            else if (c.head_size == 256) rc = att(k_attention<256>);
-            else if (c.head_size == 96) rc = att(k_attention<96>);
-            else rc = att(k_attention<32>);
-            if (rc) return rc;
-            n++;
-        }
+        const size_t att_smem = att_smem_bytes(c.head_size, c.context_length, p->att_scratch != nullptr);
+        rc = with_decode_head_size(p, c.head_size, [&](auto HS) {
+            return launch_k(p, pdl, k_attention<HS>, dim3(p->nh_l), dim3(ATT_THREADS), att_smem, p->qkv, kc, vc, (const StepState *)p->st,
+                            (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags, (const float *)L.q_norm,
+                            (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, att_score_arg(p), q8 ? p->attq : nullptr, q8 ? p->atts : nullptr, xbf, TR(4),
+                            p->tp, (unsigned)(4 * l + 0), rank * p->nh_l, p->att_scratch, c.context_length);
+        });
+        if (rc) return rc; n++;
         if (st) rc = launch_stream<SMV_RESID>(p, L.two, p->attq, p->atts, p->x, nullptr, nullptr, false, TR(5), tpar ? TP_SLOT_ATT : -1, 4 * l + 0, tpar ? TP_SLOT_X : -1, 4 * l + 1, rank * p->dim_l);
         else if (q8) rc = launch_matvec_q8<MODE_RESID>(p, L.wo, p->xq, p->xs, p->x);
         else if (sf) rc = launch_stream_f16<SF_RESID>(p, L.wo, nullptr, p->xb, p->x, TR(5));
@@ -818,8 +841,7 @@ int pd_prepare(b200_plan *p) {
         if ((rc = dalloc(p, &p->pd_trace, (size_t)p->n_sms * (c.n_layers + 1) * PD_STAMPS * 8))) return rc;
         CK(cudaMemset(p->pd_trace, 0, (size_t)p->n_sms * (c.n_layers + 1) * PD_STAMPS * 8));
     }
-    CK(set_max_dyn(k_decode_persistent<128>, maxdyn));
-    CK(set_max_dyn(k_decode_persistent<64>, maxdyn));
+    if ((rc = with_mma_head_size(p, c.head_size, [&](auto HS) { CK(set_max_dyn(k_decode_persistent<HS>, maxdyn)); return B200_OK; }))) return rc;
     p->pd_L = L;
     p->pd_ok = true;
     p->pd_why = "";
@@ -854,33 +876,45 @@ int enqueue_persistent(b200_plan *p, bool with_logits, int *launches, bool trace
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
     cfg.numAttrs = p->pd_coop ? 1 : 0;
-    if (c.head_size == 128) CK(cudaLaunchKernelEx(&cfg, k_decode_persistent<128>, a, p->pd_L));
-    else CK(cudaLaunchKernelEx(&cfg, k_decode_persistent<64>, a, p->pd_L));
     if (launches) *launches = 1;
-    return B200_OK;
+    return with_mma_head_size(p, c.head_size, [&](auto HS) { CK(cudaLaunchKernelEx(&cfg, k_decode_persistent<HS>, a, p->pd_L)); return B200_OK; });
 }
 
-int capture(b200_plan *p, bool with_logits, cudaGraphExec_t *exec, int *launches, bool trace = false, bool persistent = false) {
-    cudaGraph_t g = nullptr;
+// Captures what enqueue(&g.launches) puts on p->stream into g.
+template <typename Enqueue> int capture(b200_plan *p, Graph &g, Enqueue &&enqueue) {
+    cudaGraph_t cg = nullptr;
     CK(cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal));
-    int rc = persistent ? enqueue_persistent(p, with_logits, launches, trace) : enqueue_forward(p, with_logits, launches, trace);
-    cudaError_t e = cudaStreamEndCapture(p->stream, &g);
-    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+    int rc = enqueue(&g.launches);
+    cudaError_t e = cudaStreamEndCapture(p->stream, &cg);
+    if (rc) { if (cg) cudaGraphDestroy(cg); return rc; }
     if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(e));
-    e = cudaGraphInstantiate(exec, g, 0);
-    cudaGraphDestroy(g);
+    e = cudaGraphInstantiate(&g.exec, cg, 0);
+    cudaGraphDestroy(cg);
     if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e));
     return B200_OK;
 }
 
+void destroy(Graph &g) {
+    if (g.exec) cudaGraphExecDestroy(g.exec);
+    g = Graph{};
+}
+
+void destroy(TokenGraphs &t) {
+    for (Graph *g : {&t.decode, &t.prefill, &t.trace}) destroy(*g);
+}
+
 // Both decode implementations are captured; b200_set_decode_mode picks which one the forward calls launch.
 int capture_all(b200_plan *p) {
+    auto token = [&](Graph &g, bool persistent, bool with_logits, bool trace) {
+        return capture(p, g, [&](int *launches) {
+            return persistent ? enqueue_persistent(p, with_logits, launches, trace) : enqueue_forward(p, with_logits, launches, trace);
+        });
+    };
+    TokenGraphs &G = p->graph, &P = p->pers;
     int rc;
-    if ((rc = capture(p, true, &p->g_decode, &p->launches_decode))) return rc;
-    if ((rc = capture(p, false, &p->g_prefill, nullptr))) return rc;
+    if ((rc = token(G.decode, false, true, false)) || (rc = token(G.prefill, false, false, false))) return rc;
     if (p->use_stream || p->use_f16_stream) {
-        if ((rc = dalloc(p, &p->trace_rec, (size_t)(p->launches_decode + 8) * 32))) return rc;
-        if ((rc = capture(p, true, &p->g_trace, nullptr, true))) return rc;
+        if ((rc = dalloc(p, &p->trace_rec, (size_t)(G.decode.launches + 8) * 32)) || (rc = token(G.trace, false, true, true))) return rc;
     }
     if ((rc = pd_prepare(p))) return rc;
     if (p->pd_ok) {
@@ -888,13 +922,9 @@ int capture_all(b200_plan *p) {
         // attribute makes the driver check it.  Should a driver refuse cooperative kernel nodes in a graph, retry without.
         for (int attempt = 0; attempt < 2; attempt++) {
             p->pd_coop = attempt == 0;
-            rc = capture(p, true, &p->g_pdecode, nullptr, false, true);
-            if (!rc) rc = capture(p, false, &p->g_pprefill, nullptr, false, true);
-            if (!rc) rc = capture(p, true, &p->g_ptrace, nullptr, true, true);
-            if (!rc) break;
+            if (!(rc = token(P.decode, true, true, false)) && !(rc = token(P.prefill, true, false, false)) && !(rc = token(P.trace, true, true, true))) break;
             cudaGetLastError();
-            for (cudaGraphExec_t *g : {&p->g_pdecode, &p->g_pprefill, &p->g_ptrace})
-                if (*g) { cudaGraphExecDestroy(*g); *g = nullptr; }
+            destroy(P);
         }
         if (rc) { p->pd_ok = false; p->pd_why = "persistent decode kernel could not be captured: " + p->err; }
     }
@@ -931,10 +961,12 @@ int launch_stream_batch(b200_plan *p, const TileMat &W, int n, const int8_t *xq,
 }
 
 // One forward step of n rows: the single-sequence graph's kernel sequence, every launch serving all n rows.  prefill: a step of
-// b200_prefill_slots -- the rows come from the call's schedule (k_batch_rows_next) and there is no final norm, lm_head or argmax.
+// the exact prefills -- the rows come from the call's schedule (k_batch_rows_next) and there is no final norm, lm_head or argmax.
 // split: rows may share a sequence, so the attention runs as k_rope_kv_batch + k_attention_cached_rows (one more launch per
 // layer).  own: the K / V target is the plan's cache (key_cache / value_cache, slot 0's layout) instead of the decode slots.
-int enqueue_batch(b200_plan *p, int n, int *launches, bool prefill = false, bool split = false, bool own = false) {
+int enqueue_batch(b200_plan *p, int n, BatchKind kind, int *launches) {
+    const bool prefill = kind == BK_PREFILL || kind == BK_PREFILL_SPLIT || kind == BK_PREFILL_OWN;
+    const bool split = kind != BK_DECODE && kind != BK_PREFILL, own = kind == BK_PREFILL_OWN || kind == BK_MULTI_OWN;
     const b200_config &c = p->cfg;
     auto &B = p->bt;
     const bool pdl = p->use_pdl;
@@ -961,33 +993,22 @@ int enqueue_batch(b200_plan *p, int n, int *launches, bool prefill = false, bool
         if ((rc = norm(l == 0, L.attn_norm))) return rc;
         if ((rc = launch_stream_batch<SMV_STORE>(p, L.tqkv, n, B.xq, B.xs, B.qkv, qkvd))) return rc;
         float *kc = (own ? p->key_cache : B.slot_k) + (size_t)l * ctx_kv, *vc = (own ? p->value_cache : B.slot_v) + (size_t)l * ctx_kv;
-        // split: the two launches of a step whose rows may share a sequence
-        auto att2 = [&](auto rope_kern, auto att_kern, int hs) {
-            const int r = launch_k(p, pdl, rope_kern, dim3(p->nh_l, n), dim3(2 * hs), (size_t)0, B.qkv, qkvd, kc, vc, slot_stride, (const BatchRows *)B.rows,
+        const size_t att_smem = att_smem_bytes(c.head_size, c.context_length, B.att_scratch != nullptr);
+        rc = with_decode_head_size(p, c.head_size, [&](auto HS) {
+            if (!split)
+                return launch_k(p, pdl, k_attention_batch<HS>, dim3(p->nh_l, n), dim3(ATT_THREADS), att_smem, B.qkv, qkvd, kc, vc, slot_stride,
+                                (const BatchRows *)B.rows, (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags,
+                                (const float *)L.q_norm, (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, att_score_arg(p), B.xq,
+                                B.xs, B.att_scratch, c.context_length, TraceBuf{nullptr, 0, 0}, solo);
+            // split: the two launches of a step whose rows may share a sequence
+            const int r = launch_k(p, pdl, k_rope_kv_batch<HS>, dim3(p->nh_l, n), dim3(2 * HS), (size_t)0, B.qkv, qkvd, kc, vc, slot_stride, (const BatchRows *)B.rows,
                                    (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags, (const float *)L.q_norm,
                                    (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps);
             k++;
-            return r ? r : launch_k(p, pdl, att_kern, dim3(p->nh_l, n), dim3(ATT_THREADS), att_smem_bytes(c.head_size, c.context_length, B.att_scratch != nullptr),
-                                    B.qkv, qkvd, kc, vc, slot_stride, (const BatchRows *)B.rows, p->nh_l, p->nkv_l, p->kflags, att_score_arg(p), B.xq, B.xs,
-                                    B.att_scratch, c.context_length, TraceBuf{nullptr, 0, 0}, solo);
-        };
-        auto att = [&](auto kern) {
-            return launch_k(p, pdl, kern, dim3(p->nh_l, n), dim3(ATT_THREADS), att_smem_bytes(c.head_size, c.context_length, B.att_scratch != nullptr), B.qkv, qkvd,
-                            kc, vc, slot_stride, (const BatchRows *)B.rows, (const float *)p->rope_cr, (const float *)p->rope_ci, p->nh_l, p->nkv_l, p->kflags,
-                            (const float *)L.q_norm, (const float *)L.k_norm, (const float *)L.qkv_bias, c.rms_norm_eps, att_score_arg(p), B.xq,
-                            B.xs, B.att_scratch, c.context_length, TraceBuf{nullptr, 0, 0}, solo);
-        };
-        if (split) {
-            if (c.head_size == 128) rc = att2(k_rope_kv_batch<128>, k_attention_cached_rows<128>, 128);
-            else if (c.head_size == 64) rc = att2(k_rope_kv_batch<64>, k_attention_cached_rows<64>, 64);
-            else if (c.head_size == 256) rc = att2(k_rope_kv_batch<256>, k_attention_cached_rows<256>, 256);
-            else if (c.head_size == 96) rc = att2(k_rope_kv_batch<96>, k_attention_cached_rows<96>, 96);
-            else rc = att2(k_rope_kv_batch<32>, k_attention_cached_rows<32>, 32);
-        } else if (c.head_size == 128) rc = att(k_attention_batch<128>);
-        else if (c.head_size == 64) rc = att(k_attention_batch<64>);
-        else if (c.head_size == 256) rc = att(k_attention_batch<256>);
-        else if (c.head_size == 96) rc = att(k_attention_batch<96>);
-        else rc = att(k_attention_batch<32>);
+            return r ? r : launch_k(p, pdl, k_attention_cached_rows<HS>, dim3(p->nh_l, n), dim3(ATT_THREADS), att_smem, B.qkv, qkvd, kc, vc, slot_stride,
+                                    (const BatchRows *)B.rows, p->nh_l, p->nkv_l, p->kflags, att_score_arg(p), B.xq, B.xs, B.att_scratch, c.context_length,
+                                    TraceBuf{nullptr, 0, 0}, solo);
+        });
         if (rc) return rc;
         if ((rc = launch_stream_batch<SMV_RESID>(p, L.two, n, B.xq, B.xs, B.x, c.dim))) return rc;
         if ((rc = norm(false, L.ffn_norm))) return rc;
@@ -1006,31 +1027,19 @@ int enqueue_batch(b200_plan *p, int n, int *launches, bool prefill = false, bool
     return B200_OK;
 }
 
-int capture_batch(b200_plan *p, int n, bool prefill = false, bool split = false, bool own = false) {
-    auto &B = p->bt;
-    cudaGraph_t g = nullptr;
-    CK(cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal));
-    int *launches = split ? &B.launches_s[own][!prefill][n] : prefill ? &B.launches_p[n] : &B.launches[n];
-    int rc = enqueue_batch(p, n, launches, prefill, split, own);
-    cudaError_t e = cudaStreamEndCapture(p->stream, &g);
-    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
-    if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaStreamEndCapture: %s", cudaGetErrorString(e));
-    e = cudaGraphInstantiate(split ? &B.gs[own][!prefill][n] : prefill ? &B.gp[n] : &B.g[n], g, 0);
-    cudaGraphDestroy(g);
-    if (e != cudaSuccess) return fail(p, B200_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e));
+// The step graph of `kind` for n rows, captured on first use.
+int batch_graph(b200_plan *p, BatchKind kind, int n, const Graph **out) {
+    Graph &g = p->bt.g[kind][n];
+    int rc;
+    if (!g.exec && (rc = capture(p, g, [&](int *launches) { return enqueue_batch(p, n, kind, launches); }))) return rc;
+    *out = &g;
     return B200_OK;
 }
 
 void batch_free(b200_plan *p) {
     auto &B = p->bt;
-    for (cudaGraphExec_t &g : B.g)
-        if (g) { cudaGraphExecDestroy(g); g = nullptr; }
-    for (cudaGraphExec_t &g : B.gp)
-        if (g) { cudaGraphExecDestroy(g); g = nullptr; }
-    for (auto &by_target : B.gs)
-        for (auto &by_kind : by_target)
-            for (cudaGraphExec_t &g : by_kind)
-                if (g) { cudaGraphExecDestroy(g); g = nullptr; }
+    for (auto &by_kind : B.g)
+        for (Graph &g : by_kind) destroy(g);
     for (void *d : B.allocs) cudaFree(d);
     if (B.h_rows) cudaFreeHost(B.h_rows);
     if (B.h_out) cudaFreeHost(B.h_out);
@@ -1095,24 +1104,23 @@ int multi_ready(b200_plan *p) {
 int run_steps(b200_plan *p, const std::vector<BatchRows> &sched, const std::vector<int> &nrows, bool own, int *launches) {
     auto &B = p->bt;
     const int steps = (int)sched.size();
-    std::vector<char> split(steps, own);
-    for (int s = 0; s < steps; s++)
-        for (int i = 0; i < nrows[s] && !split[s]; i++)
-            for (int j = 0; j < i; j++)
-                if (sched[s].slot[j] == sched[s].slot[i]) { split[s] = 1; break; }
+    std::vector<const Graph *> graphs(steps);
     int rc;
     for (int s = 0; s < steps; s++) {
-        const int n = nrows[s];
-        if (split[s] ? !B.gs[own][0][n] && (rc = capture_batch(p, n, true, true, own)) : !B.gp[n] && (rc = capture_batch(p, n, true))) return rc;
+        bool split = false;
+        for (int i = 0; i < nrows[s] && !split; i++)
+            for (int j = 0; j < i; j++)
+                if (sched[s].slot[j] == sched[s].slot[i]) { split = true; break; }
+        const BatchKind kind = own ? BK_PREFILL_OWN : split ? BK_PREFILL_SPLIT : BK_PREFILL;
+        if ((rc = batch_graph(p, kind, nrows[s], &graphs[s]))) return rc;
     }
     CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
     CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
     CK(cudaEventRecord(p->ev0, p->stream));
     int k = 0;
-    for (int s = 0; s < steps; s++) {
-        const int n = nrows[s];
-        CK(cudaGraphLaunch(split[s] ? B.gs[own][0][n] : B.gp[n], p->stream));
-        k += split[s] ? B.launches_s[own][0][n] : B.launches_p[n];
+    for (const Graph *g : graphs) {
+        CK(cudaGraphLaunch(g->exec, p->stream));
+        k += g->launches;
     }
     CK(cudaEventRecord(p->ev1, p->stream));
     if (launches) *launches = k;
@@ -1152,11 +1160,15 @@ int set_smem_attrs(b200_plan *p) {
     if (done) return B200_OK;
     CK(set_max_dyn(k_rmsnorm_quant<true>, maxdyn));
     CK(set_max_dyn(k_rmsnorm_quant<false>, maxdyn));
-    CK(set_max_dyn(k_attention<32>, maxdyn));
-    CK(set_max_dyn(k_attention<64>, maxdyn));
-    CK(set_max_dyn(k_attention<128>, maxdyn));
-    CK(set_max_dyn(k_attention<96>, maxdyn));
-    CK(set_max_dyn(k_attention<256>, maxdyn));
+    for (int hs : {32, 64, 96, 128, 256}) {
+        const int rc = with_decode_head_size(p, hs, [&](auto HS) {
+            CK(set_max_dyn(k_attention<HS>, maxdyn));
+            CK(set_max_dyn(k_attention_batch<HS>, maxdyn));
+            CK(set_max_dyn(k_attention_cached_rows<HS>, maxdyn));
+            return B200_OK;
+        });
+        if (rc) return rc;
+    }
     CK(set_max_dyn(k_matvec_q8<1, MODE_STORE>, maxdyn));
     CK(set_max_dyn(k_matvec_q8<2, MODE_STORE>, maxdyn));
     CK(set_max_dyn(k_matvec_q8<4, MODE_STORE>, maxdyn));
@@ -1179,21 +1191,12 @@ int set_smem_attrs(b200_plan *p) {
     CK(set_max_dyn(k_stream_matvec_f16<8, SF_GATEUP>, maxdyn));
     CK(set_max_dyn(k_rmsnorm_quant_batch<true>, maxdyn));
     CK(set_max_dyn(k_rmsnorm_quant_batch<false>, maxdyn));
-    CK(set_max_dyn(k_attention_batch<32>, maxdyn));
-    CK(set_max_dyn(k_attention_batch<64>, maxdyn));
-    CK(set_max_dyn(k_attention_batch<128>, maxdyn));
-    CK(set_max_dyn(k_attention_batch<96>, maxdyn));
-    CK(set_max_dyn(k_attention_batch<256>, maxdyn));
-    CK(set_max_dyn(k_attention_cached_rows<32>, maxdyn));
-    CK(set_max_dyn(k_attention_cached_rows<64>, maxdyn));
-    CK(set_max_dyn(k_attention_cached_rows<128>, maxdyn));
-    CK(set_max_dyn(k_attention_cached_rows<96>, maxdyn));
-    CK(set_max_dyn(k_attention_cached_rows<256>, maxdyn));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_moe_gateup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_moe_down, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    CK(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     done = true;
     return B200_OK;
 }
@@ -1599,14 +1602,11 @@ static int prefill_scratch(b200_plan *p, bool *ok) {
     *ok = pg::make_map(&c.mA, c.A16, c.bpad, g.dim, pg::BM) == 0 && pg::make_map(&c.mATT, c.ATT16, c.bpad, p->qd, pg::BM) == 0 &&
           pg::make_map(&c.mH, c.H16, c.bpad, g.hidden_dim, pg::BM) == 0 && pg::make_map_c(&c.mX, c.X, c.bpad, g.dim) == 0 &&
           pg::make_map_c(&c.mQKV, c.QKV, c.bpad, nqkv) == 0;
-    if (g.head_size == 128) {
-        CK(cudaFuncSetAttribute(k_pf_attention_mma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>()));
-        CK(cudaFuncSetAttribute(k_pf_attention_mma_packed<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>()));
-    } else {
-        CK(cudaFuncSetAttribute(k_pf_attention_mma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<64>()));
-        CK(cudaFuncSetAttribute(k_pf_attention_mma_packed<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<64>()));
-    }
-    return B200_OK;
+    return with_mma_head_size(p, g.head_size, [&](auto HS) {
+        CK(cudaFuncSetAttribute(k_pf_attention_mma<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<HS>()));
+        CK(cudaFuncSetAttribute(k_pf_attention_mma_packed<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<HS>()));
+        return B200_OK;
+    });
 }
 
 int prefill_init(b200_plan *p) {
@@ -1748,6 +1748,7 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfP
             return fail(p, B200_ERR_CUDA, "QKV GEMM launch failed");
         nl++;
         const int qt = PM_ROWS / kv_mul;
+        int rc;
         if (pk) {
             const size_t slot_stride = (size_t)g.n_layers * ctx_kv;
             if (pk->n_hist) {
@@ -1757,13 +1758,11 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfP
                 nl++;
             }
             const dim3 ag(pk->n_tiles, g.n_kv_heads);
-            if (g.head_size == 128) {
-                k_pf_rope_kv_packed<128><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, slot_stride, pk->KH, pk->VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, pk->tok);
-                k_pf_attention_mma_packed<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), s>>>(c.QKV, nqkv, pk->KH, pk->VH, p->kvd, kv_mul, pk->tiles, inv_sqrt_hs, c.ATT16, p->qd);
-            } else {
-                k_pf_rope_kv_packed<64><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, slot_stride, pk->KH, pk->VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, pk->tok);
-                k_pf_attention_mma_packed<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), s>>>(c.QKV, nqkv, pk->KH, pk->VH, p->kvd, kv_mul, pk->tiles, inv_sqrt_hs, c.ATT16, p->qd);
-            }
+            rc = with_mma_head_size(p, g.head_size, [&](auto HS) {
+                k_pf_rope_kv_packed<HS><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, slot_stride, pk->KH, pk->VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, pk->tok);
+                k_pf_attention_mma_packed<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), s>>>(c.QKV, nqkv, pk->KH, pk->VH, p->kvd, kv_mul, pk->tiles, inv_sqrt_hs, c.ATT16, p->qd);
+                return B200_OK;
+            });
         } else {
             const dim3 ag((n + qt - 1) / qt, g.n_kv_heads);
             if (start_pos > 0) { // rows written by earlier chunks / decode steps
@@ -1771,14 +1770,13 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfP
                 k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, s>>>(kc, vc, c.KH, c.VH, n4);
                 nl++;
             }
-            if (g.head_size == 128) {
-                k_pf_rope_kv<128><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
-                k_pf_attention_mma<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
-            } else {
-                k_pf_rope_kv<64><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
-                k_pf_attention_mma<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
-            }
+            rc = with_mma_head_size(p, g.head_size, [&](auto HS) {
+                k_pf_rope_kv<HS><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
+                k_pf_attention_mma<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
+                return B200_OK;
+            });
         }
+        if (rc) return rc;
         nl += 2;
         const int sp_wo = splits(g.dim / pg::BN, p->qd), sp_w2 = splits(g.dim / pg::BN, g.hidden_dim);
         const float rs = p->mup.residual_scale;
@@ -1801,8 +1799,20 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfP
     return B200_OK;
 }
 
-cudaGraphExec_t decode_graph(b200_plan *p) { return p->decode_mode == B200_DECODE_PERSISTENT && p->g_pdecode ? p->g_pdecode : p->g_decode; }
-cudaGraphExec_t prefill_graph(b200_plan *p) { return p->decode_mode == B200_DECODE_PERSISTENT && p->g_pprefill ? p->g_pprefill : p->g_prefill; }
+// The single-token graphs the forward calls launch: the persistent kernel's when that mode is selected and captured.
+const TokenGraphs &active_graphs(const b200_plan *p) { return p->decode_mode == B200_DECODE_PERSISTENT && p->pers.decode.exec ? p->pers : p->graph; }
+cudaGraphExec_t decode_graph(const b200_plan *p) { return active_graphs(p).decode.exec; }
+cudaGraphExec_t prefill_graph(const b200_plan *p) { return active_graphs(p).prefill.exec; }
+
+// The device sampler (sampler.cuh) on one logits row: the token at out[0], its four diagnostics at out[1..4].
+int launch_sample(b200_plan *p, float *logits, float temperature, float topp, float uniform01, int *out) {
+    SamplerArgs a;
+    a.logits = logits; a.n = p->cfg.vocab_size; a.temperature = temperature; a.topp = topp; a.r01 = uniform01;
+    a.indices = p->smp_indices; a.out_id = out; a.info = out + 1;
+    k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
+    CK(cudaGetLastError());
+    return B200_OK;
+}
 
 // After a synchronize: did a device-side wait of the persistent kernel (or a tensor-parallel flag wait) give up?
 int check_device_error(b200_plan *p) {
@@ -1825,6 +1835,34 @@ int check_pos(b200_plan *p, int token, int pos) {
     if (token < 0 || token >= p->cfg.vocab_size) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", token);
     if (pos < 0 || pos >= p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "position %d outside the KV cache (%d)", pos, p->cfg.context_length);
     return B200_OK;
+}
+
+// Device memory and the result code of an entry point without a plan.  ok() keeps the first failure (an allocation failure is
+// B200_ERR_OOM, any other B200_ERR_CUDA) and answers whether everything so far succeeded; the allocations are freed at scope exit.
+struct Scratch {
+    int rc = B200_OK;
+    std::vector<void *> mem;
+    bool ok(cudaError_t e) {
+        if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA;
+        return rc == B200_OK;
+    }
+    template <typename T> bool alloc(T **ptr, size_t bytes) {
+        void *d = nullptr;
+        const cudaError_t e = cudaMalloc(&d, bytes);
+        if (e == cudaSuccess) mem.push_back(d);
+        *ptr = reinterpret_cast<T *>(d);
+        return ok(e);
+    }
+    ~Scratch() {
+        for (void *d : mem) cudaFree(d);
+    }
+};
+
+// f(std::integral_constant<int, MODE>()) for a checked run-time pg::GEMM_* mode.
+template <typename F> int with_gemm_mode(int mode, F &&f) {
+    if (mode == pg::GEMM_F32) return f(std::integral_constant<int, pg::GEMM_F32>());
+    if (mode == pg::GEMM_RESID) return f(std::integral_constant<int, pg::GEMM_RESID>());
+    return f(std::integral_constant<int, pg::GEMM_GATEUP>());
 }
 
 } // namespace
@@ -1904,7 +1942,7 @@ int b200_plan_create_granite(const b200_config *cfg, const b200_granite_config *
 
 int b200_forward_decode(b200_plan *p, int32_t token, int32_t position, float *logits, int32_t *argmax) {
     if (!p) return B200_ERR_BAD_ARG;
-    if (!p->g_decode) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
+    if (!p->graph.decode.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     if (logits && p->tp.n > 1) return fail(p, B200_ERR_UNSUPPORTED, "full logits are not gathered under tensor parallelism (argmax is)");
     int rc;
     if ((rc = check_pos(p, token, position))) return rc;
@@ -1921,7 +1959,7 @@ int b200_forward_decode(b200_plan *p, int32_t token, int32_t position, float *lo
 
 int b200_forward_decode_sample(b200_plan *p, int32_t token, int32_t position, float temperature, float topp, float uniform01, int32_t *token_out, int32_t *info) {
     if (!p || !token_out) return B200_ERR_BAD_ARG;
-    if (!p->g_decode) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
+    if (!p->graph.decode.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     if (p->tp.n > 1) return fail(p, B200_ERR_UNSUPPORTED, "the device-side temperature/top-p sampler needs the whole logits row on one GPU (tensor-parallel plans sample greedily)");
     if (!(temperature >= 0.0f) || !(uniform01 >= 0.0f && uniform01 < 1.0f)) return fail(p, B200_ERR_BAD_ARG, "temperature must be >= 0 and the uniform number in [0, 1)");
     int rc;
@@ -1931,13 +1969,7 @@ int b200_forward_decode_sample(b200_plan *p, int32_t token, int32_t position, fl
     CK(cudaGraphLaunch(decode_graph(p), p->stream));
     const bool greedy = temperature == 0.0f; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed by the forward
     if (!greedy) {
-        static bool attr = false;
-        if (!attr) { CK(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes())); attr = true; }
-        SamplerArgs a;
-        a.logits = p->logits; a.n = p->cfg.vocab_size; a.temperature = temperature; a.topp = topp; a.r01 = uniform01;
-        a.indices = p->smp_indices; a.out_id = p->smp_out; a.info = p->smp_out + 1;
-        k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
-        CK(cudaGetLastError());
+        if ((rc = launch_sample(p, p->logits, temperature, topp, uniform01, p->smp_out))) return rc;
         CK(cudaMemcpyAsync(p->h_ids, p->smp_out, 5 * 4, cudaMemcpyDeviceToHost, p->stream));
     } else CK(cudaMemcpyAsync(p->h_ids, p->out_ids, 4, cudaMemcpyDeviceToHost, p->stream));
     CK(cudaStreamSynchronize(p->stream));
@@ -1949,7 +1981,7 @@ int b200_forward_decode_sample(b200_plan *p, int32_t token, int32_t position, fl
 
 int b200_forward_prefill(b200_plan *p, int32_t token, int32_t position) {
     if (!p) return B200_ERR_BAD_ARG;
-    if (!p->g_prefill) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
+    if (!p->graph.prefill.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     int rc;
     if ((rc = check_pos(p, token, position))) return rc;
     CK(cudaSetDevice(p->device));
@@ -1962,7 +1994,7 @@ int b200_forward_prefill(b200_plan *p, int32_t token, int32_t position) {
 int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, int32_t start_pos) {
     if (!p || !tokens) return B200_ERR_BAD_ARG;
     if (n <= 0) return B200_OK;
-    if (!p->g_prefill) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
+    if (!p->graph.prefill.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     if (p->prefill_batch > 1 && n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "chunk of %d tokens exceeds prefill_batch_size %d", n, p->prefill_batch);
     if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache", start_pos, start_pos + n - 1);
     for (int i = 0; i < n; i++)
@@ -2006,7 +2038,7 @@ int b200_decode_sequence(b200_plan *p, const int32_t *tokens, int32_t n, int32_t
                          int32_t *out_ids, float *device_ms) {
     if (!p || !tokens) return B200_ERR_BAD_ARG;
     if (n <= 0) return B200_OK;
-    if (!p->g_decode) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
+    if (!p->graph.decode.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     if (n > p->seq_cap) return fail(p, B200_ERR_BAD_ARG, "sequence of %d steps exceeds capacity %d", n, p->seq_cap);
     if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache (%d)", start_pos, start_pos + n - 1, p->cfg.context_length);
     int nt = feedback ? 1 : n;
@@ -2030,7 +2062,7 @@ int b200_decode_sequence(b200_plan *p, const int32_t *tokens, int32_t n, int32_t
 
 int b200_set_decode_mode(b200_plan *p, int32_t mode) {
     if (!p || (mode != B200_DECODE_GRAPH && mode != B200_DECODE_PERSISTENT)) return B200_ERR_BAD_ARG;
-    if (!p->g_decode) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
+    if (!p->graph.decode.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     if (mode == B200_DECODE_PERSISTENT && !p->pd_ok) return fail(p, B200_ERR_UNSUPPORTED, "%s", p->pd_why.c_str());
     p->decode_mode = mode;
     return B200_OK;
@@ -2038,9 +2070,9 @@ int b200_set_decode_mode(b200_plan *p, int32_t mode) {
 
 int b200_decode_info(b200_plan *p, int32_t *mode, int32_t *launches, int32_t *ring_stages, int32_t *smem_bytes) {
     if (!p) return B200_ERR_BAD_ARG;
-    const bool pers = p->decode_mode == B200_DECODE_PERSISTENT && p->g_pdecode;
-    if (mode) *mode = pers ? B200_DECODE_PERSISTENT : B200_DECODE_GRAPH;
-    if (launches) *launches = pers ? 1 : p->launches_decode;
+    const TokenGraphs &t = active_graphs(p);
+    if (mode) *mode = &t == &p->pers ? B200_DECODE_PERSISTENT : B200_DECODE_GRAPH;
+    if (launches) *launches = t.decode.launches;
     if (ring_stages) *ring_stages = p->pd_ok ? p->pd_L.stages : 0;
     if (smem_bytes) *smem_bytes = p->pd_ok ? (int32_t)p->pd_L.total : 0;
     return B200_OK;
@@ -2048,7 +2080,7 @@ int b200_decode_info(b200_plan *p, int32_t *mode, int32_t *launches, int32_t *ri
 
 int b200_trace_persistent(b200_plan *p, int32_t token, int32_t position, uint64_t *stamps, int64_t cap, int32_t *n_ctas, int32_t *n_rows, int32_t *n_stamps) {
     if (!p || !stamps) return B200_ERR_BAD_ARG;
-    if (!p->g_ptrace) return fail(p, B200_ERR_UNSUPPORTED, "%s", p->pd_ok ? "no traced persistent graph" : p->pd_why.c_str());
+    if (!p->pers.trace.exec) return fail(p, B200_ERR_UNSUPPORTED, "%s", p->pd_ok ? "no traced persistent graph" : p->pd_why.c_str());
     int rc;
     if ((rc = check_pos(p, token, position))) return rc;
     CK(cudaSetDevice(p->device));
@@ -2056,7 +2088,7 @@ int b200_trace_persistent(b200_plan *p, int32_t token, int32_t position, uint64_
     if ((size_t)cap < words) return fail(p, B200_ERR_BAD_ARG, "stamp buffer too small: need %zu uint64", words);
     CK(cudaMemsetAsync(p->pd_trace, 0, words * 8, p->stream));
     if ((rc = set_state(p, token, position, 0, 0))) return rc;
-    CK(cudaGraphLaunch(p->g_ptrace, p->stream));
+    CK(cudaGraphLaunch(p->pers.trace.exec, p->stream));
     CK(cudaStreamSynchronize(p->stream));
     if ((rc = check_device_error(p))) return rc;
     CK(cudaMemcpy(stamps, p->pd_trace, words * 8, cudaMemcpyDeviceToHost));
@@ -2149,11 +2181,12 @@ int b200_forward_decode_batch(b200_plan *p, int32_t n, const int32_t *slots, con
     }
     CK(cudaSetDevice(p->device));
     int rc;
-    if (!B.g[n] && (rc = capture_batch(p, n))) return rc;
+    const Graph *g;
+    if ((rc = batch_graph(p, BK_DECODE, n, &g))) return rc;
     for (int i = 0; i < n; i++) { B.h_rows->token[i] = tokens[i]; B.h_rows->pos[i] = positions[i]; B.h_rows->slot[i] = slots[i]; }
     CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
     CK(cudaEventRecord(p->ev0, p->stream));
-    CK(cudaGraphLaunch(B.g[n], p->stream));
+    CK(cudaGraphLaunch(g->exec, p->stream));
     CK(cudaEventRecord(p->ev1, p->stream));
     const size_t vpad = (size_t)sampler_padded(c.vocab_size);
     if (logits) // before the sampler turns sampled rows into probabilities
@@ -2161,13 +2194,7 @@ int b200_forward_decode_batch(b200_plan *p, int32_t n, const int32_t *slots, con
     bool any_sampled = false;
     for (int i = 0; i < n; i++) {
         if (!sampling || sampling[3 * i] == 0.0f) continue; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed
-        static bool attr = false;
-        if (!attr) { CK(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes())); attr = true; }
-        SamplerArgs a;
-        a.logits = B.logits + i * vpad; a.n = c.vocab_size; a.temperature = sampling[3 * i]; a.topp = sampling[3 * i + 1]; a.r01 = sampling[3 * i + 2];
-        a.indices = p->smp_indices; a.out_id = B.smp_out + 8 * i; a.info = B.smp_out + 8 * i + 1;
-        k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
-        CK(cudaGetLastError());
+        if ((rc = launch_sample(p, B.logits + i * vpad, sampling[3 * i], sampling[3 * i + 1], sampling[3 * i + 2], B.smp_out + 8 * i))) return rc;
         any_sampled = true;
     }
     CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)n * 4, cudaMemcpyDeviceToHost, p->stream));
@@ -2360,10 +2387,11 @@ int b200_forward_decode_multi(b200_plan *p, int32_t slot, int32_t n, const int32
     int rc;
     if ((rc = multi_ready(p))) return rc;
     const bool own = slot < 0;
-    if (!B.gs[own][1][n] && (rc = capture_batch(p, n, false, true, own))) return rc;
+    const Graph *g;
+    if ((rc = batch_graph(p, own ? BK_MULTI_OWN : BK_MULTI, n, &g))) return rc;
     for (int i = 0; i < n; i++) { B.h_rows->token[i] = tokens[i]; B.h_rows->pos[i] = start_pos + i; B.h_rows->slot[i] = own ? 0 : slot; }
     CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
-    CK(cudaGraphLaunch(B.gs[own][1][n], p->stream));
+    CK(cudaGraphLaunch(g->exec, p->stream));
     const size_t vpad = (size_t)sampler_padded(c.vocab_size);
     if (logits)
         for (int i = 0; i < n; i++) CK(cudaMemcpyAsync(logits + (size_t)i * c.vocab_size, B.logits + i * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
@@ -2376,7 +2404,7 @@ int b200_forward_decode_multi(b200_plan *p, int32_t slot, int32_t n, const int32
 int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step) {
     if (!p) return B200_ERR_BAD_ARG;
     if (n_slots) *n_slots = p->bt.n_slots;
-    if (launches_per_step) *launches_per_step = p->bt.last_n ? p->bt.launches[p->bt.last_n] : 0;
+    if (launches_per_step) *launches_per_step = p->bt.g[BK_DECODE][p->bt.last_n].launches;
     if (device_ms_last_step) *device_ms_last_step = p->bt.last_ms;
     return B200_OK;
 }
@@ -2433,82 +2461,45 @@ int b200_time_kernel(b200_plan *p, int32_t which, int32_t reps, float *avg_ms, i
     if (!p || !avg_ms || reps <= 0) return B200_ERR_BAD_ARG;
     if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "b200_time_kernel is single-GPU only");
     if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "b200_time_kernel times the dense FFN and attention matrices; a Qwen2-MoE plan has no dense FFN");
+    if (which < 0 || which > 4) return fail(p, B200_ERR_BAD_ARG, "unknown kernel id %d", which);
     const b200_config &c = p->cfg;
-    const bool q8 = p->wtype == B200_GGML_Q8_0;
-    CK(cudaSetDevice(p->device));
-    std::vector<float> save(c.dim);
-    CK(cudaStreamSynchronize(p->stream));
-    CK(cudaMemcpy(save.data(), p->x, (size_t)c.dim * 4, cudaMemcpyDeviceToHost));
-    if (p->use_stream) {
-        auto tb = [&](const TileMat &m) -> int64_t { return (int64_t)m.rows * m.cols / 32 * 34; };
-        int64_t bytes = 0;
-        int launches = 0, rc;
-        auto one = [&](int l) -> int {
-            LayerW &L = p->layers[l];
-            bool keep = p->use_pdl;
-            p->use_pdl = false;
-            int r;
-            const bool fz = p->fuse_norm;
-            const int64_t nw = fz ? (int64_t)c.dim * 4 : 0; // a fused norm also reads its weights (x: an L2 hit)
-            switch (which) {
-            case 0:
-                bytes = tb(L.tgu) + nw;
-                r = fz ? launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, TraceBuf{nullptr, 0, 0})
-                       : launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs);
-                break;
-            case 1: bytes = tb(L.tw2); r = launch_stream<SMV_RESID>(p, L.tw2, p->hq, p->hs, p->x, nullptr, nullptr); break;
-            case 2:
-                bytes = tb(L.tqkv) + nw;
-                r = fz ? launch_stream_norm<SMV_STORE>(p, L.tqkv, L.attn_norm, false, p->qkv, nullptr, nullptr, false, TraceBuf{nullptr, 0, 0})
-                       : launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr);
-                break;
-            case 3: bytes = tb(L.two); r = launch_stream<SMV_RESID>(p, L.two, p->xq, p->xs, p->x, nullptr, nullptr); break;
-            default:
-                bytes = tb(p->tout) + nw;
-                r = fz ? launch_stream_norm<SMV_STORE>(p, p->tout, p->out_norm, false, p->logits, nullptr, nullptr, false, TraceBuf{nullptr, 0, 0})
-                       : launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr);
-                break;
-            }
-            p->use_pdl = keep;
-            return r;
-        };
-        if (which < 0 || which > 4) return fail(p, B200_ERR_BAD_ARG, "unknown kernel id %d", which);
-        for (int l = 0; l < c.n_layers; l++) if ((rc = one(l))) return rc;
-        CK(cudaEventRecord(p->ev0, p->stream));
-        for (int r = 0; r < reps; r++)
-            for (int l = 0; l < c.n_layers; l++) { if ((rc = one(l))) return rc; launches++; }
-        CK(cudaEventRecord(p->ev1, p->stream));
-        CK(cudaStreamSynchronize(p->stream));
-        float ms = 0;
-        CK(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
-        *avg_ms = ms / launches;
-        if (algorithmic_bytes) *algorithmic_bytes = bytes;
-        CK(cudaMemcpy(p->x, save.data(), (size_t)c.dim * 4, cudaMemcpyHostToDevice));
-        return B200_OK;
-    }
+    const bool q8 = p->wtype == B200_GGML_Q8_0, sf = p->use_f16_stream, fz = p->fuse_norm;
+    auto tb = [&](const TileMat &m) -> int64_t { return (int64_t)m.rows * m.cols / 32 * 34; };
     auto mat_bytes = [&](const DevMat &m) -> int64_t {
         int64_t e = (int64_t)m.rows * m.cols;
         return q8 ? e / 32 * 34 : e * 2;
     };
+    const int64_t nw = fz ? (int64_t)c.dim * 4 : 0; // a fused norm also reads its weights (x: an L2 hit)
+    const TraceBuf none{nullptr, 0, 0};
     int64_t bytes = 0;
-    int launches = 0;
-    const bool sf = p->use_f16_stream;
-    auto one = [&](int l) -> int {
-        LayerW &L = p->layers[l];
-        if (sf) { // FP16 streaming kernels, stand-alone (no PDL overlap)
-            const bool keep = p->use_pdl;
-            p->use_pdl = false;
-            int r;
-            switch (which) {
-            case 0: bytes = mat_bytes(L.w1) + mat_bytes(L.w3); r = launch_stream_f16<SF_GATEUP>(p, L.w1, &L.w3, p->xb, p->hb); break;
-            case 1: bytes = mat_bytes(L.w2); r = launch_stream_f16<SF_RESID>(p, L.w2, nullptr, p->hb, p->x); break;
-            case 2: bytes = mat_bytes(L.qkv); r = launch_stream_f16<SF_STORE>(p, L.qkv, nullptr, p->xb, p->qkv); break;
-            case 3: bytes = mat_bytes(L.wo); r = launch_stream_f16<SF_RESID>(p, L.wo, nullptr, p->xb, p->x); break;
-            default: bytes = mat_bytes(p->out); r = launch_stream_f16<SF_STORE>(p, p->out, nullptr, p->xb, p->logits); break;
-            }
-            p->use_pdl = keep;
-            return r;
+    auto stream = [&](LayerW &L) -> int { // Q8_0 streaming kernels
+        switch (which) {
+        case 0:
+            bytes = tb(L.tgu) + nw;
+            return fz ? launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, none)
+                      : launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs);
+        case 1: bytes = tb(L.tw2); return launch_stream<SMV_RESID>(p, L.tw2, p->hq, p->hs, p->x, nullptr, nullptr);
+        case 2:
+            bytes = tb(L.tqkv) + nw;
+            return fz ? launch_stream_norm<SMV_STORE>(p, L.tqkv, L.attn_norm, false, p->qkv, nullptr, nullptr, false, none)
+                      : launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr);
+        case 3: bytes = tb(L.two); return launch_stream<SMV_RESID>(p, L.two, p->xq, p->xs, p->x, nullptr, nullptr);
+        default:
+            bytes = tb(p->tout) + nw;
+            return fz ? launch_stream_norm<SMV_STORE>(p, p->tout, p->out_norm, false, p->logits, nullptr, nullptr, false, none)
+                      : launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr);
         }
+    };
+    auto f16_stream = [&](LayerW &L) -> int { // FP16 streaming kernels
+        switch (which) {
+        case 0: bytes = mat_bytes(L.w1) + mat_bytes(L.w3); return launch_stream_f16<SF_GATEUP>(p, L.w1, &L.w3, p->xb, p->hb);
+        case 1: bytes = mat_bytes(L.w2); return launch_stream_f16<SF_RESID>(p, L.w2, nullptr, p->hb, p->x);
+        case 2: bytes = mat_bytes(L.qkv); return launch_stream_f16<SF_STORE>(p, L.qkv, nullptr, p->xb, p->qkv);
+        case 3: bytes = mat_bytes(L.wo); return launch_stream_f16<SF_RESID>(p, L.wo, nullptr, p->xb, p->x);
+        default: bytes = mat_bytes(p->out); return launch_stream_f16<SF_STORE>(p, p->out, nullptr, p->xb, p->logits);
+        }
+    };
+    auto matvec = [&](LayerW &L) -> int { // the non-streaming kernels
         switch (which) {
         case 0:
             if (q8) {
@@ -2528,8 +2519,21 @@ int b200_time_kernel(b200_plan *p, int32_t which, int32_t reps, float *avg_ms, i
         default: bytes = mat_bytes(p->out); return q8 ? launch_matvec_q8<MODE_STORE>(p, p->out, p->xq, p->xs, p->logits) : launch_matvec_f16<MODE_STORE>(p, p->out, p->xb, p->logits);
         }
     };
-    if (which < 0 || which > 4) return fail(p, B200_ERR_BAD_ARG, "unknown kernel id %d", which);
-    int rc;
+    // one launch on layer l's matrix; the streaming kernels run stand-alone (no PDL overlap)
+    auto one = [&](int l) -> int {
+        LayerW &L = p->layers[l];
+        if (!p->use_stream && !sf) return matvec(L);
+        const bool keep = p->use_pdl;
+        p->use_pdl = false;
+        const int r = p->use_stream ? stream(L) : f16_stream(L);
+        p->use_pdl = keep;
+        return r;
+    };
+    CK(cudaSetDevice(p->device));
+    std::vector<float> save(c.dim);
+    CK(cudaStreamSynchronize(p->stream));
+    CK(cudaMemcpy(save.data(), p->x, (size_t)c.dim * 4, cudaMemcpyDeviceToHost));
+    int rc, launches = 0;
     for (int l = 0; l < c.n_layers; l++) if ((rc = one(l))) return rc; // warm-up pass (also defeats L2 for pass 1)
     CK(cudaEventRecord(p->ev0, p->stream));
     for (int r = 0; r < reps; r++)
@@ -2580,16 +2584,16 @@ int b200_tp_attach(b200_plan *p, const void *handles, int32_t n) {
 
 int b200_trace_decode(b200_plan *p, int32_t token, int32_t position, uint64_t *records, int32_t cap, int32_t *n_out) {
     if (!p || !records || !n_out) return B200_ERR_BAD_ARG;
-    if (!p->g_trace) return fail(p, B200_ERR_UNSUPPORTED, "tracing needs a streaming path (Q8_0 tiles or the FP16 rings)");
+    if (!p->graph.trace.exec) return fail(p, B200_ERR_UNSUPPORTED, "tracing needs a streaming path (Q8_0 tiles or the FP16 rings)");
     int rc;
     if ((rc = check_pos(p, token, position))) return rc;
     CK(cudaSetDevice(p->device));
-    int n = p->launches_decode;
+    int n = p->graph.trace.launches;
     std::vector<unsigned long long> init((size_t)n * 4);
     for (int i = 0; i < n; i++) { init[i * 4] = 0; init[i * 4 + 1] = ~0ull; init[i * 4 + 2] = 0; init[i * 4 + 3] = 0; }
     CK(cudaMemcpyAsync(p->trace_rec, init.data(), init.size() * 8, cudaMemcpyHostToDevice, p->stream));
     if ((rc = set_state(p, token, position, 0, 0))) return rc;
-    CK(cudaGraphLaunch(p->g_trace, p->stream));
+    CK(cudaGraphLaunch(p->graph.trace.exec, p->stream));
     CK(cudaStreamSynchronize(p->stream));
     int m = n < cap ? n : cap;
     CK(cudaMemcpy(records, p->trace_rec, (size_t)m * 32, cudaMemcpyDeviceToHost));
@@ -2619,9 +2623,9 @@ int b200_profile_norm(b200_plan *p, int64_t *cycles4) {
 int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out, int32_t *info) {
     if (!terms || !out || n <= 0 || n > 8192) return B200_ERR_BAD_ARG;
     if (threads != 256 && threads != 512 && threads != 1024) return B200_ERR_BAD_ARG;
+    Scratch s;
     float *d = nullptr, *o = nullptr;
-    if (cudaMalloc(&d, (size_t)n * 4) != cudaSuccess) return B200_ERR_OOM;
-    if (cudaMalloc(&o, 16) != cudaSuccess) { cudaFree(d); return B200_ERR_OOM; }
+    if (!s.alloc(&d, (size_t)n * 4) || !s.alloc(&o, 16)) return B200_ERR_OOM;
     cudaError_t e = cudaMemcpy(d, terms, (size_t)n * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
         if (threads == 1024) {
@@ -2644,8 +2648,6 @@ int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out
     if (e == cudaSuccess) e = cudaMemcpy(host, o, 12, cudaMemcpyDeviceToHost);
     memcpy(out, host, 4);
     if (info) { info[0] = host[1]; info[1] = host[2]; }
-    cudaFree(d);
-    cudaFree(o);
     return e == cudaSuccess ? B200_OK : B200_ERR_CUDA;
 }
 
@@ -2655,38 +2657,34 @@ int b200_test_sample(const float *logits, int32_t n, float temperature, float to
     const size_t padded = (size_t)sampler_padded(n) * 4;
     float *dl = nullptr;
     int *di = nullptr, *dout = nullptr;
-    int rc = B200_OK;
-    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
+    Scratch s;
     // the index scratch starts as 0xFF bytes: a slot the kernel did not write in this call reads as -1
-    if (ok(cudaMalloc(&dl, padded)) && ok(cudaMalloc(&di, (size_t)n * 4)) && ok(cudaMalloc(&dout, 8 * 4)) && ok(cudaMemset(dl, 0, padded)) &&
-        ok(cudaMemcpy(dl, logits, (size_t)n * 4, cudaMemcpyHostToDevice)) && ok(cudaMemset(di, 0xFF, (size_t)n * 4)) && ok(cudaMemset(dout, 0xFF, 8 * 4)) &&
-        ok(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()))) {
+    if (s.alloc(&dl, padded) && s.alloc(&di, (size_t)n * 4) && s.alloc(&dout, 8 * 4) && s.ok(cudaMemset(dl, 0, padded)) &&
+        s.ok(cudaMemcpy(dl, logits, (size_t)n * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemset(di, 0xFF, (size_t)n * 4)) && s.ok(cudaMemset(dout, 0xFF, 8 * 4)) &&
+        s.ok(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()))) {
         SamplerArgs a;
         a.logits = dl; a.n = n; a.temperature = temperature; a.topp = topp; a.r01 = uniform01;
         a.indices = di; a.out_id = dout; a.info = dout + 1;
         k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(a);
         int32_t h[5];
-        if (ok(cudaGetLastError()) && ok(cudaDeviceSynchronize()) && ok(cudaMemcpy(h, dout, 5 * 4, cudaMemcpyDeviceToHost))) {
+        if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize()) && s.ok(cudaMemcpy(h, dout, 5 * 4, cudaMemcpyDeviceToHost))) {
             *token_out = h[0];
             if (info) for (int k = 0; k < 4; k++) info[k] = h[1 + k];
-            if (probs_out) ok(cudaMemcpy(probs_out, dl, (size_t)n * 4, cudaMemcpyDeviceToHost));
+            if (probs_out) s.ok(cudaMemcpy(probs_out, dl, (size_t)n * 4, cudaMemcpyDeviceToHost));
         }
     }
-    cudaFree(dl); cudaFree(di); cudaFree(dout);
-    return rc;
+    return s.rc;
 }
 
 int b200_requant_kquant(int32_t ggml_type, const void *src, int64_t n_elems, void *dst_q8_0) {
     if (!src || !dst_q8_0 || n_elems <= 0 || n_elems % 256 || !kq_is_kquant(ggml_type)) return B200_ERR_BAD_ARG;
     const size_t raw = (size_t)(n_elems / 256) * kq_block_bytes(ggml_type), q8 = (size_t)(n_elems / 32) * 34;
     unsigned char *ds = nullptr, *dd = nullptr;
-    int rc = B200_OK;
-    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
-    if (ok(cudaMalloc(&ds, raw)) && ok(cudaMalloc(&dd, q8)) && ok(cudaMemcpy(ds, src, raw, cudaMemcpyHostToDevice)) &&
-        ok(launch_requant_kquant(ggml_type, ds, dd, n_elems / 32, 0)) && ok(cudaDeviceSynchronize()))
-        ok(cudaMemcpy(dst_q8_0, dd, q8, cudaMemcpyDeviceToHost));
-    cudaFree(ds); cudaFree(dd);
-    return rc;
+    Scratch s;
+    if (s.alloc(&ds, raw) && s.alloc(&dd, q8) && s.ok(cudaMemcpy(ds, src, raw, cudaMemcpyHostToDevice)) &&
+        s.ok(launch_requant_kquant(ggml_type, ds, dd, n_elems / 32, 0)) && s.ok(cudaDeviceSynchronize()))
+        s.ok(cudaMemcpy(dst_q8_0, dd, q8, cudaMemcpyDeviceToHost));
+    return s.rc;
 }
 
 int b200_gemm_f16(const uint16_t *a, const uint16_t *b, float *c, int32_t m, int32_t n, int32_t k, int32_t iters, float *ms) {
@@ -2697,29 +2695,27 @@ int b200_gemm_f16(const uint16_t *a, const uint16_t *b, float *c, int32_t m, int
     __half *da = nullptr, *db = nullptr;
     float *dc = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
-    int rc = B200_OK;
-    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; }; // first failure wins
-    if (ok(cudaMalloc(&da, (size_t)m * k * 2)) && ok(cudaMalloc(&db, (size_t)n * k * 2)) && ok(cudaMalloc(&dc, (size_t)m * n * 4)) &&
-        ok(cudaMemcpy(da, a, (size_t)m * k * 2, cudaMemcpyHostToDevice)) && ok(cudaMemcpy(db, b, (size_t)n * k * 2, cudaMemcpyHostToDevice)) &&
-        ok(cudaMemset(dc, resid ? 0 : 0xFF, (size_t)m * n * 4))) {
-        if (pg::gemm_f16(da, db, dc, m, n, k, stages, resid, 0)) rc = B200_ERR_CUDA;
-        ok(cudaDeviceSynchronize());
-        if (rc == B200_OK && iters > 0 && ms && ok(cudaEventCreate(&e0)) && ok(cudaEventCreate(&e1)) && ok(cudaEventRecord(e0, 0))) {
-            for (int i = 0; i < iters && rc == B200_OK; i++)
-                if (pg::gemm_f16(da, db, dc, m, n, k, stages, resid, 0)) rc = B200_ERR_CUDA;
+    Scratch s;
+    if (s.alloc(&da, (size_t)m * k * 2) && s.alloc(&db, (size_t)n * k * 2) && s.alloc(&dc, (size_t)m * n * 4) &&
+        s.ok(cudaMemcpy(da, a, (size_t)m * k * 2, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(db, b, (size_t)n * k * 2, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemset(dc, resid ? 0 : 0xFF, (size_t)m * n * 4))) {
+        if (pg::gemm_f16(da, db, dc, m, n, k, stages, resid, 0)) s.rc = B200_ERR_CUDA;
+        s.ok(cudaDeviceSynchronize());
+        if (s.rc == B200_OK && iters > 0 && ms && s.ok(cudaEventCreate(&e0)) && s.ok(cudaEventCreate(&e1)) && s.ok(cudaEventRecord(e0, 0))) {
+            for (int i = 0; i < iters && s.rc == B200_OK; i++)
+                if (pg::gemm_f16(da, db, dc, m, n, k, stages, resid, 0)) s.rc = B200_ERR_CUDA;
             float t = 0.f;
-            if (ok(cudaEventRecord(e1, 0)) && ok(cudaEventSynchronize(e1)) && ok(cudaEventElapsedTime(&t, e0, e1))) *ms = t / iters;
-            if (rc == B200_OK && resid) { // C accumulated 1 + iters products: return exactly one
-                if (ok(cudaMemset(dc, 0, (size_t)m * n * 4)) && pg::gemm_f16(da, db, dc, m, n, k, stages, resid, 0)) rc = B200_ERR_CUDA;
-                ok(cudaDeviceSynchronize());
+            if (s.ok(cudaEventRecord(e1, 0)) && s.ok(cudaEventSynchronize(e1)) && s.ok(cudaEventElapsedTime(&t, e0, e1))) *ms = t / iters;
+            if (s.rc == B200_OK && resid) { // C accumulated 1 + iters products: return exactly one
+                if (s.ok(cudaMemset(dc, 0, (size_t)m * n * 4)) && pg::gemm_f16(da, db, dc, m, n, k, stages, resid, 0)) s.rc = B200_ERR_CUDA;
+                s.ok(cudaDeviceSynchronize());
             }
         }
-        if (rc == B200_OK) ok(cudaMemcpy(c, dc, (size_t)m * n * 4, cudaMemcpyDeviceToHost));
+        if (s.rc == B200_OK) s.ok(cudaMemcpy(c, dc, (size_t)m * n * 4, cudaMemcpyDeviceToHost));
     }
     if (e0) cudaEventDestroy(e0);
     if (e1) cudaEventDestroy(e1);
-    cudaFree(da); cudaFree(db); cudaFree(dc);
-    return rc;
+    return s.rc;
 }
 
 int b200_test_gemm(int32_t mode, int32_t stages, int32_t splits, int32_t m, int32_t m_valid, int32_t n, int32_t k, const uint16_t *a, const uint16_t *b,
@@ -2731,39 +2727,31 @@ int b200_test_gemm(int32_t mode, int32_t stages, int32_t splits, int32_t m, int3
     const size_t c_bytes = (size_t)m * n * (gateup ? 2 : 4);
     __half *da = nullptr, *db = nullptr, *db2 = nullptr;
     void *dc = nullptr;
-    int rc = B200_OK;
-    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
-    if (ok(cudaMalloc(&da, (size_t)m * k * 2)) && ok(cudaMalloc(&db, (size_t)n * k * 2)) && (!gateup || ok(cudaMalloc(&db2, (size_t)n * k * 2))) &&
-        ok(cudaMalloc(&dc, c_bytes)) && ok(cudaMemcpy(da, a, (size_t)m * k * 2, cudaMemcpyHostToDevice)) &&
-        ok(cudaMemcpy(db, b, (size_t)n * k * 2, cudaMemcpyHostToDevice)) && (!gateup || ok(cudaMemcpy(db2, b2, (size_t)n * k * 2, cudaMemcpyHostToDevice))) &&
-        ok(cudaMemcpy(dc, c, c_bytes, cudaMemcpyHostToDevice))) {
+    Scratch s;
+    if (s.alloc(&da, (size_t)m * k * 2) && s.alloc(&db, (size_t)n * k * 2) && (!gateup || s.alloc(&db2, (size_t)n * k * 2)) &&
+        s.alloc(&dc, c_bytes) && s.ok(cudaMemcpy(da, a, (size_t)m * k * 2, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(db, b, (size_t)n * k * 2, cudaMemcpyHostToDevice)) && (!gateup || s.ok(cudaMemcpy(db2, b2, (size_t)n * k * 2, cudaMemcpyHostToDevice))) &&
+        s.ok(cudaMemcpy(dc, c, c_bytes, cudaMemcpyHostToDevice))) {
         // the same maps prefill_forward builds: A boxes of 128 rows, B boxes of 128 rows (64 for each half of the gate/up tile), C boxes 128 x 32 f32
         CUtensorMap ma, mb, mb2, mc;
         const uint32_t b_rows = gateup ? pg::BN / 2 : pg::BN;
         if (pg::make_map(&ma, da, (uint64_t)m, (uint64_t)k, pg::BM) || pg::make_map(&mb, db, (uint64_t)n, (uint64_t)k, b_rows) ||
             pg::make_map(&mb2, gateup ? db2 : db, (uint64_t)n, (uint64_t)k, b_rows) || (!gateup && pg::make_map_c(&mc, dc, (uint64_t)m, (uint64_t)n)))
-            rc = B200_ERR_CUDA;
+            s.rc = B200_ERR_CUDA;
         if (gateup) mc = mb; // unused by the gate/up epilogue, which stores f16 through plain pointers
-        int lr = 0;
-        if (rc == B200_OK) {
+        if (s.rc == B200_OK) {
             const int mt = m / pg::BM, nt = n / (gateup ? pg::BN / 2 : pg::BN);
             const bool deep = stages == pg::GEMM_STAGES_DEEP;
-            if (mode == pg::GEMM_F32)
-                lr = deep ? pg::gemm_launch<pg::GEMM_F32, pg::GEMM_STAGES_DEEP>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits)
-                          : pg::gemm_launch<pg::GEMM_F32, pg::GEMM_STAGES>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits);
-            else if (mode == pg::GEMM_RESID)
-                lr = deep ? pg::gemm_launch<pg::GEMM_RESID, pg::GEMM_STAGES_DEEP>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits)
-                          : pg::gemm_launch<pg::GEMM_RESID, pg::GEMM_STAGES>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits);
-            else
-                lr = deep ? pg::gemm_launch<pg::GEMM_GATEUP, pg::GEMM_STAGES_DEEP>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits)
-                          : pg::gemm_launch<pg::GEMM_GATEUP, pg::GEMM_STAGES>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits);
-            if (lr == -6) rc = B200_ERR_BAD_ARG; // splits > 1 outside GEMM_RESID, or a split with no k-block
-            else if (lr) rc = B200_ERR_CUDA;
+            const int lr = with_gemm_mode(mode, [&](auto MODE) {
+                return deep ? pg::gemm_launch<MODE, pg::GEMM_STAGES_DEEP>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits)
+                            : pg::gemm_launch<MODE, pg::GEMM_STAGES>(ma, mb, mb2, mc, dc, n, m_valid, mt, nt, k, 0, splits);
+            });
+            if (lr == -6) s.rc = B200_ERR_BAD_ARG; // splits > 1 outside GEMM_RESID, or a split with no k-block
+            else if (lr) s.rc = B200_ERR_CUDA;
         }
-        if (ok(cudaDeviceSynchronize()) && rc == B200_OK) ok(cudaMemcpy(c, dc, c_bytes, cudaMemcpyDeviceToHost));
+        if (s.ok(cudaDeviceSynchronize()) && s.rc == B200_OK) s.ok(cudaMemcpy(c, dc, c_bytes, cudaMemcpyDeviceToHost));
     }
-    cudaFree(da); cudaFree(db); cudaFree(db2); cudaFree(dc);
-    return rc;
+    return s.rc;
 }
 
 int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, int32_t m_valid, int32_t n, int32_t k, const uint16_t *a, const void *bq,
@@ -2780,46 +2768,37 @@ int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, i
     __half *da = nullptr;
     unsigned char *draw = nullptr, *dstream = nullptr;
     void *dc = nullptr;
-    int rc = B200_OK;
-    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
-    if (ok(cudaMalloc(&da, (size_t)m * k * 2)) && ok(cudaMalloc(&draw, q8_bytes * (gateup ? 2 : 1))) && ok(cudaMalloc(&dstream, stream_bytes)) &&
-        ok(cudaMalloc(&dc, c_bytes)) && ok(cudaMemcpy(da, a, (size_t)m * k * 2, cudaMemcpyHostToDevice)) && ok(cudaMemcpy(draw, bq, q8_bytes, cudaMemcpyHostToDevice)) &&
-        (!gateup || ok(cudaMemcpy(draw + q8_bytes, bq2, q8_bytes, cudaMemcpyHostToDevice))) && ok(cudaMemcpy(dc, c, c_bytes, cudaMemcpyHostToDevice))) {
+    Scratch s;
+    if (s.alloc(&da, (size_t)m * k * 2) && s.alloc(&draw, q8_bytes * (gateup ? 2 : 1)) && s.alloc(&dstream, stream_bytes) &&
+        s.alloc(&dc, c_bytes) && s.ok(cudaMemcpy(da, a, (size_t)m * k * 2, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(draw, bq, q8_bytes, cudaMemcpyHostToDevice)) &&
+        (!gateup || s.ok(cudaMemcpy(draw + q8_bytes, bq2, q8_bytes, cudaMemcpyHostToDevice))) && s.ok(cudaMemcpy(dc, c, c_bytes, cudaMemcpyHostToDevice))) {
         RepackSrc src{};
         src.raw[0] = draw;
         src.rows[0] = n;
         if (gateup) { src.raw[1] = draw + q8_bytes; src.rows[1] = n; }
         src.gateup = gateup ? 1 : 0;
         k_repack_tiles<<<(unsigned)((size_t)rows * nseg), 128>>>(src, dstream, rows, k, seg, nseg, unit);
-        ok(cudaGetLastError());
+        s.ok(cudaGetLastError());
         // the maps prefill_init_q8 builds and the A / C maps of the prefill scratch
         CUtensorMap ma, mq, ms, mc;
-        if (rc == B200_OK && (pg::make_map(&ma, da, (uint64_t)m, (uint64_t)k, pg::BM) || pg::make_map_q8(&mq, dstream, (uint64_t)rows, nseg, unit, 0) ||
-                              pg::make_map_q8(&ms, dstream, (uint64_t)rows, nseg, unit, 1) || (!gateup && pg::make_map_c(&mc, dc, (uint64_t)m, (uint64_t)n))))
-            rc = B200_ERR_CUDA;
+        if (s.rc == B200_OK && (pg::make_map(&ma, da, (uint64_t)m, (uint64_t)k, pg::BM) || pg::make_map_q8(&mq, dstream, (uint64_t)rows, nseg, unit, 0) ||
+                                pg::make_map_q8(&ms, dstream, (uint64_t)rows, nseg, unit, 1) || (!gateup && pg::make_map_c(&mc, dc, (uint64_t)m, (uint64_t)n))))
+            s.rc = B200_ERR_CUDA;
         if (gateup) mc = mq; // unused by the gate/up epilogue
-        int lr = 0;
-        if (rc == B200_OK) {
+        if (s.rc == B200_OK) {
             using pg::B_Q8;
-            constexpr int S4 = pg::GEMM_STAGES, S5 = pg::GEMM_STAGES_DEEP_Q8;
             const int mt = m / pg::BM, nt = n / (gateup ? pg::BN / 2 : pg::BN);
-            const bool deep = stages == S5;
-            if (mode == pg::GEMM_F32)
-                lr = deep ? pg::gemm_launch<pg::GEMM_F32, S5, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg)
-                          : pg::gemm_launch<pg::GEMM_F32, S4, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg);
-            else if (mode == pg::GEMM_RESID)
-                lr = deep ? pg::gemm_launch<pg::GEMM_RESID, S5, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg)
-                          : pg::gemm_launch<pg::GEMM_RESID, S4, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg);
-            else
-                lr = deep ? pg::gemm_launch<pg::GEMM_GATEUP, S5, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg)
-                          : pg::gemm_launch<pg::GEMM_GATEUP, S4, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg);
-            if (lr == -6) rc = B200_ERR_BAD_ARG;
-            else if (lr) rc = B200_ERR_CUDA;
+            const bool deep = stages == pg::GEMM_STAGES_DEEP_Q8;
+            const int lr = with_gemm_mode(mode, [&](auto MODE) {
+                return deep ? pg::gemm_launch<MODE, pg::GEMM_STAGES_DEEP_Q8, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg)
+                            : pg::gemm_launch<MODE, pg::GEMM_STAGES, B_Q8>(ma, mq, ms, mc, dc, n, m_valid, mt, nt, k, 0, splits, seg);
+            });
+            if (lr == -6) s.rc = B200_ERR_BAD_ARG;
+            else if (lr) s.rc = B200_ERR_CUDA;
         }
-        if (ok(cudaDeviceSynchronize()) && rc == B200_OK) ok(cudaMemcpy(c, dc, c_bytes, cudaMemcpyDeviceToHost));
+        if (s.ok(cudaDeviceSynchronize()) && s.rc == B200_OK) s.ok(cudaMemcpy(c, dc, c_bytes, cudaMemcpyDeviceToHost));
     }
-    cudaFree(da); cudaFree(draw); cudaFree(dstream); cudaFree(dc);
-    return rc;
+    return s.rc;
 }
 
 int b200_test_pf_attention(const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads, int32_t n_kv_heads,
@@ -2831,31 +2810,27 @@ int b200_test_pf_attention(const float *q, const float *k, const float *v, int32
     const size_t kv_elems = (size_t)nkeys * kvd;
     float *dqkv = nullptr, *dk = nullptr, *dv = nullptr;
     __half *dkh = nullptr, *dvh = nullptr, *dout = nullptr;
-    int rc = B200_OK;
-    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
+    Scratch s;
     // q sits in the q columns of a QKV row as after k_pf_rope_kv; the k / v columns hold NaN, which the kernels must never read
-    if (ok(cudaMalloc(&dqkv, (size_t)n * ldq * 4)) && ok(cudaMalloc(&dk, kv_elems * 4)) && ok(cudaMalloc(&dv, kv_elems * 4)) &&
-        ok(cudaMalloc(&dkh, kv_elems * 2)) && ok(cudaMalloc(&dvh, kv_elems * 2)) && ok(cudaMalloc(&dout, (size_t)out_rows * qd * 2)) &&
-        ok(cudaMemset(dqkv, 0xFF, (size_t)n * ldq * 4)) && ok(cudaMemcpy2D(dqkv, (size_t)ldq * 4, q, (size_t)qd * 4, (size_t)qd * 4, n, cudaMemcpyHostToDevice)) &&
-        ok(cudaMemcpy(dk, k, kv_elems * 4, cudaMemcpyHostToDevice)) && ok(cudaMemcpy(dv, v, kv_elems * 4, cudaMemcpyHostToDevice)) &&
-        ok(cudaMemcpy(dout, out, (size_t)out_rows * qd * 2, cudaMemcpyHostToDevice))) {
+    if (s.alloc(&dqkv, (size_t)n * ldq * 4) && s.alloc(&dk, kv_elems * 4) && s.alloc(&dv, kv_elems * 4) &&
+        s.alloc(&dkh, kv_elems * 2) && s.alloc(&dvh, kv_elems * 2) && s.alloc(&dout, (size_t)out_rows * qd * 2) &&
+        s.ok(cudaMemset(dqkv, 0xFF, (size_t)n * ldq * 4)) && s.ok(cudaMemcpy2D(dqkv, (size_t)ldq * 4, q, (size_t)qd * 4, (size_t)qd * 4, n, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(dk, k, kv_elems * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dv, v, kv_elems * 4, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(dout, out, (size_t)out_rows * qd * 2, cudaMemcpyHostToDevice))) {
         const float inv_sqrt_hs = (float)(1.0 / sqrt((double)hs));
         const int qt = PM_ROWS / kv_mul;
         const dim3 ag((n + qt - 1) / qt, n_kv_heads);
         // f16 K / V copies as prefill_forward makes them (k_pf_kv_to_f16 and k_pf_rope_kv round the same way)
         const size_t n4 = kv_elems / 4;
         k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, 0>>>(dk, dv, dkh, dvh, n4);
-        if (hs == 128) {
-            if (ok(cudaFuncSetAttribute(k_pf_attention_mma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>())))
-                k_pf_attention_mma<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, n, start_pos, inv_sqrt_hs, dout, qd);
-        } else {
-            if (ok(cudaFuncSetAttribute(k_pf_attention_mma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<64>())))
-                k_pf_attention_mma<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, n, start_pos, inv_sqrt_hs, dout, qd);
-        }
-        if (ok(cudaGetLastError()) && ok(cudaDeviceSynchronize())) ok(cudaMemcpy(out, dout, (size_t)out_rows * qd * 2, cudaMemcpyDeviceToHost));
+        with_mma_head_size(nullptr, hs, [&](auto HS) {
+            if (s.ok(cudaFuncSetAttribute(k_pf_attention_mma<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<HS>())))
+                k_pf_attention_mma<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, n, start_pos, inv_sqrt_hs, dout, qd);
+            return B200_OK;
+        });
+        if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize())) s.ok(cudaMemcpy(out, dout, (size_t)out_rows * qd * 2, cudaMemcpyDeviceToHost));
     }
-    cudaFree(dqkv); cudaFree(dk); cudaFree(dv); cudaFree(dkh); cudaFree(dvh); cudaFree(dout);
-    return rc;
+    return s.rc;
 }
 
 int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const int32_t *start_positions, const float *q, const float *k, const float *v,
@@ -2876,32 +2851,28 @@ int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const 
     float *dqkv = nullptr, *dk = nullptr, *dv = nullptr;
     __half *dkh = nullptr, *dvh = nullptr, *dout = nullptr;
     PfTile *dt = nullptr;
-    int rc = B200_OK;
-    auto ok = [&](cudaError_t e) { if (e != cudaSuccess && rc == B200_OK) rc = e == cudaErrorMemoryAllocation ? B200_ERR_OOM : B200_ERR_CUDA; return rc == B200_OK; };
+    Scratch s;
     // q rows of every sequence back to back in the q columns of QKV rows, K / V rows [0, start + n) of each sequence back to back: the
     // layout b200_prefill_slots gives the packed kernel
-    if (ok(cudaMalloc(&dqkv, (size_t)n * ldq * 4)) && ok(cudaMalloc(&dk, kv_elems * 4)) && ok(cudaMalloc(&dv, kv_elems * 4)) &&
-        ok(cudaMalloc(&dkh, kv_elems * 2)) && ok(cudaMalloc(&dvh, kv_elems * 2)) && ok(cudaMalloc(&dout, (size_t)n * qd * 2)) &&
-        ok(cudaMalloc(&dt, tiles.size() * sizeof(PfTile))) &&
-        ok(cudaMemset(dqkv, 0xFF, (size_t)n * ldq * 4)) && ok(cudaMemcpy2D(dqkv, (size_t)ldq * 4, q, (size_t)qd * 4, (size_t)qd * 4, n, cudaMemcpyHostToDevice)) &&
-        ok(cudaMemcpy(dk, k, kv_elems * 4, cudaMemcpyHostToDevice)) && ok(cudaMemcpy(dv, v, kv_elems * 4, cudaMemcpyHostToDevice)) &&
-        ok(cudaMemcpy(dout, out, (size_t)n * qd * 2, cudaMemcpyHostToDevice)) &&
-        ok(cudaMemcpy(dt, tiles.data(), tiles.size() * sizeof(PfTile), cudaMemcpyHostToDevice))) {
+    if (s.alloc(&dqkv, (size_t)n * ldq * 4) && s.alloc(&dk, kv_elems * 4) && s.alloc(&dv, kv_elems * 4) &&
+        s.alloc(&dkh, kv_elems * 2) && s.alloc(&dvh, kv_elems * 2) && s.alloc(&dout, (size_t)n * qd * 2) &&
+        s.alloc(&dt, tiles.size() * sizeof(PfTile)) &&
+        s.ok(cudaMemset(dqkv, 0xFF, (size_t)n * ldq * 4)) && s.ok(cudaMemcpy2D(dqkv, (size_t)ldq * 4, q, (size_t)qd * 4, (size_t)qd * 4, n, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(dk, k, kv_elems * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dv, v, kv_elems * 4, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(dout, out, (size_t)n * qd * 2, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(dt, tiles.data(), tiles.size() * sizeof(PfTile), cudaMemcpyHostToDevice))) {
         const float inv_sqrt_hs = (float)(1.0 / sqrt((double)hs));
         const dim3 ag((unsigned)tiles.size(), n_kv_heads);
         const size_t n4 = kv_elems / 4;
         k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, 0>>>(dk, dv, dkh, dvh, n4);
-        if (hs == 128) {
-            if (ok(cudaFuncSetAttribute(k_pf_attention_mma_packed<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<128>())))
-                k_pf_attention_mma_packed<128><<<ag, PM_THREADS, pm_smem_bytes<128>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, dt, inv_sqrt_hs, dout, qd);
-        } else {
-            if (ok(cudaFuncSetAttribute(k_pf_attention_mma_packed<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<64>())))
-                k_pf_attention_mma_packed<64><<<ag, PM_THREADS, pm_smem_bytes<64>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, dt, inv_sqrt_hs, dout, qd);
-        }
-        if (ok(cudaGetLastError()) && ok(cudaDeviceSynchronize())) ok(cudaMemcpy(out, dout, (size_t)n * qd * 2, cudaMemcpyDeviceToHost));
+        with_mma_head_size(nullptr, hs, [&](auto HS) {
+            if (s.ok(cudaFuncSetAttribute(k_pf_attention_mma_packed<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<HS>())))
+                k_pf_attention_mma_packed<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, dt, inv_sqrt_hs, dout, qd);
+            return B200_OK;
+        });
+        if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize())) s.ok(cudaMemcpy(out, dout, (size_t)n * qd * 2, cudaMemcpyDeviceToHost));
     }
-    cudaFree(dqkv); cudaFree(dk); cudaFree(dv); cudaFree(dkh); cudaFree(dvh); cudaFree(dout); cudaFree(dt);
-    return rc;
+    return s.rc;
 }
 
 int b200_upload_info(b200_plan *p, double *seconds, double *host_copy_seconds, int64_t *h2d_bytes) {
@@ -2914,7 +2885,7 @@ int b200_upload_info(b200_plan *p, double *seconds, double *host_copy_seconds, i
 
 int b200_launches_per_decode(b200_plan *p) {
     if (!p) return 0;
-    return (p->decode_mode == B200_DECODE_PERSISTENT && p->g_pdecode) ? 1 : p->launches_decode;
+    return active_graphs(p).decode.launches;
 }
 int64_t b200_device_bytes(b200_plan *p) { return p ? p->bytes : 0; }
 
@@ -2924,12 +2895,8 @@ void b200_plan_free(b200_plan *p) {
     if (p->stream) cudaStreamSynchronize(p->stream);
     prefill_free(p->prefill);
     batch_free(p);
-    if (p->g_decode) cudaGraphExecDestroy(p->g_decode);
-    if (p->g_prefill) cudaGraphExecDestroy(p->g_prefill);
-    if (p->g_trace) cudaGraphExecDestroy(p->g_trace);
-    if (p->g_pdecode) cudaGraphExecDestroy(p->g_pdecode);
-    if (p->g_pprefill) cudaGraphExecDestroy(p->g_pprefill);
-    if (p->g_ptrace) cudaGraphExecDestroy(p->g_ptrace);
+    destroy(p->graph);
+    destroy(p->pers);
     if (p->h_err) cudaFreeHost(p->h_err);
     for (int k = 0; k < TP_MAX; k++) if (p->peer_open[k]) cudaIpcCloseMemHandle(p->peer_open[k]);
     for (void *d : p->allocs) cudaFree(d);

@@ -56,6 +56,7 @@ def _run_schedule(pkg, orc, m, n_slots, schedule, starts, n_check_kv=True):
                 rec[s].append((toks[i], nxt[s], lg[i], int(ids[i])))
                 nxt[s] += 1
         assert plan.batch_info()[0] == n_slots
+        assert plan.batch_info()[1] == 7 * c.n_layers + 3  # 7 launches per layer, then the final norm, lm_head and argmax
         assert_bit_equal(plan.read_buffer("key_cache", nkv, layer=0), own_k, "the plan's own cache after batched steps")
         for s in range(n_slots):
             om.reset()

@@ -107,9 +107,17 @@ def test_exact_prefill_slots_packs_rows(pkg, orc, make_model, shape):
     for slots, starts, lens in [([3], [0], [13]), ([2, 5], [0, 0], [9, 30]), ([2, 5, 0], [9, 30, 0], [4, 17, 1])]:
         mode, launches, _ = _exact_run(pkg, orc, m, 8, [(slots, starts, lens)] if starts[0] == 0 else
                                        [([2, 5], [0, 0], [9, 30]), (slots, starts, lens)], decode=True)
-        T, R = sum(lens), 8
-        steps = -(-T // R)
-        assert steps * (1 + 7 * L) <= launches <= steps * (1 + 8 * L), (T, launches)
+        # the last call's steps, packed as the plan packs them: 8 rows per step, sequences in call order, each step filled first
+        steps = []
+        for s, n in zip(slots, lens):
+            for _ in range(n):
+                if not steps or len(steps[-1]) == 8:
+                    steps.append([])
+                steps[-1].append(s)
+        # k_batch_rows_next, then 7 launches per layer; a step in which a slot repeats splits its attention (one more per layer)
+        want = sum(1 + 7 * L + (L if len(set(st)) < len(st) else 0) for st in steps)
+        assert len(steps) == -(-sum(lens) // 8)
+        assert launches == want, (lens, launches, want)
 
 
 def _decode_ref(pkg, orc, m, stream, upto):

@@ -22,6 +22,9 @@ NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     # Java never contracts a*b+c; the kernels reproduce the CPU path's float order exactly.
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",
+    # The same for host code: the RoPE tables are built on the host with Java's roundings (on hosts with FMA instructions the
+    # host compiler would otherwise be free to contract a*b+c).
+    "-Xcompiler", "-ffp-contract=off",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-pthread", "-shared", "-Xptxas", "-v",
 ]
 

@@ -148,6 +148,9 @@ struct b200_plan {
 
     // Granite's µP scales (b200_plan_create_granite); 1.0f for every other family, where each multiply leaves its operand unchanged
     b200_granite_config mup{1.0f, 1.0f, 1.0f, 1.0f};
+    // Devstral's YaRN RoPE table (b200_plan_create_devstral with a non-NULL b200_yarn_config); every other plan uses the plain table
+    bool has_yarn = false;
+    b200_yarn_config yarn{};
 
     PrefillCtx prefill;
     // persistent decode kernel
@@ -810,6 +813,7 @@ int pd_prepare(b200_plan *p) {
     const b200_config &c = p->cfg;
     p->pd_ok = false;
     if (p->is_moe) { p->pd_why = "the persistent decode kernel has no Qwen2-MoE layer (MoE plans decode through the CUDA graph)"; return B200_OK; }
+    if (c.dim > 8192) { p->pd_why = "the persistent decode kernel's register-resident RMSNorm supports dim <= 8192"; return B200_OK; }
     if (!p->use_stream) { p->pd_why = "the persistent decode kernel needs the Q8_0 streaming layout"; return B200_OK; }
     if (c.head_size != 64 && c.head_size != 128) { p->pd_why = "the persistent decode kernel supports head sizes 64 and 128"; return B200_OK; }
     if (p->nh_l > p->n_sms) { p->pd_why = "more attention heads than SMs"; return B200_OK; }
@@ -1146,7 +1150,7 @@ int set_smem_attrs(b200_plan *p) {
     const b200_config &c = p->cfg;
     int maxdyn = 0;
     CK(cudaDeviceGetAttribute(&maxdyn, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device));
-    if (c.dim > 8192) return fail(p, B200_ERR_UNSUPPORTED, "dim > 8192 not supported by the RMSNorm kernel");
+    if (c.dim > 16384) return fail(p, B200_ERR_UNSUPPORTED, "dim > 16384 not supported by the RMSNorm kernel");
     size_t need_norm = norm_smem_bytes(c.dim);
     size_t need_att = att_smem_bytes(c.head_size, c.context_length, p->att_scratch != nullptr);
     int maxcols = c.hidden_dim > c.dim ? c.hidden_dim : c.dim;
@@ -1203,6 +1207,64 @@ int set_smem_attrs(b200_plan *p) {
 
 int prefill_init(b200_plan *p);
 
+// RoPE.precomputeFreqsCisYaRN (RoPE.java:39-83) with Java's float / double boundaries taken literally: every float expression is
+// rounded to float after each operation (the library is built with -ffp-contract=off, so nothing here becomes an FMA), each
+// Math.log / Math.pow / Math.cos / Math.sin is a double libm call on a widened float, and (float) casts narrow where Java's do.
+// yarnCorrDim(nDims, nCtxOrig, nRot, base) = nDims * (float)log(nCtxOrig / (nRot * 2f * (float)PI)) / (2f * (float)log(base))
+float yarn_corr_dim(int n_dims, int n_ctx_orig, float n_rot, float base) {
+    const float pi_f = (float)3.14159265358979323846;
+    const float denom = n_rot * 2.0f * pi_f;                       // nRot * 2.0f * (float) Math.PI, left to right
+    const float ratio = (float)n_ctx_orig / denom;                  // int / float: the int widens to float
+    const float num = (float)n_dims * (float)log((double)ratio);
+    return num / (2.0f * (float)log((double)base));
+}
+
+// Java's Math.max / Math.min (float): a NaN operand wins, and -0.0f orders below 0.0f (fmaxf / fminf return the other operand)
+float java_maxf(float a, float b) {
+    if (a != a) return a;
+    if (a == 0.0f && b == 0.0f && std::signbit(a)) return b;
+    return a >= b ? a : b;
+}
+float java_minf(float a, float b) {
+    if (a != a) return a;
+    if (a == 0.0f && b == 0.0f && std::signbit(b)) return b;
+    return a <= b ? a : b;
+}
+
+// yarnRamp(low, high, i0) = 1 - min(1, max(0, (i0 - low) / max(0.001f, high - low)))
+float yarn_ramp(float low, float high, int i0) {
+    const float y = ((float)i0 - low) / java_maxf(0.001f, high - low);
+    return 1.0f - java_minf(1.0f, java_maxf(0.0f, y));
+}
+
+void rope_table_yarn(const b200_config &c, const b200_yarn_config &y, std::vector<float> &cr, std::vector<float> &ci) {
+    const int hs = c.head_size, half = hs / 2;
+    cr.resize((size_t)c.context_length * half);
+    ci.resize((size_t)c.context_length * half);
+    const double theta = (double)c.rope_theta;                      // DevstralConfiguration.ropeTheta() is a float, widened
+    const float freq_scale = 1.0f / y.factor;
+    const float corr0 = yarn_corr_dim(hs, y.original_context_length, y.beta_fast, (float)theta);
+    const float corr1 = yarn_corr_dim(hs, y.original_context_length, y.beta_slow, (float)theta);
+    // mscale = 1 + 0.1f * logMultiplier * (float)Math.log(1.0f / freqScale): 1/(1/factor) in float, not factor
+    const float mscale = y.log_multiplier > 0.0f ? 1.0f + 0.1f * y.log_multiplier * (float)log((double)(1.0f / freq_scale)) : 1.0f;
+    std::vector<float> freq(half);
+    for (int i = 0; i < hs; i += 2) {
+        const float extrap = (float)(1.0 / pow(theta, i / (double)hs));
+        const float interp = freq_scale * extrap;
+        const float ramp = yarn_ramp(corr0, corr1, i / 2);
+        const float a = interp * (1.0f - ramp), b = extrap * ramp;  // two rounded products, then a rounded sum
+        freq[i / 2] = a + b;
+    }
+    size_t k = 0;
+    for (int pos = 0; pos < c.context_length; pos++)
+        for (int j = 0; j < half; j++) {
+            const float val = (float)pos * freq[j];
+            cr[k] = (float)cos((double)val) * mscale;               // narrowed first, then one float multiply
+            ci[k] = (float)sin((double)val) * mscale;
+            k++;
+        }
+}
+
 // Qwen2-MoE FFN tensors of one layer (llama.cpp's names and shapes, dims[0] innermost): the F32 router and shared-expert gate, the
 // stacked routed experts [E][rows][cols] and the shared expert.  Every routed expert becomes a TileMat of its own, cut from its
 // row range of the stacked tensor (K-quant experts are re-quantised on the way like any matrix).
@@ -1257,7 +1319,7 @@ int upload_moe_layer(b200_plan *p, const b200_tensor *tensors, int n_tensors, in
 int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     const b200_config &c = p->cfg;
     if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3 && c.arch != B200_ARCH_QWEN2 && c.arch != B200_ARCH_QWEN2_MOE &&
-        c.arch != B200_ARCH_GRANITE)
+        c.arch != B200_ARCH_GRANITE && c.arch != B200_ARCH_DEVSTRAL)
         return fail(p, B200_ERR_UNSUPPORTED, "unknown arch %d", c.arch);
     p->kflags = c.arch == B200_ARCH_QWEN3 ? (KF_NEOX | KF_QKNORM) : c.arch == B200_ARCH_PHI3 ? KF_NEOX
               : (c.arch == B200_ARCH_QWEN2 || c.arch == B200_ARCH_QWEN2_MOE) ? (KF_NEOX | KF_QKVBIAS) : c.arch == B200_ARCH_GRANITE ? KF_ATTSCALE : 0;
@@ -1282,7 +1344,8 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         return fail(p, B200_ERR_BAD_ARG, "fp16_lanes must be 0, 4, 8, 16 or 32");
     p->qd = c.n_heads * c.head_size;
     p->kvd = c.n_kv_heads * c.head_size;
-    if (c.arch != B200_ARCH_QWEN3 && p->qd != c.dim) return fail(p, B200_ERR_BAD_ARG, "llama / phi3 / qwen2: n_heads*head_size must equal dim");
+    if (c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_DEVSTRAL && p->qd != c.dim)
+        return fail(p, B200_ERR_BAD_ARG, "llama / phi3 / qwen2: n_heads*head_size must equal dim");
     {
         const int tn = c.tp_size;
         if (tn < 1 || tn > TP_MAX || c.tp_rank < 0 || c.tp_rank >= tn) return fail(p, B200_ERR_BAD_ARG, "bad tp_rank/tp_size %d/%d", c.tp_rank, tn);
@@ -1454,19 +1517,25 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     }
     // RoPE table exactly as RoPE.precomputeFreqsCis (RoPE.java:6-37, ropeScaling=false):
     // freq = (float)(1.0 / Math.pow(theta, i / (double) headSize)); val = pos * freq (float);
-    // cos/sin evaluated in double and narrowed.
+    // cos/sin evaluated in double and narrowed.  Devstral plans with YaRN parameters use rope_table_yarn instead.
     {
-        int half = c.head_size / 2;
-        std::vector<float> cr((size_t)c.context_length * half), ci((size_t)c.context_length * half);
-        size_t k = 0;
-        for (int pos = 0; pos < c.context_length; pos++)
-            for (int i = 0; i < c.head_size; i += 2) {
-                float freq = (float)(1.0 / pow((double)c.rope_theta, i / (double)c.head_size));
-                float val = (float)pos * freq;
-                cr[k] = (float)cos((double)val);
-                ci[k] = (float)sin((double)val);
-                k++;
-            }
+        std::vector<float> cr, ci;
+        if (p->has_yarn) {
+            rope_table_yarn(c, p->yarn, cr, ci);
+        } else {
+            int half = c.head_size / 2;
+            cr.resize((size_t)c.context_length * half);
+            ci.resize((size_t)c.context_length * half);
+            size_t k = 0;
+            for (int pos = 0; pos < c.context_length; pos++)
+                for (int i = 0; i < c.head_size; i += 2) {
+                    float freq = (float)(1.0 / pow((double)c.rope_theta, i / (double)c.head_size));
+                    float val = (float)pos * freq;
+                    cr[k] = (float)cos((double)val);
+                    ci[k] = (float)sin((double)val);
+                    k++;
+                }
+        }
         if ((rc = dalloc(p, &p->rope_cr, cr.size() * 4))) return rc;
         if ((rc = dalloc(p, &p->rope_ci, ci.size() * 4))) return rc;
         CK(cudaMemcpy(p->rope_cr, cr.data(), cr.size() * 4, cudaMemcpyHostToDevice));
@@ -1867,9 +1936,11 @@ template <typename F> int with_gemm_mode(int mode, F &&f) {
 
 } // namespace
 
-// b200_plan_create, b200_plan_create_moe and b200_plan_create_granite (moe / granite == nullptr: neither)
-static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const b200_granite_config *granite, const b200_tensor *tensors, int32_t n_tensors,
-                       int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len) {
+// b200_plan_create, b200_plan_create_moe, b200_plan_create_granite and b200_plan_create_devstral (moe / granite == nullptr: neither;
+// devstral: called by b200_plan_create_devstral, whose yarn may be nullptr)
+static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const b200_granite_config *granite, bool devstral,
+                       const b200_yarn_config *yarn, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size, int32_t device,
+                       b200_plan **out, char *err, size_t err_len) {
     if (out) *out = nullptr;
     if (!cfg || !tensors || !out || n_tensors <= 0) {
         if (err && err_len) snprintf(err, err_len, "null argument");
@@ -1896,10 +1967,32 @@ static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const
                 return B200_ERR_BAD_ARG;
             }
     }
+    if ((cfg->arch == B200_ARCH_DEVSTRAL) != devstral) {
+        if (err && err_len)
+            snprintf(err, err_len, devstral ? "b200_plan_create_devstral needs arch B200_ARCH_DEVSTRAL (got %d)"
+                                            : "arch %d (B200_ARCH_DEVSTRAL) needs its RoPE parameters: create the plan with b200_plan_create_devstral", cfg->arch);
+        return B200_ERR_BAD_ARG;
+    }
+    if (yarn) {
+        const float v[4] = {yarn->factor, yarn->beta_fast, yarn->beta_slow, yarn->log_multiplier};
+        const char *names[4] = {"factor", "beta_fast", "beta_slow", "log_multiplier"};
+        for (int i = 0; i < 4; i++)
+            if (!isfinite(v[i])) {
+                if (err && err_len) snprintf(err, err_len, "YaRN %s is not finite (%g)", names[i], (double)v[i]);
+                return B200_ERR_BAD_ARG;
+            }
+        if (!(yarn->factor > 0.0f) || yarn->original_context_length <= 0) {
+            if (err && err_len)
+                snprintf(err, err_len, "YaRN %s must be > 0 (factor %g, original_context_length %d)", yarn->factor > 0.0f ? "original_context_length" : "factor",
+                         (double)yarn->factor, yarn->original_context_length);
+            return B200_ERR_BAD_ARG;
+        }
+    }
     b200_plan *p = new b200_plan();
     p->cfg = *cfg;
     if (moe) { p->is_moe = true; p->moe = *moe; }
     if (granite) p->mup = *granite;
+    if (yarn) { p->has_yarn = true; p->yarn = *yarn; }
     if (p->cfg.tp_size <= 0) p->cfg.tp_size = 1;
     p->device = device;
     p->prefill_batch = prefill_batch_size;
@@ -1917,7 +2010,7 @@ extern "C" {
 
 int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
                      int32_t device, b200_plan **out, char *err, size_t err_len) {
-    return plan_create(cfg, nullptr, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
+    return plan_create(cfg, nullptr, nullptr, false, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
 }
 
 int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
@@ -1927,7 +2020,7 @@ int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, con
         if (err && err_len) snprintf(err, err_len, "null argument");
         return B200_ERR_BAD_ARG;
     }
-    return plan_create(cfg, moe, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
+    return plan_create(cfg, moe, nullptr, false, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
 }
 
 int b200_plan_create_granite(const b200_config *cfg, const b200_granite_config *granite, const b200_tensor *tensors, int32_t n_tensors,
@@ -1937,7 +2030,12 @@ int b200_plan_create_granite(const b200_config *cfg, const b200_granite_config *
         if (err && err_len) snprintf(err, err_len, "null argument");
         return B200_ERR_BAD_ARG;
     }
-    return plan_create(cfg, nullptr, granite, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
+    return plan_create(cfg, nullptr, granite, false, nullptr, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
+}
+
+int b200_plan_create_devstral(const b200_config *cfg, const b200_yarn_config *yarn, const b200_tensor *tensors, int32_t n_tensors,
+                              int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len) {
+    return plan_create(cfg, nullptr, nullptr, true, yarn, tensors, n_tensors, prefill_batch_size, device, out, err, err_len);
 }
 
 int b200_forward_decode(b200_plan *p, int32_t token, int32_t position, float *logits, int32_t *argmax) {
@@ -2425,6 +2523,8 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
     else if (s == "xs") { src = p->xs; sz = (size_t)((c.dim > p->qd ? c.dim : p->qd) / 32) * 4; }
     else if (s == "hq") { src = p->hq; sz = (size_t)(c.hidden_dim > p->moe_hv ? c.hidden_dim : p->moe_hv); }
     else if (s == "hs") { src = p->hs; sz = (size_t)((c.hidden_dim > p->moe_hv ? c.hidden_dim : p->moe_hv) / 32) * 4; }
+    else if (s == "rope_cr") { src = p->rope_cr; sz = (size_t)c.context_length * (c.head_size / 2) * 4; }
+    else if (s == "rope_ci") { src = p->rope_ci; sz = (size_t)c.context_length * (c.head_size / 2) * 4; }
     else if (s == "moe_ids" || s == "moe_weights") {
         if (!p->is_moe) return fail(p, B200_ERR_BAD_ARG, "%s: not a Qwen2-MoE plan", name);
         const size_t k = (size_t)p->moe.n_experts_used;
@@ -2621,7 +2721,7 @@ int b200_profile_norm(b200_plan *p, int64_t *cycles4) {
 }
 
 int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out, int32_t *info) {
-    if (!terms || !out || n <= 0 || n > 8192) return B200_ERR_BAD_ARG;
+    if (!terms || !out || n <= 0 || n > 16384) return B200_ERR_BAD_ARG;
     if (threads != 256 && threads != 512 && threads != 1024) return B200_ERR_BAD_ARG;
     Scratch s;
     float *d = nullptr, *o = nullptr;

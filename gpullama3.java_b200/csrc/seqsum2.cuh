@@ -197,7 +197,7 @@ __device__ float block_seqsum_exact_v2_t(const float *sq, int n, SeqSum2Scratch 
         const int e = f32_exponent(p_start);
         if (p_start > 0.0f && e > -100 && e < 128 && f32_exponent(p_end) == e) { // e == 128: inf/nan prefix -> literal adds
             const float b = __uint_as_float((unsigned)(e + 127) << 23);
-            // margin 2^-9: the sequential sum deviates from any exact prefix by < n * 2^-24 relative (n <= 8192 -> 2^-11)
+            // margin 2^-9: the sequential sum deviates from any exact prefix by < n * 2^-24 relative (n <= 16384 -> 2^-10)
             if (p_start >= b * (1.0f + 0x1p-9f) && p_end <= 2.0f * b * (1.0f - 0x1p-9f)) {
                 bool ok = true;
                 int k = 0;

@@ -51,6 +51,11 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final StructLayout GRANITE_CONFIG = MemoryLayout.structLayout(
             JAVA_FLOAT.withName("embedding_scale"), JAVA_FLOAT.withName("residual_scale"), JAVA_FLOAT.withName("attention_scale"), JAVA_FLOAT.withName("logit_scale"));
 
+    // struct b200_yarn_config: 4 x float, int32 (Devstral plans with a YaRN RoPE table)
+    private static final StructLayout YARN_CONFIG = MemoryLayout.structLayout(
+            JAVA_FLOAT.withName("factor"), JAVA_FLOAT.withName("beta_fast"), JAVA_FLOAT.withName("beta_slow"), JAVA_FLOAT.withName("log_multiplier"),
+            JAVA_INT.withName("original_context_length"));
+
     private static MethodHandle fn(String name, FunctionDescriptor fd) {
         return LINKER.downcallHandle(LIB.find(name).orElseThrow(), fd);
     }
@@ -60,6 +65,8 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle CREATE_MOE = fn("b200_plan_create_moe",
             FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS, JAVA_LONG));
     private static final MethodHandle CREATE_GRANITE = fn("b200_plan_create_granite",
+            FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS, JAVA_LONG));
+    private static final MethodHandle CREATE_DEVSTRAL = fn("b200_plan_create_devstral",
             FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS, JAVA_LONG));
     private static final MethodHandle DECODE = fn("b200_forward_decode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle PREFILL = fn("b200_forward_prefill", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
@@ -97,23 +104,31 @@ public final class B200MasterPlan implements AutoCloseable {
 
     /** One plan per GPU for tensor-parallel decode: every rank passes the same tensors, the library uploads its row slices. */
     public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int archId, int headSize, int tpRank, int tpSize) throws Throwable {
-        this(state, model, tensors, archId, headSize, tpRank, tpSize, null, null);
+        this(state, model, tensors, archId, headSize, tpRank, tpSize, null, null, false, null, 0);
     }
 
     /** Qwen2-MoE (archId = ARCH_QWEN2_MOE, single GPU): moe = {numberOfExperts, numberOfExpertsUsed, moeHiddenDim, sharedExpertHiddenDim}
      *  (Qwen2MoEConfiguration); the router, shared-expert gate, stacked experts and shared expert go in `tensors` as in the file. */
     public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int headSize, int[] moe) throws Throwable {
-        this(state, model, tensors, ARCH_QWEN2_MOE, headSize, 0, 1, moe, null);
+        this(state, model, tensors, ARCH_QWEN2_MOE, headSize, 0, 1, moe, null, false, null, 0);
     }
 
     /** Granite (archId = ARCH_GRANITE): granite = {embeddingScale, residualScale, attentionScale, logitScale} (GraniteConfiguration);
      *  Llama's tensors, tied classifier. */
     public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int headSize, int tpRank, int tpSize, float[] granite) throws Throwable {
-        this(state, model, tensors, ARCH_GRANITE, headSize, tpRank, tpSize, null, granite);
+        this(state, model, tensors, ARCH_GRANITE, headSize, tpRank, tpSize, null, granite, false, null, 0);
+    }
+
+    /** Devstral 2 (archId = ARCH_DEVSTRAL): headSize = mistral3.attention.key_length (DevstralConfiguration.headDim()); Llama's tensors;
+     *  yarn = {factor, betaFast, betaSlow, logMultiplier} and originalContextLength when mistral3.rope.scaling.type is "yarn"
+     *  (DevstralModelLoader.precomputeRopeFrequencies), yarn = null for the plain RoPE table. */
+    public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int headSize, int tpRank, int tpSize, float[] yarn,
+                          int originalContextLength) throws Throwable {
+        this(state, model, tensors, ARCH_DEVSTRAL, headSize, tpRank, tpSize, null, null, true, yarn, originalContextLength);
     }
 
     private B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int archId, int headSize, int tpRank, int tpSize, int[] moe,
-                           float[] granite) throws Throwable {
+                           float[] granite, boolean devstral, float[] yarn, int yarnContextLength) throws Throwable {
         Configuration c = model.configuration();
         MemorySegment cfg = arena.allocate(CONFIG);
         int[] ints = {archId, c.dim(), c.hiddenDim(), c.numberOfLayers(), c.numberOfHeads(), c.numberOfKeyValueHeads(), headSize,
@@ -141,7 +156,15 @@ public final class B200MasterPlan implements AutoCloseable {
         MemorySegment err = arena.allocate(512);
         int batch = TornadoVMMasterPlan.WITH_PREFILL_DECODE ? TornadoVMMasterPlan.PREFILL_BATCH_SIZE : 0;
         int rc;
-        if (moe != null) {
+        if (devstral) {
+            MemorySegment yc = MemorySegment.NULL;
+            if (yarn != null) {
+                yc = arena.allocate(YARN_CONFIG);
+                for (int k = 0; k < 4; k++) yc.setAtIndex(JAVA_FLOAT, k, yarn[k]);
+                yc.set(JAVA_INT, 16, yarnContextLength);
+            }
+            rc = (int) CREATE_DEVSTRAL.invokeExact(cfg, yc, arr, tensors.size(), batch, Integer.getInteger("b200.device", tpRank), out, err, 512L);
+        } else if (moe != null) {
             MemorySegment mc = arena.allocate(MOE_CONFIG);
             for (int k = 0; k < 4; k++) mc.setAtIndex(JAVA_INT, k, moe[k]);
             rc = (int) CREATE_MOE.invokeExact(cfg, mc, arr, tensors.size(), batch, Integer.getInteger("b200.device", tpRank), out, err, 512L);
@@ -213,7 +236,7 @@ public final class B200MasterPlan implements AutoCloseable {
 
     public static final int PREFILL_EXACT = 0, PREFILL_TENSOR_CORE = 1, PREFILL_TENSOR_CORE_W8A16 = 2;
     // b200_config.arch (include/b200llama.h): Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen pass blk.N.attn_{q,k,v}.bias (F32) with the weights
-    public static final int ARCH_LLAMA = 0, ARCH_QWEN3 = 1, ARCH_PHI3 = 2, ARCH_QWEN2 = 3, ARCH_QWEN2_MOE = 4, ARCH_GRANITE = 5;
+    public static final int ARCH_LLAMA = 0, ARCH_QWEN3 = 1, ARCH_PHI3 = 2, ARCH_QWEN2 = 3, ARCH_QWEN2_MOE = 4, ARCH_GRANITE = 5, ARCH_DEVSTRAL = 6;
 
     /** TensorCoreSupport.java's switch: 0 = exact token-by-token prefill (bit-identical KV cache), 1 = TMA + wgmma GEMMs (a Q8_0
      *  plan first builds f16 twins of its matrices, +2 bytes per weight), 2 = the same GEMMs on a Q8_0 plan reading the Q8_0 weights

@@ -1,6 +1,7 @@
 """Host-side mirror of the reference model loaders (metadata -> Configuration, tensor names ->
 weight slots).  Mirrors ``model/loader/ModelLoader.java:47-108`` (type detection on
-``general.name``), ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74`` / ``Qwen2ModelLoader.java:48-73`` / ``GraniteLoader.java:48-92``
+``general.name``), ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74`` / ``Qwen2ModelLoader.java:48-73`` / ``GraniteLoader.java:48-92`` /
+``DevstralModelLoader.java:45-110``
 (configuration keys), ``AbstractModelLoader.java:40-50`` (file_type -> quantisation) and
 ``AbstractModelLoader.java:186-195`` (tied output falls back to ``token_embd.weight``).
 Weights stay in GGUF block layout; the native library repacks at upload.
@@ -19,6 +20,18 @@ ARCH_PHI3 = 2
 ARCH_QWEN2 = 3  # Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen: Llama's forward + q/k/v biases, NeoX RoPE (InferenceCore.java:434-563)
 ARCH_QWEN2_MOE = 4  # Qwen1.5-MoE: Qwen2's attention + a routed mixture-of-experts FFN with a shared expert (InferenceCore.java:263-432)
 ARCH_GRANITE = 5  # Granite 3.x: Llama's forward with four muP scales (InferenceCore.forwardGranite, InferenceCore.java:814-921)
+ARCH_DEVSTRAL = 6  # Devstral 2 (mistral3): Llama's forward with an independent head size and a YaRN RoPE table (InferenceCore.java:178-261)
+
+
+@dataclass(frozen=True)
+class Yarn:
+    """mistral3.rope.scaling.* of a YaRN-scaled Devstral file (DevstralModelLoader.precomputeRopeFrequencies), floats as Java reads them."""
+    factor: float
+    beta_fast: float
+    beta_slow: float
+    log_multiplier: float
+    original_context_length: int
+
 
 # GraniteLoader.createConfiguration's defaults for the four scales (GraniteLoader.java:55-58)
 GRANITE_DEFAULT_SCALES = {"embedding_scale": 12.0, "residual_scale": 0.22, "attention_scale": 0.0078125, "logit_scale": 16.0}
@@ -48,6 +61,8 @@ class Configuration:
     residual_scale: float = 1.0
     attention_scale: float = 1.0
     logit_scale: float = 1.0
+    # Devstral only: the YaRN parameters of the RoPE table (None: the plain table)
+    yarn: Yarn | None = None
 
     @property
     def q_dim(self):
@@ -106,7 +121,8 @@ class Model:
 
 def model_from_tensors(shape, quant: int, tensors: dict, context_length: int) -> Model:
     """In-memory model (bench: synthetic weights never touch the disk)."""
-    arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3, "qwen2": ARCH_QWEN2, "qwen2moe": ARCH_QWEN2_MOE, "granite": ARCH_GRANITE}[shape.arch]
+    arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3, "qwen2": ARCH_QWEN2, "qwen2moe": ARCH_QWEN2_MOE, "granite": ARCH_GRANITE,
+            "devstral": ARCH_DEVSTRAL}[shape.arch]
     moe = shape.arch == "qwen2moe"
     cfg = Configuration(arch, "Q8_0" if quant == GGMLType.Q8_0 else "FP16",
                         shape.dim, 0 if moe else shape.hidden, shape.n_layers, shape.n_heads, shape.n_kv_heads, shape.head_size,
@@ -117,7 +133,13 @@ def model_from_tensors(shape, quant: int, tensors: dict, context_length: int) ->
     if shape.arch == "granite":
         for k, v in shape.granite_scales.items():
             setattr(cfg, k, float(np.float32(v)))
-    typ = {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3", "qwen2": "QWEN_2", "qwen2moe": "QWEN_2_MOE", "granite": "GRANITE"}[shape.arch]
+    if shape.arch == "devstral":
+        cfg.rms_norm_eps, cfg.rope_theta = float(np.float32(shape.eps)), float(np.float32(shape.rope_theta))
+        if shape.yarn:
+            f, bf, bs, lm, octx = shape.yarn
+            cfg.yarn = Yarn(float(np.float32(f)), float(np.float32(bf)), float(np.float32(bs)), float(np.float32(lm)), int(octx))
+    typ = {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3", "qwen2": "QWEN_2", "qwen2moe": "QWEN_2_MOE", "granite": "GRANITE",
+           "devstral": "DEVSTRAL_2"}[shape.arch]
     return Model(None, cfg, typ, tensors)
 
 
@@ -186,8 +208,11 @@ def load_model(path: str, context_length: int = -1) -> Model:
         cfg = _qwen2moe_configuration(md, g, q, context_length)
     elif typ == "GRANITE":
         cfg = granite_configuration(md, q, context_length)
+    elif typ == "DEVSTRAL_2":
+        cfg = devstral_configuration(md, q, context_length)
     else:
-        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 / Qwen2-MoE / Granite forward passes only)")
+        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 / Qwen2-MoE / Granite / "
+                               "Devstral 2 forward passes only)")
     return Model(g, cfg, typ)
 
 
@@ -243,6 +268,37 @@ def granite_configuration(md: dict, q: str, context_length: int) -> Configuratio
         residual_scale=f("granite.residual_scale", GRANITE_DEFAULT_SCALES["residual_scale"]),
         attention_scale=f("granite.attention.scale", GRANITE_DEFAULT_SCALES["attention_scale"]),
         logit_scale=f("granite.logit_scale", GRANITE_DEFAULT_SCALES["logit_scale"]))
+
+
+def devstral_configuration(md: dict, q: str, context_length: int) -> Configuration:
+    """DevstralModelLoader.createConfiguration (DevstralModelLoader.java:45-71) and the YaRN branch of its precomputeRopeFrequencies
+    (:76-110): mistral3.* keys; head size = attention.key_length (independent of dim / heads); head_count_kv defaults to head_count; the
+    vocabulary size is mistral3.vocab_size, else the token list's length; the context is clamped to the model's; eps defaults to 1e-5
+    and theta to 10000, both read as Java floats.  YaRN parameters are read only when rope.scaling.type is "yarn" (any other type gets
+    the plain table, as in the reference).  A file whose attention.value_length differs from key_length is refused: the reference sizes
+    V by key_length and would read it with the wrong width."""
+    p = "mistral3."
+    n_heads = int(md[p + "attention.head_count"])
+    head = int(md[p + "attention.key_length"])
+    if p + "attention.value_length" in md and int(md[p + "attention.value_length"]) != head:
+        raise UnsupportedModel(f"mistral3.attention.value_length {int(md[p + 'attention.value_length'])} != key_length {head}: the reference "
+                               "reads V with key_length's width, which would compute this model wrongly")
+    vocab = md.get(p + "vocab_size")
+    if vocab is None:
+        vocab = len(md["tokenizer.ggml.tokens"])
+    model_ctx = int(md[p + "context_length"])
+    ctx = model_ctx if (context_length < 0 or model_ctx < context_length) else context_length  # finalContextLength
+    f = lambda key, default: float(np.float32(md.get(key, default)))  # (float) metadata.getOrDefault(key, <float literal>)
+    yarn = None
+    if md.get(p + "rope.scaling.type", "") == "yarn":
+        s = p + "rope.scaling."
+        r = lambda key: float(np.float32(md[key]))  # (float) metadata.get(key): required
+        yarn = Yarn(r(s + "factor"), r(s + "yarn_beta_fast"), r(s + "yarn_beta_slow"), f(s + "yarn_log_multiplier", 0.0),
+                    int(md[s + "original_context_length"]))
+    return Configuration(
+        ARCH_DEVSTRAL, q, int(md[p + "embedding_length"]), int(md[p + "feed_forward_length"]), int(md[p + "block_count"]), n_heads,
+        int(md.get(p + "attention.head_count_kv", n_heads)), head, int(vocab), ctx, f(p + "attention.layer_norm_rms_epsilon", 1e-5),
+        f(p + "rope.freq_base", 10000.0), yarn=yarn)
 
 
 def tensor_as_f32(model: Model, name: str) -> np.ndarray:

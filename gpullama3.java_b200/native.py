@@ -44,12 +44,17 @@ class GraniteConfig(C.Structure):
     _fields_ = [(n, C.c_float) for n in ("embedding_scale", "residual_scale", "attention_scale", "logit_scale")]
 
 
+class YarnConfig(C.Structure):
+    """b200_yarn_config: the YaRN parameters of a B200_ARCH_DEVSTRAL plan's RoPE table."""
+    _fields_ = [(n, C.c_float) for n in ("factor", "beta_fast", "beta_slow", "log_multiplier")] + [("original_context_length", C.c_int32)]
+
+
 class Tensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("ggml_type", C.c_int32), ("n_dims", C.c_int32),
                 ("dims", C.c_int64 * 4)]
 
 
-EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
+EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
@@ -71,6 +76,7 @@ def lib() -> C.CDLL:
     L.b200_plan_create.argtypes = [C.POINTER(Config), C.POINTER(Tensor), i32, i32, i32, C.POINTER(vp), C.c_char_p, C.c_size_t]
     L.b200_plan_create_moe.argtypes = [C.POINTER(Config), C.POINTER(MoeConfig), C.POINTER(Tensor), i32, i32, i32, C.POINTER(vp), C.c_char_p, C.c_size_t]
     L.b200_plan_create_granite.argtypes = [C.POINTER(Config), C.POINTER(GraniteConfig), C.POINTER(Tensor), i32, i32, i32, C.POINTER(vp), C.c_char_p, C.c_size_t]
+    L.b200_plan_create_devstral.argtypes = [C.POINTER(Config), C.POINTER(YarnConfig), C.POINTER(Tensor), i32, i32, i32, C.POINTER(vp), C.c_char_p, C.c_size_t]
     L.b200_forward_decode.argtypes = [vp, i32, i32, vp, C.POINTER(i32)]
     L.b200_forward_prefill.argtypes = [vp, i32, i32]
     L.b200_forward_decode_sample.argtypes = [vp, i32, i32, C.c_float, C.c_float, C.c_float, C.POINTER(i32), C.POINTER(i32)]
@@ -271,7 +277,8 @@ class NativePlan:
     """Owns one ``b200_plan*``."""
 
     def __init__(self, cfg: Config, tensors: dict, prefill_batch_size: int = 0, device: int = 0, moe: MoeConfig | None = None,
-                 granite: GraniteConfig | None = None):
+                 granite: GraniteConfig | None = None, devstral: bool = False, yarn: YarnConfig | None = None):
+        """devstral: create through b200_plan_create_devstral, with `yarn` (None: the plain RoPE table)."""
         L = lib()
         arr = (Tensor * len(tensors))()
         self._keep = []
@@ -291,7 +298,10 @@ class NativePlan:
                 arr[i].dims[k] = int(d)
         out = C.c_void_p()
         err = C.create_string_buffer(512)
-        if granite is not None:
+        if devstral:
+            rc = L.b200_plan_create_devstral(C.byref(cfg), C.byref(yarn) if yarn is not None else None, arr, len(tensors), prefill_batch_size,
+                                             device, C.byref(out), err, 512)
+        elif granite is not None:
             rc = L.b200_plan_create_granite(C.byref(cfg), C.byref(granite), arr, len(tensors), prefill_batch_size, device, C.byref(out), err, 512)
         elif moe is not None:
             rc = L.b200_plan_create_moe(C.byref(cfg), C.byref(moe), arr, len(tensors), prefill_batch_size, device, C.byref(out), err, 512)

@@ -13,7 +13,7 @@ import os
 import numpy as np
 
 from . import native
-from .loader import ARCH_GRANITE, Model
+from .loader import ARCH_DEVSTRAL, ARCH_GRANITE, Model
 
 
 def _flag(name: str, default: str) -> str:
@@ -87,7 +87,10 @@ class B200MasterPlan:
             moe = native.MoeConfig(c.n_experts, c.n_experts_used, c.expert_hidden_dim, c.shared_hidden_dim)
         if c.arch == ARCH_GRANITE:  # Granite: b200_plan_create_granite
             granite = native.GraniteConfig(c.embedding_scale, c.residual_scale, c.attention_scale, c.logit_scale)
-        self._native = native.NativePlan(cfg, model.tensors, self.prefill_batch_size, device, moe=moe, granite=granite)
+        y = c.yarn  # Devstral: b200_plan_create_devstral, YaRN table or (None) the plain one
+        yarn = native.YarnConfig(y.factor, y.beta_fast, y.beta_slow, y.log_multiplier, y.original_context_length) if y is not None else None
+        self._native = native.NativePlan(cfg, model.tensors, self.prefill_batch_size, device, moe=moe, granite=granite,
+                                         devstral=c.arch == ARCH_DEVSTRAL, yarn=yarn)
         self.tp_rank, self.tp_size = tp_rank, tp_size
         if tp_size > 1:
             # one process per GPU: swap IPC handles of the communication buffers, then wire the peers

@@ -18,7 +18,7 @@ from .gguf import GGMLType, write_gguf
 
 @dataclass(frozen=True)
 class Shape:
-    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2" | "qwen2moe" | "granite"
+    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2" | "qwen2moe" | "granite" | "devstral" (GGUF architecture mistral3)
     dim: int
     hidden: int  # qwen2moe: the shared expert's hidden size
     n_layers: int
@@ -33,6 +33,7 @@ class Shape:
     n_experts: int = 0        # qwen2moe: expert_count
     n_experts_used: int = 0   # expert_used_count
     expert_hidden: int = 0    # the routed experts' hidden size (ffn_down_exps dims[0])
+    yarn: tuple = ()          # devstral: (factor, beta_fast, beta_slow, log_multiplier, original_context_length); () = no rope.scaling keys
 
     @property
     def q_dim(self):
@@ -118,6 +119,17 @@ SHAPES = {
     "granite-3-8b": Shape("granite", 4096, 12800, 40, 32, 8, 128, 49155, True, 10000.0, 1e-5, 4096),
     # a Llama model whose vocabulary is not a multiple of 4: the streaming classifier's padding rows
     "tiny-llama-vocab509": Shape("llama", 256, 512, 2, 4, 2, 64, 509, False, 500000.0, 1e-5),
+    # Devstral 2 (mistral3: head size independent of dim / heads, YaRN RoPE table): tiny-devstral has qd 256 < dim 512, GQA 2 and YaRN
+    # parameters whose ramp, mscale and correction range all show at short contexts (theta 1e4, head 64, original context 256: the
+    # correction dims are 0.84 and 12.9, inside [0, 31]); tiny-devstral-plain has no rope.scaling keys and qd == dim.  2-layer cuts of
+    # Devstral-Small-2 (24B: 5120 / 32768 / 32 x 128 / 8, qd 4096 < dim) and Devstral 2 (123B: 12288 / 28672 / 96 x 128 / 8) with an
+    # 8192-token vocabulary, and the whole Small 2 model (tools/devstral_bench.py).  The YaRN values of the larger shapes are synthetic.
+    "tiny-devstral": Shape("devstral", 512, 1024, 2, 4, 2, 64, 512, False, 10000.0, 1e-5, 1024, yarn=(4.0, 32.0, 1.0, 1.0, 256)),
+    "tiny-devstral-plain": Shape("devstral", 256, 512, 2, 4, 2, 64, 512, False, 10000.0, 1e-5, 1024),
+    "tiny-devstral-wide": Shape("devstral", 256, 512, 2, 8, 2, 64, 512, False, 10000.0, 1e-5, 1024, yarn=(4.0, 32.0, 1.0, 1.0, 256)),  # qd 512 > dim
+    "mid-devstral-small-2": Shape("devstral", 5120, 32768, 2, 32, 8, 128, 8192, False, 1000000.0, 1e-5, 4096, yarn=(16.0, 32.0, 1.0, 1.0, 2048)),
+    "mid-devstral-2": Shape("devstral", 12288, 28672, 2, 96, 8, 128, 8192, False, 1000000.0, 1e-5, 4096, yarn=(16.0, 32.0, 1.0, 1.0, 2048)),
+    "devstral-small-2": Shape("devstral", 5120, 32768, 40, 32, 8, 128, 131072, False, 1000000.0, 1e-5, 4096, yarn=(16.0, 32.0, 1.0, 1.0, 2048)),
 }
 
 
@@ -228,7 +240,7 @@ def build_vocab(vocab_size: int, arch: str = "llama", seed: int = 1234):
 
 
 def metadata_for(shape: Shape, quant: int, name: str) -> dict:
-    a = shape.arch
+    a = "mistral3" if shape.arch == "devstral" else shape.arch  # the GGUF architecture, and the prefix of its keys
     md = {
         "general.architecture": a,
         "general.name": name,  # ModelLoader.detectModelType keys on this substring (ModelLoader.java:57-80)
@@ -258,6 +270,17 @@ def metadata_for(shape: Shape, quant: int, name: str) -> dict:
         md["granite.residual_scale"] = float(s["residual_scale"])
         md["granite.attention.scale"] = float(s["attention_scale"])
         md["granite.logit_scale"] = float(s["logit_scale"])
+    if a == "mistral3":  # DevstralModelLoader.createConfiguration / precomputeRopeFrequencies
+        md["mistral3.attention.key_length"] = shape.head_size
+        md["mistral3.attention.value_length"] = shape.head_size
+        if shape.yarn:
+            f, bf, bs, lm, octx = shape.yarn
+            md["mistral3.rope.scaling.type"] = "yarn"
+            md["mistral3.rope.scaling.factor"] = float(f)
+            md["mistral3.rope.scaling.yarn_beta_fast"] = float(bf)
+            md["mistral3.rope.scaling.yarn_beta_slow"] = float(bs)
+            md["mistral3.rope.scaling.yarn_log_multiplier"] = float(lm)
+            md["mistral3.rope.scaling.original_context_length"] = int(octx)
     if shape.vocab <= 4096 or a in ("qwen2", "qwen2moe"):  # tokenizer section (Qwen2 takes its vocabulary size from the token list) (GGUF keys the loaders read: tokenizer.ggml.tokens / merges / token_type)
         tokens, merges, types, base = build_vocab(shape.vocab, a)
         md["tokenizer.ggml.model"] = "gpt2"
@@ -421,7 +444,7 @@ def write_model(path: str, shape_name: str, quant: int, seed: int = 1234, w_std:
                 display_name: str | None = None):
     shape = SHAPES[shape_name]
     name = display_name or {"llama": "Llama synthetic ", "qwen3": "Qwen3 synthetic ", "phi3": "Phi3 synthetic ", "qwen2": "Qwen2 synthetic ",
-                            "qwen2moe": "Qwen1.5 MoE synthetic ", "granite": "Granite synthetic "}[shape.arch] + shape_name
+                            "qwen2moe": "Qwen1.5 MoE synthetic ", "granite": "Granite synthetic ", "devstral": "Devstral synthetic "}[shape.arch] + shape_name
     write_gguf(path, metadata_for(shape, quant, name), build_tensors(shape, quant, seed, w_std))
     return shape
 

@@ -47,6 +47,10 @@ extern "C" {
                                * biases, NeoX RoPE) and a mixture-of-experts FFN.  Created with b200_plan_create_moe only. */
 #define B200_ARCH_GRANITE 5 /* InferenceCore.forwardGranite, InferenceCore.java:814-921 (Granite 3.x): Llama's tensors and forward with four
                              * muP scalars (b200_granite_config).  Created with b200_plan_create_granite only. */
+#define B200_ARCH_DEVSTRAL 6 /* InferenceCore.forwardJavaDevstral, InferenceCore.java:178-261 (Devstral 2, GGUF architecture mistral3): Llama's
+                              * tensors and forward with an independent head size (n_heads * head_size may differ from dim: q has that
+                              * width, RoPE rotates interleaved pairs over it, Wo takes it as columns) and a RoPE table that may be
+                              * YaRN-scaled (b200_yarn_config).  Created with b200_plan_create_devstral only. */
 
 /* GGML tensor type ids accepted for weights (tensor/GGMLType.java:5-20) */
 #define B200_GGML_F32 0
@@ -68,7 +72,7 @@ typedef struct b200_config {
     int32_t n_layers;       /* block_count */
     int32_t n_heads;        /* attention.head_count */
     int32_t n_kv_heads;     /* attention.head_count_kv */
-    int32_t head_size;      /* dim/n_heads (Llama) or attention.key_length (Qwen3) */
+    int32_t head_size;      /* dim/n_heads (Llama) or attention.key_length (Qwen3, Devstral) */
     int32_t vocab_size;
     int32_t context_length; /* KV-cache positions to allocate (Options.maxTokens) */
     float rms_norm_eps;
@@ -110,6 +114,18 @@ typedef struct b200_granite_config {
     float logit_scale;     /* granite.logit_scale, default 16.0 */
 } b200_granite_config;
 
+/* YaRN parameters of a B200_ARCH_DEVSTRAL plan's RoPE table (mistral3.rope.scaling.*, read when rope.scaling.type is "yarn";
+ * DevstralModelLoader.precomputeRopeFrequencies).  The table is RoPE.precomputeFreqsCisYaRN evaluated with Java's float / double
+ * boundaries: per pair i, freq = (freq_extrap / factor) * (1 - ramp_i) + freq_extrap * ramp_i, cos / sin narrowed to float, then times
+ * mscale = 1 + 0.1 * log_multiplier * ln(factor) (1 when log_multiplier <= 0). */
+typedef struct b200_yarn_config {
+    float factor;                    /* rope.scaling.factor, > 0 */
+    float beta_fast;                 /* rope.scaling.yarn_beta_fast */
+    float beta_slow;                 /* rope.scaling.yarn_beta_slow */
+    float log_multiplier;            /* rope.scaling.yarn_log_multiplier, default 0 */
+    int32_t original_context_length; /* rope.scaling.original_context_length, > 0 */
+} b200_yarn_config;
+
 typedef struct b200_plan b200_plan;
 
 /* TornadoVMMasterPlan.initializeTornadoVMPlan(state, model) (TornadoVMMasterPlan.java:55-70)
@@ -145,6 +161,14 @@ int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, con
  * B200_ERR_BAD_ARG and names the scale.  Every decode mode, weight format and prefill mode of a Llama plan is available. */
 int b200_plan_create_granite(const b200_config *cfg, const b200_granite_config *granite, const b200_tensor *tensors, int32_t n_tensors,
                              int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
+
+/* b200_plan_create for cfg->arch == B200_ARCH_DEVSTRAL (b200_plan_create refuses that arch with B200_ERR_BAD_ARG, and this call every
+ * other).  The tensors are Llama's; blk.N.attn_q.weight has n_heads * head_size rows and attn_output.weight that many columns.
+ * yarn == NULL: the plain RoPE table (RoPE.precomputeFreqsCis).  A YaRN field that is not finite, factor <= 0 or
+ * original_context_length <= 0 fails with B200_ERR_BAD_ARG naming the field.  Every decode mode, weight format and prefill mode of a
+ * Llama plan is available; the persistent decode kernel needs dim <= 8192 (b200_set_decode_mode reports the reason otherwise). */
+int b200_plan_create_devstral(const b200_config *cfg, const b200_yarn_config *yarn, const b200_tensor *tensors, int32_t n_tensors,
+                              int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
 
 /* TornadoVMMasterPlan.tornadoVMForwardDecode(position) with the embedding gather moved
  * device-side (replaces InferenceCore.forwardTornadoVM, InferenceCore.java:956-980, which copies
@@ -316,6 +340,7 @@ int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_ste
  * "pf_h16" (f16 bits, SwiGLU output).  Qwen2-MoE plans: "hb", "hq", "hs" hold the virtual hidden vector of the last layer (the shared
  * expert's units, then each routed slot's, shared_hidden_dim + n_experts_used * expert_hidden_dim units), "moe_ids" (int32 [layer][k], the experts the last step selected, in
  * selection order) and "moe_weights" (f32 [layer][k + 1], their routing weights, then the shared-expert weight).
+ * "rope_cr" / "rope_ci": the RoPE table every decode and prefill kernel reads (f32 [context_length][head_size / 2]).
  * Copies min(bytes, buffer size). */
 int b200_read_buffer(b200_plan *plan, const char *name, int32_t layer, void *dst, size_t bytes);
 
@@ -361,7 +386,7 @@ int b200_trace_persistent(b200_plan *plan, int32_t token, int32_t position, uint
 int b200_profile_norm(b200_plan *plan, int64_t *cycles);
 
 /* Test hook for the exact parallel evaluation of the reference's sequential float sum (csrc/seqsum2.cuh; the RMSNorm
- * accumulator of InferenceCore.java:39-48): sums n <= 8192 non-negative host floats on the device exactly as
+ * accumulator of InferenceCore.java:39-48): sums n <= 16384 non-negative host floats on the device exactly as
  * `for (i) s += t[i]` would, run by `threads` = 1024 (the RMSNorm kernel's form), 512 (the persistent decode kernel's form)
  * or 256 threads; info = {items walked, fallbacks}. */
 int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out, int32_t *info /* nullable */);

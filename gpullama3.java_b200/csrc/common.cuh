@@ -156,15 +156,6 @@ __device__ __forceinline__ int quant_block_lane(float v, float &ascale) {
     return __float2int_rz(__fadd_rn(s, copysignf(0.5f, s)));
 }
 
-// One whole Q8_0 quant block (32 bytes) per lane as two 128-bit read-only streaming loads
-// (sm_90 has no 256-bit global load).
-__device__ __forceinline__ void ldg256_stream(const void *p, int (&r)[8]) {
-    asm("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "l"(p));
-    asm("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];"
-        : "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-        : "l"(reinterpret_cast<const char *>(p) + 16));
-}
-
 __device__ __forceinline__ int4 ldg128_stream(const void *p) {
     int4 r;
     asm("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
@@ -179,10 +170,10 @@ __device__ __forceinline__ float f16_bits_to_f32_daz(unsigned h) {
     return __uint_as_float(bits);
 }
 
-// Weight matrix as stored on the device.
-//   Q8_0: qs = int8 [rows][cols] row-major, sc = f16 scale [rows][cols/32]
-//         (GGUF's 34-byte blocks split at upload so the quants are 32-byte aligned: same
-//          1.0625 B/element, one LDG.256 per block).
+// Row-major matrix as stored on the device: the embedding table, and the FP16 weight matrices (a Q8_0 plan's weight
+// matrices are tile-major streams, stream_matvec.cuh).
+//   Q8_0: qs = int8 [rows][cols], sc = f16 scale [rows][cols/32] (GGUF's 34-byte blocks split at upload: same
+//         1.0625 B/element, and a row gather reads each plane with plain indexing).
 //   F16 : qs = f16 [rows][cols], sc unused.  F32: qs = float.
 struct DevMat {
     const void *qs;

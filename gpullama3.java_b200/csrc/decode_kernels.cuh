@@ -1,12 +1,10 @@
-// decode_kernels.cuh -- single-token decode kernels (Q8_0 and FP16 weights), bit-exact with the
-// reference's CPU path.  One CUDA graph strings them together per token (plan.cu).
+// decode_kernels.cuh -- single-token decode kernels, bit-exact with the reference's CPU path: the RMSNorm, the attention
+// and the FP16 matvecs (the Q8_0 matvecs are the weight streams of stream_matvec.cuh).  One CUDA graph strings them together
+// per token (plan.cu).
 //
 // Replaces (reference kernel inventory, SURVEY.md 2.K):
 //   k_rmsnorm_quant  <- reductionOneBlockWithLayer + reductionOneBlock2WithLayer / mapContextWithQuantize
 //                       (TransformerComputeKernelsLayered.java:387-454) + convertQ8_0toFP32 embedding
-//   k_matvec_q8      <- fusedQKVMatmulQ8 / matrixVectorGenericWithResidualQ8_0Byte / matrixVectorGenericQ8Byte
-//                       (TransformerComputeKernelsLayered.java:3038-3223, 2888-2906, 2773-2787)
-//   k_gateup_q8      <- fullyFusedRmsNormFFNGateUpQ8 (:3386-3549)
 //   k_rope_kv        <- ropeRotationWithCacheCopy (:495-542), Qwen3 fusedQKRmsNorm + NeoX rope (Qwen3Kernels.java:302-361,973-1064)
 //   k_attention      <- processHeadsFlashAttention (:784-906)
 //   k_argmax_advance <- argmaxLogits (TransformerComputeKernels.java:25-56), with CPU tie-break semantics
@@ -154,153 +152,11 @@ __global__ void __launch_bounds__(T, 1) k_test_seqsum2(const float *__restrict__
 }
 
 // ------------------------------------------------------------------------------------------
-// Q8_0 dequant-matvec, bit-exact with Q8_0FloatTensor.dotQ8Activation (Q8_0FloatTensor.java:90-123):
-//   per 32-block b:  isum_b = sum aq*wq (int32, exact);  term_b = (float)isum_b * (wScale_b * aScale_b)
-//   result = ((term_0 + term_1) + term_2) + ...      strictly in block order.
-// The activation quantisation is row-independent, so it arrives pre-quantised (xq, xs).
-// Mapping: a warp owns R rows; lane l owns blocks l, l+32, ... of each row (one LDG.256 per block,
-// the warp reads 1 KB contiguous per instruction); block terms go to shared memory and lanes
-// 0..R-1 then walk their row's terms in order.
-// ------------------------------------------------------------------------------------------
-template <int R>
-__device__ __forceinline__ void q8_row_terms(const int8_t *__restrict__ qs, const __half *__restrict__ sc, size_t row0,
-                                             int cols, int nb, const int4 *__restrict__ sxq, const float *__restrict__ sxs,
-                                             float *__restrict__ terms, int nbp, int lane) {
-    constexpr int JB = R >= 4 ? 2 : 4; // 64 registers of weights in flight per lane
-    for (int b0 = 0; b0 < nb; b0 += 32 * JB) {
-        int wv[R][JB][8];
-        __half sv[R][JB];
-#pragma unroll
-        for (int r = 0; r < R; r++)
-#pragma unroll
-            for (int j = 0; j < JB; j++) {
-                int b = b0 + j * 32 + lane;
-                if (b < nb) {
-                    ldg256_stream(qs + (row0 + r) * (size_t)cols + (size_t)b * 32, wv[r][j]);
-                    sv[r][j] = sc[(row0 + r) * (size_t)nb + b];
-                }
-            }
-#pragma unroll
-        for (int j = 0; j < JB; j++) {
-            int b = b0 + j * 32 + lane;
-            if (b < nb) {
-                int4 a0 = sxq[b], a1 = sxq[nb + b];
-                float as = sxs[b];
-#pragma unroll
-                for (int r = 0; r < R; r++) {
-                    int isum = __dp4a(wv[r][j][0], a0.x, 0);
-                    isum = __dp4a(wv[r][j][1], a0.y, isum);
-                    isum = __dp4a(wv[r][j][2], a0.z, isum);
-                    isum = __dp4a(wv[r][j][3], a0.w, isum);
-                    isum = __dp4a(wv[r][j][4], a1.x, isum);
-                    isum = __dp4a(wv[r][j][5], a1.y, isum);
-                    isum = __dp4a(wv[r][j][6], a1.z, isum);
-                    isum = __dp4a(wv[r][j][7], a1.w, isum);
-                    terms[r * nbp + b] = __fmul_rn((float)isum, __fmul_rn(__half2float(sv[r][j]), as));
-                }
-            }
-        }
-    }
-}
-
-// Stage the quantised activation in shared memory as two planes of 16-byte half-blocks
-// (plane p holds bytes [16p,16p+16) of every block) so that lanes reading consecutive
-// blocks hit consecutive 16-byte slots: conflict-free LDS.128.
-__device__ __forceinline__ void stage_activation(const int8_t *__restrict__ xq, const float *__restrict__ xs, int cols,
-                                                 int4 *sxq, float *sxs) {
-    const int nb = cols >> 5;
-    const int4 *src = reinterpret_cast<const int4 *>(xq);
-    for (int c = threadIdx.x; c < cols / 16; c += blockDim.x) sxq[(c & 1) * nb + (c >> 1)] = src[c];
-    for (int b = threadIdx.x; b < nb; b += blockDim.x) sxs[b] = xs[b];
-}
-
-__host__ __device__ inline size_t q8_smem_bytes(int cols, int rows_per_warp, int warps) {
-    int nb = cols / 32, nbp = nb | 1;
-    return (size_t)cols + (size_t)nb * 4 + (size_t)warps * rows_per_warp * nbp * 4 + 64;
-}
-
-template <int R, int MODE>
-__global__ void __launch_bounds__(256) k_matvec_q8(const int8_t *__restrict__ qs, const __half *__restrict__ sc,
-                                                   const int8_t *__restrict__ xq, const float *__restrict__ xs, int rows,
-                                                   int cols, float *__restrict__ out, float oscale) {
-    extern __shared__ __align__(16) unsigned char smraw[];
-    const int nb = cols >> 5, nbp = nb | 1;
-    int4 *sxq = reinterpret_cast<int4 *>(smraw);
-    float *sxs = reinterpret_cast<float *>(smraw + cols);
-    float *terms_all = sxs + nb;
-    stage_activation(xq, xs, cols, sxq, sxs);
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float *terms = terms_all + (size_t)warp * R * nbp;
-    const int nwarps_total = gridDim.x * (blockDim.x >> 5);
-    for (size_t row0 = (size_t)(blockIdx.x * (blockDim.x >> 5) + warp) * R; row0 < (size_t)rows; row0 += (size_t)nwarps_total * R) {
-        q8_row_terms<R>(qs, sc, row0, cols, nb, sxq, sxs, terms, nbp, lane);
-        __syncwarp();
-        if (lane < R) {
-            const float *t = terms + lane * nbp;
-            float acc = 0.0f;
-            for (int b = 0; b < nb; b++) acc = __fadd_rn(acc, t[b]);
-            size_t row = row0 + lane;
-            acc = __fmul_rn(acc, oscale); // Granite's residualScale / logitScale (1.0f: unchanged)
-            if (MODE == MODE_RESID) out[row] = __fadd_rn(out[row], acc); // x[i] = x[i] + xb2[i]  (InferenceCore.java:143,164)
-            else out[row] = acc;
-        }
-        __syncwarp();
-    }
-}
-
-// ------------------------------------------------------------------------------------------
-// Fused gate/up projection + SwiGLU + Q8_0 quantisation of the result (the activation of the
-// down projection).  InferenceCore.java:150-158: hb = hb / (float)(1.0 + Math.exp(-hb)); hb *= hb2.
-// One CTA (8 warps) = one 32-element block of hb, so the CTA can quantise it in its epilogue.
+// SwiGLU of one hidden unit, InferenceCore.java:150-158: hb = hb / (float)(1.0 + Math.exp(-hb)); hb *= hb2.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float swiglu(float g, float u) {
     float s = __fdiv_rn(g, (float)(1.0 + exp((double)(-g))));
     return __fmul_rn(s, u);
-}
-
-__global__ void __launch_bounds__(256) k_gateup_q8(const int8_t *__restrict__ qs1, const __half *__restrict__ sc1,
-                                                   const int8_t *__restrict__ qs3, const __half *__restrict__ sc3,
-                                                   const int8_t *__restrict__ xq, const float *__restrict__ xs, int hidden,
-                                                   int cols, int8_t *__restrict__ hq, float *__restrict__ hs,
-                                                   float *__restrict__ hb_dbg) {
-    extern __shared__ __align__(16) unsigned char smraw[];
-    __shared__ float hvals[32];
-    const int nb = cols >> 5, nbp = nb | 1;
-    int4 *sxq = reinterpret_cast<int4 *>(smraw);
-    float *sxs = reinterpret_cast<float *>(smraw + cols);
-    float *terms_all = sxs + nb;
-    stage_activation(xq, xs, cols, sxq, sxs);
-    __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float *terms = terms_all + (size_t)warp * 4 * nbp; // 2 hidden units x {gate, up}
-    for (int blk = blockIdx.x; blk < hidden / 32; blk += gridDim.x) {
-#pragma unroll 1
-        for (int half = 0; half < 2; half++) {
-            int u0 = blk * 32 + warp * 4 + half * 2; // this warp: hidden units u0, u0+1
-            q8_row_terms<2>(qs1, sc1, (size_t)u0, cols, nb, sxq, sxs, terms, nbp, lane);
-            q8_row_terms<2>(qs3, sc3, (size_t)u0, cols, nb, sxq, sxs, terms + 2 * nbp, nbp, lane);
-            __syncwarp();
-            float acc = 0.0f;
-            if (lane < 4) {
-                const float *t = terms + lane * nbp;
-                for (int b = 0; b < nb; b++) acc = __fadd_rn(acc, t[b]);
-            }
-            float up = __shfl_down_sync(0xffffffffu, acc, 2); // lanes 0,1 = gate(u0,u0+1); lanes 2,3 = up
-            if (lane < 2) hvals[warp * 4 + half * 2 + lane] = swiglu(acc, up);
-            __syncwarp();
-        }
-        __syncthreads();
-        if (warp == 0) {
-            float v = hvals[lane];
-            if (hb_dbg) hb_dbg[blk * 32 + lane] = v;
-            float as;
-            int q = quant_block_lane(v, as);
-            hq[blk * 32 + lane] = (int8_t)q;
-            if (lane == 0) hs[blk] = as;
-        }
-        __syncthreads();
-    }
 }
 
 // ------------------------------------------------------------------------------------------

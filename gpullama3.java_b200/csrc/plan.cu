@@ -91,7 +91,7 @@ struct b200_plan {
 
     DevMat emb{}, out{};
     TileMat tout{};
-    bool use_stream = false, use_pdl = false;
+    bool use_pdl = false;
     bool fuse_norm = false; // single-GPU Q8_0 streams: QKV, gate/up and lm_head compute their RMSNorm themselves (k_stream_matvec_q8_norm)
     int kflags = 0; // KF_* (common.cuh): what the attention prologues do for this architecture
     size_t kq_off = 0; // K-quant files: offset of the raw (K-quant bytes) area inside each staging buffer; 0 = no K-quant tensor in the file
@@ -533,20 +533,6 @@ float out_scale(const b200_plan *p, bool resid, bool classifier) { return resid 
 // The attention kernels' score argument: the divisor sqrt(head size), or (KF_ATTSCALE) Granite's attentionScale multiplier.
 float att_score_arg(const b200_plan *p) { return (p->kflags & KF_ATTSCALE) ? p->mup.attention_scale : (float)sqrt((double)p->cfg.head_size); }
 
-template <int MODE> int launch_matvec_q8(b200_plan *p, const DevMat &m, const int8_t *xq, const float *xs, float *out) {
-    int R = (m.rows % 4 == 0 && m.rows >= 32768) ? 4 : (m.rows % 2 == 0 ? 2 : 1);
-    int warps = m.rows / R;
-    int ctas = (warps + 7) / 8;
-    size_t smem = q8_smem_bytes(m.cols, R, 8);
-    const int8_t *qs = (const int8_t *)m.qs;
-    const float os = out_scale(p, MODE == MODE_RESID, &m == &p->out);
-    if (R == 4) k_matvec_q8<4, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out, os);
-    else if (R == 2) k_matvec_q8<2, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out, os);
-    else k_matvec_q8<1, MODE><<<ctas, 256, smem, p->stream>>>(qs, m.sc, xq, xs, m.rows, m.cols, out, os);
-    CK(cudaGetLastError());
-    return B200_OK;
-}
-
 size_t f16_smem_bytes(int cols, int lanes) {
     int L = lanes > 0 ? lanes : 1;
     return (size_t)cols * 4 + (size_t)8 * (32 / L) * 256 * 2;
@@ -705,7 +691,7 @@ int enqueue_moe_ffn(b200_plan *p, int l, TraceBuf tr) {
 int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = false) {
     const b200_config &c = p->cfg;
     const bool q8 = p->wtype == B200_GGML_Q8_0;
-    const bool st = p->use_stream, pdl = p->use_pdl, sf = p->use_f16_stream;
+    const bool pdl = p->use_pdl, sf = p->use_f16_stream;
     const bool tpar = p->tp.n > 1;
     const bool fz = p->fuse_norm; // attention / FFN / final norm inside QKV / gate-up / lm_head: 5 launches per layer instead of 7
     int n = 0;
@@ -730,8 +716,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
         else {
             if ((rc = norm(l == 0, L.attn_norm, l == 0 ? -1 : 4 * (l - 1) + 3))) return rc;
             n++;
-            if (st) rc = launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr, false, TR(2));
-            else if (q8) rc = launch_matvec_q8<MODE_STORE>(p, L.qkv, p->xq, p->xs, p->qkv);
+            if (q8) rc = launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr, false, TR(2));
             else if (sf) rc = launch_stream_f16<SF_STORE>(p, L.qkv, nullptr, p->xb, p->qkv, TR(2));
             else rc = launch_matvec_f16<MODE_STORE>(p, L.qkv, p->xb, p->qkv);
         }
@@ -745,8 +730,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
                             p->tp, (unsigned)(4 * l + 0), rank * p->nh_l, p->att_scratch, c.context_length);
         });
         if (rc) return rc; n++;
-        if (st) rc = launch_stream<SMV_RESID>(p, L.two, p->attq, p->atts, p->x, nullptr, nullptr, false, TR(5), tpar ? TP_SLOT_ATT : -1, 4 * l + 0, tpar ? TP_SLOT_X : -1, 4 * l + 1, rank * p->dim_l);
-        else if (q8) rc = launch_matvec_q8<MODE_RESID>(p, L.wo, p->xq, p->xs, p->x);
+        if (q8) rc = launch_stream<SMV_RESID>(p, L.two, p->attq, p->atts, p->x, nullptr, nullptr, false, TR(5), tpar ? TP_SLOT_ATT : -1, 4 * l + 0, tpar ? TP_SLOT_X : -1, 4 * l + 1, rank * p->dim_l);
         else if (sf) rc = launch_stream_f16<SF_RESID>(p, L.wo, nullptr, p->xb, p->x, TR(5));
         else rc = launch_matvec_f16<MODE_RESID>(p, L.wo, p->xb, p->x);
         if (rc) return rc; n++;
@@ -759,16 +743,11 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
             if ((rc = norm(false, L.ffn_norm, 4 * l + 1))) return rc;
             n++;
         }
-        if (st) {
+        if (q8) {
             if (fz) rc = launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, TR(6)); // FFN norm + gate/up
             else rc = launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs, false, TR(6), -1, 0, tpar ? TP_SLOT_HQ : -1, 4 * l + 2, rank * p->hid_l);
             if (rc) return rc; n++;
             if ((rc = launch_stream<SMV_RESID>(p, L.tw2, p->hq, p->hs, p->x, nullptr, nullptr, false, TR(7), tpar ? TP_SLOT_HQ : -1, 4 * l + 2, tpar ? TP_SLOT_X : -1, 4 * l + 3, rank * p->dim_l))) return rc; n++;
-        } else if (q8) {
-            k_gateup_q8<<<c.hidden_dim / 32, 256, q8_smem_bytes(c.dim, 4, 8), p->stream>>>(
-                (const int8_t *)L.w1.qs, L.w1.sc, (const int8_t *)L.w3.qs, L.w3.sc, p->xq, p->xs, c.hidden_dim, c.dim, p->hq, p->hs, p->hb);
-            CK(cudaGetLastError()); n++;
-            if ((rc = launch_matvec_q8<MODE_RESID>(p, L.w2, p->hq, p->hs, p->x))) return rc; n++;
         } else if (sf) { // gate, up and SwiGLU in one launch; then the down projection
             if ((rc = launch_stream_f16<SF_GATEUP>(p, L.w1, &L.w3, p->xb, p->hb, TR(6)))) return rc; n++;
             if ((rc = launch_stream_f16<SF_RESID>(p, L.w2, nullptr, p->hb, p->x, TR(7)))) return rc; n++;
@@ -788,8 +767,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
         else {
             if ((rc = norm(false, p->out_norm, last_x_op))) return rc;
             n++;
-            if (st) rc = launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr, true, TR(8), -1, 0, -1, 0, rank * p->voc_l);
-            else if (q8) rc = launch_matvec_q8<MODE_STORE>(p, p->out, p->xq, p->xs, p->logits);
+            if (q8) rc = launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr, true, TR(8), -1, 0, -1, 0, rank * p->voc_l);
             else if (sf) rc = launch_stream_f16<SF_STORE>(p, p->out, nullptr, p->xb, p->logits, TR(8), true);
             else rc = launch_matvec_f16<MODE_STORE>(p, p->out, p->xb, p->logits);
         }
@@ -798,7 +776,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
     {
         int rc;
         if ((rc = launch_k(p, pdl, k_argmax_advance, dim3(1), dim3(1024), (size_t)0, (const float *)p->logits, c.vocab_size, p->st, (const int *)p->seq_tokens, p->out_ids, with_logits ? 1 : 0,
-                           (const float *)(st || sf ? p->part_val : nullptr), (const int *)(st || sf ? p->part_idx : nullptr),
+                           (const float *)(q8 || sf ? p->part_val : nullptr), (const int *)(q8 || sf ? p->part_idx : nullptr),
                            sf ? sf_grid(p, c.vocab_size, c.dim, false) : p->n_sms, TR(9), p->tp, with_logits ? -1 : last_x_op))) return rc;
         n++;
     }
@@ -814,7 +792,7 @@ int pd_prepare(b200_plan *p) {
     p->pd_ok = false;
     if (p->is_moe) { p->pd_why = "the persistent decode kernel has no Qwen2-MoE layer (MoE plans decode through the CUDA graph)"; return B200_OK; }
     if (c.dim > 8192) { p->pd_why = "the persistent decode kernel's register-resident RMSNorm supports dim <= 8192"; return B200_OK; }
-    if (!p->use_stream) { p->pd_why = "the persistent decode kernel needs the Q8_0 streaming layout"; return B200_OK; }
+    if (p->wtype != B200_GGML_Q8_0) { p->pd_why = "the persistent decode kernel needs Q8_0 weights"; return B200_OK; }
     if (c.head_size != 64 && c.head_size != 128) { p->pd_why = "the persistent decode kernel supports head sizes 64 and 128"; return B200_OK; }
     if (p->nh_l > p->n_sms) { p->pd_why = "more attention heads than SMs"; return B200_OK; }
     if (!gateup_fits(p->hid_l, p->n_sms)) { p->pd_why = "hidden slice per CTA exceeds the epilogue buffer"; return B200_OK; }
@@ -917,7 +895,7 @@ int capture_all(b200_plan *p) {
     TokenGraphs &G = p->graph, &P = p->pers;
     int rc;
     if ((rc = token(G.decode, false, true, false)) || (rc = token(G.prefill, false, false, false))) return rc;
-    if (p->use_stream || p->use_f16_stream) {
+    if (p->wtype == B200_GGML_Q8_0 || p->use_f16_stream) {
         if ((rc = dalloc(p, &p->trace_rec, (size_t)(G.decode.launches + 8) * 32)) || (rc = token(G.trace, false, true, true))) return rc;
     }
     if ((rc = pd_prepare(p))) return rc;
@@ -1089,7 +1067,6 @@ const char *multi_why(const b200_plan *p) {
     if (p->is_moe) return "multi-position steps have no Qwen2-MoE layer (MoE plans run one position per step)";
     if (p->cfg.tp_size > 1) return "multi-position steps run on single-GPU plans only (this plan is tensor-parallel)";
     if (p->wtype != B200_GGML_Q8_0) return "multi-position steps need Q8_0 weights (FP16 plans run one position per step)";
-    if (!p->use_stream) return "multi-position steps need the Q8_0 streaming layout (this plan uses the non-streaming matvecs)";
     if (!batch_max_rows(p)) return "no row count of the batched Q8_0 stream fits this plan's shapes";
     return nullptr;
 }
@@ -1155,10 +1132,8 @@ int set_smem_attrs(b200_plan *p) {
     size_t need_att = att_smem_bytes(c.head_size, c.context_length, p->att_scratch != nullptr);
     int maxcols = c.hidden_dim > c.dim ? c.hidden_dim : c.dim;
     if (p->qd > maxcols) maxcols = p->qd;
-    size_t need_mv = q8_smem_bytes(maxcols, 4, 8);
     size_t need_f16 = f16_smem_bytes(maxcols, p->cfg.fp16_lanes);
-    if (need_norm > (size_t)maxdyn || need_att > (size_t)maxdyn || (p->wtype == B200_GGML_Q8_0 && need_mv > (size_t)maxdyn) ||
-        (p->wtype == B200_GGML_F16 && need_f16 > (size_t)maxdyn))
+    if (need_norm > (size_t)maxdyn || need_att > (size_t)maxdyn || (p->wtype == B200_GGML_F16 && need_f16 > (size_t)maxdyn))
         return fail(p, B200_ERR_UNSUPPORTED, "shape needs more shared memory than the device offers (%d bytes)", maxdyn);
     static bool done = false; // process-wide, like the attribute itself (plans are created from one thread at a time per process)
     if (done) return B200_OK;
@@ -1173,13 +1148,6 @@ int set_smem_attrs(b200_plan *p) {
         });
         if (rc) return rc;
     }
-    CK(set_max_dyn(k_matvec_q8<1, MODE_STORE>, maxdyn));
-    CK(set_max_dyn(k_matvec_q8<2, MODE_STORE>, maxdyn));
-    CK(set_max_dyn(k_matvec_q8<4, MODE_STORE>, maxdyn));
-    CK(set_max_dyn(k_matvec_q8<1, MODE_RESID>, maxdyn));
-    CK(set_max_dyn(k_matvec_q8<2, MODE_RESID>, maxdyn));
-    CK(set_max_dyn(k_matvec_q8<4, MODE_RESID>, maxdyn));
-    CK(set_max_dyn(k_gateup_q8, maxdyn));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
@@ -1377,14 +1345,21 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     CK(cudaEventCreate(&p->ev1));
     int rc;
     CK(cudaDeviceGetAttribute(&p->n_sms, cudaDevAttrMultiProcessorCount, p->device));
+    const bool q8 = p->wtype == B200_GGML_Q8_0; // every Q8_0 weight matrix is a tile-major stream (stream_matvec.cuh)
     {
-        const char *e = getenv("B200_STREAM");
-        bool want = !(e && e[0] == '0');
-        p->use_stream = want && p->wtype == B200_GGML_Q8_0 && stream_shape_ok(p->qd_l + 2 * p->kvd_l, c.dim) && stream_shape_ok(p->dim_l, p->qd) &&
-                        (p->is_moe || (stream_shape_ok(2 * p->hid_l, c.dim) && stream_shape_ok(p->dim_l, c.hidden_dim))) && stream_shape_ok((p->voc_l + 3) & ~3, c.dim) &&
-                        gateup_fits(p->hid_l, p->n_sms);
-        const char *e3 = getenv("B200_F16_STREAM"); // FP16 plans: 0 = the round-1 k_matvec_f16 launches
-        p->use_f16_stream = !(e3 && e3[0] == '0') && p->wtype == B200_GGML_F16 && c.tp_size == 1 && sf_layout(p->qd + 2 * p->kvd, c.dim, c.fp16_lanes, false).ok &&
+        if (c.tp_size > 1 && !q8) return fail(p, B200_ERR_UNSUPPORTED, "tensor parallelism needs Q8_0 weights");
+        if (q8) {
+            const struct { const char *name; int rows, cols; } mats[5] = {
+                {"attn_qkv", p->qd_l + 2 * p->kvd_l, c.dim}, {"attn_output", p->dim_l, p->qd}, {"output", (p->voc_l + 3) & ~3, c.dim},
+                {"ffn_gate/ffn_up", 2 * p->hid_l, c.dim}, {"ffn_down", p->dim_l, c.hidden_dim}}; // the MoE FFN has its own streams (below)
+            for (int i = 0; i < (p->is_moe ? 3 : 5); i++)
+                if (!stream_shape_ok(mats[i].rows, mats[i].cols))
+                    return fail(p, B200_ERR_UNSUPPORTED, "Q8_0 matrix %s is %d columns wide: too wide for 3 ring stages of the weight stream", mats[i].name, mats[i].cols);
+            if (!gateup_fits(p->hid_l, p->n_sms))
+                return fail(p, B200_ERR_UNSUPPORTED, "Q8_0 matrix ffn_gate/ffn_up: hidden dim %d puts more hidden units on one CTA than the stream's epilogue buffer holds (%d)",
+                            c.hidden_dim, SMV_HVALS);
+        }
+        p->use_f16_stream = p->wtype == B200_GGML_F16 && c.tp_size == 1 && sf_layout(p->qd + 2 * p->kvd, c.dim, c.fp16_lanes, false).ok &&
                             sf_layout(c.dim, p->qd, c.fp16_lanes, false).ok && sf_layout(c.hidden_dim, c.dim, c.fp16_lanes, true).ok &&
                             sf_layout(c.dim, c.hidden_dim, c.fp16_lanes, false).ok && sf_layout(c.vocab_size, c.dim, c.fp16_lanes, false).ok;
         if (p->is_moe) { // the MoE FFN has its own streams (the dense FFN checks above are skipped)
@@ -1395,16 +1370,14 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
             if (!cut) return fail(p, B200_ERR_UNSUPPORTED, "expert hidden %d / shared hidden %d at dim %d: the Q8_0 stream layout cannot cut these matrices", he, hs, c.dim);
             p->moe_dl = moe_down_layout(p->moe_hv, hs / smv_pick_nseg(hs), he / smv_pick_nseg(he), SMV_SMEM_BUDGET_MAX);
             if (p->moe_dl.stages < 3) return fail(p, B200_ERR_UNSUPPORTED, "the expert down projection leaves fewer than 3 ring stages of shared memory");
-            if (!p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "Qwen2-MoE needs the Q8_0 streaming layout (this plan would use the non-streaming matvecs)");
         }
-        p->use_pdl = p->use_stream || p->use_f16_stream;
+        p->use_pdl = q8 || p->use_f16_stream;
         // Tensor parallelism keeps the separate norm: its read of x waits on every rank's slice (TP_SLOT_X).  So does Qwen2-MoE,
         // whose FFN norm must write float xb for the F32 router anyway; its plans keep 8 launches per layer.
-        p->fuse_norm = p->use_stream && c.tp_size == 1 && !p->is_moe && norm_fusion_ok(c.dim);
-        if (c.tp_size > 1 && !p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "tensor parallelism needs the Q8_0 streaming path");
+        p->fuse_norm = q8 && c.tp_size == 1 && !p->is_moe && norm_fusion_ok(c.dim);
     }
     size_t stage_bytes = (size_t)34 * (8u << 20); // 8 Mi blocks = 272 MiB
-    if (p->use_stream) {
+    if (q8) {
         size_t m1 = (size_t)c.vocab_size * c.dim, m2 = (size_t)2 * c.hidden_dim * c.dim, m3 = (size_t)(p->qd + 2 * p->kvd) * c.dim;
         size_t mx = m1 > m2 ? m1 : m2;
         if (m3 > mx) mx = m3;
@@ -1426,32 +1399,23 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     if ((rc = alloc_matrix(p, p->emb, c.vocab_size, c.dim, eff_type(emb->ggml_type)))) return rc;
     if ((rc = upload_matrix(p, emb, c.vocab_size, c.dim, p->emb, 0))) return rc;
     const b200_tensor *outw = find(tensors, n_tensors, "output.weight");
-    if (p->use_stream) {
-        if (!outw && eff_type(emb->ggml_type) != p->wtype) return fail(p, B200_ERR_UNSUPPORTED, "tied output weight type differs from the matrix type");
-        {
-            const int r0[3] = {c.tp_rank * p->voc_l, 0, 0}, fu[3] = {c.vocab_size, 0, 0};
-            if ((rc = upload_tiles(p, outw ? outw : emb, nullptr, nullptr, p->voc_l, 0, 0, c.dim, false, p->tout, r0, fu))) return rc;
-        }
+    if (!outw && eff_type(emb->ggml_type) != p->wtype) return fail(p, B200_ERR_UNSUPPORTED, "tied output weight type differs from the matrix type");
+    if (q8) {
+        const int r0[3] = {c.tp_rank * p->voc_l, 0, 0}, fu[3] = {c.vocab_size, 0, 0};
+        if ((rc = upload_tiles(p, outw ? outw : emb, nullptr, nullptr, p->voc_l, 0, 0, c.dim, false, p->tout, r0, fu))) return rc;
         p->out = p->emb;
         if ((rc = dalloc(p, &p->part_val, (size_t)p->n_sms * 4))) return rc;
         if ((rc = dalloc(p, &p->part_idx, (size_t)p->n_sms * 4))) return rc;
         const int hid = c.hidden_dim > p->moe_hv ? c.hidden_dim : p->moe_hv;
         if ((rc = dalloc(p, &p->blk_cnt, (size_t)(hid / 32) * 4))) return rc;
         CK(cudaMemset(p->blk_cnt, 0, (size_t)(hid / 32) * 4));
-    } else if (outw) {
+    } else {
         if (p->use_f16_stream) { // per-CTA argmax partials of the classifier launch (at most 3 CTAs per SM)
             if ((rc = dalloc(p, &p->part_val, (size_t)p->n_sms * 4 * 4))) return rc;
             if ((rc = dalloc(p, &p->part_idx, (size_t)p->n_sms * 4 * 4))) return rc;
         }
-        if ((rc = alloc_matrix(p, p->out, c.vocab_size, c.dim, p->wtype))) return rc;
-        if ((rc = upload_matrix(p, outw, c.vocab_size, c.dim, p->out, 0))) return rc;
-    } else {
-        if (eff_type(emb->ggml_type) != p->wtype) return fail(p, B200_ERR_UNSUPPORTED, "tied output weight type differs from the matrix type");
-        p->out = p->emb;
-        if (p->use_f16_stream) {
-            if ((rc = dalloc(p, &p->part_val, (size_t)p->n_sms * 4 * 4))) return rc;
-            if ((rc = dalloc(p, &p->part_idx, (size_t)p->n_sms * 4 * 4))) return rc;
-        }
+        if (!outw) p->out = p->emb;
+        else if ((rc = alloc_matrix(p, p->out, c.vocab_size, c.dim, p->wtype)) || (rc = upload_matrix(p, outw, c.vocab_size, c.dim, p->out, 0))) return rc;
     }
     if ((rc = upload_f32(p, find(tensors, n_tensors, "output_norm.weight"), c.dim, &p->out_norm, "output_norm.weight"))) return rc;
 
@@ -1475,7 +1439,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         const b200_tensor *tg = T(phi3 ? "ffn_up.weight" : "ffn_gate.weight"), *tu = T("ffn_up.weight");
         const int q_full = phi3 ? p->qd + 2 * p->kvd : p->qd, k_full = phi3 ? q_full : p->kvd, g_full = phi3 ? 2 * c.hidden_dim : c.hidden_dim;
         const int k_src = phi3 ? p->qd : 0, v_src = phi3 ? p->qd + p->kvd : 0, u_src = phi3 ? c.hidden_dim : 0;
-        if (p->use_stream) {
+        if (q8) {
             const int rk = c.tp_rank;
             const int qr0[3] = {rk * p->qd_l, k_src + rk * p->kvd_l, v_src + rk * p->kvd_l}, qfu[3] = {q_full, k_full, k_full};
             if ((rc = upload_tiles(p, tq, tk, tv, p->qd_l, p->kvd_l, p->kvd_l, c.dim, false, L.tqkv, qr0, qfu))) return rc;
@@ -1490,7 +1454,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
             if ((rc = upload_tiles(p, T("ffn_down.weight"), nullptr, nullptr, p->dim_l, 0, 0, c.hidden_dim, false, L.tw2, dr0, dfu))) return rc;
             continue;
         }
-        // fused [Wq; Wk; Wv] so one launch produces the packed q|k|v vector
+        // FP16: row-major matrices, fused [Wq; Wk; Wv] so one launch produces the packed q|k|v vector
         if ((rc = alloc_matrix(p, L.qkv, p->qd + 2 * p->kvd, c.dim, p->wtype))) return rc;
         if ((rc = upload_matrix(p, tq, p->qd, c.dim, L.qkv, 0, 0, q_full))) return rc;
         if ((rc = upload_matrix(p, tk, p->kvd, c.dim, L.qkv, p->qd, k_src, k_full))) return rc;
@@ -1686,8 +1650,7 @@ int prefill_init(b200_plan *p) {
     if (c.mode == B200_PREFILL_TENSOR_CORE) c.mode = B200_PREFILL_EXACT;
     const int nqkv = p->qd + 2 * p->kvd;
     if (p->wtype != B200_GGML_F16 && !p->f16_copies) {
-        c.why = p->use_stream ? "Q8_0 plan: the tensor-core prefill is opt-in (b200_set_prefill_mode builds f16 twins of the weight matrices, +2 bytes per weight)"
-                              : "tensor-core prefill needs FP16 weight matrices or a Q8_0 plan on the streaming path";
+        c.why = "Q8_0 plan: the tensor-core prefill is opt-in (b200_set_prefill_mode builds f16 twins of the weight matrices, +2 bytes per weight)";
         return B200_OK;
     }
     if ((c.why = prefill_shape_why(p))) return B200_OK;
@@ -1718,7 +1681,6 @@ int prefill_init_q8(b200_plan *p) {
     if (p->prefill_batch <= 1) { c.why_q8 = "the plan was created without a prefill batch size (prefill_batch_size <= 1)"; return B200_OK; }
     if (p->wtype != B200_GGML_Q8_0) { c.why_q8 = "W8A16 prefill needs a Q8_0 plan (FP16 plans run the tensor-core prefill on their own f16 matrices)"; return B200_OK; }
     if (g.tp_size > 1) { c.why_q8 = "tensor-core prefill is single-GPU"; return B200_OK; }
-    if (!p->use_stream) { c.why_q8 = "W8A16 prefill reads the tile-major Q8_0 streams: the plan must use the streaming layout"; return B200_OK; }
     if ((c.why_q8 = prefill_shape_why(p))) return B200_OK;
     for (int l = 0; l < g.n_layers; l++) {
         const LayerW &L = p->layers[l];
@@ -1749,7 +1711,7 @@ int prefill_init_q8(b200_plan *p) {
 int build_f16_twins(b200_plan *p) {
     const b200_config &c = p->cfg;
     if (p->f16_copies) return B200_OK;
-    if (p->wtype != B200_GGML_Q8_0 || !p->use_stream || c.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "f16 twins need a single-GPU Q8_0 plan on the streaming path");
+    if (p->wtype != B200_GGML_Q8_0 || c.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "f16 twins need a single-GPU Q8_0 plan");
     for (int l = 0; l < c.n_layers; l++) {
         LayerW &L = p->layers[l];
         int rc;
@@ -2209,7 +2171,7 @@ int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
         p->prefill.mode = mode;
         return B200_OK;
     }
-    if (mode == B200_PREFILL_TENSOR_CORE && !p->prefill.ready && p->prefill_batch > 1 && p->wtype == B200_GGML_Q8_0 && p->use_stream && p->cfg.tp_size == 1) {
+    if (mode == B200_PREFILL_TENSOR_CORE && !p->prefill.ready && p->prefill_batch > 1 && p->wtype == B200_GGML_Q8_0 && p->cfg.tp_size == 1) {
         CK(cudaSetDevice(p->device)); // opt-in on a Q8_0 plan: build the f16 twins, then the GEMM context
         int rc = build_f16_twins(p);
         if (rc) return rc;
@@ -2247,7 +2209,6 @@ int b200_set_decode_slots(b200_plan *p, int32_t n_slots) {
     if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "batched decode has no Qwen2-MoE layer (MoE plans decode one sequence per step)");
     if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "batched decode runs on single-GPU plans only (this plan is tensor-parallel)");
     if (p->wtype != B200_GGML_Q8_0) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs Q8_0 weights (FP16 plans decode one sequence per step)");
-    if (!p->use_stream) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs the Q8_0 streaming layout (this plan uses the non-streaming matvecs)");
     const int mx = batch_max_rows(p);
     if (n_slots > mx) return fail(p, B200_ERR_UNSUPPORTED, "at most %d decode slots on this plan (asked for %d)", mx, n_slots);
     batch_free(p);
@@ -2565,10 +2526,7 @@ int b200_time_kernel(b200_plan *p, int32_t which, int32_t reps, float *avg_ms, i
     const b200_config &c = p->cfg;
     const bool q8 = p->wtype == B200_GGML_Q8_0, sf = p->use_f16_stream, fz = p->fuse_norm;
     auto tb = [&](const TileMat &m) -> int64_t { return (int64_t)m.rows * m.cols / 32 * 34; };
-    auto mat_bytes = [&](const DevMat &m) -> int64_t {
-        int64_t e = (int64_t)m.rows * m.cols;
-        return q8 ? e / 32 * 34 : e * 2;
-    };
+    auto mat_bytes = [&](const DevMat &m) -> int64_t { return (int64_t)m.rows * m.cols * 2; }; // FP16
     const int64_t nw = fz ? (int64_t)c.dim * 4 : 0; // a fused norm also reads its weights (x: an L2 hit)
     const TraceBuf none{nullptr, 0, 0};
     int64_t bytes = 0;
@@ -2599,33 +2557,28 @@ int b200_time_kernel(b200_plan *p, int32_t which, int32_t reps, float *avg_ms, i
         default: bytes = mat_bytes(p->out); return launch_stream_f16<SF_STORE>(p, p->out, nullptr, p->xb, p->logits);
         }
     };
-    auto matvec = [&](LayerW &L) -> int { // the non-streaming kernels
+    auto matvec = [&](LayerW &L) -> int { // the FP16 fallback kernels
         switch (which) {
-        case 0:
-            if (q8) {
-                k_gateup_q8<<<c.hidden_dim / 32, 256, q8_smem_bytes(c.dim, 4, 8), p->stream>>>(
-                    (const int8_t *)L.w1.qs, L.w1.sc, (const int8_t *)L.w3.qs, L.w3.sc, p->xq, p->xs, c.hidden_dim, c.dim, p->hq, p->hs, p->hb);
-                CK(cudaGetLastError());
-            } else {
-                int rc;
-                if ((rc = launch_matvec_f16<MODE_STORE>(p, L.w1, p->xb, p->hb))) return rc;
-                if ((rc = launch_matvec_f16<MODE_STORE>(p, L.w3, p->xb, p->hb2))) return rc;
-            }
+        case 0: {
+            int rc;
+            if ((rc = launch_matvec_f16<MODE_STORE>(p, L.w1, p->xb, p->hb))) return rc;
+            if ((rc = launch_matvec_f16<MODE_STORE>(p, L.w3, p->xb, p->hb2))) return rc;
             bytes = mat_bytes(L.w1) + mat_bytes(L.w3);
             return B200_OK;
-        case 1: bytes = mat_bytes(L.w2); return q8 ? launch_matvec_q8<MODE_RESID>(p, L.w2, p->hq, p->hs, p->x) : launch_matvec_f16<MODE_RESID>(p, L.w2, p->hb, p->x);
-        case 2: bytes = mat_bytes(L.qkv); return q8 ? launch_matvec_q8<MODE_STORE>(p, L.qkv, p->xq, p->xs, p->qkv) : launch_matvec_f16<MODE_STORE>(p, L.qkv, p->xb, p->qkv);
-        case 3: bytes = mat_bytes(L.wo); return q8 ? launch_matvec_q8<MODE_RESID>(p, L.wo, p->xq, p->xs, p->x) : launch_matvec_f16<MODE_RESID>(p, L.wo, p->xb, p->x);
-        default: bytes = mat_bytes(p->out); return q8 ? launch_matvec_q8<MODE_STORE>(p, p->out, p->xq, p->xs, p->logits) : launch_matvec_f16<MODE_STORE>(p, p->out, p->xb, p->logits);
+        }
+        case 1: bytes = mat_bytes(L.w2); return launch_matvec_f16<MODE_RESID>(p, L.w2, p->hb, p->x);
+        case 2: bytes = mat_bytes(L.qkv); return launch_matvec_f16<MODE_STORE>(p, L.qkv, p->xb, p->qkv);
+        case 3: bytes = mat_bytes(L.wo); return launch_matvec_f16<MODE_RESID>(p, L.wo, p->xb, p->x);
+        default: bytes = mat_bytes(p->out); return launch_matvec_f16<MODE_STORE>(p, p->out, p->xb, p->logits);
         }
     };
     // one launch on layer l's matrix; the streaming kernels run stand-alone (no PDL overlap)
     auto one = [&](int l) -> int {
         LayerW &L = p->layers[l];
-        if (!p->use_stream && !sf) return matvec(L);
+        if (!q8 && !sf) return matvec(L);
         const bool keep = p->use_pdl;
         p->use_pdl = false;
-        const int r = p->use_stream ? stream(L) : f16_stream(L);
+        const int r = q8 ? stream(L) : f16_stream(L);
         p->use_pdl = keep;
         return r;
     };

@@ -37,8 +37,10 @@ struct TileMat { // device weight matrix in tile-major layout
     int unit_bytes;  // seg + seg/16 rounded up to 16
 };
 
+// The fewest segments of at most 2560 columns, each a multiple of 32: any width that is a multiple of 32 has one (at worst
+// 32-column segments).  0: the width is not a multiple of 32.
 __host__ __device__ inline int smv_pick_nseg(int cols) {
-    for (int n = 1; n <= 64; n++)
+    for (int n = 1; n <= cols / 32; n++)
         if (cols % n == 0 && (cols / n) % 32 == 0 && cols / n <= 2560) return n;
     return 0;
 }

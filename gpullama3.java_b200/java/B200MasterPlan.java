@@ -281,7 +281,7 @@ public final class B200MasterPlan implements AutoCloseable {
         if (rc != 0) check(rc, lastError());
     }
 
-    /** Up to 8 KV-cache slots (one State per conversation) for forwardDecodeBatch; 0 frees them.  Q8_0 streaming plans only. */
+    /** Up to 8 KV-cache slots (one State per conversation) for forwardDecodeBatch; 0 frees them.  Q8_0 plans only. */
     public void setDecodeSlots(int nSlots) throws Throwable {
         int rc = (int) SET_DECODE_SLOTS.invokeExact(plan, nSlots);
         if (rc != 0) check(rc, lastError());

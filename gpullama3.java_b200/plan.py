@@ -162,7 +162,7 @@ class B200MasterPlan:
         return self._native.time_kernel(which, reps)
 
     # Batched decode (csrc/decode_batch.cuh): up to 8 independent sequences per step, each on its own KV-cache slot, every weight
-    # matrix streamed once per step; each row bit-identical to forward_decode of the same token stream.  Q8_0 streaming plans only.
+    # matrix streamed once per step; each row bit-identical to forward_decode of the same token stream.  Q8_0 plans only.
     def set_decode_slots(self, n_slots: int):
         """Allocate n_slots zeroed KV-cache slots (0 frees them); UnsupportedOperation beyond what the plan can run."""
         self._native.set_decode_slots(n_slots)
@@ -193,7 +193,7 @@ class B200MasterPlan:
         """Run tokens[i] at position start_pos + i of ONE sequence in one step (slot >= 0: a decode slot; -1: the plan's own cache)
         -> (ids, logits [n, vocab] or None); ids[i] is the greedy id after position start_pos + i.  Every row is bit-identical to
         forward_decode of the same token at the same position over the same cache prefix: the verification step of draft-and-verify
-        decoding.  1 <= len(tokens) <= decode_multi_rows(); Q8_0 streaming single-GPU plans without MoE only."""
+        decoding.  1 <= len(tokens) <= decode_multi_rows(); single-GPU Q8_0 plans without MoE only."""
         return self._native.forward_decode_multi(slot, tokens, start_pos, logits)
 
     def decode_multi_rows(self) -> int:

@@ -150,8 +150,8 @@ int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t
  * products (sequential, no FMA), softmax, top-k by first strict maximum with the probabilities as weights (no renormalisation), the k
  * routed experts' SwiGLU FFNs added to x in selection order (x[i] = w * y[i] + x[i]), then the shared expert with weight
  * 1 / (1 + exp(-g)).  B200_ERR_BAD_ARG: a missing tensor, wrong dims, n_experts_used outside 1..min(E, 8).  B200_ERR_UNSUPPORTED
- * (reason in the message): a router or shared gate that is not F32, FP16 weights, tp_size > 1, the non-streaming Q8_0 layout,
- * hidden sizes the stream layout cannot cut.  The plan decodes through the CUDA graph (not the persistent kernel), prefills through
+ * (reason in the message): a router or shared gate that is not F32, FP16 weights, tp_size > 1, hidden sizes the stream layout
+ * cannot cut.  The plan decodes through the CUDA graph (not the persistent kernel), prefills through
  * the exact path only, and refuses b200_set_decode_slots (n_slots > 0) and b200_time_kernel with B200_ERR_UNSUPPORTED. */
 int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors,
                          int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
@@ -206,7 +206,7 @@ int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n
 /* How b200_forward_batch_prefill computes (the reference has the same two families:
  * LlamaFP16LayersBatchPrefill vs ...BatchPrefillMMA, selected by TensorCoreSupport.java):
  *   B200_PREFILL_EXACT       multi-position steps, then the single-token prefill graph for the chunk's last token (the
- *                            graph per token on FP16, tensor-parallel, MoE and non-streaming plans): KV cache
+ *                            graph per token on FP16, tensor-parallel and MoE plans): KV cache
  *                            bit-identical to the CPU path;
  *   B200_PREFILL_TENSOR_CORE TMA + wgmma GEMMs over the whole chunk, FP16 operands / FP32 accumulation:
  *                            KV cache within FP16 tolerance of the CPU path.  Default for FP16 plans created
@@ -215,8 +215,8 @@ int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n
  *                            there the CPU path additionally rounds activations to int8, so agreement is
  *                            percent-level, not FP16-level -- hence not the default.  Returns
  *                            B200_ERR_UNSUPPORTED with the reason in b200_last_error when unavailable.
- *   B200_PREFILL_TENSOR_CORE_W8A16  the same batched prefill on a single-GPU Q8_0 plan (K-quant plans included) on the
- *                            streaming layout, with the GEMMs' B operand dequantised to f16(q * scale) in shared memory
+ *   B200_PREFILL_TENSOR_CORE_W8A16  the same batched prefill on a single-GPU Q8_0 plan (K-quant plans included), with the
+ *                            GEMMs' B operand dequantised to f16(q * scale) in shared memory
  *                            from the tile-major Q8_0 stream the decode kernels read: no f16 twins, 1.06 instead of
  *                            2 bytes per weight streamed.  Bit-identical to B200_PREFILL_TENSOR_CORE except where a
  *                            residual GEMM splits K (the order of the f32 reduce-adds is not fixed in either mode).
@@ -238,7 +238,7 @@ int b200_prefill_info(b200_plan *plan, int32_t *mode, int32_t *launches, float *
  *                           every plan can run it; DESIGN.md section 6 has both measured);
  *   B200_DECODE_PERSISTENT  ONE persistent kernel per token (csrc/decode_persistent.cuh): one CTA per SM streams the
  *                           weights of every matrix through a shared-memory ring while epoch counters order the phases.
- *                           Available when the plan fits (Q8_0 streaming layout, head size 64/128); the environment
+ *                           Available when the plan fits (Q8_0 weights, head size 64/128); the environment
  *                           variable B200_DECODE=persistent selects it at creation.
  * Returns B200_ERR_UNSUPPORTED with the reason in b200_last_error when the plan cannot run the requested mode.
  * Under tensor parallelism every rank must switch at the same point of the call sequence. */
@@ -267,8 +267,8 @@ int b200_kv_reset(b200_plan *plan);
 /* ---- batched decode: up to B200_MAX_DECODE_SLOTS independent sequences per step ---------------------------------------------
  * One step streams every weight matrix from HBM once for all its rows (csrc/decode_batch.cuh); every dot product keeps its own
  * row, activation vector and block order, so each row is bit-identical to b200_forward_decode of the same token stream.  Single-GPU
- * Q8_0 plans on the streaming layout only (K-quant files included; every architecture and head size); FP16 plans, the
- * non-streaming Q8_0 layout and tensor-parallel plans get B200_ERR_UNSUPPORTED.  Batched steps always run as a multi-kernel CUDA
+ * Q8_0 plans only (K-quant files included; every architecture and head size); FP16 plans and tensor-parallel plans get
+ * B200_ERR_UNSUPPORTED.  Batched steps always run as a multi-kernel CUDA
  * graph with programmatic-dependent-launch edges, whatever b200_set_decode_mode selected; the plan's own KV cache, step state and
  * graphs are not touched, so single-sequence calls can be interleaved with batched ones. */
 #define B200_MAX_DECODE_SLOTS 8
@@ -319,7 +319,7 @@ int b200_prefill_slots(b200_plan *plan, int32_t n_seqs, const int32_t *slots, co
  * they are read.  Greedy only: the verification step of draft-and-verify (speculative) decoding.  With slot == -1 the plan's
  * single-token buffers and step state are not touched.  B200_ERR_BAD_ARG (naming the row) for n outside 1..b200_decode_multi_rows,
  * a slot out of range, positions outside the KV cache or a bad token; B200_ERR_UNSUPPORTED with the reason on plans that cannot run
- * it (FP16, tensor-parallel, Qwen2-MoE, the non-streaming Q8_0 layout).  The per-row buffers are allocated on first use. */
+ * it (FP16, tensor-parallel, Qwen2-MoE).  The per-row buffers are allocated on first use. */
 int b200_forward_decode_multi(b200_plan *plan, int32_t slot, int32_t n, const int32_t *tokens, int32_t start_pos, int32_t *ids_out,
                               float *logits /* nullable, n x vocab */);
 

@@ -55,11 +55,6 @@ def test_devstral_decode_bit_exact(pkg, orc, make_model, shape, quant, mode, lan
     _decode_vs_oracle(pkg, orc, m, 10, mode, lanes)
 
 
-def test_devstral_without_the_q8_stream_bit_exact(pkg, orc, make_model, monkeypatch):
-    monkeypatch.setenv("B200_STREAM", "0")
-    _decode_vs_oracle(pkg, orc, make_model("tiny-devstral", pkg.gguf.GGMLType.Q8_0, 24), 10)
-
-
 @pytest.mark.parametrize("shape", ["tiny-devstral", "tiny-devstral-plain", "mid-devstral-2"])
 def test_devstral_rope_table_bit_equal(pkg, make_model, shape):
     """The device's rope_cr / rope_ci against the oracle's independent restatement of precomputeFreqsCisYaRN / precomputeFreqsCis."""

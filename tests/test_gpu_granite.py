@@ -55,11 +55,6 @@ def test_granite_decode_bit_exact(pkg, orc, make_model, shape, quant, mode, lane
     _decode_vs_oracle(pkg, orc, m, 12, mode, lanes)
 
 
-def test_granite_without_the_q8_stream_bit_exact(pkg, orc, make_model, monkeypatch):
-    monkeypatch.setenv("B200_STREAM", "0")
-    _decode_vs_oracle(pkg, orc, make_model("tiny-granite", pkg.gguf.GGMLType.Q8_0, 24), 12)
-
-
 @pytest.mark.parametrize("shape", ["mid-granite-3-2b", "mid-granite-3-8b"])
 @pytest.mark.parametrize("quant,mode", [("Q8_0", "graph"), ("Q8_0", "persistent"), ("F16", "graph")])
 def test_granite_mid_geometries_bit_exact(pkg, orc, shape, quant, mode):
@@ -250,8 +245,8 @@ def test_granite_generate_tokens_stops(pkg, orc, make_model):
 # ---- vocabularies that are not a multiple of 4 --------------------------------------------------------------------------------
 
 def test_odd_vocab_llama_streams_its_classifier(pkg, orc, make_model):
-    """A Llama plan with vocabulary 509 runs the streaming layout: the persistent kernel and decode slots, which the non-streaming
-    layout refuses, are available; its logits stay bit-equal in both decode modes."""
+    """A Llama plan with vocabulary 509 streams its classifier in a zero-padded last group: the persistent kernel and decode slots
+    are available; its logits stay bit-equal in both decode modes."""
     m = make_model("tiny-llama-vocab509", pkg.gguf.GGMLType.Q8_0, 24)
     plan = pkg.B200MasterPlan.initialize_plan(m)
     try:

@@ -3,8 +3,6 @@
 The exact prefill (forward_batch_prefill, prefill_slots) and forward_decode_multi run rows that share a sequence through
 k_rope_kv_batch + k_attention_cached_rows, so every row's K/V is written before any row attends.  Every K/V byte, logit and id is
 held bit-equal (uint32) to the token-by-token path and to the CPU restatement."""
-import os
-
 import numpy as np
 import pytest
 
@@ -211,16 +209,6 @@ def test_forward_decode_multi_refusals(pkg, orc, make_model):
         assert np.isfinite(fp16.forward_decode(1, 0)[0]).all()
     finally:
         fp16.free()
-    os.environ["B200_STREAM"] = "0"
-    try:
-        ns = pkg.B200MasterPlan.initialize_plan(m)
-    finally:
-        del os.environ["B200_STREAM"]
-    try:
-        _expect(pkg, lambda: ns.forward_decode_multi(-1, [1, 2], 0), -2, "streaming layout")
-        assert np.isfinite(ns.forward_decode(1, 0)[0]).all()
-    finally:
-        ns.free()
 
 
 def test_forward_decode_multi_refuses_moe(pkg, make_model):

@@ -113,13 +113,6 @@ def test_decode_phi3_mini_geometry(pkg, orc, quant):
     run_stream(pkg, orc, m, 16, 4, check_kv=True)
 
 
-def test_decode_f16_round1_kernels_still_exact(pkg, orc, make_model, monkeypatch):
-    """B200_F16_STREAM=0 keeps the round-1 launches (k_matvec_f16 + separate SwiGLU), the fallback for shapes the rings do not fit."""
-    monkeypatch.setenv("B200_F16_STREAM", "0")
-    m = make_model("tiny-llama", pkg.gguf.GGMLType.F16, 24)
-    run_stream(pkg, orc, m, 16, 8)
-
-
 @pytest.mark.parametrize("mode", MODES)
 def test_decode_small_llama_q8(pkg, orc, make_model, mode):
     """dim 1536 (not a multiple of 512: exercises the column tail), 12 heads / 4 KV heads, 3 layers."""

@@ -255,12 +255,6 @@ def test_qwen2moe_refusals(pkg, orc, make_model):
     # FP16 weights
     mf = pkg.loader.model_from_tensors(sh, G.F16, pkg.synth.build_tensors_fast(sh, G.F16), 64)
     _expect(pkg, lambda: N.NativePlan(pkg.plan.make_config(mf), mf.tensors, 0, 0, moe=moe), -2, "Q8_0 only")
-    # the non-streaming Q8_0 layout
-    os.environ["B200_STREAM"] = "0"
-    try:
-        _expect(pkg, lambda: create(), -2, "streaming layout")
-    finally:
-        del os.environ["B200_STREAM"]
     # on a working plan: tensor-core prefill, persistent decode, decode slots, the kernel timer
     plan = pkg.B200MasterPlan.initialize_plan(m, prefill_batch_size=64)
     try:

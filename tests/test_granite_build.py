@@ -4,7 +4,7 @@ import pytest
 
 from test_batch_decode_build import _entries
 
-CHANGED = [r"k_stream_matvec_q8ILi", r"k_stream_matvec_f16ILi", r"k_matvec_q8ILi", r"k_matvec_f16ILi", r"k_rmsnorm_quantILb",
+CHANGED = [r"k_stream_matvec_q8ILi", r"k_stream_matvec_f16ILi", r"k_matvec_f16ILi", r"k_rmsnorm_quantILb",
            r"k_attentionILi(64|128)E", r"k_stream_matvec_q8_batch", r"k_rmsnorm_quant_batch", r"k_pf_embed", r"k_gemm_f16_wgmma"]
 
 

@@ -52,6 +52,7 @@ struct TokenGraphs {
 
 // The forms of the batched step (enqueue_batch).  PREFILL*: a step of the exact prefills, its rows from the call's schedule and
 // without the classifier.  *_SPLIT, *_OWN and MULTI*: rows may share a sequence.  *_OWN: the K / V target is the plan's own cache.
+// b200_forward_step runs DECODE (distinct slots) and MULTI (a slot repeats) with the classifier over its first e rows only.
 enum BatchKind { BK_DECODE, BK_PREFILL, BK_PREFILL_SPLIT, BK_PREFILL_OWN, BK_MULTI, BK_MULTI_OWN, BK_KINDS };
 
 } // namespace
@@ -181,8 +182,9 @@ struct b200_plan {
         // the exact prefills: the per-step rows of the call [context_length], the device step index
         BatchRows *sched = nullptr;
         int *step = nullptr;
-        Graph g[BK_KINDS][SMB_MAX_ROWS + 1];
-        int last_n = 0;
+        int *smp_indices = nullptr; // the sampler's candidate lists, [row][vocab]
+        Graph g[BK_KINDS][SMB_MAX_ROWS + 1][SMB_MAX_ROWS + 1]; // [kind][rows][rows that run the classifier]
+        int last_launches = 0; // of the last b200_forward_decode_batch / b200_forward_step graph
         float last_ms = 0.f;
     } bt;
 };
@@ -943,10 +945,11 @@ int launch_stream_batch(b200_plan *p, const TileMat &W, int n, const int8_t *xq,
 }
 
 // One forward step of n rows: the single-sequence graph's kernel sequence, every launch serving all n rows.  prefill: a step of
-// the exact prefills -- the rows come from the call's schedule (k_batch_rows_next) and there is no final norm, lm_head or argmax.
-// split: rows may share a sequence, so the attention runs as k_rope_kv_batch + k_attention_cached_rows (one more launch per
-// layer).  own: the K / V target is the plan's cache (key_cache / value_cache, slot 0's layout) instead of the decode slots.
-int enqueue_batch(b200_plan *p, int n, BatchKind kind, int *launches) {
+// the exact prefills -- the rows come from the call's schedule (k_batch_rows_next).  The final norm, lm_head and argmax run over
+// the first e rows only (e = 0: not at all, as in the prefill kinds).  split: rows may share a sequence, so the attention runs as
+// k_rope_kv_batch + k_attention_cached_rows (one more launch per layer).  own: the K / V target is the plan's cache (key_cache /
+// value_cache, slot 0's layout) instead of the decode slots.
+int enqueue_batch(b200_plan *p, int n, int e, BatchKind kind, int *launches) {
     const bool prefill = kind == BK_PREFILL || kind == BK_PREFILL_SPLIT || kind == BK_PREFILL_OWN;
     const bool split = kind != BK_DECODE && kind != BK_PREFILL, own = kind == BK_PREFILL_OWN || kind == BK_MULTI_OWN;
     const b200_config &c = p->cfg;
@@ -963,16 +966,16 @@ int enqueue_batch(b200_plan *p, int n, BatchKind kind, int *launches) {
         CK(cudaGetLastError());
         k++;
     }
-    auto norm = [&](bool embed, const float *w) {
+    auto norm = [&](bool embed, const float *w, int rows) {
         auto go = [&](auto kern) { // the first norm of a prefill step waits for k_batch_rows_next in full: the rows are read before any PDL wait
-            return launch_k(p, pdl && !(prefill && embed), kern, dim3(n), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, p->mup.embedding_scale, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
+            return launch_k(p, pdl && !(prefill && embed), kern, dim3(rows), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, p->mup.embedding_scale, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
         };
         k++;
         return embed ? go(k_rmsnorm_quant_batch<true>) : go(k_rmsnorm_quant_batch<false>);
     };
     for (int l = 0; l < c.n_layers; l++) {
         const LayerW &L = p->layers[l];
-        if ((rc = norm(l == 0, L.attn_norm))) return rc;
+        if ((rc = norm(l == 0, L.attn_norm, n))) return rc;
         if ((rc = launch_stream_batch<SMV_STORE>(p, L.tqkv, n, B.xq, B.xs, B.qkv, qkvd))) return rc;
         float *kc = (own ? p->key_cache : B.slot_k) + (size_t)l * ctx_kv, *vc = (own ? p->value_cache : B.slot_v) + (size_t)l * ctx_kv;
         const size_t att_smem = att_smem_bytes(c.head_size, c.context_length, B.att_scratch != nullptr);
@@ -993,27 +996,27 @@ int enqueue_batch(b200_plan *p, int n, BatchKind kind, int *launches) {
         });
         if (rc) return rc;
         if ((rc = launch_stream_batch<SMV_RESID>(p, L.two, n, B.xq, B.xs, B.x, c.dim))) return rc;
-        if ((rc = norm(false, L.ffn_norm))) return rc;
+        if ((rc = norm(false, L.ffn_norm, n))) return rc;
         if ((rc = launch_stream_batch<SMV_GATEUP>(p, L.tgu, n, B.xq, B.xs, B.hb, c.hidden_dim, B.hq, B.hs))) return rc;
         if ((rc = launch_stream_batch<SMV_RESID>(p, L.tw2, n, B.hq, B.hs, B.x, c.dim))) return rc;
         k += 5;
     }
-    if (prefill) {
+    if (!e) {
         if (launches) *launches = k;
         return B200_OK;
     }
-    if ((rc = norm(false, p->out_norm))) return rc;
-    if ((rc = launch_stream_batch<SMV_STORE>(p, p->tout, n, B.xq, B.xs, B.logits, sampler_padded(c.vocab_size), nullptr, nullptr, true))) return rc;
-    if ((rc = launch_k(p, pdl, k_argmax_batch, dim3(n), dim3(32), (size_t)0, (const float *)B.part_val, (const int *)B.part_idx, p->n_sms, B.ids))) return rc;
+    if ((rc = norm(false, p->out_norm, e))) return rc;
+    if ((rc = launch_stream_batch<SMV_STORE>(p, p->tout, e, B.xq, B.xs, B.logits, sampler_padded(c.vocab_size), nullptr, nullptr, true))) return rc;
+    if ((rc = launch_k(p, pdl, k_argmax_batch, dim3(e), dim3(32), (size_t)0, (const float *)B.part_val, (const int *)B.part_idx, p->n_sms, B.ids))) return rc;
     if (launches) *launches = k + 2;
     return B200_OK;
 }
 
-// The step graph of `kind` for n rows, captured on first use.
-int batch_graph(b200_plan *p, BatchKind kind, int n, const Graph **out) {
-    Graph &g = p->bt.g[kind][n];
+// The step graph of `kind` for n rows, e of them with the classifier, captured on first use.
+int batch_graph(b200_plan *p, BatchKind kind, int n, int e, const Graph **out) {
+    Graph &g = p->bt.g[kind][n][e];
     int rc;
-    if (!g.exec && (rc = capture(p, g, [&](int *launches) { return enqueue_batch(p, n, kind, launches); }))) return rc;
+    if (!g.exec && (rc = capture(p, g, [&](int *launches) { return enqueue_batch(p, n, e, kind, launches); }))) return rc;
     *out = &g;
     return B200_OK;
 }
@@ -1021,7 +1024,8 @@ int batch_graph(b200_plan *p, BatchKind kind, int n, const Graph **out) {
 void batch_free(b200_plan *p) {
     auto &B = p->bt;
     for (auto &by_kind : B.g)
-        for (Graph &g : by_kind) destroy(g);
+        for (auto &by_rows : by_kind)
+            for (Graph &g : by_rows) destroy(g);
     for (void *d : B.allocs) cudaFree(d);
     if (B.h_rows) cudaFreeHost(B.h_rows);
     if (B.h_out) cudaFreeHost(B.h_out);
@@ -1050,7 +1054,7 @@ int batch_alloc(b200_plan *p, int ns) {
         (rc = balloc(p, &B.logits, N * sampler_padded(c.vocab_size) * 4)) || (rc = balloc(p, &B.xq, N * big)) || (rc = balloc(p, &B.xs, N * (big / 32) * 4)) ||
         (rc = balloc(p, &B.hq, N * c.hidden_dim)) || (rc = balloc(p, &B.hs, N * (c.hidden_dim / 32) * 4)) ||
         (rc = balloc(p, &B.part_val, N * p->n_sms * 4)) || (rc = balloc(p, &B.part_idx, N * p->n_sms * 4)) || (rc = balloc(p, &B.ids, N * 4)) ||
-        (rc = balloc(p, &B.smp_out, N * 8 * 4)) || (rc = balloc(p, &B.blk_cnt, N * (c.hidden_dim / 32) * 4)) || (rc = balloc(p, &B.rows, sizeof(BatchRows))) ||
+        (rc = balloc(p, &B.smp_out, N * 8 * 4)) || (rc = balloc(p, &B.smp_indices, N * c.vocab_size * 4)) || (rc = balloc(p, &B.blk_cnt, N * (c.hidden_dim / 32) * 4)) || (rc = balloc(p, &B.rows, sizeof(BatchRows))) ||
         (rc = balloc(p, &B.sched, (size_t)c.context_length * sizeof(BatchRows))) || (rc = balloc(p, &B.step, 4)))
         return rc;
     if (p->att_scratch && (rc = balloc(p, &B.att_scratch, N * p->nh_l * c.context_length * 4))) return rc;
@@ -1093,7 +1097,7 @@ int run_steps(b200_plan *p, const std::vector<BatchRows> &sched, const std::vect
             for (int j = 0; j < i; j++)
                 if (sched[s].slot[j] == sched[s].slot[i]) { split = true; break; }
         const BatchKind kind = own ? BK_PREFILL_OWN : split ? BK_PREFILL_SPLIT : BK_PREFILL;
-        if ((rc = batch_graph(p, kind, nrows[s], &graphs[s]))) return rc;
+        if ((rc = batch_graph(p, kind, nrows[s], 0, &graphs[s]))) return rc;
     }
     CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
     CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
@@ -1169,6 +1173,7 @@ int set_smem_attrs(b200_plan *p) {
     CK(cudaFuncSetAttribute(k_moe_gateup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_moe_down, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
+    CK(cudaFuncSetAttribute(k_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     done = true;
     return B200_OK;
 }
@@ -1845,6 +1850,19 @@ int launch_sample(b200_plan *p, float *logits, float temperature, float topp, fl
     return B200_OK;
 }
 
+// The device sampler on the batch's logits rows row[j], j < m, one block per row in one launch: row r's token at
+// bt.smp_out[8 r], its diagnostics after it.
+int launch_sample_rows(b200_plan *p, int m, const int *row, const float *temperature, const float *topp, const float *uniform01) {
+    static_assert(SMB_MAX_ROWS <= SAMPLER_MAX_ROWS, "k_sample_rows takes every row of a batched step");
+    SamplerRowsArgs a;
+    a.logits = p->bt.logits; a.stride = sampler_padded(p->cfg.vocab_size); a.n = p->cfg.vocab_size;
+    a.indices = p->bt.smp_indices; a.out = p->bt.smp_out;
+    for (int j = 0; j < m; j++) { a.row[j] = row[j]; a.temperature[j] = temperature[j]; a.topp[j] = topp[j]; a.r01[j] = uniform01[j]; }
+    k_sample_rows<<<m, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
+    CK(cudaGetLastError());
+    return B200_OK;
+}
+
 // After a synchronize: did a device-side wait of the persistent kernel (or a tensor-parallel flag wait) give up?
 int check_device_error(b200_plan *p) {
     if (p->h_err && *reinterpret_cast<volatile unsigned *>(p->h_err)) {
@@ -2241,7 +2259,7 @@ int b200_forward_decode_batch(b200_plan *p, int32_t n, const int32_t *slots, con
     CK(cudaSetDevice(p->device));
     int rc;
     const Graph *g;
-    if ((rc = batch_graph(p, BK_DECODE, n, &g))) return rc;
+    if ((rc = batch_graph(p, BK_DECODE, n, n, &g))) return rc;
     for (int i = 0; i < n; i++) { B.h_rows->token[i] = tokens[i]; B.h_rows->pos[i] = positions[i]; B.h_rows->slot[i] = slots[i]; }
     CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
     CK(cudaEventRecord(p->ev0, p->stream));
@@ -2250,18 +2268,20 @@ int b200_forward_decode_batch(b200_plan *p, int32_t n, const int32_t *slots, con
     const size_t vpad = (size_t)sampler_padded(c.vocab_size);
     if (logits) // before the sampler turns sampled rows into probabilities
         for (int i = 0; i < n; i++) CK(cudaMemcpyAsync(logits + (size_t)i * c.vocab_size, B.logits + i * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
-    bool any_sampled = false;
+    int m = 0, row[SMB_MAX_ROWS];
+    float t[SMB_MAX_ROWS], tp[SMB_MAX_ROWS], u[SMB_MAX_ROWS];
     for (int i = 0; i < n; i++) {
         if (!sampling || sampling[3 * i] == 0.0f) continue; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed
-        if ((rc = launch_sample(p, B.logits + i * vpad, sampling[3 * i], sampling[3 * i + 1], sampling[3 * i + 2], B.smp_out + 8 * i))) return rc;
-        any_sampled = true;
+        row[m] = i; t[m] = sampling[3 * i]; tp[m] = sampling[3 * i + 1]; u[m] = sampling[3 * i + 2];
+        m++;
     }
+    if (m && (rc = launch_sample_rows(p, m, row, t, tp, u))) return rc;
     CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)n * 4, cudaMemcpyDeviceToHost, p->stream));
-    if (any_sampled) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)n * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
+    if (m) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)n * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
     CK(cudaStreamSynchronize(p->stream));
     for (int i = 0; i < n; i++) ids_out[i] = (sampling && sampling[3 * i] != 0.0f) ? B.h_out[SMB_MAX_ROWS + 8 * i] : B.h_out[i];
     CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
-    B.last_n = n;
+    B.last_launches = g->launches;
     return B200_OK;
 }
 
@@ -2447,7 +2467,7 @@ int b200_forward_decode_multi(b200_plan *p, int32_t slot, int32_t n, const int32
     if ((rc = multi_ready(p))) return rc;
     const bool own = slot < 0;
     const Graph *g;
-    if ((rc = batch_graph(p, own ? BK_MULTI_OWN : BK_MULTI, n, &g))) return rc;
+    if ((rc = batch_graph(p, own ? BK_MULTI_OWN : BK_MULTI, n, n, &g))) return rc;
     for (int i = 0; i < n; i++) { B.h_rows->token[i] = tokens[i]; B.h_rows->pos[i] = start_pos + i; B.h_rows->slot[i] = own ? 0 : slot; }
     CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
     CK(cudaGraphLaunch(g->exec, p->stream));
@@ -2460,10 +2480,76 @@ int b200_forward_decode_multi(b200_plan *p, int32_t slot, int32_t n, const int32
     return B200_OK;
 }
 
+int b200_forward_step(b200_plan *p, int32_t n, const b200_step_row *rows, int32_t *ids_out, float *logits) {
+    if (!p) return B200_ERR_BAD_ARG;
+    if (const char *why = multi_why(p)) return fail(p, B200_ERR_UNSUPPORTED, "%s", why);
+    auto &B = p->bt;
+    if (!B.n_slots) return fail(p, B200_ERR_STATE, "no decode slots: call b200_set_decode_slots first");
+    if (!rows || !ids_out) return fail(p, B200_ERR_BAD_ARG, "rows and ids_out must not be NULL");
+    const b200_config &c = p->cfg;
+    const int R = batch_max_rows(p);
+    if (n < 1 || n > R) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (b200_decode_multi_rows)", n, R);
+    bool split = false;
+    for (int i = 0; i < n; i++) {
+        const b200_step_row &r = rows[i];
+        if (r.slot < 0 || r.slot >= B.n_slots) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d out of range (%d slots)", i, r.slot, B.n_slots);
+        if (r.token < 0 || r.token >= c.vocab_size) return fail(p, B200_ERR_BAD_ARG, "row %d: token %d out of range", i, r.token);
+        if (r.position < 0 || r.position >= c.context_length)
+            return fail(p, B200_ERR_BAD_ARG, "row %d: position %d outside the KV cache (%d)", i, r.position, c.context_length);
+        for (int j = 0; j < i; j++) {
+            if (rows[j].slot != r.slot) continue;
+            split = true;
+            if (rows[j].position == r.position) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d position %d repeats row %d's", i, r.slot, r.position, j);
+        }
+        if (r.emit != 0 && r.emit != 1) return fail(p, B200_ERR_BAD_ARG, "row %d: emit must be 0 or 1 (got %d)", i, r.emit);
+        if (r.emit && (!(r.temperature >= 0.0f) || !(r.uniform01 >= 0.0f && r.uniform01 < 1.0f)))
+            return fail(p, B200_ERR_BAD_ARG, "row %d: temperature must be >= 0 and the uniform number in [0, 1)", i);
+    }
+    // The emitting rows first, so the classifier runs over rows [0, e) and no kernel indexes through a row map.
+    int order[SMB_MAX_ROWS], e = 0;
+    for (int i = 0; i < n; i++)
+        if (rows[i].emit) order[e++] = i;
+    for (int i = 0, k = e; i < n; i++)
+        if (!rows[i].emit) order[k++] = i;
+    CK(cudaSetDevice(p->device));
+    int rc;
+    const Graph *g;
+    if ((rc = batch_graph(p, split ? BK_MULTI : BK_DECODE, n, e, &g))) return rc;
+    for (int k = 0; k < n; k++) {
+        const b200_step_row &r = rows[order[k]];
+        B.h_rows->token[k] = r.token; B.h_rows->pos[k] = r.position; B.h_rows->slot[k] = r.slot;
+    }
+    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaEventRecord(p->ev0, p->stream));
+    CK(cudaGraphLaunch(g->exec, p->stream));
+    CK(cudaEventRecord(p->ev1, p->stream));
+    const size_t vpad = (size_t)sampler_padded(c.vocab_size);
+    if (logits) // before the sampler turns sampled rows into probabilities
+        for (int k = 0; k < e; k++)
+            CK(cudaMemcpyAsync(logits + (size_t)order[k] * c.vocab_size, B.logits + k * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
+    int m = 0, srow[SMB_MAX_ROWS];
+    float t[SMB_MAX_ROWS], tp[SMB_MAX_ROWS], u[SMB_MAX_ROWS];
+    for (int k = 0; k < e; k++) {
+        const b200_step_row &r = rows[order[k]];
+        if (r.temperature == 0.0f) continue; // FloatTensor.argmax, already computed
+        srow[m] = k; t[m] = r.temperature; tp[m] = r.topp; u[m] = r.uniform01;
+        m++;
+    }
+    if (m && (rc = launch_sample_rows(p, m, srow, t, tp, u))) return rc;
+    if (e) CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)e * 4, cudaMemcpyDeviceToHost, p->stream));
+    if (m) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)e * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
+    for (int i = 0; i < n; i++) ids_out[i] = -1;
+    for (int k = 0; k < e; k++) ids_out[order[k]] = rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
+    CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
+    B.last_launches = g->launches;
+    return B200_OK;
+}
+
 int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step) {
     if (!p) return B200_ERR_BAD_ARG;
     if (n_slots) *n_slots = p->bt.n_slots;
-    if (launches_per_step) *launches_per_step = p->bt.g[BK_DECODE][p->bt.last_n].launches;
+    if (launches_per_step) *launches_per_step = p->bt.last_launches;
     if (device_ms_last_step) *device_ms_last_step = p->bt.last_ms;
     return B200_OK;
 }

@@ -49,8 +49,8 @@ __device__ void sampler_sift_down(int *arr, int from, int n, const float *p) { /
     }
 }
 
-__global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample(SamplerArgs a) {
-    extern __shared__ __align__(16) unsigned char smp_sm[];
+// The sampler on one logits row, by one SAMPLER_THREADS-thread block with sampler_smem_bytes() of dynamic shared memory at smp_sm.
+__device__ __forceinline__ void sample_row(const SamplerArgs &a, unsigned char *smp_sm) {
     SeqSum2Scratch scratch = seqsum2_carve(smp_sm, SAMPLER_THREADS);
     float *red = reinterpret_cast<float *>(smp_sm + seqsum2_scratch_bytes(SAMPLER_THREADS)); // [32] floats + [33] ints
     int *redi = reinterpret_cast<int *>(red + 32);
@@ -150,4 +150,35 @@ __global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample(SamplerArgs a) {
     }
     *a.out_id = id;
     if (a.info) { a.info[0] = n0; a.info[1] = n0 - last; }
+}
+
+__global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample(SamplerArgs a) {
+    extern __shared__ __align__(16) unsigned char smp_sm[];
+    sample_row(a, smp_sm);
+}
+
+// Every sampled row of a batched step in one launch: block j samples logits row row[j] (of rows stride floats apart) into
+// out[8 * row[j]] (the id, then the four diagnostics), with that row's own triple and its own indices scratch (n ints per row).
+#define SAMPLER_MAX_ROWS 8
+
+struct SamplerRowsArgs {
+    float *logits;
+    int stride, n;
+    int *indices; // [row][n]
+    int *out;     // [row][8]
+    int row[SAMPLER_MAX_ROWS];
+    float temperature[SAMPLER_MAX_ROWS], topp[SAMPLER_MAX_ROWS], r01[SAMPLER_MAX_ROWS];
+};
+
+__global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample_rows(SamplerRowsArgs a) {
+    extern __shared__ __align__(16) unsigned char smp_sm[];
+    const int j = blockIdx.x, r = a.row[j];
+    SamplerArgs s;
+    s.logits = a.logits + (size_t)r * a.stride;
+    s.n = a.n;
+    s.temperature = a.temperature[j]; s.topp = a.topp[j]; s.r01 = a.r01[j];
+    s.indices = a.indices + (size_t)r * a.n;
+    s.out_id = a.out + 8 * r;
+    s.info = a.out + 8 * r + 1;
+    sample_row(s, smp_sm);
 }

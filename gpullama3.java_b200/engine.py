@@ -12,12 +12,17 @@ Position/token conventions decide parity, so they are restated exactly:
                               (prefill_slots), then lockstep decode
 ``generate_tokens_lookahead`` the first loop, several positions verified per step (forward_decode_multi): the rest of the
                               prompt, or drafted tokens, checked in one weight stream; the same ids for any draft
+``ContinuousBatcher`` / ``generate_tokens_continuous`` the first two loops for a stream of requests: decode rows of running
+                              requests and prompt rows of newly admitted ones share each forward_step, and freed slots are
+                              refilled from a queue
 The sampler is greedy (temperature 0 -> FloatTensor.argmax, Sampler.java:124-132) and runs on
 the device; ``forward`` is any callable (token, position) -> argmax so the same loops drive
 the oracle in the tests.
 """
 from __future__ import annotations
 
+import time
+from collections import deque
 from typing import Callable, Iterable
 
 Forward = Callable[[int, int], int]
@@ -289,3 +294,190 @@ def generate_tokens_lookahead(plan, model_type: str, latest_token: int, start_po
     if stats is not None:
         stats.update(steps=steps, drafted=drafted, accepted=accepted)
     return generated
+
+
+class _Request:
+    __slots__ = ("rid", "steps", "sampler", "kv_left", "row", "slot", "generated")
+
+    def __init__(self, rid, steps, sampler, kv_rows):
+        self.rid, self.steps, self.sampler, self.kv_left = rid, steps, sampler, kv_rows
+        self.row = None  # the (token, position) the loop asks for next
+        self.slot = -1
+        self.generated = 0
+
+
+class ContinuousBatcher:
+    """Continuous batching over the plan's decode slots: requests queue, are admitted first in, first out into free slots, and share
+    each forward_step with the requests already generating.
+
+    A step holds at most decode_multi_rows() rows: first one emitting row for every request that has generated a token, then the
+    prompt rows of the requests still in their prompt, in admission order, as many as fit.  A request's rows are exactly the
+    (token, position) sequence loop_for(model_type) runs for it -- the Llama loop's K/V-only rows are latest + prompt[:-1], the
+    Qwen3 loop's prompt[:-1] -- so a prompt may span several steps, and its last row, which yields the first generated token,
+    emits.  Both loops' budget clamps and the Qwen3 loop's skipped position come with the loop; slot_reset at admission makes the
+    skipped row read as zero.  A request ends at its stop token or budget and its slot takes the next queued request in the same
+    step().  Every forward_step row is bit-identical to forward_decode of its sequence alone, so each request's ids equal its loop
+    run alone on one slot, greedy or sampled with the same seed, whatever else shares the steps.
+
+    sampler (optional, per request): a sampler.Sampler; one next_float1() is drawn per generated token, never for a prompt row, as
+    generateTokensLlama draws it (InferenceEngine.java:81-154).  The steps are always the exact mixed steps, whatever the plan's
+    prefill mode."""
+
+    def __init__(self, plan, model_type: str, stop_tokens: Iterable[int], max_tokens: int, context_length: int):
+        self.plan = plan
+        self.rows = plan.decode_multi_rows()
+        if self.rows < 1:
+            raise ValueError("the plan cannot run mixed steps (decode_multi_rows() == 0)")
+        n_slots = plan.batch_info()[0]
+        if n_slots < 1:
+            raise ValueError("the plan has no decode slots (set_decode_slots)")
+        self.qwen = _is_qwen_loop(model_type)
+        self.stop = list(stop_tokens)
+        self.max_tokens, self.context_length = max_tokens, context_length
+        self.results: dict = {}  # request id -> generated ids so far
+        self.last_rows = 0  # rows of the last step() (0: no step ran)
+        self._queue: deque = deque()
+        self._free = list(range(n_slots))
+        self._running: list = []  # admitted requests, in admission order
+        self._next_id = 0
+
+    def submit(self, latest_token: int, start_position: int, prompt_tokens: list[int], sampler=None) -> int:
+        """Queue one request (the arguments of generate_tokens_llama / generate_tokens_qwen3); returns its id."""
+        if start_position < 0:
+            raise ValueError(f"start_position {start_position} is negative")
+        prompt = [int(t) for t in prompt_tokens]
+        make = _qwen3_steps if self.qwen else _llama_steps
+        steps = make(int(latest_token), int(start_position), prompt, self.stop, self.max_tokens, self.context_length)
+        rid = self._next_id
+        self._next_id += 1
+        self.results[rid] = []
+        self._queue.append(_Request(rid, steps, sampler, max(len(prompt) - 1, 0) if self.qwen else len(prompt)))
+        return rid
+
+    def pending(self) -> int:
+        """Requests queued but not admitted."""
+        return len(self._queue)
+
+    def running(self) -> int:
+        """Requests holding a slot."""
+        return len(self._running)
+
+    def _admit(self, out: list):
+        while self._queue and self._free:
+            r = self._queue.popleft()
+            try:
+                r.row = next(r.steps)
+            except StopIteration:  # the budget ends it before its first row
+                out.append((r.rid, None, True))
+                continue
+            r.slot = self._free.pop(0)
+            self.plan.slot_reset(r.slot)
+            self._running.append(r)
+
+    def _advance(self, r: _Request, am) -> bool:
+        """Send the row's result to the loop; False when the loop has ended."""
+        try:
+            r.row = r.steps.send(am)
+            return True
+        except StopIteration:
+            r.row = None
+            return False
+
+    def step(self) -> list:
+        """Admit what fits, run one mixed step, and return (request id, token, finished) per generated token, in row order.  A
+        request that ends without generating a token (its budget) is reported as (request id, None, True).  A step with no rows
+        is not run."""
+        out: list = []
+        self._admit(out)
+        rows, emit = [], []  # rows: (slot, token, position, emit, temperature, topp, uniform01); emit: the emitting rows' requests
+        ended = []  # requests whose loop ended on a K/V-only row of this step
+
+        def add(r, emitting):
+            smp = r.sampler if emitting else None
+            if smp is not None and smp.temperature != 0.0:
+                rows.append((r.slot, r.row[0], r.row[1], 1, smp.temperature, smp.topp, smp.rng.next_float1()))
+            else:
+                rows.append((r.slot, r.row[0], r.row[1], int(emitting), 0.0, 0.0, 0.0))
+            if emitting:
+                emit.append(r)
+
+        for r in self._running:  # one decode row per generating request
+            if r.generated:
+                add(r, True)
+        for r in self._running:  # then the prompts, in admission order
+            while not r.generated and r.row is not None and len(rows) < self.rows:
+                if r.kv_left == 0:
+                    add(r, True)
+                    break
+                add(r, False)
+                r.kv_left -= 1
+                if not self._advance(r, -1):  # a K/V-only row: the loop does not read its result
+                    ended.append(r)
+        self.last_rows = len(rows)
+        if rows:
+            ids, _ = self.plan.forward_step(rows)
+            done = list(ended)
+            k = 0
+            for row, am in zip(rows, ids):
+                if not row[3]:
+                    continue
+                r = emit[k]
+                k += 1
+                tok = int(am)
+                self.results[r.rid].append(tok)
+                r.generated += 1
+                alive = self._advance(r, tok)
+                out.append((r.rid, tok, not alive))
+                if not alive:
+                    done.append(r)
+            for r in ended:
+                out.append((r.rid, None, True))
+            for r in done:
+                self._running.remove(r)
+                self._free.append(r.slot)
+            self._free.sort()
+        self._admit(out)
+        return out
+
+
+def generate_tokens_continuous(plan, model_type: str, requests: list, arrivals: list, stop_tokens: Iterable[int], max_tokens: int,
+                               context_length: int, samplers: list | None = None, stats: dict | None = None) -> list[list[int]]:
+    """Replays a request trace through a ContinuousBatcher: request i = (latest_token, start_position, prompt_tokens) is submitted
+    before step arrivals[i] (requests of the same step in index order), with samplers[i] if given.  Steps with no rows still count.
+    Returns each request's ids, equal to loop_for(model_type) for the request alone.  stats (optional dict) receives the steps run,
+    the rows and launches of each, and per request its submission, first-token and completion times (time.perf_counter seconds,
+    None where it generated no token)."""
+    if len(arrivals) != len(requests):
+        raise ValueError(f"{len(requests)} requests but {len(arrivals)} arrival steps")
+    if samplers is not None and len(samplers) != len(requests):
+        raise ValueError(f"{len(requests)} requests but {len(samplers)} samplers")
+    if any(a < 0 for a in arrivals):
+        raise ValueError("arrival steps must be >= 0")
+    cb = ContinuousBatcher(plan, model_type, stop_tokens, max_tokens, context_length)
+    order = sorted(range(len(requests)), key=lambda i: (arrivals[i], i))
+    rid_of: dict = {}
+    t_sub, t_first, t_done = [None] * len(requests), [None] * len(requests), [None] * len(requests)
+    rows, launches = [], []
+    nxt, k = 0, 0
+    while nxt < len(order) or cb.pending() or cb.running():
+        while nxt < len(order) and arrivals[order[nxt]] <= k:
+            i = order[nxt]
+            latest, start, prompt = requests[i]
+            rid_of[cb.submit(latest, start, prompt, samplers[i] if samplers is not None else None)] = i
+            t_sub[i] = time.perf_counter()
+            nxt += 1
+        events = cb.step()
+        now = time.perf_counter()
+        if cb.last_rows:
+            rows.append(cb.last_rows)
+            launches.append(plan.batch_info()[1])
+        for rid, tok, finished in events:
+            i = rid_of[rid]
+            if tok is not None and t_first[i] is None:
+                t_first[i] = now
+            if finished:
+                t_done[i] = now
+        k += 1
+    if stats is not None:
+        stats.update(steps=len(rows), rows=rows, launches=launches, submitted=t_sub, first_token=t_first, done=t_done)
+    return [cb.results[rid] for rid in sorted(rid_of, key=lambda r: rid_of[r])]

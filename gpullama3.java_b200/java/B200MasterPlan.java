@@ -83,6 +83,7 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle SET_DECODE_SLOTS = fn("b200_set_decode_slots", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle DECODE_BATCH = fn("b200_forward_decode_batch",
             FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
+    private static final MethodHandle FORWARD_STEP = fn("b200_forward_step", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS));
     private static final MethodHandle SLOT_RESET = fn("b200_slot_reset", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle SLOT_COPY_KV = fn("b200_slot_copy_kv", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
     private static final MethodHandle PREFILL_SLOTS = fn("b200_prefill_slots", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
@@ -299,6 +300,30 @@ public final class B200MasterPlan implements AutoCloseable {
                     a.allocateFrom(JAVA_INT, positions), smp, ids, MemorySegment.NULL);
             if (rc != 0) check(rc, lastError());
             return ids.toArray(JAVA_INT);
+        }
+    }
+
+    /** One mixed step: row i = tokens[i] at positions[i] on slot slots[i]; a slot may take several rows at distinct positions.  emit[i]
+     *  false: K/V only (a prompt position), id -1; true: the id after the row, greedy or, with sampling non-null, sampled from
+     *  {temperature, topp, rng.nextFloat(1f)} of row i (temperature 0 = argmax).  Every row's K/V is written before any row attends,
+     *  so each emitting row is bit-identical to forwardDecode / forwardDecodeSample of its own sequence (b200_forward_step). */
+    public int[] forwardStep(int[] slots, int[] tokens, int[] positions, boolean[] emit, float[] sampling) throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            int n = tokens.length;
+            MemorySegment rows = a.allocate(28L * Math.max(1, n), 4); // b200_step_row: 4 int32 + 3 float
+            for (int i = 0; i < n; i++) {
+                long o = 28L * i;
+                rows.set(JAVA_INT, o, slots[i]);
+                rows.set(JAVA_INT, o + 4, tokens[i]);
+                rows.set(JAVA_INT, o + 8, positions[i]);
+                rows.set(JAVA_INT, o + 12, emit[i] ? 1 : 0);
+                for (int k = 0; k < 3; k++)
+                    rows.set(JAVA_FLOAT, o + 16 + 4L * k, sampling == null ? 0f : sampling[3 * i + k]);
+            }
+            MemorySegment ids = a.allocate(JAVA_INT, Math.max(1, n));
+            int rc = (int) FORWARD_STEP.invokeExact(plan, n, rows, ids, MemorySegment.NULL);
+            if (rc != 0) check(rc, lastError());
+            return ids.asSlice(0, 4L * n).toArray(JAVA_INT);
         }
     }
 

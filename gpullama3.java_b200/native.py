@@ -49,6 +49,11 @@ class YarnConfig(C.Structure):
     _fields_ = [(n, C.c_float) for n in ("factor", "beta_fast", "beta_slow", "log_multiplier")] + [("original_context_length", C.c_int32)]
 
 
+class StepRow(C.Structure):
+    """b200_step_row: one row of a mixed step (b200_forward_step)."""
+    _fields_ = [(n, C.c_int32) for n in ("slot", "token", "position", "emit")] + [(n, C.c_float) for n in ("temperature", "topp", "uniform01")]
+
+
 class Tensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("ggml_type", C.c_int32), ("n_dims", C.c_int32),
                 ("dims", C.c_int64 * 4)]
@@ -58,7 +63,7 @@ EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
-           "b200_forward_decode_multi", "b200_decode_multi_rows",
+           "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -109,6 +114,7 @@ def lib() -> C.CDLL:
     L.b200_batch_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
     L.b200_forward_decode_multi.argtypes = [vp, i32, i32, vp, i32, vp, vp]
     L.b200_decode_multi_rows.argtypes = [vp, C.POINTER(i32)]
+    L.b200_forward_step.argtypes = [vp, i32, C.POINTER(StepRow), vp, vp]
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     L.b200_launches_per_decode.argtypes = [vp]
     L.b200_device_bytes.argtypes = [vp]
@@ -423,6 +429,20 @@ class NativePlan:
         ids = np.empty(max(n, 1), dtype=np.int32)
         lg = np.empty((n, self.cfg.vocab_size), dtype=np.float32) if want_logits else None
         self._ck(lib().b200_forward_decode_multi(self._p, slot, n, t.ctypes.data, start_pos, ids.ctypes.data, lg.ctypes.data if want_logits else None))
+        return ids[:n], lg
+
+    def forward_step(self, rows, logits: bool = False):
+        """b200_forward_step: one mixed step.  rows: (slot, token, position, emit[, temperature, topp, uniform01]) per row.  Returns
+        (ids int32 [n], -1 where emit is 0; logits float32 [n, vocab] or None, rows with emit 0 left unwritten)."""
+        n = len(rows)
+        arr = (StepRow * max(n, 1))()
+        for i, r in enumerate(rows):
+            if len(r) not in (4, 7):
+                raise ValueError(f"row {i}: (slot, token, position, emit) or (slot, token, position, emit, temperature, topp, uniform01)")
+            arr[i] = StepRow(*[int(v) for v in r[:4]], *[float(v) for v in r[4:]])
+        ids = np.empty(max(n, 1), dtype=np.int32)
+        lg = np.zeros((n, self.cfg.vocab_size), dtype=np.float32) if logits else None
+        self._ck(lib().b200_forward_step(self._p, n, arr, ids.ctypes.data, lg.ctypes.data if logits else None))
         return ids[:n], lg
 
     def decode_multi_rows(self) -> int:

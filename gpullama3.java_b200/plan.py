@@ -196,6 +196,14 @@ class B200MasterPlan:
         decoding.  1 <= len(tokens) <= decode_multi_rows(); single-GPU Q8_0 plans without MoE only."""
         return self._native.forward_decode_multi(slot, tokens, start_pos, logits)
 
+    def forward_step(self, rows, logits: bool = False):
+        """One mixed step over the decode slots -> (ids, logits [n, vocab] or None).  Each row is (slot, token, position, emit) or
+        (slot, token, position, emit, temperature, topp, uniform01); a slot may take several rows at distinct positions, and every
+        row's K/V is written before any row attends.  emit 0: K/V only (a prompt position), id -1; emit 1: the id after the row,
+        greedy (temperature 0) or forward_decode_sample's for the triple, with logits bit-identical to forward_decode of that
+        sequence.  1 <= len(rows) <= decode_multi_rows(); needs set_decode_slots."""
+        return self._native.forward_step(rows, logits)
+
     def decode_multi_rows(self) -> int:
         """Positions per forward_decode_multi step (8 at the 8B shapes); 0 where the plan cannot run it."""
         return self._native.decode_multi_rows()

@@ -326,7 +326,29 @@ int b200_forward_decode_multi(b200_plan *plan, int32_t slot, int32_t n, const in
 /* Rows per b200_forward_decode_multi step (and per step of the exact prefills): 8 at the 8B shapes; 0 where unsupported. */
 int b200_decode_multi_rows(b200_plan *plan, int32_t *max_rows);
 
-/* Decode slots, kernels of the last batched step and its device milliseconds (CUDA events around the graph); any pointer may be NULL. */
+/* One row of a mixed step (b200_forward_step). */
+typedef struct b200_step_row {
+    int32_t slot, token, position;
+    int32_t emit;                        /* 0: K/V only (a prompt position); 1: this row's next token is wanted */
+    float temperature, topp, uniform01;  /* emit rows only: b200_forward_decode_sample's triple; temperature 0 = FloatTensor.argmax */
+} b200_step_row;
+
+/* One mixed step of n rows over the decode slots: decode rows of running sequences and prompt rows of newly admitted ones share
+ * one weight stream.  Row i consumes rows[i].token at rows[i].position of slot rows[i].slot; a slot may appear in several rows (at
+ * distinct positions).  Every row writes its K/V at (slot, position) before any row of the step attends, so each emitting row's
+ * logits are bit-identical to b200_forward_decode of the same token at the same position over the same slot prefix, and its id is
+ * that call's argmax (temperature 0) or b200_forward_decode_sample's id for the same triple.  ids_out receives n ids, -1 where emit
+ * is 0; logits (nullable) n x vocab_size floats, rows with emit 0 not written.  The final norm, lm_head and argmax run over the
+ * emitting rows only, and all sampled rows in one sampler launch.  The plan's own cache, its single-token buffers and the slots
+ * not named are not touched.  B200_ERR_UNSUPPORTED with the reason on plans that cannot run it (FP16, tensor-parallel,
+ * Qwen2-MoE); B200_ERR_STATE before b200_set_decode_slots; B200_ERR_BAD_ARG naming the row for: n outside
+ * 1..b200_decode_multi_rows, a slot, token or position out of range, the same (slot, position) twice, an emit flag other than 0 / 1,
+ * or a bad sampling triple on an emitting row. */
+int b200_forward_step(b200_plan *plan, int32_t n, const b200_step_row *rows, int32_t *ids_out /* n; -1 where emit == 0 */,
+                      float *logits /* nullable, n x vocab; rows with emit == 0 are not written */);
+
+/* Decode slots, kernels of the last batched step (b200_forward_decode_batch or b200_forward_step, whichever ran last) and its
+ * device milliseconds (CUDA events around the graph); any pointer may be NULL. */
 int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step);
 
 /* Test/diagnostic read-back of a named device buffer into host memory.  Names:

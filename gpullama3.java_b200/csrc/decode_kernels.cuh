@@ -151,6 +151,30 @@ __global__ void __launch_bounds__(T, 1) k_test_seqsum2(const float *__restrict__
     if (threadIdx.x == 0) { out[0] = s; info[0] = scratch.info[0]; info[1] = scratch.info[1]; }
 }
 
+// Profiling hook: the accumulator in the fused norm's form (chunks at seqsum2_stride, one out-of-line copy as smv_seqsum and
+// pd_seqsum have), called twice in one launch: the first call runs on a cold instruction cache, the second on a warm one.  Each
+// call is timed in clock64 cycles from a barrier before it to a barrier after it.
+template <int T>
+__device__ __noinline__ float profile_seqsum2_call(const float *sq, int n, int S, unsigned char *scratch) {
+    return block_seqsum_exact_v2_t<T>(sq, n, seqsum2_carve(scratch, T), (int)threadIdx.x, SeqSum2BlockSync(), S);
+}
+template <int T>
+__global__ void __launch_bounds__(T, 1) k_profile_seqsum2(const float *__restrict__ terms, int n, long long *__restrict__ cycles, float *__restrict__ out) {
+    extern __shared__ __align__(16) float sm[];
+    const int E = (n + T - 1) / T, S = seqsum2_stride(E);
+    unsigned char *scratch = reinterpret_cast<unsigned char *>(sm + T * S);
+    for (int i = threadIdx.x; i < T * E; i += T) sm[(i / E) * S + (i % E)] = i < n ? terms[i] : 0.0f;
+    __syncthreads();
+    const long long t0 = clock64();
+    const float s0 = profile_seqsum2_call<T>(sm, n, S, scratch);
+    __syncthreads();
+    const long long t1 = clock64();
+    const float s1 = profile_seqsum2_call<T>(sm, n, S, scratch);
+    __syncthreads();
+    const long long t2 = clock64();
+    if (threadIdx.x == 0) { cycles[0] = t1 - t0; cycles[1] = t2 - t1; out[0] = s0; out[1] = s1; }
+}
+
 // ------------------------------------------------------------------------------------------
 // SwiGLU of one hidden unit, InferenceCore.java:150-158: hb = hb / (float)(1.0 + Math.exp(-hb)); hb *= hb2.
 // ------------------------------------------------------------------------------------------

@@ -1986,6 +1986,14 @@ static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const
     return B200_OK;
 }
 
+template <int T>
+cudaError_t launch_profile_seqsum2(const float *d, int n, long long *cyc, float *o) {
+    const size_t smem = (size_t)T * seqsum2_stride((n + T - 1) / T) * 4 + seqsum2_scratch_bytes(T);
+    cudaError_t e = cudaFuncSetAttribute(k_profile_seqsum2<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) k_profile_seqsum2<T><<<1, T, smem>>>(d, n, cyc, o);
+    return e;
+}
+
 extern "C" {
 
 int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t n_tensors, int32_t prefill_batch_size,
@@ -2787,6 +2795,23 @@ int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out
     if (e == cudaSuccess) e = cudaMemcpy(host, o, 12, cudaMemcpyDeviceToHost);
     memcpy(out, host, 4);
     if (info) { info[0] = host[1]; info[1] = host[2]; }
+    return e == cudaSuccess ? B200_OK : B200_ERR_CUDA;
+}
+
+int b200_profile_seqsum2(const float *terms, int32_t n, int32_t threads, int64_t *cycles, float *out) {
+    if (!terms || !cycles || !out || n <= 0 || n > 16384) return B200_ERR_BAD_ARG;
+    if (threads != 256 && threads != 512 && threads != 1024) return B200_ERR_BAD_ARG;
+    Scratch s;
+    float *d = nullptr, *o = nullptr;
+    long long *cyc = nullptr;
+    if (!s.alloc(&d, (size_t)n * 4) || !s.alloc(&o, 16) || !s.alloc(&cyc, 16)) return B200_ERR_OOM;
+    cudaError_t e = cudaMemcpy(d, terms, (size_t)n * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = threads == 1024 ? launch_profile_seqsum2<1024>(d, n, cyc, o)
+                            : threads == 512 ? launch_profile_seqsum2<512>(d, n, cyc, o) : launch_profile_seqsum2<256>(d, n, cyc, o);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) e = cudaMemcpy(cycles, cyc, 16, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(out, o, 8, cudaMemcpyDeviceToHost);
     return e == cudaSuccess ? B200_OK : B200_ERR_CUDA;
 }
 

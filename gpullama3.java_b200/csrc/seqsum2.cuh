@@ -10,16 +10,19 @@
 //   While the running sum s stays inside one binade [2^e, 2^(e+1)) its mantissa M is an integer in units of u = 2^(e-23), and
 //   adding a term t rounds to  M + k + [f > 1/2]  with t/u = k + f (on an exact tie, f == 1/2, round-half-even makes the
 //   increment depend on the parity of M; real activations produce 3-30 ties per 4096 terms).  So inside a binade a step is the
-//   integer map  M -> M + a[M & 1], and such maps compose associatively.  The evaluation is three block-wide scans and a
-//   ~25-item serial walk:
-//   1. float prefix P over per-thread sums (E consecutive terms per thread)            -> predicted binade per thread
+//   integer map  M -> M + a[M & 1], and such maps compose associatively.  The evaluation takes three barriers and a short
+//   serial walk:
+//   1. float prefix P over per-thread sums (E consecutive terms per thread): a warp scan, barrier 1, and every warp adds
+//      the totals of the warps before it                                                  -> predicted binade per thread
 //   2. a thread whose P range lies well inside one binade composes its E steps  M -> M + a[M & 1]  (SeqPair)
 //      into one pair ("clean"); any other thread is "literal"
-//   3. segmented scan of the pairs over runs of clean threads with equal binade          (pairs compose associatively)
-//   4. item list (ballot/popc compaction): one item per literal thread and one per run
-//   5. one thread walks the items: literal = E real float adds; run = verify (exponent on entry, mantissa < 2^24 on
-//      exit) and add the integer; a failed check replays the run literally.  Predictions decide speed, never the result.
-// CPU model (20000 adversarial cases, n = 2048/4096/8192): 0 mismatches, ~3 head threads + ~24 items per sum.
+//   3. inside each warp: segmented scan of the pairs over runs of clean threads with equal binade (pairs compose
+//      associatively), and ballot/popc compaction into the warp's own item slots: one item per literal thread and one
+//      per run; a run that spans warps becomes one item per warp.  Barrier 2.
+//   4. warp 0 walks the items: literal = E real float adds; run = verify (exponent on entry, mantissa < 2^24 on exit) and
+//      add the integer; a failed check replays the item literally.  Each item is verified on its own, so where runs are
+//      cut and what the predictor says decide speed, never the result.  Barrier 3 hands the sum to every thread.
+// CPU model (tools/seqsum2/emulate_v2.py, adversarial cases up to n = 16384 at 256 / 512 / 1024 threads): 0 mismatches.
 #pragma once
 #include "common.cuh"
 
@@ -64,56 +67,28 @@ __device__ __forceinline__ bool seq_pair(float t, int e, SeqPair &pr) {
 }
 
 struct SeqItem {
-    int cls;          // SEQSUM2_LITERAL or the binade of a run
+    unsigned ebits;   // a run in binade e: e + 127, the exponent field of every sum inside it; a literal thread: ~0u
     unsigned a0, a1;  // the run's composed pair
-    int last;         // thread that closes the item (its own id for a literal thread)
+    unsigned idx;     // first thread | last thread << 10 | slot of the next item << 20 (T: the end of the list)
 };
 
+// Warp w writes its items to items[32 w ..]; every warp has at least one (its lane 31 always closes an item).
 struct SeqSum2Scratch {
-    float *wsum;      // [32] warp totals -> exclusive warp prefixes
-    SeqPair *wtail;   // [32] pair of the run that is open at the end of each warp
-    int *wtail_f;     // [32] 1: that run started inside the warp
-    int *wcls_last;   // [32] class of the warp's last thread
-    int *wcls_first;  // [32] class of the warp's first thread
-    int *wcnt;        // [32] items per warp -> exclusive offsets
-    int *cls;         // [T]  class per thread (fallback walks back over it)
     SeqItem *items;   // [T]
+    float *wsum;      // [32] warp totals of the per-thread sums
+    int *info;        // [2] {items, fallbacks}, written by thread 0 (valid in that thread on return)
     float *result;    // [1]
-    int *info;        // [2] {items, fallbacks}
 };
 __host__ __device__ inline size_t seqsum2_scratch_bytes(int T = SEQSUM2_THREADS) { // T = threads that run the accumulator
-    return 32 * 4 + 32 * sizeof(SeqPair) + 4 * 32 * 4 + (size_t)T * 4 + (size_t)T * sizeof(SeqItem) + 16 + 16;
+    return (size_t)T * sizeof(SeqItem) + 32 * 4 + 16;
 }
 __device__ __forceinline__ SeqSum2Scratch seqsum2_carve(unsigned char *p, int T = SEQSUM2_THREADS) { // p 16-byte aligned
     SeqSum2Scratch s;
     s.items = reinterpret_cast<SeqItem *>(p); p += (size_t)T * sizeof(SeqItem);
-    s.wtail = reinterpret_cast<SeqPair *>(p); p += 32 * sizeof(SeqPair);
-    s.cls = reinterpret_cast<int *>(p); p += (size_t)T * 4;
     s.wsum = reinterpret_cast<float *>(p); p += 32 * 4;
-    s.wtail_f = reinterpret_cast<int *>(p); p += 32 * 4;
-    s.wcls_last = reinterpret_cast<int *>(p); p += 32 * 4;
-    s.wcls_first = reinterpret_cast<int *>(p); p += 32 * 4;
-    s.wcnt = reinterpret_cast<int *>(p); p += 32 * 4;
-    s.result = reinterpret_cast<float *>(p); p += 16;
     s.info = reinterpret_cast<int *>(p);
+    s.result = reinterpret_cast<float *>(p + 8);
     return s;
-}
-
-// Segmented inclusive scan step set over one warp: f = 1 when the run containing this lane starts inside the covered range.
-// (Code size matters more than instruction count here: these phases run once per call on a cold instruction cache, so every
-// loop is kept rolled and the helpers out of line -- a taken branch into code that is not cached costs more than the loop.)
-__device__ __noinline__ void seq2_warp_segscan(SeqPair &p, int &f, int lane) {
-#pragma unroll 1
-    for (int d = 1; d < 32; d <<= 1) {
-        const unsigned u0 = __shfl_up_sync(0xffffffffu, p.a0, d), u1 = __shfl_up_sync(0xffffffffu, p.a1, d);
-        const int fu = __shfl_up_sync(0xffffffffu, f, d);
-        if (lane >= d && !f) {
-            SeqPair L;
-            L.a0 = u0; L.a1 = u1;
-            p = seq_compose(L, p);
-            f = fu;
-        }
-    }
 }
 
 struct SeqSum2BlockSync {
@@ -124,10 +99,19 @@ struct SeqSum2BlockSync {
 // thread t's terms live at sq[t * S .. t * S + E).  E = 16 -> 20, 8 -> 12, 32 -> 36, 4 -> 4.
 __host__ __device__ inline int seqsum2_stride(int E) { return (E % 4 == 0 && (E / 4) % 2 == 0) ? E + 4 : E; }
 
-// literal adds of one thread's E terms (16-byte loads when the layout allows)
-__device__ __noinline__ float seq2_literal(float s, const float *q, int E, bool vec) {
+// literal adds of one thread's E terms (16-byte loads when the layout allows, 16 terms requested before their adds start)
+__device__ __forceinline__ float seq2_literal(float s, const float *q, int E, bool vec) {
     int k = 0;
     if (vec) {
+#pragma unroll 1
+        for (; k + 16 <= E; k += 16) {
+            const float4 v0 = *reinterpret_cast<const float4 *>(q + k), v1 = *reinterpret_cast<const float4 *>(q + k + 4);
+            const float4 v2 = *reinterpret_cast<const float4 *>(q + k + 8), v3 = *reinterpret_cast<const float4 *>(q + k + 12);
+            s = __fadd_rn(s, v0.x); s = __fadd_rn(s, v0.y); s = __fadd_rn(s, v0.z); s = __fadd_rn(s, v0.w);
+            s = __fadd_rn(s, v1.x); s = __fadd_rn(s, v1.y); s = __fadd_rn(s, v1.z); s = __fadd_rn(s, v1.w);
+            s = __fadd_rn(s, v2.x); s = __fadd_rn(s, v2.y); s = __fadd_rn(s, v2.z); s = __fadd_rn(s, v2.w);
+            s = __fadd_rn(s, v3.x); s = __fadd_rn(s, v3.y); s = __fadd_rn(s, v3.z); s = __fadd_rn(s, v3.w);
+        }
 #pragma unroll 1
         for (; k + 4 <= E; k += 4) {
             const float4 v = *reinterpret_cast<const float4 *>(q + k);
@@ -139,31 +123,21 @@ __device__ __noinline__ float seq2_literal(float s, const float *q, int E, bool 
     return s;
 }
 
-// inclusive float prefix over the 32 lanes of a warp (predictor only: plain adds)
-__device__ __noinline__ float seq2_warp_scan_f(float v, int lane) {
-#pragma unroll 1
-    for (int d = 1; d < 32; d <<= 1) {
-        const float u = __shfl_up_sync(0xffffffffu, v, d);
-        if (lane >= d) v += u;
-    }
-    return v;
-}
-
 // sq: n terms, thread t's E = ceil(n / T) consecutive terms at sq[t * S + k] (S >= E; S = E is the plain contiguous layout),
 // zero-padded up to T whole chunks.  Exactly T threads (a multiple of 32, at most SEQSUM2_THREADS) call this with tid in
 // [0, T); `sync` is a barrier over those T threads (the whole CTA, or a named barrier over a subset of its warps as in the
 // persistent decode kernel).  When S and E are multiples of 4 and sq is 16-byte aligned the terms are read with 16-byte loads.
+// Every thread returns the sum.
 template <int T, class Sync>
 __device__ float block_seqsum_exact_v2_t(const float *sq, int n, SeqSum2Scratch sc, int tid, Sync sync, int S = 0) {
     static_assert(T % 32 == 0 && T <= SEQSUM2_THREADS, "T threads = T/32 whole warps");
-    constexpr int NW = T / 32;
     const int lane = tid & 31, warp = tid >> 5;
     const int E = (n + T - 1) / T;
     if (S == 0) S = E;
     const bool vec = ((E | S) & 3) == 0 && (reinterpret_cast<uintptr_t>(sq) & 15) == 0;
     const float *mine = sq + tid * S;
 
-    // ---- 1. float prefix over per-thread sums
+    // ---- 1. float prefix over per-thread sums (a predictor: plain adds in any order)
     float loc = 0.0f;
     {
         int k = 0;
@@ -177,16 +151,17 @@ __device__ float block_seqsum_exact_v2_t(const float *sq, int n, SeqSum2Scratch 
 #pragma unroll 1
         for (; k < E; k++) loc += mine[k];
     }
-    const float inc = seq2_warp_scan_f(loc, lane);
-    if (lane == 31) sc.wsum[warp] = inc;
-    sync();
-    if (warp == 0) {
-        const float w = lane < NW ? sc.wsum[lane] : 0.0f;
-        const float v = seq2_warp_scan_f(w, lane);
-        if (lane < NW) sc.wsum[lane] = v - w; // exclusive
+    float inc = loc;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const float u = __shfl_up_sync(0xffffffffu, inc, d);
+        if (lane >= d) inc += u;
     }
-    sync();
-    const float wex = sc.wsum[warp];
+    if (lane == 31) sc.wsum[warp] = inc;
+    sync(); // barrier 1: the warp totals
+    float wex = lane < warp ? sc.wsum[lane] : 0.0f; // every warp forms its own offset
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) wex += __shfl_xor_sync(0xffffffffu, wex, d);
     const float p_end = wex + inc, p_start = wex + (inc - loc);
 
     // ---- 2. classify, compose the thread's own steps
@@ -220,90 +195,63 @@ __device__ float block_seqsum_exact_v2_t(const float *sq, int n, SeqSum2Scratch 
             }
         }
     }
-    sc.cls[tid] = cls;
-    if (lane == 31) sc.wcls_last[warp] = cls;
-    if (lane == 0) sc.wcls_first[warp] = cls;
-    sync();
 
-    // ---- 3. segmented scan over runs of clean threads with equal binade
-    int prev_cls = __shfl_up_sync(0xffffffffu, cls, 1);
-    if (lane == 0) prev_cls = warp ? sc.wcls_last[warp - 1] : SEQSUM2_LITERAL;
-    int next_cls = __shfl_down_sync(0xffffffffu, cls, 1);
-    if (lane == 31) next_cls = warp < NW - 1 ? sc.wcls_first[warp + 1] : SEQSUM2_LITERAL;
+    // ---- 3. runs of clean threads with equal binade, cut at warp boundaries: segmented scan of the pairs inside the warp,
+    // then one item per literal thread and one per run, compacted into the warp's own slots
     const bool clean = cls != SEQSUM2_LITERAL;
-    int f = (clean && prev_cls == cls) ? 0 : 1; // 1 = a run (or a literal thread) starts here
-    seq2_warp_segscan(pr, f, lane);
-    if (lane == 31) { sc.wtail[warp] = pr; sc.wtail_f[warp] = f; }
-    sync();
-    if (warp == 0) { // carry[w] = pair of the run that is still open when warp w begins (scan over the warp tails)
-        SeqPair t;
-        t.a0 = t.a1 = 0u;
-        int tf = 1;
-        if (lane < NW) { t = sc.wtail[lane]; tf = sc.wtail_f[lane]; }
-        seq2_warp_segscan(t, tf, lane);
-        if (lane < NW) sc.wtail[lane] = t; // inclusive: run open at the END of warp `lane`, composed from its true start
-    }
-    sync();
-    if (!f && warp > 0) pr = seq_compose(sc.wtail[warp - 1], pr); // f == 0 in warp 0 cannot happen (thread 0 always starts a run)
-
-    // ---- 4. item list
-    const bool is_item = !clean || next_cls != cls;
-    const unsigned bal = __ballot_sync(0xffffffffu, is_item);
-    if (lane == 0) sc.wcnt[warp] = __popc(bal);
-    sync();
-    if (warp == 0) {
-        const int c = lane < NW ? sc.wcnt[lane] : 0;
-        int v = c;
-#pragma unroll 1
-        for (int d = 1; d < 32; d <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, v, d);
-            if (lane >= d) v += u;
+    const int prev_cls = __shfl_up_sync(0xffffffffu, cls, 1), next_cls = __shfl_down_sync(0xffffffffu, cls, 1);
+    int f = (clean && lane > 0 && prev_cls == cls) ? 0 : 1; // 1 = a run (or a literal thread) starts here
+    const bool is_item = !clean || lane == 31 || next_cls != cls;
+    const unsigned starts = __ballot_sync(0xffffffffu, f), bal = __ballot_sync(0xffffffffu, is_item);
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const unsigned u0 = __shfl_up_sync(0xffffffffu, pr.a0, d), u1 = __shfl_up_sync(0xffffffffu, pr.a1, d);
+        const int fu = __shfl_up_sync(0xffffffffu, f, d);
+        if (lane >= d && !f) {
+            SeqPair L;
+            L.a0 = u0; L.a1 = u1;
+            pr = seq_compose(L, pr);
+            f = fu;
         }
-        if (lane < NW) sc.wcnt[lane] = v - c;
-        if (lane == 31) sc.info[0] = v;
     }
-    sync();
     if (is_item) {
+        const int slot = warp * 32 + __popc(bal & ((1u << lane) - 1u));
+        const int first = warp * 32 + 31 - __clz(starts & (0xffffffffu >> (31 - lane)));
+        const int next = (bal >> lane) > 1u ? slot + 1 : (warp + 1) * 32;
         SeqItem it;
-        it.cls = cls; it.a0 = pr.a0; it.a1 = pr.a1; it.last = tid;
-        sc.items[sc.wcnt[warp] + __popc(bal & ((1u << lane) - 1u))] = it;
+        it.ebits = clean ? (unsigned)(cls + 127) : ~0u; it.a0 = pr.a0; it.a1 = pr.a1; it.idx = (unsigned)first | ((unsigned)tid << 10) | ((unsigned)next << 20);
+        sc.items[slot] = it;
     }
-    sync();
+    sync(); // barrier 2: the items
 
-    // ---- 5. resolver
-    if (tid == 0) {
-        const int n_items = sc.info[0];
-        float s = 0.0f;
-        int fallbacks = 0;
+    // ---- 4. resolver: warp 0 walks the items (every lane the same; one warp alone keeps the whole issue rate of its
+    // scheduler), barrier 3 hands the sum to the other warps
+    if (warp == 0) {
+        unsigned sb = 0u; // the bits of the running sum (s >= 0)
+        int items = 0, fallbacks = 0;
         SeqItem nxt = sc.items[0];
 #pragma unroll 1
-        for (int i = 0; i < n_items; i++) {
+        for (int i = 0; i < T; items++) {
             const SeqItem it = nxt;
-            if (i + 1 < n_items) nxt = sc.items[i + 1]; // in flight while this item is resolved
-            if (it.cls == SEQSUM2_LITERAL) {
-                s = seq2_literal(s, sq + it.last * S, E, vec);
+            i = (int)(it.idx >> 20);
+            nxt = sc.items[min(i, T - 1)]; // in flight while this item is resolved
+            // a run on the float's bits: the mantissa's parity is the bit pattern's, and M + a < 2^24 exactly when the add
+            // leaves the exponent field alone; a denormal, inf or NaN sum and a literal thread never match ebits
+            const unsigned nb = sb + ((sb & 1u) ? it.a1 : it.a0);
+            if ((sb >> 23) == it.ebits && (nb >> 23) == it.ebits) {
+                sb = nb;
                 continue;
             }
-            const unsigned sb = __float_as_uint(s);
-            bool ok = f32_exponent(s) == it.cls && (sb >> 23) != 0u;
-            if (ok) {
-                const unsigned M = (sb & 0x7fffffu) | 0x800000u;
-                const unsigned M2 = M + ((M & 1u) ? it.a1 : it.a0);
-                if (M2 < (1u << 24)) s = __uint_as_float(((unsigned)(it.cls + 127) << 23) | (M2 & 0x7fffffu));
-                else ok = false;
-            }
-            if (!ok) { // misprediction: replay the run literally (its first thread: walk back over equal classes)
-                int first = it.last;
-                while (first > 0 && sc.cls[first - 1] == it.cls) first--;
+            fallbacks += it.ebits != ~0u; // a misprediction; otherwise a literal thread: replay the item's threads literally
+            const int last = (int)((it.idx >> 10) & 1023u);
+            float s = __uint_as_float(sb);
 #pragma unroll 1
-                for (int j = first; j <= it.last; j++) s = seq2_literal(s, sq + j * S, E, vec);
-                fallbacks++;
-            }
+            for (int j = (int)(it.idx & 1023u); j <= last; j++) s = seq2_literal(s, sq + j * S, E, vec);
+            sb = __float_as_uint(s);
         }
-        sc.result[0] = s;
-        sc.info[1] = fallbacks;
+        if (lane == 0) { sc.info[0] = items; sc.info[1] = fallbacks; sc.result[0] = __uint_as_float(sb); }
     }
-    sync();
+    sync(); // barrier 3: the sum
     return sc.result[0];
 }
 

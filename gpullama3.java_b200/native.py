@@ -60,7 +60,7 @@ class Tensor(C.Structure):
 
 
 EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
-           "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
+           "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
            "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step",
@@ -97,6 +97,7 @@ def lib() -> C.CDLL:
     L.b200_decode_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     L.b200_trace_persistent.argtypes = [vp, i32, i32, vp, C.c_int64, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     L.b200_test_seqsum2.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(i32)]
+    L.b200_profile_seqsum2.argtypes = [vp, i32, i32, C.POINTER(C.c_int64), C.POINTER(C.c_float)]
     L.b200_test_sample.argtypes = [vp, i32, C.c_float, C.c_float, C.c_float, C.POINTER(i32), C.POINTER(i32), vp]
     L.b200_prefill_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
     L.b200_gemm_f16.argtypes = [vp, vp, vp, i32, i32, i32, i32, C.POINTER(C.c_float)]
@@ -143,6 +144,17 @@ def test_seqsum(terms, want_info: bool = False, threads: int = 1024):
     if rc != B200_OK:
         _raise(rc, "b200_test_seqsum2 failed")
     return (out.value, info[0], info[1]) if want_info else out.value
+
+
+def profile_seqsum(terms, threads: int = 256):
+    """Cycles of the exact sequential sum in the fused norm's chunk layout, two calls in one launch: (cold, warm, sum, sum)."""
+    t = np.ascontiguousarray(terms, dtype=np.float32)
+    cyc = (C.c_int64 * 2)()
+    out = (C.c_float * 2)()
+    rc = lib().b200_profile_seqsum2(t.ctypes.data, len(t), threads, cyc, out)
+    if rc != B200_OK:
+        _raise(rc, "b200_profile_seqsum2 failed")
+    return cyc[0], cyc[1], out[0], out[1]
 
 
 def test_sample(logits, temperature: float, topp: float, uniform01: float):

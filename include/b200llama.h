@@ -413,6 +413,10 @@ int b200_profile_norm(b200_plan *plan, int64_t *cycles);
  * or 256 threads; info = {items walked, fallbacks}. */
 int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out, int32_t *info /* nullable */);
 
+/* Diagnostic: SM-clock cycles of the same exact sum in the fused norm's chunk layout, called twice in one launch of `threads`
+ * = 1024, 512 or 256 threads: cycles[0] on a cold instruction cache, cycles[1] warm; out[0..1] = the two sums. */
+int b200_profile_seqsum2(const float *terms, int32_t n, int32_t threads, int64_t *cycles, float *out);
+
 /* Test hook for the device-side sampler (csrc/sampler.cuh): ONE launch of k_sample as b200_forward_decode_sample issues it (same
  * grid and shared memory, a logits buffer of whole 1024-float chunks with a zero pad) on n host logits.  Returns the sampled id, the
  * diagnostics {top-p candidates, tokens kept, seqsum items, seqsum fallbacks} and the n probabilities the kernel leaves in place.

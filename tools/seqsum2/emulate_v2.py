@@ -1,5 +1,7 @@
 """Thread-accurate Python emulation of csrc/seqsum2.cuh::block_seqsum_exact_v2_t (T threads, warp shuffles with CUDA semantics)
-against the literal float32 loop, on the exact inputs of tests/test_gpu_parity.py::test_exact_parallel_sequential_sum.
+against the literal float32 loop.  Without an argument: adversarial cases (ties, binade crossings, zeros, denormals, inf terms) at
+n = 2048 / 4096 / 5120 / 8192 / 16384 and T = 256 / 512 / 1024 in the fused norm's chunk layout; with T: the exact inputs of
+tests/test_gpu_parity.py::test_exact_parallel_sequential_sum at T threads.
 Usage: python tools/seqsum2/emulate_v2.py [T]"""
 import sys
 
@@ -54,17 +56,20 @@ def warp_segscan(ps, fs):
     return ps, fs
 
 
-def v2(terms, T):
+def v2(terms, T, S=None):
     n = len(terms)
     E = (n + T - 1) // T
-    sq = np.zeros(T * E, dtype=F)
-    sq[:n] = terms
+    S = E if S is None else S
+    sq = np.zeros(T * S, dtype=F)
+    for t in range(T):
+        chunk = terms[t * E:(t + 1) * E]
+        sq[t * S:t * S + len(chunk)] = chunk
     NW = T // 32
     loc = np.zeros(T, dtype=F)
     for t in range(T):
         s = F(0)
         for k in range(E):
-            s = F(s + sq[t * E + k])
+            s = F(s + sq[t * S + k])
         loc[t] = s
     inc = loc.copy()
     for w in range(NW):
@@ -77,18 +82,16 @@ def v2(terms, T):
                     v[l] = F(v[l] + u[l])
             d <<= 1
         inc[w * 32:(w + 1) * 32] = v
-    wsum = np.zeros(32, dtype=F)
+    wsum = [inc[w * 32 + 31] for w in range(NW)]
+    # barrier 1; every warp: lane l holds wsum[l] if l < warp, then an xor butterfly (__shfl_xor_sync)
+    wex = np.zeros(NW, dtype=F)
     for w in range(NW):
-        wsum[w] = inc[w * 32 + 31]
-    v = wsum.copy()
-    d = 1
-    while d < 32:
-        u = np.concatenate([v[:d], v[:-d]])
-        for l in range(32):
-            if l >= d:
-                v[l] = F(v[l] + u[l])
-        d <<= 1
-    wex = np.array([F(v[l] - wsum[l]) for l in range(32)], dtype=F)
+        v = np.array([wsum[l] if l < w else F(0) for l in range(32)], dtype=F)
+        d = 16
+        while d > 0:
+            v = np.array([F(v[l] + v[l ^ d]) for l in range(32)], dtype=F)
+            d >>= 1
+        wex[w] = v[0]
     cls = [LITERAL] * T
     pr = [(0, 0)] * T
     for t in range(T):
@@ -104,7 +107,7 @@ def v2(terms, T):
             if p_start >= lo and p_end <= F(hi):
                 ok, p = True, (0, 0)
                 for k in range(E):
-                    o, q = seq_pair(sq[t * E + k], e)
+                    o, q = seq_pair(sq[t * S + k], e)
                     if not o:
                         ok = False
                         break
@@ -112,53 +115,45 @@ def v2(terms, T):
                 if ok:
                     cls[t] = e
                     pr[t] = p
-    f = [0] * T
-    isitem = [False] * T
-    for t in range(T):
-        prev = cls[t - 1] if t > 0 else LITERAL
-        nxt = cls[t + 1] if t < T - 1 else LITERAL
-        clean = cls[t] != LITERAL
-        f[t] = 0 if (clean and prev == cls[t]) else 1
-        isitem[t] = (not clean) or nxt != cls[t]
-    wtail, wtail_f = [None] * NW, [None] * NW
+    # per warp: runs cut at the warp's edges, segmented scan, ballot compaction into slots [32 w, 32 w + count)
+    items = [None] * T
     for w in range(NW):
-        ps, fs = warp_segscan(pr[w * 32:(w + 1) * 32], f[w * 32:(w + 1) * 32])
-        pr[w * 32:(w + 1) * 32] = ps
-        f[w * 32:(w + 1) * 32] = fs
-        wtail[w], wtail_f[w] = ps[31], fs[31]
-    tp = [(wtail[l] if l < NW else (0, 0)) for l in range(32)]
-    tf = [(wtail_f[l] if l < NW else 1) for l in range(32)]
-    tp, tf = warp_segscan(tp, tf)
-    for t in range(T):
-        w = t >> 5
-        if not f[t] and w > 0:
-            pr[t] = compose(tp[w - 1], pr[t])
-    items = [(cls[t], pr[t], t) for t in range(T) if isitem[t]]
-    s = F(0)
-    fallbacks = 0
+        lo_t = w * 32
+        f = [0] * 32
+        isitem = [False] * 32
+        for l in range(32):
+            t = lo_t + l
+            clean = cls[t] != LITERAL
+            f[l] = 0 if (clean and l > 0 and cls[t - 1] == cls[t]) else 1
+            isitem[l] = (not clean) or l == 31 or cls[t + 1] != cls[t]
+        starts = [l for l in range(32) if f[l]]
+        bal = [l for l in range(32) if isitem[l]]
+        ps, _ = warp_segscan(pr[lo_t:lo_t + 32], f)
+        for rank, l in enumerate(bal):
+            first = lo_t + max(x for x in starts if x <= l)
+            nxt = lo_t + rank + 1 if rank + 1 < len(bal) else lo_t + 32
+            items[lo_t + rank] = (cls[lo_t + l], ps[l], first, lo_t + l, nxt)
+    # barrier 2; the resolver (warp 0): runs step the float's bits, literal threads and mispredictions replay their terms
+    sb = 0
+    n_items = fallbacks = 0
+    i = 0
     with np.errstate(all="ignore"):
-        for c, p, last in items:
-            if c == LITERAL:
-                for k in range(E):
-                    s = F(s + sq[last * E + k])
+        while i < T:
+            c, p, first, last, i = items[i]
+            n_items += 1
+            ebits = c + 127 if c != LITERAL else 0xFFFFFFFF
+            nb = sb + (p[1] if (sb & 1) else p[0])
+            if (sb >> 23) == ebits and (nb >> 23) == ebits:
+                sb = nb
                 continue
+            fallbacks += c != LITERAL
+            s = np.uint32(sb).view(F)
+            for j in range(first, last + 1):
+                for k in range(E):
+                    s = F(s + sq[j * S + k])
             sb = int(np.float32(s).view(np.uint32))
-            ok = f32_exponent(s) == c and (sb >> 23) != 0
-            if ok:
-                M = (sb & 0x7FFFFF) | 0x800000
-                M2 = M + (p[1] if (M & 1) else p[0])
-                if M2 < (1 << 24):
-                    s = np.uint32((((c + 127) << 23) | (M2 & 0x7FFFFF)) & 0xFFFFFFFF).view(F)
-                else:
-                    ok = False
-            if not ok:
-                first = last
-                while first > 0 and cls[first - 1] == c:
-                    first -= 1
-                for k in range(first * E, (last + 1) * E):
-                    s = F(s + sq[k])
-                fallbacks += 1
-    return s, len(items), fallbacks
+    s = np.uint32(sb).view(F)
+    return s, n_items, fallbacks
 
 
 def cases():
@@ -191,15 +186,41 @@ def cases():
     return out
 
 
+def adversarial(n, rng):
+    """Ties, binade crossings, sums parked next to a power of two, zeros, denormals, huge dynamic range and inf terms at n."""
+    out = []
+    x = rng.standard_normal(n)
+    out.append(x)                                                  # RMSNorm-like squares
+    out.append(np.round(x * 8) / 8)                                # few mantissa bits: exact ties on every binade
+    out.append(2.0 ** rng.integers(-12, 12, n))                    # powers of two: ties and binade crossings
+    z = x.copy(); z[rng.integers(0, n, n // 2)] = 0; out.append(z)  # zeros
+    d = x * 1e-3; d[rng.integers(0, n, n // 4)] = 1e-22; out.append(d)  # squares 1e-44: denormal terms
+    out.append(x * np.exp(rng.standard_normal(n) * 4))            # huge dynamic range
+    i = x.copy(); i[n // 3] = 1e30; out.append(i)                  # 1e60 overflows: an inf term
+    sq = [(v.astype(np.float32) ** 2).astype(np.float32) for v in out]
+    for eps in (-3e-7, 0.0, 3e-7):                                 # the sum parked next to 1.0
+        sq.append(np.full(n, (1.0 + eps) / n, dtype=np.float64).astype(np.float32))
+    return sq
+
+
 if __name__ == "__main__":
-    T = int(sys.argv[1]) if len(sys.argv) > 1 else 1024
+    # default: the adversarial cases at the widths of the decode norms, in the fused norm's chunk layout (seqsum2_stride);
+    # with a thread count argument: the inputs of test_gpu_parity.py in the contiguous layout at that thread count
+    def stride(E):
+        return E + 4 if E % 4 == 0 and (E // 4) % 2 == 0 else E
+    if len(sys.argv) > 1:
+        runs = [(int(sys.argv[1]), t, False) for t in cases()]
+    else:
+        rng = np.random.default_rng(1)
+        runs = [(T, t, True) for n in (2048, 4096, 5120, 8192, 16384) for t in adversarial(n, rng) for T in (256, 512, 1024)]
     bad = 0
-    for i, t in enumerate(cases()):
+    for i, (T, t, strided) in enumerate(runs):
         with np.errstate(all="ignore"):
             ref = np.add.accumulate(t, dtype=np.float32)[-1]
-        got, items, fb = v2(t, T)
+        E = (len(t) + T - 1) // T
+        got, items, fb = v2(t, T, stride(E) if strided else E)
         same = np.float32(got).view(np.uint32) == np.float32(ref).view(np.uint32) or (np.isnan(got) and np.isnan(ref))
         if not same:
             bad += 1
-            print(f"case {i}: n={len(t)} got={got!r} ref={ref!r} items={items} fallbacks={fb}")
-    print(f"T={T}: {bad} mismatches")
+            print(f"case {i}: T={T} n={len(t)} got={got!r} ref={ref!r} items={items} fallbacks={fb}")
+    print(f"{len(runs)} sums: {bad} mismatches")

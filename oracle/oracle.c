@@ -306,6 +306,10 @@ float *oracle_state_logits(ostate *s) { return s->logits; }
 float *oracle_state_x(ostate *s) { return s->x; }
 float *oracle_state_key_cache(ostate *s) { return s->key_cache; }
 float *oracle_state_value_cache(ostate *s) { return s->value_cache; }
+/* read-only views of the last layer's intermediates after a forward: the softmax weights ([n_heads][ctx], entries 0..pos of each
+ * head) and the SwiGLU output that w2 multiplies ([hidden]) */
+float *oracle_state_att(ostate *s) { return s->att; }
+float *oracle_state_hb(ostate *s) { return s->hb; }
 
 /*
  * InferenceCore.forwardJava (InferenceCore.java:50-172) and

@@ -50,7 +50,7 @@ def lib() -> C.CDLL:
         L.oracle_state_new.restype = vp
         L.oracle_state_free.argtypes = [vp]
         L.oracle_state_reset.argtypes = [C.POINTER(OModel), vp]
-        for fn in ("oracle_state_logits", "oracle_state_x", "oracle_state_key_cache", "oracle_state_value_cache"):
+        for fn in ("oracle_state_logits", "oracle_state_x", "oracle_state_key_cache", "oracle_state_value_cache", "oracle_state_att", "oracle_state_hb"):
             getattr(L, fn).argtypes = [vp]
             getattr(L, fn).restype = C.POINTER(f32)
         L.oracle_forward.argtypes = [C.POINTER(OModel), vp, i32, i32, i32]
@@ -278,6 +278,15 @@ class OracleModel:
 
     def x(self) -> np.ndarray:
         return np.ctypeslib.as_array(lib().oracle_state_x(self.state), shape=(self.cfg.dim,)).copy()
+
+    def att(self, n_keys: int) -> np.ndarray:
+        """Softmax weights [n_heads, n_keys] of the last layer of the last forward (which attended n_keys = pos + 1 keys)."""
+        a = np.ctypeslib.as_array(lib().oracle_state_att(self.state), shape=(self.cfg.n_heads, self.cfg.context_length))
+        return a[:, :n_keys].copy()
+
+    def hb(self) -> np.ndarray:
+        """silu(gate) * up of the last layer of the last forward: the activation its down projection multiplies."""
+        return np.ctypeslib.as_array(lib().oracle_state_hb(self.state), shape=(self.cfg.hidden_dim,)).copy()
 
     def close(self):
         if self.state:

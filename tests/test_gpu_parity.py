@@ -259,7 +259,8 @@ def test_long_context_score_row_in_global_memory(pkg, orc, make_model):
                                                   ("tiny-llama", "Q8_0", 20000, "graph"), ("tiny-qwen3", "Q8_0", 20000, "persistent")])
 def test_deep_context_bit_exact(pkg, orc, make_model, shape, quant, ctx, mode):
     """Depth: 700 positions.  Past 128 keys the attention kernel's score and weighted-sum loops run several software-pipelined passes
-    (next pass's K / V rows in flight during the current chain), from 512 keys on the softmax sum is the exact parallel accumulator, the
+    (next pass's K / V rows in flight during the current chain), from 512 keys on the persistent kernel's softmax sum is the exact parallel
+    accumulator (the graph's attention kernel, which the batched and multi-position steps share, sums on one thread at every length), the
     K/V rows are bulk-prefetched into L2 ahead of the dependency wait; with a 20000-token context the score row lives in global memory.
     Logits are compared on both sides of every switch-over (127|128|129 keys, 255|256|257, 511|512|513, ...) and at the end; the KV cache
     of all 700 positions must be bit-equal.  Head sizes 64 (Llama), 128 (Qwen3: q/k norm, NeoX), 96 (Phi-3)."""

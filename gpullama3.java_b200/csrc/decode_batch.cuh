@@ -1,6 +1,7 @@
-// decode_batch.cuh -- the batched decode step: up to SMB_MAX_ROWS independent sequences advance by one token each while every
-// weight matrix streams from HBM once (b200_forward_decode_batch, plan.cu).  Each dot product keeps its own row, its own
-// activation vector and its own block order, so every row stays bit-identical to the single-sequence decode (and the CPU path).
+// decode_batch.cuh -- the batched step: up to SMB_MAX_ROWS rows, each a (slot, token, position), advance together while every
+// weight matrix streams from HBM once (b200_forward_decode_batch, b200_forward_decode_multi, b200_forward_step and the exact
+// prefills, plan.cu).  Each dot product keeps its own row, its own activation vector and its own block order, so every row stays
+// bit-identical to the single-sequence decode (and the CPU path).
 //
 //   k_rmsnorm_quant_batch      one CTA per row: rmsnorm_quant_row (decode_kernels.cuh) on that row's x / token / outputs
 //   k_stream_matvec_q8_batch   the tile-major Q8_0 stream of stream_matvec.cuh; each tile is applied to every row's activation

@@ -50,10 +50,10 @@ struct TokenGraphs {
     Graph decode, prefill, trace;
 };
 
-// The forms of the batched step (enqueue_batch).  PREFILL*: a step of the exact prefills, its rows from the call's schedule and
-// without the classifier.  *_SPLIT, *_OWN and MULTI*: rows may share a sequence.  *_OWN: the K / V target is the plan's own cache.
-// b200_forward_step runs DECODE (distinct slots) and MULTI (a slot repeats) with the classifier over its first e rows only.
-enum BatchKind { BK_DECODE, BK_PREFILL, BK_PREFILL_SPLIT, BK_PREFILL_OWN, BK_MULTI, BK_MULTI_OWN, BK_KINDS };
+// The form of a batched step (enqueue_batch), three independent bits.  SCHED: a step of the exact prefills, its rows copied from
+// the call's schedule by k_batch_rows_next, without the classifier.  SPLIT: a slot repeats, so the attention runs as
+// k_rope_kv_batch + k_attention_cached_rows.  OWN: the K / V target is the plan's own cache instead of the decode slots.
+enum StepForm { SCHED = 1, SPLIT = 2, OWN = 4, STEP_FORMS = 8 };
 
 } // namespace
 
@@ -183,8 +183,8 @@ struct b200_plan {
         BatchRows *sched = nullptr;
         int *step = nullptr;
         int *smp_indices = nullptr; // the sampler's candidate lists, [row][vocab]
-        Graph g[BK_KINDS][SMB_MAX_ROWS + 1][SMB_MAX_ROWS + 1]; // [kind][rows][rows that run the classifier]
-        int last_launches = 0; // of the last b200_forward_decode_batch / b200_forward_step graph
+        Graph g[STEP_FORMS][SMB_MAX_ROWS + 1][SMB_MAX_ROWS + 1]; // [form][rows][rows that run the classifier]
+        int last_launches = 0; // of the last step with the classifier (batch_step)
         float last_ms = 0.f;
     } bt;
 };
@@ -944,14 +944,11 @@ int launch_stream_batch(b200_plan *p, const TileMat &W, int n, const int8_t *xq,
     return launch_k(p, p->use_pdl, k_stream_matvec_q8_batch<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L);
 }
 
-// One forward step of n rows: the single-sequence graph's kernel sequence, every launch serving all n rows.  prefill: a step of
-// the exact prefills -- the rows come from the call's schedule (k_batch_rows_next).  The final norm, lm_head and argmax run over
-// the first e rows only (e = 0: not at all, as in the prefill kinds).  split: rows may share a sequence, so the attention runs as
-// k_rope_kv_batch + k_attention_cached_rows (one more launch per layer).  own: the K / V target is the plan's cache (key_cache /
-// value_cache, slot 0's layout) instead of the decode slots.
-int enqueue_batch(b200_plan *p, int n, int e, BatchKind kind, int *launches) {
-    const bool prefill = kind == BK_PREFILL || kind == BK_PREFILL_SPLIT || kind == BK_PREFILL_OWN;
-    const bool split = kind != BK_DECODE && kind != BK_PREFILL, own = kind == BK_PREFILL_OWN || kind == BK_MULTI_OWN;
+// One forward step of n rows in the given form (StepForm bits): the single-sequence graph's kernel sequence, every launch serving
+// all n rows.  The final norm, lm_head and argmax run over the first e rows only (e = 0: not at all, as in the prefills).  SPLIT
+// costs one more launch per layer.  OWN writes key_cache / value_cache, whose layout is slot 0's.
+int enqueue_batch(b200_plan *p, int n, int e, int form, int *launches) {
+    const bool sched = form & SCHED, split = form & SPLIT, own = form & OWN;
     const b200_config &c = p->cfg;
     auto &B = p->bt;
     const bool pdl = p->use_pdl;
@@ -961,14 +958,14 @@ int enqueue_batch(b200_plan *p, int n, int e, BatchKind kind, int *launches) {
     TpCtx solo{};
     solo.n = 1;
     int k = 0, rc;
-    if (prefill) {
+    if (sched) {
         k_batch_rows_next<<<1, 32, 0, p->stream>>>(B.sched, B.step, B.rows);
         CK(cudaGetLastError());
         k++;
     }
     auto norm = [&](bool embed, const float *w, int rows) {
-        auto go = [&](auto kern) { // the first norm of a prefill step waits for k_batch_rows_next in full: the rows are read before any PDL wait
-            return launch_k(p, pdl && !(prefill && embed), kern, dim3(rows), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, p->mup.embedding_scale, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
+        auto go = [&](auto kern) { // the first norm of a SCHED step waits for k_batch_rows_next in full: the rows are read before any PDL wait
+            return launch_k(p, pdl && !(sched && embed), kern, dim3(rows), dim3(NORM_THREADS), norm_smem, B.x, (const BatchRows *)B.rows, p->emb, p->mup.embedding_scale, w, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo);
         };
         k++;
         return embed ? go(k_rmsnorm_quant_batch<true>) : go(k_rmsnorm_quant_batch<false>);
@@ -1012,19 +1009,29 @@ int enqueue_batch(b200_plan *p, int n, int e, BatchKind kind, int *launches) {
     return B200_OK;
 }
 
-// The step graph of `kind` for n rows, e of them with the classifier, captured on first use.
-int batch_graph(b200_plan *p, BatchKind kind, int n, int e, const Graph **out) {
-    Graph &g = p->bt.g[kind][n][e];
+// The step graph of `form` for n rows, e of them with the classifier, captured on first use.
+int batch_graph(b200_plan *p, int form, int n, int e, const Graph **out) {
+    Graph &g = p->bt.g[form][n][e];
     int rc;
-    if (!g.exec && (rc = capture(p, g, [&](int *launches) { return enqueue_batch(p, n, e, kind, launches); }))) return rc;
+    if (!g.exec && (rc = capture(p, g, [&](int *launches) { return enqueue_batch(p, n, e, form, launches); }))) return rc;
     *out = &g;
     return B200_OK;
 }
 
+// The form of a step of n rows writing the decode slots, or with own the plan's cache (every row slot 0): SPLIT when a slot
+// repeats, because k_attention_batch writes a row's K / V inside its attention CTA and rows of one sequence would race.
+int step_form(const BatchRows &r, int n, bool own) {
+    const int target = own ? OWN : 0;
+    for (int i = 1; i < n; i++)
+        for (int j = 0; j < i; j++)
+            if (r.slot[j] == r.slot[i]) return target | SPLIT;
+    return target;
+}
+
 void batch_free(b200_plan *p) {
     auto &B = p->bt;
-    for (auto &by_kind : B.g)
-        for (auto &by_rows : by_kind)
+    for (auto &by_form : B.g)
+        for (auto &by_rows : by_form)
             for (Graph &g : by_rows) destroy(g);
     for (void *d : B.allocs) cudaFree(d);
     if (B.h_rows) cudaFreeHost(B.h_rows);
@@ -1084,21 +1091,15 @@ int multi_ready(b200_plan *p) {
 }
 
 // Enqueues the steps of one call back to back without the classifier: the schedule is uploaded once and k_batch_rows_next
-// feeds each step its entry, so the caller synchronises once.  p->ev0 / ev1 bracket the steps.  own: every row writes the plan's cache (slot 0); otherwise a
-// step whose rows name distinct slots runs the b200_prefill_slots graph, and one with a repeated slot the split form.
+// feeds each step its entry, so the caller synchronises once.  p->ev0 / ev1 bracket the steps.  own: every row writes the plan's
+// cache (slot 0) instead of the decode slots.
 int run_steps(b200_plan *p, const std::vector<BatchRows> &sched, const std::vector<int> &nrows, bool own, int *launches) {
     auto &B = p->bt;
     const int steps = (int)sched.size();
     std::vector<const Graph *> graphs(steps);
     int rc;
-    for (int s = 0; s < steps; s++) {
-        bool split = false;
-        for (int i = 0; i < nrows[s] && !split; i++)
-            for (int j = 0; j < i; j++)
-                if (sched[s].slot[j] == sched[s].slot[i]) { split = true; break; }
-        const BatchKind kind = own ? BK_PREFILL_OWN : split ? BK_PREFILL_SPLIT : BK_PREFILL;
-        if ((rc = batch_graph(p, kind, nrows[s], 0, &graphs[s]))) return rc;
-    }
+    for (int s = 0; s < steps; s++)
+        if ((rc = batch_graph(p, SCHED | step_form(sched[s], nrows[s], own), nrows[s], 0, &graphs[s]))) return rc;
     CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
     CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
     CK(cudaEventRecord(p->ev0, p->stream));
@@ -1886,6 +1887,74 @@ int check_pos(b200_plan *p, int token, int pos) {
     return B200_OK;
 }
 
+// The index of the first of tokens[0, n) outside the vocabulary, or -1; each caller names it in its own terms.
+int bad_token(const b200_plan *p, const int32_t *tokens, int n) {
+    for (int i = 0; i < n; i++)
+        if (tokens[i] < 0 || tokens[i] >= p->cfg.vocab_size) return i;
+    return -1;
+}
+
+// The refusals b200_forward_decode_batch and b200_forward_step share for row i: slot, token and position out of range, and an
+// emitting row's bad sampling triple.
+int check_row(b200_plan *p, int i, const b200_step_row &r) {
+    const b200_config &c = p->cfg;
+    if (r.slot < 0 || r.slot >= p->bt.n_slots) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d out of range (%d slots)", i, r.slot, p->bt.n_slots);
+    if (bad_token(p, &r.token, 1) >= 0) return fail(p, B200_ERR_BAD_ARG, "row %d: token %d out of range", i, r.token);
+    if (r.position < 0 || r.position >= c.context_length)
+        return fail(p, B200_ERR_BAD_ARG, "row %d: position %d outside the KV cache (%d)", i, r.position, c.context_length);
+    if (r.emit && (!(r.temperature >= 0.0f) || !(r.uniform01 >= 0.0f && r.uniform01 < 1.0f)))
+        return fail(p, B200_ERR_BAD_ARG, "row %d: temperature must be >= 0 and the uniform number in [0, 1)", i);
+    return B200_OK;
+}
+
+// One batched step with the classifier over checked rows: against the decode slots, or with own the plan's cache (every row
+// slot 0).  The emitting rows go first (stable), so the final norm, lm_head and argmax run over rows [0, e) and no kernel indexes
+// through a row map; their ids and logits return to the caller's row order, ids -1 where a row does not emit.  Rows with a
+// temperature run the device sampler, all in one launch.  b200_batch_info reports the step.
+int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, int32_t *ids_out, float *logits) {
+    const b200_config &c = p->cfg;
+    auto &B = p->bt;
+    int order[SMB_MAX_ROWS], e = 0;
+    for (int i = 0; i < n; i++)
+        if (rows[i].emit) order[e++] = i;
+    for (int i = 0, k = e; i < n; i++)
+        if (!rows[i].emit) order[k++] = i;
+    BatchRows br{};
+    for (int k = 0; k < n; k++) {
+        const b200_step_row &r = rows[order[k]];
+        br.token[k] = r.token; br.pos[k] = r.position; br.slot[k] = r.slot;
+    }
+    int rc;
+    const Graph *g;
+    if ((rc = batch_graph(p, step_form(br, n, own), n, e, &g))) return rc;
+    *B.h_rows = br;
+    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaEventRecord(p->ev0, p->stream));
+    CK(cudaGraphLaunch(g->exec, p->stream));
+    CK(cudaEventRecord(p->ev1, p->stream));
+    const size_t vpad = (size_t)sampler_padded(c.vocab_size);
+    if (logits) // before the sampler turns sampled rows into probabilities
+        for (int k = 0; k < e; k++)
+            CK(cudaMemcpyAsync(logits + (size_t)order[k] * c.vocab_size, B.logits + k * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
+    int m = 0, srow[SMB_MAX_ROWS];
+    float t[SMB_MAX_ROWS], tp[SMB_MAX_ROWS], u[SMB_MAX_ROWS];
+    for (int k = 0; k < e; k++) {
+        const b200_step_row &r = rows[order[k]];
+        if (r.temperature == 0.0f) continue; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed
+        srow[m] = k; t[m] = r.temperature; tp[m] = r.topp; u[m] = r.uniform01;
+        m++;
+    }
+    if (m && (rc = launch_sample_rows(p, m, srow, t, tp, u))) return rc;
+    if (e) CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)e * 4, cudaMemcpyDeviceToHost, p->stream));
+    if (m) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)e * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
+    for (int i = 0; i < n; i++) ids_out[i] = -1;
+    for (int k = 0; k < e; k++) ids_out[order[k]] = rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
+    CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
+    B.last_launches = g->launches;
+    return B200_OK;
+}
+
 // Device memory and the result code of an entry point without a plan.  ok() keeps the first failure (an allocation failure is
 // B200_ERR_OOM, any other B200_ERR_CUDA) and answers whether everything so far succeeded; the allocations are freed at scope exit.
 struct Scratch {
@@ -2083,8 +2152,7 @@ int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, i
     if (!p->graph.prefill.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     if (p->prefill_batch > 1 && n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "chunk of %d tokens exceeds prefill_batch_size %d", n, p->prefill_batch);
     if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache", start_pos, start_pos + n - 1);
-    for (int i = 0; i < n; i++)
-        if (tokens[i] < 0 || tokens[i] >= p->cfg.vocab_size) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
+    if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
     CK(cudaSetDevice(p->device));
     if ((p->prefill.ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE) ||
         (p->prefill.q8_ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE_W8A16)) { // tensor-core GEMM path (prefill.cuh)
@@ -2128,8 +2196,7 @@ int b200_decode_sequence(b200_plan *p, const int32_t *tokens, int32_t n, int32_t
     if (n > p->seq_cap) return fail(p, B200_ERR_BAD_ARG, "sequence of %d steps exceeds capacity %d", n, p->seq_cap);
     if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache (%d)", start_pos, start_pos + n - 1, p->cfg.context_length);
     int nt = feedback ? 1 : n;
-    for (int i = 0; i < nt; i++)
-        if (tokens[i] < 0 || tokens[i] >= p->cfg.vocab_size) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
+    if (const int i = bad_token(p, tokens, nt); i >= 0) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
     CK(cudaSetDevice(p->device));
     memcpy(p->h_ids, tokens, (size_t)nt * 4);
     CK(cudaMemcpyAsync(p->seq_tokens, p->h_ids, (size_t)nt * 4, cudaMemcpyHostToDevice, p->stream));
@@ -2250,47 +2317,17 @@ int b200_forward_decode_batch(b200_plan *p, int32_t n, const int32_t *slots, con
     if (!B.n_slots) return fail(p, B200_ERR_STATE, "no decode slots: call b200_set_decode_slots first");
     if (!slots || !tokens || !positions || !ids_out) return fail(p, B200_ERR_BAD_ARG, "slots, tokens, positions and ids_out must not be NULL");
     if (n < 1 || n > B.n_slots) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (the plan's decode slots)", n, B.n_slots);
-    const b200_config &c = p->cfg;
+    b200_step_row r[SMB_MAX_ROWS];
+    int rc;
     for (int i = 0; i < n; i++) {
-        if (slots[i] < 0 || slots[i] >= B.n_slots) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d out of range (%d slots)", i, slots[i], B.n_slots);
         for (int j = 0; j < i; j++)
             if (slots[j] == slots[i]) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d repeats row %d's", i, slots[i], j);
-        if (tokens[i] < 0 || tokens[i] >= c.vocab_size) return fail(p, B200_ERR_BAD_ARG, "row %d: token %d out of range", i, tokens[i]);
-        if (positions[i] < 0 || positions[i] >= c.context_length)
-            return fail(p, B200_ERR_BAD_ARG, "row %d: position %d outside the KV cache (%d)", i, positions[i], c.context_length);
-        if (sampling) {
-            const float t = sampling[3 * i], u = sampling[3 * i + 2];
-            if (!(t >= 0.0f) || !(u >= 0.0f && u < 1.0f))
-                return fail(p, B200_ERR_BAD_ARG, "row %d: temperature must be >= 0 and the uniform number in [0, 1)", i);
-        }
+        const float *s = sampling ? sampling + 3 * i : nullptr;
+        r[i] = b200_step_row{slots[i], tokens[i], positions[i], 1, s ? s[0] : 0.0f, s ? s[1] : 0.0f, s ? s[2] : 0.0f};
+        if ((rc = check_row(p, i, r[i]))) return rc;
     }
     CK(cudaSetDevice(p->device));
-    int rc;
-    const Graph *g;
-    if ((rc = batch_graph(p, BK_DECODE, n, n, &g))) return rc;
-    for (int i = 0; i < n; i++) { B.h_rows->token[i] = tokens[i]; B.h_rows->pos[i] = positions[i]; B.h_rows->slot[i] = slots[i]; }
-    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
-    CK(cudaEventRecord(p->ev0, p->stream));
-    CK(cudaGraphLaunch(g->exec, p->stream));
-    CK(cudaEventRecord(p->ev1, p->stream));
-    const size_t vpad = (size_t)sampler_padded(c.vocab_size);
-    if (logits) // before the sampler turns sampled rows into probabilities
-        for (int i = 0; i < n; i++) CK(cudaMemcpyAsync(logits + (size_t)i * c.vocab_size, B.logits + i * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
-    int m = 0, row[SMB_MAX_ROWS];
-    float t[SMB_MAX_ROWS], tp[SMB_MAX_ROWS], u[SMB_MAX_ROWS];
-    for (int i = 0; i < n; i++) {
-        if (!sampling || sampling[3 * i] == 0.0f) continue; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed
-        row[m] = i; t[m] = sampling[3 * i]; tp[m] = sampling[3 * i + 1]; u[m] = sampling[3 * i + 2];
-        m++;
-    }
-    if (m && (rc = launch_sample_rows(p, m, row, t, tp, u))) return rc;
-    CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)n * 4, cudaMemcpyDeviceToHost, p->stream));
-    if (m) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)n * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
-    CK(cudaStreamSynchronize(p->stream));
-    for (int i = 0; i < n; i++) ids_out[i] = (sampling && sampling[3 * i] != 0.0f) ? B.h_out[SMB_MAX_ROWS + 8 * i] : B.h_out[i];
-    CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
-    B.last_launches = g->launches;
-    return B200_OK;
+    return batch_step(p, n, r, false, ids_out, logits);
 }
 
 int b200_slot_reset(b200_plan *p, int32_t slot) {
@@ -2433,9 +2470,8 @@ int b200_prefill_slots(b200_plan *p, int32_t n_seqs, const int32_t *slots, const
     }
     if (total && !tokens) return fail(p, B200_ERR_BAD_ARG, "tokens must not be NULL");
     for (int i = 0; i < n_seqs; i++)
-        for (int j = 0; j < lengths[i]; j++)
-            if (tokens[off[i] + j] < 0 || tokens[off[i] + j] >= c.vocab_size)
-                return fail(p, B200_ERR_BAD_ARG, "sequence %d: token %d (index %d) out of range", i, tokens[off[i] + j], j);
+        if (const int j = bad_token(p, tokens + off[i], lengths[i]); j >= 0)
+            return fail(p, B200_ERR_BAD_ARG, "sequence %d: token %d (index %d) out of range", i, tokens[off[i] + j], j);
     const PrefillCtx &pc = p->prefill;
     const bool tc = (pc.ready && pc.mode == B200_PREFILL_TENSOR_CORE) || (pc.q8_ready && pc.mode == B200_PREFILL_TENSOR_CORE_W8A16);
     if (tc && total > p->prefill_batch) {
@@ -2465,27 +2501,17 @@ int b200_forward_decode_multi(b200_plan *p, int32_t slot, int32_t n, const int32
     if (!tokens || !ids_out) return fail(p, B200_ERR_BAD_ARG, "tokens and ids_out must not be NULL");
     if (n < 1 || n > R) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (b200_decode_multi_rows)", n, R);
     if (slot < -1 || slot >= B.n_slots) return fail(p, B200_ERR_BAD_ARG, "slot %d out of range (%d slots; -1 is the plan's own cache)", slot, B.n_slots);
+    if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "row %d: token %d out of range", i, tokens[i]);
+    b200_step_row r[SMB_MAX_ROWS];
     for (int i = 0; i < n; i++) {
-        if (tokens[i] < 0 || tokens[i] >= c.vocab_size) return fail(p, B200_ERR_BAD_ARG, "row %d: token %d out of range", i, tokens[i]);
         if (start_pos < 0 || (int64_t)start_pos + i >= c.context_length)
             return fail(p, B200_ERR_BAD_ARG, "row %d: position %lld outside the KV cache (%d)", i, (long long)start_pos + i, c.context_length);
+        r[i] = b200_step_row{slot < 0 ? 0 : slot, tokens[i], start_pos + i, 1, 0.0f, 0.0f, 0.0f};
     }
     CK(cudaSetDevice(p->device));
     int rc;
     if ((rc = multi_ready(p))) return rc;
-    const bool own = slot < 0;
-    const Graph *g;
-    if ((rc = batch_graph(p, own ? BK_MULTI_OWN : BK_MULTI, n, n, &g))) return rc;
-    for (int i = 0; i < n; i++) { B.h_rows->token[i] = tokens[i]; B.h_rows->pos[i] = start_pos + i; B.h_rows->slot[i] = own ? 0 : slot; }
-    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
-    CK(cudaGraphLaunch(g->exec, p->stream));
-    const size_t vpad = (size_t)sampler_padded(c.vocab_size);
-    if (logits)
-        for (int i = 0; i < n; i++) CK(cudaMemcpyAsync(logits + (size_t)i * c.vocab_size, B.logits + i * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
-    CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)n * 4, cudaMemcpyDeviceToHost, p->stream));
-    CK(cudaStreamSynchronize(p->stream));
-    memcpy(ids_out, B.h_out, (size_t)n * 4);
-    return B200_OK;
+    return batch_step(p, n, r, slot < 0, ids_out, logits);
 }
 
 int b200_forward_step(b200_plan *p, int32_t n, const b200_step_row *rows, int32_t *ids_out, float *logits) {
@@ -2494,64 +2520,19 @@ int b200_forward_step(b200_plan *p, int32_t n, const b200_step_row *rows, int32_
     auto &B = p->bt;
     if (!B.n_slots) return fail(p, B200_ERR_STATE, "no decode slots: call b200_set_decode_slots first");
     if (!rows || !ids_out) return fail(p, B200_ERR_BAD_ARG, "rows and ids_out must not be NULL");
-    const b200_config &c = p->cfg;
     const int R = batch_max_rows(p);
     if (n < 1 || n > R) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (b200_decode_multi_rows)", n, R);
-    bool split = false;
+    int rc;
     for (int i = 0; i < n; i++) {
         const b200_step_row &r = rows[i];
-        if (r.slot < 0 || r.slot >= B.n_slots) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d out of range (%d slots)", i, r.slot, B.n_slots);
-        if (r.token < 0 || r.token >= c.vocab_size) return fail(p, B200_ERR_BAD_ARG, "row %d: token %d out of range", i, r.token);
-        if (r.position < 0 || r.position >= c.context_length)
-            return fail(p, B200_ERR_BAD_ARG, "row %d: position %d outside the KV cache (%d)", i, r.position, c.context_length);
-        for (int j = 0; j < i; j++) {
-            if (rows[j].slot != r.slot) continue;
-            split = true;
-            if (rows[j].position == r.position) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d position %d repeats row %d's", i, r.slot, r.position, j);
-        }
         if (r.emit != 0 && r.emit != 1) return fail(p, B200_ERR_BAD_ARG, "row %d: emit must be 0 or 1 (got %d)", i, r.emit);
-        if (r.emit && (!(r.temperature >= 0.0f) || !(r.uniform01 >= 0.0f && r.uniform01 < 1.0f)))
-            return fail(p, B200_ERR_BAD_ARG, "row %d: temperature must be >= 0 and the uniform number in [0, 1)", i);
+        if ((rc = check_row(p, i, r))) return rc;
+        for (int j = 0; j < i; j++)
+            if (rows[j].slot == r.slot && rows[j].position == r.position)
+                return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d position %d repeats row %d's", i, r.slot, r.position, j);
     }
-    // The emitting rows first, so the classifier runs over rows [0, e) and no kernel indexes through a row map.
-    int order[SMB_MAX_ROWS], e = 0;
-    for (int i = 0; i < n; i++)
-        if (rows[i].emit) order[e++] = i;
-    for (int i = 0, k = e; i < n; i++)
-        if (!rows[i].emit) order[k++] = i;
     CK(cudaSetDevice(p->device));
-    int rc;
-    const Graph *g;
-    if ((rc = batch_graph(p, split ? BK_MULTI : BK_DECODE, n, e, &g))) return rc;
-    for (int k = 0; k < n; k++) {
-        const b200_step_row &r = rows[order[k]];
-        B.h_rows->token[k] = r.token; B.h_rows->pos[k] = r.position; B.h_rows->slot[k] = r.slot;
-    }
-    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
-    CK(cudaEventRecord(p->ev0, p->stream));
-    CK(cudaGraphLaunch(g->exec, p->stream));
-    CK(cudaEventRecord(p->ev1, p->stream));
-    const size_t vpad = (size_t)sampler_padded(c.vocab_size);
-    if (logits) // before the sampler turns sampled rows into probabilities
-        for (int k = 0; k < e; k++)
-            CK(cudaMemcpyAsync(logits + (size_t)order[k] * c.vocab_size, B.logits + k * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
-    int m = 0, srow[SMB_MAX_ROWS];
-    float t[SMB_MAX_ROWS], tp[SMB_MAX_ROWS], u[SMB_MAX_ROWS];
-    for (int k = 0; k < e; k++) {
-        const b200_step_row &r = rows[order[k]];
-        if (r.temperature == 0.0f) continue; // FloatTensor.argmax, already computed
-        srow[m] = k; t[m] = r.temperature; tp[m] = r.topp; u[m] = r.uniform01;
-        m++;
-    }
-    if (m && (rc = launch_sample_rows(p, m, srow, t, tp, u))) return rc;
-    if (e) CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)e * 4, cudaMemcpyDeviceToHost, p->stream));
-    if (m) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)e * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
-    CK(cudaStreamSynchronize(p->stream));
-    for (int i = 0; i < n; i++) ids_out[i] = -1;
-    for (int k = 0; k < e; k++) ids_out[order[k]] = rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
-    CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
-    B.last_launches = g->launches;
-    return B200_OK;
+    return batch_step(p, n, rows, false, ids_out, logits);
 }
 
 int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step) {

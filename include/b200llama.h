@@ -347,8 +347,8 @@ typedef struct b200_step_row {
 int b200_forward_step(b200_plan *plan, int32_t n, const b200_step_row *rows, int32_t *ids_out /* n; -1 where emit == 0 */,
                       float *logits /* nullable, n x vocab; rows with emit == 0 are not written */);
 
-/* Decode slots, kernels of the last batched step (b200_forward_decode_batch or b200_forward_step, whichever ran last) and its
- * device milliseconds (CUDA events around the graph); any pointer may be NULL. */
+/* Decode slots, kernels of the last batched step with a classifier (b200_forward_decode_batch, b200_forward_decode_multi or
+ * b200_forward_step, whichever ran last) and its device milliseconds (CUDA events around the graph); any pointer may be NULL. */
 int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step);
 
 /* Test/diagnostic read-back of a named device buffer into host memory.  Names:

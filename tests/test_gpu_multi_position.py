@@ -140,6 +140,8 @@ def test_forward_decode_multi_bit_exact(pkg, orc, make_model, shape):
             pos = 0
             for n in range(1, R + 1):
                 ids, lg = plan.forward_decode_multi(slot, stream[pos:pos + n], pos, logits=True)
+                # one row takes the plain form; several rows of one sequence the split attention, one more launch per layer
+                assert plan.batch_info()[1] == (7 if n == 1 else 8) * c.n_layers + 3, (slot, n)
                 for i in range(n):
                     assert_bit_equal(lg[i], ref[pos + i], f"slot {slot}, n {n}, row {i}")
                     assert ids[i] == orc.argmax(ref[pos + i])

@@ -46,30 +46,45 @@ template <int TYPE> __device__ __forceinline__ void kq_read32(const unsigned cha
     }
 }
 
-// One thread per Q8_0 block; src = K-quant super-blocks (contiguous), dst = GGUF Q8_0 blocks (34 bytes each, 2-byte aligned).
-template <int TYPE> __global__ void k_requant_kquant(const unsigned char *__restrict__ src, unsigned char *__restrict__ dst, long long n_blocks) {
-    const long long blk = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (blk >= n_blocks) return;
+// The Q8_0 block the reference builds from elements [32 * sub, 32 * sub + 32) of super-block b: q[k] holds quants 4k..4k+3 packed
+// little-endian (the byte order of the GGUF block, and dp4a's operand order), the return value is the f16 scale as stored.  Shared by
+// the load-time re-quantiser and the resident weight streams (stream_matvec.cuh), so both produce the same bytes.
+template <int TYPE> __device__ __forceinline__ __half kq_q8_block(const unsigned char *b, int sub, int (&q)[8]) {
     float v[32];
-    kq_read32<TYPE>(src + (blk >> 3) * kq_block_bytes(TYPE), (int)(blk & 7), v);
+    kq_read32<TYPE>(b, sub, v);
     float max_abs = 0.0f;
 #pragma unroll
     for (int i = 0; i < 32; i++) { const float a = fabsf(v[i]); max_abs = a > max_abs ? a : max_abs; } // Math.max(maxAbs, Math.abs(x))
     const float scale = __fdiv_rn(max_abs, 127.0f);
     const float inv = scale != 0.0f ? __fdiv_rn(1.0f, scale) : 0.0f;
-    unsigned short *o = reinterpret_cast<unsigned short *>(dst + blk * 34);
-    o[0] = __half_as_ushort(__float2half_rn(scale));
 #pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-        int q[2];
+    for (int w = 0; w < 8; w++) {
+        unsigned packed = 0u;
 #pragma unroll
-        for (int k = 0; k < 2; k++) {
-            const float t = __fmul_rn(v[i + k], inv), f = floorf(t);
+        for (int k = 0; k < 4; k++) {
+            const float t = __fmul_rn(v[4 * w + k], inv), f = floorf(t);
             int r = (int)f + (__fsub_rn(t, f) >= 0.5f ? 1 : 0);
             if (t != t) r = 0;
-            q[k] = r < -128 ? -128 : (r > 127 ? 127 : r);
+            r = r < -128 ? -128 : (r > 127 ? 127 : r);
+            packed |= (unsigned)(r & 0xFF) << (8 * k);
         }
-        o[1 + (i >> 1)] = (unsigned short)((q[0] & 0xFF) | ((q[1] & 0xFF) << 8));
+        q[w] = (int)packed;
+    }
+    return __float2half_rn(scale);
+}
+
+// One thread per Q8_0 block; src = K-quant super-blocks (contiguous), dst = GGUF Q8_0 blocks (34 bytes each, 2-byte aligned).
+template <int TYPE> __global__ void k_requant_kquant(const unsigned char *__restrict__ src, unsigned char *__restrict__ dst, long long n_blocks) {
+    const long long blk = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (blk >= n_blocks) return;
+    int q[8];
+    const __half sc = kq_q8_block<TYPE>(src + (blk >> 3) * kq_block_bytes(TYPE), (int)(blk & 7), q);
+    unsigned short *o = reinterpret_cast<unsigned short *>(dst + blk * 34);
+    o[0] = __half_as_ushort(sc);
+#pragma unroll
+    for (int w = 0; w < 8; w++) {
+        o[1 + 2 * w] = (unsigned short)((unsigned)q[w] & 0xFFFFu);
+        o[2 + 2 * w] = (unsigned short)((unsigned)q[w] >> 16);
     }
 }
 

@@ -96,6 +96,10 @@ struct b200_plan {
     bool fuse_norm = false; // single-GPU Q8_0 streams: QKV, gate/up and lm_head compute their RMSNorm themselves (k_stream_matvec_q8_norm)
     int kflags = 0; // KF_* (common.cuh): what the attention prologues do for this architecture
     size_t kq_off = 0; // K-quant files: offset of the raw (K-quant bytes) area inside each staging buffer; 0 = no K-quant tensor in the file
+    // K-quant files whose Q8_0 expansion does not fit the device (weight_policy): every stream whose sources share one K-quant format
+    // keeps the raw super-blocks (TileMat::fmt); w_bytes is the plan's weight footprint, w8_bytes the one of its all-Q8_0 form
+    bool resident = false;
+    int64_t w_bytes = 0, w8_bytes = 0;
     bool use_f16_stream = false; // FP16 plans: per-warp bulk-copy rings (stream_matvec_f16.cuh) instead of k_matvec_f16
     bool f16_copies = false; // Q8_0 plan that also holds f16 weight matrices for the tensor-core prefill
     int n_sms = 148;
@@ -410,11 +414,43 @@ int upload_matrix(b200_plan *p, const b200_tensor *t, int rows, int cols, DevMat
     return B200_OK;
 }
 
-// Upload up to three stacked GGUF Q8_0 matrices (or the gate/up pair) into tile-major layout.
+const size_t SMV_SMEM_BUDGET_MAX = 96 * 1024;
+
+// Segments, unit size and format of a tile-major stream (fmt 0: Q8_0 tiles; a K-quant type: resident tiles).
+TileMat tile_geometry(int rows, int cols, int fmt) {
+    TileMat t{};
+    t.rows = rows;
+    t.cols = cols;
+    t.fmt = fmt;
+    t.nseg = smv_pick_nseg(cols, fmt ? 256 : 32);
+    t.seg = t.nseg ? cols / t.nseg : 0;
+    t.unit_bytes = smv_unit_bytes(t.seg, fmt);
+    return t;
+}
+int64_t tile_bytes(const TileMat &t) { return (int64_t)tile_groups(t) * 4 * t.nseg * t.unit_bytes; }
+
+// The format a stream of these stacked sources keeps on a resident plan: their common K-quant type when every present source has
+// it and the resident layout leaves at least 3 ring stages; else 0 (the stream is re-quantised to Q8_0 tiles at upload).
+int resident_fmt(const b200_tensor *const ts[3], const int rs[3], int rows, int cols) {
+    int fmt = -1;
+    for (int k = 0; k < 3; k++) {
+        if (!rs[k]) continue;
+        if (!ts[k] || !kq_is_kquant(ts[k]->ggml_type) || (fmt >= 0 && ts[k]->ggml_type != fmt)) return 0;
+        fmt = ts[k]->ggml_type;
+    }
+    if (fmt < 0 || cols % 256) return 0;
+    const TileMat t = tile_geometry(rows, cols, fmt);
+    return t.nseg && smv_layout(cols, t.seg, SMV_SMEM_BUDGET_MAX, fmt).stages >= 3 ? fmt : 0;
+}
+
+// Upload up to three stacked GGUF Q8_0 or K-quant matrices (or the gate/up pair) into tile-major layout: Q8_0 tiles, or on a
+// resident plan resident tiles when resident_fmt allows.
 int upload_tiles(b200_plan *p, const b200_tensor *t0, const b200_tensor *t1, const b200_tensor *t2, int r0, int r1, int r2, int cols,
                  bool gateup, TileMat &out, const int *row0 = nullptr, const int *full = nullptr) {
     const b200_tensor *ts[3] = {t0, t1, t2};
     int rs[3] = {r0, r1, r2};
+    const int rows = gateup ? r0 + r1 : r0 + r1 + r2;
+    const int fmt = p->resident ? resident_fmt(ts, rs, rows, cols) : 0;
     RepackSrc src;
     size_t off = 0;
     int rc;
@@ -439,9 +475,10 @@ int upload_tiles(b200_plan *p, const b200_tensor *t0, const b200_tensor *t1, con
         if (kq && (cols % 256 || !p->kq_off)) return fail(p, B200_ERR_BAD_ARG, "K-quant tensor %s: rows must be multiples of 256 elements", t->name);
         if (n_elems(t) != (int64_t)full_rows * cols) return fail(p, B200_ERR_BAD_ARG, "tensor %s has %lld elements, expected %lld", t->name, (long long)n_elems(t), (long long)full_rows * cols);
         if (first < 0 || first + rs[k] > full_rows) return fail(p, B200_ERR_BAD_ARG, "row range of tensor %s out of bounds", t->name);
-        const size_t row_bytes = (size_t)cols / 32 * 34, nbytes = (size_t)rs[k] * row_bytes;
+        // resident: the K-quant rows are staged as they are, and the repack copies them
+        const size_t row_bytes = fmt ? (size_t)cols / 256 * kq_block_bytes(fmt) : (size_t)cols / 32 * 34, nbytes = (size_t)rs[k] * row_bytes;
         if (off + nbytes > q8_area) return fail(p, B200_ERR_STATE, "staging buffer too small");
-        if (kq) { // the K-quant bytes land in the raw area; the Q8_0 blocks are produced on the device once the copies are in
+        if (kq && !fmt) { // the K-quant bytes land in the raw area; the Q8_0 blocks are produced on the device once the copies are in
             const size_t raw_row = (size_t)cols / 256 * kq_block_bytes(t->ggml_type), raw_bytes = (size_t)rs[k] * raw_row;
             const unsigned char *hsrc = (const unsigned char *)t->data + (size_t)first * raw_row;
             if (p->kq_off + roff + raw_bytes > stage_bytes) return fail(p, B200_ERR_STATE, "staging buffer too small");
@@ -459,19 +496,14 @@ int upload_tiles(b200_plan *p, const b200_tensor *t0, const b200_tensor *t1, con
     if ((rc = up_stage_ready(p))) return rc;
     for (int i = 0; i < n_rq; i++) CK(launch_requant_kquant(rq[i].type, rq[i].raw, rq[i].q8, rq[i].nblk, p->stream));
     src.gateup = gateup ? 1 : 0;
-    const int rows = gateup ? r0 + r1 : r0 + r1 + r2;
-    out.rows = rows;
-    out.cols = cols;
-    out.nseg = smv_pick_nseg(cols);
-    out.seg = cols / out.nseg;
-    out.unit_bytes = smv_unit_bytes(out.seg);
+    out = tile_geometry(rows, cols, fmt);
     const size_t stored_rows = (size_t)tile_groups(out) * 4; // whole 4-row groups: a ragged classifier gets zero padding rows
-    size_t total = stored_rows * out.nseg * out.unit_bytes;
     unsigned char *d;
-    rc = dalloc(p, &d, total);
+    rc = dalloc(p, &d, (size_t)tile_bytes(out));
     if (rc) return rc;
     out.base = d;
-    k_repack_tiles<<<(unsigned)(stored_rows * out.nseg), 128, 0, p->stream>>>(src, d, rows, cols, out.seg, out.nseg, out.unit_bytes);
+    if (fmt) k_repack_kq_tiles<<<(unsigned)(stored_rows * out.nseg), 128, 0, p->stream>>>(src, d, rows, cols, out.seg, out.nseg, out.unit_bytes, kq_block_bytes(fmt));
+    else k_repack_tiles<<<(unsigned)(stored_rows * out.nseg), 128, 0, p->stream>>>(src, d, rows, cols, out.seg, out.nseg, out.unit_bytes);
     CK(cudaGetLastError());
     return up_stage_release(p);
 }
@@ -596,7 +628,6 @@ int launch_k(b200_plan *p, bool pdl, void (*kern)(KA...), dim3 grid, dim3 block,
     return B200_OK;
 }
 
-const size_t SMV_SMEM_BUDGET_MAX = 96 * 1024;
 // Read ONCE per plan (b200_plan_create), never inside a launch helper.
 void read_knobs(b200_plan *p) {
     const char *d = getenv("B200_DECODE");
@@ -604,11 +635,29 @@ void read_knobs(b200_plan *p) {
     p->decode_mode = (d && !strcmp(d, "persistent")) ? B200_DECODE_PERSISTENT : B200_DECODE_GRAPH;
 }
 
+// The stream kernels of a tile format (TileMat::fmt): the Q8_0 kernels, or their resident K-quant instantiations.
+template <int MODE> void (*smv_kernel(int fmt))(SmvArgs, SmvSmem) {
+    switch (fmt) {
+    case B200_GGML_Q4_K: return k_stream_matvec_kq<MODE, B200_GGML_Q4_K>;
+    case B200_GGML_Q5_K: return k_stream_matvec_kq<MODE, B200_GGML_Q5_K>;
+    case B200_GGML_Q6_K: return k_stream_matvec_kq<MODE, B200_GGML_Q6_K>;
+    }
+    return k_stream_matvec_q8<MODE>;
+}
+template <int MODE> void (*smv_norm_kernel(int fmt))(SmvArgs, SmvSmem, SmvNormArgs) {
+    switch (fmt) {
+    case B200_GGML_Q4_K: return k_stream_matvec_kq_norm<MODE, B200_GGML_Q4_K>;
+    case B200_GGML_Q5_K: return k_stream_matvec_kq_norm<MODE, B200_GGML_Q5_K>;
+    case B200_GGML_Q6_K: return k_stream_matvec_kq_norm<MODE, B200_GGML_Q6_K>;
+    }
+    return k_stream_matvec_q8_norm<MODE>;
+}
+
 template <int MODE>
 int launch_stream(b200_plan *p, const TileMat &W, const int8_t *xq, const float *xs, float *out, int8_t *hq, float *hs, bool argmax = false,
                   TraceBuf tr = TraceBuf{nullptr, 0, 0}, int wait_slot = -1, unsigned wait_op = 0, int out_slot = -1, unsigned out_op = 0,
                   int row_base = 0) {
-    SmvSmem L = smv_layout(W.cols, W.seg, SMV_SMEM_BUDGET_MAX);
+    SmvSmem L = smv_layout(W.cols, W.seg, SMV_SMEM_BUDGET_MAX, W.fmt);
     SmvArgs a;
     a.W = W; a.xq = xq; a.xs = xs; a.out = out; a.hq = hq; a.hs = hs; a.blk_cnt = p->blk_cnt;
     a.oscale = out_scale(p, MODE == SMV_RESID, &W == &p->tout);
@@ -617,7 +666,7 @@ int launch_stream(b200_plan *p, const TileMat &W, const int8_t *xq, const float 
     a.tr = tr;
     a.tp = p->tp;
     a.wait_slot = wait_slot; a.wait_op = wait_op; a.out_slot = out_slot; a.out_op = out_op; a.row_base = row_base;
-    return launch_k(p, p->use_pdl, k_stream_matvec_q8<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L);
+    return launch_k(p, p->use_pdl, smv_kernel<MODE>(W.fmt), dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L);
 }
 
 // A stream kernel behind a fused RMSNorm of the residual stream x (weights w; from_emb: layer 0, the embedding row, which CTA 0
@@ -625,7 +674,7 @@ int launch_stream(b200_plan *p, const TileMat &W, const int8_t *xq, const float 
 template <int MODE>
 int launch_stream_norm(b200_plan *p, const TileMat &W, const float *w, bool from_emb, float *out, int8_t *hq, float *hs, bool argmax, TraceBuf tr, int row_base = 0) {
     SmvNormArgs n;
-    const SmvSmem L = smv_layout_norm(W.cols, W.seg, SMV_SMEM_BUDGET_MAX, &n.off_sq, &n.off_seq);
+    const SmvSmem L = smv_layout_norm(W.cols, W.seg, SMV_SMEM_BUDGET_MAX, &n.off_sq, &n.off_seq, W.fmt);
     n.x = p->x; n.w = w; n.st = p->st; n.emb = p->emb; n.emb_scale = p->mup.embedding_scale; n.eps = p->cfg.rms_norm_eps;
     n.from_emb = from_emb ? 1 : 0; n.x_out = p->x;
     SmvArgs a;
@@ -636,7 +685,7 @@ int launch_stream_norm(b200_plan *p, const TileMat &W, const float *w, bool from
     a.tr = tr;
     a.tp = p->tp;
     a.wait_slot = -1; a.wait_op = 0; a.out_slot = -1; a.out_op = 0; a.row_base = row_base;
-    return launch_k(p, p->use_pdl, k_stream_matvec_q8_norm<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L, n);
+    return launch_k(p, p->use_pdl, smv_norm_kernel<MODE>(W.fmt), dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L, n);
 }
 
 // The fused norm needs 256 x ceil(dim / 256) squares and the accumulator's scratch next to the ring: at least 3 stages must remain.
@@ -793,6 +842,7 @@ int pd_prepare(b200_plan *p) {
     const b200_config &c = p->cfg;
     p->pd_ok = false;
     if (p->is_moe) { p->pd_why = "the persistent decode kernel has no Qwen2-MoE layer (MoE plans decode through the CUDA graph)"; return B200_OK; }
+    if (p->resident) { p->pd_why = "the persistent decode kernel reads Q8_0 tiles only (this plan keeps K-quant weights resident: it decodes through the CUDA graph)"; return B200_OK; }
     if (c.dim > 8192) { p->pd_why = "the persistent decode kernel's register-resident RMSNorm supports dim <= 8192"; return B200_OK; }
     if (p->wtype != B200_GGML_Q8_0) { p->pd_why = "the persistent decode kernel needs Q8_0 weights"; return B200_OK; }
     if (c.head_size != 64 && c.head_size != 128) { p->pd_why = "the persistent decode kernel supports head sizes 64 and 128"; return B200_OK; }
@@ -1074,8 +1124,10 @@ int batch_alloc(b200_plan *p, int ns) {
 
 // ---- steps whose rows may share a sequence: b200_forward_decode_multi and the exact prefills ------------------------------
 // Why a plan cannot run them (nullptr: it can): the conditions of batched decode.
+const char *const RESIDENT_MULTI_WHY = "batched and multi-position steps read Q8_0 tiles only (this plan keeps K-quant weights resident: it runs one position per step)";
 const char *multi_why(const b200_plan *p) {
     if (p->is_moe) return "multi-position steps have no Qwen2-MoE layer (MoE plans run one position per step)";
+    if (p->resident) return RESIDENT_MULTI_WHY;
     if (p->cfg.tp_size > 1) return "multi-position steps run on single-GPU plans only (this plan is tensor-parallel)";
     if (p->wtype != B200_GGML_Q8_0) return "multi-position steps need Q8_0 weights (FP16 plans run one position per step)";
     if (!batch_max_rows(p)) return "no row count of the batched Q8_0 stream fits this plan's shapes";
@@ -1158,6 +1210,13 @@ int set_smem_attrs(b200_plan *p) {
     CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_norm<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_norm<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    for (int fmt : {B200_GGML_Q4_K, B200_GGML_Q5_K, B200_GGML_Q6_K}) {
+        CK(cudaFuncSetAttribute(smv_kernel<SMV_STORE>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+        CK(cudaFuncSetAttribute(smv_kernel<SMV_RESID>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+        CK(cudaFuncSetAttribute(smv_kernel<SMV_GATEUP>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+        CK(cudaFuncSetAttribute(smv_norm_kernel<SMV_STORE>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+        CK(cudaFuncSetAttribute(smv_norm_kernel<SMV_GATEUP>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    }
     CK(set_max_dyn(k_matvec_f16<MODE_STORE>, maxdyn));
     CK(set_max_dyn(k_matvec_f16<MODE_RESID>, maxdyn));
     CK(set_max_dyn(k_stream_matvec_f16<16, SF_STORE>, maxdyn));
@@ -1290,6 +1349,71 @@ int upload_moe_layer(b200_plan *p, const b200_tensor *tensors, int n_tensors, in
     return B200_OK;
 }
 
+// Weight bytes of a dense single-GPU Q8_0 plan: the embedding's Q8_0 planes plus every stream, as Q8_0 tiles or (resident) in the
+// form upload_tiles gives it on a resident plan.  The one function behind both footprints of the residency rule.
+int64_t weight_footprint(const b200_plan *p, const b200_tensor *tensors, int n_tensors, bool resident) {
+    const b200_config &c = p->cfg;
+    const bool phi3 = c.arch == B200_ARCH_PHI3;
+    auto T = [&](const std::string &s) { return find(tensors, n_tensors, s); };
+    auto stream = [&](const b200_tensor *a, const b200_tensor *b, const b200_tensor *d, int r0, int r1, int r2, int cols, bool gateup) {
+        const b200_tensor *ts[3] = {a, b, d};
+        const int rs[3] = {r0, r1, r2}, rows = gateup ? r0 + r1 : r0 + r1 + r2;
+        return tile_bytes(tile_geometry(rows, cols, resident ? resident_fmt(ts, rs, rows, cols) : 0));
+    };
+    const b200_tensor *outw = T("output.weight");
+    int64_t b = (int64_t)c.vocab_size * c.dim / 32 * 34; // embedding: int8 plane + f16 scale plane (row gather)
+    b += stream(outw ? outw : T("token_embd.weight"), nullptr, nullptr, c.vocab_size, 0, 0, c.dim, false);
+    for (int l = 0; l < c.n_layers; l++) {
+        const std::string pre = "blk." + std::to_string(l) + ".";
+        const b200_tensor *tq = T(pre + (phi3 ? "attn_qkv.weight" : "attn_q.weight"));
+        const b200_tensor *tk = phi3 ? tq : T(pre + "attn_k.weight"), *tv = phi3 ? tq : T(pre + "attn_v.weight");
+        const b200_tensor *tg = T(pre + (phi3 ? "ffn_up.weight" : "ffn_gate.weight")), *tu = T(pre + "ffn_up.weight");
+        b += stream(tq, tk, tv, p->qd, p->kvd, p->kvd, c.dim, false);
+        b += stream(T(pre + "attn_output.weight"), nullptr, nullptr, c.dim, 0, 0, p->qd, false);
+        b += stream(tg, tu, nullptr, c.hidden_dim, c.hidden_dim, 0, c.dim, true);
+        b += stream(T(pre + "ffn_down.weight"), nullptr, nullptr, c.dim, 0, 0, c.hidden_dim, false);
+    }
+    return b;
+}
+
+// Room kept free beyond what rest_footprint counts: the CUDA graphs, the scratch of the exact prefill's multi-position steps and of
+// the persistent kernel, allocator rounding, and what other processes on the device may take meanwhile.
+const int64_t RESIDENT_MARGIN = (int64_t)1 << 30;
+int64_t g_memory_budget = 0; // b200_test_set_memory_budget: replaces the free-memory figure of weight_policy (0: off)
+
+// What a plan allocates besides its weights: both KV caches, the upload's two device staging buffers (live while the weights are
+// allocated), the activations, the attention score scratch and the RoPE tables.
+int64_t rest_footprint(const b200_plan *p, size_t stage_bytes) {
+    const b200_config &c = p->cfg;
+    const int64_t big = c.dim > p->qd ? c.dim : p->qd;
+    const int64_t kv = 2LL * c.n_layers * c.context_length * p->kvd * 4;
+    const int64_t act = 4LL * (c.dim + big + p->qd + 2 * p->kvd + 2LL * c.hidden_dim + sampler_padded(c.vocab_size) + c.vocab_size) +
+                        (big + c.hidden_dim) * 33 / 8; // + int8 activations and their f32 block scales
+    const int64_t att = 3 * c.head_size + c.context_length > ATT_SMEM_FLOATS_MAX ? 4LL * c.n_heads * ((c.context_length + PD_CT - 1) / PD_CT * PD_CT) : 0;
+    const int64_t rope = 4LL * c.context_length * c.head_size;
+    return kv + 2 * (int64_t)stage_bytes + act + att + rope;
+}
+
+// The residency rule of a single-GPU dense plan with K-quant matrices: Q8_0 tiles throughout when they fit the device's free memory
+// (less RESIDENT_MARGIN) next to everything else the plan allocates; else resident streams where resident_fmt allows; else an error
+// naming both figures.  No option selects the form: the rule reads only the shapes, the tensor types and the free memory.
+int weight_policy(b200_plan *p, const b200_tensor *tensors, int n_tensors, size_t stage_bytes) {
+    p->w8_bytes = weight_footprint(p, tensors, n_tensors, false);
+    const int64_t wr = weight_footprint(p, tensors, n_tensors, true);
+    const int64_t rest = rest_footprint(p, stage_bytes) + RESIDENT_MARGIN;
+    int64_t avail = g_memory_budget;
+    if (!avail) {
+        size_t fr = 0, tot = 0;
+        CK(cudaMemGetInfo(&fr, &tot));
+        avail = (int64_t)fr;
+    }
+    if (p->w8_bytes + rest <= avail) { p->w_bytes = p->w8_bytes; return B200_OK; }
+    if (wr + rest <= avail) { p->resident = true; p->w_bytes = wr; return B200_OK; }
+    return fail(p, B200_ERR_OOM, "the model does not fit the device: %lld bytes with Q8_0 tiles and %lld bytes with K-quant weights resident are needed "
+                "(weights plus %lld bytes of KV cache, activations, upload staging and margin), %lld bytes are free",
+                (long long)(p->w8_bytes + rest), (long long)(wr + rest), (long long)rest, (long long)avail);
+}
+
 int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     const b200_config &c = p->cfg;
     if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3 && c.arch != B200_ARCH_QWEN2 && c.arch != B200_ARCH_QWEN2_MOE &&
@@ -1396,6 +1520,11 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         stage_bytes = (stage_bytes + 255) & ~(size_t)255;
         p->kq_off = stage_bytes;
         stage_bytes *= 2;
+    }
+    if (q8 && c.tp_size == 1 && !p->is_moe) {
+        if (any_kq) {
+            if ((rc = weight_policy(p, tensors, n_tensors, stage_bytes))) return rc;
+        } else p->w_bytes = p->w8_bytes = weight_footprint(p, tensors, n_tensors, false);
     }
     const auto t_up0 = std::chrono::steady_clock::now();
     if ((rc = up_init(p, stage_bytes))) return rc;
@@ -2254,6 +2383,8 @@ int b200_trace_persistent(b200_plan *p, int32_t token, int32_t position, uint64_
 int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
     if (!p || (mode != B200_PREFILL_EXACT && mode != B200_PREFILL_TENSOR_CORE && mode != B200_PREFILL_TENSOR_CORE_W8A16)) return B200_ERR_BAD_ARG;
     if (p->is_moe && mode != B200_PREFILL_EXACT) return fail(p, B200_ERR_UNSUPPORTED, "%s", MOE_PREFILL_WHY);
+    if (p->resident && mode != B200_PREFILL_EXACT)
+        return fail(p, B200_ERR_UNSUPPORTED, "this plan keeps K-quant weights resident: the tensor-core prefill reads Q8_0 tiles or f16 matrices, so prompts go through the exact prefill");
     if (mode == B200_PREFILL_TENSOR_CORE_W8A16) {
         if (!p->prefill.q8_ready) {
             CK(cudaSetDevice(p->device));
@@ -2302,6 +2433,7 @@ int b200_set_decode_slots(b200_plan *p, int32_t n_slots) {
     if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "batched decode has no Qwen2-MoE layer (MoE plans decode one sequence per step)");
     if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "batched decode runs on single-GPU plans only (this plan is tensor-parallel)");
     if (p->wtype != B200_GGML_Q8_0) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs Q8_0 weights (FP16 plans decode one sequence per step)");
+    if (p->resident) return fail(p, B200_ERR_UNSUPPORTED, "%s", RESIDENT_MULTI_WHY);
     const int mx = batch_max_rows(p);
     if (n_slots > mx) return fail(p, B200_ERR_UNSUPPORTED, "at most %d decode slots on this plan (asked for %d)", mx, n_slots);
     batch_free(p);
@@ -3018,6 +3150,20 @@ int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const 
         if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize())) s.ok(cudaMemcpy(out, dout, (size_t)n * qd * 2, cudaMemcpyDeviceToHost));
     }
     return s.rc;
+}
+
+int b200_weight_info(b200_plan *p, int32_t *resident, int64_t *weight_bytes, int64_t *q8_weight_bytes) {
+    if (!p) return B200_ERR_BAD_ARG;
+    if (resident) *resident = p->resident ? 1 : 0;
+    if (weight_bytes) *weight_bytes = p->w_bytes;
+    if (q8_weight_bytes) *q8_weight_bytes = p->w8_bytes;
+    return B200_OK;
+}
+
+int b200_test_set_memory_budget(int64_t bytes) {
+    if (bytes < 0) return B200_ERR_BAD_ARG;
+    g_memory_budget = bytes;
+    return B200_OK;
 }
 
 int b200_upload_info(b200_plan *p, double *seconds, double *host_copy_seconds, int64_t *h2d_bytes) {

@@ -18,10 +18,16 @@
 //   For the fused gate/up projection group G holds rows {gate 2G, gate 2G+1, up 2G, up 2G+1}.
 //   A classifier whose vocabulary is not a multiple of 4 is padded to whole groups with zero rows at upload; STORE never writes
 //   those rows and never offers them to the argmax (a padding row's 0 would beat real logits that are all negative).
+//
+// Resident K-quant layout (TileMat::fmt = 12 / 13 / 14, Q4_K / Q5_K / Q6_K): the same groups, segments and tile order, but SEG is a
+// multiple of 256 and a unit is the row's SEG/256 raw super-blocks (144 / 176 / 210 bytes each) padded to 16 bytes.  The consumer
+// lane that owns 32-block b rebuilds b's Q8_0 block from super-block b/8, sub-block b%8 with kq_q8_block (kquant.cuh), the function
+// the load-time re-quantiser runs, and then computes exactly the Q8_0 term.  A zero padding row is all-zero super-blocks: d = 0.
 #pragma once
 #include "common.cuh"
 #include "decode_kernels.cuh"
 #include "norm_slots.cuh"
+#include "kquant.cuh"
 
 #define SMV_CONSUMER_WARPS 8
 #define SMV_THREADS ((SMV_CONSUMER_WARPS + 1) * 32)
@@ -34,17 +40,19 @@ struct TileMat { // device weight matrix in tile-major layout
     const unsigned char *base;
     int rows, cols;  // rows = 4 * groups (for gate/up: 2 * hidden); a classifier may end in a partial group (tile_groups)
     int seg, nseg;   // columns per segment, segments per row
-    int unit_bytes;  // seg + seg/16 rounded up to 16
+    int unit_bytes;  // Q8_0: seg + seg/16 rounded up to 16; K-quant: seg/256 super-blocks rounded up to 16
+    int fmt;         // 0: Q8_0 tiles; 12 / 13 / 14: resident Q4_K / Q5_K / Q6_K tiles
 };
 
-// The fewest segments of at most 2560 columns, each a multiple of 32: any width that is a multiple of 32 has one (at worst
-// 32-column segments).  0: the width is not a multiple of 32.
-__host__ __device__ inline int smv_pick_nseg(int cols) {
-    for (int n = 1; n <= cols / 32; n++)
-        if (cols % n == 0 && (cols / n) % 32 == 0 && cols / n <= 2560) return n;
+// The fewest segments of at most 2560 columns, each a multiple of `quantum` (32 for Q8_0 tiles, 256 for K-quant tiles): any width
+// that is a multiple of the quantum has one.  0: the width is not.
+__host__ __device__ inline int smv_pick_nseg(int cols, int quantum = 32) {
+    for (int n = 1; n <= cols / quantum; n++)
+        if (cols % n == 0 && (cols / n) % quantum == 0 && cols / n <= 2560) return n;
     return 0;
 }
 __host__ __device__ inline int smv_unit_bytes(int seg) { return (seg + seg / 16 + 15) & ~15; }
+__host__ __device__ inline int smv_unit_bytes(int seg, int fmt) { return fmt ? (seg / 256 * kq_block_bytes(fmt) + 15) & ~15 : smv_unit_bytes(seg); }
 __host__ __device__ inline int tile_groups(const TileMat &W) { return (W.rows + 3) >> 2; } // 4-row groups stored, the last one zero-padded
 
 struct SmvSmem {
@@ -52,9 +60,9 @@ struct SmvSmem {
     int stages, stage_bytes, nbs_pad;
 };
 
-__host__ __device__ inline SmvSmem smv_layout(int cols, int seg, size_t budget) {
+__host__ __device__ inline SmvSmem smv_layout(int cols, int seg, size_t budget, int fmt = 0) {
     SmvSmem L;
-    int unit = smv_unit_bytes(seg);
+    int unit = smv_unit_bytes(seg, fmt);
     L.stage_bytes = (4 * unit + 127) & ~127;
     L.nbs_pad = ((seg / 32 + 3) & ~3) + 4; // row stride of the term buffer: 16-byte aligned rows, the four walker lanes on distinct banks
     size_t o = 0;
@@ -192,8 +200,8 @@ struct SmvNormArgs {
 // Layout of the normalising form: the squares and the accumulator scratch of 256 threads are dead once the activation is in
 // shared memory, so they share their bytes with the term buffer and hvals (which are live only after it); what they need
 // beyond those comes out of the ring.
-__host__ inline SmvSmem smv_layout_norm(int cols, int seg, size_t budget, unsigned *off_sq, unsigned *off_seq) {
-    SmvSmem L = smv_layout(cols, seg, budget);
+__host__ inline SmvSmem smv_layout_norm(int cols, int seg, size_t budget, unsigned *off_sq, unsigned *off_seq, int fmt = 0) {
+    SmvSmem L = smv_layout(cols, seg, budget, fmt);
     const size_t sq = (size_t)norm_slots_sq_floats(cols, SMV_CONSUMER_WARPS * 32) * 4;
     const size_t nb = sq + seqsum2_scratch_bytes(SMV_CONSUMER_WARPS * 32);
     *off_sq = (unsigned)L.off_terms;
@@ -255,7 +263,29 @@ __device__ __forceinline__ void smv_norm_prologue(const SmvNormArgs &n, int cols
                            reinterpret_cast<float *>(smem + n.off_sq), reinterpret_cast<unsigned *>(smem + off_xq), reinterpret_cast<float *>(smem + off_xs), tid);
 }
 
-template <int MODE, bool NORM>
+// The resident form's block term for the 4 rows of a tile: the lane rebuilds each row's Q8_0 block b from its K-quant sub-block and
+// computes the Q8_0 term of the consumer loop below (the quants' integer dot product is exact, so its order is free).
+template <int FMT>
+__device__ __forceinline__ void smv_kq_terms(const unsigned char *tile, int unit_bytes, int b, const unsigned char *ab, float as, float *terms, int stride) {
+    const int4 a0 = *reinterpret_cast<const int4 *>(ab), a1 = *reinterpret_cast<const int4 *>(ab + 16);
+#pragma unroll 1 // one row's 32 values live at a time: unrolling would hold four blocks in registers
+    for (int r = 0; r < 4; r++) {
+        int q[8];
+        const __half sc = kq_q8_block<FMT>(tile + (size_t)r * unit_bytes + (size_t)(b >> 3) * kq_block_bytes(FMT), b & 7, q);
+        int isum = __dp4a(q[0], a0.x, 0);
+        isum = __dp4a(q[1], a0.y, isum);
+        isum = __dp4a(q[2], a0.z, isum);
+        isum = __dp4a(q[3], a0.w, isum);
+        isum = __dp4a(q[4], a1.x, isum);
+        isum = __dp4a(q[5], a1.y, isum);
+        isum = __dp4a(q[6], a1.z, isum);
+        isum = __dp4a(q[7], a1.w, isum);
+        terms[r * stride + b] = __fmul_rn((float)isum, __fmul_rn(__half2float(sc), as));
+    }
+}
+
+// FMT 0: Q8_0 tiles; 12 / 13 / 14: resident K-quant tiles (only the consumers' block terms differ).
+template <int MODE, bool NORM, int FMT = 0>
 __device__ __forceinline__ void smv_q8_body(const SmvArgs &a, const SmvSmem &L, const SmvNormArgs &na, unsigned char *smem) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const TileMat W = a.W;
@@ -356,6 +386,10 @@ __device__ __forceinline__ void smv_q8_body(const SmvArgs &a, const SmvSmem &L, 
                 __syncwarp();
                 mbar_wait(bar0 + 8 * st, lap & 1u);
                 const unsigned char *tile = smem + L.off_ring + (size_t)st * L.stage_bytes;
+                if (FMT) {
+                    for (int b = lane; b < nbs; b += 32)
+                        smv_kq_terms<FMT>(tile, W.unit_bytes, b, sact + ((size_t)(s * nbs + b) << 5), sxs[s * nbs + b], terms, L.nbs_pad);
+                } else
                 for (int b = lane; b < nbs; b += 32) {
                     const unsigned char *ab = sact + ((size_t)(s * nbs + b) << 5);
                     const int4 a0 = *reinterpret_cast<const int4 *>(ab + 16 * hsel);
@@ -498,6 +532,20 @@ __global__ void __maxnreg__(96) k_stream_matvec_q8_norm(SmvArgs a, SmvSmem L, Sm
     smv_q8_body<MODE, true>(a, L, n, smem);
 }
 
+// The resident K-quant forms of the two kernels above (FMT = 12 / 13 / 14).  Both are held to the 96 registers the Q8_0 forms use,
+// so the next stream kernel still fits beside them under PDL (the compiler would otherwise take ~120 for the plain form).
+template <int MODE, int FMT>
+__global__ void __maxnreg__(96) k_stream_matvec_kq(SmvArgs a, SmvSmem L) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    smv_q8_body<MODE, false, FMT>(a, L, SmvNormArgs{}, smem);
+}
+template <int MODE, int FMT>
+__global__ void __maxnreg__(96) k_stream_matvec_kq_norm(SmvArgs a, SmvSmem L, SmvNormArgs n) {
+    static_assert(MODE != SMV_RESID, "a residual matvec consumes an activation, not the residual stream");
+    extern __shared__ __align__(128) unsigned char smem[];
+    smv_q8_body<MODE, true, FMT>(a, L, n, smem);
+}
+
 // ---- upload-time repack: GGUF Q8_0 blocks (34 B: f16 scale + 32 int8) -> tile-major -----------
 // One thread per 16-bit word of the destination tile payload.  src_row(g, r) gives the source row
 // of group g, slot r: identity for plain matrices, the gate/up interleave for the fused FFN matrix.
@@ -543,6 +591,32 @@ __global__ void k_repack_tiles(RepackSrc src, unsigned char *dst, int rows, int 
         }
         reinterpret_cast<unsigned short *>(u)[w] = v;
     }
+}
+
+// The resident form of the repack: the same units, each a row's segment of raw K-quant super-blocks (kb bytes each) followed by
+// zeros up to unit_bytes.  src.raw[k] holds whole rows of cols / 256 super-blocks.
+__global__ void k_repack_kq_tiles(RepackSrc src, unsigned char *dst, int rows, int cols, int seg, int nseg, int unit_bytes, int kb) {
+    const long long unit_id = blockIdx.x;
+    const int r = (int)(unit_id % 4);
+    const int s = (int)((unit_id / 4) % nseg);
+    const long long G = unit_id / (4LL * nseg);
+    long long row;
+    const unsigned char *raw;
+    if (src.gateup) {
+        raw = src.raw[r >> 1];
+        row = src.row0[r >> 1] + 2 * G + (r & 1);
+    } else {
+        row = 4 * G + r;
+        int k = 0;
+        while (k < 2 && row >= src.rows[k]) { row -= src.rows[k]; k++; }
+        raw = src.raw[k];
+        row += src.row0[k];
+    }
+    const bool pad = !src.gateup && 4 * G + r >= rows; // all-zero super-blocks: d = 0, so every value and scale is 0
+    const int payload = seg / 256 * kb;
+    const unsigned char *from = pad ? nullptr : raw + (size_t)row * (cols / 256) * kb + (size_t)s * payload;
+    unsigned char *u = dst + (size_t)unit_id * unit_bytes;
+    for (int i = threadIdx.x; i < unit_bytes; i += blockDim.x) u[i] = (pad || i >= payload) ? 0 : from[i];
 }
 
 // ---- inverse of the repack: tile-major Q8_0 stream -> row-major f16 matrix (value = f16(q * scale)) ----------------

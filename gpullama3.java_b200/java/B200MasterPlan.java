@@ -89,6 +89,7 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle PREFILL_SLOTS = fn("b200_prefill_slots", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
     private static final MethodHandle DECODE_MULTI = fn("b200_forward_decode_multi", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle MULTI_ROWS = fn("b200_decode_multi_rows", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS));
+    private static final MethodHandle WEIGHT_INFO = fn("b200_weight_info", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
     private static final MethodHandle FREE = fn("b200_plan_free", FunctionDescriptor.ofVoid(ADDRESS));
     private static final MethodHandle LAST_ERROR = fn("b200_last_error", FunctionDescriptor.of(ADDRESS, ADDRESS));
 
@@ -372,6 +373,18 @@ public final class B200MasterPlan implements AutoCloseable {
             int rc = (int) MULTI_ROWS.invokeExact(plan, r);
             if (rc != 0) check(rc, lastError());
             return r.get(JAVA_INT, 0);
+        }
+    }
+
+    /** {resident (0 / 1), weight bytes, weight bytes of the all-Q8_0 form}: a K-quant model whose Q8_0 expansion does not fit the
+     *  device keeps its K-quant weights resident (same logits; batched steps, the persistent kernel and the tensor-core prefill are
+     *  then refused with UnsupportedOperationException). */
+    public long[] weightInfo() throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            MemorySegment r = a.allocate(JAVA_INT), w = a.allocate(JAVA_LONG), w8 = a.allocate(JAVA_LONG);
+            int rc = (int) WEIGHT_INFO.invokeExact(plan, r, w, w8);
+            if (rc != 0) check(rc, lastError());
+            return new long[] {r.get(JAVA_INT, 0), w.get(JAVA_LONG, 0), w8.get(JAVA_LONG, 0)};
         }
     }
 

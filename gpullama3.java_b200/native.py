@@ -63,7 +63,7 @@ EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
-           "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step",
+           "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_weight_info", "b200_test_set_memory_budget",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -117,6 +117,8 @@ def lib() -> C.CDLL:
     L.b200_decode_multi_rows.argtypes = [vp, C.POINTER(i32)]
     L.b200_forward_step.argtypes = [vp, i32, C.POINTER(StepRow), vp, vp]
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
+    L.b200_weight_info.argtypes = [vp, C.POINTER(i32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    L.b200_test_set_memory_budget.argtypes = [C.c_int64]
     L.b200_launches_per_decode.argtypes = [vp]
     L.b200_device_bytes.argtypes = [vp]
     L.b200_device_bytes.restype = C.c_int64
@@ -168,6 +170,14 @@ def test_sample(logits, temperature: float, topp: float, uniform01: float):
     if rc != B200_OK:
         _raise(rc, "b200_test_sample failed")
     return out.value, list(info), probs
+
+
+def test_set_memory_budget(n_bytes: int):
+    """Test hook: the device free-memory figure the weight-form rule of plan creation reads, for every later plan in the process
+    (0 restores the real figure).  Puts a budget on either side of the K-quant residency threshold without filling the GPU."""
+    rc = lib().b200_test_set_memory_budget(int(n_bytes))
+    if rc != B200_OK:
+        _raise(rc, f"b200_test_set_memory_budget({n_bytes}) failed")
 
 
 def requant_kquant(ggml_type: int, raw, n_elems: int) -> np.ndarray:
@@ -509,6 +519,12 @@ class NativePlan:
         self._ck(lib().b200_upload_info(self._p, C.byref(a), C.byref(b), C.byref(c)))
         return {"seconds": a.value, "host_copy_seconds": b.value, "h2d_bytes": c.value,
                 "GB/s": (c.value / a.value / 1e9) if a.value > 0 else None}
+
+    def weight_info(self) -> dict:
+        """b200_weight_info: whether the plan keeps K-quant weights resident, its weight bytes and those of its all-Q8_0 form."""
+        r, w, w8 = C.c_int32(0), C.c_int64(0), C.c_int64(0)
+        self._ck(lib().b200_weight_info(self._p, C.byref(r), C.byref(w), C.byref(w8)))
+        return {"resident": bool(r.value), "weight_bytes": w.value, "q8_weight_bytes": w8.value}
 
     @property
     def launches_per_decode(self) -> int:

@@ -223,6 +223,12 @@ class B200MasterPlan:
         """Seconds / bytes of the weight upload pipeline of plan creation (load-time metric, ModelLoader.java:102-106)."""
         return self._native.upload_info()
 
+    def weight_info(self):
+        """{"resident", "weight_bytes", "q8_weight_bytes"}: whether plan creation kept the K-quant weights resident because their
+        Q8_0 expansion did not fit the device (decode stays bit-identical; batched steps, the persistent kernel and the tensor-core
+        prefill are then refused), and the weight footprints of the chosen and of the all-Q8_0 form."""
+        return self._native.weight_info()
+
     @property
     def launches_per_decode(self):
         return self._native.launches_per_decode

@@ -480,6 +480,25 @@ int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const 
  * stream -> double-buffered device staging -> repack kernel on the plan's stream. */
 int b200_upload_info(b200_plan *plan, double *seconds, double *host_copy_seconds, int64_t *h2d_bytes);
 
+/* The weight form b200_plan_create chose (any pointer may be NULL).  A single-GPU dense plan whose tensors hold a K-quant matrix
+ * (Q4_K / Q5_K / Q6_K) computes two weight footprints from the shapes and tile layouts: q8_weight_bytes with every matrix re-quantised
+ * to Q8_0 tiles, and the resident form, where every weight stream whose sources share one K-quant format keeps the raw K-quant
+ * super-blocks and the decode kernels rebuild the reference's Q8_0 blocks from them on the fly (bit-identical results).  It adds
+ * what the plan allocates besides the weights (KV cache, activations, upload staging) and a 1 GiB margin, and compares with the
+ * device's free memory: Q8_0 tiles when they fit (*resident = 0), else the resident form (*resident = 1), else creation fails with
+ * B200_ERR_OOM naming both figures.  weight_bytes is the footprint of the chosen form.  Other Q8_0 plans report *resident = 0 and
+ * weight_bytes == q8_weight_bytes; FP16, tensor-parallel and Qwen2-MoE plans report 0 for both (they never go resident).
+ * A resident plan decodes through the CUDA graph (b200_forward_decode, _sample, b200_decode_sequence, b200_trace_decode) and
+ * prefills through B200_PREFILL_EXACT, one token per step.  It refuses with B200_ERR_UNSUPPORTED and the reason: the persistent
+ * decode kernel, b200_set_decode_slots (n_slots > 0), b200_forward_decode_multi, b200_forward_step (b200_decode_multi_rows reports 0)
+ * and both tensor-core prefill modes. */
+int b200_weight_info(b200_plan *plan, int32_t *resident, int64_t *weight_bytes, int64_t *q8_weight_bytes);
+
+/* Test hook: replaces the device free-memory figure the weight-form rule of b200_plan_create reads (see b200_weight_info) by
+ * `bytes` for every later plan in the process; 0 restores the real figure.  Lets tests put a budget on either side of the
+ * threshold without filling a shared GPU.  bytes < 0: B200_ERR_BAD_ARG. */
+int b200_test_set_memory_budget(int64_t bytes);
+
 /* Number of kernels one decode step launches (bench.py's gpu_launches). */
 int b200_launches_per_decode(b200_plan *plan);
 

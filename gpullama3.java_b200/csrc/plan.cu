@@ -12,6 +12,7 @@
 #include "sampler.cuh"
 #include "decode_batch.cuh"
 #include "moe.cuh"
+#include "prefill_i8.cuh"
 
 #include <math.h>
 #include <stdarg.h>
@@ -158,6 +159,7 @@ struct b200_plan {
     b200_yarn_config yarn{};
 
     PrefillCtx prefill;
+    PrefillI8Ctx pi8; // B200_PREFILL_TENSOR_CORE_EXACT (prefill_i8.cuh); its mode is prefill.mode like the other three
     // persistent decode kernel
     bool pd_ok = false;           // the plan fits the kernel's restrictions
     std::string pd_why;           // ... or why not
@@ -1201,6 +1203,7 @@ int set_smem_attrs(b200_plan *p) {
             CK(set_max_dyn(k_attention<HS>, maxdyn));
             CK(set_max_dyn(k_attention_batch<HS>, maxdyn));
             CK(set_max_dyn(k_attention_cached_rows<HS>, maxdyn));
+            CK(set_max_dyn(k_i8_attention<HS>, maxdyn));
             return B200_OK;
         });
         if (rc) return rc;
@@ -1227,6 +1230,8 @@ int set_smem_attrs(b200_plan *p) {
     CK(set_max_dyn(k_stream_matvec_f16<8, SF_GATEUP>, maxdyn));
     CK(set_max_dyn(k_rmsnorm_quant_batch<true>, maxdyn));
     CK(set_max_dyn(k_rmsnorm_quant_batch<false>, maxdyn));
+    CK(set_max_dyn(k_i8_norm<true>, maxdyn));
+    CK(set_max_dyn(k_i8_norm<false>, maxdyn));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
@@ -1965,6 +1970,125 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfP
     return B200_OK;
 }
 
+// ---- the bit-exact tensor-core prefill (prefill_i8.cuh) -----------------------------------------------------------------------
+// Built on the first b200_set_prefill_mode(TENSOR_CORE_EXACT): the chunk buffers and tensor maps over the plan's own Q8_0 streams,
+// nothing per weight.  Leaves pi8.ready false with the reason in pi8.why when the plan cannot run it.
+int prefill_init_i8(b200_plan *p) {
+    PrefillI8Ctx &c = p->pi8;
+    const b200_config &g = p->cfg;
+    const int nqkv = p->qd + 2 * p->kvd;
+    if (p->prefill_batch <= 1) { c.why = "the plan was created without a prefill batch size (prefill_batch_size <= 1)"; return B200_OK; }
+    if (p->wtype != B200_GGML_Q8_0) {
+        c.why = "the bit-exact tensor-core prefill needs a Q8_0 plan (an FP16 plan's CPU dot products are FP16 lane chains, not int8 block sums)";
+        return B200_OK;
+    }
+    if (g.tp_size > 1) { c.why = "tensor-core prefill is single-GPU"; return B200_OK; }
+    if (g.dim % 64 || p->qd % 64 || nqkv % 64) { c.why = "the bit-exact tensor-core prefill needs dim, q width and q+k+v width multiples of 64"; return B200_OK; }
+    for (const LayerW &L : p->layers)
+        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
+            if (t->seg % pg::BK) { c.why = "the bit-exact tensor-core prefill needs Q8_0 stream segments that are multiples of 64 columns"; return B200_OK; }
+    if (!pg::encode_fn()) { c.why = "cuTensorMapEncodeTiled not available from the driver"; return B200_OK; }
+    if (!c.bpad) {
+        const int bpad = (p->prefill_batch + pg::BM - 1) / pg::BM * pg::BM, big = g.dim > p->qd ? g.dim : p->qd;
+        const int lds_big = pg::i8_lds(big), lds_h = pg::i8_lds(g.hidden_dim);
+        c.att_tokens = bpad;
+        if (p->att_scratch) {
+            const size_t row = (size_t)p->nh_l * g.context_length * 4;
+            c.att_tokens = I8_ATT_SCRATCH_MAX / row < 1 ? 1 : (int)(I8_ATT_SCRATCH_MAX / row < (size_t)bpad ? I8_ATT_SCRATCH_MAX / row : bpad);
+        }
+        const size_t sizes[7] = {(size_t)bpad * g.dim * 4, (size_t)bpad * nqkv * 4, (size_t)bpad * big, (size_t)bpad * lds_big * 4,
+                                 (size_t)bpad * g.hidden_dim, (size_t)bpad * lds_h * 4, (size_t)bpad * sizeof(ChunkTok)};
+        void **dst[7] = {(void **)&c.X, (void **)&c.QKV, (void **)&c.XQ, (void **)&c.XS, (void **)&c.HQ, (void **)&c.HS, (void **)&c.tok};
+        int rc;
+        for (int i = 0; i < 7; i++) {
+            if ((rc = dalloc(p, (unsigned char **)dst[i], sizes[i]))) return rc;
+            CK(cudaMemset(*dst[i], 0, sizes[i]));
+        }
+        if (p->att_scratch && (rc = dalloc(p, &c.att, (size_t)c.att_tokens * p->nh_l * g.context_length * 4))) return rc;
+        c.bpad = bpad;
+    }
+    bool ok = pg::make_map_i8_a(&c.a_dim, c.XQ, c.bpad, g.dim) == 0 && pg::make_map_i8_s(&c.s_dim, c.XS, c.bpad, pg::i8_lds(g.dim)) == 0 &&
+              pg::make_map_i8_a(&c.a_qd, c.XQ, c.bpad, p->qd) == 0 && pg::make_map_i8_s(&c.s_qd, c.XS, c.bpad, pg::i8_lds(p->qd)) == 0 &&
+              pg::make_map_i8_a(&c.a_h, c.HQ, c.bpad, g.hidden_dim) == 0 && pg::make_map_i8_s(&c.s_h, c.HS, c.bpad, pg::i8_lds(g.hidden_dim)) == 0;
+    c.maps.resize(g.n_layers);
+    for (int l = 0; ok && l < g.n_layers; l++) {
+        const LayerW &L = p->layers[l];
+        PrefillQ8Maps &m = c.maps[l];
+        auto mk = [](CUtensorMap *q, CUtensorMap *s, const TileMat &t) {
+            return pg::make_map_i8_q8(q, t.base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 0) == 0 && pg::make_map_i8_q8(s, t.base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 1) == 0;
+        };
+        ok = mk(&m.qkv_q, &m.qkv_s, L.tqkv) && mk(&m.wo_q, &m.wo_s, L.two) && mk(&m.gu_q, &m.gu_s, L.tgu) && mk(&m.w2_q, &m.w2_s, L.tw2);
+    }
+    if (!ok) { c.why = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
+    c.ready = true;
+    c.why = "";
+    return B200_OK;
+}
+
+// One chunk: tab[v] = (token, position, KV offset) of chunk row v; own: the K / V go to the plan's cache, else to the decode slots.
+// The batched step's graph (enqueue_batch) over the whole chunk, its Q8_0 streams replaced by k_gemm_i8.  Times the chunk
+// (p->prefill_ms) and counts its launches (p->launches_prefill).
+int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own) {
+    PrefillI8Ctx &c = p->pi8;
+    const b200_config &g = p->cfg;
+    cudaStream_t s = p->stream;
+    const int n = (int)tab.size(), nqkv = p->qd + 2 * p->kvd, mt = (n + pg::BM - 1) / pg::BM;
+    const int lds_d = pg::i8_lds(g.dim), lds_q = pg::i8_lds(p->qd), lds_h = pg::i8_lds(g.hidden_dim);
+    const size_t ctx_kv = (size_t)g.context_length * p->kvd, norm_smem = norm_smem_bytes(g.dim);
+    const size_t att_smem = att_smem_bytes(g.head_size, g.context_length, c.att != nullptr);
+    const TraceBuf tr{nullptr, 0, 0};
+    TpCtx solo{};
+    solo.n = 1;
+    CK(cudaMemcpyAsync(c.tok, tab.data(), (size_t)n * sizeof(ChunkTok), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(p->ev0, s));
+    int nl = 0, rc = 0;
+    auto norm = [&](bool embed, const float *w) {
+        if (embed) k_i8_norm<true><<<n, NORM_THREADS, norm_smem, s>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
+        else k_i8_norm<false><<<n, NORM_THREADS, norm_smem, s>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
+        nl++;
+    };
+    // one k_gemm_i8 over the stream W; n_tiles from W's rows (64 stream rows per tile)
+    auto gemm = [&](auto MODE, const CUtensorMap &a, const CUtensorMap &as, const CUtensorMap &bq, const CUtensorMap &bs, const TileMat &W, float *C, int ldc,
+                    float oscale) {
+        pg::I8Out o{};
+        o.C = C; o.ldc = ldc; o.hq = c.HQ; o.hs = c.HS; o.ldq = g.hidden_dim; o.lds = lds_h;
+        o.m_valid = n; o.K = W.cols; o.seg = W.seg; o.oscale = oscale;
+        nl++;
+        return pg::gemm_i8_launch<decltype(MODE)::value>(a, as, bq, bs, o, mt, W.rows / pg::I8_BN, s) ? fail(p, B200_ERR_CUDA, "int8 GEMM launch failed") : B200_OK;
+    };
+    using F32 = std::integral_constant<int, pg::GEMM_F32>;
+    using RESID = std::integral_constant<int, pg::GEMM_RESID>;
+    using GATEUP = std::integral_constant<int, pg::GEMM_GATEUP>;
+    const float rs = p->mup.residual_scale;
+    for (int l = 0; l < g.n_layers; l++) {
+        const LayerW &L = p->layers[l];
+        const PrefillQ8Maps &m = c.maps[l];
+        float *kc = (own ? p->key_cache : p->bt.slot_k) + (size_t)l * ctx_kv, *vc = (own ? p->value_cache : p->bt.slot_v) + (size_t)l * ctx_kv;
+        norm(l == 0, L.attn_norm);
+        if ((rc = gemm(F32(), c.a_dim, c.s_dim, m.qkv_q, m.qkv_s, L.tqkv, c.QKV, nqkv, 1.0f))) return rc;
+        rc = with_decode_head_size(p, g.head_size, [&](auto HS) {
+            k_i8_rope_kv<HS><<<dim3(p->nh_l, n), 2 * HS, 0, s>>>(c.QKV, nqkv, kc, vc, c.tok, p->rope_cr, p->rope_ci, p->nh_l, p->nkv_l, p->kflags, L.q_norm,
+                                                              L.k_norm, L.qkv_bias, g.rms_norm_eps);
+            nl++;
+            for (int v0 = 0; v0 < n; v0 += c.att_tokens, nl++) // every K / V row of the chunk is in the cache before any attention reads it
+                k_i8_attention<HS><<<dim3(p->nh_l, n - v0 < c.att_tokens ? n - v0 : c.att_tokens), ATT_THREADS, att_smem, s>>>(
+                    c.QKV, nqkv, kc, vc, c.tok, v0, p->nh_l, p->nkv_l, p->kflags, att_score_arg(p), c.XQ, c.XS, lds_q, c.att, g.context_length, tr, solo);
+            return B200_OK;
+        });
+        if (rc) return rc;
+        if ((rc = gemm(RESID(), c.a_qd, c.s_qd, m.wo_q, m.wo_s, L.two, c.X, g.dim, rs))) return rc;
+        norm(false, L.ffn_norm);
+        if ((rc = gemm(GATEUP(), c.a_dim, c.s_dim, m.gu_q, m.gu_s, L.tgu, nullptr, 0, 1.0f))) return rc;
+        if ((rc = gemm(RESID(), c.a_h, c.s_h, m.w2_q, m.w2_s, L.tw2, c.X, g.dim, rs))) return rc;
+    }
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(p->ev1, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
+    p->launches_prefill = nl;
+    return B200_OK;
+}
+
 // The single-token graphs the forward calls launch: the persistent kernel's when that mode is selected and captured.
 const TokenGraphs &active_graphs(const b200_plan *p) { return p->decode_mode == B200_DECODE_PERSISTENT && p->pers.decode.exec ? p->pers : p->graph; }
 cudaGraphExec_t decode_graph(const b200_plan *p) { return active_graphs(p).decode.exec; }
@@ -2283,6 +2407,11 @@ int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, i
     if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache", start_pos, start_pos + n - 1);
     if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
     CK(cudaSetDevice(p->device));
+    if (p->pi8.ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE_EXACT) { // the whole chunk through the int8 GEMMs into the plan's cache
+        std::vector<ChunkTok> tab(n);
+        for (int i = 0; i < n; i++) tab[i] = ChunkTok{tokens[i], start_pos + i, 0};
+        return prefill_forward_i8(p, tab, true);
+    }
     if ((p->prefill.ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE) ||
         (p->prefill.q8_ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE_W8A16)) { // tensor-core GEMM path (prefill.cuh)
         memcpy(p->h_ids, tokens, (size_t)n * 4);
@@ -2381,10 +2510,22 @@ int b200_trace_persistent(b200_plan *p, int32_t token, int32_t position, uint64_
 }
 
 int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
-    if (!p || (mode != B200_PREFILL_EXACT && mode != B200_PREFILL_TENSOR_CORE && mode != B200_PREFILL_TENSOR_CORE_W8A16)) return B200_ERR_BAD_ARG;
+    if (!p || (mode != B200_PREFILL_EXACT && mode != B200_PREFILL_TENSOR_CORE && mode != B200_PREFILL_TENSOR_CORE_W8A16 &&
+               mode != B200_PREFILL_TENSOR_CORE_EXACT))
+        return B200_ERR_BAD_ARG;
     if (p->is_moe && mode != B200_PREFILL_EXACT) return fail(p, B200_ERR_UNSUPPORTED, "%s", MOE_PREFILL_WHY);
     if (p->resident && mode != B200_PREFILL_EXACT)
         return fail(p, B200_ERR_UNSUPPORTED, "this plan keeps K-quant weights resident: the tensor-core prefill reads Q8_0 tiles or f16 matrices, so prompts go through the exact prefill");
+    if (mode == B200_PREFILL_TENSOR_CORE_EXACT) {
+        if (!p->pi8.ready) {
+            CK(cudaSetDevice(p->device));
+            int rc = prefill_init_i8(p);
+            if (rc) return rc;
+            if (!p->pi8.ready) return fail(p, B200_ERR_UNSUPPORTED, "%s", p->pi8.why);
+        }
+        p->prefill.mode = mode;
+        return B200_OK;
+    }
     if (mode == B200_PREFILL_TENSOR_CORE_W8A16) {
         if (!p->prefill.q8_ready) {
             CK(cudaSetDevice(p->device));
@@ -2408,7 +2549,7 @@ int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
 
 int b200_prefill_info(b200_plan *p, int32_t *mode, int32_t *launches, float *device_ms) {
     if (!p) return B200_ERR_BAD_ARG;
-    if (mode) *mode = p->prefill.ready || p->prefill.q8_ready ? p->prefill.mode : B200_PREFILL_EXACT;
+    if (mode) *mode = p->prefill.ready || p->prefill.q8_ready || p->pi8.ready ? p->prefill.mode : B200_PREFILL_EXACT;
     if (launches) *launches = p->launches_prefill;
     if (device_ms) *device_ms = p->prefill_ms;
     return B200_OK;
@@ -2605,7 +2746,8 @@ int b200_prefill_slots(b200_plan *p, int32_t n_seqs, const int32_t *slots, const
         if (const int j = bad_token(p, tokens + off[i], lengths[i]); j >= 0)
             return fail(p, B200_ERR_BAD_ARG, "sequence %d: token %d (index %d) out of range", i, tokens[off[i] + j], j);
     const PrefillCtx &pc = p->prefill;
-    const bool tc = (pc.ready && pc.mode == B200_PREFILL_TENSOR_CORE) || (pc.q8_ready && pc.mode == B200_PREFILL_TENSOR_CORE_W8A16);
+    const bool i8 = p->pi8.ready && pc.mode == B200_PREFILL_TENSOR_CORE_EXACT;
+    const bool tc = (pc.ready && pc.mode == B200_PREFILL_TENSOR_CORE) || (pc.q8_ready && pc.mode == B200_PREFILL_TENSOR_CORE_W8A16) || i8;
     if (tc && total > p->prefill_batch) {
         int i = 0;
         while (off[i] + lengths[i] <= p->prefill_batch) i++;
@@ -2614,6 +2756,13 @@ int b200_prefill_slots(b200_plan *p, int32_t n_seqs, const int32_t *slots, const
     }
     if (!total) return B200_OK;
     CK(cudaSetDevice(p->device));
+    if (i8) { // one chunk of the call's tokens, sequence after sequence, each row writing its own slot
+        const size_t slot_stride = (size_t)c.n_layers * c.context_length * p->kvd;
+        std::vector<ChunkTok> tab;
+        for (int i = 0; i < n_seqs; i++)
+            for (int j = 0; j < lengths[i]; j++) tab.push_back(ChunkTok{tokens[off[i] + j], start_positions[i] + j, (long long)(slots[i] * slot_stride)});
+        return prefill_forward_i8(p, tab, false);
+    }
     return tc ? prefill_slots_tc(p, n_seqs, slots, start_positions, lengths, off.data(), tokens, (int)total)
               : prefill_slots_exact(p, n_seqs, slots, start_positions, lengths, off.data(), tokens);
 }
@@ -3074,6 +3223,57 @@ int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, i
             else if (lr) s.rc = B200_ERR_CUDA;
         }
         if (s.ok(cudaDeviceSynchronize()) && s.rc == B200_OK) s.ok(cudaMemcpy(c, dc, c_bytes, cudaMemcpyDeviceToHost));
+    }
+    return s.rc;
+}
+
+int b200_test_gemm_i8(int32_t mode, int32_t m, int32_t n, int32_t k, const int8_t *aq, const float *as, const void *bq, const void *bq2, float oscale,
+                      float *c, int8_t *hq, float *hs) {
+    const bool gateup = mode == pg::GEMM_GATEUP;
+    if (mode < pg::GEMM_F32 || mode > pg::GEMM_GATEUP || !aq || !as || !bq || m < 1 || n < 1 || k < 1 || k % 32) return B200_ERR_BAD_ARG;
+    if (gateup ? (!bq2 || !hq || !hs || n % 32) : (!c || n % pg::I8_BN)) return B200_ERR_BAD_ARG;
+    const int nseg = smv_pick_nseg(k);
+    if (!nseg || (k / nseg) % pg::BK) return B200_ERR_BAD_ARG;
+    const int seg = k / nseg, unit = smv_unit_bytes(seg), rows = gateup ? 2 * n : n, mpad = (m + pg::BM - 1) / pg::BM * pg::BM;
+    const int lds = pg::i8_lds(k), nb = k / 32;
+    const size_t q8_bytes = (size_t)n * nb * 34, stream_bytes = (size_t)rows * nseg * unit;
+    int8_t *daq = nullptr, *dhq = nullptr;
+    float *das = nullptr, *dc = nullptr, *dhs = nullptr;
+    unsigned char *draw = nullptr, *dstream = nullptr;
+    Scratch s;
+    // rows m .. mpad - 1 of A hold large quants and scales: a tile row past m_valid is computed but must never be stored
+    if (s.alloc(&daq, (size_t)mpad * k) && s.alloc(&das, (size_t)mpad * lds * 4) && s.alloc(&draw, q8_bytes * (gateup ? 2 : 1)) &&
+        s.alloc(&dstream, stream_bytes) && s.ok(cudaMemset(daq, 0x7F, (size_t)mpad * k)) && s.ok(cudaMemset(das, 0x7F, (size_t)mpad * lds * 4)) &&
+        s.ok(cudaMemcpy(daq, aq, (size_t)m * k, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy2D(das, (size_t)lds * 4, as, (size_t)nb * 4, (size_t)nb * 4, m, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(draw, bq, q8_bytes, cudaMemcpyHostToDevice)) && (!gateup || s.ok(cudaMemcpy(draw + q8_bytes, bq2, q8_bytes, cudaMemcpyHostToDevice))) &&
+        (gateup ? s.alloc(&dhq, (size_t)m * n) && s.alloc(&dhs, (size_t)m * (n / 32) * 4) && s.ok(cudaMemcpy(dhq, hq, (size_t)m * n, cudaMemcpyHostToDevice)) &&
+                      s.ok(cudaMemcpy(dhs, hs, (size_t)m * (n / 32) * 4, cudaMemcpyHostToDevice))
+                : s.alloc(&dc, (size_t)m * n * 4) && s.ok(cudaMemcpy(dc, c, (size_t)m * n * 4, cudaMemcpyHostToDevice)))) {
+        RepackSrc src{};
+        src.raw[0] = draw;
+        src.rows[0] = n;
+        if (gateup) { src.raw[1] = draw + q8_bytes; src.rows[1] = n; }
+        src.gateup = gateup ? 1 : 0;
+        k_repack_tiles<<<(unsigned)((size_t)rows * nseg), 128>>>(src, dstream, rows, k, seg, nseg, unit);
+        s.ok(cudaGetLastError());
+        // the maps prefill_init_i8 builds
+        CUtensorMap ma, ms, mq, mqs;
+        if (s.rc == B200_OK && (pg::make_map_i8_a(&ma, daq, (uint64_t)mpad, (uint64_t)k) || pg::make_map_i8_s(&ms, das, (uint64_t)mpad, (uint64_t)lds) ||
+                                pg::make_map_i8_q8(&mq, dstream, (uint64_t)rows, nseg, unit, 0) || pg::make_map_i8_q8(&mqs, dstream, (uint64_t)rows, nseg, unit, 1)))
+            s.rc = B200_ERR_CUDA;
+        if (s.rc == B200_OK) {
+            pg::I8Out o{};
+            o.C = dc; o.ldc = n; o.hq = dhq; o.hs = dhs; o.ldq = n; o.lds = n / 32;
+            o.m_valid = m; o.K = k; o.seg = seg; o.oscale = oscale;
+            const int lr = with_gemm_mode(mode, [&](auto MODE) { return pg::gemm_i8_launch<MODE>(ma, ms, mq, mqs, o, mpad / pg::BM, rows / pg::I8_BN, 0); });
+            if (lr == -6) s.rc = B200_ERR_BAD_ARG;
+            else if (lr) s.rc = B200_ERR_CUDA;
+        }
+        if (s.ok(cudaDeviceSynchronize()) && s.rc == B200_OK) {
+            if (gateup) s.ok(cudaMemcpy(hq, dhq, (size_t)m * n, cudaMemcpyDeviceToHost)) && s.ok(cudaMemcpy(hs, dhs, (size_t)m * (n / 32) * 4, cudaMemcpyDeviceToHost));
+            else s.ok(cudaMemcpy(c, dc, (size_t)m * n * 4, cudaMemcpyDeviceToHost));
+        }
     }
     return s.rc;
 }

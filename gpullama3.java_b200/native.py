@@ -61,7 +61,7 @@ class Tensor(C.Structure):
 
 EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
-           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
+           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
            "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_weight_info", "b200_test_set_memory_budget",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
@@ -103,6 +103,7 @@ def lib() -> C.CDLL:
     L.b200_gemm_f16.argtypes = [vp, vp, vp, i32, i32, i32, i32, C.POINTER(C.c_float)]
     L.b200_test_gemm.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.b200_test_gemm_q8.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
+    L.b200_test_gemm_i8.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, C.c_float, vp, vp, vp]
     L.b200_test_pf_attention.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.b200_time_kernel.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
     L.b200_read_buffer.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
@@ -253,6 +254,38 @@ def test_gemm_q8(mode: str, a, bq, c, bq2=None, m_valid: int | None = None, stag
                                  bq2.ctypes.data if gateup else None, c.ctypes.data)
     if rc != B200_OK:
         _raise(rc, "b200_test_gemm_q8 failed")
+    return c
+
+
+def test_gemm_i8(mode: str, aq, a_scales, bq, c=None, bq2=None, oscale: float = 1.0, hq=None, hs=None):
+    """One launch of the int8 GEMM of B200_PREFILL_TENSOR_CORE_EXACT (csrc/prefill_i8.cuh) as the prefill issues it.  aq int8 [M,K],
+    a_scales float32 [M, K/32], bq (and bq2, the up projection, for "gateup") GGUF Q8_0 blocks uint8 [N, K/32*34].  "f32" / "resid":
+    c float32 [M,N] (resid adds fl(acc * oscale) to it); returns the new c.  "gateup": N hidden units, hq int8 [M,N] and hs float32
+    [M, N/32] initial contents; returns the new (hq, hs)."""
+    aq = np.ascontiguousarray(aq, dtype=np.int8)
+    a_scales = np.ascontiguousarray(a_scales, dtype=np.float32)
+    bq = np.ascontiguousarray(bq, dtype=np.uint8)
+    m, k = aq.shape
+    n = bq.shape[0]
+    if a_scales.shape != (m, k // 32) or bq.shape != (n, k // 32 * 34) or k % 32:
+        raise ValueError("shapes do not match")
+    if mode == "gateup":
+        bq2 = np.ascontiguousarray(bq2, dtype=np.uint8)
+        hq = np.array(np.zeros((m, n), np.int8) if hq is None else hq, dtype=np.int8, order="C", copy=True)
+        hs = np.array(np.zeros((m, n // 32), np.float32) if hs is None else hs, dtype=np.float32, order="C", copy=True)
+        if bq2.shape != bq.shape or hq.shape != (m, n) or hs.shape != (m, n // 32):
+            raise ValueError("shapes do not match")
+        rc = lib().b200_test_gemm_i8(GEMM_MODES[mode], m, n, k, aq.ctypes.data, a_scales.ctypes.data, bq.ctypes.data, bq2.ctypes.data, oscale, None,
+                                     hq.ctypes.data, hs.ctypes.data)
+        if rc != B200_OK:
+            _raise(rc, "b200_test_gemm_i8 failed")
+        return hq, hs
+    c = np.array(np.zeros((m, n), np.float32) if c is None else c, dtype=np.float32, order="C", copy=True)
+    if c.shape != (m, n):
+        raise ValueError("shapes do not match")
+    rc = lib().b200_test_gemm_i8(GEMM_MODES[mode], m, n, k, aq.ctypes.data, a_scales.ctypes.data, bq.ctypes.data, None, oscale, c.ctypes.data, None, None)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_gemm_i8 failed")
     return c
 
 

@@ -222,10 +222,21 @@ int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n
  *                            residual GEMM splits K (the order of the f32 reduce-adds is not fixed in either mode).
  *                            The first call allocates the prefill scratch and builds tensor maps only.  Needs every
  *                            stream segment to be a multiple of 64 columns; B200_ERR_UNSUPPORTED with the reason
- *                            otherwise.  The two tensor-core modes can be switched in either order on one plan. */
+ *                            otherwise.  The two tensor-core modes can be switched in either order on one plan.
+ *   B200_PREFILL_TENSOR_CORE_EXACT  the whole chunk (<= prefill_batch_size tokens) on a single-GPU Q8_0 plan (K-quant files
+ *                            expanded to Q8_0 tiles included) through int8 tensor-core GEMMs (wgmma s8 x s8 -> s32, one per
+ *                            32-column Q8_0 block) that read the tile-major Q8_0 streams in place and add each block's term
+ *                            fl(isum * fl(wScale * aScale)) in the CPU path's block order; norms, RoPE / KV and attention run
+ *                            the exact per-row bodies over the chunk.  KV cache bit-identical to the CPU path, as
+ *                            B200_PREFILL_EXACT.  Any head size the plan decodes.  The first call allocates the chunk buffers
+ *                            and builds tensor maps only.  B200_ERR_UNSUPPORTED with the reason (the previous mode stays in
+ *                            force) on FP16, tensor-parallel, Qwen2-MoE and resident K-quant plans, plans created without a
+ *                            prefill batch size, and plans whose dim, q or q+k+v widths or stream segments are not multiples
+ *                            of 64 columns.  Applies to b200_forward_batch_prefill and b200_prefill_slots. */
 #define B200_PREFILL_EXACT 0
 #define B200_PREFILL_TENSOR_CORE 1
 #define B200_PREFILL_TENSOR_CORE_W8A16 2
+#define B200_PREFILL_TENSOR_CORE_EXACT 3
 int b200_set_prefill_mode(b200_plan *plan, int32_t mode);
 
 /* Active mode, kernels launched and device milliseconds of the last tensor-core chunk (any pointer may be NULL). */
@@ -456,6 +467,15 @@ int b200_test_gemm(int32_t mode, int32_t stages, int32_t splits, int32_t m, int3
  * rejected with B200_ERR_BAD_ARG, like the shapes and split counts b200_test_gemm rejects. */
 int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, int32_t m_valid, int32_t n, int32_t k, const uint16_t *a, const void *bq,
                       const void *bq2 /* GATEUP only */, void *c);
+
+/* Test hook: ONE launch of the int8 GEMM of B200_PREFILL_TENSOR_CORE_EXACT exactly as the prefill launches it, on m activation
+ * rows (any m >= 1; padded to whole 128-row tiles with rows that must never be stored).  aq: int8 [m][k]; as: their f32 block
+ * scales [m][k / 32]; bq (and bq2 = the up projection for GATEUP): GGUF Q8_0 blocks [n][k / 32 * 34], repacked into the
+ * tile-major stream by the plan's upload kernel.  mode 0 (STORE): c = f32 [m][n] out; 1 (RESID): c[i][j] = fl(c + fl(acc * oscale))
+ * in/out; n a multiple of 64.  2 (GATEUP): n hidden units (a multiple of 32), hq = int8 [m][n] and hs = f32 [m][n / 32], the
+ * Q8_0 quantisation of swiglu(gate, up), in/out.  K whose stream segment is not a multiple of 64 columns: B200_ERR_BAD_ARG. */
+int b200_test_gemm_i8(int32_t mode, int32_t m, int32_t n, int32_t k, const int8_t *aq, const float *as, const void *bq, const void *bq2, float oscale,
+                      float *c, int8_t *hq, float *hs);
 
 /* Test hook: the causal attention of the tensor-core prefill over one chunk of n query tokens at positions start_pos ..
  * start_pos + n - 1.  q: f32 [n][n_heads * head_size] (rotated); k, v: f32 [start_pos + n][n_kv_heads * head_size] (the KV cache

@@ -32,6 +32,7 @@ namespace {
 struct LayerW {
     DevMat qkv, wo, w1, w3, w2;
     TileMat tqkv{}, two{}, tgu{}, tw2{}; // tile-major copies for the streaming kernel (Q8_0)
+    size_t ring_qkv = 0, ring_gu = 0;    // dynamic shared memory of the QKV and gate/up stream launches (ring_budgets)
     float *attn_norm = nullptr, *ffn_norm = nullptr, *q_norm = nullptr, *k_norm = nullptr;
     float *qkv_bias = nullptr; // Qwen2: this rank's q|k|v bias, laid out like the packed q|k|v vector
     // Qwen2-MoE (moe.cuh): the shared expert's streams, the routed experts' geometry and the device tables of their stream bases
@@ -431,6 +432,48 @@ TileMat tile_geometry(int rows, int cols, int fmt) {
 }
 int64_t tile_bytes(const TileMat &t) { return (int64_t)tile_groups(t) * 4 * t.nseg * t.unit_bytes; }
 
+// ---- ring sizes of the decode weight streams (DESIGN.md section 5a) -----------------------------------------------------------
+// Under PDL the next kernel of the chain becomes resident while its predecessor still runs, and a stream kernel's producer fills
+// its ring before the dependency wait returns.  During the chain's latency phases (the fused norm's exact sum, the attention) the
+// resident rings are all that keep HBM busy, so a ring is sized for the kernels it must stay resident beside: its CTA and each
+// neighbour's, with a per-CTA reserve each, within the SM's shared memory.  QKV sits between W2 (before it) and the attention
+// (after it); gate/up between Wo and W2.  Wo, W2 and lm_head keep SMV_SMEM_BUDGET_MAX, which is also the floor of every budget
+// and what the shape checks use, so a device with less shared memory refuses no plan it ran before.
+struct SmDev {
+    size_t sm, reserve, optin; // shared memory per SM, reserved per resident CTA, opt-in limit per CTA
+};
+
+size_t stream_smem(const TileMat &W, bool norm, size_t budget) {
+    unsigned a, b;
+    return (norm ? smv_layout_norm(W.cols, W.seg, budget, &a, &b, W.fmt) : smv_layout(W.cols, W.seg, budget, W.fmt)).total;
+}
+int slice_tiles(const TileMat &W, int n_sms) { return (tile_groups(W) + n_sms - 1) / n_sms * W.nseg; } // the largest CTA slice
+
+// The budget of stream W between CTAs that take `before` and `after` bytes of shared memory: as many stages as fit beside the
+// larger of the two, but no more than its largest CTA slice (a stage it never fills would only crowd out its neighbours).
+size_t ring_budget(const SmDev &d, const TileMat &W, bool norm, int n_sms, size_t before, size_t after) {
+    const size_t nb = (before > after ? before : after) + 2 * d.reserve;
+    size_t room = d.sm > nb ? d.sm - nb : 0;
+    if (room > d.optin) room = d.optin;
+    if (room <= SMV_SMEM_BUDGET_MAX) return SMV_SMEM_BUDGET_MAX;
+    unsigned a, b;
+    const SmvSmem L = norm ? smv_layout_norm(W.cols, W.seg, room, &a, &b, W.fmt) : smv_layout(W.cols, W.seg, room, W.fmt);
+    const int s = L.stages < slice_tiles(W, n_sms) ? L.stages : slice_tiles(W, n_sms);
+    const size_t need = L.off_ring + (size_t)s * L.stage_bytes;
+    return need > SMV_SMEM_BUDGET_MAX ? need : SMV_SMEM_BUDGET_MAX;
+}
+
+// The streams that open with a latency phase get the larger rings: QKV (the attention norm's exact sum) between W2 of layer prev
+// (l - 1; layer 0 takes its own) and the attention (att bytes), and gate/up (the FFN norm's) between Wo and W2.  Their neighbours
+// keep SMV_SMEM_BUDGET_MAX: a larger Wo would keep gate/up from entering beside it, and measured slower (DESIGN.md section 6).
+// norm: the plan's QKV and gate/up compute their RMSNorm (k_stream_matvec_q8_norm).
+void ring_budgets(const SmDev &d, int n_sms, bool norm, size_t att, const LayerW &prev, LayerW &L) {
+    // a Qwen2-MoE layer has no tw2 / tgu: its down and gate/up streams (moe.cuh) take at most SMV_SMEM_BUDGET_MAX
+    auto at_floor = [](const TileMat &W, bool nrm) { return W.nseg ? stream_smem(W, nrm, SMV_SMEM_BUDGET_MAX) : SMV_SMEM_BUDGET_MAX; };
+    L.ring_qkv = ring_budget(d, L.tqkv, norm, n_sms, at_floor(prev.tw2, false), att);
+    L.ring_gu = L.tgu.nseg ? ring_budget(d, L.tgu, norm, n_sms, at_floor(L.two, false), at_floor(L.tw2, false)) : SMV_SMEM_BUDGET_MAX;
+}
+
 // The format a stream of these stacked sources keeps on a resident plan: their common K-quant type when every present source has
 // it and the resident layout leaves at least 3 ring stages; else 0 (the stream is re-quantised to Q8_0 tiles at upload).
 int resident_fmt(const b200_tensor *const ts[3], const int rs[3], int rows, int cols) {
@@ -656,10 +699,10 @@ template <int MODE> void (*smv_norm_kernel(int fmt))(SmvArgs, SmvSmem, SmvNormAr
 }
 
 template <int MODE>
-int launch_stream(b200_plan *p, const TileMat &W, const int8_t *xq, const float *xs, float *out, int8_t *hq, float *hs, bool argmax = false,
+int launch_stream(b200_plan *p, const TileMat &W, size_t budget, const int8_t *xq, const float *xs, float *out, int8_t *hq, float *hs, bool argmax = false,
                   TraceBuf tr = TraceBuf{nullptr, 0, 0}, int wait_slot = -1, unsigned wait_op = 0, int out_slot = -1, unsigned out_op = 0,
                   int row_base = 0) {
-    SmvSmem L = smv_layout(W.cols, W.seg, SMV_SMEM_BUDGET_MAX, W.fmt);
+    SmvSmem L = smv_layout(W.cols, W.seg, budget, W.fmt);
     SmvArgs a;
     a.W = W; a.xq = xq; a.xs = xs; a.out = out; a.hq = hq; a.hs = hs; a.blk_cnt = p->blk_cnt;
     a.oscale = out_scale(p, MODE == SMV_RESID, &W == &p->tout);
@@ -674,9 +717,10 @@ int launch_stream(b200_plan *p, const TileMat &W, const int8_t *xq, const float 
 // A stream kernel behind a fused RMSNorm of the residual stream x (weights w; from_emb: layer 0, the embedding row, which CTA 0
 // also writes to x).  MODE is SMV_STORE (QKV, lm_head) or SMV_GATEUP.
 template <int MODE>
-int launch_stream_norm(b200_plan *p, const TileMat &W, const float *w, bool from_emb, float *out, int8_t *hq, float *hs, bool argmax, TraceBuf tr, int row_base = 0) {
+int launch_stream_norm(b200_plan *p, const TileMat &W, size_t budget, const float *w, bool from_emb, float *out, int8_t *hq, float *hs, bool argmax, TraceBuf tr,
+                       int row_base = 0) {
     SmvNormArgs n;
-    const SmvSmem L = smv_layout_norm(W.cols, W.seg, SMV_SMEM_BUDGET_MAX, &n.off_sq, &n.off_seq, W.fmt);
+    const SmvSmem L = smv_layout_norm(W.cols, W.seg, budget, &n.off_sq, &n.off_seq, W.fmt);
     n.x = p->x; n.w = w; n.st = p->st; n.emb = p->emb; n.emb_scale = p->mup.embedding_scale; n.eps = p->cfg.rms_norm_eps;
     n.from_emb = from_emb ? 1 : 0; n.x_out = p->x;
     SmvArgs a;
@@ -765,11 +809,11 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
         LayerW &L = p->layers[l];
         int rc;
         // TP flag epochs inside one forward: op = 4*l + {0: attention out, 1: x after Wo, 2: hb, 3: x after W2}
-        if (fz) rc = launch_stream_norm<SMV_STORE>(p, L.tqkv, L.attn_norm, l == 0, p->qkv, nullptr, nullptr, false, TR(2)); // attention norm + QKV
+        if (fz) rc = launch_stream_norm<SMV_STORE>(p, L.tqkv, L.ring_qkv, L.attn_norm, l == 0, p->qkv, nullptr, nullptr, false, TR(2)); // attention norm + QKV
         else {
             if ((rc = norm(l == 0, L.attn_norm, l == 0 ? -1 : 4 * (l - 1) + 3))) return rc;
             n++;
-            if (q8) rc = launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr, false, TR(2));
+            if (q8) rc = launch_stream<SMV_STORE>(p, L.tqkv, L.ring_qkv, p->xq, p->xs, p->qkv, nullptr, nullptr, false, TR(2));
             else if (sf) rc = launch_stream_f16<SF_STORE>(p, L.qkv, nullptr, p->xb, p->qkv, TR(2));
             else rc = launch_matvec_f16<MODE_STORE>(p, L.qkv, p->xb, p->qkv);
         }
@@ -783,7 +827,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
                             p->tp, (unsigned)(4 * l + 0), rank * p->nh_l, p->att_scratch, c.context_length);
         });
         if (rc) return rc; n++;
-        if (q8) rc = launch_stream<SMV_RESID>(p, L.two, p->attq, p->atts, p->x, nullptr, nullptr, false, TR(5), tpar ? TP_SLOT_ATT : -1, 4 * l + 0, tpar ? TP_SLOT_X : -1, 4 * l + 1, rank * p->dim_l);
+        if (q8) rc = launch_stream<SMV_RESID>(p, L.two, SMV_SMEM_BUDGET_MAX, p->attq, p->atts, p->x, nullptr, nullptr, false, TR(5), tpar ? TP_SLOT_ATT : -1, 4 * l + 0, tpar ? TP_SLOT_X : -1, 4 * l + 1, rank * p->dim_l);
         else if (sf) rc = launch_stream_f16<SF_RESID>(p, L.wo, nullptr, p->xb, p->x, TR(5));
         else rc = launch_matvec_f16<MODE_RESID>(p, L.wo, p->xb, p->x);
         if (rc) return rc; n++;
@@ -797,10 +841,10 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
             n++;
         }
         if (q8) {
-            if (fz) rc = launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, TR(6)); // FFN norm + gate/up
-            else rc = launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs, false, TR(6), -1, 0, tpar ? TP_SLOT_HQ : -1, 4 * l + 2, rank * p->hid_l);
+            if (fz) rc = launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ring_gu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, TR(6)); // FFN norm + gate/up
+            else rc = launch_stream<SMV_GATEUP>(p, L.tgu, L.ring_gu, p->xq, p->xs, p->hb, p->hq, p->hs, false, TR(6), -1, 0, tpar ? TP_SLOT_HQ : -1, 4 * l + 2, rank * p->hid_l);
             if (rc) return rc; n++;
-            if ((rc = launch_stream<SMV_RESID>(p, L.tw2, p->hq, p->hs, p->x, nullptr, nullptr, false, TR(7), tpar ? TP_SLOT_HQ : -1, 4 * l + 2, tpar ? TP_SLOT_X : -1, 4 * l + 3, rank * p->dim_l))) return rc; n++;
+            if ((rc = launch_stream<SMV_RESID>(p, L.tw2, SMV_SMEM_BUDGET_MAX, p->hq, p->hs, p->x, nullptr, nullptr, false, TR(7), tpar ? TP_SLOT_HQ : -1, 4 * l + 2, tpar ? TP_SLOT_X : -1, 4 * l + 3, rank * p->dim_l))) return rc; n++;
         } else if (sf) { // gate, up and SwiGLU in one launch; then the down projection
             if ((rc = launch_stream_f16<SF_GATEUP>(p, L.w1, &L.w3, p->xb, p->hb, TR(6)))) return rc; n++;
             if ((rc = launch_stream_f16<SF_RESID>(p, L.w2, nullptr, p->hb, p->x, TR(7)))) return rc; n++;
@@ -816,11 +860,11 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
     if (with_logits) {
         // rmsnorm(x, x, rms_final_weight) then wcls.matmul (InferenceCore.java:167-169)
         int rc;
-        if (fz) rc = launch_stream_norm<SMV_STORE>(p, p->tout, p->out_norm, false, p->logits, nullptr, nullptr, true, TR(8)); // final norm + lm_head
+        if (fz) rc = launch_stream_norm<SMV_STORE>(p, p->tout, SMV_SMEM_BUDGET_MAX, p->out_norm, false, p->logits, nullptr, nullptr, true, TR(8)); // final norm + lm_head
         else {
             if ((rc = norm(false, p->out_norm, last_x_op))) return rc;
             n++;
-            if (q8) rc = launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr, true, TR(8), -1, 0, -1, 0, rank * p->voc_l);
+            if (q8) rc = launch_stream<SMV_STORE>(p, p->tout, SMV_SMEM_BUDGET_MAX, p->xq, p->xs, p->logits, nullptr, nullptr, true, TR(8), -1, 0, -1, 0, rank * p->voc_l);
             else if (sf) rc = launch_stream_f16<SF_STORE>(p, p->out, nullptr, p->xb, p->logits, TR(8), true);
             else rc = launch_matvec_f16<MODE_STORE>(p, p->out, p->xb, p->logits);
         }
@@ -1208,17 +1252,12 @@ int set_smem_attrs(b200_plan *p) {
         });
         if (rc) return rc;
     }
-    CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-    CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_RESID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-    CK(cudaFuncSetAttribute(k_stream_matvec_q8<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-    CK(cudaFuncSetAttribute(k_stream_matvec_q8_norm<SMV_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-    CK(cudaFuncSetAttribute(k_stream_matvec_q8_norm<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-    for (int fmt : {B200_GGML_Q4_K, B200_GGML_Q5_K, B200_GGML_Q6_K}) {
-        CK(cudaFuncSetAttribute(smv_kernel<SMV_STORE>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-        CK(cudaFuncSetAttribute(smv_kernel<SMV_RESID>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-        CK(cudaFuncSetAttribute(smv_kernel<SMV_GATEUP>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-        CK(cudaFuncSetAttribute(smv_norm_kernel<SMV_STORE>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-        CK(cudaFuncSetAttribute(smv_norm_kernel<SMV_GATEUP>(fmt), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    for (int fmt : {0, B200_GGML_Q4_K, B200_GGML_Q5_K, B200_GGML_Q6_K}) { // the single-token streams: budgets up to the opt-in limit (ring_budgets)
+        CK(set_max_dyn(smv_kernel<SMV_STORE>(fmt), maxdyn));
+        CK(set_max_dyn(smv_kernel<SMV_RESID>(fmt), maxdyn));
+        CK(set_max_dyn(smv_kernel<SMV_GATEUP>(fmt), maxdyn));
+        CK(set_max_dyn(smv_norm_kernel<SMV_STORE>(fmt), maxdyn));
+        CK(set_max_dyn(smv_norm_kernel<SMV_GATEUP>(fmt), maxdyn));
     }
     CK(set_max_dyn(k_matvec_f16<MODE_STORE>, maxdyn));
     CK(set_max_dyn(k_matvec_f16<MODE_RESID>, maxdyn));
@@ -1240,6 +1279,27 @@ int set_smem_attrs(b200_plan *p) {
     CK(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     CK(cudaFuncSetAttribute(k_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     done = true;
+    return B200_OK;
+}
+
+// Every layer's QKV and gate/up ring budget (ring_budgets), from the device's shared-memory figures and this plan's attention launch.
+int size_rings(b200_plan *p) {
+    const b200_config &c = p->cfg;
+    if (p->wtype != B200_GGML_Q8_0) return B200_OK; // no tile-major streams
+    int sm = 0, reserve = 0, optin = 0;
+    CK(cudaDeviceGetAttribute(&sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, p->device));
+    CK(cudaDeviceGetAttribute(&reserve, cudaDevAttrReservedSharedMemoryPerBlock, p->device));
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device));
+    size_t att = att_smem_bytes(c.head_size, c.context_length, p->att_scratch != nullptr);
+    const int rc = with_decode_head_size(p, c.head_size, [&](auto HS) {
+        cudaFuncAttributes fa;
+        CK(cudaFuncGetAttributes(&fa, k_attention<HS>));
+        att += fa.sharedSizeBytes;
+        return B200_OK;
+    });
+    if (rc) return rc;
+    const SmDev d{(size_t)sm, (size_t)reserve, (size_t)optin};
+    for (int l = 0; l < c.n_layers; l++) ring_budgets(d, p->n_sms, p->fuse_norm, att, p->layers[l ? l - 1 : 0], p->layers[l]);
     return B200_OK;
 }
 
@@ -1724,6 +1784,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     if (3 * c.head_size + c.context_length > ATT_SMEM_FLOATS_MAX) { // long context: score rows in global memory
         if ((rc = dalloc(p, &p->att_scratch, (size_t)p->nh_l * ((c.context_length + PD_CT - 1) / PD_CT * PD_CT) * 4))) return rc;
     }
+    if ((rc = size_rings(p))) return rc;
     if ((rc = set_smem_attrs(p))) return rc;
     if (c.tp_size > 1) { CK(cudaStreamSynchronize(p->stream)); return B200_OK; } // graphs are captured by b200_tp_attach
     if ((rc = capture_all(p))) return rc;
@@ -2890,18 +2951,18 @@ int b200_time_kernel(b200_plan *p, int32_t which, int32_t reps, float *avg_ms, i
         switch (which) {
         case 0:
             bytes = tb(L.tgu) + nw;
-            return fz ? launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, none)
-                      : launch_stream<SMV_GATEUP>(p, L.tgu, p->xq, p->xs, p->hb, p->hq, p->hs);
-        case 1: bytes = tb(L.tw2); return launch_stream<SMV_RESID>(p, L.tw2, p->hq, p->hs, p->x, nullptr, nullptr);
+            return fz ? launch_stream_norm<SMV_GATEUP>(p, L.tgu, L.ring_gu, L.ffn_norm, false, p->hb, p->hq, p->hs, false, none)
+                      : launch_stream<SMV_GATEUP>(p, L.tgu, L.ring_gu, p->xq, p->xs, p->hb, p->hq, p->hs);
+        case 1: bytes = tb(L.tw2); return launch_stream<SMV_RESID>(p, L.tw2, SMV_SMEM_BUDGET_MAX, p->hq, p->hs, p->x, nullptr, nullptr);
         case 2:
             bytes = tb(L.tqkv) + nw;
-            return fz ? launch_stream_norm<SMV_STORE>(p, L.tqkv, L.attn_norm, false, p->qkv, nullptr, nullptr, false, none)
-                      : launch_stream<SMV_STORE>(p, L.tqkv, p->xq, p->xs, p->qkv, nullptr, nullptr);
-        case 3: bytes = tb(L.two); return launch_stream<SMV_RESID>(p, L.two, p->xq, p->xs, p->x, nullptr, nullptr);
+            return fz ? launch_stream_norm<SMV_STORE>(p, L.tqkv, L.ring_qkv, L.attn_norm, false, p->qkv, nullptr, nullptr, false, none)
+                      : launch_stream<SMV_STORE>(p, L.tqkv, L.ring_qkv, p->xq, p->xs, p->qkv, nullptr, nullptr);
+        case 3: bytes = tb(L.two); return launch_stream<SMV_RESID>(p, L.two, SMV_SMEM_BUDGET_MAX, p->xq, p->xs, p->x, nullptr, nullptr);
         default:
             bytes = tb(p->tout) + nw;
-            return fz ? launch_stream_norm<SMV_STORE>(p, p->tout, p->out_norm, false, p->logits, nullptr, nullptr, false, none)
-                      : launch_stream<SMV_STORE>(p, p->tout, p->xq, p->xs, p->logits, nullptr, nullptr);
+            return fz ? launch_stream_norm<SMV_STORE>(p, p->tout, SMV_SMEM_BUDGET_MAX, p->out_norm, false, p->logits, nullptr, nullptr, false, none)
+                      : launch_stream<SMV_STORE>(p, p->tout, SMV_SMEM_BUDGET_MAX, p->xq, p->xs, p->logits, nullptr, nullptr);
         }
     };
     auto f16_stream = [&](LayerW &L) -> int { // FP16 streaming kernels
@@ -3357,6 +3418,38 @@ int b200_weight_info(b200_plan *p, int32_t *resident, int64_t *weight_bytes, int
     if (resident) *resident = p->resident ? 1 : 0;
     if (weight_bytes) *weight_bytes = p->w_bytes;
     if (q8_weight_bytes) *q8_weight_bytes = p->w8_bytes;
+    return B200_OK;
+}
+
+int b200_stream_rings(const int32_t *shape, const int64_t *dev, int64_t *out) {
+    if (!shape || !dev || !out) return B200_ERR_BAD_ARG;
+    const int dim = shape[0], qd = shape[1], kvd = shape[2], hidden = shape[3], n_sms = shape[4];
+    if (dim <= 0 || qd <= 0 || kvd <= 0 || hidden <= 0 || n_sms <= 0) return B200_ERR_BAD_ARG;
+    for (int k = 0; k < 4; k++) {
+        const int f = shape[6 + k];
+        if (f != 0 && !kq_is_kquant(f)) return B200_ERR_BAD_ARG;
+    }
+    LayerW L;
+    L.tqkv = tile_geometry(qd + 2 * kvd, dim, shape[6]);
+    L.two = tile_geometry(dim, qd, shape[7]);
+    L.tgu = tile_geometry(2 * hidden, dim, shape[8]);
+    L.tw2 = tile_geometry(dim, hidden, shape[9]);
+    const TileMat *ms[4] = {&L.tqkv, &L.two, &L.tgu, &L.tw2};
+    for (const TileMat *m : ms)
+        if (!m->nseg) return B200_ERR_UNSUPPORTED;
+    const bool norm = shape[5] != 0;
+    ring_budgets(SmDev{(size_t)dev[0], (size_t)dev[1], (size_t)dev[2]}, n_sms, norm, (size_t)dev[3], L, L);
+    const size_t budgets[4] = {L.ring_qkv, SMV_SMEM_BUDGET_MAX, L.ring_gu, SMV_SMEM_BUDGET_MAX};
+    const bool norms[4] = {norm, false, norm, false};
+    for (int k = 0; k < 4; k++) {
+        const TileMat &W = *ms[k];
+        unsigned a, b;
+        const SmvSmem S = norms[k] ? smv_layout_norm(W.cols, W.seg, budgets[k], &a, &b, W.fmt) : smv_layout(W.cols, W.seg, budgets[k], W.fmt);
+        out[4 * k + 0] = (int64_t)S.total;
+        out[4 * k + 1] = S.stages;
+        out[4 * k + 2] = S.stage_bytes;
+        out[4 * k + 3] = slice_tiles(W, n_sms);
+    }
     return B200_OK;
 }
 

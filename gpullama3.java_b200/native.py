@@ -63,7 +63,7 @@ EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
-           "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_weight_info", "b200_test_set_memory_budget",
+           "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_weight_info", "b200_test_set_memory_budget", "b200_stream_rings",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -120,6 +120,7 @@ def lib() -> C.CDLL:
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     L.b200_weight_info.argtypes = [vp, C.POINTER(i32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.b200_test_set_memory_budget.argtypes = [C.c_int64]
+    L.b200_stream_rings.argtypes = [C.POINTER(i32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.b200_launches_per_decode.argtypes = [vp]
     L.b200_device_bytes.argtypes = [vp]
     L.b200_device_bytes.restype = C.c_int64
@@ -179,6 +180,21 @@ def test_set_memory_budget(n_bytes: int):
     rc = lib().b200_test_set_memory_budget(int(n_bytes))
     if rc != B200_OK:
         _raise(rc, f"b200_test_set_memory_budget({n_bytes}) failed")
+
+
+def stream_rings(dim: int, q_width: int, kv_width: int, hidden: int, n_sms: int, fused_norm: bool, fmts=(0, 0, 0, 0),
+                 sm_bytes: int = 233472, reserve_bytes: int = 1024, optin_bytes: int = 232448, att_bytes: int = 0) -> dict:
+    """b200_stream_rings: the rings plan creation gives one layer's QKV, Wo, gate/up and W2 streams (fmts: their tile formats,
+    0 or a resident K-quant type) on a device with these shared-memory figures (defaults: H100).  Per stream: smem (dynamic
+    shared memory of the launch), stages, stage_bytes and slice_tiles (the largest CTA slice)."""
+    shape = (C.c_int32 * 10)(dim, q_width, kv_width, hidden, n_sms, 1 if fused_norm else 0, *fmts)
+    dev = (C.c_int64 * 4)(sm_bytes, reserve_bytes, optin_bytes, att_bytes)
+    out = (C.c_int64 * 16)()
+    rc = lib().b200_stream_rings(shape, dev, out)
+    if rc != B200_OK:
+        _raise(rc, "b200_stream_rings failed")
+    keys = ("smem", "stages", "stage_bytes", "slice_tiles")
+    return {name: dict(zip(keys, out[4 * k:4 * k + 4])) for k, name in enumerate(("qkv", "wo", "gateup", "w2"))}
 
 
 def requant_kquant(ggml_type: int, raw, n_elems: int) -> np.ndarray:

@@ -519,6 +519,15 @@ int b200_weight_info(b200_plan *plan, int32_t *resident, int64_t *weight_bytes, 
  * threshold without filling a shared GPU.  bytes < 0: B200_ERR_BAD_ARG. */
 int b200_test_set_memory_budget(int64_t bytes);
 
+/* The shared-memory rings plan creation gives one layer's decode weight streams (a host computation: no device is needed).  QKV's
+ * and gate/up's rings are the largest that fit beside their neighbours under programmatic dependent launch (DESIGN.md §5a).
+ * shape[10]: dim, q width (n_heads * head_size), kv width, hidden, SMs, fused norm (0 / 1), then the tile format of QKV, Wo, gate/up
+ * and W2 (0: Q8_0 tiles; 12 / 13 / 14: resident Q4_K / Q5_K / Q6_K tiles).  dev[4]: shared memory per SM, reserved per resident
+ * CTA, opt-in limit per CTA, and the attention CTA's shared memory.  out[16]: for QKV, Wo, gate/up and W2 in turn, the launch's
+ * dynamic shared memory, its ring stages, the bytes of one stage and the tiles of the largest CTA slice.
+ * B200_ERR_BAD_ARG on a null pointer, a non-positive size or an unknown format; B200_ERR_UNSUPPORTED when a width has no tiling. */
+int b200_stream_rings(const int32_t *shape, const int64_t *dev, int64_t *out);
+
 /* Number of kernels one decode step launches (bench.py's gpu_launches). */
 int b200_launches_per_decode(b200_plan *plan);
 

@@ -1444,7 +1444,18 @@ int64_t weight_footprint(const b200_plan *p, const b200_tensor *tensors, int n_t
 // Room kept free beyond what rest_footprint counts: the CUDA graphs, the scratch of the exact prefill's multi-position steps and of
 // the persistent kernel, allocator rounding, and what other processes on the device may take meanwhile.
 const int64_t RESIDENT_MARGIN = (int64_t)1 << 30;
-int64_t g_memory_budget = 0; // b200_test_set_memory_budget: replaces the free-memory figure of weight_policy (0: off)
+int64_t g_memory_budget = 0; // b200_test_set_memory_budget: replaces the free-memory figure of memory_free (0: off)
+
+// The device's free memory as the weight-form rule and the resident plan's prefill scratch read it.
+int memory_free(b200_plan *p, int64_t *avail) {
+    *avail = g_memory_budget;
+    if (!*avail) {
+        size_t fr = 0, tot = 0;
+        CK(cudaMemGetInfo(&fr, &tot));
+        *avail = (int64_t)fr;
+    }
+    return B200_OK;
+}
 
 // What a plan allocates besides its weights: both KV caches, the upload's two device staging buffers (live while the weights are
 // allocated), the activations, the attention score scratch and the RoPE tables.
@@ -1466,12 +1477,9 @@ int weight_policy(b200_plan *p, const b200_tensor *tensors, int n_tensors, size_
     p->w8_bytes = weight_footprint(p, tensors, n_tensors, false);
     const int64_t wr = weight_footprint(p, tensors, n_tensors, true);
     const int64_t rest = rest_footprint(p, stage_bytes) + RESIDENT_MARGIN;
-    int64_t avail = g_memory_budget;
-    if (!avail) {
-        size_t fr = 0, tot = 0;
-        CK(cudaMemGetInfo(&fr, &tot));
-        avail = (int64_t)fr;
-    }
+    int64_t avail;
+    int rc;
+    if ((rc = memory_free(p, &avail))) return rc;
     if (p->w8_bytes + rest <= avail) { p->w_bytes = p->w8_bytes; return B200_OK; }
     if (wr + rest <= avail) { p->resident = true; p->w_bytes = wr; return B200_OK; }
     return fail(p, B200_ERR_OOM, "the model does not fit the device: %lld bytes with Q8_0 tiles and %lld bytes with K-quant weights resident are needed "
@@ -2032,8 +2040,24 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfP
 }
 
 // ---- the bit-exact tensor-core prefill (prefill_i8.cuh) -----------------------------------------------------------------------
+// The geometry of W as Q8_0 tiles: W itself, or for a resident matrix the tiles a Q8_0-tile plan of the same file holds, which
+// k_kq_tiles_to_q8 writes into the prefill's scratch before W's GEMM.
+TileMat q8_geometry(const TileMat &W) { return W.fmt ? tile_geometry(W.rows, W.cols, 0) : W; }
+
+cudaError_t launch_kq_tiles_to_q8(const TileMat &W, const TileMat &Q, unsigned char *out, cudaStream_t s) {
+    const long long n = (long long)tile_groups(Q) * 4 * Q.nseg * (Q.seg / 32);
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    if (W.fmt == 12) k_kq_tiles_to_q8<12><<<grid, 128, 0, s>>>(W, Q.seg, Q.nseg, Q.unit_bytes, out);
+    else if (W.fmt == 13) k_kq_tiles_to_q8<13><<<grid, 128, 0, s>>>(W, Q.seg, Q.nseg, Q.unit_bytes, out);
+    else if (W.fmt == 14) k_kq_tiles_to_q8<14><<<grid, 128, 0, s>>>(W, Q.seg, Q.nseg, Q.unit_bytes, out);
+    else return cudaErrorInvalidValue;
+    return cudaGetLastError();
+}
+
 // Built on the first b200_set_prefill_mode(TENSOR_CORE_EXACT): the chunk buffers and tensor maps over the plan's own Q8_0 streams,
-// nothing per weight.  Leaves pi8.ready false with the reason in pi8.why when the plan cannot run it.
+// nothing per weight.  A resident plan adds one scratch, the Q8_0 tiles of its largest resident matrix, and its resident matrices'
+// maps point there; the scratch and the chunk buffers must fit the free memory (memory_free) or the call fails with
+// B200_ERR_OOM.  Leaves pi8.ready false with the reason in pi8.why when the plan cannot run it.
 int prefill_init_i8(b200_plan *p) {
     PrefillI8Ctx &c = p->pi8;
     const b200_config &g = p->cfg;
@@ -2045,29 +2069,47 @@ int prefill_init_i8(b200_plan *p) {
     }
     if (g.tp_size > 1) { c.why = "tensor-core prefill is single-GPU"; return B200_OK; }
     if (g.dim % 64 || p->qd % 64 || nqkv % 64) { c.why = "the bit-exact tensor-core prefill needs dim, q width and q+k+v width multiples of 64"; return B200_OK; }
+    int64_t kq8_bytes = 0;
     for (const LayerW &L : p->layers)
-        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
-            if (t->seg % pg::BK) { c.why = "the bit-exact tensor-core prefill needs Q8_0 stream segments that are multiples of 64 columns"; return B200_OK; }
-    if (!pg::encode_fn()) { c.why = "cuTensorMapEncodeTiled not available from the driver"; return B200_OK; }
-    if (!c.bpad) {
-        const int bpad = (p->prefill_batch + pg::BM - 1) / pg::BM * pg::BM, big = g.dim > p->qd ? g.dim : p->qd;
-        const int lds_big = pg::i8_lds(big), lds_h = pg::i8_lds(g.hidden_dim);
-        c.att_tokens = bpad;
-        if (p->att_scratch) {
-            const size_t row = (size_t)p->nh_l * g.context_length * 4;
-            c.att_tokens = I8_ATT_SCRATCH_MAX / row < 1 ? 1 : (int)(I8_ATT_SCRATCH_MAX / row < (size_t)bpad ? I8_ATT_SCRATCH_MAX / row : bpad);
+        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2}) {
+            const TileMat q = q8_geometry(*t);
+            if (q.seg % pg::BK) { c.why = "the bit-exact tensor-core prefill needs Q8_0 stream segments that are multiples of 64 columns"; return B200_OK; }
+            if (t->fmt && tile_bytes(q) > kq8_bytes) kq8_bytes = tile_bytes(q);
         }
-        const size_t sizes[7] = {(size_t)bpad * g.dim * 4, (size_t)bpad * nqkv * 4, (size_t)bpad * big, (size_t)bpad * lds_big * 4,
-                                 (size_t)bpad * g.hidden_dim, (size_t)bpad * lds_h * 4, (size_t)bpad * sizeof(ChunkTok)};
+    if (!pg::encode_fn()) { c.why = "cuTensorMapEncodeTiled not available from the driver"; return B200_OK; }
+    const int bpad = (p->prefill_batch + pg::BM - 1) / pg::BM * pg::BM, big = g.dim > p->qd ? g.dim : p->qd;
+    const int lds_big = pg::i8_lds(big), lds_h = pg::i8_lds(g.hidden_dim);
+    int att_tokens = bpad;
+    if (p->att_scratch) {
+        const size_t row = (size_t)p->nh_l * g.context_length * 4;
+        att_tokens = I8_ATT_SCRATCH_MAX / row < 1 ? 1 : (int)(I8_ATT_SCRATCH_MAX / row < (size_t)bpad ? I8_ATT_SCRATCH_MAX / row : bpad);
+    }
+    const size_t sizes[7] = {(size_t)bpad * g.dim * 4, (size_t)bpad * nqkv * 4, (size_t)bpad * big, (size_t)bpad * lds_big * 4,
+                             (size_t)bpad * g.hidden_dim, (size_t)bpad * lds_h * 4, (size_t)bpad * sizeof(ChunkTok)};
+    const size_t att_bytes = p->att_scratch ? (size_t)att_tokens * p->nh_l * g.context_length * 4 : 0;
+    int rc;
+    if (kq8_bytes && !c.kq8) {
+        int64_t chunk_bytes = 0, avail;
+        if (!c.bpad) {
+            for (size_t b : sizes) chunk_bytes += (int64_t)b;
+            chunk_bytes += (int64_t)att_bytes;
+        }
+        if ((rc = memory_free(p, &avail))) return rc;
+        if (kq8_bytes + chunk_bytes > avail)
+            return fail(p, B200_ERR_OOM, "the bit-exact tensor-core prefill of this resident plan needs %lld bytes of Q8_0 scratch for its largest resident "
+                        "matrix and %lld bytes of chunk buffers, %lld bytes are free", (long long)kq8_bytes, (long long)chunk_bytes, (long long)avail);
+    }
+    if (!c.bpad) {
+        c.att_tokens = att_tokens;
         void **dst[7] = {(void **)&c.X, (void **)&c.QKV, (void **)&c.XQ, (void **)&c.XS, (void **)&c.HQ, (void **)&c.HS, (void **)&c.tok};
-        int rc;
         for (int i = 0; i < 7; i++) {
             if ((rc = dalloc(p, (unsigned char **)dst[i], sizes[i]))) return rc;
             CK(cudaMemset(*dst[i], 0, sizes[i]));
         }
-        if (p->att_scratch && (rc = dalloc(p, &c.att, (size_t)c.att_tokens * p->nh_l * g.context_length * 4))) return rc;
+        if (p->att_scratch && (rc = dalloc(p, &c.att, att_bytes))) return rc;
         c.bpad = bpad;
     }
+    if (kq8_bytes && !c.kq8 && (rc = dalloc(p, &c.kq8, (size_t)kq8_bytes))) return rc;
     bool ok = pg::make_map_i8_a(&c.a_dim, c.XQ, c.bpad, g.dim) == 0 && pg::make_map_i8_s(&c.s_dim, c.XS, c.bpad, pg::i8_lds(g.dim)) == 0 &&
               pg::make_map_i8_a(&c.a_qd, c.XQ, c.bpad, p->qd) == 0 && pg::make_map_i8_s(&c.s_qd, c.XS, c.bpad, pg::i8_lds(p->qd)) == 0 &&
               pg::make_map_i8_a(&c.a_h, c.HQ, c.bpad, g.hidden_dim) == 0 && pg::make_map_i8_s(&c.s_h, c.HS, c.bpad, pg::i8_lds(g.hidden_dim)) == 0;
@@ -2075,8 +2117,10 @@ int prefill_init_i8(b200_plan *p) {
     for (int l = 0; ok && l < g.n_layers; l++) {
         const LayerW &L = p->layers[l];
         PrefillQ8Maps &m = c.maps[l];
-        auto mk = [](CUtensorMap *q, CUtensorMap *s, const TileMat &t) {
-            return pg::make_map_i8_q8(q, t.base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 0) == 0 && pg::make_map_i8_q8(s, t.base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 1) == 0;
+        auto mk = [&](CUtensorMap *q, CUtensorMap *s, const TileMat &w) {
+            const TileMat t = q8_geometry(w);
+            const unsigned char *base = w.fmt ? c.kq8 : w.base;
+            return pg::make_map_i8_q8(q, base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 0) == 0 && pg::make_map_i8_q8(s, base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 1) == 0;
         };
         ok = mk(&m.qkv_q, &m.qkv_s, L.tqkv) && mk(&m.wo_q, &m.wo_s, L.two) && mk(&m.gu_q, &m.gu_s, L.tgu) && mk(&m.w2_q, &m.w2_s, L.tw2);
     }
@@ -2108,14 +2152,21 @@ int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own)
         else k_i8_norm<false><<<n, NORM_THREADS, norm_smem, s>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
         nl++;
     };
-    // one k_gemm_i8 over the stream W; n_tiles from W's rows (64 stream rows per tile)
+    // one k_gemm_i8 over the stream W; n_tiles from W's rows (64 stream rows per tile).  A resident W is first expanded to its Q8_0
+    // tiles in c.kq8, where its maps point; stream order (k_gemm_i8 is launched without PDL) orders the expansion between the
+    // previous GEMM's reads of the scratch and this GEMM's.
     auto gemm = [&](auto MODE, const CUtensorMap &a, const CUtensorMap &as, const CUtensorMap &bq, const CUtensorMap &bs, const TileMat &W, float *C, int ldc,
                     float oscale) {
+        const TileMat Q = q8_geometry(W);
+        if (W.fmt) {
+            CK(launch_kq_tiles_to_q8(W, Q, c.kq8, s));
+            nl++;
+        }
         pg::I8Out o{};
         o.C = C; o.ldc = ldc; o.hq = c.HQ; o.hs = c.HS; o.ldq = g.hidden_dim; o.lds = lds_h;
-        o.m_valid = n; o.K = W.cols; o.seg = W.seg; o.oscale = oscale;
+        o.m_valid = n; o.K = Q.cols; o.seg = Q.seg; o.oscale = oscale;
         nl++;
-        return pg::gemm_i8_launch<decltype(MODE)::value>(a, as, bq, bs, o, mt, W.rows / pg::I8_BN, s) ? fail(p, B200_ERR_CUDA, "int8 GEMM launch failed") : B200_OK;
+        return pg::gemm_i8_launch<decltype(MODE)::value>(a, as, bq, bs, o, mt, Q.rows / pg::I8_BN, s) ? fail(p, B200_ERR_CUDA, "int8 GEMM launch failed") : B200_OK;
     };
     using F32 = std::integral_constant<int, pg::GEMM_F32>;
     using RESID = std::integral_constant<int, pg::GEMM_RESID>;
@@ -2575,8 +2626,9 @@ int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
                mode != B200_PREFILL_TENSOR_CORE_EXACT))
         return B200_ERR_BAD_ARG;
     if (p->is_moe && mode != B200_PREFILL_EXACT) return fail(p, B200_ERR_UNSUPPORTED, "%s", MOE_PREFILL_WHY);
-    if (p->resident && mode != B200_PREFILL_EXACT)
-        return fail(p, B200_ERR_UNSUPPORTED, "this plan keeps K-quant weights resident: the tensor-core prefill reads Q8_0 tiles or f16 matrices, so prompts go through the exact prefill");
+    if (p->resident && (mode == B200_PREFILL_TENSOR_CORE || mode == B200_PREFILL_TENSOR_CORE_W8A16))
+        return fail(p, B200_ERR_UNSUPPORTED, "this plan keeps K-quant weights resident: the f16 and W8A16 tensor-core prefills read f16 matrices or "
+                    "Q8_0 tiles it does not hold; tensor_core_exact expands each resident matrix to Q8_0 tiles before its GEMM");
     if (mode == B200_PREFILL_TENSOR_CORE_EXACT) {
         if (!p->pi8.ready) {
             CK(cudaSetDevice(p->device));
@@ -3171,6 +3223,29 @@ int b200_requant_kquant(int32_t ggml_type, const void *src, int64_t n_elems, voi
     if (s.alloc(&ds, raw) && s.alloc(&dd, q8) && s.ok(cudaMemcpy(ds, src, raw, cudaMemcpyHostToDevice)) &&
         s.ok(launch_requant_kquant(ggml_type, ds, dd, n_elems / 32, 0)) && s.ok(cudaDeviceSynchronize()))
         s.ok(cudaMemcpy(dst_q8_0, dd, q8, cudaMemcpyDeviceToHost));
+    return s.rc;
+}
+
+int b200_test_kq_tiles_to_q8(int32_t ggml_type, int32_t rows, int32_t cols, const void *kq_rows, void *q8_tiles_out, int64_t bytes) {
+    if (!kq_rows || !q8_tiles_out || rows < 1 || cols < 256 || cols % 256 || !kq_is_kquant(ggml_type)) return B200_ERR_BAD_ARG;
+    TileMat W = tile_geometry(rows, cols, ggml_type);
+    const TileMat Q = tile_geometry(rows, cols, 0);
+    if (!W.nseg || !Q.nseg) return B200_ERR_BAD_ARG;
+    if (bytes != tile_bytes(Q)) return B200_ERR_BAD_ARG;
+    const size_t raw = (size_t)rows * (cols / 256) * kq_block_bytes(ggml_type);
+    unsigned char *draw = nullptr, *dres = nullptr, *dq8 = nullptr;
+    Scratch s;
+    // the resident tiles as upload_tiles lays them out, then the expansion as prefill_forward_i8 launches it
+    if (s.alloc(&draw, raw) && s.alloc(&dres, (size_t)tile_bytes(W)) && s.alloc(&dq8, (size_t)bytes) &&
+        s.ok(cudaMemcpy(draw, kq_rows, raw, cudaMemcpyHostToDevice)) && s.ok(cudaMemset(dq8, 0xA5, (size_t)bytes))) {
+        RepackSrc src{};
+        src.raw[0] = draw;
+        src.rows[0] = rows;
+        k_repack_kq_tiles<<<(unsigned)((size_t)tile_groups(W) * 4 * W.nseg), 128>>>(src, dres, rows, cols, W.seg, W.nseg, W.unit_bytes, kq_block_bytes(ggml_type));
+        W.base = dres;
+        if (s.ok(cudaGetLastError()) && s.ok(launch_kq_tiles_to_q8(W, Q, dq8, 0)) && s.ok(cudaDeviceSynchronize()))
+            s.ok(cudaMemcpy(q8_tiles_out, dq8, (size_t)bytes, cudaMemcpyDeviceToHost));
+    }
     return s.rc;
 }
 

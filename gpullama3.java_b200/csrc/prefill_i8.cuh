@@ -22,6 +22,9 @@
 // The chunk forms of the exact per-row bodies run around the GEMMs over a per-token table (ChunkTok): k_i8_norm
 // (rmsnorm_quant_row, one CTA per token), k_i8_rope_kv (rope_kv_prologue, grid heads x tokens) and k_i8_attention
 // (attention_head<HS, true>, grid heads x tokens, after every K / V row of the chunk is in the cache).
+//
+// On a plan that keeps K-quant weights resident, each resident matrix is first expanded to the Q8_0 tiles a Q8_0-tile plan of the
+// same file holds (k_kq_tiles_to_q8, stream_matvec.cuh) in one scratch the size of the largest, and its GEMM reads them there.
 #pragma once
 #include "decode_kernels.cuh"
 #include "prefill.cuh"
@@ -285,8 +288,10 @@ struct PrefillI8Ctx {
     float *X = nullptr, *QKV = nullptr, *XS = nullptr, *HS = nullptr, *att = nullptr;
     int8_t *XQ = nullptr, *HQ = nullptr;
     ChunkTok *tok = nullptr;
+    unsigned char *kq8 = nullptr;                   // resident plans: the Q8_0 tiles of the resident matrix the next GEMM reads
     CUtensorMap a_dim, s_dim, a_qd, s_qd, a_h, s_h; // A operands: K = dim (XQ), K = q width (XQ), K = hidden (HQ)
-    std::vector<PrefillQ8Maps> maps;                // per layer: make_map_i8_q8 quant / scale maps of the four streams
+    std::vector<PrefillQ8Maps> maps;                // per layer: make_map_i8_q8 quant / scale maps of the four streams (over kq8
+                                                    // for a resident stream)
 };
 // Global score rows of one attention launch are bounded by this many bytes (att_tokens = max(1, bound / (heads x context x 4))).
 constexpr size_t I8_ATT_SCRATCH_MAX = (size_t)64 << 20;

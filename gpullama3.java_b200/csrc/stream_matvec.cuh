@@ -638,3 +638,30 @@ __global__ void k_tiles_to_f16(TileMat W, int gateup, __half *__restrict__ out0,
         dst[i] = __floats2half2_rn((float)(signed char)(w & 0xFF) * f, (float)(signed char)(w >> 8) * f);
     }
 }
+
+// ---- resident K-quant tiles -> the Q8_0 tiles of the same matrix (the bit-exact prefill's B operand on a resident plan) --------
+// One thread per Q8_0 block.  Q8_0 unit (G, s, r) of geometry (seg, nseg, unit_bytes) takes its rows from the resident units
+// (G, s', r) of W: the slot r is shared, so the gate/up interleave carries over.  The block at column c lives in W's segment
+// c / W.seg, super-block (c % W.seg) / 256, sub-block (c % 256) / 32 (the two segmentations may differ: W.seg is a multiple of 256,
+// seg of 32).  kq_q8_block gives the bytes the load-time re-quantiser gives, laid out as k_repack_tiles lays them: the quants at
+// 32 b, the f16 scale at seg + 2 b, zeros up to unit_bytes.
+template <int FMT>
+__global__ void k_kq_tiles_to_q8(TileMat W, int seg, int nseg, int unit_bytes, unsigned char *__restrict__ out) {
+    const int nbs = seg / 32;
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)tile_groups(W) * 4 * nseg * nbs) return;
+    const long long unit_id = t / nbs;
+    const int b = (int)(t - unit_id * nbs), r = (int)(unit_id % 4), s = (int)((unit_id / 4) % nseg);
+    const long long G = unit_id / (4LL * nseg);
+    const int c = s * seg + 32 * b, s_kq = c / W.seg, cc = c - s_kq * W.seg;
+    const unsigned char *sb = W.base + ((G * W.nseg + s_kq) * 4 + r) * W.unit_bytes + (size_t)(cc >> 8) * kq_block_bytes(FMT);
+    int q[8];
+    const __half d = kq_q8_block<FMT>(sb, (cc >> 5) & 7, q);
+    unsigned char *u = out + (size_t)unit_id * unit_bytes;
+    int4 *dq = reinterpret_cast<int4 *>(u + 32 * b);
+    dq[0] = make_int4(q[0], q[1], q[2], q[3]);
+    dq[1] = make_int4(q[4], q[5], q[6], q[7]);
+    reinterpret_cast<__half *>(u + seg)[b] = d;
+    if (b == nbs - 1)
+        for (int i = seg + 2 * nbs; i < unit_bytes; i++) u[i] = 0;
+}

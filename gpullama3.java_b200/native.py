@@ -60,7 +60,7 @@ class Tensor(C.Structure):
 
 
 EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
-           "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant",
+           "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant", "b200_test_kq_tiles_to_q8",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
            "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_weight_info", "b200_test_set_memory_budget", "b200_stream_rings",
@@ -120,6 +120,7 @@ def lib() -> C.CDLL:
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     L.b200_weight_info.argtypes = [vp, C.POINTER(i32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.b200_test_set_memory_budget.argtypes = [C.c_int64]
+    L.b200_test_kq_tiles_to_q8.argtypes = [i32, i32, i32, vp, vp, C.c_int64]
     L.b200_stream_rings.argtypes = [C.POINTER(i32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.b200_launches_per_decode.argtypes = [vp]
     L.b200_device_bytes.argtypes = [vp]
@@ -205,6 +206,28 @@ def requant_kquant(ggml_type: int, raw, n_elems: int) -> np.ndarray:
     rc = lib().b200_requant_kquant(int(ggml_type), raw.ctypes.data, int(n_elems), out.ctypes.data)
     if rc != B200_OK:
         _raise(rc, "b200_requant_kquant failed")
+    return out
+
+
+def q8_tile_bytes(rows: int, cols: int) -> int:
+    """Bytes of the tile-major Q8_0 stream of a rows x cols matrix (csrc/stream_matvec.cuh: the fewest segments of at most 2560
+    columns, each a multiple of 32; a unit is a segment's quants and f16 scales padded to 16 bytes; whole 4-row groups)."""
+    nseg = next(n for n in range(1, cols // 32 + 1) if cols % n == 0 and (cols // n) % 32 == 0 and cols // n <= 2560)
+    seg = cols // nseg
+    return (rows + 3) // 4 * 4 * nseg * ((seg + seg // 16 + 15) & ~15)
+
+
+def test_kq_tiles_to_q8(ggml_type: int, rows: int, cols: int, raw) -> np.ndarray:
+    """b200_test_kq_tiles_to_q8: row-major K-quant rows (Q4_K = 12 / Q5_K = 13 / Q6_K = 14) repacked into resident tiles and expanded
+    on the device to the matrix's tile-major Q8_0 stream (uint8, q8_tile_bytes(rows, cols) bytes), as the bit-exact tensor-core
+    prefill expands a resident matrix."""
+    raw = np.ascontiguousarray(raw, dtype=np.uint8)
+    if cols % 256 or raw.size != rows * (cols // 256) * {12: 144, 13: 176, 14: 210}.get(int(ggml_type), 0):
+        raise ValueError(f"{raw.size} bytes are not {rows} rows of {cols} type-{ggml_type} elements")
+    out = np.empty(q8_tile_bytes(rows, cols), dtype=np.uint8)
+    rc = lib().b200_test_kq_tiles_to_q8(int(ggml_type), int(rows), int(cols), raw.ctypes.data, out.ctypes.data, out.size)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_kq_tiles_to_q8 failed")
     return out
 
 

@@ -133,7 +133,10 @@ class B200MasterPlan:
         builds f16 twins of its matrices) or "tensor_core_w8a16" (Q8_0 plans: the same GEMMs reading the Q8_0 weights in
         place, dequantised in shared memory; bit-identical to "tensor_core" where no residual GEMM splits K) or "tensor_core_exact"
         (Q8_0 plans: the whole chunk through int8 tensor-core GEMMs summing each Q8_0 block's term in the CPU path's order;
-        KV cache bit-identical to "exact")."""
+        KV cache bit-identical to "exact").  On a plan that keeps K-quant weights resident (weight_info()["resident"]) only
+        "exact" and "tensor_core_exact" are available: the latter expands each resident matrix to its Q8_0 tiles on the device
+        just before its GEMM, in one scratch the size of the largest resident matrix's Q8_0 tiles, and raises B200Error
+        (B200_ERR_OOM) naming the bytes when that scratch and the chunk buffers do not fit the free memory."""
         if isinstance(mode, str):
             mode = {"exact": 0, "tensor_core": 1, "tensor_core_w8a16": 2, "tensor_core_exact": 3}[mode]
         self._native.set_prefill_mode(int(mode))

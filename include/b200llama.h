@@ -229,10 +229,16 @@ int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n
  *                            fl(isum * fl(wScale * aScale)) in the CPU path's block order; norms, RoPE / KV and attention run
  *                            the exact per-row bodies over the chunk.  KV cache bit-identical to the CPU path, as
  *                            B200_PREFILL_EXACT.  Any head size the plan decodes.  The first call allocates the chunk buffers
- *                            and builds tensor maps only.  B200_ERR_UNSUPPORTED with the reason (the previous mode stays in
- *                            force) on FP16, tensor-parallel, Qwen2-MoE and resident K-quant plans, plans created without a
- *                            prefill batch size, and plans whose dim, q or q+k+v widths or stream segments are not multiples
- *                            of 64 columns.  Applies to b200_forward_batch_prefill and b200_prefill_slots. */
+ *                            and builds tensor maps only.  On a plan that keeps K-quant weights resident (b200_weight_info)
+ *                            each resident matrix is expanded on the device to the Q8_0 tiles a Q8_0-tile plan of the same
+ *                            file holds, just before its GEMM, into one scratch the size of the largest resident matrix's Q8_0
+ *                            tiles, allocated by the first call and kept until b200_plan_free; B200_ERR_OOM naming both
+ *                            figures (the previous mode stays in force) when that scratch and the chunk buffers exceed the
+ *                            device's free memory.  B200_ERR_UNSUPPORTED with the reason (the previous mode stays in
+ *                            force) on FP16, tensor-parallel and Qwen2-MoE plans, plans created without a prefill batch size,
+ *                            and plans whose dim, q or q+k+v widths or Q8_0 stream segments are not multiples of 64 columns.
+ *                            Applies to b200_forward_batch_prefill and b200_prefill_slots (a resident plan has no decode
+ *                            slots: its prompts go to the plan's own cache). */
 #define B200_PREFILL_EXACT 0
 #define B200_PREFILL_TENSOR_CORE 1
 #define B200_PREFILL_TENSOR_CORE_W8A16 2
@@ -441,6 +447,14 @@ int b200_test_sample(const float *logits, int32_t n, float temperature, float to
  * blocks (34 bytes per 32 elements) out, byte-identical to the reference's.  n_elems % 256 == 0. */
 int b200_requant_kquant(int32_t ggml_type, const void *src, int64_t n_elems, void *dst_q8_0);
 
+/* Test hook for the expansion B200_PREFILL_TENSOR_CORE_EXACT runs on a resident plan (k_kq_tiles_to_q8, csrc/stream_matvec.cuh):
+ * kq_rows, `rows` row-major rows of cols / 256 K-quant super-blocks (ggml_type 12 / 13 / 14), are repacked into resident tiles by
+ * the upload's kernel, expanded on the device, and the matrix's tile-major Q8_0 stream is copied to q8_tiles_out: `bytes` bytes,
+ * exactly the stream's size (4-row groups x segments x units, the layout of csrc/stream_matvec.cuh).  Each Q8_0 block is the one
+ * b200_requant_kquant gives.  B200_ERR_BAD_ARG on a null pointer, rows < 1, cols not a positive multiple of 256, an unknown
+ * type or a wrong `bytes`. */
+int b200_test_kq_tiles_to_q8(int32_t ggml_type, int32_t rows, int32_t cols, const void *kq_rows, void *q8_tiles_out, int64_t bytes);
+
 /* Batched-prefill GEMM building block (csrc/prefill_gemm.cuh; replaces the reference's mma.sync GEMMs
  * gemmMMA / gemmMMAQKV / gemmMMAGateUp, TransformerBatchPrefillKernels.java:792-1132) exposed for
  * tests and measurement: C[m][n] (f32) = A[m][k] (f16 bits) x B[n][k]^T (f16 bits) on the Hopper tensor
@@ -514,8 +528,9 @@ int b200_upload_info(b200_plan *plan, double *seconds, double *host_copy_seconds
  * and both tensor-core prefill modes. */
 int b200_weight_info(b200_plan *plan, int32_t *resident, int64_t *weight_bytes, int64_t *q8_weight_bytes);
 
-/* Test hook: replaces the device free-memory figure the weight-form rule of b200_plan_create reads (see b200_weight_info) by
- * `bytes` for every later plan in the process; 0 restores the real figure.  Lets tests put a budget on either side of the
+/* Test hook: replaces the device free-memory figure the weight-form rule of b200_plan_create reads (see b200_weight_info), and
+ * the one b200_set_prefill_mode(B200_PREFILL_TENSOR_CORE_EXACT) checks a resident plan's Q8_0 scratch against, by `bytes` for
+ * every later plan or call in the process; 0 restores the real figure.  Lets tests put a budget on either side of the
  * threshold without filling a shared GPU.  bytes < 0: B200_ERR_BAD_ARG. */
 int b200_test_set_memory_budget(int64_t bytes);
 

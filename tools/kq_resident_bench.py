@@ -51,11 +51,11 @@ def figures(pkg, model):
         pkg.native.test_set_memory_budget(0)
 
 
-def resident_plan(pkg, model):
+def resident_plan(pkg, model, **kw):
     q8, res = figures(pkg, model)
     pkg.native.test_set_memory_budget((q8 + res) // 2)
     try:
-        return pkg.B200MasterPlan.initialize_plan(model)
+        return pkg.B200MasterPlan.initialize_plan(model, **kw)
     finally:
         pkg.native.test_set_memory_budget(0)
 
@@ -126,14 +126,16 @@ def mem_available() -> int:
     return 0
 
 
-def bench_70b(pkg, args):
+def model_70b(pkg, ctx):
+    """(model or None, report): the whole Llama-3-70B shape in the Q4_K_M mix, every layer reusing layer 0's host tensors; None with
+    report["not_run"] when the host lacks the memory."""
     sh = pkg.synth.SHAPES["llama-3-70b"]
     one = pkg.synth.build_tensors_kquant(dataclasses.replace(sh, n_layers=1), seed=1234, mix="Q4_K_M")
     host = sum(np.asarray(r).nbytes for _, _, r in one.values())
-    out = {"workload": f"Llama-3-70B shape (80 layers), Q4_K_M mix, one GPU, context {args.ctx70}", "host_bytes": host}
+    out = {"workload": f"Llama-3-70B shape (80 layers), Q4_K_M mix, one GPU, context {ctx}", "host_bytes": host}
     if host * 1.5 > mem_available():
         out["not_run"] = f"the host has {mem_available()} bytes available, the synthetic tensors need about {host}"
-        return out
+        return None, out
     tensors = {}
     for name, v in one.items():
         if name.startswith("blk.0."):
@@ -141,7 +143,14 @@ def bench_70b(pkg, args):
                 tensors[f"blk.{l}." + name[len("blk.0."):]] = v
         else:
             tensors[name] = v
-    model = pkg.loader.model_from_tensors(sh, pkg.gguf.GGMLType.Q8_0, tensors, args.ctx70)
+    return pkg.loader.model_from_tensors(sh, pkg.gguf.GGMLType.Q8_0, tensors, ctx), out
+
+
+def bench_70b(pkg, args):
+    sh = pkg.synth.SHAPES["llama-3-70b"]
+    model, out = model_70b(pkg, args.ctx70)
+    if model is None:
+        return out
     try:
         plan = pkg.B200MasterPlan.initialize_plan(model)
     except pkg.native.B200Error as e:

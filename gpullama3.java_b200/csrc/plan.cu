@@ -13,6 +13,7 @@
 #include "decode_batch.cuh"
 #include "moe.cuh"
 #include "prefill_i8.cuh"
+#include "score.cuh"
 
 #include <math.h>
 #include <stdarg.h>
@@ -194,6 +195,17 @@ struct b200_plan {
         int last_launches = 0; // of the last step with the classifier (batch_step)
         float last_ms = 0.f;
     } bt;
+
+    // b200_score_tokens (score.cuh): the call's targets and per-row results on the device (cap rows, allocated on the first call);
+    // tensor_core_exact adds the classifier's maps and a logits scratch of SCORE_GROUP_ROWS rows of ldl floats
+    struct Score {
+        int cap = 0;
+        int *tgt = nullptr;
+        ScoreOut *out = nullptr;
+        float *logits = nullptr;
+        int ldl = 0;
+        CUtensorMap cls_q, cls_s;
+    } sc;
 };
 
 namespace {
@@ -2054,6 +2066,28 @@ cudaError_t launch_kq_tiles_to_q8(const TileMat &W, const TileMat &Q, unsigned c
     return cudaGetLastError();
 }
 
+// The quant / scale maps of W's Q8_0 tiles: W itself, or for a resident W the expansion scratch.
+bool i8_b_maps(const b200_plan *p, CUtensorMap *q, CUtensorMap *s, const TileMat &w) {
+    const TileMat t = q8_geometry(w);
+    const unsigned char *base = w.fmt ? p->pi8.kq8 : w.base;
+    const uint64_t rows = (uint64_t)tile_groups(t) * 4; // a classifier's last 4-row group is stored zero-padded
+    return pg::make_map_i8_q8(q, base, rows, t.nseg, t.unit_bytes, 0) == 0 && pg::make_map_i8_q8(s, base, rows, t.nseg, t.unit_bytes, 1) == 0;
+}
+
+// Every layer's stream maps (pi8.maps); false if a tensor map was rejected.
+bool i8_weight_maps(b200_plan *p) {
+    PrefillI8Ctx &c = p->pi8;
+    c.maps.resize(p->cfg.n_layers);
+    for (int l = 0; l < p->cfg.n_layers; l++) {
+        const LayerW &L = p->layers[l];
+        PrefillQ8Maps &m = c.maps[l];
+        if (!(i8_b_maps(p, &m.qkv_q, &m.qkv_s, L.tqkv) && i8_b_maps(p, &m.wo_q, &m.wo_s, L.two) && i8_b_maps(p, &m.gu_q, &m.gu_s, L.tgu) &&
+              i8_b_maps(p, &m.w2_q, &m.w2_s, L.tw2)))
+            return false;
+    }
+    return true;
+}
+
 // Built on the first b200_set_prefill_mode(TENSOR_CORE_EXACT): the chunk buffers and tensor maps over the plan's own Q8_0 streams,
 // nothing per weight.  A resident plan adds one scratch, the Q8_0 tiles of its largest resident matrix, and its resident matrices'
 // maps point there; the scratch and the chunk buffers must fit the free memory (memory_free) or the call fails with
@@ -2109,22 +2143,14 @@ int prefill_init_i8(b200_plan *p) {
         if (p->att_scratch && (rc = dalloc(p, &c.att, att_bytes))) return rc;
         c.bpad = bpad;
     }
-    if (kq8_bytes && !c.kq8 && (rc = dalloc(p, &c.kq8, (size_t)kq8_bytes))) return rc;
-    bool ok = pg::make_map_i8_a(&c.a_dim, c.XQ, c.bpad, g.dim) == 0 && pg::make_map_i8_s(&c.s_dim, c.XS, c.bpad, pg::i8_lds(g.dim)) == 0 &&
-              pg::make_map_i8_a(&c.a_qd, c.XQ, c.bpad, p->qd) == 0 && pg::make_map_i8_s(&c.s_qd, c.XS, c.bpad, pg::i8_lds(p->qd)) == 0 &&
-              pg::make_map_i8_a(&c.a_h, c.HQ, c.bpad, g.hidden_dim) == 0 && pg::make_map_i8_s(&c.s_h, c.HS, c.bpad, pg::i8_lds(g.hidden_dim)) == 0;
-    c.maps.resize(g.n_layers);
-    for (int l = 0; ok && l < g.n_layers; l++) {
-        const LayerW &L = p->layers[l];
-        PrefillQ8Maps &m = c.maps[l];
-        auto mk = [&](CUtensorMap *q, CUtensorMap *s, const TileMat &w) {
-            const TileMat t = q8_geometry(w);
-            const unsigned char *base = w.fmt ? c.kq8 : w.base;
-            return pg::make_map_i8_q8(q, base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 0) == 0 && pg::make_map_i8_q8(s, base, (uint64_t)t.rows, t.nseg, t.unit_bytes, 1) == 0;
-        };
-        ok = mk(&m.qkv_q, &m.qkv_s, L.tqkv) && mk(&m.wo_q, &m.wo_s, L.two) && mk(&m.gu_q, &m.gu_s, L.tgu) && mk(&m.w2_q, &m.w2_s, L.tw2);
+    if (kq8_bytes && !c.kq8) {
+        if ((rc = dalloc(p, &c.kq8, (size_t)kq8_bytes))) return rc;
+        c.kq8_bytes = kq8_bytes;
     }
-    if (!ok) { c.why = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
+    const bool ok = pg::make_map_i8_a(&c.a_dim, c.XQ, c.bpad, g.dim) == 0 && pg::make_map_i8_s(&c.s_dim, c.XS, c.bpad, pg::i8_lds(g.dim)) == 0 &&
+                    pg::make_map_i8_a(&c.a_qd, c.XQ, c.bpad, p->qd) == 0 && pg::make_map_i8_s(&c.s_qd, c.XS, c.bpad, pg::i8_lds(p->qd)) == 0 &&
+                    pg::make_map_i8_a(&c.a_h, c.HQ, c.bpad, g.hidden_dim) == 0 && pg::make_map_i8_s(&c.s_h, c.HS, c.bpad, pg::i8_lds(g.hidden_dim)) == 0;
+    if (!ok || !i8_weight_maps(p)) { c.why = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
     c.ready = true;
     c.why = "";
     return B200_OK;
@@ -2132,8 +2158,10 @@ int prefill_init_i8(b200_plan *p) {
 
 // One chunk: tab[v] = (token, position, KV offset) of chunk row v; own: the K / V go to the plan's cache, else to the decode slots.
 // The batched step's graph (enqueue_batch) over the whole chunk, its Q8_0 streams replaced by k_gemm_i8.  Times the chunk
-// (p->prefill_ms) and counts its launches (p->launches_prefill).
-int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own) {
+// (p->prefill_ms) and counts its launches (p->launches_prefill).  score (b200_score_tokens, after score_init_i8): then the final
+// norm, the classifier (expanded first on a resident plan) into p->sc.logits SCORE_GROUP_ROWS rows at a time, and k_score_rows
+// over each group into p->sc.out.
+int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own, bool score = false) {
     PrefillI8Ctx &c = p->pi8;
     const b200_config &g = p->cfg;
     cudaStream_t s = p->stream;
@@ -2192,6 +2220,27 @@ int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own)
         norm(false, L.ffn_norm);
         if ((rc = gemm(GATEUP(), c.a_dim, c.s_dim, m.gu_q, m.gu_s, L.tgu, nullptr, 0, 1.0f))) return rc;
         if ((rc = gemm(RESID(), c.a_h, c.s_h, m.w2_q, m.w2_s, L.tw2, c.X, g.dim, rs))) return rc;
+    }
+    if (score) {
+        auto &S = p->sc;
+        const TileMat Q = q8_geometry(p->tout);
+        norm(false, p->out_norm);
+        if (p->tout.fmt) {
+            CK(launch_kq_tiles_to_q8(p->tout, Q, c.kq8, s));
+            nl++;
+        }
+        for (int r0 = 0; r0 < n; r0 += SCORE_GROUP_ROWS) {
+            const int rows = n - r0 < SCORE_GROUP_ROWS ? n - r0 : SCORE_GROUP_ROWS;
+            CUtensorMap a, as; // the group's activation rows
+            if (pg::make_map_i8_a(&a, c.XQ + (size_t)r0 * g.dim, c.bpad - r0, g.dim) || pg::make_map_i8_s(&as, c.XS + (size_t)r0 * lds_d, c.bpad - r0, lds_d))
+                return fail(p, B200_ERR_CUDA, "cuTensorMapEncodeTiled rejected a tensor map");
+            pg::I8Out o{};
+            o.C = S.logits; o.ldc = S.ldl; o.m_valid = rows; o.K = Q.cols; o.seg = Q.seg; o.oscale = out_scale(p, false, true);
+            if (pg::gemm_i8_launch<pg::I8_LOGITS>(a, as, S.cls_q, S.cls_s, o, (rows + pg::BM - 1) / pg::BM, S.ldl / pg::I8_BN, s))
+                return fail(p, B200_ERR_CUDA, "int8 classifier GEMM launch failed");
+            k_score_rows<<<rows, SCORE_THREADS, 0, s>>>(S.logits, S.ldl, g.vocab_size, S.tgt + r0, S.out + r0);
+            nl += 2;
+        }
     }
     CK(cudaGetLastError());
     CK(cudaEventRecord(p->ev1, s));
@@ -2317,6 +2366,93 @@ int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, int32_t
     for (int k = 0; k < e; k++) ids_out[order[k]] = rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
     CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
     B.last_launches = g->launches;
+    return B200_OK;
+}
+
+// ---- b200_score_tokens (score.cuh) ----------------------------------------------------------------------------------------------
+// The per-row targets and results: rows for the longest call any mode takes.
+int score_ready(b200_plan *p) {
+    auto &S = p->sc;
+    if (S.tgt) return B200_OK;
+    const int cap = p->prefill_batch > p->seq_cap ? p->prefill_batch : p->seq_cap;
+    int rc;
+    if ((rc = dalloc(p, &S.tgt, (size_t)cap * 4)) || (rc = dalloc(p, &S.out, (size_t)cap * sizeof(ScoreOut)))) return rc;
+    S.cap = cap;
+    return B200_OK;
+}
+
+// tensor_core_exact: the logits scratch and the classifier's maps, built on the first score call.  A resident classifier is
+// expanded into pi8.kq8, which then grows to its Q8_0 tiles if they are larger than every layer matrix's (the layer maps are
+// rebuilt over the new scratch).  Both must fit the free memory (memory_free), or the call fails with B200_ERR_OOM.
+int score_init_i8(b200_plan *p) {
+    auto &S = p->sc;
+    PrefillI8Ctx &c = p->pi8;
+    if (S.logits) return B200_OK;
+    const TileMat Q = q8_geometry(p->tout);
+    if (Q.seg % pg::BK) return fail(p, B200_ERR_UNSUPPORTED, "the classifier's Q8_0 stream segments are not multiples of 64 columns: score in the exact prefill mode");
+    const int ldl = (p->cfg.vocab_size + pg::I8_BN - 1) / pg::I8_BN * pg::I8_BN; // whole 64-column tiles
+    const int64_t logit_bytes = (int64_t)SCORE_GROUP_ROWS * ldl * 4;
+    const int64_t cls_bytes = p->tout.fmt ? tile_bytes(Q) : 0, grow = cls_bytes > c.kq8_bytes ? cls_bytes - c.kq8_bytes : 0;
+    int64_t avail;
+    int rc;
+    if ((rc = memory_free(p, &avail))) return rc;
+    if (logit_bytes + grow > avail)
+        return fail(p, B200_ERR_OOM, "scoring in tensor_core_exact needs %lld bytes of logits scratch and %lld more bytes of Q8_0 scratch for the classifier, "
+                    "%lld bytes are free", (long long)logit_bytes, (long long)grow, (long long)avail);
+    if (grow) {
+        if (c.kq8) {
+            CK(cudaFree(c.kq8));
+            for (size_t i = 0; i < p->allocs.size(); i++)
+                if (p->allocs[i] == c.kq8) { p->allocs.erase(p->allocs.begin() + i); break; }
+            p->bytes -= c.kq8_bytes;
+            c.kq8 = nullptr;
+            c.kq8_bytes = 0;
+        }
+        if ((rc = dalloc(p, &c.kq8, (size_t)cls_bytes))) return rc;
+        c.kq8_bytes = cls_bytes;
+        if (!i8_weight_maps(p)) return fail(p, B200_ERR_CUDA, "cuTensorMapEncodeTiled rejected a tensor map");
+    }
+    if (!i8_b_maps(p, &S.cls_q, &S.cls_s, p->tout)) return fail(p, B200_ERR_CUDA, "cuTensorMapEncodeTiled rejected the classifier's tensor map");
+    if ((rc = dalloc(p, &S.logits, (size_t)logit_bytes))) return rc;
+    S.ldl = ldl;
+    return B200_OK;
+}
+
+// exact mode on a plan that runs multi-position steps: steps of batch_max_rows rows with the classifier on every row, each followed
+// by k_score_rows over its logits rows.  The schedule is uploaded once (k_batch_rows_next feeds each step its rows).
+int score_multi(b200_plan *p, const int32_t *tokens, int n, int start_pos) {
+    auto &B = p->bt;
+    int rc;
+    if ((rc = multi_ready(p))) return rc;
+    std::vector<BatchRows> sched;
+    std::vector<int> nrows;
+    pack_rows(sched, nrows, batch_max_rows(p), tokens, start_pos, n, 0);
+    const int steps = (int)sched.size();
+    std::vector<const Graph *> graphs(steps);
+    for (int k = 0; k < steps; k++)
+        if ((rc = batch_graph(p, SCHED | step_form(sched[k], nrows[k], true), nrows[k], nrows[k], &graphs[k]))) return rc;
+    CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
+    for (int k = 0, r0 = 0; k < steps; r0 += nrows[k++]) {
+        CK(cudaGraphLaunch(graphs[k]->exec, p->stream));
+        k_score_rows<<<nrows[k], SCORE_THREADS, 0, p->stream>>>(B.logits, sampler_padded(p->cfg.vocab_size), p->cfg.vocab_size, p->sc.tgt + r0, p->sc.out + r0);
+        CK(cudaGetLastError());
+    }
+    return B200_OK;
+}
+
+// exact mode on every other single-GPU plan: the single-token decode graph per position (it computes p->logits), each followed by
+// k_score_rows over that row.  The step state walks seq_tokens as b200_decode_sequence's does.
+int score_single(b200_plan *p, const int32_t *tokens, int n, int start_pos) {
+    int rc;
+    memcpy(p->h_ids, tokens, (size_t)n * 4);
+    CK(cudaMemcpyAsync(p->seq_tokens, p->h_ids, (size_t)n * 4, cudaMemcpyHostToDevice, p->stream));
+    if ((rc = set_state(p, tokens[0], start_pos, n, 0))) return rc;
+    for (int i = 0; i < n; i++) {
+        CK(cudaGraphLaunch(decode_graph(p), p->stream));
+        k_score_rows<<<1, SCORE_THREADS, 0, p->stream>>>(p->logits, 0, p->cfg.vocab_size, p->sc.tgt + i, p->sc.out + i);
+        CK(cudaGetLastError());
+    }
     return B200_OK;
 }
 
@@ -2556,6 +2692,41 @@ int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, i
     for (int i = first; i < n; i++) CK(cudaGraphLaunch(prefill_graph(p), p->stream));
     CK(cudaStreamSynchronize(p->stream));
     return check_device_error(p);
+}
+
+int b200_score_tokens(b200_plan *p, const int32_t *tokens, const int32_t *targets, int32_t n, int32_t start_pos, double *logprobs, int32_t *greedy_ids) {
+    if (!p || !tokens || !targets || !logprobs || !greedy_ids) return B200_ERR_BAD_ARG;
+    if (n <= 0) return B200_OK;
+    if (p->cfg.tp_size > 1)
+        return fail(p, B200_ERR_UNSUPPORTED, "full logits are not gathered under tensor parallelism: scoring runs on single-GPU plans");
+    const int mode = p->prefill.mode;
+    if (mode == B200_PREFILL_TENSOR_CORE || mode == B200_PREFILL_TENSOR_CORE_W8A16)
+        return fail(p, B200_ERR_UNSUPPORTED, "the %s prefill keeps f16 activations, so its logits are not the reference's: score in the exact or "
+                    "tensor_core_exact prefill mode", mode == B200_PREFILL_TENSOR_CORE ? "tensor_core" : "tensor_core_w8a16");
+    if (p->prefill_batch > 1 && n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "chunk of %d tokens exceeds prefill_batch_size %d", n, p->prefill_batch);
+    if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache", start_pos, start_pos + n - 1);
+    if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
+    for (int i = 0; i < n; i++)
+        if (targets[i] != -1 && (targets[i] < 0 || targets[i] >= p->cfg.vocab_size))
+            return fail(p, B200_ERR_BAD_ARG, "target %d of row %d out of range (-1 or a token id)", targets[i], i);
+    const bool tc = p->pi8.ready && mode == B200_PREFILL_TENSOR_CORE_EXACT;
+    if (!tc && n > p->seq_cap) return fail(p, B200_ERR_BAD_ARG, "chunk too long");
+    CK(cudaSetDevice(p->device));
+    int rc;
+    if ((rc = score_ready(p)) || (tc && (rc = score_init_i8(p)))) return rc;
+    CK(cudaMemcpyAsync(p->sc.tgt, targets, (size_t)n * 4, cudaMemcpyHostToDevice, p->stream));
+    if (tc) {
+        std::vector<ChunkTok> tab(n);
+        for (int i = 0; i < n; i++) tab[i] = ChunkTok{tokens[i], start_pos + i, 0};
+        rc = prefill_forward_i8(p, tab, true, true);
+    } else rc = multi_why(p) ? score_single(p, tokens, n, start_pos) : score_multi(p, tokens, n, start_pos);
+    if (rc) return rc;
+    std::vector<ScoreOut> out(n);
+    CK(cudaMemcpyAsync(out.data(), p->sc.out, (size_t)n * sizeof(ScoreOut), cudaMemcpyDeviceToHost, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
+    if ((rc = check_device_error(p))) return rc;
+    for (int i = 0; i < n; i++) { logprobs[i] = out[i].logprob; greedy_ids[i] = out[i].greedy; }
+    return B200_OK;
 }
 
 int b200_decode_sequence(b200_plan *p, const int32_t *tokens, int32_t n, int32_t start_pos, int32_t feedback,

@@ -14,7 +14,9 @@
 // 0 = the TMA producer (one thread), 1 and 2 = consumers of tile rows 0-63 and 64-127.  Each consumer keeps two s32 accumulator
 // sets: the wgmma of a k-block's second 32-column block runs while the terms of its first are added, and so on.
 //
-// Epilogues: STORE (QKV: out = acc), RESID (Wo, W2: x = fl(x + fl(acc * oscale)), Granite's residualScale or 1), GATEUP (the
+// Epilogues: STORE (QKV: out = acc), I8_LOGITS (k_gemm_i8_logits, the classifier of b200_score_tokens: out = fl(acc * oscale),
+// Granite's logitScale or 1, as the streaming classifier stores it; every column of the tile is written, so C's row stride covers
+// whole 64-column tiles), RESID (Wo, W2: x = fl(x + fl(acc * oscale)), Granite's residualScale or 1), GATEUP (the
 // interleaved gate/up stream: a 64-row tile is 32 gate and 32 up rows of the same 32 hidden units, so swiglu_exact and the Q8_0
 // quantisation of that 32-unit block (quant_block_lane) both finish inside the tile).  These are the batched step's epilogues
 // (decode_batch.cuh), element for element.
@@ -33,6 +35,7 @@
 namespace pg {
 
 constexpr int I8_BN = 64, I8_STAGES = 8;
+constexpr int I8_LOGITS = 3; // the epilogue of k_gemm_i8_logits, next to GEMM_F32 / GEMM_RESID / GEMM_GATEUP (prefill_gemm.cuh)
 // one stage: A quants (128 rows x 64 bytes, 64-byte swizzle), B quants (64 rows x 64 bytes, same swizzle), A scale lines (128 x 16
 // bytes), B scale lines (64 x 16 bytes).  Every part starts on a 1024-byte boundary of the stage.
 constexpr int I8_A_BYTES = BM * BK, I8_B_BYTES = I8_BN * BK, I8_AS_BYTES = BM * 16, I8_BS_BYTES = I8_BN * 16;
@@ -91,10 +94,10 @@ __device__ __forceinline__ void i8_fence_regs(int (&d)[32]) {
 // subtraction of 1.5 * 2^23 is exact (isum = 0 gives +0, as (float)0 does)
 __device__ __forceinline__ float i8_to_float(int isum) { return __fsub_rn(__int_as_float(isum + 0x4B400000), 12582912.0f); }
 
+// The GEMM of both kernels below: k_gemm_i8 (the prefill's epilogues) and k_gemm_i8_logits (I8_LOGITS).
 template <int MODE>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_i8(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_as,
-                                                          const __grid_constant__ CUtensorMap tma_bq, const __grid_constant__ CUtensorMap tma_bs,
-                                                          const I8Out o) {
+__device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUtensorMap &tma_as, const CUtensorMap &tma_bq, const CUtensorMap &tma_bs,
+                                             const I8Out &o) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     float *hbuf = reinterpret_cast<float *>(smem + I8_STAGES * I8_STAGE_BYTES);
@@ -215,11 +218,30 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_i8(const __grid_consta
                     for (int e = 0; e < 2; e++) {
                         const float v = acc[4 * jj + 2 * h + e];
                         if (MODE == GEMM_RESID) dst[8 * jj + e] = __fadd_rn(dst[8 * jj + e], __fmul_rn(v, o.oscale));
+                        else if (MODE == I8_LOGITS) dst[8 * jj + e] = __fmul_rn(v, o.oscale);
                         else dst[8 * jj + e] = v;
                     }
             }
         }
     }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_i8(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_as,
+                                                          const __grid_constant__ CUtensorMap tma_bq, const __grid_constant__ CUtensorMap tma_bs,
+                                                          const I8Out o) {
+    gemm_i8_body<MODE>(tma_a, tma_as, tma_bq, tma_bs, o);
+}
+
+__global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_i8_logits(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_as,
+                                                                 const __grid_constant__ CUtensorMap tma_bq, const __grid_constant__ CUtensorMap tma_bs,
+                                                                 const I8Out o) {
+    gemm_i8_body<I8_LOGITS>(tma_a, tma_as, tma_bq, tma_bs, o);
+}
+
+template <int MODE> constexpr auto gemm_i8_kernel() {
+    if constexpr (MODE == I8_LOGITS) return k_gemm_i8_logits;
+    else return k_gemm_i8<MODE>;
 }
 
 // ---- host side ----
@@ -260,11 +282,11 @@ inline int gemm_i8_launch(const CUtensorMap &a, const CUtensorMap &as, const CUt
                           int n_tiles, cudaStream_t stream) {
     static bool attr = false; // one flag per instantiation
     if (!attr) {
-        if (cudaFuncSetAttribute(k_gemm_i8<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)i8_smem_bytes()) != cudaSuccess) return -4;
+        if (cudaFuncSetAttribute(gemm_i8_kernel<MODE>(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)i8_smem_bytes()) != cudaSuccess) return -4;
         attr = true;
     }
     if (o.seg <= 0 || o.seg % BK || o.K <= 0 || o.K % o.seg || m_tiles < 1 || n_tiles < 1) return -6;
-    k_gemm_i8<MODE><<<dim3(m_tiles, n_tiles), GEMM_THREADS, i8_smem_bytes(), stream>>>(a, as, bq, bs, o);
+    gemm_i8_kernel<MODE>()<<<dim3(m_tiles, n_tiles), GEMM_THREADS, i8_smem_bytes(), stream>>>(a, as, bq, bs, o);
     return cudaGetLastError() == cudaSuccess ? 0 : -5;
 }
 
@@ -289,6 +311,7 @@ struct PrefillI8Ctx {
     int8_t *XQ = nullptr, *HQ = nullptr;
     ChunkTok *tok = nullptr;
     unsigned char *kq8 = nullptr;                   // resident plans: the Q8_0 tiles of the resident matrix the next GEMM reads
+    int64_t kq8_bytes = 0;                          // its size (b200_score_tokens grows it to the classifier's tiles)
     CUtensorMap a_dim, s_dim, a_qd, s_qd, a_h, s_h; // A operands: K = dim (XQ), K = q width (XQ), K = hidden (HQ)
     std::vector<PrefillQ8Maps> maps;                // per layer: make_map_i8_q8 quant / scale maps of the four streams (over kq8
                                                     // for a resident stream)

@@ -15,15 +15,19 @@ Position/token conventions decide parity, so they are restated exactly:
 ``ContinuousBatcher`` / ``generate_tokens_continuous`` the first two loops for a stream of requests: decode rows of running
                               requests and prompt rows of newly admitted ones share each forward_step, and freed slots are
                               refilled from a queue
+``score_sequence`` / ``perplexity`` teacher-forced scoring of a given text (plan.score_tokens) in chunks the plan accepts
 The sampler is greedy (temperature 0 -> FloatTensor.argmax, Sampler.java:124-132) and runs on
 the device; ``forward`` is any callable (token, position) -> argmax so the same loops drive
 the oracle in the tests.
 """
 from __future__ import annotations
 
+import math
 import time
 from collections import deque
 from typing import Callable, Iterable
+
+import numpy as np
 
 Forward = Callable[[int, int], int]
 
@@ -481,3 +485,29 @@ def generate_tokens_continuous(plan, model_type: str, requests: list, arrivals: 
     if stats is not None:
         stats.update(steps=len(rows), rows=rows, launches=launches, submitted=t_sub, first_token=t_first, done=t_done)
     return [cb.results[rid] for rid in sorted(rid_of, key=lambda r: rid_of[r])]
+
+
+def score_sequence(plan, tokens: list[int], start_pos: int = 0):
+    """Score tokens[i] at start_pos + i through plan.score_tokens, in chunks of the plan's prefill batch size (the whole sequence when
+    the plan has none).  Row i's target is tokens[i + 1] -- for a chunk's last row, the next chunk's first token -- and -1 for the
+    sequence's last row.  Returns (logprobs float64 [n], NaN in the last row; greedy ids int32 [n])."""
+    t = np.asarray(tokens, dtype=np.int32).reshape(-1)
+    n = len(t)
+    targets = np.append(t[1:], np.int32(-1))
+    pb = getattr(plan, "prefill_batch_size", 0) or 0
+    chunk = pb if pb > 1 else max(n, 1)
+    lp = np.empty(n, dtype=np.float64)
+    ids = np.empty(n, dtype=np.int32)
+    for a in range(0, n, chunk):
+        b = min(a + chunk, n)
+        lp[a:b], ids[a:b] = plan.score_tokens(t[a:b], start_pos + a, targets[a:b])
+    return lp, ids
+
+
+def perplexity(plan, tokens: list[int]) -> float:
+    """exp(-mean log p(tokens[i] | tokens[:i])) over i = 1 .. n-1, scored from position 0 after plan.kv_reset()."""
+    if len(tokens) < 2:
+        raise ValueError("perplexity needs at least two tokens")
+    plan.kv_reset()
+    lp, _ = score_sequence(plan, tokens, 0)
+    return math.exp(-float(lp[:-1].mean()))

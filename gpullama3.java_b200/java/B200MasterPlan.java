@@ -71,6 +71,7 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle DECODE = fn("b200_forward_decode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle PREFILL = fn("b200_forward_prefill", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
     private static final MethodHandle BATCH_PREFILL = fn("b200_forward_batch_prefill", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT));
+    private static final MethodHandle SCORE_TOKENS = fn("b200_score_tokens", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle SET_PREFILL_MODE = fn("b200_set_prefill_mode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle SET_DECODE_MODE = fn("b200_set_decode_mode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle DECODE_SAMPLE = fn("b200_forward_decode_sample",
@@ -219,6 +220,22 @@ public final class B200MasterPlan implements AutoCloseable {
         try (Arena a = Arena.ofConfined()) {
             int rc = (int) BATCH_PREFILL.invokeExact(plan, a.allocateFrom(JAVA_INT, tokens), tokens.length, startPos);
             if (rc != 0) check(rc, lastError());
+        }
+    }
+
+    /** Scores tokens[i] at startPos + i (their K/V go into the cache as forwardBatchPrefill writes them): logprobs[i] = the model's
+     *  log-probability of targets[i] (-1: NaN) computed in double from logits bit-identical to forwardDecode's, greedyIds[i] = their
+     *  argmax.  Prefill modes exact and tensor_core_exact only; tokens.length within forwardBatchPrefill's limit. */
+    public void scoreTokens(int[] tokens, int[] targets, int startPos, double[] logprobs, int[] greedyIds) throws Throwable {
+        if (targets.length != tokens.length || logprobs.length < tokens.length || greedyIds.length < tokens.length)
+            throw new IllegalArgumentException("targets, logprobs and greedyIds must hold tokens.length entries");
+        try (Arena a = Arena.ofConfined()) {
+            MemorySegment lp = a.allocate(java.lang.foreign.ValueLayout.JAVA_DOUBLE, tokens.length);
+            MemorySegment ids = a.allocate(JAVA_INT, tokens.length);
+            int rc = (int) SCORE_TOKENS.invokeExact(plan, a.allocateFrom(JAVA_INT, tokens), a.allocateFrom(JAVA_INT, targets), tokens.length, startPos, lp, ids);
+            if (rc != 0) check(rc, lastError());
+            MemorySegment.copy(lp, java.lang.foreign.ValueLayout.JAVA_DOUBLE, 0, logprobs, 0, tokens.length);
+            MemorySegment.copy(ids, JAVA_INT, 0, greedyIds, 0, tokens.length);
         }
     }
 

@@ -59,7 +59,7 @@ class Tensor(C.Structure):
                 ("dims", C.c_int64 * 4)]
 
 
-EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_set_prefill_mode", "b200_prefill_info",
+EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_score_tokens", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant", "b200_test_kq_tiles_to_q8",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
@@ -86,6 +86,7 @@ def lib() -> C.CDLL:
     L.b200_forward_prefill.argtypes = [vp, i32, i32]
     L.b200_forward_decode_sample.argtypes = [vp, i32, i32, C.c_float, C.c_float, C.c_float, C.POINTER(i32), C.POINTER(i32)]
     L.b200_forward_batch_prefill.argtypes = [vp, vp, i32, i32]
+    L.b200_score_tokens.argtypes = [vp, vp, vp, i32, i32, vp, vp]
     L.b200_decode_sequence.argtypes = [vp, vp, i32, i32, i32, vp, C.POINTER(C.c_float)]
     L.b200_kv_reset.argtypes = [vp]
     L.b200_profile_norm.argtypes = [vp, C.POINTER(C.c_int64)]
@@ -462,6 +463,20 @@ class NativePlan:
     def forward_batch_prefill(self, tokens, start_pos: int):
         t = np.ascontiguousarray(tokens, dtype=np.int32)
         self._ck(lib().b200_forward_batch_prefill(self._p, t.ctypes.data, len(t), start_pos))
+
+    def score_tokens(self, tokens, start_pos: int, targets=None):
+        """b200_score_tokens: run tokens[i] at start_pos + i (K/V into the plan's cache) and score each row.  targets[i] is the token
+        whose log-probability row i reports (-1: none, NaN); the default is the next token of `tokens`, -1 for the last row.
+        Returns (logprobs float64 [n], greedy ids int32 [n])."""
+        t = np.ascontiguousarray(tokens, dtype=np.int32).reshape(-1)
+        n = len(t)
+        tg = np.append(t[1:], np.int32(-1)) if targets is None else np.ascontiguousarray(targets, dtype=np.int32).reshape(-1)
+        if len(tg) != n:
+            raise ValueError("targets must have one entry per token")
+        lp = np.empty(n, dtype=np.float64)
+        ids = np.empty(n, dtype=np.int32)
+        self._ck(lib().b200_score_tokens(self._p, t.ctypes.data, tg.ctypes.data, n, start_pos, lp.ctypes.data, ids.ctypes.data))
+        return lp, ids
 
     def decode_sequence(self, tokens, n: int, start_pos: int, feedback: bool = False):
         t = np.ascontiguousarray(tokens, dtype=np.int32)

@@ -125,6 +125,13 @@ class B200MasterPlan:
     def forward_batch_prefill(self, tokens, start_pos: int):
         self._native.forward_batch_prefill(np.asarray(tokens, dtype=np.int32), start_pos)
 
+    def score_tokens(self, tokens, start_pos: int, targets=None):
+        """Score tokens[i] at start_pos + i -> (logprobs float64 [n], greedy ids int32 [n]): logprobs[i] is the log-probability of
+        targets[i] (default: the next token, -1 = NaN for the last row) under logits bit-identical to forward_decode's, in double;
+        the K/V go into the cache as forward_batch_prefill writes them.  Prefill modes "exact" and "tensor_core_exact" only, and at
+        most forward_batch_prefill's chunk length (engine.score_sequence splits longer sequences)."""
+        return self._native.score_tokens(tokens, start_pos, targets)
+
     # TensorCoreSupport.java's switch between the MMA and the plain batch-prefill layer families
     PREFILL_EXACT, PREFILL_TENSOR_CORE, PREFILL_TENSOR_CORE_W8A16, PREFILL_TENSOR_CORE_EXACT = 0, 1, 2, 3
 

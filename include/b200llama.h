@@ -248,6 +248,32 @@ int b200_set_prefill_mode(b200_plan *plan, int32_t mode);
 /* Active mode, kernels launched and device milliseconds of the last tensor-core chunk (any pointer may be NULL). */
 int b200_prefill_info(b200_plan *plan, int32_t *mode, int32_t *launches, float *device_ms);
 
+/* Score a token sequence: the model's log-probability of each row's target and its greedy id, for perplexity, log-likelihood
+ * evaluation and prompt log-probabilities.  Definition (every path below gives these bits):
+ *   - tokens[0..n) run at positions start_pos .. start_pos + n - 1, and their K/V go into the plan's cache exactly as
+ *     b200_forward_batch_prefill writes them, so decoding continues at start_pos + n;
+ *   - row i's logits l are the ones b200_forward_decode(tokens[i], start_pos + i) returns, bit for bit (Granite's logit scale
+ *     included; the classifier's padding rows are never part of l);
+ *   - greedy_ids[i] = the first index of the strict maximum m of l (FloatTensor.argmax, b200_forward_decode's argmax);
+ *   - S = sum_j exp((double)l_j - (double)m) in double, in an order fixed by vocab_size alone (not by n, the mode or the launch);
+ *   - logprobs[i] = ((double)l_t - (double)m) - log(S) for t = targets[i], NaN for targets[i] == -1.  No temperature.
+ * Limits and validation are b200_forward_batch_prefill's: n <= prefill_batch_size when that is > 1, positions inside the KV cache,
+ * tokens inside the vocabulary; a target other than -1 or a token id fails with B200_ERR_BAD_ARG.  The path follows the prefill
+ * mode (b200_set_prefill_mode):
+ *   B200_PREFILL_TENSOR_CORE_EXACT  the int8 tensor-core prefill of the chunk, then the final norm, the classifier as one int8 GEMM
+ *                                   per 256 rows (expanded from the resident tiles first on a resident plan) and the per-row
+ *                                   reduction.  The first call allocates a logits scratch of 256 rows and, on a resident plan whose
+ *                                   classifier's Q8_0 tiles exceed the prefill's expansion scratch, grows that scratch; B200_ERR_OOM
+ *                                   naming the bytes when they exceed the device's free memory;
+ *   B200_PREFILL_EXACT              on plans that run b200_forward_decode_multi: multi-position steps with the classifier on every row;
+ *                                   on every other single-GPU plan (FP16, Qwen2-MoE, resident): the single-token decode graph per
+ *                                   position.  n <= context_length + 8.
+ * B200_ERR_UNSUPPORTED with the reason on tensor-parallel plans (full logits are not gathered) and in the tensor_core and
+ * tensor_core_w8a16 modes (their f16 activations do not give the reference's logits: use exact or tensor_core_exact).  A refused
+ * or failed call leaves the plan able to decode. */
+int b200_score_tokens(b200_plan *plan, const int32_t *tokens, const int32_t *targets, int32_t n, int32_t start_pos, double *logprobs,
+                      int32_t *greedy_ids);
+
 /* How the single-token forwards (b200_forward_decode / _prefill / b200_decode_sequence) run.  Both replace
  * TornadoVMMasterPlanSingleToken.tornadoVMForwardDecode's N+2 TaskGraph executions
  * (TornadoVMMasterPlanSingleToken.java:68-95) and produce bit-identical results:

@@ -14,6 +14,7 @@
 #include "moe.cuh"
 #include "prefill_i8.cuh"
 #include "score.cuh"
+#include "logprobs.cuh"
 
 #include <math.h>
 #include <stdarg.h>
@@ -206,6 +207,15 @@ struct b200_plan {
         int ldl = 0;
         CUtensorMap cls_q, cls_s;
     } sc;
+
+    // b200_set_logprobs (logprobs.cuh): top_n < 0 is off.  While on, each emitting call runs k_token_logprobs on its rows after its
+    // graph into out (cap rows) and copies them to the pinned h_out inside its synchronise; smp holds the copies of sampled rows
+    // that the sampler turns into probabilities (SMB_MAX_ROWS padded rows), so k_token_logprobs reads the untouched logits
+    struct Logprobs {
+        int top_n = -1, cap = 0, rows = 0;
+        LogprobRow *out = nullptr, *h_out = nullptr;
+        float *smp = nullptr;
+    } lp;
 };
 
 namespace {
@@ -2265,16 +2275,37 @@ int launch_sample(b200_plan *p, float *logits, float temperature, float topp, fl
     return B200_OK;
 }
 
-// The device sampler on the batch's logits rows row[j], j < m, one block per row in one launch: row r's token at
+// The device sampler on the logits rows row[j], j < m, of the batch's layout (bt.logits, or its logprobs copy lp.smp), one block per row in one launch: row r's token at
 // bt.smp_out[8 r], its diagnostics after it.
-int launch_sample_rows(b200_plan *p, int m, const int *row, const float *temperature, const float *topp, const float *uniform01) {
+int launch_sample_rows(b200_plan *p, float *logits, int m, const int *row, const float *temperature, const float *topp, const float *uniform01) {
     static_assert(SMB_MAX_ROWS <= SAMPLER_MAX_ROWS, "k_sample_rows takes every row of a batched step");
     SamplerRowsArgs a;
-    a.logits = p->bt.logits; a.stride = sampler_padded(p->cfg.vocab_size); a.n = p->cfg.vocab_size;
+    a.logits = logits; a.stride = sampler_padded(p->cfg.vocab_size); a.n = p->cfg.vocab_size;
     a.indices = p->bt.smp_indices; a.out = p->bt.smp_out;
     for (int j = 0; j < m; j++) { a.row[j] = row[j]; a.temperature[j] = temperature[j]; a.topp[j] = topp[j]; a.r01[j] = uniform01[j]; }
     k_sample_rows<<<m, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
     CK(cudaGetLastError());
+    return B200_OK;
+}
+
+// k_token_logprobs on n rows: row k of logits (stride floats apart) emitted *ids[k] and fills result row out_row[k].
+int launch_logprobs(b200_plan *p, const float *logits, long long stride, int n, const int *const *ids, const int *out_row) {
+    static_assert(SMB_MAX_ROWS <= LOGPROB_MAX_ROWS, "k_token_logprobs takes every row of a batched step");
+    static_assert(B200_MAX_TOP_LOGPROBS == LOGPROB_MAX_TOP, "the header's limit is the kernel's");
+    LogprobArgs a{};
+    a.logits = logits; a.stride = stride; a.vocab = p->cfg.vocab_size; a.n_top = p->lp.top_n; a.out = p->lp.out;
+    for (int k = 0; k < n; k++) { a.ids[k] = ids[k]; a.out_row[k] = out_row[k]; }
+    k_token_logprobs<<<n, SCORE_THREADS, 0, p->stream>>>(a);
+    CK(cudaGetLastError());
+    return B200_OK;
+}
+
+// One row of the single-token calls: p->logits, the id at *id, result row `row`.
+int launch_logprobs_one(b200_plan *p, const int *id, int row) { return launch_logprobs(p, p->logits, 0, 1, &id, &row); }
+
+// The result rows [0, n) to the pinned table; the caller's synchronise completes the copy.
+int copy_logprobs(b200_plan *p, int n) {
+    CK(cudaMemcpyAsync(p->lp.h_out, p->lp.out, (size_t)n * sizeof(LogprobRow), cudaMemcpyDeviceToHost, p->stream));
     return B200_OK;
 }
 
@@ -2358,10 +2389,30 @@ int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, int32_t
         srow[m] = k; t[m] = r.temperature; tp[m] = r.topp; u[m] = r.uniform01;
         m++;
     }
-    if (m && (rc = launch_sample_rows(p, m, srow, t, tp, u))) return rc;
+    const bool lp = p->lp.top_n >= 0;
+    float *smp = B.logits;
+    if (lp && m) { // the sampler overwrites its rows with probabilities: it samples copies (zero pad included) in the same layout
+        smp = p->lp.smp;
+        for (int j = 0; j < m; j++) CK(cudaMemcpyAsync(smp + srow[j] * vpad, B.logits + srow[j] * vpad, vpad * 4, cudaMemcpyDeviceToDevice, p->stream));
+    }
+    if (m && (rc = launch_sample_rows(p, smp, m, srow, t, tp, u))) return rc;
+    if (lp && e) {
+        const int *ids[SMB_MAX_ROWS];
+        for (int k = 0; k < e; k++) ids[k] = rows[order[k]].temperature != 0.0f ? B.smp_out + 8 * k : B.ids + k;
+        if ((rc = launch_logprobs(p, B.logits, (long long)vpad, e, ids, order))) return rc;
+    }
+    if (lp && (rc = copy_logprobs(p, n))) return rc;
     if (e) CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)e * 4, cudaMemcpyDeviceToHost, p->stream));
     if (m) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)e * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
     CK(cudaStreamSynchronize(p->stream));
+    if (lp) {
+        for (int k = e; k < n; k++) { // rows that do not emit
+            LogprobRow &r = p->lp.h_out[order[k]];
+            r.chosen = NAN;
+            for (int j = 0; j < LOGPROB_MAX_TOP; j++) { r.id[j] = -1; r.lp[j] = NAN; }
+        }
+        p->lp.rows = n;
+    }
     for (int i = 0; i < n; i++) ids_out[i] = -1;
     for (int k = 0; k < e; k++) ids_out[order[k]] = rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
     CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
@@ -2605,10 +2656,13 @@ int b200_forward_decode(b200_plan *p, int32_t token, int32_t position, float *lo
     CK(cudaSetDevice(p->device));
     if ((rc = set_state(p, token, position, 0, 0))) return rc;
     CK(cudaGraphLaunch(decode_graph(p), p->stream));
+    const bool lp = p->lp.top_n >= 0;
+    if (lp && ((rc = launch_logprobs_one(p, p->out_ids, 0)) || (rc = copy_logprobs(p, 1)))) return rc;
     if (argmax) CK(cudaMemcpyAsync(p->h_ids, p->out_ids, 4, cudaMemcpyDeviceToHost, p->stream));
     if (logits) CK(cudaMemcpyAsync(logits, p->logits, (size_t)p->cfg.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
     CK(cudaStreamSynchronize(p->stream));
     if ((rc = check_device_error(p))) return rc;
+    if (lp) p->lp.rows = 1;
     if (argmax) *argmax = p->h_ids[0];
     return B200_OK;
 }
@@ -2624,12 +2678,20 @@ int b200_forward_decode_sample(b200_plan *p, int32_t token, int32_t position, fl
     if ((rc = set_state(p, token, position, 0, 0))) return rc;
     CK(cudaGraphLaunch(decode_graph(p), p->stream));
     const bool greedy = temperature == 0.0f; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed by the forward
+    const bool lp = p->lp.top_n >= 0;
     if (!greedy) {
-        if ((rc = launch_sample(p, p->logits, temperature, topp, uniform01, p->smp_out))) return rc;
+        float *row = p->logits;
+        if (lp) { // the sampler overwrites its row with probabilities: it samples a copy (zero pad included)
+            row = p->lp.smp;
+            CK(cudaMemcpyAsync(row, p->logits, (size_t)sampler_padded(p->cfg.vocab_size) * 4, cudaMemcpyDeviceToDevice, p->stream));
+        }
+        if ((rc = launch_sample(p, row, temperature, topp, uniform01, p->smp_out))) return rc;
         CK(cudaMemcpyAsync(p->h_ids, p->smp_out, 5 * 4, cudaMemcpyDeviceToHost, p->stream));
     } else CK(cudaMemcpyAsync(p->h_ids, p->out_ids, 4, cudaMemcpyDeviceToHost, p->stream));
+    if (lp && ((rc = launch_logprobs_one(p, greedy ? p->out_ids : p->smp_out, 0)) || (rc = copy_logprobs(p, 1)))) return rc;
     CK(cudaStreamSynchronize(p->stream));
     if ((rc = check_device_error(p))) return rc;
+    if (lp) p->lp.rows = 1;
     *token_out = p->h_ids[0];
     if (info) for (int k = 0; k < 4; k++) info[k] = greedy ? 0 : p->h_ids[1 + k];
     return B200_OK;
@@ -2743,12 +2805,18 @@ int b200_decode_sequence(b200_plan *p, const int32_t *tokens, int32_t n, int32_t
     CK(cudaMemcpyAsync(p->seq_tokens, p->h_ids, (size_t)nt * 4, cudaMemcpyHostToDevice, p->stream));
     int rc;
     if ((rc = set_state(p, tokens[0], start_pos, nt, feedback))) return rc;
+    const bool lp = p->lp.top_n >= 0;
     CK(cudaEventRecord(p->ev0, p->stream));
-    for (int i = 0; i < n; i++) CK(cudaGraphLaunch(decode_graph(p), p->stream));
+    for (int i = 0; i < n; i++) {
+        CK(cudaGraphLaunch(decode_graph(p), p->stream));
+        if (lp && (rc = launch_logprobs_one(p, p->out_ids + i, i))) return rc; // before the next step overwrites p->logits
+    }
     CK(cudaEventRecord(p->ev1, p->stream));
+    if (lp && (rc = copy_logprobs(p, n))) return rc;
     if (out_ids) CK(cudaMemcpyAsync(p->h_ids, p->out_ids, (size_t)n * 4, cudaMemcpyDeviceToHost, p->stream));
     CK(cudaStreamSynchronize(p->stream));
     if ((rc = check_device_error(p))) return rc;
+    if (lp) p->lp.rows = n;
     if (out_ids) memcpy(out_ids, p->h_ids, (size_t)n * 4);
     if (device_ms) CK(cudaEventElapsedTime(device_ms, p->ev0, p->ev1));
     return B200_OK;
@@ -3108,6 +3176,52 @@ int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, 
     return B200_OK;
 }
 
+int b200_set_logprobs(b200_plan *p, int32_t top_n) {
+    if (!p) return B200_ERR_BAD_ARG;
+    if (top_n < -1 || top_n > B200_MAX_TOP_LOGPROBS)
+        return fail(p, B200_ERR_BAD_ARG, "top_n = %d: -1 (off) or 0..%d alternatives", top_n, B200_MAX_TOP_LOGPROBS);
+    auto &L = p->lp;
+    if (top_n >= 0) {
+        if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "full logits are not gathered under tensor parallelism: logprobs run on single-GPU plans");
+        if (top_n > p->cfg.vocab_size) return fail(p, B200_ERR_BAD_ARG, "top_n = %d exceeds the vocabulary (%d)", top_n, p->cfg.vocab_size);
+        // each buffer on its own: a call that failed part-way leaves the rest to the next call, and logprobs stay off until all exist
+        CK(cudaSetDevice(p->device));
+        const int cap = p->seq_cap > SMB_MAX_ROWS ? p->seq_cap : SMB_MAX_ROWS;
+        int rc;
+        if (!L.out && (rc = dalloc(p, &L.out, (size_t)cap * sizeof(LogprobRow)))) return rc;
+        if (!L.smp && (rc = dalloc(p, &L.smp, (size_t)SMB_MAX_ROWS * sampler_padded(p->cfg.vocab_size) * 4))) return rc;
+        if (!L.h_out) {
+            if (cudaMallocHost(&L.h_out, (size_t)cap * sizeof(LogprobRow)) != cudaSuccess) {
+                L.h_out = nullptr;
+                return fail(p, B200_ERR_OOM, "pinned host memory for the logprobs table (%zu bytes)", (size_t)cap * sizeof(LogprobRow));
+            }
+        }
+        L.cap = cap;
+    }
+    L.top_n = top_n;
+    L.rows = 0;
+    return B200_OK;
+}
+
+int b200_read_logprobs(b200_plan *p, int32_t max_rows, int32_t *n_rows, double *chosen, int32_t *top_ids, double *top_logprobs) {
+    if (!p || !n_rows) return B200_ERR_BAD_ARG;
+    const auto &L = p->lp;
+    if (L.top_n < 0) return fail(p, B200_ERR_STATE, "logprobs are off: call b200_set_logprobs first");
+    *n_rows = L.rows;
+    if (!chosen && !top_ids && !top_logprobs) return B200_OK; // the row count alone
+    if (max_rows < L.rows) return fail(p, B200_ERR_BAD_ARG, "the table has %d rows, max_rows is %d", L.rows, max_rows);
+    const int N = L.top_n;
+    for (int i = 0; i < L.rows; i++) {
+        const LogprobRow &r = L.h_out[i];
+        if (chosen) chosen[i] = r.chosen;
+        for (int k = 0; k < N; k++) {
+            if (top_ids) top_ids[(size_t)i * N + k] = r.id[k];
+            if (top_logprobs) top_logprobs[(size_t)i * N + k] = r.lp[k];
+        }
+    }
+    return B200_OK;
+}
+
 int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, size_t bytes) {
     if (!p || !name || !dst) return B200_ERR_BAD_ARG;
     const b200_config &c = p->cfg;
@@ -3342,6 +3456,41 @@ int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out
     memcpy(out, host, 4);
     if (info) { info[0] = host[1]; info[1] = host[2]; }
     return e == cudaSuccess ? B200_OK : B200_ERR_CUDA;
+}
+
+int b200_test_logprobs(const float *logits, int32_t vocab, int32_t chosen_id, int32_t top_n, int32_t reps, double *chosen, int32_t *top_ids,
+                       double *top_logprobs, float *avg_ms) {
+    if (!logits || vocab <= 0 || chosen_id < 0 || chosen_id >= vocab || top_n < 0 || top_n > LOGPROB_MAX_TOP || top_n > vocab || reps < 1)
+        return B200_ERR_BAD_ARG;
+    Scratch s;
+    float *d = nullptr;
+    int *id = nullptr;
+    LogprobRow *out = nullptr;
+    if (!s.alloc(&d, (size_t)vocab * 4) || !s.alloc(&id, 4) || !s.alloc(&out, sizeof(LogprobRow))) return s.rc;
+    LogprobArgs a{};
+    a.logits = d; a.stride = 0; a.vocab = vocab; a.n_top = top_n; a.ids[0] = id; a.out_row[0] = 0; a.out = out;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    s.ok(cudaMemcpy(d, logits, (size_t)vocab * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(id, &chosen_id, 4, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaEventCreate(&e0)) && s.ok(cudaEventCreate(&e1));
+    if (s.rc == B200_OK) {
+        k_token_logprobs<<<1, SCORE_THREADS>>>(a); // warm-up
+        s.ok(cudaEventRecord(e0));
+        for (int r = 0; r < reps; r++) k_token_logprobs<<<1, SCORE_THREADS>>>(a);
+        s.ok(cudaEventRecord(e1)) && s.ok(cudaGetLastError()) && s.ok(cudaEventSynchronize(e1));
+    }
+    float ms = 0.f;
+    LogprobRow h{};
+    if (s.rc == B200_OK && s.ok(cudaEventElapsedTime(&ms, e0, e1)) && s.ok(cudaMemcpy(&h, out, sizeof(LogprobRow), cudaMemcpyDeviceToHost))) {
+        if (avg_ms) *avg_ms = ms / reps;
+        if (chosen) *chosen = h.chosen;
+        for (int k = 0; k < top_n; k++) {
+            if (top_ids) top_ids[k] = h.id[k];
+            if (top_logprobs) top_logprobs[k] = h.lp[k];
+        }
+    }
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+    return s.rc;
 }
 
 int b200_profile_seqsum2(const float *terms, int32_t n, int32_t threads, int64_t *cycles, float *out) {
@@ -3732,6 +3881,7 @@ void b200_plan_free(b200_plan *p) {
     for (void *d : p->allocs) cudaFree(d);
     if (p->h_st) cudaFreeHost(p->h_st);
     if (p->h_ids) cudaFreeHost(p->h_ids);
+    if (p->lp.h_out) cudaFreeHost(p->lp.h_out);
     if (p->ev0) cudaEventDestroy(p->ev0);
     if (p->ev1) cudaEventDestroy(p->ev1);
     if (p->stream) cudaStreamDestroy(p->stream);

@@ -23,17 +23,16 @@ struct ScoreOut {
     int greedy, pad;
 };
 
-__global__ void __launch_bounds__(SCORE_THREADS) k_score_rows(const float *__restrict__ logits, long long stride, int vocab,
-                                                              const int *__restrict__ targets, ScoreOut *__restrict__ out) {
-    __shared__ float sv[SCORE_THREADS / 32];
-    __shared__ int si[SCORE_THREADS / 32];
-    __shared__ double ss[SCORE_THREADS / 32];
-    __shared__ float s_m;
-    __shared__ int s_i;
+// Row blockIdx.x's maximum m and the first index of it (s_m, s_i) and S = sum_j exp((double)l_j - m), by a SCORE_THREADS-thread
+// block over its shared scratch sv / si / ss; thread 0 then runs tail(row, S, m).  k_score_rows and k_token_logprobs (logprobs.cuh)
+// both call it, so their m and S are the same code and the same bits.
+template <typename Tail>
+__device__ __forceinline__ void score_row(const float *logits, long long stride, int vocab, float (&sv)[SCORE_THREADS / 32], int (&si)[SCORE_THREADS / 32],
+                                          double (&ss)[SCORE_THREADS / 32], float &s_m, int &s_i, Tail &&tail) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float *l = logits + (size_t)blockIdx.x * stride;
-    float best = -INFINITY;
     int best_i = 0x7fffffff;
+    float best = -INFINITY;
     for (int j = tid; j < vocab; j += SCORE_THREADS) {
         const float v = l[j];
         if (v > best) { best = v; best_i = j; }
@@ -62,8 +61,20 @@ __global__ void __launch_bounds__(SCORE_THREADS) k_score_rows(const float *__res
         double S = 0.0;
 #pragma unroll
         for (int w = 0; w < SCORE_THREADS / 32; w++) S = __dadd_rn(S, ss[w]);
+        tail(l, S, m);
+    }
+}
+
+__global__ void __launch_bounds__(SCORE_THREADS) k_score_rows(const float *__restrict__ logits, long long stride, int vocab,
+                                                              const int *__restrict__ targets, ScoreOut *__restrict__ out) {
+    __shared__ float sv[SCORE_THREADS / 32];
+    __shared__ int si[SCORE_THREADS / 32];
+    __shared__ double ss[SCORE_THREADS / 32];
+    __shared__ float s_m;
+    __shared__ int s_i;
+    score_row(logits, stride, vocab, sv, si, ss, s_m, s_i, [&](const float *l, double S, double m) {
         const int t = targets[blockIdx.x];
         out[blockIdx.x].logprob = t < 0 ? __longlong_as_double(0x7ff8000000000000ll) : __dsub_rn(__dsub_rn((double)l[t], m), log(S));
         out[blockIdx.x].greedy = s_i;
-    }
+    });
 }

@@ -16,6 +16,13 @@ Position/token conventions decide parity, so they are restated exactly:
                               requests and prompt rows of newly admitted ones share each forward_step, and freed slots are
                               refilled from a queue
 ``score_sequence`` / ``perplexity`` teacher-forced scoring of a given text (plan.score_tokens) in chunks the plan accepts
+The plan-driven loops take an optional ``logprobs`` list: with the plan's log-probabilities on (plan.set_logprobs(N)) it receives
+one entry (chosen, [(id, logprob), ...]) per generated id -- per request, one list per request -- from plan.last_logprobs().
+``generate_tokens_llama`` / ``_qwen3`` take a callable; it reads them itself, e.g.
+    def forward(tok, pos):
+        _, am = plan.forward_decode(tok, pos, logits=False)
+        rows.append(plan.last_logprobs())  # the row of the id just emitted
+        return am
 The sampler is greedy (temperature 0 -> FloatTensor.argmax, Sampler.java:124-132) and runs on
 the device; ``forward`` is any callable (token, position) -> argmax so the same loops drive
 the oracle in the tests.
@@ -33,12 +40,13 @@ Forward = Callable[[int, int], int]
 
 
 def _llama_steps(latest_token: int, start_position: int, prompt_tokens: list[int], stop_tokens: Iterable[int], max_tokens: int,
-                 context_length: int):
-    """generate_tokens_llama as a generator: yields each forward's (token, position), receives its argmax, returns the ids."""
+                 context_length: int, generated: list | None = None):
+    """generate_tokens_llama as a generator: yields each forward's (token, position), receives its argmax, returns the ids
+    (`generated` if given, so a caller can see which results became ids)."""
     if max_tokens < 0 or context_length < max_tokens:
         max_tokens = context_length
     stop = set(stop_tokens)
-    generated: list[int] = []
+    generated = [] if generated is None else generated
     current, prompt_index, pos = latest_token, 0, start_position
     while pos < max_tokens:
         am = yield current, pos
@@ -56,12 +64,12 @@ def _llama_steps(latest_token: int, start_position: int, prompt_tokens: list[int
 
 
 def _qwen3_steps(latest_token: int, start_position: int, prompt_tokens: list[int], stop_tokens: Iterable[int], max_tokens: int,
-                 context_length: int):
+                 context_length: int, generated: list | None = None):
     """generate_tokens_qwen3 as a generator (see _llama_steps)."""
     if max_tokens < 0 or context_length < max_tokens:
         max_tokens = context_length
     stop = set(stop_tokens)
-    generated: list[int] = []
+    generated = [] if generated is None else generated
     current, prompt_index = latest_token, 0
     position = start_position
     while position < max_tokens:
@@ -113,22 +121,33 @@ def _is_qwen_loop(model_type: str) -> bool:
     return model_type.upper() in ("QWEN_3", "QWEN_2", "QWEN_2_MOE", "DEEPSEEK_R1_DISTILL_QWEN")
 
 
+def _logprob_rows(plan) -> list:
+    """plan.last_logprobs() as one (chosen, [(id, logprob), ...]) entry per row of the last emitting call."""
+    chosen, ids, lps = plan.last_logprobs()
+    return [(float(chosen[r]), [(int(i), float(v)) for i, v in zip(ids[r], lps[r])]) for r in range(len(chosen))]
+
+
 def generate_tokens_batch(plan, model_type: str, requests: list, stop_tokens: Iterable[int], max_tokens: int,
-                          context_length: int) -> list[list[int]]:
+                          context_length: int, logprobs: list | None = None) -> list[list[int]]:
     """Several independent generations in lockstep on the plan's decode slots (request i on slot i, reset first): one
     forward_decode_batch per step for every request still running.  Each request is (latest_token, start_position,
     prompt_tokens) and follows the loop loop_for(model_type) runs, so each result equals that loop's for the request alone;
-    a request leaves the batch at its stop token or budget."""
+    a request leaves the batch at its stop token or budget.  logprobs (optional list, plan.set_logprobs on) receives one list per
+    request, one entry per generated id."""
     n_slots = plan.batch_info()[0]
     if len(requests) > n_slots:
         raise ValueError(f"{len(requests)} requests but the plan has {n_slots} decode slots (set_decode_slots)")
     make = _qwen3_steps if _is_qwen_loop(model_type) else _llama_steps
     stop = list(stop_tokens)
     results: list = [None] * len(requests)
+    gen = [[] for _ in requests]
+    lp = [[] for _ in requests]
+    if logprobs is not None:
+        logprobs.extend(lp)
     live: dict = {}  # request index -> (generator, pending (token, position))
     for i, (latest, start, prompt) in enumerate(requests):
         plan.slot_reset(i)
-        g = make(latest, start, list(prompt), stop, max_tokens, context_length)
+        g = make(latest, start, list(prompt), stop, max_tokens, context_length, gen[i])
         try:
             live[i] = (g, next(g))
         except StopIteration as done:
@@ -136,21 +155,27 @@ def generate_tokens_batch(plan, model_type: str, requests: list, stop_tokens: It
     while live:
         rows = sorted(live)
         ids, _ = plan.forward_decode_batch(rows, [live[i][1][0] for i in rows], [live[i][1][1] for i in rows])
-        for i, am in zip(rows, ids):
+        entries = _logprob_rows(plan) if logprobs is not None else None
+        for k, (i, am) in enumerate(zip(rows, ids)):
             g = live[i][0]
+            n0 = len(gen[i])
             try:
                 live[i] = (g, g.send(int(am)))
             except StopIteration as done:
                 results[i] = done.value
                 del live[i]
+            if entries is not None and len(gen[i]) > n0:  # the row's id became a generated token
+                lp[i].append(entries[k])
     return results
 
 
 def generate_tokens_llama_batch_prefill(plan, latest_token: int, start_position: int, prompt_tokens: list[int],
-                                        stop_tokens: Iterable[int], max_tokens: int, context_length: int, batch_size: int) -> list[int]:
+                                        stop_tokens: Iterable[int], max_tokens: int, context_length: int, batch_size: int,
+                                        logprobs: list | None = None) -> list[int]:
     """prefillSeq = [latestToken, prompt[0..N-2]] at positions startPosition.. in chunks of B through the batched
     prefill, clamped to the token budget, then decode from the last prompt token at startPosition+N
-    (InferenceEngineWithBatchPrefillDecode.java:163-251; the chunk clamp is :204-205)."""
+    (InferenceEngineWithBatchPrefillDecode.java:163-251; the chunk clamp is :204-205).  logprobs (optional list, plan.set_logprobs
+    on) receives one entry per generated id."""
     if max_tokens < 0 or context_length < max_tokens:
         max_tokens = context_length
     stop = set(stop_tokens)
@@ -169,6 +194,8 @@ def generate_tokens_llama_batch_prefill(plan, latest_token: int, start_position:
     while pos < max_tokens:
         _, nxt = plan.forward_decode(current, pos, logits=False)
         generated.append(nxt)
+        if logprobs is not None:
+            logprobs.extend(_logprob_rows(plan))
         if nxt in stop:
             break
         current = nxt
@@ -177,13 +204,14 @@ def generate_tokens_llama_batch_prefill(plan, latest_token: int, start_position:
 
 
 def generate_tokens_batch_prefill(plan, model_type: str, requests: list, stop_tokens: Iterable[int], max_tokens: int,
-                                  context_length: int, batch_size: int) -> list[list[int]]:
+                                  context_length: int, batch_size: int, logprobs: list | None = None) -> list[list[int]]:
     """The batched counterpart of generate_tokens_llama_batch_prefill on the plan's decode slots (request i on slot i).  Each request
     (latest_token, start_position, prompt_tokens) prefills [latest] + prompt[:-1] into its slot, clamped to the token budget as that
     function clamps it; the prompts of all requests are packed into prefill_slots calls of at most batch_size tokens (a prompt may
     span two calls).  Then every request decodes in lockstep through forward_decode_batch from prompt[-1] at start + len(prompt)
     until its stop token or the budget, so each result equals generate_tokens_llama_batch_prefill for the request alone.  Only the
-    Llama loop has this form: a slot's rows past its prompt are never read, so the slots are not reset first."""
+    Llama loop has this form: a slot's rows past its prompt are never read, so the slots are not reset first.  logprobs (optional
+    list, plan.set_logprobs on) receives one list per request, one entry per generated id."""
     if _is_qwen_loop(model_type):
         raise ValueError(f"{model_type} runs the Qwen3 loop, which has no batched-prefill form: use generate_tokens_batch")
     n_slots = plan.batch_info()[0]
@@ -214,13 +242,19 @@ def generate_tokens_batch_prefill(plan, model_type: str, requests: list, stop_to
                 room -= take
         plan.prefill_slots(slots, starts, pieces)
     results: list = [[] for _ in requests]
+    lp = [[] for _ in requests]
+    if logprobs is not None:
+        logprobs.extend(lp)
     live = {i: (int(prompt[-1]), start + len(prompt)) for i, (_, start, prompt) in enumerate(requests) if start + len(prompt) < max_tokens}
     while live:
         rows = sorted(live)
         ids, _ = plan.forward_decode_batch(rows, [live[i][0] for i in rows], [live[i][1] for i in rows])
-        for i, am in zip(rows, ids):
+        entries = _logprob_rows(plan) if logprobs is not None else None
+        for k, (i, am) in enumerate(zip(rows, ids)):
             nxt = int(am)
             results[i].append(nxt)
+            if entries is not None:
+                lp[i].append(entries[k])
             pos = live[i][1] + 1
             if nxt in stop or pos >= max_tokens:
                 del live[i]
@@ -245,7 +279,8 @@ def prompt_lookup(history: list[int], max_tokens: int = 8) -> list[int]:
 
 def generate_tokens_lookahead(plan, model_type: str, latest_token: int, start_position: int, prompt_tokens: list[int],
                               stop_tokens: Iterable[int], max_tokens: int, context_length: int,
-                              draft: Callable[[list[int]], list[int]] = prompt_lookup, stats: dict | None = None) -> list[int]:
+                              draft: Callable[[list[int]], list[int]] = prompt_lookup, stats: dict | None = None,
+                              logprobs: list | None = None) -> list[int]:
     """generate_tokens_llama on the plan's own cache, verifying several positions per step with forward_decode_multi.
 
     Each step runs [current] + drafts (up to decode_multi_rows() - 1 drafts) at consecutive positions.  While prompt tokens remain
@@ -256,6 +291,8 @@ def generate_tokens_lookahead(plan, model_type: str, latest_token: int, start_po
     forward_decode of its token over the same cache prefix, and a rejected draft's K/V rows are rewritten before any later row
     reads them, so the result equals generate_tokens_llama for any draft function.  stats (optional dict) receives the steps run,
     the drafted tokens that were generated rather than forced, and how many of those were accepted.
+
+    logprobs (optional list, plan.set_logprobs on) receives one entry per generated id: the accepted rows' only.
 
     Llama loop only: the Qwen3 loop reads a skipped position as a zero row, which a rejected draft may have written."""
     if _is_qwen_loop(model_type):
@@ -276,6 +313,7 @@ def generate_tokens_lookahead(plan, model_type: str, latest_token: int, start_po
         guesses = prompt[prompt_index:] if forced else list(draft(list(history)))
         guesses = [int(t) for t in guesses[:min(rows, max_tokens - pos) - 1]]
         ids, _ = plan.forward_decode_multi(-1, [current] + guesses, pos)
+        entries = _logprob_rows(plan) if logprobs is not None else None
         steps += 1
         for i, am in enumerate(ids):
             if prompt_index < len(prompt):
@@ -285,6 +323,8 @@ def generate_tokens_lookahead(plan, model_type: str, latest_token: int, start_po
                 nxt = int(am)
                 generated.append(nxt)
                 history.append(nxt)
+                if entries is not None:
+                    logprobs.append(entries[i])
                 if i < len(guesses) and not forced:
                     drafted += 1
                     accepted += guesses[i] == nxt
@@ -325,7 +365,10 @@ class ContinuousBatcher:
 
     sampler (optional, per request): a sampler.Sampler; one next_float1() is drawn per generated token, never for a prompt row, as
     generateTokensLlama draws it (InferenceEngine.java:81-154).  The steps are always the exact mixed steps, whatever the plan's
-    prefill mode."""
+    prefill mode.
+
+    When the plan's log-probabilities are on (plan.set_logprobs), logprobs[rid] receives one entry (chosen, [(id, logprob), ...])
+    per generated id, next to results[rid]."""
 
     def __init__(self, plan, model_type: str, stop_tokens: Iterable[int], max_tokens: int, context_length: int):
         self.plan = plan
@@ -339,6 +382,7 @@ class ContinuousBatcher:
         self.stop = list(stop_tokens)
         self.max_tokens, self.context_length = max_tokens, context_length
         self.results: dict = {}  # request id -> generated ids so far
+        self.logprobs: dict = {}  # request id -> their log-probability entries (the plan's logprobs on)
         self.last_rows = 0  # rows of the last step() (0: no step ran)
         self._queue: deque = deque()
         self._free = list(range(n_slots))
@@ -355,6 +399,7 @@ class ContinuousBatcher:
         rid = self._next_id
         self._next_id += 1
         self.results[rid] = []
+        self.logprobs[rid] = []
         self._queue.append(_Request(rid, steps, sampler, max(len(prompt) - 1, 0) if self.qwen else len(prompt)))
         return rid
 
@@ -420,15 +465,19 @@ class ContinuousBatcher:
         self.last_rows = len(rows)
         if rows:
             ids, _ = self.plan.forward_step(rows)
+            lp_on = getattr(self.plan, "logprobs_top_n", lambda: -1)() >= 0  # a stand-in plan without log-probabilities: off
+            entries = _logprob_rows(self.plan) if lp_on else None
             done = list(ended)
             k = 0
-            for row, am in zip(rows, ids):
+            for j, (row, am) in enumerate(zip(rows, ids)):
                 if not row[3]:
                     continue
                 r = emit[k]
                 k += 1
                 tok = int(am)
                 self.results[r.rid].append(tok)
+                if entries is not None:
+                    self.logprobs[r.rid].append(entries[j])
                 r.generated += 1
                 alive = self._advance(r, tok)
                 out.append((r.rid, tok, not alive))
@@ -445,12 +494,14 @@ class ContinuousBatcher:
 
 
 def generate_tokens_continuous(plan, model_type: str, requests: list, arrivals: list, stop_tokens: Iterable[int], max_tokens: int,
-                               context_length: int, samplers: list | None = None, stats: dict | None = None) -> list[list[int]]:
+                               context_length: int, samplers: list | None = None, stats: dict | None = None,
+                               logprobs: list | None = None) -> list[list[int]]:
     """Replays a request trace through a ContinuousBatcher: request i = (latest_token, start_position, prompt_tokens) is submitted
     before step arrivals[i] (requests of the same step in index order), with samplers[i] if given.  Steps with no rows still count.
     Returns each request's ids, equal to loop_for(model_type) for the request alone.  stats (optional dict) receives the steps run,
     the rows and launches of each, and per request its submission, first-token and completion times (time.perf_counter seconds,
-    None where it generated no token)."""
+    None where it generated no token).  logprobs (optional list, plan.set_logprobs on) receives one list per request, one entry per
+    generated id."""
     if len(arrivals) != len(requests):
         raise ValueError(f"{len(requests)} requests but {len(arrivals)} arrival steps")
     if samplers is not None and len(samplers) != len(requests):
@@ -484,7 +535,10 @@ def generate_tokens_continuous(plan, model_type: str, requests: list, arrivals: 
         k += 1
     if stats is not None:
         stats.update(steps=len(rows), rows=rows, launches=launches, submitted=t_sub, first_token=t_first, done=t_done)
-    return [cb.results[rid] for rid in sorted(rid_of, key=lambda r: rid_of[r])]
+    rids = sorted(rid_of, key=lambda r: rid_of[r])
+    if logprobs is not None:
+        logprobs.extend(cb.logprobs[rid] for rid in rids)
+    return [cb.results[rid] for rid in rids]
 
 
 def score_sequence(plan, tokens: list[int], start_pos: int = 0):

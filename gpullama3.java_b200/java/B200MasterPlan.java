@@ -72,6 +72,8 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle PREFILL = fn("b200_forward_prefill", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
     private static final MethodHandle BATCH_PREFILL = fn("b200_forward_batch_prefill", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT));
     private static final MethodHandle SCORE_TOKENS = fn("b200_score_tokens", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS));
+    private static final MethodHandle SET_LOGPROBS = fn("b200_set_logprobs", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
+    private static final MethodHandle READ_LOGPROBS = fn("b200_read_logprobs", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
     private static final MethodHandle SET_PREFILL_MODE = fn("b200_set_prefill_mode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle SET_DECODE_MODE = fn("b200_set_decode_mode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle DECODE_SAMPLE = fn("b200_forward_decode_sample",
@@ -236,6 +238,45 @@ public final class B200MasterPlan implements AutoCloseable {
             if (rc != 0) check(rc, lastError());
             MemorySegment.copy(lp, java.lang.foreign.ValueLayout.JAVA_DOUBLE, 0, logprobs, 0, tokens.length);
             MemorySegment.copy(ids, JAVA_INT, 0, greedyIds, 0, tokens.length);
+        }
+    }
+
+    /** The last emitting call's log-probabilities: chosen[i] for its i-th emitted id, topIds[i][k] / topLogprobs[i][k] for the k-th
+     *  most likely alternative (ties to the lower id).  Rows of forwardStep that do not emit hold NaN and id -1. */
+    public record Logprobs(double[] chosen, int[][] topIds, double[][] topLogprobs) {}
+
+    private int logprobsTopN = -1;
+
+    /** Log-probabilities of generated tokens (b200_set_logprobs): -1 off (the default), 0..20 alternatives per emitted id.  While on,
+     *  every call that emits ids records one row per id, in double and under the raw logits (temperature 1), read with lastLogprobs.
+     *  Single-GPU plans only. */
+    public void setLogprobs(int topN) throws Throwable {
+        int rc = (int) SET_LOGPROBS.invokeExact(plan, topN);
+        if (rc != 0) check(rc, lastError());
+        logprobsTopN = topN;
+    }
+
+    /** The rows the last emitting call recorded (b200_read_logprobs); setLogprobs must be on. */
+    public Logprobs lastLogprobs() throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            MemorySegment nRows = a.allocate(JAVA_INT);
+            int rc = (int) READ_LOGPROBS.invokeExact(plan, 0, nRows, MemorySegment.NULL, MemorySegment.NULL, MemorySegment.NULL);
+            if (rc != 0) check(rc, lastError());
+            int rows = nRows.get(JAVA_INT, 0), n = Math.max(logprobsTopN, 0);
+            MemorySegment ch = a.allocate(java.lang.foreign.ValueLayout.JAVA_DOUBLE, Math.max(rows, 1));
+            MemorySegment ids = a.allocate(JAVA_INT, Math.max(rows * n, 1));
+            MemorySegment lps = a.allocate(java.lang.foreign.ValueLayout.JAVA_DOUBLE, Math.max(rows * n, 1));
+            rc = (int) READ_LOGPROBS.invokeExact(plan, rows, nRows, ch, ids, lps);
+            if (rc != 0) check(rc, lastError());
+            double[] chosen = new double[rows];
+            int[][] topIds = new int[rows][n];
+            double[][] topLogprobs = new double[rows][n];
+            MemorySegment.copy(ch, java.lang.foreign.ValueLayout.JAVA_DOUBLE, 0, chosen, 0, rows);
+            for (int i = 0; i < rows; i++) {
+                MemorySegment.copy(ids, JAVA_INT, (long) i * n * 4, topIds[i], 0, n);
+                MemorySegment.copy(lps, java.lang.foreign.ValueLayout.JAVA_DOUBLE, (long) i * n * 8, topLogprobs[i], 0, n);
+            }
+            return new Logprobs(chosen, topIds, topLogprobs);
         }
     }
 

@@ -59,7 +59,7 @@ class Tensor(C.Structure):
                 ("dims", C.c_int64 * 4)]
 
 
-EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_score_tokens", "b200_set_prefill_mode", "b200_prefill_info",
+EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_score_tokens", "b200_set_logprobs", "b200_read_logprobs", "b200_test_logprobs", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant", "b200_test_kq_tiles_to_q8",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
@@ -87,6 +87,9 @@ def lib() -> C.CDLL:
     L.b200_forward_decode_sample.argtypes = [vp, i32, i32, C.c_float, C.c_float, C.c_float, C.POINTER(i32), C.POINTER(i32)]
     L.b200_forward_batch_prefill.argtypes = [vp, vp, i32, i32]
     L.b200_score_tokens.argtypes = [vp, vp, vp, i32, i32, vp, vp]
+    L.b200_set_logprobs.argtypes = [vp, i32]
+    L.b200_read_logprobs.argtypes = [vp, i32, C.POINTER(i32), vp, vp, vp]
+    L.b200_test_logprobs.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, C.POINTER(C.c_float)]
     L.b200_decode_sequence.argtypes = [vp, vp, i32, i32, i32, vp, C.POINTER(C.c_float)]
     L.b200_kv_reset.argtypes = [vp]
     L.b200_profile_norm.argtypes = [vp, C.POINTER(C.c_int64)]
@@ -374,6 +377,19 @@ def test_pf_attention(q, k, v, n_heads: int, n_kv_heads: int, start_pos: int, im
 GGML_SIZES = {0: (4, 1), 1: (2, 1), 8: (34, 32), 12: (144, 256), 13: (176, 256), 14: (210, 256)}  # (bytes, elements) per block, GGMLType.java:5-20
 
 
+def test_logprobs(logits, chosen_id: int, top_n: int, reps: int = 1):
+    """b200_test_logprobs: k_token_logprobs on one row -> (chosen, top ids int32 [top_n], top logprobs float64 [top_n], ms per launch)."""
+    lg = np.ascontiguousarray(logits, dtype=np.float32).reshape(-1)
+    c = C.c_double(0)
+    ids = np.empty(top_n, np.int32)
+    lps = np.empty(top_n, np.float64)
+    ms = C.c_float(0)
+    rc = lib().b200_test_logprobs(lg.ctypes.data, len(lg), int(chosen_id), int(top_n), int(reps), C.byref(c), ids.ctypes.data, lps.ctypes.data, C.byref(ms))
+    if rc != B200_OK:
+        _raise(rc, "b200_test_logprobs failed")
+    return c.value, ids, lps, ms.value
+
+
 class NativePlan:
     """Owns one ``b200_plan*``."""
 
@@ -477,6 +493,29 @@ class NativePlan:
         ids = np.empty(n, dtype=np.int32)
         self._ck(lib().b200_score_tokens(self._p, t.ctypes.data, tg.ctypes.data, n, start_pos, lp.ctypes.data, ids.ctypes.data))
         return lp, ids
+
+    MAX_TOP_LOGPROBS = 20  # B200_MAX_TOP_LOGPROBS
+
+    def set_logprobs(self, top_n: int):
+        """b200_set_logprobs: -1 off (the default); 0..20 alternatives per emitted row while on."""
+        self._ck(lib().b200_set_logprobs(self._p, int(top_n)))
+        self._top_n = int(top_n)
+
+    def logprobs_top_n(self) -> int:
+        return getattr(self, "_top_n", -1)
+
+    def last_logprobs(self):
+        """b200_read_logprobs: the last emitting call's rows -> (chosen float64 [rows], top_ids int32 [rows, N],
+        top_logprobs float64 [rows, N])."""
+        n_top = max(self.logprobs_top_n(), 0)
+        rows = C.c_int32(0)
+        self._ck(lib().b200_read_logprobs(self._p, 0, C.byref(rows), None, None, None))  # the row count alone
+        r = rows.value
+        chosen = np.empty(r, dtype=np.float64)
+        ids = np.empty((r, n_top), dtype=np.int32)
+        lps = np.empty((r, n_top), dtype=np.float64)
+        self._ck(lib().b200_read_logprobs(self._p, r, C.byref(rows), chosen.ctypes.data, ids.ctypes.data, lps.ctypes.data))
+        return chosen, ids, lps
 
     def decode_sequence(self, tokens, n: int, start_pos: int, feedback: bool = False):
         t = np.ascontiguousarray(tokens, dtype=np.int32)

@@ -132,6 +132,22 @@ class B200MasterPlan:
         most forward_batch_prefill's chunk length (engine.score_sequence splits longer sequences)."""
         return self._native.score_tokens(tokens, start_pos, targets)
 
+    def set_logprobs(self, top_n: int):
+        """Log-probabilities of generated tokens (b200_set_logprobs): -1 off (the default), 0..20 alternatives per row.  While on, every
+        call that emits ids (forward_decode, forward_decode_sample, decode_sequence, forward_decode_batch, forward_decode_multi,
+        forward_step) records one row per emitted id, read back with last_logprobs().  Single-GPU plans only."""
+        self._native.set_logprobs(top_n)
+
+    def logprobs_top_n(self) -> int:
+        """The set_logprobs setting: -1 off, else the alternatives per row."""
+        return self._native.logprobs_top_n()
+
+    def last_logprobs(self):
+        """The last emitting call's rows -> (chosen float64 [rows], top_ids int32 [rows, N], top_logprobs float64 [rows, N]): the
+        emitted id's log-probability under the raw logits (temperature 1, in double; bit-equal to score_tokens') and the N most
+        likely ids, ties to the lower index, with theirs.  Rows of forward_step that do not emit: NaN and ids -1."""
+        return self._native.last_logprobs()
+
     # TensorCoreSupport.java's switch between the MMA and the plain batch-prefill layer families
     PREFILL_EXACT, PREFILL_TENSOR_CORE, PREFILL_TENSOR_CORE_W8A16, PREFILL_TENSOR_CORE_EXACT = 0, 1, 2, 3
 

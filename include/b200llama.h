@@ -274,6 +274,43 @@ int b200_prefill_info(b200_plan *plan, int32_t *mode, int32_t *launches, float *
 int b200_score_tokens(b200_plan *plan, const int32_t *tokens, const int32_t *targets, int32_t n, int32_t start_pos, double *logprobs,
                       int32_t *greedy_ids);
 
+/* Log-probabilities of generated tokens: each emitted id's log-probability and its top-N alternatives, computed on the device, for
+ * OpenAI-style logprobs / top_logprobs, confidence filtering and evaluation harnesses that record completion likelihoods.
+ * b200_set_logprobs(plan, top_n): -1 turns them off (the default), 0..B200_MAX_TOP_LOGPROBS turns them on with top_n alternatives per
+ * row.  While on, each call that emits ids fills the plan's result table with its rows, and b200_read_logprobs reads it:
+ *   b200_forward_decode, b200_forward_decode_sample      one row;
+ *   b200_decode_sequence                                  n rows, one per step;
+ *   b200_forward_decode_batch, _multi, b200_forward_step  n rows in the call's row order.
+ * Every other call leaves the table alone; b200_set_logprobs empties it.  Definition, for an emitting row whose logits l[0, vocab) are
+ * exactly the row the call returns through its `logits` argument and whose id c is exactly the id it returns (the argmax or the
+ * sampler's id):
+ *   - m and S are b200_score_tokens' (its sum order, fixed by vocab_size alone);
+ *   - chosen = ((double)l_c - m) - log(S): bit-equal to b200_score_tokens' logprob of target c at the same position over the same
+ *     cache prefix;
+ *   - t_k, k = 1..top_n: the first index of the strict maximum among the entries not yet taken; when no remaining entry is > -inf
+ *     (NaN rows included), the lowest index not yet taken.  t_1 is the greedy id.  top_logprob_k = ((double)l_{t_k} - m) - log(S);
+ *   - the raw logits' values: temperature 1, no top-p truncation, Granite's logit scale included, so a sampled token's value is the
+ *     model's probability, not the sampler's; the classifier's padding rows never appear;
+ *   - rows of b200_forward_step with emit == 0: chosen NaN, ids -1, logprobs NaN.
+ * The kernel (k_token_logprobs, one block per row) runs on the plan's stream after the call's graph and is never part of a graph:
+ * b200_decode_info's and b200_batch_info's launch counts and b200_batch_info's device time are unchanged, while
+ * b200_decode_sequence's device_ms includes the one launch per step.  Sampled rows are copied before the sampler turns them into
+ * probabilities; the sampler reads the copy, so the ids equal those with logprobs off for the same uniform numbers.  The results
+ * reach pinned host memory inside the call's own synchronise.  The table holds max(the plan's sequence capacity, 8) rows.
+ * B200_ERR_BAD_ARG for top_n outside -1..20 or above vocab_size; B200_ERR_UNSUPPORTED on tensor-parallel plans (full logits are
+ * not gathered). */
+#define B200_MAX_TOP_LOGPROBS 20
+int b200_set_logprobs(b200_plan *plan, int32_t top_n);
+/* The last emitting call's table: *n_rows rows; chosen[i], top_ids[i * top_n + k] and top_logprobs[i * top_n + k] (any of the
+ * three may be NULL; with all three NULL only *n_rows is set).  B200_ERR_STATE while logprobs are off; B200_ERR_BAD_ARG if the table
+ * has more than max_rows rows. */
+int b200_read_logprobs(b200_plan *plan, int32_t max_rows, int32_t *n_rows, double *chosen, int32_t *top_ids /* max_rows x top_n */,
+                       double *top_logprobs /* max_rows x top_n */);
+/* Test and measurement hook (no plan): k_token_logprobs on one host row logits[0, vocab) with emitted id chosen_id, run reps times on
+ * the default stream after one warm-up; *avg_ms = the CUDA-event time per launch (any output may be NULL). */
+int b200_test_logprobs(const float *logits, int32_t vocab, int32_t chosen_id, int32_t top_n, int32_t reps, double *chosen, int32_t *top_ids,
+                       double *top_logprobs, float *avg_ms);
+
 /* How the single-token forwards (b200_forward_decode / _prefill / b200_decode_sequence) run.  Both replace
  * TornadoVMMasterPlanSingleToken.tornadoVMForwardDecode's N+2 TaskGraph executions
  * (TornadoVMMasterPlanSingleToken.java:68-95) and produce bit-identical results:

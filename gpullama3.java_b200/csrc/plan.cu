@@ -216,6 +216,19 @@ struct b200_plan {
         LogprobRow *out = nullptr, *h_out = nullptr;
         float *smp = nullptr;
     } lp;
+
+    // b200_set_sampling_controls (sampler.cuh, k_sample_ctl): sequence s = slot + 1 (s = 0: the plan's own cache).  The host keeps
+    // each sequence's controls; the device buffers are allocated by the first call that sets controls and hold a row for every
+    // sequence the plan can address, so b200_set_decode_slots never reallocates them.  rows: the modified rows of one call.
+    struct Controls {
+        bool on[SMB_MAX_ROWS + 1] = {};
+        b200_sampling_controls c[SMB_MAX_ROWS + 1] = {}; // bias pointers cleared: the list lives in bias_id / bias_val
+        float min_p_log[SMB_MAX_ROWS + 1] = {};
+        int *cnt = nullptr;        // [sequence][vocab]
+        int *bias_id = nullptr;    // [sequence][B200_MAX_LOGIT_BIAS]
+        float *bias_val = nullptr; // [sequence][B200_MAX_LOGIT_BIAS]
+        float *rows = nullptr;     // [SMB_MAX_ROWS][sampler_padded(vocab)]
+    } ctl;
 };
 
 namespace {
@@ -1300,6 +1313,7 @@ int set_smem_attrs(b200_plan *p) {
     CK(cudaFuncSetAttribute(k_moe_down, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     CK(cudaFuncSetAttribute(k_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
+    CK(cudaFuncSetAttribute(k_sample_ctl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     done = true;
     return B200_OK;
 }
@@ -2288,6 +2302,58 @@ int launch_sample_rows(b200_plan *p, float *logits, int m, const int *row, const
     return B200_OK;
 }
 
+// The checks b200_set_sampling_controls and b200_test_sample_controls share (p may be NULL).
+int check_controls(b200_plan *p, const b200_sampling_controls &c, int vocab) {
+    if (c.top_k < 0 || c.top_k > vocab) return fail(p, B200_ERR_BAD_ARG, "top_k = %d outside [0, %d]", c.top_k, vocab);
+    if (!(c.min_p >= 0.0f && c.min_p <= 1.0f)) return fail(p, B200_ERR_BAD_ARG, "min_p = %g outside [0, 1]", c.min_p);
+    if (!(isfinite(c.repetition_penalty) && c.repetition_penalty > 0.0f))
+        return fail(p, B200_ERR_BAD_ARG, "repetition_penalty = %g: must be finite and > 0", c.repetition_penalty);
+    if (!isfinite(c.frequency_penalty) || !isfinite(c.presence_penalty))
+        return fail(p, B200_ERR_BAD_ARG, "frequency_penalty = %g, presence_penalty = %g: must be finite", c.frequency_penalty, c.presence_penalty);
+    if (c.n_bias < 0 || c.n_bias > B200_MAX_LOGIT_BIAS) return fail(p, B200_ERR_BAD_ARG, "n_bias = %d outside [0, %d]", c.n_bias, B200_MAX_LOGIT_BIAS);
+    if (c.n_bias && (!c.bias_ids || !c.bias_values)) return fail(p, B200_ERR_BAD_ARG, "n_bias = %d with a NULL bias list", c.n_bias);
+    std::vector<char> seen(c.n_bias ? vocab : 0, 0);
+    for (int b = 0; b < c.n_bias; b++) {
+        const int i = c.bias_ids[b];
+        if (i < 0 || i >= vocab) return fail(p, B200_ERR_BAD_ARG, "bias entry %d: id %d out of range", b, i);
+        if (seen[i]++) return fail(p, B200_ERR_BAD_ARG, "bias entry %d: id %d repeats an earlier entry", b, i);
+        if (!isfinite(c.bias_values[b])) return fail(p, B200_ERR_BAD_ARG, "bias entry %d: value %g is not finite", b, c.bias_values[b]);
+    }
+    return B200_OK;
+}
+
+float min_p_log(float min_p) { return (float)log((double)min_p); } // -inf for 0: the min-p mask keeps everything
+
+// One k_sample_ctl row: sequence s's controls and counts, raw row src, modified row dst, the sampler's scratch and outputs.
+SampleCtlRow ctl_row(b200_plan *p, int s, const float *src, float *dst, int *indices, int *out, float temperature, float topp, float uniform01) {
+    const auto &S = p->ctl;
+    const b200_sampling_controls &c = S.c[s];
+    SampleCtlRow r;
+    r.src = src; r.dst = dst; r.row_out = nullptr; r.cnt = S.cnt + (size_t)s * p->cfg.vocab_size;
+    r.bias_id = S.bias_id + (size_t)s * B200_MAX_LOGIT_BIAS; r.bias_val = S.bias_val + (size_t)s * B200_MAX_LOGIT_BIAS; r.n_bias = c.n_bias;
+    r.top_k = c.top_k; r.min_p_log = S.min_p_log[s]; r.rep = c.repetition_penalty; r.freq = c.frequency_penalty; r.pres = c.presence_penalty;
+    r.temperature = temperature; r.topp = topp; r.r01 = uniform01;
+    r.indices = indices; r.out = out;
+    return r;
+}
+
+int launch_sample_ctl(b200_plan *p, int m, const SampleCtlRow *rows) {
+    static_assert(SMB_MAX_ROWS <= SAMPLER_MAX_ROWS, "k_sample_ctl takes every row of a batched step");
+    static_assert(B200_MAX_LOGIT_BIAS == SAMPLER_CTL_MAX_BIAS, "the header's limit is the kernel's");
+    SampleCtlArgs a;
+    a.n = p->cfg.vocab_size;
+    for (int j = 0; j < m; j++) a.row[j] = rows[j];
+    k_sample_ctl<<<m, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
+    CK(cudaGetLastError());
+    return B200_OK;
+}
+
+// Zero the counts of sequences [s0, s1) if the tables exist (on the plan's stream; the caller synchronises).
+int clear_counts(b200_plan *p, int s0, int s1) {
+    if (p->ctl.cnt) CK(cudaMemsetAsync(p->ctl.cnt + (size_t)s0 * p->cfg.vocab_size, 0, (size_t)(s1 - s0) * p->cfg.vocab_size * 4, p->stream));
+    return B200_OK;
+}
+
 // k_token_logprobs on n rows: row k of logits (stride floats apart) emitted *ids[k] and fills result row out_row[k].
 int launch_logprobs(b200_plan *p, const float *logits, long long stride, int n, const int *const *ids, const int *out_row) {
     static_assert(SMB_MAX_ROWS <= LOGPROB_MAX_ROWS, "k_token_logprobs takes every row of a batched step");
@@ -2355,8 +2421,9 @@ int check_row(b200_plan *p, int i, const b200_step_row &r) {
 // One batched step with the classifier over checked rows: against the decode slots, or with own the plan's cache (every row
 // slot 0).  The emitting rows go first (stable), so the final norm, lm_head and argmax run over rows [0, e) and no kernel indexes
 // through a row map; their ids and logits return to the caller's row order, ids -1 where a row does not emit.  Rows with a
-// temperature run the device sampler, all in one launch.  b200_batch_info reports the step.
-int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, int32_t *ids_out, float *logits) {
+// temperature run the device sampler, all in one launch.  With controls, the emitting rows of slots with sampling controls run
+// k_sample_ctl instead, all in one launch of their own.  b200_batch_info reports the step.
+int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, bool controls, int32_t *ids_out, float *logits) {
     const b200_config &c = p->cfg;
     auto &B = p->bt;
     int order[SMB_MAX_ROWS], e = 0;
@@ -2381,14 +2448,23 @@ int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, int32_t
     if (logits) // before the sampler turns sampled rows into probabilities
         for (int k = 0; k < e; k++)
             CK(cudaMemcpyAsync(logits + (size_t)order[k] * c.vocab_size, B.logits + k * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
-    int m = 0, srow[SMB_MAX_ROWS];
+    int m = 0, mc = 0, srow[SMB_MAX_ROWS];
+    bool ctl[SMB_MAX_ROWS];
     float t[SMB_MAX_ROWS], tp[SMB_MAX_ROWS], u[SMB_MAX_ROWS];
+    SampleCtlRow crow[SMB_MAX_ROWS];
     for (int k = 0; k < e; k++) {
         const b200_step_row &r = rows[order[k]];
+        ctl[k] = controls && p->ctl.on[r.slot + 1];
+        if (ctl[k]) {
+            crow[mc++] = ctl_row(p, r.slot + 1, B.logits + k * vpad, p->ctl.rows + k * vpad, B.smp_indices + (size_t)k * c.vocab_size, B.smp_out + 8 * k,
+                                 r.temperature, r.topp, r.uniform01);
+            continue;
+        }
         if (r.temperature == 0.0f) continue; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed
         srow[m] = k; t[m] = r.temperature; tp[m] = r.topp; u[m] = r.uniform01;
         m++;
     }
+    if (mc && (rc = launch_sample_ctl(p, mc, crow))) return rc;
     const bool lp = p->lp.top_n >= 0;
     float *smp = B.logits;
     if (lp && m) { // the sampler overwrites its rows with probabilities: it samples copies (zero pad included) in the same layout
@@ -2398,12 +2474,12 @@ int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, int32_t
     if (m && (rc = launch_sample_rows(p, smp, m, srow, t, tp, u))) return rc;
     if (lp && e) {
         const int *ids[SMB_MAX_ROWS];
-        for (int k = 0; k < e; k++) ids[k] = rows[order[k]].temperature != 0.0f ? B.smp_out + 8 * k : B.ids + k;
+        for (int k = 0; k < e; k++) ids[k] = ctl[k] || rows[order[k]].temperature != 0.0f ? B.smp_out + 8 * k : B.ids + k;
         if ((rc = launch_logprobs(p, B.logits, (long long)vpad, e, ids, order))) return rc;
     }
     if (lp && (rc = copy_logprobs(p, n))) return rc;
     if (e) CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)e * 4, cudaMemcpyDeviceToHost, p->stream));
-    if (m) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)e * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
+    if (m || mc) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)e * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
     CK(cudaStreamSynchronize(p->stream));
     if (lp) {
         for (int k = e; k < n; k++) { // rows that do not emit
@@ -2414,7 +2490,7 @@ int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, int32_t
         p->lp.rows = n;
     }
     for (int i = 0; i < n; i++) ids_out[i] = -1;
-    for (int k = 0; k < e; k++) ids_out[order[k]] = rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
+    for (int k = 0; k < e; k++) ids_out[order[k]] = ctl[k] || rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
     CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
     B.last_launches = g->launches;
     return B200_OK;
@@ -2679,7 +2755,12 @@ int b200_forward_decode_sample(b200_plan *p, int32_t token, int32_t position, fl
     CK(cudaGraphLaunch(decode_graph(p), p->stream));
     const bool greedy = temperature == 0.0f; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed by the forward
     const bool lp = p->lp.top_n >= 0;
-    if (!greedy) {
+    const bool ctl = p->ctl.on[0];
+    if (ctl) { // the controls modify a copy of the row: the raw logits stay for the logprobs
+        const SampleCtlRow r = ctl_row(p, 0, p->logits, p->ctl.rows, p->smp_indices, p->smp_out, temperature, topp, uniform01);
+        if ((rc = launch_sample_ctl(p, 1, &r))) return rc;
+        CK(cudaMemcpyAsync(p->h_ids, p->smp_out, 5 * 4, cudaMemcpyDeviceToHost, p->stream));
+    } else if (!greedy) {
         float *row = p->logits;
         if (lp) { // the sampler overwrites its row with probabilities: it samples a copy (zero pad included)
             row = p->lp.smp;
@@ -2688,7 +2769,7 @@ int b200_forward_decode_sample(b200_plan *p, int32_t token, int32_t position, fl
         if ((rc = launch_sample(p, row, temperature, topp, uniform01, p->smp_out))) return rc;
         CK(cudaMemcpyAsync(p->h_ids, p->smp_out, 5 * 4, cudaMemcpyDeviceToHost, p->stream));
     } else CK(cudaMemcpyAsync(p->h_ids, p->out_ids, 4, cudaMemcpyDeviceToHost, p->stream));
-    if (lp && ((rc = launch_logprobs_one(p, greedy ? p->out_ids : p->smp_out, 0)) || (rc = copy_logprobs(p, 1)))) return rc;
+    if (lp && ((rc = launch_logprobs_one(p, greedy && !ctl ? p->out_ids : p->smp_out, 0)) || (rc = copy_logprobs(p, 1)))) return rc;
     CK(cudaStreamSynchronize(p->stream));
     if ((rc = check_device_error(p))) return rc;
     if (lp) p->lp.rows = 1;
@@ -2913,6 +2994,8 @@ int b200_kv_reset(b200_plan *p) {
     size_t kv_bytes = (size_t)p->cfg.n_layers * p->cfg.context_length * p->kvd_l * 4;
     CK(cudaMemsetAsync(p->key_cache, 0, kv_bytes, p->stream));
     CK(cudaMemsetAsync(p->value_cache, 0, kv_bytes, p->stream));
+    int rc;
+    if ((rc = clear_counts(p, 0, 1))) return rc;
     CK(cudaStreamSynchronize(p->stream));
     return B200_OK;
 }
@@ -2922,7 +3005,7 @@ int b200_set_decode_slots(b200_plan *p, int32_t n_slots) {
     if (n_slots < 0) return fail(p, B200_ERR_BAD_ARG, "n_slots must be >= 0");
     CK(cudaSetDevice(p->device));
     CK(cudaStreamSynchronize(p->stream));
-    if (n_slots == 0) { batch_free(p); return B200_OK; }
+    if (n_slots == 0) { batch_free(p); return clear_counts(p, 1, SMB_MAX_ROWS + 1); } // the memset orders before any later call's work
     if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "batched decode has no Qwen2-MoE layer (MoE plans decode one sequence per step)");
     if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "batched decode runs on single-GPU plans only (this plan is tensor-parallel)");
     if (p->wtype != B200_GGML_Q8_0) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs Q8_0 weights (FP16 plans decode one sequence per step)");
@@ -2932,7 +3015,7 @@ int b200_set_decode_slots(b200_plan *p, int32_t n_slots) {
     batch_free(p);
     const int rc = batch_alloc(p, n_slots);
     if (rc) { batch_free(p); return rc; }
-    return B200_OK;
+    return clear_counts(p, 1, SMB_MAX_ROWS + 1);
 }
 
 int b200_forward_decode_batch(b200_plan *p, int32_t n, const int32_t *slots, const int32_t *tokens, const int32_t *positions, const float *sampling,
@@ -2952,7 +3035,7 @@ int b200_forward_decode_batch(b200_plan *p, int32_t n, const int32_t *slots, con
         if ((rc = check_row(p, i, r[i]))) return rc;
     }
     CK(cudaSetDevice(p->device));
-    return batch_step(p, n, r, false, ids_out, logits);
+    return batch_step(p, n, r, false, sampling != nullptr, ids_out, logits);
 }
 
 int b200_slot_reset(b200_plan *p, int32_t slot) {
@@ -2962,6 +3045,8 @@ int b200_slot_reset(b200_plan *p, int32_t slot) {
     const size_t kv = (size_t)p->cfg.n_layers * p->cfg.context_length * p->kvd;
     CK(cudaMemsetAsync(p->bt.slot_k + (size_t)slot * kv, 0, kv * 4, p->stream));
     CK(cudaMemsetAsync(p->bt.slot_v + (size_t)slot * kv, 0, kv * 4, p->stream));
+    int rc;
+    if ((rc = clear_counts(p, slot + 1, slot + 2))) return rc;
     CK(cudaStreamSynchronize(p->stream));
     return B200_OK;
 }
@@ -3144,7 +3229,7 @@ int b200_forward_decode_multi(b200_plan *p, int32_t slot, int32_t n, const int32
     CK(cudaSetDevice(p->device));
     int rc;
     if ((rc = multi_ready(p))) return rc;
-    return batch_step(p, n, r, slot < 0, ids_out, logits);
+    return batch_step(p, n, r, slot < 0, false, ids_out, logits);
 }
 
 int b200_forward_step(b200_plan *p, int32_t n, const b200_step_row *rows, int32_t *ids_out, float *logits) {
@@ -3163,9 +3248,14 @@ int b200_forward_step(b200_plan *p, int32_t n, const b200_step_row *rows, int32_
         for (int j = 0; j < i; j++)
             if (rows[j].slot == r.slot && rows[j].position == r.position)
                 return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d position %d repeats row %d's", i, r.slot, r.position, j);
+        if (r.emit && p->ctl.on[r.slot + 1])
+            for (int j = 0; j < i; j++)
+                if (rows[j].emit && rows[j].slot == r.slot)
+                    return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d has sampling controls and already emits in row %d (its counts would depend on "
+                                                     "that row's id)", i, r.slot, j);
     }
     CK(cudaSetDevice(p->device));
-    return batch_step(p, n, rows, false, ids_out, logits);
+    return batch_step(p, n, rows, false, true, ids_out, logits);
 }
 
 int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step) {
@@ -3219,6 +3309,76 @@ int b200_read_logprobs(b200_plan *p, int32_t max_rows, int32_t *n_rows, double *
             if (top_logprobs) top_logprobs[(size_t)i * N + k] = r.lp[k];
         }
     }
+    return B200_OK;
+}
+
+// The slot argument of the sampling-control calls: -1 (the plan's own cache) or a decode slot.
+static int check_ctl_slot(b200_plan *p, int slot) {
+    if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "sampling controls run on single-GPU plans only: the sampler needs the whole logits row on one GPU");
+    if (slot < -1 || slot >= p->bt.n_slots) return fail(p, B200_ERR_BAD_ARG, "slot %d out of range (%d slots; -1 is the plan's own cache)", slot, p->bt.n_slots);
+    return B200_OK;
+}
+
+int b200_set_sampling_controls(b200_plan *p, int32_t slot, const b200_sampling_controls *c) {
+    if (!p) return B200_ERR_BAD_ARG;
+    int rc;
+    if ((rc = check_ctl_slot(p, slot))) return rc;
+    auto &S = p->ctl;
+    const int s = slot + 1, V = p->cfg.vocab_size;
+    if (!c) { S.on[s] = false; return B200_OK; }
+    if ((rc = check_controls(p, *c, V))) return rc;
+    CK(cudaSetDevice(p->device));
+    CK(cudaStreamSynchronize(p->stream));
+    // each buffer on its own: a call that failed part-way leaves the rest to the next call, and no sequence has controls until all exist
+    const size_t seqs = SMB_MAX_ROWS + 1;
+    if (!S.cnt) {
+        int *cnt = nullptr;
+        if ((rc = dalloc(p, &cnt, seqs * V * 4))) return rc;
+        CK(cudaMemsetAsync(cnt, 0, seqs * V * 4, p->stream));
+        CK(cudaStreamSynchronize(p->stream));
+        S.cnt = cnt;
+    }
+    if (!S.bias_id && (rc = dalloc(p, &S.bias_id, seqs * B200_MAX_LOGIT_BIAS * 4))) return rc;
+    if (!S.bias_val && (rc = dalloc(p, &S.bias_val, seqs * B200_MAX_LOGIT_BIAS * 4))) return rc;
+    if (!S.rows && (rc = dalloc(p, &S.rows, (size_t)SMB_MAX_ROWS * sampler_padded(V) * 4))) return rc;
+    if (c->n_bias) { // on the plan's stream, which k_sample_ctl runs on, and complete before the caller's lists may change
+        CK(cudaMemcpyAsync(S.bias_id + (size_t)s * B200_MAX_LOGIT_BIAS, c->bias_ids, (size_t)c->n_bias * 4, cudaMemcpyHostToDevice, p->stream));
+        CK(cudaMemcpyAsync(S.bias_val + (size_t)s * B200_MAX_LOGIT_BIAS, c->bias_values, (size_t)c->n_bias * 4, cudaMemcpyHostToDevice, p->stream));
+        CK(cudaStreamSynchronize(p->stream));
+    }
+    S.c[s] = *c;
+    S.c[s].bias_ids = nullptr;
+    S.c[s].bias_values = nullptr;
+    S.min_p_log[s] = min_p_log(c->min_p);
+    S.on[s] = true;
+    return B200_OK;
+}
+
+int b200_set_sample_history(b200_plan *p, int32_t slot, const int32_t *tokens, int32_t n) {
+    if (!p) return B200_ERR_BAD_ARG;
+    int rc;
+    if ((rc = check_ctl_slot(p, slot))) return rc;
+    if (!p->ctl.cnt) return fail(p, B200_ERR_STATE, "no count tables yet: call b200_set_sampling_controls first");
+    if (n < 0 || (n && !tokens)) return fail(p, B200_ERR_BAD_ARG, "n = %d history tokens with %s", n, tokens ? "a list" : "a NULL list");
+    if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "history token %d: %d out of range", i, tokens[i]);
+    const int V = p->cfg.vocab_size;
+    std::vector<int32_t> h(V, 0);
+    for (int i = 0; i < n; i++) h[tokens[i]]++;
+    CK(cudaSetDevice(p->device));
+    CK(cudaMemcpyAsync(p->ctl.cnt + (size_t)(slot + 1) * V, h.data(), (size_t)V * 4, cudaMemcpyHostToDevice, p->stream));
+    CK(cudaStreamSynchronize(p->stream)); // h is freed on return
+    return B200_OK;
+}
+
+int b200_read_sample_counts(b200_plan *p, int32_t slot, int32_t *counts) {
+    if (!p || !counts) return B200_ERR_BAD_ARG;
+    int rc;
+    if ((rc = check_ctl_slot(p, slot))) return rc;
+    if (!p->ctl.cnt) return fail(p, B200_ERR_STATE, "no count tables yet: call b200_set_sampling_controls first");
+    const int V = p->cfg.vocab_size;
+    CK(cudaSetDevice(p->device));
+    CK(cudaMemcpyAsync(counts, p->ctl.cnt + (size_t)(slot + 1) * V, (size_t)V * 4, cudaMemcpyDeviceToHost, p->stream));
+    CK(cudaStreamSynchronize(p->stream));
     return B200_OK;
 }
 
@@ -3532,6 +3692,87 @@ int b200_test_sample(const float *logits, int32_t n, float temperature, float to
             if (probs_out) s.ok(cudaMemcpy(probs_out, dl, (size_t)n * 4, cudaMemcpyDeviceToHost));
         }
     }
+    return s.rc;
+}
+
+int b200_test_sample_controls(const float *logits, int32_t n, int32_t *counts, const b200_sampling_controls *c, float temperature, float topp,
+                              float uniform01, int32_t *token_out, int32_t *info, float *row_out) {
+    if (!logits || !counts || !c || !token_out || n < 1) return B200_ERR_BAD_ARG;
+    if (!(temperature >= 0.0f) || !(uniform01 >= 0.0f && uniform01 < 1.0f)) return B200_ERR_BAD_ARG;
+    if (check_controls(nullptr, *c, n)) return B200_ERR_BAD_ARG;
+    const size_t padded = (size_t)sampler_padded(n) * 4, nb = (size_t)(c->n_bias ? c->n_bias : 1) * 4;
+    float *dl = nullptr, *drow = nullptr, *dout_row = nullptr, *dbv = nullptr;
+    int *dcnt = nullptr, *di = nullptr, *dout = nullptr, *dbi = nullptr;
+    Scratch s;
+    if (s.alloc(&dl, (size_t)n * 4) && s.alloc(&drow, padded) && s.alloc(&dout_row, (size_t)n * 4) && s.alloc(&dcnt, (size_t)n * 4) &&
+        s.alloc(&di, (size_t)n * 4) && s.alloc(&dout, 8 * 4) && s.alloc(&dbi, nb) && s.alloc(&dbv, nb) &&
+        s.ok(cudaMemcpy(dl, logits, (size_t)n * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dcnt, counts, (size_t)n * 4, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemset(dout, 0xFF, 8 * 4)) &&
+        (!c->n_bias || (s.ok(cudaMemcpy(dbi, c->bias_ids, nb, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dbv, c->bias_values, nb, cudaMemcpyHostToDevice)))) &&
+        s.ok(cudaFuncSetAttribute(k_sample_ctl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()))) {
+        SampleCtlArgs a;
+        a.n = n;
+        SampleCtlRow &r = a.row[0];
+        r.src = dl; r.dst = drow; r.row_out = dout_row; r.cnt = dcnt; r.bias_id = dbi; r.bias_val = dbv; r.n_bias = c->n_bias;
+        r.top_k = c->top_k; r.min_p_log = min_p_log(c->min_p); r.rep = c->repetition_penalty; r.freq = c->frequency_penalty; r.pres = c->presence_penalty;
+        r.temperature = temperature; r.topp = topp; r.r01 = uniform01; r.indices = di; r.out = dout;
+        k_sample_ctl<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(a);
+        int32_t h[5];
+        if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize()) && s.ok(cudaMemcpy(h, dout, 5 * 4, cudaMemcpyDeviceToHost)) &&
+            s.ok(cudaMemcpy(counts, dcnt, (size_t)n * 4, cudaMemcpyDeviceToHost))) {
+            *token_out = h[0];
+            if (info) for (int k = 0; k < 4; k++) info[k] = h[1 + k];
+            if (row_out) s.ok(cudaMemcpy(row_out, dout_row, (size_t)n * 4, cudaMemcpyDeviceToHost));
+        }
+    }
+    return s.rc;
+}
+
+int b200_time_sample_controls(const float *logits, int32_t n, const int32_t *counts, const b200_sampling_controls *c, float temperature, float topp,
+                              float uniform01, int32_t reps, float *ctl_ms, float *plain_ms) {
+    if (!logits || !counts || !c || !ctl_ms || !plain_ms || n < 1 || reps < 1) return B200_ERR_BAD_ARG;
+    if (!(temperature > 0.0f) || !(uniform01 >= 0.0f && uniform01 < 1.0f)) return B200_ERR_BAD_ARG;
+    if (check_controls(nullptr, *c, n)) return B200_ERR_BAD_ARG;
+    // k_sample turns its row into probabilities and k_sample_ctl counts its id: every launch, the warm-up's included, gets its own copy
+    const size_t pad = (size_t)sampler_padded(n), copies = (size_t)reps + 1, nb = (size_t)(c->n_bias ? c->n_bias : 1) * 4;
+    float *dl = nullptr, *drow = nullptr, *dbv = nullptr;
+    int *dcnt = nullptr, *di = nullptr, *dout = nullptr, *dbi = nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr, e2 = nullptr;
+    Scratch s;
+    if (!(s.alloc(&dl, copies * pad * 4) && s.alloc(&drow, pad * 4) && s.alloc(&dcnt, copies * n * 4) && s.alloc(&di, (size_t)n * 4) &&
+          s.alloc(&dout, 8 * 4) && s.alloc(&dbi, nb) && s.alloc(&dbv, nb) && s.ok(cudaMemset(dl, 0, copies * pad * 4)) &&
+          s.ok(cudaMemcpy(dl, logits, (size_t)n * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dcnt, counts, (size_t)n * 4, cudaMemcpyHostToDevice)) &&
+          (!c->n_bias || (s.ok(cudaMemcpy(dbi, c->bias_ids, nb, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dbv, c->bias_values, nb, cudaMemcpyHostToDevice)))) &&
+          s.ok(cudaFuncSetAttribute(k_sample_ctl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes())) &&
+          s.ok(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes())) &&
+          s.ok(cudaEventCreate(&e0)) && s.ok(cudaEventCreate(&e1)) && s.ok(cudaEventCreate(&e2))))
+        return s.rc;
+    for (size_t r = 1; r < copies && s.rc == B200_OK; r++)
+        s.ok(cudaMemcpy(dl + r * pad, dl, (size_t)n * 4, cudaMemcpyDeviceToDevice)) && s.ok(cudaMemcpy(dcnt + r * n, dcnt, (size_t)n * 4, cudaMemcpyDeviceToDevice));
+    float ms_ctl = 0.f, ms_plain = 0.f;
+    if (s.rc == B200_OK) {
+        SampleCtlArgs a;
+        a.n = n;
+        SampleCtlRow &w = a.row[0];
+        w.dst = drow; w.row_out = nullptr; w.bias_id = dbi; w.bias_val = dbv; w.n_bias = c->n_bias;
+        w.top_k = c->top_k; w.min_p_log = min_p_log(c->min_p); w.rep = c->repetition_penalty; w.freq = c->frequency_penalty; w.pres = c->presence_penalty;
+        w.temperature = temperature; w.topp = topp; w.r01 = uniform01; w.indices = di; w.out = dout;
+        SamplerArgs b;
+        b.n = n; b.temperature = temperature; b.topp = topp; b.r01 = uniform01; b.indices = di; b.out_id = dout; b.info = dout + 1;
+        auto ctl = [&](size_t r) { w.src = dl + r * pad; w.cnt = dcnt + r * n; k_sample_ctl<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(a); };
+        auto plain = [&](size_t r) { b.logits = dl + r * pad; k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(b); };
+        ctl(reps); // warm-up on the last copy: k_sample_ctl only reads the row, so k_sample's warm-up can follow on it
+        plain(reps);
+        s.ok(cudaEventRecord(e0));
+        for (int r = 0; r < reps; r++) ctl(r);
+        s.ok(cudaEventRecord(e1));
+        for (int r = 0; r < reps; r++) plain(r);
+        s.ok(cudaEventRecord(e2)) && s.ok(cudaGetLastError()) && s.ok(cudaEventSynchronize(e2)) && s.ok(cudaEventElapsedTime(&ms_ctl, e0, e1)) &&
+            s.ok(cudaEventElapsedTime(&ms_plain, e1, e2));
+    }
+    if (s.rc == B200_OK) { *ctl_ms = ms_ctl / reps; *plain_ms = ms_plain / reps; }
+    for (cudaEvent_t e : {e0, e1, e2})
+        if (e) cudaEventDestroy(e);
     return s.rc;
 }
 

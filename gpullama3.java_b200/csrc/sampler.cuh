@@ -182,3 +182,152 @@ __global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample_rows(SamplerRowsA
     s.info = a.out + 8 * r + 1;
     sample_row(s, smp_sm);
 }
+
+// ---- sampling controls (b200_set_sampling_controls): logit bias, repetition / frequency / presence penalties, top-k and min-p on
+// the raw row of a sequence with controls, then the choice and the count of the emitted id, all in one launch with one block per
+// row.  The raw row is only read: the modified row goes to dst (the sampler then turns it into probabilities there), so the logits
+// output and k_token_logprobs still see the model's values.  Every operation is rounded once, in include/b200llama.h's order:
+//   l = fl(l + bias);  where cnt > 0: l = l <= 0 ? fl(l * rep) : fl(l / rep), then l = fl(l - fl(fl(cnt * freq) + pres));
+//   keep l >= v_k (the top_k-th largest value, ties at it all kept) and l >= fl(m + log(min_p)), the rest -inf;
+//   temperature 0: the first strict maximum; otherwise sample_row on the modified row;  cnt[id] += 1.
+// v_k comes from a radix select over order-preserving integer keys: four 8-bit digit passes, each a shared-memory histogram of
+// the keys that share the digits found so far (warp-aggregated with __match_any_sync), no sort and no host work.
+#define SAMPLER_CTL_MAX_BIAS 1024
+
+struct SampleCtlRow {
+    const float *src; // the raw logits row [n]
+    float *dst;       // [sampler_padded(n)]: the modified row with a zero pad, then the sampler's probabilities
+    float *row_out;   // nullable: a copy of the modified row before the choice (the test hook)
+    int *cnt;         // the sequence's counts [n]; the emitted id's is incremented
+    const int *bias_id;
+    const float *bias_val;
+    int n_bias, top_k;
+    float min_p_log, rep, freq, pres; // min_p_log = (float)log((double)min_p): -inf for min_p 0
+    float temperature, topp, r01;
+    int *indices; // [n] the sampler's candidate list
+    int *out;     // [5]: the id, then the sampler's four diagnostics (zeros at temperature 0)
+};
+
+struct SampleCtlArgs {
+    int n;
+    SampleCtlRow row[SAMPLER_MAX_ROWS];
+};
+
+__device__ __forceinline__ unsigned ctl_key(float v) { // ordered like the floats, -0 just below +0
+    const unsigned u = __float_as_uint(v);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float ctl_unkey(unsigned k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
+__global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample_ctl(SampleCtlArgs args) {
+    extern __shared__ __align__(16) unsigned char smp_sm[];
+    __shared__ int hist[256];
+    __shared__ float s_max[32];
+    __shared__ int s_idx[32], s_digit, s_above;
+    const int j = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, n = args.n, npad = sampler_padded(n);
+    const float *src = args.row[j].src;
+    float *dst = args.row[j].dst, *row_out = args.row[j].row_out;
+    int *cnt = args.row[j].cnt;
+    const float rep = args.row[j].rep, freq = args.row[j].freq, pres = args.row[j].pres;
+
+    // ---- 1. logit bias (the ids are distinct)
+    for (int i = tid; i < npad; i += SAMPLER_THREADS) dst[i] = i < n ? src[i] : 0.0f;
+    __syncthreads();
+    for (int b = tid; b < args.row[j].n_bias; b += SAMPLER_THREADS) {
+        const int i = args.row[j].bias_id[b];
+        dst[i] = __fadd_rn(dst[i], args.row[j].bias_val[b]);
+    }
+    __syncthreads();
+    // ---- 2. penalties, and the row maximum m
+    float mx = -INFINITY;
+    for (int i = tid; i < n; i += SAMPLER_THREADS) {
+        float v = dst[i];
+        const int c = cnt[i];
+        if (c > 0) {
+            v = v <= 0.0f ? __fmul_rn(v, rep) : __fdiv_rn(v, rep);
+            v = __fsub_rn(v, __fadd_rn(__fmul_rn(__int2float_rn(c), freq), pres));
+            dst[i] = v;
+        }
+        mx = fmaxf(mx, v);
+    }
+    mx = warp_max_f(mx);
+    if (lane == 0) s_max[warp] = mx;
+    __syncthreads();
+    mx = s_max[0];
+    for (int w = 1; w < SAMPLER_THREADS / 32; w++) mx = fmaxf(mx, s_max[w]);
+    // ---- 3. v_k: the key with fewer than top_k keys above it and at least top_k at or above it
+    float vk = -INFINITY;
+    const int top_k = args.row[j].top_k;
+    if (top_k > 0 && top_k < n) {
+        unsigned prefix = 0, pmask = 0;
+        int krem = top_k;
+        for (int shift = 24; shift >= 0; shift -= 8) {
+            if (tid < 256) hist[tid] = 0;
+            __syncthreads();
+            for (int i = tid; i < npad; i += SAMPLER_THREADS) { // npad is whole blocks: every lane runs every iteration
+                const unsigned key = i < n ? ctl_key(dst[i]) : 0u;
+                const bool in = i < n && (key & pmask) == prefix;
+                const int bin = in ? (int)((key >> shift) & 255u) : 256;
+                const unsigned peers = __match_any_sync(0xffffffffu, bin);
+                if (in && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], __popc(peers));
+            }
+            __syncthreads();
+            if (warp == 0) { // lane l holds digits 255 - 8 l down to 248 - 8 l; the first lane whose running count reaches krem has v_k's
+                int s = 0;
+#pragma unroll
+                for (int d = 0; d < 8; d++) s += hist[255 - 8 * lane - d];
+                int incl = s;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) {
+                    const int u = __shfl_up_sync(0xffffffffu, incl, d);
+                    if (lane >= d) incl += u;
+                }
+                const int hit = __ffs(__ballot_sync(0xffffffffu, incl >= krem)) - 1;
+                if (lane == hit) {
+                    int c = incl - s;
+                    for (int d = 0; d < 8; d++) {
+                        const int b = 255 - 8 * lane - d, h = hist[b];
+                        if (c + h >= krem) { s_digit = b; s_above = c; break; }
+                        c += h;
+                    }
+                }
+            }
+            __syncthreads();
+            prefix |= (unsigned)s_digit << shift;
+            pmask |= 255u << shift;
+            krem -= s_above;
+        }
+        vk = ctl_unkey(prefix);
+    }
+    // ---- 4. masks (the maximum passes both), and the first index of the maximum
+    const float thr = __fadd_rn(mx, args.row[j].min_p_log);
+    int best = 0x7fffffff;
+    for (int i = tid; i < n; i += SAMPLER_THREADS) {
+        float v = dst[i];
+        if (!(v >= vk && v >= thr)) { v = -INFINITY; dst[i] = v; }
+        if (row_out) row_out[i] = v;
+        if (v == mx && i < best) best = i;
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, d));
+    if (lane == 0) s_idx[warp] = best;
+    __syncthreads();
+    int *out = args.row[j].out;
+    // ---- 5. the choice and the count
+    if (args.row[j].temperature == 0.0f) {
+        if (tid == 0) {
+            for (int w = 1; w < SAMPLER_THREADS / 32; w++) best = min(best, s_idx[w]);
+            best = min(best, s_idx[0]);
+            out[0] = best;
+            for (int k = 1; k < 5; k++) out[k] = 0;
+            cnt[best] += 1;
+        }
+        return;
+    }
+    SamplerArgs s;
+    s.logits = dst; s.n = n;
+    s.temperature = args.row[j].temperature; s.topp = args.row[j].topp; s.r01 = args.row[j].r01;
+    s.indices = args.row[j].indices; s.out_id = out; s.info = out + 1;
+    sample_row(s, smp_sm);
+    if (tid == 0) cnt[*out] += 1;
+}

@@ -365,7 +365,8 @@ class ContinuousBatcher:
 
     sampler (optional, per request): a sampler.Sampler; one next_float1() is drawn per generated token, never for a prompt row, as
     generateTokensLlama draws it (InferenceEngine.java:81-154).  The steps are always the exact mixed steps, whatever the plan's
-    prefill mode.
+    prefill mode.  A sampler's controls (sampler.SamplingControls) and history go onto the request's slot at admission, after
+    slot_reset (a request without controls turns its slot's off); the device applies them to the request's emitting rows.
 
     When the plan's log-probabilities are on (plan.set_logprobs), logprobs[rid] receives one entry (chosen, [(id, logprob), ...])
     per generated id, next to results[rid]."""
@@ -421,6 +422,11 @@ class ContinuousBatcher:
                 continue
             r.slot = self._free.pop(0)
             self.plan.slot_reset(r.slot)
+            controls = getattr(r.sampler, "controls", None)
+            if controls is not None or hasattr(self.plan, "set_sampling_controls"):  # a stand-in plan without them: no controls
+                self.plan.set_sampling_controls(r.slot, controls)
+                if controls is not None:
+                    self.plan.set_sample_history(r.slot, r.sampler.history)
             self._running.append(r)
 
     def _advance(self, r: _Request, am) -> bool:

@@ -74,6 +74,8 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle SCORE_TOKENS = fn("b200_score_tokens", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS, ADDRESS, JAVA_INT, JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle SET_LOGPROBS = fn("b200_set_logprobs", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle READ_LOGPROBS = fn("b200_read_logprobs", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
+    private static final MethodHandle SET_SAMPLING_CONTROLS = fn("b200_set_sampling_controls", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS));
+    private static final MethodHandle SET_SAMPLE_HISTORY = fn("b200_set_sample_history", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle SET_PREFILL_MODE = fn("b200_set_prefill_mode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle SET_DECODE_MODE = fn("b200_set_decode_mode", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle DECODE_SAMPLE = fn("b200_forward_decode_sample",
@@ -277,6 +279,44 @@ public final class B200MasterPlan implements AutoCloseable {
                 MemorySegment.copy(lps, java.lang.foreign.ValueLayout.JAVA_DOUBLE, (long) i * n * 8, topLogprobs[i], 0, n);
             }
             return new Logprobs(chosen, topIds, topLogprobs);
+        }
+    }
+
+    /** One sequence's sampling controls (b200_sampling_controls): top-k (0 off; every token tied at the k-th value kept), min-p in
+     *  logit space (0 off), llama.cpp's repetition (1 off) / frequency / presence (0 off) penalties over the sequence's token counts,
+     *  and a logit bias per token id (biasIds / biasValues of equal length, distinct ids, finite values; at most 1024). */
+    public record SamplingControls(int topK, float minP, float repetitionPenalty, float frequencyPenalty, float presencePenalty,
+                                   int[] biasIds, float[] biasValues) {}
+
+    /** b200_set_sampling_controls: controls for one sequence (slot -1: the plan's own cache), applied on the device by
+     *  forwardDecodeSample, forwardDecodeBatch with sampling and forwardStep's emitting rows; null turns them off. */
+    public void setSamplingControls(int slot, SamplingControls c) throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            MemorySegment s = MemorySegment.NULL;
+            if (c != null) {
+                int nb = c.biasIds() == null ? 0 : c.biasIds().length;
+                if (nb != (c.biasValues() == null ? 0 : c.biasValues().length)) throw new IllegalArgumentException("biasIds and biasValues differ in length");
+                s = a.allocate(40, 8); // {int32 top_k; float min_p, rep, freq, pres; int32 n_bias; const int32_t *ids; const float *values}
+                s.set(JAVA_INT, 0, c.topK());
+                s.set(java.lang.foreign.ValueLayout.JAVA_FLOAT, 4, c.minP());
+                s.set(java.lang.foreign.ValueLayout.JAVA_FLOAT, 8, c.repetitionPenalty());
+                s.set(java.lang.foreign.ValueLayout.JAVA_FLOAT, 12, c.frequencyPenalty());
+                s.set(java.lang.foreign.ValueLayout.JAVA_FLOAT, 16, c.presencePenalty());
+                s.set(JAVA_INT, 20, nb);
+                s.set(ADDRESS, 24, nb == 0 ? MemorySegment.NULL : a.allocateFrom(JAVA_INT, c.biasIds()));
+                s.set(ADDRESS, 32, nb == 0 ? MemorySegment.NULL : a.allocateFrom(java.lang.foreign.ValueLayout.JAVA_FLOAT, c.biasValues()));
+            }
+            int rc = (int) SET_SAMPLING_CONTROLS.invokeExact(plan, slot, s);
+            if (rc != 0) check(rc, lastError());
+        }
+    }
+
+    /** b200_set_sample_history: the sequence's token counts become those of tokens (e.g. the prompt). */
+    public void setSampleHistory(int slot, int[] tokens) throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            MemorySegment t = tokens.length == 0 ? MemorySegment.NULL : a.allocateFrom(JAVA_INT, tokens);
+            int rc = (int) SET_SAMPLE_HISTORY.invokeExact(plan, slot, t, tokens.length);
+            if (rc != 0) check(rc, lastError());
         }
     }
 

@@ -10,6 +10,8 @@ import os
 
 import numpy as np
 
+from .sampler import SamplingControls
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libb200llama.so")
 
@@ -54,12 +56,28 @@ class StepRow(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("slot", "token", "position", "emit")] + [(n, C.c_float) for n in ("temperature", "topp", "uniform01")]
 
 
+class SamplingControlsC(C.Structure):
+    """b200_sampling_controls."""
+    _fields_ = [("top_k", C.c_int32)] + [(n, C.c_float) for n in ("min_p", "repetition_penalty", "frequency_penalty", "presence_penalty")] + \
+               [("n_bias", C.c_int32), ("bias_ids", C.c_void_p), ("bias_values", C.c_void_p)]
+
+
+def _controls_c(c: SamplingControls):
+    """(b200_sampling_controls, the arrays its pointers reference: keep them alive across the call)."""
+    bias = c.logit_bias or {}
+    ids = np.ascontiguousarray(list(bias.keys()), dtype=np.int32)
+    vals = np.ascontiguousarray(list(bias.values()), dtype=np.float32)
+    s = SamplingControlsC(int(c.top_k), c.min_p, c.repetition_penalty, c.frequency_penalty, c.presence_penalty, len(ids),
+                          ids.ctypes.data if len(ids) else None, vals.ctypes.data if len(ids) else None)
+    return s, (ids, vals)
+
+
 class Tensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("ggml_type", C.c_int32), ("n_dims", C.c_int32),
                 ("dims", C.c_int64 * 4)]
 
 
-EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_score_tokens", "b200_set_logprobs", "b200_read_logprobs", "b200_test_logprobs", "b200_set_prefill_mode", "b200_prefill_info",
+EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_score_tokens", "b200_set_logprobs", "b200_read_logprobs", "b200_test_logprobs", "b200_set_sampling_controls", "b200_set_sample_history", "b200_read_sample_counts", "b200_test_sample_controls", "b200_time_sample_controls", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant", "b200_test_kq_tiles_to_q8",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
@@ -90,6 +108,12 @@ def lib() -> C.CDLL:
     L.b200_set_logprobs.argtypes = [vp, i32]
     L.b200_read_logprobs.argtypes = [vp, i32, C.POINTER(i32), vp, vp, vp]
     L.b200_test_logprobs.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, C.POINTER(C.c_float)]
+    L.b200_set_sampling_controls.argtypes = [vp, i32, C.POINTER(SamplingControlsC)]
+    L.b200_set_sample_history.argtypes = [vp, i32, vp, i32]
+    L.b200_read_sample_counts.argtypes = [vp, i32, vp]
+    L.b200_test_sample_controls.argtypes = [vp, i32, vp, C.POINTER(SamplingControlsC), C.c_float, C.c_float, C.c_float, C.POINTER(i32), C.POINTER(i32), vp]
+    L.b200_time_sample_controls.argtypes = [vp, i32, vp, C.POINTER(SamplingControlsC), C.c_float, C.c_float, C.c_float, i32, C.POINTER(C.c_float),
+                                            C.POINTER(C.c_float)]
     L.b200_decode_sequence.argtypes = [vp, vp, i32, i32, i32, vp, C.POINTER(C.c_float)]
     L.b200_kv_reset.argtypes = [vp]
     L.b200_profile_norm.argtypes = [vp, C.POINTER(C.c_int64)]
@@ -177,6 +201,40 @@ def test_sample(logits, temperature: float, topp: float, uniform01: float):
     if rc != B200_OK:
         _raise(rc, "b200_test_sample failed")
     return out.value, list(info), probs
+
+
+def test_sample_controls(logits, counts, controls: SamplingControls, temperature: float, topp: float, uniform01: float):
+    """One launch of the controlled sampler (k_sample_ctl, csrc/sampler.cuh) as the plans issue it, on host logits and counts.
+    temperature 0 takes the first maximum of the modified row.  Returns (token id, the sampler's four diagnostics, the modified row
+    float32 before the choice, the counts after the launch)."""
+    lg = np.ascontiguousarray(logits, dtype=np.float32)
+    cnt = np.array(counts, dtype=np.int32, copy=True)
+    if cnt.shape != lg.shape:
+        raise ValueError("one count per logit")
+    row = np.empty(len(lg), dtype=np.float32)
+    out = C.c_int32(-1)
+    info = (C.c_int32 * 4)()
+    cs, keep = _controls_c(controls)
+    rc = lib().b200_test_sample_controls(lg.ctypes.data, len(lg), cnt.ctypes.data, C.byref(cs), temperature, topp, uniform01, C.byref(out), info,
+                                         row.ctypes.data)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_sample_controls failed")
+    return out.value, list(info), row, cnt
+
+
+def time_sample_controls(logits, counts, controls: SamplingControls, temperature: float, topp: float, uniform01: float, reps: int):
+    """b200_time_sample_controls: CUDA-event ms per launch of (k_sample_ctl under controls, k_sample) on the same row, reps each."""
+    lg = np.ascontiguousarray(logits, dtype=np.float32)
+    cnt = np.ascontiguousarray(counts, dtype=np.int32)
+    if cnt.shape != lg.shape:
+        raise ValueError("one count per logit")
+    cs, keep = _controls_c(controls)
+    a, b = C.c_float(0), C.c_float(0)
+    rc = lib().b200_time_sample_controls(lg.ctypes.data, len(lg), cnt.ctypes.data, C.byref(cs), temperature, topp, uniform01, int(reps),
+                                         C.byref(a), C.byref(b))
+    if rc != B200_OK:
+        _raise(rc, "b200_time_sample_controls failed")
+    return a.value, b.value
 
 
 def test_set_memory_budget(n_bytes: int):
@@ -516,6 +574,25 @@ class NativePlan:
         lps = np.empty((r, n_top), dtype=np.float64)
         self._ck(lib().b200_read_logprobs(self._p, r, C.byref(rows), chosen.ctypes.data, ids.ctypes.data, lps.ctypes.data))
         return chosen, ids, lps
+
+    def set_sampling_controls(self, slot: int, controls: SamplingControls | None):
+        """b200_set_sampling_controls: controls for one sequence (slot -1: the plan's own cache); None turns them off."""
+        if controls is None:
+            self._ck(lib().b200_set_sampling_controls(self._p, slot, None))
+            return
+        cs, keep = _controls_c(controls)
+        self._ck(lib().b200_set_sampling_controls(self._p, slot, C.byref(cs)))
+
+    def set_sample_history(self, slot: int, tokens):
+        """b200_set_sample_history: the sequence's counts become those of tokens."""
+        t = np.ascontiguousarray(tokens, dtype=np.int32).reshape(-1)
+        self._ck(lib().b200_set_sample_history(self._p, slot, t.ctypes.data if len(t) else None, len(t)))
+
+    def sample_counts(self, slot: int) -> np.ndarray:
+        """b200_read_sample_counts: the sequence's count per token id, int32 [vocab]."""
+        out = np.empty(self.cfg.vocab_size, dtype=np.int32)
+        self._ck(lib().b200_read_sample_counts(self._p, slot, out.ctypes.data))
+        return out
 
     def decode_sequence(self, tokens, n: int, start_pos: int, feedback: bool = False):
         t = np.ascontiguousarray(tokens, dtype=np.int32)

@@ -92,6 +92,7 @@ class B200MasterPlan:
         self._native = native.NativePlan(cfg, model.tensors, self.prefill_batch_size, device, moe=moe, granite=granite,
                                          devstral=c.arch == ARCH_DEVSTRAL, yarn=yarn)
         self.tp_rank, self.tp_size = tp_rank, tp_size
+        self._controls = {}  # slot -> (the SamplingControls set there, who set them); the device state lives in the plan
         if tp_size > 1:
             # one process per GPU: swap IPC handles of the communication buffers, then wire the peers
             import torch.distributed as dist
@@ -151,6 +152,37 @@ class B200MasterPlan:
     # TensorCoreSupport.java's switch between the MMA and the plain batch-prefill layer families
     PREFILL_EXACT, PREFILL_TENSOR_CORE, PREFILL_TENSOR_CORE_W8A16, PREFILL_TENSOR_CORE_EXACT = 0, 1, 2, 3
 
+    def set_sampling_controls(self, slot: int, controls, owner=None):
+        """Sampling controls (sampler.SamplingControls, or None to turn them off) for one sequence: a decode slot, or -1 for the plan's
+        own cache.  forward_decode_sample (slot -1), forward_decode_batch with sampling and forward_step's emitting rows apply them
+        on the device and count each emitted id; every other call ignores them.  Single-GPU plans only.  owner: who holds the
+        sequence's controls and counts (a sampler.Sampler), until they are replaced or a reset clears the counts."""
+        self._native.set_sampling_controls(slot, controls)
+        self._controls[slot] = (controls, owner) if controls is not None else None
+
+    def sampling_controls(self, slot: int):
+        """The controls set on the sequence through set_sampling_controls, or None."""
+        e = self._controls.get(slot)
+        return e[0] if e else None
+
+    def sampling_controls_owner(self, slot: int):
+        """The owner given with the sequence's controls; None once slot_reset / kv_reset / set_decode_slots cleared its counts."""
+        e = self._controls.get(slot)
+        return e[1] if e else None
+
+    def _counts_cleared(self, slots):
+        for s in slots:
+            if self._controls.get(s):
+                self._controls[s] = (self._controls[s][0], None)
+
+    def set_sample_history(self, slot: int, tokens):
+        """Replace the sequence's token counts with those of tokens (e.g. the prompt); slot_reset / kv_reset clear them."""
+        self._native.set_sample_history(slot, tokens)
+
+    def sample_counts(self, slot: int):
+        """The sequence's count per token id (int32 [vocab])."""
+        return self._native.sample_counts(slot)
+
     def set_prefill_mode(self, mode):
         """"exact" (token-by-token graph, bit-identical KV cache), "tensor_core" (wgmma GEMMs, FP16 tolerance; a Q8_0 plan
         builds f16 twins of its matrices) or "tensor_core_w8a16" (Q8_0 plans: the same GEMMs reading the Q8_0 weights in
@@ -194,6 +226,7 @@ class B200MasterPlan:
     def set_decode_slots(self, n_slots: int):
         """Allocate n_slots zeroed KV-cache slots (0 frees them); UnsupportedOperation beyond what the plan can run."""
         self._native.set_decode_slots(n_slots)
+        self._counts_cleared([s for s in self._controls if s >= 0])
 
     def forward_decode_batch(self, slots, tokens, positions, sampling=None, logits: bool = False):
         """One step for len(slots) rows -> (ids, logits [n, vocab] or None).  sampling: None (greedy) or one
@@ -202,6 +235,7 @@ class B200MasterPlan:
 
     def slot_reset(self, slot: int):
         self._native.slot_reset(slot)
+        self._counts_cleared([slot])
 
     def slot_copy_kv(self, slot: int, n_positions: int):
         """Copy positions [0, n_positions) of the plan's own KV cache (e.g. after forward_batch_prefill) into the slot; zero the rest."""
@@ -243,6 +277,7 @@ class B200MasterPlan:
 
     def kv_reset(self):
         self._native.kv_reset()
+        self._counts_cleared([-1])
 
     def read_buffer(self, *a, **kw):
         return self._native.read_buffer(*a, **kw)

@@ -10,7 +10,11 @@ checks this restatement against the oracle's independent C restatement.
 """
 from __future__ import annotations
 
+import math
+from dataclasses import dataclass
+
 M32 = 0xFFFFFFFF
+MAX_LOGIT_BIAS = 1024  # B200_MAX_LOGIT_BIAS
 
 
 def _mix_murmur32(z: int) -> int:
@@ -57,18 +61,76 @@ class L32X64MixRandom:
         return (self.next_int() >> 8) * (2.0 ** -24)
 
 
-class Sampler:
-    """``Sampler.selectSampler(vocabularySize, temperature, topp, rngSeed)``: greedy when temperature == 0, otherwise
-    temperature + softmax + categorical (topp outside (0,1)) or top-p sampling.  ``sample_token`` runs one decode forward and
-    returns the sampled id; the logits never leave the GPU."""
+@dataclass(frozen=True)
+class SamplingControls:
+    """One sequence's sampling controls (b200_sampling_controls, include/b200llama.h): logit bias, llama.cpp's repetition /
+    frequency / presence penalties over the sequence's token counts, top-k (every token tied at the k-th value is kept) and min-p
+    (logit space, before temperature), applied on the device to the raw row before the sampler.  The defaults change nothing.
+    logit_bias: {token id: added logit}."""
+    top_k: int = 0
+    min_p: float = 0.0
+    repetition_penalty: float = 1.0
+    frequency_penalty: float = 0.0
+    presence_penalty: float = 0.0
+    logit_bias: dict | None = None
 
-    def __init__(self, vocabulary_size: int, temperature: float, topp: float, rng_seed: int):
+    def validate(self, vocabulary_size: int) -> "SamplingControls":
+        """Raises ValueError where b200_set_sampling_controls returns B200_ERR_BAD_ARG; returns self."""
+        if not 0 <= int(self.top_k) <= vocabulary_size:
+            raise ValueError(f"top_k = {self.top_k} outside [0, {vocabulary_size}]")
+        if not 0.0 <= self.min_p <= 1.0:
+            raise ValueError(f"min_p = {self.min_p} outside [0, 1]")
+        if not (math.isfinite(self.repetition_penalty) and self.repetition_penalty > 0.0):
+            raise ValueError(f"repetition_penalty = {self.repetition_penalty}: must be finite and > 0")
+        if not (math.isfinite(self.frequency_penalty) and math.isfinite(self.presence_penalty)):
+            raise ValueError(f"frequency_penalty = {self.frequency_penalty}, presence_penalty = {self.presence_penalty}: must be finite")
+        bias = self.logit_bias or {}
+        if len(bias) > MAX_LOGIT_BIAS:
+            raise ValueError(f"{len(bias)} logit_bias entries: at most {MAX_LOGIT_BIAS}")
+        for i, b in bias.items():
+            if not 0 <= int(i) < vocabulary_size:
+                raise ValueError(f"logit_bias id {i} out of range")
+            if not math.isfinite(b):
+                raise ValueError(f"logit_bias[{i}] = {b} is not finite")
+        return self
+
+
+class Sampler:
+    """``Sampler.selectSampler(vocabulary_size, temperature, topp, rngSeed)``: greedy when temperature == 0, otherwise
+    temperature + softmax + categorical (topp outside (0,1)) or top-p sampling.  ``sample_token`` runs one decode forward and
+    returns the sampled id; the logits never leave the GPU.
+
+    controls (optional SamplingControls) and history (optional token ids, e.g. the prompt, counted by the penalties): with controls,
+    every token goes through forward_decode_sample, temperature 0 included, and the device applies them to the plan's own sequence
+    (slot -1).  The sampler's counts are its history plus every id it has emitted; whenever slot -1 does not hold this sampler's
+    controls and counts (another sampler or the caller set controls there, or kv_reset cleared the counts), sample_token installs
+    them again first.  Without controls, sample_token first turns off any controls left on slot -1, so a plain sampler samples the
+    raw model whatever ran before it.  The RNG draws one next_float1() per token when temperature > 0 and none otherwise, with or
+    without controls."""
+
+    def __init__(self, vocabulary_size: int, temperature: float, topp: float, rng_seed: int, controls: SamplingControls | None = None,
+                 history=None):
         self.vocabulary_size = vocabulary_size
         self.temperature = float(temperature)
         self.topp = float(topp)
         self.rng = None if self.temperature == 0.0 else L32X64MixRandom(rng_seed)
+        self.controls = None if controls is None else controls.validate(vocabulary_size)
+        self.history = [int(t) for t in (history or [])]
+        if any(not 0 <= t < vocabulary_size for t in self.history):
+            raise ValueError("history token out of range")
+        self.counted = list(self.history)  # then each id sample_token emits
 
     def sample_token(self, plan, token: int, position: int) -> int:
+        if self.controls is not None:
+            if plan.sampling_controls_owner(-1) is not self:
+                plan.set_sampling_controls(-1, self.controls, owner=self)
+                plan.set_sample_history(-1, self.counted)
+            u = 0.0 if self.temperature == 0.0 else self.rng.next_float1()
+            tok = plan.forward_decode_sample(token, position, self.temperature, self.topp, u)
+            self.counted.append(tok)
+            return tok
+        if getattr(plan, "sampling_controls", lambda slot: None)(-1) is not None:  # a stand-in plan without controls: none to clear
+            plan.set_sampling_controls(-1, None)
         if self.temperature == 0.0:
             return plan.forward_decode(token, position, logits=False)[1]
         return plan.forward_decode_sample(token, position, self.temperature, self.topp, self.rng.next_float1())

@@ -311,6 +311,62 @@ int b200_read_logprobs(b200_plan *plan, int32_t max_rows, int32_t *n_rows, doubl
 int b200_test_logprobs(const float *logits, int32_t vocab, int32_t chosen_id, int32_t top_n, int32_t reps, double *chosen, int32_t *top_ids,
                        double *top_logprobs, float *avg_ms);
 
+/* ---- sampling controls: logit bias, repetition / frequency / presence penalties, top-k and min-p, per sequence ------------------
+ * A sequence is a decode slot, or slot -1 for the plan's own cache.  For an emitting row of a sequence with controls, l[0, vocab)
+ * the raw logits of the step (Granite's logit scale included) and cnt[i] the sequence's count of token i, the row is modified in
+ * float32, every operation rounded once (csrc/sampler.cuh, k_sample_ctl):
+ *   1. logit bias: l[i] = fl(l[i] + b) for each (i, b) of the bias list;
+ *   2. where cnt[i] > 0 (llama.cpp's penalties): l[i] = l[i] <= 0 ? fl(l[i] * rep) : fl(l[i] / rep), then
+ *      l[i] = fl(l[i] - fl(fl((float)cnt[i] * freq) + pres));
+ *   3. both masks on the row of step 2, applied together, masked entries -inf: top-k keeps l[i] >= v_k, v_k the top_k-th largest
+ *      value counting repeats, and EVERY token tied at v_k (more than top_k can survive; llama.cpp keeps the first in sort order
+ *      instead); min-p keeps l[i] >= fl(m + (float)log((double)min_p)), m the row maximum (llama.cpp's min-p in logit space, before
+ *      temperature).  The maximum passes both, so no row is empty;
+ *   4. temperature 0: the first strict maximum; otherwise b200_forward_decode_sample's sampler, unchanged, on the modified row.  A
+ *      -inf entry has probability 0, so it never passes the top-p cutoff and the categorical walk never stops on it, with the
+ *      reference's two fallbacks as the only exception: when the float cdf ends at or below the uniform number, or no probability
+ *      reaches the top-p cutoff, the sampler returns vocab_size - 1, masked or not (CategoricalSampler.java:28-40,
+ *      ToppSampler.java:71-77);
+ *   5. the emitted id's count is incremented on the device.
+ * Neutral values (top_k 0, min_p 0, rep 1, freq 0, pres 0, no bias) give exactly the ids of a sequence without controls.  The
+ * controls apply on the calls whose ids are generated tokens: b200_forward_decode_sample (slot -1), b200_forward_decode_batch with
+ * non-NULL sampling, and the emitting rows of b200_forward_step.  Every other call (b200_forward_decode, the batch without sampling,
+ * b200_decode_sequence, b200_forward_decode_multi, b200_score_tokens, the prefills) neither reads nor changes them.  The logits
+ * outputs and the log-probabilities stay those of the raw logits.  b200_forward_step refuses (B200_ERR_BAD_ARG, naming the row) two
+ * emitting rows of one slot with controls: the second row's counts would depend on the first row's id.  Rows of sequences without
+ * controls run exactly as before. */
+#define B200_MAX_LOGIT_BIAS 1024
+typedef struct b200_sampling_controls {
+    int32_t top_k;      /* 0 = off; 1..vocab_size */
+    float min_p;        /* [0, 1]; 0 = off */
+    float repetition_penalty, frequency_penalty, presence_penalty; /* rep finite > 0 (1 = off); freq, pres finite (0 = off) */
+    int32_t n_bias;     /* 0..B200_MAX_LOGIT_BIAS entries of distinct ids in [0, vocab_size) and finite values */
+    const int32_t *bias_ids;
+    const float *bias_values;
+} b200_sampling_controls;
+/* Set (c non-NULL, copied) or turn off (c NULL) the controls of one sequence; they stay until replaced, through b200_slot_reset,
+ * b200_kv_reset and b200_set_decode_slots.  The first call that sets controls allocates the count tables, one vocab_size-int32 row
+ * for slot -1 and for each of B200_MAX_DECODE_SLOTS slots, and the modified-row scratch; plans that never set controls hold none of
+ * it.  Slot -1 works on every single-GPU plan (Q8_0, FP16, Qwen2-MoE, resident K-quant).  B200_ERR_BAD_ARG naming the field for a
+ * slot or value out of range; B200_ERR_UNSUPPORTED on tensor-parallel plans (the sampler needs the whole row on one GPU). */
+int b200_set_sampling_controls(b200_plan *plan, int32_t slot, const b200_sampling_controls *c);
+/* Replace one sequence's counts with those of tokens[0, n) (how a caller counts the prompt, which is not counted otherwise).
+ * b200_slot_reset clears its slot's counts, b200_kv_reset slot -1's and b200_set_decode_slots every slot's.  B200_ERR_STATE before
+ * the first b200_set_sampling_controls that set controls; B200_ERR_BAD_ARG for a slot or token out of range. */
+int b200_set_sample_history(b200_plan *plan, int32_t slot, const int32_t *tokens, int32_t n);
+/* One sequence's counts, vocab_size int32 into counts.  B200_ERR_STATE before the count tables exist. */
+int b200_read_sample_counts(b200_plan *plan, int32_t slot, int32_t *counts);
+/* Test hook (no plan): ONE launch of k_sample_ctl as the plans issue it, on n host logits, the host counts (in/out: the emitted id's
+ * is incremented) and controls c (validated as b200_set_sampling_controls does).  temperature 0 is allowed.  Returns the id, the
+ * sampler's four diagnostics (zeros at temperature 0) and, in row_out (nullable, n floats), the modified row before the choice. */
+int b200_test_sample_controls(const float *logits, int32_t n, int32_t *counts, const b200_sampling_controls *c, float temperature, float topp,
+                              float uniform01, int32_t *token_out, int32_t *info, float *row_out);
+/* Measurement hook (no plan): CUDA-event time per launch of k_sample_ctl under controls c and of k_sample (b200_test_sample's kernel)
+ * on the same host row, reps launches of each after one warm-up, each launch on its own copy of the row and counts.  temperature
+ * must be > 0 (k_sample's range). */
+int b200_time_sample_controls(const float *logits, int32_t n, const int32_t *counts, const b200_sampling_controls *c, float temperature, float topp,
+                              float uniform01, int32_t reps, float *ctl_ms, float *plain_ms);
+
 /* How the single-token forwards (b200_forward_decode / _prefill / b200_decode_sequence) run.  Both replace
  * TornadoVMMasterPlanSingleToken.tornadoVMForwardDecode's N+2 TaskGraph executions
  * (TornadoVMMasterPlanSingleToken.java:68-95) and produce bit-identical results:

@@ -153,7 +153,8 @@ __global__ void __launch_bounds__(T, 1) k_test_seqsum2(const float *__restrict__
 
 // Profiling hook: the accumulator in the fused norm's form (chunks at seqsum2_stride, one out-of-line copy as smv_seqsum and
 // pd_seqsum have), called twice in one launch: the first call runs on a cold instruction cache, the second on a warm one.  Each
-// call is timed in clock64 cycles from a barrier before it to a barrier after it.
+// call is timed in clock64 cycles from a barrier before it to a barrier after it; the second call's {items, literal items,
+// fallbacks} follow the two cycle counts.
 template <int T>
 __device__ __noinline__ float profile_seqsum2_call(const float *sq, int n, int S, unsigned char *scratch) {
     return block_seqsum_exact_v2_t<T>(sq, n, seqsum2_carve(scratch, T), (int)threadIdx.x, SeqSum2BlockSync(), S);
@@ -172,7 +173,11 @@ __global__ void __launch_bounds__(T, 1) k_profile_seqsum2(const float *__restric
     const float s1 = profile_seqsum2_call<T>(sm, n, S, scratch);
     __syncthreads();
     const long long t2 = clock64();
-    if (threadIdx.x == 0) { cycles[0] = t1 - t0; cycles[1] = t2 - t1; out[0] = s0; out[1] = s1; }
+    if (threadIdx.x == 0) {
+        const int *info = seqsum2_carve(scratch, T).info;
+        cycles[0] = t1 - t0; cycles[1] = t2 - t1; cycles[2] = info[0]; cycles[3] = info[2]; cycles[4] = info[1];
+        out[0] = s0; out[1] = s1;
+    }
 }
 
 // ------------------------------------------------------------------------------------------

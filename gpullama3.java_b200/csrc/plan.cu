@@ -3659,13 +3659,13 @@ int b200_profile_seqsum2(const float *terms, int32_t n, int32_t threads, int64_t
     Scratch s;
     float *d = nullptr, *o = nullptr;
     long long *cyc = nullptr;
-    if (!s.alloc(&d, (size_t)n * 4) || !s.alloc(&o, 16) || !s.alloc(&cyc, 16)) return B200_ERR_OOM;
+    if (!s.alloc(&d, (size_t)n * 4) || !s.alloc(&o, 16) || !s.alloc(&cyc, 40)) return B200_ERR_OOM;
     cudaError_t e = cudaMemcpy(d, terms, (size_t)n * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = threads == 1024 ? launch_profile_seqsum2<1024>(d, n, cyc, o)
                             : threads == 512 ? launch_profile_seqsum2<512>(d, n, cyc, o) : launch_profile_seqsum2<256>(d, n, cyc, o);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(cycles, cyc, 16, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess) e = cudaMemcpy(cycles, cyc, 40, cudaMemcpyDeviceToHost);
     if (e == cudaSuccess) e = cudaMemcpy(out, o, 8, cudaMemcpyDeviceToHost);
     return e == cudaSuccess ? B200_OK : B200_ERR_CUDA;
 }

@@ -43,27 +43,18 @@ __device__ __forceinline__ SeqPair seq_compose(SeqPair L, SeqPair R) { // apply 
 
 __device__ __forceinline__ int f32_exponent(float f) { return (int)((__float_as_uint(f) >> 23) & 0xffu) - 127; }
 
-// Parity pair of adding t to a running sum in binade e (ulp 2^(e-23)).  Returns false when t >= 2^(e+1)
-// (not a within-binade step).
-__device__ __forceinline__ bool seq_pair(float t, int e, SeqPair &pr) {
-    const unsigned tb = __float_as_uint(t);
-    const int et = (int)(tb >> 23);
-    pr.a0 = pr.a1 = 0u;
-    if (et == 0) return true; // zero / denormal term: far below half an ulp (e >= -90)
-    const unsigned m = (tb & 0x7fffffu) | 0x800000u;
-    int shift = (e + 127) - et; // t / ulp = m * 2^-shift
-    if (shift < 0) return false;
-    if (shift > 25) shift = 25;
-    const unsigned k = m >> shift;
-    const unsigned rem = m & ((1u << shift) - 1u);
-    const unsigned half = shift ? (1u << (shift - 1)) : 0u;
-    if (shift && rem == half) { // exact tie: the result mantissa M + k + r must be even
-        pr.a0 = k + (k & 1u);
-        pr.a1 = k + ((k + 1u) & 1u);
-    } else {
-        pr.a0 = pr.a1 = k + ((shift && rem > half) ? 1u : 0u);
-    }
-    return true;
+// Parity pair of adding t to a running sum in binade e, with scale = 2^(23-e): t / ulp = t * scale is exact, and one fused
+// multiply-add rounds it to an integer with ties to even, which is the step when M is even.  When M is odd only an exact tie
+// (rounding error +-1/2) steps differently: to the other, odd, neighbour.  Returns false when t * scale >= 2^23, i.e.
+// t >= 2^e (no step of a sum that stays inside [2^e, 2^(e+1)) with margin), or t is inf / NaN.  Zero and denormal terms
+// give (0, 0).
+__device__ __forceinline__ bool seq_pair(float t, float scale, SeqPair &pr) {
+    const float kf = __fmul_rn(t, scale), r = __fmaf_rn(t, scale, 0x1p23f);
+    const unsigned a0 = __float_as_uint(r) - 0x4b000000u; // r = 2^23 + the rounded integer
+    const float d = __fsub_rn(__fsub_rn(r, 0x1p23f), kf);  // exact: the rounding error, in [-1/2, 1/2]
+    pr.a0 = a0;
+    pr.a1 = fabsf(d) == 0.5f ? (d > 0.0f ? a0 - 1u : a0 + 1u) : a0;
+    return kf < 0x1p23f;
 }
 
 struct SeqItem {
@@ -76,7 +67,7 @@ struct SeqItem {
 struct SeqSum2Scratch {
     SeqItem *items;   // [T]
     float *wsum;      // [32] warp totals of the per-thread sums
-    int *info;        // [2] {items, fallbacks}, written by thread 0 (valid in that thread on return)
+    int *info;        // [3] {items, fallbacks, literal items}, written by thread 0 (valid in that thread on return)
     float *result;    // [1]
 };
 __host__ __device__ inline size_t seqsum2_scratch_bytes(int T = SEQSUM2_THREADS) { // T = threads that run the accumulator
@@ -87,7 +78,7 @@ __device__ __forceinline__ SeqSum2Scratch seqsum2_carve(unsigned char *p, int T 
     s.items = reinterpret_cast<SeqItem *>(p); p += (size_t)T * sizeof(SeqItem);
     s.wsum = reinterpret_cast<float *>(p); p += 32 * 4;
     s.info = reinterpret_cast<int *>(p);
-    s.result = reinterpret_cast<float *>(p + 8);
+    s.result = reinterpret_cast<float *>(p + 12);
     return s;
 }
 
@@ -171,7 +162,7 @@ __device__ float block_seqsum_exact_v2_t(const float *sq, int n, SeqSum2Scratch 
     {
         const int e = f32_exponent(p_start);
         if (p_start > 0.0f && e > -100 && e < 128 && f32_exponent(p_end) == e) { // e == 128: inf/nan prefix -> literal adds
-            const float b = __uint_as_float((unsigned)(e + 127) << 23);
+            const float b = __uint_as_float((unsigned)(e + 127) << 23), scale = __uint_as_float((unsigned)(150 - e) << 23);
             // margin 2^-9: the sequential sum deviates from any exact prefix by < n * 2^-24 relative (n <= 16384 -> 2^-10)
             if (p_start >= b * (1.0f + 0x1p-9f) && p_end <= 2.0f * b * (1.0f - 0x1p-9f)) {
                 bool ok = true;
@@ -181,14 +172,14 @@ __device__ float block_seqsum_exact_v2_t(const float *sq, int n, SeqSum2Scratch 
                     for (; k < E; k += 4) { // four independent pair evaluations, composed as a tree: the dependent chain is E/4 + 2 composes, not E
                         const float4 v = *reinterpret_cast<const float4 *>(mine + k);
                         SeqPair q0, q1, q2, q3;
-                        const bool o0 = seq_pair(v.x, e, q0), o1 = seq_pair(v.y, e, q1), o2 = seq_pair(v.z, e, q2), o3 = seq_pair(v.w, e, q3);
+                        const bool o0 = seq_pair(v.x, scale, q0), o1 = seq_pair(v.y, scale, q1), o2 = seq_pair(v.z, scale, q2), o3 = seq_pair(v.w, scale, q3);
                         ok = ok && o0 && o1 && o2 && o3; // composing an invalid pair is harmless: the result is discarded
                         pr = seq_compose(pr, seq_compose(seq_compose(q0, q1), seq_compose(q2, q3)));
                     }
 #pragma unroll 1
                 for (; ok && k < E; k++) {
                     SeqPair q;
-                    if (!seq_pair(mine[k], e, q)) { ok = false; break; }
+                    if (!seq_pair(mine[k], scale, q)) { ok = false; break; }
                     pr = seq_compose(pr, q);
                 }
                 if (ok) cls = e;
@@ -228,7 +219,7 @@ __device__ float block_seqsum_exact_v2_t(const float *sq, int n, SeqSum2Scratch 
     // scheduler), barrier 3 hands the sum to the other warps
     if (warp == 0) {
         unsigned sb = 0u; // the bits of the running sum (s >= 0)
-        int items = 0, fallbacks = 0;
+        int items = 0, fallbacks = 0, literals = 0;
         SeqItem nxt = sc.items[0];
 #pragma unroll 1
         for (int i = 0; i < T; items++) {
@@ -243,13 +234,14 @@ __device__ float block_seqsum_exact_v2_t(const float *sq, int n, SeqSum2Scratch 
                 continue;
             }
             fallbacks += it.ebits != ~0u; // a misprediction; otherwise a literal thread: replay the item's threads literally
+            literals += it.ebits == ~0u;
             const int last = (int)((it.idx >> 10) & 1023u);
             float s = __uint_as_float(sb);
 #pragma unroll 1
             for (int j = (int)(it.idx & 1023u); j <= last; j++) s = seq2_literal(s, sq + j * S, E, vec);
             sb = __float_as_uint(s);
         }
-        if (lane == 0) { sc.info[0] = items; sc.info[1] = fallbacks; sc.result[0] = __uint_as_float(sb); }
+        if (lane == 0) { sc.info[0] = items; sc.info[1] = fallbacks; sc.info[2] = literals; sc.result[0] = __uint_as_float(sb); }
     }
     sync(); // barrier 3: the sum
     return sc.result[0];

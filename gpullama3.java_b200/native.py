@@ -180,14 +180,15 @@ def test_seqsum(terms, want_info: bool = False, threads: int = 1024):
 
 
 def profile_seqsum(terms, threads: int = 256):
-    """Cycles of the exact sequential sum in the fused norm's chunk layout, two calls in one launch: (cold, warm, sum, sum)."""
+    """Cycles of the exact sequential sum in the fused norm's chunk layout, two calls in one launch:
+    (cold, warm, sum, sum, items, literal items, fallbacks)."""
     t = np.ascontiguousarray(terms, dtype=np.float32)
-    cyc = (C.c_int64 * 2)()
+    cyc = (C.c_int64 * 5)()
     out = (C.c_float * 2)()
     rc = lib().b200_profile_seqsum2(t.ctypes.data, len(t), threads, cyc, out)
     if rc != B200_OK:
         _raise(rc, "b200_profile_seqsum2 failed")
-    return cyc[0], cyc[1], out[0], out[1]
+    return cyc[0], cyc[1], out[0], out[1], cyc[2], cyc[3], cyc[4]
 
 
 def test_sample(logits, temperature: float, topp: float, uniform01: float):

@@ -550,7 +550,8 @@ int b200_profile_norm(b200_plan *plan, int64_t *cycles);
 int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out, int32_t *info /* nullable */);
 
 /* Diagnostic: SM-clock cycles of the same exact sum in the fused norm's chunk layout, called twice in one launch of `threads`
- * = 1024, 512 or 256 threads: cycles[0] on a cold instruction cache, cycles[1] warm; out[0..1] = the two sums. */
+ * = 1024, 512 or 256 threads: cycles[0] on a cold instruction cache, cycles[1] warm, cycles[2..4] = {items walked, literal
+ * items, fallbacks} of the second call (cycles holds 5 int64); out[0..1] = the two sums. */
 int b200_profile_seqsum2(const float *terms, int32_t n, int32_t threads, int64_t *cycles, float *out);
 
 /* Test hook for the device-side sampler (csrc/sampler.cuh): ONE launch of k_sample as b200_forward_decode_sample issues it (same

@@ -16,23 +16,17 @@ def f32_exponent(f):
 
 
 def seq_pair(t, e):
-    tb = int(np.float32(t).view(np.uint32))
-    et = tb >> 23
-    if et == 0:
-        return True, (0, 0)
-    m = (tb & 0x7FFFFF) | 0x800000
-    shift = (e + 127) - et
-    if shift < 0:
-        return False, (0, 0)
-    if shift > 25:
-        shift = 25
-    k = m >> shift
-    rem = m & ((1 << shift) - 1)
-    half = (1 << (shift - 1)) if shift else 0
-    if shift and rem == half:
-        return True, (k + (k & 1), k + ((k + 1) & 1))
-    v = k + (1 if (shift and rem > half) else 0)
-    return True, (v, v)
+    """csrc/seqsum2.cuh::seq_pair with scale = 2^(23-e): t * scale is exact, so the fused multiply-add's single rounding is
+    the float64 sum rounded to float32."""
+    t = F(t)
+    scale = np.uint32((150 - e) << 23).view(F)
+    with np.errstate(all="ignore"):
+        kf = F(t * scale)
+        r = F(np.float64(t) * np.float64(scale) + 2.0 ** 23)
+        a0 = int(r.view(np.uint32)) - 0x4B000000
+        d = F(F(r - F(2.0 ** 23)) - kf)
+    a1 = (a0 - 1 if d > 0 else a0 + 1) if abs(d) == F(0.5) else a0
+    return bool(kf < F(2.0 ** 23)), (a0, a1)
 
 
 def compose(L, R):
@@ -56,7 +50,9 @@ def warp_segscan(ps, fs):
     return ps, fs
 
 
-def v2(terms, T, S=None):
+def v2(terms, T, S=None, m=2.0 ** -9):
+    """Returns (sum, items walked, fallbacks, literal items).  m overrides the predictor's margin (0 or below: predictions that
+    are wrong on purpose next to binade edges, which the resolver must catch)."""
     n = len(terms)
     E = (n + T - 1) // T
     S = E if S is None else S
@@ -102,8 +98,8 @@ def v2(terms, T, S=None):
         if p_start > 0 and e > -100 and e < 128 and f32_exponent(p_end) == e:
             b = np.uint32((e + 127) << 23).view(F) if 0 <= e + 127 < 256 else F(np.inf)
             with np.errstate(all="ignore"):
-                lo = F(b * F(1.0 + 2.0 ** -9))
-                hi = F(F(2.0) * b) * F(1.0 - 2.0 ** -9)
+                lo = F(b * F(1.0 + m))
+                hi = F(F(2.0) * b) * F(1.0 - m)
             if p_start >= lo and p_end <= F(hi):
                 ok, p = True, (0, 0)
                 for k in range(E):
@@ -135,7 +131,7 @@ def v2(terms, T, S=None):
             items[lo_t + rank] = (cls[lo_t + l], ps[l], first, lo_t + l, nxt)
     # barrier 2; the resolver (warp 0): runs step the float's bits, literal threads and mispredictions replay their terms
     sb = 0
-    n_items = fallbacks = 0
+    n_items = fallbacks = literals = 0
     i = 0
     with np.errstate(all="ignore"):
         while i < T:
@@ -147,13 +143,14 @@ def v2(terms, T, S=None):
                 sb = nb
                 continue
             fallbacks += c != LITERAL
+            literals += c == LITERAL
             s = np.uint32(sb).view(F)
             for j in range(first, last + 1):
                 for k in range(E):
                     s = F(s + sq[j * S + k])
             sb = int(np.float32(s).view(np.uint32))
     s = np.uint32(sb).view(F)
-    return s, n_items, fallbacks
+    return s, n_items, fallbacks, literals
 
 
 def cases():
@@ -218,7 +215,7 @@ if __name__ == "__main__":
         with np.errstate(all="ignore"):
             ref = np.add.accumulate(t, dtype=np.float32)[-1]
         E = (len(t) + T - 1) // T
-        got, items, fb = v2(t, T, stride(E) if strided else E)
+        got, items, fb, _ = v2(t, T, stride(E) if strided else E)
         same = np.float32(got).view(np.uint32) == np.float32(ref).view(np.uint32) or (np.isnan(got) and np.isnan(ref))
         if not same:
             bad += 1

@@ -1,6 +1,7 @@
 """Cycles of the exact RMSNorm sum (csrc/seqsum2.cuh) at 256 / 512 / 1024 threads, cold and warm instruction cache, on the
 squares of a real residual row: the residual stream x of the synthetic Llama-3-8B Q8_0 model of bench.py after a few decode steps
-(dim 4096), and that row extended by its own first 1024 values (dim 5120, the Devstral-Small-2 width).
+(dim 4096), and that row extended by its own first 1024 values (dim 5120, the Devstral-Small-2 width).  Next to the cycles: the
+items the resolver walked, how many of them were literal stretches, and how many runs were mispredicted and replayed.
 Usage: python tools/seqsum_profile.py [steps] [repeats]"""
 import os, subprocess, sys
 import numpy as np
@@ -30,14 +31,15 @@ def seq(t):
     return s
 
 
-print("dim   threads  cold cycles  warm cycles   (median of %d launches)" % reps)
+print("dim   threads  cold cycles  warm cycles  items  literals  fallbacks   (median of %d launches)" % reps)
 for dim, row in rows.items():
     sq = (row * row).astype(np.float32)
     ref = seq(sq)
     for T in (256, 512, 1024):
         runs = [pkg.native.profile_seqsum(sq, threads=T) for _ in range(reps)]
-        for _, _, a, b in runs:
+        for _, _, a, b, *_ in runs:
             assert np.float32(a).view(np.uint32) == ref.view(np.uint32) == np.float32(b).view(np.uint32), (dim, T, a, b, ref)
         cold = int(np.median([r[0] for r in runs]))
         warm = int(np.median([r[1] for r in runs]))
-        print(f"{dim:5d} {T:8d} {cold:12d} {warm:12d}")
+        items, lits, fbs = runs[-1][4:]
+        print(f"{dim:5d} {T:8d} {cold:12d} {warm:12d} {items:6d} {lits:9d} {fbs:10d}")

@@ -1881,7 +1881,6 @@ static int prefill_scratch(b200_plan *p, bool *ok) {
           pg::make_map(&c.mH, c.H16, c.bpad, g.hidden_dim, pg::BM) == 0 && pg::make_map_c(&c.mX, c.X, c.bpad, g.dim) == 0 &&
           pg::make_map_c(&c.mQKV, c.QKV, c.bpad, nqkv) == 0;
     return with_mma_head_size(p, g.head_size, [&](auto HS) {
-        CK(cudaFuncSetAttribute(k_pf_attention_mma<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<HS>()));
         CK(cudaFuncSetAttribute(k_pf_attention_mma_packed<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<HS>()));
         return B200_OK;
     });
@@ -1979,25 +1978,26 @@ int build_f16_twins(b200_plan *p) {
     return B200_OK;
 }
 
-// A packed chunk of b200_prefill_slots: the device tables of prefill.cuh and the f16 scratch the sequences' regions live in
-struct PfPacked {
+// A chunk of the tensor-core prefill (prefill_chunk): the device tables of prefill.cuh, the f16 scratch the sequences' regions live
+// in, and the K / V target: the plan's own cache (own, one sequence in slot 0) or the decode slots
+struct PfChunk {
     const PfTok *tok;
     const PfTile *tiles;
     int n_tiles;
     const PfHist *hist; // sequences with start > 0
     int n_hist, max_start;
     __half *KH, *VH;
+    bool own;
 };
 
-// n tokens already in c.tok (device), positions start_pos .. start_pos + n - 1 of the plan's cache; or, with pk, the packed
-// tokens of several sequences, each written to its own decode slot (start_pos unused)
-int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfPacked *pk = nullptr) {
+// The chunk's n tokens already in c.tok (device).  Times the chunk (p->prefill_ms) and counts its launches (p->launches_prefill).
+int prefill_forward(b200_plan *p, int n, const PfChunk &ck) {
     PrefillCtx &c = p->prefill;
     const b200_config &g = p->cfg;
     cudaStream_t s = p->stream;
     const int nqkv = p->qd + 2 * p->kvd, mt = (n + pg::BM - 1) / pg::BM, kv_mul = g.n_heads / g.n_kv_heads;
-    const size_t ctx_kv = (size_t)g.context_length * p->kvd;
-    // k_pf_attention_mma scales q by this times log2(e): 1/sqrt(head size), or Granite's attentionScale
+    const size_t ctx_kv = (size_t)g.context_length * p->kvd, slot_stride = (size_t)g.n_layers * ctx_kv;
+    // k_pf_attention_mma_packed scales q by this times log2(e): 1/sqrt(head size), or Granite's attentionScale
     const float inv_sqrt_hs = (p->kflags & KF_ATTSCALE) ? p->mup.attention_scale : (float)(1.0 / sqrt((double)g.head_size));
     int nl = 0;
     constexpr int ST = pg::GEMM_STAGES;
@@ -2012,46 +2012,30 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfP
         while (sp > 1 && (nk / sp < 8 || (sp - 1) * ((nk + sp - 1) / sp) >= nk)) sp--;
         return sp < 1 ? 1 : sp;
     };
+    CK(cudaEventRecord(p->ev0, s));
     k_pf_embed<<<n, 256, 0, s>>>(c.tok, p->emb, p->mup.embedding_scale, c.X, g.dim); nl++;
     for (int l = 0; l < g.n_layers; l++) {
         const LayerW &L = p->layers[l];
         const PrefillLayerMaps *m = q8 ? nullptr : &c.maps[l];
         const PrefillQ8Maps *mq = q8 ? &c.maps_q8[l] : nullptr;
-        float *kc = (pk ? p->bt.slot_k : p->key_cache) + (size_t)l * ctx_kv, *vc = (pk ? p->bt.slot_v : p->value_cache) + (size_t)l * ctx_kv;
+        float *kc = (ck.own ? p->key_cache : p->bt.slot_k) + (size_t)l * ctx_kv, *vc = (ck.own ? p->value_cache : p->bt.slot_v) + (size_t)l * ctx_kv;
         k_pf_rmsnorm_f16<<<n, 256, 0, s>>>(c.X, L.attn_norm, g.rms_norm_eps, g.dim, c.A16); nl++;
         if (q8 ? pg::gemm_launch<pg::GEMM_F32, ST, B_Q8>(c.mA, mq->qkv_q, mq->qkv_s, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s, 1, L.tqkv.seg)
                : pg::gemm_launch<pg::GEMM_F32, ST>(c.mA, m->qkv, m->qkv, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s))
             return fail(p, B200_ERR_CUDA, "QKV GEMM launch failed");
         nl++;
-        const int qt = PM_ROWS / kv_mul;
-        int rc;
-        if (pk) {
-            const size_t slot_stride = (size_t)g.n_layers * ctx_kv;
-            if (pk->n_hist) {
-                const size_t n4 = (size_t)pk->max_start * p->kvd / 4;
-                const dim3 hg((unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), pk->n_hist);
-                k_pf_kv_to_f16_packed<<<hg, 256, 0, s>>>(kc, vc, slot_stride, pk->KH, pk->VH, p->kvd, pk->hist);
-                nl++;
-            }
-            const dim3 ag(pk->n_tiles, g.n_kv_heads);
-            rc = with_mma_head_size(p, g.head_size, [&](auto HS) {
-                k_pf_rope_kv_packed<HS><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, slot_stride, pk->KH, pk->VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, pk->tok);
-                k_pf_attention_mma_packed<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), s>>>(c.QKV, nqkv, pk->KH, pk->VH, p->kvd, kv_mul, pk->tiles, inv_sqrt_hs, c.ATT16, p->qd);
-                return B200_OK;
-            });
-        } else {
-            const dim3 ag((n + qt - 1) / qt, g.n_kv_heads);
-            if (start_pos > 0) { // rows written by earlier chunks / decode steps
-                const size_t n4 = (size_t)start_pos * p->kvd / 4;
-                k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, s>>>(kc, vc, c.KH, c.VH, n4);
-                nl++;
-            }
-            rc = with_mma_head_size(p, g.head_size, [&](auto HS) {
-                k_pf_rope_kv<HS><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, c.KH, c.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, start_pos);
-                k_pf_attention_mma<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), s>>>(c.QKV, nqkv, c.KH, c.VH, p->kvd, kv_mul, n, start_pos, inv_sqrt_hs, c.ATT16, p->qd);
-                return B200_OK;
-            });
+        if (ck.n_hist) { // rows written by earlier chunks / decode steps
+            const size_t n4 = (size_t)ck.max_start * p->kvd / 4;
+            const dim3 hg((unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), ck.n_hist);
+            k_pf_kv_to_f16_packed<<<hg, 256, 0, s>>>(kc, vc, slot_stride, ck.KH, ck.VH, p->kvd, ck.hist);
+            nl++;
         }
+        const dim3 ag(ck.n_tiles, g.n_kv_heads);
+        const int rc = with_mma_head_size(p, g.head_size, [&](auto HS) {
+            k_pf_rope_kv_packed<HS><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, slot_stride, ck.KH, ck.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, ck.tok);
+            k_pf_attention_mma_packed<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), s>>>(c.QKV, nqkv, ck.KH, ck.VH, p->kvd, kv_mul, ck.tiles, inv_sqrt_hs, c.ATT16, p->qd);
+            return B200_OK;
+        });
         if (rc) return rc;
         nl += 2;
         const int sp_wo = splits(g.dim / pg::BN, p->qd), sp_w2 = splits(g.dim / pg::BN, g.hidden_dim);
@@ -2071,7 +2055,10 @@ int prefill_forward(b200_plan *p, int n, int start_pos, int *launches, const PfP
         nl++;
     }
     CK(cudaGetLastError());
-    if (launches) *launches = nl;
+    CK(cudaEventRecord(p->ev1, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
+    p->launches_prefill = nl;
     return B200_OK;
 }
 
@@ -2272,6 +2259,84 @@ int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own,
     CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
     p->launches_prefill = nl;
     return B200_OK;
+}
+
+// The chunk path the plan's prefill mode runs: the bit-exact int8 one (prefill_i8.cuh), the f16 / W8A16 one (prefill.cuh), or
+// none (the exact token-by-token and multi-position paths).
+enum ChunkPath { CHUNK_NONE, CHUNK_TC, CHUNK_I8 };
+ChunkPath chunk_path(const b200_plan *p) {
+    const PrefillCtx &c = p->prefill;
+    if (c.mode == B200_PREFILL_TENSOR_CORE_EXACT && p->pi8.ready) return CHUNK_I8;
+    if ((c.mode == B200_PREFILL_TENSOR_CORE && c.ready) || (c.mode == B200_PREFILL_TENSOR_CORE_W8A16 && c.q8_ready)) return CHUNK_TC;
+    return CHUNK_NONE;
+}
+
+// One chunk on the tensor-core path chunk_path selects: the tokens of ns sequences back to back (call order, no padding),
+// sequence i at positions start[i] .. start[i] + len[i] - 1 of slot slots[i] -- of the decode slots, or, own, of the plan's cache
+// (one sequence, slot 0).  Sequences of length 0 take no part.  score: see prefill_forward_i8.
+int prefill_chunk(b200_plan *p, int ns, const int *slots, const int *start, const int *len, const int *tokens, bool own, bool score = false) {
+    const b200_config &g = p->cfg;
+    if (chunk_path(p) == CHUNK_I8) {
+        const size_t slot_stride = (size_t)g.n_layers * g.context_length * p->kvd;
+        std::vector<ChunkTok> tab;
+        for (int i = 0, off = 0; i < ns; off += len[i++])
+            for (int j = 0; j < len[i]; j++) tab.push_back(ChunkTok{tokens[off + j], start[i] + j, (long long)(slots[i] * slot_stride)});
+        return prefill_forward_i8(p, tab, own, score);
+    }
+    // Sequence i's f16 K / V region holds its rows [0, start + len) from scratch row hrow[i].
+    PrefillCtx &c = p->prefill;
+    std::vector<int> n, st, row0, hrow;
+    std::vector<PfTok> tok;
+    std::vector<PfHist> hist;
+    size_t rows = 0;
+    int total = 0, max_start = 0;
+    for (int i = 0; i < ns; total += len[i++]) {
+        if (!len[i]) continue;
+        n.push_back(len[i]); st.push_back(start[i]); row0.push_back(total); hrow.push_back((int)rows);
+        for (int j = 0; j < len[i]; j++) tok.push_back(PfTok{start[i] + j, slots[i], (int)rows + start[i] + j});
+        if (start[i] > 0) {
+            hist.push_back(PfHist{slots[i], start[i], (int)rows});
+            if (start[i] > max_start) max_start = start[i];
+        }
+        rows += (size_t)start[i] + len[i];
+    }
+    const std::vector<PfTile> tiles = pf_tiles((int)n.size(), n.data(), st.data(), row0.data(), hrow.data(), g.n_heads / g.n_kv_heads);
+    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
+    const size_t o_tiles = up16(tok.size() * sizeof(PfTok)), o_hist = o_tiles + up16(tiles.size() * sizeof(PfTile));
+    const size_t bytes = o_hist + hist.size() * sizeof(PfHist) + 16;
+    const bool big = rows > (size_t)g.context_length; // more than one sequence's worth: the grown regions
+    if ((big && rows > c.pk_rows) || bytes > c.ptab_bytes) CK(cudaStreamSynchronize(p->stream)); // the buffers below are reallocated
+    if (big && rows > c.pk_rows) {
+        CK(cudaFree(c.PKH)); CK(cudaFree(c.PVH));
+        c.PKH = c.PVH = nullptr; c.pk_rows = 0;
+        CK(cudaMalloc(&c.PKH, rows * p->kvd * 2));
+        CK(cudaMalloc(&c.PVH, rows * p->kvd * 2));
+        c.pk_rows = rows;
+    }
+    if (bytes > c.ptab_bytes) {
+        CK(cudaFree(c.ptab));
+        c.ptab = nullptr; c.ptab_bytes = 0;
+        CK(cudaMalloc(&c.ptab, bytes));
+        c.ptab_bytes = bytes;
+    }
+    std::vector<unsigned char> h(bytes, 0);
+    memcpy(h.data(), tok.data(), tok.size() * sizeof(PfTok));
+    memcpy(h.data() + o_tiles, tiles.data(), tiles.size() * sizeof(PfTile));
+    if (!hist.empty()) memcpy(h.data() + o_hist, hist.data(), hist.size() * sizeof(PfHist));
+    // pageable sources: both copies are staged before cudaMemcpyAsync returns
+    CK(cudaMemcpyAsync(c.ptab, h.data(), bytes, cudaMemcpyHostToDevice, p->stream));
+    CK(cudaMemcpyAsync(c.tok, tokens, (size_t)total * 4, cudaMemcpyHostToDevice, p->stream));
+    PfChunk ck{};
+    ck.tok = reinterpret_cast<const PfTok *>(c.ptab);
+    ck.tiles = reinterpret_cast<const PfTile *>(c.ptab + o_tiles);
+    ck.n_tiles = (int)tiles.size();
+    ck.hist = reinterpret_cast<const PfHist *>(c.ptab + o_hist);
+    ck.n_hist = (int)hist.size();
+    ck.max_start = max_start;
+    ck.KH = big ? c.PKH : c.KH;
+    ck.VH = big ? c.PVH : c.VH;
+    ck.own = own;
+    return prefill_forward(p, total, ck);
 }
 
 // The single-token graphs the forward calls launch: the persistent kernel's when that mode is selected and captured.
@@ -2798,22 +2863,9 @@ int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, i
     if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache", start_pos, start_pos + n - 1);
     if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
     CK(cudaSetDevice(p->device));
-    if (p->pi8.ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE_EXACT) { // the whole chunk through the int8 GEMMs into the plan's cache
-        std::vector<ChunkTok> tab(n);
-        for (int i = 0; i < n; i++) tab[i] = ChunkTok{tokens[i], start_pos + i, 0};
-        return prefill_forward_i8(p, tab, true);
-    }
-    if ((p->prefill.ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE) ||
-        (p->prefill.q8_ready && p->prefill.mode == B200_PREFILL_TENSOR_CORE_W8A16)) { // tensor-core GEMM path (prefill.cuh)
-        memcpy(p->h_ids, tokens, (size_t)n * 4);
-        CK(cudaMemcpyAsync(p->prefill.tok, p->h_ids, (size_t)n * 4, cudaMemcpyHostToDevice, p->stream));
-        CK(cudaEventRecord(p->ev0, p->stream));
-        int rc2 = prefill_forward(p, n, start_pos, &p->launches_prefill);
-        if (rc2) return rc2;
-        CK(cudaEventRecord(p->ev1, p->stream));
-        CK(cudaStreamSynchronize(p->stream));
-        CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
-        return B200_OK;
+    if (chunk_path(p) != CHUNK_NONE) { // the whole chunk on the tensor cores into the plan's cache
+        const int slot = 0;
+        return prefill_chunk(p, 1, &slot, &start_pos, &n, tokens, true);
     }
     // Exact path (bit-identical KV cache to the CPU batchForwardJavaPrefill, InferenceCoreBatchPrefillDecode.java:62-168).  Plans
     // that run multi-position steps take positions start .. start + n - 2 in steps of batch_max_rows rows into the plan's cache;
@@ -2843,7 +2895,8 @@ int b200_score_tokens(b200_plan *p, const int32_t *tokens, const int32_t *target
     if (p->cfg.tp_size > 1)
         return fail(p, B200_ERR_UNSUPPORTED, "full logits are not gathered under tensor parallelism: scoring runs on single-GPU plans");
     const int mode = p->prefill.mode;
-    if (mode == B200_PREFILL_TENSOR_CORE || mode == B200_PREFILL_TENSOR_CORE_W8A16)
+    const ChunkPath path = chunk_path(p);
+    if (path == CHUNK_TC)
         return fail(p, B200_ERR_UNSUPPORTED, "the %s prefill keeps f16 activations, so its logits are not the reference's: score in the exact or "
                     "tensor_core_exact prefill mode", mode == B200_PREFILL_TENSOR_CORE ? "tensor_core" : "tensor_core_w8a16");
     if (p->prefill_batch > 1 && n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "chunk of %d tokens exceeds prefill_batch_size %d", n, p->prefill_batch);
@@ -2852,16 +2905,15 @@ int b200_score_tokens(b200_plan *p, const int32_t *tokens, const int32_t *target
     for (int i = 0; i < n; i++)
         if (targets[i] != -1 && (targets[i] < 0 || targets[i] >= p->cfg.vocab_size))
             return fail(p, B200_ERR_BAD_ARG, "target %d of row %d out of range (-1 or a token id)", targets[i], i);
-    const bool tc = p->pi8.ready && mode == B200_PREFILL_TENSOR_CORE_EXACT;
+    const bool tc = path == CHUNK_I8;
     if (!tc && n > p->seq_cap) return fail(p, B200_ERR_BAD_ARG, "chunk too long");
     CK(cudaSetDevice(p->device));
     int rc;
     if ((rc = score_ready(p)) || (tc && (rc = score_init_i8(p)))) return rc;
     CK(cudaMemcpyAsync(p->sc.tgt, targets, (size_t)n * 4, cudaMemcpyHostToDevice, p->stream));
     if (tc) {
-        std::vector<ChunkTok> tab(n);
-        for (int i = 0; i < n; i++) tab[i] = ChunkTok{tokens[i], start_pos + i, 0};
-        rc = prefill_forward_i8(p, tab, true, true);
+        const int slot = 0;
+        rc = prefill_chunk(p, 1, &slot, &start_pos, &n, tokens, true, true);
     } else rc = multi_why(p) ? score_single(p, tokens, n, start_pos) : score_multi(p, tokens, n, start_pos);
     if (rc) return rc;
     std::vector<ScoreOut> out(n);
@@ -2982,7 +3034,7 @@ int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
 
 int b200_prefill_info(b200_plan *p, int32_t *mode, int32_t *launches, float *device_ms) {
     if (!p) return B200_ERR_BAD_ARG;
-    if (mode) *mode = p->prefill.ready || p->prefill.q8_ready || p->pi8.ready ? p->prefill.mode : B200_PREFILL_EXACT;
+    if (mode) *mode = chunk_path(p) == CHUNK_NONE ? B200_PREFILL_EXACT : p->prefill.mode;
     if (launches) *launches = p->launches_prefill;
     if (device_ms) *device_ms = p->prefill_ms;
     return B200_OK;
@@ -3091,71 +3143,6 @@ int prefill_slots_exact(b200_plan *p, int ns, const int *slots, const int *start
     p->launches_prefill = launches;
     return B200_OK;
 }
-
-// Tensor-core b200_prefill_slots: one chunk of the concatenated tokens (call order, no padding).  Sequence i's f16 K / V region
-// holds its rows [0, start + len) from scratch row hrow[i]; sequences of length 0 take no part.
-int prefill_slots_tc(b200_plan *p, int ns, const int *slots, const int *start, const int *len, const int *off, const int *tokens, int total) {
-    PrefillCtx &c = p->prefill;
-    const b200_config &g = p->cfg;
-    std::vector<int> n, st, row0, hrow;
-    std::vector<PfTok> tok(total);
-    std::vector<PfHist> hist;
-    size_t rows = 0;
-    int max_start = 0;
-    for (int i = 0; i < ns; i++) {
-        if (!len[i]) continue;
-        n.push_back(len[i]); st.push_back(start[i]); row0.push_back(off[i]); hrow.push_back((int)rows);
-        for (int j = 0; j < len[i]; j++) tok[off[i] + j] = PfTok{start[i] + j, slots[i], (int)rows + start[i] + j};
-        if (start[i] > 0) {
-            hist.push_back(PfHist{slots[i], start[i], (int)rows});
-            if (start[i] > max_start) max_start = start[i];
-        }
-        rows += (size_t)start[i] + len[i];
-    }
-    const std::vector<PfTile> tiles = pf_tiles((int)n.size(), n.data(), st.data(), row0.data(), hrow.data(), g.n_heads / g.n_kv_heads);
-    CK(cudaStreamSynchronize(p->stream)); // the buffers below may be reallocated
-    PfPacked pk{};
-    pk.KH = c.KH; pk.VH = c.VH;
-    if (rows > (size_t)g.context_length) { // more than one sequence's worth: the grown regions
-        if (rows > c.pk_rows) {
-            CK(cudaFree(c.PKH)); CK(cudaFree(c.PVH));
-            c.PKH = c.PVH = nullptr; c.pk_rows = 0;
-            CK(cudaMalloc(&c.PKH, rows * p->kvd * 2));
-            CK(cudaMalloc(&c.PVH, rows * p->kvd * 2));
-            c.pk_rows = rows;
-        }
-        pk.KH = c.PKH; pk.VH = c.PVH;
-    }
-    auto up16 = [](size_t x) { return (x + 15) & ~(size_t)15; };
-    const size_t o_tiles = up16(tok.size() * sizeof(PfTok)), o_hist = o_tiles + up16(tiles.size() * sizeof(PfTile));
-    const size_t bytes = o_hist + hist.size() * sizeof(PfHist) + 16;
-    if (bytes > c.ptab_bytes) {
-        CK(cudaFree(c.ptab));
-        c.ptab = nullptr; c.ptab_bytes = 0;
-        CK(cudaMalloc(&c.ptab, bytes));
-        c.ptab_bytes = bytes;
-    }
-    std::vector<unsigned char> h(bytes, 0);
-    memcpy(h.data(), tok.data(), tok.size() * sizeof(PfTok));
-    memcpy(h.data() + o_tiles, tiles.data(), tiles.size() * sizeof(PfTile));
-    if (!hist.empty()) memcpy(h.data() + o_hist, hist.data(), hist.size() * sizeof(PfHist));
-    CK(cudaMemcpyAsync(c.ptab, h.data(), bytes, cudaMemcpyHostToDevice, p->stream));
-    pk.tok = reinterpret_cast<const PfTok *>(c.ptab);
-    pk.tiles = reinterpret_cast<const PfTile *>(c.ptab + o_tiles);
-    pk.n_tiles = (int)tiles.size();
-    pk.hist = reinterpret_cast<const PfHist *>(c.ptab + o_hist);
-    pk.n_hist = (int)hist.size();
-    pk.max_start = max_start;
-    // pageable sources: both copies are staged before cudaMemcpyAsync returns (the pinned p->h_ids holds one sequence's worth)
-    CK(cudaMemcpyAsync(c.tok, tokens, (size_t)total * 4, cudaMemcpyHostToDevice, p->stream));
-    CK(cudaEventRecord(p->ev0, p->stream));
-    int rc = prefill_forward(p, total, 0, &p->launches_prefill, &pk);
-    if (rc) return rc;
-    CK(cudaEventRecord(p->ev1, p->stream));
-    CK(cudaStreamSynchronize(p->stream));
-    CK(cudaEventElapsedTime(&p->prefill_ms, p->ev0, p->ev1));
-    return B200_OK;
-}
 } // namespace
 
 int b200_prefill_slots(b200_plan *p, int32_t n_seqs, const int32_t *slots, const int32_t *start_positions, const int32_t *lengths, const int32_t *tokens) {
@@ -3182,9 +3169,7 @@ int b200_prefill_slots(b200_plan *p, int32_t n_seqs, const int32_t *slots, const
     for (int i = 0; i < n_seqs; i++)
         if (const int j = bad_token(p, tokens + off[i], lengths[i]); j >= 0)
             return fail(p, B200_ERR_BAD_ARG, "sequence %d: token %d (index %d) out of range", i, tokens[off[i] + j], j);
-    const PrefillCtx &pc = p->prefill;
-    const bool i8 = p->pi8.ready && pc.mode == B200_PREFILL_TENSOR_CORE_EXACT;
-    const bool tc = (pc.ready && pc.mode == B200_PREFILL_TENSOR_CORE) || (pc.q8_ready && pc.mode == B200_PREFILL_TENSOR_CORE_W8A16) || i8;
+    const bool tc = chunk_path(p) != CHUNK_NONE;
     if (tc && total > p->prefill_batch) {
         int i = 0;
         while (off[i] + lengths[i] <= p->prefill_batch) i++;
@@ -3193,14 +3178,7 @@ int b200_prefill_slots(b200_plan *p, int32_t n_seqs, const int32_t *slots, const
     }
     if (!total) return B200_OK;
     CK(cudaSetDevice(p->device));
-    if (i8) { // one chunk of the call's tokens, sequence after sequence, each row writing its own slot
-        const size_t slot_stride = (size_t)c.n_layers * c.context_length * p->kvd;
-        std::vector<ChunkTok> tab;
-        for (int i = 0; i < n_seqs; i++)
-            for (int j = 0; j < lengths[i]; j++) tab.push_back(ChunkTok{tokens[off[i] + j], start_positions[i] + j, (long long)(slots[i] * slot_stride)});
-        return prefill_forward_i8(p, tab, false);
-    }
-    return tc ? prefill_slots_tc(p, n_seqs, slots, start_positions, lengths, off.data(), tokens, (int)total)
+    return tc ? prefill_chunk(p, n_seqs, slots, start_positions, lengths, tokens, false)
               : prefill_slots_exact(p, n_seqs, slots, start_positions, lengths, off.data(), tokens);
 }
 
@@ -3975,43 +3953,11 @@ int b200_test_gemm_i8(int32_t mode, int32_t m, int32_t n, int32_t k, const int8_
     return s.rc;
 }
 
-int b200_test_pf_attention(const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads, int32_t n_kv_heads,
-                           int32_t head_size, int32_t out_rows, uint16_t *out) {
-    if (!q || !k || !v || !out || n < 1 || start_pos < 0 || out_rows < n || n_kv_heads < 1 || n_heads % n_kv_heads) return B200_ERR_BAD_ARG;
-    const int kv_mul = n_heads / n_kv_heads, hs = head_size;
-    if ((hs != 64 && hs != 128) || kv_mul > 64) return B200_ERR_BAD_ARG; // what prefill_init accepts
-    const int qd = n_heads * hs, kvd = n_kv_heads * hs, ldq = qd + 2 * kvd, nkeys = start_pos + n;
-    const size_t kv_elems = (size_t)nkeys * kvd;
-    float *dqkv = nullptr, *dk = nullptr, *dv = nullptr;
-    __half *dkh = nullptr, *dvh = nullptr, *dout = nullptr;
-    Scratch s;
-    // q sits in the q columns of a QKV row as after k_pf_rope_kv; the k / v columns hold NaN, which the kernels must never read
-    if (s.alloc(&dqkv, (size_t)n * ldq * 4) && s.alloc(&dk, kv_elems * 4) && s.alloc(&dv, kv_elems * 4) &&
-        s.alloc(&dkh, kv_elems * 2) && s.alloc(&dvh, kv_elems * 2) && s.alloc(&dout, (size_t)out_rows * qd * 2) &&
-        s.ok(cudaMemset(dqkv, 0xFF, (size_t)n * ldq * 4)) && s.ok(cudaMemcpy2D(dqkv, (size_t)ldq * 4, q, (size_t)qd * 4, (size_t)qd * 4, n, cudaMemcpyHostToDevice)) &&
-        s.ok(cudaMemcpy(dk, k, kv_elems * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dv, v, kv_elems * 4, cudaMemcpyHostToDevice)) &&
-        s.ok(cudaMemcpy(dout, out, (size_t)out_rows * qd * 2, cudaMemcpyHostToDevice))) {
-        const float inv_sqrt_hs = (float)(1.0 / sqrt((double)hs));
-        const int qt = PM_ROWS / kv_mul;
-        const dim3 ag((n + qt - 1) / qt, n_kv_heads);
-        // f16 K / V copies as prefill_forward makes them (k_pf_kv_to_f16 and k_pf_rope_kv round the same way)
-        const size_t n4 = kv_elems / 4;
-        k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, 0>>>(dk, dv, dkh, dvh, n4);
-        with_mma_head_size(nullptr, hs, [&](auto HS) {
-            if (s.ok(cudaFuncSetAttribute(k_pf_attention_mma<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<HS>())))
-                k_pf_attention_mma<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, n, start_pos, inv_sqrt_hs, dout, qd);
-            return B200_OK;
-        });
-        if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize())) s.ok(cudaMemcpy(out, dout, (size_t)out_rows * qd * 2, cudaMemcpyDeviceToHost));
-    }
-    return s.rc;
-}
-
 int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const int32_t *start_positions, const float *q, const float *k, const float *v,
-                                  int32_t n_heads, int32_t n_kv_heads, int32_t head_size, uint16_t *out) {
+                                  int32_t n_heads, int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out) {
     if (!lengths || !start_positions || !q || !k || !v || !out || n_seqs < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return B200_ERR_BAD_ARG;
     const int kv_mul = n_heads / n_kv_heads, hs = head_size;
-    if ((hs != 64 && hs != 128) || kv_mul > 64) return B200_ERR_BAD_ARG;
+    if ((hs != 64 && hs != 128) || kv_mul > 64) return B200_ERR_BAD_ARG; // what prefill_init accepts
     const int qd = n_heads * hs, kvd = n_kv_heads * hs, ldq = qd + 2 * kvd;
     std::vector<int> row0(n_seqs), hrow(n_seqs);
     int n = 0, rows = 0;
@@ -4020,31 +3966,35 @@ int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const 
         row0[i] = n; hrow[i] = rows;
         n += lengths[i]; rows += start_positions[i] + lengths[i];
     }
+    if (out_rows < n) return B200_ERR_BAD_ARG;
     const std::vector<PfTile> tiles = pf_tiles(n_seqs, lengths, start_positions, row0.data(), hrow.data(), kv_mul);
+    const PfHist hist{0, rows, 0}; // every K / V row, in place
     const size_t kv_elems = (size_t)rows * kvd;
     float *dqkv = nullptr, *dk = nullptr, *dv = nullptr;
     __half *dkh = nullptr, *dvh = nullptr, *dout = nullptr;
     PfTile *dt = nullptr;
+    PfHist *dh = nullptr;
     Scratch s;
-    // q rows of every sequence back to back in the q columns of QKV rows, K / V rows [0, start + n) of each sequence back to back: the
-    // layout b200_prefill_slots gives the packed kernel
+    // q rows of every sequence back to back in the q columns of QKV rows (as after k_pf_rope_kv_packed; the k / v columns hold NaN,
+    // which the kernel must never read), K / V rows [0, start + n) of each sequence back to back: the layout a chunk gives the kernel
     if (s.alloc(&dqkv, (size_t)n * ldq * 4) && s.alloc(&dk, kv_elems * 4) && s.alloc(&dv, kv_elems * 4) &&
-        s.alloc(&dkh, kv_elems * 2) && s.alloc(&dvh, kv_elems * 2) && s.alloc(&dout, (size_t)n * qd * 2) &&
-        s.alloc(&dt, tiles.size() * sizeof(PfTile)) &&
+        s.alloc(&dkh, kv_elems * 2) && s.alloc(&dvh, kv_elems * 2) && s.alloc(&dout, (size_t)out_rows * qd * 2) &&
+        s.alloc(&dt, tiles.size() * sizeof(PfTile)) && s.alloc(&dh, sizeof(PfHist)) &&
         s.ok(cudaMemset(dqkv, 0xFF, (size_t)n * ldq * 4)) && s.ok(cudaMemcpy2D(dqkv, (size_t)ldq * 4, q, (size_t)qd * 4, (size_t)qd * 4, n, cudaMemcpyHostToDevice)) &&
         s.ok(cudaMemcpy(dk, k, kv_elems * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dv, v, kv_elems * 4, cudaMemcpyHostToDevice)) &&
-        s.ok(cudaMemcpy(dout, out, (size_t)n * qd * 2, cudaMemcpyHostToDevice)) &&
-        s.ok(cudaMemcpy(dt, tiles.data(), tiles.size() * sizeof(PfTile), cudaMemcpyHostToDevice))) {
+        s.ok(cudaMemcpy(dout, out, (size_t)out_rows * qd * 2, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(dt, tiles.data(), tiles.size() * sizeof(PfTile), cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dh, &hist, sizeof(PfHist), cudaMemcpyHostToDevice))) {
         const float inv_sqrt_hs = (float)(1.0 / sqrt((double)hs));
         const dim3 ag((unsigned)tiles.size(), n_kv_heads);
+        // f16 K / V copies as a chunk makes them (k_pf_kv_to_f16_packed and k_pf_rope_kv_packed round the same way)
         const size_t n4 = kv_elems / 4;
-        k_pf_kv_to_f16<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, 0>>>(dk, dv, dkh, dvh, n4);
+        k_pf_kv_to_f16_packed<<<(unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), 256, 0, 0>>>(dk, dv, 0, dkh, dvh, kvd, dh);
         with_mma_head_size(nullptr, hs, [&](auto HS) {
             if (s.ok(cudaFuncSetAttribute(k_pf_attention_mma_packed<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pm_smem_bytes<HS>())))
                 k_pf_attention_mma_packed<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), 0>>>(dqkv, ldq, dkh, dvh, kvd, kv_mul, dt, inv_sqrt_hs, dout, qd);
             return B200_OK;
         });
-        if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize())) s.ok(cudaMemcpy(out, dout, (size_t)n * qd * 2, cudaMemcpyDeviceToHost));
+        if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize())) s.ok(cudaMemcpy(out, dout, (size_t)out_rows * qd * 2, cudaMemcpyDeviceToHost));
     }
     return s.rc;
 }

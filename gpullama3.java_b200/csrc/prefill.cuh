@@ -1,13 +1,16 @@
 // prefill.cuh -- batched prefill (--batch-prefill-size N) on the tensor cores.
 //
-// One chunk of n <= B prompt tokens at positions start .. start+n-1 goes through every layer as GEMMs
-// (prefill_gemm.cuh: TMA + wgmma, FP32 accumulation in registers) instead of n matvec passes:
+// One chunk of n <= B prompt tokens goes through every layer as GEMMs (prefill_gemm.cuh: TMA + wgmma, FP32 accumulation in
+// registers) instead of n matvec passes.  A chunk packs one or more sequences back to back, each at its own positions
+// start .. start+len-1 and with its own KV target: the plan's cache (one sequence, b200_forward_batch_prefill) or a decode slot
+// (b200_prefill_slots).  Per-token, per-tile and history tables (PfTok, PfTile, PfHist) tell the kernels where each row goes.
 //
 //   X[n][dim] <- embedding rows                                      k_pf_embed
 //   per layer:  A16 <- f16(rmsnorm(X) * w)                            k_pf_rmsnorm_f16   (batchedRmsReduce + batchedRmsApplyFP16)
 //               QKV <- A16 * [Wq;Wk;Wv]^T                             GEMM_F32           (gemmMMAQKV)
-//               q,k <- (Qwen3: per-head RMSNorm) RoPE; k,v -> cache   k_pf_rope_kv       (batchedRopeWithKVCachePacked)
-//               ATT16 <- causal softmax(q k^T / sqrt(hs)) v           k_pf_attention_mma (batchedFlashAttentionFP16Out)
+//               f16 copies of the K/V rows before each sequence        k_pf_kv_to_f16_packed (only when some start > 0)
+//               q,k <- (Qwen3: per-head RMSNorm) RoPE; k,v -> cache   k_pf_rope_kv_packed       (batchedRopeWithKVCachePacked)
+//               ATT16 <- causal softmax(q k^T / sqrt(hs)) v           k_pf_attention_mma_packed (batchedFlashAttentionFP16Out)
 //               X += ATT16 * Wo^T                                     GEMM_RESID         (gemmMMA + residual)
 //               A16 <- f16(rmsnorm(X) * w)
 //               H16 <- f16(silu(A16 W1^T) * (A16 W3^T))               GEMM_GATEUP        (gemmMMAGateUp + batchedFFNSwiGLUFP16Packed)
@@ -42,9 +45,9 @@ struct PrefillCtx {
     float *X = nullptr, *QKV = nullptr;
     __half *A16 = nullptr, *ATT16 = nullptr, *H16 = nullptr;
     int *tok = nullptr;
-    __half *KH = nullptr, *VH = nullptr; // f16 K / V rows [0, start+n) of the layer in flight
-    // b200_prefill_slots: f16 K / V regions of every packed sequence when they need more than KH / VH's context_length rows
-    // (grown on demand, owned here), and the per-token / per-tile / history tables of the call
+    __half *KH = nullptr, *VH = nullptr; // f16 K / V regions of the chunk's sequences, rows [0, start+len) each, of the layer in flight
+    // grown on demand, owned here: the f16 K / V regions when a packed chunk needs more than KH / VH's context_length rows, and the
+    // chunk's per-token / per-tile / history tables
     __half *PKH = nullptr, *PVH = nullptr;
     size_t pk_rows = 0;
     unsigned char *ptab = nullptr;
@@ -102,19 +105,19 @@ __global__ void __launch_bounds__(256) k_pf_rmsnorm_f16(const float *__restrict_
 // Qwen3 normalises the head, then rotates NeoX pairs (:594-619); Qwen2 adds the q / k / v biases first (:456-459),
 // exactly (one rounded add), then rotates NeoX pairs.  q is rotated in place; k and v go to the FP32 KV cache
 // (what decode reads) and, as f16, to the per-layer scratch the attention kernel streams.
-// PACKED (b200_prefill_slots): token b's position, slot and scratch row come from tok[b] (see PfTok below); kc / vc are this layer's
-// rows of slot 0, slot s slot_stride floats further.
+// Token b's position, slot and scratch row come from tok[b]; kc / vc are this layer's rows of slot 0, slot s slot_stride floats
+// further (the plan's own cache is slot 0).
 struct PfTok {
     int pos, slot, hrow;
 };
 
-template <int HS, bool PACKED>
-__device__ __forceinline__ void pf_rope_kv_body(float *__restrict__ qkv, int ldq, float *__restrict__ kc, float *__restrict__ vc, __half *__restrict__ kh,
-                                                __half *__restrict__ vh, int kvd, int n_heads, int n_kv_heads, int arch, const float *__restrict__ qnw,
-                                                const float *__restrict__ knw, const float *__restrict__ qkvb, float eps, const float *__restrict__ cr,
-                                                const float *__restrict__ ci, int start_pos, const PfTok *__restrict__ tok, size_t slot_stride) {
+template <int HS>
+__global__ void __launch_bounds__(256) k_pf_rope_kv_packed(float *__restrict__ qkv, int ldq, float *__restrict__ kc, float *__restrict__ vc, size_t slot_stride,
+                                                          __half *__restrict__ kh, __half *__restrict__ vh, int kvd, int n_heads, int n_kv_heads, int arch,
+                                                          const float *__restrict__ qnw, const float *__restrict__ knw, const float *__restrict__ qkvb, float eps,
+                                                          const float *__restrict__ cr, const float *__restrict__ ci, const PfTok *__restrict__ tok) {
     constexpr int HALF = HS / 2, PPL = HALF / 32; // pairs per lane
-    const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, pos = PACKED ? tok[b].pos : start_pos + b;
+    const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, pos = tok[b].pos;
     const int qd = n_heads * HS;
     for (int hh = warp; hh < n_heads + n_kv_heads; hh += 8) {
         const bool is_q = hh < n_heads;
@@ -153,8 +156,8 @@ __device__ __forceinline__ void pf_rope_kv_body(float *__restrict__ qkv, int ldq
                 src[i0[u]] = r0;
                 src[i1[u]] = r1;
             } else {
-                const size_t o = PACKED ? (size_t)tok[b].slot * slot_stride + (size_t)pos * kvd + kvh * HS : (size_t)pos * kvd + kvh * HS;
-                const size_t oh = PACKED ? (size_t)tok[b].hrow * kvd + kvh * HS : o;
+                const size_t o = (size_t)tok[b].slot * slot_stride + (size_t)pos * kvd + kvh * HS;
+                const size_t oh = (size_t)tok[b].hrow * kvd + kvh * HS;
                 const float *vsrc = qkv + (size_t)b * ldq + qd + kvd + kvh * HS;
                 float w0 = vsrc[i0[u]], w1 = vsrc[i1[u]];
                 if (arch & KF_QKVBIAS) {
@@ -172,42 +175,7 @@ __device__ __forceinline__ void pf_rope_kv_body(float *__restrict__ qkv, int ldq
 }
 
 
-template <int HS>
-__global__ void __launch_bounds__(256) k_pf_rope_kv(float *__restrict__ qkv, int ldq, float *__restrict__ kc, float *__restrict__ vc, __half *__restrict__ kh,
-                                                   __half *__restrict__ vh, int kvd, int n_heads, int n_kv_heads, int arch, const float *__restrict__ qnw,
-                                                   const float *__restrict__ knw, const float *__restrict__ qkvb, float eps, const float *__restrict__ cr,
-                                                   const float *__restrict__ ci, int start_pos) {
-    pf_rope_kv_body<HS, false>(qkv, ldq, kc, vc, kh, vh, kvd, n_heads, n_kv_heads, arch, qnw, knw, qkvb, eps, cr, ci, start_pos, nullptr, 0);
-}
-
-// Several sequences packed into one chunk (b200_prefill_slots): each token's K / V go to its own slot and its sequence's scratch region.
-template <int HS>
-__global__ void __launch_bounds__(256) k_pf_rope_kv_packed(float *__restrict__ qkv, int ldq, float *__restrict__ kc, float *__restrict__ vc, size_t slot_stride,
-                                                          __half *__restrict__ kh, __half *__restrict__ vh, int kvd, int n_heads, int n_kv_heads, int arch,
-                                                          const float *__restrict__ qnw, const float *__restrict__ knw, const float *__restrict__ qkvb, float eps,
-                                                          const float *__restrict__ cr, const float *__restrict__ ci, const PfTok *__restrict__ tok) {
-    pf_rope_kv_body<HS, true>(qkv, ldq, kc, vc, kh, vh, kvd, n_heads, n_kv_heads, arch, qnw, knw, qkvb, eps, cr, ci, 0, tok, slot_stride);
-}
-
-// f16 copies of cache rows written before this chunk (start_pos > 0): rows [0, rows) of one layer
-__device__ __forceinline__ void pf_kv_to_f16_rows(const float *__restrict__ kc, const float *__restrict__ vc, __half *__restrict__ kh, __half *__restrict__ vh,
-                                                  size_t n4) {
-    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256) {
-        const float4 a = reinterpret_cast<const float4 *>(kc)[i], c = reinterpret_cast<const float4 *>(vc)[i];
-        const __half2 a0 = __floats2half2_rn(a.x, a.y), a1 = __floats2half2_rn(a.z, a.w), c0 = __floats2half2_rn(c.x, c.y), c1 = __floats2half2_rn(c.z, c.w);
-        uint2 pk;
-        pk.x = *reinterpret_cast<const uint32_t *>(&a0); pk.y = *reinterpret_cast<const uint32_t *>(&a1);
-        reinterpret_cast<uint2 *>(kh)[i] = pk;
-        pk.x = *reinterpret_cast<const uint32_t *>(&c0); pk.y = *reinterpret_cast<const uint32_t *>(&c1);
-        reinterpret_cast<uint2 *>(vh)[i] = pk;
-    }
-}
-__global__ void __launch_bounds__(256) k_pf_kv_to_f16(const float *__restrict__ kc, const float *__restrict__ vc, __half *__restrict__ kh, __half *__restrict__ vh,
-                                                     size_t n4) {
-    pf_kv_to_f16_rows(kc, vc, kh, vh, n4);
-}
-
-// Packed chunk: grid.y = the sequences that continue a slot (start > 0); rows [0, start) of slot `slot` (kc / vc: this layer's rows
+// grid.y = the sequences that continue a slot (start > 0): f16 copies of rows [0, start) of slot `slot` (kc / vc: this layer's rows
 // of slot 0) into that sequence's scratch region, which starts at row hrow.
 struct PfHist {
     int slot, start, hrow;
@@ -215,8 +183,18 @@ struct PfHist {
 __global__ void __launch_bounds__(256) k_pf_kv_to_f16_packed(const float *__restrict__ kc, const float *__restrict__ vc, size_t slot_stride, __half *__restrict__ kh,
                                                             __half *__restrict__ vh, int kvd, const PfHist *__restrict__ hist) {
     const PfHist h = hist[blockIdx.y];
-    const size_t src = (size_t)h.slot * slot_stride, dst = (size_t)h.hrow * kvd;
-    pf_kv_to_f16_rows(kc + src, vc + src, kh + dst, vh + dst, (size_t)h.start * kvd / 4);
+    const size_t src = (size_t)h.slot * slot_stride, dst = (size_t)h.hrow * kvd, n4 = (size_t)h.start * kvd / 4;
+    const float4 *k4 = reinterpret_cast<const float4 *>(kc + src), *v4 = reinterpret_cast<const float4 *>(vc + src);
+    uint2 *kh2 = reinterpret_cast<uint2 *>(kh + dst), *vh2 = reinterpret_cast<uint2 *>(vh + dst);
+    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n4; i += (size_t)gridDim.x * 256) {
+        const float4 a = k4[i], c = v4[i];
+        const __half2 a0 = __floats2half2_rn(a.x, a.y), a1 = __floats2half2_rn(a.z, a.w), c0 = __floats2half2_rn(c.x, c.y), c1 = __floats2half2_rn(c.z, c.w);
+        uint2 pk;
+        pk.x = *reinterpret_cast<const uint32_t *>(&a0); pk.y = *reinterpret_cast<const uint32_t *>(&a1);
+        kh2[i] = pk;
+        pk.x = *reinterpret_cast<const uint32_t *>(&c0); pk.y = *reinterpret_cast<const uint32_t *>(&c1);
+        vh2[i] = pk;
+    }
 }
 
 // ---- causal attention over the chunk + everything already in the cache ---------------------------
@@ -246,16 +224,16 @@ __device__ __forceinline__ uint32_t pack_h2(float lo, float hi) {
 }
 
 // One CTA: query tokens q0 .. q0+QT-1 of a sequence of n tokens at positions start_pos.. (q rows of qkv and out from row 0), keys
-// from rows [0, start_pos + n) of kh / vh, KV head blockIdx.y.  q0: from blockIdx.x, or the packed tile's (PACKED).
-template <int HS, bool PACKED>
+// from rows [0, start_pos + n) of kh / vh, KV head blockIdx.y.
+template <int HS>
 __device__ __forceinline__ void pm_attend(const float *__restrict__ qkv, int ldq, const __half *__restrict__ kh, const __half *__restrict__ vh, int kvd, int kv_mul,
-                                          int n, int start_pos, float inv_sqrt_hs, __half *__restrict__ out, int ldo, int tile_q0) {
+                                          int n, int start_pos, float inv_sqrt_hs, __half *__restrict__ out, int ldo, int q0) {
     extern __shared__ __align__(16) unsigned char pm_sm[];
     constexpr int RP = HS + 8, H4 = HS / 4, KS = HS / 16, NB = HS / 8; // row pitch (halves): 16 B of padding keeps fragment loads conflict-free
     __half *sQ = reinterpret_cast<__half *>(pm_sm), *sKV = sQ + PM_ROWS * RP; // stage s: K at sKV + s*2*64*RP, V right after it
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int QT = PM_ROWS / kv_mul, RV = QT * kv_mul; // rows >= RV: padding (token n: no Q, every key masked, not stored)
-    const int q0 = PACKED ? tile_q0 : ((int)gridDim.x - 1 - (int)blockIdx.x) * QT, grp = blockIdx.y; // longest (latest) query tiles first
+    const int grp = blockIdx.y;
     const int q_end = (q0 + QT < n ? q0 + QT : n), nkeys = start_pos + q_end, ntiles = (nkeys + PM_KT - 1) / PM_KT;
     const uint32_t sKV_addr = (uint32_t)__cvta_generic_to_shared(sKV);
     // K/V tile -> shared memory with cp.async (16 bytes per request, rows past nkeys zero-filled), double buffered
@@ -412,15 +390,9 @@ __device__ __forceinline__ void pm_attend(const float *__restrict__ qkv, int ldq
     }
 }
 
-template <int HS>
-__global__ void __launch_bounds__(PM_THREADS) k_pf_attention_mma(const float *__restrict__ qkv, int ldq, const __half *__restrict__ kh, const __half *__restrict__ vh,
-                                                                int kvd, int kv_mul, int n, int start_pos, float inv_sqrt_hs, __half *__restrict__ out, int ldo) {
-    pm_attend<HS, false>(qkv, ldq, kh, vh, kvd, kv_mul, n, start_pos, inv_sqrt_hs, out, ldo, 0);
-}
-
-// Packed chunk: tile blockIdx.x of the table (built longest first across every sequence, pf_tiles in plan.cu) is query tile q0 of
-// a sequence whose n tokens start at packed row row0 and whose keys start at scratch row hrow.  The tile runs exactly what
-// k_pf_attention_mma runs for that sequence alone, so each sequence's output is bit-identical to a single-sequence launch.
+// Tile blockIdx.x of the table (built longest first across every sequence, pf_tiles below) is query tile q0 of a sequence whose n
+// tokens start at packed row row0 and whose keys start at scratch row hrow.  A tile reads nothing of the other sequences, so each
+// sequence's output is bit-identical to a chunk that holds it alone.
 struct PfTile {
     int row0, n, start, q0, hrow;
 };
@@ -430,7 +402,7 @@ __global__ void __launch_bounds__(PM_THREADS) k_pf_attention_mma_packed(const fl
                                                                        const __half *__restrict__ vh, int kvd, int kv_mul, const PfTile *__restrict__ tiles,
                                                                        float inv_sqrt_hs, __half *__restrict__ out, int ldo) {
     const PfTile t = tiles[blockIdx.x];
-    pm_attend<HS, true>(qkv + (size_t)t.row0 * ldq, ldq, kh + (size_t)t.hrow * kvd, vh + (size_t)t.hrow * kvd, kvd, kv_mul, t.n, t.start, inv_sqrt_hs,
+    pm_attend<HS>(qkv + (size_t)t.row0 * ldq, ldq, kh + (size_t)t.hrow * kvd, vh + (size_t)t.hrow * kvd, kvd, kv_mul, t.n, t.start, inv_sqrt_hs,
                   out + (size_t)t.row0 * ldo, ldo, t.q0);
 }
 
@@ -447,7 +419,7 @@ inline std::vector<PfTile> pf_tiles(int n_seqs, const int *n, const int *start, 
     return t;
 }
 
-// device buffers are owned by the plan's allocation list, except the ones b200_prefill_slots grows
+// device buffers are owned by the plan's allocation list, except the ones a chunk grows
 inline void prefill_free(PrefillCtx &c) {
     for (void *d : {(void *)c.PKH, (void *)c.PVH, (void *)c.ptab}) cudaFree(d);
     c.PKH = c.PVH = nullptr;

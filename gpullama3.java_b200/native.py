@@ -79,7 +79,7 @@ class Tensor(C.Structure):
 
 EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_score_tokens", "b200_set_logprobs", "b200_read_logprobs", "b200_test_logprobs", "b200_set_sampling_controls", "b200_set_sample_history", "b200_read_sample_counts", "b200_test_sample_controls", "b200_time_sample_controls", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant", "b200_test_kq_tiles_to_q8",
-           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_pf_attention", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
+           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
            "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_weight_info", "b200_test_set_memory_budget", "b200_stream_rings",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
@@ -132,7 +132,6 @@ def lib() -> C.CDLL:
     L.b200_test_gemm.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.b200_test_gemm_q8.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.b200_test_gemm_i8.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, C.c_float, vp, vp, vp]
-    L.b200_test_pf_attention.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     L.b200_time_kernel.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
     L.b200_read_buffer.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
     L.b200_set_decode_slots.argtypes = [vp, i32]
@@ -140,7 +139,7 @@ def lib() -> C.CDLL:
     L.b200_slot_reset.argtypes = [vp, i32]
     L.b200_slot_copy_kv.argtypes = [vp, i32, i32]
     L.b200_prefill_slots.argtypes = [vp, i32, vp, vp, vp, vp]
-    L.b200_test_pf_attention_packed.argtypes = [i32, vp, vp, vp, vp, vp, i32, i32, i32, vp]
+    L.b200_test_pf_attention_packed.argtypes = [i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     L.b200_batch_info.argtypes = [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(C.c_float)]
     L.b200_forward_decode_multi.argtypes = [vp, i32, i32, vp, i32, vp, vp]
     L.b200_decode_multi_rows.argtypes = [vp, C.POINTER(i32)]
@@ -391,46 +390,34 @@ def test_gemm_i8(mode: str, aq, a_scales, bq, c=None, bq2=None, oscale: float = 
     return c
 
 
-def test_pf_attention_packed(qs, ks, vs, starts, n_heads: int, n_kv_heads: int, sentinel: int = 0x7E5A) -> list:
-    """The packed prefill attention (k_pf_attention_mma_packed) over several sequences in one launch.  qs[i] float32
-    [n_i, n_heads*hs]; ks[i], vs[i] float32 [starts[i]+n_i, n_kv_heads*hs].  Returns each sequence's f16 bits [n_i, n_heads*hs]."""
+def _pf_attention_packed(qs, ks, vs, starts, n_heads: int, n_kv_heads: int, out_rows: int | None, sentinel: int) -> np.ndarray:
     lens = np.array([len(q) for q in qs], dtype=np.int32)
     st = np.ascontiguousarray(starts, dtype=np.int32)
     hs = qs[0].shape[1] // n_heads
     q = np.ascontiguousarray(np.concatenate(qs), dtype=np.float32)
     k = np.ascontiguousarray(np.concatenate(ks), dtype=np.float32)
     v = np.ascontiguousarray(np.concatenate(vs), dtype=np.float32)
-    if len(st) != len(qs) or any(len(ks[i]) != st[i] + lens[i] or len(vs[i]) != st[i] + lens[i] for i in range(len(qs))):
+    if len(st) != len(qs) or any(np.shape(ks[i]) != (st[i] + lens[i], n_kv_heads * hs) or np.shape(vs[i]) != np.shape(ks[i]) for i in range(len(qs))):
         raise ValueError("ks[i] / vs[i] must be [starts[i] + n_i, n_kv_heads * head_size]")
-    out = np.full((int(lens.sum()), n_heads * hs), sentinel, dtype=np.uint16)
+    out = np.full((int(lens.sum()) if out_rows is None else out_rows, n_heads * hs), sentinel, dtype=np.uint16)
     rc = lib().b200_test_pf_attention_packed(len(qs), lens.ctypes.data, st.ctypes.data, q.ctypes.data, k.ctypes.data, v.ctypes.data, n_heads,
-                                             n_kv_heads, hs, out.ctypes.data)
+                                             n_kv_heads, hs, len(out), out.ctypes.data)
     if rc != B200_OK:
         _raise(rc, "b200_test_pf_attention_packed failed")
-    return np.split(out, np.cumsum(lens)[:-1])
-
-
-def test_pf_attention(q, k, v, n_heads: int, n_kv_heads: int, start_pos: int, impl: str = "mma", out_rows: int | None = None,
-                      sentinel: int = 0x7E5A) -> np.ndarray:
-    """The prefill's causal attention over one chunk (csrc/prefill.cuh).  q float32 [n, n_heads*hs]; k, v float32
-    [start_pos+n, n_kv_heads*hs].  impl names the kernel: "mma" (k_pf_attention_mma) is the only one.  Returns the f16 bits
-    (uint16) of [out_rows, n_heads*hs]: rows >= n keep `sentinel`."""
-    if impl != "mma":
-        raise ValueError(f"no prefill attention kernel {impl!r}: the prefill runs k_pf_attention_mma (impl='mma')")
-    q = np.ascontiguousarray(q, dtype=np.float32)
-    k = np.ascontiguousarray(k, dtype=np.float32)
-    v = np.ascontiguousarray(v, dtype=np.float32)
-    n, qd = q.shape
-    hs = qd // n_heads
-    if k.shape != (start_pos + n, n_kv_heads * hs) or v.shape != k.shape:
-        raise ValueError("k / v must be [start_pos + n, n_kv_heads * head_size]")
-    rows = n if out_rows is None else out_rows
-    out = np.full((rows, qd), sentinel, dtype=np.uint16)
-    rc = lib().b200_test_pf_attention(q.ctypes.data, k.ctypes.data, v.ctypes.data, n, start_pos, n_heads, n_kv_heads, hs,
-                                      rows, out.ctypes.data)
-    if rc != B200_OK:
-        _raise(rc, "b200_test_pf_attention failed")
     return out
+
+
+def test_pf_attention_packed(qs, ks, vs, starts, n_heads: int, n_kv_heads: int, sentinel: int = 0x7E5A) -> list:
+    """The prefill's causal attention (k_pf_attention_mma_packed, csrc/prefill.cuh) over several sequences in one launch.  qs[i]
+    float32 [n_i, n_heads*hs]; ks[i], vs[i] float32 [starts[i]+n_i, n_kv_heads*hs].  Returns each sequence's f16 bits [n_i, n_heads*hs]."""
+    lens = [len(q) for q in qs]
+    return np.split(_pf_attention_packed(qs, ks, vs, starts, n_heads, n_kv_heads, None, sentinel), np.cumsum(lens)[:-1])
+
+
+def test_pf_attention(q, k, v, n_heads: int, n_kv_heads: int, start_pos: int, out_rows: int | None = None, sentinel: int = 0x7E5A) -> np.ndarray:
+    """The prefill's causal attention over one sequence: a chunk that holds it alone.  q float32 [n, n_heads*hs]; k, v float32
+    [start_pos+n, n_kv_heads*hs].  Returns the f16 bits (uint16) of [out_rows, n_heads*hs]: rows >= n keep `sentinel`."""
+    return _pf_attention_packed([q], [k], [v], [start_pos], n_heads, n_kv_heads, out_rows, sentinel)
 
 
 GGML_SIZES = {0: (4, 1), 1: (2, 1), 8: (34, 32), 12: (144, 256), 13: (176, 256), 14: (210, 256)}  # (bytes, elements) per block, GGMLType.java:5-20

@@ -611,21 +611,16 @@ int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, i
 int b200_test_gemm_i8(int32_t mode, int32_t m, int32_t n, int32_t k, const int8_t *aq, const float *as, const void *bq, const void *bq2, float oscale,
                       float *c, int8_t *hq, float *hs);
 
-/* Test hook: the causal attention of the tensor-core prefill over one chunk of n query tokens at positions start_pos ..
- * start_pos + n - 1.  q: f32 [n][n_heads * head_size] (rotated); k, v: f32 [start_pos + n][n_kv_heads * head_size] (the KV cache
- * rows), run by k_pf_attention_mma on f16 K / V copies built by k_pf_kv_to_f16, as in the prefill.  q is placed in rows of
- * stride q + 2 * kv width whose k / v columns hold NaN; grid and shared memory are the prefill's.  out: f16 bits [out_rows][n_heads * head_size], out_rows >= n, in/out: rows >= n must come back untouched.
- * head_size 64 or 128, n_heads % n_kv_heads == 0 and n_heads / n_kv_heads <= 64 (any ratio: a CTA serves floor(64 / ratio) query
- * tokens, the remaining rows of its 64-row tile are padding). */
-int b200_test_pf_attention(const float *q, const float *k, const float *v, int32_t n, int32_t start_pos, int32_t n_heads,
-                           int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out);
-
-/* Test hook: the packed form of the same attention (k_pf_attention_mma_packed, as b200_prefill_slots runs it) over n_seqs sequences
- * at once.  Sequence i has lengths[i] >= 1 query tokens at positions start_positions[i]..; q: f32 [sum lengths][n_heads * head_size]
- * (the sequences' rows back to back); k, v: f32 [sum (start_positions[i] + lengths[i])][n_kv_heads * head_size] (each sequence's
- * rows 0 .. start + length - 1, back to back).  out: f16 bits [sum lengths][n_heads * head_size], in/out. */
+/* Test hook: the causal attention of the tensor-core prefill (k_pf_attention_mma_packed, on f16 K / V copies built by
+ * k_pf_kv_to_f16_packed, as a chunk runs it) over n_seqs sequences at once.  Sequence i has lengths[i] >= 1 query tokens at positions
+ * start_positions[i]..; q: f32 [sum lengths][n_heads * head_size] (rotated; the sequences' rows back to back, placed in rows of
+ * stride q + 2 * kv width whose k / v columns hold NaN); k, v: f32 [sum (start_positions[i] + lengths[i])][n_kv_heads * head_size]
+ * (each sequence's KV cache rows 0 .. start + length - 1, back to back); grid and shared memory are the prefill's.  out: f16 bits
+ * [out_rows][n_heads * head_size], out_rows >= sum lengths, in/out: rows >= sum lengths must come back untouched.  head_size 64 or
+ * 128, n_heads % n_kv_heads == 0 and n_heads / n_kv_heads <= 64 (any ratio: a CTA serves floor(64 / ratio) query tokens, the
+ * remaining rows of its 64-row tile are padding). */
 int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const int32_t *start_positions, const float *q, const float *k,
-                                  const float *v, int32_t n_heads, int32_t n_kv_heads, int32_t head_size, uint16_t *out);
+                                  const float *v, int32_t n_heads, int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out);
 
 /* Weight upload of b200_plan_create (the counterpart of the reference's load-time metrics, ModelLoader.java:102-106 and the
  * copy-in timing of TornadoVMMasterPlanSingleToken.java:51-54): wall seconds from the first tensor to the last repack kernel,

@@ -192,7 +192,7 @@ def test_gemm_hook_rejections(pkg):
 def _attention_ref(q, k, v, n_heads, n_kv, start, equal_scores=False):
     """(float64 causal softmax attention, elementwise bound of the kernel's f16 output) for queries at start .. start+n-1.
 
-    The inputs are rounded as k_pf_attention_mma rounds them -- qh = f16(f32(q) * f32(inv_sqrt_hs * log2e)),
+    The inputs are rounded as k_pf_attention_mma_packed rounds them -- qh = f16(f32(q) * f32(inv_sqrt_hs * log2e)),
     kh = f16(k), vh = f16(v) -- and scores are in log2 units.
     The bound, with vmax = max |v| over the row's visible keys:
       2^-11 |ref| + 2^-25           the f16 output rounding (subnormal floor)
@@ -270,19 +270,18 @@ def _attention_cases(kv_mul):
     return cases
 
 
-def _check_attention(pkg, impl, q, k, v, n_heads, n_kv, start, kind, what):
+def _check_attention(pkg, q, k, v, n_heads, n_kv, start, kind, what):
     n = q.shape[0]
-    out = pkg.native.test_pf_attention(q, k, v, n_heads, n_kv, start, impl=impl, out_rows=n + 64, sentinel=ATT_SENTINEL)
+    out = pkg.native.test_pf_attention(q, k, v, n_heads, n_kv, start, out_rows=n + 64, sentinel=ATT_SENTINEL)
     assert np.all(out[n:] == ATT_SENTINEL), f"{what}: a padding row past n was written"
     assert not np.any(out[:n] == ATT_SENTINEL), f"{what}: a (row < n, head) slot was not written"
     ref, bound = _attention_ref(q, k, v, n_heads, n_kv, start, equal_scores=kind == "equal")
     return _assert_within(what, out[:n].view(np.float16), ref, bound)
 
 
-@pytest.mark.parametrize("impl", ["mma"])
 @pytest.mark.parametrize("kv_mul", [1, 2, 4, 8, 16, 64])
-def test_pf_attention_matches_float64(pkg, impl, kv_mul):
-    """k_pf_attention_mma (what the prefill runs), elementwise against float64 softmax attention, at every GQA ratio
+def test_pf_attention_matches_float64(pkg, kv_mul):
+    """k_pf_attention_mma_packed on a one-sequence chunk (what the prefill runs), elementwise against float64 softmax attention, at every GQA ratio
     prefill_init accepts (at 64 a query tile is one token), across key-tile boundaries."""
     n_kv = 2 if kv_mul <= 8 else 1
     n_heads = n_kv * kv_mul
@@ -291,9 +290,9 @@ def test_pf_attention_matches_float64(pkg, impl, kv_mul):
         for kind in ATT_KINDS:
             rng = np.random.default_rng(zlib.crc32(repr((kv_mul, n, start, hs, kind)).encode()))
             q, k, v = _attention_inputs(kind, n, start, n_heads, n_kv, hs, rng)
-            what = f"{impl} kv_mul={kv_mul} hs={hs} n={n} start={start} {kind}"
-            worst = max(worst, _check_attention(pkg, impl, q, k, v, n_heads, n_kv, start, kind, what))
-    print(f"attention {impl} kv_mul={kv_mul}: worst |err| / bound over all cases = {worst:.3g}")
+            what = f"kv_mul={kv_mul} hs={hs} n={n} start={start} {kind}"
+            worst = max(worst, _check_attention(pkg, q, k, v, n_heads, n_kv, start, kind, what))
+    print(f"attention kv_mul={kv_mul}: worst |err| / bound over all cases = {worst:.3g}")
 
 
 def _prefill_and_compare(pkg, orc, m, n_tok, batch, tol=FP16_TOL):
@@ -417,7 +416,7 @@ def _check_prefill_stages(pkg, m, first, second):
         # K cache rows of the chunk: RoPE (after the Qwen3 k norm) of the k part
         kref, kbound = _k_cache_ref(m, qkv[:, qd:qd + kvd], start, L)
         r_k = _assert_within(f"{name} K cache = RoPE(k)", kc[start:], kref, kbound)
-        # attention over the rotated q and the KV cache, as k_pf_attention_mma computes it
+        # attention over the rotated q and the KV cache, as k_pf_attention_mma_packed computes it
         aref, abound = _attention_ref(qkv[:, :qd], kc, vc, c.n_heads, c.n_kv_heads, start)
         r_a = _assert_within(f"{name} attention", att16, aref, abound)
         # gate/up + SwiGLU on the FFN input

@@ -166,9 +166,8 @@ def test_qwen2_plan_without_a_bias_fails_and_names_it(pkg, make_model):
 ATT_STARTS = [0, 1, 63, 64, 65, 200]
 
 
-@pytest.mark.parametrize("impl", ["mma"])
 @pytest.mark.parametrize("kv_mul", [3, 5, 6, 7, 12])
-def test_pf_attention_any_gqa_ratio_matches_float64(pkg, impl, kv_mul):
+def test_pf_attention_any_gqa_ratio_matches_float64(pkg, kv_mul):
     """QT = floor(64 / kv_mul) query tokens per CTA: rows QT * kv_mul .. 63 are padding.  n around QT and across tiles, several
     start positions, both head sizes; rows >= n must come back untouched (the check inside _check_attention)."""
     n_kv = 2
@@ -181,9 +180,9 @@ def test_pf_attention_any_gqa_ratio_matches_float64(pkg, impl, kv_mul):
             for kind in ATT_KINDS:
                 rng = np.random.default_rng(zlib.crc32(repr(("qwen2", kv_mul, n, start, hs, kind)).encode()))
                 q, k, v = _attention_inputs(kind, n, start, n_heads, n_kv, hs, rng)
-                what = f"{impl} kv_mul={kv_mul} hs={hs} n={n} start={start} {kind}"
-                worst = max(worst, _check_attention(pkg, impl, q, k, v, n_heads, n_kv, start, kind, what))
-    print(f"attention {impl} kv_mul={kv_mul}: worst |err| / bound = {worst:.3g}")
+                what = f"kv_mul={kv_mul} hs={hs} n={n} start={start} {kind}"
+                worst = max(worst, _check_attention(pkg, q, k, v, n_heads, n_kv, start, kind, what))
+    print(f"attention kv_mul={kv_mul}: worst |err| / bound = {worst:.3g}")
 
 
 def _tc_prefill(pkg, orc, m, n_tok, batch, tol, mode="tensor_core"):

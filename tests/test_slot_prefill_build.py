@@ -14,6 +14,8 @@ def test_slot_prefill_kernels_do_not_spill():
     assert len([n for n in e if "k_batch_rows_next" in n]) == 1, sorted(e)
     for name, (stack, st, ld) in e.items():
         assert (stack, st, ld) == (0, 0, 0), f"{name}: stack / spill stores / loads = {stack} / {st} / {ld}"
+    # every tensor-core chunk is a packed chunk: no single-sequence form of these kernels is left
+    assert not _entries(r"k_pf_rope_kvI|k_pf_kv_to_f16P|k_pf_attention_mmaI"), "a k_pf_* kernel without the _packed suffix"
 
 
 class _FakePlan:

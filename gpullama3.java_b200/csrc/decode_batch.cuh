@@ -116,19 +116,13 @@ __host__ __device__ inline SmbSmem smb_layout(int seg, int nrow, size_t budget) 
     SmbSmem L;
     L.stage_bytes = (4 * smv_unit_bytes(seg) + 127) & ~127;
     size_t o = 0;
-    L.off_bar = o; o += 2 * SMV_MAX_STAGES * 8 + SMV_MAX_STAGES * 4;
+    L.off_bar = o; o += ring_bar_bytes(SMV_MAX_STAGES);
     o = (o + 15) & ~(size_t)15;
     L.off_act = o; o += (size_t)nrow * seg + (size_t)nrow * (seg / 32) * 4; // quants [row][seg], then scales [row][seg / 32]
     o = (o + 15) & ~(size_t)15;
     L.off_terms = o; o += (size_t)SMV_CONSUMER_WARPS * 4 * nrow * SMB_TSTRIDE * 4;
     L.off_cand = o; o += (size_t)SMV_CONSUMER_WARPS * 32 * 8; // lm_head: per-lane (max, first index)
-    o = (o + 127) & ~(size_t)127;
-    L.off_ring = o;
-    const long room = (long)budget - (long)o;
-    int s = room > 0 ? (int)(room / L.stage_bytes) : 0;
-    if (s > SMV_MAX_STAGES) s = SMV_MAX_STAGES;
-    L.stages = s;
-    L.total = o + (size_t)s * L.stage_bytes;
+    ring_fit<SMV_MAX_STAGES>(L, o, budget);
     return L;
 }
 
@@ -160,7 +154,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8_batch(SmbAr
     const int nseg = W.nseg;
     const unsigned tile_bytes = 4u * (unsigned)W.unit_bytes;
     volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + L.off_bar + 2 * SMV_MAX_STAGES * 8);
-    if (tid == 0) {
+    if (tid == 0) { // stream_ring_init's work, written out: through the shared helper this kernel's machine code changes
         for (int s = 0; s < S; s++) {
             mbar_init(bar0 + 8 * s, 1);
             mbar_init(bar0 + 8 * (SMV_MAX_STAGES + s), 1);
@@ -171,7 +165,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_stream_matvec_q8_batch(SmbAr
     __syncthreads();
     pdl_launch_dependents();
 
-    if (warp == SMV_CONSUMER_WARPS) { // producer: the same walk as k_stream_matvec_q8's
+    if (warp == SMV_CONSUMER_WARPS) { // producer: k_stream_matvec_q8's walk
         if (lane == 0) {
             unsigned seq = 0;
             const unsigned long long pol = l2_policy_evict_first();

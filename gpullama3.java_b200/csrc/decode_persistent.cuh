@@ -101,7 +101,7 @@ __host__ __device__ inline PdSmem pd_layout(int dim, int qd, int hidden, int hea
     const int sq_floats = PD_CT * seqsum2_stride(E); // squares of the norm in the accumulator's bank-conflict-free chunk layout
     L.nbuf_floats = sq_floats > att_floats ? sq_floats : att_floats;
     size_t o = 0;
-    L.off_bar = o; o += 2 * PD_MAX_STAGES * 8 + PD_MAX_STAGES * 4;
+    L.off_bar = o; o += ring_bar_bytes(PD_MAX_STAGES);
     o = (o + 15) & ~(size_t)15;
     L.off_xq = o; o += (size_t)maxc;
     L.off_xs = o; o += (size_t)(maxc / 32) * 4;
@@ -117,13 +117,7 @@ __host__ __device__ inline PdSmem pd_layout(int dim, int qd, int hidden, int hea
     L.off_terms = o; o += (size_t)PD_WARPS * 4 * L.tstride * 4;
     L.off_hvals = o; o += SMV_HVALS * 4;
     L.off_misc = o; o += 96 * 4; // red[16], s_val[2] @16, norm scale @20, argmax merge scratch @32 (16 floats) / @48 (16 ints)
-    o = (o + 127) & ~(size_t)127;
-    L.off_ring = o;
-    long room = (long)budget - (long)o;
-    int s = room > 0 ? (int)(room / L.stage_bytes) : 0;
-    if (s > PD_MAX_STAGES) s = PD_MAX_STAGES;
-    L.stages = s;
-    L.total = o + (size_t)s * L.stage_bytes;
+    ring_fit<PD_MAX_STAGES>(L, o, budget);
     return L;
 }
 
@@ -745,7 +739,7 @@ __global__ void __launch_bounds__(PD_THREADS, 1) k_decode_persistent(const __gri
     const int S = L.stages;
     const unsigned bar0 = smem_u32(smem + L.off_bar);
     volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + L.off_bar + 2 * PD_MAX_STAGES * 8);
-    if (tid == 0) {
+    if (tid == 0) { // stream_ring_init's work, written out: through the shared helper this kernel's machine code changes
         for (int s = 0; s < S; s++) {
             mbar_init(bar0 + 8 * s, 1);
             mbar_init(bar0 + 8 * (PD_MAX_STAGES + s), 1);

@@ -120,19 +120,13 @@ __host__ __device__ inline MoeDownSmem moe_down_layout(int hv, int seg_s, int se
     L.stage_bytes = (4 * ub + 127) & ~127;
     L.nbs_pad = ((seg / 32 + 3) & ~3) + 4;
     size_t o = 0;
-    L.off_bar = o; o += 2 * SMV_MAX_STAGES * 8 + SMV_MAX_STAGES * 4;
+    L.off_bar = o; o += ring_bar_bytes(SMV_MAX_STAGES);
     L.off_xq = o; o += (size_t)hv;
     o = (o + 15) & ~(size_t)15;
     L.off_xs = o; o += (size_t)(hv / 32) * 4;
     o = (o + 15) & ~(size_t)15;
     L.off_terms = o; o += (size_t)SMV_CONSUMER_WARPS * 4 * L.nbs_pad * 4;
-    o = (o + 127) & ~(size_t)127;
-    L.off_ring = o;
-    long room = (long)budget - (long)o;
-    int s = room > 0 ? (int)(room / L.stage_bytes) : 0;
-    if (s > SMV_MAX_STAGES) s = SMV_MAX_STAGES;
-    L.stages = s;
-    L.total = o + (size_t)s * L.stage_bytes;
+    ring_fit<SMV_MAX_STAGES>(L, o, budget);
     return L;
 }
 
@@ -165,20 +159,6 @@ __device__ __forceinline__ void moe_tile_terms(const unsigned char *tile, const 
     }
 }
 
-// Ring bookkeeping shared by both kernels (the dense stream's protocol): full[s] / empty[s] mbarriers and release counters.
-__device__ __forceinline__ void moe_ring_init(unsigned char *smem, size_t off_bar, int S) {
-    volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + off_bar + 2 * SMV_MAX_STAGES * 8);
-    const unsigned bar0 = smem_u32(smem + off_bar);
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < S; s++) {
-            mbar_init(bar0 + 8 * s, 1);
-            mbar_init(bar0 + 8 * (SMV_MAX_STAGES + s), 1);
-            rel[s] = 0u;
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-}
-
 // Gate/up of the shared expert and the k routed experts as ONE virtual gate/up matrix: groups [0, Hs/2) are the shared expert's,
 // then He/2 groups per routed slot.  Output unit u of the virtual hidden vector = silu(gate) * up of group u / 2, exactly as
 // k_stream_matvec_q8<SMV_GATEUP> computes a dense layer's; its Q8_0 epilogue is the dense one over the virtual vector.
@@ -195,7 +175,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_gateup(MoeStreamArgs a, 
     const int nseg = a.S.nseg; // the shared and the routed gate/up streams have the same columns (dim), so the same tiles
     const unsigned tile_bytes = 4u * (unsigned)a.S.unit_bytes;
     volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + L.off_bar + 2 * SMV_MAX_STAGES * 8);
-    moe_ring_init(smem, L.off_bar, S);
+    stream_ring_init<SMV_MAX_STAGES>(smem, L.off_bar, S);
     __syncthreads();
     trace_entry(a.tr);
     pdl_launch_dependents();
@@ -340,7 +320,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_down(MoeStreamArgs a, Mo
     const int g1 = (int)(((long long)(blockIdx.x + 1) * ngroups) / gridDim.x);
     const int nm = a.k + 1;
     volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + L.off_bar + 2 * SMV_MAX_STAGES * 8);
-    moe_ring_init(smem, L.off_bar, S);
+    stream_ring_init<SMV_MAX_STAGES>(smem, L.off_bar, S);
     __syncthreads();
     trace_entry(a.tr);
     pdl_launch_dependents();

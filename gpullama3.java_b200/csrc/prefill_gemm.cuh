@@ -16,6 +16,7 @@
 // SWIZZLE_128B layout TMA gives the f16 path, then arrive on the stage's full barrier.  The wgmma loop and the
 // epilogues are the same code for both sources.
 #pragma once
+#include "common.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -35,24 +36,6 @@ enum { B_F16 = 0, B_Q8 = 1 };
 constexpr int Q8_QUANT_BYTES = BN * BK, Q8_SCALE_BYTES = BN * 16, Q8_RAW_BYTES = Q8_QUANT_BYTES + Q8_SCALE_BYTES;
 constexpr int Q8_CONVERTERS = 96; // warps 1-3 of the producer warp group
 
-__device__ __forceinline__ uint32_t s32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t cnt) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(cnt)); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "PG_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra PG_DONE;\n"
-        "bra PG_WAIT;\n"
-        "PG_DONE:\n"
-        "}\n" ::"r"(bar), "r"(parity)
-        : "memory");
-}
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, int c0, int c1, uint32_t bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
                  "l"(map), "r"(c0), "r"(c1), "r"(bar)
@@ -139,7 +122,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid
     uint64_t *bars = reinterpret_cast<uint64_t *>(sR + RSTAGES * RAW_BYTES);
     // raw: a W8A16 raw stage has landed.  The converters own the raw ring: they refill a stage once all of them have
     // converted it, so its loads run up to RSTAGES k-blocks ahead, independent of the operand ring.
-    const uint32_t full0 = s32(bars), empty0 = s32(bars + STAGES), raw0 = s32(bars + 2 * STAGES);
+    const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + STAGES), raw0 = smem_u32(bars + 2 * STAGES);
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
@@ -164,16 +147,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid
                 const int kc = (kb0 + kb) * BK;
                 if (BSRC == B_Q8) { // B arrives through the converters
                     mbar_expect_tx(full0 + 8 * st, A_BYTES);
-                    tma_load_2d(s32(sA + st * A_BYTES), &tma_a, kc, m0, full0 + 8 * st);
+                    tma_load_2d(smem_u32(sA + st * A_BYTES), &tma_a, kc, m0, full0 + 8 * st);
                     continue;
                 }
                 mbar_expect_tx(full0 + 8 * st, A_BYTES + B_BYTES);
-                tma_load_2d(s32(sA + st * A_BYTES), &tma_a, kc, m0, full0 + 8 * st);
+                tma_load_2d(smem_u32(sA + st * A_BYTES), &tma_a, kc, m0, full0 + 8 * st);
                 if (MODE == GEMM_GATEUP) {
-                    tma_load_2d(s32(sB + st * B_BYTES), &tma_b, kc, n0, full0 + 8 * st);
-                    tma_load_2d(s32(sB + st * B_BYTES + B_BYTES / 2), &tma_b2, kc, n0, full0 + 8 * st);
+                    tma_load_2d(smem_u32(sB + st * B_BYTES), &tma_b, kc, n0, full0 + 8 * st);
+                    tma_load_2d(smem_u32(sB + st * B_BYTES + B_BYTES / 2), &tma_b2, kc, n0, full0 + 8 * st);
                 } else {
-                    tma_load_2d(s32(sB + st * B_BYTES), &tma_b, kc, n0, full0 + 8 * st);
+                    tma_load_2d(smem_u32(sB + st * B_BYTES), &tma_b, kc, n0, full0 + 8 * st);
                 }
             }
         } else if constexpr (BSRC == B_Q8) {
@@ -189,8 +172,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid
             auto load_raw = [&](int kb) {
                 const int kc = (kb0 + kb) * BK, s = kc / seg, j = kc - s * seg, rs = kb % RSTAGES;
                 mbar_expect_tx(raw0 + 8 * rs, RAW_BYTES);
-                tma_load_4d(s32(sR + rs * RAW_BYTES), &tma_b, j, 0, s, g0, raw0 + 8 * rs);
-                tma_load_4d(s32(sR + rs * RAW_BYTES + Q8_QUANT_BYTES), &tma_b2, seg + ((j >> 8) << 4), 0, s, g0, raw0 + 8 * rs);
+                tma_load_4d(smem_u32(sR + rs * RAW_BYTES), &tma_b, j, 0, s, g0, raw0 + 8 * rs);
+                tma_load_4d(smem_u32(sR + rs * RAW_BYTES + Q8_QUANT_BYTES), &tma_b2, seg + ((j >> 8) << 4), 0, s, g0, raw0 + 8 * rs);
             };
             if (ct == 0)
                 for (int kb = 0; kb < RSTAGES && kb < nk; kb++) load_raw(kb);
@@ -232,7 +215,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid
         const int st = kb % STAGES;
         mbar_wait(full0 + 8 * st, (kb / STAGES) & 1);
         asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
-        const uint64_t da = wgmma_desc_sw128(s32(sA + st * A_BYTES + c * (64 * 128))), db = wgmma_desc_sw128(s32(sB + st * B_BYTES));
+        const uint64_t da = wgmma_desc_sw128(smem_u32(sA + st * A_BYTES + c * (64 * 128))), db = wgmma_desc_sw128(smem_u32(sB + st * B_BYTES));
 #pragma unroll
         for (int k = 0; k < BK / 16; k++) // K step of 16 fp16 = 32 bytes = +2 in the (addr >> 4) field, inside the 128-byte swizzle atom
             wgmma_m64n128k16(acc, da + 2 * k, db + 2 * k, (kb | k) != 0);
@@ -286,7 +269,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_f16_wgmma(const __grid
         if (t == 0 && c == 0) {
 #pragma unroll
             for (int b = 0; b < BN / 32; b++) {
-                const uint32_t src = s32(smem + b * (BM * 32 * 4));
+                const uint32_t src = smem_u32(smem + b * (BM * 32 * 4));
                 if (MODE == GEMM_RESID)
                     asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(&tma_c), "r"(src),
                                  "r"(n0 + b * 32), "r"(m0)

@@ -102,7 +102,7 @@ __device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUt
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     float *hbuf = reinterpret_cast<float *>(smem + I8_STAGES * I8_STAGE_BYTES);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + I8_STAGES * I8_STAGE_BYTES + I8_HBUF_BYTES);
-    const uint32_t full0 = s32(bars), empty0 = s32(bars + I8_STAGES);
+    const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + I8_STAGES);
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         // full: the producer's expect_tx; empty: one arrival per consumer warp once it has read the stage (operands and scales)
@@ -118,7 +118,7 @@ __device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUt
                 const int st = kb % I8_STAGES;
                 mbar_wait(empty0 + 8 * st, ((kb / I8_STAGES) & 1) ^ 1);
                 const int kc = kb * BK, s = kc / o.seg, j = kc - s * o.seg;
-                const uint32_t base = s32(smem + st * I8_STAGE_BYTES), full = full0 + 8 * st;
+                const uint32_t base = smem_u32(smem + st * I8_STAGE_BYTES), full = full0 + 8 * st;
                 mbar_expect_tx(full, I8_STAGE_BYTES);
                 tma_load_2d(base, &tma_a, kc, m0, full);
                 tma_load_4d(base + I8_A_BYTES, &tma_bq, j, 0, s, g0, full);
@@ -138,7 +138,7 @@ __device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUt
 #pragma unroll
     for (int i = 0; i < 32; i++) { acc[i] = 0.0f; da[i] = 0; db[i] = 0; }
     auto issue = [&](int (&d)[32], int st, int sub) { // sub: the k-block's first or second 32-column block (+32 bytes = +2 in the address field)
-        const uint32_t base = s32(smem + st * I8_STAGE_BYTES);
+        const uint32_t base = smem_u32(smem + st * I8_STAGE_BYTES);
         asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
         wgmma_i8_m64n64k32(d, wgmma_desc_sw64(base + c * 64 * BK) + 2 * sub, wgmma_desc_sw64(base + I8_A_BYTES) + 2 * sub);
         asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");

@@ -55,6 +55,20 @@ __host__ __device__ inline int smv_unit_bytes(int seg) { return (seg + seg / 16 
 __host__ __device__ inline int smv_unit_bytes(int seg, int fmt) { return fmt ? (seg / 256 * kq_block_bytes(fmt) + 15) & ~15 : smv_unit_bytes(seg); }
 __host__ __device__ inline int tile_groups(const TileMat &W) { return (W.rows + 3) >> 2; } // 4-row groups stored, the last one zero-padded
 
+// Shared memory of a weight ring: its barrier block (full[], empty[] mbarriers and release counters) and its stages.  ring_fit places the
+// stages of a layout whose other buffers end at o: from the next 128-byte boundary, as many as fit in budget, at most MAX.
+__host__ __device__ constexpr size_t ring_bar_bytes(int max_stages) { return 2 * (size_t)max_stages * 8 + (size_t)max_stages * 4; }
+template <int MAX, class Layout>
+__host__ __device__ inline void ring_fit(Layout &L, size_t o, size_t budget) {
+    o = (o + 127) & ~(size_t)127;
+    L.off_ring = o;
+    const long room = (long)budget - (long)o;
+    int s = room > 0 ? (int)(room / L.stage_bytes) : 0;
+    if (s > MAX) s = MAX;
+    L.stages = s;
+    L.total = o + (size_t)s * L.stage_bytes;
+}
+
 struct SmvSmem {
     size_t off_bar, off_xq, off_xs, off_terms, off_hvals, off_ring, total;
     int stages, stage_bytes, nbs_pad;
@@ -66,45 +80,17 @@ __host__ __device__ inline SmvSmem smv_layout(int cols, int seg, size_t budget, 
     L.stage_bytes = (4 * unit + 127) & ~127;
     L.nbs_pad = ((seg / 32 + 3) & ~3) + 4; // row stride of the term buffer: 16-byte aligned rows, the four walker lanes on distinct banks
     size_t o = 0;
-    L.off_bar = o; o += 2 * SMV_MAX_STAGES * 8 + SMV_MAX_STAGES * 4; // full[], empty[] mbarriers + release counters
+    L.off_bar = o; o += ring_bar_bytes(SMV_MAX_STAGES);
     L.off_xq = o; o += (size_t)cols;
     L.off_xs = o; o += (size_t)(cols / 32) * 4;
     o = (o + 15) & ~(size_t)15;
     L.off_terms = o; o += (size_t)SMV_CONSUMER_WARPS * 4 * L.nbs_pad * 4;
     L.off_hvals = o; o += SMV_HVALS * 4; // GATEUP: this CTA's swiglu outputs; STORE+argmax: per-warp candidates
-    o = (o + 127) & ~(size_t)127;
-    L.off_ring = o;
-    long room = (long)budget - (long)o;
-    int s = room > 0 ? (int)(room / L.stage_bytes) : 0;
-    if (s > SMV_MAX_STAGES) s = SMV_MAX_STAGES;
-    L.stages = s;
-    L.total = o + (size_t)s * L.stage_bytes;
+    ring_fit<SMV_MAX_STAGES>(L, o, budget);
     return L;
 }
 
-// ---- mbarrier / bulk-copy / PDL primitives (inline PTX) ---------------------------------------
-__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(unsigned bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra WAIT_DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "WAIT_DONE:\n"
-        "}\n" ::"r"(bar), "r"(parity)
-        : "memory");
-}
+// ---- bulk-copy primitives (inline PTX; the mbarrier wrappers are in common.cuh) ------------------------------------------
 // Bulk global -> shared copy with an L2 evict_first policy: single-use weight tiles must not push the KV rows, activations and norm weights out of L2
 // (it made the persistent kernel faster where it was measured).
 __device__ __forceinline__ unsigned long long l2_policy_evict_first() {
@@ -116,6 +102,23 @@ __device__ __forceinline__ void bulk_g2s_evict_first(unsigned dst, const void *s
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst), "l"(src),
                  "r"(bytes), "r"(bar), "l"(pol)
                  : "memory");
+}
+// The ring bookkeeping of the Q8_0 weight streams: by thread 0, full[s] / empty[s] mbarriers at off_bar + 8 s / + 8 (MAX + s) and the
+// release counters rel[s] = 0; a __syncthreads() must follow.  k_stream_matvec_q8_batch and k_decode_persistent write the same code
+// out, and every kernel keeps its own producer walk and consumer acquire / release: behind shared helpers those change the kernels'
+// machine code (the dense and batched streams measured 0.5 to 1.2 % slower).
+template <int MAX>
+__device__ __forceinline__ void stream_ring_init(unsigned char *smem, size_t off_bar, int S) {
+    volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + off_bar + 2 * MAX * 8);
+    const unsigned bar0 = smem_u32(smem + off_bar);
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < S; s++) {
+            mbar_init(bar0 + 8 * s, 1);
+            mbar_init(bar0 + 8 * (MAX + s), 1);
+            rel[s] = 0u;
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
 }
 __device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(SMV_CONSUMER_WARPS * 32) : "memory"); }
 struct SmvConsumerSync {
@@ -207,14 +210,7 @@ __host__ inline SmvSmem smv_layout_norm(int cols, int seg, size_t budget, unsign
     *off_sq = (unsigned)L.off_terms;
     *off_seq = (unsigned)(L.off_terms + sq); // sq is a multiple of 16 bytes
     const size_t dead = L.off_ring - L.off_terms;
-    size_t o = L.off_terms + (nb > dead ? nb : dead);
-    o = (o + 127) & ~(size_t)127;
-    L.off_ring = o;
-    long room = (long)budget - (long)o;
-    int s = room > 0 ? (int)(room / L.stage_bytes) : 0;
-    if (s > SMV_MAX_STAGES) s = SMV_MAX_STAGES;
-    L.stages = s;
-    L.total = o + (size_t)s * L.stage_bytes;
+    ring_fit<SMV_MAX_STAGES>(L, L.off_terms + (nb > dead ? nb : dead), budget);
     return L;
 }
 
@@ -301,14 +297,7 @@ __device__ __forceinline__ void smv_q8_body(const SmvArgs &a, const SmvSmem &L, 
     // independently, so a warp can reach the tile of lap k+2 of a stage while lap k+1 is still in
     // flight; a parity wait cannot tell those apart, the counter can.
     volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + L.off_bar + 2 * SMV_MAX_STAGES * 8);
-    if (tid == 0) {
-        for (int s = 0; s < S; s++) {
-            mbar_init(bar0 + 8 * s, 1);
-            mbar_init(bar0 + 8 * (SMV_MAX_STAGES + s), 1);
-            rel[s] = 0u;
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    stream_ring_init<SMV_MAX_STAGES>(smem, L.off_bar, S);
     __syncthreads();
     trace_entry(a.tr);
     pdl_launch_dependents(); // let the next kernel become resident and start prefetching its weights

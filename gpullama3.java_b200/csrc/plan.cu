@@ -22,10 +22,12 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <chrono>
 #include <string>
 #include <thread>
 #include <type_traits>
+#include <unordered_map>
 #include <utility>
 #include <vector>
 
@@ -1075,6 +1077,23 @@ int launch_stream_batch(b200_plan *p, const TileMat &W, int n, const int8_t *xq,
     return launch_k(p, p->use_pdl, k_stream_matvec_q8_batch<MODE>, dim3(p->n_sms), dim3(SMV_THREADS), L.total, a, L);
 }
 
+// The classifier of a batched step over its first e rows, whose final residuals are rows [0, e) of x (dim floats apart): the final
+// norm (k_rmsnorm_quant_batch), the Q8_0 lm_head stream with per-row argmax partials, and k_argmax_batch -> bt.logits / bt.ids rows
+// [0, e).  enqueue_batch ends with it over bt.x, b200_forward_chunk over the chunk's residual rows (pi8.X).
+const int CLASSIFIER_LAUNCHES = 3;
+int enqueue_classifier(b200_plan *p, float *x, int e) {
+    const b200_config &c = p->cfg;
+    auto &B = p->bt;
+    TpCtx solo{};
+    solo.n = 1;
+    int rc;
+    if ((rc = launch_k(p, p->use_pdl, k_rmsnorm_quant_batch<false>, dim3(e), dim3(NORM_THREADS), norm_smem_bytes(c.dim), x, (const BatchRows *)B.rows, p->emb,
+                       p->mup.embedding_scale, (const float *)p->out_norm, c.rms_norm_eps, c.dim, B.xq, B.xs, TraceBuf{nullptr, 0, 0}, solo)))
+        return rc;
+    if ((rc = launch_stream_batch<SMV_STORE>(p, p->tout, e, B.xq, B.xs, B.logits, sampler_padded(c.vocab_size), nullptr, nullptr, true))) return rc;
+    return launch_k(p, p->use_pdl, k_argmax_batch, dim3(e), dim3(32), (size_t)0, (const float *)B.part_val, (const int *)B.part_idx, p->n_sms, B.ids);
+}
+
 // One forward step of n rows in the given form (StepForm bits): the single-sequence graph's kernel sequence, every launch serving
 // all n rows.  The final norm, lm_head and argmax run over the first e rows only (e = 0: not at all, as in the prefills).  SPLIT
 // costs one more launch per layer.  OWN writes key_cache / value_cache, whose layout is slot 0's.
@@ -1129,14 +1148,8 @@ int enqueue_batch(b200_plan *p, int n, int e, int form, int *launches) {
         if ((rc = launch_stream_batch<SMV_RESID>(p, L.tw2, n, B.hq, B.hs, B.x, c.dim))) return rc;
         k += 5;
     }
-    if (!e) {
-        if (launches) *launches = k;
-        return B200_OK;
-    }
-    if ((rc = norm(false, p->out_norm, e))) return rc;
-    if ((rc = launch_stream_batch<SMV_STORE>(p, p->tout, e, B.xq, B.xs, B.logits, sampler_padded(c.vocab_size), nullptr, nullptr, true))) return rc;
-    if ((rc = launch_k(p, pdl, k_argmax_batch, dim3(e), dim3(32), (size_t)0, (const float *)B.part_val, (const int *)B.part_idx, p->n_sms, B.ids))) return rc;
-    if (launches) *launches = k + 2;
+    if (e && (rc = enqueue_classifier(p, B.x, e))) return rc;
+    if (launches) *launches = k + (e ? CLASSIFIER_LAUNCHES : 0);
     return B200_OK;
 }
 
@@ -2099,6 +2112,22 @@ bool i8_weight_maps(b200_plan *p) {
     return true;
 }
 
+// Why the plan's shape or type rules the bit-exact tensor-core prefill out (nullptr: it can run), before anything is allocated.
+const char *i8_why(const b200_plan *p) {
+    const b200_config &g = p->cfg;
+    const int nqkv = p->qd + 2 * p->kvd;
+    if (p->prefill_batch <= 1) return "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
+    if (p->wtype != B200_GGML_Q8_0)
+        return "the bit-exact tensor-core prefill needs a Q8_0 plan (an FP16 plan's CPU dot products are FP16 lane chains, not int8 block sums)";
+    if (g.tp_size > 1) return "tensor-core prefill is single-GPU";
+    if (g.dim % 64 || p->qd % 64 || nqkv % 64) return "the bit-exact tensor-core prefill needs dim, q width and q+k+v width multiples of 64";
+    for (const LayerW &L : p->layers)
+        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
+            if (q8_geometry(*t).seg % pg::BK) return "the bit-exact tensor-core prefill needs Q8_0 stream segments that are multiples of 64 columns";
+    if (!pg::encode_fn()) return "cuTensorMapEncodeTiled not available from the driver";
+    return nullptr;
+}
+
 // Built on the first b200_set_prefill_mode(TENSOR_CORE_EXACT): the chunk buffers and tensor maps over the plan's own Q8_0 streams,
 // nothing per weight.  A resident plan adds one scratch, the Q8_0 tiles of its largest resident matrix, and its resident matrices'
 // maps point there; the scratch and the chunk buffers must fit the free memory (memory_free) or the call fails with
@@ -2107,21 +2136,11 @@ int prefill_init_i8(b200_plan *p) {
     PrefillI8Ctx &c = p->pi8;
     const b200_config &g = p->cfg;
     const int nqkv = p->qd + 2 * p->kvd;
-    if (p->prefill_batch <= 1) { c.why = "the plan was created without a prefill batch size (prefill_batch_size <= 1)"; return B200_OK; }
-    if (p->wtype != B200_GGML_Q8_0) {
-        c.why = "the bit-exact tensor-core prefill needs a Q8_0 plan (an FP16 plan's CPU dot products are FP16 lane chains, not int8 block sums)";
-        return B200_OK;
-    }
-    if (g.tp_size > 1) { c.why = "tensor-core prefill is single-GPU"; return B200_OK; }
-    if (g.dim % 64 || p->qd % 64 || nqkv % 64) { c.why = "the bit-exact tensor-core prefill needs dim, q width and q+k+v width multiples of 64"; return B200_OK; }
+    if ((c.why = i8_why(p))) return B200_OK;
     int64_t kq8_bytes = 0;
     for (const LayerW &L : p->layers)
-        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2}) {
-            const TileMat q = q8_geometry(*t);
-            if (q.seg % pg::BK) { c.why = "the bit-exact tensor-core prefill needs Q8_0 stream segments that are multiples of 64 columns"; return B200_OK; }
-            if (t->fmt && tile_bytes(q) > kq8_bytes) kq8_bytes = tile_bytes(q);
-        }
-    if (!pg::encode_fn()) { c.why = "cuTensorMapEncodeTiled not available from the driver"; return B200_OK; }
+        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
+            if (t->fmt && tile_bytes(q8_geometry(*t)) > kq8_bytes) kq8_bytes = tile_bytes(q8_geometry(*t));
     const int bpad = (p->prefill_batch + pg::BM - 1) / pg::BM * pg::BM, big = g.dim > p->qd ? g.dim : p->qd;
     const int lds_big = pg::i8_lds(big), lds_h = pg::i8_lds(g.hidden_dim);
     int att_tokens = bpad;
@@ -2167,28 +2186,37 @@ int prefill_init_i8(b200_plan *p) {
     return B200_OK;
 }
 
-// One chunk: tab[v] = (token, position, KV offset) of chunk row v; own: the K / V go to the plan's cache, else to the decode slots.
-// The batched step's graph (enqueue_batch) over the whole chunk, its Q8_0 streams replaced by k_gemm_i8.  Times the chunk
-// (p->prefill_ms) and counts its launches (p->launches_prefill).  score (b200_score_tokens, after score_init_i8): then the final
-// norm, the classifier (expanded first on a resident plan) into p->sc.logits SCORE_GROUP_ROWS rows at a time, and k_score_rows
-// over each group into p->sc.out.
-int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own, bool score = false) {
+// k_i8_norm over chunk rows [0, n) of c.X into XQ / XS; embed (layer 0): each row's embedding is gathered into c.X first.
+void i8_norm(b200_plan *p, int n, bool embed, const float *w) {
+    PrefillI8Ctx &c = p->pi8;
+    const b200_config &g = p->cfg;
+    const size_t norm_smem = norm_smem_bytes(g.dim);
+    const int lds_d = pg::i8_lds(g.dim);
+    const TraceBuf tr{nullptr, 0, 0};
+    TpCtx solo{};
+    solo.n = 1;
+    if (embed) k_i8_norm<true><<<n, NORM_THREADS, norm_smem, p->stream>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
+    else k_i8_norm<false><<<n, NORM_THREADS, norm_smem, p->stream>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
+}
+
+// The layers of one chunk over its n rows, whose ChunkTok entries (token, position, KV offset) are already in c.tok: the batched
+// step's graph (enqueue_batch) over the whole chunk, its Q8_0 streams replaced by k_gemm_i8.  own: the K / V go to the plan's cache,
+// else to the decode slots.  Leaves each row's final residual in row v of c.X and adds its launches to *nl; enqueued only (no events,
+// no synchronise), so prefill_forward_i8 and b200_forward_chunk wrap it in their own tails.
+int enqueue_chunk_i8(b200_plan *p, int n, bool own, int *nl_out) {
     PrefillI8Ctx &c = p->pi8;
     const b200_config &g = p->cfg;
     cudaStream_t s = p->stream;
-    const int n = (int)tab.size(), nqkv = p->qd + 2 * p->kvd, mt = (n + pg::BM - 1) / pg::BM;
-    const int lds_d = pg::i8_lds(g.dim), lds_q = pg::i8_lds(p->qd), lds_h = pg::i8_lds(g.hidden_dim);
-    const size_t ctx_kv = (size_t)g.context_length * p->kvd, norm_smem = norm_smem_bytes(g.dim);
+    const int nqkv = p->qd + 2 * p->kvd, mt = (n + pg::BM - 1) / pg::BM;
+    const int lds_q = pg::i8_lds(p->qd), lds_h = pg::i8_lds(g.hidden_dim);
+    const size_t ctx_kv = (size_t)g.context_length * p->kvd;
     const size_t att_smem = att_smem_bytes(g.head_size, g.context_length, c.att != nullptr);
     const TraceBuf tr{nullptr, 0, 0};
     TpCtx solo{};
     solo.n = 1;
-    CK(cudaMemcpyAsync(c.tok, tab.data(), (size_t)n * sizeof(ChunkTok), cudaMemcpyHostToDevice, s));
-    CK(cudaEventRecord(p->ev0, s));
-    int nl = 0, rc = 0;
+    int &nl = *nl_out, rc = 0;
     auto norm = [&](bool embed, const float *w) {
-        if (embed) k_i8_norm<true><<<n, NORM_THREADS, norm_smem, s>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
-        else k_i8_norm<false><<<n, NORM_THREADS, norm_smem, s>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
+        i8_norm(p, n, embed, w);
         nl++;
     };
     // one k_gemm_i8 over the stream W; n_tiles from W's rows (64 stream rows per tile).  A resident W is first expanded to its Q8_0
@@ -2232,10 +2260,28 @@ int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own,
         if ((rc = gemm(GATEUP(), c.a_dim, c.s_dim, m.gu_q, m.gu_s, L.tgu, nullptr, 0, 1.0f))) return rc;
         if ((rc = gemm(RESID(), c.a_h, c.s_h, m.w2_q, m.w2_s, L.tw2, c.X, g.dim, rs))) return rc;
     }
+    CK(cudaGetLastError());
+    return B200_OK;
+}
+
+// One chunk: tab[v] = (token, position, KV offset) of chunk row v; own: the K / V go to the plan's cache, else to the decode slots.
+// enqueue_chunk_i8, timed (p->prefill_ms) with its launches counted (p->launches_prefill).  score (b200_score_tokens, after
+// score_init_i8): then the final norm, the classifier (expanded first on a resident plan) into p->sc.logits SCORE_GROUP_ROWS rows at
+// a time, and k_score_rows over each group into p->sc.out.
+int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own, bool score = false) {
+    PrefillI8Ctx &c = p->pi8;
+    const b200_config &g = p->cfg;
+    cudaStream_t s = p->stream;
+    const int n = (int)tab.size(), lds_d = pg::i8_lds(g.dim);
+    CK(cudaMemcpyAsync(c.tok, tab.data(), (size_t)n * sizeof(ChunkTok), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(p->ev0, s));
+    int nl = 0, rc;
+    if ((rc = enqueue_chunk_i8(p, n, own, &nl))) return rc;
     if (score) {
         auto &S = p->sc;
         const TileMat Q = q8_geometry(p->tout);
-        norm(false, p->out_norm);
+        i8_norm(p, n, false, p->out_norm);
+        nl++;
         if (p->tout.fmt) {
             CK(launch_kq_tiles_to_q8(p->tout, Q, c.kq8, s));
             nl++;
@@ -2483,32 +2529,25 @@ int check_row(b200_plan *p, int i, const b200_step_row &r) {
     return B200_OK;
 }
 
-// One batched step with the classifier over checked rows: against the decode slots, or with own the plan's cache (every row
-// slot 0).  The emitting rows go first (stable), so the final norm, lm_head and argmax run over rows [0, e) and no kernel indexes
-// through a row map; their ids and logits return to the caller's row order, ids -1 where a row does not emit.  Rows with a
-// temperature run the device sampler, all in one launch.  With controls, the emitting rows of slots with sampling controls run
-// k_sample_ctl instead, all in one launch of their own.  b200_batch_info reports the step.
-int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, bool controls, int32_t *ids_out, float *logits) {
-    const b200_config &c = p->cfg;
-    auto &B = p->bt;
-    int order[SMB_MAX_ROWS], e = 0;
+// The emitting rows first (stable), then the others: order[k] = the caller's index of step row k; returns the emitting rows' count.
+int emit_first(int n, const b200_step_row *rows, int *order) {
+    int e = 0;
     for (int i = 0; i < n; i++)
         if (rows[i].emit) order[e++] = i;
     for (int i = 0, k = e; i < n; i++)
         if (!rows[i].emit) order[k++] = i;
-    BatchRows br{};
-    for (int k = 0; k < n; k++) {
-        const b200_step_row &r = rows[order[k]];
-        br.token[k] = r.token; br.pos[k] = r.position; br.slot[k] = r.slot;
-    }
+    return e;
+}
+
+// What a step with the classifier does after it, for b200_forward_step and b200_forward_chunk alike: bt.logits / bt.ids rows [0, e)
+// hold the emitting rows (step row k is the caller's row order[k], order from emit_first over n rows).  Their logits go back to the
+// caller's row order, ids -1 where a row does not emit.  Rows with a temperature run the device sampler, all in one launch.  With
+// controls, the emitting rows of slots with sampling controls run k_sample_ctl instead, all in one launch of their own.  Then the
+// log-probabilities, the readback and the call's one synchronise.
+int step_outputs(b200_plan *p, int n, const b200_step_row *rows, const int *order, int e, bool controls, int32_t *ids_out, float *logits) {
+    const b200_config &c = p->cfg;
+    auto &B = p->bt;
     int rc;
-    const Graph *g;
-    if ((rc = batch_graph(p, step_form(br, n, own), n, e, &g))) return rc;
-    *B.h_rows = br;
-    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
-    CK(cudaEventRecord(p->ev0, p->stream));
-    CK(cudaGraphLaunch(g->exec, p->stream));
-    CK(cudaEventRecord(p->ev1, p->stream));
     const size_t vpad = (size_t)sampler_padded(c.vocab_size);
     if (logits) // before the sampler turns sampled rows into probabilities
         for (int k = 0; k < e; k++)
@@ -2556,8 +2595,62 @@ int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, bool co
     }
     for (int i = 0; i < n; i++) ids_out[i] = -1;
     for (int k = 0; k < e; k++) ids_out[order[k]] = ctl[k] || rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
+    return B200_OK;
+}
+
+// One batched step with the classifier over checked rows: against the decode slots, or with own the plan's cache (every row
+// slot 0).  The emitting rows go first, so the final norm, lm_head and argmax run over rows [0, e) and no kernel indexes through a
+// row map; step_outputs does the rest.  b200_batch_info reports the step.
+int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, bool controls, int32_t *ids_out, float *logits) {
+    auto &B = p->bt;
+    int order[SMB_MAX_ROWS];
+    const int e = emit_first(n, rows, order);
+    BatchRows br{};
+    for (int k = 0; k < n; k++) {
+        const b200_step_row &r = rows[order[k]];
+        br.token[k] = r.token; br.pos[k] = r.position; br.slot[k] = r.slot;
+    }
+    int rc;
+    const Graph *g;
+    if ((rc = batch_graph(p, step_form(br, n, own), n, e, &g))) return rc;
+    *B.h_rows = br;
+    CK(cudaMemcpyAsync(B.rows, B.h_rows, sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaEventRecord(p->ev0, p->stream));
+    CK(cudaGraphLaunch(g->exec, p->stream));
+    CK(cudaEventRecord(p->ev1, p->stream));
+    if ((rc = step_outputs(p, n, rows, order, e, controls, ids_out, logits))) return rc;
     CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
     B.last_launches = g->launches;
+    return B200_OK;
+}
+
+// b200_forward_chunk over checked rows in the tensor_core_exact mode: the chunk laid out with the emitting rows first, as batch_step
+// lays out its step, runs enqueue_chunk_i8 (K / V to the decode slots); its first e residual rows go through the batched step's
+// classifier, read in place from pi8.X, and step_outputs does the rest.  b200_batch_info reports the call (CUDA events around the
+// chunk and the classifier); b200_prefill_info is left alone.
+int chunk_step(b200_plan *p, int n, const b200_step_row *rows, int32_t *ids_out, float *logits) {
+    const b200_config &g = p->cfg;
+    auto &B = p->bt;
+    std::vector<int> order(n);
+    const int e = emit_first(n, rows, order.data());
+    const size_t slot_stride = (size_t)g.n_layers * g.context_length * p->kvd;
+    std::vector<ChunkTok> tab(n);
+    for (int k = 0; k < n; k++) {
+        const b200_step_row &r = rows[order[k]];
+        tab[k] = ChunkTok{r.token, r.position, (long long)(r.slot * slot_stride)};
+    }
+    int rc, nl = 0;
+    CK(cudaMemcpyAsync(p->pi8.tok, tab.data(), (size_t)n * sizeof(ChunkTok), cudaMemcpyHostToDevice, p->stream));
+    CK(cudaEventRecord(p->ev0, p->stream));
+    if ((rc = enqueue_chunk_i8(p, n, false, &nl))) return rc;
+    if (e) {
+        if ((rc = enqueue_classifier(p, p->pi8.X, e))) return rc;
+        nl += CLASSIFIER_LAUNCHES;
+    }
+    CK(cudaEventRecord(p->ev1, p->stream));
+    if ((rc = step_outputs(p, n, rows, order.data(), e, true, ids_out, logits))) return rc;
+    CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
+    B.last_launches = nl;
     return B200_OK;
 }
 
@@ -3236,6 +3329,55 @@ int b200_forward_step(b200_plan *p, int32_t n, const b200_step_row *rows, int32_
     return batch_step(p, n, rows, false, true, ids_out, logits);
 }
 
+namespace {
+// Why a plan can never run b200_forward_chunk (nullptr: it can, in tensor_core_exact with decode slots): what rules out batched
+// steps, then what rules out the bit-exact tensor-core prefill.
+const char *chunk_why(const b200_plan *p) {
+    const char *why = multi_why(p);
+    return why ? why : i8_why(p);
+}
+const char *const PREFILL_MODE_NAMES[4] = {"exact", "tensor_core", "tensor_core_w8a16", "tensor_core_exact"};
+} // namespace
+
+int b200_chunk_rows(b200_plan *p, int32_t *max_rows) {
+    if (!p || !max_rows) return B200_ERR_BAD_ARG;
+    *max_rows = !chunk_why(p) && p->bt.n_slots && chunk_path(p) == CHUNK_I8 ? p->prefill_batch : 0;
+    return B200_OK;
+}
+
+int b200_forward_chunk(b200_plan *p, int32_t n, const b200_step_row *rows, int32_t *ids_out, float *logits) {
+    if (!p) return B200_ERR_BAD_ARG;
+    if (const char *why = chunk_why(p)) return fail(p, B200_ERR_UNSUPPORTED, "%s", why);
+    auto &B = p->bt;
+    if (!B.n_slots) return fail(p, B200_ERR_STATE, "no decode slots: call b200_set_decode_slots first");
+    if (chunk_path(p) != CHUNK_I8) {
+        const int mode = chunk_path(p) == CHUNK_NONE ? B200_PREFILL_EXACT : p->prefill.mode;
+        return fail(p, B200_ERR_STATE, "the plan's prefill mode is %s%s: b200_forward_chunk runs in tensor_core_exact (b200_set_prefill_mode)",
+                    PREFILL_MODE_NAMES[mode], mode == B200_PREFILL_EXACT ? "" : ", whose f16 GEMMs are not bit-exact");
+    }
+    if (!rows || !ids_out) return fail(p, B200_ERR_BAD_ARG, "rows and ids_out must not be NULL");
+    if (n < 1 || n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (b200_chunk_rows)", n, p->prefill_batch);
+    const int max_emit = batch_max_rows(p); // the batched classifier's rows
+    int rc, e = 0, emits[SMB_MAX_ROWS];     // emits[s]: the first emitting row of slot s, or -1
+    for (int s = 0; s < SMB_MAX_ROWS; s++) emits[s] = -1;
+    std::unordered_map<long long, int> seen; // slot * context_length + position -> row
+    for (int i = 0; i < n; i++) {
+        const b200_step_row &r = rows[i];
+        if (r.emit != 0 && r.emit != 1) return fail(p, B200_ERR_BAD_ARG, "row %d: emit must be 0 or 1 (got %d)", i, r.emit);
+        if ((rc = check_row(p, i, r))) return rc;
+        const auto at = seen.emplace((long long)r.slot * p->cfg.context_length + r.position, i);
+        if (!at.second) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d position %d repeats row %d's", i, r.slot, r.position, at.first->second);
+        if (!r.emit) continue;
+        if (++e > max_emit) return fail(p, B200_ERR_BAD_ARG, "row %d: more than %d emitting rows in one call", i, max_emit);
+        if (emits[r.slot] >= 0 && p->ctl.on[r.slot + 1])
+            return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d has sampling controls and already emits in row %d (its counts would depend on "
+                                             "that row's id)", i, r.slot, emits[r.slot]);
+        if (emits[r.slot] < 0) emits[r.slot] = i;
+    }
+    CK(cudaSetDevice(p->device));
+    return chunk_step(p, n, rows, ids_out, logits);
+}
+
 int b200_batch_info(b200_plan *p, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step) {
     if (!p) return B200_ERR_BAD_ARG;
     if (n_slots) *n_slots = p->bt.n_slots;
@@ -3254,7 +3396,7 @@ int b200_set_logprobs(b200_plan *p, int32_t top_n) {
         if (top_n > p->cfg.vocab_size) return fail(p, B200_ERR_BAD_ARG, "top_n = %d exceeds the vocabulary (%d)", top_n, p->cfg.vocab_size);
         // each buffer on its own: a call that failed part-way leaves the rest to the next call, and logprobs stay off until all exist
         CK(cudaSetDevice(p->device));
-        const int cap = p->seq_cap > SMB_MAX_ROWS ? p->seq_cap : SMB_MAX_ROWS;
+        const int cap = std::max({p->seq_cap, p->prefill_batch, SMB_MAX_ROWS}); // b200_forward_chunk: a row per chunk row
         int rc;
         if (!L.out && (rc = dalloc(p, &L.out, (size_t)cap * sizeof(LogprobRow)))) return rc;
         if (!L.smp && (rc = dalloc(p, &L.smp, (size_t)SMB_MAX_ROWS * sampler_padded(p->cfg.vocab_size) * 4))) return rc;

@@ -13,8 +13,8 @@ Position/token conventions decide parity, so they are restated exactly:
 ``generate_tokens_lookahead`` the first loop, several positions verified per step (forward_decode_multi): the rest of the
                               prompt, or drafted tokens, checked in one weight stream; the same ids for any draft
 ``ContinuousBatcher`` / ``generate_tokens_continuous`` the first two loops for a stream of requests: decode rows of running
-                              requests and prompt rows of newly admitted ones share each forward_step, and freed slots are
-                              refilled from a queue
+                              requests and prompt rows of newly admitted ones share each forward_step (or, opted in, each
+                              forward_chunk on the tensor cores), and freed slots are refilled from a queue
 ``score_sequence`` / ``perplexity`` teacher-forced scoring of a given text (plan.score_tokens) in chunks the plan accepts
 The plan-driven loops take an optional ``logprobs`` list: with the plan's log-probabilities on (plan.set_logprobs(N)) it receives
 one entry (chosen, [(id, logprob), ...]) per generated id -- per request, one list per request -- from plan.last_logprobs().
@@ -341,13 +341,21 @@ def generate_tokens_lookahead(plan, model_type: str, latest_token: int, start_po
 
 
 class _Request:
-    __slots__ = ("rid", "steps", "sampler", "kv_left", "row", "slot", "generated")
+    __slots__ = ("rid", "steps", "sampler", "kv_left", "limit", "row", "slot", "generated")
 
-    def __init__(self, rid, steps, sampler, kv_rows):
+    def __init__(self, rid, steps, sampler, kv_rows, limit):
         self.rid, self.steps, self.sampler, self.kv_left = rid, steps, sampler, kv_rows
+        self.limit = limit  # the loop's clamped max_tokens: it yields positions below it only
         self.row = None  # the (token, position) the loop asks for next
         self.slot = -1
         self.generated = 0
+
+    def rows_left(self) -> int:
+        """Rows the request can put into one step: its decode row, or its prompt rows up to and including the emitting one (prompt
+        rows sit at consecutive positions, and the loop ends at the first position >= limit)."""
+        if self.generated:
+            return 1
+        return min(self.kv_left + 1, self.limit - self.row[1])
 
 
 class ContinuousBatcher:
@@ -363,15 +371,24 @@ class ContinuousBatcher:
     step().  Every forward_step row is bit-identical to forward_decode of its sequence alone, so each request's ids equal its loop
     run alone on one slot, greedy or sampled with the same seed, whatever else shares the steps.
 
+    chunk_rows > 0 admits prompts on the tensor cores (the plan in set_prefill_mode("tensor_core_exact")): a step gathers its rows
+    the same way with a budget of chunk_rows, capped at plan.chunk_rows(), and runs them as one forward_chunk when at least
+    min_chunk_rows rows are available; otherwise it is today's step of decode_multi_rows() rows through forward_step.  forward_chunk
+    is bit-identical to forward_step on the same rows, so every request's ids are its loop's alone whichever call a step takes.  The
+    default of 32 rows is where the int8 prefill overtakes the exact multi-position step on prompts alone (DESIGN.md section 6); a
+    starting point, not a tuned value.  chunk_rows = 0 (the default) never calls forward_chunk.
+
     sampler (optional, per request): a sampler.Sampler; one next_float1() is drawn per generated token, never for a prompt row, as
-    generateTokensLlama draws it (InferenceEngine.java:81-154).  The steps are always the exact mixed steps, whatever the plan's
-    prefill mode.  A sampler's controls (sampler.SamplingControls) and history go onto the request's slot at admission, after
-    slot_reset (a request without controls turns its slot's off); the device applies them to the request's emitting rows.
+    generateTokensLlama draws it (InferenceEngine.java:81-154).  Without chunk_rows the steps are always the exact mixed steps,
+    whatever the plan's prefill mode.  A sampler's controls (sampler.SamplingControls) and history go onto the request's slot at
+    admission, after slot_reset (a request without controls turns its slot's off); the device applies them to the request's emitting
+    rows.
 
     When the plan's log-probabilities are on (plan.set_logprobs), logprobs[rid] receives one entry (chosen, [(id, logprob), ...])
     per generated id, next to results[rid]."""
 
-    def __init__(self, plan, model_type: str, stop_tokens: Iterable[int], max_tokens: int, context_length: int):
+    def __init__(self, plan, model_type: str, stop_tokens: Iterable[int], max_tokens: int, context_length: int, chunk_rows: int = 0,
+                 min_chunk_rows: int = 32):
         self.plan = plan
         self.rows = plan.decode_multi_rows()
         if self.rows < 1:
@@ -379,12 +396,22 @@ class ContinuousBatcher:
         n_slots = plan.batch_info()[0]
         if n_slots < 1:
             raise ValueError("the plan has no decode slots (set_decode_slots)")
+        if chunk_rows < 0 or min_chunk_rows < 1:
+            raise ValueError(f"chunk_rows = {chunk_rows} must be >= 0 and min_chunk_rows = {min_chunk_rows} >= 1")
+        self.chunk_rows = 0
+        if chunk_rows:
+            cap = plan.chunk_rows()
+            if cap < 1:
+                raise ValueError("the plan cannot run chunk steps (chunk_rows() == 0: set_prefill_mode('tensor_core_exact') first)")
+            self.chunk_rows = min(chunk_rows, cap)
+        self.min_chunk_rows = min_chunk_rows
         self.qwen = _is_qwen_loop(model_type)
         self.stop = list(stop_tokens)
         self.max_tokens, self.context_length = max_tokens, context_length
         self.results: dict = {}  # request id -> generated ids so far
         self.logprobs: dict = {}  # request id -> their log-probability entries (the plan's logprobs on)
         self.last_rows = 0  # rows of the last step() (0: no step ran)
+        self.last_kind = None  # "step" (forward_step) or "chunk" (forward_chunk) of the last step() that ran
         self._queue: deque = deque()
         self._free = list(range(n_slots))
         self._running: list = []  # admitted requests, in admission order
@@ -401,7 +428,8 @@ class ContinuousBatcher:
         self._next_id += 1
         self.results[rid] = []
         self.logprobs[rid] = []
-        self._queue.append(_Request(rid, steps, sampler, max(len(prompt) - 1, 0) if self.qwen else len(prompt)))
+        limit = self.context_length if self.max_tokens < 0 or self.context_length < self.max_tokens else self.max_tokens
+        self._queue.append(_Request(rid, steps, sampler, max(len(prompt) - 1, 0) if self.qwen else len(prompt), limit))
         return rid
 
     def pending(self) -> int:
@@ -456,11 +484,16 @@ class ContinuousBatcher:
             if emitting:
                 emit.append(r)
 
+        budget, chunk = self.rows, False
+        if self.chunk_rows:
+            chunk = min(sum(r.rows_left() for r in self._running if r.row is not None), self.chunk_rows) >= self.min_chunk_rows
+            if chunk:
+                budget = self.chunk_rows
         for r in self._running:  # one decode row per generating request
             if r.generated:
                 add(r, True)
         for r in self._running:  # then the prompts, in admission order
-            while not r.generated and r.row is not None and len(rows) < self.rows:
+            while not r.generated and r.row is not None and len(rows) < budget:
                 if r.kv_left == 0:
                     add(r, True)
                     break
@@ -470,7 +503,8 @@ class ContinuousBatcher:
                     ended.append(r)
         self.last_rows = len(rows)
         if rows:
-            ids, _ = self.plan.forward_step(rows)
+            ids, _ = (self.plan.forward_chunk if chunk else self.plan.forward_step)(rows)
+            self.last_kind = "chunk" if chunk else "step"
             lp_on = getattr(self.plan, "logprobs_top_n", lambda: -1)() >= 0  # a stand-in plan without log-probabilities: off
             entries = _logprob_rows(self.plan) if lp_on else None
             done = list(ended)
@@ -501,24 +535,24 @@ class ContinuousBatcher:
 
 def generate_tokens_continuous(plan, model_type: str, requests: list, arrivals: list, stop_tokens: Iterable[int], max_tokens: int,
                                context_length: int, samplers: list | None = None, stats: dict | None = None,
-                               logprobs: list | None = None) -> list[list[int]]:
+                               logprobs: list | None = None, chunk_rows: int = 0, min_chunk_rows: int = 32) -> list[list[int]]:
     """Replays a request trace through a ContinuousBatcher: request i = (latest_token, start_position, prompt_tokens) is submitted
     before step arrivals[i] (requests of the same step in index order), with samplers[i] if given.  Steps with no rows still count.
     Returns each request's ids, equal to loop_for(model_type) for the request alone.  stats (optional dict) receives the steps run,
-    the rows and launches of each, and per request its submission, first-token and completion times (time.perf_counter seconds,
-    None where it generated no token).  logprobs (optional list, plan.set_logprobs on) receives one list per request, one entry per
-    generated id."""
+    the rows, launches and kind ("step" or "chunk") of each, and per request its submission, first-token and completion times
+    (time.perf_counter seconds, None where it generated no token).  logprobs (optional list, plan.set_logprobs on) receives one list
+    per request, one entry per generated id.  chunk_rows / min_chunk_rows: ContinuousBatcher's chunked admission (0: off)."""
     if len(arrivals) != len(requests):
         raise ValueError(f"{len(requests)} requests but {len(arrivals)} arrival steps")
     if samplers is not None and len(samplers) != len(requests):
         raise ValueError(f"{len(requests)} requests but {len(samplers)} samplers")
     if any(a < 0 for a in arrivals):
         raise ValueError("arrival steps must be >= 0")
-    cb = ContinuousBatcher(plan, model_type, stop_tokens, max_tokens, context_length)
+    cb = ContinuousBatcher(plan, model_type, stop_tokens, max_tokens, context_length, chunk_rows, min_chunk_rows)
     order = sorted(range(len(requests)), key=lambda i: (arrivals[i], i))
     rid_of: dict = {}
     t_sub, t_first, t_done = [None] * len(requests), [None] * len(requests), [None] * len(requests)
-    rows, launches = [], []
+    rows, launches, kinds = [], [], []
     nxt, k = 0, 0
     while nxt < len(order) or cb.pending() or cb.running():
         while nxt < len(order) and arrivals[order[nxt]] <= k:
@@ -532,6 +566,7 @@ def generate_tokens_continuous(plan, model_type: str, requests: list, arrivals: 
         if cb.last_rows:
             rows.append(cb.last_rows)
             launches.append(plan.batch_info()[1])
+            kinds.append(cb.last_kind)
         for rid, tok, finished in events:
             i = rid_of[rid]
             if tok is not None and t_first[i] is None:
@@ -540,7 +575,7 @@ def generate_tokens_continuous(plan, model_type: str, requests: list, arrivals: 
                 t_done[i] = now
         k += 1
     if stats is not None:
-        stats.update(steps=len(rows), rows=rows, launches=launches, submitted=t_sub, first_token=t_first, done=t_done)
+        stats.update(steps=len(rows), rows=rows, launches=launches, kinds=kinds, submitted=t_sub, first_token=t_first, done=t_done)
     rids = sorted(rid_of, key=lambda r: rid_of[r])
     if logprobs is not None:
         logprobs.extend(cb.logprobs[rid] for rid in rids)

@@ -89,6 +89,8 @@ public final class B200MasterPlan implements AutoCloseable {
     private static final MethodHandle DECODE_BATCH = fn("b200_forward_decode_batch",
             FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
     private static final MethodHandle FORWARD_STEP = fn("b200_forward_step", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS));
+    private static final MethodHandle FORWARD_CHUNK = fn("b200_forward_chunk", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS));
+    private static final MethodHandle CHUNK_ROWS = fn("b200_chunk_rows", FunctionDescriptor.of(JAVA_INT, ADDRESS, ADDRESS));
     private static final MethodHandle SLOT_RESET = fn("b200_slot_reset", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT));
     private static final MethodHandle SLOT_COPY_KV = fn("b200_slot_copy_kv", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, JAVA_INT));
     private static final MethodHandle PREFILL_SLOTS = fn("b200_prefill_slots", FunctionDescriptor.of(JAVA_INT, ADDRESS, JAVA_INT, ADDRESS, ADDRESS, ADDRESS, ADDRESS));
@@ -407,6 +409,17 @@ public final class B200MasterPlan implements AutoCloseable {
      *  {temperature, topp, rng.nextFloat(1f)} of row i (temperature 0 = argmax).  Every row's K/V is written before any row attends,
      *  so each emitting row is bit-identical to forwardDecode / forwardDecodeSample of its own sequence (b200_forward_step). */
     public int[] forwardStep(int[] slots, int[] tokens, int[] positions, boolean[] emit, float[] sampling) throws Throwable {
+        return stepRows(FORWARD_STEP, slots, tokens, positions, emit, sampling);
+    }
+
+    /** forwardStep on the tensor cores: the same rows and ids, run as one chunk of the bit-exact int8 prefill (the plan's prefill
+     *  mode must be tensor_core_exact), so prompt rows ride in the chunk's GEMMs with the decode rows.  Up to chunkRows() rows, at
+     *  most 8 of them emitting (b200_forward_chunk). */
+    public int[] forwardChunk(int[] slots, int[] tokens, int[] positions, boolean[] emit, float[] sampling) throws Throwable {
+        return stepRows(FORWARD_CHUNK, slots, tokens, positions, emit, sampling);
+    }
+
+    private int[] stepRows(MethodHandle call, int[] slots, int[] tokens, int[] positions, boolean[] emit, float[] sampling) throws Throwable {
         try (Arena a = Arena.ofConfined()) {
             int n = tokens.length;
             MemorySegment rows = a.allocate(28L * Math.max(1, n), 4); // b200_step_row: 4 int32 + 3 float
@@ -420,7 +433,7 @@ public final class B200MasterPlan implements AutoCloseable {
                     rows.set(JAVA_FLOAT, o + 16 + 4L * k, sampling == null ? 0f : sampling[3 * i + k]);
             }
             MemorySegment ids = a.allocate(JAVA_INT, Math.max(1, n));
-            int rc = (int) FORWARD_STEP.invokeExact(plan, n, rows, ids, MemorySegment.NULL);
+            int rc = (int) call.invokeExact(plan, n, rows, ids, MemorySegment.NULL);
             if (rc != 0) check(rc, lastError());
             return ids.asSlice(0, 4L * n).toArray(JAVA_INT);
         }
@@ -469,6 +482,16 @@ public final class B200MasterPlan implements AutoCloseable {
         try (Arena a = Arena.ofConfined()) {
             MemorySegment r = a.allocate(JAVA_INT);
             int rc = (int) MULTI_ROWS.invokeExact(plan, r);
+            if (rc != 0) check(rc, lastError());
+            return r.get(JAVA_INT, 0);
+        }
+    }
+
+    /** Rows per forwardChunk call: prefill_batch_size in tensor_core_exact with decode slots, else 0 (b200_chunk_rows). */
+    public int chunkRows() throws Throwable {
+        try (Arena a = Arena.ofConfined()) {
+            MemorySegment r = a.allocate(JAVA_INT);
+            int rc = (int) CHUNK_ROWS.invokeExact(plan, r);
             if (rc != 0) check(rc, lastError());
             return r.get(JAVA_INT, 0);
         }

@@ -81,7 +81,7 @@ EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant", "b200_test_kq_tiles_to_q8",
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
-           "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_weight_info", "b200_test_set_memory_budget", "b200_stream_rings",
+           "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_forward_chunk", "b200_chunk_rows", "b200_weight_info", "b200_test_set_memory_budget", "b200_stream_rings",
            "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
@@ -144,6 +144,8 @@ def lib() -> C.CDLL:
     L.b200_forward_decode_multi.argtypes = [vp, i32, i32, vp, i32, vp, vp]
     L.b200_decode_multi_rows.argtypes = [vp, C.POINTER(i32)]
     L.b200_forward_step.argtypes = [vp, i32, C.POINTER(StepRow), vp, vp]
+    L.b200_forward_chunk.argtypes = [vp, i32, C.POINTER(StepRow), vp, vp]
+    L.b200_chunk_rows.argtypes = [vp, C.POINTER(i32)]
     L.b200_upload_info.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int64)]
     L.b200_weight_info.argtypes = [vp, C.POINTER(i32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.b200_test_set_memory_budget.argtypes = [C.c_int64]
@@ -647,6 +649,13 @@ class NativePlan:
     def forward_step(self, rows, logits: bool = False):
         """b200_forward_step: one mixed step.  rows: (slot, token, position, emit[, temperature, topp, uniform01]) per row.  Returns
         (ids int32 [n], -1 where emit is 0; logits float32 [n, vocab] or None, rows with emit 0 left unwritten)."""
+        return self._step_rows(lib().b200_forward_step, rows, logits)
+
+    def forward_chunk(self, rows, logits: bool = False):
+        """b200_forward_chunk: forward_step's rows and results, run as one chunk of the tensor_core_exact prefill."""
+        return self._step_rows(lib().b200_forward_chunk, rows, logits)
+
+    def _step_rows(self, fn, rows, logits):
         n = len(rows)
         arr = (StepRow * max(n, 1))()
         for i, r in enumerate(rows):
@@ -655,8 +664,13 @@ class NativePlan:
             arr[i] = StepRow(*[int(v) for v in r[:4]], *[float(v) for v in r[4:]])
         ids = np.empty(max(n, 1), dtype=np.int32)
         lg = np.zeros((n, self.cfg.vocab_size), dtype=np.float32) if logits else None
-        self._ck(lib().b200_forward_step(self._p, n, arr, ids.ctypes.data, lg.ctypes.data if logits else None))
+        self._ck(fn(self._p, n, arr, ids.ctypes.data, lg.ctypes.data if logits else None))
         return ids[:n], lg
+
+    def chunk_rows(self) -> int:
+        r = C.c_int32(0)
+        self._ck(lib().b200_chunk_rows(self._p, C.byref(r)))
+        return r.value
 
     def decode_multi_rows(self) -> int:
         r = C.c_int32(0)

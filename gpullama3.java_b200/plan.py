@@ -270,6 +270,17 @@ class B200MasterPlan:
         """Positions per forward_decode_multi step (8 at the 8B shapes); 0 where the plan cannot run it."""
         return self._native.decode_multi_rows()
 
+    def forward_chunk(self, rows, logits: bool = False):
+        """forward_step on the tensor cores -> (ids, logits [n, vocab] or None): the same row tuples and results, every emitting row
+        bit-identical to forward_decode of its sequence, run as one chunk of the tensor_core_exact prefill, so prompt rows of newly
+        admitted sequences ride in the chunk's GEMMs with the decode rows.  1 <= len(rows) <= chunk_rows(), at most 8 of them
+        emitting; needs set_prefill_mode("tensor_core_exact") and set_decode_slots."""
+        return self._native.forward_chunk(rows, logits)
+
+    def chunk_rows(self) -> int:
+        """Rows per forward_chunk call: prefill_batch_size in tensor_core_exact with decode slots; 0 where the plan cannot run it."""
+        return self._native.chunk_rows()
+
     def moe_routing(self):
         """Qwen2-MoE plans: (ids [layer, k], weights [layer, k + 1]) of the last step (selected experts in selection order, their
         routing weights, then the shared-expert weight)."""

@@ -296,7 +296,8 @@ int b200_score_tokens(b200_plan *plan, const int32_t *tokens, const int32_t *tar
  * b200_decode_info's and b200_batch_info's launch counts and b200_batch_info's device time are unchanged, while
  * b200_decode_sequence's device_ms includes the one launch per step.  Sampled rows are copied before the sampler turns them into
  * probabilities; the sampler reads the copy, so the ids equal those with logprobs off for the same uniform numbers.  The results
- * reach pinned host memory inside the call's own synchronise.  The table holds max(the plan's sequence capacity, 8) rows.
+ * reach pinned host memory inside the call's own synchronise.  The table holds max(the plan's sequence capacity, prefill_batch_size,
+ * 8) rows.  b200_forward_chunk fills one row per call row, as b200_forward_step does.
  * B200_ERR_BAD_ARG for top_n outside -1..20 or above vocab_size; B200_ERR_UNSUPPORTED on tensor-parallel plans (full logits are
  * not gathered). */
 #define B200_MAX_TOP_LOGPROBS 20
@@ -483,8 +484,28 @@ typedef struct b200_step_row {
 int b200_forward_step(b200_plan *plan, int32_t n, const b200_step_row *rows, int32_t *ids_out /* n; -1 where emit == 0 */,
                       float *logits /* nullable, n x vocab; rows with emit == 0 are not written */);
 
-/* Decode slots, kernels of the last batched step with a classifier (b200_forward_decode_batch, b200_forward_decode_multi or
- * b200_forward_step, whichever ran last) and its device milliseconds (CUDA events around the graph); any pointer may be NULL. */
+/* b200_forward_step on the tensor cores: the same rows and outputs, run as one chunk of the bit-exact int8 prefill
+ * (B200_PREFILL_TENSOR_CORE_EXACT), so prompt rows of newly admitted sequences and decode rows of running ones share the chunk's
+ * GEMMs.  Up to prefill_batch_size rows (b200_chunk_rows), at most B200_MAX_DECODE_SLOTS of them emitting; any mix of slots, a slot
+ * at several distinct positions.  The chunk runs the emitting rows first; their final residual rows then go through the batched
+ * step's classifier (final norm, Q8_0 lm_head stream, argmax), so each emitting row's logits are bit-identical to
+ * b200_forward_decode of that token at that position over the same slot prefix, whatever the chunk's length or the row's place in
+ * it, and its id, sampling controls, log-probabilities (one row per call row) and counts are b200_forward_step's.  Only the named
+ * (slot, position) K/V rows are written; the plan's own cache, its single-token buffers and the other slots are not touched.
+ * b200_batch_info reports the call (its launches, and CUDA events around the chunk and the classifier); b200_prefill_info is left
+ * alone.  One synchronise per call.
+ * B200_ERR_UNSUPPORTED with the reason on plans that cannot run it (FP16, tensor-parallel, Qwen2-MoE, resident K-quant, created
+ * without a prefill batch size, or a shape the int8 prefill refuses); B200_ERR_STATE without decode slots or when the prefill mode
+ * is not tensor_core_exact (the message names the mode); B200_ERR_BAD_ARG naming the row for: n outside 1..prefill_batch_size,
+ * more emitting rows than b200_decode_multi_rows, and every refusal of b200_forward_step's rows. */
+int b200_forward_chunk(b200_plan *plan, int32_t n, const b200_step_row *rows, int32_t *ids_out /* n; -1 where emit == 0 */,
+                       float *logits /* nullable, n x vocab; rows with emit == 0 are not written */);
+/* Rows per b200_forward_chunk call: prefill_batch_size when the call can run (tensor_core_exact and decode slots), else 0. */
+int b200_chunk_rows(b200_plan *plan, int32_t *max_rows);
+
+/* Decode slots, kernels of the last batched step with a classifier (b200_forward_decode_batch, b200_forward_decode_multi,
+ * b200_forward_step or b200_forward_chunk, whichever ran last) and its device milliseconds (CUDA events around the graph, or around
+ * the chunk and its classifier); any pointer may be NULL. */
 int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_step, float *device_ms_last_step);
 
 /* Test/diagnostic read-back of a named device buffer into host memory.  Names:

@@ -125,7 +125,7 @@ struct b200_plan {
     int *seq_tokens = nullptr, *out_ids = nullptr;
     int seq_cap = 0;
     StepState *h_st = nullptr; // pinned
-    int *h_ids = nullptr;      // pinned, seq_cap
+    int *h_ids = nullptr;      // pinned, seq_cap (also the single-token calls' step_outputs block, 9 ints)
 
     TokenGraphs graph; // the multi-kernel decode graph (round 1)
     TokenGraphs pers;  // one persistent kernel per token (decode_persistent.cuh)
@@ -189,7 +189,7 @@ struct b200_plan {
         int *part_idx = nullptr, *ids = nullptr, *smp_out = nullptr;
         unsigned *blk_cnt = nullptr;
         BatchRows *rows = nullptr, *h_rows = nullptr; // device / pinned host
-        int *h_out = nullptr;                         // pinned: ids [SMB_MAX_ROWS] then sampler outputs [SMB_MAX_ROWS][8]
+        int *h_out = nullptr;                         // pinned: step_outputs' readback block, 9 ints a row
         // the exact prefills: the per-step rows of the call [context_length], the device step index
         BatchRows *sched = nullptr;
         int *step = nullptr;
@@ -1236,23 +1236,28 @@ int multi_ready(b200_plan *p) {
     return rc;
 }
 
-// Enqueues the steps of one call back to back without the classifier: the schedule is uploaded once and k_batch_rows_next
-// feeds each step its entry, so the caller synchronises once.  p->ev0 / ev1 bracket the steps.  own: every row writes the plan's
-// cache (slot 0) instead of the decode slots.
-int run_steps(b200_plan *p, const std::vector<BatchRows> &sched, const std::vector<int> &nrows, bool own, int *launches) {
+// Enqueues the steps of one call back to back: the schedule is uploaded once and k_batch_rows_next feeds each step its entry, so
+// the caller synchronises once.  p->ev0 / ev1 bracket the steps.  own: every row writes the plan's cache (slot 0) instead of the
+// decode slots.  Without scored the steps run no classifier; with it every row of every step runs it, and scored(s, r0) enqueues
+// after step s, whose rows are the call's rows from r0 on, the work that reads its logits.
+template <typename Scored = std::nullptr_t>
+int run_steps(b200_plan *p, const std::vector<BatchRows> &sched, const std::vector<int> &nrows, bool own, int *launches, Scored scored = nullptr) {
+    constexpr bool classify = !std::is_same_v<Scored, std::nullptr_t>;
     auto &B = p->bt;
     const int steps = (int)sched.size();
     std::vector<const Graph *> graphs(steps);
     int rc;
     for (int s = 0; s < steps; s++)
-        if ((rc = batch_graph(p, SCHED | step_form(sched[s], nrows[s], own), nrows[s], 0, &graphs[s]))) return rc;
+        if ((rc = batch_graph(p, SCHED | step_form(sched[s], nrows[s], own), nrows[s], classify ? nrows[s] : 0, &graphs[s]))) return rc;
     CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
     CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
     CK(cudaEventRecord(p->ev0, p->stream));
     int k = 0;
-    for (const Graph *g : graphs) {
-        CK(cudaGraphLaunch(g->exec, p->stream));
-        k += g->launches;
+    for (int s = 0, r0 = 0; s < steps; r0 += nrows[s++]) {
+        CK(cudaGraphLaunch(graphs[s]->exec, p->stream));
+        k += graphs[s]->launches;
+        if constexpr (classify)
+            if ((rc = scored(s, r0))) return rc;
     }
     CK(cudaEventRecord(p->ev1, p->stream));
     if (launches) *launches = k;
@@ -1324,7 +1329,6 @@ int set_smem_attrs(b200_plan *p) {
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_moe_gateup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_moe_down, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
-    CK(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     CK(cudaFuncSetAttribute(k_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     CK(cudaFuncSetAttribute(k_sample_ctl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     done = true;
@@ -2390,29 +2394,6 @@ const TokenGraphs &active_graphs(const b200_plan *p) { return p->decode_mode == 
 cudaGraphExec_t decode_graph(const b200_plan *p) { return active_graphs(p).decode.exec; }
 cudaGraphExec_t prefill_graph(const b200_plan *p) { return active_graphs(p).prefill.exec; }
 
-// The device sampler (sampler.cuh) on one logits row: the token at out[0], its four diagnostics at out[1..4].
-int launch_sample(b200_plan *p, float *logits, float temperature, float topp, float uniform01, int *out) {
-    SamplerArgs a;
-    a.logits = logits; a.n = p->cfg.vocab_size; a.temperature = temperature; a.topp = topp; a.r01 = uniform01;
-    a.indices = p->smp_indices; a.out_id = out; a.info = out + 1;
-    k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
-    CK(cudaGetLastError());
-    return B200_OK;
-}
-
-// The device sampler on the logits rows row[j], j < m, of the batch's layout (bt.logits, or its logprobs copy lp.smp), one block per row in one launch: row r's token at
-// bt.smp_out[8 r], its diagnostics after it.
-int launch_sample_rows(b200_plan *p, float *logits, int m, const int *row, const float *temperature, const float *topp, const float *uniform01) {
-    static_assert(SMB_MAX_ROWS <= SAMPLER_MAX_ROWS, "k_sample_rows takes every row of a batched step");
-    SamplerRowsArgs a;
-    a.logits = logits; a.stride = sampler_padded(p->cfg.vocab_size); a.n = p->cfg.vocab_size;
-    a.indices = p->bt.smp_indices; a.out = p->bt.smp_out;
-    for (int j = 0; j < m; j++) { a.row[j] = row[j]; a.temperature[j] = temperature[j]; a.topp[j] = topp[j]; a.r01[j] = uniform01[j]; }
-    k_sample_rows<<<m, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
-    CK(cudaGetLastError());
-    return B200_OK;
-}
-
 // The checks b200_set_sampling_controls and b200_test_sample_controls share (p may be NULL).
 int check_controls(b200_plan *p, const b200_sampling_controls &c, int vocab) {
     if (c.top_k < 0 || c.top_k > vocab) return fail(p, B200_ERR_BAD_ARG, "top_k = %d outside [0, %d]", c.top_k, vocab);
@@ -2448,17 +2429,6 @@ SampleCtlRow ctl_row(b200_plan *p, int s, const float *src, float *dst, int *ind
     return r;
 }
 
-int launch_sample_ctl(b200_plan *p, int m, const SampleCtlRow *rows) {
-    static_assert(SMB_MAX_ROWS <= SAMPLER_MAX_ROWS, "k_sample_ctl takes every row of a batched step");
-    static_assert(B200_MAX_LOGIT_BIAS == SAMPLER_CTL_MAX_BIAS, "the header's limit is the kernel's");
-    SampleCtlArgs a;
-    a.n = p->cfg.vocab_size;
-    for (int j = 0; j < m; j++) a.row[j] = rows[j];
-    k_sample_ctl<<<m, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(a);
-    CK(cudaGetLastError());
-    return B200_OK;
-}
-
 // Zero the counts of sequences [s0, s1) if the tables exist (on the plan's stream; the caller synchronises).
 int clear_counts(b200_plan *p, int s0, int s1) {
     if (p->ctl.cnt) CK(cudaMemsetAsync(p->ctl.cnt + (size_t)s0 * p->cfg.vocab_size, 0, (size_t)(s1 - s0) * p->cfg.vocab_size * 4, p->stream));
@@ -2477,7 +2447,7 @@ int launch_logprobs(b200_plan *p, const float *logits, long long stride, int n, 
     return B200_OK;
 }
 
-// One row of the single-token calls: p->logits, the id at *id, result row `row`.
+// One step of b200_decode_sequence: p->logits, the id at *id, result row `row`.
 int launch_logprobs_one(b200_plan *p, const int *id, int row) { return launch_logprobs(p, p->logits, 0, 1, &id, &row); }
 
 // The result rows [0, n) to the pinned table; the caller's synchronise completes the copy.
@@ -2529,6 +2499,28 @@ int check_row(b200_plan *p, int i, const b200_step_row &r) {
     return B200_OK;
 }
 
+// The refusals b200_forward_step and b200_forward_chunk share, for the first offending row: an emit flag other than 0 / 1, check_row,
+// a (slot, position) pair that repeats, more than max_emit emitting rows, and a second emitting row of a slot with sampling controls.
+int check_step_rows(b200_plan *p, int n, const b200_step_row *rows, int max_emit) {
+    int rc, e = 0, emits[SMB_MAX_ROWS]; // emits[s]: the first emitting row of slot s, or -1
+    for (int s = 0; s < SMB_MAX_ROWS; s++) emits[s] = -1;
+    std::unordered_map<long long, int> seen; // slot * context_length + position -> row
+    for (int i = 0; i < n; i++) {
+        const b200_step_row &r = rows[i];
+        if (r.emit != 0 && r.emit != 1) return fail(p, B200_ERR_BAD_ARG, "row %d: emit must be 0 or 1 (got %d)", i, r.emit);
+        if ((rc = check_row(p, i, r))) return rc;
+        const auto at = seen.emplace((long long)r.slot * p->cfg.context_length + r.position, i);
+        if (!at.second) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d position %d repeats row %d's", i, r.slot, r.position, at.first->second);
+        if (!r.emit) continue;
+        if (++e > max_emit) return fail(p, B200_ERR_BAD_ARG, "row %d: more than %d emitting rows in one call", i, max_emit);
+        if (emits[r.slot] >= 0 && p->ctl.on[r.slot + 1])
+            return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d has sampling controls and already emits in row %d (its counts would depend on "
+                                             "that row's id)", i, r.slot, emits[r.slot]);
+        if (emits[r.slot] < 0) emits[r.slot] = i;
+    }
+    return B200_OK;
+}
+
 // The emitting rows first (stable), then the others: order[k] = the caller's index of step row k; returns the emitting rows' count.
 int emit_first(int n, const b200_step_row *rows, int *order) {
     int e = 0;
@@ -2539,51 +2531,69 @@ int emit_first(int n, const b200_step_row *rows, int *order) {
     return e;
 }
 
-// What a step with the classifier does after it, for b200_forward_step and b200_forward_chunk alike: bt.logits / bt.ids rows [0, e)
-// hold the emitting rows (step row k is the caller's row order[k], order from emit_first over n rows).  Their logits go back to the
-// caller's row order, ids -1 where a row does not emit.  Rows with a temperature run the device sampler, all in one launch.  With
-// controls, the emitting rows of slots with sampling controls run k_sample_ctl instead, all in one launch of their own.  Then the
-// log-probabilities, the readback and the call's one synchronise.
-int step_outputs(b200_plan *p, int n, const b200_step_row *rows, const int *order, int e, bool controls, int32_t *ids_out, float *logits) {
+// The buffers step_outputs works on: logits rows sampler_padded(vocab) floats apart and their argmax ids, the sampler's outputs
+// (8 ints a row: the id, then its four diagnostics) and candidate lists (vocab ints a row), and a pinned block of 9 ints a row
+// that receives the e ids, then the e rows of sampler outputs.  The batched steps pass bt's, the single-token calls the plan's own.
+struct RowBufs {
+    float *logits;
+    int *ids, *smp_out, *smp_indices, *h_out;
+};
+
+// What a step with the classifier does after it, for every emitting call but b200_decode_sequence: R's rows [0, e) hold the
+// emitting rows (step row k is the caller's row order[k], order from emit_first over n rows).  Their logits go back to the caller's
+// row order, ids -1 where a row does not emit.  Rows with a temperature run the device sampler, all in one launch.  With controls,
+// the emitting rows of sequences with sampling controls (slot + 1; slot -1 is the plan's own) run k_sample_ctl instead, all in one
+// launch of their own.  Then the log-probabilities, the readback and the call's one synchronise.  info_out (nullable, 4 ints per
+// caller row): an emitting row's sampler diagnostics, zeros where it takes the argmax.
+int step_outputs(b200_plan *p, int n, const b200_step_row *rows, const int *order, int e, bool controls, const RowBufs &R, int32_t *ids_out,
+                 float *logits, int32_t *info_out = nullptr) {
+    static_assert(SMB_MAX_ROWS <= SAMPLER_MAX_ROWS, "k_sample_rows and k_sample_ctl take every row of a batched step");
+    static_assert(B200_MAX_LOGIT_BIAS == SAMPLER_CTL_MAX_BIAS, "the header's limit is the kernel's");
     const b200_config &c = p->cfg;
-    auto &B = p->bt;
     int rc;
     const size_t vpad = (size_t)sampler_padded(c.vocab_size);
     if (logits) // before the sampler turns sampled rows into probabilities
         for (int k = 0; k < e; k++)
-            CK(cudaMemcpyAsync(logits + (size_t)order[k] * c.vocab_size, B.logits + k * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
-    int m = 0, mc = 0, srow[SMB_MAX_ROWS];
+            CK(cudaMemcpyAsync(logits + (size_t)order[k] * c.vocab_size, R.logits + k * vpad, (size_t)c.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
+    int m = 0, mc = 0;
     bool ctl[SMB_MAX_ROWS];
-    float t[SMB_MAX_ROWS], tp[SMB_MAX_ROWS], u[SMB_MAX_ROWS];
-    SampleCtlRow crow[SMB_MAX_ROWS];
+    SamplerRowsArgs sa;
+    SampleCtlArgs ca;
     for (int k = 0; k < e; k++) {
         const b200_step_row &r = rows[order[k]];
         ctl[k] = controls && p->ctl.on[r.slot + 1];
         if (ctl[k]) {
-            crow[mc++] = ctl_row(p, r.slot + 1, B.logits + k * vpad, p->ctl.rows + k * vpad, B.smp_indices + (size_t)k * c.vocab_size, B.smp_out + 8 * k,
-                                 r.temperature, r.topp, r.uniform01);
+            ca.row[mc++] = ctl_row(p, r.slot + 1, R.logits + k * vpad, p->ctl.rows + k * vpad, R.smp_indices + (size_t)k * c.vocab_size, R.smp_out + 8 * k,
+                                   r.temperature, r.topp, r.uniform01);
             continue;
         }
         if (r.temperature == 0.0f) continue; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed
-        srow[m] = k; t[m] = r.temperature; tp[m] = r.topp; u[m] = r.uniform01;
+        sa.row[m] = k; sa.temperature[m] = r.temperature; sa.topp[m] = r.topp; sa.r01[m] = r.uniform01;
         m++;
     }
-    if (mc && (rc = launch_sample_ctl(p, mc, crow))) return rc;
-    const bool lp = p->lp.top_n >= 0;
-    float *smp = B.logits;
-    if (lp && m) { // the sampler overwrites its rows with probabilities: it samples copies (zero pad included) in the same layout
-        smp = p->lp.smp;
-        for (int j = 0; j < m; j++) CK(cudaMemcpyAsync(smp + srow[j] * vpad, B.logits + srow[j] * vpad, vpad * 4, cudaMemcpyDeviceToDevice, p->stream));
+    if (mc) {
+        ca.n = c.vocab_size;
+        k_sample_ctl<<<mc, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(ca);
+        CK(cudaGetLastError());
     }
-    if (m && (rc = launch_sample_rows(p, smp, m, srow, t, tp, u))) return rc;
+    const bool lp = p->lp.top_n >= 0;
+    sa.logits = R.logits; sa.stride = (int)vpad; sa.n = c.vocab_size; sa.indices = R.smp_indices; sa.out = R.smp_out;
+    if (lp && m) { // the sampler overwrites its rows with probabilities: it samples copies (zero pad included) in the same layout
+        sa.logits = p->lp.smp;
+        for (int j = 0; j < m; j++) CK(cudaMemcpyAsync(sa.logits + sa.row[j] * vpad, R.logits + sa.row[j] * vpad, vpad * 4, cudaMemcpyDeviceToDevice, p->stream));
+    }
+    if (m) {
+        k_sample_rows<<<m, SAMPLER_THREADS, sampler_smem_bytes(), p->stream>>>(sa);
+        CK(cudaGetLastError());
+    }
     if (lp && e) {
         const int *ids[SMB_MAX_ROWS];
-        for (int k = 0; k < e; k++) ids[k] = ctl[k] || rows[order[k]].temperature != 0.0f ? B.smp_out + 8 * k : B.ids + k;
-        if ((rc = launch_logprobs(p, B.logits, (long long)vpad, e, ids, order))) return rc;
+        for (int k = 0; k < e; k++) ids[k] = ctl[k] || rows[order[k]].temperature != 0.0f ? R.smp_out + 8 * k : R.ids + k;
+        if ((rc = launch_logprobs(p, R.logits, (long long)vpad, e, ids, order))) return rc;
     }
     if (lp && (rc = copy_logprobs(p, n))) return rc;
-    if (e) CK(cudaMemcpyAsync(B.h_out, B.ids, (size_t)e * 4, cudaMemcpyDeviceToHost, p->stream));
-    if (m || mc) CK(cudaMemcpyAsync(B.h_out + SMB_MAX_ROWS, B.smp_out, (size_t)e * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
+    if (e) CK(cudaMemcpyAsync(R.h_out, R.ids, (size_t)e * 4, cudaMemcpyDeviceToHost, p->stream));
+    if (m || mc) CK(cudaMemcpyAsync(R.h_out + e, R.smp_out, (size_t)e * 8 * 4, cudaMemcpyDeviceToHost, p->stream));
     CK(cudaStreamSynchronize(p->stream));
     if (lp) {
         for (int k = e; k < n; k++) { // rows that do not emit
@@ -2594,7 +2604,12 @@ int step_outputs(b200_plan *p, int n, const b200_step_row *rows, const int *orde
         p->lp.rows = n;
     }
     for (int i = 0; i < n; i++) ids_out[i] = -1;
-    for (int k = 0; k < e; k++) ids_out[order[k]] = ctl[k] || rows[order[k]].temperature != 0.0f ? B.h_out[SMB_MAX_ROWS + 8 * k] : B.h_out[k];
+    for (int k = 0; k < e; k++) {
+        const bool sampled = ctl[k] || rows[order[k]].temperature != 0.0f;
+        ids_out[order[k]] = sampled ? R.h_out[e + 8 * k] : R.h_out[k];
+        if (info_out)
+            for (int d = 0; d < 4; d++) info_out[4 * order[k] + d] = rows[order[k]].temperature != 0.0f ? R.h_out[e + 8 * k + 1 + d] : 0;
+    }
     return B200_OK;
 }
 
@@ -2618,7 +2633,7 @@ int batch_step(b200_plan *p, int n, const b200_step_row *rows, bool own, bool co
     CK(cudaEventRecord(p->ev0, p->stream));
     CK(cudaGraphLaunch(g->exec, p->stream));
     CK(cudaEventRecord(p->ev1, p->stream));
-    if ((rc = step_outputs(p, n, rows, order, e, controls, ids_out, logits))) return rc;
+    if ((rc = step_outputs(p, n, rows, order, e, controls, RowBufs{B.logits, B.ids, B.smp_out, B.smp_indices, B.h_out}, ids_out, logits))) return rc;
     CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
     B.last_launches = g->launches;
     return B200_OK;
@@ -2648,10 +2663,22 @@ int chunk_step(b200_plan *p, int n, const b200_step_row *rows, int32_t *ids_out,
         nl += CLASSIFIER_LAUNCHES;
     }
     CK(cudaEventRecord(p->ev1, p->stream));
-    if ((rc = step_outputs(p, n, rows, order.data(), e, true, ids_out, logits))) return rc;
+    if ((rc = step_outputs(p, n, rows, order.data(), e, true, RowBufs{B.logits, B.ids, B.smp_out, B.smp_indices, B.h_out}, ids_out, logits))) return rc;
     CK(cudaEventElapsedTime(&B.last_ms, p->ev0, p->ev1));
     B.last_launches = nl;
     return B200_OK;
+}
+
+// b200_forward_decode and b200_forward_decode_sample over a checked row r of slot -1: the single-token decode graph, then
+// step_outputs on its one row in the plan's own buffers (h_ids as the readback block).
+int decode_one(b200_plan *p, const b200_step_row &r, bool controls, int32_t *id, float *logits, int32_t *info) {
+    CK(cudaSetDevice(p->device));
+    int rc;
+    if ((rc = set_state(p, r.token, r.position, 0, 0))) return rc;
+    CK(cudaGraphLaunch(decode_graph(p), p->stream));
+    const int order = 0;
+    if ((rc = step_outputs(p, 1, &r, &order, 1, controls, RowBufs{p->logits, p->out_ids, p->smp_out, p->smp_indices, p->h_ids}, id, logits, info))) return rc;
+    return check_device_error(p);
 }
 
 // ---- b200_score_tokens (score.cuh) ----------------------------------------------------------------------------------------------
@@ -2706,24 +2733,16 @@ int score_init_i8(b200_plan *p) {
 // exact mode on a plan that runs multi-position steps: steps of batch_max_rows rows with the classifier on every row, each followed
 // by k_score_rows over its logits rows.  The schedule is uploaded once (k_batch_rows_next feeds each step its rows).
 int score_multi(b200_plan *p, const int32_t *tokens, int n, int start_pos) {
-    auto &B = p->bt;
     int rc;
     if ((rc = multi_ready(p))) return rc;
     std::vector<BatchRows> sched;
     std::vector<int> nrows;
     pack_rows(sched, nrows, batch_max_rows(p), tokens, start_pos, n, 0);
-    const int steps = (int)sched.size();
-    std::vector<const Graph *> graphs(steps);
-    for (int k = 0; k < steps; k++)
-        if ((rc = batch_graph(p, SCHED | step_form(sched[k], nrows[k], true), nrows[k], nrows[k], &graphs[k]))) return rc;
-    CK(cudaMemcpyAsync(B.sched, sched.data(), (size_t)steps * sizeof(BatchRows), cudaMemcpyHostToDevice, p->stream));
-    CK(cudaMemsetAsync(B.step, 0, 4, p->stream));
-    for (int k = 0, r0 = 0; k < steps; r0 += nrows[k++]) {
-        CK(cudaGraphLaunch(graphs[k]->exec, p->stream));
-        k_score_rows<<<nrows[k], SCORE_THREADS, 0, p->stream>>>(B.logits, sampler_padded(p->cfg.vocab_size), p->cfg.vocab_size, p->sc.tgt + r0, p->sc.out + r0);
+    return run_steps(p, sched, nrows, true, nullptr, [&](int s, int r0) {
+        k_score_rows<<<nrows[s], SCORE_THREADS, 0, p->stream>>>(p->bt.logits, sampler_padded(p->cfg.vocab_size), p->cfg.vocab_size, p->sc.tgt + r0, p->sc.out + r0);
         CK(cudaGetLastError());
-    }
-    return B200_OK;
+        return B200_OK;
+    });
 }
 
 // exact mode on every other single-GPU plan: the single-token decode graph per position (it computes p->logits), each followed by
@@ -2885,19 +2904,10 @@ int b200_forward_decode(b200_plan *p, int32_t token, int32_t position, float *lo
     if (!p) return B200_ERR_BAD_ARG;
     if (!p->graph.decode.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     if (logits && p->tp.n > 1) return fail(p, B200_ERR_UNSUPPORTED, "full logits are not gathered under tensor parallelism (argmax is)");
-    int rc;
+    int rc, id;
     if ((rc = check_pos(p, token, position))) return rc;
-    CK(cudaSetDevice(p->device));
-    if ((rc = set_state(p, token, position, 0, 0))) return rc;
-    CK(cudaGraphLaunch(decode_graph(p), p->stream));
-    const bool lp = p->lp.top_n >= 0;
-    if (lp && ((rc = launch_logprobs_one(p, p->out_ids, 0)) || (rc = copy_logprobs(p, 1)))) return rc;
-    if (argmax) CK(cudaMemcpyAsync(p->h_ids, p->out_ids, 4, cudaMemcpyDeviceToHost, p->stream));
-    if (logits) CK(cudaMemcpyAsync(logits, p->logits, (size_t)p->cfg.vocab_size * 4, cudaMemcpyDeviceToHost, p->stream));
-    CK(cudaStreamSynchronize(p->stream));
-    if ((rc = check_device_error(p))) return rc;
-    if (lp) p->lp.rows = 1;
-    if (argmax) *argmax = p->h_ids[0];
+    if ((rc = decode_one(p, b200_step_row{-1, token, position, 1, 0.0f, 0.0f, 0.0f}, false, &id, logits, nullptr))) return rc; // sequence 0's controls stay unused
+    if (argmax) *argmax = id;
     return B200_OK;
 }
 
@@ -2906,33 +2916,10 @@ int b200_forward_decode_sample(b200_plan *p, int32_t token, int32_t position, fl
     if (!p->graph.decode.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
     if (p->tp.n > 1) return fail(p, B200_ERR_UNSUPPORTED, "the device-side temperature/top-p sampler needs the whole logits row on one GPU (tensor-parallel plans sample greedily)");
     if (!(temperature >= 0.0f) || !(uniform01 >= 0.0f && uniform01 < 1.0f)) return fail(p, B200_ERR_BAD_ARG, "temperature must be >= 0 and the uniform number in [0, 1)");
-    int rc;
+    int rc, id;
     if ((rc = check_pos(p, token, position))) return rc;
-    CK(cudaSetDevice(p->device));
-    if ((rc = set_state(p, token, position, 0, 0))) return rc;
-    CK(cudaGraphLaunch(decode_graph(p), p->stream));
-    const bool greedy = temperature == 0.0f; // Sampler.selectSampler: temperature 0 -> FloatTensor.argmax, already computed by the forward
-    const bool lp = p->lp.top_n >= 0;
-    const bool ctl = p->ctl.on[0];
-    if (ctl) { // the controls modify a copy of the row: the raw logits stay for the logprobs
-        const SampleCtlRow r = ctl_row(p, 0, p->logits, p->ctl.rows, p->smp_indices, p->smp_out, temperature, topp, uniform01);
-        if ((rc = launch_sample_ctl(p, 1, &r))) return rc;
-        CK(cudaMemcpyAsync(p->h_ids, p->smp_out, 5 * 4, cudaMemcpyDeviceToHost, p->stream));
-    } else if (!greedy) {
-        float *row = p->logits;
-        if (lp) { // the sampler overwrites its row with probabilities: it samples a copy (zero pad included)
-            row = p->lp.smp;
-            CK(cudaMemcpyAsync(row, p->logits, (size_t)sampler_padded(p->cfg.vocab_size) * 4, cudaMemcpyDeviceToDevice, p->stream));
-        }
-        if ((rc = launch_sample(p, row, temperature, topp, uniform01, p->smp_out))) return rc;
-        CK(cudaMemcpyAsync(p->h_ids, p->smp_out, 5 * 4, cudaMemcpyDeviceToHost, p->stream));
-    } else CK(cudaMemcpyAsync(p->h_ids, p->out_ids, 4, cudaMemcpyDeviceToHost, p->stream));
-    if (lp && ((rc = launch_logprobs_one(p, greedy && !ctl ? p->out_ids : p->smp_out, 0)) || (rc = copy_logprobs(p, 1)))) return rc;
-    CK(cudaStreamSynchronize(p->stream));
-    if ((rc = check_device_error(p))) return rc;
-    if (lp) p->lp.rows = 1;
-    *token_out = p->h_ids[0];
-    if (info) for (int k = 0; k < 4; k++) info[k] = greedy ? 0 : p->h_ids[1 + k];
+    if ((rc = decode_one(p, b200_step_row{-1, token, position, 1, temperature, topp, uniform01}, true, &id, nullptr, info))) return rc;
+    *token_out = id;
     return B200_OK;
 }
 
@@ -3312,19 +3299,7 @@ int b200_forward_step(b200_plan *p, int32_t n, const b200_step_row *rows, int32_
     const int R = batch_max_rows(p);
     if (n < 1 || n > R) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (b200_decode_multi_rows)", n, R);
     int rc;
-    for (int i = 0; i < n; i++) {
-        const b200_step_row &r = rows[i];
-        if (r.emit != 0 && r.emit != 1) return fail(p, B200_ERR_BAD_ARG, "row %d: emit must be 0 or 1 (got %d)", i, r.emit);
-        if ((rc = check_row(p, i, r))) return rc;
-        for (int j = 0; j < i; j++)
-            if (rows[j].slot == r.slot && rows[j].position == r.position)
-                return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d position %d repeats row %d's", i, r.slot, r.position, j);
-        if (r.emit && p->ctl.on[r.slot + 1])
-            for (int j = 0; j < i; j++)
-                if (rows[j].emit && rows[j].slot == r.slot)
-                    return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d has sampling controls and already emits in row %d (its counts would depend on "
-                                                     "that row's id)", i, r.slot, j);
-    }
+    if ((rc = check_step_rows(p, n, rows, R))) return rc;
     CK(cudaSetDevice(p->device));
     return batch_step(p, n, rows, false, true, ids_out, logits);
 }
@@ -3357,23 +3332,8 @@ int b200_forward_chunk(b200_plan *p, int32_t n, const b200_step_row *rows, int32
     }
     if (!rows || !ids_out) return fail(p, B200_ERR_BAD_ARG, "rows and ids_out must not be NULL");
     if (n < 1 || n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (b200_chunk_rows)", n, p->prefill_batch);
-    const int max_emit = batch_max_rows(p); // the batched classifier's rows
-    int rc, e = 0, emits[SMB_MAX_ROWS];     // emits[s]: the first emitting row of slot s, or -1
-    for (int s = 0; s < SMB_MAX_ROWS; s++) emits[s] = -1;
-    std::unordered_map<long long, int> seen; // slot * context_length + position -> row
-    for (int i = 0; i < n; i++) {
-        const b200_step_row &r = rows[i];
-        if (r.emit != 0 && r.emit != 1) return fail(p, B200_ERR_BAD_ARG, "row %d: emit must be 0 or 1 (got %d)", i, r.emit);
-        if ((rc = check_row(p, i, r))) return rc;
-        const auto at = seen.emplace((long long)r.slot * p->cfg.context_length + r.position, i);
-        if (!at.second) return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d position %d repeats row %d's", i, r.slot, r.position, at.first->second);
-        if (!r.emit) continue;
-        if (++e > max_emit) return fail(p, B200_ERR_BAD_ARG, "row %d: more than %d emitting rows in one call", i, max_emit);
-        if (emits[r.slot] >= 0 && p->ctl.on[r.slot + 1])
-            return fail(p, B200_ERR_BAD_ARG, "row %d: slot %d has sampling controls and already emits in row %d (its counts would depend on "
-                                             "that row's id)", i, r.slot, emits[r.slot]);
-        if (emits[r.slot] < 0) emits[r.slot] = i;
-    }
+    int rc;
+    if ((rc = check_step_rows(p, n, rows, batch_max_rows(p)))) return rc; // at most the batched classifier's rows emit
     CK(cudaSetDevice(p->device));
     return chunk_step(p, n, rows, ids_out, logits);
 }
@@ -3800,11 +3760,11 @@ int b200_test_sample(const float *logits, int32_t n, float temperature, float to
     // the index scratch starts as 0xFF bytes: a slot the kernel did not write in this call reads as -1
     if (s.alloc(&dl, padded) && s.alloc(&di, (size_t)n * 4) && s.alloc(&dout, 8 * 4) && s.ok(cudaMemset(dl, 0, padded)) &&
         s.ok(cudaMemcpy(dl, logits, (size_t)n * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemset(di, 0xFF, (size_t)n * 4)) && s.ok(cudaMemset(dout, 0xFF, 8 * 4)) &&
-        s.ok(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()))) {
-        SamplerArgs a;
-        a.logits = dl; a.n = n; a.temperature = temperature; a.topp = topp; a.r01 = uniform01;
-        a.indices = di; a.out_id = dout; a.info = dout + 1;
-        k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(a);
+        s.ok(cudaFuncSetAttribute(k_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()))) {
+        SamplerRowsArgs a;
+        a.logits = dl; a.stride = 0; a.n = n; a.indices = di; a.out = dout;
+        a.row[0] = 0; a.temperature[0] = temperature; a.topp[0] = topp; a.r01[0] = uniform01;
+        k_sample_rows<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(a);
         int32_t h[5];
         if (s.ok(cudaGetLastError()) && s.ok(cudaDeviceSynchronize()) && s.ok(cudaMemcpy(h, dout, 5 * 4, cudaMemcpyDeviceToHost))) {
             *token_out = h[0];
@@ -3853,7 +3813,7 @@ int b200_time_sample_controls(const float *logits, int32_t n, const int32_t *cou
     if (!logits || !counts || !c || !ctl_ms || !plain_ms || n < 1 || reps < 1) return B200_ERR_BAD_ARG;
     if (!(temperature > 0.0f) || !(uniform01 >= 0.0f && uniform01 < 1.0f)) return B200_ERR_BAD_ARG;
     if (check_controls(nullptr, *c, n)) return B200_ERR_BAD_ARG;
-    // k_sample turns its row into probabilities and k_sample_ctl counts its id: every launch, the warm-up's included, gets its own copy
+    // k_sample_rows turns its row into probabilities and k_sample_ctl counts its id: every launch, the warm-up's included, gets its own copy
     const size_t pad = (size_t)sampler_padded(n), copies = (size_t)reps + 1, nb = (size_t)(c->n_bias ? c->n_bias : 1) * 4;
     float *dl = nullptr, *drow = nullptr, *dbv = nullptr;
     int *dcnt = nullptr, *di = nullptr, *dout = nullptr, *dbi = nullptr;
@@ -3864,7 +3824,7 @@ int b200_time_sample_controls(const float *logits, int32_t n, const int32_t *cou
           s.ok(cudaMemcpy(dl, logits, (size_t)n * 4, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dcnt, counts, (size_t)n * 4, cudaMemcpyHostToDevice)) &&
           (!c->n_bias || (s.ok(cudaMemcpy(dbi, c->bias_ids, nb, cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dbv, c->bias_values, nb, cudaMemcpyHostToDevice)))) &&
           s.ok(cudaFuncSetAttribute(k_sample_ctl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes())) &&
-          s.ok(cudaFuncSetAttribute(k_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes())) &&
+          s.ok(cudaFuncSetAttribute(k_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes())) &&
           s.ok(cudaEventCreate(&e0)) && s.ok(cudaEventCreate(&e1)) && s.ok(cudaEventCreate(&e2))))
         return s.rc;
     for (size_t r = 1; r < copies && s.rc == B200_OK; r++)
@@ -3877,11 +3837,12 @@ int b200_time_sample_controls(const float *logits, int32_t n, const int32_t *cou
         w.dst = drow; w.row_out = nullptr; w.bias_id = dbi; w.bias_val = dbv; w.n_bias = c->n_bias;
         w.top_k = c->top_k; w.min_p_log = min_p_log(c->min_p); w.rep = c->repetition_penalty; w.freq = c->frequency_penalty; w.pres = c->presence_penalty;
         w.temperature = temperature; w.topp = topp; w.r01 = uniform01; w.indices = di; w.out = dout;
-        SamplerArgs b;
-        b.n = n; b.temperature = temperature; b.topp = topp; b.r01 = uniform01; b.indices = di; b.out_id = dout; b.info = dout + 1;
+        SamplerRowsArgs b;
+        b.stride = 0; b.n = n; b.indices = di; b.out = dout;
+        b.row[0] = 0; b.temperature[0] = temperature; b.topp[0] = topp; b.r01[0] = uniform01;
         auto ctl = [&](size_t r) { w.src = dl + r * pad; w.cnt = dcnt + r * n; k_sample_ctl<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(a); };
-        auto plain = [&](size_t r) { b.logits = dl + r * pad; k_sample<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(b); };
-        ctl(reps); // warm-up on the last copy: k_sample_ctl only reads the row, so k_sample's warm-up can follow on it
+        auto plain = [&](size_t r) { b.logits = dl + r * pad; k_sample_rows<<<1, SAMPLER_THREADS, sampler_smem_bytes()>>>(b); };
+        ctl(reps); // warm-up on the last copy: k_sample_ctl only reads the row, so k_sample_rows' warm-up can follow on it
         plain(reps);
         s.ok(cudaEventRecord(e0));
         for (int r = 0; r < reps; r++) ctl(r);

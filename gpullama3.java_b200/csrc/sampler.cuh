@@ -152,12 +152,7 @@ __device__ __forceinline__ void sample_row(const SamplerArgs &a, unsigned char *
     if (a.info) { a.info[0] = n0; a.info[1] = n0 - last; }
 }
 
-__global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample(SamplerArgs a) {
-    extern __shared__ __align__(16) unsigned char smp_sm[];
-    sample_row(a, smp_sm);
-}
-
-// Every sampled row of a batched step in one launch: block j samples logits row row[j] (of rows stride floats apart) into
+// Every sampled row of a step in one launch: block j samples logits row row[j] (of rows stride floats apart) into
 // out[8 * row[j]] (the id, then the four diagnostics), with that row's own triple and its own indices scratch (n ints per row).
 #define SAMPLER_MAX_ROWS 8
 
@@ -175,9 +170,13 @@ __global__ void __launch_bounds__(SAMPLER_THREADS, 1) k_sample_rows(SamplerRowsA
     const int j = blockIdx.x, r = a.row[j];
     SamplerArgs s;
     s.logits = a.logits + (size_t)r * a.stride;
+    s.indices = a.indices + (size_t)r * a.n;
+    // Opaque to the optimiser: otherwise it keeps the row offsets as separate 64-bit terms and adds them back on every p[idx[i]]
+    // load of sample_row's single-thread top-p heap and CDF walk, which makes those latency-bound loops measurably slower.
+    asm("mov.b64 %0, %0;" : "+l"(s.logits));
+    asm("mov.b64 %0, %0;" : "+l"(s.indices));
     s.n = a.n;
     s.temperature = a.temperature[j]; s.topp = a.topp[j]; s.r01 = a.r01[j];
-    s.indices = a.indices + (size_t)r * a.n;
     s.out_id = a.out + 8 * r;
     s.info = a.out + 8 * r + 1;
     sample_row(s, smp_sm);

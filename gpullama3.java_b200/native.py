@@ -225,7 +225,7 @@ def test_sample_controls(logits, counts, controls: SamplingControls, temperature
 
 
 def time_sample_controls(logits, counts, controls: SamplingControls, temperature: float, topp: float, uniform01: float, reps: int):
-    """b200_time_sample_controls: CUDA-event ms per launch of (k_sample_ctl under controls, k_sample) on the same row, reps each."""
+    """b200_time_sample_controls: CUDA-event ms per launch of (k_sample_ctl under controls, one-row k_sample_rows) on the same row, reps each."""
     lg = np.ascontiguousarray(logits, dtype=np.float32)
     cnt = np.ascontiguousarray(counts, dtype=np.int32)
     if cnt.shape != lg.shape:

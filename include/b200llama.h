@@ -362,9 +362,9 @@ int b200_read_sample_counts(b200_plan *plan, int32_t slot, int32_t *counts);
  * sampler's four diagnostics (zeros at temperature 0) and, in row_out (nullable, n floats), the modified row before the choice. */
 int b200_test_sample_controls(const float *logits, int32_t n, int32_t *counts, const b200_sampling_controls *c, float temperature, float topp,
                               float uniform01, int32_t *token_out, int32_t *info, float *row_out);
-/* Measurement hook (no plan): CUDA-event time per launch of k_sample_ctl under controls c and of k_sample (b200_test_sample's kernel)
+/* Measurement hook (no plan): CUDA-event time per launch of k_sample_ctl under controls c and of k_sample_rows on one row (b200_test_sample's launch)
  * on the same host row, reps launches of each after one warm-up, each launch on its own copy of the row and counts.  temperature
- * must be > 0 (k_sample's range). */
+ * must be > 0 (the plain sampler's range). */
 int b200_time_sample_controls(const float *logits, int32_t n, const int32_t *counts, const b200_sampling_controls *c, float temperature, float topp,
                               float uniform01, int32_t reps, float *ctl_ms, float *plain_ms);
 
@@ -575,8 +575,8 @@ int b200_test_seqsum2(const float *terms, int32_t n, int32_t threads, float *out
  * items, fallbacks} of the second call (cycles holds 5 int64); out[0..1] = the two sums. */
 int b200_profile_seqsum2(const float *terms, int32_t n, int32_t threads, int64_t *cycles, float *out);
 
-/* Test hook for the device-side sampler (csrc/sampler.cuh): ONE launch of k_sample as b200_forward_decode_sample issues it (same
- * grid and shared memory, a logits buffer of whole 1024-float chunks with a zero pad) on n host logits.  Returns the sampled id, the
+/* Test hook for the device-side sampler (csrc/sampler.cuh): ONE one-row launch of k_sample_rows as b200_forward_decode_sample issues it
+ * (same block and shared memory, a logits buffer of whole 1024-float chunks with a zero pad) on n host logits.  Returns the sampled id, the
  * diagnostics {top-p candidates, tokens kept, seqsum items, seqsum fallbacks} and the n probabilities the kernel leaves in place.
  * The index scratch starts as 0xFF bytes, so a slot the kernel did not write in this call reads as -1.  temperature must be > 0
  * (0 is the plan's argmax path, not this kernel), uniform01 in [0, 1), n >= 1; B200_ERR_BAD_ARG otherwise. */

@@ -300,6 +300,8 @@ def test_refusals(pkg, make_model):
         _expect(pkg, lambda: plan.forward_chunk([(0, 1, 0, 1, 0.7, 0.9, 1.0)]), -1, "row 0: temperature")
         plan.set_sampling_controls(1, pkg.sampler.SamplingControls(top_k=3))
         _expect(pkg, lambda: plan.forward_chunk([(1, 1, 0, 1), (2, 1, 0, 0), (1, 2, 1, 1)]), -1, "row 2: slot 1 has sampling controls")
+        _expect(pkg, lambda: plan.forward_chunk([(2, 1, 0, 0), (1, 1, 0, 1), (1, 2, 1, 1)]), -1,
+                "row 2: slot 1 has sampling controls and already emits in row 1")
         ids, _ = plan.forward_chunk([(2, 1, 0, 0), (2, 2, 1, 1), (0, 3, 0, 1), (0, 4, 1, 1)])  # a slot without controls may emit twice
         assert ids[0] == -1 and all(0 <= i < V for i in ids[1:])
         assert np.isfinite(plan.forward_decode(1, 0)[0]).all()

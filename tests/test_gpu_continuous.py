@@ -262,6 +262,9 @@ def test_forward_step_refusals(pkg, make_model):
         _expect(pkg, lambda: plan.forward_step([(0, 1, 0, 0), (1, 1, 0, 1, -1.0, 0.9, 0.5)]), -1, "row 1: temperature")
         _expect(pkg, lambda: plan.forward_step([(0, 1, 0, 1, 0.7, 0.9, 1.0)]), -1, "row 0: temperature")
         _expect(pkg, lambda: plan.forward_step([(0, 1, 0, 1, float("nan"), 0.9, 0.5)]), -1, "row 0: temperature")
+        plan.set_sampling_controls(1, pkg.sampler.SamplingControls(top_k=3))
+        _expect(pkg, lambda: plan.forward_step([(1, 1, 0, 1), (0, 1, 0, 0), (1, 2, 1, 1)]), -1,
+                "row 2: slot 1 has sampling controls and already emits in row 0")
         ids, _ = plan.forward_step([(2, 1, 0, 0), (2, 2, 1, 1)])  # a valid call still works after the rejected ones
         assert ids[0] == -1 and 0 <= ids[1] < V
         assert np.isfinite(plan.forward_decode(1, 0)[0]).all()

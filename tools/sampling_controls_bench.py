@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Sampling controls (b200_set_sampling_controls) on the H100:
 
-  kernel_<vocab>_<setting>  k_sample_ctl against k_sample on one random row at vocabularies 128256 and 151936, temperature 0.8
-                            with top-p 0.9 and without top-p; settings: penalties over a 512-token history with top-k off, and the
+  kernel_<vocab>_<setting>  k_sample_ctl against a one-row k_sample_rows on one random row at vocabularies 128256 and 151936,
+                            temperature 0.8 with top-p 0.9 and without top-p; settings: penalties over a 512-token history with top-k off, and the
                             same with top-k 40.  b200_time_sample_controls: CUDA events around --kernel-reps launches of each
                             kernel, every launch on its own copy of the row and counts, ms per launch
   tg_<setting>              the Llama-3-8B-shaped Q8_0 model of bench.py, --tokens sampled tokens through forward_decode_sample
@@ -56,7 +56,7 @@ def main():
                             ("penalties_top_k40", S(top_k=40, repetition_penalty=1.1, frequency_penalty=0.1, presence_penalty=0.2))):
                 ctl_ms, plain_ms = N.time_sample_controls(row, counts, c, 0.8, topp, 0.5, args.kernel_reps)
                 out[f"{tag}_{name}_us"] = round(ctl_ms * 1e3, 1)
-                out[f"{tag}_k_sample_us"] = round(plain_ms * 1e3, 1)
+                out[f"{tag}_k_sample_rows_us"] = round(plain_ms * 1e3, 1)
 
     print(json.dumps(out), file=sys.stderr, flush=True)  # progress: each section's figures as soon as they exist
     n = args.tokens

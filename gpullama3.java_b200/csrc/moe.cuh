@@ -1,5 +1,7 @@
 // moe.cuh -- the FFN half of a Qwen2-MoE decode layer (InferenceCore.forwardJavaQwen2MoE, InferenceCore.java:366-424): the router,
 // the gate/up projections of the shared expert and the k routed experts, and their down projections with the ordered combine.
+// Qwen3-MoE runs the same FFN without the shared expert and with the top-k weights renormalised to sum to one: k_routed_route and
+// the <SHARED = false> instantiations of the two expert streams (k_routed_gateup, k_routed_down).
 //
 // Every other weight stream of the decode step has addresses that never depend on activations, so its producer starts copying
 // before the previous kernel has finished (programmatic dependent launch).  Here the router's top-k, computed in the same step,
@@ -9,7 +11,8 @@
 //
 // Device layout: every expert is a TileMat of its own (stream_matvec.cuh), gate/up interleaved as in the dense plan's L.tgu,
 // down as in L.tw2; a per-layer device table holds the base of each routed expert's two streams, indexed by expert id.  The
-// hidden activations of one step form one "virtual" vector of Hs + k * He units: [shared | routed slot 0 | ... | slot k-1].
+// hidden activations of one step form one "virtual" vector of Hs + k * He units: [shared | routed slot 0 | ... | slot k-1] (without
+// a shared expert: k * He units, [slot 0 | ... | slot k-1]; its producers have nothing to issue before the dependency wait).
 // Both Hs and He are multiples of 32, so no Q8_0 activation block straddles two experts and each expert's down projection reads
 // exactly the per-32-block quantisation of its own hidden vector (Q8_0FloatTensor.java:100-117).
 #pragma once
@@ -82,6 +85,95 @@ __global__ void __launch_bounds__(MOE_ROUTE_THREADS, 1) k_moe_route(MoeRouteArgs
     trace_mark(a.tr, 3);
 }
 
+// Qwen3-MoE's router: one CTA per router row (no shared-expert gate), the same scalarDot per row, and a tail on one warp of the last
+// CTA.  The max, the exps and the top-k scans are order-free given the lowest-index tie-break, so each lane takes experts
+// lane, lane + 32, ...; the softmax sum and the renormalisation sum stay sequential on lane 0:
+// softmaxInPlace; k scans for the first strict maximum, each pick then set to -inf; s = 0f, s += p_j in selection order; w_j = p_j / s.
+__global__ void __launch_bounds__(MOE_ROUTE_THREADS, 1) k_routed_route(MoeRouteArgs a) {
+    extern __shared__ __align__(16) float t[]; // dim terms
+    __shared__ float pr[MOE_MAX_EXPERTS];
+    __shared__ unsigned s_last;
+    constexpr int PER_LANE = MOE_MAX_EXPERTS / 32;
+    const int tid = threadIdx.x, e = blockIdx.x;
+    const float *w = a.router + (size_t)e * a.dim;
+    trace_entry(a.tr);
+    for (int i = tid; i < a.dim; i += MOE_ROUTE_THREADS) t[i] = w[i]; // the router is immutable: read before the dependency wait
+    pdl_launch_dependents();
+    pdl_wait();
+    trace_mark(a.tr, 2);
+    for (int i = tid; i < a.dim; i += MOE_ROUTE_THREADS) t[i] = __fmul_rn(t[i], ldcg_f32(a.xb + i));
+    __syncthreads();
+    if (tid == 0) {
+        a.logits[e] = pd_walk_terms(0.0f, t, a.dim); // float result = 0f; result += ... in index order
+        __threadfence();
+        s_last = atomicAdd(a.done, 1u) == (unsigned)(a.n_experts - 1) ? 1u : 0u;
+    }
+    __syncthreads();
+    if (!s_last || tid >= 32) { trace_mark(a.tr, 3); return; }
+    __threadfence();
+    const int lane = tid, E = a.n_experts;
+    if (lane == 0) *a.done = 0u;
+    float v[PER_LANE];
+    float mx = -INFINITY;
+#pragma unroll
+    for (int r = 0; r < PER_LANE; r++) {
+        const int j = lane + 32 * r;
+        v[r] = j < E ? ldcg_f32(a.logits + j) : -INFINITY;
+        mx = fmaxf(mx, v[r]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+#pragma unroll
+    for (int r = 0; r < PER_LANE; r++) {
+        const int j = lane + 32 * r;
+        if (j < E) pr[j] = v[r] = (float)exp((double)__fsub_rn(v[r], mx));
+    }
+    __syncwarp();
+    float sum = 0.0f;
+    if (lane == 0)
+        for (int j = 0; j < E; j++) sum = __fadd_rn(sum, pr[j]);
+    sum = __shfl_sync(0xffffffffu, sum, 0);
+#pragma unroll
+    for (int r = 0; r < PER_LANE; r++) v[r] = lane + 32 * r < E ? __fdiv_rn(v[r], sum) : -INFINITY;
+    float pick[MOE_MAX_K];
+    int pick_id[MOE_MAX_K];
+#pragma unroll
+    for (int i = 0; i < MOE_MAX_K; i++) {
+        if (i >= a.k) break;
+        // the lane's first strict maximum (its experts in index order), then the lowest index among the lanes' equal maxima
+        float best = -INFINITY;
+        int idx = 0x7fffffff;
+#pragma unroll
+        for (int r = 0; r < PER_LANE; r++)
+            if (v[r] > best) { best = v[r]; idx = lane + 32 * r; }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+            if (ob > best || (ob == best && oi < idx)) { best = ob; idx = oi; }
+        }
+        if (idx == 0x7fffffff) idx = 0; // no probability above -inf: the scan keeps index 0
+#pragma unroll
+        for (int r = 0; r < PER_LANE; r++)
+            if (lane + 32 * r == idx) v[r] = -INFINITY;
+        pick[i] = best;
+        pick_id[i] = idx;
+    }
+    if (lane == 0) {
+        float s = 0.0f;
+#pragma unroll
+        for (int i = 0; i < MOE_MAX_K; i++)
+            if (i < a.k) s = __fadd_rn(s, pick[i]);
+#pragma unroll
+        for (int i = 0; i < MOE_MAX_K; i++)
+            if (i < a.k) {
+                a.ids[i] = pick_id[i];
+                a.weights[i] = __fdiv_rn(pick[i], s);
+            }
+    }
+    trace_mark(a.tr, 3);
+}
+
 // ---- the expert streams --------------------------------------------------------------------------------------------------
 struct MoeStreamArgs {
     TileMat S;                         // shared expert: gate/up (rows 2 * Hs) or down (rows dim, cols Hs)
@@ -99,11 +191,13 @@ struct MoeStreamArgs {
     TraceBuf tr;
 };
 
-// Stream geometry of one matrix of the down projection's sequence: shared (m = 0) or routed slot m - 1.
+// Stream geometry of one matrix of the down projection's sequence: shared (m = 0) or routed slot m - 1; without a shared expert,
+// routed slot m.
 struct MoeMat {
     int seg, nseg, unit_bytes, act_off; // act_off: first unit of its activation in the virtual hidden vector
 };
-__device__ __forceinline__ MoeMat moe_mat(const MoeStreamArgs &a, int m) {
+template <bool SHARED> __device__ __forceinline__ MoeMat moe_mat(const MoeStreamArgs &a, int m) {
+    if (!SHARED) return MoeMat{a.X.seg, a.X.nseg, a.X.unit_bytes, m * a.X.cols};
     const TileMat &T = m == 0 ? a.S : a.X;
     return MoeMat{T.seg, T.nseg, T.unit_bytes, m == 0 ? 0 : a.S.cols + (m - 1) * a.X.cols};
 }
@@ -160,20 +254,23 @@ __device__ __forceinline__ void moe_tile_terms(const unsigned char *tile, const 
 }
 
 // Gate/up of the shared expert and the k routed experts as ONE virtual gate/up matrix: groups [0, Hs/2) are the shared expert's,
-// then He/2 groups per routed slot.  Output unit u of the virtual hidden vector = silu(gate) * up of group u / 2, exactly as
-// k_stream_matvec_q8<SMV_GATEUP> computes a dense layer's; its Q8_0 epilogue is the dense one over the virtual vector.
-__global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_gateup(MoeStreamArgs a, SmvSmem L) {
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ const unsigned char *s_base[MOE_MAX_K];
+// then He/2 groups per routed slot (SHARED = false: the routed slots only).  Output unit u of the virtual hidden vector =
+// silu(gate) * up of group u / 2, exactly as k_stream_matvec_q8<SMV_GATEUP> computes a dense layer's; its Q8_0 epilogue is the
+// dense one over the virtual vector.
+// smem: the kernel's dynamic shared memory; s_base: its MOE_MAX_K stream bases (both declared in the kernel, so that every other
+// kernel's shared-memory layout stays as it was).
+template <bool SHARED>
+__device__ __forceinline__ void moe_gateup(const MoeStreamArgs &a, const SmvSmem &L, unsigned char *smem, const unsigned char **s_base) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int S = L.stages;
     const unsigned bar0 = smem_u32(smem + L.off_bar);
-    const int gs = a.S.rows >> 2, gx = a.X.rows >> 2;
+    const TileMat &T0 = SHARED ? a.S : a.X; // the shared and the routed gate/up streams have the same columns (dim), so the same tiles
+    const int gs = SHARED ? a.S.rows >> 2 : 0, gx = a.X.rows >> 2;
     const int ngroups = gs + a.k * gx;
     const int g0 = (int)(((long long)blockIdx.x * ngroups) / gridDim.x);
     const int g1 = (int)(((long long)(blockIdx.x + 1) * ngroups) / gridDim.x);
-    const int nseg = a.S.nseg; // the shared and the routed gate/up streams have the same columns (dim), so the same tiles
-    const unsigned tile_bytes = 4u * (unsigned)a.S.unit_bytes;
+    const int nseg = T0.nseg;
+    const unsigned tile_bytes = 4u * (unsigned)T0.unit_bytes;
     volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + L.off_bar + 2 * SMV_MAX_STAGES * 8);
     stream_ring_init<SMV_MAX_STAGES>(smem, L.off_bar, S);
     __syncthreads();
@@ -193,7 +290,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_gateup(MoeStreamArgs a, 
                         const int G = gb + w;
                         const unsigned char *base;
                         int lg;
-                        if (G < gs) { base = a.S.base; lg = G; }
+                        if (SHARED && G < gs) { base = a.S.base; lg = G; }
                         else {
                             if (!routed) { // the routed experts' addresses are known once the router has finished
                                 pdl_wait();
@@ -219,7 +316,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_gateup(MoeStreamArgs a, 
 
     pdl_wait();
     trace_mark(a.tr, 2);
-    const int cols = a.S.cols;
+    const int cols = T0.cols;
     {
         int4 *sxq = reinterpret_cast<int4 *>(smem + L.off_xq);
         float *sxs = reinterpret_cast<float *>(smem + L.off_xs);
@@ -229,7 +326,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_gateup(MoeStreamArgs a, 
     }
     consumer_bar_sync();
 
-    const int seg = a.S.seg, nbs = seg >> 5;
+    const int seg = T0.seg, nbs = seg >> 5;
     float *terms = reinterpret_cast<float *>(smem + L.off_terms) + (size_t)warp * 4 * L.nbs_pad;
     const unsigned char *sact = smem + L.off_xq;
     const float *sxs = reinterpret_cast<const float *>(smem + L.off_xs);
@@ -250,7 +347,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_gateup(MoeStreamArgs a, 
                 __syncwarp();
                 mbar_wait(bar0 + 8 * st, lap & 1u);
                 const unsigned char *tile = smem + L.off_ring + (size_t)st * L.stage_bytes;
-                moe_tile_terms(tile, sact + ((size_t)s * seg), sxs + s * nbs, a.S.unit_bytes, seg, nbs, terms, L.nbs_pad, lane);
+                moe_tile_terms(tile, sact + ((size_t)s * seg), sxs + s * nbs, T0.unit_bytes, seg, nbs, terms, L.nbs_pad, lane);
                 __syncwarp();
                 if (lane == 0) {
                     rel[st] = lap + 1u;
@@ -307,18 +404,17 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_gateup(MoeStreamArgs a, 
 
 // Down projections of the shared expert and the k routed experts, one CTA owning rows [4 g0, 4 g1) of all k + 1 matrices, and
 // the combine as the epilogue: saxpyInPlace (FloatTensor.java:221-227) x[i] = w_j * y_j[i] + x[i] -- a float multiply, then a
-// float add -- for j in selection order, then the shared expert with its sigmoid weight (InferenceCore.java:404-423).
-__global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_down(MoeStreamArgs a, MoeDownSmem L) {
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ const unsigned char *s_base[MOE_MAX_K];
-    __shared__ float s_w[MOE_MAX_K + 1];
+// float add -- for j in selection order, then the shared expert with its sigmoid weight (InferenceCore.java:404-423).  SHARED =
+// false: the k routed matrices and their combine only.
+template <bool SHARED>
+__device__ __forceinline__ void moe_down(const MoeStreamArgs &a, const MoeDownSmem &L, unsigned char *smem, const unsigned char **s_base, float *s_w) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int S = L.stages;
     const unsigned bar0 = smem_u32(smem + L.off_bar);
-    const int ngroups = a.S.rows >> 2; // rows = dim for every matrix
+    const int ngroups = (SHARED ? a.S : a.X).rows >> 2; // rows = dim for every matrix
     const int g0 = (int)(((long long)blockIdx.x * ngroups) / gridDim.x);
     const int g1 = (int)(((long long)(blockIdx.x + 1) * ngroups) / gridDim.x);
-    const int nm = a.k + 1;
+    const int nm = SHARED ? a.k + 1 : a.k;
     volatile unsigned *rel = reinterpret_cast<volatile unsigned *>(smem + L.off_bar + 2 * SMV_MAX_STAGES * 8);
     stream_ring_init<SMV_MAX_STAGES>(smem, L.off_bar, S);
     __syncthreads();
@@ -334,15 +430,15 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_down(MoeStreamArgs a, Mo
                 const int nw = min(SMV_CONSUMER_WARPS, g1 - gb);
                 for (int m = 0; m < nm; m++) {
                     const unsigned char *base = a.S.base;
-                    if (m > 0) {
+                    if (!SHARED || m > 0) {
                         if (!routed) {
                             pdl_wait();
                             for (int j = 0; j < a.k; j++) s_base[j] = a.bases[__ldcg(a.ids + j)];
                             routed = true;
                         }
-                        base = s_base[m - 1];
+                        base = s_base[SHARED ? m - 1 : m];
                     }
-                    const MoeMat M = moe_mat(a, m);
+                    const MoeMat M = moe_mat<SHARED>(a, m);
                     const unsigned tile_bytes = 4u * (unsigned)M.unit_bytes;
                     for (int s = 0; s < M.nseg; s++)
 #pragma unroll 1
@@ -363,7 +459,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_down(MoeStreamArgs a, Mo
 
     pdl_wait();
     trace_mark(a.tr, 2);
-    const int hv = a.S.cols + a.k * a.X.cols;
+    const int hv = (SHARED ? a.S.cols : 0) + a.k * a.X.cols;
     {
         int4 *sxq = reinterpret_cast<int4 *>(smem + L.off_xq);
         float *sxs = reinterpret_cast<float *>(smem + L.off_xs);
@@ -386,7 +482,7 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_down(MoeStreamArgs a, Mo
             const int row = 4 * (gb + warp) + (lane & 3);
             float xv = lane < 4 ? ldcg_f32(a.out + row) : 0.0f, ysh = 0.0f;
             for (int m = 0; m < nm; m++) {
-                const MoeMat M = moe_mat(a, m);
+                const MoeMat M = moe_mat<SHARED>(a, m);
                 const int nbs = M.seg >> 5;
                 float acc = 0.0f;
                 for (int s = 0; s < M.nseg; s++) {
@@ -409,15 +505,39 @@ __global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_down(MoeStreamArgs a, Mo
                     __syncwarp();
                 }
                 off += (unsigned)(M.nseg * nw);
-                if (m == 0) ysh = acc;                              // the shared expert is added last
-                else xv = __fadd_rn(__fmul_rn(s_w[m - 1], acc), xv); // routed slot m - 1, in selection order
+                if (!SHARED) xv = __fadd_rn(__fmul_rn(s_w[m], acc), xv); // routed slot m, in selection order
+                else if (m == 0) ysh = acc;                              // the shared expert is added last
+                else xv = __fadd_rn(__fmul_rn(s_w[m - 1], acc), xv);     // routed slot m - 1, in selection order
             }
-            xv = __fadd_rn(__fmul_rn(s_w[a.k], ysh), xv);
+            if (SHARED) xv = __fadd_rn(__fmul_rn(s_w[a.k], ysh), xv);
             if (lane < 4) a.out[row] = xv;
         } else {
-            for (int m = 0; m < nm; m++) off += (unsigned)(moe_mat(a, m).nseg * nw);
+            for (int m = 0; m < nm; m++) off += (unsigned)(moe_mat<SHARED>(a, m).nseg * nw);
         }
         seq_base += off;
     }
     trace_mark(a.tr, 3);
+}
+
+__global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_gateup(MoeStreamArgs a, SmvSmem L) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ const unsigned char *s_base[MOE_MAX_K];
+    moe_gateup<true>(a, L, smem, s_base);
+}
+__global__ void __launch_bounds__(SMV_THREADS, 1) k_moe_down(MoeStreamArgs a, MoeDownSmem L) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ const unsigned char *s_base[MOE_MAX_K];
+    __shared__ float s_w[MOE_MAX_K + 1];
+    moe_down<true>(a, L, smem, s_base, s_w);
+}
+__global__ void __launch_bounds__(SMV_THREADS, 1) k_routed_gateup(MoeStreamArgs a, SmvSmem L) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ const unsigned char *s_base[MOE_MAX_K];
+    moe_gateup<false>(a, L, smem, s_base);
+}
+__global__ void __launch_bounds__(SMV_THREADS, 1) k_routed_down(MoeStreamArgs a, MoeDownSmem L) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ const unsigned char *s_base[MOE_MAX_K];
+    __shared__ float s_w[MOE_MAX_K];
+    moe_down<false>(a, L, smem, s_base, s_w);
 }

@@ -39,7 +39,8 @@ struct LayerW {
     size_t ring_qkv = 0, ring_gu = 0;    // dynamic shared memory of the QKV and gate/up stream launches (ring_budgets)
     float *attn_norm = nullptr, *ffn_norm = nullptr, *q_norm = nullptr, *k_norm = nullptr;
     float *qkv_bias = nullptr; // Qwen2: this rank's q|k|v bias, laid out like the packed q|k|v vector
-    // Qwen2-MoE (moe.cuh): the shared expert's streams, the routed experts' geometry and the device tables of their stream bases
+    // Qwen2-MoE / Qwen3-MoE (moe.cuh): the shared expert's streams (Qwen2-MoE only), the routed experts' geometry and the device
+    // tables of their stream bases
     TileMat sgu{}, sdn{}, xgu{}, xdn{};
     const unsigned char **gu_bases = nullptr, **dn_bases = nullptr;
     float *router = nullptr, *shared_gate = nullptr; // F32 [n_experts][dim] and [dim]
@@ -147,9 +148,12 @@ struct b200_plan {
     float prefill_ms = 0.f; // device time of the last tensor-core prefill chunk
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 
-    // Qwen2-MoE: the routing buffers [layer][k] ids and [layer][k + 1] weights of the last step, the router logits scratch and
-    // arrival counters, the down projection's shared-memory layout
+    // Qwen2-MoE / Qwen3-MoE: the routing buffers [layer][k] ids and [layer][moe_nw] weights of the last step, the router logits
+    // scratch and arrival counters, the down projection's shared-memory layout
     bool is_moe = false;
+    bool moe_shared = false; // Qwen2-MoE: a shared expert with its sigmoid gate; Qwen3-MoE: none, the top-k weights renormalised
+    int moe_nw = 0;          // routing weights per layer: k, plus the shared-expert weight on Qwen2-MoE
+    const char *moe_name = ""; // the family the MoE refusals name
     b200_moe_config moe{};
     int moe_hv = 0; // units of the virtual hidden vector: shared_hidden_dim + n_experts_used * expert_hidden_dim
     int *moe_ids = nullptr;
@@ -793,9 +797,9 @@ bool gateup_fits(int hidden, int n_sms) { // epilogue buffer holds this CTA's hi
 // k_attention's dynamic shared memory: q | k | out | score row (the row lives in a global scratch buffer for long contexts).
 size_t att_smem_bytes(int head_size, int ctx, bool scratch) { return (size_t)(3 * head_size + (scratch ? 0 : ctx)) * 4; }
 
-// The FFN half of a Qwen2-MoE layer (moe.cuh): the FFN norm (float xb for the F32 router, xq/xs for the experts), the router,
-// the shared + routed gate/up stream and the down streams with the ordered combine.  Four launches, all under PDL; `tr` is the
-// norm's trace record, the three MoE kernels take the next three (trace ids 10, 11, 12).
+// The FFN half of a Qwen2-MoE or Qwen3-MoE layer (moe.cuh): the FFN norm (float xb for the F32 router, xq/xs for the experts), the
+// router, the (shared +) routed gate/up stream and the down streams with the ordered combine.  Four launches, all under PDL; `tr` is
+// the norm's trace record, the three MoE kernels take the next three (trace ids 10, 11, 12).
 int enqueue_moe_ffn(b200_plan *p, int l, TraceBuf tr) {
     const b200_config &c = p->cfg;
     const LayerW &L = p->layers[l];
@@ -804,20 +808,21 @@ int enqueue_moe_ffn(b200_plan *p, int l, TraceBuf tr) {
     if ((rc = launch_k(p, p->use_pdl, k_rmsnorm_quant<false>, dim3(1), dim3(NORM_THREADS), norm_smem_bytes(c.dim), p->x, (const StepState *)p->st, p->emb,
                        p->mup.embedding_scale, (const float *)L.ffn_norm, c.rms_norm_eps, c.dim, p->xq, p->xs, p->xb, (long long *)nullptr, tr, p->tp, -1)))
         return rc;
+    const bool sh = p->moe_shared;
     int *ids = p->moe_ids + (size_t)l * k;
-    float *w = p->moe_w + (size_t)l * (k + 1);
+    float *w = p->moe_w + (size_t)l * p->moe_nw;
     MoeRouteArgs ra;
     ra.router = L.router; ra.shared_gate = L.shared_gate; ra.xb = p->xb; ra.logits = p->moe_logits + (size_t)l * (E + 1); ra.done = p->moe_done + l;
     ra.ids = ids; ra.weights = w; ra.dim = c.dim; ra.n_experts = E; ra.k = k; ra.tr = TraceBuf{tr.rec, tr.slot + 1, 10};
-    if ((rc = launch_k(p, p->use_pdl, k_moe_route, dim3(E + 1), dim3(MOE_ROUTE_THREADS), (size_t)c.dim * 4, ra))) return rc;
+    if ((rc = launch_k(p, p->use_pdl, sh ? k_moe_route : k_routed_route, dim3(sh ? E + 1 : E), dim3(MOE_ROUTE_THREADS), (size_t)c.dim * 4, ra))) return rc;
     MoeStreamArgs a;
     a.S = L.sgu; a.X = L.xgu; a.bases = L.gu_bases; a.ids = ids; a.weights = w; a.k = k;
     a.xq = p->xq; a.xs = p->xs; a.out = p->hb; a.hq = p->hq; a.hs = p->hs; a.blk_cnt = p->blk_cnt; a.tr = TraceBuf{tr.rec, tr.slot + 2, 11};
-    const SmvSmem GL = smv_layout(c.dim, L.sgu.seg, SMV_SMEM_BUDGET_MAX);
-    if ((rc = launch_k(p, p->use_pdl, k_moe_gateup, dim3(p->n_sms), dim3(SMV_THREADS), GL.total, a, GL))) return rc;
+    const SmvSmem GL = smv_layout(c.dim, (sh ? L.sgu : L.xgu).seg, SMV_SMEM_BUDGET_MAX);
+    if ((rc = launch_k(p, p->use_pdl, sh ? k_moe_gateup : k_routed_gateup, dim3(p->n_sms), dim3(SMV_THREADS), GL.total, a, GL))) return rc;
     a.S = L.sdn; a.X = L.xdn; a.bases = L.dn_bases;
     a.xq = p->hq; a.xs = p->hs; a.out = p->x; a.hq = nullptr; a.hs = nullptr; a.blk_cnt = nullptr; a.tr = TraceBuf{tr.rec, tr.slot + 3, 12};
-    return launch_k(p, p->use_pdl, k_moe_down, dim3(p->n_sms), dim3(SMV_THREADS), p->moe_dl.total, a, p->moe_dl);
+    return launch_k(p, p->use_pdl, sh ? k_moe_down : k_routed_down, dim3(p->n_sms), dim3(SMV_THREADS), p->moe_dl.total, a, p->moe_dl);
 }
 
 // Enqueue one single-token forward on p->stream (captured into a CUDA graph at creation).
@@ -924,7 +929,11 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
 int pd_prepare(b200_plan *p) {
     const b200_config &c = p->cfg;
     p->pd_ok = false;
-    if (p->is_moe) { p->pd_why = "the persistent decode kernel has no Qwen2-MoE layer (MoE plans decode through the CUDA graph)"; return B200_OK; }
+    if (p->is_moe) {
+        p->pd_why = p->moe_shared ? "the persistent decode kernel has no Qwen2-MoE layer (MoE plans decode through the CUDA graph)"
+                                  : "the persistent decode kernel has no Qwen3-MoE layer (MoE plans decode through the CUDA graph)";
+        return B200_OK;
+    }
     if (p->resident) { p->pd_why = "the persistent decode kernel reads Q8_0 tiles only (this plan keeps K-quant weights resident: it decodes through the CUDA graph)"; return B200_OK; }
     if (c.dim > 8192) { p->pd_why = "the persistent decode kernel's register-resident RMSNorm supports dim <= 8192"; return B200_OK; }
     if (p->wtype != B200_GGML_Q8_0) { p->pd_why = "the persistent decode kernel needs Q8_0 weights"; return B200_OK; }
@@ -1220,7 +1229,9 @@ int batch_alloc(b200_plan *p, int ns) {
 // Why a plan cannot run them (nullptr: it can): the conditions of batched decode.
 const char *const RESIDENT_MULTI_WHY = "batched and multi-position steps read Q8_0 tiles only (this plan keeps K-quant weights resident: it runs one position per step)";
 const char *multi_why(const b200_plan *p) {
-    if (p->is_moe) return "multi-position steps have no Qwen2-MoE layer (MoE plans run one position per step)";
+    if (p->is_moe)
+        return p->moe_shared ? "multi-position steps have no Qwen2-MoE layer (MoE plans run one position per step)"
+                             : "multi-position steps have no Qwen3-MoE layer (MoE plans run one position per step)";
     if (p->resident) return RESIDENT_MULTI_WHY;
     if (p->cfg.tp_size > 1) return "multi-position steps run on single-GPU plans only (this plan is tensor-parallel)";
     if (p->wtype != B200_GGML_Q8_0) return "multi-position steps need Q8_0 weights (FP16 plans run one position per step)";
@@ -1329,6 +1340,8 @@ int set_smem_attrs(b200_plan *p) {
     CK(cudaFuncSetAttribute(k_stream_matvec_q8_batch<SMV_GATEUP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
     CK(cudaFuncSetAttribute(k_moe_gateup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_moe_down, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    CK(cudaFuncSetAttribute(k_routed_gateup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
+    CK(cudaFuncSetAttribute(k_routed_down, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMV_SMEM_BUDGET_MAX));
     CK(cudaFuncSetAttribute(k_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     CK(cudaFuncSetAttribute(k_sample_ctl, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sampler_smem_bytes()));
     done = true;
@@ -1416,9 +1429,10 @@ void rope_table_yarn(const b200_config &c, const b200_yarn_config &y, std::vecto
         }
 }
 
-// Qwen2-MoE FFN tensors of one layer (llama.cpp's names and shapes, dims[0] innermost): the F32 router and shared-expert gate, the
-// stacked routed experts [E][rows][cols] and the shared expert.  Every routed expert becomes a TileMat of its own, cut from its
-// row range of the stacked tensor (K-quant experts are re-quantised on the way like any matrix).
+// MoE FFN tensors of one layer (llama.cpp's names and shapes, dims[0] innermost): the F32 router, the stacked routed experts
+// [E][rows][cols] and, on Qwen2-MoE, the shared-expert gate and the shared expert (Qwen3-MoE has neither).  Every routed expert
+// becomes a TileMat of its own, cut from its row range of the stacked tensor (K-quant experts are re-quantised on the way like any
+// matrix).
 int upload_moe_layer(b200_plan *p, const b200_tensor *tensors, int n_tensors, int l) {
     const b200_config &c = p->cfg;
     LayerW &L = p->layers[l];
@@ -1430,6 +1444,7 @@ int upload_moe_layer(b200_plan *p, const b200_tensor *tensors, int n_tensors, in
                           {"ffn_up_shexp.weight", 2, {D, Hs, 0}, false},   {"ffn_down_shexp.weight", 2, {Hs, D, 0}, false}};
     const b200_tensor *t[8];
     for (int i = 0; i < 8; i++) {
+        if (!p->moe_shared && (i == 1 || i >= 5)) continue; // the shared-expert tensors
         const std::string name = "blk." + std::to_string(l) + "." + want[i].name;
         t[i] = find(tensors, n_tensors, name);
         if (!t[i]) return fail(p, B200_ERR_BAD_ARG, "missing tensor %s", name.c_str());
@@ -1447,10 +1462,12 @@ int upload_moe_layer(b200_plan *p, const b200_tensor *tensors, int n_tensors, in
     int rc;
     if ((rc = dalloc(p, &L.router, (size_t)E * D * 4))) return rc;
     CK(cudaMemcpy(L.router, t[0]->data, (size_t)E * D * 4, cudaMemcpyHostToDevice));
-    if ((rc = dalloc(p, &L.shared_gate, (size_t)D * 4))) return rc;
-    CK(cudaMemcpy(L.shared_gate, t[1]->data, (size_t)D * 4, cudaMemcpyHostToDevice));
-    if ((rc = upload_tiles(p, t[5], t[6], nullptr, Hs, Hs, 0, D, true, L.sgu))) return rc;
-    if ((rc = upload_tiles(p, t[7], nullptr, nullptr, D, 0, 0, Hs, false, L.sdn))) return rc;
+    if (p->moe_shared) {
+        if ((rc = dalloc(p, &L.shared_gate, (size_t)D * 4))) return rc;
+        CK(cudaMemcpy(L.shared_gate, t[1]->data, (size_t)D * 4, cudaMemcpyHostToDevice));
+        if ((rc = upload_tiles(p, t[5], t[6], nullptr, Hs, Hs, 0, D, true, L.sgu))) return rc;
+        if ((rc = upload_tiles(p, t[7], nullptr, nullptr, D, 0, 0, Hs, false, L.sdn))) return rc;
+    }
     std::vector<const unsigned char *> hg(E), hd(E);
     for (int e = 0; e < E; e++) {
         const int gr0[3] = {e * He, e * He, 0}, gfu[3] = {E * He, E * He, 0};
@@ -1543,20 +1560,25 @@ int weight_policy(b200_plan *p, const b200_tensor *tensors, int n_tensors, size_
 int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     const b200_config &c = p->cfg;
     if (c.arch != B200_ARCH_LLAMA && c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_PHI3 && c.arch != B200_ARCH_QWEN2 && c.arch != B200_ARCH_QWEN2_MOE &&
-        c.arch != B200_ARCH_GRANITE && c.arch != B200_ARCH_DEVSTRAL)
+        c.arch != B200_ARCH_GRANITE && c.arch != B200_ARCH_DEVSTRAL && c.arch != B200_ARCH_QWEN3_MOE)
         return fail(p, B200_ERR_UNSUPPORTED, "unknown arch %d", c.arch);
-    p->kflags = c.arch == B200_ARCH_QWEN3 ? (KF_NEOX | KF_QKNORM) : c.arch == B200_ARCH_PHI3 ? KF_NEOX
+    const bool qwen3_attn = c.arch == B200_ARCH_QWEN3 || c.arch == B200_ARCH_QWEN3_MOE; // q/k RMSNorm, NeoX RoPE, head size of its own
+    p->kflags = qwen3_attn ? (KF_NEOX | KF_QKNORM) : c.arch == B200_ARCH_PHI3 ? KF_NEOX
               : (c.arch == B200_ARCH_QWEN2 || c.arch == B200_ARCH_QWEN2_MOE) ? (KF_NEOX | KF_QKVBIAS) : c.arch == B200_ARCH_GRANITE ? KF_ATTSCALE : 0;
     if (p->is_moe) {
         const b200_moe_config &m = p->moe;
-        if (c.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "Qwen2-MoE plans are single-GPU (tensor parallelism has no expert layout)");
+        if (c.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "%s plans are single-GPU (tensor parallelism has no expert layout)", p->moe_name);
         if (m.n_experts < 1 || m.n_experts > MOE_MAX_EXPERTS) return fail(p, B200_ERR_BAD_ARG, "n_experts = %d: need 1..%d", m.n_experts, MOE_MAX_EXPERTS);
         const int kmax = m.n_experts < MOE_MAX_K ? m.n_experts : MOE_MAX_K;
         if (m.n_experts_used < 1 || m.n_experts_used > kmax)
             return fail(p, B200_ERR_BAD_ARG, "n_experts_used = %d: need 1..%d (min(n_experts, %d))", m.n_experts_used, kmax, MOE_MAX_K);
-        if (m.expert_hidden_dim <= 0 || m.shared_hidden_dim <= 0 || m.expert_hidden_dim % 32 || m.shared_hidden_dim % 32)
+        if (p->moe_shared && (m.expert_hidden_dim <= 0 || m.shared_hidden_dim <= 0 || m.expert_hidden_dim % 32 || m.shared_hidden_dim % 32))
             return fail(p, B200_ERR_UNSUPPORTED, "expert hidden %d / shared hidden %d: the Q8_0 stream needs positive multiples of 32", m.expert_hidden_dim,
                         m.shared_hidden_dim);
+        if (!p->moe_shared && m.shared_hidden_dim != 0)
+            return fail(p, B200_ERR_BAD_ARG, "shared_hidden_dim = %d: Qwen3-MoE has no shared expert (pass 0)", m.shared_hidden_dim);
+        if (!p->moe_shared && (m.expert_hidden_dim <= 0 || m.expert_hidden_dim % 32))
+            return fail(p, B200_ERR_UNSUPPORTED, "expert hidden %d: the Q8_0 stream needs a positive multiple of 32", m.expert_hidden_dim);
         if (c.dim > 8192) // k_moe_route stages dim floats in (default-sized) dynamic shared memory, as the RMSNorm kernel caps dim
             return fail(p, B200_ERR_UNSUPPORTED, "dim %d: the MoE router kernel supports dim <= 8192", c.dim);
         p->moe_hv = m.shared_hidden_dim + m.n_experts_used * m.expert_hidden_dim;
@@ -1568,7 +1590,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         return fail(p, B200_ERR_BAD_ARG, "fp16_lanes must be 0, 4, 8, 16 or 32");
     p->qd = c.n_heads * c.head_size;
     p->kvd = c.n_kv_heads * c.head_size;
-    if (c.arch != B200_ARCH_QWEN3 && c.arch != B200_ARCH_DEVSTRAL && p->qd != c.dim)
+    if (!qwen3_attn && c.arch != B200_ARCH_DEVSTRAL && p->qd != c.dim)
         return fail(p, B200_ERR_BAD_ARG, "llama / phi3 / qwen2: n_heads*head_size must equal dim");
     {
         const int tn = c.tp_size;
@@ -1590,7 +1612,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     if (p->wtype != B200_GGML_Q8_0 && p->wtype != B200_GGML_F16)
         return fail(p, B200_ERR_UNSUPPORTED, "Type: %d currently not supported by this engine (Q8_0, F16 and the K-quants Q4_K/Q5_K/Q6_K only)", wq0->ggml_type);
     if (p->is_moe && p->wtype != B200_GGML_Q8_0)
-        return fail(p, B200_ERR_UNSUPPORTED, "Qwen2-MoE runs in Q8_0 only (FP16 MoE plans are not supported, as in the reference)");
+        return fail(p, B200_ERR_UNSUPPORTED, "%s runs in Q8_0 only (FP16 MoE plans are not supported, as in the reference)", p->moe_name);
     bool any_kq = false;
     for (int i = 0; i < n_tensors; i++) any_kq = any_kq || kq_is_kquant(tensors[i].ggml_type);
 
@@ -1621,14 +1643,15 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         if (p->is_moe) { // the MoE FFN has its own streams (the dense FFN checks above are skipped)
             const b200_moe_config &m = p->moe;
             const int hs = m.shared_hidden_dim, he = m.expert_hidden_dim;
-            const bool cut = stream_shape_ok(2 * hs, c.dim) && stream_shape_ok(c.dim, hs) && stream_shape_ok(2 * he, c.dim) && stream_shape_ok(c.dim, he) &&
-                             gateup_fits(p->moe_hv, p->n_sms);
+            const bool cut = (!p->moe_shared || (stream_shape_ok(2 * hs, c.dim) && stream_shape_ok(c.dim, hs))) && stream_shape_ok(2 * he, c.dim) &&
+                             stream_shape_ok(c.dim, he) && gateup_fits(p->moe_hv, p->n_sms);
             if (!cut) return fail(p, B200_ERR_UNSUPPORTED, "expert hidden %d / shared hidden %d at dim %d: the Q8_0 stream layout cannot cut these matrices", he, hs, c.dim);
-            p->moe_dl = moe_down_layout(p->moe_hv, hs / smv_pick_nseg(hs), he / smv_pick_nseg(he), SMV_SMEM_BUDGET_MAX);
+            const int seg_x = he / smv_pick_nseg(he);
+            p->moe_dl = moe_down_layout(p->moe_hv, p->moe_shared ? hs / smv_pick_nseg(hs) : seg_x, seg_x, SMV_SMEM_BUDGET_MAX);
             if (p->moe_dl.stages < 3) return fail(p, B200_ERR_UNSUPPORTED, "the expert down projection leaves fewer than 3 ring stages of shared memory");
         }
         p->use_pdl = q8 || p->use_f16_stream;
-        // Tensor parallelism keeps the separate norm: its read of x waits on every rank's slice (TP_SLOT_X).  So does Qwen2-MoE,
+        // Tensor parallelism keeps the separate norm: its read of x waits on every rank's slice (TP_SLOT_X).  So does MoE,
         // whose FFN norm must write float xb for the F32 router anyway; its plans keep 8 launches per layer.
         p->fuse_norm = q8 && c.tp_size == 1 && !p->is_moe && norm_fusion_ok(c.dim);
     }
@@ -1687,7 +1710,7 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
         auto T = [&](const char *s) { return find(tensors, n_tensors, pre + s); };
         if ((rc = upload_f32(p, T("attn_norm.weight"), c.dim, &L.attn_norm, "attn_norm.weight"))) return rc;
         if ((rc = upload_f32(p, T("ffn_norm.weight"), c.dim, &L.ffn_norm, "ffn_norm.weight"))) return rc;
-        if (c.arch == B200_ARCH_QWEN3) {
+        if (qwen3_attn) {
             if ((rc = upload_f32(p, T("attn_q_norm.weight"), c.head_size, &L.q_norm, "attn_q_norm.weight"))) return rc;
             if ((rc = upload_f32(p, T("attn_k_norm.weight"), c.head_size, &L.k_norm, "attn_k_norm.weight"))) return rc;
         }
@@ -1826,11 +1849,11 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     if (p->is_moe) {
         const int E = p->moe.n_experts, k = p->moe.n_experts_used;
         if ((rc = dalloc(p, &p->moe_ids, (size_t)c.n_layers * k * 4))) return rc;
-        if ((rc = dalloc(p, &p->moe_w, (size_t)c.n_layers * (k + 1) * 4))) return rc;
+        if ((rc = dalloc(p, &p->moe_w, (size_t)c.n_layers * p->moe_nw * 4))) return rc;
         if ((rc = dalloc(p, &p->moe_logits, (size_t)c.n_layers * (E + 1) * 4))) return rc;
         if ((rc = dalloc(p, &p->moe_done, (size_t)c.n_layers * 4))) return rc;
         CK(cudaMemset(p->moe_ids, 0, (size_t)c.n_layers * k * 4));
-        CK(cudaMemset(p->moe_w, 0, (size_t)c.n_layers * (k + 1) * 4));
+        CK(cudaMemset(p->moe_w, 0, (size_t)c.n_layers * p->moe_nw * 4));
         CK(cudaMemset(p->moe_done, 0, (size_t)c.n_layers * 4));
     }
 
@@ -1857,11 +1880,13 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
 
 // ---- batched prefill on the tensor cores (prefill.cuh) -------------------------------------------
 static const char *const MOE_PREFILL_WHY = "Qwen2-MoE plans have no tensor-core prefill: prompts go through the exact token-by-token prefill";
+static const char *const MOE3_PREFILL_WHY = "Qwen3-MoE plans have no tensor-core prefill: prompts go through the exact token-by-token prefill";
+static const char *moe_prefill_why(const b200_plan *p) { return p->moe_shared ? MOE_PREFILL_WHY : MOE3_PREFILL_WHY; }
 // What both tensor-core modes need of the plan's shape; nullptr when the chunk GEMMs and the attention can run it.
 static const char *prefill_shape_why(const b200_plan *p) {
     const b200_config &g = p->cfg;
     const int kv_mul = g.n_heads / g.n_kv_heads, nqkv = p->qd + 2 * p->kvd;
-    if (p->is_moe) return MOE_PREFILL_WHY;
+    if (p->is_moe) return moe_prefill_why(p);
     if (g.tp_size > 1) return "tensor-core prefill is single-GPU";
     if (g.head_size != 64 && g.head_size != 128) return "tensor-core prefill supports head sizes 64 and 128";
     if (g.n_heads % g.n_kv_heads || kv_mul > 64) return "tensor-core prefill needs n_heads % n_kv_heads == 0 and a GQA ratio <= 64";
@@ -2800,10 +2825,12 @@ static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const
         if (err && err_len) snprintf(err, err_len, "null argument");
         return B200_ERR_BAD_ARG;
     }
-    if ((cfg->arch == B200_ARCH_QWEN2_MOE) != (moe != nullptr)) {
+    if ((cfg->arch == B200_ARCH_QWEN2_MOE || cfg->arch == B200_ARCH_QWEN3_MOE) != (moe != nullptr)) {
         if (err && err_len)
-            snprintf(err, err_len, moe ? "b200_plan_create_moe needs arch B200_ARCH_QWEN2_MOE (got %d)"
-                                       : "arch %d (B200_ARCH_QWEN2_MOE) needs its expert configuration: create the plan with b200_plan_create_moe", cfg->arch);
+            snprintf(err, err_len, moe ? "b200_plan_create_moe needs arch B200_ARCH_QWEN2_MOE or B200_ARCH_QWEN3_MOE (got %d)"
+                     : cfg->arch == B200_ARCH_QWEN2_MOE ? "arch %d (B200_ARCH_QWEN2_MOE) needs its expert configuration: create the plan with b200_plan_create_moe"
+                                                        : "arch %d (B200_ARCH_QWEN3_MOE) needs its expert configuration: create the plan with b200_plan_create_moe",
+                     cfg->arch);
         return B200_ERR_BAD_ARG;
     }
     if ((cfg->arch == B200_ARCH_GRANITE) != (granite != nullptr)) {
@@ -2844,7 +2871,13 @@ static int plan_create(const b200_config *cfg, const b200_moe_config *moe, const
     }
     b200_plan *p = new b200_plan();
     p->cfg = *cfg;
-    if (moe) { p->is_moe = true; p->moe = *moe; }
+    if (moe) {
+        p->is_moe = true;
+        p->moe = *moe;
+        p->moe_shared = cfg->arch == B200_ARCH_QWEN2_MOE;
+        p->moe_nw = moe->n_experts_used + (p->moe_shared ? 1 : 0);
+        p->moe_name = p->moe_shared ? "Qwen2-MoE" : "Qwen3-MoE";
+    }
     if (granite) p->mup = *granite;
     if (yarn) { p->has_yarn = true; p->yarn = *yarn; }
     if (p->cfg.tp_size <= 0) p->cfg.tp_size = 1;
@@ -3077,7 +3110,7 @@ int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
     if (!p || (mode != B200_PREFILL_EXACT && mode != B200_PREFILL_TENSOR_CORE && mode != B200_PREFILL_TENSOR_CORE_W8A16 &&
                mode != B200_PREFILL_TENSOR_CORE_EXACT))
         return B200_ERR_BAD_ARG;
-    if (p->is_moe && mode != B200_PREFILL_EXACT) return fail(p, B200_ERR_UNSUPPORTED, "%s", MOE_PREFILL_WHY);
+    if (p->is_moe && mode != B200_PREFILL_EXACT) return fail(p, B200_ERR_UNSUPPORTED, "%s", moe_prefill_why(p));
     if (p->resident && (mode == B200_PREFILL_TENSOR_CORE || mode == B200_PREFILL_TENSOR_CORE_W8A16))
         return fail(p, B200_ERR_UNSUPPORTED, "this plan keeps K-quant weights resident: the f16 and W8A16 tensor-core prefills read f16 matrices or "
                     "Q8_0 tiles it does not hold; tensor_core_exact expands each resident matrix to Q8_0 tiles before its GEMM");
@@ -3138,7 +3171,7 @@ int b200_set_decode_slots(b200_plan *p, int32_t n_slots) {
     CK(cudaSetDevice(p->device));
     CK(cudaStreamSynchronize(p->stream));
     if (n_slots == 0) { batch_free(p); return clear_counts(p, 1, SMB_MAX_ROWS + 1); } // the memset orders before any later call's work
-    if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "batched decode has no Qwen2-MoE layer (MoE plans decode one sequence per step)");
+    if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "batched decode has no %s layer (MoE plans decode one sequence per step)", p->moe_name);
     if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "batched decode runs on single-GPU plans only (this plan is tensor-parallel)");
     if (p->wtype != B200_GGML_Q8_0) return fail(p, B200_ERR_UNSUPPORTED, "batched decode needs Q8_0 weights (FP16 plans decode one sequence per step)");
     if (p->resident) return fail(p, B200_ERR_UNSUPPORTED, "%s", RESIDENT_MULTI_WHY);
@@ -3484,7 +3517,7 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
         if (!p->is_moe) return fail(p, B200_ERR_BAD_ARG, "%s: not a Qwen2-MoE plan", name);
         const size_t k = (size_t)p->moe.n_experts_used;
         if (s == "moe_ids") { src = p->moe_ids; sz = (size_t)c.n_layers * k * 4; }
-        else { src = p->moe_w; sz = (size_t)c.n_layers * (k + 1) * 4; }
+        else { src = p->moe_w; sz = (size_t)c.n_layers * p->moe_nw * 4; }
     }
     else if (s == "key_cache" || s == "value_cache") {
         if (layer < 0 || layer >= c.n_layers) return fail(p, B200_ERR_BAD_ARG, "layer out of range");
@@ -3515,7 +3548,7 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
 int b200_time_kernel(b200_plan *p, int32_t which, int32_t reps, float *avg_ms, int64_t *algorithmic_bytes) {
     if (!p || !avg_ms || reps <= 0) return B200_ERR_BAD_ARG;
     if (p->cfg.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "b200_time_kernel is single-GPU only");
-    if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "b200_time_kernel times the dense FFN and attention matrices; a Qwen2-MoE plan has no dense FFN");
+    if (p->is_moe) return fail(p, B200_ERR_UNSUPPORTED, "b200_time_kernel times the dense FFN and attention matrices; a %s plan has no dense FFN", p->moe_name);
     if (which < 0 || which > 4) return fail(p, B200_ERR_BAD_ARG, "unknown kernel id %d", which);
     const b200_config &c = p->cfg;
     const bool q8 = p->wtype == B200_GGML_Q8_0, sf = p->use_f16_stream, fz = p->fuse_norm;

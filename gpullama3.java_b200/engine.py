@@ -111,14 +111,14 @@ def generate_tokens_qwen3(forward: Forward, latest_token: int, start_position: i
 
 
 def loop_for(model_type: str):
-    """The generation loop the reference's model class uses: Qwen3, Qwen2, Qwen2-MoE and DeepSeek-R1-Distill-Qwen run
+    """The generation loop the reference's model class uses: Qwen3, Qwen3-MoE, Qwen2, Qwen2-MoE and DeepSeek-R1-Distill-Qwen run
     generateTokensQwen3 (Qwen3.java, Qwen2.java:95-115, Qwen2MoE.java:84-98), the others generateTokensLlama (Granite's
     generateTokensGranite is generateTokensLlama with forwardGranite, InferenceEngine.java:554-616)."""
     return generate_tokens_qwen3 if _is_qwen_loop(model_type) else generate_tokens_llama
 
 
 def _is_qwen_loop(model_type: str) -> bool:
-    return model_type.upper() in ("QWEN_3", "QWEN_2", "QWEN_2_MOE", "DEEPSEEK_R1_DISTILL_QWEN")
+    return model_type.upper() in ("QWEN_3", "QWEN_3_MOE", "QWEN_2", "QWEN_2_MOE", "DEEPSEEK_R1_DISTILL_QWEN")
 
 
 def _logprob_rows(plan) -> list:

@@ -43,7 +43,7 @@ public final class B200MasterPlan implements AutoCloseable {
             ADDRESS.withName("name"), ADDRESS.withName("data"), JAVA_INT.withName("ggml_type"), JAVA_INT.withName("n_dims"),
             MemoryLayout.sequenceLayout(4, JAVA_LONG).withName("dims"));
 
-    // struct b200_moe_config: 4 x int32 (Qwen2-MoE plans)
+    // struct b200_moe_config: 4 x int32 (Qwen2-MoE and Qwen3-MoE plans)
     private static final StructLayout MOE_CONFIG = MemoryLayout.structLayout(
             JAVA_INT.withName("n_experts"), JAVA_INT.withName("n_experts_used"), JAVA_INT.withName("expert_hidden_dim"), JAVA_INT.withName("shared_hidden_dim"));
 
@@ -120,6 +120,14 @@ public final class B200MasterPlan implements AutoCloseable {
      *  (Qwen2MoEConfiguration); the router, shared-expert gate, stacked experts and shared expert go in `tensors` as in the file. */
     public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int headSize, int[] moe) throws Throwable {
         this(state, model, tensors, ARCH_QWEN2_MOE, headSize, 0, 1, moe, null, false, null, 0);
+    }
+
+    /** Qwen2-MoE or Qwen3-MoE (archId = ARCH_QWEN2_MOE or ARCH_QWEN3_MOE, single GPU).  Qwen3-MoE: moe = {numberOfExperts,
+     *  numberOfExpertsUsed, moeHiddenDim, 0} (no shared expert), headSize = attention.key_length; `tensors` holds Qwen3's attention
+     *  tensors (with attn_q_norm / attn_k_norm), the router and the stacked experts, as in the file.  The top-k weights are
+     *  renormalised to sum to one, and b200_read_buffer("moe_weights") gives k weights per layer. */
+    public B200MasterPlan(State state, Model model, Map<String, GGMLTensorEntry> tensors, int archId, int headSize, int[] moe) throws Throwable {
+        this(state, model, tensors, archId, headSize, 0, 1, moe, null, false, null, 0);
     }
 
     /** Granite (archId = ARCH_GRANITE): granite = {embeddingScale, residualScale, attentionScale, logitScale} (GraniteConfiguration);
@@ -338,7 +346,8 @@ public final class B200MasterPlan implements AutoCloseable {
 
     public static final int PREFILL_EXACT = 0, PREFILL_TENSOR_CORE = 1, PREFILL_TENSOR_CORE_W8A16 = 2, PREFILL_TENSOR_CORE_EXACT = 3;
     // b200_config.arch (include/b200llama.h): Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen pass blk.N.attn_{q,k,v}.bias (F32) with the weights
-    public static final int ARCH_LLAMA = 0, ARCH_QWEN3 = 1, ARCH_PHI3 = 2, ARCH_QWEN2 = 3, ARCH_QWEN2_MOE = 4, ARCH_GRANITE = 5, ARCH_DEVSTRAL = 6;
+    public static final int ARCH_LLAMA = 0, ARCH_QWEN3 = 1, ARCH_PHI3 = 2, ARCH_QWEN2 = 3, ARCH_QWEN2_MOE = 4, ARCH_GRANITE = 5, ARCH_DEVSTRAL = 6,
+            ARCH_QWEN3_MOE = 7;
 
     /** TensorCoreSupport.java's switch: 0 = exact token-by-token prefill (bit-identical KV cache), 1 = TMA + wgmma GEMMs (a Q8_0
      *  plan first builds f16 twins of its matrices, +2 bytes per weight), 2 = the same GEMMs on a Q8_0 plan reading the Q8_0 weights

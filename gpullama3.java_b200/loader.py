@@ -21,6 +21,7 @@ ARCH_QWEN2 = 3  # Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen: Llama's forward + 
 ARCH_QWEN2_MOE = 4  # Qwen1.5-MoE: Qwen2's attention + a routed mixture-of-experts FFN with a shared expert (InferenceCore.java:263-432)
 ARCH_GRANITE = 5  # Granite 3.x: Llama's forward with four muP scales (InferenceCore.forwardGranite, InferenceCore.java:814-921)
 ARCH_DEVSTRAL = 6  # Devstral 2 (mistral3): Llama's forward with an independent head size and a YaRN RoPE table (InferenceCore.java:178-261)
+ARCH_QWEN3_MOE = 7  # Qwen3-MoE (qwen3moe, Qwen3-30B-A3B): Qwen3's attention + routed experts without a shared expert, top-k renormalised
 
 
 @dataclass(frozen=True)
@@ -51,7 +52,7 @@ class Configuration:
     context_length: int
     rms_norm_eps: float
     rope_theta: float
-    # Qwen2-MoE only (Qwen2MoEConfiguration); 0 for every dense model
+    # Qwen2-MoE and Qwen3-MoE only (Qwen2MoEConfiguration; Qwen3-MoE has no shared expert: shared_hidden_dim 0); 0 for every dense model
     n_experts: int = 0
     n_experts_used: int = 0
     expert_hidden_dim: int = 0
@@ -80,6 +81,8 @@ class UnsupportedModel(Exception):
 def detect_model_type(metadata: dict) -> str:
     if metadata.get("general.architecture") == "qwen2moe":  # checked before the name (ModelLoader.java:50)
         return "QWEN_2_MOE"
+    if metadata.get("general.architecture") == "qwen3moe":  # before the name too: a Qwen3-MoE file's name contains "qwen3"
+        return "QWEN_3_MOE"
     name = metadata.get("general.name")
     if name is not None:
         low = name.lower()
@@ -122,14 +125,14 @@ class Model:
 def model_from_tensors(shape, quant: int, tensors: dict, context_length: int) -> Model:
     """In-memory model (bench: synthetic weights never touch the disk)."""
     arch = {"llama": ARCH_LLAMA, "qwen3": ARCH_QWEN3, "phi3": ARCH_PHI3, "qwen2": ARCH_QWEN2, "qwen2moe": ARCH_QWEN2_MOE, "granite": ARCH_GRANITE,
-            "devstral": ARCH_DEVSTRAL}[shape.arch]
-    moe = shape.arch == "qwen2moe"
+            "devstral": ARCH_DEVSTRAL, "qwen3moe": ARCH_QWEN3_MOE}[shape.arch]
+    moe = shape.arch in ("qwen2moe", "qwen3moe")
     cfg = Configuration(arch, "Q8_0" if quant == GGMLType.Q8_0 else "FP16",
                         shape.dim, 0 if moe else shape.hidden, shape.n_layers, shape.n_heads, shape.n_kv_heads, shape.head_size,
                         shape.vocab, context_length, float(shape.eps), float(shape.rope_theta))
     if moe:
         cfg.n_experts, cfg.n_experts_used = shape.n_experts, shape.n_experts_used
-        cfg.expert_hidden_dim, cfg.shared_hidden_dim = shape.expert_hidden, shape.hidden
+        cfg.expert_hidden_dim, cfg.shared_hidden_dim = shape.expert_hidden, shape.hidden if shape.arch == "qwen2moe" else 0
     if shape.arch == "granite":
         for k, v in shape.granite_scales.items():
             setattr(cfg, k, float(np.float32(v)))
@@ -139,7 +142,7 @@ def model_from_tensors(shape, quant: int, tensors: dict, context_length: int) ->
             f, bf, bs, lm, octx = shape.yarn
             cfg.yarn = Yarn(float(np.float32(f)), float(np.float32(bf)), float(np.float32(bs)), float(np.float32(lm)), int(octx))
     typ = {"llama": "LLAMA_3", "qwen3": "QWEN_3", "phi3": "PHI_3", "qwen2": "QWEN_2", "qwen2moe": "QWEN_2_MOE", "granite": "GRANITE",
-           "devstral": "DEVSTRAL_2"}[shape.arch]
+           "devstral": "DEVSTRAL_2", "qwen3moe": "QWEN_3_MOE"}[shape.arch]
     return Model(None, cfg, typ, tensors)
 
 
@@ -206,13 +209,15 @@ def load_model(path: str, context_length: int = -1) -> Model:
             float(md["qwen2.attention.layer_norm_rms_epsilon"]), float(md["qwen2.rope.freq_base"]))
     elif typ == "QWEN_2_MOE":
         cfg = _qwen2moe_configuration(md, g, q, context_length)
+    elif typ == "QWEN_3_MOE":
+        cfg = qwen3moe_configuration(md, g, q, context_length)
     elif typ == "GRANITE":
         cfg = granite_configuration(md, q, context_length)
     elif typ == "DEVSTRAL_2":
         cfg = devstral_configuration(md, q, context_length)
     else:
-        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 / Qwen2-MoE / Granite / "
-                               "Devstral 2 forward passes only)")
+        raise UnsupportedModel(f"model type {typ} is outside the hot-path scope (Llama / Mistral / Qwen3 / Phi-3 / Qwen2 / Qwen2-MoE / Qwen3-MoE / "
+                               "Granite / Devstral 2 forward passes only)")
     return Model(g, cfg, typ)
 
 
@@ -238,6 +243,30 @@ def _qwen2moe_configuration(md: dict, g: GGUFFile, q: str, context_length: int) 
         len(md["tokenizer.ggml.tokens"]), ctx, float(md["qwen2moe.attention.layer_norm_rms_epsilon"]), float(md["qwen2moe.rope.freq_base"]),
         n_experts=int(md["qwen2moe.expert_count"]), n_experts_used=int(md["qwen2moe.expert_used_count"]),
         expert_hidden_dim=expert_hidden, shared_hidden_dim=shared_hidden)
+
+
+def qwen3moe_configuration(md: dict, g: GGUFFile, q: str, context_length: int) -> Configuration:
+    """Qwen3-MoE's configuration from the qwen3moe.* keys: Qwen3's attention geometry (head size = attention.key_length, head_count_kv
+    defaulting to head_count, a value_length that differs is refused as Devstral's is), the context clamped to the model's, the
+    vocabulary size the token list's, hidden_dim 0 (feed_forward_length describes no matrix the MoE FFN reads), and the expert
+    configuration: expert_count, expert_used_count, the expert hidden size from ffn_down_exps dims[0] (a file whose
+    expert_feed_forward_length disagrees is refused) and no shared expert.  FP16 files load; the plan refuses them."""
+    p = "qwen3moe."
+    model_ctx = int(md[p + "context_length"])
+    ctx = model_ctx if (context_length < 0 or model_ctx < context_length) else context_length
+    n_heads = int(md[p + "attention.head_count"])
+    head = int(md[p + "attention.key_length"])
+    if int(md[p + "attention.value_length"]) != head:
+        raise UnsupportedModel(f"qwen3moe.attention.value_length {int(md[p + 'attention.value_length'])} != key_length {head}: V would be read "
+                               "with key_length's width, which would compute this model wrongly")
+    expert_hidden = int(g.tensor_infos["blk.0.ffn_down_exps.weight"].dims[0])
+    if int(md[p + "expert_feed_forward_length"]) != expert_hidden:
+        raise UnsupportedModel(f"qwen3moe.expert_feed_forward_length is {int(md[p + 'expert_feed_forward_length'])} but the experts "
+                               f"(blk.0.ffn_down_exps.weight) have {expert_hidden} hidden units")
+    return Configuration(
+        ARCH_QWEN3_MOE, q, int(md[p + "embedding_length"]), 0, int(md[p + "block_count"]), n_heads, int(md.get(p + "attention.head_count_kv", n_heads)),
+        head, len(md["tokenizer.ggml.tokens"]), ctx, float(md[p + "attention.layer_norm_rms_epsilon"]), float(md[p + "rope.freq_base"]),
+        n_experts=int(md[p + "expert_count"]), n_experts_used=int(md[p + "expert_used_count"]), expert_hidden_dim=expert_hidden, shared_hidden_dim=0)
 
 
 def granite_configuration(md: dict, q: str, context_length: int) -> Configuration:

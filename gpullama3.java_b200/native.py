@@ -37,7 +37,7 @@ class Config(C.Structure):
 
 
 class MoeConfig(C.Structure):
-    """b200_moe_config: the expert configuration of a B200_ARCH_QWEN2_MOE plan."""
+    """b200_moe_config: the expert configuration of a B200_ARCH_QWEN2_MOE or B200_ARCH_QWEN3_MOE plan (shared_hidden_dim 0)."""
     _fields_ = [(n, C.c_int32) for n in ("n_experts", "n_experts_used", "expert_hidden_dim", "shared_hidden_dim")]
 
 
@@ -713,10 +713,11 @@ class NativePlan:
 
     def moe_routing(self):
         """(ids int32 [layer, k], weights float32 [layer, k + 1]) of the last step: the selected experts in selection order, their
-        routing weights, then the shared-expert weight."""
+        routing weights, then the shared-expert weight.  Without a shared expert (Qwen3-MoE) the weights are [layer, k]."""
         k = self.moe.n_experts_used
+        nw = k + 1 if self.moe.shared_hidden_dim else k
         ids = self.read_buffer("moe_ids", self.cfg.n_layers * k, np.int32).reshape(self.cfg.n_layers, k)
-        w = self.read_buffer("moe_weights", self.cfg.n_layers * (k + 1)).reshape(self.cfg.n_layers, k + 1)
+        w = self.read_buffer("moe_weights", self.cfg.n_layers * nw).reshape(self.cfg.n_layers, nw)
         return ids, w
 
     def upload_info(self) -> dict:

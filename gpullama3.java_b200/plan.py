@@ -83,7 +83,7 @@ class B200MasterPlan:
             tp_shard_plan(model.configuration, tp_size)  # raises early on shapes that do not split
         c = model.configuration
         moe = granite = None
-        if c.n_experts:  # Qwen2-MoE: b200_plan_create_moe
+        if c.n_experts:  # Qwen2-MoE / Qwen3-MoE (shared_hidden_dim 0): b200_plan_create_moe
             moe = native.MoeConfig(c.n_experts, c.n_experts_used, c.expert_hidden_dim, c.shared_hidden_dim)
         if c.arch == ARCH_GRANITE:  # Granite: b200_plan_create_granite
             granite = native.GraniteConfig(c.embedding_scale, c.residual_scale, c.attention_scale, c.logit_scale)
@@ -282,8 +282,8 @@ class B200MasterPlan:
         return self._native.chunk_rows()
 
     def moe_routing(self):
-        """Qwen2-MoE plans: (ids [layer, k], weights [layer, k + 1]) of the last step (selected experts in selection order, their
-        routing weights, then the shared-expert weight)."""
+        """MoE plans: (ids [layer, k], weights [layer, k + 1]) of the last step (selected experts in selection order, their
+        routing weights, then the shared-expert weight); Qwen3-MoE has no shared expert, its weights are [layer, k]."""
         return self._native.moe_routing()
 
     def kv_reset(self):

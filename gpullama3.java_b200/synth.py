@@ -5,7 +5,8 @@ norm weights F32, matrices and the embedding table in the model quantisation, me
 per ``LlamaModelLoader.java:47-63`` / ``Qwen3ModelLoader.java:48-74`` / ``Qwen2ModelLoader.java:48-73``.  Qwen2 files
 add F32 biases ``blk.N.attn_{q,k,v}.bias`` (``Qwen2ModelLoader.java:100-102``).  Qwen2-MoE files (``qwen2moe``) replace the dense FFN by
 an F32 router ``ffn_gate_inp``, an F32 shared-expert gate ``ffn_gate_inp_shexp``, stacked 3-D expert tensors ``ffn_{gate,up,down}_exps``
-and the shared expert ``ffn_{gate,up,down}_shexp``, as llama.cpp writes them (``Qwen2MoEModelLoader.java``).
+and the shared expert ``ffn_{gate,up,down}_shexp``, as llama.cpp writes them (``Qwen2MoEModelLoader.java``).  Qwen3-MoE files (``qwen3moe``)
+carry Qwen3's attention tensors (``attn_q_norm`` / ``attn_k_norm``, no biases) and the router and stacked experts only: no ``*_shexp``.
 """
 from __future__ import annotations
 
@@ -18,9 +19,9 @@ from .gguf import GGMLType, write_gguf
 
 @dataclass(frozen=True)
 class Shape:
-    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2" | "qwen2moe" | "granite" | "devstral" (GGUF architecture mistral3)
+    arch: str  # "llama" | "qwen3" | "phi3" | "qwen2" | "qwen2moe" | "qwen3moe" | "granite" | "devstral" (GGUF architecture mistral3)
     dim: int
-    hidden: int  # qwen2moe: the shared expert's hidden size
+    hidden: int  # qwen2moe: the shared expert's hidden size; qwen3moe: the file's feed_forward_length, which no MoE matrix uses
     n_layers: int
     n_heads: int
     n_kv_heads: int
@@ -50,7 +51,8 @@ class Shape:
 
     def matmul_elements(self) -> int:
         """Weight elements streamed per decoded token (SURVEY.md 8d)."""
-        per_layer = 2 * self.q_dim * self.dim + 2 * self.kv_dim * self.dim + 3 * self.hidden * self.dim
+        dense_ffn = 0 if self.arch == "qwen3moe" else self.hidden  # qwen2moe: the shared expert
+        per_layer = 2 * self.q_dim * self.dim + 2 * self.kv_dim * self.dim + 3 * dense_ffn * self.dim
         per_layer += 3 * self.n_experts_used * self.expert_hidden * self.dim  # qwen2moe: the k routed experts (active weights only)
         return self.n_layers * per_layer + self.vocab * self.dim
 
@@ -110,6 +112,14 @@ SHAPES = {
     "tiny-qwen2moe-gqa": Shape("qwen2moe", 512, 512, 2, 8, 2, 64, 512, True, 1000000.0, 1e-6, 8192, 16, 8, 256),
     "mid-qwen1.5-moe-a2.7b": Shape("qwen2moe", 2048, 5632, 2, 16, 16, 128, 8192, False, 1000000.0, 1e-6, 8192, 60, 4, 1408),
     "qwen1.5-moe-a2.7b": Shape("qwen2moe", 2048, 5632, 24, 16, 16, 128, 151936, False, 1000000.0, 1e-6, 8192, 60, 4, 1408),
+    # Qwen3-MoE (Qwen3 attention, no shared expert, renormalised top-k): GQA with q width 512 != dim 256 and top-2 of 8; top-8 of 16 (the
+    # k cap); a tied classifier; the real Qwen3-30B-A3B layer geometry (dim 2048, 32 / 4 heads of 128, 128 experts, top-8, expert hidden
+    # 768) cut to 2 layers, and the whole 48-layer model (tools/qwen3moe_bench.py).  `hidden` is the file's feed_forward_length.
+    "tiny-qwen3moe": Shape("qwen3moe", 256, 768, 2, 4, 2, 128, 512, False, 1000000.0, 1e-6, 40960, 8, 2, 256),
+    "tiny-qwen3moe-k8": Shape("qwen3moe", 512, 1024, 2, 8, 2, 64, 512, False, 1000000.0, 1e-6, 40960, 16, 8, 256),
+    "tiny-qwen3moe-tied": Shape("qwen3moe", 256, 768, 2, 4, 4, 64, 640, True, 1000000.0, 1e-6, 40960, 8, 4, 512),
+    "mid-qwen3-30b-a3b": Shape("qwen3moe", 2048, 6144, 2, 32, 4, 128, 151936, False, 1000000.0, 1e-6, 40960, 128, 8, 768),
+    "qwen3-30b-a3b": Shape("qwen3moe", 2048, 6144, 48, 32, 4, 128, 151936, False, 1000000.0, 1e-6, 40960, 128, 8, 768),
     # Granite 3.x (muP scales, tied classifier): multi-head with head size 64 and an odd vocabulary, GQA with head size 128; 2-layer cuts
     # of the Granite-3.x-2B and -8B layer geometries with their 49155-token vocabulary, and the whole 8B model (tools/granite_bench.py)
     "tiny-granite": Shape("granite", 256, 512, 2, 4, 4, 64, 515, True, 10000.0, 1e-5, 4096),
@@ -186,7 +196,7 @@ def gpt2_byte_symbols() -> list[str]:
 def build_vocab(vocab_size: int, arch: str = "llama", seed: int = 1234):
     """(tokens, merge_lines, token_types, base_tokens): 256 byte symbols, BPE merges trained on a small fixed corpus
     (ids in merge order, so the vocabulary is a consistent BPE vocabulary), padding tokens, then the special tokens."""
-    specials = QWEN3_SPECIALS if arch in ("qwen3", "qwen2", "qwen2moe") else LLAMA_SPECIALS
+    specials = QWEN3_SPECIALS if arch in ("qwen3", "qwen2", "qwen2moe", "qwen3moe") else LLAMA_SPECIALS
     n_merges = vocab_size - 256 - len(specials)
     if n_merges < 0:
         raise ValueError("vocabulary too small for the byte symbols and the special tokens")
@@ -233,7 +243,7 @@ def build_vocab(vocab_size: int, arch: str = "llama", seed: int = 1234):
     types = [1] * base + [3] * len(specials)  # 1 normal, 3 control
     for i in range(base - pad, base):
         types[i] = 5
-    if arch in ("qwen3", "qwen2", "qwen2moe"):
+    if arch in ("qwen3", "qwen2", "qwen2moe", "qwen3moe"):
         for t in ("<think>", "</think>", "<tool_call>", "</tool_call>"):
             types[tokens.index(t)] = 4  # user defined: displayed (Qwen3Tokenizer.shouldDisplayToken)
     return tokens, merges, types, base
@@ -255,9 +265,14 @@ def metadata_for(shape: Shape, quant: int, name: str) -> dict:
         f"{a}.rope.freq_base": float(shape.rope_theta),
         f"{a}.vocab_size": shape.vocab,
     }
-    if a == "qwen3":
-        md["qwen3.attention.key_length"] = shape.head_size
-        md["qwen3.attention.value_length"] = shape.head_size
+    if a in ("qwen3", "qwen3moe"):
+        md[f"{a}.attention.key_length"] = shape.head_size
+        md[f"{a}.attention.value_length"] = shape.head_size
+    if a == "qwen3moe":  # llama.cpp's qwen3moe keys; no shared expert
+        md["qwen3moe.expert_count"] = shape.n_experts
+        md["qwen3moe.expert_used_count"] = shape.n_experts_used
+        md["qwen3moe.expert_feed_forward_length"] = shape.expert_hidden
+        del md["qwen3moe.vocab_size"]  # the vocabulary size is the token list's
     if a == "qwen2moe":  # Qwen2MoEModelLoader.createConfiguration
         md["qwen2moe.expert_count"] = shape.n_experts
         md["qwen2moe.expert_used_count"] = shape.n_experts_used
@@ -281,7 +296,7 @@ def metadata_for(shape: Shape, quant: int, name: str) -> dict:
             md["mistral3.rope.scaling.yarn_beta_slow"] = float(bs)
             md["mistral3.rope.scaling.yarn_log_multiplier"] = float(lm)
             md["mistral3.rope.scaling.original_context_length"] = int(octx)
-    if shape.vocab <= 4096 or a in ("qwen2", "qwen2moe"):  # tokenizer section (Qwen2 takes its vocabulary size from the token list) (GGUF keys the loaders read: tokenizer.ggml.tokens / merges / token_type)
+    if shape.vocab <= 4096 or a in ("qwen2", "qwen2moe", "qwen3moe"):  # tokenizer section (Qwen2 takes its vocabulary size from the token list) (GGUF keys the loaders read: tokenizer.ggml.tokens / merges / token_type)
         tokens, merges, types, base = build_vocab(shape.vocab, a)
         md["tokenizer.ggml.model"] = "gpt2"
         md["tokenizer.ggml.tokens"] = tokens
@@ -319,9 +334,19 @@ def tensor_plan(shape: Shape, quant: int):
             t += [(p + "attn_q.bias", GGMLType.F32, (shape.q_dim,), b),
                   (p + "attn_k.bias", GGMLType.F32, (shape.kv_dim,), b),
                   (p + "attn_v.bias", GGMLType.F32, (shape.kv_dim,), b)]
-        if shape.arch == "qwen3":
+        if shape.arch in ("qwen3", "qwen3moe"):
             t += [(p + "attn_q_norm.weight", GGMLType.F32, (shape.head_size,), "n"),
                   (p + "attn_k_norm.weight", GGMLType.F32, (shape.head_size,), "n")]
+        if shape.arch == "qwen3moe":  # llama.cpp's qwen3moe tensors: the router and the stacked experts, no shared expert
+            E, he = shape.n_experts, shape.expert_hidden
+            t += [
+                (p + "ffn_norm.weight", GGMLType.F32, (shape.dim,), "n"),
+                (p + "ffn_gate_inp.weight", GGMLType.F32, (shape.dim, E), "r"),
+                (p + "ffn_gate_exps.weight", quant, (shape.dim, he, E), "w"),
+                (p + "ffn_up_exps.weight", quant, (shape.dim, he, E), "w"),
+                (p + "ffn_down_exps.weight", quant, (he, shape.dim, E), "w"),
+            ]
+            continue
         if shape.arch == "qwen2moe":  # llama.cpp's qwen2moe tensors; the stacked experts are [E][rows][cols] (dims innermost first)
             E, he = shape.n_experts, shape.expert_hidden
             t += [
@@ -444,7 +469,8 @@ def write_model(path: str, shape_name: str, quant: int, seed: int = 1234, w_std:
                 display_name: str | None = None):
     shape = SHAPES[shape_name]
     name = display_name or {"llama": "Llama synthetic ", "qwen3": "Qwen3 synthetic ", "phi3": "Phi3 synthetic ", "qwen2": "Qwen2 synthetic ",
-                            "qwen2moe": "Qwen1.5 MoE synthetic ", "granite": "Granite synthetic ", "devstral": "Devstral synthetic "}[shape.arch] + shape_name
+                            "qwen2moe": "Qwen1.5 MoE synthetic ", "qwen3moe": "Qwen3 MoE synthetic ", "granite": "Granite synthetic ",
+                            "devstral": "Devstral synthetic "}[shape.arch] + shape_name
     write_gguf(path, metadata_for(shape, quant, name), build_tensors(shape, quant, seed, w_std))
     return shape
 

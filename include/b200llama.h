@@ -51,6 +51,9 @@ extern "C" {
                               * tensors and forward with an independent head size (n_heads * head_size may differ from dim: q has that
                               * width, RoPE rotates interleaved pairs over it, Wo takes it as columns) and a RoPE table that may be
                               * YaRN-scaled (b200_yarn_config).  Created with b200_plan_create_devstral only. */
+#define B200_ARCH_QWEN3_MOE 7 /* Qwen3-MoE (GGUF architecture qwen3moe: Qwen3-30B-A3B, Qwen3-Coder-30B-A3B): Qwen3's attention (q/k
+                               * RMSNorm, NeoX RoPE, head size of its own) and a mixture-of-experts FFN without a shared expert, the
+                               * top-k weights renormalised to sum to one.  Created with b200_plan_create_moe only, shared_hidden_dim 0. */
 
 /* GGML tensor type ids accepted for weights (tensor/GGMLType.java:5-20) */
 #define B200_GGML_F32 0
@@ -94,13 +97,13 @@ typedef struct b200_tensor {
     int64_t dims[4];
 } b200_tensor;
 
-/* Expert configuration of a B200_ARCH_QWEN2_MOE plan (Qwen2MoEModelLoader.createConfiguration).  b200_config.hidden_dim is unused
- * (0, as the reference's configuration has it). */
+/* Expert configuration of a B200_ARCH_QWEN2_MOE or B200_ARCH_QWEN3_MOE plan (Qwen2MoEModelLoader.createConfiguration).
+ * b200_config.hidden_dim is unused (0, as the reference's configuration has it). */
 typedef struct b200_moe_config {
     int32_t n_experts;         /* expert_count (E), 1..256 */
     int32_t n_experts_used;    /* expert_used_count (k), 1..min(E, 8) */
     int32_t expert_hidden_dim; /* ffn_down_exps dims[0] (He) */
-    int32_t shared_hidden_dim; /* ffn_gate_shexp dims[1] (Hs) */
+    int32_t shared_hidden_dim; /* ffn_gate_shexp dims[1] (Hs), > 0; B200_ARCH_QWEN3_MOE: 0 (no shared expert) */
 } b200_moe_config;
 
 /* The four scalars of a B200_ARCH_GRANITE plan (GraniteConfiguration).  Each is ONE float multiply, rounded once, where the CPU path
@@ -137,8 +140,8 @@ typedef struct b200_plan b200_plan;
 int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t n_tensors,
                      int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
 
-/* b200_plan_create for cfg->arch == B200_ARCH_QWEN2_MOE (b200_plan_create refuses that arch with B200_ERR_BAD_ARG, and this call
- * every other).  Per layer it requires, besides Qwen2's attention tensors and biases and the two norms (dims[0] innermost, as
+/* b200_plan_create for cfg->arch == B200_ARCH_QWEN2_MOE or B200_ARCH_QWEN3_MOE (b200_plan_create refuses those archs with
+ * B200_ERR_BAD_ARG, and this call every other).  B200_ARCH_QWEN2_MOE:  Per layer it requires, besides Qwen2's attention tensors and biases and the two norms (dims[0] innermost, as
  * llama.cpp writes them):
  *   blk.N.ffn_gate_inp.weight        F32 [dim, E]          the router
  *   blk.N.ffn_gate_inp_shexp.weight  F32 [dim]             the shared-expert gate
@@ -152,7 +155,18 @@ int b200_plan_create(const b200_config *cfg, const b200_tensor *tensors, int32_t
  * 1 / (1 + exp(-g)).  B200_ERR_BAD_ARG: a missing tensor, wrong dims, n_experts_used outside 1..min(E, 8).  B200_ERR_UNSUPPORTED
  * (reason in the message): a router or shared gate that is not F32, FP16 weights, tp_size > 1, hidden sizes the stream layout
  * cannot cut.  The plan decodes through the CUDA graph (not the persistent kernel), prefills through
- * the exact path only, and refuses b200_set_decode_slots (n_slots > 0) and b200_time_kernel with B200_ERR_UNSUPPORTED. */
+ * the exact path only, and refuses b200_set_decode_slots (n_slots > 0) and b200_time_kernel with B200_ERR_UNSUPPORTED.
+ *
+ * B200_ARCH_QWEN3_MOE (moe->shared_hidden_dim must be 0, else B200_ERR_BAD_ARG): Qwen3's attention tensors (no biases; the F32
+ * blk.N.attn_q_norm.weight and attn_k_norm.weight of head_size floats, head_size = attention.key_length, so n_heads * head_size may
+ * differ from dim) and, per layer, only
+ *   blk.N.ffn_gate_inp.weight        F32 [dim, E]          the router
+ *   blk.N.ffn_{gate,up}_exps.weight  [dim, He, E]          the routed experts, stacked [E][He][dim]
+ *   blk.N.ffn_down_exps.weight       [He, dim, E]          stacked [E][dim][He]
+ * Each layer's FFN: the F32 router dot products (sequential, no FMA), softmax, top-k by first strict maximum (ties to the lower
+ * index), then the renormalisation s = 0, s += p_j over the picks in selection order, w_j = p_j / s, and the k routed experts'
+ * SwiGLU FFNs added to x in selection order (x[i] = w_j * y[i] + x[i]).  The refusals are those of B200_ARCH_QWEN2_MOE, naming
+ * Qwen3-MoE. */
 int b200_plan_create_moe(const b200_config *cfg, const b200_moe_config *moe, const b200_tensor *tensors, int32_t n_tensors,
                          int32_t prefill_batch_size, int32_t device, b200_plan **out, char *err, size_t err_len);
 
@@ -518,7 +532,8 @@ int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_ste
  * q rotated in place (after its Qwen2 bias), k before RoPE and v, both before their Qwen2 bias), "pf_a16" (f16 bits, the FFN input), "pf_att16" (f16 bits, attention output),
  * "pf_h16" (f16 bits, SwiGLU output).  Qwen2-MoE plans: "hb", "hq", "hs" hold the virtual hidden vector of the last layer (the shared
  * expert's units, then each routed slot's, shared_hidden_dim + n_experts_used * expert_hidden_dim units), "moe_ids" (int32 [layer][k], the experts the last step selected, in
- * selection order) and "moe_weights" (f32 [layer][k + 1], their routing weights, then the shared-expert weight).
+ * selection order) and "moe_weights" (f32 [layer][k + 1], their routing weights, then the shared-expert weight).  Qwen3-MoE plans: the
+ * same without the shared expert: n_experts_used * expert_hidden_dim units, and "moe_weights" is f32 [layer][k], the renormalised weights.
  * "rope_cr" / "rope_ci": the RoPE table every decode and prefill kernel reads (f32 [context_length][head_size / 2]).
  * Copies min(bytes, buffer size). */
 int b200_read_buffer(b200_plan *plan, const char *name, int32_t layer, void *dst, size_t bytes);

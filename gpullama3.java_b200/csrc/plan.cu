@@ -167,8 +167,13 @@ struct b200_plan {
     bool has_yarn = false;
     b200_yarn_config yarn{};
 
-    PrefillCtx prefill;
-    PrefillI8Ctx pi8; // B200_PREFILL_TENSOR_CORE_EXACT (prefill_i8.cuh); its mode is prefill.mode like the other three
+    // The prefill modes (B200_PREFILL_*, PREFILL_MODE_NAMES): the active one, and per mode whether its buffers and tensor maps are
+    // built or why not.  exact is always ready; b200_set_prefill_mode builds the others (build() an FP16 plan's tensor_core) and
+    // selects a mode only once it is ready.
+    int pf_mode = B200_PREFILL_EXACT;
+    struct PrefillMode { bool ready; const char *why; } pf[4] = {{true, ""}, {false, ""}, {false, ""}, {false, ""}};
+    PrefillCtx prefill; // tensor_core and tensor_core_w8a16 (prefill.cuh)
+    PrefillI8Ctx pi8;   // tensor_core_exact (prefill_i8.cuh)
     // persistent decode kernel
     bool pd_ok = false;           // the plan fits the kernel's restrictions
     std::string pd_why;           // ... or why not
@@ -1369,6 +1374,7 @@ int size_rings(b200_plan *p) {
     return B200_OK;
 }
 
+const char *prefill_why(const b200_plan *p, int mode);
 int prefill_init(b200_plan *p);
 
 // RoPE.precomputeFreqsCisYaRN (RoPE.java:39-83) with Java's float / double boundaries taken literally: every float expression is
@@ -1870,10 +1876,16 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
     }
     if ((rc = size_rings(p))) return rc;
     if ((rc = set_smem_attrs(p))) return rc;
+    // tensor_core: why the plan cannot run it, or on a Q8_0 plan that it is opt-in; an FP16 plan that can run it builds and selects it
+    auto &tc = p->pf[B200_PREFILL_TENSOR_CORE];
+    if (!(tc.why = prefill_why(p, B200_PREFILL_TENSOR_CORE)) && p->wtype == B200_GGML_Q8_0)
+        tc.why = "Q8_0 plan: the tensor-core prefill is opt-in (b200_set_prefill_mode builds f16 twins of the weight matrices, +2 bytes per weight)";
     if (c.tp_size > 1) { CK(cudaStreamSynchronize(p->stream)); return B200_OK; } // graphs are captured by b200_tp_attach
     if ((rc = capture_all(p))) return rc;
-    if (p->prefill_batch > 1)
+    if (!tc.why) {
         if ((rc = prefill_init(p))) return rc;
+        if (tc.ready) p->pf_mode = B200_PREFILL_TENSOR_CORE;
+    }
     CK(cudaStreamSynchronize(p->stream));
     return B200_OK;
 }
@@ -1882,28 +1894,64 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
 static const char *const MOE_PREFILL_WHY = "Qwen2-MoE plans have no tensor-core prefill: prompts go through the exact token-by-token prefill";
 static const char *const MOE3_PREFILL_WHY = "Qwen3-MoE plans have no tensor-core prefill: prompts go through the exact token-by-token prefill";
 static const char *moe_prefill_why(const b200_plan *p) { return p->moe_shared ? MOE_PREFILL_WHY : MOE3_PREFILL_WHY; }
-// What both tensor-core modes need of the plan's shape; nullptr when the chunk GEMMs and the attention can run it.
-static const char *prefill_shape_why(const b200_plan *p) {
+
+// The geometry of W as Q8_0 tiles: W itself, or for a resident matrix the tiles a Q8_0-tile plan of the same file holds, which
+// k_kq_tiles_to_q8 writes into the prefill's scratch before W's GEMM.
+TileMat q8_geometry(const TileMat &W) { return W.fmt ? tile_geometry(W.rows, W.cols, 0) : W; }
+
+// Why the plan cannot run prefill mode `mode` (nullptr: it can), decided before anything is allocated: MoE, then resident weights,
+// then the prefill batch size, the weight type, tensor parallelism, the shape, the stream segments and the tensor-map encoder, in
+// the order each mode has always checked them.
+const char *prefill_why(const b200_plan *p, int mode) {
     const b200_config &g = p->cfg;
     const int kv_mul = g.n_heads / g.n_kv_heads, nqkv = p->qd + 2 * p->kvd;
+    const bool exact = mode == B200_PREFILL_TENSOR_CORE_EXACT, w8a16 = mode == B200_PREFILL_TENSOR_CORE_W8A16;
+    auto segs_ok = [&] { // every Q8_0 stream's segment (as Q8_0 tiles) a whole number of GEMM k-blocks
+        for (const LayerW &L : p->layers)
+            for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
+                if (q8_geometry(*t).seg % pg::BK) return false;
+        return true;
+    };
+    if (mode == B200_PREFILL_EXACT) return nullptr;
     if (p->is_moe) return moe_prefill_why(p);
+    if (p->resident && !exact)
+        return "this plan keeps K-quant weights resident: the f16 and W8A16 tensor-core prefills read f16 matrices or Q8_0 tiles it does not "
+               "hold; tensor_core_exact expands each resident matrix to Q8_0 tiles before its GEMM";
+    if (p->prefill_batch <= 1) return "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
+    if (w8a16 && p->wtype != B200_GGML_Q8_0) return "W8A16 prefill needs a Q8_0 plan (FP16 plans run the tensor-core prefill on their own f16 matrices)";
+    if (exact && p->wtype != B200_GGML_Q8_0)
+        return "the bit-exact tensor-core prefill needs a Q8_0 plan (an FP16 plan's CPU dot products are FP16 lane chains, not int8 block sums)";
     if (g.tp_size > 1) return "tensor-core prefill is single-GPU";
+    if (exact) {
+        if (g.dim % 64 || p->qd % 64 || nqkv % 64) return "the bit-exact tensor-core prefill needs dim, q width and q+k+v width multiples of 64";
+        if (!segs_ok()) return "the bit-exact tensor-core prefill needs Q8_0 stream segments that are multiples of 64 columns";
+        return pg::encode_fn() ? nullptr : "cuTensorMapEncodeTiled not available from the driver";
+    }
     if (g.head_size != 64 && g.head_size != 128) return "tensor-core prefill supports head sizes 64 and 128";
     if (g.n_heads % g.n_kv_heads || kv_mul > 64) return "tensor-core prefill needs n_heads % n_kv_heads == 0 and a GQA ratio <= 64";
     if (g.dim % 128 || p->qd % 128 || nqkv % 128 || g.hidden_dim % 64) return "tensor-core prefill needs dim, q width and q+k+v width multiples of 128, hidden a multiple of 64";
     if (!pg::encode_fn()) return "cuTensorMapEncodeTiled not available from the driver";
+    if (w8a16 && !segs_ok()) return "W8A16 prefill needs Q8_0 stream segments that are multiples of 64 columns";
     return nullptr;
 }
 
-// The chunk's scratch buffers, their tensor maps and the attention kernels' shared-memory attributes: allocated once per
-// plan, shared by both tensor-core modes.  *ok = false if a tensor map was rejected.
+// The end of a mode's init: the mode is ready, or refused with the encoder's rejection if one of its tensor maps was not accepted.
+int prefill_built(b200_plan *p, int mode, bool maps_ok) {
+    p->pf[mode] = maps_ok ? b200_plan::PrefillMode{true, ""} : b200_plan::PrefillMode{false, "cuTensorMapEncodeTiled rejected a tensor map"};
+    return B200_OK;
+}
+
+// The chunk's scratch buffers, their tensor maps, both modes' per-layer map slots and the attention kernels' shared-memory
+// attributes: allocated once per plan, shared by both tensor-core modes.  *ok = false if a tensor map was rejected.
 static int prefill_scratch(b200_plan *p, bool *ok) {
     PrefillCtx &c = p->prefill;
     const b200_config &g = p->cfg;
     const int nqkv = p->qd + 2 * p->kvd;
     *ok = true;
     if (c.bpad) return B200_OK;
-    c.bpad = (c.batch + pg::BM - 1) / pg::BM * pg::BM; // whole 128-row GEMM tiles
+    c.bpad = (p->prefill_batch + pg::BM - 1) / pg::BM * pg::BM; // whole 128-row GEMM tiles
+    c.maps.resize(g.n_layers);
+    c.maps_q8.resize(g.n_layers);
     int rc;
     if ((rc = dalloc(p, &c.X, (size_t)c.bpad * g.dim * 4))) return rc;
     if ((rc = dalloc(p, &c.QKV, (size_t)c.bpad * nqkv * 4))) return rc;
@@ -1928,55 +1976,14 @@ static int prefill_scratch(b200_plan *p, bool *ok) {
     });
 }
 
-int prefill_init(b200_plan *p) {
-    PrefillCtx &c = p->prefill;
-    const b200_config &g = p->cfg;
-    c.batch = p->prefill_batch;
-    c.ready = false;
-    if (c.mode == B200_PREFILL_TENSOR_CORE) c.mode = B200_PREFILL_EXACT;
-    const int nqkv = p->qd + 2 * p->kvd;
-    if (p->wtype != B200_GGML_F16 && !p->f16_copies) {
-        c.why = "Q8_0 plan: the tensor-core prefill is opt-in (b200_set_prefill_mode builds f16 twins of the weight matrices, +2 bytes per weight)";
-        return B200_OK;
-    }
-    if ((c.why = prefill_shape_why(p))) return B200_OK;
-    bool ok;
-    int rc;
-    if ((rc = prefill_scratch(p, &ok))) return rc;
-    c.maps.resize(g.n_layers);
-    for (int l = 0; ok && l < g.n_layers; l++) {
-        const LayerW &L = p->layers[l];
-        PrefillLayerMaps &m = c.maps[l];
-        ok = pg::make_map(&m.qkv, L.qkv.qs, nqkv, g.dim, pg::BN) == 0 && pg::make_map(&m.wo, L.wo.qs, g.dim, p->qd, pg::BN) == 0 &&
-             pg::make_map(&m.w1, L.w1.qs, g.hidden_dim, g.dim, pg::BN / 2) == 0 && pg::make_map(&m.w3, L.w3.qs, g.hidden_dim, g.dim, pg::BN / 2) == 0 &&
-             pg::make_map(&m.w2, L.w2.qs, g.dim, g.hidden_dim, pg::BN) == 0;
-    }
-    if (!ok) { c.why = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
-    c.ready = true;
-    c.mode = B200_PREFILL_TENSOR_CORE;
-    c.why = "";
-    return B200_OK;
-}
-
 // W8A16: the GEMMs read B from the tile-major Q8_0 streams the decode kernels use (L.tqkv, L.two, L.tgu, L.tw2) -- no
 // per-weight memory.  Built on the first b200_set_prefill_mode(TENSOR_CORE_W8A16).
 int prefill_init_q8(b200_plan *p) {
     PrefillCtx &c = p->prefill;
     const b200_config &g = p->cfg;
-    c.batch = p->prefill_batch;
-    if (p->prefill_batch <= 1) { c.why_q8 = "the plan was created without a prefill batch size (prefill_batch_size <= 1)"; return B200_OK; }
-    if (p->wtype != B200_GGML_Q8_0) { c.why_q8 = "W8A16 prefill needs a Q8_0 plan (FP16 plans run the tensor-core prefill on their own f16 matrices)"; return B200_OK; }
-    if (g.tp_size > 1) { c.why_q8 = "tensor-core prefill is single-GPU"; return B200_OK; }
-    if ((c.why_q8 = prefill_shape_why(p))) return B200_OK;
-    for (int l = 0; l < g.n_layers; l++) {
-        const LayerW &L = p->layers[l];
-        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
-            if (t->seg % pg::BK) { c.why_q8 = "W8A16 prefill needs Q8_0 stream segments that are multiples of 64 columns"; return B200_OK; }
-    }
     bool ok;
     int rc;
     if ((rc = prefill_scratch(p, &ok))) return rc;
-    c.maps_q8.resize(g.n_layers);
     for (int l = 0; ok && l < g.n_layers; l++) {
         const LayerW &L = p->layers[l];
         PrefillQ8Maps &m = c.maps_q8[l];
@@ -1985,19 +1992,15 @@ int prefill_init_q8(b200_plan *p) {
         };
         ok = mk(&m.qkv_q, &m.qkv_s, L.tqkv) && mk(&m.wo_q, &m.wo_s, L.two) && mk(&m.gu_q, &m.gu_s, L.tgu) && mk(&m.w2_q, &m.w2_s, L.tw2);
     }
-    if (!ok) { c.why_q8 = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
-    c.q8_ready = true;
-    c.why_q8 = "";
-    return B200_OK;
+    return prefill_built(p, B200_PREFILL_TENSOR_CORE_W8A16, ok);
 }
 
 // Q8_0 plan: f16 twins of the weight matrices, dequantised on the device from the tile-major stream (value = f16(q * scale),
 // Q8_0FloatTensor.getFloat rounded once) -- the B operands of the tensor-core GEMMs; the reference's Q8_0 MMA prefill also
-// feeds FP16 tiles (LlamaQ8_0LayersBatchPrefillMMA.java).  Built on the first b200_set_prefill_mode(TENSOR_CORE).
+// feeds FP16 tiles (LlamaQ8_0LayersBatchPrefillMMA.java).  Built once the plan is found able to run tensor_core.
 int build_f16_twins(b200_plan *p) {
     const b200_config &c = p->cfg;
     if (p->f16_copies) return B200_OK;
-    if (p->wtype != B200_GGML_Q8_0 || c.tp_size > 1) return fail(p, B200_ERR_UNSUPPORTED, "f16 twins need a single-GPU Q8_0 plan");
     for (int l = 0; l < c.n_layers; l++) {
         LayerW &L = p->layers[l];
         int rc;
@@ -2018,6 +2021,25 @@ int build_f16_twins(b200_plan *p) {
     CK(cudaStreamSynchronize(p->stream));
     p->f16_copies = true;
     return B200_OK;
+}
+
+// tensor_core: on a Q8_0 plan the f16 twins first, then the chunk scratch and the f16 matrices' tensor maps.
+int prefill_init(b200_plan *p) {
+    PrefillCtx &c = p->prefill;
+    const b200_config &g = p->cfg;
+    const int nqkv = p->qd + 2 * p->kvd;
+    int rc;
+    if (p->wtype == B200_GGML_Q8_0 && (rc = build_f16_twins(p))) return rc;
+    bool ok;
+    if ((rc = prefill_scratch(p, &ok))) return rc;
+    for (int l = 0; ok && l < g.n_layers; l++) {
+        const LayerW &L = p->layers[l];
+        PrefillLayerMaps &m = c.maps[l];
+        ok = pg::make_map(&m.qkv, L.qkv.qs, nqkv, g.dim, pg::BN) == 0 && pg::make_map(&m.wo, L.wo.qs, g.dim, p->qd, pg::BN) == 0 &&
+             pg::make_map(&m.w1, L.w1.qs, g.hidden_dim, g.dim, pg::BN / 2) == 0 && pg::make_map(&m.w3, L.w3.qs, g.hidden_dim, g.dim, pg::BN / 2) == 0 &&
+             pg::make_map(&m.w2, L.w2.qs, g.dim, g.hidden_dim, pg::BN) == 0;
+    }
+    return prefill_built(p, B200_PREFILL_TENSOR_CORE, ok);
 }
 
 // A chunk of the tensor-core prefill (prefill_chunk): the device tables of prefill.cuh, the f16 scratch the sequences' regions live
@@ -2041,10 +2063,23 @@ int prefill_forward(b200_plan *p, int n, const PfChunk &ck) {
     const size_t ctx_kv = (size_t)g.context_length * p->kvd, slot_stride = (size_t)g.n_layers * ctx_kv;
     // k_pf_attention_mma_packed scales q by this times log2(e): 1/sqrt(head size), or Granite's attentionScale
     const float inv_sqrt_hs = (p->kflags & KF_ATTSCALE) ? p->mup.attention_scale : (float)(1.0 / sqrt((double)g.head_size));
-    int nl = 0;
+    int nl = 0, rc;
     constexpr int ST = pg::GEMM_STAGES;
-    const bool q8 = c.mode == B200_PREFILL_TENSOR_CORE_W8A16; // B from the Q8_0 streams (c.maps_q8) instead of the f16 matrices (c.maps)
-    using pg::B_Q8;
+    const bool q8 = p->pf_mode == B200_PREFILL_TENSOR_CORE_W8A16;
+    // One GEMM, counted: B through the f16 matrices' maps b / b2 (gate/up: W1, W3; c.maps) or, W8A16, through the quant / scale
+    // maps bq / bs of the Q8_0 stream W (c.maps_q8)
+    auto gemm = [&](auto MODE, const char *name, const CUtensorMap &a, const CUtensorMap &b, const CUtensorMap &b2, const CUtensorMap &bq,
+                    const CUtensorMap &bs, const TileMat &W, const CUtensorMap &mc, void *C, int ldc, int n_tiles, int K, int sp, float oscale) {
+        constexpr int M = decltype(MODE)::value;
+        if (q8 ? pg::gemm_launch<M, ST, pg::B_Q8>(a, bq, bs, mc, C, ldc, n, mt, n_tiles, K, s, sp, W.seg, oscale)
+               : pg::gemm_launch<M, ST>(a, b, b2, mc, C, ldc, n, mt, n_tiles, K, s, sp, 0, oscale))
+            return fail(p, B200_ERR_CUDA, "%s GEMM launch failed", name);
+        nl++;
+        return B200_OK;
+    };
+    using F32 = std::integral_constant<int, pg::GEMM_F32>;
+    using RESID = std::integral_constant<int, pg::GEMM_RESID>;
+    using GATEUP = std::integral_constant<int, pg::GEMM_GATEUP>;
     // the x += A W^T GEMMs (N = dim only) split K until the grid fills the SMs -- every split reduce-adds its partial
     // product through TMA -- keeping at least 8 k-blocks per split
     auto splits = [&](int n_tiles, int K) {
@@ -2058,14 +2093,11 @@ int prefill_forward(b200_plan *p, int n, const PfChunk &ck) {
     k_pf_embed<<<n, 256, 0, s>>>(c.tok, p->emb, p->mup.embedding_scale, c.X, g.dim); nl++;
     for (int l = 0; l < g.n_layers; l++) {
         const LayerW &L = p->layers[l];
-        const PrefillLayerMaps *m = q8 ? nullptr : &c.maps[l];
-        const PrefillQ8Maps *mq = q8 ? &c.maps_q8[l] : nullptr;
+        const PrefillLayerMaps &m = c.maps[l];
+        const PrefillQ8Maps &mq = c.maps_q8[l];
         float *kc = (ck.own ? p->key_cache : p->bt.slot_k) + (size_t)l * ctx_kv, *vc = (ck.own ? p->value_cache : p->bt.slot_v) + (size_t)l * ctx_kv;
         k_pf_rmsnorm_f16<<<n, 256, 0, s>>>(c.X, L.attn_norm, g.rms_norm_eps, g.dim, c.A16); nl++;
-        if (q8 ? pg::gemm_launch<pg::GEMM_F32, ST, B_Q8>(c.mA, mq->qkv_q, mq->qkv_s, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s, 1, L.tqkv.seg)
-               : pg::gemm_launch<pg::GEMM_F32, ST>(c.mA, m->qkv, m->qkv, c.mQKV, c.QKV, nqkv, n, mt, nqkv / pg::BN, g.dim, s))
-            return fail(p, B200_ERR_CUDA, "QKV GEMM launch failed");
-        nl++;
+        if ((rc = gemm(F32(), "QKV", c.mA, m.qkv, m.qkv, mq.qkv_q, mq.qkv_s, L.tqkv, c.mQKV, c.QKV, nqkv, nqkv / pg::BN, g.dim, 1, 1.0f))) return rc;
         if (ck.n_hist) { // rows written by earlier chunks / decode steps
             const size_t n4 = (size_t)ck.max_start * p->kvd / 4;
             const dim3 hg((unsigned)((n4 + 255) / 256 < 1184 ? (n4 + 255) / 256 : 1184), ck.n_hist);
@@ -2073,7 +2105,7 @@ int prefill_forward(b200_plan *p, int n, const PfChunk &ck) {
             nl++;
         }
         const dim3 ag(ck.n_tiles, g.n_kv_heads);
-        const int rc = with_mma_head_size(p, g.head_size, [&](auto HS) {
+        rc = with_mma_head_size(p, g.head_size, [&](auto HS) {
             k_pf_rope_kv_packed<HS><<<n, 256, 0, s>>>(c.QKV, nqkv, kc, vc, slot_stride, ck.KH, ck.VH, p->kvd, g.n_heads, g.n_kv_heads, p->kflags, L.q_norm, L.k_norm, L.qkv_bias, g.rms_norm_eps, p->rope_cr, p->rope_ci, ck.tok);
             k_pf_attention_mma_packed<HS><<<ag, PM_THREADS, pm_smem_bytes<HS>(), s>>>(c.QKV, nqkv, ck.KH, ck.VH, p->kvd, kv_mul, ck.tiles, inv_sqrt_hs, c.ATT16, p->qd);
             return B200_OK;
@@ -2082,19 +2114,11 @@ int prefill_forward(b200_plan *p, int n, const PfChunk &ck) {
         nl += 2;
         const int sp_wo = splits(g.dim / pg::BN, p->qd), sp_w2 = splits(g.dim / pg::BN, g.hidden_dim);
         const float rs = p->mup.residual_scale;
-        if (q8 ? pg::gemm_launch<pg::GEMM_RESID, ST, B_Q8>(c.mATT, mq->wo_q, mq->wo_s, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, sp_wo, L.two.seg, rs)
-               : pg::gemm_launch<pg::GEMM_RESID, ST>(c.mATT, m->wo, m->wo, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, p->qd, s, sp_wo, 0, rs))
-            return fail(p, B200_ERR_CUDA, "Wo GEMM launch failed");
-        nl++;
+        if ((rc = gemm(RESID(), "Wo", c.mATT, m.wo, m.wo, mq.wo_q, mq.wo_s, L.two, c.mX, c.X, g.dim, g.dim / pg::BN, p->qd, sp_wo, rs))) return rc;
         k_pf_rmsnorm_f16<<<n, 256, 0, s>>>(c.X, L.ffn_norm, g.rms_norm_eps, g.dim, c.A16); nl++;
-        if (q8 ? pg::gemm_launch<pg::GEMM_GATEUP, ST, B_Q8>(c.mA, mq->gu_q, mq->gu_s, c.mX, c.H16, g.hidden_dim, n, mt, g.hidden_dim / (pg::BN / 2), g.dim, s, 1, L.tgu.seg)
-               : pg::gemm_launch<pg::GEMM_GATEUP, ST>(c.mA, m->w1, m->w3, c.mX, c.H16, g.hidden_dim, n, mt, g.hidden_dim / (pg::BN / 2), g.dim, s))
-            return fail(p, B200_ERR_CUDA, "gate/up GEMM launch failed");
-        nl++;
-        if (q8 ? pg::gemm_launch<pg::GEMM_RESID, ST, B_Q8>(c.mH, mq->w2_q, mq->w2_s, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, sp_w2, L.tw2.seg, rs)
-               : pg::gemm_launch<pg::GEMM_RESID, ST>(c.mH, m->w2, m->w2, c.mX, c.X, g.dim, n, mt, g.dim / pg::BN, g.hidden_dim, s, sp_w2, 0, rs))
-            return fail(p, B200_ERR_CUDA, "W2 GEMM launch failed");
-        nl++;
+        if ((rc = gemm(GATEUP(), "gate/up", c.mA, m.w1, m.w3, mq.gu_q, mq.gu_s, L.tgu, c.mX, c.H16, g.hidden_dim, g.hidden_dim / (pg::BN / 2), g.dim, 1, 1.0f)))
+            return rc;
+        if ((rc = gemm(RESID(), "W2", c.mH, m.w2, m.w2, mq.w2_q, mq.w2_s, L.tw2, c.mX, c.X, g.dim, g.dim / pg::BN, g.hidden_dim, sp_w2, rs))) return rc;
     }
     CK(cudaGetLastError());
     CK(cudaEventRecord(p->ev1, s));
@@ -2105,10 +2129,6 @@ int prefill_forward(b200_plan *p, int n, const PfChunk &ck) {
 }
 
 // ---- the bit-exact tensor-core prefill (prefill_i8.cuh) -----------------------------------------------------------------------
-// The geometry of W as Q8_0 tiles: W itself, or for a resident matrix the tiles a Q8_0-tile plan of the same file holds, which
-// k_kq_tiles_to_q8 writes into the prefill's scratch before W's GEMM.
-TileMat q8_geometry(const TileMat &W) { return W.fmt ? tile_geometry(W.rows, W.cols, 0) : W; }
-
 cudaError_t launch_kq_tiles_to_q8(const TileMat &W, const TileMat &Q, unsigned char *out, cudaStream_t s) {
     const long long n = (long long)tile_groups(Q) * 4 * Q.nseg * (Q.seg / 32);
     const unsigned grid = (unsigned)((n + 127) / 128);
@@ -2141,31 +2161,14 @@ bool i8_weight_maps(b200_plan *p) {
     return true;
 }
 
-// Why the plan's shape or type rules the bit-exact tensor-core prefill out (nullptr: it can run), before anything is allocated.
-const char *i8_why(const b200_plan *p) {
-    const b200_config &g = p->cfg;
-    const int nqkv = p->qd + 2 * p->kvd;
-    if (p->prefill_batch <= 1) return "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
-    if (p->wtype != B200_GGML_Q8_0)
-        return "the bit-exact tensor-core prefill needs a Q8_0 plan (an FP16 plan's CPU dot products are FP16 lane chains, not int8 block sums)";
-    if (g.tp_size > 1) return "tensor-core prefill is single-GPU";
-    if (g.dim % 64 || p->qd % 64 || nqkv % 64) return "the bit-exact tensor-core prefill needs dim, q width and q+k+v width multiples of 64";
-    for (const LayerW &L : p->layers)
-        for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
-            if (q8_geometry(*t).seg % pg::BK) return "the bit-exact tensor-core prefill needs Q8_0 stream segments that are multiples of 64 columns";
-    if (!pg::encode_fn()) return "cuTensorMapEncodeTiled not available from the driver";
-    return nullptr;
-}
-
 // Built on the first b200_set_prefill_mode(TENSOR_CORE_EXACT): the chunk buffers and tensor maps over the plan's own Q8_0 streams,
 // nothing per weight.  A resident plan adds one scratch, the Q8_0 tiles of its largest resident matrix, and its resident matrices'
 // maps point there; the scratch and the chunk buffers must fit the free memory (memory_free) or the call fails with
-// B200_ERR_OOM.  Leaves pi8.ready false with the reason in pi8.why when the plan cannot run it.
+// B200_ERR_OOM.
 int prefill_init_i8(b200_plan *p) {
     PrefillI8Ctx &c = p->pi8;
     const b200_config &g = p->cfg;
     const int nqkv = p->qd + 2 * p->kvd;
-    if ((c.why = i8_why(p))) return B200_OK;
     int64_t kq8_bytes = 0;
     for (const LayerW &L : p->layers)
         for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
@@ -2209,10 +2212,7 @@ int prefill_init_i8(b200_plan *p) {
     const bool ok = pg::make_map_i8_a(&c.a_dim, c.XQ, c.bpad, g.dim) == 0 && pg::make_map_i8_s(&c.s_dim, c.XS, c.bpad, pg::i8_lds(g.dim)) == 0 &&
                     pg::make_map_i8_a(&c.a_qd, c.XQ, c.bpad, p->qd) == 0 && pg::make_map_i8_s(&c.s_qd, c.XS, c.bpad, pg::i8_lds(p->qd)) == 0 &&
                     pg::make_map_i8_a(&c.a_h, c.HQ, c.bpad, g.hidden_dim) == 0 && pg::make_map_i8_s(&c.s_h, c.HS, c.bpad, pg::i8_lds(g.hidden_dim)) == 0;
-    if (!ok || !i8_weight_maps(p)) { c.why = "cuTensorMapEncodeTiled rejected a tensor map"; return B200_OK; }
-    c.ready = true;
-    c.why = "";
-    return B200_OK;
+    return prefill_built(p, B200_PREFILL_TENSOR_CORE_EXACT, ok && i8_weight_maps(p));
 }
 
 // k_i8_norm over chunk rows [0, n) of c.X into XQ / XS; embed (layer 0): each row's embedding is gathered into c.X first.
@@ -2336,14 +2336,14 @@ int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own,
     return B200_OK;
 }
 
+const char *const PREFILL_MODE_NAMES[4] = {"exact", "tensor_core", "tensor_core_w8a16", "tensor_core_exact"};
+
 // The chunk path the plan's prefill mode runs: the bit-exact int8 one (prefill_i8.cuh), the f16 / W8A16 one (prefill.cuh), or
 // none (the exact token-by-token and multi-position paths).
 enum ChunkPath { CHUNK_NONE, CHUNK_TC, CHUNK_I8 };
 ChunkPath chunk_path(const b200_plan *p) {
-    const PrefillCtx &c = p->prefill;
-    if (c.mode == B200_PREFILL_TENSOR_CORE_EXACT && p->pi8.ready) return CHUNK_I8;
-    if ((c.mode == B200_PREFILL_TENSOR_CORE && c.ready) || (c.mode == B200_PREFILL_TENSOR_CORE_W8A16 && c.q8_ready)) return CHUNK_TC;
-    return CHUNK_NONE;
+    constexpr ChunkPath PATHS[4] = {CHUNK_NONE, CHUNK_TC, CHUNK_TC, CHUNK_I8};
+    return PATHS[p->pf_mode];
 }
 
 // One chunk on the tensor-core path chunk_path selects: the tokens of ns sequences back to back (call order, no padding),
@@ -2509,6 +2509,16 @@ int bad_token(const b200_plan *p, const int32_t *tokens, int n) {
     for (int i = 0; i < n; i++)
         if (tokens[i] < 0 || tokens[i] >= p->cfg.vocab_size) return i;
     return -1;
+}
+
+// The checks b200_forward_batch_prefill and b200_score_tokens make of a chunk: its length against prefill_batch_size, its positions,
+// its tokens, and on the token-by-token path the step buffers' capacity.
+int check_chunk(b200_plan *p, const int32_t *tokens, int32_t n, int32_t start_pos) {
+    if (p->prefill_batch > 1 && n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "chunk of %d tokens exceeds prefill_batch_size %d", n, p->prefill_batch);
+    if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache", start_pos, start_pos + n - 1);
+    if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
+    if (chunk_path(p) == CHUNK_NONE && n > p->seq_cap) return fail(p, B200_ERR_BAD_ARG, "chunk too long");
+    return B200_OK;
 }
 
 // The refusals b200_forward_decode_batch and b200_forward_step share for row i: slot, token and position out of range, and an
@@ -2972,9 +2982,8 @@ int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, i
     if (!p || !tokens) return B200_ERR_BAD_ARG;
     if (n <= 0) return B200_OK;
     if (!p->graph.prefill.exec) return fail(p, B200_ERR_STATE, "tensor-parallel plan: call b200_tp_attach on every rank first");
-    if (p->prefill_batch > 1 && n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "chunk of %d tokens exceeds prefill_batch_size %d", n, p->prefill_batch);
-    if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache", start_pos, start_pos + n - 1);
-    if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
+    int rc;
+    if ((rc = check_chunk(p, tokens, n, start_pos))) return rc;
     CK(cudaSetDevice(p->device));
     if (chunk_path(p) != CHUNK_NONE) { // the whole chunk on the tensor cores into the plan's cache
         const int slot = 0;
@@ -2984,10 +2993,9 @@ int b200_forward_batch_prefill(b200_plan *p, const int32_t *tokens, int32_t n, i
     // that run multi-position steps take positions start .. start + n - 2 in steps of batch_max_rows rows into the plan's cache;
     // the last token, and every token elsewhere, runs through the single-token prefill graph, with the step state as the
     // token-by-token loop leaves it before its last step.
-    if (n > p->seq_cap) return fail(p, B200_ERR_BAD_ARG, "chunk too long");
     memcpy(p->h_ids, tokens, (size_t)n * 4);
     CK(cudaMemcpyAsync(p->seq_tokens, p->h_ids, (size_t)n * 4, cudaMemcpyHostToDevice, p->stream));
-    int rc, first = 0;
+    int first = 0;
     if (n > 1 && !multi_why(p)) {
         if ((rc = multi_ready(p))) return rc;
         std::vector<BatchRows> sched;
@@ -3007,21 +3015,17 @@ int b200_score_tokens(b200_plan *p, const int32_t *tokens, const int32_t *target
     if (n <= 0) return B200_OK;
     if (p->cfg.tp_size > 1)
         return fail(p, B200_ERR_UNSUPPORTED, "full logits are not gathered under tensor parallelism: scoring runs on single-GPU plans");
-    const int mode = p->prefill.mode;
     const ChunkPath path = chunk_path(p);
     if (path == CHUNK_TC)
         return fail(p, B200_ERR_UNSUPPORTED, "the %s prefill keeps f16 activations, so its logits are not the reference's: score in the exact or "
-                    "tensor_core_exact prefill mode", mode == B200_PREFILL_TENSOR_CORE ? "tensor_core" : "tensor_core_w8a16");
-    if (p->prefill_batch > 1 && n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "chunk of %d tokens exceeds prefill_batch_size %d", n, p->prefill_batch);
-    if (start_pos < 0 || start_pos + n > p->cfg.context_length) return fail(p, B200_ERR_BAD_ARG, "positions %d..%d outside the KV cache", start_pos, start_pos + n - 1);
-    if (const int i = bad_token(p, tokens, n); i >= 0) return fail(p, B200_ERR_BAD_ARG, "token %d out of range", tokens[i]);
+                    "tensor_core_exact prefill mode", PREFILL_MODE_NAMES[p->pf_mode]);
+    int rc;
+    if ((rc = check_chunk(p, tokens, n, start_pos))) return rc;
     for (int i = 0; i < n; i++)
         if (targets[i] != -1 && (targets[i] < 0 || targets[i] >= p->cfg.vocab_size))
             return fail(p, B200_ERR_BAD_ARG, "target %d of row %d out of range (-1 or a token id)", targets[i], i);
     const bool tc = path == CHUNK_I8;
-    if (!tc && n > p->seq_cap) return fail(p, B200_ERR_BAD_ARG, "chunk too long");
     CK(cudaSetDevice(p->device));
-    int rc;
     if ((rc = score_ready(p)) || (tc && (rc = score_init_i8(p)))) return rc;
     CK(cudaMemcpyAsync(p->sc.tgt, targets, (size_t)n * 4, cudaMemcpyHostToDevice, p->stream));
     if (tc) {
@@ -3107,47 +3111,22 @@ int b200_trace_persistent(b200_plan *p, int32_t token, int32_t position, uint64_
 }
 
 int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
-    if (!p || (mode != B200_PREFILL_EXACT && mode != B200_PREFILL_TENSOR_CORE && mode != B200_PREFILL_TENSOR_CORE_W8A16 &&
-               mode != B200_PREFILL_TENSOR_CORE_EXACT))
-        return B200_ERR_BAD_ARG;
-    if (p->is_moe && mode != B200_PREFILL_EXACT) return fail(p, B200_ERR_UNSUPPORTED, "%s", moe_prefill_why(p));
-    if (p->resident && (mode == B200_PREFILL_TENSOR_CORE || mode == B200_PREFILL_TENSOR_CORE_W8A16))
-        return fail(p, B200_ERR_UNSUPPORTED, "this plan keeps K-quant weights resident: the f16 and W8A16 tensor-core prefills read f16 matrices or "
-                    "Q8_0 tiles it does not hold; tensor_core_exact expands each resident matrix to Q8_0 tiles before its GEMM");
-    if (mode == B200_PREFILL_TENSOR_CORE_EXACT) {
-        if (!p->pi8.ready) {
-            CK(cudaSetDevice(p->device));
-            int rc = prefill_init_i8(p);
-            if (rc) return rc;
-            if (!p->pi8.ready) return fail(p, B200_ERR_UNSUPPORTED, "%s", p->pi8.why);
-        }
-        p->prefill.mode = mode;
-        return B200_OK;
-    }
-    if (mode == B200_PREFILL_TENSOR_CORE_W8A16) {
-        if (!p->prefill.q8_ready) {
-            CK(cudaSetDevice(p->device));
-            int rc = prefill_init_q8(p);
-            if (rc) return rc;
-            if (!p->prefill.q8_ready) return fail(p, B200_ERR_UNSUPPORTED, "%s", p->prefill.why_q8);
-        }
-        p->prefill.mode = mode;
-        return B200_OK;
-    }
-    if (mode == B200_PREFILL_TENSOR_CORE && !p->prefill.ready && p->prefill_batch > 1 && p->wtype == B200_GGML_Q8_0 && p->cfg.tp_size == 1) {
-        CK(cudaSetDevice(p->device)); // opt-in on a Q8_0 plan: build the f16 twins, then the GEMM context
-        int rc = build_f16_twins(p);
+    if (!p || mode < B200_PREFILL_EXACT || mode > B200_PREFILL_TENSOR_CORE_EXACT) return B200_ERR_BAD_ARG;
+    const b200_plan::PrefillMode &m = p->pf[mode];
+    if (!m.ready) { // refused before anything is allocated, else built (each init leaves the mode ready or says why not)
+        if (const char *why = prefill_why(p, mode)) return fail(p, B200_ERR_UNSUPPORTED, "%s", why);
+        CK(cudaSetDevice(p->device));
+        const int rc = mode == B200_PREFILL_TENSOR_CORE ? prefill_init(p) : mode == B200_PREFILL_TENSOR_CORE_W8A16 ? prefill_init_q8(p) : prefill_init_i8(p);
         if (rc) return rc;
-        if ((rc = prefill_init(p))) return rc;
+        if (!m.ready) return fail(p, B200_ERR_UNSUPPORTED, "%s", m.why);
     }
-    if (mode == B200_PREFILL_TENSOR_CORE && !p->prefill.ready) return fail(p, B200_ERR_UNSUPPORTED, "%s", p->prefill.why);
-    p->prefill.mode = mode;
+    p->pf_mode = mode;
     return B200_OK;
 }
 
 int b200_prefill_info(b200_plan *p, int32_t *mode, int32_t *launches, float *device_ms) {
     if (!p) return B200_ERR_BAD_ARG;
-    if (mode) *mode = chunk_path(p) == CHUNK_NONE ? B200_PREFILL_EXACT : p->prefill.mode;
+    if (mode) *mode = p->pf_mode;
     if (launches) *launches = p->launches_prefill;
     if (device_ms) *device_ms = p->prefill_ms;
     return B200_OK;
@@ -3342,9 +3321,8 @@ namespace {
 // steps, then what rules out the bit-exact tensor-core prefill.
 const char *chunk_why(const b200_plan *p) {
     const char *why = multi_why(p);
-    return why ? why : i8_why(p);
+    return why ? why : prefill_why(p, B200_PREFILL_TENSOR_CORE_EXACT);
 }
-const char *const PREFILL_MODE_NAMES[4] = {"exact", "tensor_core", "tensor_core_w8a16", "tensor_core_exact"};
 } // namespace
 
 int b200_chunk_rows(b200_plan *p, int32_t *max_rows) {
@@ -3358,11 +3336,9 @@ int b200_forward_chunk(b200_plan *p, int32_t n, const b200_step_row *rows, int32
     if (const char *why = chunk_why(p)) return fail(p, B200_ERR_UNSUPPORTED, "%s", why);
     auto &B = p->bt;
     if (!B.n_slots) return fail(p, B200_ERR_STATE, "no decode slots: call b200_set_decode_slots first");
-    if (chunk_path(p) != CHUNK_I8) {
-        const int mode = chunk_path(p) == CHUNK_NONE ? B200_PREFILL_EXACT : p->prefill.mode;
+    if (const int mode = p->pf_mode; mode != B200_PREFILL_TENSOR_CORE_EXACT)
         return fail(p, B200_ERR_STATE, "the plan's prefill mode is %s%s: b200_forward_chunk runs in tensor_core_exact (b200_set_prefill_mode)",
                     PREFILL_MODE_NAMES[mode], mode == B200_PREFILL_EXACT ? "" : ", whose f16 GEMMs are not bit-exact");
-    }
     if (!rows || !ids_out) return fail(p, B200_ERR_BAD_ARG, "rows and ids_out must not be NULL");
     if (n < 1 || n > p->prefill_batch) return fail(p, B200_ERR_BAD_ARG, "n = %d rows: need 1 <= n <= %d (b200_chunk_rows)", n, p->prefill_batch);
     int rc;
@@ -3529,7 +3505,8 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
         sz = ctx_kv * 4;
     } else if (s.rfind("pf_", 0) == 0) { // tensor-core prefill scratch: [padded rows][width], the last layer of the last chunk
         const PrefillCtx &pc = p->prefill;
-        if (!pc.ready && !pc.q8_ready) return fail(p, B200_ERR_STATE, "%s: the plan has no tensor-core prefill buffers (%s)", name, pc.why);
+        if (!p->pf[B200_PREFILL_TENSOR_CORE].ready && !p->pf[B200_PREFILL_TENSOR_CORE_W8A16].ready)
+            return fail(p, B200_ERR_STATE, "%s: the plan has no tensor-core prefill buffers (%s)", name, p->pf[B200_PREFILL_TENSOR_CORE].why);
         const size_t rows = (size_t)pc.bpad;
         if (s == "pf_x") { src = pc.X; sz = rows * c.dim * 4; }
         else if (s == "pf_qkv") { src = pc.QKV; sz = rows * (p->qd + 2 * p->kvd) * 4; }
@@ -4093,7 +4070,7 @@ int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const 
                                   int32_t n_heads, int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out) {
     if (!lengths || !start_positions || !q || !k || !v || !out || n_seqs < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return B200_ERR_BAD_ARG;
     const int kv_mul = n_heads / n_kv_heads, hs = head_size;
-    if ((hs != 64 && hs != 128) || kv_mul > 64) return B200_ERR_BAD_ARG; // what prefill_init accepts
+    if ((hs != 64 && hs != 128) || kv_mul > 64) return B200_ERR_BAD_ARG; // what prefill_why accepts for tensor_core
     const int qd = n_heads * hs, kvd = n_kv_heads * hs, ldq = qd + 2 * kvd;
     std::vector<int> row0(n_seqs), hrow(n_seqs);
     int n = 0, rows = 0;

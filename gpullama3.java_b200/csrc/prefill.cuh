@@ -37,11 +37,9 @@ struct PrefillQ8Maps {
     CUtensorMap qkv_q, qkv_s, wo_q, wo_s, gu_q, gu_s, w2_q, w2_s;
 };
 
+// The buffers and maps of the tensor_core (f16 B) and tensor_core_w8a16 (Q8_0 B) modes; which of them is ready is the plan's record.
 struct PrefillCtx {
-    int batch = 0, bpad = 0; // bpad > 0: the scratch buffers below exist
-    bool ready = false;    // tensor-core path with f16 weight matrices usable for this plan
-    bool q8_ready = false; // W8A16 tensor-core path (B from the Q8_0 streams) usable for this plan
-    int mode = 0;          // 0 = exact token-by-token graph, 1 = tensor-core GEMMs (f16 B), 2 = tensor-core GEMMs (Q8_0 B, W8A16)
+    int bpad = 0; // bpad > 0: the scratch buffers below exist
     float *X = nullptr, *QKV = nullptr;
     __half *A16 = nullptr, *ATT16 = nullptr, *H16 = nullptr;
     int *tok = nullptr;
@@ -54,10 +52,8 @@ struct PrefillCtx {
     size_t ptab_bytes = 0;
     CUtensorMap mA, mATT, mH; // GEMM A operands (f16 activations)
     CUtensorMap mX, mQKV;     // GEMM outputs written by TMA (f32)
-    std::vector<PrefillLayerMaps> maps;
+    std::vector<PrefillLayerMaps> maps; // per layer, both sized with the scratch; each filled by its own mode's init
     std::vector<PrefillQ8Maps> maps_q8;
-    const char *why = "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
-    const char *why_q8 = "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
 };
 
 // ---- elementwise kernels ------------------------------------------------------------------------

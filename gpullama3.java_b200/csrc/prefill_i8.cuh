@@ -304,8 +304,6 @@ struct ChunkTok {
 // step keeps them per row; XQ / XS the int8 activations of the QKV, gate/up (row stride dim) and Wo (row stride q width) GEMMs, HQ /
 // HS those of W2; the token table; score rows for ATT_TOKENS tokens at a time when the context needs global score rows.
 struct PrefillI8Ctx {
-    bool ready = false;
-    const char *why = "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
     int bpad = 0, att_tokens = 0;
     float *X = nullptr, *QKV = nullptr, *XS = nullptr, *HS = nullptr, *att = nullptr;
     int8_t *XQ = nullptr, *HQ = nullptr;

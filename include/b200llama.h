@@ -224,8 +224,8 @@ int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n
  *                            bit-identical to the CPU path;
  *   B200_PREFILL_TENSOR_CORE TMA + wgmma GEMMs over the whole chunk, FP16 operands / FP32 accumulation:
  *                            KV cache within FP16 tolerance of the CPU path.  Default for FP16 plans created
- *                            with prefill_batch_size > 1.  Opt-in for single-GPU Q8_0 plans: the first call
- *                            dequantises f16 twins of the weight matrices on the device (+2 bytes/weight);
+ *                            with prefill_batch_size > 1.  Opt-in for single-GPU Q8_0 plans: the first call the
+ *                            plan can run dequantises f16 twins of the weight matrices on the device (+2 bytes/weight);
  *                            there the CPU path additionally rounds activations to int8, so agreement is
  *                            percent-level, not FP16-level -- hence not the default.  Returns
  *                            B200_ERR_UNSUPPORTED with the reason in b200_last_error when unavailable.

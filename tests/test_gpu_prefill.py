@@ -282,7 +282,7 @@ def _check_attention(pkg, q, k, v, n_heads, n_kv, start, kind, what):
 @pytest.mark.parametrize("kv_mul", [1, 2, 4, 8, 16, 64])
 def test_pf_attention_matches_float64(pkg, kv_mul):
     """k_pf_attention_mma_packed on a one-sequence chunk (what the prefill runs), elementwise against float64 softmax attention, at every GQA ratio
-    prefill_init accepts (at 64 a query tile is one token), across key-tile boundaries."""
+    the tensor-core prefill accepts (at 64 a query tile is one token), across key-tile boundaries."""
     n_kv = 2 if kv_mul <= 8 else 1
     n_heads = n_kv * kv_mul
     worst = 0.0
@@ -521,5 +521,38 @@ def test_tensor_core_prefill_unsupported_is_loud(pkg, make_model):
         with pytest.raises(Exception, match="prefill batch size"):
             plan.set_prefill_mode("tensor_core")
         plan.set_prefill_mode("exact")
+    finally:
+        plan.free()
+
+
+def test_tensor_core_refusal_allocates_nothing(pkg, make_model):
+    """A Q8_0 plan whose shape the tensor-core prefill cannot run (Phi-3's head size 96) refuses "tensor_core" before it builds
+    the f16 twins: the device bytes are unchanged and the previous mode stays in force."""
+    m = make_model("tiny-phi3", pkg.gguf.GGMLType.Q8_0, 32)
+    plan = pkg.B200MasterPlan.initialize_plan(m, prefill_batch_size=16)
+    try:
+        plan.set_prefill_mode("tensor_core_exact")
+        b0 = plan.device_bytes
+        with pytest.raises(pkg.native.UnsupportedOperation, match="head size"):
+            plan.set_prefill_mode("tensor_core")
+        assert plan.device_bytes == b0, (plan.device_bytes, b0)
+        assert plan.prefill_info()[0] == plan.PREFILL_TENSOR_CORE_EXACT
+    finally:
+        plan.free()
+
+
+def test_tensor_parallel_plan_refuses_tensor_core_modes(pkg, make_model):
+    """Rank 0 of a two-way tensor-parallel plan with a prefill batch size, created without its peer: every tensor-core mode names
+    the single-GPU rule and the exact mode stays in force."""
+    m = make_model("tiny-qwen3", pkg.gguf.GGMLType.Q8_0, ctx=64, seed=28)
+    cfg = pkg.plan.make_config(m)
+    cfg.tp_rank, cfg.tp_size = 0, 2
+    plan = pkg.native.NativePlan(cfg, m.tensors, 16, 0)
+    P = pkg.B200MasterPlan
+    try:
+        for mode in (P.PREFILL_TENSOR_CORE, P.PREFILL_TENSOR_CORE_W8A16, P.PREFILL_TENSOR_CORE_EXACT):
+            with pytest.raises(pkg.native.UnsupportedOperation, match="single-GPU"):
+                plan.set_prefill_mode(mode)
+            assert plan.prefill_info()[0] == P.PREFILL_EXACT
     finally:
         plan.free()

@@ -677,11 +677,10 @@ template <int MODE> int launch_matvec_f16(b200_plan *p, const DevMat &m, const f
 
 // FP16 plans on the streaming path (stream_matvec_f16.cuh); m2 = ffn_up for SF_GATEUP.
 template <typename... KA, typename... A> int launch_k(b200_plan *p, bool pdl, void (*kern)(KA...), dim3 grid, dim3 block, size_t smem, A... args);
-int sf_grid(const b200_plan *p, int rows, int cols, bool gateup) { // CTAs of an FP16 streaming launch
-    const int lanes = p->cfg.fp16_lanes;
+int sf_grid(int n_sms, int lanes, int rows, int cols, bool gateup) { // CTAs of an FP16 streaming launch
     const SfLayout L = sf_layout(rows, cols, lanes, gateup);
     const int rw = 64 / lanes, mr = gateup ? rw / 2 : rw;
-    const int grid = L.ctas_per_sm * p->n_sms;
+    const int grid = L.ctas_per_sm * n_sms;
     const int groups = (rows + mr - 1) / mr; // a ragged classifier ends in a partial group
     return grid > groups ? groups : grid;
 }
@@ -696,7 +695,7 @@ template <int MODE> int launch_stream_f16(b200_plan *p, const DevMat &m, const D
     a.seg = L.seg; a.nseg = L.nseg; a.stages = L.stages; a.tr = tr;
     a.part_val = argmax ? p->part_val : nullptr;
     a.part_idx = argmax ? p->part_idx : nullptr;
-    const int grid = sf_grid(p, m.rows, m.cols, MODE == SF_GATEUP);
+    const int grid = sf_grid(p->n_sms, lanes, m.rows, m.cols, MODE == SF_GATEUP);
     if (lanes == 16) return launch_k(p, p->use_pdl, k_stream_matvec_f16<16, MODE>, dim3(grid), dim3(SF_THREADS), L.total, a);
     return launch_k(p, p->use_pdl, k_stream_matvec_f16<8, MODE>, dim3(grid), dim3(SF_THREADS), L.total, a);
 }
@@ -704,18 +703,22 @@ template <int MODE> int launch_stream_f16(b200_plan *p, const DevMat &m, const D
 // Kernel launch with the programmatic-dependent-launch attribute (captured into the CUDA graph as
 // a programmatic edge): the kernel may become resident while its predecessor is still running.
 template <typename... KA, typename... A>
-int launch_k(b200_plan *p, bool pdl, void (*kern)(KA...), dim3 grid, dim3 block, size_t smem, A... args) {
+cudaError_t launch_on(cudaStream_t stream, bool pdl, void (*kern)(KA...), dim3 grid, dim3 block, size_t smem, A... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
-    cfg.stream = p->stream;
+    cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl ? 1 : 0;
-    CK(cudaLaunchKernelEx(&cfg, kern, static_cast<KA>(args)...));
+    return cudaLaunchKernelEx(&cfg, kern, static_cast<KA>(args)...);
+}
+template <typename... KA, typename... A>
+int launch_k(b200_plan *p, bool pdl, void (*kern)(KA...), dim3 grid, dim3 block, size_t smem, A... args) {
+    CK(launch_on(p->stream, pdl, kern, grid, block, smem, args...));
     return B200_OK;
 }
 
@@ -921,7 +924,7 @@ int enqueue_forward(b200_plan *p, bool with_logits, int *launches, bool trace = 
         int rc;
         if ((rc = launch_k(p, pdl, k_argmax_advance, dim3(1), dim3(1024), (size_t)0, (const float *)p->logits, c.vocab_size, p->st, (const int *)p->seq_tokens, p->out_ids, with_logits ? 1 : 0,
                            (const float *)(q8 || sf ? p->part_val : nullptr), (const int *)(q8 || sf ? p->part_idx : nullptr),
-                           sf ? sf_grid(p, c.vocab_size, c.dim, false) : p->n_sms, TR(9), p->tp, with_logits ? -1 : last_x_op))) return rc;
+                           sf ? sf_grid(p->n_sms, c.fp16_lanes, c.vocab_size, c.dim, false) : p->n_sms, TR(9), p->tp, with_logits ? -1 : last_x_op))) return rc;
         n++;
     }
     if (launches) *launches = n;
@@ -4062,6 +4065,273 @@ int b200_test_gemm_i8(int32_t mode, int32_t m, int32_t n, int32_t k, const int8_
             if (gateup) s.ok(cudaMemcpy(hq, dhq, (size_t)m * n, cudaMemcpyDeviceToHost)) && s.ok(cudaMemcpy(hs, dhs, (size_t)m * (n / 32) * 4, cudaMemcpyDeviceToHost));
             else s.ok(cudaMemcpy(c, dc, (size_t)m * n * 4, cudaMemcpyDeviceToHost));
         }
+    }
+    return s.rc;
+}
+
+} // extern "C"
+
+namespace {
+// What b200_test_stream launches, decided from its arguments alone (grid 0 with n_sms 0: the grid is not known yet).
+struct StreamTest {
+    TileMat W, Wd;   // Q8_0 / resident: the stream and, in pair mode, the down projection (bases unset)
+    SmvSmem L, Ld;   // single-row layouts
+    SmbSmem B;       // batched layout
+    SfLayout F;      // F16 layout
+    unsigned off_sq = 0, off_seq = 0;
+    int stages = 0, grid = 0, gmax = 0, gmin = 0;
+    size_t total = 0;
+};
+
+int stream_test_plan(const b200_stream_test &t, int n_sms, StreamTest &c) {
+    const bool f16 = t.form == B200_GGML_F16, kq = kq_is_kquant(t.form), batch = t.nrow > 0, gateup = t.mode == SMV_GATEUP;
+    const bool norm_in = t.norm && !t.from_emb;
+    if (!f16 && !kq && t.form != B200_GGML_Q8_0) return B200_ERR_BAD_ARG;
+    if (t.mode < SMV_STORE || t.mode > SMV_GATEUP || t.rows < 1 || t.cols < 32 || t.grid < 0 || t.stages < 0 || t.budget < 0) return B200_ERR_BAD_ARG;
+    if (t.nrow < 0 || t.nrow > SMB_MAX_ROWS || (batch && (kq || f16 || t.norm))) return B200_ERR_BAD_ARG;
+    if (t.launches != 1 && t.launches != 2) return B200_ERR_BAD_ARG;
+    if (t.norm && (t.mode == SMV_RESID || f16 || !norm_fusion_ok(t.cols) || !t.norm_w)) return B200_ERR_BAD_ARG;
+    if (t.from_emb && (!t.norm || !t.emb || !t.tokens || !t.x_out || t.emb_rows < 1)) return B200_ERR_BAD_ARG;
+    for (int l = 0; t.from_emb && l < t.launches; l++)
+        if (t.tokens[l] < 0 || t.tokens[l] >= t.emb_rows) return B200_ERR_BAD_ARG;
+    if (t.argmax && (t.mode != SMV_STORE || !t.ids)) return B200_ERR_BAD_ARG;
+    if (t.pair && (!gateup || batch || f16 || !t.w_down || t.down_rows < 1 || !t.out_init || !t.out_down)) return B200_ERR_BAD_ARG;
+    if (!t.w || !t.out || (gateup && !t.w_up) || (gateup && !f16 && (!t.hq || !t.hs)) || (t.mode == SMV_RESID && !t.out_init)) return B200_ERR_BAD_ARG;
+    if ((f16 || norm_in) ? !t.x : (!t.norm && (!t.xq || !t.xs))) return B200_ERR_BAD_ARG;
+    if (f16) {
+        c.F = sf_layout(t.rows, t.cols, t.lanes, gateup);
+        if (!c.F.ok || t.budget) return B200_ERR_BAD_ARG;
+        c.stages = t.stages ? t.stages : c.F.stages;
+        if (c.stages < 3 || c.stages > SF_MAX_STAGES) return B200_ERR_BAD_ARG;
+        const int rw = 64 / t.lanes, mr = gateup ? rw / 2 : rw, ngroups = (t.rows + mr - 1) / mr;
+        c.total = (size_t)t.cols * 4 + SF_WARPS * SF_MAX_STAGES * 8 + 256 + (size_t)SF_WARPS * c.stages * ((size_t)rw * (c.F.seg * 2 + SF_ROW_PAD));
+        c.grid = t.grid ? t.grid : n_sms ? sf_grid(n_sms, t.lanes, t.rows, t.cols, gateup) : 0;
+        for (int b = 0; b < c.grid; b++) { // k_stream_matvec_f16's warp-interleaved assignment
+            int g = 0;
+            for (int w = 0; w < SF_WARPS; w++) {
+                const int gw = w * c.grid + b, G = c.grid * SF_WARPS;
+                g += gw < ngroups ? (ngroups - gw + G - 1) / G : 0;
+            }
+            c.gmax = b ? std::max(c.gmax, g) : g;
+            c.gmin = b ? std::min(c.gmin, g) : g;
+        }
+        return B200_OK;
+    }
+    if (gateup && t.rows % 32) return B200_ERR_BAD_ARG; // whole 32-unit blocks of hq
+    if (t.stages && (t.stages < 3 || t.stages > SMV_MAX_STAGES)) return B200_ERR_BAD_ARG;
+    c.W = tile_geometry(gateup ? 2 * t.rows : t.rows, t.cols, kq ? t.form : 0);
+    if (!c.W.nseg) return B200_ERR_BAD_ARG;
+    if (batch) {
+        const size_t budget = t.stages ? smb_layout(c.W.seg, t.nrow, 0).off_ring + (size_t)t.stages * smb_layout(c.W.seg, t.nrow, 0).stage_bytes
+                              : t.budget ? (size_t)t.budget : SMB_SMEM_BUDGET;
+        if (budget > SMB_SMEM_BUDGET) return B200_ERR_BAD_ARG; // the batched kernels are set up for at most this much
+        c.B = smb_layout(c.W.seg, t.nrow, budget);
+        c.stages = c.B.stages;
+        c.total = c.B.total;
+    } else {
+        const int fmt = c.W.fmt;
+        auto lay = [&](size_t b) { return t.norm ? smv_layout_norm(t.cols, c.W.seg, b, &c.off_sq, &c.off_seq, fmt) : smv_layout(t.cols, c.W.seg, b, fmt); };
+        const SmvSmem L0 = lay(0);
+        c.L = lay(t.stages ? L0.off_ring + (size_t)t.stages * L0.stage_bytes : t.budget ? (size_t)t.budget : SMV_SMEM_BUDGET_MAX);
+        c.stages = c.L.stages;
+        c.total = c.L.total;
+        if (t.pair) {
+            c.Wd = tile_geometry(t.down_rows, t.rows, fmt);
+            if (!c.Wd.nseg) return B200_ERR_BAD_ARG;
+            c.Ld = smv_layout(t.rows, c.Wd.seg, SMV_SMEM_BUDGET_MAX, fmt);
+            if (c.Ld.stages < 3) return B200_ERR_BAD_ARG;
+        }
+    }
+    if (c.stages < 3 || (t.stages && c.stages != t.stages)) return B200_ERR_BAD_ARG;
+    c.grid = t.grid ? t.grid : n_sms;
+    if (gateup && c.grid && !gateup_fits(t.rows, c.grid)) return B200_ERR_BAD_ARG;
+    const int G = tile_groups(c.W);
+    for (int b = 0; b < c.grid; b++) { // the kernels' static slice [g0, g1)
+        const int g = (int)(((long long)(b + 1) * G) / c.grid - ((long long)b * G) / c.grid);
+        c.gmax = b ? std::max(c.gmax, g) : g;
+        c.gmin = b ? std::min(c.gmin, g) : g;
+    }
+    return B200_OK;
+}
+
+template <typename F> void with_stream_mode(int mode, F &&f) { // SMV_* and SF_* share their values
+    if (mode == SMV_STORE) f(std::integral_constant<int, SMV_STORE>());
+    else if (mode == SMV_RESID) f(std::integral_constant<int, SMV_RESID>());
+    else f(std::integral_constant<int, SMV_GATEUP>());
+}
+} // namespace
+
+extern "C" {
+
+int b200_test_stream(b200_stream_test *t) {
+    if (!t) return B200_ERR_BAD_ARG;
+    StreamTest c;
+    int rc = stream_test_plan(*t, 0, c);
+    if (rc) return rc;
+    auto report = [&] {
+        const int64_t v[5] = {c.stages, c.grid, c.gmax, c.gmin, (int64_t)c.total};
+        for (int k = 0; k < 5; k++) t->info[k] = v[k];
+    };
+    if (t->dry) {
+        if (!t->grid) return B200_ERR_BAD_ARG;
+        report();
+        return B200_OK;
+    }
+    int dev = 0, n_sms = 0, optin = 0;
+    Scratch s;
+    if (!s.ok(cudaGetDevice(&dev)) || !s.ok(cudaDeviceGetAttribute(&n_sms, cudaDevAttrMultiProcessorCount, dev)) ||
+        !s.ok(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)))
+        return s.rc;
+    if ((rc = stream_test_plan(*t, n_sms, c))) return rc;
+    if (c.total > (size_t)optin) return B200_ERR_BAD_ARG;
+    report();
+
+    const bool f16 = t->form == B200_GGML_F16, batch = t->nrow > 0, gateup = t->mode == SMV_GATEUP;
+    const int V = batch ? t->nrow : 1, rows = t->rows, cols = t->cols, nb = cols / 32, fmt = f16 ? 0 : c.W.fmt;
+    const size_t rb = f16 ? (size_t)cols * 2 : fmt ? (size_t)cols / 256 * kq_block_bytes(fmt) : (size_t)nb * 34;
+    const size_t wbytes = (size_t)rows * rb, obytes = (size_t)V * rows * 4;
+    TpCtx solo{};
+    solo.n = 1;
+    const TraceBuf none{nullptr, 0, 0};
+    unsigned char *dw = nullptr, *dtile = nullptr, *dwd = nullptr, *dtd = nullptr;
+    int8_t *dxq = nullptr, *dhq = nullptr, *dembq = nullptr;
+    float *dxs = nullptr, *dx = nullptr, *dnw = nullptr, *dout = nullptr, *dhs = nullptr, *dres = nullptr, *dpv = nullptr;
+    __half *dembs = nullptr;
+    int *dpi = nullptr, *dids = nullptr;
+    unsigned *dblk = nullptr;
+    StepState *dst = nullptr;
+    // the weights: raw rows (gate then up), repacked as upload_tiles repacks them
+    // out ends in GUARD words that no store may reach (a padding row of a ragged STORE would land there)
+    const int GUARD = 4;
+    if (!s.alloc(&dw, wbytes * (gateup ? 2 : 1)) || !s.ok(cudaMemcpy(dw, t->w, wbytes, cudaMemcpyHostToDevice)) ||
+        (gateup && !s.ok(cudaMemcpy(dw + wbytes, t->w_up, wbytes, cudaMemcpyHostToDevice))) || !s.alloc(&dout, obytes + GUARD * 4) ||
+        !s.ok(cudaMemset(dout, 0xFF, obytes + GUARD * 4)) || (t->mode == SMV_RESID && !s.ok(cudaMemcpy(dout, t->out_init, obytes, cudaMemcpyHostToDevice))))
+        return s.rc;
+    auto repack = [&](const TileMat &W, const unsigned char *raw, int nrows, int ncols, bool gu, unsigned char **tiles) {
+        RepackSrc src{};
+        src.raw[0] = raw;
+        src.rows[0] = nrows;
+        if (gu) { src.raw[1] = raw + (size_t)nrows * rb; src.rows[1] = nrows; }
+        src.gateup = gu ? 1 : 0;
+        if (!s.alloc(tiles, (size_t)tile_bytes(W))) return false;
+        const unsigned n = (unsigned)((size_t)tile_groups(W) * 4 * W.nseg);
+        if (W.fmt) k_repack_kq_tiles<<<n, 128>>>(src, *tiles, W.rows, ncols, W.seg, W.nseg, W.unit_bytes, kq_block_bytes(W.fmt));
+        else k_repack_tiles<<<n, 128>>>(src, *tiles, W.rows, ncols, W.seg, W.nseg, W.unit_bytes);
+        return s.ok(cudaGetLastError());
+    };
+    if (!f16) {
+        if (!repack(c.W, dw, rows, cols, gateup, &dtile)) return s.rc;
+        c.W.base = dtile;
+    }
+    if (t->pair) {
+        const size_t db = (size_t)t->down_rows * (fmt ? (size_t)rows / 256 * kq_block_bytes(fmt) : (size_t)rows / 32 * 34);
+        if (!s.alloc(&dwd, db) || !s.ok(cudaMemcpy(dwd, t->w_down, db, cudaMemcpyHostToDevice)) || !repack(c.Wd, dwd, t->down_rows, rows, false, &dtd) ||
+            !s.alloc(&dres, (size_t)t->down_rows * 4) || !s.ok(cudaMemcpy(dres, t->out_init, (size_t)t->down_rows * 4, cudaMemcpyHostToDevice)))
+            return s.rc;
+        c.Wd.base = dtd;
+    }
+    // activations, epilogue buffers, the step state and the argmax partials
+    if (f16 || t->norm) {
+        if (!s.alloc(&dx, (size_t)cols * 4)) return s.rc;
+    } else if (!s.alloc(&dxq, (size_t)V * cols) || !s.alloc(&dxs, (size_t)V * nb * 4)) return s.rc;
+    if (t->norm && (!s.alloc(&dnw, (size_t)cols * 4) || !s.ok(cudaMemcpy(dnw, t->norm_w, (size_t)cols * 4, cudaMemcpyHostToDevice)))) return s.rc;
+    DevMat emb{};
+    if (t->from_emb) { // the embedding as the plan keeps a Q8_0 one: quants and f16 scales in separate planes
+        const size_t n = (size_t)t->emb_rows * cols;
+        std::vector<int8_t> q(n);
+        std::vector<uint16_t> sc(n / 32);
+        const unsigned char *raw = (const unsigned char *)t->emb;
+        for (size_t b = 0; b < n / 32; b++) {
+            memcpy(&sc[b], raw + b * 34, 2);
+            memcpy(&q[b * 32], raw + b * 34 + 2, 32);
+        }
+        if (!s.alloc(&dembq, n) || !s.alloc(&dembs, n / 32 * 2) || !s.ok(cudaMemcpy(dembq, q.data(), n, cudaMemcpyHostToDevice)) ||
+            !s.ok(cudaMemcpy(dembs, sc.data(), n / 32 * 2, cudaMemcpyHostToDevice)))
+            return s.rc;
+        emb = DevMat{dembq, dembs, t->emb_rows, cols, B200_GGML_Q8_0};
+    }
+    if (gateup && !f16 &&
+        (!s.alloc(&dhq, (size_t)V * rows) || !s.alloc(&dhs, (size_t)V * (rows / 32) * 4) || !s.alloc(&dblk, (size_t)V * (rows / 32) * 4) ||
+         !s.ok(cudaMemset(dhq, 0x5A, (size_t)V * rows)) || !s.ok(cudaMemset(dhs, 0xFF, (size_t)V * (rows / 32) * 4)) ||
+         !s.ok(cudaMemset(dblk, 0, (size_t)V * (rows / 32) * 4))))
+        return s.rc;
+    if (!s.alloc(&dst, sizeof(StepState))) return s.rc;
+    if (t->argmax && (!s.alloc(&dpv, (size_t)V * c.grid * 4) || !s.alloc(&dpi, (size_t)V * c.grid * 4) || !s.alloc(&dids, (size_t)t->launches * V * 4)))
+        return s.rc;
+
+    // the shared-memory attributes set_smem_attrs gives every plan
+    with_stream_mode(t->mode, [&](auto M) {
+        constexpr int MODE = decltype(M)::value;
+        if (f16) s.ok(t->lanes == 16 ? set_max_dyn(k_stream_matvec_f16<16, MODE>, optin) : set_max_dyn(k_stream_matvec_f16<8, MODE>, optin));
+        else if (batch) s.ok(cudaFuncSetAttribute(k_stream_matvec_q8_batch<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMB_SMEM_BUDGET));
+        else if (!t->norm) s.ok(set_max_dyn(smv_kernel<MODE>(fmt), optin));
+        else if constexpr (MODE != SMV_RESID) s.ok(set_max_dyn(smv_norm_kernel<MODE>(fmt), optin));
+    });
+    if (t->pair) s.ok(set_max_dyn(smv_kernel<SMV_RESID>(fmt), optin));
+    if (s.rc) return s.rc;
+
+    for (int l = 0; l < t->launches; l++) {
+        const StepState st{t->from_emb ? t->tokens[l] : 0, 0, l, 0, 0, {0, 0, 0}};
+        if (!s.ok(cudaMemcpy(dst, &st, sizeof st, cudaMemcpyHostToDevice))) return s.rc;
+        if (t->from_emb) {
+            if (!s.ok(cudaMemset(dx, 0xFF, (size_t)cols * 4))) return s.rc;
+        } else if (dx) {
+            if (!s.ok(cudaMemcpy(dx, t->x + (size_t)l * cols, (size_t)cols * 4, cudaMemcpyHostToDevice))) return s.rc;
+        } else if (!s.ok(cudaMemcpy(dxq, t->xq + (size_t)l * V * cols, (size_t)V * cols, cudaMemcpyHostToDevice)) ||
+                   !s.ok(cudaMemcpy(dxs, t->xs + (size_t)l * V * nb, (size_t)V * nb * 4, cudaMemcpyHostToDevice)))
+            return s.rc;
+        with_stream_mode(t->mode, [&](auto M) {
+            constexpr int MODE = decltype(M)::value;
+            const dim3 grid(c.grid);
+            if (f16) {
+                SfArgs a{};
+                a.w0 = (const __half *)dw; a.w1 = gateup ? (const __half *)(dw + wbytes) : nullptr; a.x = dx; a.out = dout; a.oscale = t->oscale;
+                a.rows = rows; a.cols = cols; a.seg = c.F.seg; a.nseg = c.F.nseg; a.stages = c.stages; a.tr = none;
+                a.part_val = dpv; a.part_idx = dpi;
+                s.ok(t->lanes == 16 ? launch_on(0, true, k_stream_matvec_f16<16, MODE>, grid, dim3(SF_THREADS), c.total, a)
+                                    : launch_on(0, true, k_stream_matvec_f16<8, MODE>, grid, dim3(SF_THREADS), c.total, a));
+            } else if (batch) {
+                SmbArgs a{};
+                a.W = c.W; a.nrow = t->nrow; a.xq = dxq; a.xs = dxs; a.out = dout; a.oscale = t->oscale; a.ostride = rows; a.hq = dhq; a.hs = dhs;
+                a.blk_cnt = dblk; a.part_val = dpv; a.part_idx = dpi;
+                s.ok(launch_on(0, true, k_stream_matvec_q8_batch<MODE>, grid, dim3(SMV_THREADS), c.total, a, c.B));
+            } else {
+                SmvArgs a{};
+                a.W = c.W; a.xq = dxq; a.xs = dxs; a.out = dout; a.oscale = t->oscale; a.hq = dhq; a.hs = dhs; a.blk_cnt = dblk;
+                a.part_val = dpv; a.part_idx = dpi; a.tr = none; a.tp = solo; a.wait_slot = -1; a.out_slot = -1;
+                if (!t->norm) s.ok(launch_on(0, true, smv_kernel<MODE>(fmt), grid, dim3(SMV_THREADS), c.total, a, c.L));
+                else if constexpr (MODE != SMV_RESID) {
+                    SmvNormArgs n{};
+                    n.x = dx; n.w = dnw; n.st = dst; n.emb = emb; n.emb_scale = t->emb_scale; n.eps = t->eps; n.from_emb = t->from_emb ? 1 : 0;
+                    n.x_out = dx; n.off_sq = c.off_sq; n.off_seq = c.off_seq;
+                    s.ok(launch_on(0, true, smv_norm_kernel<MODE>(fmt), grid, dim3(SMV_THREADS), c.total, a, c.L, n));
+                }
+            }
+        });
+        if (t->pair && s.rc == B200_OK) { // W2 after gate/up, as the decode graph chains them
+            SmvArgs a{};
+            a.W = c.Wd; a.xq = dhq; a.xs = dhs; a.out = dres; a.oscale = t->oscale; a.tr = none; a.tp = solo; a.wait_slot = -1; a.out_slot = -1;
+            s.ok(launch_on(0, true, smv_kernel<SMV_RESID>(fmt), dim3(c.grid), dim3(SMV_THREADS), c.Ld.total, a, c.Ld));
+        }
+        if (t->argmax && s.rc == B200_OK) {
+            if (batch) s.ok(launch_on(0, true, k_argmax_batch, dim3(V), dim3(32), (size_t)0, (const float *)dpv, (const int *)dpi, c.grid, dids + (size_t)l * V));
+            else
+                s.ok(launch_on(0, true, k_argmax_advance, dim3(1), dim3(1024), (size_t)0, (const float *)dout, rows, dst, (const int *)nullptr, dids, 1,
+                               (const float *)dpv, (const int *)dpi, c.grid, none, solo, -1));
+        }
+        unsigned guard[GUARD];
+        if (!s.ok(cudaGetLastError()) || !s.ok(cudaDeviceSynchronize()) ||
+            !s.ok(cudaMemcpy(t->out + (size_t)l * V * rows, dout, obytes, cudaMemcpyDeviceToHost)) ||
+            !s.ok(cudaMemcpy(guard, (const unsigned char *)dout + obytes, sizeof guard, cudaMemcpyDeviceToHost)))
+            return s.rc;
+        for (unsigned g : guard)
+            if (g != 0xFFFFFFFFu) return B200_ERR_STATE;
+        if (dhq && (!s.ok(cudaMemcpy(t->hq + (size_t)l * V * rows, dhq, (size_t)V * rows, cudaMemcpyDeviceToHost)) ||
+                    !s.ok(cudaMemcpy(t->hs + (size_t)l * V * (rows / 32), dhs, (size_t)V * (rows / 32) * 4, cudaMemcpyDeviceToHost))))
+            return s.rc;
+        if (t->pair && !s.ok(cudaMemcpy(t->out_down + (size_t)l * t->down_rows, dres, (size_t)t->down_rows * 4, cudaMemcpyDeviceToHost))) return s.rc;
+        if (t->from_emb && !s.ok(cudaMemcpy(t->x_out + (size_t)l * cols, dx, (size_t)cols * 4, cudaMemcpyDeviceToHost))) return s.rc;
+        if (t->argmax && !s.ok(cudaMemcpy(t->ids + (size_t)l * V, batch ? dids + (size_t)l * V : dids + l, (size_t)V * 4, cudaMemcpyDeviceToHost))) return s.rc;
     }
     return s.rc;
 }

@@ -72,6 +72,15 @@ def _controls_c(c: SamplingControls):
     return s, (ids, vals)
 
 
+class StreamTest(C.Structure):
+    """b200_stream_test: the arguments and the reported configuration of b200_test_stream."""
+    _fields_ = [(n, C.c_int32) for n in ("form", "mode", "norm", "nrow", "lanes", "rows", "cols", "grid", "stages")] + [("budget", C.c_int64)] + \
+               [(n, C.c_int32) for n in ("argmax", "launches", "pair", "down_rows", "from_emb", "emb_rows", "dry")] + \
+               [(n, C.c_float) for n in ("oscale", "eps", "emb_scale")] + \
+               [(n, C.c_void_p) for n in ("w", "w_up", "w_down", "xq", "xs", "x", "norm_w", "emb", "tokens", "out_init", "out", "hq", "hs", "out_down",
+                                          "x_out", "ids")] + [("info", C.c_int64 * 5)]
+
+
 class Tensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("ggml_type", C.c_int32), ("n_dims", C.c_int32),
                 ("dims", C.c_int64 * 4)]
@@ -82,7 +91,7 @@ EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
            "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_forward_chunk", "b200_chunk_rows", "b200_weight_info", "b200_test_set_memory_budget", "b200_stream_rings",
-           "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
+           "b200_test_stream", "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
 
@@ -151,6 +160,7 @@ def lib() -> C.CDLL:
     L.b200_test_set_memory_budget.argtypes = [C.c_int64]
     L.b200_test_kq_tiles_to_q8.argtypes = [i32, i32, i32, vp, vp, C.c_int64]
     L.b200_stream_rings.argtypes = [C.POINTER(i32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    L.b200_test_stream.argtypes = [C.POINTER(StreamTest)]
     L.b200_launches_per_decode.argtypes = [vp]
     L.b200_device_bytes.argtypes = [vp]
     L.b200_device_bytes.restype = C.c_int64
@@ -390,6 +400,62 @@ def test_gemm_i8(mode: str, aq, a_scales, bq, c=None, bq2=None, oscale: float = 
     if rc != B200_OK:
         _raise(rc, "b200_test_gemm_i8 failed")
     return c
+
+
+STREAM_MODES = {"store": 0, "resid": 1, "gateup": 2}
+STREAM_INFO = ("stages", "grid", "max_groups", "min_groups", "smem")
+
+
+def test_stream(form: int, mode: str, w, rows: int, cols: int, *, w_up=None, w_down=None, down_rows: int = 0, xq=None, xs=None, x=None,
+                norm_w=None, eps: float = 1e-5, emb=None, emb_rows: int = 0, tokens=None, emb_scale: float = 1.0, out_init=None,
+                oscale: float = 1.0, nrow: int = 0, lanes: int = 16, grid: int = 0, stages: int = 0, budget: int = 0, argmax: bool = False,
+                launches: int = 1, pair: bool = False, dry: bool = False) -> dict:
+    """b200_test_stream: one decode weight stream launched as the plan launches it, at any grid and ring depth.  form: 8 (Q8_0 tiles),
+    12 / 13 / 14 (resident K-quant tiles) or 1 (F16 rings); w (and w_up for "gateup", w_down for pair) are raw GGUF rows of that type.
+    Activations per launch: xq int8 [launches][V][cols] and xs [launches][V][cols / 32] (V = max(nrow, 1)), or x float32 [launches][cols]
+    for F16 and the fused norm (norm_w given; emb + tokens instead of x: the embedding rows).  Returns {"info": the configuration run,
+    and per launch "out", "hq", "hs", "out_down", "x_out", "ids" where they apply}.  dry: only the checks and "info" (grid must be given)."""
+    V = max(nrow, 1)
+    keep = []
+
+    def arr(a, dtype):
+        if a is None:
+            return None
+        a = np.ascontiguousarray(a, dtype=dtype)
+        keep.append(a)
+        return a.ctypes.data
+
+    t = StreamTest()
+    t.form, t.mode, t.norm, t.nrow, t.lanes, t.rows, t.cols = form, STREAM_MODES[mode], norm_w is not None, nrow, lanes, rows, cols
+    t.grid, t.stages, t.budget, t.argmax, t.launches, t.pair, t.down_rows = grid, stages, budget, argmax, launches, pair, down_rows
+    t.from_emb, t.emb_rows, t.dry, t.oscale, t.eps, t.emb_scale = emb is not None, emb_rows, dry, oscale, eps, emb_scale
+    t.w, t.w_up, t.w_down = arr(w, np.uint8 if form != 1 else np.uint16), arr(w_up, np.uint8 if form != 1 else np.uint16), arr(w_down, np.uint8)
+    t.xq, t.xs, t.x, t.norm_w, t.emb, t.tokens = arr(xq, np.int8), arr(xs, np.float32), arr(x, np.float32), arr(norm_w, np.float32), arr(emb, np.uint8), \
+        arr(tokens, np.int32)
+    t.out_init = arr(out_init, np.float32)
+    res = {}
+    if not dry:
+        res["out"] = np.empty((launches, V, rows), np.float32)
+        t.out = res["out"].ctypes.data
+        if mode == "gateup" and form != 1:
+            res["hq"], res["hs"] = np.empty((launches, V, rows), np.int8), np.empty((launches, V, rows // 32), np.float32)
+            t.hq, t.hs = res["hq"].ctypes.data, res["hs"].ctypes.data
+        if pair:
+            res["out_down"] = np.empty((launches, down_rows), np.float32)
+            t.out_down = res["out_down"].ctypes.data
+        if emb is not None:
+            res["x_out"] = np.empty((launches, cols), np.float32)
+            t.x_out = res["x_out"].ctypes.data
+        if argmax:
+            res["ids"] = np.empty((launches, V), np.int32)
+            t.ids = res["ids"].ctypes.data
+    else:  # the pointer checks of a real launch, without the buffers
+        t.out = t.hq = t.hs = t.x_out = t.ids = t.out_down = 1
+    rc = lib().b200_test_stream(C.byref(t))
+    if rc != B200_OK:
+        _raise(rc, "b200_test_stream failed")
+    res["info"] = dict(zip(STREAM_INFO, t.info))
+    return res
 
 
 def _pf_attention_packed(qs, ks, vs, starts, n_heads: int, n_kv_heads: int, out_rows: int | None, sentinel: int) -> np.ndarray:

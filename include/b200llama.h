@@ -647,6 +647,53 @@ int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, i
 int b200_test_gemm_i8(int32_t mode, int32_t m, int32_t n, int32_t k, const int8_t *aq, const float *as, const void *bq, const void *bq2, float oscale,
                       float *c, int8_t *hq, float *hs);
 
+/* One decode weight stream launched on its own (b200_test_stream).  Arrays are indexed [launch][row][...]; V = max(nrow, 1). */
+typedef struct b200_stream_test {
+    int32_t form;      /* B200_GGML_Q8_0 (Q8_0 tiles), B200_GGML_Q4_K / Q5_K / Q6_K (resident tiles) or B200_GGML_F16 (row-major rings) */
+    int32_t mode;      /* 0 STORE, 1 RESID, 2 GATEUP */
+    int32_t norm;      /* 1: the fused-RMSNorm kernel (STORE or GATEUP, Q8_0 or resident tiles, cols <= 5120) */
+    int32_t nrow;      /* 0: the single-row stream; 1..8: the batched Q8_0 stream over nrow activation rows */
+    int32_t lanes;     /* F16: 16 or 8 */
+    int32_t rows;      /* output rows; GATEUP: hidden units (the gate and the up matrix have `rows` rows each) */
+    int32_t cols;
+    int32_t grid;      /* CTAs; 0: what the plan launches */
+    int32_t stages;    /* ring stages, turned into the budget that yields them (F16: SfArgs::stages); 0: from `budget` */
+    int64_t budget;    /* Q8_0 / resident ring budget in bytes; 0: the plan's (96 KB single-row, 112 KB batched, sf_layout for F16) */
+    int32_t argmax;    /* STORE: per-CTA argmax partials, then the plan's merge (k_argmax_advance / k_argmax_batch) into ids */
+    int32_t launches;  /* 1 or 2: the second launch reuses every buffer (blk_cnt too) with the second set of activations */
+    int32_t pair;      /* GATEUP, single row: then a RESID stream of w_down [down_rows][rows] reading its hq / hs, both under PDL */
+    int32_t down_rows;
+    int32_t from_emb;  /* norm: the activation is row tokens[launch] of emb (GGUF Q8_0, emb_rows x cols) times emb_scale */
+    int32_t emb_rows;
+    int32_t dry;       /* 1: return after the checks with info filled in; makes no CUDA call (grid must be given) */
+    float oscale, eps, emb_scale;
+    const void *w;        /* GGUF Q8_0 rows, raw K-quant rows or f16 rows [rows][cols]; GATEUP: the gate matrix */
+    const void *w_up;     /* GATEUP: the up matrix, same format */
+    const void *w_down;   /* pair: [down_rows][rows], same format */
+    const int8_t *xq;     /* Q8_0 / resident without norm: the quantised activation [launches][V][cols] ... */
+    const float *xs;      /* ... and its block scales [launches][V][cols / 32] */
+    const float *x;       /* norm (without from_emb) and F16: the activation [launches][cols] */
+    const float *norm_w;  /* norm: [cols] */
+    const void *emb;
+    const int32_t *tokens;   /* from_emb: [launches] */
+    const float *out_init;   /* RESID: the initial out [V][rows]; pair: the initial residual [down_rows] */
+    float *out;              /* out: [launches][V][rows] after each launch (GATEUP: the float hidden values) */
+    int8_t *hq;              /* GATEUP out: [launches][V][rows] ... */
+    float *hs;               /* ... and [launches][V][rows / 32] */
+    float *out_down;         /* pair out: the residual after each launch [launches][down_rows] */
+    float *x_out;            /* from_emb out: CTA 0's write of x [launches][cols] */
+    int32_t *ids;            /* argmax out: [launches][V] */
+    int64_t info[5];         /* out: ring stages, grid, largest and smallest 4-row groups (F16: row groups) per CTA, dynamic shared memory */
+} b200_stream_test;
+
+/* Test hook: the decode weight stream of `form` launched as the plan launches it (upload repack, layout, kernel, shared-memory
+ * attribute), but at any grid and ring depth the caller asks for.  B200_ERR_BAD_ARG, before any CUDA call, for what the plan would
+ * never launch: a width that is not whole segments of the form, stages outside 3..SMV_MAX_STAGES (F16: SF_MAX_STAGES), a GATEUP whose
+ * largest CTA slice exceeds the epilogue buffer at that grid, a fused norm with RESID or cols > 5120, nrow > 8 or a batch on a
+ * resident or F16 form; and, once the device is known, a ring above its opt-in shared-memory limit.  B200_ERR_STATE when a store
+ * reached the guard words past `out` (a padding row of a ragged STORE). */
+int b200_test_stream(b200_stream_test *t);
+
 /* Test hook: the causal attention of the tensor-core prefill (k_pf_attention_mma_packed, on f16 K / V copies built by
  * k_pf_kv_to_f16_packed, as a chunk runs it) over n_seqs sequences at once.  Sequence i has lengths[i] >= 1 query tokens at positions
  * start_positions[i]..; q: f32 [sum lengths][n_heads * head_size] (rotated; the sequences' rows back to back, placed in rows of

@@ -22,11 +22,103 @@
 #define MOE_MAX_EXPERTS 256
 #define MOE_ROUTE_THREADS 256
 
+// ---- the routing tails: one per family, shared by the decode routers below and the chunk router k_xp_route ---------------------
+// logit(j): router logit j (j = n_experts: the shared-expert gate's); pr: n_experts floats of scratch.
+
+// Qwen2-MoE, on one thread, in the reference's order: softmaxInPlace (FloatTensor.java:211-219: max; (float) Math.exp(f - max);
+// sequential sum from 0f; divide); k scans for the first strict maximum, each pick then set to -inf, its weight the probability
+// itself (no renormalisation); then the shared-expert weight 1f / (1f + (float) Math.exp(-g)) into weights[k].
+template <class Logit>
+__device__ __forceinline__ void moe_route_tail(Logit logit, int E, int k, float *pr, int *ids, float *weights) {
+    float mx = -INFINITY;
+    for (int j = 0; j < E; j++) { pr[j] = logit(j); mx = fmaxf(mx, pr[j]); }
+    for (int j = 0; j < E; j++) pr[j] = (float)exp((double)__fsub_rn(pr[j], mx));
+    float sum = 0.0f;
+    for (int j = 0; j < E; j++) sum = __fadd_rn(sum, pr[j]);
+    for (int j = 0; j < E; j++) pr[j] = __fdiv_rn(pr[j], sum);
+    for (int i = 0; i < k; i++) {
+        float best = -INFINITY;
+        int idx = 0;
+        for (int j = 0; j < E; j++)
+            if (pr[j] > best) { best = pr[j]; idx = j; }
+        ids[i] = idx;
+        weights[i] = best;
+        pr[idx] = -INFINITY;
+    }
+    const float g = logit(E);
+    weights[k] = __fdiv_rn(1.0f, __fadd_rn(1.0f, (float)exp((double)(-g))));
+}
+
+// Qwen3-MoE, on one warp (every lane calls it).  The max, the exps and the top-k scans are order-free given the lowest-index
+// tie-break, so each lane takes experts lane, lane + 32, ...; the softmax sum and the renormalisation sum stay sequential on lane 0:
+// softmaxInPlace; k scans for the first strict maximum, each pick then set to -inf; s = 0f, s += p_j in selection order; w_j = p_j / s.
+template <class Logit>
+__device__ __forceinline__ void routed_route_tail(Logit logit, int E, int k, float *pr, int *ids, float *weights, int lane) {
+    constexpr int PER_LANE = MOE_MAX_EXPERTS / 32;
+    float v[PER_LANE];
+    float mx = -INFINITY;
+#pragma unroll
+    for (int r = 0; r < PER_LANE; r++) {
+        const int j = lane + 32 * r;
+        v[r] = j < E ? logit(j) : -INFINITY;
+        mx = fmaxf(mx, v[r]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+#pragma unroll
+    for (int r = 0; r < PER_LANE; r++) {
+        const int j = lane + 32 * r;
+        if (j < E) pr[j] = v[r] = (float)exp((double)__fsub_rn(v[r], mx));
+    }
+    __syncwarp();
+    float sum = 0.0f;
+    if (lane == 0)
+        for (int j = 0; j < E; j++) sum = __fadd_rn(sum, pr[j]);
+    sum = __shfl_sync(0xffffffffu, sum, 0);
+#pragma unroll
+    for (int r = 0; r < PER_LANE; r++) v[r] = lane + 32 * r < E ? __fdiv_rn(v[r], sum) : -INFINITY;
+    float pick[MOE_MAX_K];
+    int pick_id[MOE_MAX_K];
+#pragma unroll
+    for (int i = 0; i < MOE_MAX_K; i++) {
+        if (i >= k) break;
+        // the lane's first strict maximum (its experts in index order), then the lowest index among the lanes' equal maxima
+        float best = -INFINITY;
+        int idx = 0x7fffffff;
+#pragma unroll
+        for (int r = 0; r < PER_LANE; r++)
+            if (v[r] > best) { best = v[r]; idx = lane + 32 * r; }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+            if (ob > best || (ob == best && oi < idx)) { best = ob; idx = oi; }
+        }
+        if (idx == 0x7fffffff) idx = 0; // no probability above -inf: the scan keeps index 0
+#pragma unroll
+        for (int r = 0; r < PER_LANE; r++)
+            if (lane + 32 * r == idx) v[r] = -INFINITY;
+        pick[i] = best;
+        pick_id[i] = idx;
+    }
+    if (lane == 0) {
+        float s = 0.0f;
+#pragma unroll
+        for (int i = 0; i < MOE_MAX_K; i++)
+            if (i < k) s = __fadd_rn(s, pick[i]);
+#pragma unroll
+        for (int i = 0; i < MOE_MAX_K; i++)
+            if (i < k) {
+                ids[i] = pick_id[i];
+                weights[i] = __fdiv_rn(pick[i], s);
+            }
+    }
+}
+
 // ---- router --------------------------------------------------------------------------------------------------------------
 // One CTA per router row plus one for the shared-expert gate (blockIdx.x == n_experts): each evaluates FloatTensor.scalarDot
 // (FloatTensor.java:86-92) -- result += w[j] * x[j], one float multiply and one float add per term, strictly in index order.
-// The products are formed in parallel; one thread walks the sum.  The last CTA to finish runs softmaxInPlace, the top-k scans
-// and the shared-expert sigmoid on one thread, in the reference's order.
+// The products are formed in parallel; one thread walks the sum.  The last CTA to finish runs moe_route_tail on one thread.
 struct MoeRouteArgs {
     const float *router;      // [n_experts][dim] F32 (ffn_gate_inp)
     const float *shared_gate; // [dim] F32 (ffn_gate_inp_shexp)
@@ -61,39 +153,16 @@ __global__ void __launch_bounds__(MOE_ROUTE_THREADS, 1) k_moe_route(MoeRouteArgs
     if (!s_last || tid != 0) { trace_mark(a.tr, 3); return; }
     __threadfence();
     *a.done = 0u;
-    const int E = a.n_experts;
-    // softmaxInPlace (FloatTensor.java:211-219): max; (float) Math.exp(f - max); sequential sum from 0f; divide
-    float mx = -INFINITY;
-    for (int j = 0; j < E; j++) { pr[j] = ldcg_f32(a.logits + j); mx = fmaxf(mx, pr[j]); }
-    for (int j = 0; j < E; j++) pr[j] = (float)exp((double)__fsub_rn(pr[j], mx));
-    float sum = 0.0f;
-    for (int j = 0; j < E; j++) sum = __fadd_rn(sum, pr[j]);
-    for (int j = 0; j < E; j++) pr[j] = __fdiv_rn(pr[j], sum);
-    // top-k: k scans for the first strict maximum, each pick then set to -inf; the weight is the probability itself (no renormalisation)
-    for (int i = 0; i < a.k; i++) {
-        float best = -INFINITY;
-        int idx = 0;
-        for (int j = 0; j < E; j++)
-            if (pr[j] > best) { best = pr[j]; idx = j; }
-        a.ids[i] = idx;
-        a.weights[i] = best;
-        pr[idx] = -INFINITY;
-    }
-    // shared-expert weight: 1f / (1f + (float) Math.exp(-g))
-    const float g = ldcg_f32(a.logits + E);
-    a.weights[a.k] = __fdiv_rn(1.0f, __fadd_rn(1.0f, (float)exp((double)(-g))));
+    moe_route_tail([&](int j) { return ldcg_f32(a.logits + j); }, a.n_experts, a.k, pr, a.ids, a.weights);
     trace_mark(a.tr, 3);
 }
 
-// Qwen3-MoE's router: one CTA per router row (no shared-expert gate), the same scalarDot per row, and a tail on one warp of the last
-// CTA.  The max, the exps and the top-k scans are order-free given the lowest-index tie-break, so each lane takes experts
-// lane, lane + 32, ...; the softmax sum and the renormalisation sum stay sequential on lane 0:
-// softmaxInPlace; k scans for the first strict maximum, each pick then set to -inf; s = 0f, s += p_j in selection order; w_j = p_j / s.
+// Qwen3-MoE's router: one CTA per router row (no shared-expert gate), the same scalarDot per row, and routed_route_tail on one warp
+// of the last CTA.
 __global__ void __launch_bounds__(MOE_ROUTE_THREADS, 1) k_routed_route(MoeRouteArgs a) {
     extern __shared__ __align__(16) float t[]; // dim terms
     __shared__ float pr[MOE_MAX_EXPERTS];
     __shared__ unsigned s_last;
-    constexpr int PER_LANE = MOE_MAX_EXPERTS / 32;
     const int tid = threadIdx.x, e = blockIdx.x;
     const float *w = a.router + (size_t)e * a.dim;
     trace_entry(a.tr);
@@ -111,67 +180,60 @@ __global__ void __launch_bounds__(MOE_ROUTE_THREADS, 1) k_routed_route(MoeRouteA
     __syncthreads();
     if (!s_last || tid >= 32) { trace_mark(a.tr, 3); return; }
     __threadfence();
-    const int lane = tid, E = a.n_experts;
-    if (lane == 0) *a.done = 0u;
-    float v[PER_LANE];
-    float mx = -INFINITY;
-#pragma unroll
-    for (int r = 0; r < PER_LANE; r++) {
-        const int j = lane + 32 * r;
-        v[r] = j < E ? ldcg_f32(a.logits + j) : -INFINITY;
-        mx = fmaxf(mx, v[r]);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-#pragma unroll
-    for (int r = 0; r < PER_LANE; r++) {
-        const int j = lane + 32 * r;
-        if (j < E) pr[j] = v[r] = (float)exp((double)__fsub_rn(v[r], mx));
-    }
-    __syncwarp();
-    float sum = 0.0f;
-    if (lane == 0)
-        for (int j = 0; j < E; j++) sum = __fadd_rn(sum, pr[j]);
-    sum = __shfl_sync(0xffffffffu, sum, 0);
-#pragma unroll
-    for (int r = 0; r < PER_LANE; r++) v[r] = lane + 32 * r < E ? __fdiv_rn(v[r], sum) : -INFINITY;
-    float pick[MOE_MAX_K];
-    int pick_id[MOE_MAX_K];
-#pragma unroll
-    for (int i = 0; i < MOE_MAX_K; i++) {
-        if (i >= a.k) break;
-        // the lane's first strict maximum (its experts in index order), then the lowest index among the lanes' equal maxima
-        float best = -INFINITY;
-        int idx = 0x7fffffff;
-#pragma unroll
-        for (int r = 0; r < PER_LANE; r++)
-            if (v[r] > best) { best = v[r]; idx = lane + 32 * r; }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-            if (ob > best || (ob == best && oi < idx)) { best = ob; idx = oi; }
-        }
-        if (idx == 0x7fffffff) idx = 0; // no probability above -inf: the scan keeps index 0
-#pragma unroll
-        for (int r = 0; r < PER_LANE; r++)
-            if (lane + 32 * r == idx) v[r] = -INFINITY;
-        pick[i] = best;
-        pick_id[i] = idx;
-    }
-    if (lane == 0) {
-        float s = 0.0f;
-#pragma unroll
-        for (int i = 0; i < MOE_MAX_K; i++)
-            if (i < a.k) s = __fadd_rn(s, pick[i]);
-#pragma unroll
-        for (int i = 0; i < MOE_MAX_K; i++)
-            if (i < a.k) {
-                a.ids[i] = pick_id[i];
-                a.weights[i] = __fdiv_rn(pick[i], s);
-            }
-    }
+    if (tid == 0) *a.done = 0u;
+    routed_route_tail([&](int j) { return ldcg_f32(a.logits + j); }, a.n_experts, a.k, pr, a.ids, a.weights, tid);
     trace_mark(a.tr, 3);
+}
+
+// ---- the chunk router of B200_PREFILL_TENSOR_CORE_EXACT_MOE ---------------------------------------------------------------------
+// XP_ROUTE_TOKENS chunk rows per CTA.  Thread e evaluates router row e (and, with a shared expert, the gate row at e = n_experts)
+// against each row's float FFN-norm output as the decode router does: result = 0f, result += fl(w[j] * x[j]) in index order, one
+// independent chain per row.  Then warp v runs the family's routing tail for row v.  The routing of row t goes to ids[t][k] and
+// weights[t][nw] (nw = k, + 1 with a shared expert).
+#define XP_ROUTE_TOKENS 4
+struct XpRouteArgs {
+    const float *router, *shared_gate; // as MoeRouteArgs
+    const float *xb;                   // [n][dim] float FFN-norm rows of the chunk
+    int *ids;                          // [n][k]
+    float *weights;                    // [n][nw]
+    int n, dim, n_experts, k, nw;
+};
+
+template <bool SHARED>
+__global__ void __launch_bounds__(MOE_ROUTE_THREADS, 1) k_xp_route(XpRouteArgs a) {
+    __shared__ float lg[XP_ROUTE_TOKENS][MOE_MAX_EXPERTS + 1];
+    __shared__ float pr[XP_ROUTE_TOKENS][MOE_MAX_EXPERTS];
+    const int t0 = blockIdx.x * XP_ROUTE_TOKENS, nt = min(XP_ROUTE_TOKENS, a.n - t0);
+    const int nrow = a.n_experts + (SHARED ? 1 : 0);
+    for (int e = threadIdx.x; e < nrow; e += MOE_ROUTE_THREADS) {
+        const float4 *w = reinterpret_cast<const float4 *>(e < a.n_experts ? a.router + (size_t)e * a.dim : a.shared_gate);
+        float acc[XP_ROUTE_TOKENS];
+#pragma unroll
+        for (int v = 0; v < XP_ROUTE_TOKENS; v++) acc[v] = 0.0f;
+        for (int i = 0; i < a.dim / 4; i++) {
+            const float4 w4 = __ldg(w + i);
+#pragma unroll
+            for (int v = 0; v < XP_ROUTE_TOKENS; v++) {
+                const float4 x4 = __ldg(reinterpret_cast<const float4 *>(a.xb + (size_t)(t0 + min(v, nt - 1)) * a.dim) + i);
+                acc[v] = __fadd_rn(acc[v], __fmul_rn(w4.x, x4.x));
+                acc[v] = __fadd_rn(acc[v], __fmul_rn(w4.y, x4.y));
+                acc[v] = __fadd_rn(acc[v], __fmul_rn(w4.z, x4.z));
+                acc[v] = __fadd_rn(acc[v], __fmul_rn(w4.w, x4.w));
+            }
+        }
+#pragma unroll
+        for (int v = 0; v < XP_ROUTE_TOKENS; v++) lg[v][e] = acc[v];
+    }
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (warp >= nt) return;
+    const int t = t0 + warp;
+    auto logit = [&](int j) { return lg[warp][j]; };
+    if (SHARED) {
+        if (lane == 0) moe_route_tail(logit, a.n_experts, a.k, pr[warp], a.ids + (size_t)t * a.k, a.weights + (size_t)t * a.nw);
+    } else {
+        routed_route_tail(logit, a.n_experts, a.k, pr[warp], a.ids + (size_t)t * a.k, a.weights + (size_t)t * a.nw, lane);
+    }
 }
 
 // ---- the expert streams --------------------------------------------------------------------------------------------------

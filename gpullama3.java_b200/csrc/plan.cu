@@ -171,9 +171,9 @@ struct b200_plan {
     // built or why not.  exact is always ready; b200_set_prefill_mode builds the others (build() an FP16 plan's tensor_core) and
     // selects a mode only once it is ready.
     int pf_mode = B200_PREFILL_EXACT;
-    struct PrefillMode { bool ready; const char *why; } pf[4] = {{true, ""}, {false, ""}, {false, ""}, {false, ""}};
+    struct PrefillMode { bool ready; const char *why; } pf[5] = {{true, ""}, {false, ""}, {false, ""}, {false, ""}, {false, ""}};
     PrefillCtx prefill; // tensor_core and tensor_core_w8a16 (prefill.cuh)
-    PrefillI8Ctx pi8;   // tensor_core_exact (prefill_i8.cuh)
+    PrefillI8Ctx pi8;   // tensor_core_exact and, on MoE plans, tensor_core_exact_moe (prefill_i8.cuh)
     // persistent decode kernel
     bool pd_ok = false;           // the plan fits the kernel's restrictions
     std::string pd_why;           // ... or why not
@@ -1894,8 +1894,10 @@ int build(b200_plan *p, const b200_tensor *tensors, int n_tensors) {
 }
 
 // ---- batched prefill on the tensor cores (prefill.cuh) -------------------------------------------
-static const char *const MOE_PREFILL_WHY = "Qwen2-MoE plans have no tensor-core prefill: prompts go through the exact token-by-token prefill";
-static const char *const MOE3_PREFILL_WHY = "Qwen3-MoE plans have no tensor-core prefill: prompts go through the exact token-by-token prefill";
+static const char *const MOE_PREFILL_WHY = "Qwen2-MoE plans have no tensor-core prefill in this mode: prompts go through the exact token-by-token "
+                                           "prefill, or through tensor_core_exact_moe on the tensor cores";
+static const char *const MOE3_PREFILL_WHY = "Qwen3-MoE plans have no tensor-core prefill in this mode: prompts go through the exact token-by-token "
+                                            "prefill, or through tensor_core_exact_moe on the tensor cores";
 static const char *moe_prefill_why(const b200_plan *p) { return p->moe_shared ? MOE_PREFILL_WHY : MOE3_PREFILL_WHY; }
 
 // The geometry of W as Q8_0 tiles: W itself, or for a resident matrix the tiles a Q8_0-tile plan of the same file holds, which
@@ -1904,18 +1906,27 @@ TileMat q8_geometry(const TileMat &W) { return W.fmt ? tile_geometry(W.rows, W.c
 
 // Why the plan cannot run prefill mode `mode` (nullptr: it can), decided before anything is allocated: MoE, then resident weights,
 // then the prefill batch size, the weight type, tensor parallelism, the shape, the stream segments and the tensor-map encoder, in
-// the order each mode has always checked them.
+// the order each mode has always checked them.  tensor_core_exact_moe: MoE plans only (always single-GPU Q8_0 tiles), then the
+// prefill batch size, the shape, every stream's segments (the experts' and the shared expert's included) and the encoder.
 const char *prefill_why(const b200_plan *p, int mode) {
     const b200_config &g = p->cfg;
     const int kv_mul = g.n_heads / g.n_kv_heads, nqkv = p->qd + 2 * p->kvd;
     const bool exact = mode == B200_PREFILL_TENSOR_CORE_EXACT, w8a16 = mode == B200_PREFILL_TENSOR_CORE_W8A16;
-    auto segs_ok = [&] { // every Q8_0 stream's segment (as Q8_0 tiles) a whole number of GEMM k-blocks
+    auto segs_ok = [&] { // every Q8_0 stream's segment (as Q8_0 tiles) a whole number of GEMM k-blocks (an absent stream has none)
         for (const LayerW &L : p->layers)
-            for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
+            for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2, &L.sgu, &L.sdn, &L.xgu, &L.xdn})
                 if (q8_geometry(*t).seg % pg::BK) return false;
         return true;
     };
     if (mode == B200_PREFILL_EXACT) return nullptr;
+    if (mode == B200_PREFILL_TENSOR_CORE_EXACT_MOE) {
+        if (!p->is_moe)
+            return "tensor_core_exact_moe runs the MoE FFN of Qwen2-MoE / Qwen3-MoE plans: a dense Q8_0 plan's bit-exact tensor-core prefill is tensor_core_exact";
+        if (p->prefill_batch <= 1) return "the plan was created without a prefill batch size (prefill_batch_size <= 1)";
+        if (g.dim % 64 || p->qd % 64 || nqkv % 64) return "the bit-exact tensor-core prefill needs dim, q width and q+k+v width multiples of 64";
+        if (!segs_ok()) return "the bit-exact tensor-core prefill needs Q8_0 stream segments (every expert's included) that are multiples of 64 columns";
+        return pg::encode_fn() ? nullptr : "cuTensorMapEncodeTiled not available from the driver";
+    }
     if (p->is_moe) return moe_prefill_why(p);
     if (p->resident && !exact)
         return "this plan keeps K-quant weights resident: the f16 and W8A16 tensor-core prefills read f16 matrices or Q8_0 tiles it does not "
@@ -2150,18 +2161,71 @@ bool i8_b_maps(const b200_plan *p, CUtensorMap *q, CUtensorMap *s, const TileMat
     return pg::make_map_i8_q8(q, base, rows, t.nseg, t.unit_bytes, 0) == 0 && pg::make_map_i8_q8(s, base, rows, t.nseg, t.unit_bytes, 1) == 0;
 }
 
-// Every layer's stream maps (pi8.maps); false if a tensor map was rejected.
+// Every layer's stream maps (pi8.maps); false if a tensor map was rejected.  An MoE layer has no dense FFN: its gate/up and W2
+// slots hold the shared expert's streams (Qwen2-MoE) or nothing (Qwen3-MoE).
 bool i8_weight_maps(b200_plan *p) {
     PrefillI8Ctx &c = p->pi8;
     c.maps.resize(p->cfg.n_layers);
     for (int l = 0; l < p->cfg.n_layers; l++) {
         const LayerW &L = p->layers[l];
         PrefillQ8Maps &m = c.maps[l];
-        if (!(i8_b_maps(p, &m.qkv_q, &m.qkv_s, L.tqkv) && i8_b_maps(p, &m.wo_q, &m.wo_s, L.two) && i8_b_maps(p, &m.gu_q, &m.gu_s, L.tgu) &&
-              i8_b_maps(p, &m.w2_q, &m.w2_s, L.tw2)))
+        if (!(i8_b_maps(p, &m.qkv_q, &m.qkv_s, L.tqkv) && i8_b_maps(p, &m.wo_q, &m.wo_s, L.two)))
             return false;
+        if (p->is_moe && !p->moe_shared) continue;
+        const TileMat &gu = p->is_moe ? L.sgu : L.tgu, &w2 = p->is_moe ? L.sdn : L.tw2;
+        if (!(i8_b_maps(p, &m.gu_q, &m.gu_s, gu) && i8_b_maps(p, &m.w2_q, &m.w2_s, w2))) return false;
     }
     return true;
+}
+
+// The FFN hidden width of the chunk's HQ / HS rows: the dense hidden dim, or an MoE plan's shared expert's (0 on Qwen3-MoE).
+int i8_hidden(const b200_plan *p) { return p->is_moe ? p->moe.shared_hidden_dim : p->cfg.hidden_dim; }
+
+// tensor_core_exact_moe's buffers (pi8.xp) for bpad chunk rows, and the per-expert tensor maps: 4 per expert per layer, encoded
+// on the host from each layer's stream-base tables and copied to the device once.  *ok = false if a tensor map was rejected.
+int prefill_init_xp(b200_plan *p, bool *ok) {
+    PrefillI8Ctx &c = p->pi8;
+    XpCtx &x = c.xp;
+    const b200_config &g = p->cfg;
+    const int E = p->moe.n_experts, k = p->moe.n_experts_used, He = p->moe.expert_hidden_dim, nl = g.n_layers;
+    const size_t na = (size_t)c.bpad * k, ga = na + pg::BM; // grouped rows, and what a tile of the last one may read
+    const int lds_d = pg::i8_lds(g.dim), lds_e = pg::i8_lds(He);
+    *ok = true;
+    if (x.maps) return B200_OK;
+    int rc;
+    auto zero = [&](auto **ptr, size_t bytes) {
+        int r = dalloc(p, ptr, bytes);
+        if (!r && cudaMemset(*ptr, 0, bytes) != cudaSuccess) r = fail(p, B200_ERR_CUDA, "cudaMemset failed");
+        return r;
+    };
+    if ((rc = zero(&x.XB, (size_t)c.bpad * g.dim * 4)) || (rc = zero(&x.ids, (size_t)nl * na * 4)) || (rc = zero(&x.w, (size_t)nl * c.bpad * p->moe_nw * 4)) ||
+        (rc = zero(&x.row_of, na * 4)) || (rc = zero(&x.offsets, (size_t)(E + 1) * 4)) || (rc = zero(&x.n_tiles, 4)) ||
+        (rc = zero(&x.tiles, (size_t)pg::xp_max_tiles((int)na, E) * sizeof(pg::XpTile))) || (rc = zero(&x.GQ, ga * g.dim)) ||
+        (rc = zero(&x.GS, ga * lds_d * 4)) || (rc = zero(&x.HQg, ga * He)) || (rc = zero(&x.HSg, ga * lds_e * 4)) || (rc = zero(&x.Yg, na * g.dim * 4)) ||
+        (p->moe_shared && (rc = zero(&x.Ys, (size_t)c.bpad * g.dim * 4))))
+        return rc;
+    *ok = pg::make_map_i8_a(&x.a_g, x.GQ, ga, g.dim) == 0 && pg::make_map_i8_s(&x.s_g, x.GS, ga, lds_d) == 0 && pg::make_map_i8_a(&x.a_hg, x.HQg, ga, He) == 0 &&
+          pg::make_map_i8_s(&x.s_hg, x.HSg, ga, lds_e) == 0;
+    std::vector<CUtensorMap> h((size_t)nl * E * 4);
+    std::vector<const unsigned char *> gu(E), dn(E);
+    for (int l = 0; l < nl && *ok; l++) {
+        const LayerW &L = p->layers[l];
+        CK(cudaMemcpy(gu.data(), L.gu_bases, (size_t)E * sizeof(void *), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(dn.data(), L.dn_bases, (size_t)E * sizeof(void *), cudaMemcpyDeviceToHost));
+        for (int e = 0; e < E && *ok; e++) {
+            TileMat tg = L.xgu, td = L.xdn;
+            tg.base = gu[e];
+            td.base = dn[e];
+            CUtensorMap *m = &h[((size_t)l * E + e) * 4];
+            *ok = i8_b_maps(p, m, m + 1, tg) && i8_b_maps(p, m + 2, m + 3, td);
+        }
+    }
+    if (!*ok) return B200_OK;
+    CUtensorMap *maps = nullptr;
+    if ((rc = dalloc(p, &maps, h.size() * sizeof(CUtensorMap)))) return rc;
+    CK(cudaMemcpy(maps, h.data(), h.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
+    x.maps = maps;
+    return B200_OK;
 }
 
 // Built on the first b200_set_prefill_mode(TENSOR_CORE_EXACT): the chunk buffers and tensor maps over the plan's own Q8_0 streams,
@@ -2176,15 +2240,15 @@ int prefill_init_i8(b200_plan *p) {
     for (const LayerW &L : p->layers)
         for (const TileMat *t : {&L.tqkv, &L.two, &L.tgu, &L.tw2})
             if (t->fmt && tile_bytes(q8_geometry(*t)) > kq8_bytes) kq8_bytes = tile_bytes(q8_geometry(*t));
-    const int bpad = (p->prefill_batch + pg::BM - 1) / pg::BM * pg::BM, big = g.dim > p->qd ? g.dim : p->qd;
-    const int lds_big = pg::i8_lds(big), lds_h = pg::i8_lds(g.hidden_dim);
+    const int bpad = (p->prefill_batch + pg::BM - 1) / pg::BM * pg::BM, big = g.dim > p->qd ? g.dim : p->qd, hid = i8_hidden(p);
+    const int lds_big = pg::i8_lds(big), lds_h = pg::i8_lds(hid);
     int att_tokens = bpad;
     if (p->att_scratch) {
         const size_t row = (size_t)p->nh_l * g.context_length * 4;
         att_tokens = I8_ATT_SCRATCH_MAX / row < 1 ? 1 : (int)(I8_ATT_SCRATCH_MAX / row < (size_t)bpad ? I8_ATT_SCRATCH_MAX / row : bpad);
     }
     const size_t sizes[7] = {(size_t)bpad * g.dim * 4, (size_t)bpad * nqkv * 4, (size_t)bpad * big, (size_t)bpad * lds_big * 4,
-                             (size_t)bpad * g.hidden_dim, (size_t)bpad * lds_h * 4, (size_t)bpad * sizeof(ChunkTok)};
+                             (size_t)bpad * hid, (size_t)bpad * lds_h * 4, (size_t)bpad * sizeof(ChunkTok)};
     const size_t att_bytes = p->att_scratch ? (size_t)att_tokens * p->nh_l * g.context_length * 4 : 0;
     int rc;
     if (kq8_bytes && !c.kq8) {
@@ -2212,14 +2276,20 @@ int prefill_init_i8(b200_plan *p) {
         if ((rc = dalloc(p, &c.kq8, (size_t)kq8_bytes))) return rc;
         c.kq8_bytes = kq8_bytes;
     }
-    const bool ok = pg::make_map_i8_a(&c.a_dim, c.XQ, c.bpad, g.dim) == 0 && pg::make_map_i8_s(&c.s_dim, c.XS, c.bpad, pg::i8_lds(g.dim)) == 0 &&
-                    pg::make_map_i8_a(&c.a_qd, c.XQ, c.bpad, p->qd) == 0 && pg::make_map_i8_s(&c.s_qd, c.XS, c.bpad, pg::i8_lds(p->qd)) == 0 &&
-                    pg::make_map_i8_a(&c.a_h, c.HQ, c.bpad, g.hidden_dim) == 0 && pg::make_map_i8_s(&c.s_h, c.HS, c.bpad, pg::i8_lds(g.hidden_dim)) == 0;
-    return prefill_built(p, B200_PREFILL_TENSOR_CORE_EXACT, ok && i8_weight_maps(p));
+    bool ok = pg::make_map_i8_a(&c.a_dim, c.XQ, c.bpad, g.dim) == 0 && pg::make_map_i8_s(&c.s_dim, c.XS, c.bpad, pg::i8_lds(g.dim)) == 0 &&
+              pg::make_map_i8_a(&c.a_qd, c.XQ, c.bpad, p->qd) == 0 && pg::make_map_i8_s(&c.s_qd, c.XS, c.bpad, pg::i8_lds(p->qd)) == 0 &&
+              (!hid || (pg::make_map_i8_a(&c.a_h, c.HQ, c.bpad, hid) == 0 && pg::make_map_i8_s(&c.s_h, c.HS, c.bpad, lds_h) == 0));
+    if (p->is_moe) {
+        bool xp_ok = false;
+        if ((rc = prefill_init_xp(p, &xp_ok))) return rc;
+        ok = ok && xp_ok;
+    }
+    return prefill_built(p, p->is_moe ? B200_PREFILL_TENSOR_CORE_EXACT_MOE : B200_PREFILL_TENSOR_CORE_EXACT, ok && i8_weight_maps(p));
 }
 
-// k_i8_norm over chunk rows [0, n) of c.X into XQ / XS; embed (layer 0): each row's embedding is gathered into c.X first.
-void i8_norm(b200_plan *p, int n, bool embed, const float *w) {
+// k_i8_norm over chunk rows [0, n) of c.X into XQ / XS (and the float rows into xb, if given); embed (layer 0): each row's
+// embedding is gathered into c.X first.
+void i8_norm(b200_plan *p, int n, bool embed, const float *w, float *xb = nullptr) {
     PrefillI8Ctx &c = p->pi8;
     const b200_config &g = p->cfg;
     const size_t norm_smem = norm_smem_bytes(g.dim);
@@ -2227,8 +2297,44 @@ void i8_norm(b200_plan *p, int n, bool embed, const float *w) {
     const TraceBuf tr{nullptr, 0, 0};
     TpCtx solo{};
     solo.n = 1;
-    if (embed) k_i8_norm<true><<<n, NORM_THREADS, norm_smem, p->stream>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
-    else k_i8_norm<false><<<n, NORM_THREADS, norm_smem, p->stream>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, tr, solo);
+    if (embed) k_i8_norm<true><<<n, NORM_THREADS, norm_smem, p->stream>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, xb, tr, solo);
+    else k_i8_norm<false><<<n, NORM_THREADS, norm_smem, p->stream>>>(c.X, c.tok, p->emb, p->mup.embedding_scale, w, g.rms_norm_eps, g.dim, c.XQ, c.XS, lds_d, xb, tr, solo);
+}
+
+// The routed experts of MoE layer l over the chunk's n rows (tensor_core_exact_moe), after the FFN norm (XQ / XS and the float rows
+// xp.XB) and, on Qwen2-MoE, the shared expert's down projection into xp.Ys: the chunk router, the grouping of the n * k
+// assignments by expert, the gather of each assignment's activation row, the grouped gate/up and down GEMMs, and the ordered
+// combine into c.X.  Six launches.
+int enqueue_chunk_moe(b200_plan *p, int l, int n, int *nl) {
+    PrefillI8Ctx &c = p->pi8;
+    XpCtx &x = c.xp;
+    const b200_config &g = p->cfg;
+    const LayerW &L = p->layers[l];
+    cudaStream_t s = p->stream;
+    const int E = p->moe.n_experts, k = p->moe.n_experts_used, He = p->moe.expert_hidden_dim, nw = p->moe_nw, na = n * k;
+    int *ids = x.ids + (size_t)l * c.bpad * k;
+    float *w = x.w + (size_t)l * c.bpad * nw;
+    XpRouteArgs ra{L.router, L.shared_gate, x.XB, ids, w, n, g.dim, E, k, nw};
+    const unsigned rg = (unsigned)((n + XP_ROUTE_TOKENS - 1) / XP_ROUTE_TOKENS);
+    if (p->moe_shared) k_xp_route<true><<<rg, MOE_ROUTE_THREADS, 0, s>>>(ra);
+    else k_xp_route<false><<<rg, MOE_ROUTE_THREADS, 0, s>>>(ra);
+    pg::k_xp_group<<<1, pg::XP_GROUP_THREADS, 0, s>>>(ids, na, E, x.row_of, x.offsets, x.tiles, x.n_tiles);
+    pg::k_xp_gather<<<na, 128, 0, s>>>(c.XQ, c.XS, g.dim, pg::i8_lds(g.dim), k, x.row_of, x.GQ, x.GS);
+    CK(cudaGetLastError());
+    const CUtensorMap *maps = x.maps + (size_t)l * E * 4;
+    const int gm = pg::xp_max_tiles(na, E);
+    pg::I8Out o{};
+    o.hq = x.HQg; o.hs = x.HSg; o.ldq = He; o.lds = pg::i8_lds(He); o.K = g.dim; o.seg = L.xgu.seg; o.oscale = 1.0f;
+    if (pg::xp_gemm_launch<pg::GEMM_GATEUP>(x.a_g, x.s_g, maps, x.tiles, x.n_tiles, o, gm, L.xgu.rows / pg::I8_BN, s))
+        return fail(p, B200_ERR_CUDA, "grouped expert gate/up GEMM launch failed");
+    o = pg::I8Out{};
+    o.C = x.Yg; o.ldc = g.dim; o.K = He; o.seg = L.xdn.seg; o.oscale = 1.0f;
+    if (pg::xp_gemm_launch<pg::GEMM_F32>(x.a_hg, x.s_hg, maps, x.tiles, x.n_tiles, o, gm, L.xdn.rows / pg::I8_BN, s))
+        return fail(p, B200_ERR_CUDA, "grouped expert down GEMM launch failed");
+    pg::k_xp_combine<<<n, 256, 0, s>>>(c.X, g.dim, x.Yg, x.row_of, w, k, nw, p->moe_shared ? x.Ys : nullptr);
+    CK(cudaGetLastError());
+    *nl += 6;
+    return B200_OK;
 }
 
 // The layers of one chunk over its n rows, whose ChunkTok entries (token, position, KV offset) are already in c.tok: the batched
@@ -2239,8 +2345,8 @@ int enqueue_chunk_i8(b200_plan *p, int n, bool own, int *nl_out) {
     PrefillI8Ctx &c = p->pi8;
     const b200_config &g = p->cfg;
     cudaStream_t s = p->stream;
-    const int nqkv = p->qd + 2 * p->kvd, mt = (n + pg::BM - 1) / pg::BM;
-    const int lds_q = pg::i8_lds(p->qd), lds_h = pg::i8_lds(g.hidden_dim);
+    const int nqkv = p->qd + 2 * p->kvd, mt = (n + pg::BM - 1) / pg::BM, hid = i8_hidden(p);
+    const int lds_q = pg::i8_lds(p->qd), lds_h = pg::i8_lds(hid);
     const size_t ctx_kv = (size_t)g.context_length * p->kvd;
     const size_t att_smem = att_smem_bytes(g.head_size, g.context_length, c.att != nullptr);
     const TraceBuf tr{nullptr, 0, 0};
@@ -2262,7 +2368,7 @@ int enqueue_chunk_i8(b200_plan *p, int n, bool own, int *nl_out) {
             nl++;
         }
         pg::I8Out o{};
-        o.C = C; o.ldc = ldc; o.hq = c.HQ; o.hs = c.HS; o.ldq = g.hidden_dim; o.lds = lds_h;
+        o.C = C; o.ldc = ldc; o.hq = c.HQ; o.hs = c.HS; o.ldq = hid; o.lds = lds_h;
         o.m_valid = n; o.K = Q.cols; o.seg = Q.seg; o.oscale = oscale;
         nl++;
         return pg::gemm_i8_launch<decltype(MODE)::value>(a, as, bq, bs, o, mt, Q.rows / pg::I8_BN, s) ? fail(p, B200_ERR_CUDA, "int8 GEMM launch failed") : B200_OK;
@@ -2288,6 +2394,16 @@ int enqueue_chunk_i8(b200_plan *p, int n, bool own, int *nl_out) {
         });
         if (rc) return rc;
         if ((rc = gemm(RESID(), c.a_qd, c.s_qd, m.wo_q, m.wo_s, L.two, c.X, g.dim, rs))) return rc;
+        if (p->is_moe) { // the MoE FFN over the chunk: the FFN norm with float rows for the router, then enqueue_chunk_moe
+            i8_norm(p, n, false, L.ffn_norm, c.xp.XB);
+            nl++;
+            if (p->moe_shared) { // the shared expert on the token rows: gate/up into HQ / HS, down into Ys
+                if ((rc = gemm(GATEUP(), c.a_dim, c.s_dim, m.gu_q, m.gu_s, L.sgu, nullptr, 0, 1.0f))) return rc;
+                if ((rc = gemm(F32(), c.a_h, c.s_h, m.w2_q, m.w2_s, L.sdn, c.xp.Ys, g.dim, 1.0f))) return rc;
+            }
+            if ((rc = enqueue_chunk_moe(p, l, n, &nl))) return rc;
+            continue;
+        }
         norm(false, L.ffn_norm);
         if ((rc = gemm(GATEUP(), c.a_dim, c.s_dim, m.gu_q, m.gu_s, L.tgu, nullptr, 0, 1.0f))) return rc;
         if ((rc = gemm(RESID(), c.a_h, c.s_h, m.w2_q, m.w2_s, L.tw2, c.X, g.dim, rs))) return rc;
@@ -2306,6 +2422,7 @@ int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own,
     cudaStream_t s = p->stream;
     const int n = (int)tab.size(), lds_d = pg::i8_lds(g.dim);
     CK(cudaMemcpyAsync(c.tok, tab.data(), (size_t)n * sizeof(ChunkTok), cudaMemcpyHostToDevice, s));
+    if (p->is_moe) c.xp.rows = n;
     CK(cudaEventRecord(p->ev0, s));
     int nl = 0, rc;
     if ((rc = enqueue_chunk_i8(p, n, own, &nl))) return rc;
@@ -2339,13 +2456,13 @@ int prefill_forward_i8(b200_plan *p, const std::vector<ChunkTok> &tab, bool own,
     return B200_OK;
 }
 
-const char *const PREFILL_MODE_NAMES[4] = {"exact", "tensor_core", "tensor_core_w8a16", "tensor_core_exact"};
+const char *const PREFILL_MODE_NAMES[5] = {"exact", "tensor_core", "tensor_core_w8a16", "tensor_core_exact", "tensor_core_exact_moe"};
 
 // The chunk path the plan's prefill mode runs: the bit-exact int8 one (prefill_i8.cuh), the f16 / W8A16 one (prefill.cuh), or
 // none (the exact token-by-token and multi-position paths).
 enum ChunkPath { CHUNK_NONE, CHUNK_TC, CHUNK_I8 };
 ChunkPath chunk_path(const b200_plan *p) {
-    constexpr ChunkPath PATHS[4] = {CHUNK_NONE, CHUNK_TC, CHUNK_TC, CHUNK_I8};
+    constexpr ChunkPath PATHS[5] = {CHUNK_NONE, CHUNK_TC, CHUNK_TC, CHUNK_I8, CHUNK_I8};
     return PATHS[p->pf_mode];
 }
 
@@ -3020,8 +3137,8 @@ int b200_score_tokens(b200_plan *p, const int32_t *tokens, const int32_t *target
         return fail(p, B200_ERR_UNSUPPORTED, "full logits are not gathered under tensor parallelism: scoring runs on single-GPU plans");
     const ChunkPath path = chunk_path(p);
     if (path == CHUNK_TC)
-        return fail(p, B200_ERR_UNSUPPORTED, "the %s prefill keeps f16 activations, so its logits are not the reference's: score in the exact or "
-                    "tensor_core_exact prefill mode", PREFILL_MODE_NAMES[p->pf_mode]);
+        return fail(p, B200_ERR_UNSUPPORTED, "the %s prefill keeps f16 activations, so its logits are not the reference's: score in the exact, "
+                    "tensor_core_exact or tensor_core_exact_moe prefill mode", PREFILL_MODE_NAMES[p->pf_mode]);
     int rc;
     if ((rc = check_chunk(p, tokens, n, start_pos))) return rc;
     for (int i = 0; i < n; i++)
@@ -3114,7 +3231,7 @@ int b200_trace_persistent(b200_plan *p, int32_t token, int32_t position, uint64_
 }
 
 int b200_set_prefill_mode(b200_plan *p, int32_t mode) {
-    if (!p || mode < B200_PREFILL_EXACT || mode > B200_PREFILL_TENSOR_CORE_EXACT) return B200_ERR_BAD_ARG;
+    if (!p || mode < B200_PREFILL_EXACT || mode > B200_PREFILL_TENSOR_CORE_EXACT_MOE) return B200_ERR_BAD_ARG;
     const b200_plan::PrefillMode &m = p->pf[mode];
     if (!m.ready) { // refused before anything is allocated, else built (each init leaves the mode ready or says why not)
         if (const char *why = prefill_why(p, mode)) return fail(p, B200_ERR_UNSUPPORTED, "%s", why);
@@ -3497,6 +3614,15 @@ int b200_read_buffer(b200_plan *p, const char *name, int32_t layer, void *dst, s
         const size_t k = (size_t)p->moe.n_experts_used;
         if (s == "moe_ids") { src = p->moe_ids; sz = (size_t)c.n_layers * k * 4; }
         else { src = p->moe_w; sz = (size_t)c.n_layers * p->moe_nw * 4; }
+    }
+    else if (s == "moe_chunk_ids" || s == "moe_chunk_weights") { // the last tensor_core_exact_moe chunk's routing of layer `layer`
+        if (!p->is_moe || !p->pi8.xp.maps)
+            return fail(p, B200_ERR_STATE, "%s: the plan has no tensor_core_exact_moe buffers (b200_set_prefill_mode)", name);
+        if (layer < 0 || layer >= c.n_layers) return fail(p, B200_ERR_BAD_ARG, "layer out of range");
+        const XpCtx &x = p->pi8.xp;
+        const size_t k = (size_t)p->moe.n_experts_used, rows = (size_t)x.rows, bpad = (size_t)p->pi8.bpad;
+        if (s == "moe_chunk_ids") { src = x.ids + (size_t)layer * bpad * k; sz = rows * k * 4; }
+        else { src = x.w + (size_t)layer * bpad * p->moe_nw; sz = rows * p->moe_nw * 4; }
     }
     else if (s == "key_cache" || s == "value_cache") {
         if (layer < 0 || layer >= c.n_layers) return fail(p, B200_ERR_BAD_ARG, "layer out of range");
@@ -4058,6 +4184,84 @@ int b200_test_gemm_i8(int32_t mode, int32_t m, int32_t n, int32_t k, const int8_
             o.C = dc; o.ldc = n; o.hq = dhq; o.hs = dhs; o.ldq = n; o.lds = n / 32;
             o.m_valid = m; o.K = k; o.seg = seg; o.oscale = oscale;
             const int lr = with_gemm_mode(mode, [&](auto MODE) { return pg::gemm_i8_launch<MODE>(ma, ms, mq, mqs, o, mpad / pg::BM, rows / pg::I8_BN, 0); });
+            if (lr == -6) s.rc = B200_ERR_BAD_ARG;
+            else if (lr) s.rc = B200_ERR_CUDA;
+        }
+        if (s.ok(cudaDeviceSynchronize()) && s.rc == B200_OK) {
+            if (gateup) s.ok(cudaMemcpy(hq, dhq, (size_t)m * n, cudaMemcpyDeviceToHost)) && s.ok(cudaMemcpy(hs, dhs, (size_t)m * (n / 32) * 4, cudaMemcpyDeviceToHost));
+            else s.ok(cudaMemcpy(c, dc, (size_t)m * n * 4, cudaMemcpyDeviceToHost));
+        }
+    }
+    return s.rc;
+}
+
+int b200_test_gemm_i8_experts(int32_t mode, int32_t n_experts, const int32_t *counts, int32_t n, int32_t k, const int8_t *aq, const float *as,
+                              const void *bq, const void *bq2, float *c, int8_t *hq, float *hs) {
+    const bool gateup = mode == pg::GEMM_GATEUP;
+    if ((mode != pg::GEMM_F32 && !gateup) || n_experts < 1 || n_experts > MOE_MAX_EXPERTS || !counts || !bq || n < 1 || k < 1 || k % 32) return B200_ERR_BAD_ARG;
+    if (gateup ? (!bq2 || n % 32) : n % pg::I8_BN) return B200_ERR_BAD_ARG;
+    const int E = n_experts;
+    std::vector<int> off(E + 1, 0);
+    for (int e = 0; e < E; e++) {
+        if (counts[e] < 0) return B200_ERR_BAD_ARG;
+        off[e + 1] = off[e] + counts[e];
+    }
+    const int m = off[E];
+    if (m && (!aq || !as || (gateup ? !hq || !hs : !c))) return B200_ERR_BAD_ARG;
+    const int nseg = smv_pick_nseg(k);
+    if (!nseg || (k / nseg) % pg::BK) return B200_ERR_BAD_ARG;
+    if (!m) return B200_OK;
+    const int seg = k / nseg, unit = smv_unit_bytes(seg), rows = gateup ? 2 * n : n, ga = m + pg::BM; // a tile of the last rows reads up to BM past them
+    const int lds = pg::i8_lds(k), nb = k / 32;
+    const size_t q8_bytes = (size_t)n * nb * 34, stream_bytes = (size_t)rows * nseg * unit;
+    std::vector<pg::XpTile> tiles(pg::xp_max_tiles(m, E));
+    const int nt = pg::xp_tile_table(counts, off.data(), E, tiles.data());
+    int8_t *daq = nullptr, *dhq = nullptr;
+    float *das = nullptr, *dc = nullptr, *dhs = nullptr;
+    unsigned char *draw = nullptr, *dstream = nullptr;
+    CUtensorMap *dmaps = nullptr;
+    pg::XpTile *dtiles = nullptr;
+    int *dnt = nullptr;
+    Scratch s;
+    // rows m .. ga - 1 of A hold large quants and scales: a tile row past its expert's rows is computed but must never be stored
+    if (s.alloc(&daq, (size_t)ga * k) && s.alloc(&das, (size_t)ga * lds * 4) && s.alloc(&draw, q8_bytes * (gateup ? 2 : 1)) &&
+        s.alloc(&dstream, stream_bytes * E) && s.alloc(&dmaps, (size_t)E * 4 * sizeof(CUtensorMap)) && s.alloc(&dtiles, tiles.size() * sizeof(pg::XpTile)) &&
+        s.alloc(&dnt, 4) && s.ok(cudaMemset(daq, 0x7F, (size_t)ga * k)) && s.ok(cudaMemset(das, 0x7F, (size_t)ga * lds * 4)) &&
+        s.ok(cudaMemcpy(daq, aq, (size_t)m * k, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy2D(das, (size_t)lds * 4, as, (size_t)nb * 4, (size_t)nb * 4, m, cudaMemcpyHostToDevice)) &&
+        s.ok(cudaMemcpy(dtiles, tiles.data(), tiles.size() * sizeof(pg::XpTile), cudaMemcpyHostToDevice)) && s.ok(cudaMemcpy(dnt, &nt, 4, cudaMemcpyHostToDevice)) &&
+        (gateup ? s.alloc(&dhq, (size_t)m * n) && s.alloc(&dhs, (size_t)m * (n / 32) * 4) && s.ok(cudaMemcpy(dhq, hq, (size_t)m * n, cudaMemcpyHostToDevice)) &&
+                      s.ok(cudaMemcpy(dhs, hs, (size_t)m * (n / 32) * 4, cudaMemcpyHostToDevice))
+                : s.alloc(&dc, (size_t)m * n * 4) && s.ok(cudaMemcpy(dc, c, (size_t)m * n * 4, cudaMemcpyHostToDevice)))) {
+        // each expert's stream as the upload repacks it, and its quant / scale maps (entries 0 / 1 for GATEUP, 2 / 3 for STORE)
+        std::vector<CUtensorMap> h((size_t)E * 4);
+        for (int e = 0; e < E && s.rc == B200_OK; e++) {
+            const unsigned char *src0 = static_cast<const unsigned char *>(bq) + (size_t)e * q8_bytes;
+            if (!s.ok(cudaMemcpy(draw, src0, q8_bytes, cudaMemcpyHostToDevice)) ||
+                (gateup && !s.ok(cudaMemcpy(draw + q8_bytes, static_cast<const unsigned char *>(bq2) + (size_t)e * q8_bytes, q8_bytes, cudaMemcpyHostToDevice))))
+                break;
+            RepackSrc src{};
+            src.raw[0] = draw;
+            src.rows[0] = n;
+            if (gateup) { src.raw[1] = draw + q8_bytes; src.rows[1] = n; }
+            src.gateup = gateup ? 1 : 0;
+            unsigned char *dst = dstream + (size_t)e * stream_bytes;
+            k_repack_tiles<<<(unsigned)((size_t)rows * nseg), 128>>>(src, dst, rows, k, seg, nseg, unit);
+            if (!s.ok(cudaGetLastError()) || !s.ok(cudaDeviceSynchronize())) break; // draw is reused by the next expert
+            CUtensorMap *mm = &h[(size_t)e * 4 + (gateup ? 0 : 2)];
+            if (pg::make_map_i8_q8(mm, dst, (uint64_t)rows, nseg, unit, 0) || pg::make_map_i8_q8(mm + 1, dst, (uint64_t)rows, nseg, unit, 1)) s.rc = B200_ERR_CUDA;
+        }
+        CUtensorMap ma, ms;
+        if (s.rc == B200_OK && (pg::make_map_i8_a(&ma, daq, (uint64_t)ga, (uint64_t)k) || pg::make_map_i8_s(&ms, das, (uint64_t)ga, (uint64_t)lds)))
+            s.rc = B200_ERR_CUDA;
+        if (s.rc == B200_OK) s.ok(cudaMemcpy(dmaps, h.data(), h.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
+        if (s.rc == B200_OK) {
+            pg::I8Out o{};
+            o.C = dc; o.ldc = n; o.hq = dhq; o.hs = dhs; o.ldq = n; o.lds = n / 32;
+            o.K = k; o.seg = seg; o.oscale = 1.0f;
+            const int gm = pg::xp_max_tiles(m, E), nn = rows / pg::I8_BN;
+            const int lr = gateup ? pg::xp_gemm_launch<pg::GEMM_GATEUP>(ma, ms, dmaps, dtiles, dnt, o, gm, nn, 0)
+                                  : pg::xp_gemm_launch<pg::GEMM_F32>(ma, ms, dmaps, dtiles, dnt, o, gm, nn, 0);
             if (lr == -6) s.rc = B200_ERR_BAD_ARG;
             else if (lr) s.rc = B200_ERR_CUDA;
         }

@@ -25,10 +25,15 @@
 // (rmsnorm_quant_row, one CTA per token), k_i8_rope_kv (rope_kv_prologue, grid heads x tokens) and k_i8_attention
 // (attention_head<HS, true>, grid heads x tokens, after every K / V row of the chunk is in the cache).
 //
+// MoE plans (B200_PREFILL_TENSOR_CORE_EXACT_MOE) run the same attention half; their FFN half groups the chunk's (token, expert)
+// assignments by expert (k_xp_group, k_xp_gather) and runs gemm_i8_body over every expert's rows as one grouped launch per
+// projection (k_xp_gemm), then adds the results in the decode's order (k_xp_combine).  The chunk router is in moe.cuh (k_xp_route).
+//
 // On a plan that keeps K-quant weights resident, each resident matrix is first expanded to the Q8_0 tiles a Q8_0-tile plan of the
 // same file holds (k_kq_tiles_to_q8, stream_matvec.cuh) in one scratch the size of the largest, and its GEMM reads them there.
 #pragma once
 #include "decode_kernels.cuh"
+#include "moe.cuh"
 #include "prefill.cuh"
 #include "stream_matvec.cuh"
 
@@ -54,7 +59,7 @@ struct I8Out {
     int8_t *hq;  // GATEUP: quantised hidden rows [rows][ldq] and their block scales [rows][lds]
     float *hs;
     int ldq, lds;
-    int m_valid; // rows >= m_valid are never written
+    int m_valid; // k_gemm_i8: rows >= m_valid are never written (the grouped kernel k_xp_gemm takes its bound from its tile table)
     int K, seg;  // K: a multiple of seg; seg: the stream's segment width, a multiple of 64
     float oscale;
 };
@@ -94,10 +99,12 @@ __device__ __forceinline__ void i8_fence_regs(int (&d)[32]) {
 // subtraction of 1.5 * 2^23 is exact (isum = 0 gives +0, as (float)0 does)
 __device__ __forceinline__ float i8_to_float(int isum) { return __fsub_rn(__int_as_float(isum + 0x4B400000), 12582912.0f); }
 
-// The GEMM of both kernels below: k_gemm_i8 (the prefill's epilogues) and k_gemm_i8_logits (I8_LOGITS).
+// The GEMM of the kernels below: k_gemm_i8 (the prefill's epilogues), k_gemm_i8_logits (I8_LOGITS) and k_xp_gemm (the grouped
+// expert GEMMs): the 128-row tile from A row m0, rows >= m_valid never written.  A consumer warp group whose 64 rows all lie at or
+// past m_valid computes nothing: it only releases each stage once it has landed (so its arrival counts for that stage's lap).
 template <int MODE>
 __device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUtensorMap &tma_as, const CUtensorMap &tma_bq, const CUtensorMap &tma_bs,
-                                             const I8Out &o) {
+                                             const I8Out &o, int m0, int m_valid) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     float *hbuf = reinterpret_cast<float *>(smem + I8_STAGES * I8_STAGE_BYTES);
@@ -110,7 +117,7 @@ __device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUt
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    const int nk = o.K / BK, m0 = blockIdx.x * BM, g0 = blockIdx.y * (I8_BN / 4);
+    const int nk = o.K / BK, g0 = blockIdx.y * (I8_BN / 4);
 
     if (wg == 0) {
         if (warp == 0 && lane == 0) {
@@ -131,6 +138,15 @@ __device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUt
 
     // ===== consumers: warp group c = wg - 1 owns tile rows 64c .. 64c+63 =====
     const int c = wg - 1, t = threadIdx.x & 127;
+    if (m0 + c * 64 >= m_valid) {
+        for (int kb = 0; kb < nk; kb++) {
+            const int st = kb % I8_STAGES;
+            mbar_wait(full0 + 8 * st, (kb / I8_STAGES) & 1);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty0 + 8 * st);
+        }
+        return;
+    }
     const int r_lo = c * 64 + (t >> 5) * 16 + ((t & 31) >> 2); // tile row of d[4j], d[4j+1]; d[4j+2], d[4j+3] are row r_lo + 8
     const int cq = 2 * (t & 3);
     float acc[32];
@@ -200,7 +216,7 @@ __device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUt
         asm volatile("bar.sync %0, 128;" ::"r"(2 + c) : "memory");
         for (int r = (t >> 5); r < 64; r += 4) {
             const int row = m0 + c * 64 + r;
-            if (row >= o.m_valid) break; // warp-uniform
+            if (row >= m_valid) break; // warp-uniform
             float as;
             const int q = quant_block_lane(hb[r * 32 + lane], as);
             o.hq[(size_t)row * o.ldq + blockIdx.y * 32 + lane] = (int8_t)q;
@@ -210,7 +226,7 @@ __device__ __forceinline__ void gemm_i8_body(const CUtensorMap &tma_a, const CUt
 #pragma unroll
         for (int h = 0; h < 2; h++) {
             const int row = m0 + r_lo + 8 * h;
-            if (row < o.m_valid) {
+            if (row < m_valid) {
                 float *dst = o.C + (size_t)row * o.ldc + n0 + cq;
 #pragma unroll
                 for (int jj = 0; jj < 8; jj++)
@@ -230,18 +246,130 @@ template <int MODE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_i8(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_as,
                                                           const __grid_constant__ CUtensorMap tma_bq, const __grid_constant__ CUtensorMap tma_bs,
                                                           const I8Out o) {
-    gemm_i8_body<MODE>(tma_a, tma_as, tma_bq, tma_bs, o);
+    gemm_i8_body<MODE>(tma_a, tma_as, tma_bq, tma_bs, o, blockIdx.x * BM, o.m_valid);
 }
 
 __global__ void __launch_bounds__(GEMM_THREADS, 1) k_gemm_i8_logits(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_as,
                                                                  const __grid_constant__ CUtensorMap tma_bq, const __grid_constant__ CUtensorMap tma_bs,
                                                                  const I8Out o) {
-    gemm_i8_body<I8_LOGITS>(tma_a, tma_as, tma_bq, tma_bs, o);
+    gemm_i8_body<I8_LOGITS>(tma_a, tma_as, tma_bq, tma_bs, o, blockIdx.x * BM, o.m_valid);
 }
 
 template <int MODE> constexpr auto gemm_i8_kernel() {
     if constexpr (MODE == I8_LOGITS) return k_gemm_i8_logits;
     else return k_gemm_i8<MODE>;
+}
+
+
+// ---- the grouped expert GEMMs of B200_PREFILL_TENSOR_CORE_EXACT_MOE ----------------------------------------------------------
+// The chunk's n * k (token, slot) assignments, grouped by expert (k_xp_group), form the rows of one A operand: expert e's rows are
+// [offset[e], offset[e] + count[e]), in token order.  Each expert's rows are cut into 128-row M tiles; one tile table entry per tile.
+struct XpTile {
+    int expert, row0, rows, pad;
+};
+// Upper bound of the tile table: every expert's last tile may be partial.
+__host__ __device__ inline int xp_max_tiles(int assignments, int n_experts) {
+    return (assignments + BM - 1) / BM + (n_experts < assignments ? n_experts : assignments);
+}
+// The tile table of per-expert row counts and offsets, experts in index order; returns its length.  k_xp_group and the test hook
+// build it with this one function.
+__host__ __device__ inline int xp_tile_table(const int *count, const int *offset, int E, XpTile *tiles) {
+    int nt = 0;
+    for (int e = 0; e < E; e++)
+        for (int r = 0; r < count[e]; r += BM) tiles[nt++] = XpTile{e, offset[e] + r, count[e] - r < BM ? count[e] - r : BM, 0};
+    return nt;
+}
+
+// The grouped kernel: blockIdx.x indexes the tile table (CTAs past its length return before any barrier), blockIdx.y the 64-column
+// N tile.  maps: the layer's per-expert tensor maps [expert][4] = gate/up quants, gate/up scales, down quants, down scales, written
+// by the host before the first launch; GATEUP reads entries 0 / 1, STORE entries 2 / 3.
+template <int MODE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) k_xp_gemm(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_as,
+                                                          const CUtensorMap *__restrict__ maps, const XpTile *__restrict__ tiles,
+                                                          const int *__restrict__ n_tiles, const I8Out o) {
+    if ((int)blockIdx.x >= *n_tiles) return;
+    const XpTile tl = tiles[blockIdx.x];
+    const CUtensorMap *m = maps + 4 * tl.expert + (MODE == GEMM_GATEUP ? 0 : 2);
+    if (threadIdx.x == 0) // the maps live in global memory: acquire them for the tensor-map proxy before the producer's first copy
+        asm volatile("fence.proxy.tensormap::generic.acquire.sys [%0], 128;\n\tfence.proxy.tensormap::generic.acquire.sys [%1], 128;" ::"l"(m), "l"(m + 1)
+                     : "memory");
+    gemm_i8_body<MODE>(tma_a, tma_as, m[0], m[1], o, tl.row0, tl.row0 + tl.rows);
+}
+
+// grid_m = xp_max_tiles(...) M slots, n_tiles N tiles.  -6: a shape the kernel does not take.
+template <int MODE>
+inline int xp_gemm_launch(const CUtensorMap &a, const CUtensorMap &as, const CUtensorMap *maps, const XpTile *tiles, const int *n_tiles, const I8Out &o,
+                          int grid_m, int n_tiles_n, cudaStream_t stream) {
+    static bool attr = false; // one flag per instantiation
+    if (!attr) {
+        if (cudaFuncSetAttribute(k_xp_gemm<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)i8_smem_bytes()) != cudaSuccess) return -4;
+        attr = true;
+    }
+    if (o.seg <= 0 || o.seg % BK || o.K <= 0 || o.K % o.seg || grid_m < 1 || n_tiles_n < 1) return -6;
+    k_xp_gemm<MODE><<<dim3(grid_m, n_tiles_n), GEMM_THREADS, i8_smem_bytes(), stream>>>(a, as, maps, tiles, n_tiles, o);
+    return cudaGetLastError() == cudaSuccess ? 0 : -5;
+}
+
+// Deterministic, stable counting sort of the na = n * k assignments (ids [n][k], assignment a = t * k + j) by expert, on one CTA:
+// XP_SLICES slices of the assignments, one thread per (slice, expert) counting, then placing its slice's assignments in order.
+// row_of[a]: the assignment's grouped row; offsets[e] (e <= E): first grouped row of expert e; tiles / *n_tiles: the tile table.
+constexpr int XP_GROUP_THREADS = 1024, XP_SLICES = XP_GROUP_THREADS / MOE_MAX_EXPERTS;
+__global__ void __launch_bounds__(XP_GROUP_THREADS, 1) k_xp_group(const int *__restrict__ ids, int na, int E, int *__restrict__ row_of,
+                                                                  int *__restrict__ offsets, XpTile *__restrict__ tiles, int *__restrict__ n_tiles) {
+    __shared__ int cnt[XP_SLICES][MOE_MAX_EXPERTS], base[XP_SLICES][MOE_MAX_EXPERTS], tot[MOE_MAX_EXPERTS], off[MOE_MAX_EXPERTS + 1];
+    const int e = threadIdx.x % MOE_MAX_EXPERTS, s = threadIdx.x / MOE_MAX_EXPERTS;
+    const int a0 = (int)((long long)na * s / XP_SLICES), a1 = (int)((long long)na * (s + 1) / XP_SLICES);
+    int c = 0;
+    if (e < E)
+        for (int i = a0; i < a1; i++) c += ids[i] == e;
+    cnt[s][e] = c;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int o = 0;
+        for (int x = 0; x < E; x++) {
+            off[x] = o;
+            for (int q = 0; q < XP_SLICES; q++) { base[q][x] = o; o += cnt[q][x]; }
+            tot[x] = o - off[x];
+        }
+        off[E] = o;
+        *n_tiles = xp_tile_table(tot, off, E, tiles);
+    }
+    __syncthreads();
+    if (e < E) {
+        int r = base[s][e];
+        for (int i = a0; i < a1; i++)
+            if (ids[i] == e) row_of[i] = r++;
+    }
+    if ((int)threadIdx.x <= E) offsets[threadIdx.x] = off[threadIdx.x];
+}
+
+// One CTA per assignment: token t's int8 row (dim bytes) and its block scales (lds floats) into grouped row row_of[a].
+__global__ void __launch_bounds__(128) k_xp_gather(const int8_t *__restrict__ xq, const float *__restrict__ xs, int dim, int lds, int k,
+                                                   const int *__restrict__ row_of, int8_t *__restrict__ gq, float *__restrict__ gs) {
+    const int a = blockIdx.x, t = a / k, r = row_of[a];
+    const int4 *src = reinterpret_cast<const int4 *>(xq + (size_t)t * dim);
+    int4 *dst = reinterpret_cast<int4 *>(gq + (size_t)r * dim);
+    for (int i = threadIdx.x; i < dim / 16; i += blockDim.x) dst[i] = src[i];
+    for (int i = threadIdx.x; i < lds; i += blockDim.x) gs[(size_t)r * lds + i] = xs[(size_t)t * lds + i];
+}
+
+// The ordered combine, one CTA per chunk row (moe_down's epilogue order): x = fl(fl(w_j * Yg[row(t, j)]) + x) for j in selection
+// order, then with a shared expert x = fl(fl(w_shared * Ys[t]) + x).
+__global__ void __launch_bounds__(256) k_xp_combine(float *__restrict__ x, int dim, const float *__restrict__ yg, const int *__restrict__ row_of,
+                                                    const float *__restrict__ w, int k, int nw, const float *__restrict__ ys) {
+    __shared__ int rows[MOE_MAX_K];
+    __shared__ float ws[MOE_MAX_K + 1];
+    const int t = blockIdx.x;
+    if ((int)threadIdx.x < k) rows[threadIdx.x] = row_of[(size_t)t * k + threadIdx.x];
+    if ((int)threadIdx.x < nw) ws[threadIdx.x] = w[(size_t)t * nw + threadIdx.x];
+    __syncthreads();
+    float *xr = x + (size_t)t * dim;
+    for (int i = threadIdx.x; i < dim; i += blockDim.x) {
+        float v = xr[i];
+        for (int j = 0; j < k; j++) v = __fadd_rn(__fmul_rn(ws[j], yg[(size_t)rows[j] * dim + i]), v);
+        if (ys) v = __fadd_rn(__fmul_rn(ws[k], ys[(size_t)t * dim + i]), v);
+        xr[i] = v;
+    }
 }
 
 // ---- host side ----
@@ -300,9 +428,24 @@ struct ChunkTok {
     long long kv;
 };
 
+// B200_PREFILL_TENSOR_CORE_EXACT_MOE (MoE plans, built with the chunk buffers): the FFN norm's float rows XB (the router's input), the
+// chunk routing of every layer (ids [layer][bpad][k], w [layer][bpad][nw]), the grouping (row_of, offsets, the tile table), the
+// grouped A rows GQ / GS and hidden rows HQg / HSg (n * k + 128 rows: a tile may read past its expert's rows), the grouped down
+// outputs Yg [n * k][dim], the shared expert's down outputs Ys [bpad][dim] (Qwen2-MoE) and the per-expert tensor maps.
+struct XpCtx {
+    float *XB = nullptr, *w = nullptr, *GS = nullptr, *HSg = nullptr, *Yg = nullptr, *Ys = nullptr;
+    int *ids = nullptr, *row_of = nullptr, *offsets = nullptr, *n_tiles = nullptr;
+    int8_t *GQ = nullptr, *HQg = nullptr;
+    pg::XpTile *tiles = nullptr;
+    CUtensorMap *maps = nullptr;      // device [layer][expert][4]: make_map_i8_q8 quant / scale maps of gate/up, then of down
+    CUtensorMap a_g, s_g, a_hg, s_hg; // A operands of the grouped gate/up (K = dim) and down (K = expert hidden) GEMMs
+    int rows = 0;                     // rows of the last chunk (b200_read_buffer "moe_chunk_ids" / "moe_chunk_weights")
+};
+
 // The mode's chunk buffers for bpad rows (built on the first b200_set_prefill_mode(TENSOR_CORE_EXACT)): X and QKV as the batched
 // step keeps them per row; XQ / XS the int8 activations of the QKV, gate/up (row stride dim) and Wo (row stride q width) GEMMs, HQ /
-// HS those of W2; the token table; score rows for ATT_TOKENS tokens at a time when the context needs global score rows.
+// HS those of W2 (MoE: of the shared expert's down projection, K = shared hidden); the token table; score rows for ATT_TOKENS tokens
+// at a time when the context needs global score rows.
 struct PrefillI8Ctx {
     int bpad = 0, att_tokens = 0;
     float *X = nullptr, *QKV = nullptr, *XS = nullptr, *HS = nullptr, *att = nullptr;
@@ -312,7 +455,9 @@ struct PrefillI8Ctx {
     int64_t kq8_bytes = 0;                          // its size (b200_score_tokens grows it to the classifier's tiles)
     CUtensorMap a_dim, s_dim, a_qd, s_qd, a_h, s_h; // A operands: K = dim (XQ), K = q width (XQ), K = hidden (HQ)
     std::vector<PrefillQ8Maps> maps;                // per layer: make_map_i8_q8 quant / scale maps of the four streams (over kq8
-                                                    // for a resident stream)
+                                                    // for a resident stream); MoE layers: the shared expert's gate/up
+                                                    // and down (Qwen2-MoE) in the gate/up and W2 slots, or none
+    XpCtx xp;
 };
 // Global score rows of one attention launch are bounded by this many bytes (att_tokens = max(1, bound / (heads x context x 4))).
 constexpr size_t I8_ATT_SCRATCH_MAX = (size_t)64 << 20;
@@ -320,10 +465,10 @@ constexpr size_t I8_ATT_SCRATCH_MAX = (size_t)64 << 20;
 template <bool EMBED>
 __global__ void __launch_bounds__(NORM_THREADS, 1) k_i8_norm(float *__restrict__ x, const ChunkTok *__restrict__ tok, DevMat emb, float emb_scale,
                                                          const float *__restrict__ w, float eps, int dim, int8_t *__restrict__ xq,
-                                                         float *__restrict__ xs, int lds, TraceBuf tr, TpCtx tp) {
+                                                         float *__restrict__ xs, int lds, float *__restrict__ xb, TraceBuf tr, TpCtx tp) {
     const int v = blockIdx.x;
-    rmsnorm_quant_row<EMBED>(x + (size_t)v * dim, &tok[v].token, emb, emb_scale, w, eps, dim, xq + (size_t)v * dim, xs + (size_t)v * lds, nullptr,
-                             nullptr, tr, tp, -1);
+    rmsnorm_quant_row<EMBED>(x + (size_t)v * dim, &tok[v].token, emb, emb_scale, w, eps, dim, xq + (size_t)v * dim, xs + (size_t)v * lds,
+                             xb ? xb + (size_t)v * dim : nullptr, nullptr, tr, tp, -1);
 }
 
 template <int HS>

@@ -345,6 +345,8 @@ public final class B200MasterPlan implements AutoCloseable {
     }
 
     public static final int PREFILL_EXACT = 0, PREFILL_TENSOR_CORE = 1, PREFILL_TENSOR_CORE_W8A16 = 2, PREFILL_TENSOR_CORE_EXACT = 3;
+    /** PREFILL_TENSOR_CORE_EXACT for Qwen2-MoE / Qwen3-MoE plans: the chunk routed on the device, grouped int8 expert GEMMs, KV cache bit-identical to PREFILL_EXACT. */
+    public static final int PREFILL_TENSOR_CORE_EXACT_MOE = 4;
     // b200_config.arch (include/b200llama.h): Qwen2 / Qwen2.5 / DeepSeek-R1-Distill-Qwen pass blk.N.attn_{q,k,v}.bias (F32) with the weights
     public static final int ARCH_LLAMA = 0, ARCH_QWEN3 = 1, ARCH_PHI3 = 2, ARCH_QWEN2 = 3, ARCH_QWEN2_MOE = 4, ARCH_GRANITE = 5, ARCH_DEVSTRAL = 6,
             ARCH_QWEN3_MOE = 7;

@@ -88,7 +88,7 @@ class Tensor(C.Structure):
 
 EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite", "b200_plan_create_devstral", "b200_forward_decode", "b200_forward_prefill", "b200_forward_batch_prefill", "b200_score_tokens", "b200_set_logprobs", "b200_read_logprobs", "b200_test_logprobs", "b200_set_sampling_controls", "b200_set_sample_history", "b200_read_sample_counts", "b200_test_sample_controls", "b200_time_sample_controls", "b200_set_prefill_mode", "b200_prefill_info",
            "b200_set_decode_mode", "b200_decode_info", "b200_trace_persistent", "b200_test_seqsum2", "b200_profile_seqsum2", "b200_test_sample", "b200_forward_decode_sample", "b200_upload_info", "b200_requant_kquant", "b200_test_kq_tiles_to_q8",
-           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
+           "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_gemm_i8_experts", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
            "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_forward_chunk", "b200_chunk_rows", "b200_weight_info", "b200_test_set_memory_budget", "b200_stream_rings",
            "b200_test_stream", "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
@@ -141,6 +141,7 @@ def lib() -> C.CDLL:
     L.b200_test_gemm.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.b200_test_gemm_q8.argtypes = [i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]
     L.b200_test_gemm_i8.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, C.c_float, vp, vp, vp]
+    L.b200_test_gemm_i8_experts.argtypes = [i32, i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     L.b200_time_kernel.argtypes = [vp, i32, i32, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
     L.b200_read_buffer.argtypes = [vp, C.c_char_p, i32, vp, C.c_size_t]
     L.b200_set_decode_slots.argtypes = [vp, i32]
@@ -402,6 +403,41 @@ def test_gemm_i8(mode: str, aq, a_scales, bq, c=None, bq2=None, oscale: float = 
     return c
 
 
+def test_gemm_i8_experts(mode: str, counts, aq, a_scales, bq, bq2=None, c=None, hq=None, hs=None):
+    """One launch of the grouped expert GEMM of B200_PREFILL_TENSOR_CORE_EXACT_MOE (csrc/prefill_i8.cuh) as the prefill issues it.
+    counts: grouped rows per expert (M = their sum, expert after expert); aq int8 [M,K], a_scales float32 [M, K/32]; bq (and bq2, the
+    up projections, for "gateup") every expert's GGUF Q8_0 blocks uint8 [E, N, K/32*34].  "f32": returns c float32 [M,N] (initial
+    contents c, default zeros).  "gateup": N hidden units; returns (hq int8 [M,N], hs float32 [M, N/32]) from the given initial
+    contents."""
+    counts = np.ascontiguousarray(counts, dtype=np.int32)
+    aq = np.ascontiguousarray(aq, dtype=np.int8)
+    a_scales = np.ascontiguousarray(a_scales, dtype=np.float32)
+    bq = np.ascontiguousarray(bq, dtype=np.uint8)
+    m, k = aq.shape
+    e, n = bq.shape[:2]
+    if counts.shape != (e,) or int(counts.sum()) != m or a_scales.shape != (m, k // 32) or bq.shape != (e, n, k // 32 * 34) or k % 32:
+        raise ValueError("shapes do not match")
+    if mode == "gateup":
+        bq2 = np.ascontiguousarray(bq2, dtype=np.uint8)
+        hq = np.array(np.zeros((m, n), np.int8) if hq is None else hq, dtype=np.int8, order="C", copy=True)
+        hs = np.array(np.zeros((m, n // 32), np.float32) if hs is None else hs, dtype=np.float32, order="C", copy=True)
+        if bq2.shape != bq.shape or hq.shape != (m, n) or hs.shape != (m, n // 32):
+            raise ValueError("shapes do not match")
+        rc = lib().b200_test_gemm_i8_experts(GEMM_MODES[mode], e, counts.ctypes.data, n, k, aq.ctypes.data, a_scales.ctypes.data, bq.ctypes.data,
+                                             bq2.ctypes.data, None, hq.ctypes.data, hs.ctypes.data)
+        if rc != B200_OK:
+            _raise(rc, "b200_test_gemm_i8_experts failed")
+        return hq, hs
+    c = np.array(np.zeros((m, n), np.float32) if c is None else c, dtype=np.float32, order="C", copy=True)
+    if c.shape != (m, n):
+        raise ValueError("shapes do not match")
+    rc = lib().b200_test_gemm_i8_experts(GEMM_MODES[mode], e, counts.ctypes.data, n, k, aq.ctypes.data, a_scales.ctypes.data, bq.ctypes.data, None,
+                                         c.ctypes.data, None, None)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_gemm_i8_experts failed")
+    return c
+
+
 STREAM_MODES = {"store": 0, "resid": 1, "gateup": 2}
 STREAM_INFO = ("stages", "grid", "max_groups", "min_groups", "smem")
 
@@ -593,6 +629,7 @@ class NativePlan:
     def forward_batch_prefill(self, tokens, start_pos: int):
         t = np.ascontiguousarray(tokens, dtype=np.int32)
         self._ck(lib().b200_forward_batch_prefill(self._p, t.ctypes.data, len(t), start_pos))
+        self._chunk_rows = len(t)
 
     def score_tokens(self, tokens, start_pos: int, targets=None):
         """b200_score_tokens: run tokens[i] at start_pos + i (K/V into the plan's cache) and score each row.  targets[i] is the token
@@ -606,6 +643,7 @@ class NativePlan:
         lp = np.empty(n, dtype=np.float64)
         ids = np.empty(n, dtype=np.int32)
         self._ck(lib().b200_score_tokens(self._p, t.ctypes.data, tg.ctypes.data, n, start_pos, lp.ctypes.data, ids.ctypes.data))
+        self._chunk_rows = n
         return lp, ids
 
     MAX_TOP_LOGPROBS = 20  # B200_MAX_TOP_LOGPROBS
@@ -784,6 +822,18 @@ class NativePlan:
         nw = k + 1 if self.moe.shared_hidden_dim else k
         ids = self.read_buffer("moe_ids", self.cfg.n_layers * k, np.int32).reshape(self.cfg.n_layers, k)
         w = self.read_buffer("moe_weights", self.cfg.n_layers * nw).reshape(self.cfg.n_layers, nw)
+        return ids, w
+
+    def moe_chunk_routing(self, rows: int | None = None):
+        """(ids int32 [layer, rows, k], weights float32 [layer, rows, k + 1]) of the last tensor_core_exact_moe chunk: every row's
+        selected experts in selection order, their routing weights, then the shared-expert weight (Qwen3-MoE: [layer, rows, k]).
+        rows defaults to the length of the last forward_batch_prefill / score_tokens call."""
+        rows = getattr(self, "_chunk_rows", 0) if rows is None else rows
+        k = self.moe.n_experts_used
+        nw = k + 1 if self.moe.shared_hidden_dim else k
+        L = self.cfg.n_layers
+        ids = np.stack([self.read_buffer("moe_chunk_ids", rows * k, np.int32, layer=l).reshape(rows, k) for l in range(L)])
+        w = np.stack([self.read_buffer("moe_chunk_weights", rows * nw, layer=l).reshape(rows, nw) for l in range(L)])
         return ids, w
 
     def upload_info(self) -> dict:

@@ -151,6 +151,7 @@ class B200MasterPlan:
 
     # TensorCoreSupport.java's switch between the MMA and the plain batch-prefill layer families
     PREFILL_EXACT, PREFILL_TENSOR_CORE, PREFILL_TENSOR_CORE_W8A16, PREFILL_TENSOR_CORE_EXACT = 0, 1, 2, 3
+    PREFILL_TENSOR_CORE_EXACT_MOE = 4
 
     def set_sampling_controls(self, slot: int, controls, owner=None):
         """Sampling controls (sampler.SamplingControls, or None to turn them off) for one sequence: a decode slot, or -1 for the plan's
@@ -191,9 +192,13 @@ class B200MasterPlan:
         KV cache bit-identical to "exact").  On a plan that keeps K-quant weights resident (weight_info()["resident"]) only
         "exact" and "tensor_core_exact" are available: the latter expands each resident matrix to its Q8_0 tiles on the device
         just before its GEMM, in one scratch the size of the largest resident matrix's Q8_0 tiles, and raises B200Error
-        (B200_ERR_OOM) naming the bytes when that scratch and the chunk buffers do not fit the free memory."""
+        (B200_ERR_OOM) naming the bytes when that scratch and the chunk buffers do not fit the free memory.
+        "tensor_core_exact_moe" is "tensor_core_exact" for Qwen2-MoE / Qwen3-MoE plans (which refuse the other tensor-core modes;
+        dense plans refuse this one): the chunk's rows are routed on the device, each expert's rows run as one grouped int8 GEMM, and
+        the results are combined in the decode's order, so the KV cache is bit-identical to "exact" and score_tokens' results are
+        exact mode's; moe_chunk_routing() returns each row's routing of the last chunk."""
         if isinstance(mode, str):
-            mode = {"exact": 0, "tensor_core": 1, "tensor_core_w8a16": 2, "tensor_core_exact": 3}[mode]
+            mode = {"exact": 0, "tensor_core": 1, "tensor_core_w8a16": 2, "tensor_core_exact": 3, "tensor_core_exact_moe": 4}[mode]
         self._native.set_prefill_mode(int(mode))
 
     def prefill_info(self):
@@ -285,6 +290,11 @@ class B200MasterPlan:
         """MoE plans: (ids [layer, k], weights [layer, k + 1]) of the last step (selected experts in selection order, their
         routing weights, then the shared-expert weight); Qwen3-MoE has no shared expert, its weights are [layer, k]."""
         return self._native.moe_routing()
+
+    def moe_chunk_routing(self, rows=None):
+        """MoE plans after a tensor_core_exact_moe chunk: (ids [layer, rows, k], weights [layer, rows, k + 1]) of every row of the
+        last chunk, as moe_routing() reports one step's (Qwen3-MoE: weights [layer, rows, k]); rows defaults to the last chunk's."""
+        return self._native.moe_chunk_routing(rows)
 
     def kv_reset(self):
         self._native.kv_reset()

@@ -252,11 +252,27 @@ int b200_forward_batch_prefill(b200_plan *plan, const int32_t *tokens, int32_t n
  *                            force) on FP16, tensor-parallel and Qwen2-MoE plans, plans created without a prefill batch size,
  *                            and plans whose dim, q or q+k+v widths or Q8_0 stream segments are not multiples of 64 columns.
  *                            Applies to b200_forward_batch_prefill and b200_prefill_slots (a resident plan has no decode
- *                            slots: its prompts go to the plan's own cache). */
+ *                            slots: its prompts go to the plan's own cache).
+ *   B200_PREFILL_TENSOR_CORE_EXACT_MOE  B200_PREFILL_TENSOR_CORE_EXACT for Qwen2-MoE / Qwen3-MoE plans (K-quant files included: their
+ *                            experts are Q8_0 tiles), whose tensor_core_exact stays refused.  Per layer the attention half is
+ *                            tensor_core_exact's; the FFN half routes every row of the chunk on the device (each router logit one
+ *                            float dot product in index order, then the decode routers' own softmax / top-k / renormalisation /
+ *                            shared-gate tail), sorts the n * k assignments by expert (stable: token order within each expert),
+ *                            gathers each assignment's int8 row, runs every expert's rows as one grouped int8 gate/up and one
+ *                            grouped down GEMM (the int8 GEMM's block order and epilogues, B read from that expert's tile-major
+ *                            Q8_0 stream in place), the shared expert's GEMMs on the token rows (Qwen2-MoE), and adds the results
+ *                            in the decode's order: x = fl(fl(w_j * y_j) + x) for j in selection order, the shared expert last.
+ *                            KV cache bit-identical to B200_PREFILL_EXACT; b200_score_tokens' results bit-identical to exact
+ *                            mode's; the decode routing buffers (b200_read_buffer "moe_ids") are left as they were.  Needs
+ *                            prefill_batch_size > 1, dim, q width and q+k+v width multiples of 64 and every Q8_0 stream segment
+ *                            (attention, every expert's gate/up and down, the shared expert's) a multiple of 64 columns.  The first
+ *                            call allocates the chunk buffers and encodes 4 tensor maps per expert per layer into device memory.
+ *                            Dense plans refuse it with B200_ERR_UNSUPPORTED (their mode is B200_PREFILL_TENSOR_CORE_EXACT). */
 #define B200_PREFILL_EXACT 0
 #define B200_PREFILL_TENSOR_CORE 1
 #define B200_PREFILL_TENSOR_CORE_W8A16 2
 #define B200_PREFILL_TENSOR_CORE_EXACT 3
+#define B200_PREFILL_TENSOR_CORE_EXACT_MOE 4
 int b200_set_prefill_mode(b200_plan *plan, int32_t mode);
 
 /* Active mode, kernels launched and device milliseconds of the last tensor-core chunk (any pointer may be NULL). */
@@ -534,6 +550,8 @@ int b200_batch_info(b200_plan *plan, int32_t *n_slots, int32_t *launches_per_ste
  * expert's units, then each routed slot's, shared_hidden_dim + n_experts_used * expert_hidden_dim units), "moe_ids" (int32 [layer][k], the experts the last step selected, in
  * selection order) and "moe_weights" (f32 [layer][k + 1], their routing weights, then the shared-expert weight).  Qwen3-MoE plans: the
  * same without the shared expert: n_experts_used * expert_hidden_dim units, and "moe_weights" is f32 [layer][k], the renormalised weights.
+ * "moe_chunk_ids" (int32 [rows][k]) and "moe_chunk_weights" (f32 [rows][k], + 1 with a shared expert) of layer `layer`: the routing of
+ * every row of the last B200_PREFILL_TENSOR_CORE_EXACT_MOE chunk (B200_ERR_STATE before the mode's buffers exist).
  * "rope_cr" / "rope_ci": the RoPE table every decode and prefill kernel reads (f32 [context_length][head_size / 2]).
  * Copies min(bytes, buffer size). */
 int b200_read_buffer(b200_plan *plan, const char *name, int32_t layer, void *dst, size_t bytes);
@@ -646,6 +664,16 @@ int b200_test_gemm_q8(int32_t mode, int32_t stages, int32_t splits, int32_t m, i
  * Q8_0 quantisation of swiglu(gate, up), in/out.  K whose stream segment is not a multiple of 64 columns: B200_ERR_BAD_ARG. */
 int b200_test_gemm_i8(int32_t mode, int32_t m, int32_t n, int32_t k, const int8_t *aq, const float *as, const void *bq, const void *bq2, float oscale,
                       float *c, int8_t *hq, float *hs);
+
+/* Test hook: ONE launch of the grouped expert GEMM of B200_PREFILL_TENSOR_CORE_EXACT_MOE exactly as the prefill launches it.
+ * n_experts experts; counts[e] >= 0 grouped rows of expert e, expert after expert (m = sum of counts).  aq: int8 [m][k]; as: f32
+ * [m][k / 32]; bq (and bq2 = the up projections for GATEUP): each expert's GGUF Q8_0 blocks, [n_experts][n][k / 32 * 34], repacked
+ * into one tile-major stream per expert by the plan's upload kernel, with one tensor map pair per expert in device memory; the
+ * tile table is the one the prefill's grouping kernel writes for these counts.  mode 0 (STORE): c = f32 [m][n] out, n a multiple
+ * of 64; 2 (GATEUP): n hidden units (a multiple of 32), hq = int8 [m][n], hs = f32 [m][n / 32] in/out.  B200_ERR_BAD_ARG for any
+ * other mode, a negative count, more than 256 experts, or K whose stream segment is not a multiple of 64 columns. */
+int b200_test_gemm_i8_experts(int32_t mode, int32_t n_experts, const int32_t *counts, int32_t n, int32_t k, const int8_t *aq, const float *as,
+                              const void *bq, const void *bq2, float *c, int8_t *hq, float *hs);
 
 /* One decode weight stream launched on its own (b200_test_stream).  Arrays are indexed [launch][row][...]; V = max(nrow, 1). */
 typedef struct b200_stream_test {

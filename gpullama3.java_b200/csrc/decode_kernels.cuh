@@ -188,6 +188,16 @@ __device__ __forceinline__ float swiglu(float g, float u) {
     return __fmul_rn(s, u);
 }
 
+// Test hook: the two exp expressions of the bit-exact paths (the softmaxes and routers, swiglu's denominator) on the n float bit
+// patterns first, first + 1, ...
+__global__ void __launch_bounds__(256) k_test_exp(unsigned first, unsigned n, float *__restrict__ e, float *__restrict__ e1) {
+    for (unsigned i = blockIdx.x * 256u + threadIdx.x; i < n; i += gridDim.x * 256u) {
+        const double d = exp((double)__uint_as_float(first + i));
+        e[i] = (float)d;
+        e1[i] = (float)(1.0 + d);
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // FP16 dequant-matvec, bit-exact with FP16FloatTensor.vectorDot (FP16FloatTensor.java:62-110)
 // for an L-lane species: L independent strided FMA chains (fused, as FloatVector.fma), then

@@ -543,8 +543,9 @@ __device__ __noinline__ void pd_load_act(const int8_t *q, const float *s, int co
 }
 
 // ---- one attention head with the consumer warps: k_attention's body (exact CPU order, InferenceCore.java:98-137) -------------
-// h = local head index on this rank.
-template <int HS>
+// h = local head index on this rank.  TEST = 1: the instantiation k_test_pd_attention calls -- a function with a second caller would be
+// optimised for both, so k_decode_persistent keeps an instantiation of its own.
+template <int HS, int TEST = 0>
 __device__ __noinline__ void pd_attention_head(const PdArgs &a, const PdLayer &Ly, int h, int pos, unsigned char *smem, const PdSmem &L, int tid, int layer) {
     float *sm = reinterpret_cast<float *>(smem + L.off_nbuf);
     float *misc = reinterpret_cast<float *>(smem + L.off_misc);
@@ -729,6 +730,22 @@ __device__ __noinline__ void pd_attention_head(const PdArgs &a, const PdLayer &L
         }
     }
     pd_stamp(a, layer, 15, tid);
+}
+
+// Test hook (b200_test_attention): pd_attention_head<HS> for head blockIdx.x at position pos, in a CTA of k_decode_persistent's shape
+// whose producer warp leaves at once, with this position's rope row staged at off_rope as k_decode_persistent stages it.
+template <int HS>
+__global__ void __launch_bounds__(PD_THREADS, 1) k_test_pd_attention(const __grid_constant__ PdArgs a, const __grid_constant__ PdSmem L,
+                                                                     const __grid_constant__ PdLayer Ly, int pos) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const int tid = threadIdx.x;
+    if (tid >= PD_CT) return;
+    if (tid < HS) {
+        float *srope = reinterpret_cast<float *>(smem + L.off_rope);
+        srope[tid] = tid < HS / 2 ? __ldg(a.rope_cr + (size_t)pos * (HS / 2) + tid) : __ldg(a.rope_ci + (size_t)pos * (HS / 2) + (tid - HS / 2));
+    }
+    pd_bar_sync();
+    pd_attention_head<HS, 1>(a, Ly, blockIdx.x, pos, smem, L, tid, 0);
 }
 
 // ---- the kernel -----------------------------------------------------------------------------------------------------------

@@ -4540,6 +4540,192 @@ int b200_test_stream(b200_stream_test *t) {
     return s.rc;
 }
 
+} // extern "C"
+
+namespace {
+// What b200_test_attention launches, decided from its arguments alone.
+struct AttTest {
+    int qd = 0, kvd = 0, nqkv = 0, grid_y = 0, launches = 0;
+    bool global = false;   // score rows in a global scratch (the plan's rule: 3 * head size + context > ATT_SMEM_FLOATS_MAX)
+    size_t smem = 0;       // dynamic shared memory of the attention launch
+    size_t scratch = 0;    // floats of that scratch, as the plan sizes it for the form
+    PdSmem L{};            // persistent form: the offsets pd_attention_head uses
+};
+
+int att_test_plan(const b200_attention_test &t, AttTest &c) {
+    const int f = t.form, hs = t.head_size;
+    if (f < B200_ATT_SINGLE || f > B200_ATT_PERSISTENT) return B200_ERR_BAD_ARG;
+    const bool pers = f == B200_ATT_PERSISTENT;
+    if (pers ? hs != 64 && hs != 128 : hs != 32 && hs != 64 && hs != 96 && hs != 128 && hs != 256) return B200_ERR_BAD_ARG;
+    if (t.n_heads < 1 || t.n_kv_heads < 1 || t.n_heads % t.n_kv_heads || t.ctx < 1 || t.slots < 1) return B200_ERR_BAD_ARG;
+    if (t.arch & ~(KF_NEOX | KF_QKNORM | KF_QKVBIAS | KF_ATTSCALE)) return B200_ERR_BAD_ARG;
+    const int max_rows = f == B200_ATT_BATCH || f == B200_ATT_CACHED_ROWS ? SMB_MAX_ROWS : f == B200_ATT_CHUNK ? 1 << 20 : 1;
+    if (t.rows < 1 || t.rows > max_rows) return B200_ERR_BAD_ARG;
+    if (f == B200_ATT_CHUNK ? t.att_tokens < 1 || t.att_tokens > t.rows : t.att_tokens != 0) return B200_ERR_BAD_ARG;
+    if (!t.slot || !t.pos || !t.qkv || !t.k_cache || !t.v_cache || !t.rope_cr || !t.rope_ci || !t.qkv_out || !t.k_out || !t.v_out || !t.xq ||
+        !t.xs || ((t.arch & KF_QKNORM) && (!t.q_norm || !t.k_norm)) || ((t.arch & KF_QKVBIAS) && !t.qkv_bias))
+        return B200_ERR_BAD_ARG;
+    for (int r = 0; r < t.rows; r++) {
+        if (t.slot[r] < 0 || t.slot[r] >= t.slots || t.pos[r] < 0 || t.pos[r] >= t.ctx) return B200_ERR_BAD_ARG;
+        for (int q = 0; q < r; q++) // a batch row writes its K / V inside its attention CTAs: one slot per row; no two rows write one cache row
+            if (t.slot[q] == t.slot[r] && (f == B200_ATT_BATCH || t.pos[q] == t.pos[r])) return B200_ERR_BAD_ARG;
+    }
+    c.qd = t.n_heads * hs; c.kvd = t.n_kv_heads * hs; c.nqkv = c.qd + 2 * c.kvd;
+    c.global = 3 * hs + t.ctx > ATT_SMEM_FLOATS_MAX;
+    const int ctx_pad = (t.ctx + PD_CT - 1) / PD_CT * PD_CT; // the plan's scratch rows are padded for the persistent kernel
+    c.grid_y = f == B200_ATT_CHUNK ? t.att_tokens : f == B200_ATT_BATCH || f == B200_ATT_CACHED_ROWS ? t.rows : 1;
+    c.launches = f == B200_ATT_CHUNK ? (t.rows + t.att_tokens - 1) / t.att_tokens : 1;
+    if (pers) {
+        c.L = pd_layout(c.qd, c.qd, c.qd, hs, 3 * hs + (c.global ? 0 : ctx_pad), 32, 0); // no ring: the offsets before it
+        c.smem = c.L.total;
+        c.scratch = c.global ? (size_t)t.n_heads * ctx_pad : 0;
+    } else {
+        c.smem = att_smem_bytes(hs, t.ctx, c.global);
+        c.scratch = !c.global ? 0 : f == B200_ATT_SINGLE ? (size_t)t.n_heads * ctx_pad : (size_t)c.grid_y * t.n_heads * t.ctx;
+    }
+    return B200_OK;
+}
+} // namespace
+
+extern "C" {
+
+int b200_test_attention(b200_attention_test *t) {
+    if (!t) return B200_ERR_BAD_ARG;
+    AttTest c;
+    int rc = att_test_plan(*t, c);
+    if (rc) return rc;
+    const int64_t info[5] = {t->n_heads, c.grid_y, (int64_t)c.smem, c.global ? 1 : 0, c.launches};
+    for (int k = 0; k < 5; k++) t->info[k] = info[k];
+    if (t->dry) return B200_OK;
+    int dev = 0, optin = 0;
+    Scratch s;
+    if (!s.ok(cudaGetDevice(&dev)) || !s.ok(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev))) return s.rc;
+    if (c.smem > (size_t)optin) return B200_ERR_BAD_ARG;
+
+    const int R = t->rows, hs = t->head_size, nh = t->n_heads, nkv = t->n_kv_heads, f = t->form;
+    const size_t slot_stride = (size_t)t->ctx * c.kvd, cache = (size_t)t->slots * slot_stride, rope = (size_t)t->ctx * (hs / 2);
+    const int lds = pg::i8_lds(c.qd); // the chunk form's block-scale row stride (the plan's XS rows)
+    const size_t xs_rows = f == B200_ATT_CHUNK ? (size_t)lds : (size_t)c.qd / 32;
+    // Every output sits between GUARD bytes of 0xA5 that no store may reach; outputs start as 0xFF bytes (xs, xb: NaN).
+    const size_t GUARD = 256;
+    std::vector<std::pair<unsigned char *, size_t>> guarded;
+    auto buf = [&](auto **p, size_t bytes, const void *init) {
+        unsigned char *d = nullptr;
+        if (!s.alloc(&d, bytes + 2 * GUARD) || !s.ok(cudaMemset(d, 0xA5, bytes + 2 * GUARD)) ||
+            !s.ok(init ? cudaMemcpy(d + GUARD, init, bytes, cudaMemcpyHostToDevice) : cudaMemset(d + GUARD, 0xFF, bytes)))
+            return false;
+        guarded.push_back({d, bytes});
+        *p = reinterpret_cast<std::remove_pointer_t<decltype(p)>>(d + GUARD);
+        return true;
+    };
+    float *dqkv = nullptr, *dk = nullptr, *dv = nullptr, *dxs = nullptr, *dxb = nullptr, *dcr = nullptr, *dci = nullptr, *dqn = nullptr, *dkn = nullptr;
+    float *dbias = nullptr, *datt = nullptr;
+    int8_t *dxq = nullptr;
+    StepState *dst = nullptr;
+    BatchRows *drows = nullptr;
+    ChunkTok *dtok = nullptr;
+    if (!buf(&dqkv, (size_t)R * c.nqkv * 4, t->qkv) || !buf(&dk, cache * 4, t->k_cache) || !buf(&dv, cache * 4, t->v_cache) ||
+        !buf(&dxq, (size_t)R * c.qd, nullptr) || !buf(&dxs, (size_t)R * xs_rows * 4, nullptr) || (t->xb && !buf(&dxb, (size_t)c.qd * 4, nullptr)))
+        return s.rc;
+    if (!s.alloc(&dcr, rope * 4) || !s.alloc(&dci, rope * 4) || !s.ok(cudaMemcpy(dcr, t->rope_cr, rope * 4, cudaMemcpyHostToDevice)) ||
+        !s.ok(cudaMemcpy(dci, t->rope_ci, rope * 4, cudaMemcpyHostToDevice)))
+        return s.rc;
+    if ((t->arch & KF_QKNORM) && (!s.alloc(&dqn, (size_t)hs * 4) || !s.alloc(&dkn, (size_t)hs * 4) ||
+                                  !s.ok(cudaMemcpy(dqn, t->q_norm, (size_t)hs * 4, cudaMemcpyHostToDevice)) ||
+                                  !s.ok(cudaMemcpy(dkn, t->k_norm, (size_t)hs * 4, cudaMemcpyHostToDevice))))
+        return s.rc;
+    if ((t->arch & KF_QKVBIAS) && (!s.alloc(&dbias, (size_t)c.nqkv * 4) || !s.ok(cudaMemcpy(dbias, t->qkv_bias, (size_t)c.nqkv * 4, cudaMemcpyHostToDevice))))
+        return s.rc;
+    if (c.scratch && (!s.alloc(&datt, c.scratch * 4) || !s.ok(cudaMemset(datt, 0xFF, c.scratch * 4)))) return s.rc;
+    if (f == B200_ATT_SINGLE || f == B200_ATT_PERSISTENT) {
+        const StepState st{0, t->pos[0], 0, 0, 0, {0, 0, 0}};
+        if (!s.alloc(&dst, sizeof st) || !s.ok(cudaMemcpy(dst, &st, sizeof st, cudaMemcpyHostToDevice))) return s.rc;
+    } else if (f == B200_ATT_CHUNK) {
+        std::vector<ChunkTok> tab(R);
+        for (int r = 0; r < R; r++) tab[r] = ChunkTok{0, t->pos[r], (long long)(t->slot[r] * slot_stride)};
+        if (!s.alloc(&dtok, (size_t)R * sizeof(ChunkTok)) || !s.ok(cudaMemcpy(dtok, tab.data(), (size_t)R * sizeof(ChunkTok), cudaMemcpyHostToDevice)))
+            return s.rc;
+    } else {
+        BatchRows br{};
+        for (int r = 0; r < R; r++) { br.pos[r] = t->pos[r]; br.slot[r] = t->slot[r]; }
+        if (!s.alloc(&drows, sizeof br) || !s.ok(cudaMemcpy(drows, &br, sizeof br, cudaMemcpyHostToDevice))) return s.rc;
+    }
+
+    const TraceBuf none{nullptr, 0, 0};
+    TpCtx solo{};
+    solo.n = 1;
+    const float eps = t->eps, sa = t->score_arg;
+    const int arch = t->arch, ctx = t->ctx;
+    if (f == B200_ATT_PERSISTENT) {
+        PdArgs a;
+        memset(&a, 0, sizeof a);
+        a.qd = c.qd; a.n_heads = nh; a.n_kv_heads = nkv; a.head_size = hs; a.arch = arch; a.ctx = ctx; a.eps = eps; a.sqrt_hs = sa;
+        a.rope_cr = dcr; a.rope_ci = dci; a.qkv = dqkv; a.attq = dxq; a.atts = dxs; a.att_scratch = datt; a.tp.n = 1;
+        PdLayer Ly;
+        memset(&Ly, 0, sizeof Ly);
+        Ly.q_norm = dqn; Ly.k_norm = dkn; Ly.qkv_bias = dbias;
+        Ly.kc = dk + (size_t)t->slot[0] * slot_stride; Ly.vc = dv + (size_t)t->slot[0] * slot_stride;
+        with_mma_head_size(nullptr, hs, [&](auto HS) {
+            if (s.ok(cudaFuncSetAttribute(k_test_pd_attention<HS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c.smem)))
+                k_test_pd_attention<HS><<<nh, PD_THREADS, c.smem>>>(a, c.L, Ly, t->pos[0]);
+            return B200_OK;
+        });
+    } else {
+        with_decode_head_size(nullptr, hs, [&](auto HS) { // the shared-memory attributes set_smem_attrs gives every plan, then the plan's launches
+            const size_t sm = c.smem;
+            if (f == B200_ATT_SINGLE) {
+                float *kc = dk + (size_t)t->slot[0] * slot_stride, *vc = dv + (size_t)t->slot[0] * slot_stride;
+                if (s.ok(set_max_dyn(k_attention<HS>, optin)))
+                    s.ok(launch_on(0, true, k_attention<HS>, dim3(nh), dim3(ATT_THREADS), sm, dqkv, kc, vc, (const StepState *)dst, (const float *)dcr,
+                                   (const float *)dci, nh, nkv, arch, (const float *)dqn, (const float *)dkn, (const float *)dbias, eps, sa, dxq, dxs, dxb,
+                                   none, solo, 0u, 0, datt, ctx));
+            } else if (f == B200_ATT_BATCH) {
+                if (s.ok(set_max_dyn(k_attention_batch<HS>, optin)))
+                    s.ok(launch_on(0, true, k_attention_batch<HS>, dim3(nh, R), dim3(ATT_THREADS), sm, dqkv, c.nqkv, dk, dv, slot_stride,
+                                   (const BatchRows *)drows, (const float *)dcr, (const float *)dci, nh, nkv, arch, (const float *)dqn, (const float *)dkn,
+                                   (const float *)dbias, eps, sa, dxq, dxs, datt, ctx, none, solo));
+            } else if (f == B200_ATT_CACHED_ROWS) {
+                if (s.ok(set_max_dyn(k_attention_cached_rows<HS>, optin)) &&
+                    s.ok(launch_on(0, true, k_rope_kv_batch<HS>, dim3(nh, R), dim3(2 * HS), (size_t)0, dqkv, c.nqkv, dk, dv, slot_stride,
+                                   (const BatchRows *)drows, (const float *)dcr, (const float *)dci, nh, nkv, arch, (const float *)dqn, (const float *)dkn,
+                                   (const float *)dbias, eps)))
+                    s.ok(launch_on(0, true, k_attention_cached_rows<HS>, dim3(nh, R), dim3(ATT_THREADS), sm, dqkv, c.nqkv, dk, dv, slot_stride,
+                                   (const BatchRows *)drows, nh, nkv, arch, sa, dxq, dxs, datt, ctx, none, solo));
+            } else if (s.ok(set_max_dyn(k_i8_attention<HS>, optin))) { // the chunk: enqueue_chunk_i8's two launches
+                k_i8_rope_kv<HS><<<dim3(nh, R), 2 * HS, 0>>>(dqkv, c.nqkv, dk, dv, dtok, dcr, dci, nh, nkv, arch, dqn, dkn, dbias, eps);
+                for (int v0 = 0; v0 < R; v0 += t->att_tokens)
+                    k_i8_attention<HS><<<dim3(nh, R - v0 < t->att_tokens ? R - v0 : t->att_tokens), ATT_THREADS, sm>>>(
+                        dqkv, c.nqkv, dk, dv, dtok, v0, nh, nkv, arch, sa, dxq, dxs, lds, datt, ctx, none, solo);
+            }
+            return B200_OK;
+        });
+    }
+    if (s.rc || !s.ok(cudaGetLastError()) || !s.ok(cudaDeviceSynchronize())) return s.rc;
+    if (!s.ok(cudaMemcpy(t->qkv_out, dqkv, (size_t)R * c.nqkv * 4, cudaMemcpyDeviceToHost)) || !s.ok(cudaMemcpy(t->k_out, dk, cache * 4, cudaMemcpyDeviceToHost)) ||
+        !s.ok(cudaMemcpy(t->v_out, dv, cache * 4, cudaMemcpyDeviceToHost)) || !s.ok(cudaMemcpy(t->xq, dxq, (size_t)R * c.qd, cudaMemcpyDeviceToHost)) ||
+        !s.ok(cudaMemcpy2D(t->xs, (size_t)c.qd / 32 * 4, dxs, xs_rows * 4, (size_t)c.qd / 32 * 4, R, cudaMemcpyDeviceToHost)) ||
+        (t->xb && !s.ok(cudaMemcpy(t->xb, dxb, (size_t)c.qd * 4, cudaMemcpyDeviceToHost))))
+        return s.rc;
+    std::vector<unsigned char> g(GUARD);
+    for (const auto &b : guarded)
+        for (size_t off : {(size_t)0, GUARD + b.second}) {
+            if (!s.ok(cudaMemcpy(g.data(), b.first + off, GUARD, cudaMemcpyDeviceToHost))) return s.rc;
+            for (unsigned char x : g)
+                if (x != 0xA5) return B200_ERR_STATE;
+        }
+    return B200_OK;
+}
+
+int b200_test_exp(uint32_t first, int64_t n, float *e, float *e1) {
+    if (!e || !e1 || n < 1 || n > ((int64_t)1 << 31) || (uint64_t)first + (uint64_t)n - 1 > 0xFFFFFFFFull) return B200_ERR_BAD_ARG;
+    Scratch s;
+    float *de = nullptr, *de1 = nullptr;
+    if (!s.alloc(&de, (size_t)n * 4) || !s.alloc(&de1, (size_t)n * 4)) return s.rc;
+    k_test_exp<<<(unsigned)std::min<int64_t>((n + 255) / 256, 65536), 256>>>(first, (unsigned)n, de, de1);
+    if (s.ok(cudaGetLastError()) && s.ok(cudaMemcpy(e, de, (size_t)n * 4, cudaMemcpyDeviceToHost))) s.ok(cudaMemcpy(e1, de1, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    return s.rc;
+}
+
 int b200_test_pf_attention_packed(int32_t n_seqs, const int32_t *lengths, const int32_t *start_positions, const float *q, const float *k, const float *v,
                                   int32_t n_heads, int32_t n_kv_heads, int32_t head_size, int32_t out_rows, uint16_t *out) {
     if (!lengths || !start_positions || !q || !k || !v || !out || n_seqs < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return B200_ERR_BAD_ARG;

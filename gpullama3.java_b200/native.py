@@ -81,6 +81,14 @@ class StreamTest(C.Structure):
                                           "x_out", "ids")] + [("info", C.c_int64 * 5)]
 
 
+class AttentionTest(C.Structure):
+    """b200_attention_test: the arguments and the reported configuration of b200_test_attention."""
+    _fields_ = [(n, C.c_int32) for n in ("form", "head_size", "n_heads", "n_kv_heads", "arch", "ctx", "rows", "slots", "att_tokens", "dry")] + \
+               [(n, C.c_float) for n in ("eps", "score_arg")] + \
+               [(n, C.c_void_p) for n in ("slot", "pos", "qkv", "k_cache", "v_cache", "rope_cr", "rope_ci", "q_norm", "k_norm", "qkv_bias", "qkv_out",
+                                          "k_out", "v_out", "xq", "xs", "xb")] + [("info", C.c_int64 * 5)]
+
+
 class Tensor(C.Structure):
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("ggml_type", C.c_int32), ("n_dims", C.c_int32),
                 ("dims", C.c_int64 * 4)]
@@ -91,7 +99,7 @@ EXPORTS = ["b200_plan_create", "b200_plan_create_moe", "b200_plan_create_granite
            "b200_decode_sequence", "b200_time_kernel", "b200_tp_handle", "b200_tp_attach", "b200_trace_decode", "b200_profile_norm", "b200_gemm_f16", "b200_test_gemm", "b200_test_gemm_q8", "b200_test_gemm_i8", "b200_test_gemm_i8_experts", "b200_kv_reset", "b200_read_buffer", "b200_launches_per_decode",
            "b200_set_decode_slots", "b200_forward_decode_batch", "b200_slot_reset", "b200_slot_copy_kv", "b200_prefill_slots", "b200_test_pf_attention_packed", "b200_batch_info",
            "b200_forward_decode_multi", "b200_decode_multi_rows", "b200_forward_step", "b200_forward_chunk", "b200_chunk_rows", "b200_weight_info", "b200_test_set_memory_budget", "b200_stream_rings",
-           "b200_test_stream", "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
+           "b200_test_stream", "b200_test_attention", "b200_test_exp", "b200_device_bytes", "b200_plan_free", "b200_last_error", "b200_version"]
 
 _lib = None
 
@@ -162,6 +170,8 @@ def lib() -> C.CDLL:
     L.b200_test_kq_tiles_to_q8.argtypes = [i32, i32, i32, vp, vp, C.c_int64]
     L.b200_stream_rings.argtypes = [C.POINTER(i32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     L.b200_test_stream.argtypes = [C.POINTER(StreamTest)]
+    L.b200_test_attention.argtypes = [C.POINTER(AttentionTest)]
+    L.b200_test_exp.argtypes = [C.c_uint32, C.c_int64, vp, vp]
     L.b200_launches_per_decode.argtypes = [vp]
     L.b200_device_bytes.argtypes = [vp]
     L.b200_device_bytes.restype = C.c_int64
@@ -492,6 +502,69 @@ def test_stream(form: int, mode: str, w, rows: int, cols: int, *, w_up=None, w_d
         _raise(rc, "b200_test_stream failed")
     res["info"] = dict(zip(STREAM_INFO, t.info))
     return res
+
+
+ATTENTION_FORMS = {"single": 0, "batch": 1, "cached_rows": 2, "chunk": 3, "persistent": 4}
+ATTENTION_INFO = ("grid_x", "grid_y", "smem", "global_scores", "launches")
+
+
+def test_attention(form: str, head_size: int, n_heads: int, n_kv_heads: int, ctx: int, slots, positions, qkv, k_cache, v_cache, rope_cr,
+                   rope_ci, *, arch: int = 0, eps: float = 1e-6, score_arg: float | None = None, q_norm=None, k_norm=None, qkv_bias=None,
+                   att_tokens: int = 0, want_xb: bool = False, n_slots: int | None = None, dry: bool = False) -> dict:
+    """b200_test_attention: one exact attention form launched as the plan launches it.  form: a key of ATTENTION_FORMS; row r is
+    (slots[r], positions[r]); qkv float32 [rows][q | k | v]; caches float32 [n_slots][ctx][kv width]; rope tables [ctx][head_size / 2].
+    score_arg: sqrt(head_size) by default (Granite: its attention multiplier with arch & 8).  Returns {"info": the configuration run, and
+    "qkv", "k_cache", "v_cache" after the launch, "xq" [rows][q width], "xs" [rows][q width / 32], "xb" (want_xb, single form)}.
+    dry: only the checks and "info" (n_slots then stands for the caches' first dimension)."""
+    slots = np.ascontiguousarray(slots, dtype=np.int32)
+    positions = np.ascontiguousarray(positions, dtype=np.int32)
+    keep = [slots, positions]
+
+    def arr(a):
+        if a is None:
+            return None
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        keep.append(a)
+        return a.ctypes.data
+
+    rows, qd = len(slots), n_heads * head_size
+    t = AttentionTest()
+    t.form, t.head_size, t.n_heads, t.n_kv_heads, t.arch, t.ctx = ATTENTION_FORMS[form], head_size, n_heads, n_kv_heads, arch, ctx
+    t.rows, t.att_tokens, t.dry, t.eps = rows, att_tokens, dry, eps
+    t.score_arg = float(np.sqrt(np.float64(head_size))) if score_arg is None else score_arg
+    t.slot, t.pos = slots.ctypes.data, positions.ctypes.data
+    t.qkv, t.rope_cr, t.rope_ci, t.q_norm, t.k_norm, t.qkv_bias = arr(qkv), arr(rope_cr), arr(rope_ci), arr(q_norm), arr(k_norm), arr(qkv_bias)
+    res = {}
+    if dry:  # the pointer checks of a real launch, without the buffers
+        t.slots = n_slots
+        t.qkv = t.k_cache = t.v_cache = t.rope_cr = t.rope_ci = t.qkv_out = t.k_out = t.v_out = t.xq = t.xs = 1
+        t.q_norm, t.k_norm, t.qkv_bias = t.q_norm or 1, t.k_norm or 1, t.qkv_bias or 1
+    else:
+        kc, vc = np.ascontiguousarray(k_cache, dtype=np.float32), np.ascontiguousarray(v_cache, dtype=np.float32)
+        keep += [kc, vc]
+        t.slots = kc.shape[0]
+        t.k_cache, t.v_cache = kc.ctypes.data, vc.ctypes.data
+        res["qkv"], res["k_cache"], res["v_cache"] = np.empty((rows, qkv.shape[-1]), np.float32), np.empty_like(kc), np.empty_like(vc)
+        res["xq"], res["xs"] = np.empty((rows, qd), np.int8), np.empty((rows, qd // 32), np.float32)
+        t.qkv_out, t.k_out, t.v_out = res["qkv"].ctypes.data, res["k_cache"].ctypes.data, res["v_cache"].ctypes.data
+        t.xq, t.xs = res["xq"].ctypes.data, res["xs"].ctypes.data
+        if want_xb:
+            res["xb"] = np.empty(qd, np.float32)
+            t.xb = res["xb"].ctypes.data
+    rc = lib().b200_test_attention(C.byref(t))
+    if rc != B200_OK:
+        _raise(rc, "b200_test_attention failed")
+    res["info"] = dict(zip(ATTENTION_INFO, t.info))
+    return res
+
+
+def test_exp(first: int, n: int):
+    """b200_test_exp: ((float)exp((double)x), (float)(1.0 + exp((double)x))) on the device for the n float bit patterns from `first`."""
+    e, e1 = np.empty(n, np.float32), np.empty(n, np.float32)
+    rc = lib().b200_test_exp(first, n, e.ctypes.data, e1.ctypes.data)
+    if rc != B200_OK:
+        _raise(rc, "b200_test_exp failed")
+    return e, e1
 
 
 def _pf_attention_packed(qs, ks, vs, starts, n_heads: int, n_kv_heads: int, out_rows: int | None, sentinel: int) -> np.ndarray:

@@ -722,6 +722,61 @@ typedef struct b200_stream_test {
  * reached the guard words past `out` (a padding row of a ragged STORE). */
 int b200_test_stream(b200_stream_test *t);
 
+/* The exact attention forms of b200_test_attention. */
+enum {
+    B200_ATT_SINGLE = 0,      /* k_attention: the decode graph (one row) */
+    B200_ATT_BATCH = 1,       /* k_attention_batch: a batched step over distinct slots (rows 1..8) */
+    B200_ATT_CACHED_ROWS = 2, /* k_rope_kv_batch + k_attention_cached_rows: multi-position steps, the exact multi-slot prefill (rows 1..8) */
+    B200_ATT_CHUNK = 3,       /* k_i8_rope_kv + k_i8_attention: the bit-exact tensor-core prefill (any rows, att_tokens rows per launch) */
+    B200_ATT_PERSISTENT = 4   /* pd_attention_head, the persistent decode kernel's copy of the body (one row, head size 64 or 128) */
+};
+
+/* One exact attention launched on its own (b200_test_attention).  One layer; row r is (slot[r], pos[r]).  The caches hold
+ * `slots` slots of [ctx][n_kv_heads * head_size] floats each. */
+typedef struct b200_attention_test {
+    int32_t form;          /* B200_ATT_* */
+    int32_t head_size;     /* 32, 64, 96, 128 or 256 (persistent: 64 or 128) */
+    int32_t n_heads, n_kv_heads;
+    int32_t arch;          /* KF_* flags: 1 NeoX rotation, 2 Qwen3 q/k RMSNorm, 4 Qwen2 q|k|v bias, 8 Granite's attention scale */
+    int32_t ctx;           /* context length: picks shared or global score rows as the plan does (3 * head_size + ctx > 4096: global) */
+    int32_t rows;          /* single / persistent: 1; batch / cached rows: 1..8; chunk: any >= 1 */
+    int32_t slots;         /* cache slots (>= 1) */
+    int32_t att_tokens;    /* chunk: rows per attention launch, 1..rows (the plan's rule for its scratch bound); other forms: 0 */
+    int32_t dry;           /* 1: return after the checks with info filled in; makes no CUDA call */
+    float eps;             /* the q/k RMSNorm's epsilon */
+    float score_arg;       /* sqrt(head_size) (scores are divided by it), or with arch & 8 Granite's attention multiplier */
+    const int32_t *slot;   /* [rows] */
+    const int32_t *pos;    /* [rows], each < ctx */
+    const float *qkv;      /* [rows][q | k | v width]: unrotated, without bias */
+    const float *k_cache;  /* [slots][ctx][kv width] before the launch */
+    const float *v_cache;
+    const float *rope_cr;  /* [ctx][head_size / 2] */
+    const float *rope_ci;
+    const float *q_norm;   /* arch & 2: [head_size] */
+    const float *k_norm;
+    const float *qkv_bias; /* arch & 4: [q | k | v width] */
+    float *qkv_out;        /* out: the qkv rows after the launch (rotated q written back) */
+    float *k_out;          /* out: both caches after the launch */
+    float *v_out;
+    int8_t *xq;            /* out: each row's attention output quantised to Q8_0, [rows][q width] ... */
+    float *xs;             /* ... and its block scales [rows][q width / 32] */
+    float *xb;             /* single form, nullable: the float output [q width] (an FP16 plan's form) */
+    int64_t info[5];       /* out: grid x (heads), grid y (rows per attention launch), dynamic shared memory, score rows in global
+                              memory (0 / 1), attention launches */
+} b200_attention_test;
+
+/* Test hook: one exact attention form launched as the plan launches it (grid, dynamic shared memory and its attribute, score-row
+ * scratch rule and indexing).  B200_ERR_BAD_ARG, before any CUDA call, for what the plan would never launch or what could read out
+ * of bounds: a head size without a kernel of that form, n_heads % n_kv_heads != 0, a position outside 0..ctx-1, a slot outside
+ * the caches, rows outside the form's range, att_tokens outside 1..rows, two batch rows on one slot or two rows of a slot at one
+ * position.  B200_ERR_STATE when the launch wrote past the end of an output. */
+int b200_test_attention(b200_attention_test *t);
+
+/* Test hook: the two exp expressions of the bit-exact paths on the device, for the n float bit patterns first, first + 1, ...:
+ * e[i] = (float)exp((double)x) (softmaxes, routers, the shared-expert gate) and e1[i] = (float)(1.0 + exp((double)x)) (the SwiGLU
+ * denominator), computed as the kernels compute them.  Host arrays of n floats; first + n - 1 must not wrap. */
+int b200_test_exp(uint32_t first, int64_t n, float *e, float *e1);
+
 /* Test hook: the causal attention of the tensor-core prefill (k_pf_attention_mma_packed, on f16 K / V copies built by
  * k_pf_kv_to_f16_packed, as a chunk runs it) over n_seqs sequences at once.  Sequence i has lengths[i] >= 1 query tokens at positions
  * start_positions[i]..; q: f32 [sum lengths][n_heads * head_size] (rotated; the sequences' rows back to back, placed in rows of

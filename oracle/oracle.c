@@ -65,6 +65,7 @@ typedef struct {
 
 typedef struct {
     float *x, *xb, *xb2, *q, *k, *v, *hb, *hb2, *att, *logits;
+    float *xo;                      /* the attention output of the last layer, before wo ([n_heads * head_size]) */
     float *key_cache, *value_cache; /* [L][ctx][kvDim] */
     float *rope_cr, *rope_ci;       /* [ctx][head/2] */
     int8_t *aq;                     /* hoisted activation quants */
@@ -265,6 +266,42 @@ static void softmax(float *a, int n) {
     for (int i = 0; i < n; i++) a[i] = a[i] / sum;
 }
 
+/* ---- (float)Math.exp(double) over n floats: the softmax's exp (and, at -g, the shared-expert gate's), for restatements of it */
+void oracle_exp_narrow(const float *x, float *y, int64_t n) {
+    for (int64_t i = 0; i < n; i++) y[i] = (float)exp((double)x[i]);
+}
+
+/* Checks a device's evaluation of the exp expressions of the bit-exact paths against this library's exp: for the float x with
+ * bit pattern first + i, e[i] must equal (float)exp((double)x) (softmaxes, routers, shared-expert gate) and e1[i]
+ * (float)(1.0 + exp((double)x)) (the SwiGLU denominator), bit for bit.  Returns the number of inputs where either differs; the
+ * lowest max_report of them go to bad (bit patterns, ascending). */
+int64_t oracle_exp_sweep(uint32_t first, int64_t n, const float *e, const float *e1, uint32_t *bad, int32_t max_report) {
+    int64_t count = 0;
+    int32_t nbad = 0;
+#pragma omp parallel for schedule(static, 65536) reduction(+ : count)
+    for (int64_t i = 0; i < n; i++) {
+        const uint32_t b = first + (uint32_t)i;
+        float x, r, r1;
+        memcpy(&x, &b, 4);
+        const double d = exp((double)x);
+        r = (float)d;
+        r1 = (float)(1.0 + d);
+        if (memcmp(&r, e + i, 4) == 0 && memcmp(&r1, e1 + i, 4) == 0) continue;
+        count++;
+#pragma omp critical(oracle_exp_sweep)
+        { /* keep the lowest max_report patterns, sorted */
+            int k = nbad < max_report ? nbad++ : max_report;
+            if (k == max_report && (max_report == 0 || b > bad[max_report - 1])) k = -1;
+            else if (k == max_report) k = max_report - 1;
+            if (k >= 0) {
+                while (k > 0 && bad[k - 1] > b) { bad[k] = bad[k - 1]; k--; }
+                bad[k] = b;
+            }
+        }
+    }
+    return count;
+}
+
 /* ---- FloatTensor.argmax, FloatTensor.java:138-151 (first strict maximum) */
 int oracle_argmax(const float *v, int n) {
     int mi = 0; float mv = v[0];
@@ -284,7 +321,7 @@ ostate *oracle_state_new(const omodel *m) {
     s->q = calloc(qd > m->dim ? qd : m->dim, 4); s->k = calloc(m->dim > kvd ? m->dim : kvd, 4);
     s->v = calloc(m->dim > kvd ? m->dim : kvd, 4);
     s->hb = calloc(m->hidden, 4); s->hb2 = calloc(m->hidden, 4);
-    s->att = calloc((size_t)m->n_heads * m->ctx, 4); s->logits = calloc(m->vocab, 4);
+    s->att = calloc((size_t)m->n_heads * m->ctx, 4); s->logits = calloc(m->vocab, 4); s->xo = calloc(qd, 4);
     s->key_cache = calloc((size_t)m->n_layers * m->ctx * kvd, 4);   /* Java arrays are zero-filled */
     s->value_cache = calloc((size_t)m->n_layers * m->ctx * kvd, 4);
     s->rope_cr = malloc((size_t)m->ctx * (m->head_size / 2) * 4);
@@ -295,7 +332,7 @@ ostate *oracle_state_new(const omodel *m) {
 }
 void oracle_state_free(ostate *s) {
     free(s->x); free(s->xb); free(s->xb2); free(s->q); free(s->k); free(s->v); free(s->hb); free(s->hb2);
-    free(s->att); free(s->logits); free(s->key_cache); free(s->value_cache); free(s->rope_cr); free(s->rope_ci);
+    free(s->att); free(s->logits); free(s->xo); free(s->key_cache); free(s->value_cache); free(s->rope_cr); free(s->rope_ci);
     free(s->aq); free(s->ascale); free(s);
 }
 void oracle_state_reset(const omodel *m, ostate *s) {
@@ -307,9 +344,12 @@ float *oracle_state_x(ostate *s) { return s->x; }
 float *oracle_state_key_cache(ostate *s) { return s->key_cache; }
 float *oracle_state_value_cache(ostate *s) { return s->value_cache; }
 /* read-only views of the last layer's intermediates after a forward: the softmax weights ([n_heads][ctx], entries 0..pos of each
- * head) and the SwiGLU output that w2 multiplies ([hidden]) */
+ * head), the SwiGLU output that w2 multiplies ([hidden]), the rotated q ([n_heads * head_size]) and the attention output that wo
+ * multiplies ([n_heads * head_size]) */
 float *oracle_state_att(ostate *s) { return s->att; }
 float *oracle_state_hb(ostate *s) { return s->hb; }
+float *oracle_state_q(ostate *s) { return s->q; }
+float *oracle_state_att_out(ostate *s) { return s->xo; }
 
 /*
  * InferenceCore.forwardJava (InferenceCore.java:50-172) and
@@ -401,6 +441,7 @@ float *oracle_forward(const omodel *m, ostate *s, int token, int pos, int want_l
                 for (int i = 0; i < hs; i++) xb[i] = a * v[i] + xb[i]; /* saxpyInPlace, FloatTensor.java:221-227 */
             }
         }
+        memcpy(s->xo, s->xb, (size_t)qd * 4);
 
         matmul(m, s, &m->wo[l], s->xb, s->xb2, dim, qd);
         for (int i = 0; i < dim; i++) s->x[i] = s->x[i] + s->xb2[i];

@@ -50,12 +50,16 @@ def lib() -> C.CDLL:
         L.oracle_state_new.restype = vp
         L.oracle_state_free.argtypes = [vp]
         L.oracle_state_reset.argtypes = [C.POINTER(OModel), vp]
-        for fn in ("oracle_state_logits", "oracle_state_x", "oracle_state_key_cache", "oracle_state_value_cache", "oracle_state_att", "oracle_state_hb"):
+        for fn in ("oracle_state_logits", "oracle_state_x", "oracle_state_key_cache", "oracle_state_value_cache", "oracle_state_att", "oracle_state_hb",
+                   "oracle_state_q", "oracle_state_att_out"):
             getattr(L, fn).argtypes = [vp]
             getattr(L, fn).restype = C.POINTER(f32)
         L.oracle_forward.argtypes = [C.POINTER(OModel), vp, i32, i32, i32]
         L.oracle_forward.restype = C.POINTER(f32)
         L.oracle_argmax.argtypes = [vp, i32]
+        L.oracle_exp_narrow.argtypes = [vp, vp, C.c_int64]
+        L.oracle_exp_sweep.argtypes = [C.c_uint32, C.c_int64, vp, vp, vp, i32]
+        L.oracle_exp_sweep.restype = C.c_int64
         L.oracle_q8_dot_ref.argtypes = [vp, C.c_int64, vp, i32]
         L.oracle_q8_dot_ref.restype = f32
         L.oracle_f16_dot.argtypes = [vp, vp, i32, i32]
@@ -288,6 +292,14 @@ class OracleModel:
         """silu(gate) * up of the last layer of the last forward: the activation its down projection multiplies."""
         return np.ctypeslib.as_array(lib().oracle_state_hb(self.state), shape=(self.cfg.hidden_dim,)).copy()
 
+    def q(self) -> np.ndarray:
+        """The rotated q [n_heads * head_size] of the last layer of the last forward."""
+        return np.ctypeslib.as_array(lib().oracle_state_q(self.state), shape=(self.cfg.n_heads * self.cfg.head_size,)).copy()
+
+    def att_out(self) -> np.ndarray:
+        """The attention output [n_heads * head_size] of the last layer of the last forward: the activation its wo multiplies."""
+        return np.ctypeslib.as_array(lib().oracle_state_att_out(self.state), shape=(self.cfg.n_heads * self.cfg.head_size,)).copy()
+
     def close(self):
         if self.state:
             lib().oracle_state_free(self.state)
@@ -303,6 +315,23 @@ class OracleModel:
 def argmax(v: np.ndarray) -> int:
     v = np.ascontiguousarray(v, dtype=np.float32)
     return int(lib().oracle_argmax(v.ctypes.data, len(v)))
+
+
+def exp_narrow(x: np.ndarray) -> np.ndarray:
+    """(float)Math.exp((double)x) elementwise, with this library's exp (the one every oracle softmax uses)."""
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    y = np.empty_like(x)
+    lib().oracle_exp_narrow(x.ctypes.data, y.ctypes.data, x.size)
+    return y
+
+
+def exp_sweep(first: int, e: np.ndarray, e1: np.ndarray, max_report: int = 16):
+    """(mismatches, their lowest bit patterns) of a device's (float)exp((double)x) in e and (float)(1.0 + exp((double)x)) in e1 for the
+    floats x with bit patterns first, first + 1, ... (oracle_exp_sweep)."""
+    e, e1 = np.ascontiguousarray(e, dtype=np.float32), np.ascontiguousarray(e1, dtype=np.float32)
+    bad = np.zeros(max_report, dtype=np.uint32)
+    n = int(lib().oracle_exp_sweep(first, len(e), e.ctypes.data, e1.ctypes.data, bad.ctypes.data, max_report))
+    return n, [int(b) for b in bad[:min(n, max_report)]]
 
 
 def bench_tokens(vocab: int, n: int, seed: int = 42) -> np.ndarray:
